@@ -9,15 +9,15 @@ normalisation -> 80 policy-gradient steps (+ final KL pass) -> old-policy sync -
 (early stop disabled: max_kl = inf, so the work is fixed; SURVEY.md section 8d).
 Workload at N GPUs: 1024 envs x 1000 steps PER GPU (BASELINE configs[1]; configs[4] at N = 8) -- weak scaling.
 
-  value : transitions/s with the batch already resident in HBM (engine.update only).
+  value : transitions/s with the batch already resident in HBM (engine.update only).  --dump-outputs DIR writes what
+          the last timed engine.update computed (parameters, Adam moments, update statistics, scalar history) as .npy.
   e2e   : same through the public API, PPO.train(experience) with a PackedExperience in pinned host memory (the
           rollout store a sampler fills): host -> device copies of the batch, parameter / optimizer-state upload, the
           update, and the device -> host read-back of parameters, optimizer state and the logged scalars, all inside the
           timed region.
 
-The CPU legs (`cpu_baseline` of the default run, `--impl reference`) run the UNMODIFIED reference, pip-installed from
-/root/reference into git-ignored baseline/_ref by __graft_entry__.build() (kind "reference"); only if that package is
-absent they fall back to oracle/torch_port.py (kind "port").  The measured arm imports neither: it builds its learners
+The CPU legs (`cpu_baseline` of the default run, `--impl reference`) run the UNMODIFIED reference when it is installed
+under git-ignored baseline/_ref (kind "reference"); otherwise they run oracle/torch_port.py (kind "port").  The measured arm imports neither: it builds its learners
 and synthetic data from `rl_replicas_b200.synthetic` alone.
 """
 from __future__ import annotations
@@ -52,7 +52,8 @@ def peaks():
         with open(path) as f:
             p = json.load(f)
         return dict(hbm=p["hbm_gbs"], tf_burst=p["bf16_tflops"], tf_sust=p["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s -- ceilings, not measured rates
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet")
 
 
 def make_nets(seed=0):
@@ -77,7 +78,7 @@ def make_batch(n_envs, horizon, pl, seed):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -230,6 +231,23 @@ def run_reference_arm(args):
     print(json.dumps(line))
 
 
+def dump_outputs(out_dir, engine, stats):
+    """What a caller of engine.update holds after the last timed step: both networks' parameters and Adam moments,
+    the update statistics and the per-iteration scalar history (float32 / float64, about 0.2 MB in all)."""
+    from rl_replicas_b200.engine import POLICY, VALUE
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {}
+    for which, name in ((POLICY, "policy"), (VALUE, "value")):
+        arrays[f"{name}_params"] = engine.get_params(which)
+        m, v, _ = engine.get_adam(which)
+        arrays[f"{name}_adam_exp_avg"], arrays[f"{name}_adam_exp_avg_sq"] = m, v
+    arrays["update_stats"] = np.array([float(getattr(stats, f[0])) for f in stats._fields_], dtype=np.float64)
+    arrays["scalar_history"] = np.asarray(engine.scalar_history(), dtype=np.float64)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float64 if a.dtype == np.float64 else np.float32))
+
+
 def workload_config(n_gpus, envs=1024, horizon=1000):
     return {"workload": f"PPO synthetic HalfCheetah-shaped obs({OBS}) act({ACT}), {envs} envs x {horizon} steps per GPU"
                         f" ({envs * n_gpus} envs total), MLP(64,64) Gaussian policy + value, {N_POLICY}+{N_VALUE} "
@@ -241,13 +259,22 @@ def workload_config(n_gpus, envs=1024, horizon=1000):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=3)
-    ap.add_argument("--warmup", type=int, default=3)
+    def count(minimum):
+        def parse(text):
+            v = int(text)
+            if v < minimum:
+                raise argparse.ArgumentTypeError(f"must be >= {minimum}")
+            return v
+        return parse
+
+    ap.add_argument("--steps", type=count(1), default=3)
+    ap.add_argument("--warmup", type=count(0), default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--envs", type=int, default=1024)
     ap.add_argument("--horizon", type=int, default=1000)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the TRPO (config 3) / TD3 (config 4) side measurements")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed update's outputs to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference_arm(args)
@@ -333,11 +360,15 @@ def main():
     engine = ppo._engine
     hp = ppo._hparams(engine, n_local * world if distributed else 0)
 
+    last = {}
+
     def device_step():
-        engine.update(hp, "ppo", None, distributed)
+        last["stats"] = engine.update(hp, "ppo", None, distributed)
 
     ms_dev = timed(device_step, args.steps, args.warmup)
     clocks = sampler.summary() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, engine, last["stats"])
 
     # ---------------- kernel-level rooflines (rank 0, N = 1 semantics: per-GPU kernels) ----------------
     def stage_ms(stage, reps):
@@ -358,18 +389,6 @@ def main():
     ms_pol = stage_ms("policy_grad_kernel", 10)
     ms_val = stage_ms("value_grad_kernel", 10)
     tf_fused = FLOP_FUSED_STEP * n_local / (ms_fused * 1e-3) / 1e12
-    ncu = {}
-    try:  # dram bytes per launch of the dominant kernel, from the committed ncu --set full capture (tools/ncu_summary.py)
-        with open(os.path.join(ROOT, "profiles", "r02_tc3_ncu.json")) as f:
-            ncu = json.load(f)
-    except Exception:
-        pass
-    ncu_scan = {}
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_scan_ncu.json")) as f:
-            ncu_scan = json.load(f)
-    except Exception:
-        pass
     scan_reps = 20
     engine.run_stage("values", hp)
     ms_scan_pair = stage_ms("scan", scan_reps)
@@ -378,7 +397,7 @@ def main():
     scan_bytes = (8 + 4 + 4 + 4) * n_local  # f64 rewards + values in, adv + ret out
     gbs_scan = scan_bytes / (ms_scan_pair * 1e-3) / 1e9
 
-    # the same scan kernel on a shape whose traffic (1.3 GB) cannot live in the 126 MB L2: the HBM-bandwidth figure
+    # the same scan kernel on a shape whose traffic (1.3 GB) cannot live in the 50 MB L2: the HBM-bandwidth figure
     def scan_large():
         import ctypes as C
         E2, T2 = 65536, 1000
@@ -473,7 +492,7 @@ def main():
                 "ms_per_fvp": ms_fvp, "fvp_per_s": 1e3 / ms_fvp, "fvp_launches": int(ts.fvp_launches),
                 "fvp_tflops_fp32": flop_fvp * E * T / (ms_fvp * 1e-3) / 1e12,
                 "accepted_ratio_index": int(ts.accepted_index), "rejected": int(ts.rejected), "kl": ts.kl,
-                "kernel": "mlp_tc_fvp_kernel (tcgen05 fp16x2: forward + tangents + metric + backward, fp32 re-run predicated behind it)"}
+                "kernel": "mlp_tc_fvp_kernel (wgmma fp16x2: forward + tangents + metric + backward, fp32 re-run predicated behind it)"}
 
     def td3_config4():
         """TD3 synthetic Hopper-shaped replay (obs 11, act 3), minibatch 256, 256-256 nets, 50 train steps per call."""
@@ -555,19 +574,15 @@ def main():
             "gpu_launches": int(launches_per_step * args.steps),
             "gpu_launches_per_step": int(launches_per_step),
             "fused_step_path": fused_path,
-            "roofline": {"kernel": "mlp_tc3_kernel (tcgen05 fp16x2: policy fwd + PPO-clip loss + bwd AND value fwd + MSE + "
+            "roofline": {"kernel": "mlp_tc3_kernel (wgmma fp16x2: policy fwd + PPO-clip loss + bwd AND value fwd + MSE + "
                                    "bwd over the same 128-row tile, one launch per PPO iteration; observations packed "
                                    "once per update and staged by cp.async.bulk)",
                          "bound": "tensor", "achieved": tf_fused, "peak": pk["tf_sust"], "unit": "TFLOP/s",
                          "frac": tf_fused / pk["tf_sust"],
-                         "traffic": ncu.get("dram_bytes_per_launch") if (E, T) == (1024, 1000) else None,
-                         "traffic_note": "dram__bytes_read.sum + dram__bytes_write.sum per launch of one ncu --set full "
-                                         "capture at this shape (profiles/r02_tc3_ncu.json); algorithmic: 104 B per row "
-                                         "of reference data (fp32 obs 68 + act 24 + adv 4 + old log-prob 4 + return 4) "
-                                         "= 106.5 MB; the kernel reads the packed fp16-pair observations (128 B per row) "
-                                         "instead of the fp32 ones: 164 B per row = 167.9 MB",
-                         "ncu": {k: ncu.get(k) for k in ("issue_active_pct", "tensor_pipe_active_pct", "duration_us",
-                                                         "warp_instructions", "registers", "source")},
+                         "traffic": None,
+                         "traffic_note": "algorithmic: 104 B per row of reference data (fp32 obs 68 + act 24 + adv 4 + "
+                                         "old log-prob 4 + return 4) = 106.5 MB; the kernel reads the packed fp16-pair "
+                                         "observations (128 B per row) instead of the fp32 ones: 164 B per row = 167.9 MB",
                          "note": f"fp32-equivalent algorithmic FLOPs ({FLOP_FUSED_STEP}/row: policy {FLOP_POLICY_STEP} + "
                                  f"value {FLOP_VALUE_STEP}) over the CUDA-event launch time; peak = 16-bit dense sustained "
                                  f"GEMM ({pk['src']}); the kernel executes 3 fp16 MMAs per logical fp32 product (2 for "
@@ -585,10 +600,7 @@ def main():
                               "note": "16.4 MB problem: launch-latency bound at this size (SURVEY 7.3-3)"},
             "roofline_scan_large": {"kernel": "gae_scan_episode_kernel<double>", "bound": "hbm", "achieved": gbs_big,
                                     "peak": pk["hbm"], "unit": "GB/s", "frac": gbs_big / pk["hbm"],
-                                    "traffic": ncu_scan.get("dram_bytes_per_launch"),
-                                    "traffic_note": "dram__bytes_read.sum + dram__bytes_write.sum of one ncu --set full "
-                                                    "capture at this shape (profiles/r02_scan_ncu.json; algorithmic "
-                                                    "1.311 GB, the last written lines are still in L2 when it ends)",
+                                    "traffic": None, "traffic_note": "algorithmic 1.311 GB",
                                     "transitions": n_big, "bytes_per_transition": 20, "ms_per_launch": ms_big,
                                     "note": "65536 episodes x 1000 steps: 1.31 GB of algorithmic traffic (> L2)"},
             "update_flops_per_transition": FLOP_PER_TRANSITION,

@@ -1,5 +1,5 @@
 /*
- * b200rl.h -- C ABI of the B200-native policy-gradient update engine (libb200rl.so).
+ * b200rl.h -- C ABI of the H100-native (sm_90a) policy-gradient update engine (libb200rl.so).
  *
  * The reference (rl_replicas 0.0.7) is pure Python and has NO FFI / plugin layer: its drop-in seam is the Python
  * class API (SURVEY.md section 8b).  This header is the native boundary underneath our Python mirror of that API:
@@ -399,15 +399,6 @@ int b200rl_offpolicy_train_gather_rng(b200rl_offpolicy* h, const b200rl_offpolic
 /* The draws of the last train_gather / train_gather_rng call: physical rows idx [S*B] (host int64), noise [S*B*A]
  * (host float32, or NULL) -- what a test replays through the oracle. */
 int b200rl_offpolicy_get_draws(b200rl_offpolicy* h, int32_t S, int32_t B, int64_t* idx, float* noise, void* stream);
-
-/* ------------------------------------------------------------------------------------------------------------
- * Diagnostics (not on the product path): issue a chain of tcgen05.mma kind::tf32 instructions on a caller-supplied
- * shared-memory image and return the raw TMEM contents [128 lanes, read_cols]; tests use it to pin the descriptor
- * and TMEM layouts the tensor-core kernels rely on.  mmas: array of {u64 adesc, u64 bdesc, u32 idesc, u32 dcol,
- * u32 accumulate, u32 pad}, descriptor start addresses relative to the 1024-byte-aligned image base.
- * ------------------------------------------------------------------------------------------------------------ */
-int b200rl_tc_probe(const uint32_t* image_dev, int image_words, const void* mmas_dev, int n_mma, int read_cols,
-                    float* out_dev, void* stream);
 
 #ifdef __cplusplus
 }

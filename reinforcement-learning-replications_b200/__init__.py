@@ -1,4 +1,4 @@
-"""rl_replicas_b200 -- B200-native policy-gradient update engine behind rl_replicas' Python API.
+"""rl_replicas_b200 -- H100-native (sm_90a) policy-gradient update engine behind rl_replicas' Python API.
 
 The directory is named after the reference repository (``reinforcement-learning-replications_b200``), which is not
 an importable identifier; import it as ``rl_replicas_b200`` (the repo-root shim ``rl_replicas_b200.py`` maps the

@@ -153,7 +153,6 @@ SIGNATURES = {
                                           [C.c_void_p] * 5 + [C.c_int64] * 3 + [C.c_uint64] * 2 + [C.c_void_p] * 5 +
                                           [C.POINTER(C.c_int32), C.c_void_p]),
     "b200rl_offpolicy_get_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "b200rl_tc_probe": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "b200rl_discounted_cumsum": (C.c_int, [C.c_void_p, C.c_int64, C.c_double, C.c_void_p, C.c_void_p]),
     "b200rl_gae_f64": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_double, C.c_double, C.c_void_p,
                                  C.c_void_p]),
@@ -181,7 +180,7 @@ def load() -> C.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise B200RLError(
-            f"{LIB_PATH} is missing: build it with `python __graft_entry__.py` (nvcc, sm_100a). "
+            f"{LIB_PATH} is missing: build it with `python __graft_entry__.py` (nvcc, sm_90a). "
             "There is no CPU fallback for the update path.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():

@@ -28,7 +28,7 @@ def describe_mlp(module: nn.Module) -> Tuple[List[int], str, str, List[nn.Linear
     seq = getattr(module, "network", module)
     mods = list(seq.children()) if isinstance(seq, nn.Sequential) else None
     if not mods:
-        raise NotImplementedError(f"B200 engine supports MLP(Linear/activation pairs) networks only, got {type(module).__name__}")
+        raise NotImplementedError(f"the update engine supports MLP(Linear/activation pairs) networks only, got {type(module).__name__}")
     linears, acts = [], []
     for i, m in enumerate(mods):
         if i % 2 == 0:

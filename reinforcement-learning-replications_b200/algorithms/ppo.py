@@ -1,5 +1,5 @@
 """PPO-clip with approximate-KL early stopping -- the reference's class surface (ref: algorithms/ppo.py:29-306) over
-the B200 update engine.  ``learn`` / ``save_model`` keep the reference's host-side behaviour; ``train`` is the hot
+the GPU update engine.  ``learn`` / ``save_model`` keep the reference's host-side behaviour; ``train`` is the hot
 path: pack -> engine (CUDA) -> write-back."""
 from __future__ import annotations
 

@@ -1,5 +1,5 @@
 """TD3 and DDPG -- the reference's class surfaces (ref: algorithms/td3.py:25-382, algorithms/ddpg.py:24-314) over the
-B200 off-policy engine.  ``learn`` keeps the reference's host-side loop; ``train`` is the hot path."""
+GPU off-policy engine.  ``learn`` keeps the reference's host-side loop; ``train`` is the hot path."""
 from __future__ import annotations
 
 import copy

@@ -1,4 +1,4 @@
-"""TRPO -- the reference's class surface (ref: algorithms/trpo.py:28-277) over the B200 update engine."""
+"""TRPO -- the reference's class surface (ref: algorithms/trpo.py:28-277) over the GPU update engine."""
 from __future__ import annotations
 
 import logging

@@ -1,4 +1,4 @@
-// Shared helpers for libb200rl (sm_100a only).
+// Shared helpers for libb200rl (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -34,6 +34,9 @@ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 inline int pad4(int x) { return (x + 3) & ~3; }
 
 int device_sm_count();
+
+// accumulator memory of the tensor-core kernels (tc_common.cuh) for a launch of `grid` CTAs on stream `s`
+float* acc_mem(int grid, cudaStream_t s);
 
 // global launch counter (bench.py reports gpu_launches from it)
 void count_launch(int n = 1);

@@ -5,9 +5,11 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <mutex>
 #include <vector>
 
 #include "common.cuh"
+#include "tc_common.cuh"
 #include "tc3.cuh"
 
 namespace b200rl {
@@ -33,6 +35,33 @@ int device_sm_count() {
   if (cudaGetDevice(&dev) != cudaSuccess) return -1;
   if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return -1;
   return sms;
+}
+
+// One buffer per (device, stream): launches on one stream run one after the other, so they can share it, and
+// launches on different streams (data-parallel engines on one GPU) never do.  Every tensor-core grid is at most one
+// CTA per SM, so the buffer is allocated once at that size (132 x 256 KB = 33 MB on an H100) and never resized or
+// freed while the process runs.  Launches under stream capture are refused: a captured graph could be replayed on
+// another stream while this one uses the same buffer.
+float* acc_mem(int grid, cudaStream_t s) {
+  struct Entry {
+    int dev;
+    cudaStream_t stream;
+    float* ptr;
+  };
+  static std::mutex mu;
+  static std::vector<Entry> entries;
+  int dev = 0;
+  const int sms = device_sm_count();
+  if (grid <= 0 || grid > sms || cudaGetDevice(&dev) != cudaSuccess) return nullptr;
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(s, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone) return nullptr;
+  std::lock_guard<std::mutex> lock(mu);
+  for (const Entry& e : entries)
+    if (e.dev == dev && e.stream == s) return e.ptr;
+  float* p = nullptr;
+  if (cudaMalloc(&p, (size_t)sms * ACC_CTA_FLOATS * sizeof(float)) != cudaSuccess) return nullptr;
+  entries.push_back(Entry{dev, s, p});
+  return p;
 }
 
 }  // namespace b200rl

@@ -4,7 +4,7 @@
 // policies/categorical_policy.py:22-32, algorithms/ppo.py:237-257 + autograd backward (:234), :259-269, :282-287
 // (+ :277), algorithms/vpg.py:200-206, algorithms/trpo.py:154-165, utils.py:60-71 and utils.py:90-92 (on load).
 //
-// Data flow (fp32 CUDA-core path; the tcgen05 path in mlp_tc.cu keeps the same flow):
+// Data flow (fp32 CUDA-core path; the tensor-core path in mlp_tc.cu keeps the same flow):
 //   * grid = min(#tiles, #SMs) persistent CTAs, tile = 64 rows, static round-robin tile -> CTA map (deterministic).
 //   * all weights live in shared memory for the whole launch, in both [out][in] and [in][out] order, so every
 //     tile product is the SAME k-major inner loop  C[m][n] += A[k][m] * B[k][n]  with float4 shared loads:

@@ -1,16 +1,16 @@
-// mlp_tc: the fused MLP step on the 5th-generation tensor cores (tcgen05 + TMEM), sm_100a only.
+// mlp_tc: the fused MLP step on the tensor cores (wgmma), sm_90a.
 //
 // Same contract and data flow as mlp_fused.cu (see there for the reference file:line map); this kernel is selected
 // for the shapes the reference's on-policy recipes use: 3 Linear layers, hidden widths 64/64, tanh hidden,
 // identity output, obs width <= 32, output width <= 15.  Everything else takes the fp32 kernel.
 //
-// Precision: tcgen05 has no fp32 MMA kind and plain TF32 violates the 1e-5 parity bar (SURVEY 7.3-1), so every fp32
+// Precision: the tensor cores have no fp32 MMA and plain TF32 violates the 1e-5 parity bar, so every fp32
 // operand is split into THREE bf16 values x = h + m + l (24 mantissa bits) and every logical product is the six
-// kind::f16 MMAs  mm + hl + lh + hm + mh + hh  with fp32 accumulation in TMEM -- measured 1.3e-7 relative error
-// against float64 (tests/test_gpu_tc_probe.py).  bf16 (not tf32) because a SWIZZLE_128B buffer of 16-bit elements can
+// kind::f16 MMAs  mm + hl + lh + hm + mh + hh  with fp32 accumulation -- 2^-24-grade relative error per
+// product, which the golden / oracle parity tests hold to 1e-5.  bf16 (not tf32) because a SWIZZLE_128B buffer of 16-bit elements can
 // be read BOTH K-major (activations as the A operand of the next layer) and MN-major (the same activations as an
 // operand of the dW = dZ^T X product, whose reduction runs over the tile's rows); tf32 MN-major needs a different
-// swizzle, i.e. a second copy of every activation (pinned on hardware by the probe tests).
+// swizzle, i.e. a second copy of every activation .
 //
 // Per CTA: 128-row tiles, persistent over tiles (grid = min(#tiles, #SMs)), 8 epilogue warps + 1 MMA-issuing warp.
 //   shared memory  operand buffers, 64 bf16 columns x 128-byte rows, SWIZZLE_128B, three splits each:
@@ -18,10 +18,10 @@
 //                  H1, H2 [128][64]: activations, overwritten in place by dZ1 / dZ2 during the backward pass
 //                  W1, W2 [64][64], W3 [16][64]: torch [out][in] order = K-major B operand in the forward pass and,
 //                  unchanged, MN-major B operand of dX = dZ W in the backward pass
-//   tensor memory  Z1/H1, Z2/H2 (fp32, kept for tanh'), OUT, dH2, dH1 (M = 128) and the per-CTA gradient
+//   accumulator memory  Z1/H1, Z2/H2 (fp32, kept for tanh'), OUT, dH2, dH1 (M = 128) and the per-CTA gradient
 //                  accumulators dW2, dW1, dW3^T, db2, db1 (M = 64) that persist across the CTA's tiles.
 //   stages / tile  X -> [F1] -> tanh -> [F2] -> tanh -> [F3] -> log-prob/loss/dOut -> [dW3^T, dH2] -> dZ2 ->
-//                  [dW2, db2, dH1] -> dZ1 -> [dW1, db1]; one tcgen05.commit + mbarrier wait per bracketed stage.
+//                  [dW2, db2, dH1] -> dZ1 -> [dW1, db1]; one acc_commit + mbarrier wait per bracketed stage.
 #include <cuda_bf16.h>
 
 #include <cmath>
@@ -33,7 +33,7 @@ namespace b200rl {
 
 constexpr int TC_ROWS = 128;
 constexpr int TC_EPI_WARPS = 8;
-constexpr int TC_THREADS = (TC_EPI_WARPS + 1) * 32;
+constexpr int TC_THREADS = TC_EPI_WARPS * 32 + 128;  // + the issuing warpgroup
 constexpr float TC_LOG_SQRT_2PI = 0.91893853320467274178f;
 constexpr float TC_ENT_CONST = 1.4189385332046727418f;
 
@@ -81,6 +81,7 @@ struct TcArgs {
   const unsigned* run_if;  // when set: run only if *run_if == seq (wide-range re-run of an mlp_tc2 launch)
   unsigned seq;
   int total_rows;          // partial rows the consumer reduces (> gridDim.x when standing in for mlp_tc2)
+  float* acc_mem;              // accumulator memory, ACC_CTA_FLOATS per CTA (tc_common.cuh)
 };
 
 // byte offset of element (r, c) inside one split buffer (c < 64)
@@ -114,26 +115,6 @@ __device__ __forceinline__ void store_chunk3(uint8_t* sm, uint32_t buf, uint32_t
   *reinterpret_cast<uint4*>(sm + off + 2 * split_stride) = l;
 }
 
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
-      "%30,%31,%32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-      "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-
 __device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_dst), "l"(gsrc) : "memory");
 }
@@ -155,39 +136,18 @@ __device__ __forceinline__ OpDesc op_mnmajor(uint32_t addr, uint32_t rows, uint3
   return OpDesc{(uint32_t)d, (uint32_t)(d >> 32), split_bytes >> 4, 2048u >> 4};
 }
 
-// the six split products, smallest terms first: (m,m) (h,l) (l,h) (h,m) (m,h) (h,h); k-loop kept rolled (code size)
+// the six split products, smallest terms first: (m,m) (h,l) (l,h) (h,m) (m,h) (h,h)
 __device__ __forceinline__ void issue6(uint32_t d_tmem, uint32_t idesc, int ksteps, bool accumulate_first,
                                        const OpDesc a, const OpDesc b) {
-  constexpr int TI[6] = {1, 0, 2, 0, 1, 0};
-  constexpr int TJ[6] = {1, 2, 0, 1, 0, 0};
-  uint32_t acc = accumulate_first ? 1u : 0u;
-#pragma unroll
-  for (int t = 0; t < 6; ++t) {
-    uint32_t alo = a.lo + TI[t] * a.split_step, blo = b.lo + TJ[t] * b.split_step;
-#pragma unroll 1
-    for (int k = 0; k < ksteps; ++k) {
-      umma_f16_elect2(d_tmem, alo, a.hi, blo, b.hi, idesc, acc);
-      acc = 1u;
-      alo += a.k_step;
-      blo += b.k_step;
-    }
-  }
+  const uint32_t alo[6] = {a.lo + a.split_step, a.lo, a.lo + 2 * a.split_step, a.lo, a.lo + a.split_step, a.lo};
+  const uint32_t blo[6] = {b.lo + b.split_step, b.lo + 2 * b.split_step, b.lo, b.lo + b.split_step, b.lo, b.lo};
+  mma_product(d_tmem, idesc, alo, blo, 6, a.hi, b.hi, a.k_step, b.k_step, ksteps, accumulate_first);
 }
 // A (three splits) times an operand that is exact in bf16 (the ones column, split 0 only): three products
 __device__ __forceinline__ void issue3(uint32_t d_tmem, uint32_t idesc, int ksteps, bool accumulate_first,
                                        const OpDesc a, const OpDesc b) {
-  uint32_t acc = accumulate_first ? 1u : 0u;
-#pragma unroll
-  for (int sp = 2; sp >= 0; --sp) {
-    uint32_t alo = a.lo + sp * a.split_step, blo = b.lo;
-#pragma unroll 1
-    for (int k = 0; k < ksteps; ++k) {
-      umma_f16_elect2(d_tmem, alo, a.hi, blo, b.hi, idesc, acc);
-      acc = 1u;
-      alo += a.k_step;
-      blo += b.k_step;
-    }
-  }
+  const uint32_t alo[3] = {a.lo + 2 * a.split_step, a.lo + a.split_step, a.lo}, blo[3] = {b.lo, b.lo, b.lo};
+  mma_product(d_tmem, idesc, alo, blo, 3, a.hi, b.hi, a.k_step, b.k_step, ksteps, accumulate_first);
 }
 
 #ifdef B200RL_TC_TIMING
@@ -264,10 +224,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
         s_dist[16 + a] = logf(scale);
       }
   }
-  if (warp == TC_EPI_WARPS) {
-    tmem_alloc(smem_u32(&tmem_holder), 512);
-    tmem_relinquish();
-  }
+  if (tid == 0) acc_bind(p.acc_mem, &tmem_holder);
   if (tid == 0) {
     mbar_init(smem_u32(&mbar), 1);
     fence_mbar_init();
@@ -282,7 +239,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
   const long long num_tiles = (p.n_rows + TC_ROWS - 1) / TC_ROWS;
   constexpr int STAGES = BACKWARD ? 6 : 3;
 
-  if (warp == TC_EPI_WARPS) {
+  if (warp >= TC_EPI_WARPS) {
     // =============================== MMA issuer warp =================================================
     const uint32_t I_128_64_KK = make_idesc_bf16(128, 64, 0, 0), I_128_16_KK = make_idesc_bf16(128, 16, 0, 0);
     const uint32_t I_128_64_KM = make_idesc_bf16(128, 64, 0, 1), I_64_64_MM = make_idesc_bf16(64, 64, 1, 1);
@@ -325,7 +282,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
           issue6(ut + TM_DW1, I_64_32_MM, 8, !first, H1_M, XD_M0);
           issue3(ut + TM_DB1, I_64_16_MM, 8, !first, H1_M, XD_M32);
         }
-        umma_commit_elect(bar);
+        acc_commit(bar);
         __syncwarp();
       }
       first = false;
@@ -333,8 +290,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
   } else {
     // =============================== epilogue warps ==================================================
     const int q = warp & 3, half = warp >> 2;
-    const int r = 32 * q + lane;                         // row of the tile == TMEM lane
-    const uint32_t lane_addr = (uint32_t)(32 * q) << 16;  // this warp's TMEM lane quadrant
+    const int r = 32 * q + lane;                         // row of the tile == accumulator memory lane
+    const uint32_t lane_addr = (uint32_t)(32 * q) << 16;  // this warp's accumulator memory lane quadrant
     const int c0 = 32 * half;                            // this warp's column half
     uint32_t phase = 0;
 
@@ -350,17 +307,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
 #pragma unroll
     for (int a = 0; a < 16; ++a) db3[a] = 0.f;
 
-    // tanh layer epilogue: Z (TMEM) + bias -> tanh -> fp32 copy back to TMEM (for tanh') + bf16 splits to smem
+    // tanh layer epilogue: Z (accumulator memory) + bias -> tanh -> fp32 copy back to accumulator memory (for tanh') + bf16 splits to smem
     auto act_epilogue = [&](uint32_t tm_col, const float* bias, uint32_t dst_buf) {
 #pragma unroll
       for (int sub = 0; sub < 2; ++sub) {  // 16 columns at a time keeps the live register set small
         const int cs = c0 + 16 * sub;
         uint32_t v[16];
-        tmem_ld16(tmem + lane_addr + tm_col + cs, v);
-        tmem_wait_ld();
+        acc_ld16(tmem + lane_addr + tm_col + cs, v);
 #pragma unroll
         for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(tanhf(__uint_as_float(v[j]) + bias[cs + j]));
-        if (BACKWARD) tmem_st16(tmem + lane_addr + tm_col + cs, v);
+        if (BACKWARD) acc_st16(tmem + lane_addr + tm_col + cs, v);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8];
@@ -369,7 +325,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
           store_chunk3(sm, dst_buf, ACT_BUF, r, (cs >> 3) + ch, x);
         }
       }
-      if (BACKWARD) tmem_wait_st();
     };
     // backward epilogue: dZ = dH * (1 - H^2), bf16 splits over the activation buffer (in place)
     auto dz_epilogue = [&](uint32_t tm_dh, uint32_t tm_h, uint32_t dst_buf) {
@@ -377,9 +332,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
       for (int sub = 0; sub < 2; ++sub) {
         const int cs = c0 + 16 * sub;
         uint32_t g[16], h[16];
-        tmem_ld16(tmem + lane_addr + tm_dh + cs, g);
-        tmem_ld16(tmem + lane_addr + tm_h + cs, h);
-        tmem_wait_ld();
+        acc_ld16(tmem + lane_addr + tm_dh + cs, g);
+        acc_ld16(tmem + lane_addr + tm_h + cs, h);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8];
@@ -474,8 +428,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
       // ---- distribution / loss epilogue (one thread per row: warps 0..3) ----
       if (half == 0) {
         uint32_t o[16];
-        tmem_ld16(tmem + lane_addr + TM_OUT, o);
-        tmem_wait_ld();
+        acc_ld16(tmem + lane_addr + TM_OUT, o);
         float out[16], dout[16];
 #pragma unroll
         for (int a = 0; a < 16; ++a) {
@@ -599,37 +552,32 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
     if (tid == 0 && blockIdx.x == 0 && BACKWARD)
       for (int i = 0; i < 16; ++i) g_tc_t[i] = tacc[i];
 #endif
-    // ---- per-CTA results: gradient accumulators (TMEM, M = 64 layout: row m -> lane (m%16) + 32*(m/16)) ----
+    // ---- per-CTA results: gradient accumulators (accumulator memory, M = 64 layout: row m -> lane (m%16) + 32*(m/16)) ----
     if (BACKWARD && half == 0) {
       float* dst = p.partials + (size_t)blockIdx.x * p.P;
       const int m = 16 * q + lane;  // valid for lane < 16
       uint32_t v[32];
       for (int cb = 0; cb < 2; ++cb) {  // dW2 [64 o][64 i]
-        tmem_ld32(tmem + lane_addr + TM_DW2 + 32 * cb, v);
-        tmem_wait_ld();
+        acc_ld32(tmem + lane_addr + TM_DW2 + 32 * cb, v);
         if (lane < 16 && m < h2)
 #pragma unroll
           for (int j = 0; j < 32; ++j)
             if (32 * cb + j < h1) dst[p.w_off[1] + m * h1 + 32 * cb + j] = __uint_as_float(v[j]);
       }
-      tmem_ld32(tmem + lane_addr + TM_DW1, v);  // dW1 [64 o][32 i]
-      tmem_wait_ld();
+      acc_ld32(tmem + lane_addr + TM_DW1, v);  // dW1 [64 o][32 i]
       if (lane < 16 && m < h1)
 #pragma unroll
         for (int j = 0; j < 32; ++j)
           if (j < n_in) dst[p.w_off[0] + m * n_in + j] = __uint_as_float(v[j]);
       uint32_t w[16];
-      tmem_ld16(tmem + lane_addr + TM_DW3, w);  // dW3^T [64 i][16 o]
-      tmem_wait_ld();
+      acc_ld16(tmem + lane_addr + TM_DW3, w);  // dW3^T [64 i][16 o]
       if (lane < 16 && m < h2)
 #pragma unroll
         for (int a = 0; a < 15; ++a)
           if (a < A_out) dst[p.w_off[2] + a * h2 + m] = __uint_as_float(w[a]);
-      tmem_ld16(tmem + lane_addr + TM_DB2, w);  // column 15 = sum_r dZ2[r][o]
-      tmem_wait_ld();
+      acc_ld16(tmem + lane_addr + TM_DB2, w);  // column 15 = sum_r dZ2[r][o]
       if (lane < 16 && m < h2) dst[p.b_off[1] + m] = __uint_as_float(w[15]);
-      tmem_ld16(tmem + lane_addr + TM_DB1, w);
-      tmem_wait_ld();
+      acc_ld16(tmem + lane_addr + TM_DB1, w);
       if (lane < 16 && m < h1) dst[p.b_off[0] + m] = __uint_as_float(w[15]);
       // db3: fixed-order reduction of the per-row accumulators
 #pragma unroll
@@ -665,7 +613,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
   // ---- teardown ----
   tc_fence_before_sync();
   __syncthreads();
-  if (warp == TC_EPI_WARPS) tmem_dealloc(tmem, 512);
 }
 
 #ifdef B200RL_TC_TIMING
@@ -725,6 +672,9 @@ static int launch_mlp_tc_impl(const b200rl_mlp_loss_grad_args* a, int64_t n_glob
   k.skip_flag = a->skip_flag;
   const int grid = tc_grid(a->n_rows);
   B200RL_REQUIRE(grid > 0, "mlp_tc: no CUDA device");
+  k.acc_mem = acc_mem(grid, s);
+  B200RL_REQUIRE(k.acc_mem != nullptr, "mlp_tc: no accumulator memory (allocation failed, or the stream is being captured): %s",
+                 cudaGetErrorString(cudaGetLastError()));
   if (a->loss != B200RL_LOSS_EVAL) {
     B200RL_CUDA(cudaFuncSetAttribute(mlp_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)TC_SMEM_BYTES));

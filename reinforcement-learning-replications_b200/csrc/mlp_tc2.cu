@@ -1,11 +1,11 @@
-// mlp_tc2: second-generation tensor-core kernel for the fused MLP step (tcgen05 + TMEM, sm_100a only).
+// mlp_tc2: second-generation tensor-core kernel for the fused MLP step (wgmma, sm_90a).
 //
 // Same contract and data flow as mlp_tc.cu / mlp_fused.cu (see mlp_fused.cu for the reference file:line map) and the
 // same shape gate (3 Linear layers, tanh hidden layers of width <= 64 -- zero-padded to 64 --, obs <= 32, out <= 15).
-// What changed, and why -- measured on B200 with the per-stage clocks of tools/profile_step.py and the instruction
-// micro-benchmark tools/tc_mma_bench.cu:
-//   * a tcgen05.mma of these small shapes costs 30..50 cycles whatever its size (instruction floor / SS-mode operand
-//     feed), so the 282 MMAs per 128-row tile of the bf16 x 3 kernel -- not the math -- set its pace.  Here every
+// What changed against the bf16 x 3 kernel, and why.  The kernels were first written for B200 (tcgen05); the figures in
+// this note were measured there with the per-stage clocks of tools/profile_step.py, not on H100:
+//   * a tcgen05.mma of these small shapes cost 30..50 cycles on B200 whatever its size (instruction floor / SS-mode
+//     operand feed), so the 282 MMAs per 128-row tile of the bf16 x 3 kernel -- not the math -- set its pace.  Here every
 //     fp32 operand is split into TWO fp16 values x*2^e = h + l (22 mantissa bits, 3.0e-7 worst-case relative error
 //     per product with the (l,l) term dropped) after an exact power-of-two pre-scale that parks it in fp16's normal
 //     range.  A logical product is then 3 MMAs (h.l, l.h, h.h) on the forward/back-propagation chain and 2 MMAs for
@@ -40,9 +40,9 @@
 namespace b200rl {
 
 constexpr int T2_ROWS = 128;
-constexpr int T2_EPI_WARPS = 16;  // one pool: 4 warps per TMEM lane quadrant, 16 columns each
+constexpr int T2_EPI_WARPS = 16;  // one pool: 4 warps per accumulator memory lane quadrant, 16 columns each
 constexpr int T2_EPI_THREADS = T2_EPI_WARPS * 32;
-constexpr int T2_THREADS = T2_EPI_THREADS + 32;
+constexpr int T2_THREADS = T2_EPI_THREADS + 128;  // + the issuing warpgroup
 constexpr float T2_LOG_SQRT_2PI = 0.91893853320467274178f;
 constexpr float T2_ENT_CONST = 1.4189385332046727418f;
 
@@ -62,9 +62,9 @@ constexpr uint32_t S2_BIAS = S2_OPERANDS_END;  // b1[64] b2[64] b3[16] floats
 constexpr uint32_t S2_DIST = S2_BIAS + 640;    // var[16], log_scale[16], 1/(2 var)[16], 1/var[16] floats
 constexpr uint32_t S2_DB3 = S2_DIST + 256;     // [16 warps][16] floats: running sum_r dOut[r][a] per warp
 constexpr uint32_t S2_SCALE = S2_DB3 + 1024;   // scale factors (floats)
-constexpr uint32_t S2_RED = S2_SCALE + 64;     // block reduction scratch [17 warps][4] floats
+constexpr uint32_t S2_RED = S2_SCALE + 64;     // block reduction scratch [20 warps][4] floats
 constexpr uint32_t S2_SC = S2_RED + 320;       // [16 warps][7] doubles: running scalar sums per warp
-constexpr uint32_t S2_BARS = S2_SC + 896;      // mbarriers: ready[2], chain[2], off[2]; tmem holder; bad flag
+constexpr uint32_t S2_BARS = S2_SC + 896;      // mbarriers: ready[2], chain[2], off[2]; accumulator base address (acc_bind); bad flag
 constexpr uint32_t S2_XS = S2_BARS + 64;       // per-feature observation scales 2^ex_k [32] and their inverses [32]
 constexpr uint32_t S2_ROWMAX = S2_XS + 256;    // [2 slots][128] largest scaled |obs| of each row (precision guard)
 constexpr uint32_t S2_TOTAL = S2_ROWMAX + 1024;
@@ -108,6 +108,7 @@ struct Tc2Args {
   int total_rows;              // partial rows the consumer reduces when that is more than two per CTA (else 0)
   unsigned* status;            // status-ring slot of this launch
   unsigned seq;                // value to store there when the launch must be redone by the wide-range kernel
+  float* acc_mem;              // accumulator memory, ACC_CTA_FLOATS per CTA (tc_common.cuh)
 };
 
 #ifdef B200RL_TC_TIMING
@@ -277,15 +278,12 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
   }
   if (bad) *s_bad = 1;  // non-finite bias
   bad = false;
-  if (warp == T2_EPI_WARPS) {
-    tmem_alloc(smem_u32(s_tmem), 512);
-    tmem_relinquish();
-  }
+  if (tid == 0) acc_bind(p.acc_mem, s_tmem);
   if (tid == 0) {
     for (int s = 0; s < 2; ++s) {
       mbar_init(bars + 8 * s, T2_EPI_THREADS);   // ready[s]: every epilogue thread arrives once per job of slot s
-      mbar_init(bars + 16 + 8 * s, 1);           // chain[s]: tcgen05.commit
-      mbar_init(bars + 32 + 8 * s, 1);           // off[s]:   tcgen05.commit
+      mbar_init(bars + 16 + 8 * s, 1);           // chain[s]: acc_commit
+      mbar_init(bars + 32 + 8 * s, 1);           // off[s]:   acc_commit
     }
     fence_mbar_init();
   }
@@ -300,15 +298,14 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
   const long long cta_tiles = (num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;
   constexpr int STAGES = BACKWARD ? 6 : 3;
 
-  if (warp == T2_EPI_WARPS) {
-    // =============================== MMA issuer warp =================================================
+  if (warp >= T2_EPI_WARPS) {
+    // =============================== MMA issuer warpgroup =================================================
     constexpr uint32_t I_128_64_KK = make_idesc_f16(128, 64, 0, 0), I_128_16_KK = make_idesc_f16(128, 16, 0, 0),
                        I_128_64_KM = make_idesc_f16(128, 64, 0, 1), I_128_64_MM = make_idesc_f16(128, 64, 1, 1),
                        I_128_48_MM = make_idesc_f16(128, 48, 1, 1), I_128_16_MM = make_idesc_f16(128, 16, 1, 1);
-    // warp-uniform by construction: `base` comes from the shared-memory window, and a 512-column allocation is the
-    // whole tensor memory, whose base address is 0 (checked once below)
+    // warp-uniform by construction: `base` comes from the shared-memory window, and accumulator addresses are
+    // (lane << 16) | column within this CTA's block of the accumulator memory (acc_bind), so column 0 is address 0
     const uint32_t ub = base, ut = 0u, ubar = bars;
-    if (tmem != 0u) __trap();
     // slot-0 views of the per-slot buffers (slot 1 = T2_SLOT further)
     const Op2 XD_K = op2_kmajor(ub + S2_XD, T2_ACT), H1_K = op2_kmajor(ub + S2_H1, T2_ACT),
               H2_K = op2_kmajor(ub + S2_H2, T2_ACT);
@@ -347,32 +344,32 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
 #endif
       if (stage == 0) {  // Z1 = X W1^T
         issue_chain3<2>(tz + M2_Z1, I_128_64_KM, op2_at(XD_K, so), W1T_M);
-        umma_commit_elect(bar_chain);
+        acc_commit(bar_chain);
       } else if (stage == 1) {  // Z2 = H1 W2^T
         issue_chain3<4>(tz + M2_ZB, I_128_64_KK, op2_at(H1_K, so), W2_K);
-        umma_commit_elect(bar_chain);
+        acc_commit(bar_chain);
       } else if (stage == 2) {  // OUT = H2 W3^T
         issue_chain3<4>(tz + M2_OUT, I_128_16_KK, op2_at(H2_K, so), W3_K);
-        umma_commit_elect(bar_chain);
+        acc_commit(bar_chain);
       } else if (stage == 3) {
         // dH2 = dOut W3 (A: XD cols 32..47; B: W3 read MN-major, K = output index);
         // dW3^T[i][o] += sum_r H2[r][i] dOut[r][o]  -- must retire before the epilogue turns H2 into dZ2 in place
         issue_chain3<1>(tz + M2_ZB, I_128_64_KM, op2_at(XD_K2, so), W3_M);
         issue_stacked<8, 2>(ut + M2_DW3, I_128_16_MM, acc_dw3, op2_at(H2_M, so), op2_at(XD_M32, so));
         acc_dw3 = true;
-        umma_commit_elect(bar_chain);
+        acc_commit(bar_chain);
       } else if (stage == 4) {
         // dH1 = dZ2 W2 ; dW2[o][i] += sum_r dZ2[r][o] H1[r][i] ; db2[o] += sum_r dZ2[r][o] * 1
         issue_chain3<4>(tz + M2_ZB, I_128_64_KM, op2_at(H2_K, so), W2_M);
         issue_stacked<8, 2>(ut + M2_DW2, I_128_64_MM, acc_dw2, op2_at(H2_M, so), op2_at(H1_M, so));
         issue_stacked<8, 1>(ut + M2_DB2, I_128_16_MM, acc_dw2, op2_at(H2_M, so), op2_at(XD_M32, so));
         acc_dw2 = true;
-        umma_commit_elect(bar_chain);
+        acc_commit(bar_chain);
       } else {
         // dW1[o][i] += sum_r dZ1[r][o] X[r][i] and, through the ones column, db1[o] += sum_r dZ1[r][o]
         issue_stacked<8, 2>(ut + M2_DW1, I_128_48_MM, acc_dw1, op2_at(H1_M, so), op2_at(XD_M0, so));
         acc_dw1 = true;
-        umma_commit_elect(bar_off);
+        acc_commit(bar_off);
       }
       __syncwarp();
 #ifdef B200RL_TC_TIMING
@@ -394,15 +391,15 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
   } else {
     // =============================== epilogue warps: one pool of 16 ===================================
     // Two tiles ("slots") are in flight, but the epilogue warps are NOT bound to a slot: all 16 work on one epilogue
-    // job at a time (16 columns each: 4 warps per TMEM lane quadrant), alternating between the slots in a fixed order
+    // job at a time (16 columns each: 4 warps per accumulator memory lane quadrant), alternating between the slots in a fixed order
     //   (slot 0, E0) (slot 1, E0) (slot 0, E1) (slot 1, E1) ... (slot 1, E5) | next pair of tiles
     // so the MMAs a job hands to the issuer run under the OTHER slot's next job.  (Binding 8 warps to each slot left
     // every epilogue latency bound -- 8 warps cannot fill the SM's issue slots -- and made both slots wait for their
-    // MMAs at the same time; measured 0.45 ms vs this scheme's figure in profiles/.)  The one-row-per-thread loss
+    // MMAs at the same time; measured slower on B200.)  The one-row-per-thread loss
     // job needs only 4 warps; it rotates over the four column groups from tile to tile and the other 12 warps move on.
     const int q = warp & 3, part = warp >> 2;
-    const int r = 32 * q + lane;                          // row of the tile == TMEM lane
-    const uint32_t lane_addr = (uint32_t)(32 * q) << 16;  // this warp's TMEM lane quadrant
+    const int r = 32 * q + lane;                          // row of the tile == accumulator memory lane
+    const uint32_t lane_addr = (uint32_t)(32 * q) << 16;  // this warp's accumulator memory lane quadrant
     const int cs = 16 * part;                             // this warp's 16 columns of a 64-column epilogue
     uint32_t ph_chain0 = 0, ph_chain1 = 0, ph_off0 = 0, ph_off1 = 0;
     bool first0 = true, first1 = true;
@@ -478,22 +475,21 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
         store_chunk2(sm, so + S2_XD, r, part, x);
         arrive();
       } else if (stage == 1 || stage == 2) {
-        // ---- E1 / E2: Z (TMEM) * unscale + bias -> tanh -> [fp32 back to TMEM for tanh'] + fp16 splits ----
+        // ---- E1 / E2: Z (accumulator memory) * unscale + bias -> tanh -> [fp32 back to accumulator memory for tanh'] + fp16 splits ----
         wait_chain();
         const uint32_t tm_col = stage == 1 ? M2_Z1 : M2_ZB;
         const float* bias = stage == 1 ? s_bias : s_bias + 64;
         const float unscale = s_scale[stage == 1 ? SC_U1 : SC_U2];
         const uint32_t dst = so + (stage == 1 ? S2_H1 : S2_H2);
         uint32_t v[16];
-        tmem_ld16(tz + tm_col + cs, v);
-        tmem_wait_ld();
+        acc_ld16(tz + tm_col + cs, v);
         float z[16];
 #pragma unroll
         for (int j = 0; j < 16; ++j) z[j] = fmaf(__uint_as_float(v[j]), unscale, bias[cs + j]);
         tanh16_scaled(z, 1.f);  // |tanh| <= 1, and Z is finite: observations, weights and biases were all checked
 #pragma unroll
         for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(z[j]);
-        if (BACKWARD && stage == 1) t2_tmem_st16(tz + tm_col + cs, v);
+        if (BACKWARD && stage == 1) acc_st16(tz + tm_col + cs, v);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8];
@@ -501,7 +497,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
           for (int j = 0; j < 8; ++j) x[j] = __uint_as_float(v[8 * ch + j]) * sH;
           store_chunk2(sm, dst, r, (cs >> 3) + ch, x);
         }
-        if (BACKWARD && stage == 1) tmem_wait_st();
         arrive();
       } else if (stage == 3) {
         // ---- E3: distribution / loss epilogue, one row per thread, on this tile's loss warps ----
@@ -528,8 +523,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
             if (valid && rm > 0.f && rm < 0.03125f) bad = true;
           }
           uint32_t o[16];
-          tmem_ld16(tz + M2_OUT, o);
-          tmem_wait_ld();
+          acc_ld16(tz + M2_OUT, o);
           float out[16], dout[16];
           const float u3 = s_scale[SC_U3];
 #pragma unroll
@@ -678,8 +672,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
         wait_chain();  // dH2 (and dW3: H2 may be overwritten now)
         const float unscale = s_scale[SC_UH2], hh = pow2i(-2 * T2_H_EXP);
         uint32_t g[16];
-        tmem_ld16(tz + M2_ZB + cs, g);
-        tmem_wait_ld();
+        acc_ld16(tz + M2_ZB + cs, g);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8];
@@ -691,13 +684,12 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
         }
         arrive();
       } else {
-        // ---- E5: dZ1 (scaled) = dH1_acc * 2^-ew2 * (1 - H1^2), H1 kept as fp32 in tensor memory, written over H1 ----
+        // ---- E5: dZ1 (scaled) = dH1_acc * 2^-ew2 * (1 - H1^2), H1 kept as fp32 in accumulator memory, written over H1 ----
         wait_chain();  // dH1 (and dW2 / db2: H1 may be overwritten now)
         const float unscale = s_scale[SC_UH1];
         uint32_t g[16], h[16];
-        tmem_ld16(tz + M2_ZB + cs, g);
-        tmem_ld16(tz + M2_Z1 + cs, h);
-        tmem_wait_ld();
+        acc_ld16(tz + M2_ZB + cs, g);
+        acc_ld16(tz + M2_Z1 + cs, h);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8];
@@ -753,8 +745,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
 #pragma unroll
         for (int cb = 0; cb < 2; ++cb) {
           const int cc = 32 * part + 16 * cb;
-          tmem_ld16(ta + M2_DW2 + cc, v);
-          tmem_wait_ld();
+          acc_ld16(ta + M2_DW2 + cc, v);
           const float u = s_scale[SC_OW2];
           if (m < h2)
 #pragma unroll
@@ -764,8 +755,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
       } else if (part == 2) {  // dW1 [h1 o][n_in i] in cols 0..31, db1 in col 47
 #pragma unroll
         for (int cb = 0; cb < 3; ++cb) {
-          tmem_ld16(ta + M2_DW1 + 16 * cb, v);
-          tmem_wait_ld();
+          acc_ld16(ta + M2_DW1 + 16 * cb, v);
           if (m < h1) {
             if (cb < 2) {
               const float u = s_scale[SC_OW1];
@@ -779,15 +769,13 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
           }
         }
       } else {  // dW3^T [h2 i][16 o] and db2 (col 15 = sum_r dZ2[r][o])
-        tmem_ld16(ta + M2_DW3, v);
-        tmem_wait_ld();
+        acc_ld16(ta + M2_DW3, v);
         const float u = s_scale[SC_OW3];
         if (m < h2)
 #pragma unroll
           for (int a = 0; a < 15; ++a)
             if (a < A_out) dst[p.w_off[2] + a * h2 + m] = __uint_as_float(v[a]) * u;
-        tmem_ld16(ta + M2_DB2, v);
-        tmem_wait_ld();
+        acc_ld16(ta + M2_DB2, v);
         if (m < h2) dst[p.b_off[1] + m] = __uint_as_float(v[15]) * s_scale[SC_OB];
       }
     }
@@ -834,7 +822,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
   tc_fence_before_sync();
   __syncthreads();
   if (tid == 0 && *s_bad != 0) *p.status = p.seq;  // this launch is redone by the bf16 x 3 kernel queued behind it
-  if (warp == T2_EPI_WARPS) tmem_dealloc(tmem, 512);
 }
 
 // max |x| over a device array (pre-pass for the observation / target scale when the caller gave no hint)
@@ -909,7 +896,7 @@ int tc2_take_slot(unsigned** status, unsigned* seq, float** scratch) {
 
 int launch_absmax_cols(const float* x, long long rows, int cols, float* out, cudaStream_t s) {
   if (rows > 0 && cols > 0) {
-    absmax_cols_kernel<<<(int)std::min<long long>((rows + 7) / 8, 4LL * 148), 256, 0, s>>>(x, rows, cols, out);
+    absmax_cols_kernel<<<(int)std::min<long long>((rows + 7) / 8, 4LL * 132), 256, 0, s>>>(x, rows, cols, out);
     B200RL_CUDA(cudaGetLastError());
     count_launch(1);
   }
@@ -980,7 +967,7 @@ int launch_mlp_tc2(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, int total
     if (launch_absmax_cols(a->obs, a->n_rows, k.n_in, scratch, s)) return 1;
   }
   if (need_tgt) {
-    absmax_kernel<<<(int)std::min<long long>((a->n_rows + 255) / 256, 2LL * 148), 256, 0, s>>>(a->target, a->n_rows,
+    absmax_kernel<<<(int)std::min<long long>((a->n_rows + 255) / 256, 2LL * 132), 256, 0, s>>>(a->target, a->n_rows,
                                                                                               scratch + 32);
     ++launches;
   }
@@ -988,6 +975,9 @@ int launch_mlp_tc2(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, int total
   k.target_absmax = need_tgt ? scratch + 32 : a->target_absmax;
   const int grid = tc2_grid(a->n_rows);
   B200RL_REQUIRE(grid > 0, "mlp_tc2: no CUDA device");
+  k.acc_mem = acc_mem(grid, s);
+  B200RL_REQUIRE(k.acc_mem != nullptr, "mlp_tc2: no accumulator memory (allocation failed, or the stream is being captured): %s",
+                 cudaGetErrorString(cudaGetLastError()));
   if (backward)
     mlp_tc2_kernel<true><<<grid, T2_THREADS, T2_SMEM_BYTES, s>>>(k);
   else
@@ -1024,7 +1014,7 @@ extern "C" int b200rl_absmax(const float* x, int64_t n, float* out, void* stream
   B200RL_REQUIRE(x != nullptr && out != nullptr && n >= 0, "absmax: bad argument");
   B200RL_CUDA(cudaMemsetAsync(out, 0, sizeof(float), s));
   if (n > 0) {
-    absmax_kernel<<<(int)std::min<long long>((n + 255) / 256, 2LL * 148), 256, 0, s>>>(x, (long long)n, out);
+    absmax_kernel<<<(int)std::min<long long>((n + 255) / 256, 2LL * 132), 256, 0, s>>>(x, (long long)n, out);
     B200RL_CUDA(cudaGetLastError());
     count_launch(1);
   }

@@ -1,5 +1,5 @@
 // mlp_tc3: ONE kernel per PPO iteration -- the policy step AND the value step over the same 128-row tile of the batch
-// (tcgen05 + TMEM, fp16 x 2 operand splitting as in mlp_tc2.cu; sm_100a only).
+// (wgmma, fp16 x 2 operand splitting as in mlp_tc2.cu; sm_90a).
 //
 // Why (reference: /root/reference/src/rl_replicas/algorithms/ppo.py:173-181 policy loop, :186-192 value loop): the two
 // loops touch disjoint parameters and read the same fixed inputs (advantages and returns are computed before either
@@ -14,7 +14,7 @@
 //   * dLoss/dOut of both chains goes into the X buffer of the OTHER parity (it is idle between the previous tile's
 //     dW1 and the next tile's bulk copy), which is what makes two X buffers fit next to 4 x 32 KB of activations and
 //     2 x 28 KB of weights;
-//   * tanh'(H1) is taken from the fp16 pair in shared memory like tanh'(H2): no fp32 copy of H1 in tensor memory,
+//   * tanh'(H1) is taken from the fp16 pair in shared memory like tanh'(H2): no fp32 copy of H1 in accumulator memory,
 //     which is what makes both chains' accumulators fit (416 of 512 columns);
 //   * one reduction + Adam launch for both networks (reduce_adam3_kernel), one all-reduce per iteration.
 // A range / precision trip (fp16 operands) raises a sticky flag; the engine then restores its snapshot and redoes the
@@ -33,7 +33,7 @@ namespace b200rl {
 constexpr int T3_ROWS = 128;
 constexpr int T3_EPI_WARPS = 16;
 constexpr int T3_EPI_THREADS = T3_EPI_WARPS * 32;
-constexpr int T3_THREADS = T3_EPI_THREADS + 32;
+constexpr int T3_THREADS = T3_EPI_THREADS + 128;  // + the issuing warpgroup
 constexpr float T3_LOG_SQRT_2PI = 0.91893853320467274178f;
 constexpr float T3_ENT_CONST = 1.4189385332046727418f;
 
@@ -49,8 +49,8 @@ constexpr uint32_t S3_BIAS = S3_OPERANDS_END;        // per net: b1[64] b2[64] b
 constexpr uint32_t S3_DIST = S3_BIAS + 2 * 640;      // var[16], log_scale[16], 1/(2 var)[16], 1/var[16]
 constexpr uint32_t S3_SCALE = S3_DIST + 256;         // per net 16 floats
 constexpr uint32_t S3_XS = S3_SCALE + 128;           // 2^ex_k [32], 2^-ex_k [32]
-constexpr uint32_t S3_RED = S3_XS + 256;             // setup reduction scratch [17 warps][8] floats
-constexpr uint32_t S3_BARS = S3_RED + 576;           // ready[2] chain[2] xfull[2] free[2] (8 B each), tmem holder, bad flag
+constexpr uint32_t S3_RED = S3_XS + 256;             // setup reduction scratch [20 warps][8] floats
+constexpr uint32_t S3_BARS = S3_RED + 640;           // ready[2] chain[2] xfull[2] free[2] (8 B each), accumulator base address (acc_bind), bad flag
 constexpr uint32_t S3_TOTAL = S3_BARS + 128;
 constexpr uint32_t T3_SMEM_BYTES = S3_TOTAL + 1024;  // + alignment slack
 static_assert(T3_SMEM_BYTES <= 227 * 1024, "mlp_tc3 shared memory");
@@ -63,7 +63,7 @@ constexpr uint32_t M3_CHAIN = 80, M3_Z = 0, M3_OUT = 64;          // per chain: 
 // per net: DW2 (64) | DB2 (16, col 15 = db2) | DW1 (64: products with X's h columns, then with its l columns; col 31 =
 // db1) | DW3 (32: products with dOut's h columns, then l).  The B operands of dW1 / dW3 hold their two splits side
 // by side in one swizzle atom, so ONE product per k-step covers both; the halves are added when the accumulators
-// are read, once per launch.  2 x 80 + 2 x 176 = 512 columns: all of tensor memory.
+// are read, once per launch.  2 x 80 + 2 x 176 = 512 columns: all of accumulator memory.
 constexpr uint32_t M3_ACC = 160, M3_ACC_NET = 176;
 constexpr uint32_t M3_DW2 = 0, M3_DB2 = 64, M3_DW1 = 80, M3_DW3 = 144;
 
@@ -181,7 +181,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   // Only the weight operands need zero padding (X tiles arrive whole by bulk copy, H and dOut are fully written by
   // their jobs before any MMA reads them).  Both parameter vectors (44 KB) are first brought into the still unused
   // activation buffers with independent, coalesced loads: the two passes below (maxima, then conversion) would
-  // otherwise pay an L2 round trip per element, one after the other -- 17 of the 18 us this set-up used to take.
+  // otherwise pay an L2 round trip per element, one after the other (17 of the 18 us this set-up took on B200).
   for (uint32_t i = S3_W / 16 + tid; i < S3_OPERANDS_END / 16; i += T3_THREADS) reinterpret_cast<uint4*>(sm)[i] = make_uint4(0, 0, 0, 0);
   if (tid == 0) *s_bad = 0;
   if (tid < 64) s_xs[tid] = __ldg(p.xscale + tid);
@@ -312,14 +312,11 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     }
   if (bad) *s_bad = 1;  // non-finite bias
   bad = false;
-  if (warp == T3_EPI_WARPS) {
-    tmem_alloc(smem_u32(s_tmem), 512);
-    tmem_relinquish();
-  }
+  if (tid == 0) acc_bind(p.acc_mem, s_tmem);
   if (tid == 0) {
     for (int c = 0; c < 2; ++c) {
       mbar_init(bars + 8 * c, T3_EPI_THREADS);  // ready[c]: every epilogue thread arrives once per job of chain c
-      mbar_init(bars + 16 + 8 * c, 1);          // chain[c]: tcgen05.commit
+      mbar_init(bars + 16 + 8 * c, 1);          // chain[c]: acc_commit
       mbar_init(bars + 32 + 8 * c, 1);          // xfull[b]: arrive.expect_tx by the MMA warp + the copy's bytes
       mbar_init(bars + 48 + 8 * c, 1);          // (spare)
     }
@@ -335,14 +332,13 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   const long long cta_tiles = (num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;  // tiles blockIdx.x + k * gridDim.x
   const int c_first = run_p ? 0 : 1, c_last = run_v ? 1 : 0;
 
-  if (warp == T3_EPI_WARPS) {
-    // =============================== MMA issuer (and bulk-copy producer) warp =============================
+  if (warp >= T3_EPI_WARPS) {
+    // =============================== MMA issuer (and bulk-copy producer) warpgroup =============================
     constexpr uint32_t I_128_64_KK = make_idesc_f16(128, 64, 0, 0), I_128_16_KK = make_idesc_f16(128, 16, 0, 0),
                        I_128_64_KM = make_idesc_f16(128, 64, 0, 1), I_128_64_MM = make_idesc_f16(128, 64, 1, 1),
                        I_128_32_MM = make_idesc_f16(128, 32, 1, 1), I_128_16_MM = make_idesc_f16(128, 16, 1, 1);
     (void)I_128_16_MM;
     const uint32_t ub = base, ubar = bars;
-    if (tmem != 0u) __trap();  // a 512-column allocation is the whole tensor memory: base 0 (uniform by construction)
     // views at chain 0 / net 0 / X buffer 0; the others are reached by adding byte offsets to the descriptors
     const Op2 X_K = op2_kmajor(ub + S3_XB, 64);                     // A: X, h at +0, l at +64 bytes
     const Op2 X_M = op2_mnmajor(ub + S3_XB, T2_ACT, 64);            // B, N = 64: features h 0..31 (col 31 = ones) | l
@@ -362,7 +358,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
       const long long tile = blockIdx.x + k * gridDim.x;
       uint32_t e;
       asm volatile("{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\tselp.u32 %0, 1, 0, q;\n\t}" : "=r"(e));
-      if (e) {
+      if (e && warp == T3_EPI_WARPS) {  // one thread of the warpgroup
         mbar_arrive_expect_tx(ubar + 32 + 8 * b, T2_ACT);
         bulk_copy_g2s(ub + S3_XB + b * T2_ACT, p.ximg + (size_t)tile * T2_ACT, T2_ACT, ubar + 32 + 8 * b);
       }
@@ -385,7 +381,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
 #pragma unroll 1
       for (int c = c_first; c <= c_last; ++c) {
         issue_z1(c, 0);
-        umma_commit_elect(ubar + 16 + 8 * c);
+        acc_commit(ubar + 16 + 8 * c);
       }
     }
 #pragma unroll 1
@@ -432,7 +428,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
             accmask |= 1u << (3 * c + 2);
             if (k + 1 < cta_tiles) issue_z1(c, k + 1);
           }
-          umma_commit_elect(ubar + 16 + 8 * c);
+          acc_commit(ubar + 16 + 8 * c);
           __syncwarp();
 #ifdef B200RL_TC3_TIMING
           tacc[30 + 2 * (stage - 1) + c] += (unsigned long long)(clock64() - it1);
@@ -451,7 +447,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     // Jobs run in the fixed order (policy, E1) (value, E1) (policy, E2) ... (value, E5) | next tile, all 16 warps on
     // one job at a time (16 columns each), so the MMAs a job hands over run under the other chain's next job.
     const int q = warp & 3, part = warp >> 2;
-    const int r = 32 * q + lane;                          // row of the tile == TMEM lane
+    const int r = 32 * q + lane;                          // row of the tile == accumulator memory lane
     const uint32_t lane_addr = (uint32_t)(32 * q) << 16;
     const int cs = 16 * part;
     uint32_t ph_chain = 0u;  // bit c: phase parity of chain[c]
@@ -505,14 +501,13 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
 #endif
       };
       if (stage == 1 || stage == 2) {
-        // ---- E1 / E2: Z (TMEM) * unscale + bias -> tanh -> fp16 pairs ----
+        // ---- E1 / E2: Z (accumulator memory) * unscale + bias -> tanh -> fp16 pairs ----
         wait_chain();
         const float unscale = scl[stage == 1 ? C3_U1 : C3_U2];
         const float* bs = bias + (stage == 1 ? 0 : 64);
         const uint32_t dst = so + (stage == 1 ? 0u : 2 * T2_ACT);
         uint32_t v[16];
-        tmem_ld16(tz + M3_Z + cs, v);
-        tmem_wait_ld();
+        acc_ld16(tz + M3_Z + cs, v);
         float z[16];
 #pragma unroll
         for (int j = 0; j < 16; ++j) z[j] = fmaf(__uint_as_float(v[j]), unscale, bs[cs + j]);
@@ -549,8 +544,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
           wait_chain();
           if (loss_warp) {
             uint32_t o[16];
-            tmem_ld16(tz + M3_OUT, o);
-            tmem_wait_ld();
+            acc_ld16(tz + M3_OUT, o);
             float out[16], dout[16];
             const float u3 = scl[C3_U3];
 #pragma unroll
@@ -626,8 +620,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
           wait_chain();
           if (loss_warp) {
             uint32_t o[8];
-            tmem_ld8(tz + M3_OUT, o);
-            tmem_wait_ld();
+            acc_ld8(tz + M3_OUT, o);
             if (valid) {  // ppo.py:282-287
               const float vout = fmaf(__uint_as_float(o[0]), scl[C3_U3], bias[128]);
               const float diff = vout - pf_tgt;
@@ -660,7 +653,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
         arrive();
       } else {
         // ---- E4 / E5: dZ (scaled) = dH_acc * unscale * (1 - H^2), H re-read from its fp16 pair, written in place ----
-        // (loading this thread's H chunks BEFORE the wait -- it wrote them itself two jobs ago -- to hide the
+        // (Alternatives measured on B200, before the port to wgmma -- loading this thread's H chunks BEFORE the wait -- it wrote them itself two jobs ago -- to hide the
         // shared-memory latency under the barrier: 0.551 vs 0.525 ms, the 16 extra live registers spill at the 96 cap;
         // a second commit right behind the dH product, so that this job computes while the weight-gradient products
         // still read H and only its stores wait for them, measured 2 % SLOWER: 0.5515 vs 0.540 ms.  With `setmaxnreg`
@@ -674,8 +667,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
         const uint32_t buf = so + (stage == 4 ? 2 * T2_ACT : 0u);
         const float one28 = 268435456.f;
         uint32_t g[16];
-        tmem_ld16(tz + M3_Z + cs, g);
-        tmem_wait_ld();
+        acc_ld16(tz + M3_Z + cs, g);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8];
@@ -740,12 +732,11 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
           const uint32_t col = jb < 4 ? M3_DW2 + 16 * jb : (jb < 6 ? M3_DW1 + 16 * (jb - 4) : (jb == 6 ? M3_DW3 : M3_DB2));
           const uint32_t col2 = jb < 4 ? col : (jb < 6 ? col + 32 : (jb == 6 ? col + 16 : col));
           if (have) {
-            tmem_ld16(tn + col, v);
-            tmem_ld16(tn + col2, w);
-            tmem_wait_ld();
+            acc_ld16(tn + col, v);
+            acc_ld16(tn + col2, w);
           } else {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = w[j] = 0u;  // a CTA without tiles: tensor memory was never written
+            for (int j = 0; j < 16; ++j) v[j] = w[j] = 0u;  // a CTA without tiles: accumulator memory was never written
           }
           if (jb < 4) {  // dW2 [h2 o][h1 i]: columns 16 jb .. +15
             const float u = scl[C3_OW2];
@@ -843,7 +834,6 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   tc_fence_before_sync();
   __syncthreads();
   if (tid == 0 && *s_bad != 0) *p.status = 1.0f;  // sticky: the engine redoes the update on the wide-range path
-  if (warp == T3_EPI_WARPS) tmem_dealloc(tmem, 512);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -857,7 +847,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
 // memory (NVLink / NVSwitch): mode 3 reduces and stores this rank's [gradient | scalars] into its exchange buffer,
 // the last block to finish publishes the sequence number (release, system scope); mode 4 waits for every rank's
 // sequence number (acquire; wait_peers_kernel, one warp), reads ALL ranks' buffers -- its own included -- and adds them in rank order, so every
-// rank applies bit-identical updates, then runs Adam.  22 KB per rank: latency bound, ~2 us per peer read.
+// rank applies bit-identical updates, then runs Adam.  22 KB per rank: latency bound (~2 us per peer read over NVLink on B200).
 // Buffers alternate between two parities: a rank can only be one exchange ahead of its slowest peer (it needs that
 // peer's next sequence number to finish its own), so the buffer it overwrites was read by everybody.
 // mode 5 = modes 3 and 4 in ONE launch (the blocks wait for the sequence numbers themselves): a data-parallel iteration
@@ -865,7 +855,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
 // ------------------------------------------------------------------------------------------------------------------
 constexpr int RA3_WARPS = 8;
 
-// One float from every rank's exchange buffer.  The loads are issued back to back (a peer read over NVLink is ~2 us:
+// One float from every rank's exchange buffer.  The loads are issued back to back (a peer read over NVLink took ~2 us on B200:
 // a loop with one load per trip would pay that once per rank) and added in rank order, the same sum on every rank.
 template <typename Acc>
 __device__ __forceinline__ Acc ra3_gather(float* const* peers, int world, long long offset) {
@@ -1076,7 +1066,7 @@ int launch_pack_obs(const float* obs, int64_t n_rows, int n_in, const float* abs
                     float* bad_flag, cudaStream_t s) {
   const int64_t tiles = (n_rows + T3_ROWS - 1) / T3_ROWS;
   if (tiles <= 0) return 0;
-  const int grid = (int)std::min<int64_t>(tiles, 8LL * 148);
+  const int grid = (int)std::min<int64_t>(tiles, 8LL * 132);
   pack_obs_kernel<<<grid, 128, 0, s>>>(obs, n_rows, n_in, absmax, ximg, xscale, bad_flag);
   B200RL_CUDA(cudaGetLastError());
   count_launch(1);
@@ -1087,7 +1077,11 @@ int launch_mlp_tc3(const Tc3Args& k, cudaStream_t s) {
   if (tc3_configure()) return 1;
   const int grid = tc3_grid(k.n_rows);
   B200RL_REQUIRE(grid > 0, "mlp_tc3: no CUDA device");
-  mlp_tc3_kernel<<<grid, T3_THREADS, T3_SMEM_BYTES, s>>>(k);
+  Tc3Args kk = k;
+  kk.acc_mem = acc_mem(grid, s);
+  B200RL_REQUIRE(kk.acc_mem != nullptr, "mlp_tc3: no accumulator memory (allocation failed, or the stream is being captured): %s",
+                 cudaGetErrorString(cudaGetLastError()));
+  mlp_tc3_kernel<<<grid, T3_THREADS, T3_SMEM_BYTES, s>>>(kk);
   B200RL_CUDA(cudaGetLastError());
   count_launch(1);
   return 0;

@@ -1,4 +1,4 @@
-// mlp_tc_fvp: TRPO's Fisher-vector product on the tensor cores (tcgen05 + TMEM, sm_100a only).
+// mlp_tc_fvp: TRPO's Fisher-vector product on the tensor cores (wgmma, sm_90a).
 //
 // Contract of B200RL_LOSS_FVP (see mlp_fused.cu, MODE 2, for the reference map: conjugate_gradient_optimizer.py:133-167
 // double-backprops mean KL(old || new); at theta = theta_old that Hessian is the Fisher matrix (1/N) J^T M J):
@@ -13,7 +13,7 @@
 // weights V need the shared memory the second slot uses there.
 // Scales of the tangent operands come from bounds, not typical values (the direction's magnitude changes from one CG
 // iteration to the next): |T1| <= n_in max|X| max|V1| + max|vb1| and so on; two products that accumulate into one
-// TMEM region (T1 W2^T + H1 V2^T) must share ONE scale, so the pair (scale of T1, scale of V2) is chosen with
+// accumulator memory region (T1 W2^T + H1 V2^T) must share ONE scale, so the pair (scale of T1, scale of V2) is chosen with
 // e_T1 + e_W2 = 14 + e_V2 and both inside their ranges.
 #include <cuda_fp16.h>
 
@@ -26,9 +26,9 @@
 namespace b200rl {
 
 constexpr int FV_ROWS = 128;
-constexpr int FV_EPI_WARPS = 16;  // 4 lane groups x 4 column groups of 16 (8 warps with 32 columns each: 0.59 ms per F v)
+constexpr int FV_EPI_WARPS = 16;  // 4 lane groups x 4 column groups of 16 (8 warps with 32 columns each measured slower on B200)
 constexpr int FV_EPI_THREADS = FV_EPI_WARPS * 32;
-constexpr int FV_THREADS = FV_EPI_THREADS + 32;
+constexpr int FV_THREADS = FV_EPI_THREADS + 128;  // + the issuing warpgroup
 
 // shared-memory map (bytes from the 1024-aligned base)
 constexpr uint32_t FV_W1T = 32 * 128, FV_W = 64 * 128, FV_W3 = 16 * 128;  // one split each
@@ -43,8 +43,8 @@ constexpr uint32_t SF_OPERANDS_END = SF_V3 + 2 * FV_W3;
 constexpr uint32_t SF_BIAS = SF_OPERANDS_END;   // b1[64] b2[64] b3[16] | vb1[64] vb2[64] vb3[16] floats
 constexpr uint32_t SF_DIST = SF_BIAS + 1152;    // 1/var[16] floats
 constexpr uint32_t SF_SCALE = SF_DIST + 64;     // scale factors
-constexpr uint32_t SF_RED = SF_SCALE + 128;     // block reduction scratch [17 warps][8] floats (read-out: [4][16] + 4 + 4)
-constexpr uint32_t SF_BARS = SF_RED + 576;      // mbarriers ready, chain, off; tmem holder; bad flag
+constexpr uint32_t SF_RED = SF_SCALE + 128;     // block reduction scratch [20 warps][8] floats (read-out: [4][16] + 4 + 4)
+constexpr uint32_t SF_BARS = SF_RED + 640;      // mbarriers ready, chain, off; accumulator base address (acc_bind); bad flag
 constexpr uint32_t SF_XS = SF_BARS + 64;        // per-feature observation scales [32] and inverses [32]
 constexpr uint32_t SF_ROWMAX = SF_XS + 256;     // [128] largest scaled |obs| of each row (precision guard)
 constexpr uint32_t SF_TOTAL = SF_ROWMAX + 512;
@@ -77,6 +77,7 @@ struct FvpArgs {
   unsigned* status;
   unsigned seq;
   int total_rows;  // partial rows the consumer reduces (>= 2 * gridDim.x); the surplus is zeroed
+  float* acc_mem;  // accumulator memory, ACC_CTA_FLOATS per CTA (tc_common.cuh)
 };
 
 __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs p) {
@@ -233,10 +234,7 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
   }
   if (bad) *s_bad = 1;  // non-finite bias
   bad = false;
-  if (warp == FV_EPI_WARPS) {
-    tmem_alloc(smem_u32(s_tmem), 512);
-    tmem_relinquish();
-  }
+  if (tid == 0) acc_bind(p.acc_mem, s_tmem);
   if (tid == 0) {
     mbar_init(bars, FV_EPI_THREADS);
     mbar_init(bars + 8, 1);
@@ -251,13 +249,12 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
   const long long num_tiles = (p.n_rows + FV_ROWS - 1) / FV_ROWS;
   const long long cta_tiles = (num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;
 
-  if (warp == FV_EPI_WARPS) {
+  if (warp >= FV_EPI_WARPS) {
     // =============================== MMA issuer warp =================================================
     constexpr uint32_t I_128_64_KK = make_idesc_f16(128, 64, 0, 0), I_128_16_KK = make_idesc_f16(128, 16, 0, 0),
                        I_128_64_KM = make_idesc_f16(128, 64, 0, 1), I_128_64_MM = make_idesc_f16(128, 64, 1, 1),
                        I_128_48_MM = make_idesc_f16(128, 48, 1, 1), I_128_16_MM = make_idesc_f16(128, 16, 1, 1);
-    const uint32_t ub = base, ut = 0u;  // a 512-column allocation is the whole tensor memory: base 0
-    if (tmem != 0u) __trap();
+    const uint32_t ub = base, ut = 0u;  // accumulator address of column 0 of this CTA's block (acc_bind)
     const Op2 XD_K = op2_kmajor(ub + SF_XD, T2_ACT), H1_K = op2_kmajor(ub + SF_H1, T2_ACT),
               H2_K = op2_kmajor(ub + SF_H2, T2_ACT), T1_K = op2_kmajor(ub + SF_T1, T2_ACT),
               T2_K = op2_kmajor(ub + SF_T2, T2_ACT), XD_K2 = op2_kmajor(ub + SF_XD + 64, T2_ACT);
@@ -279,29 +276,29 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
         if (stage == 0) {  // Z1 = X W1^T ; TZ = X V1^T
           issue_chain3<2>(ut + MF_Z1, I_128_64_KM, XD_K, W1T_M);
           issue_chain3<2>(ut + MF_TZ, I_128_64_KM, XD_K, V1T_M);
-          umma_commit_elect(bars + 8);
+          acc_commit(bars + 8);
         } else if (stage == 1) {  // Z2 = H1 W2^T ; TZ = T1 W2^T + H1 V2^T
           issue_chain3<4>(ut + MF_ZB, I_128_64_KK, H1_K, W2_K);
           issue_chain3<4>(ut + MF_TZ, I_128_64_KK, T1_K, W2_K);
           issue_chain3<4, true>(ut + MF_TZ, I_128_64_KK, H1_K, V2_K);
-          umma_commit_elect(bars + 8);
+          acc_commit(bars + 8);
         } else if (stage == 2) {  // OUT = H2 W3^T ; TOUT = T2 W3^T + H2 V3^T
           issue_chain3<4>(ut + MF_OUT, I_128_16_KK, H2_K, W3_K);
           issue_chain3<4>(ut + MF_TOUT, I_128_16_KK, T2_K, W3_K);
           issue_chain3<4, true>(ut + MF_TOUT, I_128_16_KK, H2_K, V3_K);
-          umma_commit_elect(bars + 8);
+          acc_commit(bars + 8);
         } else if (stage == 3) {  // dH2 = dOut W3 ; dW3^T += H2^T dOut (must retire before H2 becomes dZ2)
           issue_chain3<1>(ut + MF_ZB, I_128_64_KM, XD_K2, W3_M);
           issue_stacked<8, 2>(ut + MF_DW3, I_128_16_MM, acc, H2_M, XD_M32);
-          umma_commit_elect(bars + 8);
+          acc_commit(bars + 8);
         } else if (stage == 4) {  // dH1 = dZ2 W2 ; dW2 += dZ2^T H1 ; db2 += dZ2^T 1
           issue_chain3<4>(ut + MF_ZB, I_128_64_KM, H2_K, W2_M);
           issue_stacked<8, 2>(ut + MF_DW2, I_128_64_MM, acc, H2_M, H1_M);
           issue_stacked<8, 1>(ut + MF_DB2, I_128_16_MM, acc, H2_M, XD_M32);
-          umma_commit_elect(bars + 8);
+          acc_commit(bars + 8);
         } else {  // dW1 += dZ1^T X, db1 through the ones column
           issue_stacked<8, 2>(ut + MF_DW1, I_128_48_MM, acc, H1_M, XD_M0);
-          umma_commit_elect(bars + 16);
+          acc_commit(bars + 16);
           acc = true;
         }
         __syncwarp();
@@ -333,22 +330,21 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
       ph_chain ^= 1u;
       tc_fence_after_sync();
     };
-    // forward + tangent epilogue of a tanh layer: H = tanh(Z u + b) -> fp16 splits (and fp32 to TMEM when kept);
+    // forward + tangent epilogue of a tanh layer: H = tanh(Z u + b) -> fp16 splits (and fp32 to accumulator memory when kept);
     // T = (1 - H^2) (TZ ut + vb) -> fp16 splits of the tangent buffer
     auto layer_epilogue = [&](uint32_t tm_z, const float* bias, const float* vbias, float unscale, float unscale_t,
                               float t_scale, uint32_t dst_h, uint32_t dst_t, bool keep_fp32) {
       {
         uint32_t v[16], w[16];
-        tmem_ld16(tz + tm_z + cs, v);
-        tmem_ld16(tz + MF_TZ + cs, w);
-        tmem_wait_ld();
+        acc_ld16(tz + tm_z + cs, v);
+        acc_ld16(tz + MF_TZ + cs, w);
         float z[16];
 #pragma unroll
         for (int j = 0; j < 16; ++j) z[j] = fmaf(__uint_as_float(v[j]), unscale, bias[cs + j]);
         tanh16_scaled(z, 1.f);  // Z is finite: observations, weights and biases were all checked
 #pragma unroll
         for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(z[j]);
-        if (keep_fp32) t2_tmem_st16(tz + tm_z + cs, v);
+        if (keep_fp32) acc_st16(tz + tm_z + cs, v);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8], t[8];
@@ -363,7 +359,6 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
           store_chunk2(sm, dst_t, r, (cs >> 3) + ch, t);
         }
       }
-      if (keep_fp32) tmem_wait_st();
     };
 
     bool first = true;
@@ -411,9 +406,8 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
           if (valid && rm > 0.f && rm < 0.03125f) bad = true;
         }
         uint32_t o[16], t[16];
-        tmem_ld16(tz + MF_OUT, o);
-        tmem_ld16(tz + MF_TOUT, t);
-        tmem_wait_ld();
+        acc_ld16(tz + MF_OUT, o);
+        acc_ld16(tz + MF_TOUT, t);
         float dout[16];
 #pragma unroll
         for (int a = 0; a < 16; ++a) dout[a] = 0.f;
@@ -489,8 +483,7 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
         const float unscale = s_scale[FS_UH2], hh = pow2i(-2 * T2_H_EXP);
         {
           uint32_t g[16];
-          tmem_ld16(tz + MF_ZB + cs, g);
-          tmem_wait_ld();
+          acc_ld16(tz + MF_ZB + cs, g);
 #pragma unroll
           for (int ch = 0; ch < 2; ++ch) {
             float x[8];
@@ -509,9 +502,8 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
         const float unscale = s_scale[FS_UH1];
         {
           uint32_t g[16], h[16];
-          tmem_ld16(tz + MF_ZB + cs, g);
-          tmem_ld16(tz + MF_Z1 + cs, h);
-          tmem_wait_ld();
+          acc_ld16(tz + MF_ZB + cs, g);
+          acc_ld16(tz + MF_Z1 + cs, h);
 #pragma unroll
           for (int ch = 0; ch < 2; ++ch) {
             float x[8];
@@ -542,8 +534,7 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
 #pragma unroll
         for (int c2 = 0; c2 < 2; ++c2) {
           const int cb = 2 * half + c2;
-          tmem_ld16(tz + MF_DW2 + 16 * cb, v);
-          tmem_wait_ld();
+          acc_ld16(tz + MF_DW2 + 16 * cb, v);
           const float u = s_scale[FS_OW2];
           if (m < h2)
 #pragma unroll
@@ -553,8 +544,7 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
       } else if (half == 2) {
 #pragma unroll
         for (int cb = 0; cb < 3; ++cb) {
-          tmem_ld16(tz + MF_DW1 + 16 * cb, v);
-          tmem_wait_ld();
+          acc_ld16(tz + MF_DW1 + 16 * cb, v);
           if (m < h1) {
             if (cb < 2) {
               const float u = s_scale[FS_OW1];
@@ -568,15 +558,13 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
           }
         }
       } else {
-        tmem_ld16(tz + MF_DW3, v);
-        tmem_wait_ld();
+        acc_ld16(tz + MF_DW3, v);
         const float u = s_scale[FS_OW3];
         if (m < h2)
 #pragma unroll
           for (int a = 0; a < 15; ++a)
             if (a < A_out) dst[p.w_off[2] + a * h2 + m] = __uint_as_float(v[a]) * u;
-        tmem_ld16(tz + MF_DB2, v);
-        tmem_wait_ld();
+        acc_ld16(tz + MF_DB2, v);
         if (m < h2) dst[p.b_off[1] + m] = __uint_as_float(v[15]) * s_scale[FS_OB];
       }
       if (half == 0) {
@@ -611,7 +599,6 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
   tc_fence_before_sync();
   __syncthreads();
   if (tid == 0 && *s_bad != 0) *p.status = p.seq;  // redone by the fp32 kernel queued behind this launch
-  if (warp == FV_EPI_WARPS) tmem_dealloc(tmem, 512);
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------
@@ -667,6 +654,9 @@ int launch_mlp_tc_fvp(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, int to
   }
   const int grid = tc2_grid(a->n_rows);
   B200RL_REQUIRE(grid > 0, "mlp_tc_fvp: no CUDA device");
+  k.acc_mem = acc_mem(grid, s);
+  B200RL_REQUIRE(k.acc_mem != nullptr, "mlp_tc_fvp: no accumulator memory (allocation failed, or the stream is being captured): %s",
+                 cudaGetErrorString(cudaGetLastError()));
   mlp_tc_fvp_kernel<<<grid, FV_THREADS, FV_SMEM_BYTES, s>>>(k);
   B200RL_CUDA(cudaGetLastError());
   count_launch(1);

@@ -275,7 +275,7 @@ __global__ void polyak_kernel(const PolyakArgs a, float rho, float one_minus_rho
 
 // ---------------------------------------------------------------------------------------------------------------
 // The persistent step kernel.  A train() call of S steps is ~46 S small dependent kernels; even replayed as a CUDA
-// graph each costs a launch-to-launch gap (~200 us per TD3 step at B = 256).  Here the SAME tile code runs as ONE
+// graph each costs a launch-to-launch gap (~200 us per TD3 step at B = 256, measured on B200).  Here the SAME tile code runs as ONE
 // cooperative launch: the host compiles the S steps into a program of ops grouped into PHASES (ops of a phase are
 // independent: the four critics' forward passes of a layer, dW and dX of a layer, ...), every CTA walks the phases,
 // takes virtual blocks `blockIdx.x, + gridDim.x, ...` of the phase's ops, and a grid barrier separates phases (~18 per
@@ -1209,7 +1209,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   B200RL_CUDA(cudaMemcpyAsync(h->adam_tab, h->h_adam_tab, 3 * (size_t)maxS * sizeof(float2), cudaMemcpyHostToDevice, s));
 
   int n_pol = 0;
-  // opt-in: measured 12.1 ms per 50 TD3 steps against 11.1 ms for the graph replay (B = 256, 256-wide nets) -- the
+  // opt-in: on B200 it measured 12.1 ms per 50 TD3 steps against 11.1 ms for the graph replay (B = 256, 256-wide nets) -- the
   // 32 x 32 fp32 tiles themselves, two per SM in the phases that merge four networks, are the cost, not the launches
   const char* menv = getenv("B200RL_OFFPOLICY_MEGAKERNEL");
   const bool use_mega = menv != nullptr && menv[0] == '1';

@@ -33,6 +33,7 @@ struct Tc3Args {
   const float* x_bad;         // raised (1.0f) by pack_obs_kernel: observations outside the fp16 range
   float* status;              // raised (1.0f) by this kernel on a range trip (floats: the flags ride an all-reduce)
   int run_policy, run_value;  // host-known: iteration index below the loop lengths
+  float* acc_mem;             // accumulator memory, ACC_CTA_FLOATS per CTA (tc_common.cuh)
 };
 
 struct Ra3Seg {

@@ -1,5 +1,17 @@
-// Hand-written sm_100a primitives: tcgen05 (MMA / TMEM ld-st / alloc / commit / fences), mbarrier, proxy fences.
-// PTX spellings follow the CUDA 12.9 ISA (cross-checked against the CUTLASS sm100 headers vendored in the image).
+// Hand-written sm_90a primitives of the tensor-core kernels: warpgroup MMA (wgmma) on shared-memory descriptors,
+// the per-CTA accumulator memory the kernels address by (lane, column), mbarrier and proxy fences.
+// PTX spellings follow the CUDA 12.9 ISA.
+//
+// Work split.  The epilogue warps of a kernel hold one row of a 128-row tile per thread and read or write
+// accumulators as (lane = row, column) pairs; one warpgroup (four warps) issues the products.  A product
+// D[M x N] (+)= sum_t A_t B_t runs as wgmma m64nNk16 over each 64-row half of M, with the accumulator fragment in the
+// issuing warpgroup's registers: it is loaded from the accumulator memory when the product accumulates, and stored
+// back when the product is done.  The issuing warpgroup then arrives once on the stage's mbarrier (acc_commit).
+//
+// Accumulator memory.  An H100 SM has 227 KB of shared memory for a block and the kernels' operand buffers fill most
+// of it, so the fp32 accumulators (up to 512 columns x 128 lanes = 256 KB per CTA) live in a per-launch global buffer
+// of gridDim.x such blocks, column-major (a warp reading one column of its 32 lanes touches one 128-byte line).  It is
+// written and read back by the same CTA within a tile's stages, so it stays in the 50 MB L2.
 #pragma once
 #include <cstdint>
 
@@ -39,153 +51,248 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   __trap();
 }
 
-// ---- proxy / tcgen05 fences -----------------------------------------------------------------------------------
+// ---- proxy fences ----------------------------------------------------------------------------------------------
+// generic-proxy shared-memory writes (operand buffers) -> visible to wgmma, which reads through the async proxy
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// accumulator memory is ordinary global memory: the mbarrier arrive / wait pairs (release / acquire) order it; these
+// mark the hand-over points for the compiler
+__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("" ::: "memory"); }
+__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("" ::: "memory"); }
 
-// ---- TMEM allocation (one full warp, .sync.aligned) -------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
+// ---- accumulator memory ----------------------------------------------------------------------------------------
+constexpr uint32_t ACC_COLS = 512, ACC_LANES = 128;
+constexpr size_t ACC_CTA_FLOATS = (size_t)ACC_COLS * ACC_LANES;
 
-// ---- MMA: D[tmem] (+)= A[smem desc] * B[smem desc], kind::tf32, issued by ONE thread -----------------------------
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same with kind::f16 (fp16 / bf16 operands selected by the instruction descriptor, fp32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Warp-convergent variants: the whole warp executes the call with warp-uniform operands and ONE lane, chosen by
-// elect.sync, issues the instruction.  Keeping the issuing warp convergent lets ptxas hold the descriptors in uniform
-// registers; issuing from inside a divergent `if (lane == 0)` region forces every descriptor through R2UR.
-__device__ __forceinline__ void umma_f16_elect(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p, e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same, descriptors passed as (lo, hi) 32-bit halves so that per-k-step advances are plain 32-bit adds on `lo`
-__device__ __forceinline__ void umma_f16_elect2(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo,
-                                                uint32_t b_hi, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p, e;\n\t"
-      ".reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t"
-      "}"
-      :
-      : "r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_elect(uint32_t bar) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t"
-      "}" ::"r"(bar)
-      : "memory");
-}
-// all previously issued MMAs of this thread arrive (once) on the mbarrier when they have completed;
-// implies tcgen05.fence::before_thread_sync
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
+static __shared__ float* s_acc_cta;  // this CTA's block of the launch's accumulator memory
 
-// ---- TMEM <-> registers: 32 lanes x 32-bit, N consecutive columns per thread (thread = lane = row) ---------------
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr)
-               : "memory");
+// one thread, before the block's first __syncthreads: binds the CTA's block and writes accumulator address 0 (lane 0,
+// column 0) into `holder`.  Addresses are (lane << 16) | column, as the kernels compute them.
+__device__ __forceinline__ void acc_bind(float* acc_mem, uint32_t* holder) {
+  s_acc_cta = acc_mem + (size_t)blockIdx.x * ACC_CTA_FLOATS;
+  *holder = 0u;
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
+__device__ __forceinline__ float* acc_ptr(uint32_t taddr) {  // this thread's lane of the warp at `taddr`
+  return s_acc_cta + (taddr & 0xFFFFu) * ACC_LANES + (taddr >> 16) + (threadIdx.x & 31u);
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
-      "%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
+// N consecutive columns of one lane per thread (thread i of the warp = lane (taddr >> 16) + i)
+template <int N>
+__device__ __forceinline__ void acc_ld(uint32_t taddr, uint32_t (&v)[N]) {
+  const float* p = acc_ptr(taddr);
+#pragma unroll
+  for (int j = 0; j < N; ++j) v[j] = __float_as_uint(p[j * ACC_LANES]);
 }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_zero8(uint32_t taddr) {
-  const uint32_t z = 0;
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%1,%1,%1,%1,%1,%1,%1};" ::"r"(taddr), "r"(z)
-               : "memory");
+template <int N>
+__device__ __forceinline__ void acc_st(uint32_t taddr, const uint32_t (&v)[N]) {
+  float* p = acc_ptr(taddr);
+#pragma unroll
+  for (int j = 0; j < N; ++j) p[j * ACC_LANES] = __uint_as_float(v[j]);
+}
+__device__ __forceinline__ void acc_ld8(uint32_t taddr, uint32_t (&v)[8]) { acc_ld<8>(taddr, v); }
+__device__ __forceinline__ void acc_ld16(uint32_t taddr, uint32_t (&v)[16]) { acc_ld<16>(taddr, v); }
+__device__ __forceinline__ void acc_ld32(uint32_t taddr, uint32_t (&v)[32]) { acc_ld<32>(taddr, v); }
+__device__ __forceinline__ void acc_st16(uint32_t taddr, const uint32_t (&v)[16]) { acc_st<16>(taddr, v); }
+__device__ __forceinline__ void acc_st32(uint32_t taddr, const uint32_t (&v)[32]) { acc_st<32>(taddr, v); }
+
+// The issuing warpgroup's products are complete and stored: one arrive on `bar` (count 1) for the whole warpgroup.
+// Named barrier 8 is reserved for the issuing warpgroup (the epilogue warps use 1..3).
+__device__ __forceinline__ void acc_commit(uint32_t bar) {
+  __threadfence_block();
+  asm volatile("bar.sync 8, 128;" ::: "memory");
+  if ((threadIdx.x & 127u) == 0) mbar_arrive(bar);
 }
 
 // ---- descriptors ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (tcgen05 "version 1"), SWIZZLE_128B:
+// Shared-memory matrix descriptor (wgmma), SWIZZLE_128B:
 //   [0,14) start address >> 4   [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4
-//   [46,48) version = 1         [49,52) base offset = 0            [61,64) layout type (2 = SWIZZLE_128B)
+//   [49,52) base offset = 0     [62,64) layout type (1 = SWIZZLE_128B)
+// K-major: 128-byte rows, 8-row groups `sbo` = 1024 bytes apart.  MN-major: `lbo` = distance between 64-element
+// atoms along M / N, `sbo` = distance between 8-row groups along K.
 __host__ __device__ constexpr uint64_t make_smem_desc_sw128(uint32_t addr_bytes, uint32_t lbo_bytes,
                                                             uint32_t sbo_bytes) {
   return (uint64_t)((addr_bytes >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 46) | (2ull << 61);
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 62);
 }
-// Instruction descriptor, kind::tf32, fp32 accumulate:
-//   [4,6) D format (1 = f32)  [7,10) A format (2 = tf32)  [10,13) B format (2 = tf32)
-//   [15] A major (0 = K, 1 = MN)  [16] B major  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// Instruction descriptor, kind::f16 with bf16 operands (format 1), fp32 accumulate; same field positions.
+// Product descriptor: what mma_product needs to pick the wgmma shape, operand types and majors.
+//   [7,10) operand type (0 = fp16, 1 = bf16)  [15] A major (0 = K, 1 = MN)  [16] B major  [17,23) N >> 3
+//   [24,29) M >> 4 (128: two 64-row halves; 64: one, stored to lanes (m % 16) + 32 (m / 16))
 __host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
   return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
          ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+}
+__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, int a_mn_major, int b_mn_major) {
+  return (1u << 4) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) |
+         ((uint32_t)(M >> 4) << 24);
+}
+
+// ---- wgmma -----------------------------------------------------------------------------------------------------
+// D[64 x N] (+)= A[64 x 16] B[16 x N], fp32 accumulate in registers; TA / TB: operand read MN-major (transposed).
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_f16_n16(float (&d)[8], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
+      : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_f16_n32(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
+      : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_f16_n48(float (&d)[24], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, %27, %28;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
+      : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
+      : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_n16(float (&d)[8], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
+      : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_n32(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
+      : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_n48(float (&d)[24], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, %27, %28;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
+      : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
+      : "memory");
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+template <int N, bool BF16, int TA, int TB>
+__device__ __forceinline__ void wgmma_run(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
+  if constexpr (BF16) {
+    if constexpr (N == 16) wgmma_bf16_n16<TA, TB>(d, a, b, scale_d);
+    else if constexpr (N == 32) wgmma_bf16_n32<TA, TB>(d, a, b, scale_d);
+    else if constexpr (N == 48) wgmma_bf16_n48<TA, TB>(d, a, b, scale_d);
+    else wgmma_bf16_n64<TA, TB>(d, a, b, scale_d);
+  } else {
+    if constexpr (N == 16) wgmma_f16_n16<TA, TB>(d, a, b, scale_d);
+    else if constexpr (N == 32) wgmma_f16_n32<TA, TB>(d, a, b, scale_d);
+    else if constexpr (N == 48) wgmma_f16_n48<TA, TB>(d, a, b, scale_d);
+    else wgmma_f16_n64<TA, TB>(d, a, b, scale_d);
+  }
+}
+
+// D (+)= sum over `terms` of A_t B_t, each `ksteps` k-steps of 16 (descriptor low words advance by a_k / b_k per
+// k-step; the high words are shared).  Executed by all 128 threads of the issuing warpgroup.  `a_half` advances A's
+// low word to rows 64..127 when M = 128.
+template <int N, bool BF16, int TA, int TB, int T>
+__device__ __forceinline__ void mma_terms(uint32_t d_col, bool m64, const uint32_t (&alo)[T], const uint32_t (&blo)[T],
+                                          int terms, uint32_t a_hi, uint32_t b_hi, uint32_t a_k, uint32_t b_k,
+                                          int ksteps, bool acc_first, uint32_t a_half) {
+  const int t = (int)(threadIdx.x & 127u), w = t >> 5, l = t & 31;
+  float* acc = s_acc_cta + d_col * ACC_LANES;
+#pragma unroll 1
+  for (int h = 0; h < (m64 ? 1 : 2); ++h) {
+    // fragment rows of this thread: m0 and m0 + 8 (wgmma D layout); M = 64 results go to lanes (m % 16) + 32 (m / 16)
+    const int m0 = 16 * w + (l >> 2) + 64 * h;
+    const int lane0 = m64 ? (m0 & 15) + 32 * (m0 >> 4) : m0;
+    float d[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) {
+      const int col = 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
+      d[i] = acc_first ? acc[col * ACC_LANES + lane0 + 8 * ((i >> 1) & 1)] : 0.f;
+    }
+    wgmma_fence();
+    uint32_t scale = acc_first ? 1u : 0u;
+#pragma unroll
+    for (int s = 0; s < T; ++s) {
+      if (s >= terms) break;
+      uint32_t a = alo[s] + (uint32_t)h * a_half, b = blo[s];
+#pragma unroll 1
+      for (int k = 0; k < ksteps; ++k) {
+        wgmma_run<N, BF16, TA, TB>(d, ((uint64_t)a_hi << 32) | a, ((uint64_t)b_hi << 32) | b, scale);
+        scale = 1u;
+        a += a_k;
+        b += b_k;
+      }
+    }
+    wgmma_commit();
+    wgmma_wait_all();
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) {
+      const int col = 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
+      acc[col * ACC_LANES + lane0 + 8 * ((i >> 1) & 1)] = d[i];
+    }
+  }
+}
+
+// Shape / type / majors come from the product descriptor (a compile-time constant at every call site).
+template <int T>
+__device__ __forceinline__ void mma_product(uint32_t d_tmem, uint32_t idesc, const uint32_t (&alo)[T],
+                                            const uint32_t (&blo)[T], int terms, uint32_t a_hi, uint32_t b_hi,
+                                            uint32_t a_k, uint32_t b_k, int ksteps, bool acc_first) {
+  const uint32_t N = ((idesc >> 17) & 63u) << 3, M = ((idesc >> 24) & 31u) << 4;
+  const uint32_t a_mn = (idesc >> 15) & 1u, b_mn = (idesc >> 16) & 1u, bf16 = (idesc >> 7) & 7u;
+  const uint32_t d_col = d_tmem & 0xFFFFu;
+  const bool m64 = M == 64;
+  // rows 64..127 of A: the next 64-element atom (MN-major: one leading byte offset further) or 64 rows of 128 bytes
+  const uint32_t a_half = a_mn ? ((alo[0] >> 16) & 0x3FFFu) : (64u * 128u) >> 4;
+#define B200RL_MMA_CASE(NN, BF, TA, TB)                                                                       \
+  if (N == NN && bf16 == BF && a_mn == TA && b_mn == TB) {                                                    \
+    mma_terms<NN, BF, TA, TB>(d_col, m64, alo, blo, terms, a_hi, b_hi, a_k, b_k, ksteps, acc_first, a_half); \
+    return;                                                                                                   \
+  }
+#define B200RL_MMA_CASES(NN, BF) \
+  B200RL_MMA_CASE(NN, BF, 0, 0)  \
+  B200RL_MMA_CASE(NN, BF, 0, 1)  \
+  B200RL_MMA_CASE(NN, BF, 1, 1)
+  B200RL_MMA_CASES(64, 0)
+  B200RL_MMA_CASES(48, 0)
+  B200RL_MMA_CASES(32, 0)
+  B200RL_MMA_CASES(16, 0)
+  B200RL_MMA_CASES(64, 1)
+  B200RL_MMA_CASES(48, 1)
+  B200RL_MMA_CASES(32, 1)
+  B200RL_MMA_CASES(16, 1)
+#undef B200RL_MMA_CASES
+#undef B200RL_MMA_CASE
+  __trap();  // a shape no kernel uses
 }
 
 }  // namespace b200rl

@@ -36,7 +36,7 @@ class _CudaArray:
 def current_stream_handle() -> int:
     import torch
     if not torch.cuda.is_available():
-        raise _lib.B200RLError("no CUDA device: the B200 update engine has no CPU fallback")
+        raise _lib.B200RLError("no CUDA device: the update engine has no CPU fallback")
     return int(torch.cuda.current_stream().cuda_stream)
 
 

@@ -135,5 +135,5 @@ class NativeClosure:
 
     def __call__(self):
         raise NotImplementedError(
-            f"the TRPO {self.what} closure of rl_replicas_b200 is evaluated inside the B200 engine; only "
+            f"the TRPO {self.what} closure of rl_replicas_b200 is evaluated inside the GPU engine; only "
             "ConjugateGradientOptimizer.step can consume it")

@@ -1,6 +1,6 @@
 """Per-kernel totals of an `ncu --metrics gpu__time_duration.sum --csv` launch list.
 
-    python tools/launch_summary.py profiles/r02_launches_final.csv
+    python tools/launch_summary.py launches.csv
 """
 import csv
 import re

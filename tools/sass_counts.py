@@ -1,4 +1,4 @@
-"""Mnemonic counts per kernel of libb200rl.so (the table of profiles/r02_sass_evidence.md).
+"""Mnemonic counts per kernel of libb200rl.so.
 
     python tools/sass_counts.py [path/to/libb200rl.so]
 """

@@ -37,6 +37,11 @@ int device_sm_count();
 
 // accumulator memory of the tensor-core kernels (tc_common.cuh) for a launch of `grid` CTAs on stream `s`
 float* acc_mem(int grid, cudaStream_t s);
+// grid of a tensor-core kernel: one CTA per 128-row tile, at most one per SM (-1: no device)
+int tc_grid(int64_t n_rows);
+// offsets of the weights and biases of a 3-Linear-layer network in its flat parameter vector (torch order: W1 b1 W2 b2
+// W3 b3); returns the parameter count
+int mlp3_offsets(const b200rl_mlp_desc& d, int w_off[3], int b_off[3]);
 
 // global launch counter (bench.py reports gpu_launches from it)
 void count_launch(int n = 1);

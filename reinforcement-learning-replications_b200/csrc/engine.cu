@@ -42,6 +42,24 @@ int device_sm_count() {
 // CTA per SM, so the buffer is allocated once at that size (132 x 256 KB = 33 MB on an H100) and never resized or
 // freed while the process runs.  Launches under stream capture are refused: a captured graph could be replayed on
 // another stream while this one uses the same buffer.
+int tc_grid(int64_t n_rows) {
+  const int64_t tiles = (n_rows + 127) / 128;
+  const int sms = device_sm_count();
+  if (sms <= 0) return -1;
+  return (int)(tiles < sms ? (tiles < 1 ? 1 : tiles) : sms);
+}
+
+int mlp3_offsets(const b200rl_mlp_desc& d, int w_off[3], int b_off[3]) {
+  int off = 0;
+  for (int l = 0; l < 3; ++l) {
+    w_off[l] = off;
+    off += d.sizes[l + 1] * d.sizes[l];
+    b_off[l] = off;
+    off += d.sizes[l + 1];
+  }
+  return off;
+}
+
 float* acc_mem(int grid, cudaStream_t s) {
   struct Entry {
     int dev;
@@ -454,14 +472,7 @@ static void fill_tc3_net(const b200rl_mlp_desc& d, Tc3Net* n, int* P) {
   n->n_out = d.sizes[3];
   n->h1 = d.sizes[1];
   n->h2 = d.sizes[2];
-  int off = 0;
-  for (int l = 0; l < 3; ++l) {
-    n->w_off[l] = off;
-    off += d.sizes[l + 1] * d.sizes[l];
-    n->b_off[l] = off;
-    off += d.sizes[l + 1];
-  }
-  *P = off;
+  *P = mlp3_offsets(d, n->w_off, n->b_off);
 }
 
 static void fill_seg(Ra3Seg* g, float* params, float* m, float* v, int64_t step, double lr, double b1, double b2,
@@ -514,7 +525,7 @@ static int run_fused_iterations(b200rl_onpolicy* h, const b200rl_ppo_hparams* hp
   memset(&a, 0, sizeof(a));
   a.partials = h->partials;
   a.scalar_partials = h->scalar_partials;
-  a.rows = 2 * tc3_grid(h->n_rows);
+  a.rows = 2 * tc_grid(h->n_rows);
   a.P[0] = h->Pp;
   a.P[1] = h->Pv;
   a.grad = h->grad_all;
@@ -1144,7 +1155,7 @@ extern "C" int b200rl_onpolicy_run_stage(b200rl_onpolicy* h, const char* stage, 
     a.mode = 1;
     a.partials = h->partials;
     a.scalar_partials = h->scalar_partials;
-    a.rows = 2 * tc3_grid(h->n_rows);
+    a.rows = 2 * tc_grid(h->n_rows);
     a.P[0] = h->Pp;
     a.P[1] = h->Pv;
     a.grad = h->grad_all;

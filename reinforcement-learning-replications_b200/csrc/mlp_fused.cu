@@ -637,10 +637,8 @@ static int fused_grid(const MlpLayout& lay, int64_t n_rows) {
 
 // tensor-core path (mlp_tc.cu)
 bool tc_shape_ok(const b200rl_mlp_desc& d);
-int tc_grid(int64_t n_rows);
 int launch_mlp_tc(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, cudaStream_t s);
 // second-generation tensor-core path (mlp_tc2.cu): fp16 x 2 splits, two partial rows per CTA
-int tc2_grid(int64_t n_rows);
 int launch_mlp_tc2(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, int total_rows, cudaStream_t s);
 // B200RL_TC_MODE=bf16 pins the bf16 x 3 kernel (A/B runs); default is the fp16 x 2 kernel with bf16 x 3 as its
 // wide-range fallback
@@ -682,7 +680,7 @@ extern "C" int b200rl_mlp_grid(const b200rl_mlp_desc* mlp, int64_t n_rows, int w
   if (!mlp) return -1;
   if (with_backward >= 0 && with_backward < 2 && use_tc(*mlp)) {
     if (!use_tc2()) return tc_grid(n_rows);
-    const int g = tc2_grid(n_rows);
+    const int g = tc_grid(n_rows);
     return g > 0 ? 2 * g : -1;
   }
   if (with_backward == 2 && use_tc(*mlp) && use_tc2()) return tc_fvp_total_rows(*mlp, n_rows);
@@ -770,7 +768,7 @@ int launch_fused_fallback(const b200rl_mlp_loss_grad_args* a, const unsigned* ru
 int tc_fwd_total_rows(const b200rl_mlp_desc& mlp, int64_t n_rows) {
   MlpLayout lay;
   if (build_layout(mlp, false, &lay, false)) return -1;
-  const int g = tc2_grid(n_rows), f = fused_grid(lay, n_rows);
+  const int g = tc_grid(n_rows), f = fused_grid(lay, n_rows);
   if (g <= 0 || f <= 0) return -1;
   return 2 * g > f ? 2 * g : f;
 }
@@ -779,7 +777,7 @@ int tc_fwd_total_rows(const b200rl_mlp_desc& mlp, int64_t n_rows) {
 int tc_fvp_total_rows(const b200rl_mlp_desc& mlp, int64_t n_rows) {
   MlpLayout lay;
   if (build_layout(mlp, true, &lay, true)) return -1;
-  const int g = tc2_grid(n_rows), f = fused_grid(lay, n_rows);
+  const int g = tc_grid(n_rows), f = fused_grid(lay, n_rows);
   if (g <= 0 || f <= 0) return -1;
   return 2 * g > f ? 2 * g : f;
 }

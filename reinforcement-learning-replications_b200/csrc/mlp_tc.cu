@@ -6,13 +6,13 @@
 //
 // Precision: the tensor cores have no fp32 MMA and plain TF32 violates the 1e-5 parity bar, so every fp32
 // operand is split into THREE bf16 values x = h + m + l (24 mantissa bits) and every logical product is the six
-// kind::f16 MMAs  mm + hl + lh + hm + mh + hh  with fp32 accumulation -- 2^-24-grade relative error per
+// bf16 wgmma products  mm + hl + lh + hm + mh + hh  with fp32 accumulation -- 2^-24-grade relative error per
 // product, which the golden / oracle parity tests hold to 1e-5.  bf16 (not tf32) because a SWIZZLE_128B buffer of 16-bit elements can
 // be read BOTH K-major (activations as the A operand of the next layer) and MN-major (the same activations as an
 // operand of the dW = dZ^T X product, whose reduction runs over the tile's rows); tf32 MN-major needs a different
 // swizzle, i.e. a second copy of every activation .
 //
-// Per CTA: 128-row tiles, persistent over tiles (grid = min(#tiles, #SMs)), 8 epilogue warps + 1 MMA-issuing warp.
+// Per CTA: 128-row tiles, persistent over tiles (grid = min(#tiles, #SMs)), 8 epilogue warps + 1 MMA-issuing warpgroup.
 //   shared memory  operand buffers, 64 bf16 columns x 128-byte rows, SWIZZLE_128B, three splits each:
 //                  XD [128][64]: obs in cols 0..31, dOut in cols 32..46, ones in col 47 (bias gradients for free)
 //                  H1, H2 [128][64]: activations, overwritten in place by dZ1 / dZ2 during the backward pass
@@ -55,9 +55,9 @@ constexpr uint32_t SM_STAGE = SM_DB3 + 512;         // fp32 staging of the NEXT 
 constexpr uint32_t SM_TOTAL = SM_STAGE + 128 * 32 * 4;
 constexpr uint32_t TC_SMEM_BYTES = SM_TOTAL + 1024;  // + alignment slack
 
-// tensor-memory column map
-constexpr uint32_t TM_Z1 = 0, TM_Z2 = 64, TM_OUT = 128, TM_DH2 = 160, TM_DH1 = 224, TM_DW2 = 288, TM_DW1 = 352,
-                   TM_DW3 = 384, TM_DB2 = 400, TM_DB1 = 416;
+// accumulator column map
+constexpr uint32_t ACC_Z1 = 0, ACC_Z2 = 64, ACC_OUT = 128, ACC_DH2 = 160, ACC_DH1 = 224, ACC_DW2 = 288, ACC_DW1 = 352,
+                   ACC_DW3 = 384, ACC_DB2 = 400, ACC_DB1 = 416;
 
 struct TcArgs {
   int n_in, n_out;
@@ -122,32 +122,18 @@ __device__ __forceinline__ void cp_async_commit_wait_all() {
   asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
 }
 
-// One operand of a split product: 32-bit halves of the descriptor of split 0 / k-step 0, the low-word advance per
-// split (buffer stride >> 4) and per k-step (bytes >> 4).  All fields are warp-uniform.
-struct OpDesc {
-  uint32_t lo, hi, split_step, k_step;
-};
-__device__ __forceinline__ OpDesc op_kmajor(uint32_t addr, uint32_t split_bytes) {  // K along the 128-byte rows
-  const uint64_t d = make_smem_desc_sw128(addr, 16, 1024);
-  return OpDesc{(uint32_t)d, (uint32_t)(d >> 32), split_bytes >> 4, 32u >> 4};
-}
-__device__ __forceinline__ OpDesc op_mnmajor(uint32_t addr, uint32_t rows, uint32_t split_bytes) {  // K along rows
-  const uint64_t d = make_smem_desc_sw128(addr, rows * 128, 1024);
-  return OpDesc{(uint32_t)d, (uint32_t)(d >> 32), split_bytes >> 4, 2048u >> 4};
-}
-
 // the six split products, smallest terms first: (m,m) (h,l) (l,h) (h,m) (m,h) (h,h)
-__device__ __forceinline__ void issue6(uint32_t d_tmem, uint32_t idesc, int ksteps, bool accumulate_first,
-                                       const OpDesc a, const OpDesc b) {
+template <int N, int TA, int TB, bool M64, int KSTEPS>
+__device__ __forceinline__ void issue6(float* acc, uint32_t acc_col, bool accumulate_first, const Op2 a, const Op2 b) {
   const uint32_t alo[6] = {a.lo + a.split_step, a.lo, a.lo + 2 * a.split_step, a.lo, a.lo + a.split_step, a.lo};
   const uint32_t blo[6] = {b.lo + b.split_step, b.lo + 2 * b.split_step, b.lo, b.lo + b.split_step, b.lo, b.lo};
-  mma_product(d_tmem, idesc, alo, blo, 6, a.hi, b.hi, a.k_step, b.k_step, ksteps, accumulate_first);
+  mma_product<N, true, TA, TB, M64>(acc, acc_col, alo, blo, 6, a.hi, b.hi, a.k_step, b.k_step, KSTEPS, accumulate_first);
 }
 // A (three splits) times an operand that is exact in bf16 (the ones column, split 0 only): three products
-__device__ __forceinline__ void issue3(uint32_t d_tmem, uint32_t idesc, int ksteps, bool accumulate_first,
-                                       const OpDesc a, const OpDesc b) {
+template <int N, int TA, int TB, bool M64, int KSTEPS>
+__device__ __forceinline__ void issue3(float* acc, uint32_t acc_col, bool accumulate_first, const Op2 a, const Op2 b) {
   const uint32_t alo[3] = {a.lo + 2 * a.split_step, a.lo + a.split_step, a.lo}, blo[3] = {b.lo, b.lo, b.lo};
-  mma_product(d_tmem, idesc, alo, blo, 3, a.hi, b.hi, a.k_step, b.k_step, ksteps, accumulate_first);
+  mma_product<N, true, TA, TB, M64>(acc, acc_col, alo, blo, 3, a.hi, b.hi, a.k_step, b.k_step, KSTEPS, accumulate_first);
 }
 
 #ifdef B200RL_TC_TIMING
@@ -170,13 +156,13 @@ template <bool BACKWARD>
 __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) unsigned long long mbar;
-  __shared__ uint32_t tmem_holder;
   __shared__ double s_sc[6][TC_EPI_WARPS];
   if (p.skip_flag != nullptr && *p.skip_flag != 0) return;  // early stop: whole launch is a no-op
   if (p.run_if != nullptr && *p.run_if != p.seq) return;    // the fp16 kernel's result stands
   if (p.run_if != nullptr && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&g_tc_fallbacks, 1ull);
 
   const int tid = threadIdx.x, lane = tid & 31;
+  float* const acc = p.acc_mem + (size_t)blockIdx.x * ACC_CTA_FLOATS;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // provably warp-uniform: role branches need no vote
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;  // SWIZZLE_128B atoms are 1024-byte aligned
@@ -224,16 +210,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
         s_dist[16 + a] = logf(scale);
       }
   }
-  if (tid == 0) acc_bind(p.acc_mem, &tmem_holder);
   if (tid == 0) {
     mbar_init(smem_u32(&mbar), 1);
     fence_mbar_init();
   }
   fence_proxy_async_smem();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = tmem_holder;
   const uint32_t bar = smem_u32(&mbar);
 
   const long long num_tiles = (p.n_rows + TC_ROWS - 1) / TC_ROWS;
@@ -241,46 +223,44 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
 
   if (warp >= TC_EPI_WARPS) {
     // =============================== MMA issuer warp =================================================
-    const uint32_t I_128_64_KK = make_idesc_bf16(128, 64, 0, 0), I_128_16_KK = make_idesc_bf16(128, 16, 0, 0);
-    const uint32_t I_128_64_KM = make_idesc_bf16(128, 64, 0, 1), I_64_64_MM = make_idesc_bf16(64, 64, 1, 1);
-    const uint32_t I_64_32_MM = make_idesc_bf16(64, 32, 1, 1), I_64_16_MM = make_idesc_bf16(64, 16, 1, 1);
-    // warp-uniform copies (ptxas keeps them in uniform registers: no per-instruction R2UR)
+    constexpr int K = K_MAJOR, MN = MN_MAJOR;
+    // warp-uniform copy (ptxas keeps it in a uniform register: no per-instruction R2UR)
     const uint32_t ub = __shfl_sync(0xffffffffu, base, 0);
-    const uint32_t ut = __shfl_sync(0xffffffffu, tmem, 0);
-    const OpDesc XD_K = op_kmajor(ub + SM_XD, ACT_BUF), H1_K = op_kmajor(ub + SM_H1, ACT_BUF),
-                 H2_K = op_kmajor(ub + SM_H2, ACT_BUF), W1_K = op_kmajor(ub + SM_W1, W_BUF),
-                 W2_K = op_kmajor(ub + SM_W2, W_BUF), W3_K = op_kmajor(ub + SM_W3, W3_BUF);
-    const OpDesc XD_K2 = op_kmajor(ub + SM_XD + 64, ACT_BUF);  // cols 32..47 (dOut) as a K-major A operand
-    const OpDesc H1_M = op_mnmajor(ub + SM_H1, 128, ACT_BUF), H2_M = op_mnmajor(ub + SM_H2, 128, ACT_BUF),
-                 XD_M0 = op_mnmajor(ub + SM_XD, 128, ACT_BUF),        // X    (cols 0..31)
-                 XD_M32 = op_mnmajor(ub + SM_XD + 64, 128, ACT_BUF),  // dOut (cols 32..47, col 47 = ones)
-                 W2_M = op_mnmajor(ub + SM_W2, 64, W_BUF), W3_M = op_mnmajor(ub + SM_W3, 16, W3_BUF);
+    const Op2 XD_K = op2_kmajor(ub + SM_XD, ACT_BUF), H1_K = op2_kmajor(ub + SM_H1, ACT_BUF),
+              H2_K = op2_kmajor(ub + SM_H2, ACT_BUF), W1_K = op2_kmajor(ub + SM_W1, W_BUF),
+              W2_K = op2_kmajor(ub + SM_W2, W_BUF), W3_K = op2_kmajor(ub + SM_W3, W3_BUF);
+    const Op2 XD_K2 = op2_kmajor(ub + SM_XD + 64, ACT_BUF);  // cols 32..47 (dOut) as a K-major A operand
+    // MN-major views: 64-element atoms along M / N are one buffer height (rows x 128 bytes) apart
+    const Op2 H1_M = op2_mnmajor(ub + SM_H1, 128 * 128, ACT_BUF), H2_M = op2_mnmajor(ub + SM_H2, 128 * 128, ACT_BUF),
+              XD_M0 = op2_mnmajor(ub + SM_XD, 128 * 128, ACT_BUF),        // X    (cols 0..31)
+              XD_M32 = op2_mnmajor(ub + SM_XD + 64, 128 * 128, ACT_BUF),  // dOut (cols 32..47, col 47 = ones)
+              W2_M = op2_mnmajor(ub + SM_W2, 64 * 128, W_BUF), W3_M = op2_mnmajor(ub + SM_W3, 16 * 128, W3_BUF);
     bool first = true;
     for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
 #pragma unroll 1
       for (int s = 0; s < STAGES; ++s) {
         __syncthreads();  // operands of stage s are in shared memory (and the previous stage's MMAs have retired)
-        tc_fence_after_sync();
+        // issue6 / issue3 <N, A major, B major, M = 64, k-steps>
         if (s == 0) {  // Z1 = X W1^T
-          issue6(ut + TM_Z1, I_128_64_KK, 2, false, XD_K, W1_K);
+          issue6<64, K, K, false, 2>(acc, ACC_Z1, false, XD_K, W1_K);
         } else if (s == 1) {  // Z2 = H1 W2^T
-          issue6(ut + TM_Z2, I_128_64_KK, 4, false, H1_K, W2_K);
+          issue6<64, K, K, false, 4>(acc, ACC_Z2, false, H1_K, W2_K);
         } else if (s == 2) {  // OUT = H2 W3^T
-          issue6(ut + TM_OUT, I_128_16_KK, 4, false, H2_K, W3_K);
+          issue6<16, K, K, false, 4>(acc, ACC_OUT, false, H2_K, W3_K);
         } else if (s == 3) {
           // dW3^T[i][o] += sum_r H2[r][i] dOut[r][o]   (both read MN-major: the reduction runs over rows)
-          issue6(ut + TM_DW3, I_64_16_MM, 8, !first, H2_M, XD_M32);
+          issue6<16, MN, MN, true, 8>(acc, ACC_DW3, !first, H2_M, XD_M32);
           // dH2 = dOut W3   (A: XD cols 32..47; B: W3 read MN-major, K = output index)
-          issue6(ut + TM_DH2, I_128_64_KM, 1, false, XD_K2, W3_M);
+          issue6<64, K, MN, false, 1>(acc, ACC_DH2, false, XD_K2, W3_M);
         } else if (s == 4) {
           // dW2[o][i] += sum_r dZ2[r][o] H1[r][i] ; db2[o] += sum_r dZ2[r][o] * 1 ; dH1 = dZ2 W2
-          issue6(ut + TM_DW2, I_64_64_MM, 8, !first, H2_M, H1_M);
-          issue3(ut + TM_DB2, I_64_16_MM, 8, !first, H2_M, XD_M32);
-          issue6(ut + TM_DH1, I_128_64_KM, 4, false, H2_K, W2_M);
+          issue6<64, MN, MN, true, 8>(acc, ACC_DW2, !first, H2_M, H1_M);
+          issue3<16, MN, MN, true, 8>(acc, ACC_DB2, !first, H2_M, XD_M32);
+          issue6<64, K, MN, false, 4>(acc, ACC_DH1, false, H2_K, W2_M);
         } else {
           // dW1[o][i] += sum_r dZ1[r][o] X[r][i] ; db1[o] += sum_r dZ1[r][o]
-          issue6(ut + TM_DW1, I_64_32_MM, 8, !first, H1_M, XD_M0);
-          issue3(ut + TM_DB1, I_64_16_MM, 8, !first, H1_M, XD_M32);
+          issue6<32, MN, MN, true, 8>(acc, ACC_DW1, !first, H1_M, XD_M0);
+          issue3<16, MN, MN, true, 8>(acc, ACC_DB1, !first, H1_M, XD_M32);
         }
         acc_commit(bar);
         __syncwarp();
@@ -290,8 +270,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
   } else {
     // =============================== epilogue warps ==================================================
     const int q = warp & 3, half = warp >> 2;
-    const int r = 32 * q + lane;                         // row of the tile == accumulator memory lane
-    const uint32_t lane_addr = (uint32_t)(32 * q) << 16;  // this warp's accumulator memory lane quadrant
+    const int r = 32 * q + lane;                         // row of the tile == accumulator row
     const int c0 = 32 * half;                            // this warp's column half
     uint32_t phase = 0;
 
@@ -308,39 +287,39 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
     for (int a = 0; a < 16; ++a) db3[a] = 0.f;
 
     // tanh layer epilogue: Z (accumulator memory) + bias -> tanh -> fp32 copy back to accumulator memory (for tanh') + bf16 splits to smem
-    auto act_epilogue = [&](uint32_t tm_col, const float* bias, uint32_t dst_buf) {
+    auto act_epilogue = [&](uint32_t acc_col, const float* bias, uint32_t dst_buf) {
 #pragma unroll
       for (int sub = 0; sub < 2; ++sub) {  // 16 columns at a time keeps the live register set small
         const int cs = c0 + 16 * sub;
-        uint32_t v[16];
-        acc_ld16(tmem + lane_addr + tm_col + cs, v);
+        float v[16];
+        acc_ld<16>(acc, r, acc_col + cs, v);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(tanhf(__uint_as_float(v[j]) + bias[cs + j]));
-        if (BACKWARD) acc_st16(tmem + lane_addr + tm_col + cs, v);
+        for (int j = 0; j < 16; ++j) v[j] = tanhf(v[j] + bias[cs + j]);
+        if (BACKWARD) acc_st<16>(acc, r, acc_col + cs, v);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8];
 #pragma unroll
-          for (int j = 0; j < 8; ++j) x[j] = __uint_as_float(v[8 * ch + j]);
+          for (int j = 0; j < 8; ++j) x[j] = v[8 * ch + j];
           store_chunk3(sm, dst_buf, ACT_BUF, r, (cs >> 3) + ch, x);
         }
       }
     };
     // backward epilogue: dZ = dH * (1 - H^2), bf16 splits over the activation buffer (in place)
-    auto dz_epilogue = [&](uint32_t tm_dh, uint32_t tm_h, uint32_t dst_buf) {
+    auto dz_epilogue = [&](uint32_t acc_dh, uint32_t acc_h, uint32_t dst_buf) {
 #pragma unroll
       for (int sub = 0; sub < 2; ++sub) {
         const int cs = c0 + 16 * sub;
-        uint32_t g[16], h[16];
-        acc_ld16(tmem + lane_addr + tm_dh + cs, g);
-        acc_ld16(tmem + lane_addr + tm_h + cs, h);
+        float g[16], h[16];
+        acc_ld<16>(acc, r, acc_dh + cs, g);
+        acc_ld<16>(acc, r, acc_h + cs, h);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8];
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
-            const float hv = __uint_as_float(h[8 * ch + j]);
-            x[j] = __uint_as_float(g[8 * ch + j]) * (1.f - hv * hv);
+            const float hv = h[8 * ch + j];
+            x[j] = g[8 * ch + j] * (1.f - hv * hv);
           }
           store_chunk3(sm, dst_buf, ACT_BUF, r, (cs >> 3) + ch, x);
         }
@@ -348,11 +327,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
     };
     auto stage_done = [&]() {  // publish smem writes to the tensor core, hand over to the issuer, wait for its MMAs
       fence_proxy_async_smem();
-      tc_fence_before_sync();
       __syncthreads();
       mbar_wait(bar, phase);
       phase ^= 1u;
-      tc_fence_after_sync();
     };
 
     float pf_act[15], pf_adv = 0.f, pf_old = 0.f, pf_tgt = 0.f;
@@ -413,11 +390,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
       TC_T(0);
       stage_done();                                   // F1
       TC_T(1);
-      act_epilogue(TM_Z1, s_bias, SM_H1);
+      act_epilogue(ACC_Z1, s_bias, SM_H1);
       TC_T(2);
       stage_done();                                   // F2
       TC_T(3);
-      act_epilogue(TM_Z2, s_bias + 64, SM_H2);
+      act_epilogue(ACC_Z2, s_bias + 64, SM_H2);
       TC_T(4);
       stage_done();                                   // F3
       TC_T(5);
@@ -427,12 +404,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
 
       // ---- distribution / loss epilogue (one thread per row: warps 0..3) ----
       if (half == 0) {
-        uint32_t o[16];
-        acc_ld16(tmem + lane_addr + TM_OUT, o);
+        float o[16];
+        acc_ld<16>(acc, r, ACC_OUT, o);
         float out[16], dout[16];
 #pragma unroll
         for (int a = 0; a < 16; ++a) {
-          out[a] = __uint_as_float(o[a]) + s_bias[128 + a];
+          out[a] = o[a] + s_bias[128 + a];
           dout[a] = 0.f;
         }
         if (valid) {
@@ -532,19 +509,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
       if (BACKWARD) {
         stage_done();                                 // dW3^T, dH2
         TC_T(7);
-        dz_epilogue(TM_DH2, TM_Z2, SM_H2);
+        dz_epilogue(ACC_DH2, ACC_Z2, SM_H2);
         TC_T(8);
         stage_done();                                 // dW2, db2, dH1
         TC_T(9);
-        dz_epilogue(TM_DH1, TM_Z1, SM_H1);
+        dz_epilogue(ACC_DH1, ACC_Z1, SM_H1);
         TC_T(10);
         stage_done();                                 // dW1, db1
         TC_T(11);
       } else {
-        // forward only: the next tile's F1 may not overwrite TM_OUT/XD before everyone has read them
-        tc_fence_before_sync();
+        // forward only: the next tile's F1 may not overwrite ACC_OUT/XD before everyone has read them
         asm volatile("bar.sync 1, %0;" ::"n"(TC_EPI_WARPS * 32) : "memory");
-        tc_fence_after_sync();
       }
     }
 
@@ -552,33 +527,33 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
     if (tid == 0 && blockIdx.x == 0 && BACKWARD)
       for (int i = 0; i < 16; ++i) g_tc_t[i] = tacc[i];
 #endif
-    // ---- per-CTA results: gradient accumulators (accumulator memory, M = 64 layout: row m -> lane (m%16) + 32*(m/16)) ----
+    // ---- per-CTA results: gradient accumulators (M = 64 products: thread r < 16 of warp q holds row m = 16 q + r) ----
     if (BACKWARD && half == 0) {
       float* dst = p.partials + (size_t)blockIdx.x * p.P;
       const int m = 16 * q + lane;  // valid for lane < 16
-      uint32_t v[32];
+      float v[32];
       for (int cb = 0; cb < 2; ++cb) {  // dW2 [64 o][64 i]
-        acc_ld32(tmem + lane_addr + TM_DW2 + 32 * cb, v);
+        acc_ld<32>(acc, r, ACC_DW2 + 32 * cb, v);
         if (lane < 16 && m < h2)
 #pragma unroll
           for (int j = 0; j < 32; ++j)
-            if (32 * cb + j < h1) dst[p.w_off[1] + m * h1 + 32 * cb + j] = __uint_as_float(v[j]);
+            if (32 * cb + j < h1) dst[p.w_off[1] + m * h1 + 32 * cb + j] = v[j];
       }
-      acc_ld32(tmem + lane_addr + TM_DW1, v);  // dW1 [64 o][32 i]
+      acc_ld<32>(acc, r, ACC_DW1, v);  // dW1 [64 o][32 i]
       if (lane < 16 && m < h1)
 #pragma unroll
         for (int j = 0; j < 32; ++j)
-          if (j < n_in) dst[p.w_off[0] + m * n_in + j] = __uint_as_float(v[j]);
-      uint32_t w[16];
-      acc_ld16(tmem + lane_addr + TM_DW3, w);  // dW3^T [64 i][16 o]
+          if (j < n_in) dst[p.w_off[0] + m * n_in + j] = v[j];
+      float w[16];
+      acc_ld<16>(acc, r, ACC_DW3, w);  // dW3^T [64 i][16 o]
       if (lane < 16 && m < h2)
 #pragma unroll
         for (int a = 0; a < 15; ++a)
-          if (a < A_out) dst[p.w_off[2] + a * h2 + m] = __uint_as_float(w[a]);
-      acc_ld16(tmem + lane_addr + TM_DB2, w);  // column 15 = sum_r dZ2[r][o]
-      if (lane < 16 && m < h2) dst[p.b_off[1] + m] = __uint_as_float(w[15]);
-      acc_ld16(tmem + lane_addr + TM_DB1, w);
-      if (lane < 16 && m < h1) dst[p.b_off[0] + m] = __uint_as_float(w[15]);
+          if (a < A_out) dst[p.w_off[2] + a * h2 + m] = w[a];
+      acc_ld<16>(acc, r, ACC_DB2, w);  // column 15 = sum_r dZ2[r][o]
+      if (lane < 16 && m < h2) dst[p.b_off[1] + m] = w[15];
+      acc_ld<16>(acc, r, ACC_DB1, w);
+      if (lane < 16 && m < h1) dst[p.b_off[0] + m] = w[15];
       // db3: fixed-order reduction of the per-row accumulators
 #pragma unroll
       for (int a = 0; a < 15; ++a) {
@@ -611,7 +586,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
   }
 
   // ---- teardown ----
-  tc_fence_before_sync();
   __syncthreads();
 }
 
@@ -627,13 +601,6 @@ bool tc_shape_ok(const b200rl_mlp_desc& d) {
          d.sizes[3] >= 1 && d.sizes[3] <= 15 && d.hidden_act == B200RL_ACT_TANH && d.out_act == B200RL_ACT_IDENTITY;
 }
 
-int tc_grid(int64_t n_rows) {
-  const int64_t tiles = (n_rows + TC_ROWS - 1) / TC_ROWS;
-  const int sms = device_sm_count();
-  if (sms <= 0) return -1;
-  return (int)(tiles < sms ? (tiles < 1 ? 1 : tiles) : sms);
-}
-
 static int launch_mlp_tc_impl(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, const unsigned* run_if, unsigned seq,
                               int partial_rows, cudaStream_t s) {
   TcArgs k{};
@@ -644,14 +611,7 @@ static int launch_mlp_tc_impl(const b200rl_mlp_loss_grad_args* a, int64_t n_glob
   k.n_out = a->mlp.sizes[3];
   k.h1 = a->mlp.sizes[1];
   k.h2 = a->mlp.sizes[2];
-  int off = 0;
-  for (int l = 0; l < 3; ++l) {
-    k.w_off[l] = off;
-    off += a->mlp.sizes[l + 1] * a->mlp.sizes[l];
-    k.b_off[l] = off;
-    off += a->mlp.sizes[l + 1];
-  }
-  k.P = off;
+  k.P = mlp3_offsets(a->mlp, k.w_off, k.b_off);
   k.loss = a->loss;
   k.dist = a->dist;
   k.n_rows = a->n_rows;

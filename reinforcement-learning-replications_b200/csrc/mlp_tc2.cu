@@ -40,7 +40,7 @@
 namespace b200rl {
 
 constexpr int T2_ROWS = 128;
-constexpr int T2_EPI_WARPS = 16;  // one pool: 4 warps per accumulator memory lane quadrant, 16 columns each
+constexpr int T2_EPI_WARPS = 16;  // one pool: 4 warps per 32-row quarter of the tile, 16 columns each
 constexpr int T2_EPI_THREADS = T2_EPI_WARPS * 32;
 constexpr int T2_THREADS = T2_EPI_THREADS + 128;  // + the issuing warpgroup
 constexpr float T2_LOG_SQRT_2PI = 0.91893853320467274178f;
@@ -64,18 +64,18 @@ constexpr uint32_t S2_DB3 = S2_DIST + 256;     // [16 warps][16] floats: running
 constexpr uint32_t S2_SCALE = S2_DB3 + 1024;   // scale factors (floats)
 constexpr uint32_t S2_RED = S2_SCALE + 64;     // block reduction scratch [20 warps][4] floats
 constexpr uint32_t S2_SC = S2_RED + 320;       // [16 warps][7] doubles: running scalar sums per warp
-constexpr uint32_t S2_BARS = S2_SC + 896;      // mbarriers: ready[2], chain[2], off[2]; accumulator base address (acc_bind); bad flag
+constexpr uint32_t S2_BARS = S2_SC + 896;      // mbarriers: ready[2], chain[2], off[2]; bad flag
 constexpr uint32_t S2_XS = S2_BARS + 64;       // per-feature observation scales 2^ex_k [32] and their inverses [32]
 constexpr uint32_t S2_ROWMAX = S2_XS + 256;    // [2 slots][128] largest scaled |obs| of each row (precision guard)
 constexpr uint32_t S2_TOTAL = S2_ROWMAX + 1024;
 constexpr uint32_t T2_SMEM_BYTES = S2_TOTAL + 1024;  // + alignment slack
 static_assert(T2_SMEM_BYTES <= 227 * 1024, "mlp_tc2 shared memory");
 
-// tensor-memory column map (fp32).  Per slot (base = slot * 144): Z1 (kept as H1 for tanh'), ZB (Z2, then dH2, then
+// accumulator column map (fp32).  Per slot (base = slot * 144): Z1 (kept as H1 for tanh'), ZB (Z2, then dH2, then
 // dH1 -- each consumed by its epilogue before the next product overwrites it), OUT.  Shared stacked accumulators,
-// lane = feature (+64 for the l-split half): DW2, DW1 (cols 0..31 dW1, col 47 db1), DW3, DB2 (col 15).
-constexpr uint32_t M2_SLOT = 144, M2_Z1 = 0, M2_ZB = 64, M2_OUT = 128;
-constexpr uint32_t M2_DW2 = 288, M2_DW1 = 352, M2_DW3 = 400, M2_DB2 = 416;
+// row = feature (+64 for the l-split half): DW2, DW1 (cols 0..31 dW1, col 47 db1), DW3, DB2 (col 15).
+constexpr uint32_t ACC_SLOT = 144, ACC_Z1 = 0, ACC_ZB = 64, ACC_OUT = 128;
+constexpr uint32_t ACC_DW2 = 288, ACC_DW1 = 352, ACC_DW3 = 400, ACC_DB2 = 416;
 
 // indices into the scale table in shared memory
 enum { SC_X = 0, SC_G, SC_U1, SC_U2, SC_U3, SC_UH2, SC_UH1, SC_W1, SC_W2, SC_W3, SC_OW3, SC_OW2, SC_OW1, SC_OB, SC_N };
@@ -131,6 +131,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
   if (p.skip_flag != nullptr && *p.skip_flag != 0) return;  // early stop: whole launch is a no-op
 
   const int tid = threadIdx.x, lane = tid & 31;
+  float* const acc = p.acc_mem + (size_t)blockIdx.x * ACC_CTA_FLOATS;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // provably warp-uniform: role branches need no vote
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;  // SWIZZLE_128B atoms are 1024-byte aligned
@@ -141,8 +142,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
   float* s_scale = reinterpret_cast<float*>(sm + S2_SCALE);
   float* s_red = reinterpret_cast<float*>(sm + S2_RED);
   double* s_sc = reinterpret_cast<double*>(sm + S2_SC);
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(sm + S2_BARS + 48);
-  int* s_bad = reinterpret_cast<int*>(sm + S2_BARS + 52);
+  int* s_bad = reinterpret_cast<int*>(sm + S2_BARS + 48);
   const uint32_t bars = base + S2_BARS;  // ready[s] at +8s, chain[s] at +16+8s, off[s] at +32+8s
   const int n_in = p.n_in, A_out = p.n_out, h1 = p.h1, h2 = p.h2;
   bool bad = false;
@@ -278,7 +278,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
   }
   if (bad) *s_bad = 1;  // non-finite bias
   bad = false;
-  if (tid == 0) acc_bind(p.acc_mem, s_tmem);
   if (tid == 0) {
     for (int s = 0; s < 2; ++s) {
       mbar_init(bars + 8 * s, T2_EPI_THREADS);   // ready[s]: every epilogue thread arrives once per job of slot s
@@ -288,10 +287,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
     fence_mbar_init();
   }
   fence_proxy_async_smem();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = *s_tmem;
 
   const long long num_tiles = (p.n_rows + T2_ROWS - 1) / T2_ROWS;
   // tiles of this CTA: blockIdx.x + k * gridDim.x; slot s takes k = s, s + 2, ...
@@ -300,12 +296,8 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
 
   if (warp >= T2_EPI_WARPS) {
     // =============================== MMA issuer warpgroup =================================================
-    constexpr uint32_t I_128_64_KK = make_idesc_f16(128, 64, 0, 0), I_128_16_KK = make_idesc_f16(128, 16, 0, 0),
-                       I_128_64_KM = make_idesc_f16(128, 64, 0, 1), I_128_64_MM = make_idesc_f16(128, 64, 1, 1),
-                       I_128_48_MM = make_idesc_f16(128, 48, 1, 1), I_128_16_MM = make_idesc_f16(128, 16, 1, 1);
-    // warp-uniform by construction: `base` comes from the shared-memory window, and accumulator addresses are
-    // (lane << 16) | column within this CTA's block of the accumulator memory (acc_bind), so column 0 is address 0
-    const uint32_t ub = base, ut = 0u, ubar = bars;
+    constexpr int K = K_MAJOR, MN = MN_MAJOR;
+    const uint32_t ub = base, ubar = bars;  // warp-uniform by construction: from the shared-memory window
     // slot-0 views of the per-slot buffers (slot 1 = T2_SLOT further)
     const Op2 XD_K = op2_kmajor(ub + S2_XD, T2_ACT), H1_K = op2_kmajor(ub + S2_H1, T2_ACT),
               H2_K = op2_kmajor(ub + S2_H2, T2_ACT);
@@ -329,7 +321,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
     // bit-reproducible.
     auto serve = [&](const int S, const int stage) {
       const uint32_t so = (uint32_t)S * T2_SLOT;
-      const uint32_t tz = ut + (uint32_t)S * M2_SLOT;
+      const uint32_t acol = (uint32_t)S * ACC_SLOT;
       const uint32_t bar_chain = ubar + 16 + 8 * S, bar_off = ubar + 32 + 8 * S;
       uint32_t& par = S == 0 ? par0 : par1;
 #ifdef B200RL_TC_TIMING
@@ -337,37 +329,37 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
 #endif
       mbar_wait(ubar + 8 * S, par);  // every epilogue thread has delivered its share of the stage inputs
       par ^= 1u;
-      tc_fence_after_sync();
 #ifdef B200RL_TC_TIMING
       long long it1 = clock64();
       iacc[6] += (unsigned long long)(it1 - it0);
 #endif
+      // issue_chain3 <N, B major, k-steps>, issue_stacked <N, k-steps, B splits>
       if (stage == 0) {  // Z1 = X W1^T
-        issue_chain3<2>(tz + M2_Z1, I_128_64_KM, op2_at(XD_K, so), W1T_M);
+        issue_chain3<64, MN, 2>(acc, acol + ACC_Z1, op2_at(XD_K, so), W1T_M);
         acc_commit(bar_chain);
       } else if (stage == 1) {  // Z2 = H1 W2^T
-        issue_chain3<4>(tz + M2_ZB, I_128_64_KK, op2_at(H1_K, so), W2_K);
+        issue_chain3<64, K, 4>(acc, acol + ACC_ZB, op2_at(H1_K, so), W2_K);
         acc_commit(bar_chain);
       } else if (stage == 2) {  // OUT = H2 W3^T
-        issue_chain3<4>(tz + M2_OUT, I_128_16_KK, op2_at(H2_K, so), W3_K);
+        issue_chain3<16, K, 4>(acc, acol + ACC_OUT, op2_at(H2_K, so), W3_K);
         acc_commit(bar_chain);
       } else if (stage == 3) {
         // dH2 = dOut W3 (A: XD cols 32..47; B: W3 read MN-major, K = output index);
         // dW3^T[i][o] += sum_r H2[r][i] dOut[r][o]  -- must retire before the epilogue turns H2 into dZ2 in place
-        issue_chain3<1>(tz + M2_ZB, I_128_64_KM, op2_at(XD_K2, so), W3_M);
-        issue_stacked<8, 2>(ut + M2_DW3, I_128_16_MM, acc_dw3, op2_at(H2_M, so), op2_at(XD_M32, so));
+        issue_chain3<64, MN, 1>(acc, acol + ACC_ZB, op2_at(XD_K2, so), W3_M);
+        issue_stacked<16, 8, 2>(acc, ACC_DW3, acc_dw3, op2_at(H2_M, so), op2_at(XD_M32, so));
         acc_dw3 = true;
         acc_commit(bar_chain);
       } else if (stage == 4) {
         // dH1 = dZ2 W2 ; dW2[o][i] += sum_r dZ2[r][o] H1[r][i] ; db2[o] += sum_r dZ2[r][o] * 1
-        issue_chain3<4>(tz + M2_ZB, I_128_64_KM, op2_at(H2_K, so), W2_M);
-        issue_stacked<8, 2>(ut + M2_DW2, I_128_64_MM, acc_dw2, op2_at(H2_M, so), op2_at(H1_M, so));
-        issue_stacked<8, 1>(ut + M2_DB2, I_128_16_MM, acc_dw2, op2_at(H2_M, so), op2_at(XD_M32, so));
+        issue_chain3<64, MN, 4>(acc, acol + ACC_ZB, op2_at(H2_K, so), W2_M);
+        issue_stacked<64, 8, 2>(acc, ACC_DW2, acc_dw2, op2_at(H2_M, so), op2_at(H1_M, so));
+        issue_stacked<16, 8, 1>(acc, ACC_DB2, acc_dw2, op2_at(H2_M, so), op2_at(XD_M32, so));
         acc_dw2 = true;
         acc_commit(bar_chain);
       } else {
         // dW1[o][i] += sum_r dZ1[r][o] X[r][i] and, through the ones column, db1[o] += sum_r dZ1[r][o]
-        issue_stacked<8, 2>(ut + M2_DW1, I_128_48_MM, acc_dw1, op2_at(H1_M, so), op2_at(XD_M0, so));
+        issue_stacked<48, 8, 2>(acc, ACC_DW1, acc_dw1, op2_at(H1_M, so), op2_at(XD_M0, so));
         acc_dw1 = true;
         acc_commit(bar_off);
       }
@@ -391,15 +383,14 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
   } else {
     // =============================== epilogue warps: one pool of 16 ===================================
     // Two tiles ("slots") are in flight, but the epilogue warps are NOT bound to a slot: all 16 work on one epilogue
-    // job at a time (16 columns each: 4 warps per accumulator memory lane quadrant), alternating between the slots in a fixed order
+    // job at a time (16 columns each: 4 warps per 32-row quarter of the tile), alternating between the slots in a fixed order
     //   (slot 0, E0) (slot 1, E0) (slot 0, E1) (slot 1, E1) ... (slot 1, E5) | next pair of tiles
     // so the MMAs a job hands to the issuer run under the OTHER slot's next job.  (Binding 8 warps to each slot left
     // every epilogue latency bound -- 8 warps cannot fill the SM's issue slots -- and made both slots wait for their
     // MMAs at the same time; measured slower on B200.)  The one-row-per-thread loss
     // job needs only 4 warps; it rotates over the four column groups from tile to tile and the other 12 warps move on.
     const int q = warp & 3, part = warp >> 2;
-    const int r = 32 * q + lane;                          // row of the tile == accumulator memory lane
-    const uint32_t lane_addr = (uint32_t)(32 * q) << 16;  // this warp's accumulator memory lane quadrant
+    const int r = 32 * q + lane;                          // row of the tile == accumulator row
     const int cs = 16 * part;                             // this warp's 16 columns of a 64-column epilogue
     uint32_t ph_chain0 = 0, ph_chain1 = 0, ph_off0 = 0, ph_off1 = 0;
     bool first0 = true, first1 = true;
@@ -429,7 +420,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
     long long tlast = clock64();
 #endif
     auto job = [&](const int slot, const int stage, const long long k) {
-      const uint32_t tz = tmem + lane_addr + (uint32_t)slot * M2_SLOT;
+      const uint32_t acol = (uint32_t)slot * ACC_SLOT;
       const uint32_t so = (uint32_t)slot * T2_SLOT;
       const uint32_t bar_ready = bars + 8 * slot, bar_chain = bars + 16 + 8 * slot, bar_off = bars + 32 + 8 * slot;
       const long long tile = blockIdx.x + k * gridDim.x;
@@ -438,7 +429,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
       const bool loss_warp = part == (int)(k & 3);  // rotates: every warp does the loss job of one tile in four
       auto arrive = [&]() {  // -> issuer: "this thread's share of the slot's next stage inputs is in shared memory"
         fence_proxy_async_smem();
-        tc_fence_before_sync();
         mbar_arrive(bar_ready);
       };
       auto wait_chain = [&]() {
@@ -446,7 +436,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
         uint32_t& ph = slot == 0 ? ph_chain0 : ph_chain1;
         mbar_wait(bar_chain, ph);
         ph ^= 1u;
-        tc_fence_after_sync();
         T2_T(2 * stage);  // wait
       };
       if (stage == 0) {
@@ -460,7 +449,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
           uint32_t& ph = slot == 0 ? ph_off0 : ph_off1;
           mbar_wait(bar_off, ph);
           ph ^= 1u;
-          tc_fence_after_sync();
         }
         first = false;
         float rmax = 0.f, nan_probe = 0.f;
@@ -477,24 +465,21 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
       } else if (stage == 1 || stage == 2) {
         // ---- E1 / E2: Z (accumulator memory) * unscale + bias -> tanh -> [fp32 back to accumulator memory for tanh'] + fp16 splits ----
         wait_chain();
-        const uint32_t tm_col = stage == 1 ? M2_Z1 : M2_ZB;
+        const uint32_t col = acol + (stage == 1 ? ACC_Z1 : ACC_ZB) + cs;
         const float* bias = stage == 1 ? s_bias : s_bias + 64;
         const float unscale = s_scale[stage == 1 ? SC_U1 : SC_U2];
         const uint32_t dst = so + (stage == 1 ? S2_H1 : S2_H2);
-        uint32_t v[16];
-        acc_ld16(tz + tm_col + cs, v);
         float z[16];
+        acc_ld<16>(acc, r, col, z);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) z[j] = fmaf(__uint_as_float(v[j]), unscale, bias[cs + j]);
+        for (int j = 0; j < 16; ++j) z[j] = fmaf(z[j], unscale, bias[cs + j]);
         tanh16_scaled(z, 1.f);  // |tanh| <= 1, and Z is finite: observations, weights and biases were all checked
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(z[j]);
-        if (BACKWARD && stage == 1) acc_st16(tz + tm_col + cs, v);
+        if (BACKWARD && stage == 1) acc_st<16>(acc, r, col, z);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8];
 #pragma unroll
-          for (int j = 0; j < 8; ++j) x[j] = __uint_as_float(v[8 * ch + j]) * sH;
+          for (int j = 0; j < 8; ++j) x[j] = z[8 * ch + j] * sH;
           store_chunk2(sm, dst, r, (cs >> 3) + ch, x);
         }
         arrive();
@@ -522,13 +507,13 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
             s_rowmax[slot * 128 + r] = 0.f;
             if (valid && rm > 0.f && rm < 0.03125f) bad = true;
           }
-          uint32_t o[16];
-          acc_ld16(tz + M2_OUT, o);
+          float o[16];
+          acc_ld<16>(acc, r, acol + ACC_OUT, o);
           float out[16], dout[16];
           const float u3 = s_scale[SC_U3];
 #pragma unroll
           for (int a = 0; a < 16; ++a) {
-            out[a] = fmaf(__uint_as_float(o[a]), u3, s_bias[128 + a]);
+            out[a] = fmaf(o[a], u3, s_bias[128 + a]);
             dout[a] = 0.f;
           }
           if (valid) {
@@ -671,14 +656,14 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
         // ---- E4: dZ2 (scaled) = dH2_acc * 2^-ew3 * (1 - H2^2), H2 re-read from its fp16 splits, written in place ----
         wait_chain();  // dH2 (and dW3: H2 may be overwritten now)
         const float unscale = s_scale[SC_UH2], hh = pow2i(-2 * T2_H_EXP);
-        uint32_t g[16];
-        acc_ld16(tz + M2_ZB + cs, g);
+        float g[16];
+        acc_ld<16>(acc, r, acol + ACC_ZB + cs, g);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8];
           load_chunk2(sm, so + S2_H2, r, (cs >> 3) + ch, x);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) x[j] = (__uint_as_float(g[8 * ch + j]) * unscale) * fmaf(-(x[j] * hh), x[j], 1.f);
+          for (int j = 0; j < 8; ++j) x[j] = (g[8 * ch + j] * unscale) * fmaf(-(x[j] * hh), x[j], 1.f);
           if (too_large8(x)) bad = true;
           store_chunk2(sm, so + S2_H2, r, (cs >> 3) + ch, x);
         }
@@ -687,16 +672,16 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
         // ---- E5: dZ1 (scaled) = dH1_acc * 2^-ew2 * (1 - H1^2), H1 kept as fp32 in accumulator memory, written over H1 ----
         wait_chain();  // dH1 (and dW2 / db2: H1 may be overwritten now)
         const float unscale = s_scale[SC_UH1];
-        uint32_t g[16], h[16];
-        acc_ld16(tz + M2_ZB + cs, g);
-        acc_ld16(tz + M2_Z1 + cs, h);
+        float g[16], h[16];
+        acc_ld<16>(acc, r, acol + ACC_ZB + cs, g);
+        acc_ld<16>(acc, r, acol + ACC_Z1 + cs, h);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8];
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
-            const float hv = __uint_as_float(h[8 * ch + j]);
-            x[j] = (__uint_as_float(g[8 * ch + j]) * unscale) * (1.f - hv * hv);
+            const float hv = h[8 * ch + j];
+            x[j] = (g[8 * ch + j] * unscale) * (1.f - hv * hv);
           }
           if (too_large8(x)) bad = true;
           store_chunk2(sm, so + S2_H1, r, (cs >> 3) + ch, x);
@@ -723,60 +708,51 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
 
     // ---- per-CTA results ----
     if (BACKWARD) {  // the last dW1 of each slot that had a tile
-      if (!first0) {
-        mbar_wait(bars + 32, ph_off0);
-        tc_fence_after_sync();
-      }
-      if (!first1) {
-        mbar_wait(bars + 40, ph_off1);
-        tc_fence_after_sync();
-      }
+      if (!first0) mbar_wait(bars + 32, ph_off0);
+      if (!first1) mbar_wait(bars + 40, ph_off1);
     }
-    tc_fence_before_sync();
     asm volatile("bar.sync 2, %0;" ::"n"(T2_EPI_THREADS) : "memory");  // every MMA of the CTA has retired
-    tc_fence_after_sync();
     if (BACKWARD) {
-      // stacked accumulators: lanes 0..63 = h-split half (partial row 2b), lanes 64..127 = l-split half (row 2b+1)
+      // stacked accumulators: rows 0..63 = h-split half (partial row 2b), rows 64..127 = l-split half (row 2b+1)
       float* dst = p.partials + ((size_t)blockIdx.x * 2 + (q >> 1)) * p.P;
       const int m = 32 * (q & 1) + lane;  // feature index
-      const uint32_t ta = tmem + lane_addr;
-      uint32_t v[16];
+      float v[16];
       if (part < 2) {  // dW2 [h2 o][h1 i]: columns 32*part .. +31
 #pragma unroll
         for (int cb = 0; cb < 2; ++cb) {
           const int cc = 32 * part + 16 * cb;
-          acc_ld16(ta + M2_DW2 + cc, v);
+          acc_ld<16>(acc, r, ACC_DW2 + cc, v);
           const float u = s_scale[SC_OW2];
           if (m < h2)
 #pragma unroll
             for (int j = 0; j < 16; ++j)
-              if (cc + j < h1) dst[p.w_off[1] + m * h1 + cc + j] = __uint_as_float(v[j]) * u;
+              if (cc + j < h1) dst[p.w_off[1] + m * h1 + cc + j] = v[j] * u;
         }
       } else if (part == 2) {  // dW1 [h1 o][n_in i] in cols 0..31, db1 in col 47
 #pragma unroll
         for (int cb = 0; cb < 3; ++cb) {
-          acc_ld16(ta + M2_DW1 + 16 * cb, v);
+          acc_ld<16>(acc, r, ACC_DW1 + 16 * cb, v);
           if (m < h1) {
             if (cb < 2) {
               const float u = s_scale[SC_OW1];
 #pragma unroll
               for (int j = 0; j < 16; ++j)
                 if (16 * cb + j < n_in)
-                  dst[p.w_off[0] + m * n_in + 16 * cb + j] = (__uint_as_float(v[j]) * u) * s_xs[32 + 16 * cb + j];
+                  dst[p.w_off[0] + m * n_in + 16 * cb + j] = (v[j] * u) * s_xs[32 + 16 * cb + j];
             } else {
-              dst[p.b_off[0] + m] = __uint_as_float(v[15]) * s_scale[SC_OB];
+              dst[p.b_off[0] + m] = v[15] * s_scale[SC_OB];
             }
           }
         }
       } else {  // dW3^T [h2 i][16 o] and db2 (col 15 = sum_r dZ2[r][o])
-        acc_ld16(ta + M2_DW3, v);
+        acc_ld<16>(acc, r, ACC_DW3, v);
         const float u = s_scale[SC_OW3];
         if (m < h2)
 #pragma unroll
           for (int a = 0; a < 15; ++a)
-            if (a < A_out) dst[p.w_off[2] + a * h2 + m] = __uint_as_float(v[a]) * u;
-        acc_ld16(ta + M2_DB2, v);
-        if (m < h2) dst[p.b_off[1] + m] = __uint_as_float(v[15]) * s_scale[SC_OB];
+            if (a < A_out) dst[p.w_off[2] + a * h2 + m] = v[a] * u;
+        acc_ld<16>(acc, r, ACC_DB2, v);
+        if (m < h2) dst[p.b_off[1] + m] = v[15] * s_scale[SC_OB];
       }
     }
     // per-thread sums -> per-warp sums (tree) -> the 16 warps in order (below): fixed order => reproducible
@@ -819,7 +795,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
   }
 
   // ---- teardown ----
-  tc_fence_before_sync();
   __syncthreads();
   if (tid == 0 && *s_bad != 0) *p.status = p.seq;  // this launch is redone by the bf16 x 3 kernel queued behind it
 }
@@ -903,13 +878,6 @@ int launch_absmax_cols(const float* x, long long rows, int cols, float* out, cud
   return 0;
 }
 
-int tc2_grid(int64_t n_rows) {
-  const int64_t tiles = (n_rows + T2_ROWS - 1) / T2_ROWS;
-  const int sms = device_sm_count();
-  if (sms <= 0) return -1;
-  return (int)(tiles < sms ? (tiles < 1 ? 1 : tiles) : sms);
-}
-
 int launch_mlp_tc_fallback(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, const unsigned* run_if, unsigned seq,
                            int partial_rows, cudaStream_t s);
 int launch_fused_fallback(const b200rl_mlp_loss_grad_args* a, const unsigned* run_if, unsigned seq, int total_rows,
@@ -925,14 +893,7 @@ int launch_mlp_tc2(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, int total
   k.n_out = a->mlp.sizes[3];
   k.h1 = a->mlp.sizes[1];
   k.h2 = a->mlp.sizes[2];
-  int off = 0;
-  for (int l = 0; l < 3; ++l) {
-    k.w_off[l] = off;
-    off += a->mlp.sizes[l + 1] * a->mlp.sizes[l];
-    k.b_off[l] = off;
-    off += a->mlp.sizes[l + 1];
-  }
-  k.P = off;
+  k.P = mlp3_offsets(a->mlp, k.w_off, k.b_off);
   k.loss = a->loss;
   k.dist = a->dist;
   k.n_rows = a->n_rows;
@@ -973,7 +934,7 @@ int launch_mlp_tc2(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, int total
   }
   k.obs_absmax = need_obs ? scratch : a->obs_absmax;
   k.target_absmax = need_tgt ? scratch + 32 : a->target_absmax;
-  const int grid = tc2_grid(a->n_rows);
+  const int grid = tc_grid(a->n_rows);
   B200RL_REQUIRE(grid > 0, "mlp_tc2: no CUDA device");
   k.acc_mem = acc_mem(grid, s);
   B200RL_REQUIRE(k.acc_mem != nullptr, "mlp_tc2: no accumulator memory (allocation failed, or the stream is being captured): %s",

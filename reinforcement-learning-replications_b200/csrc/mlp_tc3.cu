@@ -50,7 +50,7 @@ constexpr uint32_t S3_DIST = S3_BIAS + 2 * 640;      // var[16], log_scale[16], 
 constexpr uint32_t S3_SCALE = S3_DIST + 256;         // per net 16 floats
 constexpr uint32_t S3_XS = S3_SCALE + 128;           // 2^ex_k [32], 2^-ex_k [32]
 constexpr uint32_t S3_RED = S3_XS + 256;             // setup reduction scratch [20 warps][8] floats
-constexpr uint32_t S3_BARS = S3_RED + 640;           // ready[2] chain[2] xfull[2] free[2] (8 B each), accumulator base address (acc_bind), bad flag
+constexpr uint32_t S3_BARS = S3_RED + 640;           // ready[2] chain[2] xfull[2] (8 B each), bad flag
 constexpr uint32_t S3_TOTAL = S3_BARS + 128;
 constexpr uint32_t T3_SMEM_BYTES = S3_TOTAL + 1024;  // + alignment slack
 static_assert(T3_SMEM_BYTES <= 227 * 1024, "mlp_tc3 shared memory");
@@ -58,14 +58,14 @@ static_assert(T3_SMEM_BYTES <= 227 * 1024, "mlp_tc3 shared memory");
 constexpr uint32_t S3_END_DB3 = 0;                   // [16 warps][16] floats
 constexpr uint32_t S3_END_SC = 1024;                 // [16 warps][8] doubles
 
-// ---- tensor-memory column map (fp32) ----
-constexpr uint32_t M3_CHAIN = 80, M3_Z = 0, M3_OUT = 64;          // per chain: Z1 -> Z2 -> dH2 -> dH1 share Z
+// ---- accumulator column map (fp32) ----
+constexpr uint32_t ACC_CHAIN = 80, ACC_Z = 0, ACC_OUT = 64;       // per chain: Z1 -> Z2 -> dH2 -> dH1 share Z
 // per net: DW2 (64) | DB2 (16, col 15 = db2) | DW1 (64: products with X's h columns, then with its l columns; col 31 =
 // db1) | DW3 (32: products with dOut's h columns, then l).  The B operands of dW1 / dW3 hold their two splits side
 // by side in one swizzle atom, so ONE product per k-step covers both; the halves are added when the accumulators
 // are read, once per launch.  2 x 80 + 2 x 176 = 512 columns: all of accumulator memory.
-constexpr uint32_t M3_ACC = 160, M3_ACC_NET = 176;
-constexpr uint32_t M3_DW2 = 0, M3_DB2 = 64, M3_DW1 = 80, M3_DW3 = 144;
+constexpr uint32_t ACC_GRAD = 160, ACC_GRAD_NET = 176;
+constexpr uint32_t ACC_DW2 = 0, ACC_DB2 = 64, ACC_DW1 = 80, ACC_DW3 = 144;
 
 #ifdef B200RL_TC3_TIMING
 // CTA 0: [0..9] job wait cycles (2 * (stage - 1) + chain), [10..19] job work cycles, [20..29] issuer: wait for the
@@ -156,6 +156,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   if (!run_p && !run_v) return;
   if (*p.x_bad != 0.f) return;  // the packed observations left the fp16 range: the engine redoes the update (wide-range path)
   const int tid = threadIdx.x, lane = tid & 31;
+  float* const acc = p.acc_mem + (size_t)blockIdx.x * ACC_CTA_FLOATS;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // provably warp-uniform (see mlp_tc2.cu)
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
@@ -165,9 +166,8 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   float* s_scale = reinterpret_cast<float*>(sm + S3_SCALE);
   float* s_xs = reinterpret_cast<float*>(sm + S3_XS);
   float* s_red = reinterpret_cast<float*>(sm + S3_RED);
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(sm + S3_BARS + 64);
-  int* s_bad = reinterpret_cast<int*>(sm + S3_BARS + 68);
-  // ready[c] at +8c, chain[c] at +16+8c, xfull[b] at +32+8b, free[c] at +48+8c
+  int* s_bad = reinterpret_cast<int*>(sm + S3_BARS + 48);
+  // ready[c] at +8c, chain[c] at +16+8c, xfull[b] at +32+8b
   const uint32_t bars = base + S3_BARS;
   const int n_in = p.n_in;
   bool bad = false;
@@ -312,21 +312,16 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     }
   if (bad) *s_bad = 1;  // non-finite bias
   bad = false;
-  if (tid == 0) acc_bind(p.acc_mem, s_tmem);
   if (tid == 0) {
     for (int c = 0; c < 2; ++c) {
       mbar_init(bars + 8 * c, T3_EPI_THREADS);  // ready[c]: every epilogue thread arrives once per job of chain c
       mbar_init(bars + 16 + 8 * c, 1);          // chain[c]: acc_commit
       mbar_init(bars + 32 + 8 * c, 1);          // xfull[b]: arrive.expect_tx by the MMA warp + the copy's bytes
-      mbar_init(bars + 48 + 8 * c, 1);          // (spare)
     }
     fence_mbar_init();
   }
   fence_proxy_async_smem();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = *s_tmem;
 
   const long long num_tiles = (p.n_rows + T3_ROWS - 1) / T3_ROWS;
   const long long cta_tiles = (num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;  // tiles blockIdx.x + k * gridDim.x
@@ -334,10 +329,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
 
   if (warp >= T3_EPI_WARPS) {
     // =============================== MMA issuer (and bulk-copy producer) warpgroup =============================
-    constexpr uint32_t I_128_64_KK = make_idesc_f16(128, 64, 0, 0), I_128_16_KK = make_idesc_f16(128, 16, 0, 0),
-                       I_128_64_KM = make_idesc_f16(128, 64, 0, 1), I_128_64_MM = make_idesc_f16(128, 64, 1, 1),
-                       I_128_32_MM = make_idesc_f16(128, 32, 1, 1), I_128_16_MM = make_idesc_f16(128, 16, 1, 1);
-    (void)I_128_16_MM;
+    constexpr int K = K_MAJOR, MN = MN_MAJOR;
     const uint32_t ub = base, ubar = bars;
     // views at chain 0 / net 0 / X buffer 0; the others are reached by adding byte offsets to the descriptors
     const Op2 X_K = op2_kmajor(ub + S3_XB, 64);                     // A: X, h at +0, l at +64 bytes
@@ -370,11 +362,10 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
       const long long xt0 = clock64();
 #endif
       mbar_wait(ubar + 32 + 8 * b, (uint32_t)((k >> 1) & 1));
-      tc_fence_after_sync();
 #ifdef B200RL_TC3_TIMING
       tacc[40] += (unsigned long long)(clock64() - xt0);
 #endif
-      issue_chain3<2>(c * M3_CHAIN + M3_Z, I_128_64_KM, op2_at(X_K, b * T2_ACT), op2_at(W1T_M, c * S3_WNET));
+      issue_chain3<64, MN, 2>(acc, c * ACC_CHAIN + ACC_Z, op2_at(X_K, b * T2_ACT), op2_at(W1T_M, c * S3_WNET));
     };
     if (cta_tiles > 0) {
       load_x(0);
@@ -392,39 +383,39 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
 #pragma unroll 1
         for (int c = c_first; c <= c_last; ++c) {
           const uint32_t co = c * S3_CHAIN, wo = c * S3_WNET;
-          const uint32_t tz = c * M3_CHAIN, ta = M3_ACC + c * M3_ACC_NET;
+          const uint32_t acol = c * ACC_CHAIN, gcol = ACC_GRAD + c * ACC_GRAD_NET;
 #ifdef B200RL_TC3_TIMING
           const long long it0 = clock64();
 #endif
           mbar_wait(ubar + 8 * c, (par_ready >> c) & 1u);  // every epilogue thread has delivered the stage inputs
           par_ready ^= 1u << c;
-          tc_fence_after_sync();
 #ifdef B200RL_TC3_TIMING
           const long long it1 = clock64();
           tacc[20 + 2 * (stage - 1) + c] += (unsigned long long)(it1 - it0);
 #endif
+          // issue_chain3 <N, B major, k-steps>, issue_stacked <N, k-steps, B splits>
           if (stage == 1) {  // Z2 = H1 W2^T
-            issue_chain3<4>(tz + M3_Z, I_128_64_KK, op2_at(H1_K, co), op2_at(W2_K, wo));
+            issue_chain3<64, K, 4>(acc, acol + ACC_Z, op2_at(H1_K, co), op2_at(W2_K, wo));
           } else if (stage == 2) {  // OUT = H2 W3^T
-            issue_chain3<4>(tz + M3_OUT, I_128_16_KK, op2_at(H2_K, co), op2_at(W3_K, wo));
+            issue_chain3<16, K, 4>(acc, acol + ACC_OUT, op2_at(H2_K, co), op2_at(W3_K, wo));
           } else if (stage == 3) {
             // dH2 = dOut W3 ; dW3^T[i][o] += sum_r H2[r][i] dOut[r][o] (must retire before H2 becomes dZ2 in place)
-            issue_chain3<1>(tz + M3_Z, I_128_64_KM, op2_at(DO_K, dob + c * 64), op2_at(W3_M, wo));
-            issue_stacked<8, 1>(ta + M3_DW3, I_128_32_MM, (accmask >> (3 * c)) & 1u, op2_at(H2_M, co),
-                                op2_at(DO_M, dob + c * 64));  // N = 32: dOut h | l
+            issue_chain3<64, MN, 1>(acc, acol + ACC_Z, op2_at(DO_K, dob + c * 64), op2_at(W3_M, wo));
+            issue_stacked<32, 8, 1>(acc, gcol + ACC_DW3, (accmask >> (3 * c)) & 1u, op2_at(H2_M, co),
+                                    op2_at(DO_M, dob + c * 64));  // N = 32: dOut h | l
             accmask |= 1u << (3 * c);
           } else if (stage == 4) {
             // both chains' stage-3 products have retired (their E4 jobs waited for them before arriving here): the
             // dOut buffer is free -> bring the NEXT tile's observations into it
             if (c == c_last && k + 1 < cta_tiles) load_x(k + 1);
             // dH1 = dZ2 W2 ; dW2[o][i] += sum_r dZ2[r][o] H1[r][i] ; db2[o] += sum_r dZ2[r][o] * 1 (ones column of X)
-            issue_chain3<4>(tz + M3_Z, I_128_64_KM, op2_at(H2_K, co), op2_at(W2_M, wo));
-            issue_stacked<8, 2>(ta + M3_DW2, I_128_64_MM, (accmask >> (3 * c + 1)) & 1u, op2_at(H2_M, co), op2_at(H1_M, co));
-            issue_stacked<8, 1>(ta + M3_DB2, I_128_16_MM, (accmask >> (3 * c + 1)) & 1u, op2_at(H2_M, co), op2_at(X_M16, xo));
+            issue_chain3<64, MN, 4>(acc, acol + ACC_Z, op2_at(H2_K, co), op2_at(W2_M, wo));
+            issue_stacked<64, 8, 2>(acc, gcol + ACC_DW2, (accmask >> (3 * c + 1)) & 1u, op2_at(H2_M, co), op2_at(H1_M, co));
+            issue_stacked<16, 8, 1>(acc, gcol + ACC_DB2, (accmask >> (3 * c + 1)) & 1u, op2_at(H2_M, co), op2_at(X_M16, xo));
             accmask |= 1u << (3 * c + 1);
           } else {
             // dW1[o][i] += sum_r dZ1[r][o] X[r][i]; column 31 (ones) collects db1.  Then the next tile's Z1.
-            issue_stacked<8, 1>(ta + M3_DW1, I_128_64_MM, (accmask >> (3 * c + 2)) & 1u, op2_at(H1_M, co), op2_at(X_M, xo));
+            issue_stacked<64, 8, 1>(acc, gcol + ACC_DW1, (accmask >> (3 * c + 2)) & 1u, op2_at(H1_M, co), op2_at(X_M, xo));
             accmask |= 1u << (3 * c + 2);
             if (k + 1 < cta_tiles) issue_z1(c, k + 1);
           }
@@ -447,8 +438,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     // Jobs run in the fixed order (policy, E1) (value, E1) (policy, E2) ... (value, E5) | next tile, all 16 warps on
     // one job at a time (16 columns each), so the MMAs a job hands over run under the other chain's next job.
     const int q = warp & 3, part = warp >> 2;
-    const int r = 32 * q + lane;                          // row of the tile == accumulator memory lane
-    const uint32_t lane_addr = (uint32_t)(32 * q) << 16;
+    const int r = 32 * q + lane;                          // row of the tile == accumulator row
     const int cs = 16 * part;
     uint32_t ph_chain = 0u;  // bit c: phase parity of chain[c]
     const float sH = pow2i(T2_H_EXP), hh = pow2i(-2 * T2_H_EXP);
@@ -471,7 +461,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     long long t_work0 = 0;
 #endif
     auto job = [&](const int c, const int stage, const long long k) {
-      const uint32_t tz = tmem + lane_addr + (uint32_t)c * M3_CHAIN;
+      const uint32_t acol = (uint32_t)c * ACC_CHAIN;
       const uint32_t so = S3_H + (uint32_t)c * S3_CHAIN;
       const uint32_t bar_ready = bars + 8 * c, bar_chain = bars + 16 + 8 * c;
       const float* scl = s_scale + 16 * c;
@@ -482,7 +472,6 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
       const bool loss_warp = part == (int)((k + 2 * c) & 3);  // rotates; the two chains use different warps
       auto arrive = [&]() {
         fence_proxy_async_smem();
-        tc_fence_before_sync();
         mbar_arrive(bar_ready);
       };
       auto wait_chain = [&]() {
@@ -491,7 +480,6 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
 #endif
         mbar_wait(bar_chain, (ph_chain >> c) & 1u);
         ph_chain ^= 1u << c;
-        tc_fence_after_sync();
 #ifdef B200RL_TC3_TIMING
         {
           const long long w1 = clock64();
@@ -506,11 +494,10 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
         const float unscale = scl[stage == 1 ? C3_U1 : C3_U2];
         const float* bs = bias + (stage == 1 ? 0 : 64);
         const uint32_t dst = so + (stage == 1 ? 0u : 2 * T2_ACT);
-        uint32_t v[16];
-        acc_ld16(tz + M3_Z + cs, v);
         float z[16];
+        acc_ld<16>(acc, r, acol + ACC_Z + cs, z);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) z[j] = fmaf(__uint_as_float(v[j]), unscale, bs[cs + j]);
+        for (int j = 0; j < 16; ++j) z[j] = fmaf(z[j], unscale, bs[cs + j]);
         tanh16_scaled(z, sH);  // tanh(z) * 2^14
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
@@ -543,13 +530,13 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
           }
           wait_chain();
           if (loss_warp) {
-            uint32_t o[16];
-            acc_ld16(tz + M3_OUT, o);
+            float o[16];
+            acc_ld<16>(acc, r, acol + ACC_OUT, o);
             float out[16], dout[16];
             const float u3 = scl[C3_U3];
 #pragma unroll
             for (int a = 0; a < 16; ++a) {
-              out[a] = fmaf(__uint_as_float(o[a]), u3, bias[128 + a]);
+              out[a] = fmaf(o[a], u3, bias[128 + a]);
               dout[a] = 0.f;
             }
             if (valid) {
@@ -619,10 +606,10 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
           if (loss_warp && valid) pf_tgt = __ldg(p.target + row);
           wait_chain();
           if (loss_warp) {
-            uint32_t o[8];
-            acc_ld8(tz + M3_OUT, o);
+            float o[8];
+            acc_ld<8>(acc, r, acol + ACC_OUT, o);
             if (valid) {  // ppo.py:282-287
-              const float vout = fmaf(__uint_as_float(o[0]), scl[C3_U3], bias[128]);
+              const float vout = fmaf(o[0], scl[C3_U3], bias[128]);
               const float diff = vout - pf_tgt;
               const float dout = (2.f * diff) * p.inv_n;
               vs += (double)(diff * diff);
@@ -666,14 +653,14 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
         const float unscale = scl[stage == 4 ? C3_UH2 : C3_UH1] * hh;
         const uint32_t buf = so + (stage == 4 ? 2 * T2_ACT : 0u);
         const float one28 = 268435456.f;
-        uint32_t g[16];
-        acc_ld16(tz + M3_Z + cs, g);
+        float g[16];
+        acc_ld<16>(acc, r, acol + ACC_Z + cs, g);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8];
           load_chunk2(sm, buf, r, (cs >> 3) + ch, x);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) x[j] = (__uint_as_float(g[8 * ch + j]) * unscale) * fmaf(-x[j], x[j], one28);
+          for (int j = 0; j < 8; ++j) x[j] = (g[8 * ch + j] * unscale) * fmaf(-x[j], x[j], one28);
           if (too_large8(x)) bad = true;
           store_chunk2(sm, buf, r, (cs >> 3) + ch, x);
         }
@@ -704,46 +691,41 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     // ---- per-CTA results ----
     if (cta_tiles > 0) {
 #pragma unroll 1
-      for (int c = c_first; c <= c_last; ++c) {  // the last dW1 of each chain
+      for (int c = c_first; c <= c_last; ++c)  // the last dW1 of each chain
         mbar_wait(bars + 16 + 8 * c, (ph_chain >> c) & 1u);
-        tc_fence_after_sync();
-      }
     }
-    tc_fence_before_sync();
     asm volatile("bar.sync 2, %0;" ::"n"(T3_EPI_THREADS) : "memory");  // every MMA of the CTA has retired
-    tc_fence_after_sync();
     {
-      // stacked accumulators: lanes 0..63 = h-split half (partial row 2b), lanes 64..127 = l-split half (row 2b + 1);
+      // stacked accumulators: rows 0..63 = h-split half (partial row 2b), rows 64..127 = l-split half (row 2b + 1);
       // 8 jobs per net (dW2 x 4 column blocks, dW1 x 2, dW3, db2); warp `part` takes jobs part, part + 4 of both nets
       float* dst_row = p.partials + ((size_t)blockIdx.x * 2 + (q >> 1)) * (size_t)(p.P[0] + p.P[1]);
       const int m = 32 * (q & 1) + lane;  // feature index
-      const uint32_t ta = tmem + lane_addr + M3_ACC;
-      uint32_t v[16], w[16];
+      float v[16], w[16];
 #pragma unroll 1
       for (int c = c_first; c <= c_last; ++c) {
         const Tc3Net& nn = p.net[c];
         float* dst = dst_row + (c == 0 ? 0 : p.P[0]);
         const float* scl = s_scale + 16 * c;
         const bool have = cta_tiles > 0;
-        const uint32_t tn = ta + c * M3_ACC_NET;
+        const uint32_t gcol = ACC_GRAD + c * ACC_GRAD_NET;
 #pragma unroll 1
         for (int jb = part; jb < 8; jb += 4) {
           // columns of this job, and of its second half where the operand's l columns went to their own block
-          const uint32_t col = jb < 4 ? M3_DW2 + 16 * jb : (jb < 6 ? M3_DW1 + 16 * (jb - 4) : (jb == 6 ? M3_DW3 : M3_DB2));
+          const uint32_t col = jb < 4 ? ACC_DW2 + 16 * jb : (jb < 6 ? ACC_DW1 + 16 * (jb - 4) : (jb == 6 ? ACC_DW3 : ACC_DB2));
           const uint32_t col2 = jb < 4 ? col : (jb < 6 ? col + 32 : (jb == 6 ? col + 16 : col));
           if (have) {
-            acc_ld16(tn + col, v);
-            acc_ld16(tn + col2, w);
+            acc_ld<16>(acc, r, gcol + col, v);
+            acc_ld<16>(acc, r, gcol + col2, w);
           } else {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = w[j] = 0u;  // a CTA without tiles: accumulator memory was never written
+            for (int j = 0; j < 16; ++j) v[j] = w[j] = 0.f;  // a CTA without tiles: accumulator memory was never written
           }
           if (jb < 4) {  // dW2 [h2 o][h1 i]: columns 16 jb .. +15
             const float u = scl[C3_OW2];
             if (m < nn.h2)
 #pragma unroll
               for (int j = 0; j < 16; ++j)
-                if (16 * jb + j < nn.h1) dst[nn.w_off[1] + m * nn.h1 + 16 * jb + j] = __uint_as_float(v[j]) * u;
+                if (16 * jb + j < nn.h1) dst[nn.w_off[1] + m * nn.h1 + 16 * jb + j] = v[j] * u;
           } else if (jb < 6) {  // dW1 [h1 o][n_in i] in columns 0..30, db1 in column 31
             const int c0 = 16 * (jb - 4);
             const float u = scl[C3_OW1];
@@ -751,18 +733,17 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
 #pragma unroll
               for (int j = 0; j < 16; ++j)
                 if (c0 + j < n_in)
-                  dst[nn.w_off[0] + m * n_in + c0 + j] =
-                      ((__uint_as_float(v[j]) + __uint_as_float(w[j])) * u) * s_xs[32 + c0 + j];
-              if (jb == 5) dst[nn.b_off[0] + m] = (__uint_as_float(v[15]) + __uint_as_float(w[15])) * scl[C3_OB];
+                  dst[nn.w_off[0] + m * n_in + c0 + j] = ((v[j] + w[j]) * u) * s_xs[32 + c0 + j];
+              if (jb == 5) dst[nn.b_off[0] + m] = (v[15] + w[15]) * scl[C3_OB];
             }
           } else if (jb == 6) {  // dW3^T [h2 i][16 o]
             const float u = scl[C3_OW3];
             if (m < nn.h2)
 #pragma unroll
               for (int a = 0; a < 15; ++a)
-                if (a < nn.n_out) dst[nn.w_off[2] + a * nn.h2 + m] = (__uint_as_float(v[a]) + __uint_as_float(w[a])) * u;
+                if (a < nn.n_out) dst[nn.w_off[2] + a * nn.h2 + m] = (v[a] + w[a]) * u;
           } else {  // db2 (column 15 = sum_r dZ2[r][o] * ones)
-            if (m < nn.h2) dst[nn.b_off[1] + m] = __uint_as_float(v[15]) * scl[C3_OB];
+            if (m < nn.h2) dst[nn.b_off[1] + m] = v[15] * scl[C3_OB];
           }
         }
       }
@@ -831,7 +812,6 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   }
 
   // ---- teardown ----
-  tc_fence_before_sync();
   __syncthreads();
   if (tid == 0 && *s_bad != 0) *p.status = 1.0f;  // sticky: the engine redoes the update on the wide-range path
 }
@@ -1046,13 +1026,6 @@ int tc3_configure() {
 
 size_t tc3_ximg_bytes(int64_t n_rows) { return (size_t)((n_rows + T3_ROWS - 1) / T3_ROWS) * T2_ACT; }
 
-int tc3_grid(int64_t n_rows) {
-  const int64_t tiles = (n_rows + T3_ROWS - 1) / T3_ROWS;
-  const int sms = device_sm_count();
-  if (sms <= 0) return -1;
-  return (int)(tiles < sms ? (tiles < 1 ? 1 : tiles) : sms);
-}
-
 bool tc3_shape_ok(const b200rl_mlp_desc& pol, const b200rl_mlp_desc& val) {
   auto ok = [](const b200rl_mlp_desc& d) {
     return d.n_layers == 3 && d.hidden_act == B200RL_ACT_TANH && d.out_act == B200RL_ACT_IDENTITY && d.sizes[0] >= 1 &&
@@ -1075,7 +1048,7 @@ int launch_pack_obs(const float* obs, int64_t n_rows, int n_in, const float* abs
 
 int launch_mlp_tc3(const Tc3Args& k, cudaStream_t s) {
   if (tc3_configure()) return 1;
-  const int grid = tc3_grid(k.n_rows);
+  const int grid = tc_grid(k.n_rows);
   B200RL_REQUIRE(grid > 0, "mlp_tc3: no CUDA device");
   Tc3Args kk = k;
   kk.acc_mem = acc_mem(grid, s);

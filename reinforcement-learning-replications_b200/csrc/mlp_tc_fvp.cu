@@ -44,16 +44,16 @@ constexpr uint32_t SF_BIAS = SF_OPERANDS_END;   // b1[64] b2[64] b3[16] | vb1[64
 constexpr uint32_t SF_DIST = SF_BIAS + 1152;    // 1/var[16] floats
 constexpr uint32_t SF_SCALE = SF_DIST + 64;     // scale factors
 constexpr uint32_t SF_RED = SF_SCALE + 128;     // block reduction scratch [20 warps][8] floats (read-out: [4][16] + 4 + 4)
-constexpr uint32_t SF_BARS = SF_RED + 640;      // mbarriers ready, chain, off; accumulator base address (acc_bind); bad flag
+constexpr uint32_t SF_BARS = SF_RED + 640;      // mbarriers ready, chain, off; bad flag
 constexpr uint32_t SF_XS = SF_BARS + 64;        // per-feature observation scales [32] and inverses [32]
 constexpr uint32_t SF_ROWMAX = SF_XS + 256;     // [128] largest scaled |obs| of each row (precision guard)
 constexpr uint32_t SF_TOTAL = SF_ROWMAX + 512;
 constexpr uint32_t FV_SMEM_BYTES = SF_TOTAL + 1024;
 static_assert(FV_SMEM_BYTES <= 227 * 1024, "mlp_tc_fvp shared memory");
 
-// tensor-memory columns
-constexpr uint32_t MF_Z1 = 0, MF_ZB = 64, MF_OUT = 128, MF_TZ = 144, MF_TOUT = 208;
-constexpr uint32_t MF_DW2 = 288, MF_DW1 = 352, MF_DW3 = 400, MF_DB2 = 416;
+// accumulator columns
+constexpr uint32_t ACC_Z1 = 0, ACC_ZB = 64, ACC_OUT = 128, ACC_TZ = 144, ACC_TOUT = 208;
+constexpr uint32_t ACC_DW2 = 288, ACC_DW1 = 352, ACC_DW3 = 400, ACC_DB2 = 416;
 
 enum {
   FS_X = 0, FS_G, FS_U1, FS_U2, FS_U3, FS_UT1, FS_UT2, FS_UT3, FS_T1, FS_T2, FS_UH2, FS_UH1, FS_OW3, FS_OW2, FS_OW1,
@@ -85,6 +85,7 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
   if (p.skip_flag != nullptr && *p.skip_flag != 0) return;
 
   const int tid = threadIdx.x, lane = tid & 31;
+  float* const acc = p.acc_mem + (size_t)blockIdx.x * ACC_CTA_FLOATS;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // provably warp-uniform: role branches need no vote
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
@@ -94,8 +95,7 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
   float* s_ivar = reinterpret_cast<float*>(sm + SF_DIST);
   float* s_scale = reinterpret_cast<float*>(sm + SF_SCALE);
   float* s_red = reinterpret_cast<float*>(sm + SF_RED);
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(sm + SF_BARS + 48);
-  int* s_bad = reinterpret_cast<int*>(sm + SF_BARS + 52);
+  int* s_bad = reinterpret_cast<int*>(sm + SF_BARS + 48);
   const uint32_t bars = base + SF_BARS;  // ready +0, chain +8, off +16
   const int n_in = p.n_in, A_out = p.n_out, h1 = p.h1, h2 = p.h2;
   bool bad = false;
@@ -234,7 +234,6 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
   }
   if (bad) *s_bad = 1;  // non-finite bias
   bad = false;
-  if (tid == 0) acc_bind(p.acc_mem, s_tmem);
   if (tid == 0) {
     mbar_init(bars, FV_EPI_THREADS);
     mbar_init(bars + 8, 1);
@@ -242,19 +241,14 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
     fence_mbar_init();
   }
   fence_proxy_async_smem();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = *s_tmem;
   const long long num_tiles = (p.n_rows + FV_ROWS - 1) / FV_ROWS;
   const long long cta_tiles = (num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;
 
   if (warp >= FV_EPI_WARPS) {
-    // =============================== MMA issuer warp =================================================
-    constexpr uint32_t I_128_64_KK = make_idesc_f16(128, 64, 0, 0), I_128_16_KK = make_idesc_f16(128, 16, 0, 0),
-                       I_128_64_KM = make_idesc_f16(128, 64, 0, 1), I_128_64_MM = make_idesc_f16(128, 64, 1, 1),
-                       I_128_48_MM = make_idesc_f16(128, 48, 1, 1), I_128_16_MM = make_idesc_f16(128, 16, 1, 1);
-    const uint32_t ub = base, ut = 0u;  // accumulator address of column 0 of this CTA's block (acc_bind)
+    // =============================== MMA issuer warpgroup ============================================
+    constexpr int K = K_MAJOR, MN = MN_MAJOR;
+    const uint32_t ub = base;
     const Op2 XD_K = op2_kmajor(ub + SF_XD, T2_ACT), H1_K = op2_kmajor(ub + SF_H1, T2_ACT),
               H2_K = op2_kmajor(ub + SF_H2, T2_ACT), T1_K = op2_kmajor(ub + SF_T1, T2_ACT),
               T2_K = op2_kmajor(ub + SF_T2, T2_ACT), XD_K2 = op2_kmajor(ub + SF_XD + 64, T2_ACT);
@@ -266,40 +260,40 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
     const Op2 V1T_M = op2_mnmajor(ub + SF_V1T, 32 * 128, FV_W1T), V2_K = op2_kmajor(ub + SF_V2, FV_W),
               V3_K = op2_kmajor(ub + SF_V3, FV_W3);
     uint32_t par = 0u;
-    bool acc = false;
+    bool accum = false;
     for (long long k = 0; k < cta_tiles; ++k) {
 #pragma unroll 1
       for (int stage = 0; stage < 6; ++stage) {
         mbar_wait(bars, par);
         par ^= 1u;
-        tc_fence_after_sync();
+        // issue_chain3 <N, B major, k-steps[, accumulate]>, issue_stacked <N, k-steps, B splits>
         if (stage == 0) {  // Z1 = X W1^T ; TZ = X V1^T
-          issue_chain3<2>(ut + MF_Z1, I_128_64_KM, XD_K, W1T_M);
-          issue_chain3<2>(ut + MF_TZ, I_128_64_KM, XD_K, V1T_M);
+          issue_chain3<64, MN, 2>(acc, ACC_Z1, XD_K, W1T_M);
+          issue_chain3<64, MN, 2>(acc, ACC_TZ, XD_K, V1T_M);
           acc_commit(bars + 8);
         } else if (stage == 1) {  // Z2 = H1 W2^T ; TZ = T1 W2^T + H1 V2^T
-          issue_chain3<4>(ut + MF_ZB, I_128_64_KK, H1_K, W2_K);
-          issue_chain3<4>(ut + MF_TZ, I_128_64_KK, T1_K, W2_K);
-          issue_chain3<4, true>(ut + MF_TZ, I_128_64_KK, H1_K, V2_K);
+          issue_chain3<64, K, 4>(acc, ACC_ZB, H1_K, W2_K);
+          issue_chain3<64, K, 4>(acc, ACC_TZ, T1_K, W2_K);
+          issue_chain3<64, K, 4, true>(acc, ACC_TZ, H1_K, V2_K);
           acc_commit(bars + 8);
         } else if (stage == 2) {  // OUT = H2 W3^T ; TOUT = T2 W3^T + H2 V3^T
-          issue_chain3<4>(ut + MF_OUT, I_128_16_KK, H2_K, W3_K);
-          issue_chain3<4>(ut + MF_TOUT, I_128_16_KK, T2_K, W3_K);
-          issue_chain3<4, true>(ut + MF_TOUT, I_128_16_KK, H2_K, V3_K);
+          issue_chain3<16, K, 4>(acc, ACC_OUT, H2_K, W3_K);
+          issue_chain3<16, K, 4>(acc, ACC_TOUT, T2_K, W3_K);
+          issue_chain3<16, K, 4, true>(acc, ACC_TOUT, H2_K, V3_K);
           acc_commit(bars + 8);
         } else if (stage == 3) {  // dH2 = dOut W3 ; dW3^T += H2^T dOut (must retire before H2 becomes dZ2)
-          issue_chain3<1>(ut + MF_ZB, I_128_64_KM, XD_K2, W3_M);
-          issue_stacked<8, 2>(ut + MF_DW3, I_128_16_MM, acc, H2_M, XD_M32);
+          issue_chain3<64, MN, 1>(acc, ACC_ZB, XD_K2, W3_M);
+          issue_stacked<16, 8, 2>(acc, ACC_DW3, accum, H2_M, XD_M32);
           acc_commit(bars + 8);
         } else if (stage == 4) {  // dH1 = dZ2 W2 ; dW2 += dZ2^T H1 ; db2 += dZ2^T 1
-          issue_chain3<4>(ut + MF_ZB, I_128_64_KM, H2_K, W2_M);
-          issue_stacked<8, 2>(ut + MF_DW2, I_128_64_MM, acc, H2_M, H1_M);
-          issue_stacked<8, 1>(ut + MF_DB2, I_128_16_MM, acc, H2_M, XD_M32);
+          issue_chain3<64, MN, 4>(acc, ACC_ZB, H2_K, W2_M);
+          issue_stacked<64, 8, 2>(acc, ACC_DW2, accum, H2_M, H1_M);
+          issue_stacked<16, 8, 1>(acc, ACC_DB2, accum, H2_M, XD_M32);
           acc_commit(bars + 8);
         } else {  // dW1 += dZ1^T X, db1 through the ones column
-          issue_stacked<8, 2>(ut + MF_DW1, I_128_48_MM, acc, H1_M, XD_M0);
+          issue_stacked<48, 8, 2>(acc, ACC_DW1, accum, H1_M, XD_M0);
           acc_commit(bars + 16);
-          acc = true;
+          accum = true;
         }
         __syncwarp();
       }
@@ -307,9 +301,7 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
   } else {
     // =============================== epilogue warps ==================================================
     const int q = warp & 3, half = warp >> 2;  // lane group, column group (16 columns each)
-    const int r = 32 * q + lane;
-    const uint32_t lane_addr = (uint32_t)(32 * q) << 16;
-    const uint32_t tz = tmem + lane_addr;
+    const int r = 32 * q + lane;  // row of the tile == accumulator row
     const int cs = 16 * half;
     uint32_t ph_chain = 0, ph_off = 0;
     const float sH = pow2i(T2_H_EXP);
@@ -322,29 +314,24 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
 
     auto epi_arrive = [&]() {
       fence_proxy_async_smem();
-      tc_fence_before_sync();
       mbar_arrive(bars);
     };
     auto wait_chain = [&]() {
       mbar_wait(bars + 8, ph_chain);
       ph_chain ^= 1u;
-      tc_fence_after_sync();
     };
     // forward + tangent epilogue of a tanh layer: H = tanh(Z u + b) -> fp16 splits (and fp32 to accumulator memory when kept);
     // T = (1 - H^2) (TZ ut + vb) -> fp16 splits of the tangent buffer
-    auto layer_epilogue = [&](uint32_t tm_z, const float* bias, const float* vbias, float unscale, float unscale_t,
+    auto layer_epilogue = [&](uint32_t acc_z, const float* bias, const float* vbias, float unscale, float unscale_t,
                               float t_scale, uint32_t dst_h, uint32_t dst_t, bool keep_fp32) {
       {
-        uint32_t v[16], w[16];
-        acc_ld16(tz + tm_z + cs, v);
-        acc_ld16(tz + MF_TZ + cs, w);
-        float z[16];
+        float z[16], w[16];
+        acc_ld<16>(acc, r, acc_z + cs, z);
+        acc_ld<16>(acc, r, ACC_TZ + cs, w);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) z[j] = fmaf(__uint_as_float(v[j]), unscale, bias[cs + j]);
+        for (int j = 0; j < 16; ++j) z[j] = fmaf(z[j], unscale, bias[cs + j]);
         tanh16_scaled(z, 1.f);  // Z is finite: observations, weights and biases were all checked
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(z[j]);
-        if (keep_fp32) acc_st16(tz + tm_z + cs, v);
+        if (keep_fp32) acc_st<16>(acc, r, acc_z + cs, z);
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           float x[8], t[8];
@@ -352,7 +339,7 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
           for (int j = 0; j < 8; ++j) {
             const float h = z[8 * ch + j];
             x[j] = h * sH;
-            t[j] = (fmaf(__uint_as_float(w[8 * ch + j]), unscale_t, vbias[cs + 8 * ch + j]) * fmaf(-h, h, 1.f)) * t_scale;
+            t[j] = (fmaf(w[8 * ch + j], unscale_t, vbias[cs + 8 * ch + j]) * fmaf(-h, h, 1.f)) * t_scale;
           }
           if (out_of_range8(t)) bad = true;
           store_chunk2(sm, dst_h, r, (cs >> 3) + ch, x);
@@ -374,7 +361,6 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
         if (!first) {
           mbar_wait(bars + 16, ph_off);
           ph_off ^= 1u;
-          tc_fence_after_sync();
         }
         first = false;
         float rmax = 0.f;
@@ -391,7 +377,7 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
       for (int layer = 0; layer < 2; ++layer) {  // one copy of the (large) layer epilogue: instruction-cache pressure
         epi_arrive();
         wait_chain();
-        layer_epilogue(layer == 0 ? MF_Z1 : MF_ZB, s_bias + 64 * layer, s_vb + 64 * layer,
+        layer_epilogue(layer == 0 ? ACC_Z1 : ACC_ZB, s_bias + 64 * layer, s_vb + 64 * layer,
                        s_scale[layer == 0 ? FS_U1 : FS_U2], s_scale[layer == 0 ? FS_UT1 : FS_UT2],
                        s_scale[layer == 0 ? FS_T1 : FS_T2], layer == 0 ? SF_H1 : SF_H2, layer == 0 ? SF_T1 : SF_T2,
                        layer == 0);
@@ -405,9 +391,9 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
           s_rowmax[r] = 0.f;
           if (valid && rm > 0.f && rm < 0.03125f) bad = true;
         }
-        uint32_t o[16], t[16];
-        acc_ld16(tz + MF_OUT, o);
-        acc_ld16(tz + MF_TOUT, t);
+        float o[16], t[16];
+        acc_ld<16>(acc, r, ACC_OUT, o);
+        acc_ld<16>(acc, r, ACC_TOUT, t);
         float dout[16];
 #pragma unroll
         for (int a = 0; a < 16; ++a) dout[a] = 0.f;
@@ -415,7 +401,7 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
           float tout[16];
           const float ut3 = s_scale[FS_UT3];
 #pragma unroll
-          for (int a = 0; a < 16; ++a) tout[a] = fmaf(__uint_as_float(t[a]), ut3, s_vb[128 + a]);
+          for (int a = 0; a < 16; ++a) tout[a] = fmaf(t[a], ut3, s_vb[128 + a]);
           if (p.dist == B200RL_DIST_GAUSSIAN) {
 #pragma unroll
             for (int a = 0; a < 15; ++a)
@@ -424,7 +410,7 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
             float out[16];
             const float u3 = s_scale[FS_U3];
 #pragma unroll
-            for (int a = 0; a < 16; ++a) out[a] = fmaf(__uint_as_float(o[a]), u3, s_bias[128 + a]);
+            for (int a = 0; a < 16; ++a) out[a] = fmaf(o[a], u3, s_bias[128 + a]);
             float m = out[0];
 #pragma unroll
             for (int a = 1; a < 15; ++a)
@@ -482,15 +468,15 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
       {
         const float unscale = s_scale[FS_UH2], hh = pow2i(-2 * T2_H_EXP);
         {
-          uint32_t g[16];
-          acc_ld16(tz + MF_ZB + cs, g);
+          float g[16];
+          acc_ld<16>(acc, r, ACC_ZB + cs, g);
 #pragma unroll
           for (int ch = 0; ch < 2; ++ch) {
             float x[8];
             load_chunk2(sm, SF_H2, r, (cs >> 3) + ch, x);
 #pragma unroll
             for (int j = 0; j < 8; ++j)
-              x[j] = (__uint_as_float(g[8 * ch + j]) * unscale) * fmaf(-(x[j] * hh), x[j], 1.f);
+              x[j] = (g[8 * ch + j] * unscale) * fmaf(-(x[j] * hh), x[j], 1.f);
             if (too_large8(x)) bad = true;
             store_chunk2(sm, SF_H2, r, (cs >> 3) + ch, x);
           }
@@ -501,16 +487,16 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
       {
         const float unscale = s_scale[FS_UH1];
         {
-          uint32_t g[16], h[16];
-          acc_ld16(tz + MF_ZB + cs, g);
-          acc_ld16(tz + MF_Z1 + cs, h);
+          float g[16], h[16];
+          acc_ld<16>(acc, r, ACC_ZB + cs, g);
+          acc_ld<16>(acc, r, ACC_Z1 + cs, h);
 #pragma unroll
           for (int ch = 0; ch < 2; ++ch) {
             float x[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-              const float hv = __uint_as_float(h[8 * ch + j]);
-              x[j] = (__uint_as_float(g[8 * ch + j]) * unscale) * (1.f - hv * hv);
+              const float hv = h[8 * ch + j];
+              x[j] = (g[8 * ch + j] * unscale) * (1.f - hv * hv);
             }
             if (too_large8(x)) bad = true;
             store_chunk2(sm, SF_H1, r, (cs >> 3) + ch, x);
@@ -521,51 +507,48 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
     }
 
     // ---- per-CTA results ----
-    if (!first) {
-      mbar_wait(bars + 16, ph_off);
-      tc_fence_after_sync();
-    }
+    if (!first) mbar_wait(bars + 16, ph_off);
     {
       float* dst = p.partials + ((size_t)blockIdx.x * 2 + (q >> 1)) * p.P;
       const int m = 32 * (q & 1) + lane;
-      uint32_t v[16];
+      float v[16];
       // column groups 0, 1: dW2 (32 columns each); 2: dW1 + db1; 3: dW3^T, db2
       if (half < 2) {
 #pragma unroll
         for (int c2 = 0; c2 < 2; ++c2) {
           const int cb = 2 * half + c2;
-          acc_ld16(tz + MF_DW2 + 16 * cb, v);
+          acc_ld<16>(acc, r, ACC_DW2 + 16 * cb, v);
           const float u = s_scale[FS_OW2];
           if (m < h2)
 #pragma unroll
             for (int j = 0; j < 16; ++j)
-              if (16 * cb + j < h1) dst[p.w_off[1] + m * h1 + 16 * cb + j] = __uint_as_float(v[j]) * u;
+              if (16 * cb + j < h1) dst[p.w_off[1] + m * h1 + 16 * cb + j] = v[j] * u;
         }
       } else if (half == 2) {
 #pragma unroll
         for (int cb = 0; cb < 3; ++cb) {
-          acc_ld16(tz + MF_DW1 + 16 * cb, v);
+          acc_ld<16>(acc, r, ACC_DW1 + 16 * cb, v);
           if (m < h1) {
             if (cb < 2) {
               const float u = s_scale[FS_OW1];
 #pragma unroll
               for (int j = 0; j < 16; ++j)
                 if (16 * cb + j < n_in)
-                  dst[p.w_off[0] + m * n_in + 16 * cb + j] = (__uint_as_float(v[j]) * u) * s_xs[32 + 16 * cb + j];
+                  dst[p.w_off[0] + m * n_in + 16 * cb + j] = (v[j] * u) * s_xs[32 + 16 * cb + j];
             } else {
-              dst[p.b_off[0] + m] = __uint_as_float(v[15]) * s_scale[FS_OB];
+              dst[p.b_off[0] + m] = v[15] * s_scale[FS_OB];
             }
           }
         }
       } else {
-        acc_ld16(tz + MF_DW3, v);
+        acc_ld<16>(acc, r, ACC_DW3, v);
         const float u = s_scale[FS_OW3];
         if (m < h2)
 #pragma unroll
           for (int a = 0; a < 15; ++a)
-            if (a < A_out) dst[p.w_off[2] + a * h2 + m] = __uint_as_float(v[a]) * u;
-        acc_ld16(tz + MF_DB2, v);
-        if (m < h2) dst[p.b_off[1] + m] = __uint_as_float(v[15]) * s_scale[FS_OB];
+            if (a < A_out) dst[p.w_off[2] + a * h2 + m] = v[a] * u;
+        acc_ld<16>(acc, r, ACC_DB2, v);
+        if (m < h2) dst[p.b_off[1] + m] = v[15] * s_scale[FS_OB];
       }
       if (half == 0) {
 #pragma unroll
@@ -596,13 +579,11 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
     if (bad) *s_bad = 1;
   }
 
-  tc_fence_before_sync();
   __syncthreads();
   if (tid == 0 && *s_bad != 0) *p.status = p.seq;  // redone by the fp32 kernel queued behind this launch
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------
-int tc2_grid(int64_t n_rows);
 int tc2_take_slot(unsigned** status, unsigned* seq, float** scratch);
 int launch_absmax_cols(const float* x, long long rows, int cols, float* out, cudaStream_t s);
 int launch_fused_fallback(const b200rl_mlp_loss_grad_args* a, const unsigned* run_if, unsigned seq, int total_rows,
@@ -623,14 +604,7 @@ int launch_mlp_tc_fvp(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, int to
   k.h1 = a->mlp.sizes[1];
   k.h2 = a->mlp.sizes[2];
   k.n_out = a->mlp.sizes[3];
-  int off = 0;
-  for (int l = 0; l < 3; ++l) {
-    k.w_off[l] = off;
-    off += a->mlp.sizes[l + 1] * a->mlp.sizes[l];
-    k.b_off[l] = off;
-    off += a->mlp.sizes[l + 1];
-  }
-  k.P = off;
+  k.P = mlp3_offsets(a->mlp, k.w_off, k.b_off);
   k.dist = a->dist;
   k.n_rows = a->n_rows;
   k.inv_n = 1.0f / (float)n_glob;
@@ -652,7 +626,7 @@ int launch_mlp_tc_fvp(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, int to
   } else {
     k.obs_absmax = a->obs_absmax;
   }
-  const int grid = tc2_grid(a->n_rows);
+  const int grid = tc_grid(a->n_rows);
   B200RL_REQUIRE(grid > 0, "mlp_tc_fvp: no CUDA device");
   k.acc_mem = acc_mem(grid, s);
   B200RL_REQUIRE(k.acc_mem != nullptr, "mlp_tc_fvp: no accumulator memory (allocation failed, or the stream is being captured): %s",

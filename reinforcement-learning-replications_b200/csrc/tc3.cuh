@@ -71,7 +71,6 @@ struct Ra3Args {
 
 bool tc3_shape_ok(const b200rl_mlp_desc& pol, const b200rl_mlp_desc& val);
 size_t tc3_ximg_bytes(int64_t n_rows);
-int tc3_grid(int64_t n_rows);
 int launch_pack_obs(const float* obs, int64_t n_rows, int n_in, const float* absmax, uint8_t* ximg, float* xscale,
                     float* bad_flag, cudaStream_t s);
 int launch_mlp_tc3(const Tc3Args& k, cudaStream_t s);

@@ -1,17 +1,17 @@
 // Hand-written sm_90a primitives of the tensor-core kernels: warpgroup MMA (wgmma) on shared-memory descriptors,
-// the per-CTA accumulator memory the kernels address by (lane, column), mbarrier and proxy fences.
+// the per-CTA accumulator memory the kernels address by (row, column), mbarrier and proxy fences.
 // PTX spellings follow the CUDA 12.9 ISA.
 //
 // Work split.  The epilogue warps of a kernel hold one row of a 128-row tile per thread and read or write
-// accumulators as (lane = row, column) pairs; one warpgroup (four warps) issues the products.  A product
+// accumulators by (row, column); one warpgroup (four warps) issues the products.  A product
 // D[M x N] (+)= sum_t A_t B_t runs as wgmma m64nNk16 over each 64-row half of M, with the accumulator fragment in the
 // issuing warpgroup's registers: it is loaded from the accumulator memory when the product accumulates, and stored
 // back when the product is done.  The issuing warpgroup then arrives once on the stage's mbarrier (acc_commit).
 //
 // Accumulator memory.  An H100 SM has 227 KB of shared memory for a block and the kernels' operand buffers fill most
-// of it, so the fp32 accumulators (up to 512 columns x 128 lanes = 256 KB per CTA) live in a per-launch global buffer
-// of gridDim.x such blocks, column-major (a warp reading one column of its 32 lanes touches one 128-byte line).  It is
-// written and read back by the same CTA within a tile's stages, so it stays in the 50 MB L2.
+// of it, so the fp32 accumulators (up to 512 columns x 128 rows = 256 KB per CTA) live in a per-launch global buffer
+// of gridDim.x such blocks, column-major (ACC_LANES floats per column).  It is written and read back by the same CTA
+// within a tile's stages, so it stays in the 50 MB L2.
 #pragma once
 #include <cstdint>
 
@@ -51,47 +51,32 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   __trap();
 }
 
-// ---- proxy fences ----------------------------------------------------------------------------------------------
+// ---- proxy fence ----------------------------------------------------------------------------------------------
 // generic-proxy shared-memory writes (operand buffers) -> visible to wgmma, which reads through the async proxy
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// accumulator memory is ordinary global memory: the mbarrier arrive / wait pairs (release / acquire) order it; these
-// mark the hand-over points for the compiler
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("" ::: "memory"); }
 
 // ---- accumulator memory ----------------------------------------------------------------------------------------
+// Accumulator memory is ordinary global memory: the mbarrier arrive / wait pairs (release / acquire) and the named
+// barriers order it between the issuing warpgroup and the epilogue warps.
 constexpr uint32_t ACC_COLS = 512, ACC_LANES = 128;
 constexpr size_t ACC_CTA_FLOATS = (size_t)ACC_COLS * ACC_LANES;
 
-static __shared__ float* s_acc_cta;  // this CTA's block of the launch's accumulator memory
+// `acc` below is the CTA's block: acc_mem + blockIdx.x * ACC_CTA_FLOATS.
 
-// one thread, before the block's first __syncthreads: binds the CTA's block and writes accumulator address 0 (lane 0,
-// column 0) into `holder`.  Addresses are (lane << 16) | column, as the kernels compute them.
-__device__ __forceinline__ void acc_bind(float* acc_mem, uint32_t* holder) {
-  s_acc_cta = acc_mem + (size_t)blockIdx.x * ACC_CTA_FLOATS;
-  *holder = 0u;
-}
-__device__ __forceinline__ float* acc_ptr(uint32_t taddr) {  // this thread's lane of the warp at `taddr`
-  return s_acc_cta + (taddr & 0xFFFFu) * ACC_LANES + (taddr >> 16) + (threadIdx.x & 31u);
-}
-// N consecutive columns of one lane per thread (thread i of the warp = lane (taddr >> 16) + i)
+// N consecutive columns from `col` of accumulator row `row`.  The epilogue threads hold one row each, so a warp reading
+// one column of its 32 rows touches one 128-byte line.
 template <int N>
-__device__ __forceinline__ void acc_ld(uint32_t taddr, uint32_t (&v)[N]) {
-  const float* p = acc_ptr(taddr);
+__device__ __forceinline__ void acc_ld(const float* acc, int row, uint32_t col, float (&v)[N]) {
+  const float* p = acc + col * ACC_LANES + row;
 #pragma unroll
-  for (int j = 0; j < N; ++j) v[j] = __float_as_uint(p[j * ACC_LANES]);
+  for (int j = 0; j < N; ++j) v[j] = p[j * ACC_LANES];
 }
 template <int N>
-__device__ __forceinline__ void acc_st(uint32_t taddr, const uint32_t (&v)[N]) {
-  float* p = acc_ptr(taddr);
+__device__ __forceinline__ void acc_st(float* acc, int row, uint32_t col, const float (&v)[N]) {
+  float* p = acc + col * ACC_LANES + row;
 #pragma unroll
-  for (int j = 0; j < N; ++j) p[j * ACC_LANES] = __uint_as_float(v[j]);
+  for (int j = 0; j < N; ++j) p[j * ACC_LANES] = v[j];
 }
-__device__ __forceinline__ void acc_ld8(uint32_t taddr, uint32_t (&v)[8]) { acc_ld<8>(taddr, v); }
-__device__ __forceinline__ void acc_ld16(uint32_t taddr, uint32_t (&v)[16]) { acc_ld<16>(taddr, v); }
-__device__ __forceinline__ void acc_ld32(uint32_t taddr, uint32_t (&v)[32]) { acc_ld<32>(taddr, v); }
-__device__ __forceinline__ void acc_st16(uint32_t taddr, const uint32_t (&v)[16]) { acc_st<16>(taddr, v); }
-__device__ __forceinline__ void acc_st32(uint32_t taddr, const uint32_t (&v)[32]) { acc_st<32>(taddr, v); }
 
 // The issuing warpgroup's products are complete and stored: one arrive on `bar` (count 1) for the whole warpgroup.
 // Named barrier 8 is reserved for the issuing warpgroup (the epilogue warps use 1..3).
@@ -112,16 +97,25 @@ __host__ __device__ constexpr uint64_t make_smem_desc_sw128(uint32_t addr_bytes,
   return (uint64_t)((addr_bytes >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
          ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 62);
 }
-// Product descriptor: what mma_product needs to pick the wgmma shape, operand types and majors.
-//   [7,10) operand type (0 = fp16, 1 = bf16)  [15] A major (0 = K, 1 = MN)  [16] B major  [17,23) N >> 3
-//   [24,29) M >> 4 (128: two 64-row halves; 64: one, stored to lanes (m % 16) + 32 (m / 16))
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+
+// One operand of a split product: 32-bit halves of the descriptor of split 0 / k-step 0, the low-word advance per
+// split (buffer stride >> 4) and per k-step (bytes >> 4).  All fields are warp-uniform.
+struct Op2 {
+  uint32_t lo, hi, split_step, k_step;
+};
+__device__ __forceinline__ Op2 op2_kmajor(uint32_t addr, uint32_t split_bytes) {  // K along the 128-byte rows
+  const uint64_t d = make_smem_desc_sw128(addr, 16, 1024);
+  return Op2{(uint32_t)d, (uint32_t)(d >> 32), split_bytes >> 4, 32u >> 4};
 }
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
+// K along the rows; `atom_stride` = byte distance between 64-element atoms along M/N (the next split buffer when the
+// operand is read with M = 128 "stacked")
+__device__ __forceinline__ Op2 op2_mnmajor(uint32_t addr, uint32_t atom_stride, uint32_t split_bytes) {
+  const uint64_t d = make_smem_desc_sw128(addr, atom_stride, 1024);
+  return Op2{(uint32_t)d, (uint32_t)(d >> 32), split_bytes >> 4, 2048u >> 4};
+}
+__device__ __forceinline__ Op2 op2_at(Op2 o, uint32_t byte_off) {  // same view, `byte_off` further (slot select)
+  o.lo += byte_off >> 4;
+  return o;
 }
 
 // ---- wgmma -----------------------------------------------------------------------------------------------------
@@ -218,26 +212,33 @@ __device__ __forceinline__ void wgmma_run(float (&d)[N / 2], uint64_t a, uint64_
   }
 }
 
-// D (+)= sum over `terms` of A_t B_t, each `ksteps` k-steps of 16 (descriptor low words advance by a_k / b_k per
-// k-step; the high words are shared).  Executed by all 128 threads of the issuing warpgroup.  `a_half` advances A's
-// low word to rows 64..127 when M = 128.
-template <int N, bool BF16, int TA, int TB, int T>
-__device__ __forceinline__ void mma_terms(uint32_t d_col, bool m64, const uint32_t (&alo)[T], const uint32_t (&blo)[T],
-                                          int terms, uint32_t a_hi, uint32_t b_hi, uint32_t a_k, uint32_t b_k,
-                                          int ksteps, bool acc_first, uint32_t a_half) {
+// Operand majors (template arguments TA / TB of the products): K-major, or MN-major (read transposed).
+constexpr int K_MAJOR = 0, MN_MAJOR = 1;
+
+// Accumulator columns acc_col .. acc_col + N - 1 (+)= sum over `terms` of A_t B_t, each `ksteps` k-steps of 16
+// (descriptor low words advance by a_k / b_k per k-step; the high words are shared); the first product overwrites
+// unless `acc_first`.  M = 128 runs as two m64nNk16 halves (A's low word advanced to rows 64..127); M = 64 as one, its
+// row m stored at row (m % 16) + 32 (m / 16).  Executed by all 128 threads of the issuing warpgroup.
+template <int N, bool BF16, int TA, int TB, bool M64, int T>
+__device__ __forceinline__ void mma_product(float* acc_cta, uint32_t acc_col, const uint32_t (&alo)[T],
+                                            const uint32_t (&blo)[T], int terms, uint32_t a_hi, uint32_t b_hi,
+                                            uint32_t a_k, uint32_t b_k, int ksteps, bool acc_first) {
+  static_assert(N == 16 || N == 32 || N == 48 || N == 64, "wgmma shape without a wrapper");
   const int t = (int)(threadIdx.x & 127u), w = t >> 5, l = t & 31;
-  float* acc = s_acc_cta + d_col * ACC_LANES;
+  // rows 64..127 of A: the next 64-element atom (MN-major: one leading byte offset further) or 64 rows of 128 bytes
+  const uint32_t a_half = TA == MN_MAJOR ? ((alo[0] >> 16) & 0x3FFFu) : (64u * 128u) >> 4;
+  float* acc = acc_cta + acc_col * ACC_LANES;
 #pragma unroll 1
-  for (int h = 0; h < (m64 ? 1 : 2); ++h) {
-    // fragment rows of this thread: m0 and m0 + 8 (wgmma D layout); M = 64 results go to lanes (m % 16) + 32 (m / 16)
+  for (int h = 0; h < (M64 ? 1 : 2); ++h) {
+    // this thread's fragment (wgmma D layout): rows m0 and m0 + 8, columns 2 (l % 4) + 8 j + {0, 1}.  One base
+    // pointer, the rest immediate offsets: per-element offsets would be loop-invariant and kept live across the issuer.
     const int m0 = 16 * w + (l >> 2) + 64 * h;
-    const int lane0 = m64 ? (m0 & 15) + 32 * (m0 >> 4) : m0;
+    const int row0 = M64 ? (m0 & 15) + 32 * (m0 >> 4) : m0;
+    float* frag = acc + 2 * (l & 3) * ACC_LANES + row0;
     float d[N / 2];
 #pragma unroll
-    for (int i = 0; i < N / 2; ++i) {
-      const int col = 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
-      d[i] = acc_first ? acc[col * ACC_LANES + lane0 + 8 * ((i >> 1) & 1)] : 0.f;
-    }
+    for (int i = 0; i < N / 2; ++i)
+      d[i] = acc_first ? frag[(8 * (i >> 2) + (i & 1)) * ACC_LANES + 8 * ((i >> 1) & 1)] : 0.f;
     wgmma_fence();
     uint32_t scale = acc_first ? 1u : 0u;
 #pragma unroll
@@ -255,44 +256,8 @@ __device__ __forceinline__ void mma_terms(uint32_t d_col, bool m64, const uint32
     wgmma_commit();
     wgmma_wait_all();
 #pragma unroll
-    for (int i = 0; i < N / 2; ++i) {
-      const int col = 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
-      acc[col * ACC_LANES + lane0 + 8 * ((i >> 1) & 1)] = d[i];
-    }
+    for (int i = 0; i < N / 2; ++i) frag[(8 * (i >> 2) + (i & 1)) * ACC_LANES + 8 * ((i >> 1) & 1)] = d[i];
   }
-}
-
-// Shape / type / majors come from the product descriptor (a compile-time constant at every call site).
-template <int T>
-__device__ __forceinline__ void mma_product(uint32_t d_tmem, uint32_t idesc, const uint32_t (&alo)[T],
-                                            const uint32_t (&blo)[T], int terms, uint32_t a_hi, uint32_t b_hi,
-                                            uint32_t a_k, uint32_t b_k, int ksteps, bool acc_first) {
-  const uint32_t N = ((idesc >> 17) & 63u) << 3, M = ((idesc >> 24) & 31u) << 4;
-  const uint32_t a_mn = (idesc >> 15) & 1u, b_mn = (idesc >> 16) & 1u, bf16 = (idesc >> 7) & 7u;
-  const uint32_t d_col = d_tmem & 0xFFFFu;
-  const bool m64 = M == 64;
-  // rows 64..127 of A: the next 64-element atom (MN-major: one leading byte offset further) or 64 rows of 128 bytes
-  const uint32_t a_half = a_mn ? ((alo[0] >> 16) & 0x3FFFu) : (64u * 128u) >> 4;
-#define B200RL_MMA_CASE(NN, BF, TA, TB)                                                                       \
-  if (N == NN && bf16 == BF && a_mn == TA && b_mn == TB) {                                                    \
-    mma_terms<NN, BF, TA, TB>(d_col, m64, alo, blo, terms, a_hi, b_hi, a_k, b_k, ksteps, acc_first, a_half); \
-    return;                                                                                                   \
-  }
-#define B200RL_MMA_CASES(NN, BF) \
-  B200RL_MMA_CASE(NN, BF, 0, 0)  \
-  B200RL_MMA_CASE(NN, BF, 0, 1)  \
-  B200RL_MMA_CASE(NN, BF, 1, 1)
-  B200RL_MMA_CASES(64, 0)
-  B200RL_MMA_CASES(48, 0)
-  B200RL_MMA_CASES(32, 0)
-  B200RL_MMA_CASES(16, 0)
-  B200RL_MMA_CASES(64, 1)
-  B200RL_MMA_CASES(48, 1)
-  B200RL_MMA_CASES(32, 1)
-  B200RL_MMA_CASES(16, 1)
-#undef B200RL_MMA_CASES
-#undef B200RL_MMA_CASE
-  __trap();  // a shape no kernel uses
 }
 
 }  // namespace b200rl

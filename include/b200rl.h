@@ -323,21 +323,21 @@ int b200rl_normalize(const float* x, int64_t n, float* out, void* stream);
 int b200rl_polyak(float* target, const float* param, int64_t n, double rho, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * Off-policy update engine (DDPG / TD3): the reference's `train(replay_buffer, num_train_steps, minibatch_size)`
- * (algorithms/td3.py:214-358, algorithms/ddpg.py:195-293) on device.  Networks: 0 policy, 1 Q1, 2 Q2, 3 target
- * policy, 4 target Q1, 5 target Q2 (2 and 5 absent when n_q = 1).  Minibatch sampling (numpy RNG) and the
+ * Off-policy update engine (DDPG / TD3, and SAC below): the reference's `train(replay_buffer, num_train_steps,
+ * minibatch_size)` (algorithms/td3.py:214-358, algorithms/ddpg.py:195-293) on device.  Networks: 0 policy, 1 Q1, 2 Q2,
+ * 3 target policy, 4 target Q1, 5 target Q2 (2 and 5 absent when n_q = 1, 3 absent for SAC).  Minibatch sampling (numpy RNG) and the
  * target-smoothing noise (torch CPU RNG) stay on the host so the reference's random streams are reproduced; ALL
  * minibatches of one train() call are handed over at once.
  * ------------------------------------------------------------------------------------------------------------ */
 typedef struct b200rl_offpolicy b200rl_offpolicy;
 
 typedef struct {
-  b200rl_mlp_desc policy;  /* [obs, hidden..., act]      (ref: policies/deterministic_policy.py) */
+  b200rl_mlp_desc policy;  /* [obs, hidden..., act]      (ref: policies/deterministic_policy.py); SAC: [obs, ..., 2 act] */
   b200rl_mlp_desc q;       /* [obs + act, hidden..., 1]  (ref: q_function.py:20-32) */
-  int32_t n_q;             /* 1 = DDPG, 2 = TD3 */
+  int32_t n_q;             /* 1 = DDPG, 2 = TD3 (algo 0); SAC needs 2 */
   int32_t max_minibatch;   /* capacity: rows per minibatch */
   int32_t max_steps;       /* capacity: train steps per call */
-  int32_t reserved;
+  int32_t algo;            /* 0 = DDPG / TD3 (by n_q), 1 = SAC (see b200rl_offpolicy_set_sac) */
 } b200rl_offpolicy_config;
 
 typedef struct {
@@ -399,6 +399,42 @@ int b200rl_offpolicy_train_gather_rng(b200rl_offpolicy* h, const b200rl_offpolic
 /* The draws of the last train_gather / train_gather_rng call: physical rows idx [S*B] (host int64), noise [S*B*A]
  * (host float32, or NULL) -- what a test replays through the oracle. */
 int b200rl_offpolicy_get_draws(b200rl_offpolicy* h, int32_t S, int32_t B, int64_t* idx, float* noise, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Soft Actor-Critic on the same engine (config algo = 1, n_q = 2; Spinning Up sac/core.py, sac/sac.py).  The policy
+ * network maps obs -> [mean | log_std] (2A outputs, Identity output layer); network 3 (target policy) is absent, so the
+ * state blob holds networks 0, 1, 2, 4, 5.  Per train step, with draws eps' (for s') and eps (for s) and alpha:
+ *   head(o, e): log_std = clamp(log_std, log_std_min, log_std_max), u = mean + exp(log_std) e, a = limit tanh(u),
+ *               log pi = sum_j Normal(mean, std).log_prob(u) - sum_j 2 (log 2 - u - softplus(-2u))
+ *               (limit = hparams.action_limit; the constant -A log(limit) is omitted, as in Spinning Up)
+ *   critics:    y = r + gamma (1 - d) (min(Q1targ, Q2targ)(s', a') - alpha log pi'), a', log pi' = head(pi(s'), eps');
+ *               one Adam step each on mean((Qi(s, a) - y)^2)
+ *   policy:     one Adam step on mean(alpha log pi - min(Q1, Q2)(s, a_pi)), a_pi, log pi = head(pi(s), eps), with the
+ *               critics just updated (torch.min's tie rule: equal values share the gradient)
+ *   alpha:      learn_alpha = 1: one Adam step on -mean(log_alpha (log pi + target_entropy)), alpha = exp(log_alpha)
+ *               from the next step on; learn_alpha = 0: alpha is the fixed value
+ *   polyak:     Q1targ, Q2targ every step.  hparams.policy_delay / use_target_noise / target_noise_* do not apply.
+ * train / train_gather take noise [S, 2, B, A] (per step the draw for s', then the one for s), required; train_gather_rng
+ * draws it on the device and get_draws returns it in the same layout.  policy_losses has S entries.  The persistent
+ * step kernel (B200RL_OFFPOLICY_MEGAKERNEL=1) does not apply: SAC runs as a CUDA graph, or as plain launches with
+ * B200RL_OFFPOLICY_GRAPH=0.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  double alpha;                 /* the fixed entropy coefficient (learn_alpha = 0) */
+  double target_entropy;        /* H-bar, usually -A */
+  double alpha_lr, alpha_beta1, alpha_beta2, alpha_eps; /* torch.optim.Adam over log_alpha */
+  double log_std_min, log_std_max;                      /* -20, 2 */
+  int32_t learn_alpha;          /* 0 or 1 */
+  int32_t reserved;
+} b200rl_sac_hparams;
+
+/* Required once before the first train call of a SAC engine; part of the cached graph's key. */
+int b200rl_offpolicy_set_sac(b200rl_offpolicy* h, const b200rl_sac_hparams* hp);
+/* The temperature's state: float32 log_alpha, its Adam exp_avg / exp_avg_sq and step count. */
+int b200rl_offpolicy_set_alpha(b200rl_offpolicy* h, float log_alpha, float exp_avg, float exp_avg_sq, int64_t step);
+int b200rl_offpolicy_get_alpha(b200rl_offpolicy* h, float* log_alpha, float* exp_avg, float* exp_avg_sq, int64_t* step);
+/* After a train call of S steps: mean log pi of each policy step and the alpha each step used (host [S] each). */
+int b200rl_offpolicy_sac_outputs(b200rl_offpolicy* h, int32_t S, float* log_prob_means, float* alphas);
 
 #ifdef __cplusplus
 }

@@ -79,7 +79,14 @@ class TrpoStats(C.Structure):
 
 class OffPolicyConfig(C.Structure):
     _fields_ = [("policy", MlpDesc), ("q", MlpDesc), ("n_q", C.c_int32), ("max_minibatch", C.c_int32),
-                ("max_steps", C.c_int32), ("reserved", C.c_int32)]
+                ("max_steps", C.c_int32), ("algo", C.c_int32)]
+
+
+class SacHparams(C.Structure):
+    _fields_ = [("alpha", C.c_double), ("target_entropy", C.c_double), ("alpha_lr", C.c_double),
+                ("alpha_beta1", C.c_double), ("alpha_beta2", C.c_double), ("alpha_eps", C.c_double),
+                ("log_std_min", C.c_double), ("log_std_max", C.c_double), ("learn_alpha", C.c_int32),
+                ("reserved", C.c_int32)]
 
 
 class OffPolicyHparams(C.Structure):
@@ -153,6 +160,11 @@ SIGNATURES = {
                                           [C.c_void_p] * 5 + [C.c_int64] * 3 + [C.c_uint64] * 2 + [C.c_void_p] * 5 +
                                           [C.POINTER(C.c_int32), C.c_void_p]),
     "b200rl_offpolicy_get_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200rl_offpolicy_set_sac": (C.c_int, [C.c_void_p, C.POINTER(SacHparams)]),
+    "b200rl_offpolicy_set_alpha": (C.c_int, [C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_int64]),
+    "b200rl_offpolicy_get_alpha": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float),
+                                             C.POINTER(C.c_float), C.POINTER(C.c_int64)]),
+    "b200rl_offpolicy_sac_outputs": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "b200rl_discounted_cumsum": (C.c_int, [C.c_void_p, C.c_int64, C.c_double, C.c_void_p, C.c_void_p]),
     "b200rl_gae_f64": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_double, C.c_double, C.c_void_p,
                                  C.c_void_p]),

@@ -1,6 +1,7 @@
 from .ppo import PPO
+from .sac import SAC
 from .td3 import DDPG, TD3
 from .trpo import TRPO
 from .vpg import VPG
 
-__all__ = ["VPG", "TRPO", "PPO", "DDPG", "TD3"]
+__all__ = ["VPG", "TRPO", "PPO", "DDPG", "TD3", "SAC"]

@@ -22,6 +22,8 @@ logger = logging.getLogger(__name__)
 
 class _OffPolicyBase:
     n_q = 1
+    algo = OffPolicyEngine.TD3  # the engine's step program (DDPG / TD3 by n_q, or SAC)
+    target_slots = (3, 4, 5)    # engine network index of each target network
     use_device_replay = True  # replay columns mirrored in HBM, minibatches gathered on the device (SURVEY 8f-4)
     use_device_rng = False    # opt-in: indices and target-smoothing noise drawn on the device (Philox) instead of with
     device_rng_seed = 0       # the reference's numpy / torch CPU streams -- same distributions, different numbers
@@ -62,7 +64,7 @@ class _OffPolicyBase:
                 or e.policy_acts != (pact, pout) or e.q_acts != (qact, qout)):
             if e is not None:
                 e.close()
-            e = OffPolicyEngine(psz, qsz, self.n_q, B, S, (pact, pout), (qact, qout))
+            e = OffPolicyEngine(psz, qsz, self.n_q, B, S, (pact, pout), (qact, qout), algo=self.algo)
             self._engine = e
         return e
 
@@ -82,7 +84,7 @@ class _OffPolicyBase:
         assert blob.numel() == total
         blob_np = blob.numpy()  # shares the page-locked memory
         mods = {i: (m, l) for i, (m, l) in enumerate(zip(trainable, lins))}
-        mods.update({3 + i: (m, l) for i, (m, l) in enumerate(zip(targets, lins[len(trainable):]))})
+        mods.update({k: (m, l) for k, m, l in zip(self.target_slots, targets, lins[len(trainable):])})
         slots = []
         for kind, i, off, count in layout:
             m, l = mods[i]
@@ -170,24 +172,26 @@ class _OffPolicyBase:
         hp.q_beta1, hp.q_beta2, hp.q_eps = q1[1], q1[2], q1[3]
         return hp
 
+    def _noise(self, S: int, B: int) -> np.ndarray:
+        """S draws of torch.randn(B, A), the reference's stream (td3.py:328), gathered without torch.stack."""
+        A = self.policy.network.sizes[-1] if hasattr(self.policy.network, "sizes") else describe_mlp(self.policy.network)[0][-1]
+        out = np.empty((S, B, A), dtype=np.float32)
+        for i in range(S):
+            out[i] = torch.randn(B, A).numpy()
+        return out
+
     def _run(self, replay_buffer, num_train_steps: int, minibatch_size: int, noisy: bool, delay: int):
         S, B = int(num_train_steps), int(minibatch_size)
         trainable, targets = self._nets()
         # host side, same random streams as the reference: numpy RNG for the indices (replay_buffer.py:58), torch CPU
         # RNG for the target-smoothing noise (td3.py:328); the two streams are independent, so drawing all minibatches
         # first and all noise second consumes each exactly as the interleaved reference loop does.
-        A = self.policy.network.sizes[-1] if hasattr(self.policy.network, "sizes") else describe_mlp(self.policy.network)[0][-1]
         device_replay = (S > 0 and getattr(self, "use_device_replay", True) and hasattr(replay_buffer, "device_columns")
                          and hasattr(replay_buffer, "sample_indices"))
         # opt-in (SURVEY 8f-4): indices and smoothing noise drawn on the device -- not the reference's random streams
         device_rng = device_replay and getattr(self, "use_device_rng", False) and hasattr(replay_buffer, "ring")
-        def noise_of():  # S draws of torch.randn(B, A), the reference's stream (td3.py:328), gathered without torch.stack
-            if not (noisy and S > 0):
-                return None
-            out = np.empty((S, B, A), dtype=np.float32)
-            for i in range(S):
-                out[i] = torch.randn(B, A).numpy()
-            return out
+        def noise_of():
+            return self._noise(S, B) if noisy and S > 0 else None
         if device_rng:
             idx = noise = None
         elif device_replay:
@@ -343,7 +347,7 @@ def _make_eval_env(env):
 
 def _learn(self, num_epochs, batch_size, minibatch_size, num_start_steps, num_steps_before_update, num_train_steps,
            num_evaluation_episodes, evaluation_interval, model_saving_interval, output_dir) -> None:
-    """Shared host loop of TD3.learn / DDPG.learn (ref: td3.py:94-212, ddpg.py:85-193)."""
+    """Shared host loop of TD3.learn / DDPG.learn / SAC.learn (ref: td3.py:94-212, ddpg.py:85-193)."""
     started = time.time()
     self.current_total_steps = 0
     self.current_total_episodes = 0
@@ -371,7 +375,8 @@ def _learn(self, num_epochs, batch_size, minibatch_size, num_start_steps, num_st
         if self.current_total_steps >= num_steps_before_update:
             self.train(self.replay_buffer, num_train_steps, minibatch_size)
         if num_evaluation_episodes > 0 and self.current_total_steps % evaluation_interval == 0:
-            ev_returns, ev_lengths = self.evaluator.evaluate(self.policy, self.evaluation_env, num_evaluation_episodes)
+            ev_policy = getattr(self, "evaluation_policy", self.policy)  # SAC: the deterministic view of its policy
+            ev_returns, ev_lengths = self.evaluator.evaluate(ev_policy, self.evaluation_env, num_evaluation_episodes)
             mm.record_scalar("evaluation/average_episode_return", float(np.mean(ev_returns)), self.current_total_steps,
                              tensorboard=True)
             mm.record_scalar("evaluation/episode_return_std", float(np.std(ev_returns)))

@@ -14,6 +14,8 @@
 // the opt-in persistent step kernel (offpolicy_mega_kernel) and its program builder; the engine (one state slab);
 // enqueue_steps = the S steps as a four-stream dependency graph (captured once, replayed); the three entry points
 // train (host-staged minibatches), train_gather (host-drawn indices, device gather), train_gather_rng (device draws).
+// SAC (config algo = 1) is a second step program on the same engine: its head / soft-loss / temperature kernels and
+// enqueue_sac_steps, run as a captured graph or as plain launches (the persistent step kernel does not apply to it).
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -421,6 +423,137 @@ __global__ void __launch_bounds__(GTHREADS, 2) offpolicy_mega_kernel(const MkBlo
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// SAC (algo = 1; Spinning Up sac/core.py SquashedGaussianMLPActor, sac/sac.py compute_loss_q / compute_loss_pi).  The
+// policy network's output is [mu | log_std] [B, 2A]; the kernels below are the head and the soft losses around it.
+// ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float softplus_f(float x) { return x > 20.f ? x : log1pf(expf(x)); }  // F.softplus
+
+// One thread per row: u = mu + exp(clamp(log_std)) * eps, act = limit * tanh(u),
+// logp = sum_j Normal(mu, sigma).log_prob(u)_j - sum_j 2 (log 2 - u_j - softplus(-2 u_j))
+__global__ void sac_squash_kernel(const float* out, const float* eps, int B, int A, float lmin, float lmax, float limit,
+                                  float* act, float* logp) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= B) return;
+  float lp = 0.f, corr = 0.f;
+  for (int j = 0; j < A; ++j) {
+    const float mu = out[(size_t)r * 2 * A + j];
+    const float ls = fminf(fmaxf(out[(size_t)r * 2 * A + A + j], lmin), lmax);
+    const float sigma = expf(ls);
+    const float u = __fadd_rn(mu, __fmul_rn(sigma, eps[(size_t)r * A + j]));  // rsample: loc + eps * scale
+    const float d = u - mu;
+    lp += -(d * d) / (2.f * (sigma * sigma)) - ls - 0.918938533204672742f;  // - log sqrt(2 pi)
+    corr += 2.f * (0.693147180559945309f - u - softplus_f(-2.f * u));
+    act[(size_t)r * A + j] = limit * tanhf(u);
+  }
+  logp[r] = lp - corr;
+}
+
+// One CTA per critic: y = r + gamma (1 - d) (min(Q1targ, Q2targ)(s', a') - alpha log pi(a' | s')), loss = mean((q - y)^2),
+// dq = 2 (q - y) / B, q_copy = q (the logged Q-values)
+__global__ void __launch_bounds__(GTHREADS) sac_q_loss_kernel(const float* q, const float* rew, const float* done,
+                                                             const float* q1t, const float* q2t, const float* logp_next,
+                                                             const float* alpha, float gamma, int n, float* dq,
+                                                             float* loss_out, float* q_copy) {
+  __shared__ double red[32];
+  const float a = *alpha;
+  const float inv = 1.0f / (float)n;
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float qi = q[i];
+    q_copy[i] = qi;
+    const float y = rew[i] + gamma * (1.f - done[i]) * (fminf(q1t[i], q2t[i]) - a * logp_next[i]);
+    const float d = qi - y;
+    acc += (double)d * (double)d;
+    dq[i] = (2.f * d) * inv;
+  }
+  mk_block_mean(acc, n, loss_out, red);
+}
+
+// One CTA: loss = mean(alpha log pi - min(q1, q2)) at a = pi(s), the per-row gradients w.r.t. q1 and q2 (torch.min's
+// rule: equal values share the gradient half and half), and mean(log pi)
+__global__ void __launch_bounds__(GTHREADS) sac_policy_loss_kernel(const float* q1, const float* q2, const float* logp,
+                                                                  const float* alpha, int n, float* dq1, float* dq2,
+                                                                  float* loss_out, float* logp_mean_out) {
+  __shared__ double red[32], red_lp[32];
+  const float a = *alpha;
+  const float inv = 1.0f / (float)n;
+  double acc = 0.0, acc_lp = 0.0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float x1 = q1[i], x2 = q2[i], lp = logp[i];
+    acc += (double)(a * lp - fminf(x1, x2));
+    acc_lp += (double)lp;
+    const float w1 = x1 < x2 ? 1.f : (x1 == x2 ? 0.5f : 0.f);
+    dq1[i] = -(w1 * inv);
+    dq2[i] = -((1.f - w1) * inv);
+  }
+  mk_block_mean(acc, n, loss_out, red);
+  mk_block_mean(acc_lp, n, logp_mean_out, red_lp);
+}
+
+// One thread per (row, j): the gradient of the policy loss w.r.t. the network output [mu | log_std], from
+// dA = dQ1/da + dQ2/da (the action columns of the critics' input gradients, row stride ldx) and the alpha log pi term;
+// u and sigma are recomputed from the output and eps exactly as sac_squash_kernel computed them.  With t = tanh(u) and
+// c = alpha / B:  g_u = dA limit (1 - t^2) + 2 c t,  d mu = g_u,  d log_std = g_u sigma eps - c inside the clamp, else 0
+// (the Gaussian term's u - mu = sigma eps cancels from d mu and leaves -1 in d log_std).
+__global__ void sac_squash_backward_kernel(const float* out, const float* eps, const float* dx1, const float* dx2, int ldx,
+                                           int B, int A, float lmin, float lmax, float limit, const float* alpha,
+                                           float* dout) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * A) return;
+  const int r = i / A, j = i - r * A;
+  const float c = *alpha / (float)B;
+  const float mu = out[(size_t)r * 2 * A + j], raw = out[(size_t)r * 2 * A + A + j];
+  const float sigma = expf(fminf(fmaxf(raw, lmin), lmax));
+  const float e = eps[(size_t)r * A + j];
+  const float u = __fadd_rn(mu, __fmul_rn(sigma, e));
+  const float t = tanhf(u);
+  const float dA = dx1[(size_t)r * ldx + j] + dx2[(size_t)r * ldx + j];
+  const float gu = dA * limit * (1.f - t * t) + 2.f * c * t;
+  dout[(size_t)r * 2 * A + j] = gu;
+  dout[(size_t)r * 2 * A + A + j] = (raw >= lmin && raw <= lmax) ? gu * sigma * e - c : 0.f;
+}
+
+// alpha[0..n) = the fixed alpha (learn == 0), or alpha[0] = exp(log_alpha) (learn == 1: the alpha steps fill the rest)
+__global__ void sac_alpha_init_kernel(float* alpha, int n, const float* log_alpha, int learn, float fixed) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (learn) {
+    if (i == 0) alpha[0] = expf(*log_alpha);
+  } else if (i < n) {
+    alpha[i] = fixed;
+  }
+}
+
+// One CTA: the temperature step.  grad = -mean(log pi + target_entropy) (a fixed-order reduction), then torch.optim.Adam
+// on the scalar log_alpha (state = {log_alpha, exp_avg, exp_avg_sq}) with the scalars of table[idx]; alpha_next =
+// exp(log_alpha), the alpha of the next step
+__global__ void __launch_bounds__(GTHREADS) sac_alpha_step_kernel(const float* logp, int n, float target_entropy,
+                                                                 float* state, const float2* table, int idx,
+                                                                 float one_minus_b1, float b2, float one_minus_b2,
+                                                                 float eps, float* alpha_next) {
+  __shared__ double red[32];
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) acc += (double)(logp[i] + target_entropy);
+  acc = warp_sum(acc);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double tot = 0.0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tot += red[w];
+    const float g = -(float)(tot / (double)n);
+    const float2 t = table[idx];
+    float p = state[0], m = state[1], v = state[2];
+    m = m + one_minus_b1 * (g - m);  // the arithmetic of adam_step_kernel (adam.cu)
+    v = v * b2 + one_minus_b2 * (g * g);
+    const float denom = sqrtf(v) / t.y + eps;
+    p = p - t.x * (m / denom);
+    state[0] = p;
+    state[1] = m;
+    state[2] = v;
+    *alpha_next = expf(p);
+  }
+}
+
 }  // namespace b200rl
 
 using namespace b200rl;
@@ -476,6 +609,16 @@ struct b200rl_offpolicy {
   size_t mk_prog_cap = 0;
   float* state = nullptr;  // parameters + Adam state of every network, blob order (see b200rl_offpolicy_create)
   int64_t state_n = 0;
+  // SAC (cfg.algo == 1): network 3 is absent; h->eps holds [S, 2, B, A] (the draw for s', then the one for s)
+  bool sac = false, sac_set = false;
+  b200rl_sac_hparams sac_hp{}, graph_sac_hp{};
+  float *sac_act_next = nullptr, *sac_logp_next = nullptr;  // [B, A] / [B]: a' and log pi(a' | s')
+  float *sac_act = nullptr, *sac_logp = nullptr;            // the same at s (the policy step)
+  float* sac_dout = nullptr;                                // [B, 2A] gradient w.r.t. the policy output
+  float* sac_alpha = nullptr;                               // [max_steps + 1] alpha of step st at [st]
+  float* sac_state = nullptr;                               // {log_alpha, exp_avg, exp_avg_sq}
+  float* out_logp = nullptr;                                // [max_steps] mean log pi of each policy step
+  int64_t alpha_step = 0;
   std::vector<void*> allocs;
 };
 
@@ -593,11 +736,18 @@ int adam_net(NetBuf& nb, const float2* table, int idx, double b1, double b2, dou
 extern "C" int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200rl_offpolicy** out) {
   B200RL_REQUIRE(cfg && out, "offpolicy_create: NULL argument");
   B200RL_REQUIRE(cfg->n_q == 1 || cfg->n_q == 2, "offpolicy_create: n_q must be 1 (DDPG) or 2 (TD3)");
+  B200RL_REQUIRE(cfg->algo == 0 || cfg->algo == 1, "offpolicy_create: algo must be 0 (DDPG / TD3) or 1 (SAC), got %d",
+                 cfg->algo);
+  const bool sac = cfg->algo == 1;
+  B200RL_REQUIRE(!sac || cfg->n_q == 2, "offpolicy_create: SAC needs n_q = 2 (twin soft critics), got %d", cfg->n_q);
   B200RL_REQUIRE(cfg->max_minibatch >= 1 && cfg->max_minibatch <= 65536 && cfg->max_steps >= 1,
                  "offpolicy_create: bad capacities");
   const int64_t Pp = b200rl_mlp_param_count(&cfg->policy), Pq = b200rl_mlp_param_count(&cfg->q);
   B200RL_REQUIRE(Pp > 0 && Pq > 0, "offpolicy_create: invalid MLP description");
-  const int O = cfg->policy.sizes[0], A = cfg->policy.sizes[cfg->policy.n_layers];
+  const int O = cfg->policy.sizes[0], P_out = cfg->policy.sizes[cfg->policy.n_layers];
+  const int A = sac ? cfg->q.sizes[0] - O : P_out;  // SAC: the policy outputs [mean | log_std], 2A wide
+  B200RL_REQUIRE(!sac || (A >= 1 && P_out == 2 * A),
+                 "offpolicy_create: the SAC policy must output [mean | log_std] = 2 x %d values, got %d", A, P_out);
   B200RL_REQUIRE(cfg->q.sizes[0] == O + A && cfg->q.sizes[cfg->q.n_layers] == 1,
                  "offpolicy_create: Q network must map [obs %d + act %d] -> 1", O, A);
   B200RL_REQUIRE(device_sm_count() > 0, "offpolicy_create: no CUDA device");
@@ -605,6 +755,7 @@ extern "C" int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200r
   h->cfg = *cfg;
   h->O = O;
   h->A = A;
+  h->sac = sac;
   int rc = 0;
   int maxw = O + A;
   for (int i = 0; i < 6; ++i) {
@@ -620,6 +771,7 @@ extern "C" int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200r
       maxw = nb.d.sizes[l + 1] > maxw ? nb.d.sizes[l + 1] : maxw;
     }
     if (cfg->n_q == 1 && (i == 2 || i == 5)) continue;
+    if (sac && i == 3) continue;  // SAC has no target policy
     nb.present = true;
     if (i < 3) rc |= oalloc(h, &nb.grad, (size_t)nb.P);
   }
@@ -656,7 +808,7 @@ extern "C" int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200r
   rc |= oalloc(h, &h->rew, S * B);
   rc |= oalloc(h, &h->nobs, S * B * O);
   rc |= oalloc(h, &h->done, S * B);
-  rc |= oalloc(h, &h->eps, S * B * A);
+  rc |= oalloc(h, &h->eps, (sac ? 2 : 1) * S * B * A);
   for (int k = 0; k < 5; ++k)
     for (int l = 0; l <= B200RL_MAX_LAYERS; ++l) rc |= oalloc(h, &h->acts[k][l], B * (size_t)maxw);
   for (int l = 0; l <= B200RL_MAX_LAYERS; ++l) rc |= oalloc(h, &h->acts_tq[l], B * (size_t)maxw);
@@ -677,9 +829,20 @@ extern "C" int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200r
   rc |= oalloc(h, &h->out_l1, S);
   rc |= oalloc(h, &h->out_l2, S);
   rc |= oalloc(h, &h->out_lp, S);
-  rc |= oalloc(h, &h->adam_tab, 3 * S);
+  const size_t n_tab = sac ? 4 : 3;  // SAC: a fourth row for log_alpha's optimizer
+  rc |= oalloc(h, &h->adam_tab, n_tab * S);
   rc |= oalloc(h, &h->idx, S * B);
-  if (!rc && cudaMallocHost(reinterpret_cast<void**>(&h->h_adam_tab), 3 * S * sizeof(float2)) != cudaSuccess) rc = 1;
+  if (sac) {
+    rc |= oalloc(h, &h->sac_act_next, B * (size_t)A);
+    rc |= oalloc(h, &h->sac_logp_next, B);
+    rc |= oalloc(h, &h->sac_act, B * (size_t)A);
+    rc |= oalloc(h, &h->sac_logp, B);
+    rc |= oalloc(h, &h->sac_dout, B * (size_t)(2 * A));
+    rc |= oalloc(h, &h->sac_alpha, S + 1);
+    rc |= oalloc(h, &h->sac_state, 3);
+    rc |= oalloc(h, &h->out_logp, S);
+  }
+  if (!rc && cudaMallocHost(reinterpret_cast<void**>(&h->h_adam_tab), n_tab * S * sizeof(float2)) != cudaSuccess) rc = 1;
   if (!rc && cudaStreamCreateWithFlags(&h->gs, cudaStreamNonBlocking) != cudaSuccess) rc = 1;
   if (!rc && cudaEventCreateWithFlags(&h->ev, cudaEventDisableTiming) != cudaSuccess) rc = 1;
   if (!rc && cudaStreamCreateWithFlags(&h->s2, cudaStreamNonBlocking) != cudaSuccess) rc = 1;
@@ -786,6 +949,50 @@ extern "C" int b200rl_offpolicy_set_state(b200rl_offpolicy* h, const float* blob
   for (int i = 0; i < 3; ++i)
     if (h->net[i].m) h->net[i].step = steps[i];
   B200RL_CUDA(cudaStreamSynchronize(s));  // `blob` may be reused by the caller right away
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_set_sac(b200rl_offpolicy* h, const b200rl_sac_hparams* sp) {
+  B200RL_REQUIRE(h && sp, "offpolicy_set_sac: NULL argument");
+  B200RL_REQUIRE(h->sac, "offpolicy_set_sac: the engine was not created with algo = 1 (SAC)");
+  B200RL_REQUIRE(sp->learn_alpha == 0 || sp->learn_alpha == 1, "offpolicy_set_sac: learn_alpha must be 0 or 1");
+  B200RL_REQUIRE(sp->log_std_min <= sp->log_std_max, "offpolicy_set_sac: log_std_min > log_std_max");
+  h->sac_hp = *sp;
+  h->sac_hp.reserved = 0;  // part of the graph cache key
+  h->sac_set = true;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_set_alpha(b200rl_offpolicy* h, float log_alpha, float exp_avg, float exp_avg_sq,
+                                          int64_t step) {
+  B200RL_REQUIRE(h && h->sac, "offpolicy_set_alpha: not a SAC engine");
+  B200RL_REQUIRE(step >= 0, "offpolicy_set_alpha: negative step count");
+  const float v[3] = {log_alpha, exp_avg, exp_avg_sq};
+  B200RL_CUDA(cudaMemcpyAsync(h->sac_state, v, sizeof(v), cudaMemcpyHostToDevice, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  h->alpha_step = step;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_get_alpha(b200rl_offpolicy* h, float* log_alpha, float* exp_avg, float* exp_avg_sq,
+                                          int64_t* step) {
+  B200RL_REQUIRE(h && h->sac && log_alpha && exp_avg && exp_avg_sq && step, "offpolicy_get_alpha: bad arguments");
+  float v[3];
+  B200RL_CUDA(cudaMemcpyAsync(v, h->sac_state, sizeof(v), cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  *log_alpha = v[0];
+  *exp_avg = v[1];
+  *exp_avg_sq = v[2];
+  *step = h->alpha_step;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_sac_outputs(b200rl_offpolicy* h, int32_t S, float* log_prob_means, float* alphas) {
+  B200RL_REQUIRE(h && h->sac && log_prob_means && alphas && S >= 0 && S <= h->cfg.max_steps,
+                 "offpolicy_sac_outputs: bad arguments");
+  B200RL_CUDA(cudaMemcpyAsync(log_prob_means, h->out_logp, (size_t)S * 4, cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaMemcpyAsync(alphas, h->sac_alpha, (size_t)S * 4, cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
   return 0;
 }
 
@@ -902,6 +1109,139 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
     }
   }
   *n_pol_out = n_pol;
+  return 0;
+}
+
+// The S SAC steps (sac/sac.py update(): one critic step, one policy step, the optional temperature step and polyak).
+// Per step the branches are:
+//   s  : pi(s') -> squash -> Q1targ ----+-> soft Q1 loss -> Q1 bwd, Adam -+-> Q1(s, a_pi) -+-> policy loss -> Q1 dX -+->
+//   s2 :                    -> Q2targ --+-> soft Q2 loss -> Q2 bwd, Adam -+-> Q2(s, a_pi) -+                -> Q2 dX -+
+//   s3 : Q1 on [s | a] -> pi(s) -> squash ............ Q1's dW products ......... (then pi's dW products)
+//   s4 : Q2 on [s | a] ............................... Q2's dW products -> polyak (both critic pairs)
+//        ... -> squash backward -> pi bwd, Adam on s; the temperature step rides on s2 behind Q2's dX chain.
+// Step st reads alpha[st]; the temperature step writes alpha[st + 1], so nothing it writes is read in the same step.
+static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s) {
+  const int O = h->O, A = h->A;
+  const int maxS = h->cfg.max_steps;
+  const b200rl_sac_hparams& sp = h->sac_hp;
+  NetBuf &pi = h->net[0], &q1 = h->net[1], &q2 = h->net[2], &q1t = h->net[4], &q2t = h->net[5];
+  const int Lq = q1.d.n_layers, Lp = pi.d.n_layers;
+  const float lmin = (float)sp.log_std_min, lmax = (float)sp.log_std_max, limit = (float)hp->action_limit;
+  const int ew = 256, rows_grid = (B + 127) / 128;
+  cudaStream_t s2 = h->s2, s3 = h->s3, s4 = h->s4;
+  auto edge = [&](cudaStream_t from, cudaStream_t to) -> int {
+    B200RL_CUDA(cudaEventRecord(h->ev_fork, from));
+    B200RL_CUDA(cudaStreamWaitEvent(to, h->ev_fork, 0));
+    return 0;
+  };
+  auto launched = [&]() -> int {
+    B200RL_CUDA(cudaGetLastError());
+    count_launch(1);
+    return 0;
+  };
+  sac_alpha_init_kernel<<<(S + 1 + ew - 1) / ew, ew, 0, s>>>(h->sac_alpha, S + 1, h->sac_state, sp.learn_alpha,
+                                                             (float)sp.alpha);
+  if (launched()) return 1;
+  PolyakArgs pk{};  // 1 -> 4, 2 -> 5
+  pk.n_nets = 2;
+  for (int k = 0; k < 2; ++k) {
+    pk.target[k] = h->net[4 + k].params;
+    pk.param[k] = h->net[1 + k].params;
+    pk.n[k] = (int)h->net[1 + k].P;
+  }
+  for (int st = 0; st < S; ++st) {
+    const float* s_obs = h->obs + (size_t)st * B * O;
+    const float* s_act = h->act + (size_t)st * B * A;
+    const float* s_rew = h->rew + (size_t)st * B;
+    const float* s_nobs = h->nobs + (size_t)st * B * O;
+    const float* s_done = h->done + (size_t)st * B;
+    const float* eps_next = h->eps + (size_t)(2 * st) * B * A;  // [S, 2, B, A]: the draw for s', then the one for s
+    const float* eps_cur = eps_next + (size_t)B * A;
+    const float* alpha = h->sac_alpha + st;
+    // ---- the critics on [s | a] (the logged Q-values); pi(s) with the pre-update policy behind Q1's ----
+    float* qa[2][B200RL_MAX_LAYERS + 1];
+    for (int qi = 0; qi < 2; ++qi) {
+      qa[qi][0] = const_cast<float*>(s_obs);
+      for (int l = 1; l <= Lq; ++l) qa[qi][l] = h->acts[qi == 0 ? 1 : 4][l];
+      cudaStream_t qs = qi == 0 ? s3 : s4;
+      if (edge(s, qs)) return 1;
+      if (net_forward(qi == 0 ? q1 : q2, qa[qi], B, qs, s_act, A, O)) return 1;
+    }
+    float* pa[B200RL_MAX_LAYERS + 1];
+    pa[0] = const_cast<float*>(s_obs);
+    for (int l = 1; l <= Lp; ++l) pa[l] = h->acts[2][l];
+    if (net_forward(pi, pa, B, s3)) return 1;
+    sac_squash_kernel<<<rows_grid, 128, 0, s3>>>(pa[Lp], eps_cur, B, A, lmin, lmax, limit, h->sac_act, h->sac_logp);
+    if (launched()) return 1;
+    // ---- soft targets: a', log pi' from the current policy at s'; the target critics read [s' | a'] in place ----
+    float* ta[B200RL_MAX_LAYERS + 1];
+    ta[0] = const_cast<float*>(s_nobs);
+    for (int l = 1; l <= Lp; ++l) ta[l] = h->acts[0][l];
+    if (net_forward(pi, ta, B, s)) return 1;
+    sac_squash_kernel<<<rows_grid, 128, 0, s>>>(ta[Lp], eps_next, B, A, lmin, lmax, limit, h->sac_act_next,
+                                                h->sac_logp_next);
+    if (launched()) return 1;
+    float* tq[2][B200RL_MAX_LAYERS + 1];
+    for (int qi = 0; qi < 2; ++qi) {
+      tq[qi][0] = const_cast<float*>(s_nobs);
+      for (int l = 1; l < Lq; ++l) tq[qi][l] = qi == 0 ? h->acts_tq[l] : h->acts[3][l];
+      tq[qi][Lq] = qi == 0 ? h->qt1 : h->qt2;
+    }
+    if (edge(s, s2)) return 1;
+    if (net_forward(q2t, tq[1], B, s2, h->sac_act_next, A, O)) return 1;
+    if (net_forward(q1t, tq[0], B, s, h->sac_act_next, A, O)) return 1;
+    if (edge(s2, s)) return 1;
+    // ---- critic step: soft TD target + MSE + dq, backward, Adam (Q2 on s2, Q1 on s) ----
+    if (edge(s, s2)) return 1;
+    if (edge(s4, s2)) return 1;
+    if (edge(s3, s)) return 1;
+    for (int qi = 1; qi >= 0; --qi) {
+      NetBuf& qn = qi == 0 ? q1 : q2;
+      cudaStream_t qs = qi == 0 ? s : s2;
+      float* dq = qi == 0 ? h->dq : h->dq2;
+      sac_q_loss_kernel<<<1, GTHREADS, 0, qs>>>(qa[qi][Lq], s_rew, s_done, h->qt1, h->qt2, h->sac_logp_next, alpha,
+                                                (float)hp->gamma, B, dq, (qi == 0 ? h->out_l1 : h->out_l2) + st,
+                                                (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B);
+      if (launched()) return 1;
+      if (net_backward(h, qn, qa[qi], dq, 1, B, true, nullptr, qs, qi != 0, s_act, A, O, qi == 0 ? s3 : s4)) return 1;
+      if (adam_net(qn, h->adam_tab + (size_t)(1 + qi) * maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, qs)) return 1;
+    }
+    if (edge(s2, s)) return 1;
+    // ---- polyak beside the policy step: the targets are next read by the next step ----
+    if (edge(s, s4)) return 1;
+    polyak_kernel<<<(pk.n[0] + ew - 1) / ew, ew, 0, s4>>>(pk, (float)hp->polyak_rho, (float)(1.0 - hp->polyak_rho));
+    if (launched()) return 1;
+    // ---- policy step: both updated critics on [s | a_pi], differentiated w.r.t. their input only ----
+    float* qp[2][B200RL_MAX_LAYERS + 1];
+    for (int qi = 0; qi < 2; ++qi) {
+      qp[qi][0] = const_cast<float*>(s_obs);
+      for (int l = 1; l <= Lq; ++l) qp[qi][l] = h->acts[qi == 0 ? 1 : 4][l];
+    }
+    if (edge(s, s2)) return 1;
+    if (net_forward(q2, qp[1], B, s2, h->sac_act, A, O)) return 1;
+    if (net_forward(q1, qp[0], B, s, h->sac_act, A, O)) return 1;
+    if (edge(s2, s)) return 1;
+    sac_policy_loss_kernel<<<1, GTHREADS, 0, s>>>(qp[0][Lq], qp[1][Lq], h->sac_logp, alpha, B, h->dq, h->dq2,
+                                                  h->out_lp + st, h->out_logp + st);
+    if (launched()) return 1;
+    if (edge(s, s2)) return 1;
+    if (net_backward(h, q2, qp[1], h->dq2, 1, B, false, h->x_cat2, s2, true)) return 1;
+    if (sp.learn_alpha) {  // -mean(log_alpha (log pi + target_entropy)), one Adam step; alpha[st + 1] = exp(log_alpha)
+      sac_alpha_step_kernel<<<1, GTHREADS, 0, s2>>>(h->sac_logp, B, (float)sp.target_entropy, h->sac_state,
+                                                    h->adam_tab + (size_t)3 * maxS, st, (float)(1.0 - sp.alpha_beta1),
+                                                    (float)sp.alpha_beta2, (float)(1.0 - sp.alpha_beta2),
+                                                    (float)sp.alpha_eps, h->sac_alpha + st + 1);
+      if (launched()) return 1;
+    }
+    if (net_backward(h, q1, qp[0], h->dq, 1, B, false, h->x_cat, s)) return 1;
+    if (edge(s2, s)) return 1;
+    sac_squash_backward_kernel<<<(B * A + ew - 1) / ew, ew, 0, s>>>(pa[Lp], eps_cur, h->x_cat + O, h->x_cat2 + O, O + A,
+                                                                   B, A, lmin, lmax, limit, alpha, h->sac_dout);
+    if (launched()) return 1;
+    if (net_backward(h, pi, pa, h->sac_dout, 2 * A, B, true, nullptr, s, false, nullptr, 0, 0, s3)) return 1;
+    if (adam_net(pi, h->adam_tab, st, hp->policy_beta1, hp->policy_beta2, hp->policy_eps, s)) return 1;
+    if (edge(s4, s)) return 1;
+  }
   return 0;
 }
 
@@ -1188,6 +1528,14 @@ static int build_program(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
   return 0;
 }
 
+// SAC engines: b200rl_offpolicy_set_sac must have been called, and the host paths must hand over the [S, 2, B, A] draws
+static int sac_ready(const b200rl_offpolicy* h, bool noise_given, const char* what) {
+  if (!h->sac) return 0;
+  B200RL_REQUIRE(h->sac_set, "%s: a SAC engine needs b200rl_offpolicy_set_sac before it trains", what);
+  B200RL_REQUIRE(noise_given, "%s: SAC needs the noise draws [S, 2, B, A]", what);
+  return 0;
+}
+
 // Runs the S steps on minibatches ALREADY staged in h->obs ... h->eps (stream h->gs) and reads the logs back.
 static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int32_t S, int32_t B, float* q1_values,
                       float* q2_values, float* q1_losses, float* q2_losses, float* policy_losses,
@@ -1198,7 +1546,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
 
   // Adam's step-dependent scalars for the steps of this call (torch's host-side double arithmetic), one small upload
   const int maxS = h->cfg.max_steps;
-  const int n_pol_expected = (S + hp->policy_delay - 1) / hp->policy_delay;
+  const int n_pol_expected = h->sac ? S : (S + hp->policy_delay - 1) / hp->policy_delay;  // SAC: no delay
   for (int k = 0; k < n_pol_expected; ++k)
     adam_scalars(h->net[0].step + k + 1, hp->policy_lr, hp->policy_beta1, hp->policy_beta2, &h->h_adam_tab[k].x,
                  &h->h_adam_tab[k].y);
@@ -1206,13 +1554,20 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
     for (int k = 0; k < S; ++k)
       adam_scalars(h->net[1 + qi].step + k + 1, qi == 0 ? hp->q1_lr : hp->q2_lr, hp->q_beta1, hp->q_beta2,
                    &h->h_adam_tab[(size_t)(1 + qi) * maxS + k].x, &h->h_adam_tab[(size_t)(1 + qi) * maxS + k].y);
-  B200RL_CUDA(cudaMemcpyAsync(h->adam_tab, h->h_adam_tab, 3 * (size_t)maxS * sizeof(float2), cudaMemcpyHostToDevice, s));
+  const bool learn_alpha = h->sac && h->sac_hp.learn_alpha;
+  if (learn_alpha)
+    for (int k = 0; k < S; ++k)
+      adam_scalars(h->alpha_step + k + 1, h->sac_hp.alpha_lr, h->sac_hp.alpha_beta1, h->sac_hp.alpha_beta2,
+                   &h->h_adam_tab[(size_t)3 * maxS + k].x, &h->h_adam_tab[(size_t)3 * maxS + k].y);
+  B200RL_CUDA(cudaMemcpyAsync(h->adam_tab, h->h_adam_tab, (h->sac ? 4 : 3) * (size_t)maxS * sizeof(float2),
+                              cudaMemcpyHostToDevice, s));
 
   int n_pol = 0;
   // opt-in: on B200 it measured 12.1 ms per 50 TD3 steps against 11.1 ms for the graph replay (B = 256, 256-wide nets) -- the
-  // 32 x 32 fp32 tiles themselves, two per SM in the phases that merge four networks, are the cost, not the launches
+  // 32 x 32 fp32 tiles themselves, two per SM in the phases that merge four networks, are the cost, not the launches.
+  // SAC has no program for it and always takes the graph (or plain launches).
   const char* menv = getenv("B200RL_OFFPOLICY_MEGAKERNEL");
-  const bool use_mega = menv != nullptr && menv[0] == '1';
+  const bool use_mega = menv != nullptr && menv[0] == '1' && !h->sac;
   const char* genv = getenv("B200RL_OFFPOLICY_GRAPH");
   const bool use_graph = !(genv != nullptr && genv[0] == '0');
   if (use_mega) {
@@ -1242,16 +1597,28 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
                                             dim3(GTHREADS), kargs, 0, s));
     count_launch(1);
   } else if (!use_graph) {
-    if (enqueue_steps(h, hp, S, B, s, &n_pol)) return 1;
+    if (h->sac) {
+      if (enqueue_sac_steps(h, hp, S, B, s)) return 1;
+      n_pol = S;
+    } else if (enqueue_steps(h, hp, S, B, s, &n_pol)) {
+      return 1;
+    }
   } else {
-    if (h->graph == nullptr || h->graph_S != S || h->graph_B != B || memcmp(&h->graph_hp, hp, sizeof(*hp)) != 0) {
+    if (h->graph == nullptr || h->graph_S != S || h->graph_B != B || memcmp(&h->graph_hp, hp, sizeof(*hp)) != 0 ||
+        memcmp(&h->graph_sac_hp, &h->sac_hp, sizeof(h->sac_hp)) != 0) {
       if (h->graph) {
         cudaGraphExecDestroy(h->graph);
         h->graph = nullptr;
       }
       const int64_t l0 = launches_total();
       B200RL_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-      const int rc = enqueue_steps(h, hp, S, B, s, &n_pol);
+      int rc;
+      if (h->sac) {
+        rc = enqueue_sac_steps(h, hp, S, B, s);
+        n_pol = S;
+      } else {
+        rc = enqueue_steps(h, hp, S, B, s, &n_pol);
+      }
       cudaGraph_t g = nullptr;
       const cudaError_t ce = cudaStreamEndCapture(s, &g);
       if (rc || ce != cudaSuccess || g == nullptr) {
@@ -1271,6 +1638,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
       h->graph_S = S;
       h->graph_B = B;
       h->graph_hp = *hp;
+      h->graph_sac_hp = h->sac_hp;
       h->graph_npol = n_pol;
     }
     n_pol = h->graph_npol;
@@ -1280,6 +1648,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   h->net[0].step += n_pol;
   h->net[1].step += S;
   if (td3) h->net[2].step += S;
+  if (learn_alpha) h->alpha_step += S;
   // one device -> host read of everything train() logs
   B200RL_CUDA(cudaMemcpyAsync(q1_values, h->out_q1, SB * 4, cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaMemcpyAsync(q1_losses, h->out_l1, (size_t)S * 4, cudaMemcpyDeviceToHost, s));
@@ -1306,6 +1675,7 @@ extern "C" int b200rl_offpolicy_train(b200rl_offpolicy* h, const b200rl_offpolic
   B200RL_REQUIRE(!td3 || (q2_values && q2_losses), "offpolicy_train: TD3 needs the Q2 outputs");
   B200RL_REQUIRE(!hp->use_target_noise || noise, "offpolicy_train: target noise requested but no noise given");
   B200RL_REQUIRE(hp->policy_delay >= 1, "offpolicy_train: policy_delay must be >= 1");
+  if (sac_ready(h, noise != nullptr, "offpolicy_train")) return 2;
   cudaStream_t user = static_cast<cudaStream_t>(stream);
   cudaStream_t s = h->gs;  // everything runs on the engine's stream, ordered after the caller's
   const int O = h->O, A = h->A;
@@ -1320,7 +1690,8 @@ extern "C" int b200rl_offpolicy_train(b200rl_offpolicy* h, const b200rl_offpolic
   B200RL_CUDA(cudaMemcpyAsync(h->rew, rew, SB * 4, cudaMemcpyHostToDevice, s));
   B200RL_CUDA(cudaMemcpyAsync(h->nobs, next_obs, SB * O * 4, cudaMemcpyHostToDevice, s));
   B200RL_CUDA(cudaMemcpyAsync(h->done, done, SB * 4, cudaMemcpyHostToDevice, s));
-  if (hp->use_target_noise) B200RL_CUDA(cudaMemcpyAsync(h->eps, noise, SB * A * 4, cudaMemcpyHostToDevice, s));
+  if (h->sac) B200RL_CUDA(cudaMemcpyAsync(h->eps, noise, 2 * SB * A * 4, cudaMemcpyHostToDevice, s));
+  else if (hp->use_target_noise) B200RL_CUDA(cudaMemcpyAsync(h->eps, noise, SB * A * 4, cudaMemcpyHostToDevice, s));
 
 
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
@@ -1340,6 +1711,7 @@ extern "C" int b200rl_offpolicy_train_gather(b200rl_offpolicy* h, const b200rl_o
   B200RL_REQUIRE(!td3 || (q2_values && q2_losses), "offpolicy_train_gather: TD3 needs the Q2 outputs");
   B200RL_REQUIRE(!hp->use_target_noise || noise, "offpolicy_train_gather: target noise requested but no noise given");
   B200RL_REQUIRE(hp->policy_delay >= 1, "offpolicy_train_gather: policy_delay must be >= 1");
+  if (sac_ready(h, noise != nullptr, "offpolicy_train_gather")) return 2;
   const size_t SB = (size_t)S * B;
   for (size_t i = 0; i < SB; ++i)
     B200RL_REQUIRE(idx[i] >= 0 && idx[i] < rows, "offpolicy_train_gather: index %lld outside the %lld replay rows",
@@ -1353,7 +1725,8 @@ extern "C" int b200rl_offpolicy_train_gather(b200rl_offpolicy* h, const b200rl_o
   B200RL_CUDA(cudaStreamWaitEvent(s, h->ev, 0));
   // the minibatches are gathered on the device from the replay columns: only the indices (and noise) cross PCIe
   B200RL_CUDA(cudaMemcpyAsync(h->idx, idx, SB * sizeof(long long), cudaMemcpyHostToDevice, s));
-  if (hp->use_target_noise) B200RL_CUDA(cudaMemcpyAsync(h->eps, noise, SB * A * 4, cudaMemcpyHostToDevice, s));
+  if (h->sac) B200RL_CUDA(cudaMemcpyAsync(h->eps, noise, 2 * SB * A * 4, cudaMemcpyHostToDevice, s));
+  else if (hp->use_target_noise) B200RL_CUDA(cudaMemcpyAsync(h->eps, noise, SB * A * 4, cudaMemcpyHostToDevice, s));
   const struct { const float* src; float* dst; int w; } cols[5] = {
       {d_obs, h->obs, O}, {d_act, h->act, A}, {d_rew, h->rew, 1}, {d_next_obs, h->nobs, O}, {d_done, h->done, 1}};
   for (const auto& c : cols) {
@@ -1386,6 +1759,7 @@ extern "C" int b200rl_offpolicy_train_gather_rng(b200rl_offpolicy* h, const b200
   const bool td3 = h->cfg.n_q == 2;
   B200RL_REQUIRE(!td3 || (q2_values && q2_losses), "offpolicy_train_gather_rng: TD3 needs the Q2 outputs");
   B200RL_REQUIRE(hp->policy_delay >= 1, "offpolicy_train_gather_rng: policy_delay must be >= 1");
+  if (sac_ready(h, true, "offpolicy_train_gather_rng")) return 2;
   cudaStream_t user = static_cast<cudaStream_t>(stream);
   cudaStream_t s = h->gs;
   const int O = h->O, A = h->A;
@@ -1394,7 +1768,7 @@ extern "C" int b200rl_offpolicy_train_gather_rng(b200rl_offpolicy* h, const b200
   if (S == 0) return 0;
   B200RL_CUDA(cudaEventRecord(h->ev, user));
   B200RL_CUDA(cudaStreamWaitEvent(s, h->ev, 0));
-  const long long n_eps = hp->use_target_noise ? SB * A : 0;
+  const long long n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise ? SB * A : 0);
   const long long n_thr = ((SB > n_eps ? SB : n_eps) + 3) / 4;
   draw_minibatches_kernel<<<(int)((n_thr + 255) / 256), 256, 0, s>>>(h->idx, SB, n_eps ? h->eps : nullptr, n_eps, seed, call,
                                                                     ring_start, ring_size, rows);
@@ -1422,7 +1796,7 @@ extern "C" int b200rl_offpolicy_get_draws(b200rl_offpolicy* h, int32_t S, int32_
   const size_t SB = (size_t)S * B;
   static_assert(sizeof(long long) == sizeof(int64_t), "index width");
   B200RL_CUDA(cudaMemcpyAsync(idx, h->idx, SB * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-  if (noise) B200RL_CUDA(cudaMemcpyAsync(noise, h->eps, SB * h->A * 4, cudaMemcpyDeviceToHost, s));
+  if (noise) B200RL_CUDA(cudaMemcpyAsync(noise, h->eps, (h->sac ? 2 : 1) * SB * h->A * 4, cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaStreamSynchronize(s));
   return 0;
 }

@@ -319,12 +319,15 @@ class OnPolicyEngine:
 
 
 class OffPolicyEngine:
-    """Device-resident state of one DDPG / TD3 learner (C ABI: b200rl_offpolicy_*)."""
+    """Device-resident state of one DDPG / TD3 (``algo`` 0) or SAC (``algo`` 1) learner (C ABI: b200rl_offpolicy_*).
+    SAC: ``n_q`` = 2, the policy maps obs -> [mean | log_std] (2A outputs), there is no target policy (network 3), and
+    ``set_sac`` must be called before the first train call."""
 
     NETS = {"policy": 0, "q1": 1, "q2": 2, "target_policy": 3, "target_q1": 4, "target_q2": 5}
+    TD3, SAC = 0, 1
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
-                 q_acts=("relu", "identity")):
+                 q_acts=("relu", "identity"), algo: int = 0):
         from ._lib import OffPolicyConfig
         self.lib = _lib.load()
         current_stream_handle()
@@ -332,6 +335,8 @@ class OffPolicyEngine:
         cfg.policy = MlpDesc.make(policy_sizes, *policy_acts)
         cfg.q = MlpDesc.make(q_sizes, *q_acts)
         cfg.n_q, cfg.max_minibatch, cfg.max_steps = int(n_q), int(max_minibatch), int(max_steps)
+        cfg.algo = int(algo)
+        self.algo = int(algo)
         self.n_q, self.max_minibatch, self.max_steps = int(n_q), int(max_minibatch), int(max_steps)
         self.policy_sizes, self.q_sizes = list(policy_sizes), list(q_sizes)
         self.policy_acts, self.q_acts = tuple(policy_acts), tuple(q_acts)
@@ -386,7 +391,8 @@ class OffPolicyEngine:
         """[(kind, net index, offset, count)] of the state blob: ("params", 0..5) then ("m" / "v", 0..2); every
         segment starts on a multiple of 64 floats (b200rl.h)."""
         pad = lambda n: (n + 63) & ~63
-        present = [0, 1] + ([2] if self.n_q == 2 else []) + [3, 4] + ([5] if self.n_q == 2 else [])
+        present = [0, 1] + ([2] if self.n_q == 2 else []) + ([] if self.algo == self.SAC else [3]) + [4] + \
+            ([5] if self.n_q == 2 else [])
         out, off = [], 0
         for i in present:
             out.append(("params", i, off, self._n(i)))
@@ -430,8 +436,37 @@ class OffPolicyEngine:
         check(self.lib.b200rl_offpolicy_set_state(self.h, C.c_void_p(buf.data_ptr()), buf.numel(), st,
                                                   current_stream_handle()), "set_state")
 
+    # ---- SAC ----
+    def set_sac(self, sp) -> None:
+        """``sp``: a ``_lib.SacHparams`` (fixed or learned temperature, its Adam settings, the log_std clamp)."""
+        check(self.lib.b200rl_offpolicy_set_sac(self.h, C.byref(sp)), "set_sac")
+
+    def set_alpha(self, log_alpha: float, exp_avg: float = 0.0, exp_avg_sq: float = 0.0, step: int = 0) -> None:
+        check(self.lib.b200rl_offpolicy_set_alpha(self.h, float(log_alpha), float(exp_avg), float(exp_avg_sq), int(step)),
+              "set_alpha")
+
+    def get_alpha(self):
+        """(log_alpha, exp_avg, exp_avg_sq, step) of the temperature, float32 values as Python floats."""
+        la, m, v, step = C.c_float(), C.c_float(), C.c_float(), C.c_int64()
+        check(self.lib.b200rl_offpolicy_get_alpha(self.h, C.byref(la), C.byref(m), C.byref(v), C.byref(step)),
+              "get_alpha")
+        return la.value, m.value, v.value, int(step.value)
+
+    def sac_outputs(self, S: int):
+        """(mean log pi per step [S], alpha used by each step [S]) of the last train call."""
+        lp, al = np.zeros(S, np.float32), np.zeros(S, np.float32)
+        check(self.lib.b200rl_offpolicy_sac_outputs(self.h, int(S), _ptr(lp), _ptr(al)), "sac_outputs")
+        return lp, al
+
+    def _outputs(self, S, q1v, q2v, l1, l2, lp, npol):
+        out = dict(q1_values=q1v, q2_values=q2v, q1_losses=l1, q2_losses=l2, policy_losses=lp[:npol.value])
+        if self.algo == self.SAC:
+            out["log_prob_means"], out["alphas"] = self.sac_outputs(S)
+        return out
+
     def train(self, hp, obs, act, rew, next_obs, done, noise=None):
-        """obs/next_obs [S,B,O], act [S,B,A], rew/done [S,B], noise [S,B,A] or None -> dict of logged quantities."""
+        """obs/next_obs [S,B,O], act [S,B,A], rew/done [S,B], noise [S,B,A] or None (SAC: [S,2,B,A], required) -> dict
+        of logged quantities (SAC adds log_prob_means and alphas)."""
         obs, act, next_obs = _c(obs, np.float32), _c(act, np.float32), _c(next_obs, np.float32)
         rew, done = _c(rew, np.float32), _c(done, np.float32)
         noise = None if noise is None else _c(noise, np.float32)
@@ -442,7 +477,7 @@ class OffPolicyEngine:
         check(self.lib.b200rl_offpolicy_train(self.h, C.byref(hp), S, B, _ptr(obs), _ptr(act), _ptr(rew), _ptr(next_obs),
                                               _ptr(done), _ptr(noise), _ptr(q1v), _ptr(q2v), _ptr(l1), _ptr(l2), _ptr(lp),
                                               C.byref(npol), current_stream_handle()), "offpolicy_train")
-        return dict(q1_values=q1v, q2_values=q2v, q1_losses=l1, q2_losses=l2, policy_losses=lp[:npol.value])
+        return self._outputs(S, q1v, q2v, l1, l2, lp, npol)
 
     def train_gather_rng(self, hp, columns, rows: int, ring_start: int, ring_size: int, S: int, B: int, seed: int, call: int):
         """``train_gather`` with the indices and the smoothing noise drawn on the device (Philox keyed by ``seed``, block
@@ -456,13 +491,17 @@ class OffPolicyEngine:
                                                          int(ring_size), int(seed) & (2 ** 64 - 1), int(call), _ptr(q1v),
                                                          _ptr(q2v), _ptr(l1), _ptr(l2), _ptr(lp), C.byref(npol),
                                                          current_stream_handle()), "offpolicy_train_gather_rng")
-        return dict(q1_values=q1v, q2_values=q2v, q1_losses=l1, q2_losses=l2, policy_losses=lp[:npol.value])
+        return self._outputs(S, q1v, q2v, l1, l2, lp, npol)
 
     def get_draws(self, S: int, B: int, with_noise: bool = True):
-        """(physical rows [S,B] int64, noise [S,B,A] float32 or None) of the last train_gather / train_gather_rng call."""
+        """(physical rows [S,B] int64, noise [S,B,A] (SAC: [S,2,B,A]) float32 or None) of the last train_gather /
+        train_gather_rng call."""
         idx = np.empty((S, B), np.int64)
-        A = self.policy_sizes[-1]
-        noise = np.empty((S, B, A), np.float32) if with_noise else None
+        if self.algo == self.SAC:
+            shape = (S, 2, B, self.policy_sizes[-1] // 2)
+        else:
+            shape = (S, B, self.policy_sizes[-1])
+        noise = np.empty(shape, np.float32) if with_noise else None
         check(self.lib.b200rl_offpolicy_get_draws(self.h, S, B, _ptr(idx), _ptr(noise), current_stream_handle()), "get_draws")
         return idx, noise
 
@@ -479,4 +518,4 @@ class OffPolicyEngine:
         check(self.lib.b200rl_offpolicy_train_gather(self.h, C.byref(hp), S, B, *ptrs, int(rows), _ptr(idx), _ptr(noise),
                                                      _ptr(q1v), _ptr(q2v), _ptr(l1), _ptr(l2), _ptr(lp), C.byref(npol),
                                                      current_stream_handle()), "offpolicy_train_gather")
-        return dict(q1_values=q1v, q2_values=q2v, q1_losses=l1, q2_losses=l2, policy_losses=lp[:npol.value])
+        return self._outputs(S, q1v, q2v, l1, l2, lp, npol)

@@ -1,3 +1,5 @@
-from .base import (CategoricalPolicy, DeterministicPolicy, GaussianPolicy, Policy, RandomPolicy, StochasticPolicy)
+from .base import (CategoricalPolicy, DeterministicPolicy, GaussianPolicy, Policy, RandomPolicy,
+                   SquashedGaussianPolicy, StochasticPolicy)
 
-__all__ = ["Policy", "StochasticPolicy", "CategoricalPolicy", "GaussianPolicy", "DeterministicPolicy", "RandomPolicy"]
+__all__ = ["Policy", "StochasticPolicy", "CategoricalPolicy", "GaussianPolicy", "SquashedGaussianPolicy",
+           "DeterministicPolicy", "RandomPolicy"]

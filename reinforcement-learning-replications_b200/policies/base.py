@@ -68,6 +68,52 @@ class GaussianPolicy(StochasticPolicy):
         return Independent(Normal(loc=self.network(observation), scale=torch.exp(self.log_std)), 1)
 
 
+class SquashedGaussianPolicy(StochasticPolicy):
+    """The SAC actor (Spinning Up sac/core.py SquashedGaussianMLPActor) with its mean and log_std layers stacked as the
+    network's last Linear: network(obs) = [mu | log_std] (2A outputs, Identity output).  log_std is clamped to
+    [log_std_min, log_std_max]; the action is action_limit * tanh(u), u ~ Normal(mu, exp(log_std))."""
+
+    def __init__(self, network: nn.Module, optimizer: Optimizer, action_limit: float = 1.0, log_std_min: float = -20.0,
+                 log_std_max: float = 2.0):
+        super().__init__()
+        self.network = network
+        self.optimizer = optimizer
+        self.action_limit, self.log_std_min, self.log_std_max = float(action_limit), float(log_std_min), float(log_std_max)
+
+    def forward(self, observation: Tensor, deterministic: bool = False, with_logprob: bool = True):
+        """(action, log pi(action | observation) or None).  deterministic: u = mu."""
+        out = self.network(observation)
+        A = out.shape[-1] // 2
+        mu, log_std = out[..., :A], torch.clamp(out[..., A:], self.log_std_min, self.log_std_max)
+        dist = Normal(mu, torch.exp(log_std))
+        u = mu if deterministic else dist.rsample()
+        log_prob = None
+        if with_logprob:  # the tanh change of variables in its numerically stable form (Spinning Up, SAC paper eq. 21)
+            log_prob = dist.log_prob(u).sum(-1) - (2 * (np.log(2) - u - nn.functional.softplus(-2 * u))).sum(-1)
+        return self.action_limit * torch.tanh(u), log_prob
+
+    def get_action_tensor(self, observation: Tensor) -> Tensor:
+        with torch.no_grad():
+            return self.forward(observation, with_logprob=False)[0]
+
+    def deterministic(self) -> "Policy":
+        """A view that acts with action_limit * tanh(mu) (evaluation); it shares this policy's network."""
+        return _SquashedMeanPolicy(self)
+
+
+class _SquashedMeanPolicy(Policy):
+    def __init__(self, policy: SquashedGaussianPolicy):
+        super().__init__()
+        self.policy = policy
+
+    def get_action_tensor(self, observation: Tensor) -> Tensor:
+        with torch.no_grad():
+            return self.policy.forward(observation, deterministic=True, with_logprob=False)[0]
+
+    def get_action_numpy(self, observation: np.ndarray) -> np.ndarray:
+        return np.asarray(self.get_action_tensor(torch.from_numpy(observation).float()).numpy())
+
+
 class DeterministicPolicy(Policy):
     """ref: policies/deterministic_policy.py:9-45"""
 

@@ -27,6 +27,7 @@ extern "C" {
 
 #define B200RL_VERSION 100
 #define B200RL_MAX_LAYERS 4   /* Linear layers per MLP */
+#define B200RL_MAX_LEARNERS 16 /* learners in one off-policy group (b200rl_offpolicy_create_group) */
 #define B200RL_N_SCALARS 8    /* per-launch scalar sums, see b200rl_mlp_loss_grad */
 
 enum b200rl_activation { B200RL_ACT_IDENTITY = 0, B200RL_ACT_TANH = 1, B200RL_ACT_RELU = 2 };
@@ -435,6 +436,48 @@ int b200rl_offpolicy_set_alpha(b200rl_offpolicy* h, float log_alpha, float exp_a
 int b200rl_offpolicy_get_alpha(b200rl_offpolicy* h, float* log_alpha, float* exp_avg, float* exp_avg_sq, int64_t* step);
 /* After a train call of S steps: mean log pi of each policy step and the alpha each step used (host [S] each). */
 int b200rl_offpolicy_sac_outputs(b200rl_offpolicy* h, int32_t S, float* log_prob_means, float* alphas);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Learner groups: K independent off-policy learners (same config, same hyper-parameters, their own parameters, Adam
+ * states, step counts, minibatches, noise, replay buffers and temperature) trained by one engine, every operation of a
+ * step ONE launch for all K.  Each learner's arithmetic -- tile shapes, summation order, Adam's operation order -- is
+ * that of a solo engine, so learner z of a group produces bit for bit what a solo engine fed learner z's inputs does.
+ * Everything the engine owns for one learner lives in one arena; the K arenas lie at a fixed stride (a multiple of
+ * 256 bytes), and a kernel finds learner z's buffers at + z * stride.
+ *
+ * b200rl_offpolicy_create is the group of one.  For K > 1 the calls above take and return a leading [K] axis, which
+ * for K = 1 is exactly the solo layout: state_floats = K x the per-learner blob, get_state / set_state move
+ * [K][blob] with steps[K][3]; train takes [K, S, B, ...] minibatches and [K, S, B, A] noise (SAC [K, S, 2, B, A]) and
+ * returns values [K, S, B], losses [K, S] and policy_losses [K, S] (the first *n_policy_updates of each row; the
+ * policy-delay schedule is shared); get_draws and sac_outputs likewise.  train_gather, train_gather_rng, set_alpha and
+ * get_alpha are the group calls below with K = 1 and refuse K > 1; the per-network accessors (set_params, get_params,
+ * set_adam, get_adam) refuse K > 1: a group's state moves as the blob.  The persistent step kernel
+ * (B200RL_OFFPOLICY_MEGAKERNEL=1) does not apply to K > 1: a group runs as a CUDA graph, or as plain launches with
+ * B200RL_OFFPOLICY_GRAPH=0.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  const float *obs, *act, *rew, *next_obs, *done; /* device replay columns, as for b200rl_offpolicy_train_gather */
+  int64_t rows;
+} b200rl_offpolicy_replay;
+
+/* 1 <= n_learners <= B200RL_MAX_LEARNERS */
+int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg, int32_t n_learners, b200rl_offpolicy** out);
+/* replay[K]: each learner's own columns and row count; idx [K, S, B] physical rows of each learner's buffer */
+int b200rl_offpolicy_train_gather_group(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int32_t S, int32_t B,
+                                        const b200rl_offpolicy_replay* replay, const int64_t* idx, const float* noise,
+                                        float* q1_values, float* q2_values, float* q1_losses, float* q2_losses,
+                                        float* policy_losses, int32_t* n_policy_updates, void* stream);
+/* ring_start / ring_size / seed / call [K]: learner z's draws equal those of a solo engine with seed[z], call[z] */
+int b200rl_offpolicy_train_gather_rng_group(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int32_t S,
+                                            int32_t B, const b200rl_offpolicy_replay* replay, const int64_t* ring_start,
+                                            const int64_t* ring_size, const uint64_t* seed, const uint64_t* call,
+                                            float* q1_values, float* q2_values, float* q1_losses, float* q2_losses,
+                                            float* policy_losses, int32_t* n_policy_updates, void* stream);
+/* [K] entries each */
+int b200rl_offpolicy_set_alpha_group(b200rl_offpolicy* h, const float* log_alpha, const float* exp_avg,
+                                     const float* exp_avg_sq, const int64_t* step);
+int b200rl_offpolicy_get_alpha_group(b200rl_offpolicy* h, float* log_alpha, float* exp_avg, float* exp_avg_sq,
+                                     int64_t* step);
 
 #ifdef __cplusplus
 }

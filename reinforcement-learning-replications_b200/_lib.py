@@ -11,6 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200RL_LIB") or os.path.join(HERE, "libb200rl.so")  # B200RL_LIB: an A/B build of the library
 
 MAX_LAYERS = 4
+MAX_LEARNERS = 16
 N_SCALARS = 8
 ACT = {"identity": 0, "tanh": 1, "relu": 2}
 DIST = {"none": 0, "gaussian": 1, "categorical": 2}
@@ -89,6 +90,11 @@ class SacHparams(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+class OffPolicyReplay(C.Structure):
+    _fields_ = [("obs", C.c_void_p), ("act", C.c_void_p), ("rew", C.c_void_p), ("next_obs", C.c_void_p),
+                ("done", C.c_void_p), ("rows", C.c_int64)]
+
+
 class OffPolicyHparams(C.Structure):
     _fields_ = [("gamma", C.c_double), ("polyak_rho", C.c_double), ("target_noise_scale", C.c_double),
                 ("target_noise_clip", C.c_double), ("action_limit", C.c_double), ("policy_delay", C.c_int32),
@@ -165,6 +171,15 @@ SIGNATURES = {
     "b200rl_offpolicy_get_alpha": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float),
                                              C.POINTER(C.c_float), C.POINTER(C.c_int64)]),
     "b200rl_offpolicy_sac_outputs": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "b200rl_offpolicy_create_group": (C.c_int, [C.POINTER(OffPolicyConfig), C.c_int32, C.POINTER(C.c_void_p)]),
+    "b200rl_offpolicy_train_gather_group": (C.c_int, [C.c_void_p, C.POINTER(OffPolicyHparams), C.c_int32, C.c_int32,
+                                                      C.POINTER(OffPolicyReplay)] + [C.c_void_p] * 7 +
+                                            [C.POINTER(C.c_int32), C.c_void_p]),
+    "b200rl_offpolicy_train_gather_rng_group": (C.c_int, [C.c_void_p, C.POINTER(OffPolicyHparams), C.c_int32, C.c_int32,
+                                                          C.POINTER(OffPolicyReplay)] + [C.c_void_p] * 9 +
+                                                [C.POINTER(C.c_int32), C.c_void_p]),
+    "b200rl_offpolicy_set_alpha_group": (C.c_int, [C.c_void_p] * 5),
+    "b200rl_offpolicy_get_alpha_group": (C.c_int, [C.c_void_p] * 5),
     "b200rl_discounted_cumsum": (C.c_int, [C.c_void_p, C.c_int64, C.c_double, C.c_void_p, C.c_void_p]),
     "b200rl_gae_f64": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_double, C.c_double, C.c_void_p,
                                  C.c_void_p]),

@@ -1,7 +1,8 @@
+from .group import LearnerGroup
 from .ppo import PPO
 from .sac import SAC
 from .td3 import DDPG, TD3
 from .trpo import TRPO
 from .vpg import VPG
 
-__all__ = ["VPG", "TRPO", "PPO", "DDPG", "TD3", "SAC"]
+__all__ = ["VPG", "TRPO", "PPO", "DDPG", "TD3", "SAC", "LearnerGroup"]

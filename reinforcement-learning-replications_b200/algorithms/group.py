@@ -1,0 +1,211 @@
+"""LearnerGroup: several independent TD3 / DDPG / SAC learners (typically one per seed) trained side by side by ONE
+off-policy engine, every operation of a train step one launch for all of them (b200rl_offpolicy_create_group).
+
+The contract: each member ends up bit for bit where it would be had it run alone.  Members keep everything of their
+own -- environment, sampler, replay buffer, evaluator, networks, Adam states and step counts, temperature -- and their
+own random streams: ``add`` records the current state of the generators ``set_seed_for_libraries`` seeds (Python
+``random``, NumPy's global ``np.random``, torch's default CPU generator) as that member's stream, and every piece of
+host work the group does for a member (minibatch index draws, target-smoothing / SAC noise, sampling, exploration,
+evaluation) runs with that stream installed.  After a group call the global generators are as they were before it.
+
+    group = LearnerGroup()
+    for seed in (0, 1, 2):
+        set_seed_for_libraries(seed)
+        group.add(build_td3(seed))
+    group.learn(num_epochs=..., output_dirs=["seed-0", "seed-1", "seed-2"])
+"""
+from __future__ import annotations
+
+import contextlib
+import random
+from typing import List, Sequence
+
+import numpy as np
+import torch
+
+from .._lib import MAX_LEARNERS
+from ..engine import OffPolicyEngine
+from ._onpolicy import adam_hparams, describe_mlp
+from .td3 import _learn_begin, _learn_evaluate_save, _learn_sample, _OffPolicyBase
+
+
+def _signature(agent) -> list:
+    """[(attribute, value)] that every member of a group shares (one engine trains them all), in the order in which a
+    refusal reports the first difference."""
+    trainable, _ = agent._nets()
+    names = ["policy"] + (["q_function_1", "q_function_2"] if agent.n_q == 2 else ["q_function"])
+    sig = [("class", type(agent).__name__)]
+    for name, m in zip(names, trainable):
+        sizes, hidden_act, out_act, lins = describe_mlp(m.network)
+        sig.append((f"{name} network", (tuple(sizes), hidden_act, out_act)))
+        sig.append((f"{name} optimizer (lr, beta1, beta2, eps)", adam_hparams(m.optimizer, lins, f"{name} optimizer")))
+    sig.append(("action limit", float(agent.env.action_space.high[0])))
+    for attr in ("gamma", "polyak_rho", "target_noise_scale", "target_noise_clip", "policy_delay", "use_device_replay",
+                 "use_device_rng"):
+        sig.append((attr, getattr(agent, attr, None)))
+    if agent.algo == OffPolicyEngine.SAC:
+        sig += [("alpha", agent.alpha), ("learn_alpha", agent.learn_alpha), ("target_entropy", agent.target_entropy),
+                ("alpha optimizer (lr, beta1, beta2, eps)",
+                 adam_hparams(agent.alpha_optimizer, [], "alpha optimizer", extra=[agent.log_alpha])),
+                ("log_std bounds", (agent.policy.log_std_min, agent.policy.log_std_max))]
+    return sig
+
+
+def _rng_state():
+    return random.getstate(), np.random.get_state(), torch.get_rng_state()
+
+
+def _set_rng_state(state) -> None:
+    random.setstate(state[0])
+    np.random.set_state(state[1])
+    torch.set_rng_state(state[2])
+
+
+class LearnerGroup:
+    """Up to ``MAX_LEARNERS`` (16) off-policy learners of one class with the same network shapes and hyper-parameters
+    (Adam step counts may differ), trained in lockstep by one engine."""
+
+    def __init__(self) -> None:
+        self.members: List[_OffPolicyBase] = []
+        self._streams: list = []
+        self._engine = None
+
+    def __len__(self) -> int:
+        return len(self.members)
+
+    def add(self, agent) -> None:
+        """Add ``agent``; the current state of the global random generators becomes its private stream."""
+        if not isinstance(agent, _OffPolicyBase):
+            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC learners, got {type(agent).__name__}")
+        if any(m is agent for m in self.members):
+            raise ValueError("LearnerGroup: this agent is already a member")
+        if len(self.members) >= MAX_LEARNERS:
+            raise ValueError(f"LearnerGroup: at most {MAX_LEARNERS} members")
+        if self.members:
+            for (name, want), (_, got) in zip(_signature(self.members[0]), _signature(agent)):
+                if got != want:
+                    raise ValueError(f"LearnerGroup: {name} differs from the first member's ({got!r} != {want!r})")
+        self.members.append(agent)
+        self._streams.append(_rng_state())
+        self._close_engine()
+
+    @contextlib.contextmanager
+    def stream(self, k: int):
+        """Run the body with member ``k``'s random stream installed; its advance is kept for the member, and the global
+        generators are restored afterwards."""
+        saved = _rng_state()
+        _set_rng_state(self._streams[k])
+        try:
+            yield
+        finally:
+            self._streams[k] = _rng_state()
+            _set_rng_state(saved)
+
+    def _check(self) -> List[_OffPolicyBase]:
+        if not self.members:
+            raise ValueError("LearnerGroup: the group has no members")
+        return self.members
+
+    def _close_engine(self) -> None:
+        if self._engine is not None:
+            self._engine.close()
+            self._engine = None
+
+    def _ensure_engine(self, S: int, B: int) -> OffPolicyEngine:
+        m = self.members[0]
+        psz, pact, pout, _ = describe_mlp(m.policy.network)
+        qsz, qact, qout, _ = describe_mlp(m._nets()[0][1].network)
+        e = self._engine
+        if (e is None or e.K != len(self.members) or e.max_minibatch < B or e.max_steps < S or e.policy_sizes != psz
+                or e.q_sizes != qsz or e.policy_acts != (pact, pout) or e.q_acts != (qact, qout)):
+            self._close_engine()
+            e = OffPolicyEngine(psz, qsz, m.n_q, B, S, (pact, pout), (qact, qout), algo=m.algo,
+                                n_learners=len(self.members))
+            self._engine = e
+        return e
+
+    def train(self, num_train_steps: int, minibatch_size: int) -> None:
+        """``agent.train(agent.replay_buffer, num_train_steps, minibatch_size)`` for every member, each on its own replay
+        buffer and random stream, as one engine call."""
+        members = self._check()
+        S, B = int(num_train_steps), int(minibatch_size)
+        if len(members) == 1 or S == 0:  # nothing to batch: the members' own calls
+            for k, m in enumerate(members):
+                with self.stream(k):
+                    m.train(m.replay_buffer, S, B)
+            return
+        noisy, delay = members[0]._train_schedule()
+        staged = []
+        for k, m in enumerate(members):
+            with self.stream(k):
+                staged.append(m._stage_inputs(m.replay_buffer, S, B, noisy))
+        mode = staged[0][0]
+        if any(st[0] != mode for st in staged):
+            raise ValueError("LearnerGroup: the members' replay buffers do not all support the same minibatch path")
+        e = self._ensure_engine(S, B)
+        plans, steps = [], []
+        for k, m in enumerate(members):
+            trainable, targets, lins = m._learner_nets()
+            slots = m._state_plan(e, trainable, targets, lins, lane=k)
+            steps.append(m._fill_state(slots, trainable, lins))
+            plans.append((slots, trainable))
+        e.set_state(None, steps)
+        sac = members[0].algo == OffPolicyEngine.SAC
+        if sac:
+            e.set_sac(members[0]._sac_hparams())
+            e.set_alpha_group([m._alpha_state() for m in members])
+        hp = members[0]._hparams(noisy, delay)
+        if mode == "rng":
+            replays = [m.replay_buffer.device_columns() for m in members]
+            rings = [m.replay_buffer.ring() for m in members]
+            out = e.train_gather_rng_group(hp, replays, [r[0] for r in rings], [r[1] for r in rings], S, B,
+                                           [st[1][0] for st in staged], [st[1][1] for st in staged])
+        elif mode == "gather":
+            replays = [m.replay_buffer.device_columns() for m in members]
+            noise = None if staged[0][1][1] is None else np.stack([st[1][1] for st in staged])
+            out = e.train_gather_group(hp, replays, np.stack([st[1][0] for st in staged]), noise)
+        else:
+            cols = [None if staged[0][1][i] is None else np.stack([st[1][i] for st in staged]) for i in range(6)]
+            out = e.train(hp, *cols)
+        _, steps = e.get_state()
+        for (slots, trainable), m, st in zip(plans, members, steps):
+            m._read_state(slots, trainable, st)
+        if sac:
+            for m, a in zip(members, e.get_alpha_group()):
+                m._store_alpha_state(*a)
+        for k, m in enumerate(members):
+            m.last_train_output = {key: v[k] for key, v in out.items()}
+            m._record_train(m.last_train_output)
+
+    def learn(self, output_dirs: Sequence[str], num_epochs: int = 2000, batch_size: int = 50, minibatch_size: int = 100,
+              num_start_steps: int = 10000, num_steps_before_update: int = 1000, num_train_steps: int = 50,
+              num_evaluation_episodes: int = 5, evaluation_interval: int = 4000, model_saving_interval: int = 4000) -> None:
+        """Every member's ``learn`` (TD3.learn's arguments, one output directory per member) in lockstep: per epoch each
+        member samples under its own stream, the members train in one group call, then each evaluates and saves.  An
+        epoch in which only some members train (their step counts differ) trains those alone."""
+        members = self._check()
+        if len(output_dirs) != len(members):
+            raise ValueError(f"LearnerGroup.learn: {len(members)} members need {len(members)} output_dirs, "
+                             f"got {len(output_dirs)}")
+        started = []
+        for k, m in enumerate(members):
+            with self.stream(k):
+                started.append(_learn_begin(m, output_dirs[k]))
+        for epoch in range(1, num_epochs + 1):
+            trains = []
+            for k, m in enumerate(members):
+                with self.stream(k):
+                    trains.append(_learn_sample(m, epoch, batch_size, num_start_steps, num_steps_before_update))
+            if all(trains):
+                self.train(num_train_steps, minibatch_size)
+            else:
+                for k, m in enumerate(members):
+                    if trains[k]:
+                        with self.stream(k):
+                            m.train(m.replay_buffer, num_train_steps, minibatch_size)
+            for k, m in enumerate(members):
+                with self.stream(k):
+                    _learn_evaluate_save(m, epoch, started[k], num_evaluation_episodes, evaluation_interval,
+                                         model_saving_interval, output_dirs[k])
+        for m in members:
+            m.metrics_manager.close()

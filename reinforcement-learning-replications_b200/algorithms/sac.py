@@ -90,15 +90,21 @@ class SAC(_OffPolicyBase):
     def _upload_state(self, e, trainable, targets, lins) -> None:
         super()._upload_state(e, trainable, targets, lins)
         e.set_sac(self._sac_hparams())
+        e.set_alpha(*self._alpha_state())
+
+    def _download_state(self, e, trainable, targets, lins) -> None:
+        super()._download_state(e, trainable, targets, lins)
+        self._store_alpha_state(*e.get_alpha())
+
+    def _alpha_state(self):
+        """(log_alpha, exp_avg, exp_avg_sq, step) of the temperature, as the engine takes it."""
         st = self.alpha_optimizer.state.get(self.log_alpha, {})
         step = int(float(st["step"])) if "exp_avg" in st else 0
         m = float(st["exp_avg"]) if step else 0.0
         v = float(st["exp_avg_sq"]) if step else 0.0
-        e.set_alpha(float(self.log_alpha.detach()), m, v, step)
+        return float(self.log_alpha.detach()), m, v, step
 
-    def _download_state(self, e, trainable, targets, lins) -> None:
-        super()._download_state(e, trainable, targets, lins)
-        log_alpha, m, v, step = e.get_alpha()
+    def _store_alpha_state(self, log_alpha, m, v, step) -> None:
         with torch.no_grad():
             self.log_alpha.fill_(log_alpha)
         if step > 0:
@@ -114,8 +120,10 @@ class SAC(_OffPolicyBase):
         _learn(self, num_epochs, batch_size, minibatch_size, num_start_steps, num_steps_before_update, num_train_steps,
                num_evaluation_episodes, evaluation_interval, model_saving_interval, output_dir)
 
-    def train(self, replay_buffer, num_train_steps: int, minibatch_size: int) -> None:
-        out = self._run(replay_buffer, num_train_steps, minibatch_size, noisy=True, delay=1)
+    def _train_schedule(self):
+        return True, 1
+
+    def _record_train(self, out) -> None:
         mm, steps = getattr(self, "metrics_manager", None), getattr(self, "current_total_steps", 0)
         if mm is None or out is None:
             return

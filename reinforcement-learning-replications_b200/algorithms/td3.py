@@ -72,17 +72,18 @@ class _OffPolicyBase:
     # user may edit or load weights), so every call moves the whole learner state down and up again -- as ONE blob per
     # direction with one synchronisation each (24 separate synchronous copies per call before: the transfers cost more
     # than the 50 train steps between them).
-    def _state_plan(self, e, trainable, targets, lins):
+    def _state_plan(self, e, trainable, targets, lins, lane: int = 0):
         """[(kind, host parameter, owning module, numpy view into the engine's host blob)] in blob order, built once per
-        (engine, networks): the blob is persistent (page-locked), so the views stay valid between calls."""
-        key = (id(e),) + tuple(id(l) for ls in lins for l in ls)
+        (engine, learner, networks): the blob is persistent (page-locked), so the views stay valid between calls.
+        ``lane``: this learner's place in a group engine's blob."""
+        key = (id(e), lane) + tuple(id(l) for ls in lins for l in ls)
         plan = getattr(self, "_plan", None)
         if plan is not None and plan[0] == key:
             return plan[1]
         layout, total = e.state_layout()
         blob = e.state_buffer()
-        assert blob.numel() == total
-        blob_np = blob.numpy()  # shares the page-locked memory
+        assert blob.numel() == total * getattr(e, "K", 1)
+        blob_np = blob.numpy()[lane * total:(lane + 1) * total]  # shares the page-locked memory
         mods = {i: (m, l) for i, (m, l) in enumerate(zip(trainable, lins))}
         mods.update({k: (m, l) for k, m, l in zip(self.target_slots, targets, lins[len(trainable):])})
         slots = []
@@ -111,7 +112,10 @@ class _OffPolicyBase:
     # kernels go parallel above 32768 elements (the 256 x 256 weights), and on a many-core host the OpenMP workers that
     # linger after such a region cost the calling thread tens of milliseconds every few train() calls.
     def _upload_state(self, e, trainable, targets, lins) -> None:
-        slots = self._state_plan(e, trainable, targets, lins)
+        e.set_state(None, self._fill_state(self._state_plan(e, trainable, targets, lins), trainable, lins))
+
+    def _fill_state(self, slots, trainable, lins):
+        """Host modules and Adam states -> this learner's part of the blob; returns its [3] Adam step counts."""
         steps = [0, 0, 0]
         for i, (m, l) in enumerate(zip(trainable, lins)):
             adam_hparams(m.optimizer, l, "optimizer")  # refuses anything but a plain Adam over exactly this network
@@ -127,11 +131,15 @@ class _OffPolicyBase:
                 view.fill(0.0)
             else:
                 np.copyto(view, src.numpy(), casting="same_kind")
-        e.set_state(None, steps)
+        return steps
 
     def _download_state(self, e, trainable, targets, lins) -> None:
         slots = self._state_plan(e, trainable, targets, lins)
         _, steps = e.get_state()
+        self._read_state(slots, trainable, steps)
+
+    def _read_state(self, slots, trainable, steps) -> None:
+        """This learner's part of the blob -> host modules and Adam states."""
         index = {id(m): i for i, m in enumerate(trainable)}
         for kind, p_, m, view in slots:
             if kind == "params":
@@ -180,9 +188,12 @@ class _OffPolicyBase:
             out[i] = torch.randn(B, A).numpy()
         return out
 
-    def _run(self, replay_buffer, num_train_steps: int, minibatch_size: int, noisy: bool, delay: int):
-        S, B = int(num_train_steps), int(minibatch_size)
-        trainable, targets = self._nets()
+    # A train() call in three phases -- draw and stage the inputs (_stage_inputs), the engine call (_call_engine), the
+    # write-back (_download_state) -- so that a LearnerGroup can run the host phases per learner and make ONE engine
+    # call for all of them.
+    def _stage_inputs(self, replay_buffer, S: int, B: int, noisy: bool):
+        """Everything of one train() call that uses the host's random streams: the minibatch indices (or, without a
+        device replay, the gathered minibatches) and the noise.  Returns (mode, inputs)."""
         # host side, same random streams as the reference: numpy RNG for the indices (replay_buffer.py:58), torch CPU
         # RNG for the target-smoothing noise (td3.py:328); the two streams are independent, so drawing all minibatches
         # first and all noise second consumes each exactly as the interleaved reference loop does.
@@ -192,13 +203,16 @@ class _OffPolicyBase:
         device_rng = device_replay and getattr(self, "use_device_rng", False) and hasattr(replay_buffer, "ring")
         def noise_of():
             return self._noise(S, B) if noisy and S > 0 else None
+        if S == 0:
+            return None, None
         if device_rng:
-            idx = noise = None
-        elif device_replay:
+            self._device_rng_calls = getattr(self, "_device_rng_calls", 0) + 1
+            return "rng", (getattr(self, "device_rng_seed", 0), self._device_rng_calls)
+        if device_replay:
             # device-resident replay columns: S index draws on the host (the same numpy stream as S sample_minibatch
             # calls); the gather happens on the GPU, only indices and noise cross PCIe
             idx = replay_buffer.physical_rows(np.stack([replay_buffer.sample_indices(B) for _ in range(S)]))
-            noise = noise_of()
+            return "gather", (idx, noise_of())
         else:
             if S > 0 and hasattr(replay_buffer, "sample_indices") and hasattr(replay_buffer, "gather"):
                 idx_l = np.stack([replay_buffer.sample_indices(B) for _ in range(S)])
@@ -212,25 +226,45 @@ class _OffPolicyBase:
             rew = stack("rewards", np.float32)                      # rewards f64 -> .float() (td3.py:226)
             nobs = stack("next_observations", np.float32)
             done = stack("dones", np.float32)                       # bool -> .int() (td3.py:228), used as (1 - d)
-        e = self._ensure_engine(max(S, 1), B)
-        lins = [describe_mlp(m.network)[3] for m in trainable + targets]
-        self._upload_state(e, trainable, targets, lins)
-        if S == 0:
-            out = None
-        elif device_rng:
+            return "host", (obs, act, rew, nobs, done, noise)
+
+    @staticmethod
+    def _call_engine(e, hp, replay_buffer, S: int, B: int, mode, inputs):
+        """The engine call of one learner (``e`` solo) on what ``_stage_inputs`` returned."""
+        if mode is None:
+            return None
+        if mode == "rng":
             columns, rows = replay_buffer.device_columns()
             start, size, _ = replay_buffer.ring()
-            self._device_rng_calls = getattr(self, "_device_rng_calls", 0) + 1
-            out = e.train_gather_rng(self._hparams(noisy, delay), columns, rows, start, size, S, B,
-                                     getattr(self, "device_rng_seed", 0), self._device_rng_calls)
-        elif device_replay:
+            return e.train_gather_rng(hp, columns, rows, start, size, S, B, *inputs)
+        if mode == "gather":
             columns, rows = replay_buffer.device_columns()
-            out = e.train_gather(self._hparams(noisy, delay), columns, rows, idx, noise)
-        else:
-            out = e.train(self._hparams(noisy, delay), obs, act, rew, nobs, done, noise)
+            return e.train_gather(hp, columns, rows, *inputs)
+        return e.train(hp, *inputs)
+
+    def _learner_nets(self):
+        """(trainable, targets, Linear layers of each) in the blob's order."""
+        trainable, targets = self._nets()
+        return trainable, targets, [describe_mlp(m.network)[3] for m in trainable + targets]
+
+    def _run(self, replay_buffer, num_train_steps: int, minibatch_size: int, noisy: bool, delay: int):
+        S, B = int(num_train_steps), int(minibatch_size)
+        mode, inputs = self._stage_inputs(replay_buffer, S, B, noisy)
+        e = self._ensure_engine(max(S, 1), B)
+        trainable, targets, lins = self._learner_nets()
+        self._upload_state(e, trainable, targets, lins)
+        out = self._call_engine(e, self._hparams(noisy, delay), replay_buffer, S, B, mode, inputs)
         self._download_state(e, trainable, targets, lins)
         self.last_train_output = out
         return out
+
+    def _train_schedule(self):
+        """(noisy, policy delay) of this algorithm's train steps."""
+        return True, int(self.policy_delay)
+
+    def train(self, replay_buffer, num_train_steps: int, minibatch_size: int) -> None:
+        noisy, delay = self._train_schedule()
+        self._record_train(self._run(replay_buffer, num_train_steps, minibatch_size, noisy=noisy, delay=delay))
 
 
 class TD3(_OffPolicyBase):
@@ -256,8 +290,7 @@ class TD3(_OffPolicyBase):
         _learn(self, num_epochs, batch_size, minibatch_size, num_start_steps, num_steps_before_update, num_train_steps,
                num_evaluation_episodes, evaluation_interval, model_saving_interval, output_dir)
 
-    def train(self, replay_buffer, num_train_steps: int, minibatch_size: int) -> None:
-        out = self._run(replay_buffer, num_train_steps, minibatch_size, noisy=True, delay=self.policy_delay)
+    def _record_train(self, out) -> None:
         mm, steps = getattr(self, "metrics_manager", None), getattr(self, "current_total_steps", 0)
         if mm is None or out is None:
             return
@@ -307,8 +340,10 @@ class DDPG(_OffPolicyBase):
         _learn(self, num_epochs, batch_size, minibatch_size, num_start_steps, num_steps_before_update, num_train_steps,
                num_evaluation_episodes, evaluation_interval, model_saving_interval, output_dir)
 
-    def train(self, replay_buffer, num_train_steps: int, minibatch_size: int) -> None:
-        out = self._run(replay_buffer, num_train_steps, minibatch_size, noisy=False, delay=1)
+    def _train_schedule(self):
+        return False, 1
+
+    def _record_train(self, out) -> None:
         mm, steps = getattr(self, "metrics_manager", None), getattr(self, "current_total_steps", 0)
         if mm is None or out is None:
             return
@@ -347,45 +382,63 @@ def _make_eval_env(env):
 
 def _learn(self, num_epochs, batch_size, minibatch_size, num_start_steps, num_steps_before_update, num_train_steps,
            num_evaluation_episodes, evaluation_interval, model_saving_interval, output_dir) -> None:
-    """Shared host loop of TD3.learn / DDPG.learn / SAC.learn (ref: td3.py:94-212, ddpg.py:85-193)."""
+    """Shared host loop of TD3.learn / DDPG.learn / SAC.learn (ref: td3.py:94-212, ddpg.py:85-193).  One epoch is three
+    phases (sample, train, evaluate and save), which LearnerGroup.learn runs in lockstep for its learners."""
+    started = _learn_begin(self, output_dir)
+    for epoch in range(1, num_epochs + 1):
+        if _learn_sample(self, epoch, batch_size, num_start_steps, num_steps_before_update):
+            self.train(self.replay_buffer, num_train_steps, minibatch_size)
+        _learn_evaluate_save(self, epoch, started, num_evaluation_episodes, evaluation_interval, model_saving_interval,
+                             output_dir)
+    self.metrics_manager.close()
+
+
+def _learn_begin(self, output_dir) -> float:
     started = time.time()
     self.current_total_steps = 0
     self.current_total_episodes = 0
     os.makedirs(output_dir, exist_ok=True)
     self.metrics_manager = MetricsManager(output_dir)
+    return started
+
+
+def _learn_sample(self, epoch, batch_size, num_start_steps, num_steps_before_update) -> bool:
+    """Sample, add to the replay buffer and log; returns whether this epoch trains."""
     mm = self.metrics_manager
-    for epoch in range(1, num_epochs + 1):
-        actor = self.exploration_policy if self.current_total_steps < num_start_steps else self.noised_policy
-        experience = self.sampler.sample(batch_size, actor)
-        self.replay_buffer.add_experience(experience)
-        returns, lengths = experience.episode_returns, experience.episode_lengths
-        self.current_total_steps += sum(lengths)
-        self.current_total_episodes += sum(experience.flattened_dones)
-        mm.record_scalar("epoch", epoch)
-        mm.record_scalar("total_steps", self.current_total_steps)
-        mm.record_scalar("total_episodes", self.current_total_episodes)
-        if len(lengths) > 0:
-            mm.record_scalar("sampling/average_episode_return", float(np.mean(returns)), self.current_total_steps,
-                             tensorboard=True)
-            mm.record_scalar("sampling/episode_return_std", float(np.std(returns)))
-            mm.record_scalar("sampling/max_episode_return", float(np.max(returns)))
-            mm.record_scalar("sampling/min_episode_return", float(np.min(returns)))
-            mm.record_scalar("sampling/average_episode_length", float(np.mean(lengths)), self.current_total_steps,
-                             tensorboard=True)
-        if self.current_total_steps >= num_steps_before_update:
-            self.train(self.replay_buffer, num_train_steps, minibatch_size)
-        if num_evaluation_episodes > 0 and self.current_total_steps % evaluation_interval == 0:
-            ev_policy = getattr(self, "evaluation_policy", self.policy)  # SAC: the deterministic view of its policy
-            ev_returns, ev_lengths = self.evaluator.evaluate(ev_policy, self.evaluation_env, num_evaluation_episodes)
-            mm.record_scalar("evaluation/average_episode_return", float(np.mean(ev_returns)), self.current_total_steps,
-                             tensorboard=True)
-            mm.record_scalar("evaluation/episode_return_std", float(np.std(ev_returns)))
-            mm.record_scalar("evaluation/max_episode_return", float(np.max(ev_returns)))
-            mm.record_scalar("evaluation/min_episode_return", float(np.min(ev_returns)))
-            mm.record_scalar("evaluation/average_episode_length", float(np.mean(ev_lengths)), self.current_total_steps,
-                             tensorboard=True)
-        if self.current_total_steps % model_saving_interval == 0:
-            self.save_model(epoch, os.path.join(output_dir, "model.pt"))
-        mm.record_scalar("time", time.time() - started)
-        mm.dump()
-    mm.close()
+    actor = self.exploration_policy if self.current_total_steps < num_start_steps else self.noised_policy
+    experience = self.sampler.sample(batch_size, actor)
+    self.replay_buffer.add_experience(experience)
+    returns, lengths = experience.episode_returns, experience.episode_lengths
+    self.current_total_steps += sum(lengths)
+    self.current_total_episodes += sum(experience.flattened_dones)
+    mm.record_scalar("epoch", epoch)
+    mm.record_scalar("total_steps", self.current_total_steps)
+    mm.record_scalar("total_episodes", self.current_total_episodes)
+    if len(lengths) > 0:
+        mm.record_scalar("sampling/average_episode_return", float(np.mean(returns)), self.current_total_steps,
+                         tensorboard=True)
+        mm.record_scalar("sampling/episode_return_std", float(np.std(returns)))
+        mm.record_scalar("sampling/max_episode_return", float(np.max(returns)))
+        mm.record_scalar("sampling/min_episode_return", float(np.min(returns)))
+        mm.record_scalar("sampling/average_episode_length", float(np.mean(lengths)), self.current_total_steps,
+                         tensorboard=True)
+    return self.current_total_steps >= num_steps_before_update
+
+
+def _learn_evaluate_save(self, epoch, started, num_evaluation_episodes, evaluation_interval, model_saving_interval,
+                         output_dir) -> None:
+    mm = self.metrics_manager
+    if num_evaluation_episodes > 0 and self.current_total_steps % evaluation_interval == 0:
+        ev_policy = getattr(self, "evaluation_policy", self.policy)  # SAC: the deterministic view of its policy
+        ev_returns, ev_lengths = self.evaluator.evaluate(ev_policy, self.evaluation_env, num_evaluation_episodes)
+        mm.record_scalar("evaluation/average_episode_return", float(np.mean(ev_returns)), self.current_total_steps,
+                         tensorboard=True)
+        mm.record_scalar("evaluation/episode_return_std", float(np.std(ev_returns)))
+        mm.record_scalar("evaluation/max_episode_return", float(np.max(ev_returns)))
+        mm.record_scalar("evaluation/min_episode_return", float(np.min(ev_returns)))
+        mm.record_scalar("evaluation/average_episode_length", float(np.mean(ev_lengths)), self.current_total_steps,
+                         tensorboard=True)
+    if self.current_total_steps % model_saving_interval == 0:
+        self.save_model(epoch, os.path.join(output_dir, "model.pt"))
+    mm.record_scalar("time", time.time() - started)
+    mm.dump()

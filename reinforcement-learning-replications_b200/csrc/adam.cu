@@ -82,7 +82,19 @@ struct AdamArgs {
   int table_idx;        // arguments stay fixed while the host refreshes the table before each launch)
 };
 
-__global__ void __launch_bounds__(256) adam_step_kernel(const AdamArgs a) {
+// LANES (the off-policy engine's learner groups): learner blockIdx.z works on params / grad / m / v / table shifted by
+// blockIdx.z * lane_stride bytes (one arena per learner, see offpolicy.cu); the arithmetic is the same for every learner.
+template <bool LANES>
+__global__ void __launch_bounds__(256) adam_step_kernel(const AdamArgs args, size_t lane_stride) {
+  AdamArgs a = args;
+  if (LANES) {
+    const size_t off = blockIdx.z * lane_stride;
+    a.params = reinterpret_cast<float*>(reinterpret_cast<char*>(a.params) + off);
+    a.grad = reinterpret_cast<const float*>(reinterpret_cast<const char*>(a.grad) + off);
+    a.m = reinterpret_cast<float*>(reinterpret_cast<char*>(a.m) + off);
+    a.v = reinterpret_cast<float*>(reinterpret_cast<char*>(a.v) + off);
+    a.table = reinterpret_cast<const float2*>(reinterpret_cast<const char*>(a.table) + off);
+  }
   // early stop (ppo.py:176-181): the KL carried by this step's forward pass is the KL of the PREVIOUS update
   bool stop = false;
   if (a.stop_flag != nullptr) {
@@ -103,7 +115,11 @@ __global__ void __launch_bounds__(256) adam_step_kernel(const AdamArgs a) {
     const float g = a.grad[i];
     float m = a.m[i], v = a.v[i];
     m = m + a.one_minus_b1 * (g - m);                     // exp_avg.lerp_(grad, 1 - beta1)
-    v = v * a.b2 + a.one_minus_b2 * (g * g);              // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2)
+    // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2).  The compiler fuses a different product of this sum in
+    // the LANES instantiation, so there the solo kernel's rounding is spelled out: a learner in a group must round
+    // exactly as a solo learner does.
+    if (LANES) v = __fmaf_rn(v, a.b2, __fmul_rn(__fmul_rn(g, g), a.one_minus_b2));
+    else v = v * a.b2 + a.one_minus_b2 * (g * g);
     const float denom = sqrtf(v) / bc2_sqrt + a.eps;      // (exp_avg_sq.sqrt() / bias_correction2_sqrt).add_(eps)
     a.m[i] = m;
     a.v[i] = v;
@@ -169,7 +185,7 @@ extern "C" int b200rl_adam_step(float* params, const float* grad, float* exp_avg
   a.table = nullptr;
   a.table_idx = 0;
   const int blocks = (int)((n_params + 255) / 256);
-  adam_step_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
+  adam_step_kernel<false><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(a, 0);
   B200RL_CUDA(cudaGetLastError());
   count_launch(1);
   return 0;
@@ -181,9 +197,10 @@ void adam_scalars(int64_t step, double lr, double beta1, double beta2, float* st
   *step_size = (float)(lr / (1.0 - pow(beta1, (double)step)));
   *bc2_sqrt = (float)sqrt(1.0 - pow(beta2, (double)step));
 }
-// Adam step whose two step-dependent scalars come from table[idx] in device memory (off-policy engine, graph replay)
+// Adam step whose two step-dependent scalars come from table[idx] in device memory (off-policy engine, graph replay);
+// lanes > 1: one launch for `lanes` learners whose buffers (table included) lie lane_stride bytes apart
 int adam_step_table(float* params, const float* grad, float* m, float* v, int64_t n, const float2* table, int idx,
-                    double beta1, double beta2, double eps, cudaStream_t s) {
+                    double beta1, double beta2, double eps, cudaStream_t s, int lanes, size_t lane_stride) {
   AdamArgs a{};
   a.params = params;
   a.grad = grad;
@@ -196,7 +213,8 @@ int adam_step_table(float* params, const float* grad, float* m, float* v, int64_
   a.eps = (float)eps;
   a.table = table;
   a.table_idx = idx;
-  adam_step_kernel<<<(int)((n + 255) / 256), 256, 0, s>>>(a);
+  if (lanes == 1) adam_step_kernel<false><<<(int)((n + 255) / 256), 256, 0, s>>>(a, 0);
+  else adam_step_kernel<true><<<dim3((unsigned)((n + 255) / 256), 1, (unsigned)lanes), 256, 0, s>>>(a, lane_stride);
   B200RL_CUDA(cudaGetLastError());
   count_launch(1);
   return 0;

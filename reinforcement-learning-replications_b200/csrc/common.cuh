@@ -50,7 +50,7 @@ int64_t launches_total();
 // Adam helpers shared with the off-policy engine (adam.cu)
 void adam_scalars(int64_t step, double lr, double beta1, double beta2, float* step_size, float* bc2_sqrt);
 int adam_step_table(float* params, const float* grad, float* m, float* v, int64_t n, const float2* table, int idx,
-                    double beta1, double beta2, double eps, cudaStream_t s);
+                    double beta1, double beta2, double eps, cudaStream_t s, int lanes = 1, size_t lane_stride = 0);
 
 // TRPO vector kernels (trpo.cu)
 int trpo_cg_init(const float* g, float* x, float* r, float* pv, int n, double* sc, int* flags, cudaStream_t s);

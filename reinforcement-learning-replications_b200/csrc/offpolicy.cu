@@ -14,6 +14,8 @@
 // the opt-in persistent step kernel (offpolicy_mega_kernel) and its program builder; the engine (one state slab);
 // enqueue_steps = the S steps as a four-stream dependency graph (captured once, replayed); the three entry points
 // train (host-staged minibatches), train_gather (host-drawn indices, device gather), train_gather_rng (device draws).
+// Learner groups (create_group): K learners in K arenas at a fixed stride, every kernel above with a LANES
+// instantiation that serves all of them in one launch; a K = 1 engine runs the solo instantiations.
 // SAC (config algo = 1) is a second step program on the same engine: its head / soft-loss / temperature kernels and
 // enqueue_sac_steps, run as a captured graph or as plain launches (the persistent step kernel does not apply to it).
 #include <cmath>
@@ -166,10 +168,33 @@ __device__ __forceinline__ void gemm_tile(const GemmArgs& g, int bx, int by, Gem
   }
 }
 
-template <int MODE>
-__global__ void __launch_bounds__(GTHREADS) gemm_kernel(const GemmArgs g) {
+// Learner groups (b200rl_offpolicy_create_group): everything the engine owns for one learner lives in one arena, and
+// the K arenas lie lane_stride bytes apart, so learner z's copy of any engine buffer is ptr + z * lane_stride.  Every
+// kernel below has a LANES instantiation that serves all K learners in one launch (learner = blockIdx.z) with the
+// arithmetic of the solo kernel; a K = 1 engine launches the LANES = false instantiation, which is the solo kernel.
+template <typename T>
+__device__ __forceinline__ T* lane_ptr(T* p, size_t off) {  // NULL stays NULL (optional operands)
+  return p == nullptr ? p : reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(p) + off);
+}
+
+template <int MODE, bool LANES>
+__global__ void __launch_bounds__(GTHREADS) gemm_kernel(const GemmArgs g, size_t lane_stride) {
   __shared__ GemmTile As, Bs;
-  gemm_tile<MODE, 8>(g, blockIdx.x, blockIdx.y, As, Bs);  // K = 256 is ONE round of loads
+  if (LANES) {
+    const size_t off = blockIdx.z * lane_stride;
+    GemmArgs a = g;
+    a.A = lane_ptr(a.A, off);
+    a.B = lane_ptr(a.B, off);
+    a.C = lane_ptr(a.C, off);
+    a.bias = lane_ptr(a.bias, off);
+    a.Y = lane_ptr(a.Y, off);
+    a.dbias = lane_ptr(a.dbias, off);
+    a.A2 = lane_ptr(a.A2, off);
+    a.eps = lane_ptr(a.eps, off);
+    gemm_tile<MODE, 8>(a, blockIdx.x, blockIdx.y, As, Bs);
+  } else {
+    gemm_tile<MODE, 8>(g, blockIdx.x, blockIdx.y, As, Bs);  // K = 256 is ONE round of loads
+  }
 }
 
 // ---- device-side draws (opt-in; SURVEY 8f-4): Philox4x32-10, counter-based, so a (seed, call) pair names the whole
@@ -185,11 +210,27 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
   return c;
 }
 
+// (seed, call, ring) of every learner of a launch: one entry for the solo kernel, one per learner for LANES
+template <bool LANES>
+struct DrawKeys {
+  static constexpr int N = LANES ? B200RL_MAX_LEARNERS : 1;
+  unsigned long long seed[N], call[N];
+  long long start[N], size[N], capacity[N];
+};
+
 // idx[j] = physical row of a uniform draw over the `size` live rows of the ring (logical row u sits at
 // (start + u) % capacity);  eps[j] = N(0, 1) by Box-Muller.  One thread = one Philox block = 4 values of each.
+// A learner's draws depend on its (seed, call) only: in a group they equal those of a solo engine with that key.
+template <bool LANES>
 __global__ void draw_minibatches_kernel(long long* idx, long long n_idx, float* eps, long long n_eps,
-                                        unsigned long long seed, unsigned long long call, long long start,
-                                        long long size, long long capacity) {
+                                        const DrawKeys<LANES> keys, size_t lane_stride) {
+  const int z = LANES ? blockIdx.z : 0;
+  if (LANES) {
+    idx = lane_ptr(idx, blockIdx.z * lane_stride);
+    eps = lane_ptr(eps, blockIdx.z * lane_stride);
+  }
+  const unsigned long long seed = keys.seed[z], call = keys.call[z];
+  const long long start = keys.start[z], size = keys.size[z], capacity = keys.capacity[z];
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const uint2 key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
   if (4 * t < n_idx) {
@@ -217,8 +258,21 @@ __global__ void draw_minibatches_kernel(long long* idx, long long n_idx, float* 
   }
 }
 
+// one replay column of every learner of a launch (each learner has its own replay buffer)
+template <bool LANES>
+struct LaneSrc {
+  const float* p[LANES ? B200RL_MAX_LEARNERS : 1];
+};
+
 // staged[i, :] = table[idx[i], :]  (replay-buffer gather; one launch per column)
-__global__ void gather_rows_kernel(const float* table, const long long* idx, int width, long long n_out, float* out) {
+template <bool LANES>
+__global__ void gather_rows_kernel(const LaneSrc<LANES> src, const long long* idx, int width, long long n_out, float* out,
+                                   size_t lane_stride) {
+  const float* table = src.p[LANES ? blockIdx.z : 0];
+  if (LANES) {
+    idx = lane_ptr(idx, blockIdx.z * lane_stride);
+    out = lane_ptr(out, blockIdx.z * lane_stride);
+  }
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_out * width) return;
   const long long r = i / width;
@@ -234,10 +288,16 @@ __device__ __forceinline__ float td_target(float rew, float done, float q1t, con
 // One CTA: the critic's loss with its TD target computed on the fly: y as above, loss = mean((q - y)^2),
 // dq = 2 (q - y) / B (F.mse_loss + backward), q_copy = q (the logged Q-values);  rew == NULL: the policy loss
 // -mean(q), dq = -1/B
+template <bool LANES>
 __global__ void __launch_bounds__(GTHREADS) q_loss_kernel(const float* q, const float* rew, const float* done,
                                                          const float* q1t, const float* q2t, float gamma, int n,
-                                                         float* dq, float* loss_out, float* q_copy) {
+                                                         float* dq, float* loss_out, float* q_copy, size_t lane_stride) {
   __shared__ double red[32];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q = lane_ptr(q, o), rew = lane_ptr(rew, o), done = lane_ptr(done, o), q1t = lane_ptr(q1t, o);
+    q2t = lane_ptr(q2t, o), dq = lane_ptr(dq, o), loss_out = lane_ptr(loss_out, o), q_copy = lane_ptr(q_copy, o);
+  }
   double acc = 0.0;
   const float inv = 1.0f / (float)n;
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
@@ -262,17 +322,28 @@ __global__ void __launch_bounds__(GTHREADS) q_loss_kernel(const float* q, const 
   }
 }
 
-// target <- rho * target + (1 - rho) * param   (utils.py:47-57: f32 tensors tensor(rho), tensor(1 - rho))
+// target <- rho * target + (1 - rho) * param   (utils.py:47-57: f32 tensors tensor(rho), tensor(1 - rho)); the LANES
+// instantiation spells out the product the solo kernel fuses (left to the compiler, it fuses the other one)
 struct PolyakArgs {
   float* target[3];
   const float* param[3];
   int n[3];
   int n_nets;
 };
-__global__ void polyak_kernel(const PolyakArgs a, float rho, float one_minus_rho) {  // every network in one launch
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  for (int k = 0; k < a.n_nets; ++k)
-    if (i < a.n[k]) a.target[k][i] = rho * a.target[k][i] + one_minus_rho * a.param[k][i];
+template <bool LANES>
+__global__ void polyak_kernel(const PolyakArgs a, float rho, float one_minus_rho, size_t lane_stride) {  // every network
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;                                                   // in one launch
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    for (int k = 0; k < a.n_nets; ++k) {
+      float* t = lane_ptr(a.target[k], o);
+      const float* p = lane_ptr(a.param[k], o);
+      if (i < a.n[k]) t[i] = __fmaf_rn(t[i], rho, __fmul_rn(p[i], one_minus_rho));
+    }
+  } else {
+    for (int k = 0; k < a.n_nets; ++k)
+      if (i < a.n[k]) a.target[k][i] = rho * a.target[k][i] + one_minus_rho * a.param[k][i];
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -431,8 +502,13 @@ __device__ __forceinline__ float softplus_f(float x) { return x > 20.f ? x : log
 
 // One thread per row: u = mu + exp(clamp(log_std)) * eps, act = limit * tanh(u),
 // logp = sum_j Normal(mu, sigma).log_prob(u)_j - sum_j 2 (log 2 - u_j - softplus(-2 u_j))
+template <bool LANES>
 __global__ void sac_squash_kernel(const float* out, const float* eps, int B, int A, float lmin, float lmax, float limit,
-                                  float* act, float* logp) {
+                                  float* act, float* logp, size_t lane_stride) {
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    out = lane_ptr(out, o), eps = lane_ptr(eps, o), act = lane_ptr(act, o), logp = lane_ptr(logp, o);
+  }
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= B) return;
   float lp = 0.f, corr = 0.f;
@@ -451,11 +527,18 @@ __global__ void sac_squash_kernel(const float* out, const float* eps, int B, int
 
 // One CTA per critic: y = r + gamma (1 - d) (min(Q1targ, Q2targ)(s', a') - alpha log pi(a' | s')), loss = mean((q - y)^2),
 // dq = 2 (q - y) / B, q_copy = q (the logged Q-values)
+template <bool LANES>
 __global__ void __launch_bounds__(GTHREADS) sac_q_loss_kernel(const float* q, const float* rew, const float* done,
                                                              const float* q1t, const float* q2t, const float* logp_next,
                                                              const float* alpha, float gamma, int n, float* dq,
-                                                             float* loss_out, float* q_copy) {
+                                                             float* loss_out, float* q_copy, size_t lane_stride) {
   __shared__ double red[32];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q = lane_ptr(q, o), rew = lane_ptr(rew, o), done = lane_ptr(done, o), q1t = lane_ptr(q1t, o), q2t = lane_ptr(q2t, o);
+    logp_next = lane_ptr(logp_next, o), alpha = lane_ptr(alpha, o), dq = lane_ptr(dq, o);
+    loss_out = lane_ptr(loss_out, o), q_copy = lane_ptr(q_copy, o);
+  }
   const float a = *alpha;
   const float inv = 1.0f / (float)n;
   double acc = 0.0;
@@ -472,10 +555,18 @@ __global__ void __launch_bounds__(GTHREADS) sac_q_loss_kernel(const float* q, co
 
 // One CTA: loss = mean(alpha log pi - min(q1, q2)) at a = pi(s), the per-row gradients w.r.t. q1 and q2 (torch.min's
 // rule: equal values share the gradient half and half), and mean(log pi)
+template <bool LANES>
 __global__ void __launch_bounds__(GTHREADS) sac_policy_loss_kernel(const float* q1, const float* q2, const float* logp,
                                                                   const float* alpha, int n, float* dq1, float* dq2,
-                                                                  float* loss_out, float* logp_mean_out) {
+                                                                  float* loss_out, float* logp_mean_out,
+                                                                  size_t lane_stride) {
   __shared__ double red[32], red_lp[32];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q1 = lane_ptr(q1, o), q2 = lane_ptr(q2, o), logp = lane_ptr(logp, o), alpha = lane_ptr(alpha, o);
+    dq1 = lane_ptr(dq1, o), dq2 = lane_ptr(dq2, o), loss_out = lane_ptr(loss_out, o);
+    logp_mean_out = lane_ptr(logp_mean_out, o);
+  }
   const float a = *alpha;
   const float inv = 1.0f / (float)n;
   double acc = 0.0, acc_lp = 0.0;
@@ -496,9 +587,15 @@ __global__ void __launch_bounds__(GTHREADS) sac_policy_loss_kernel(const float* 
 // u and sigma are recomputed from the output and eps exactly as sac_squash_kernel computed them.  With t = tanh(u) and
 // c = alpha / B:  g_u = dA limit (1 - t^2) + 2 c t,  d mu = g_u,  d log_std = g_u sigma eps - c inside the clamp, else 0
 // (the Gaussian term's u - mu = sigma eps cancels from d mu and leaves -1 in d log_std).
+template <bool LANES>
 __global__ void sac_squash_backward_kernel(const float* out, const float* eps, const float* dx1, const float* dx2, int ldx,
                                            int B, int A, float lmin, float lmax, float limit, const float* alpha,
-                                           float* dout) {
+                                           float* dout, size_t lane_stride) {
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    out = lane_ptr(out, o), eps = lane_ptr(eps, o), dx1 = lane_ptr(dx1, o), dx2 = lane_ptr(dx2, o);
+    alpha = lane_ptr(alpha, o), dout = lane_ptr(dout, o);
+  }
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * A) return;
   const int r = i / A, j = i - r * A;
@@ -515,7 +612,10 @@ __global__ void sac_squash_backward_kernel(const float* out, const float* eps, c
 }
 
 // alpha[0..n) = the fixed alpha (learn == 0), or alpha[0] = exp(log_alpha) (learn == 1: the alpha steps fill the rest)
-__global__ void sac_alpha_init_kernel(float* alpha, int n, const float* log_alpha, int learn, float fixed) {
+template <bool LANES>
+__global__ void sac_alpha_init_kernel(float* alpha, int n, const float* log_alpha, int learn, float fixed,
+                                      size_t lane_stride) {
+  if (LANES) alpha = lane_ptr(alpha, blockIdx.z * lane_stride), log_alpha = lane_ptr(log_alpha, blockIdx.z * lane_stride);
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (learn) {
     if (i == 0) alpha[0] = expf(*log_alpha);
@@ -527,11 +627,17 @@ __global__ void sac_alpha_init_kernel(float* alpha, int n, const float* log_alph
 // One CTA: the temperature step.  grad = -mean(log pi + target_entropy) (a fixed-order reduction), then torch.optim.Adam
 // on the scalar log_alpha (state = {log_alpha, exp_avg, exp_avg_sq}) with the scalars of table[idx]; alpha_next =
 // exp(log_alpha), the alpha of the next step
+template <bool LANES>
 __global__ void __launch_bounds__(GTHREADS) sac_alpha_step_kernel(const float* logp, int n, float target_entropy,
                                                                  float* state, const float2* table, int idx,
                                                                  float one_minus_b1, float b2, float one_minus_b2,
-                                                                 float eps, float* alpha_next) {
+                                                                 float eps, float* alpha_next, size_t lane_stride) {
   __shared__ double red[32];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    logp = lane_ptr(logp, o), state = lane_ptr(state, o), table = lane_ptr(table, o);
+    alpha_next = lane_ptr(alpha_next, o);
+  }
   double acc = 0.0;
   for (int i = threadIdx.x; i < n; i += blockDim.x) acc += (double)(logp[i] + target_entropy);
   acc = warp_sum(acc);
@@ -543,8 +649,9 @@ __global__ void __launch_bounds__(GTHREADS) sac_alpha_step_kernel(const float* l
     const float g = -(float)(tot / (double)n);
     const float2 t = table[idx];
     float p = state[0], m = state[1], v = state[2];
-    m = m + one_minus_b1 * (g - m);  // the arithmetic of adam_step_kernel (adam.cu)
-    v = v * b2 + one_minus_b2 * (g * g);
+    m = m + one_minus_b1 * (g - m);  // the arithmetic of adam_step_kernel (adam.cu); LANES: the solo kernel's rounding
+    if (LANES) v = __fmaf_rn(__fmul_rn(g, g), one_minus_b2, __fmul_rn(v, b2));
+    else v = v * b2 + one_minus_b2 * (g * g);
     const float denom = sqrtf(v) / t.y + eps;
     p = p - t.x * (m / denom);
     state[0] = p;
@@ -566,12 +673,18 @@ struct NetBuf {
   float *m = nullptr, *v = nullptr;  // Adam state (trainable nets only)
   float* grad = nullptr;
   bool present = false;
-  int64_t step = 0;
+  int64_t step[B200RL_MAX_LEARNERS] = {};  // Adam step count of each learner
   int w_off[B200RL_MAX_LAYERS], b_off[B200RL_MAX_LAYERS];
 };
 
 struct b200rl_offpolicy {
   b200rl_offpolicy_config cfg;
+  // learners of the group (1 = a solo engine) and the byte distance between their arenas: every pointer below is
+  // learner 0's copy, learner z's is at + z * lane_stride (see lane_ptr)
+  int K = 1;
+  size_t lane_stride = 0;
+  std::vector<std::pair<void**, size_t>> pieces;  // (pointer to set, offset in the arena) of every engine buffer
+  size_t arena_bytes = 0;
   NetBuf net[6];  // 0 pi, 1 Q1, 2 Q2, 3 pi_targ, 4 Q1_targ, 5 Q2_targ
   int O = 0, A = 0, maxw = 0;
   // staged minibatches [S,B,*]
@@ -594,7 +707,7 @@ struct b200rl_offpolicy {
   // (minibatch contents, Adam bias-correction scalars) lives in device buffers refreshed before each launch
   long long* idx = nullptr;      // [max_steps * max_minibatch] replay rows of train_gather
   float2* adam_tab = nullptr;    // [3][max_steps] {lr / (1 - beta1^t), sqrt(1 - beta2^t)} for policy, Q1, Q2
-  float2* h_adam_tab = nullptr;  // pinned mirror
+  float2* h_adam_tab = nullptr;  // pinned mirror, [K][table]
   cudaStream_t gs = nullptr;     // internal stream (the caller's may be the legacy default stream: not capturable)
   cudaEvent_t ev = nullptr;
   cudaGraphExec_t graph = nullptr;
@@ -618,7 +731,7 @@ struct b200rl_offpolicy {
   float* sac_alpha = nullptr;                               // [max_steps + 1] alpha of step st at [st]
   float* sac_state = nullptr;                               // {log_alpha, exp_avg, exp_avg_sq}
   float* out_logp = nullptr;                                // [max_steps] mean log pi of each policy step
-  int64_t alpha_step = 0;
+  int64_t alpha_step[B200RL_MAX_LEARNERS] = {};
   std::vector<void*> allocs;
 };
 
@@ -626,20 +739,44 @@ namespace {
 
 inline int64_t state_pad(int64_t n) { return (n + 63) & ~(int64_t)63; }
 
+// A piece of the learner arena: recorded here (256-byte aligned), placed by arena_commit
 template <typename T>
 int oalloc(b200rl_offpolicy* h, T** p, size_t count) {
-  void* q = nullptr;
-  B200RL_CUDA(cudaMalloc(&q, (count ? count : 1) * sizeof(T)));
-  B200RL_CUDA(cudaMemset(q, 0, (count ? count : 1) * sizeof(T)));
-  h->allocs.push_back(q);
-  *p = static_cast<T*>(q);
+  h->pieces.emplace_back(reinterpret_cast<void**>(p), h->arena_bytes);
+  h->arena_bytes += ((count ? count : 1) * sizeof(T) + 255) & ~(size_t)255;
   return 0;
 }
 
+// ONE zeroed allocation of K arenas at a fixed stride (a multiple of 256 bytes); every recorded buffer points into
+// learner 0's arena
+int arena_commit(b200rl_offpolicy* h) {
+  h->lane_stride = h->arena_bytes;
+  void* q = nullptr;
+  B200RL_CUDA(cudaMalloc(&q, (size_t)h->K * h->lane_stride));
+  h->allocs.push_back(q);
+  B200RL_CUDA(cudaMemset(q, 0, (size_t)h->K * h->lane_stride));
+  for (const auto& pc : h->pieces) *pc.first = static_cast<char*>(q) + pc.second;
+  h->pieces.clear();
+  return 0;
+}
+
+inline dim3 lane_grid(dim3 g, int K) {
+  g.z = (unsigned)K;
+  return g;
+}
+
+// one launch for every learner: a solo engine runs kern<false> (the solo kernel), a group kern<true> over blockIdx.z
+#define LAUNCH_LANES(h, kern, grid, block, s, ...)                                                 \
+  do {                                                                                             \
+    if ((h)->K == 1) kern<false><<<(grid), (block), 0, (s)>>>(__VA_ARGS__, (size_t)0);             \
+    else kern<true><<<lane_grid((grid), (h)->K), (block), 0, (s)>>>(__VA_ARGS__, (h)->lane_stride); \
+  } while (0)
+
 template <int MODE>
-int gemm(const GemmArgs& g, cudaStream_t s) {
+int gemm(const b200rl_offpolicy* h, const GemmArgs& g, cudaStream_t s) {
   dim3 grid((g.N + GT - 1) / GT, (g.M + GT - 1) / GT);
-  gemm_kernel<MODE><<<grid, GTHREADS, 0, s>>>(g);
+  if (h->K == 1) gemm_kernel<MODE, false><<<grid, GTHREADS, 0, s>>>(g, 0);
+  else gemm_kernel<MODE, true><<<lane_grid(grid, h->K), GTHREADS, 0, s>>>(g, h->lane_stride);
   B200RL_CUDA(cudaGetLastError());
   count_launch(1);
   return 0;
@@ -648,8 +785,9 @@ int gemm(const GemmArgs& g, cudaStream_t s) {
 // forward through one network: acts[0] = input [rows, n0] (ld = n0); acts[l+1] = layer outputs.
 // in_b != NULL: the input is torch.cat([acts[0] (ksplit columns), in_b (ld_b)], -1), read in place by the first layer
 // (q_function.py:30); eps != NULL: target-policy smoothing on the output (td3.py:326-332)
-int net_forward(const NetBuf& nb, float* const* acts, int rows, cudaStream_t s, const float* in_b = nullptr, int ld_b = 0,
-                int ksplit = 0, const float* eps = nullptr, const b200rl_offpolicy_hparams* hp = nullptr) {
+int net_forward(const b200rl_offpolicy* h, const NetBuf& nb, float* const* acts, int rows, cudaStream_t s,
+                const float* in_b = nullptr, int ld_b = 0, int ksplit = 0, const float* eps = nullptr,
+                const b200rl_offpolicy_hparams* hp = nullptr) {
   const int L = nb.d.n_layers;
   for (int l = 0; l < L; ++l) {
     GemmArgs g{};
@@ -669,7 +807,7 @@ int net_forward(const NetBuf& nb, float* const* acts, int rows, cudaStream_t s, 
     g.bias = nb.params + nb.b_off[l];
     g.act = (l == L - 1) ? nb.d.out_act : nb.d.hidden_act;
     g.M = rows; g.N = nb.d.sizes[l + 1]; g.K = nb.d.sizes[l];
-    if (gemm<0>(g, s)) return 1;
+    if (gemm<0>(h, g, s)) return 1;
   }
   return 0;
 }
@@ -706,7 +844,7 @@ int net_backward(b200rl_offpolicy* h, const NetBuf& nb, float* const* acts, cons
         B200RL_CUDA(cudaEventRecord(h->ev_side, s));
         B200RL_CUDA(cudaStreamWaitEvent(s_dw, h->ev_side, 0));
       }
-      if (gemm<2>(g, side ? s_dw : s)) return 1;
+      if (gemm<2>(h, g, side ? s_dw : s)) return 1;
     }
     if (l > 0 || dx_out) {
       float* dst = (l == 0) ? dx_out : pp[l & 1];
@@ -715,7 +853,7 @@ int net_backward(b200rl_offpolicy* h, const NetBuf& nb, float* const* acts, cons
       g.B = nb.params + nb.w_off[l]; g.ldb = nin;
       g.C = dst; g.ldc = nin;
       g.M = rows; g.N = nin; g.K = nout;
-      if (gemm<1>(g, s)) return 1;
+      if (gemm<1>(h, g, s)) return 1;
       dY = dst;
       ldd = nin;
     }
@@ -727,14 +865,22 @@ int net_backward(b200rl_offpolicy* h, const NetBuf& nb, float* const* acts, cons
   return 0;
 }
 
-int adam_net(NetBuf& nb, const float2* table, int idx, double b1, double b2, double eps, cudaStream_t s) {
-  return adam_step_table(nb.params, nb.grad, nb.m, nb.v, nb.P, table, idx, b1, b2, eps, s);
+int adam_net(const b200rl_offpolicy* h, NetBuf& nb, const float2* table, int idx, double b1, double b2, double eps,
+             cudaStream_t s) {
+  return adam_step_table(nb.params, nb.grad, nb.m, nb.v, nb.P, table, idx, b1, b2, eps, s, h->K, h->lane_stride);
 }
 
 }  // namespace
 
 extern "C" int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200rl_offpolicy** out) {
+  return b200rl_offpolicy_create_group(cfg, 1, out);
+}
+
+extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg, int32_t n_learners,
+                                             b200rl_offpolicy** out) {
   B200RL_REQUIRE(cfg && out, "offpolicy_create: NULL argument");
+  B200RL_REQUIRE(n_learners >= 1 && n_learners <= B200RL_MAX_LEARNERS,
+                 "offpolicy_create_group: n_learners must be 1..%d, got %d", B200RL_MAX_LEARNERS, n_learners);
   B200RL_REQUIRE(cfg->n_q == 1 || cfg->n_q == 2, "offpolicy_create: n_q must be 1 (DDPG) or 2 (TD3)");
   B200RL_REQUIRE(cfg->algo == 0 || cfg->algo == 1, "offpolicy_create: algo must be 0 (DDPG / TD3) or 1 (SAC), got %d",
                  cfg->algo);
@@ -753,6 +899,7 @@ extern "C" int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200r
   B200RL_REQUIRE(device_sm_count() > 0, "offpolicy_create: no CUDA device");
   b200rl_offpolicy* h = new b200rl_offpolicy();
   h->cfg = *cfg;
+  h->K = n_learners;
   h->O = O;
   h->A = A;
   h->sac = sac;
@@ -785,21 +932,6 @@ extern "C" int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200r
       if (h->net[i].present) n += 2 * state_pad(h->net[i].P);
     h->state_n = n;
     rc |= oalloc(h, &h->state, (size_t)n);
-    if (rc == 0) {
-      float* q = h->state;
-      for (int i = 0; i < 6; ++i)
-        if (h->net[i].present) {
-          h->net[i].params = q;
-          q += state_pad(h->net[i].P);
-        }
-      for (int i = 0; i < 3; ++i)
-        if (h->net[i].present) {
-          h->net[i].m = q;
-          q += state_pad(h->net[i].P);
-          h->net[i].v = q;
-          q += state_pad(h->net[i].P);
-        }
-    }
   }
   h->maxw = maxw;
   const size_t B = (size_t)cfg->max_minibatch, S = (size_t)cfg->max_steps;
@@ -842,7 +974,24 @@ extern "C" int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200r
     rc |= oalloc(h, &h->sac_state, 3);
     rc |= oalloc(h, &h->out_logp, S);
   }
-  if (!rc && cudaMallocHost(reinterpret_cast<void**>(&h->h_adam_tab), n_tab * S * sizeof(float2)) != cudaSuccess) rc = 1;
+  rc |= arena_commit(h);
+  if (rc == 0) {
+    float* q = h->state;
+    for (int i = 0; i < 6; ++i)
+      if (h->net[i].present) {
+        h->net[i].params = q;
+        q += state_pad(h->net[i].P);
+      }
+    for (int i = 0; i < 3; ++i)
+      if (h->net[i].present) {
+        h->net[i].m = q;
+        q += state_pad(h->net[i].P);
+        h->net[i].v = q;
+        q += state_pad(h->net[i].P);
+      }
+  }
+  if (!rc && cudaMallocHost(reinterpret_cast<void**>(&h->h_adam_tab), h->K * n_tab * S * sizeof(float2)) != cudaSuccess)
+    rc = 1;
   if (!rc && cudaStreamCreateWithFlags(&h->gs, cudaStreamNonBlocking) != cudaSuccess) rc = 1;
   if (!rc && cudaEventCreateWithFlags(&h->ev, cudaEventDisableTiming) != cudaSuccess) rc = 1;
   if (!rc && cudaStreamCreateWithFlags(&h->s2, cudaStreamNonBlocking) != cudaSuccess) rc = 1;
@@ -878,6 +1027,7 @@ extern "C" void b200rl_offpolicy_destroy(b200rl_offpolicy* h) {
 
 extern "C" int b200rl_offpolicy_set_params(b200rl_offpolicy* h, int which, const float* host_flat, int64_t n,
                                            void* stream) {
+  B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_set_params: a learner group moves its state with get_state / set_state");
   B200RL_REQUIRE(h && host_flat && which >= 0 && which < 6 && h->net[which].params, "offpolicy_set_params: bad net");
   B200RL_REQUIRE(n == h->net[which].P, "offpolicy_set_params: expects %lld floats", (long long)h->net[which].P);
   B200RL_CUDA(cudaMemcpyAsync(h->net[which].params, host_flat, (size_t)n * 4, cudaMemcpyHostToDevice,
@@ -886,6 +1036,7 @@ extern "C" int b200rl_offpolicy_set_params(b200rl_offpolicy* h, int which, const
 }
 
 extern "C" int b200rl_offpolicy_get_params(b200rl_offpolicy* h, int which, float* host_flat, int64_t n, void* stream) {
+  B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_get_params: a learner group moves its state with get_state / set_state");
   B200RL_REQUIRE(h && host_flat && which >= 0 && which < 6 && h->net[which].params, "offpolicy_get_params: bad net");
   B200RL_REQUIRE(n == h->net[which].P, "offpolicy_get_params: expects %lld floats", (long long)h->net[which].P);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -896,6 +1047,7 @@ extern "C" int b200rl_offpolicy_get_params(b200rl_offpolicy* h, int which, float
 
 extern "C" int b200rl_offpolicy_set_adam(b200rl_offpolicy* h, int which, const float* exp_avg, const float* exp_avg_sq,
                                          int64_t n, int64_t step, void* stream) {
+  B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_set_adam: a learner group moves its state with get_state / set_state");
   B200RL_REQUIRE(h && which >= 0 && which < 3 && h->net[which].m, "offpolicy_set_adam: bad net");
   NetBuf& nb = h->net[which];
   B200RL_REQUIRE(n == nb.P && step >= 0, "offpolicy_set_adam: expects %lld floats", (long long)nb.P);
@@ -904,12 +1056,13 @@ extern "C" int b200rl_offpolicy_set_adam(b200rl_offpolicy* h, int which, const f
   else B200RL_CUDA(cudaMemsetAsync(nb.m, 0, (size_t)n * 4, s));
   if (exp_avg_sq) B200RL_CUDA(cudaMemcpyAsync(nb.v, exp_avg_sq, (size_t)n * 4, cudaMemcpyHostToDevice, s));
   else B200RL_CUDA(cudaMemsetAsync(nb.v, 0, (size_t)n * 4, s));
-  nb.step = step;
+  nb.step[0] = step;
   return 0;
 }
 
 extern "C" int b200rl_offpolicy_get_adam(b200rl_offpolicy* h, int which, float* exp_avg, float* exp_avg_sq, int64_t n,
                                          int64_t* step, void* stream) {
+  B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_get_adam: a learner group moves its state with get_state / set_state");
   B200RL_REQUIRE(h && which >= 0 && which < 3 && h->net[which].m && exp_avg && exp_avg_sq && step,
                  "offpolicy_get_adam: bad arguments");
   NetBuf& nb = h->net[which];
@@ -918,13 +1071,14 @@ extern "C" int b200rl_offpolicy_get_adam(b200rl_offpolicy* h, int which, float* 
   B200RL_CUDA(cudaMemcpyAsync(exp_avg, nb.m, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaMemcpyAsync(exp_avg_sq, nb.v, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaStreamSynchronize(s));
-  *step = nb.step;
+  *step = nb.step[0];
   return 0;
 }
 
 // Whole learner state in ONE call and ONE synchronisation: blob = for every present network 0..5 its parameters, then
-// for every optimizer 0..2 (policy, Q1, Q2) exp_avg and exp_avg_sq; steps[3] = Adam step counts.
-static int64_t state_floats(const b200rl_offpolicy* h) { return h->state_n; }
+// for every optimizer 0..2 (policy, Q1, Q2) exp_avg and exp_avg_sq; steps[3] = Adam step counts.  A group moves
+// [K][blob] and steps[K][3] with one strided copy (the slab heads every learner's arena).
+static int64_t state_floats(const b200rl_offpolicy* h) { return h->K * h->state_n; }
 
 extern "C" int64_t b200rl_offpolicy_state_floats(b200rl_offpolicy* h) { return h ? state_floats(h) : -1; }
 
@@ -933,8 +1087,10 @@ extern "C" int b200rl_offpolicy_get_state(b200rl_offpolicy* h, float* blob, int6
                                           void* stream) {
   B200RL_REQUIRE(h && blob && steps && n_floats == state_floats(h), "offpolicy_get_state: bad arguments");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  B200RL_CUDA(cudaMemcpyAsync(blob, h->state, (size_t)h->state_n * 4, cudaMemcpyDeviceToHost, s));
-  for (int i = 0; i < 3; ++i) steps[i] = h->net[i].m ? h->net[i].step : 0;
+  B200RL_CUDA(cudaMemcpy2DAsync(blob, (size_t)h->state_n * 4, h->state, h->lane_stride, (size_t)h->state_n * 4, h->K,
+                                cudaMemcpyDeviceToHost, s));
+  for (int z = 0; z < h->K; ++z)
+    for (int i = 0; i < 3; ++i) steps[3 * z + i] = h->net[i].m ? h->net[i].step[z] : 0;
   B200RL_CUDA(cudaStreamSynchronize(s));
   return 0;
 }
@@ -943,11 +1099,14 @@ extern "C" int b200rl_offpolicy_set_state(b200rl_offpolicy* h, const float* blob
                                           void* stream) {
   B200RL_REQUIRE(h && blob && steps && n_floats == state_floats(h), "offpolicy_set_state: bad arguments");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  for (int i = 0; i < 3; ++i)
-    if (h->net[i].m) B200RL_REQUIRE(steps[i] >= 0, "offpolicy_set_state: negative step count");
-  B200RL_CUDA(cudaMemcpyAsync(h->state, blob, (size_t)h->state_n * 4, cudaMemcpyHostToDevice, s));
-  for (int i = 0; i < 3; ++i)
-    if (h->net[i].m) h->net[i].step = steps[i];
+  for (int z = 0; z < h->K; ++z)
+    for (int i = 0; i < 3; ++i)
+      if (h->net[i].m) B200RL_REQUIRE(steps[3 * z + i] >= 0, "offpolicy_set_state: negative step count");
+  B200RL_CUDA(cudaMemcpy2DAsync(h->state, h->lane_stride, blob, (size_t)h->state_n * 4, (size_t)h->state_n * 4, h->K,
+                                cudaMemcpyHostToDevice, s));
+  for (int z = 0; z < h->K; ++z)
+    for (int i = 0; i < 3; ++i)
+      if (h->net[i].m) h->net[i].step[z] = steps[3 * z + i];
   B200RL_CUDA(cudaStreamSynchronize(s));  // `blob` may be reused by the caller right away
   return 0;
 }
@@ -963,35 +1122,56 @@ extern "C" int b200rl_offpolicy_set_sac(b200rl_offpolicy* h, const b200rl_sac_hp
   return 0;
 }
 
+extern "C" int b200rl_offpolicy_set_alpha_group(b200rl_offpolicy* h, const float* log_alpha, const float* exp_avg,
+                                                const float* exp_avg_sq, const int64_t* step) {
+  B200RL_REQUIRE(h && h->sac, "offpolicy_set_alpha: not a SAC engine");
+  B200RL_REQUIRE(log_alpha && exp_avg && exp_avg_sq && step, "offpolicy_set_alpha: NULL argument");
+  float v[B200RL_MAX_LEARNERS][3];
+  for (int z = 0; z < h->K; ++z) {
+    B200RL_REQUIRE(step[z] >= 0, "offpolicy_set_alpha: negative step count");
+    v[z][0] = log_alpha[z], v[z][1] = exp_avg[z], v[z][2] = exp_avg_sq[z];
+  }
+  B200RL_CUDA(cudaMemcpy2DAsync(h->sac_state, h->lane_stride, v, sizeof(v[0]), sizeof(v[0]), h->K,
+                                cudaMemcpyHostToDevice, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  for (int z = 0; z < h->K; ++z) h->alpha_step[z] = step[z];
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_get_alpha_group(b200rl_offpolicy* h, float* log_alpha, float* exp_avg,
+                                                float* exp_avg_sq, int64_t* step) {
+  B200RL_REQUIRE(h && h->sac && log_alpha && exp_avg && exp_avg_sq && step, "offpolicy_get_alpha: bad arguments");
+  float v[B200RL_MAX_LEARNERS][3];
+  B200RL_CUDA(cudaMemcpy2DAsync(v, sizeof(v[0]), h->sac_state, h->lane_stride, sizeof(v[0]), h->K,
+                                cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  for (int z = 0; z < h->K; ++z) {
+    log_alpha[z] = v[z][0], exp_avg[z] = v[z][1], exp_avg_sq[z] = v[z][2];
+    step[z] = h->alpha_step[z];
+  }
+  return 0;
+}
+
 extern "C" int b200rl_offpolicy_set_alpha(b200rl_offpolicy* h, float log_alpha, float exp_avg, float exp_avg_sq,
                                           int64_t step) {
-  B200RL_REQUIRE(h && h->sac, "offpolicy_set_alpha: not a SAC engine");
-  B200RL_REQUIRE(step >= 0, "offpolicy_set_alpha: negative step count");
-  const float v[3] = {log_alpha, exp_avg, exp_avg_sq};
-  B200RL_CUDA(cudaMemcpyAsync(h->sac_state, v, sizeof(v), cudaMemcpyHostToDevice, h->gs));
-  B200RL_CUDA(cudaStreamSynchronize(h->gs));
-  h->alpha_step = step;
-  return 0;
+  B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_set_alpha: a learner group takes offpolicy_set_alpha_group");
+  return b200rl_offpolicy_set_alpha_group(h, &log_alpha, &exp_avg, &exp_avg_sq, &step);
 }
 
 extern "C" int b200rl_offpolicy_get_alpha(b200rl_offpolicy* h, float* log_alpha, float* exp_avg, float* exp_avg_sq,
                                           int64_t* step) {
-  B200RL_REQUIRE(h && h->sac && log_alpha && exp_avg && exp_avg_sq && step, "offpolicy_get_alpha: bad arguments");
-  float v[3];
-  B200RL_CUDA(cudaMemcpyAsync(v, h->sac_state, sizeof(v), cudaMemcpyDeviceToHost, h->gs));
-  B200RL_CUDA(cudaStreamSynchronize(h->gs));
-  *log_alpha = v[0];
-  *exp_avg = v[1];
-  *exp_avg_sq = v[2];
-  *step = h->alpha_step;
-  return 0;
+  B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_get_alpha: a learner group takes offpolicy_get_alpha_group");
+  return b200rl_offpolicy_get_alpha_group(h, log_alpha, exp_avg, exp_avg_sq, step);
 }
 
 extern "C" int b200rl_offpolicy_sac_outputs(b200rl_offpolicy* h, int32_t S, float* log_prob_means, float* alphas) {
   B200RL_REQUIRE(h && h->sac && log_prob_means && alphas && S >= 0 && S <= h->cfg.max_steps,
                  "offpolicy_sac_outputs: bad arguments");
-  B200RL_CUDA(cudaMemcpyAsync(log_prob_means, h->out_logp, (size_t)S * 4, cudaMemcpyDeviceToHost, h->gs));
-  B200RL_CUDA(cudaMemcpyAsync(alphas, h->sac_alpha, (size_t)S * 4, cudaMemcpyDeviceToHost, h->gs));
+  const size_t w = (size_t)S * 4;
+  if (S > 0) {
+    B200RL_CUDA(cudaMemcpy2DAsync(log_prob_means, w, h->out_logp, h->lane_stride, w, h->K, cudaMemcpyDeviceToHost, h->gs));
+    B200RL_CUDA(cudaMemcpy2DAsync(alphas, w, h->sac_alpha, h->lane_stride, w, h->K, cudaMemcpyDeviceToHost, h->gs));
+  }
   B200RL_CUDA(cudaStreamSynchronize(h->gs));
   return 0;
 }
@@ -1033,14 +1213,14 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
       for (int l = 1; l <= Lq; ++l) qa[qi][l] = h->acts[qi == 0 ? 1 : 4][l];
       cudaStream_t qs = qi == 0 ? s3 : s4;
       if (edge(s, qs)) return 1;
-      if (net_forward(qi == 0 ? q1 : q2, qa[qi], B, qs, s_act, A, O)) return 1;
+      if (net_forward(h, qi == 0 ? q1 : q2, qa[qi], B, qs, s_act, A, O)) return 1;
     }
     // ---- targets (td3.py:325-341 / ddpg.py:275-282): the smoothing noise rides on the last layer's epilogue;
     //      [s' | a'] is read in place by the target critics' first layer ----
     float* ta[B200RL_MAX_LAYERS + 1];
     ta[0] = const_cast<float*>(s_nobs);
     for (int l = 1; l <= Lp; ++l) ta[l] = h->acts[0][l];
-    if (net_forward(pit, ta, B, s, nullptr, 0, 0, hp->use_target_noise ? h->eps + (size_t)st * B * A : nullptr, hp))
+    if (net_forward(h, pit, ta, B, s, nullptr, 0, 0, hp->use_target_noise ? h->eps + (size_t)st * B * A : nullptr, hp))
       return 1;
     float* tq[B200RL_MAX_LAYERS + 1];
     tq[0] = const_cast<float*>(s_nobs);
@@ -1052,9 +1232,9 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
       tq2[0] = const_cast<float*>(s_nobs);
       for (int l = 1; l < Lq; ++l) tq2[l] = h->acts[3][l];
       tq2[Lq] = h->qt2;
-      if (net_forward(q2t, tq2, B, s2, ta[Lp], A, O)) return 1;
+      if (net_forward(h, q2t, tq2, B, s2, ta[Lp], A, O)) return 1;
     }
-    if (net_forward(q1t, tq, B, s, ta[Lp], A, O)) return 1;
+    if (net_forward(h, q1t, tq, B, s, ta[Lp], A, O)) return 1;
     if (td3 && edge(s2, s)) return 1;  // both target values are complete on `s`
     // ---- Q steps (td3.py:343-358): TD target + MSE + dq in one kernel, backward, Adam ----
     if (td3) {
@@ -1066,13 +1246,13 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
       NetBuf& qn = qi == 0 ? q1 : q2;
       cudaStream_t qs = qi == 0 ? s : s2;
       float* dq = qi == 0 ? h->dq : h->dq2;
-      q_loss_kernel<<<1, GTHREADS, 0, qs>>>(qa[qi][Lq], s_rew, s_done, h->qt1, td3 ? h->qt2 : nullptr, (float)hp->gamma, B,
-                                            dq, (qi == 0 ? h->out_l1 : h->out_l2) + st,
-                                            (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B);
+      LAUNCH_LANES(h, q_loss_kernel, 1, GTHREADS, qs, qa[qi][Lq], s_rew, s_done, h->qt1, td3 ? h->qt2 : nullptr,
+                   (float)hp->gamma, B, dq, (qi == 0 ? h->out_l1 : h->out_l2) + st,
+                   (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B);
       B200RL_CUDA(cudaGetLastError());
       count_launch(1);
       if (net_backward(h, qn, qa[qi], dq, 1, B, true, nullptr, qs, qi != 0, s_act, A, O, qi == 0 ? s3 : s4)) return 1;
-      if (adam_net(qn, h->adam_tab + (size_t)(1 + qi) * maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, qs)) return 1;
+      if (adam_net(h, qn, h->adam_tab + (size_t)(1 + qi) * maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, qs)) return 1;
     }
     if (td3 && edge(s2, s)) return 1;
     // ---- delayed policy step + polyak (td3.py:244-263, 301-323; ddpg: every step) ----
@@ -1080,19 +1260,19 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
       float* pa[B200RL_MAX_LAYERS + 1];
       pa[0] = const_cast<float*>(s_obs);
       for (int l = 1; l <= Lp; ++l) pa[l] = h->acts[2][l];
-      if (net_forward(pi, pa, B, s)) return 1;
+      if (net_forward(h, pi, pa, B, s)) return 1;
       float* qp[B200RL_MAX_LAYERS + 1];
       qp[0] = const_cast<float*>(s_obs);
       for (int l = 1; l <= Lq; ++l) qp[l] = h->acts[1][l];
-      if (net_forward(q1, qp, B, s, pa[Lp], A, O)) return 1;  // Q1 with its freshly updated parameters (td3.py:309)
-      q_loss_kernel<<<1, GTHREADS, 0, s>>>(qp[Lq], nullptr, nullptr, nullptr, nullptr, 0.f, B, h->dq, h->out_lp + n_pol,
-                                           nullptr);
+      if (net_forward(h, q1, qp, B, s, pa[Lp], A, O)) return 1;  // Q1 with its freshly updated parameters (td3.py:309)
+      LAUNCH_LANES(h, q_loss_kernel, 1, GTHREADS, s, qp[Lq], nullptr, nullptr, nullptr, nullptr, 0.f, B, h->dq,
+                   h->out_lp + n_pol, nullptr);
       B200RL_CUDA(cudaGetLastError());
       count_launch(1);
       // gradient w.r.t. Q1's input; its action columns are the gradient w.r.t. pi(s) (Q parameters frozen)
       if (net_backward(h, q1, qp, h->dq, 1, B, false, h->x_cat, s)) return 1;
       if (net_backward(h, pi, pa, h->x_cat + O, O + A, B, true, nullptr, s, false, nullptr, 0, 0, s3)) return 1;
-      if (adam_net(pi, h->adam_tab, n_pol, hp->policy_beta1, hp->policy_beta2, hp->policy_eps, s)) return 1;
+      if (adam_net(h, pi, h->adam_tab, n_pol, hp->policy_beta1, hp->policy_beta2, hp->policy_eps, s)) return 1;
       PolyakArgs pk{};
       pk.n_nets = td3 ? 3 : 2;
       int nmax = 0;
@@ -1102,7 +1282,8 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
         pk.n[k] = (int)h->net[k].P;
         nmax = pk.n[k] > nmax ? pk.n[k] : nmax;
       }
-      polyak_kernel<<<(nmax + ew - 1) / ew, ew, 0, s>>>(pk, (float)hp->polyak_rho, (float)(1.0 - hp->polyak_rho));
+      LAUNCH_LANES(h, polyak_kernel, (nmax + ew - 1) / ew, ew, s, pk, (float)hp->polyak_rho,
+                   (float)(1.0 - hp->polyak_rho));
       B200RL_CUDA(cudaGetLastError());
       count_launch(1);
       ++n_pol;
@@ -1139,8 +1320,8 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
     count_launch(1);
     return 0;
   };
-  sac_alpha_init_kernel<<<(S + 1 + ew - 1) / ew, ew, 0, s>>>(h->sac_alpha, S + 1, h->sac_state, sp.learn_alpha,
-                                                             (float)sp.alpha);
+  LAUNCH_LANES(h, sac_alpha_init_kernel, (S + 1 + ew - 1) / ew, ew, s, h->sac_alpha, S + 1, h->sac_state,
+               sp.learn_alpha, (float)sp.alpha);
   if (launched()) return 1;
   PolyakArgs pk{};  // 1 -> 4, 2 -> 5
   pk.n_nets = 2;
@@ -1165,21 +1346,22 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
       for (int l = 1; l <= Lq; ++l) qa[qi][l] = h->acts[qi == 0 ? 1 : 4][l];
       cudaStream_t qs = qi == 0 ? s3 : s4;
       if (edge(s, qs)) return 1;
-      if (net_forward(qi == 0 ? q1 : q2, qa[qi], B, qs, s_act, A, O)) return 1;
+      if (net_forward(h, qi == 0 ? q1 : q2, qa[qi], B, qs, s_act, A, O)) return 1;
     }
     float* pa[B200RL_MAX_LAYERS + 1];
     pa[0] = const_cast<float*>(s_obs);
     for (int l = 1; l <= Lp; ++l) pa[l] = h->acts[2][l];
-    if (net_forward(pi, pa, B, s3)) return 1;
-    sac_squash_kernel<<<rows_grid, 128, 0, s3>>>(pa[Lp], eps_cur, B, A, lmin, lmax, limit, h->sac_act, h->sac_logp);
+    if (net_forward(h, pi, pa, B, s3)) return 1;
+    LAUNCH_LANES(h, sac_squash_kernel, rows_grid, 128, s3, pa[Lp], eps_cur, B, A, lmin, lmax, limit, h->sac_act,
+                 h->sac_logp);
     if (launched()) return 1;
     // ---- soft targets: a', log pi' from the current policy at s'; the target critics read [s' | a'] in place ----
     float* ta[B200RL_MAX_LAYERS + 1];
     ta[0] = const_cast<float*>(s_nobs);
     for (int l = 1; l <= Lp; ++l) ta[l] = h->acts[0][l];
-    if (net_forward(pi, ta, B, s)) return 1;
-    sac_squash_kernel<<<rows_grid, 128, 0, s>>>(ta[Lp], eps_next, B, A, lmin, lmax, limit, h->sac_act_next,
-                                                h->sac_logp_next);
+    if (net_forward(h, pi, ta, B, s)) return 1;
+    LAUNCH_LANES(h, sac_squash_kernel, rows_grid, 128, s, ta[Lp], eps_next, B, A, lmin, lmax, limit, h->sac_act_next,
+                 h->sac_logp_next);
     if (launched()) return 1;
     float* tq[2][B200RL_MAX_LAYERS + 1];
     for (int qi = 0; qi < 2; ++qi) {
@@ -1188,8 +1370,8 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
       tq[qi][Lq] = qi == 0 ? h->qt1 : h->qt2;
     }
     if (edge(s, s2)) return 1;
-    if (net_forward(q2t, tq[1], B, s2, h->sac_act_next, A, O)) return 1;
-    if (net_forward(q1t, tq[0], B, s, h->sac_act_next, A, O)) return 1;
+    if (net_forward(h, q2t, tq[1], B, s2, h->sac_act_next, A, O)) return 1;
+    if (net_forward(h, q1t, tq[0], B, s, h->sac_act_next, A, O)) return 1;
     if (edge(s2, s)) return 1;
     // ---- critic step: soft TD target + MSE + dq, backward, Adam (Q2 on s2, Q1 on s) ----
     if (edge(s, s2)) return 1;
@@ -1199,17 +1381,18 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
       NetBuf& qn = qi == 0 ? q1 : q2;
       cudaStream_t qs = qi == 0 ? s : s2;
       float* dq = qi == 0 ? h->dq : h->dq2;
-      sac_q_loss_kernel<<<1, GTHREADS, 0, qs>>>(qa[qi][Lq], s_rew, s_done, h->qt1, h->qt2, h->sac_logp_next, alpha,
-                                                (float)hp->gamma, B, dq, (qi == 0 ? h->out_l1 : h->out_l2) + st,
-                                                (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B);
+      LAUNCH_LANES(h, sac_q_loss_kernel, 1, GTHREADS, qs, qa[qi][Lq], s_rew, s_done, h->qt1, h->qt2, h->sac_logp_next,
+                   alpha, (float)hp->gamma, B, dq, (qi == 0 ? h->out_l1 : h->out_l2) + st,
+                   (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B);
       if (launched()) return 1;
       if (net_backward(h, qn, qa[qi], dq, 1, B, true, nullptr, qs, qi != 0, s_act, A, O, qi == 0 ? s3 : s4)) return 1;
-      if (adam_net(qn, h->adam_tab + (size_t)(1 + qi) * maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, qs)) return 1;
+      if (adam_net(h, qn, h->adam_tab + (size_t)(1 + qi) * maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, qs)) return 1;
     }
     if (edge(s2, s)) return 1;
     // ---- polyak beside the policy step: the targets are next read by the next step ----
     if (edge(s, s4)) return 1;
-    polyak_kernel<<<(pk.n[0] + ew - 1) / ew, ew, 0, s4>>>(pk, (float)hp->polyak_rho, (float)(1.0 - hp->polyak_rho));
+    LAUNCH_LANES(h, polyak_kernel, (pk.n[0] + ew - 1) / ew, ew, s4, pk, (float)hp->polyak_rho,
+                 (float)(1.0 - hp->polyak_rho));
     if (launched()) return 1;
     // ---- policy step: both updated critics on [s | a_pi], differentiated w.r.t. their input only ----
     float* qp[2][B200RL_MAX_LAYERS + 1];
@@ -1218,28 +1401,27 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
       for (int l = 1; l <= Lq; ++l) qp[qi][l] = h->acts[qi == 0 ? 1 : 4][l];
     }
     if (edge(s, s2)) return 1;
-    if (net_forward(q2, qp[1], B, s2, h->sac_act, A, O)) return 1;
-    if (net_forward(q1, qp[0], B, s, h->sac_act, A, O)) return 1;
+    if (net_forward(h, q2, qp[1], B, s2, h->sac_act, A, O)) return 1;
+    if (net_forward(h, q1, qp[0], B, s, h->sac_act, A, O)) return 1;
     if (edge(s2, s)) return 1;
-    sac_policy_loss_kernel<<<1, GTHREADS, 0, s>>>(qp[0][Lq], qp[1][Lq], h->sac_logp, alpha, B, h->dq, h->dq2,
-                                                  h->out_lp + st, h->out_logp + st);
+    LAUNCH_LANES(h, sac_policy_loss_kernel, 1, GTHREADS, s, qp[0][Lq], qp[1][Lq], h->sac_logp, alpha, B, h->dq, h->dq2,
+                 h->out_lp + st, h->out_logp + st);
     if (launched()) return 1;
     if (edge(s, s2)) return 1;
     if (net_backward(h, q2, qp[1], h->dq2, 1, B, false, h->x_cat2, s2, true)) return 1;
     if (sp.learn_alpha) {  // -mean(log_alpha (log pi + target_entropy)), one Adam step; alpha[st + 1] = exp(log_alpha)
-      sac_alpha_step_kernel<<<1, GTHREADS, 0, s2>>>(h->sac_logp, B, (float)sp.target_entropy, h->sac_state,
-                                                    h->adam_tab + (size_t)3 * maxS, st, (float)(1.0 - sp.alpha_beta1),
-                                                    (float)sp.alpha_beta2, (float)(1.0 - sp.alpha_beta2),
-                                                    (float)sp.alpha_eps, h->sac_alpha + st + 1);
+      LAUNCH_LANES(h, sac_alpha_step_kernel, 1, GTHREADS, s2, h->sac_logp, B, (float)sp.target_entropy, h->sac_state,
+                   h->adam_tab + (size_t)3 * maxS, st, (float)(1.0 - sp.alpha_beta1), (float)sp.alpha_beta2,
+                   (float)(1.0 - sp.alpha_beta2), (float)sp.alpha_eps, h->sac_alpha + st + 1);
       if (launched()) return 1;
     }
     if (net_backward(h, q1, qp[0], h->dq, 1, B, false, h->x_cat, s)) return 1;
     if (edge(s2, s)) return 1;
-    sac_squash_backward_kernel<<<(B * A + ew - 1) / ew, ew, 0, s>>>(pa[Lp], eps_cur, h->x_cat + O, h->x_cat2 + O, O + A,
-                                                                   B, A, lmin, lmax, limit, alpha, h->sac_dout);
+    LAUNCH_LANES(h, sac_squash_backward_kernel, (B * A + ew - 1) / ew, ew, s, pa[Lp], eps_cur, h->x_cat + O,
+                 h->x_cat2 + O, O + A, B, A, lmin, lmax, limit, alpha, h->sac_dout);
     if (launched()) return 1;
     if (net_backward(h, pi, pa, h->sac_dout, 2 * A, B, true, nullptr, s, false, nullptr, 0, 0, s3)) return 1;
-    if (adam_net(pi, h->adam_tab, st, hp->policy_beta1, hp->policy_beta2, hp->policy_eps, s)) return 1;
+    if (adam_net(h, pi, h->adam_tab, st, hp->policy_beta1, hp->policy_beta2, hp->policy_eps, s)) return 1;
     if (edge(s4, s)) return 1;
   }
   return 0;
@@ -1545,29 +1727,33 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   const size_t SB = (size_t)S * B;
 
   // Adam's step-dependent scalars for the steps of this call (torch's host-side double arithmetic), one small upload
+  // (a group: one table per learner, from that learner's step counts, uploaded with one strided copy)
   const int maxS = h->cfg.max_steps;
   const int n_pol_expected = h->sac ? S : (S + hp->policy_delay - 1) / hp->policy_delay;  // SAC: no delay
-  for (int k = 0; k < n_pol_expected; ++k)
-    adam_scalars(h->net[0].step + k + 1, hp->policy_lr, hp->policy_beta1, hp->policy_beta2, &h->h_adam_tab[k].x,
-                 &h->h_adam_tab[k].y);
-  for (int qi = 0; qi < (td3 ? 2 : 1); ++qi)
-    for (int k = 0; k < S; ++k)
-      adam_scalars(h->net[1 + qi].step + k + 1, qi == 0 ? hp->q1_lr : hp->q2_lr, hp->q_beta1, hp->q_beta2,
-                   &h->h_adam_tab[(size_t)(1 + qi) * maxS + k].x, &h->h_adam_tab[(size_t)(1 + qi) * maxS + k].y);
+  const size_t tab_n = (h->sac ? 4 : 3) * (size_t)maxS;
   const bool learn_alpha = h->sac && h->sac_hp.learn_alpha;
-  if (learn_alpha)
-    for (int k = 0; k < S; ++k)
-      adam_scalars(h->alpha_step + k + 1, h->sac_hp.alpha_lr, h->sac_hp.alpha_beta1, h->sac_hp.alpha_beta2,
-                   &h->h_adam_tab[(size_t)3 * maxS + k].x, &h->h_adam_tab[(size_t)3 * maxS + k].y);
-  B200RL_CUDA(cudaMemcpyAsync(h->adam_tab, h->h_adam_tab, (h->sac ? 4 : 3) * (size_t)maxS * sizeof(float2),
-                              cudaMemcpyHostToDevice, s));
+  for (int z = 0; z < h->K; ++z) {
+    float2* tab = h->h_adam_tab + z * tab_n;
+    for (int k = 0; k < n_pol_expected; ++k)
+      adam_scalars(h->net[0].step[z] + k + 1, hp->policy_lr, hp->policy_beta1, hp->policy_beta2, &tab[k].x, &tab[k].y);
+    for (int qi = 0; qi < (td3 ? 2 : 1); ++qi)
+      for (int k = 0; k < S; ++k)
+        adam_scalars(h->net[1 + qi].step[z] + k + 1, qi == 0 ? hp->q1_lr : hp->q2_lr, hp->q_beta1, hp->q_beta2,
+                     &tab[(size_t)(1 + qi) * maxS + k].x, &tab[(size_t)(1 + qi) * maxS + k].y);
+    if (learn_alpha)
+      for (int k = 0; k < S; ++k)
+        adam_scalars(h->alpha_step[z] + k + 1, h->sac_hp.alpha_lr, h->sac_hp.alpha_beta1, h->sac_hp.alpha_beta2,
+                     &tab[(size_t)3 * maxS + k].x, &tab[(size_t)3 * maxS + k].y);
+  }
+  B200RL_CUDA(cudaMemcpy2DAsync(h->adam_tab, h->lane_stride, h->h_adam_tab, tab_n * sizeof(float2),
+                                tab_n * sizeof(float2), h->K, cudaMemcpyHostToDevice, s));
 
   int n_pol = 0;
   // opt-in: on B200 it measured 12.1 ms per 50 TD3 steps against 11.1 ms for the graph replay (B = 256, 256-wide nets) -- the
   // 32 x 32 fp32 tiles themselves, two per SM in the phases that merge four networks, are the cost, not the launches.
-  // SAC has no program for it and always takes the graph (or plain launches).
+  // SAC and learner groups have no program for it and always take the graph (or plain launches).
   const char* menv = getenv("B200RL_OFFPOLICY_MEGAKERNEL");
-  const bool use_mega = menv != nullptr && menv[0] == '1' && !h->sac;
+  const bool use_mega = menv != nullptr && menv[0] == '1' && !h->sac && h->K == 1;
   const char* genv = getenv("B200RL_OFFPOLICY_GRAPH");
   const bool use_graph = !(genv != nullptr && genv[0] == '0');
   if (use_mega) {
@@ -1645,18 +1831,23 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
     B200RL_CUDA(cudaGraphLaunch(h->graph, s));
     count_launch(h->graph_launches);
   }
-  h->net[0].step += n_pol;
-  h->net[1].step += S;
-  if (td3) h->net[2].step += S;
-  if (learn_alpha) h->alpha_step += S;
-  // one device -> host read of everything train() logs
-  B200RL_CUDA(cudaMemcpyAsync(q1_values, h->out_q1, SB * 4, cudaMemcpyDeviceToHost, s));
-  B200RL_CUDA(cudaMemcpyAsync(q1_losses, h->out_l1, (size_t)S * 4, cudaMemcpyDeviceToHost, s));
-  if (td3) {
-    B200RL_CUDA(cudaMemcpyAsync(q2_values, h->out_q2, SB * 4, cudaMemcpyDeviceToHost, s));
-    B200RL_CUDA(cudaMemcpyAsync(q2_losses, h->out_l2, (size_t)S * 4, cudaMemcpyDeviceToHost, s));
+  for (int z = 0; z < h->K; ++z) {
+    h->net[0].step[z] += n_pol;
+    h->net[1].step[z] += S;
+    if (td3) h->net[2].step[z] += S;
+    if (learn_alpha) h->alpha_step[z] += S;
   }
-  if (n_pol > 0) B200RL_CUDA(cudaMemcpyAsync(policy_losses, h->out_lp, (size_t)n_pol * 4, cudaMemcpyDeviceToHost, s));
+  // one device -> host read of everything train() logs: [K, S, B] values, [K, S] losses
+  const size_t ls = h->lane_stride, K = (size_t)h->K;
+  B200RL_CUDA(cudaMemcpy2DAsync(q1_values, SB * 4, h->out_q1, ls, SB * 4, K, cudaMemcpyDeviceToHost, s));
+  B200RL_CUDA(cudaMemcpy2DAsync(q1_losses, (size_t)S * 4, h->out_l1, ls, (size_t)S * 4, K, cudaMemcpyDeviceToHost, s));
+  if (td3) {
+    B200RL_CUDA(cudaMemcpy2DAsync(q2_values, SB * 4, h->out_q2, ls, SB * 4, K, cudaMemcpyDeviceToHost, s));
+    B200RL_CUDA(cudaMemcpy2DAsync(q2_losses, (size_t)S * 4, h->out_l2, ls, (size_t)S * 4, K, cudaMemcpyDeviceToHost, s));
+  }
+  if (n_pol > 0)
+    B200RL_CUDA(cudaMemcpy2DAsync(policy_losses, (size_t)S * 4, h->out_lp, ls, (size_t)n_pol * 4, K,
+                                  cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaStreamSynchronize(s));
   *n_policy_updates = n_pol;
   return 0;
@@ -1684,16 +1875,88 @@ extern "C" int b200rl_offpolicy_train(b200rl_offpolicy* h, const b200rl_offpolic
   if (S == 0) return 0;
   B200RL_CUDA(cudaEventRecord(h->ev, user));
   B200RL_CUDA(cudaStreamWaitEvent(s, h->ev, 0));
-  // one host -> device upload of every minibatch of this train() call
-  B200RL_CUDA(cudaMemcpyAsync(h->obs, obs, SB * O * 4, cudaMemcpyHostToDevice, s));
-  B200RL_CUDA(cudaMemcpyAsync(h->act, act, SB * A * 4, cudaMemcpyHostToDevice, s));
-  B200RL_CUDA(cudaMemcpyAsync(h->rew, rew, SB * 4, cudaMemcpyHostToDevice, s));
-  B200RL_CUDA(cudaMemcpyAsync(h->nobs, next_obs, SB * O * 4, cudaMemcpyHostToDevice, s));
-  B200RL_CUDA(cudaMemcpyAsync(h->done, done, SB * 4, cudaMemcpyHostToDevice, s));
-  if (h->sac) B200RL_CUDA(cudaMemcpyAsync(h->eps, noise, 2 * SB * A * 4, cudaMemcpyHostToDevice, s));
-  else if (hp->use_target_noise) B200RL_CUDA(cudaMemcpyAsync(h->eps, noise, SB * A * 4, cudaMemcpyHostToDevice, s));
+  // one host -> device upload of every minibatch of this train() call ([K, S, B, ...] into the K arenas)
+  auto up = [&](void* dst, const void* src, size_t bytes) -> int {
+    B200RL_CUDA(cudaMemcpy2DAsync(dst, h->lane_stride, src, bytes, bytes, h->K, cudaMemcpyHostToDevice, s));
+    return 0;
+  };
+  if (up(h->obs, obs, SB * O * 4) || up(h->act, act, SB * A * 4) || up(h->rew, rew, SB * 4) ||
+      up(h->nobs, next_obs, SB * O * 4) || up(h->done, done, SB * 4))
+    return 1;
+  if (h->sac && up(h->eps, noise, 2 * SB * A * 4)) return 1;
+  if (!h->sac && hp->use_target_noise && up(h->eps, noise, SB * A * 4)) return 1;
 
+  return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
+}
 
+// The five staged columns (obs, act, rew, next_obs, done) gathered from each learner's replay columns at the rows in
+// h->idx: one launch per column for all learners
+static int gather_columns(b200rl_offpolicy* h, const b200rl_offpolicy_replay* rb, long long SB, cudaStream_t s) {
+  const int O = h->O, A = h->A;
+  float* dst[5] = {h->obs, h->act, h->rew, h->nobs, h->done};
+  const int w[5] = {O, A, 1, O, 1};
+  for (int c = 0; c < 5; ++c) {
+    const long long n = SB * w[c];
+    const dim3 grid((unsigned)((n + 255) / 256));
+    auto col = [&](int z) {
+      const float* p[5] = {rb[z].obs, rb[z].act, rb[z].rew, rb[z].next_obs, rb[z].done};
+      return p[c];
+    };
+    if (h->K == 1) {
+      gather_rows_kernel<false><<<grid, 256, 0, s>>>(LaneSrc<false>{{col(0)}}, h->idx, w[c], SB, dst[c], 0);
+    } else {
+      LaneSrc<true> src{};
+      for (int z = 0; z < h->K; ++z) src.p[z] = col(z);
+      gather_rows_kernel<true><<<lane_grid(grid, h->K), 256, 0, s>>>(src, h->idx, w[c], SB, dst[c], h->lane_stride);
+    }
+    B200RL_CUDA(cudaGetLastError());
+    count_launch(1);
+  }
+  return 0;
+}
+
+static int check_replay(const b200rl_offpolicy* h, const b200rl_offpolicy_replay* rb, const char* what) {
+  B200RL_REQUIRE(rb != nullptr, "%s: NULL replay columns", what);
+  for (int z = 0; z < h->K; ++z)
+    B200RL_REQUIRE(rb[z].obs && rb[z].act && rb[z].rew && rb[z].next_obs && rb[z].done && rb[z].rows >= 1,
+                   "%s: learner %d: NULL replay column or no rows", what, z);
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_train_gather_group(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int32_t S,
+                                                   int32_t B, const b200rl_offpolicy_replay* rb, const int64_t* idx,
+                                                   const float* noise, float* q1_values, float* q2_values,
+                                                   float* q1_losses, float* q2_losses, float* policy_losses,
+                                                   int32_t* n_policy_updates, void* stream) {
+  B200RL_REQUIRE(h && hp && idx && q1_values && q1_losses && policy_losses && n_policy_updates,
+                 "offpolicy_train_gather: NULL argument");
+  if (int rc = check_replay(h, rb, "offpolicy_train_gather")) return rc;
+  B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
+                 "offpolicy_train_gather: S=%d B=%d exceed the capacities", S, B);
+  const bool td3 = h->cfg.n_q == 2;
+  B200RL_REQUIRE(!td3 || (q2_values && q2_losses), "offpolicy_train_gather: TD3 needs the Q2 outputs");
+  B200RL_REQUIRE(!hp->use_target_noise || noise, "offpolicy_train_gather: target noise requested but no noise given");
+  B200RL_REQUIRE(hp->policy_delay >= 1, "offpolicy_train_gather: policy_delay must be >= 1");
+  if (sac_ready(h, noise != nullptr, "offpolicy_train_gather")) return 2;
+  const size_t SB = (size_t)S * B;
+  for (int z = 0; z < h->K; ++z)
+    for (size_t i = 0; i < SB; ++i)
+      B200RL_REQUIRE(idx[z * SB + i] >= 0 && idx[z * SB + i] < rb[z].rows,
+                     "offpolicy_train_gather: index %lld outside the %lld replay rows", (long long)idx[z * SB + i],
+                     (long long)rb[z].rows);
+  cudaStream_t user = static_cast<cudaStream_t>(stream);
+  cudaStream_t s = h->gs;
+  const int A = h->A;
+  *n_policy_updates = 0;
+  if (S == 0) return 0;
+  B200RL_CUDA(cudaEventRecord(h->ev, user));
+  B200RL_CUDA(cudaStreamWaitEvent(s, h->ev, 0));
+  // the minibatches are gathered on the device from the replay columns: only the indices (and noise) cross PCIe
+  const size_t ls = h->lane_stride;
+  B200RL_CUDA(cudaMemcpy2DAsync(h->idx, ls, idx, SB * 8, SB * 8, h->K, cudaMemcpyHostToDevice, s));
+  const size_t n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise ? SB * A : 0);
+  if (n_eps) B200RL_CUDA(cudaMemcpy2DAsync(h->eps, ls, noise, n_eps * 4, n_eps * 4, h->K, cudaMemcpyHostToDevice, s));
+  if (gather_columns(h, rb, (long long)SB, s)) return 1;
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
 }
 
@@ -1703,66 +1966,41 @@ extern "C" int b200rl_offpolicy_train_gather(b200rl_offpolicy* h, const b200rl_o
                                              const int64_t* idx, const float* noise, float* q1_values,
                                              float* q2_values, float* q1_losses, float* q2_losses,
                                              float* policy_losses, int32_t* n_policy_updates, void* stream) {
-  B200RL_REQUIRE(h && hp && d_obs && d_act && d_rew && d_next_obs && d_done && idx && q1_values && q1_losses &&
-                     policy_losses && n_policy_updates, "offpolicy_train_gather: NULL argument");
-  B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
-                 "offpolicy_train_gather: S=%d B=%d exceed the capacities", S, B);
-  const bool td3 = h->cfg.n_q == 2;
-  B200RL_REQUIRE(!td3 || (q2_values && q2_losses), "offpolicy_train_gather: TD3 needs the Q2 outputs");
-  B200RL_REQUIRE(!hp->use_target_noise || noise, "offpolicy_train_gather: target noise requested but no noise given");
-  B200RL_REQUIRE(hp->policy_delay >= 1, "offpolicy_train_gather: policy_delay must be >= 1");
-  if (sac_ready(h, noise != nullptr, "offpolicy_train_gather")) return 2;
-  const size_t SB = (size_t)S * B;
-  for (size_t i = 0; i < SB; ++i)
-    B200RL_REQUIRE(idx[i] >= 0 && idx[i] < rows, "offpolicy_train_gather: index %lld outside the %lld replay rows",
-                   (long long)idx[i], (long long)rows);
-  cudaStream_t user = static_cast<cudaStream_t>(stream);
-  cudaStream_t s = h->gs;
-  const int O = h->O, A = h->A;
-  *n_policy_updates = 0;
-  if (S == 0) return 0;
-  B200RL_CUDA(cudaEventRecord(h->ev, user));
-  B200RL_CUDA(cudaStreamWaitEvent(s, h->ev, 0));
-  // the minibatches are gathered on the device from the replay columns: only the indices (and noise) cross PCIe
-  B200RL_CUDA(cudaMemcpyAsync(h->idx, idx, SB * sizeof(long long), cudaMemcpyHostToDevice, s));
-  if (h->sac) B200RL_CUDA(cudaMemcpyAsync(h->eps, noise, 2 * SB * A * 4, cudaMemcpyHostToDevice, s));
-  else if (hp->use_target_noise) B200RL_CUDA(cudaMemcpyAsync(h->eps, noise, SB * A * 4, cudaMemcpyHostToDevice, s));
-  const struct { const float* src; float* dst; int w; } cols[5] = {
-      {d_obs, h->obs, O}, {d_act, h->act, A}, {d_rew, h->rew, 1}, {d_next_obs, h->nobs, O}, {d_done, h->done, 1}};
-  for (const auto& c : cols) {
-    const long long n = (long long)SB * c.w;
-    gather_rows_kernel<<<(int)((n + 255) / 256), 256, 0, s>>>(c.src, h->idx, c.w, (long long)SB, c.dst);
-    B200RL_CUDA(cudaGetLastError());
-    count_launch(1);
-  }
-  return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
+  B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_train_gather: a learner group takes train_gather_group");
+  B200RL_REQUIRE(d_obs && d_act && d_rew && d_next_obs && d_done, "offpolicy_train_gather: NULL argument");
+  const b200rl_offpolicy_replay rb = {d_obs, d_act, d_rew, d_next_obs, d_done, rows};
+  return b200rl_offpolicy_train_gather_group(h, hp, S, B, &rb, idx, noise, q1_values, q2_values, q1_losses, q2_losses,
+                                             policy_losses, n_policy_updates, stream);
 }
 
 /* Opt-in: the minibatch indices and the target-smoothing noise are DRAWN ON THE DEVICE (Philox4x32-10 keyed by `seed`,
  * block `call`), so nothing but the hyper-parameters crosses PCIe on the way in.  The streams are not the reference's
  * (numpy's MT19937 / torch's CPU generator): same distributions, different numbers -- callers that need the reference's
  * draws use b200rl_offpolicy_train_gather.  The ring: `size` live rows, logical row u at physical (start + u) % rows. */
-extern "C" int b200rl_offpolicy_train_gather_rng(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int32_t S,
-                                                 int32_t B, const float* d_obs, const float* d_act, const float* d_rew,
-                                                 const float* d_next_obs, const float* d_done, int64_t rows,
-                                                 int64_t ring_start, int64_t ring_size, uint64_t seed, uint64_t call,
-                                                 float* q1_values, float* q2_values, float* q1_losses,
-                                                 float* q2_losses, float* policy_losses, int32_t* n_policy_updates,
-                                                 void* stream) {
-  B200RL_REQUIRE(h && hp && d_obs && d_act && d_rew && d_next_obs && d_done && q1_values && q1_losses &&
-                     policy_losses && n_policy_updates, "offpolicy_train_gather_rng: NULL argument");
+extern "C" int b200rl_offpolicy_train_gather_rng_group(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp,
+                                                       int32_t S, int32_t B, const b200rl_offpolicy_replay* rb,
+                                                       const int64_t* ring_start, const int64_t* ring_size,
+                                                       const uint64_t* seed, const uint64_t* call, float* q1_values,
+                                                       float* q2_values, float* q1_losses, float* q2_losses,
+                                                       float* policy_losses, int32_t* n_policy_updates, void* stream) {
+  B200RL_REQUIRE(h && hp && ring_start && ring_size && seed && call && q1_values && q1_losses && policy_losses &&
+                     n_policy_updates, "offpolicy_train_gather_rng: NULL argument");
+  if (int rc = check_replay(h, rb, "offpolicy_train_gather_rng")) return rc;
   B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
                  "offpolicy_train_gather_rng: S=%d B=%d exceed the capacities", S, B);
-  B200RL_REQUIRE(rows >= 1 && ring_size >= 1 && ring_size <= rows && ring_start >= 0 && ring_start < rows,
-                 "offpolicy_train_gather_rng: bad ring (rows %lld, start %lld, size %lld)", (long long)rows,
-                 (long long)ring_start, (long long)ring_size);
+  for (int z = 0; z < h->K; ++z) {
+    const long long rows = rb[z].rows;
+    B200RL_REQUIRE(ring_size[z] >= 1 && ring_size[z] <= rows && ring_start[z] >= 0 && ring_start[z] < rows,
+                   "offpolicy_train_gather_rng: bad ring (rows %lld, start %lld, size %lld)", rows,
+                   (long long)ring_start[z], (long long)ring_size[z]);
+  }
   const bool td3 = h->cfg.n_q == 2;
   B200RL_REQUIRE(!td3 || (q2_values && q2_losses), "offpolicy_train_gather_rng: TD3 needs the Q2 outputs");
   B200RL_REQUIRE(hp->policy_delay >= 1, "offpolicy_train_gather_rng: policy_delay must be >= 1");
   if (sac_ready(h, true, "offpolicy_train_gather_rng")) return 2;
   cudaStream_t user = static_cast<cudaStream_t>(stream);
   cudaStream_t s = h->gs;
-  const int O = h->O, A = h->A;
+  const int A = h->A;
   const long long SB = (long long)S * B;
   *n_policy_updates = 0;
   if (S == 0) return 0;
@@ -1770,19 +2008,37 @@ extern "C" int b200rl_offpolicy_train_gather_rng(b200rl_offpolicy* h, const b200
   B200RL_CUDA(cudaStreamWaitEvent(s, h->ev, 0));
   const long long n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise ? SB * A : 0);
   const long long n_thr = ((SB > n_eps ? SB : n_eps) + 3) / 4;
-  draw_minibatches_kernel<<<(int)((n_thr + 255) / 256), 256, 0, s>>>(h->idx, SB, n_eps ? h->eps : nullptr, n_eps, seed, call,
-                                                                    ring_start, ring_size, rows);
+  const dim3 grid((unsigned)((n_thr + 255) / 256));
+  if (h->K == 1) {
+    const DrawKeys<false> k = {{seed[0]}, {call[0]}, {ring_start[0]}, {ring_size[0]}, {rb[0].rows}};
+    draw_minibatches_kernel<false><<<grid, 256, 0, s>>>(h->idx, SB, n_eps ? h->eps : nullptr, n_eps, k, 0);
+  } else {
+    DrawKeys<true> k{};
+    for (int z = 0; z < h->K; ++z)
+      k.seed[z] = seed[z], k.call[z] = call[z], k.start[z] = ring_start[z], k.size[z] = ring_size[z],
+      k.capacity[z] = rb[z].rows;
+    draw_minibatches_kernel<true><<<lane_grid(grid, h->K), 256, 0, s>>>(h->idx, SB, n_eps ? h->eps : nullptr, n_eps, k,
+                                                                        h->lane_stride);
+  }
   B200RL_CUDA(cudaGetLastError());
   count_launch(1);
-  const struct { const float* src; float* dst; int w; } cols[5] = {
-      {d_obs, h->obs, O}, {d_act, h->act, A}, {d_rew, h->rew, 1}, {d_next_obs, h->nobs, O}, {d_done, h->done, 1}};
-  for (const auto& c : cols) {
-    const long long n = SB * c.w;
-    gather_rows_kernel<<<(int)((n + 255) / 256), 256, 0, s>>>(c.src, h->idx, c.w, SB, c.dst);
-    B200RL_CUDA(cudaGetLastError());
-    count_launch(1);
-  }
+  if (gather_columns(h, rb, SB, s)) return 1;
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
+}
+
+extern "C" int b200rl_offpolicy_train_gather_rng(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int32_t S,
+                                                 int32_t B, const float* d_obs, const float* d_act, const float* d_rew,
+                                                 const float* d_next_obs, const float* d_done, int64_t rows,
+                                                 int64_t ring_start, int64_t ring_size, uint64_t seed, uint64_t call,
+                                                 float* q1_values, float* q2_values, float* q1_losses,
+                                                 float* q2_losses, float* policy_losses, int32_t* n_policy_updates,
+                                                 void* stream) {
+  B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_train_gather_rng: a learner group takes train_gather_rng_group");
+  B200RL_REQUIRE(d_obs && d_act && d_rew && d_next_obs && d_done, "offpolicy_train_gather_rng: NULL argument");
+  const b200rl_offpolicy_replay rb = {d_obs, d_act, d_rew, d_next_obs, d_done, rows};
+  return b200rl_offpolicy_train_gather_rng_group(h, hp, S, B, &rb, &ring_start, &ring_size, &seed, &call, q1_values,
+                                                 q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates,
+                                                 stream);
 }
 
 /* The draws of the last train_gather / train_gather_rng call (physical rows [S*B], noise [S*B*A] or NULL): what a test
@@ -1795,8 +2051,10 @@ extern "C" int b200rl_offpolicy_get_draws(b200rl_offpolicy* h, int32_t S, int32_
   (void)stream;
   const size_t SB = (size_t)S * B;
   static_assert(sizeof(long long) == sizeof(int64_t), "index width");
-  B200RL_CUDA(cudaMemcpyAsync(idx, h->idx, SB * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-  if (noise) B200RL_CUDA(cudaMemcpyAsync(noise, h->eps, (h->sac ? 2 : 1) * SB * h->A * 4, cudaMemcpyDeviceToHost, s));
+  const size_t n_eps = (h->sac ? 2 : 1) * SB * h->A;
+  B200RL_CUDA(cudaMemcpy2DAsync(idx, SB * 8, h->idx, h->lane_stride, SB * 8, h->K, cudaMemcpyDeviceToHost, s));
+  if (noise)
+    B200RL_CUDA(cudaMemcpy2DAsync(noise, n_eps * 4, h->eps, h->lane_stride, n_eps * 4, h->K, cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaStreamSynchronize(s));
   return 0;
 }

@@ -321,13 +321,17 @@ class OnPolicyEngine:
 class OffPolicyEngine:
     """Device-resident state of one DDPG / TD3 (``algo`` 0) or SAC (``algo`` 1) learner (C ABI: b200rl_offpolicy_*).
     SAC: ``n_q`` = 2, the policy maps obs -> [mean | log_std] (2A outputs), there is no target policy (network 3), and
-    ``set_sac`` must be called before the first train call."""
+    ``set_sac`` must be called before the first train call.
+
+    ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
+    launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
+    is [K][per-learner blob] with [K][3] step counts, and the per-network accessors are refused."""
 
     NETS = {"policy": 0, "q1": 1, "q2": 2, "target_policy": 3, "target_q1": 4, "target_q2": 5}
     TD3, SAC = 0, 1
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
-                 q_acts=("relu", "identity"), algo: int = 0):
+                 q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1):
         from ._lib import OffPolicyConfig
         self.lib = _lib.load()
         current_stream_handle()
@@ -342,8 +346,9 @@ class OffPolicyEngine:
         self.policy_acts, self.q_acts = tuple(policy_acts), tuple(q_acts)
         self.n_policy = int(self.lib.b200rl_mlp_param_count(cfg.policy))
         self.n_qp = int(self.lib.b200rl_mlp_param_count(cfg.q))
+        self.K = int(n_learners)
         h = C.c_void_p()
-        check(self.lib.b200rl_offpolicy_create(C.byref(cfg), C.byref(h)), "offpolicy_create")
+        check(self.lib.b200rl_offpolicy_create_group(C.byref(cfg), self.K, C.byref(h)), "offpolicy_create")
         self.h = h
 
     def close(self):
@@ -388,8 +393,8 @@ class OffPolicyEngine:
 
     # ---- whole state in one transfer ----
     def state_layout(self):
-        """[(kind, net index, offset, count)] of the state blob: ("params", 0..5) then ("m" / "v", 0..2); every
-        segment starts on a multiple of 64 floats (b200rl.h)."""
+        """[(kind, net index, offset, count)] of one learner's state blob: ("params", 0..5) then ("m" / "v", 0..2);
+        every segment starts on a multiple of 64 floats (b200rl.h).  A group's blob is K of these back to back."""
         pad = lambda n: (n + 63) & ~63
         present = [0, 1] + ([2] if self.n_q == 2 else []) + ([] if self.algo == self.SAC else [3]) + [4] + \
             ([5] if self.n_q == 2 else [])
@@ -401,7 +406,7 @@ class OffPolicyEngine:
             for kind in ("m", "v"):
                 out.append((kind, i, off, self._n(i)))
                 off += pad(self._n(i))
-        assert off == int(self.lib.b200rl_offpolicy_state_floats(self.h))
+        assert off * self.K == int(self.lib.b200rl_offpolicy_state_floats(self.h))
         return out, off
 
     def state_buffer(self):
@@ -420,19 +425,24 @@ class OffPolicyEngine:
         return buf
 
     def get_state(self):
-        """Device -> the persistent blob; returns (blob as numpy view, [3 Adam step counts])."""
+        """Device -> the persistent blob; returns (blob as numpy view, [3 Adam step counts]; a group: [K][3])."""
         buf = self.state_buffer()
-        steps = (C.c_int64 * 3)()
+        steps = (C.c_int64 * (3 * self.K))()
         check(self.lib.b200rl_offpolicy_get_state(self.h, C.c_void_p(buf.data_ptr()), buf.numel(), steps,
                                                   current_stream_handle()), "get_state")
-        return buf.numpy(), [int(x) for x in steps]
+        st = [int(x) for x in steps]
+        return buf.numpy(), st if self.K == 1 else [st[3 * z:3 * z + 3] for z in range(self.K)]
 
     def set_state(self, blob, steps):
-        """``blob`` = None sends the persistent blob (fill ``state_buffer()`` first), else any float32 array of that size."""
+        """``blob`` = None sends the persistent blob (fill ``state_buffer()`` first), else any float32 array of that size.
+        ``steps``: [3] Adam step counts (a group: [K][3])."""
         buf = self.state_buffer()
         if blob is not None and not (isinstance(blob, np.ndarray) and blob.ctypes.data == buf.data_ptr()):
             buf.numpy()[:] = np.asarray(blob, dtype=np.float32).reshape(-1)
-        st = (C.c_int64 * 3)(*[int(x) for x in steps])
+        flat = np.asarray(steps, dtype=np.int64).reshape(-1)
+        if flat.size != 3 * self.K:
+            raise ValueError(f"set_state: expected {3 * self.K} step counts, got {flat.size}")
+        st = (C.c_int64 * (3 * self.K))(*[int(x) for x in flat])
         check(self.lib.b200rl_offpolicy_set_state(self.h, C.c_void_p(buf.data_ptr()), buf.numel(), st,
                                                   current_stream_handle()), "set_state")
 
@@ -452,28 +462,58 @@ class OffPolicyEngine:
               "get_alpha")
         return la.value, m.value, v.value, int(step.value)
 
+    def set_alpha_group(self, states) -> None:
+        """``states``: K tuples (log_alpha, exp_avg, exp_avg_sq, step), one per learner."""
+        la, m, v = (np.array([float(x[i]) for x in states], np.float32) for i in range(3))
+        st = np.array([int(x[3]) for x in states], np.int64)
+        if st.size != self.K:
+            raise ValueError(f"set_alpha_group: expected {self.K} learners, got {st.size}")
+        check(self.lib.b200rl_offpolicy_set_alpha_group(self.h, _ptr(la), _ptr(m), _ptr(v), _ptr(st)), "set_alpha")
+
+    def get_alpha_group(self):
+        """[(log_alpha, exp_avg, exp_avg_sq, step)] of every learner."""
+        la, m, v = (np.zeros(self.K, np.float32) for _ in range(3))
+        st = np.zeros(self.K, np.int64)
+        check(self.lib.b200rl_offpolicy_get_alpha_group(self.h, _ptr(la), _ptr(m), _ptr(v), _ptr(st)), "get_alpha")
+        return [(float(la[z]), float(m[z]), float(v[z]), int(st[z])) for z in range(self.K)]
+
     def sac_outputs(self, S: int):
-        """(mean log pi per step [S], alpha used by each step [S]) of the last train call."""
-        lp, al = np.zeros(S, np.float32), np.zeros(S, np.float32)
+        """(mean log pi per step [S], alpha used by each step [S]) of the last train call (a group: [K, S] each)."""
+        lp, al = np.zeros((self.K, S), np.float32), np.zeros((self.K, S), np.float32)
         check(self.lib.b200rl_offpolicy_sac_outputs(self.h, int(S), _ptr(lp), _ptr(al)), "sac_outputs")
-        return lp, al
+        return (lp[0], al[0]) if self.K == 1 else (lp, al)
+
+    def _out_buffers(self, S, B):
+        K = self.K
+        return (np.zeros((K, S, B), np.float32), np.zeros((K, S, B), np.float32), np.zeros((K, S), np.float32),
+                np.zeros((K, S), np.float32), np.zeros((K, max(S, 1)), np.float32), C.c_int32())
 
     def _outputs(self, S, q1v, q2v, l1, l2, lp, npol):
-        out = dict(q1_values=q1v, q2_values=q2v, q1_losses=l1, q2_losses=l2, policy_losses=lp[:npol.value])
+        """The logged quantities; a solo engine drops the leading [K] axis."""
+        out = dict(q1_values=q1v, q2_values=q2v, q1_losses=l1, q2_losses=l2, policy_losses=lp[:, :npol.value])
+        if self.K == 1:
+            out = {k: v[0] for k, v in out.items()}
         if self.algo == self.SAC:
             out["log_prob_means"], out["alphas"] = self.sac_outputs(S)
         return out
 
+    def _lead(self, a, dtype, ndim):
+        """A solo engine's input without the [K] axis, a group's with it, as one contiguous [K, ...] array."""
+        a = _c(a, dtype)
+        if self.K == 1 and a.ndim == ndim - 1:
+            a = a[None]
+        if a.shape[0] != self.K:
+            raise ValueError(f"expected a leading axis of {self.K} learners, got shape {a.shape}")
+        return a
+
     def train(self, hp, obs, act, rew, next_obs, done, noise=None):
         """obs/next_obs [S,B,O], act [S,B,A], rew/done [S,B], noise [S,B,A] or None (SAC: [S,2,B,A], required) -> dict
-        of logged quantities (SAC adds log_prob_means and alphas)."""
-        obs, act, next_obs = _c(obs, np.float32), _c(act, np.float32), _c(next_obs, np.float32)
-        rew, done = _c(rew, np.float32), _c(done, np.float32)
-        noise = None if noise is None else _c(noise, np.float32)
-        S, B = obs.shape[0], obs.shape[1]
-        q1v, q2v = np.zeros((S, B), np.float32), np.zeros((S, B), np.float32)
-        l1, l2, lp = np.zeros(S, np.float32), np.zeros(S, np.float32), np.zeros(max(S, 1), np.float32)
-        npol = C.c_int32()
+        of logged quantities (SAC adds log_prob_means and alphas).  A group: every array with a leading [K] axis."""
+        obs, act, next_obs = (self._lead(x, np.float32, 4) for x in (obs, act, next_obs))
+        rew, done = self._lead(rew, np.float32, 3), self._lead(done, np.float32, 3)
+        noise = None if noise is None else self._lead(noise, np.float32, 5 if self.algo == self.SAC else 4)
+        S, B = obs.shape[1], obs.shape[2]
+        q1v, q2v, l1, l2, lp, npol = self._out_buffers(S, B)
         check(self.lib.b200rl_offpolicy_train(self.h, C.byref(hp), S, B, _ptr(obs), _ptr(act), _ptr(rew), _ptr(next_obs),
                                               _ptr(done), _ptr(noise), _ptr(q1v), _ptr(q2v), _ptr(l1), _ptr(l2), _ptr(lp),
                                               C.byref(npol), current_stream_handle()), "offpolicy_train")
@@ -483,39 +523,58 @@ class OffPolicyEngine:
         """``train_gather`` with the indices and the smoothing noise drawn on the device (Philox keyed by ``seed``, block
         ``call``); ``ring_size`` live rows, logical row u at physical ``(ring_start + u) % rows``.  Opt-in: the streams
         are not the reference's numpy / torch ones."""
-        q1v, q2v = np.zeros((S, B), np.float32), np.zeros((S, B), np.float32)
-        l1, l2, lp = np.zeros(S, np.float32), np.zeros(S, np.float32), np.zeros(max(S, 1), np.float32)
-        npol = C.c_int32()
-        ptrs = [C.c_void_p(t.data_ptr()) for t in columns]
-        check(self.lib.b200rl_offpolicy_train_gather_rng(self.h, C.byref(hp), S, B, *ptrs, int(rows), int(ring_start),
-                                                         int(ring_size), int(seed) & (2 ** 64 - 1), int(call), _ptr(q1v),
-                                                         _ptr(q2v), _ptr(l1), _ptr(l2), _ptr(lp), C.byref(npol),
-                                                         current_stream_handle()), "offpolicy_train_gather_rng")
+        return self.train_gather_rng_group(hp, [(columns, rows)], [ring_start], [ring_size], S, B, [seed], [call])
+
+    def train_gather_rng_group(self, hp, replays, ring_starts, ring_sizes, S: int, B: int, seeds, calls):
+        """``train_gather_rng`` for every learner: ``replays`` = K (columns, rows) pairs, the other sequences K long;
+        learner z's draws are those of a solo engine keyed by (seeds[z], calls[z])."""
+        rb = self._replays(replays)
+        ring = [np.asarray(x, np.int64).reshape(-1) for x in (ring_starts, ring_sizes)]
+        keys = [np.asarray([int(x) & (2 ** 64 - 1) for x in v], np.uint64) for v in (seeds, calls)]
+        q1v, q2v, l1, l2, lp, npol = self._out_buffers(S, B)
+        check(self.lib.b200rl_offpolicy_train_gather_rng_group(self.h, C.byref(hp), S, B, rb, *[_ptr(x) for x in ring],
+                                                               *[_ptr(x) for x in keys], _ptr(q1v), _ptr(q2v), _ptr(l1),
+                                                               _ptr(l2), _ptr(lp), C.byref(npol), current_stream_handle()),
+              "offpolicy_train_gather_rng")
         return self._outputs(S, q1v, q2v, l1, l2, lp, npol)
 
     def get_draws(self, S: int, B: int, with_noise: bool = True):
         """(physical rows [S,B] int64, noise [S,B,A] (SAC: [S,2,B,A]) float32 or None) of the last train_gather /
-        train_gather_rng call."""
-        idx = np.empty((S, B), np.int64)
+        train_gather_rng call; a group: both with a leading [K] axis."""
+        idx = np.empty((self.K, S, B), np.int64)
         if self.algo == self.SAC:
-            shape = (S, 2, B, self.policy_sizes[-1] // 2)
+            shape = (self.K, S, 2, B, self.policy_sizes[-1] // 2)
         else:
-            shape = (S, B, self.policy_sizes[-1])
+            shape = (self.K, S, B, self.policy_sizes[-1])
         noise = np.empty(shape, np.float32) if with_noise else None
         check(self.lib.b200rl_offpolicy_get_draws(self.h, S, B, _ptr(idx), _ptr(noise), current_stream_handle()), "get_draws")
+        if self.K == 1:
+            return idx[0], None if noise is None else noise[0]
         return idx, noise
+
+    def _replays(self, replays):
+        if len(replays) != self.K:
+            raise ValueError(f"expected the replay columns of {self.K} learners, got {len(replays)}")
+        rb = (_lib.OffPolicyReplay * self.K)()
+        for z, (columns, rows) in enumerate(replays):
+            rb[z] = _lib.OffPolicyReplay(*[t.data_ptr() for t in columns], int(rows))
+        return rb
 
     def train_gather(self, hp, columns, rows: int, idx, noise=None):
         """Minibatches gathered on the device: ``columns`` = CUDA float32 tensors (obs [rows,O], act [rows,A], rew [rows],
         next_obs [rows,O], done [rows]) of a device-resident replay buffer, ``idx`` [S,B] int64 physical rows (host)."""
-        idx = _c(idx, np.int64)
-        noise = None if noise is None else _c(noise, np.float32)
-        S, B = idx.shape
-        q1v, q2v = np.zeros((S, B), np.float32), np.zeros((S, B), np.float32)
-        l1, l2, lp = np.zeros(S, np.float32), np.zeros(S, np.float32), np.zeros(max(S, 1), np.float32)
-        npol = C.c_int32()
-        ptrs = [C.c_void_p(t.data_ptr()) for t in columns]
-        check(self.lib.b200rl_offpolicy_train_gather(self.h, C.byref(hp), S, B, *ptrs, int(rows), _ptr(idx), _ptr(noise),
-                                                     _ptr(q1v), _ptr(q2v), _ptr(l1), _ptr(l2), _ptr(lp), C.byref(npol),
-                                                     current_stream_handle()), "offpolicy_train_gather")
+        return self.train_gather_group(hp, [(columns, rows)], idx, noise)
+
+    def train_gather_group(self, hp, replays, idx, noise=None):
+        """``train_gather`` for every learner: ``replays`` = K (columns, rows) pairs, one replay buffer per learner;
+        ``idx`` [K,S,B], ``noise`` [K,S,B,A] (SAC [K,S,2,B,A]); a solo engine also takes them without the [K] axis."""
+        rb = self._replays(replays)
+        idx = self._lead(idx, np.int64, 3)
+        noise = None if noise is None else self._lead(noise, np.float32, 5 if self.algo == self.SAC else 4)
+        S, B = idx.shape[1], idx.shape[2]
+        q1v, q2v, l1, l2, lp, npol = self._out_buffers(S, B)
+        check(self.lib.b200rl_offpolicy_train_gather_group(self.h, C.byref(hp), S, B, rb, _ptr(idx), _ptr(noise),
+                                                           _ptr(q1v), _ptr(q2v), _ptr(l1), _ptr(l2), _ptr(lp),
+                                                           C.byref(npol), current_stream_handle()),
+              "offpolicy_train_gather")
         return self._outputs(S, q1v, q2v, l1, l2, lp, npol)

@@ -140,7 +140,7 @@ struct b200rl_onpolicy {
   float* grad_all = nullptr; // [Pp + Pv + 16]: both gradients + both scalar tails, the ONE all-reduce buffer per iteration
   float* snap = nullptr;     // snapshot [3 Pp + 3 Pv + Pp]: restored when a fused update must be redone
   float* h_trip = nullptr;   // pinned
-  int last_fused = 0;        // the last update ran on the fused path (diagnostics)
+  int last_fused = 0;        // the last update / gradient stage ran on the fused path (which buffer device_view shows)
   // trainable log_std (policies/gaussian_policy.py:25-37 with log_std inside the optimizer): the policy vector is then
   // [network parameters | log_std] for set / get_params, Adam and the gradient; policy steps run on the fp32 kernel
   int train_log_std = 0;
@@ -1092,7 +1092,9 @@ extern "C" int b200rl_onpolicy_run_stage(b200rl_onpolicy* h, const char* stage, 
   if (strcmp(stage, "old_logp") == 0)
     return launch_fused(h, h->cfg.policy, B200RL_LOSS_EVAL, h->cfg.dist, h->old_pol, h->obs, h->n_rows, n_glob, 0.0,
                         false, false, h->old_logp, false, nullptr, s);
+  // the gradient stages leave device_view("policy_grad" / "value_grad") on the buffer they write
   if (strcmp(stage, "policy_grad") == 0) {
+    h->last_fused = 0;
     if (launch_fused(h, h->cfg.policy, B200RL_LOSS_PPO_CLIP, h->cfg.dist, h->pol, h->obs, h->n_rows, n_glob,
                      hp->clip_range, true, true, nullptr, true, nullptr, s)) return 1;
     return b200rl_reduce_partials(h->partials, h->scalar_partials, b200rl_mlp_grid(&h->cfg.policy, h->n_rows, 1),
@@ -1102,6 +1104,7 @@ extern "C" int b200rl_onpolicy_run_stage(b200rl_onpolicy* h, const char* stage, 
     return launch_fused(h, h->cfg.policy, B200RL_LOSS_PPO_CLIP, h->cfg.dist, h->pol, h->obs, h->n_rows, n_glob,
                         hp->clip_range, true, true, nullptr, true, nullptr, s);
   if (strcmp(stage, "value_grad") == 0) {
+    h->last_fused = 0;
     if (launch_fused(h, h->cfg.value, B200RL_LOSS_MSE, B200RL_DIST_NONE, h->val, h->obs, h->n_rows, n_glob, 0.0, false,
                      false, nullptr, true, nullptr, s)) return 1;
     return b200rl_reduce_partials(h->partials, h->scalar_partials, b200rl_mlp_grid(&h->cfg.value, h->n_rows, 1), h->Pv,
@@ -1160,6 +1163,7 @@ extern "C" int b200rl_onpolicy_run_stage(b200rl_onpolicy* h, const char* stage, 
     a.P[1] = h->Pv;
     a.grad = h->grad_all;
     a.run_policy = a.run_value = 1;
+    h->last_fused = 1;
     return launch_reduce_adam3(a, s);
   }
   if (strcmp(stage, "fvp") == 0) {  // one Fisher-vector product (kernel + fixed-order reduction) on the current direction

@@ -15,6 +15,7 @@
 //   * activations never touch HBM; per-CTA weight gradients accumulate in shared memory across the CTA's tiles and
 //     are written once as partials[cta][P]; b200rl_reduce_partials sums them in a fixed order.
 //   * HBM reads per row: obs (4*O) + actions (4*A) + adv_raw (4) + old_logp (4) [policy] or target (4) [value].
+#include <atomic>
 #include <cmath>
 #include <cstdlib>
 
@@ -109,11 +110,17 @@ static int build_layout_tm(const b200rl_mlp_desc& d, bool backward, bool fvp, in
   return 0;
 }
 
-// largest tile height whose shared-memory footprint fits
+// shared memory a block may use on sm_90 (dynamic + static)
+constexpr size_t SMEM_LIMIT = 227 * 1024;
+// static shared memory of mlp_fused_kernel<tm, mode> (defined below); 0 if it cannot be queried
+static size_t fused_static_smem(int tm, int mode);
+
+// largest tile height whose shared-memory footprint (the layout plus the kernel's static arrays) fits
 int build_layout(const b200rl_mlp_desc& d, bool backward, MlpLayout* out, bool fvp = false) {
   for (int tm = TM_MAX; tm >= 16; tm >>= 1) {
     if (build_layout_tm(d, backward, fvp, tm, out)) return 2;
-    if ((size_t)out->total_floats * sizeof(float) <= 227 * 1024) return 0;
+    const size_t st = fused_static_smem(tm, fvp ? 2 : (backward ? 1 : 0));
+    if ((size_t)out->total_floats * sizeof(float) + st <= SMEM_LIMIT) return 0;
   }
   return 0;  // caller reports the size
 }
@@ -628,6 +635,25 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_fused_kernel(const FusedAr
   }
 }
 
+static size_t fused_static_smem(int tm, int mode) {
+  // bytes + 1 once known, 0 before: threads that query concurrently store the same value
+  static std::atomic<size_t> cache[3][3];
+  const int t = tm == 64 ? 0 : (tm == 32 ? 1 : 2);
+  const size_t c = cache[t][mode].load(std::memory_order_relaxed);
+  if (c != 0) return c - 1;
+  static const void* const fns[3][3] = {
+      {(const void*)mlp_fused_kernel<64, 0>, (const void*)mlp_fused_kernel<64, 1>, (const void*)mlp_fused_kernel<64, 2>},
+      {(const void*)mlp_fused_kernel<32, 0>, (const void*)mlp_fused_kernel<32, 1>, (const void*)mlp_fused_kernel<32, 2>},
+      {(const void*)mlp_fused_kernel<16, 0>, (const void*)mlp_fused_kernel<16, 1>, (const void*)mlp_fused_kernel<16, 2>}};
+  cudaFuncAttributes fa;
+  if (cudaFuncGetAttributes(&fa, fns[t][mode]) != cudaSuccess) {
+    (void)cudaGetLastError();  // no device: nothing launches, and the grid query reports that
+    return 0;
+  }
+  cache[t][mode].store(fa.sharedSizeBytes + 1, std::memory_order_relaxed);
+  return fa.sharedSizeBytes;
+}
+
 static int fused_grid(const MlpLayout& lay, int64_t n_rows) {
   const int64_t tiles = (n_rows + lay.tm - 1) / lay.tm;
   const int sms = device_sm_count();
@@ -706,10 +732,13 @@ static int launch_fused(const b200rl_mlp_loss_grad_args* a, const unsigned* run_
   k.seq = seq;
   k.total_rows = total_rows;
   k.rerun_counter = run_if != nullptr ? tc_fallback_counter_ptr() : nullptr;
+  const int mode = fvp ? 2 : (backward ? 1 : 0);
   const size_t smem_bytes = (size_t)k.lay.total_floats * sizeof(float);
-  B200RL_REQUIRE(smem_bytes <= 227 * 1024,
-                 "mlp_loss_grad: network needs %zu bytes of shared memory (> 227 KiB); too large for the fused kernel",
-                 smem_bytes);
+  const size_t static_bytes = fused_static_smem(k.lay.tm, mode);
+  B200RL_REQUIRE(smem_bytes + static_bytes <= SMEM_LIMIT,
+                 "mlp_loss_grad: network needs %zu bytes of shared memory (%zu for its layout + %zu static; > 227 KiB); "
+                 "too large for the fused kernel",
+                 smem_bytes + static_bytes, smem_bytes, static_bytes);
   const int64_t n_glob = a->n_global > 0 ? a->n_global : a->n_rows;
   k.loss = a->loss;
   k.dist = a->dist;
@@ -735,7 +764,6 @@ static int launch_fused(const b200rl_mlp_loss_grad_args* a, const unsigned* run_
   k.train_log_std = (a->train_log_std != 0 && backward && a->dist == B200RL_DIST_GAUSSIAN) ? 1 : 0;
   const int grid = fused_grid(k.lay, a->n_rows);
   B200RL_REQUIRE(grid > 0, "mlp_loss_grad: no CUDA device");
-  const int mode = fvp ? 2 : (backward ? 1 : 0);
 #define B200RL_LAUNCH_FUSED(TMV, MODEV)                                                                       \
   do {                                                                                                         \
     B200RL_CUDA(cudaFuncSetAttribute(mlp_fused_kernel<TMV, MODEV>, cudaFuncAttributeMaxDynamicSharedMemorySize, \

@@ -416,9 +416,8 @@ int b200rl_offpolicy_get_draws(b200rl_offpolicy* h, int32_t S, int32_t B, int64_
  *               from the next step on; learn_alpha = 0: alpha is the fixed value
  *   polyak:     Q1targ, Q2targ every step.  hparams.policy_delay / use_target_noise / target_noise_* do not apply.
  * train / train_gather take noise [S, 2, B, A] (per step the draw for s', then the one for s), required; train_gather_rng
- * draws it on the device and get_draws returns it in the same layout.  policy_losses has S entries.  The persistent
- * step kernel (B200RL_OFFPOLICY_MEGAKERNEL=1) does not apply: SAC runs as a CUDA graph, or as plain launches with
- * B200RL_OFFPOLICY_GRAPH=0.
+ * draws it on the device and get_draws returns it in the same layout.  policy_losses has S entries.  SAC runs as a
+ * CUDA graph, or as plain launches with B200RL_OFFPOLICY_GRAPH=0.
  * ------------------------------------------------------------------------------------------------------------ */
 typedef struct {
   double alpha;                 /* the fixed entropy coefficient (learn_alpha = 0) */
@@ -451,9 +450,8 @@ int b200rl_offpolicy_sac_outputs(b200rl_offpolicy* h, int32_t S, float* log_prob
  * returns values [K, S, B], losses [K, S] and policy_losses [K, S] (the first *n_policy_updates of each row; the
  * policy-delay schedule is shared); get_draws and sac_outputs likewise.  train_gather, train_gather_rng, set_alpha and
  * get_alpha are the group calls below with K = 1 and refuse K > 1; the per-network accessors (set_params, get_params,
- * set_adam, get_adam) refuse K > 1: a group's state moves as the blob.  The persistent step kernel
- * (B200RL_OFFPOLICY_MEGAKERNEL=1) does not apply to K > 1: a group runs as a CUDA graph, or as plain launches with
- * B200RL_OFFPOLICY_GRAPH=0.
+ * set_adam, get_adam) refuse K > 1: a group's state moves as the blob.  A group runs as a CUDA graph, or as plain
+ * launches with B200RL_OFFPOLICY_GRAPH=0.
  * ------------------------------------------------------------------------------------------------------------ */
 typedef struct {
   const float *obs, *act, *rew, *next_obs, *done; /* device replay columns, as for b200rl_offpolicy_train_gather */

@@ -11,13 +11,13 @@
 // GEMMs are one generic 32x32x32 shared-memory-tiled fp32 kernel in three operand arrangements (forward NT, dX NN,
 // dW TN) with the activation derivative fused into the operand load, so activations are never rewritten; torch.cat of
 // [s | a] is a split operand, the target-smoothing noise an epilogue.  File map: tile function and elementwise kernels;
-// the opt-in persistent step kernel (offpolicy_mega_kernel) and its program builder; the engine (one state slab);
-// enqueue_steps = the S steps as a four-stream dependency graph (captured once, replayed); the three entry points
+// the engine (one state slab); enqueue_steps = the S steps as a four-stream dependency graph (captured once, replayed,
+// or issued as plain launches with B200RL_OFFPOLICY_GRAPH=0); the three entry points
 // train (host-staged minibatches), train_gather (host-drawn indices, device gather), train_gather_rng (device draws).
 // Learner groups (create_group): K learners in K arenas at a fixed stride, every kernel above with a LANES
 // instantiation that serves all of them in one launch; a K = 1 engine runs the solo instantiations.
 // SAC (config algo = 1) is a second step program on the same engine: its head / soft-loss / temperature kernels and
-// enqueue_sac_steps, run as a captured graph or as plain launches (the persistent step kernel does not apply to it).
+// enqueue_sac_steps, run as a captured graph or as plain launches like the TD3 / DDPG steps.
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -61,7 +61,7 @@ struct GemmArgs {
   const float* Y; int ldy; int act;  // MODE 0: output activation; MODE 1/2: activation whose derivative gates A
   int M, N, K;
   float* dbias;                      // MODE 2 only
-  // MODE 0 extras (the persistent step kernel fuses the small elementwise kernels into its GEMMs):
+  // the critics' [s | a] input and the target-policy smoothing, fused into the operand load and the epilogue:
   const float* A2; int lda2; int ksplit;  // A2 != NULL: columns >= ksplit of A (MODE 0) / of B (MODE 2) come from
                                           // A2[:, col - ksplit]: the operand is torch.cat([left, A2], -1), never built
   const float* eps; float sigma, clipv, limit;  // eps != NULL: target-policy smoothing on the output (td3.py:326-332)
@@ -72,8 +72,9 @@ struct GemmArgs {
 // multiplied out of shared memory tile by tile.
 typedef float GemmTile[GK][GT + 2];
 
-template <int MODE, int KT>  // KT = k-tiles fetched ahead (registers: 8 per k-tile)
+template <int MODE>
 __device__ __forceinline__ void gemm_tile(const GemmArgs& g, int bx, int by, GemmTile& As, GemmTile& Bs) {
+  constexpr int KT = 8;  // k-tiles fetched ahead (registers: 8 per k-tile): K = 256 is ONE round of loads
   const int tid = threadIdx.x;
   const int m0 = by * GT, n0 = bx * GT;
   const int tm = (tid / 16) * 2, tn = (tid % 16) * 2;  // 16 x 16 threads, 2 x 2 outputs each
@@ -191,9 +192,9 @@ __global__ void __launch_bounds__(GTHREADS) gemm_kernel(const GemmArgs g, size_t
     a.dbias = lane_ptr(a.dbias, off);
     a.A2 = lane_ptr(a.A2, off);
     a.eps = lane_ptr(a.eps, off);
-    gemm_tile<MODE, 8>(a, blockIdx.x, blockIdx.y, As, Bs);
+    gemm_tile<MODE>(a, blockIdx.x, blockIdx.y, As, Bs);
   } else {
-    gemm_tile<MODE, 8>(g, blockIdx.x, blockIdx.y, As, Bs);  // K = 256 is ONE round of loads
+    gemm_tile<MODE>(g, blockIdx.x, blockIdx.y, As, Bs);
   }
 }
 
@@ -346,53 +347,9 @@ __global__ void polyak_kernel(const PolyakArgs a, float rho, float one_minus_rho
   }
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// The persistent step kernel.  A train() call of S steps is ~46 S small dependent kernels; even replayed as a CUDA
-// graph each costs a launch-to-launch gap (~200 us per TD3 step at B = 256, measured on B200).  Here the SAME tile code runs as ONE
-// cooperative launch: the host compiles the S steps into a program of ops grouped into PHASES (ops of a phase are
-// independent: the four critics' forward passes of a layer, dW and dX of a layer, ...), every CTA walks the phases,
-// takes virtual blocks `blockIdx.x, + gridDim.x, ...` of the phase's ops, and a grid barrier separates phases (~18 per
-// TD3 step instead of ~46 launches).  The GEMM tiles are the functions above, so the arithmetic -- tile shapes,
-// summation order, Adam's operation order -- is that of the launch-per-kernel path, which stays as the A/B reference
-// (B200RL_OFFPOLICY_MEGAKERNEL=0) and must give bit-identical results.  concat / target smoothing are fused into the
-// GEMMs' operand load and epilogue (GemmArgs: A2 / eps), the TD target into the loss op.
-// ---------------------------------------------------------------------------------------------------------------
-enum MkType : int { MK_GEMM_NT = 0, MK_GEMM_NN = 1, MK_GEMM_TN = 2, MK_TD_LOSS = 3, MK_POLICY_LOSS = 4, MK_ADAM = 5,
-                    MK_POLYAK = 6, MK_FILL = 7 };
-
-struct MkOp {
-  int type;
-  int n_vb;    // virtual blocks of this op
-  int grid_x;  // GEMM: tiles along N (vb = by * grid_x + bx)
-  int n;       // elementwise ops: element count
-  GemmArgs g;
-  // MK_TD_LOSS: q, rew, done, qt1, qt2 (NULL: single target critic) -> dq, loss_out, q_copy;  f0 = gamma
-  // MK_POLICY_LOSS: q -> loss_out  (dq is the constant -1/B, filled once per program by MK_FILL)
-  // MK_ADAM: params(o0) grad(p0) m(o1) v(o2), f0 = 1-b1, f1 = b2, f2 = 1-b2, f3 = eps, table + table_idx
-  // MK_POLYAK: target(o0) param(p0), f0 = rho, f1 = 1 - rho;   MK_FILL: o0[0..n) = f0
-  const float *p0, *p1, *p2, *p3, *p4;
-  float *o0, *o1, *o2;
-  float f0, f1, f2, f3;
-  const float2* table;
-  int table_idx;
-  int pad;
-};
-
-struct MkPhase {
-  int op0, n_ops, total_vb, pad;
-};
-// The program in device memory: one fixed-size block per phase, so that a CTA can stage the NEXT phase's descriptors
-// into shared memory with cp.async while it works on the current one (descriptor reads are off the critical path).
-constexpr int MK_MAX_OPS = 8;
-struct __align__(16) MkBlock {
-  MkPhase hdr;
-  MkOp ops[MK_MAX_OPS];
-};
-static_assert(sizeof(MkBlock) % 16 == 0, "MkBlock is copied in 16-byte pieces");
-
-// mean((q - y)^2) / -mean(q) exactly as q_loss_kernel sums them: per-thread partial over a stride of the block size, a
-// shuffle tree per warp, the warp totals in warp order
-__device__ __forceinline__ void mk_block_mean(double acc, int n, float* loss_out, double* red) {
+// *loss_out = (sum of every thread's `acc`) / n, summed as q_loss_kernel sums: a shuffle tree per warp, then the warp
+// totals in warp order
+__device__ __forceinline__ void block_mean(double acc, int n, float* loss_out, double* red) {
   acc = warp_sum(acc);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
   __syncthreads();
@@ -400,97 +357,6 @@ __device__ __forceinline__ void mk_block_mean(double acc, int n, float* loss_out
     double t = 0.0;
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
     *loss_out = (float)(t / (double)n);
-  }
-}
-
-__global__ void __launch_bounds__(GTHREADS, 2) offpolicy_mega_kernel(const MkBlock* __restrict__ prog, int n_phases,
-                                                                      unsigned* bar) {
-  __shared__ GemmTile As, Bs;
-  __shared__ double red[32];
-  __shared__ MkBlock s_blk[2];
-  const unsigned n_cta = gridDim.x;
-  constexpr int PIECES = (int)(sizeof(MkBlock) / 16);
-  auto stage = [&](int ph) {  // asynchronous: lands while this CTA works; completed before the phase barrier
-    if (ph < n_phases) {
-      const char* src = reinterpret_cast<const char*>(prog + ph);
-      const uint32_t dst = (uint32_t)__cvta_generic_to_shared(&s_blk[ph & 1]);
-      for (int i = threadIdx.x; i < PIECES; i += GTHREADS)
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + 16u * i), "l"(src + 16 * i) : "memory");
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-  };
-  stage(0);
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
-  __syncthreads();
-  for (int ph = 0; ph < n_phases; ++ph) {
-    const MkBlock& blk = s_blk[ph & 1];
-    stage(ph + 1);
-    const int total_vb = blk.hdr.total_vb;
-    for (int vb = blockIdx.x; vb < total_vb; vb += (int)n_cta) {
-      int o = 0, local = vb;
-      while (local >= blk.ops[o].n_vb) {
-        local -= blk.ops[o].n_vb;
-        ++o;
-      }
-      const MkOp& op = blk.ops[o];
-      const int type = op.type;
-      if (type <= MK_GEMM_TN) {
-        const int bx = local % op.grid_x, by = local / op.grid_x;
-        // four k-tiles ahead: two CTAs per SM leave 128 registers per thread
-        if (type == MK_GEMM_NT) gemm_tile<0, 4>(op.g, bx, by, As, Bs);
-        else if (type == MK_GEMM_NN) gemm_tile<1, 4>(op.g, bx, by, As, Bs);
-        else gemm_tile<2, 4>(op.g, bx, by, As, Bs);
-      } else if (type == MK_TD_LOSS) {  // q_loss_kernel of one critic
-        const int n = op.n;
-        const float inv = 1.0f / (float)n;
-        double acc = 0.0;
-        for (int i = threadIdx.x; i < n; i += blockDim.x) {
-          const float qi = op.p0[i];
-          op.o2[i] = qi;
-          const float d = qi - td_target(op.p1[i], op.p2[i], op.p3[i], op.p4, i, op.f0);
-          acc += (double)d * (double)d;
-          op.o0[i] = (2.f * d) * inv;
-        }
-        mk_block_mean(acc, n, op.o1, red);
-      } else if (type == MK_POLICY_LOSS) {
-        double acc = 0.0;
-        for (int i = threadIdx.x; i < op.n; i += blockDim.x) acc -= (double)op.p0[i];
-        mk_block_mean(acc, op.n, op.o1, red);
-      } else if (type == MK_ADAM) {
-        const int i = local * GTHREADS + threadIdx.x;
-        if (i < op.n) {
-          const float2 t = op.table[op.table_idx];
-          const float g = op.p0[i];
-          float m = op.o1[i], v = op.o2[i];
-          m = m + op.f0 * (g - m);                       // the arithmetic of adam_step_kernel (adam.cu)
-          v = v * op.f1 + op.f2 * (g * g);
-          const float denom = sqrtf(v) / t.y + op.f3;
-          op.o1[i] = m;
-          op.o2[i] = v;
-          op.o0[i] = op.o0[i] - t.x * (m / denom);
-        }
-      } else if (type == MK_POLYAK) {
-        const int i = local * GTHREADS + threadIdx.x;
-        if (i < op.n) op.o0[i] = op.f0 * op.o0[i] + op.f1 * op.p0[i];
-      } else {  // MK_FILL
-        const int i = local * GTHREADS + threadIdx.x;
-        if (i < op.n) op.o0[i] = op.f0;
-      }
-      __syncthreads();  // the tiles / the reduction scratch are reused by the next virtual block
-    }
-    // grid barrier: a monotonically increasing ticket counter (every CTA is resident: cooperative launch)
-    asm volatile("cp.async.wait_group 0;" ::: "memory");  // the next phase's descriptors have landed
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      __threadfence();
-      const unsigned target = (unsigned)(ph + 1) * n_cta;
-      atomicAdd(bar, 1u);
-      unsigned seen;
-      do {
-        asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(bar) : "memory");
-      } while (seen < target);
-    }
-    __syncthreads();
   }
 }
 
@@ -550,7 +416,7 @@ __global__ void __launch_bounds__(GTHREADS) sac_q_loss_kernel(const float* q, co
     acc += (double)d * (double)d;
     dq[i] = (2.f * d) * inv;
   }
-  mk_block_mean(acc, n, loss_out, red);
+  block_mean(acc, n, loss_out, red);
 }
 
 // One CTA: loss = mean(alpha log pi - min(q1, q2)) at a = pi(s), the per-row gradients w.r.t. q1 and q2 (torch.min's
@@ -578,8 +444,8 @@ __global__ void __launch_bounds__(GTHREADS) sac_policy_loss_kernel(const float* 
     dq1[i] = -(w1 * inv);
     dq2[i] = -((1.f - w1) * inv);
   }
-  mk_block_mean(acc, n, loss_out, red);
-  mk_block_mean(acc_lp, n, logp_mean_out, red_lp);
+  block_mean(acc, n, loss_out, red);
+  block_mean(acc_lp, n, logp_mean_out, red_lp);
 }
 
 // One thread per (row, j): the gradient of the policy loss w.r.t. the network output [mu | log_std], from
@@ -692,8 +558,9 @@ struct b200rl_offpolicy {
   // per-step workspace
   float* acts[5][B200RL_MAX_LAYERS + 1];  // activation stacks [B, width]: 0 scratch/target (Q1 side), 1 Q1, 2 policy,
                                           // 3 target Q2, 4 Q2 (the twin critic runs on a second stream)
-  float* acts_tq[B200RL_MAX_LAYERS + 1];  // the persistent kernel: Q1's target critic gets a stack of its own (there the
-                                          // critics' first layers run beside the target policy's, which owns stack 0)
+  float* acts_tq[B200RL_MAX_LAYERS + 1];  // Q1's target critic gets a stack of its own: in stack 0, a critic deeper than
+                                          // the policy would overwrite the target action, which the twin target
+                                          // critic on s2 may still be reading
   float *x_cat = nullptr, *x_cat2 = nullptr, *qt1 = nullptr, *qt2 = nullptr, *dq = nullptr;
   float *dbuf0 = nullptr, *dbuf1 = nullptr;  // gradient ping-pong [B, maxw]
   float *dbuf2 = nullptr, *dbuf3 = nullptr, *dq2 = nullptr;  // the same for the twin critic's branch
@@ -713,13 +580,6 @@ struct b200rl_offpolicy {
   cudaGraphExec_t graph = nullptr;
   b200rl_offpolicy_hparams graph_hp;
   int graph_S = -1, graph_B = -1, graph_npol = 0, graph_launches = 0;
-  // the persistent step kernel's program for (S, B, hyper-parameters), see offpolicy_mega_kernel
-  MkBlock* mk_prog = nullptr;
-  unsigned* mk_bar = nullptr;
-  float* dq_pol = nullptr;  // [max_minibatch] the constant -1/B gradient of the policy loss
-  b200rl_offpolicy_hparams mk_hp;
-  int mk_S = -1, mk_B = -1, mk_npol = 0, mk_n_phases = 0, mk_grid = 0;
-  size_t mk_prog_cap = 0;
   float* state = nullptr;  // parameters + Adam state of every network, blob order (see b200rl_offpolicy_create)
   int64_t state_n = 0;
   // SAC (cfg.algo == 1): network 3 is absent; h->eps holds [S, 2, B, A] (the draw for s', then the one for s)
@@ -954,8 +814,6 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
   rc |= oalloc(h, &h->dbuf2, B * (size_t)maxw);
   rc |= oalloc(h, &h->dbuf3, B * (size_t)maxw);
   rc |= oalloc(h, &h->dq2, B);
-  rc |= oalloc(h, &h->dq_pol, B);
-  rc |= oalloc(h, &h->mk_bar, 1);
   rc |= oalloc(h, &h->out_q1, S * B);
   rc |= oalloc(h, &h->out_q2, S * B);
   rc |= oalloc(h, &h->out_l1, S);
@@ -1011,7 +869,6 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
 extern "C" void b200rl_offpolicy_destroy(b200rl_offpolicy* h) {
   if (!h) return;
   if (h->graph) cudaGraphExecDestroy(h->graph);
-  if (h->mk_prog) cudaFree(h->mk_prog);
   if (h->ev) cudaEventDestroy(h->ev);
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
   if (h->ev_join) cudaEventDestroy(h->ev_join);
@@ -1427,289 +1284,6 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
   return 0;
 }
 
-// ---- the program of the persistent step kernel: enqueue_steps restated as ops in dependency phases ----------------
-namespace {
-struct MkBuilder {
-  std::vector<MkOp> ops;
-  std::vector<MkPhase> phases;
-  int op0 = 0;
-  void end_phase() {
-    if ((int)ops.size() == op0) return;
-    MkPhase p{};
-    p.op0 = op0;
-    p.n_ops = (int)ops.size() - op0;
-    for (int i = op0; i < (int)ops.size(); ++i) p.total_vb += ops[i].n_vb;
-    phases.push_back(p);
-    op0 = (int)ops.size();
-  }
-  void gemm(int mode, const GemmArgs& g) {
-    MkOp o{};
-    o.type = mode;
-    o.g = g;
-    o.grid_x = (g.N + GT - 1) / GT;
-    o.n_vb = o.grid_x * ((g.M + GT - 1) / GT);
-    ops.push_back(o);
-  }
-  void elementwise(MkOp o, int n) {
-    o.n = n;
-    o.n_vb = (n + GTHREADS - 1) / GTHREADS;
-    ops.push_back(o);
-  }
-  void single(MkOp o, int n) {
-    o.n = n;
-    o.n_vb = 1;
-    ops.push_back(o);
-  }
-};
-
-// forward layer l of a network; input = acts[0] (or the torch.cat of in_a | in_b when in_b != NULL)
-void mk_forward_layer(MkBuilder& b, const NetBuf& nb, float* const* acts, int l, int rows, const float* in_b = nullptr,
-                      int ld_b = 0, int ksplit = 0, const float* eps = nullptr, const b200rl_offpolicy_hparams* hp = nullptr) {
-  const int L = nb.d.n_layers;
-  GemmArgs g{};
-  g.A = acts[l];
-  g.lda = nb.d.sizes[l];
-  if (l == 0 && in_b != nullptr) {
-    g.lda = ksplit;  // acts[0] is the left block [rows, ksplit]
-    g.A2 = in_b;
-    g.lda2 = ld_b;
-    g.ksplit = ksplit;
-  }
-  g.B = nb.params + nb.w_off[l];
-  g.ldb = nb.d.sizes[l];
-  g.C = acts[l + 1];
-  g.ldc = nb.d.sizes[l + 1];
-  g.bias = nb.params + nb.b_off[l];
-  g.act = (l == L - 1) ? nb.d.out_act : nb.d.hidden_act;
-  g.M = rows;
-  g.N = nb.d.sizes[l + 1];
-  g.K = nb.d.sizes[l];
-  if (l == L - 1 && eps != nullptr) {
-    g.eps = eps;
-    g.sigma = (float)hp->target_noise_scale;
-    g.clipv = (float)hp->target_noise_clip;
-    g.limit = (float)hp->action_limit;
-  }
-  b.gemm(MK_GEMM_NT, g);
-}
-
-// backward layer l (net_backward's loop body): dY / ldd = the gradient entering the layer, pp = ping-pong buffers
-void mk_backward_layer(MkBuilder& b, const NetBuf& nb, float* const* acts, int l, const float* dY, int ldd, int rows,
-                       bool want_param_grads, float* dst_dx) {
-  const int L = nb.d.n_layers;
-  const int nout = nb.d.sizes[l + 1], nin = nb.d.sizes[l];
-  const int act = (l == L - 1) ? nb.d.out_act : nb.d.hidden_act;
-  const float* Y = acts[l + 1];
-  if (want_param_grads) {
-    GemmArgs g{};
-    g.A = dY; g.lda = ldd; g.Y = Y; g.ldy = nout; g.act = act;
-    g.B = acts[l]; g.ldb = nin;
-    g.C = nb.grad + nb.w_off[l]; g.ldc = nin;
-    g.M = nout; g.N = nin; g.K = rows;
-    g.dbias = nb.grad + nb.b_off[l];
-    b.gemm(MK_GEMM_TN, g);
-  }
-  if (dst_dx != nullptr) {
-    GemmArgs g{};
-    g.A = dY; g.lda = ldd; g.Y = Y; g.ldy = nout; g.act = act;
-    g.B = nb.params + nb.w_off[l]; g.ldb = nin;
-    g.C = dst_dx; g.ldc = nin;
-    g.M = rows; g.N = nin; g.K = nout;
-    b.gemm(MK_GEMM_NN, g);
-  }
-}
-
-void mk_adam(MkBuilder& b, NetBuf& nb, const float2* table, int idx, double b1, double b2, double eps) {
-  MkOp o{};
-  o.type = MK_ADAM;
-  o.o0 = nb.params; o.p0 = nb.grad; o.o1 = nb.m; o.o2 = nb.v;
-  o.f0 = (float)(1.0 - b1); o.f1 = (float)b2; o.f2 = (float)(1.0 - b2); o.f3 = (float)eps;
-  o.table = table;
-  o.table_idx = idx;
-  b.elementwise(o, (int)nb.P);
-}
-}  // namespace
-
-static int build_program(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, int* n_pol_out,
-                         cudaStream_t s) {
-  const bool td3 = h->cfg.n_q == 2;
-  const int O = h->O, A = h->A;
-  const int maxS = h->cfg.max_steps;
-  NetBuf &pi = h->net[0], &q1 = h->net[1], &q2 = h->net[2], &pit = h->net[3], &q1t = h->net[4], &q2t = h->net[5];
-  const int Lq = q1.d.n_layers, Lp = pi.d.n_layers;
-  const int nq = td3 ? 2 : 1;
-  MkBuilder b;
-  {  // the policy loss's gradient w.r.t. Q is the constant -1/B (q_loss_kernel with y == NULL)
-    MkOp o{};
-    o.type = MK_FILL;
-    o.o0 = h->dq_pol;
-    o.f0 = -(1.0f / (float)B);
-    b.elementwise(o, B);
-    b.end_phase();
-  }
-  int n_pol = 0;
-  for (int st = 0; st < S; ++st) {
-    const float* s_obs = h->obs + (size_t)st * B * O;
-    const float* s_act = h->act + (size_t)st * B * A;
-    const float* s_rew = h->rew + (size_t)st * B;
-    const float* s_nobs = h->nobs + (size_t)st * B * O;
-    const float* s_done = h->done + (size_t)st * B;
-    // ---- target action (td3.py:325-332): the smoothing noise rides on the last layer's epilogue ----
-    float* ta[B200RL_MAX_LAYERS + 1];
-    ta[0] = const_cast<float*>(s_nobs);
-    for (int l = 1; l <= Lp; ++l) ta[l] = h->acts[0][l];
-    // the critics' forward passes on [s | a] do not depend on the targets: their layers share the phases
-    float* qa[2][B200RL_MAX_LAYERS + 1];
-    for (int qi = 0; qi < nq; ++qi) {
-      qa[qi][0] = const_cast<float*>(s_obs);
-      for (int l = 1; l <= Lq; ++l) qa[qi][l] = h->acts[qi == 0 ? 1 : 4][l];
-    }
-    float* tq[2][B200RL_MAX_LAYERS + 1];
-    for (int qi = 0; qi < nq; ++qi) {
-      tq[qi][0] = const_cast<float*>(s_nobs);
-      // the target critics' hidden activations: stack 3 for the twin, and a stack of their own for Q1's target (stack 0
-      // holds the target policy's activations, which layer 0 still reads)
-      for (int l = 1; l < Lq; ++l) tq[qi][l] = qi == 0 ? h->acts_tq[l] : h->acts[3][l];
-      tq[qi][Lq] = qi == 0 ? h->qt1 : h->qt2;
-    }
-    const int lead = Lp < Lq ? Lp : Lq;  // the critics' first layers run beside the target policy's layers
-    for (int l = 0; l < Lp; ++l) {
-      mk_forward_layer(b, pit, ta, l, B, nullptr, 0, 0,
-                       (l == Lp - 1 && hp->use_target_noise) ? h->eps + (size_t)st * B * A : nullptr, hp);
-      if (l < lead)
-        for (int qi = 0; qi < nq; ++qi) mk_forward_layer(b, qi == 0 ? q1 : q2, qa[qi], l, B, s_act, A, O);
-      b.end_phase();
-    }
-    for (int l = 0; l < Lq; ++l) {
-      for (int qi = 0; qi < nq; ++qi) mk_forward_layer(b, qi == 0 ? q1t : q2t, tq[qi], l, B, ta[Lp], A, O);
-      if (l + lead < Lq)
-        for (int qi = 0; qi < nq; ++qi) mk_forward_layer(b, qi == 0 ? q1 : q2, qa[qi], l + lead, B, s_act, A, O);
-      b.end_phase();
-    }
-    // ---- TD target + MSE + dq (td3.py:337-339, 343-358) ----
-    for (int qi = 0; qi < nq; ++qi) {
-      MkOp o{};
-      o.type = MK_TD_LOSS;
-      o.p0 = qa[qi][Lq]; o.p1 = s_rew; o.p2 = s_done; o.p3 = h->qt1; o.p4 = td3 ? h->qt2 : nullptr;
-      o.f0 = (float)hp->gamma;
-      o.o0 = qi == 0 ? h->dq : h->dq2;
-      o.o1 = (qi == 0 ? h->out_l1 : h->out_l2) + st;
-      o.o2 = (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B;
-      b.single(o, B);
-    }
-    b.end_phase();
-    // ---- critics' backward: dW and dX of a layer side by side, both critics ----
-    {
-      const float* dY[2] = {h->dq, h->dq2};
-      int ldd[2] = {1, 1};
-      for (int l = Lq - 1; l >= 0; --l) {
-        for (int qi = 0; qi < nq; ++qi) {
-          float* pp[2] = {qi == 0 ? h->dbuf0 : h->dbuf2, qi == 0 ? h->dbuf1 : h->dbuf3};
-          float* dst = l > 0 ? pp[l & 1] : nullptr;
-          // layer 0 reads the concatenated input: dW0 = dZ0^T [s | a]  ->  the B operand of the TN product is split too
-          mk_backward_layer(b, qi == 0 ? q1 : q2, qa[qi], l, dY[qi], ldd[qi], B, true, dst);
-          if (l == 0) {
-            GemmArgs& g = b.ops.back().g;  // the TN op just added (no dX at layer 0): its B operand is [s | a]
-            g.ldb = O;
-            g.A2 = s_act;
-            g.lda2 = A;
-            g.ksplit = O;
-          }
-          if (dst) {
-            dY[qi] = dst;
-            ldd[qi] = q1.d.sizes[l];
-          }
-        }
-        b.end_phase();
-      }
-    }
-    for (int qi = 0; qi < nq; ++qi)
-      mk_adam(b, qi == 0 ? q1 : q2, h->adam_tab + (size_t)(1 + qi) * maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps);
-    b.end_phase();
-    // ---- delayed policy step + polyak (td3.py:244-263, 301-323) ----
-    if (st % hp->policy_delay == 0) {
-      float* pa[B200RL_MAX_LAYERS + 1];
-      pa[0] = const_cast<float*>(s_obs);
-      for (int l = 1; l <= Lp; ++l) pa[l] = h->acts[2][l];
-      for (int l = 0; l < Lp; ++l) {
-        mk_forward_layer(b, pi, pa, l, B);
-        b.end_phase();
-      }
-      float* qp[B200RL_MAX_LAYERS + 1];
-      qp[0] = const_cast<float*>(s_obs);
-      for (int l = 1; l <= Lq; ++l) qp[l] = h->acts[1][l];
-      for (int l = 0; l < Lq; ++l) {
-        mk_forward_layer(b, q1, qp, l, B, pa[Lp], A, O);  // Q1 with its freshly updated parameters (td3.py:309)
-        b.end_phase();
-      }
-      {  // -mean(Q1(s, pi(s))) is only logged; its gradient is the constant filled above
-        MkOp o{};
-        o.type = MK_POLICY_LOSS;
-        o.p0 = qp[Lq];
-        o.o1 = h->out_lp + n_pol;
-        b.single(o, B);
-      }
-      const float* dY = h->dq_pol;
-      int ldd = 1;
-      for (int l = Lq - 1; l >= 0; --l) {  // gradient w.r.t. Q1's input, parameters frozen
-        float* pp[2] = {h->dbuf0, h->dbuf1};
-        float* dst = l == 0 ? h->x_cat2 : pp[l & 1];
-        mk_backward_layer(b, q1, qp, l, dY, ldd, B, false, dst);
-        b.end_phase();
-        dY = dst;
-        ldd = q1.d.sizes[l];
-      }
-      dY = h->x_cat2 + O;  // the action columns of dQ/d[s | a]
-      ldd = O + A;
-      for (int l = Lp - 1; l >= 0; --l) {
-        float* pp[2] = {h->dbuf0, h->dbuf1};
-        float* dst = l > 0 ? pp[l & 1] : nullptr;
-        mk_backward_layer(b, pi, pa, l, dY, ldd, B, true, dst);
-        b.end_phase();
-        if (dst) {
-          dY = dst;
-          ldd = pi.d.sizes[l];
-        }
-      }
-      mk_adam(b, pi, h->adam_tab, n_pol, hp->policy_beta1, hp->policy_beta2, hp->policy_eps);
-      b.end_phase();
-      for (int k = 0; k < (td3 ? 3 : 2); ++k) {
-        MkOp o{};
-        o.type = MK_POLYAK;
-        o.o0 = h->net[3 + k].params;
-        o.p0 = h->net[k].params;
-        o.f0 = (float)hp->polyak_rho;
-        o.f1 = (float)(1.0 - hp->polyak_rho);
-        b.elementwise(o, (int)h->net[k].P);
-      }
-      b.end_phase();
-      ++n_pol;
-    }
-  }
-  *n_pol_out = n_pol;
-  // upload: one fixed-size block per phase
-  std::vector<MkBlock> prog(b.phases.size());
-  for (size_t i = 0; i < b.phases.size(); ++i) {
-    const MkPhase& ph = b.phases[i];
-    B200RL_REQUIRE(ph.n_ops <= MK_MAX_OPS, "offpolicy_train: a phase of %d ops exceeds the block size", ph.n_ops);
-    memset(&prog[i], 0, sizeof(MkBlock));
-    prog[i].hdr = ph;
-    for (int k = 0; k < ph.n_ops; ++k) prog[i].ops[k] = b.ops[ph.op0 + k];
-    for (int k = ph.n_ops; k < MK_MAX_OPS; ++k) prog[i].ops[k].n_vb = 0x7fffffff;  // the op search stops here at the latest
-  }
-  if (prog.size() > h->mk_prog_cap) {
-    if (h->mk_prog) cudaFree(h->mk_prog);
-    h->mk_prog = nullptr;
-    h->mk_prog_cap = 0;
-    B200RL_CUDA(cudaMalloc(reinterpret_cast<void**>(&h->mk_prog), prog.size() * sizeof(MkBlock)));
-    h->mk_prog_cap = prog.size();
-  }
-  B200RL_CUDA(cudaMemcpyAsync(h->mk_prog, prog.data(), prog.size() * sizeof(MkBlock), cudaMemcpyHostToDevice, s));
-  B200RL_CUDA(cudaStreamSynchronize(s));  // the host vectors go away; the launches behind are ordered on `s` anyway
-  h->mk_n_phases = (int)b.phases.size();
-  return 0;
-}
-
 // SAC engines: b200rl_offpolicy_set_sac must have been called, and the host paths must hand over the [S, 2, B, A] draws
 static int sac_ready(const b200rl_offpolicy* h, bool noise_given, const char* what) {
   if (!h->sac) return 0;
@@ -1749,40 +1323,9 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
                                 tab_n * sizeof(float2), h->K, cudaMemcpyHostToDevice, s));
 
   int n_pol = 0;
-  // opt-in: on B200 it measured 12.1 ms per 50 TD3 steps against 11.1 ms for the graph replay (B = 256, 256-wide nets) -- the
-  // 32 x 32 fp32 tiles themselves, two per SM in the phases that merge four networks, are the cost, not the launches.
-  // SAC and learner groups have no program for it and always take the graph (or plain launches).
-  const char* menv = getenv("B200RL_OFFPOLICY_MEGAKERNEL");
-  const bool use_mega = menv != nullptr && menv[0] == '1' && !h->sac && h->K == 1;
   const char* genv = getenv("B200RL_OFFPOLICY_GRAPH");
   const bool use_graph = !(genv != nullptr && genv[0] == '0');
-  if (use_mega) {
-    // ONE cooperative launch runs all S steps (see offpolicy_mega_kernel); the program is rebuilt only when the shape
-    // or the hyper-parameters change -- minibatches and Adam's scalars are read from device buffers
-    if (h->mk_S != S || h->mk_B != B || memcmp(&h->mk_hp, hp, sizeof(*hp)) != 0) {
-      B200RL_CUDA(cudaStreamSynchronize(s));  // the previous program may still be in use
-      if (build_program(h, hp, S, B, &n_pol, s)) return 1;
-      h->mk_S = S;
-      h->mk_B = B;
-      h->mk_hp = *hp;
-      h->mk_npol = n_pol;
-      if (h->mk_grid == 0) {
-        int per_sm = 0;
-        B200RL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, offpolicy_mega_kernel, GTHREADS, 0));
-        B200RL_REQUIRE(per_sm >= 1, "offpolicy_train: the step kernel does not fit an SM");
-        h->mk_grid = (per_sm > 2 ? 2 : per_sm) * device_sm_count();
-      }
-    }
-    n_pol = h->mk_npol;
-    B200RL_CUDA(cudaMemsetAsync(h->mk_bar, 0, sizeof(unsigned), s));
-    const MkBlock* prog = h->mk_prog;
-    int n_phases = h->mk_n_phases;
-    unsigned* bar = h->mk_bar;
-    void* kargs[] = {&prog, &n_phases, &bar};
-    B200RL_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(offpolicy_mega_kernel), dim3(h->mk_grid),
-                                            dim3(GTHREADS), kargs, 0, s));
-    count_launch(1);
-  } else if (!use_graph) {
+  if (!use_graph) {
     if (h->sac) {
       if (enqueue_sac_steps(h, hp, S, B, s)) return 1;
       n_pol = S;

@@ -149,11 +149,10 @@ def test_train_vs_oracle_benchmark_shape(twin):
 
 
 @pytest.mark.parametrize("twin", [True, False])
-def test_device_replay_graph_replay_and_the_persistent_kernel_match_the_staged_path(twin):
-    """b200rl_offpolicy_train_gather (replay columns in HBM, only indices uploaded), the CUDA-graph replay of the
-    S-step loop and the persistent step kernel (one cooperative launch for all S steps, concat / target smoothing /
-    TD target fused into its GEMM tiles) give BIT-IDENTICAL results to host-staged minibatches run with plain launches
-    of one kernel per operation.  TD3 (twin critics, delayed policy step, smoothing noise) and DDPG."""
+def test_device_replay_and_graph_replay_match_the_staged_path(twin):
+    """b200rl_offpolicy_train_gather (replay columns in HBM, only indices uploaded) and the CUDA-graph replay of the
+    S-step loop give BIT-IDENTICAL results to host-staged minibatches run with plain launches of one kernel per
+    operation.  TD3 (twin critics, delayed policy step, smoothing noise) and DDPG."""
     import os
     from rl_replicas_b200.experience import Experience
     rng = np.random.default_rng(3)
@@ -170,17 +169,16 @@ def test_device_replay_graph_replay_and_the_persistent_kernel_match_the_staged_p
     ex.dones = [[bool(x) for x in (rng.random(n) < 0.01)]]
     ex.last_observations = [obs[n]]
 
-    def run(device_replay, graph, mega):
+    def run(device_replay, graph):
         os.environ["B200RL_OFFPOLICY_GRAPH"] = "1" if graph else "0"
-        os.environ["B200RL_OFFPOLICY_MEGAKERNEL"] = "1" if mega else "0"
         algo, rb = build(twin, H, p0, [q10, q20] if twin else [q10])
         rb.add_experience(ex)
         algo.use_device_replay = device_replay  # False: minibatches gathered on the host and uploaded
         outs = []
-        for call in range(3):  # the 2nd and 3rd calls replay the captured graph / the compiled program
+        for call in range(3):  # the 2nd call replays the captured graph
             np.random.seed(10 + call)
             torch.manual_seed(10 + call)
-            algo.train(rb, S + (call == 2), B)  # the third call changes the shape: graph / program are rebuilt
+            algo.train(rb, S + (call == 2), B)  # the third call changes the shape: the graph is recaptured
             outs.append(algo.last_train_output)
         qs = (algo.q_function_1, algo.q_function_2) if twin else (algo.q_function,)
         tq = (algo.target_q_function_1, algo.target_q_function_2) if twin else (algo.target_q_function,)
@@ -188,18 +186,16 @@ def test_device_replay_graph_replay_and_the_persistent_kernel_match_the_staged_p
         return outs, nets
 
     try:
-        ref_outs, ref_nets = run(False, False, False)
-        for dev, graph, mega in ((True, True, False), (False, True, False), (True, False, False), (True, False, True),
-                                 (False, False, True)):
-            outs, nets = run(dev, graph, mega)
+        ref_outs, ref_nets = run(False, False)
+        for dev, graph in ((True, True), (False, True), (True, False)):
+            outs, nets = run(dev, graph)
             for a, b in zip(outs, ref_outs):
                 for k in a:
-                    np.testing.assert_array_equal(a[k], b[k], err_msg=f"{k} dev={dev} graph={graph} mega={mega}")
+                    np.testing.assert_array_equal(a[k], b[k], err_msg=f"{k} dev={dev} graph={graph}")
             for i, (a, b) in enumerate(zip(nets, ref_nets)):
-                np.testing.assert_array_equal(a, b, err_msg=f"net {i} dev={dev} graph={graph} mega={mega}")
+                np.testing.assert_array_equal(a, b, err_msg=f"net {i} dev={dev} graph={graph}")
     finally:
         os.environ.pop("B200RL_OFFPOLICY_GRAPH", None)
-        os.environ.pop("B200RL_OFFPOLICY_MEGAKERNEL", None)
 
 
 def test_train_gather_rejects_indices_outside_the_replay_columns():

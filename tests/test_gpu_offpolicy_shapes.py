@@ -64,10 +64,9 @@ class Case:
         return self.q[0] - self.policy[0]
 
 
-# The GEMM tile fetches 8 k-tiles (K = 256) per prefetch round, the persistent step kernel 4 (K = 128); B is the K of
-# the weight-gradient products.
+# The GEMM tile fetches 8 k-tiles (K = 256) per prefetch round; B is the K of the weight-gradient products.
 CASES = {
-    # K = 400: two rounds (four in the persistent kernel); N = 300 ragged; B ragged
+    # K = 400: two rounds; N = 300 ragged; B ragged
     "td3_paper": Case("td3", [17, 400, 300, 6], [23, 400, 300, 1], 100, "relu"),
     # first-layer K = 376 / 393 with the [s | a] split at column 376, inside the second round; A = 17
     "humanoid": Case("td3", [376, 256, 256, 17], [393, 256, 256, 1], 256, "relu"),
@@ -77,7 +76,7 @@ CASES = {
     "odd": Case("td3", [5, 33, 31, 2], [7, 33, 31, 1], 33, "tanh", limit=0.5, noise=0.4, clip=0.3),
     # 4 layers (no side-stream dW), dW K = 257: the bias column sums cross a prefetch round
     "deep": Case("td3", [11, 64, 48, 40, 3], [14, 96, 64, 32, 1], 257, "tanh"),
-    # policy and critics of different depth (the persistent kernel interleaves their layers)
+    # policy and critics of different depth: the target critic has more hidden layers than the target policy
     "mixed_depth": Case("ddpg", [8, 300, 2], [10, 40, 70, 50, 1], 64, "relu"),
     # dW K in four rounds; the single-CTA loss over 1000 rows
     "big_batch": Case("td3", [11, 256, 256, 3], [14, 256, 256, 1], 1000, "tanh"),
@@ -373,17 +372,16 @@ def test_sac_head_edges(edge):
 
 
 # ---- execution paths ---------------------------------------------------------------------------------------------
-PATHS = {  # name: (B200RL_OFFPOLICY_GRAPH, B200RL_OFFPOLICY_MEGAKERNEL, device gather)
-    "graph": ("1", "0", False), "gather": ("1", "0", True), "gather_plain": ("0", "0", True),
-    "persistent": ("0", "1", False), "gather_persistent": ("0", "1", True)}
+PATHS = {  # name: (B200RL_OFFPOLICY_GRAPH, device gather)
+    "graph": ("1", False), "gather": ("1", True), "gather_plain": ("0", True)}
 
 
-def run_path(case, nets, delay, graph, mega, gather, data, S, calls=2):
-    os.environ["B200RL_OFFPOLICY_GRAPH"], os.environ["B200RL_OFFPOLICY_MEGAKERNEL"] = graph, mega
+def run_path(case, nets, delay, graph, gather, data, S, calls=2):
+    os.environ["B200RL_OFFPOLICY_GRAPH"] = graph
     e = make_engine(case, nets, case.B, S)
     hp = hparams(case, delay)
     outs = []
-    for c in range(calls):  # the second call replays the captured graph / the built program
+    for c in range(calls):  # the second call replays the captured graph
         table, idx, noise = data[c]
         if gather:
             dev = [torch.as_tensor(table[k], device="cuda") for k in
@@ -401,9 +399,9 @@ def run_path(case, nets, delay, graph, mega, gather, data, S, calls=2):
 @pytest.mark.parametrize("delay", [2, 3])
 @pytest.mark.parametrize("name", ["td3_paper", "deep", "mixed_depth"])
 def test_execution_paths_are_bit_identical(name, delay):
-    """Host-staged plain launches, the CUDA graph, the device gather and the persistent step kernel give identical
-    outputs and networks over S = 5 steps with a delayed policy step, at shapes whose GEMMs need several prefetch
-    rounds (K = 400, B = 257) and with 4-layer / mixed-depth networks."""
+    """Host-staged plain launches, the CUDA graph and the device gather give identical outputs and networks over S = 5
+    steps with a delayed policy step, at shapes whose GEMMs need several prefetch rounds (K = 400, B = 257) and with
+    4-layer / mixed-depth networks."""
     case = CASES[name]
     S = 5
     rng = np.random.default_rng(11)
@@ -415,10 +413,10 @@ def test_execution_paths_are_bit_identical(name, delay):
         noise = rng.standard_normal((S, case.B, case.A)).astype(np.float32) if case.algo == "td3" else None
         data.append((table, idx, noise))
     try:
-        ref_outs, ref_blob, ref_steps = run_path(case, nets, delay, "0", "0", False, data, S)
+        ref_outs, ref_blob, ref_steps = run_path(case, nets, delay, "0", False, data, S)
         assert len(ref_outs[0]["policy_losses"]) == (S + delay - 1) // delay
-        for path, (graph, mega, gather) in PATHS.items():
-            outs, blob, steps = run_path(case, nets, delay, graph, mega, gather, data, S)
+        for path, (graph, gather) in PATHS.items():
+            outs, blob, steps = run_path(case, nets, delay, graph, gather, data, S)
             for c, (a, b) in enumerate(zip(outs, ref_outs)):
                 assert a.keys() == b.keys()
                 for k in a:
@@ -427,19 +425,19 @@ def test_execution_paths_are_bit_identical(name, delay):
             np.testing.assert_array_equal(blob, ref_blob, err_msg=f"{name} delay={delay} {path}: networks / Adam")
     finally:
         os.environ.pop("B200RL_OFFPOLICY_GRAPH", None)
-        os.environ.pop("B200RL_OFFPOLICY_MEGAKERNEL", None)
 
 
-@pytest.mark.parametrize("mega", ["0", "1"])
-def test_shape_change_on_a_live_engine_matches_a_fresh_engine(mega):
-    """An engine keeps its workspace, graph and program across calls while max_minibatch >= B: B = 256, then 100, then
-    256 again on one engine gives, call by call, what a fresh engine of exactly that B gives from the same state."""
+@pytest.mark.parametrize("graph", ["0", "1"])
+def test_shape_change_on_a_live_engine_matches_a_fresh_engine(graph):
+    """An engine keeps its workspace across calls while max_minibatch >= B, and recaptures its graph when B changes:
+    B = 256, then 100, then 256 again on one engine gives, call by call, what a fresh engine of exactly that B gives
+    from the same state.  With plain launches and with the graph."""
     case = CASES["td3_paper"]
     S = 3
     rng = np.random.default_rng(13)
     nets = init_nets(case, rng)
     try:
-        os.environ["B200RL_OFFPOLICY_MEGAKERNEL"] = mega
+        os.environ["B200RL_OFFPOLICY_GRAPH"] = graph
         live = make_engine(case, nets, 256, S)
         hp = hparams(case, 2)
         for B in (256, 100, 256):
@@ -455,9 +453,9 @@ def test_shape_change_on_a_live_engine_matches_a_fresh_engine(mega):
             fresh.set_state(blob, steps)
             want = fresh.train(hp, *cols, noise)
             for k in want:
-                np.testing.assert_array_equal(got[k], want[k], err_msg=f"B={B} mega={mega}: {k}")
-            np.testing.assert_array_equal(got_blob, fresh.get_state()[0], err_msg=f"B={B} mega={mega}: state")
+                np.testing.assert_array_equal(got[k], want[k], err_msg=f"B={B} graph={graph}: {k}")
+            np.testing.assert_array_equal(got_blob, fresh.get_state()[0], err_msg=f"B={B} graph={graph}: state")
             fresh.close()
         live.close()
     finally:
-        os.environ.pop("B200RL_OFFPOLICY_MEGAKERNEL", None)
+        os.environ.pop("B200RL_OFFPOLICY_GRAPH", None)

@@ -142,14 +142,12 @@ def test_train_matches_the_oracle(shape, learn_alpha):
 
 def test_host_staged_graph_replay_and_device_gather_are_bit_identical():
     """Plain launches on host-staged minibatches, the captured graph replayed across calls (the third call changes S
-    and recaptures), the device-replay gather, and B200RL_OFFPOLICY_MEGAKERNEL=1 (which SAC ignores) all agree bit
-    for bit."""
+    and recaptures) and the device-replay gather all agree bit for bit."""
     O, A, _, _, L, _ = SHAPES["small_tanh"]
     S, B = 6, 32
 
-    def run(device_replay, graph, mega=False):
+    def run(device_replay, graph):
         os.environ["B200RL_OFFPOLICY_GRAPH"] = "1" if graph else "0"
-        os.environ["B200RL_OFFPOLICY_MEGAKERNEL"] = "1" if mega else "0"
         algo = build("small_tanh", learn_alpha=True)
         fill(algo.replay_buffer, O, A, L, n=3000, seed=3)
         algo.use_device_replay = device_replay
@@ -165,17 +163,16 @@ def test_host_staged_graph_replay_and_device_gather_are_bit_identical():
 
     try:
         ref_outs, ref_nets = run(False, False)
-        for dev, graph, mega in ((True, True, False), (False, True, False), (True, False, False), (True, True, True)):
-            outs, nets = run(dev, graph, mega)
+        for dev, graph in ((True, True), (False, True), (True, False)):
+            outs, nets = run(dev, graph)
             for a, b in zip(outs, ref_outs):
                 assert a.keys() == b.keys()
                 for k in a:
-                    np.testing.assert_array_equal(a[k], b[k], err_msg=f"{k} dev={dev} graph={graph} mega={mega}")
+                    np.testing.assert_array_equal(a[k], b[k], err_msg=f"{k} dev={dev} graph={graph}")
             for i, (a, b) in enumerate(zip(nets, ref_nets)):
-                np.testing.assert_array_equal(a, b, err_msg=f"net {i} dev={dev} graph={graph} mega={mega}")
+                np.testing.assert_array_equal(a, b, err_msg=f"net {i} dev={dev} graph={graph}")
     finally:
         os.environ.pop("B200RL_OFFPOLICY_GRAPH", None)
-        os.environ.pop("B200RL_OFFPOLICY_MEGAKERNEL", None)
 
 
 def test_device_side_draws_replay_through_the_oracle():

@@ -9,7 +9,7 @@ import sys
 lib = sys.argv[1] if len(sys.argv) > 1 else "reinforcement-learning-replications_b200/libb200rl.so"
 sass = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True).stdout
 cols = ["UTCHMMA", "LDTM", "STTM", "UTCBAR", "UBLKCP", "SYNCS", "LDGSTS", "MUFU"]
-want = re.compile(r"gae_scan|mlp_tc|tc_probe|offpolicy_mega|reduce_adam3")
+want = re.compile(r"gae_scan|mlp_tc|tc_probe|reduce_adam3")
 print("| kernel | instructions | " + " | ".join(cols) + " |")
 print("|---|" + "---|" * (len(cols) + 1))
 for block in sass.split("Function : ")[1:]:

@@ -475,23 +475,8 @@ static void fill_tc3_net(const b200rl_mlp_desc& d, Tc3Net* n, int* P) {
   *P = mlp3_offsets(d, n->w_off, n->b_off);
 }
 
-static void fill_seg(Ra3Seg* g, float* params, float* m, float* v, int64_t step, double lr, double b1, double b2,
-                     double eps) {
-  g->params = params;
-  g->m = m;
-  g->v = v;
-  g->one_minus_b1 = (float)(1.0 - b1);
-  g->b2 = (float)b2;
-  g->one_minus_b2 = (float)(1.0 - b2);
-  adam_scalars(step, lr, b1, b2, &g->step_size, &g->bc2_sqrt);
-  g->eps = (float)eps;
-}
-
-// Iterations [0, n_iter) of the policy AND the value loop.  Every `poll` iterations the host looks at the early-stop
-// flag (one 4-byte read-back): once the policy loop has stopped, the remaining value steps are faster on the
-// two-tiles-in-flight value kernel than as the lone chain of the fused one.  Returns the iterations done in *done.
-static int run_fused_iterations(b200rl_onpolicy* h, const b200rl_ppo_hparams* hp, b200rl_allreduce_fn ar, void* user,
-                                int64_t n_glob, int K, int n_iter, cudaStream_t s, int* done) {
+// both chains of the step kernel on the engine's buffers; no early-stop flag (stop_flag = NULL)
+static Tc3Args tc3_args(const b200rl_onpolicy* h, const b200rl_ppo_hparams* hp, int64_t n_glob) {
   Tc3Args k;
   memset(&k, 0, sizeof(k));
   k.n_in = h->obs_dim;
@@ -516,11 +501,31 @@ static int run_fused_iterations(b200rl_onpolicy* h, const b200rl_ppo_hparams* hp
   k.target_absmax = h->absmax + 64;
   k.partials = h->partials;
   k.scalar_partials = h->scalar_partials;
-  k.stop_flag = h->flags;
   k.x_bad = h->trip;
   k.status = h->trip + 1;
-  k.run_policy = 1;
-  k.run_value = 1;
+  k.run_policy = k.run_value = 1;
+  return k;
+}
+
+static void fill_seg(Ra3Seg* g, float* params, float* m, float* v, int64_t step, double lr, double b1, double b2,
+                     double eps) {
+  g->params = params;
+  g->m = m;
+  g->v = v;
+  g->one_minus_b1 = (float)(1.0 - b1);
+  g->b2 = (float)b2;
+  g->one_minus_b2 = (float)(1.0 - b2);
+  adam_scalars(step, lr, b1, b2, &g->step_size, &g->bc2_sqrt);
+  g->eps = (float)eps;
+}
+
+// Iterations [0, n_iter) of the policy AND the value loop.  Every `poll` iterations the host looks at the early-stop
+// flag (one 4-byte read-back): once the policy loop has stopped, the remaining value steps are faster on the
+// two-tiles-in-flight value kernel than as the lone chain of the fused one.  Returns the iterations done in *done.
+static int run_fused_iterations(b200rl_onpolicy* h, const b200rl_ppo_hparams* hp, b200rl_allreduce_fn ar, void* user,
+                                int64_t n_glob, int K, int n_iter, cudaStream_t s, int* done) {
+  Tc3Args k = tc3_args(h, hp, n_glob);
+  k.stop_flag = h->flags;
   Ra3Args a;
   memset(&a, 0, sizeof(a));
   a.partials = h->partials;
@@ -1122,36 +1127,7 @@ extern "C" int b200rl_onpolicy_run_stage(b200rl_onpolicy* h, const char* stage, 
     }
     // one iteration of both loops on the packed observations ("pack_obs" and "preamble" first): the step kernel
     // alone, or with the reduction of its partial rows (mode 1: parameters stay as they are)
-    b200rl_ppo_hparams one = *hp;
-    one.num_policy_gradients = one.num_value_gradients = 0;
-    Tc3Args k;
-    memset(&k, 0, sizeof(k));
-    k.n_in = h->obs_dim;
-    k.dist = h->cfg.dist;
-    fill_tc3_net(h->cfg.policy, &k.net[0], &k.P[0]);
-    fill_tc3_net(h->cfg.value, &k.net[1], &k.P[1]);
-    k.params[0] = h->pol;
-    k.params[1] = h->val;
-    k.n_rows = h->n_rows;
-    k.inv_n = 1.0f / (float)n_glob;
-    k.n_glob_f = (float)n_glob;
-    k.clip_lo = (float)(1.0 - hp->clip_range);
-    k.clip_hi = (float)(1.0 + hp->clip_range);
-    k.ximg = h->ximg;
-    k.xscale = h->xscale;
-    k.actions = h->act;
-    k.log_std = h->log_std;
-    k.adv_raw = h->adv_raw;
-    k.adv_stats = h->adv_stats;
-    k.old_logp = h->old_logp;
-    k.target = h->ret;
-    k.target_absmax = h->absmax + 64;
-    k.partials = h->partials;
-    k.scalar_partials = h->scalar_partials;
-    k.x_bad = h->trip;
-    k.status = h->trip + 1;
-    k.run_policy = k.run_value = 1;
-    if (launch_mlp_tc3(k, s)) return 1;
+    if (launch_mlp_tc3(tc3_args(h, hp, n_glob), s)) return 1;
     if (strcmp(stage, "fused_step_kernel") == 0) return 0;
     Ra3Args a;
     memset(&a, 0, sizeof(a));

@@ -20,14 +20,13 @@
 #include <cstdlib>
 
 #include "common.cuh"
+#include "policy_head.cuh"
 
 namespace b200rl {
 
 constexpr int TM_MAX = 64;         // rows per tile (64, or 32 / 16 when the network needs more shared memory)
 constexpr int MLP_THREADS = 256;   // 8 warps
 constexpr int MAXL = B200RL_MAX_LAYERS;
-constexpr float LOG_SQRT_2PI = 0.91893853320467274178f;
-constexpr float ENT_CONST = 1.4189385332046727418f;  // 0.5 + 0.5*log(2*pi)
 
 struct MlpLayout {
   int tm;  // rows per tile
@@ -282,9 +281,9 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_fused_kernel(const FusedAr
   const int A_out = Y.n[L];
   if (p.dist == B200RL_DIST_GAUSSIAN) {
     for (int a = tid; a < A_out; a += MLP_THREADS) {
-      const float scale = expf(__ldg(p.log_std + a));  // gaussian_policy.py:34
-      smem[Y.s_dist + a] = scale * scale;              // Normal.log_prob: var = scale ** 2
-      smem[Y.s_dist + Y.ld[L] + a] = logf(scale);      // log_scale = scale.log()
+      const NormalConsts c = normal_consts(p.log_std, a);
+      smem[Y.s_dist + a] = c.var;
+      smem[Y.s_dist + Y.ld[L] + a] = c.log_scale;
     }
   }
   // pad columns of the row-major activations are only ever read into discarded accumulators; zero them once
@@ -293,15 +292,8 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_fused_kernel(const FusedAr
   if (BACKWARD)
     for (int idx = tid; idx < 2 * TM * Y.ldz; idx += MLP_THREADS) smem[Y.s_dz[0] + idx] = 0.f;
 
-  // normalize_tensor statistics (utils.py:90-92): mean and UNBIASED std, no epsilon
-  float adv_mean = 0.f, adv_std = 1.f;
-  if (p.adv_stats != nullptr) {
-    const double s1 = p.adv_stats[0], s2 = p.adv_stats[1], cnt = p.adv_stats[2];
-    const double mean = s1 / cnt;
-    const double var = (s2 - cnt * mean * mean) / (cnt - 1.0);
-    adv_mean = (float)mean;
-    adv_std = (float)sqrt(var);
-  }
+  float adv_mean, adv_std;
+  adv_mean_std(p.adv_stats, adv_mean, adv_std);
   __syncthreads();
 
   double sc[7] = {0, 0, 0, 0, 0, 0, 0};  // loss terms, old_logp - logp, entropy, logp, logp^2, rows, KL(old||new)
@@ -390,43 +382,25 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_fused_kernel(const FusedAr
       const float* out = smem + Y.s_xrm[L] + r * Y.ld[L];
       float* dzrm = BACKWARD ? smem + Y.s_dz[L & 1] + r * Y.ldz : nullptr;
       float* dzt = smem + Y.s_xt[L];
-      float lp = 0.f, ent = 0.f;
       if (valid && FVP) {
-        // metric of the distribution applied to the output tangent: u = M (J v); dOut = u / N.
-        // Gaussian with fixed std: M = diag(1/var).  Categorical: M = diag(p) - p p^T.
+        // dOut = M (J v) / N, written row-major and then feature-major
         const float* t = smem + Y.s_trm + r * Y.ld[L];
-        if (p.dist == B200RL_DIST_GAUSSIAN) {
-          const float* var = smem + Y.s_dist;
-          for (int a = 0; a < A_out; ++a) {
-            const float g = (t[a] / var[a]) * p.inv_n;
-            dzrm[a] = g;
-            dzt[a * TM + r] = g;
-          }
-        } else {
-          float m = out[0];
-          for (int a = 1; a < A_out; ++a) m = fmaxf(m, out[a]);
-          float se = 0.f;
-          for (int a = 0; a < A_out; ++a) se += expf(out[a] - m);
-          const float lse = m + logf(se);
-          float pt = 0.f;
-          for (int a = 0; a < A_out; ++a) pt += expf(out[a] - lse) * t[a];
-          for (int a = 0; a < A_out; ++a) {
-            const float g = expf(out[a] - lse) * (t[a] - pt) * p.inv_n;
-            dzrm[a] = g;
-            dzt[a * TM + r] = g;
-          }
-        }
+        if (p.dist == B200RL_DIST_GAUSSIAN)
+          gaussian_metric<16>(t, VarDiv{smem + Y.s_dist}, A_out, p.inv_n, dzrm);
+        else
+          categorical_metric<16>(out, t, A_out, p.inv_n, dzrm);
+        for (int a = 0; a < A_out; ++a) dzt[a * TM + r] = dzrm[a];
         sc[5] += 1.0;
       } else if (valid) {
-        float coef = 0.f, term = 0.f;
         if (p.dist == B200RL_DIST_NONE) {
           const float vout = out[0];
           if (p.row_out) p.row_out[row] = vout;
+          float term = 0.f;
           if (p.loss == B200RL_LOSS_MSE) {
-            const float diff = vout - __ldg(p.target + row);
-            term = diff * diff;
+            float dv;
+            term = value_mse(vout, __ldg(p.target + row), p.inv_n, dv);
             if (BACKWARD) {
-              const float g = (2.f * diff) * p.inv_n * act_prime_from_output(vout, Y.out_act);
+              const float g = dv * act_prime_from_output(vout, Y.out_act);
               dzrm[0] = g;
               dzt[r] = g;
             }
@@ -434,63 +408,19 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_fused_kernel(const FusedAr
           sc[0] += (double)term;
           sc[5] += 1.0;
         } else {
-          // ---- log-prob, entropy and d logp / d out ----
-          float dlp[16];
-          if (p.dist == B200RL_DIST_GAUSSIAN) {
-            const float* var = smem + Y.s_dist;
-            const float* lsc = smem + Y.s_dist + Y.ld[L];
-            const float* act = p.actions + row * A_out;
-            for (int a = 0; a < A_out; ++a) {
-              const float d = __ldg(act + a) - out[a];
-              lp += -(d * d) / (2.f * var[a]) - lsc[a] - LOG_SQRT_2PI;  // torch Normal.log_prob
-              ent += ENT_CONST + lsc[a];                                // torch Normal.entropy
-              if (a < 16) dlp[a] = d / var[a];
-            }
-          } else {
-            float m = out[0];
-            for (int a = 1; a < A_out; ++a) m = fmaxf(m, out[a]);
-            float se = 0.f;
-            for (int a = 0; a < A_out; ++a) se += expf(out[a] - m);
-            const float lse = m + logf(se);
-            const int ai = (int)__ldg(p.actions + row);  // value.long()
-            for (int a = 0; a < A_out; ++a) {
-              const float lg = out[a] - lse;  // Categorical(logits=...) normalisation
-              const float pa = expf(lg);
-              ent -= lg * pa;
-              if (a == ai) lp = lg;
-              if (a < 16) dlp[a] = (a == ai ? 1.f : 0.f) - pa;
-            }
-          }
+          const VarDiv var{smem + Y.s_dist};
+          float lp, ent, dlp[16];
+          if (p.dist == B200RL_DIST_GAUSSIAN)
+            gaussian_logp<16>(Ldg{p.actions + row * A_out}, out, smem + Y.s_dist + Y.ld[L], var, A_out, lp, ent, dlp);
+          else
+            categorical_logp<16>(out, (int)__ldg(p.actions + row), A_out, lp, ent, dlp);  // value.long()
           if (p.row_out) p.row_out[row] = lp;
           if (p.out_full)
             for (int a = 0; a < A_out; ++a) p.out_full[row * A_out + a] = out[a];
-          if (p.old_out) {  // kl_divergence(old_dist, dist), trpo.py:167-175
-            const float* oo = p.old_out + row * A_out;
-            float kl = 0.f;
-            if (p.dist == B200RL_DIST_GAUSSIAN) {  // same std: 0.5 * ((mu_old - mu) / std)^2 summed
-              const float* var = smem + Y.s_dist;
-              for (int a = 0; a < A_out; ++a) {
-                const float d = __ldg(oo + a) - out[a];
-                kl += 0.5f * ((d * d) / var[a]);
-              }
-            } else {
-              float mo = __ldg(oo), mn = out[0];
-              for (int a = 1; a < A_out; ++a) {
-                mo = fmaxf(mo, __ldg(oo + a));
-                mn = fmaxf(mn, out[a]);
-              }
-              float so = 0.f, sn = 0.f;
-              for (int a = 0; a < A_out; ++a) {
-                so += expf(__ldg(oo + a) - mo);
-                sn += expf(out[a] - mn);
-              }
-              const float lo = mo + logf(so), ln = mn + logf(sn);
-              for (int a = 0; a < A_out; ++a) {
-                const float lpo = __ldg(oo + a) - lo;
-                kl += expf(lpo) * (lpo - (out[a] - ln));
-              }
-            }
-            sc[6] += (double)kl;
+          if (p.old_out) {
+            const Ldg oo{p.old_out + row * A_out};
+            sc[6] += (double)(p.dist == B200RL_DIST_GAUSSIAN ? gaussian_kl<16>(oo, out, var, A_out)
+                                                              : categorical_kl<16>(oo, out, A_out));
           }
           float adv = 0.f, oldlp = 0.f;
           if (p.loss != B200RL_LOSS_EVAL) {
@@ -498,21 +428,8 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_fused_kernel(const FusedAr
             if (p.adv_stats != nullptr) adv = (adv - adv_mean) / adv_std;  // utils.py:91
           }
           if (p.old_logp != nullptr) oldlp = __ldg(p.old_logp + row);
-          if (p.loss == B200RL_LOSS_PPO_CLIP) {  // ppo.py:245-255
-            const float ratio = expf(lp - oldlp);
-            const float s1 = ratio * adv;
-            const float s2 = fminf(fmaxf(ratio, p.clip_lo), p.clip_hi) * adv;
-            term = -fminf(s1, s2);
-            const bool pass = adv >= 0.f ? (ratio <= p.clip_hi) : (ratio >= p.clip_lo);
-            coef = pass ? (-p.inv_n * adv) * ratio : 0.f;
-          } else if (p.loss == B200RL_LOSS_VPG) {  // vpg.py:203
-            term = -(lp * adv);
-            coef = -p.inv_n * adv;
-          } else if (p.loss == B200RL_LOSS_TRPO_SURROGATE) {  // trpo.py:161-163
-            const float ratio = expf(lp - oldlp);
-            term = -(ratio * adv);
-            coef = (-p.inv_n * adv) * ratio;
-          }
+          float coef;
+          const float term = policy_loss(p.loss, lp, oldlp, adv, p.inv_n, p.clip_lo, p.clip_hi, coef);
           if (BACKWARD) {
             for (int a = 0; a < A_out; ++a) {
               const float g = coef * dlp[a] * act_prime_from_output(out[a], Y.out_act);
@@ -528,11 +445,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_fused_kernel(const FusedAr
                 if (a < A_out) dls[a] += coef * ((__ldg(act + a) - out[a]) * dlp[a] - 1.f);
             }
           }
-          sc[0] += (double)term;
-          if (p.old_logp != nullptr) sc[1] += (double)(oldlp - lp);
-          sc[2] += (double)ent;
-          sc[3] += (double)lp;
-          sc[4] += (double)lp * (double)lp;
+          add_policy_row_sums(sc, term, lp, ent, oldlp, p.old_logp != nullptr);
           sc[5] += 1.0;
         }
       } else if (BACKWARD) {

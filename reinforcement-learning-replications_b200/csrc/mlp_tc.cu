@@ -27,6 +27,7 @@
 #include <cmath>
 
 #include "common.cuh"
+#include "policy_head.cuh"
 #include "tc_common.cuh"
 
 namespace b200rl {
@@ -34,8 +35,6 @@ namespace b200rl {
 constexpr int TC_ROWS = 128;
 constexpr int TC_EPI_WARPS = 8;
 constexpr int TC_THREADS = TC_EPI_WARPS * 32 + 128;  // + the issuing warpgroup
-constexpr float TC_LOG_SQRT_2PI = 0.91893853320467274178f;
-constexpr float TC_ENT_CONST = 1.4189385332046727418f;
 
 // shared-memory map (bytes from the 1024-aligned base)
 constexpr uint32_t ACT_BUF = 128 * 128;  // one split of a [128][64] bf16 buffer
@@ -205,9 +204,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
     for (int i = tid; i < 16; i += TC_THREADS) s_bias[128 + i] = i < A_out ? __ldg(p.params + p.b_off[2] + i) : 0.f;
     if (p.dist == B200RL_DIST_GAUSSIAN)
       for (int a = tid; a < A_out; a += TC_THREADS) {
-        const float scale = expf(__ldg(p.log_std + a));  // gaussian_policy.py:34
-        s_dist[a] = scale * scale;                       // Normal.log_prob: var = scale ** 2
-        s_dist[16 + a] = logf(scale);
+        const NormalConsts c = normal_consts(p.log_std, a);
+        s_dist[a] = c.var;
+        s_dist[16 + a] = c.log_scale;
       }
   }
   if (tid == 0) {
@@ -274,13 +273,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
     const int c0 = 32 * half;                            // this warp's column half
     uint32_t phase = 0;
 
-    float adv_mean = 0.f, adv_std = 1.f;  // normalize_tensor (utils.py:90-92): mean, UNBIASED std, no epsilon
-    if (p.adv_stats != nullptr) {
-      const double s1 = p.adv_stats[0], s2 = p.adv_stats[1], cnt = p.adv_stats[2];
-      const double mean = s1 / cnt;
-      adv_mean = (float)mean;
-      adv_std = (float)sqrt((s2 - cnt * mean * mean) / (cnt - 1.0));
-    }
+    float adv_mean, adv_std;
+    adv_mean_std(p.adv_stats, adv_mean, adv_std);
     double sc[6] = {0, 0, 0, 0, 0, 0};
     float db3[16];
 #pragma unroll
@@ -413,52 +407,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
           dout[a] = 0.f;
         }
         if (valid) {
-          float coef = 0.f, term = 0.f, lp = 0.f, ent = 0.f;
           if (p.dist == B200RL_DIST_NONE) {
             const float vout = out[0];
             if (p.row_out) p.row_out[row] = vout;
-            if (p.loss == B200RL_LOSS_MSE) {  // ppo.py:282-287
-              const float diff = vout - pf_tgt;
-              term = diff * diff;
-              dout[0] = (2.f * diff) * p.inv_n;
-            }
+            float term = 0.f;
+            if (p.loss == B200RL_LOSS_MSE) term = value_mse(vout, pf_tgt, p.inv_n, dout[0]);
             sc[0] += (double)term;
             sc[5] += 1.0;
           } else {
-            float dlp[16];
+            float lp, ent, dlp[16];
 #pragma unroll
             for (int a = 0; a < 16; ++a) dlp[a] = 0.f;
-            if (p.dist == B200RL_DIST_GAUSSIAN) {
-#pragma unroll
-              for (int a = 0; a < 15; ++a)
-                if (a < A_out) {
-                  const float var = s_dist[a], lsc = s_dist[16 + a];
-                  const float d = pf_act[a] - out[a];
-                  lp += -(d * d) / (2.f * var) - lsc - TC_LOG_SQRT_2PI;  // torch Normal.log_prob
-                  ent += TC_ENT_CONST + lsc;                             // torch Normal.entropy
-                  dlp[a] = d / var;
-                }
-            } else {
-              float m = out[0];
-#pragma unroll
-              for (int a = 1; a < 15; ++a)
-                if (a < A_out) m = fmaxf(m, out[a]);
-              float se = 0.f;
-#pragma unroll
-              for (int a = 0; a < 15; ++a)
-                if (a < A_out) se += expf(out[a] - m);
-              const float lse = m + logf(se);
-              const int ai = (int)pf_act[0];  // value.long()
-#pragma unroll
-              for (int a = 0; a < 15; ++a)
-                if (a < A_out) {
-                  const float lg = out[a] - lse;
-                  const float pa = expf(lg);
-                  ent -= lg * pa;
-                  if (a == ai) lp = lg;
-                  dlp[a] = (a == ai ? 1.f : 0.f) - pa;
-                }
-            }
+            if (p.dist == B200RL_DIST_GAUSSIAN)
+              gaussian_logp<15>(pf_act, out, s_dist + 16, VarDiv{s_dist}, A_out, lp, ent, dlp);
+            else
+              categorical_logp<15>(out, (int)pf_act[0], A_out, lp, ent, dlp);  // value.long()
             if (p.row_out) p.row_out[row] = lp;
             float adv = 0.f, oldlp = 0.f;
             if (p.loss != B200RL_LOSS_EVAL) {
@@ -466,28 +429,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mlp_tc_kernel(const TcArgs p) {
               if (p.adv_stats != nullptr) adv = (adv - adv_mean) / adv_std;  // utils.py:91
             }
             if (p.old_logp != nullptr) oldlp = pf_old;
-            if (p.loss == B200RL_LOSS_PPO_CLIP) {  // ppo.py:245-255
-              const float ratio = expf(lp - oldlp);
-              const float s1 = ratio * adv;
-              const float s2 = fminf(fmaxf(ratio, p.clip_lo), p.clip_hi) * adv;
-              term = -fminf(s1, s2);
-              const bool pass = adv >= 0.f ? (ratio <= p.clip_hi) : (ratio >= p.clip_lo);
-              coef = pass ? (-p.inv_n * adv) * ratio : 0.f;
-            } else if (p.loss == B200RL_LOSS_VPG) {  // vpg.py:203
-              term = -(lp * adv);
-              coef = -p.inv_n * adv;
-            } else if (p.loss == B200RL_LOSS_TRPO_SURROGATE) {  // trpo.py:161-163
-              const float ratio = expf(lp - oldlp);
-              term = -(ratio * adv);
-              coef = (-p.inv_n * adv) * ratio;
-            }
+            float coef;
+            const float term = policy_loss(p.loss, lp, oldlp, adv, p.inv_n, p.clip_lo, p.clip_hi, coef);
 #pragma unroll
             for (int a = 0; a < 15; ++a) dout[a] = coef * dlp[a];
-            sc[0] += (double)term;
-            if (p.old_logp != nullptr) sc[1] += (double)(oldlp - lp);
-            sc[2] += (double)ent;
-            sc[3] += (double)lp;
-            sc[4] += (double)lp * (double)lp;
+            add_policy_row_sums(sc, term, lp, ent, oldlp, p.old_logp != nullptr);
             sc[5] += 1.0;
           }
         }

@@ -34,6 +34,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "policy_head.cuh"
 #include "tc2_common.cuh"
 #include "tc_common.cuh"
 
@@ -43,8 +44,6 @@ constexpr int T2_ROWS = 128;
 constexpr int T2_EPI_WARPS = 16;  // one pool: 4 warps per 32-row quarter of the tile, 16 columns each
 constexpr int T2_EPI_THREADS = T2_EPI_WARPS * 32;
 constexpr int T2_THREADS = T2_EPI_THREADS + 128;  // + the issuing warpgroup
-constexpr float T2_LOG_SQRT_2PI = 0.91893853320467274178f;
-constexpr float T2_ENT_CONST = 1.4189385332046727418f;
 
 // shared-memory map (bytes from the 1024-aligned base); every operand buffer = 2 fp16 splits, 128-byte rows, SW128
 constexpr uint32_t T2_SLOT = 6 * T2_ACT;    // XD, H1, H2 of one slot
@@ -269,11 +268,11 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
     }
     if (p.dist == B200RL_DIST_GAUSSIAN)
       for (int a = tid; a < A_out; a += T2_THREADS) {
-        const float scale = expf(__ldg(p.log_std + a));  // gaussian_policy.py:34
-        s_dist[a] = scale * scale;                       // Normal.log_prob: var = scale ** 2
-        s_dist[16 + a] = logf(scale);
-        s_dist[32 + a] = 1.f / (2.f * (scale * scale));  // reciprocals: one multiply per row instead of a division
-        s_dist[48 + a] = 1.f / (scale * scale);
+        const NormalConsts c = normal_consts(p.log_std, a);
+        s_dist[a] = c.var;
+        s_dist[16 + a] = c.log_scale;
+        s_dist[32 + a] = c.inv_2var;
+        s_dist[48 + a] = c.inv_var;
       }
   }
   if (bad) *s_bad = 1;  // non-finite bias
@@ -405,13 +404,8 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
 #pragma unroll
     for (int a = 0; a < 15; ++a) db3[a] = 0.f;
 
-    float adv_mean = 0.f, adv_std = 1.f;  // normalize_tensor (utils.py:90-92): mean, UNBIASED std, no epsilon
-    if (p.adv_stats != nullptr) {
-      const double s1 = p.adv_stats[0], s2 = p.adv_stats[1], cnt = p.adv_stats[2];
-      const double mean = s1 / cnt;
-      adv_mean = (float)mean;
-      adv_std = (float)sqrt((s2 - cnt * mean * mean) / (cnt - 1.0));
-    }
+    float adv_mean, adv_std;
+    adv_mean_std(p.adv_stats, adv_mean, adv_std);
     const float adv_inv_std = 1.f / adv_std;
 
 #ifdef B200RL_TC_TIMING
@@ -517,52 +511,22 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
             dout[a] = 0.f;
           }
           if (valid) {
-            float coef = 0.f, term = 0.f, lp = 0.f, ent = 0.f;
             if (p.dist == B200RL_DIST_NONE) {
               const float vout = out[0];
               if (p.row_out) p.row_out[row] = vout;
-              if (p.loss == B200RL_LOSS_MSE) {  // ppo.py:282-287
-                const float diff = vout - pf_tgt;
-                term = diff * diff;
-                dout[0] = (2.f * diff) * p.inv_n;
-              }
+              float term = 0.f;
+              if (p.loss == B200RL_LOSS_MSE) term = value_mse(vout, pf_tgt, p.inv_n, dout[0]);
               sc[0] += (double)term;
               sc[5] += 1.0;
             } else {
-              float dlp[16];
+              const VarRecip var{s_dist + 48, s_dist + 32};
+              float lp, ent, dlp[16];
 #pragma unroll
               for (int a = 0; a < 16; ++a) dlp[a] = 0.f;
-              if (p.dist == B200RL_DIST_GAUSSIAN) {
-#pragma unroll
-                for (int a = 0; a < 15; ++a)
-                  if (a < A_out) {
-                    const float lsc = s_dist[16 + a];
-                    const float d = pf_act[a] - out[a];
-                    lp += -(d * d) * s_dist[32 + a] - lsc - T2_LOG_SQRT_2PI;  // torch Normal.log_prob
-                    ent += T2_ENT_CONST + lsc;                                // torch Normal.entropy
-                    dlp[a] = d * s_dist[48 + a];
-                  }
-              } else {
-                float m = out[0];
-#pragma unroll
-                for (int a = 1; a < 15; ++a)
-                  if (a < A_out) m = fmaxf(m, out[a]);
-                float se = 0.f;
-#pragma unroll
-                for (int a = 0; a < 15; ++a)
-                  if (a < A_out) se += expf(out[a] - m);
-                const float lse = m + logf(se);
-                const int ai = (int)pf_act[0];  // value.long()
-#pragma unroll
-                for (int a = 0; a < 15; ++a)
-                  if (a < A_out) {
-                    const float lg = out[a] - lse;
-                    const float pa = expf(lg);
-                    ent -= lg * pa;
-                    if (a == ai) lp = lg;
-                    dlp[a] = (a == ai ? 1.f : 0.f) - pa;
-                  }
-              }
+              if (p.dist == B200RL_DIST_GAUSSIAN)
+                gaussian_logp<15>(pf_act, out, s_dist + 16, var, A_out, lp, ent, dlp);
+              else
+                categorical_logp<15>(out, (int)pf_act[0], A_out, lp, ent, dlp);  // value.long()
               if (p.row_out) p.row_out[row] = lp;
               if (!BACKWARD) {
                 if (p.out_full != nullptr) {
@@ -570,40 +534,10 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
                   for (int a = 0; a < 15; ++a)
                     if (a < A_out) p.out_full[row * A_out + a] = out[a];
                 }
-                if (p.old_out != nullptr) {  // kl_divergence(old_dist, dist), trpo.py:167-175
-                  const float* oo = p.old_out + row * A_out;
-                  float kl = 0.f;
-                  if (p.dist == B200RL_DIST_GAUSSIAN) {  // same std: 0.5 ((mu_old - mu) / std)^2 summed
-#pragma unroll
-                    for (int a = 0; a < 15; ++a)
-                      if (a < A_out) {
-                        const float d = __ldg(oo + a) - out[a];
-                        kl += 0.5f * ((d * d) * s_dist[48 + a]);
-                      }
-                  } else {
-                    float mo = __ldg(oo), mn = out[0];
-#pragma unroll
-                    for (int a = 1; a < 15; ++a)
-                      if (a < A_out) {
-                        mo = fmaxf(mo, __ldg(oo + a));
-                        mn = fmaxf(mn, out[a]);
-                      }
-                    float so = 0.f, sn = 0.f;
-#pragma unroll
-                    for (int a = 0; a < 15; ++a)
-                      if (a < A_out) {
-                        so += expf(__ldg(oo + a) - mo);
-                        sn += expf(out[a] - mn);
-                      }
-                    const float lo = mo + logf(so), ln = mn + logf(sn);
-#pragma unroll
-                    for (int a = 0; a < 15; ++a)
-                      if (a < A_out) {
-                        const float lpo = __ldg(oo + a) - lo;
-                        kl += expf(lpo) * (lpo - (out[a] - ln));
-                      }
-                  }
-                  sc_kl += (double)kl;
+                if (p.old_out != nullptr) {
+                  const Ldg oo{p.old_out + row * A_out};
+                  sc_kl += (double)(p.dist == B200RL_DIST_GAUSSIAN ? gaussian_kl<15>(oo, out, var, A_out)
+                                                                    : categorical_kl<15>(oo, out, A_out));
                 }
               }
               float adv = 0.f, oldlp = 0.f;
@@ -612,28 +546,11 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
                 if (p.adv_stats != nullptr) adv = (adv - adv_mean) * adv_inv_std;  // utils.py:91
               }
               if (p.old_logp != nullptr) oldlp = pf_old;
-              if (p.loss == B200RL_LOSS_PPO_CLIP) {  // ppo.py:245-255
-                const float ratio = expf(lp - oldlp);
-                const float s1 = ratio * adv;
-                const float s2 = fminf(fmaxf(ratio, p.clip_lo), p.clip_hi) * adv;
-                term = -fminf(s1, s2);
-                const bool pass = adv >= 0.f ? (ratio <= p.clip_hi) : (ratio >= p.clip_lo);
-                coef = pass ? (-p.inv_n * adv) * ratio : 0.f;
-              } else if (p.loss == B200RL_LOSS_VPG) {  // vpg.py:203
-                term = -(lp * adv);
-                coef = -p.inv_n * adv;
-              } else if (p.loss == B200RL_LOSS_TRPO_SURROGATE) {  // trpo.py:161-163
-                const float ratio = expf(lp - oldlp);
-                term = -(ratio * adv);
-                coef = (-p.inv_n * adv) * ratio;
-              }
+              float coef;
+              const float term = policy_loss(p.loss, lp, oldlp, adv, p.inv_n, p.clip_lo, p.clip_hi, coef);
 #pragma unroll
               for (int a = 0; a < 15; ++a) dout[a] = coef * dlp[a];
-              sc[0] += (double)term;
-              if (p.old_logp != nullptr) sc[1] += (double)(oldlp - lp);
-              sc[2] += (double)ent;
-              sc[3] += (double)lp;
-              sc[4] += (double)lp * (double)lp;
+              add_policy_row_sums(sc, term, lp, ent, oldlp, p.old_logp != nullptr);
               sc[5] += 1.0;
             }
           }

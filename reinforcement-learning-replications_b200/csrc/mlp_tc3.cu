@@ -24,6 +24,7 @@
 #include <cmath>
 
 #include "common.cuh"
+#include "policy_head.cuh"
 #include "tc2_common.cuh"
 #include "tc_common.cuh"
 #include "tc3.cuh"
@@ -34,8 +35,6 @@ constexpr int T3_ROWS = 128;
 constexpr int T3_EPI_WARPS = 16;
 constexpr int T3_EPI_THREADS = T3_EPI_WARPS * 32;
 constexpr int T3_THREADS = T3_EPI_THREADS + 128;  // + the issuing warpgroup
-constexpr float T3_LOG_SQRT_2PI = 0.91893853320467274178f;
-constexpr float T3_ENT_CONST = 1.4189385332046727418f;
 
 // ---- shared-memory map (bytes from the 1024-aligned base) ----
 constexpr uint32_t S3_XB = 0;                        // X(k) | dOut(k) buffers, parity k & 1 and (k + 1) & 1
@@ -304,11 +303,11 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   }
   if (p.dist == B200RL_DIST_GAUSSIAN)
     for (int a = tid; a < p.net[0].n_out; a += T3_THREADS) {
-      const float scale = expf(__ldg(p.log_std + a));  // gaussian_policy.py:34
-      s_dist[a] = scale * scale;
-      s_dist[16 + a] = logf(scale);
-      s_dist[32 + a] = 1.f / (2.f * (scale * scale));
-      s_dist[48 + a] = 1.f / (scale * scale);
+      const NormalConsts c = normal_consts(p.log_std, a);
+      s_dist[a] = c.var;
+      s_dist[16 + a] = c.log_scale;
+      s_dist[32 + a] = c.inv_2var;
+      s_dist[48 + a] = c.inv_var;
     }
   if (bad) *s_bad = 1;  // non-finite bias
   bad = false;
@@ -449,13 +448,9 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     float db3[15], db3v = 0.f;
 #pragma unroll
     for (int a = 0; a < 15; ++a) db3[a] = 0.f;
-    float adv_mean = 0.f, adv_inv_std = 1.f;  // normalize_tensor (utils.py:90-92): mean, UNBIASED std, no epsilon
-    if (p.adv_stats != nullptr) {
-      const double s1 = p.adv_stats[0], s2 = p.adv_stats[1], cnt = p.adv_stats[2];
-      const double mean = s1 / cnt;
-      adv_mean = (float)mean;
-      adv_inv_std = 1.f / (float)sqrt((s2 - cnt * mean * mean) / (cnt - 1.0));
-    }
+    float adv_mean, adv_std;
+    adv_mean_std(p.adv_stats, adv_mean, adv_std);
+    const float adv_inv_std = 1.f / adv_std;
 
 #ifdef B200RL_TC3_TIMING
     long long t_work0 = 0;
@@ -540,56 +535,20 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
               dout[a] = 0.f;
             }
             if (valid) {
-              float lp = 0.f, ent = 0.f, dlp[16];
+              float lp, ent, dlp[16];
 #pragma unroll
               for (int a = 0; a < 16; ++a) dlp[a] = 0.f;
-              if (p.dist == B200RL_DIST_GAUSSIAN) {
-#pragma unroll
-                for (int a = 0; a < 15; ++a)
-                  if (a < A_out) {
-                    const float lsc = s_dist[16 + a];
-                    const float d = pf_act[a] - out[a];
-                    lp += -(d * d) * s_dist[32 + a] - lsc - T3_LOG_SQRT_2PI;  // torch Normal.log_prob
-                    ent += T3_ENT_CONST + lsc;                                // torch Normal.entropy
-                    dlp[a] = d * s_dist[48 + a];
-                  }
-              } else {
-                float m = out[0];
-#pragma unroll
-                for (int a = 1; a < 15; ++a)
-                  if (a < A_out) m = fmaxf(m, out[a]);
-                float se = 0.f;
-#pragma unroll
-                for (int a = 0; a < 15; ++a)
-                  if (a < A_out) se += expf(out[a] - m);
-                const float lse = m + logf(se);
-                const int ai = (int)pf_act[0];  // value.long()
-#pragma unroll
-                for (int a = 0; a < 15; ++a)
-                  if (a < A_out) {
-                    const float lg = out[a] - lse;
-                    const float pa = expf(lg);
-                    ent -= lg * pa;
-                    if (a == ai) lp = lg;
-                    dlp[a] = (a == ai ? 1.f : 0.f) - pa;
-                  }
-              }
+              if (p.dist == B200RL_DIST_GAUSSIAN)
+                gaussian_logp<15>(pf_act, out, s_dist + 16, VarRecip{s_dist + 48, s_dist + 32}, A_out, lp, ent, dlp);
+              else
+                categorical_logp<15>(out, (int)pf_act[0], A_out, lp, ent, dlp);  // value.long()
               float adv = pf_adv;
               if (p.adv_stats != nullptr) adv = (adv - adv_mean) * adv_inv_std;  // utils.py:91
-              // ppo.py:245-255
-              const float ratio = expf(lp - pf_old);
-              const float s1 = ratio * adv;
-              const float s2 = fminf(fmaxf(ratio, p.clip_lo), p.clip_hi) * adv;
-              const float term = -fminf(s1, s2);
-              const bool pass = adv >= 0.f ? (ratio <= p.clip_hi) : (ratio >= p.clip_lo);
-              const float coef = pass ? (-p.inv_n * adv) * ratio : 0.f;
+              float coef;
+              const float term = policy_loss(B200RL_LOSS_PPO_CLIP, lp, pf_old, adv, p.inv_n, p.clip_lo, p.clip_hi, coef);
 #pragma unroll
               for (int a = 0; a < 15; ++a) dout[a] = coef * dlp[a];
-              sc[0] += (double)term;
-              sc[1] += (double)(pf_old - lp);
-              sc[2] += (double)ent;
-              sc[3] += (double)lp;
-              sc[4] += (double)lp * (double)lp;
+              add_policy_row_sums(sc, term, lp, ent, pf_old, true);
               rows_done += 1;
             }
             const float sG = scl[C3_G];
@@ -608,11 +567,9 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
           if (loss_warp) {
             float o[8];
             acc_ld<8>(acc, r, acol + ACC_OUT, o);
-            if (valid) {  // ppo.py:282-287
-              const float vout = fmaf(o[0], scl[C3_U3], bias[128]);
-              const float diff = vout - pf_tgt;
-              const float dout = (2.f * diff) * p.inv_n;
-              vs += (double)(diff * diff);
+            if (valid) {
+              float dout;
+              vs += (double)value_mse(fmaf(o[0], scl[C3_U3], bias[128]), pf_tgt, p.inv_n, dout);
               db3v += dout;
               x0[0] = dout * scl[C3_G];
             }

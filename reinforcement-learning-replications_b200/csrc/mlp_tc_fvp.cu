@@ -20,6 +20,7 @@
 #include <cmath>
 
 #include "common.cuh"
+#include "policy_head.cuh"
 #include "tc2_common.cuh"
 #include "tc_common.cuh"
 
@@ -227,10 +228,7 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
       }
     }
     if (p.dist == B200RL_DIST_GAUSSIAN)
-      for (int a = tid; a < 16; a += FV_THREADS) {
-        const float scale = a < A_out ? expf(__ldg(p.log_std + a)) : 1.f;  // gaussian_policy.py:34
-        s_ivar[a] = 1.f / (scale * scale);
-      }
+      for (int a = tid; a < 16; a += FV_THREADS) s_ivar[a] = a < A_out ? normal_consts(p.log_std, a).inv_var : 1.f;
   }
   if (bad) *s_bad = 1;  // non-finite bias
   bad = false;
@@ -403,30 +401,13 @@ __global__ void __launch_bounds__(FV_THREADS, 1) mlp_tc_fvp_kernel(const FvpArgs
 #pragma unroll
           for (int a = 0; a < 16; ++a) tout[a] = fmaf(t[a], ut3, s_vb[128 + a]);
           if (p.dist == B200RL_DIST_GAUSSIAN) {
-#pragma unroll
-            for (int a = 0; a < 15; ++a)
-              if (a < A_out) dout[a] = (tout[a] * s_ivar[a]) * p.inv_n;
+            gaussian_metric<15>(tout, VarRecip{s_ivar, nullptr}, A_out, p.inv_n, dout);
           } else {
             float out[16];
             const float u3 = s_scale[FS_U3];
 #pragma unroll
             for (int a = 0; a < 16; ++a) out[a] = fmaf(o[a], u3, s_bias[128 + a]);
-            float m = out[0];
-#pragma unroll
-            for (int a = 1; a < 15; ++a)
-              if (a < A_out) m = fmaxf(m, out[a]);
-            float se = 0.f;
-#pragma unroll
-            for (int a = 0; a < 15; ++a)
-              if (a < A_out) se += expf(out[a] - m);
-            const float lse = m + logf(se);
-            float pt = 0.f;
-#pragma unroll
-            for (int a = 0; a < 15; ++a)
-              if (a < A_out) pt += expf(out[a] - lse) * tout[a];
-#pragma unroll
-            for (int a = 0; a < 15; ++a)
-              if (a < A_out) dout[a] = expf(out[a] - lse) * (tout[a] - pt) * p.inv_n;
+            categorical_metric<15>(out, tout, A_out, p.inv_n, dout);
           }
           rows_done += 1.0;
         }

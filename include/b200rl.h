@@ -335,10 +335,11 @@ typedef struct b200rl_offpolicy b200rl_offpolicy;
 typedef struct {
   b200rl_mlp_desc policy;  /* [obs, hidden..., act]      (ref: policies/deterministic_policy.py); SAC: [obs, ..., 2 act] */
   b200rl_mlp_desc q;       /* [obs + act, hidden..., 1]  (ref: q_function.py:20-32) */
-  int32_t n_q;             /* 1 = DDPG, 2 = TD3 (algo 0); SAC needs 2 */
+  int32_t n_q;             /* 1 = DDPG, 2 = TD3 (algo 0); SAC needs 2, DQN 1 */
   int32_t max_minibatch;   /* capacity: rows per minibatch */
   int32_t max_steps;       /* capacity: train steps per call */
-  int32_t algo;            /* 0 = DDPG / TD3 (by n_q), 1 = SAC (see b200rl_offpolicy_set_sac) */
+  int32_t algo;            /* 0 = DDPG / TD3 (by n_q), 1 = SAC (see b200rl_offpolicy_set_sac), 2 = DQN (see
+                            * b200rl_offpolicy_set_dqn) */
 } b200rl_offpolicy_config;
 
 typedef struct {
@@ -435,6 +436,33 @@ int b200rl_offpolicy_set_alpha(b200rl_offpolicy* h, float log_alpha, float exp_a
 int b200rl_offpolicy_get_alpha(b200rl_offpolicy* h, float* log_alpha, float* exp_avg, float* exp_avg_sq, int64_t* step);
 /* After a train call of S steps: mean log pi of each policy step and the alpha each step used (host [S] each). */
 int b200rl_offpolicy_sac_outputs(b200rl_offpolicy* h, int32_t S, float* log_prob_means, float* alphas);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * DQN on the same engine (config algo = 2, n_q = 1; Mnih et al. 2015, Double DQN: van Hasselt et al. 2016).  The
+ * policy description must be zeroed; q = [obs, hidden..., n_actions] maps obs -> one value per action (n_actions >= 1).
+ * Networks 1 (Q) and 4 (target Q) are present, so the state blob holds their parameters followed by optimizer 1's
+ * exp_avg / exp_avg_sq; steps[3] keeps its layout (steps[1] is the Q optimizer's count, the others 0).  The action
+ * column is one float32 per row holding the action index (act [S,B] for train, d_act [rows] for the gather paths).
+ * Per train step, with t = the Q optimizer's step count after the step:
+ *   v = Q_targ(s')[argmax_j Q(s')_j] (double_q = 1; Q at the start of the step) or max_j Q_targ(s')_j
+ *       (torch's max / argmax: a NaN wins, ties go to the first index)
+ *   y = r + gamma (1 - d) v;  one Adam step (optimizer 1) on F.smooth_l1_loss(Q(s)[a], y) (beta = 1, mean over B)
+ *   target Q <- Q (exact copy) when t % target_update_interval == 0: the schedule follows each learner's own count,
+ *       across calls and across get_state / set_state
+ * hparams: only gamma and the q1_lr / q_beta1 / q_beta2 / q_eps Adam fields apply; every other field is ignored.
+ * Outputs: q1_values [S,B] (Q(s)[a] before the update) and q1_losses [S]; *n_policy_updates = 0, and q2_values,
+ * q2_losses and policy_losses may be NULL.  No noise is used: train / train_gather take noise = NULL, train_gather_rng
+ * draws indices only.  A row whose action is not an integer in [0, n_actions) is never used as an index and adds nothing
+ * to the update; the call then returns an error naming the learner and the step (the update has still run).  DQN
+ * runs as a CUDA graph, or as plain launches with B200RL_OFFPOLICY_GRAPH=0, and in learner groups like the others.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t target_update_interval; /* >= 1: copy Q to the target every this many Q optimizer steps */
+  int32_t double_q;               /* 0 = DQN target, 1 = Double DQN target */
+} b200rl_dqn_hparams;
+
+/* Required once before the first train call of a DQN engine; part of the cached graph's key. */
+int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hparams* hp);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Learner groups: K independent off-policy learners (same config, same hyper-parameters, their own parameters, Adam

@@ -90,6 +90,10 @@ class SacHparams(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+class DqnHparams(C.Structure):
+    _fields_ = [("target_update_interval", C.c_int32), ("double_q", C.c_int32)]
+
+
 class OffPolicyReplay(C.Structure):
     _fields_ = [("obs", C.c_void_p), ("act", C.c_void_p), ("rew", C.c_void_p), ("next_obs", C.c_void_p),
                 ("done", C.c_void_p), ("rows", C.c_int64)]
@@ -171,6 +175,7 @@ SIGNATURES = {
     "b200rl_offpolicy_get_alpha": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float),
                                              C.POINTER(C.c_float), C.POINTER(C.c_int64)]),
     "b200rl_offpolicy_sac_outputs": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "b200rl_offpolicy_set_dqn": (C.c_int, [C.c_void_p, C.POINTER(DqnHparams)]),
     "b200rl_offpolicy_create_group": (C.c_int, [C.POINTER(OffPolicyConfig), C.c_int32, C.POINTER(C.c_void_p)]),
     "b200rl_offpolicy_train_gather_group": (C.c_int, [C.c_void_p, C.POINTER(OffPolicyHparams), C.c_int32, C.c_int32,
                                                       C.POINTER(OffPolicyReplay)] + [C.c_void_p] * 7 +

@@ -1,3 +1,4 @@
+from .dqn import DQN
 from .group import LearnerGroup
 from .ppo import PPO
 from .sac import SAC
@@ -5,4 +6,4 @@ from .td3 import DDPG, TD3
 from .trpo import TRPO
 from .vpg import VPG
 
-__all__ = ["VPG", "TRPO", "PPO", "DDPG", "TD3", "SAC", "LearnerGroup"]
+__all__ = ["VPG", "TRPO", "PPO", "DDPG", "TD3", "SAC", "DQN", "LearnerGroup"]

@@ -1,0 +1,142 @@
+"""DQN (Mnih et al. 2015) with optional Double DQN targets (van Hasselt et al. 2016) over the GPU off-policy engine.
+``learn`` is the shared off-policy host loop; ``train`` is the hot path (enqueue_dqn_steps in csrc/offpolicy.cu)."""
+from __future__ import annotations
+
+import copy
+
+import numpy as np
+import torch
+
+from .._lib import OffPolicyHparams
+from ..engine import OffPolicyEngine
+from ..policies import EpsilonGreedyPolicy, GreedyPolicy
+from ._onpolicy import adam_hparams, describe_mlp
+from .td3 import _learn, _make_eval_env, _OffPolicyBase
+
+
+class DQN(_OffPolicyBase):
+    """Per train step, on a minibatch (s, a, r, s', d) with a the action index:
+    y = r + gamma (1 - d) Q_targ(s', argmax_a' Q(s', a')) (``double_q``) or r + gamma (1 - d) max_a' Q_targ(s', a'),
+    one Adam step on F.smooth_l1_loss(Q(s, a), y), and Q_targ <- Q whenever the Q optimizer's step count reaches a
+    multiple of ``target_update_interval`` (the count carries across train() calls and checkpoints).
+
+    Acting: ``exploration_policy`` before ``num_start_steps``, then epsilon-greedy with epsilon falling linearly from
+    ``epsilon_start`` to ``epsilon_end`` over the first ``epsilon_decay_steps`` environment steps; evaluation is greedy."""
+    n_q = 1
+    algo = OffPolicyEngine.DQN
+    trainable_slots = (1,)  # the Q network is engine network 1, its optimizer row 1
+    target_slots = (4,)
+
+    def __init__(self, q_function, exploration_policy, env, sampler, replay_buffer, evaluator, gamma: float = 0.99,
+                 target_update_interval: int = 1000, double_q: bool = False, epsilon_start: float = 1.0,
+                 epsilon_end: float = 0.05, epsilon_decay_steps: int = 10000) -> None:
+        n = getattr(env.action_space, "n", None)
+        if n is None:
+            raise ValueError("DQN needs a discrete action space (one with .n)")
+        sizes, _, _, lins = describe_mlp(q_function.network)
+        obs_shape = getattr(getattr(env, "observation_space", None), "shape", None)
+        if sizes[-1] != int(n) or (obs_shape and sizes[0] != int(np.prod(obs_shape))):
+            want = f"{int(np.prod(obs_shape))} -> {int(n)}" if obs_shape else f"obs -> {int(n)}"
+            raise ValueError(f"the Q network must map {want} (one value per action), got {sizes[0]} -> {sizes[-1]}")
+        adam_hparams(q_function.optimizer, lins, "q-function optimizer")
+        if int(target_update_interval) < 1:
+            raise ValueError(f"target_update_interval must be >= 1, got {target_update_interval}")
+        self.q_function, self.exploration_policy = q_function, exploration_policy
+        self.env, self.sampler, self.replay_buffer, self.evaluator = env, sampler, replay_buffer, evaluator
+        self.gamma = gamma
+        self.target_update_interval, self.double_q = int(target_update_interval), bool(double_q)
+        self.epsilon_start, self.epsilon_end = float(epsilon_start), float(epsilon_end)
+        self.epsilon_decay_steps = int(epsilon_decay_steps)
+        self.n_actions = int(n)
+        self.epsilon_greedy_policy = EpsilonGreedyPolicy(q_function, env.action_space, epsilon_start)
+        self.policy = self.evaluation_policy = GreedyPolicy(q_function)  # acting greedily (evaluation)
+        self.evaluation_env = _make_eval_env(env)
+        self.target_q_function = copy.deepcopy(q_function)
+        for p in self.target_q_function.network.parameters():
+            p.requires_grad = False
+
+    def epsilon(self) -> float:
+        """epsilon at the current total step count: linear from epsilon_start to epsilon_end, then constant."""
+        t = getattr(self, "current_total_steps", 0)
+        frac = min(t / self.epsilon_decay_steps, 1.0) if self.epsilon_decay_steps > 0 else 1.0
+        return self.epsilon_start + frac * (self.epsilon_end - self.epsilon_start)
+
+    @property
+    def noised_policy(self):
+        """The acting policy after warm-up (the shared learn loop's name for it), at the current epsilon."""
+        self.epsilon_greedy_policy.epsilon = self.epsilon()
+        return self.epsilon_greedy_policy
+
+    def _trainable(self):
+        return [self.q_function]
+
+    def _nets(self):
+        return [self.q_function], [self.target_q_function]
+
+    def _ensure_engine(self, S: int, B: int) -> OffPolicyEngine:
+        qsz, qact, qout, _ = describe_mlp(self.q_function.network)
+        e = getattr(self, "_engine", None)
+        if e is None or e.q_sizes != qsz or e.max_minibatch < B or e.max_steps < S or e.q_acts != (qact, qout):
+            if e is not None:
+                e.close()
+            e = OffPolicyEngine(None, qsz, 1, B, S, q_acts=(qact, qout), algo=self.algo)
+            self._engine = e
+        return e
+
+    def _hparams(self, noisy: bool, delay: int) -> OffPolicyHparams:
+        hp = OffPolicyHparams()
+        hp.gamma, hp.policy_delay = self.gamma, 1
+        lr, b1, b2, eps = adam_hparams(self.q_function.optimizer, describe_mlp(self.q_function.network)[3],
+                                       "q-function optimizer")
+        hp.q1_lr, hp.q2_lr, hp.q_beta1, hp.q_beta2, hp.q_eps = lr, lr, b1, b2, eps
+        return hp
+
+    def _upload_state(self, e, trainable, targets, lins) -> None:
+        super()._upload_state(e, trainable, targets, lins)
+        e.set_dqn(self.target_update_interval, self.double_q)
+
+    def _stage_inputs(self, replay_buffer, S: int, B: int, noisy: bool):
+        mode, inputs = super()._stage_inputs(replay_buffer, S, B, noisy)
+        if mode == "host":  # the action column as [S, B] indices
+            obs, act, rew, nobs, done, _ = inputs
+            inputs = (obs, act.reshape(S, B), rew, nobs, done, None)
+        return mode, inputs
+
+    def _train_schedule(self):
+        return False, 1
+
+    def learn(self, num_epochs: int = 2000, batch_size: int = 50, minibatch_size: int = 100,
+              num_start_steps: int = 10000, num_steps_before_update: int = 1000, num_train_steps: int = 50,
+              num_evaluation_episodes: int = 5, evaluation_interval: int = 4000, model_saving_interval: int = 4000,
+              output_dir: str = ".") -> None:
+        _learn(self, num_epochs, batch_size, minibatch_size, num_start_steps, num_steps_before_update, num_train_steps,
+               num_evaluation_episodes, evaluation_interval, model_saving_interval, output_dir)
+
+    def _record_train(self, out) -> None:
+        mm, steps = getattr(self, "metrics_manager", None), getattr(self, "current_total_steps", 0)
+        if mm is None or out is None:
+            return
+        q = out["q1_values"].astype(np.float64)  # DDPG's critic tags
+        mm.record_scalar("q-function/average_loss", float(np.mean(out["q1_losses"])), steps, tensorboard=True)
+        mm.record_scalar("q-function/avarage_q-value", float(np.mean(q)), steps, tensorboard=True)
+        mm.record_scalar("q-function/max_q-value", float(np.max(q)))
+        mm.record_scalar("q-function/min_q-value", float(np.min(q)))
+        mm.record_scalar("exploration/epsilon", self.epsilon(), steps, tensorboard=True)
+
+    def save_model(self, current_epoch: int, model_path: str) -> None:
+        torch.save({
+            "epoch": current_epoch, "total_steps": getattr(self, "current_total_steps", 0),
+            "q_function_state_dict": self.q_function.network.state_dict(),
+            "q_function_optimizer_state_dict": self.q_function.optimizer.state_dict(),
+            "target_q_function_state_dict": self.target_q_function.network.state_dict(),
+        }, model_path)
+
+    def load_model(self, model_path: str, trust_checkpoint: bool = False) -> int:
+        """Resume from a checkpoint written by ``save_model``: the Q network, its Adam state (and so the step count
+        the target-copy schedule follows), the target network and the step total; returns the saved epoch."""
+        ckpt = torch.load(model_path, map_location="cpu", weights_only=not trust_checkpoint)
+        self.q_function.network.load_state_dict(ckpt["q_function_state_dict"])
+        self.q_function.optimizer.load_state_dict(ckpt["q_function_optimizer_state_dict"])
+        self.target_q_function.network.load_state_dict(ckpt["target_q_function_state_dict"])
+        self.current_total_steps = int(ckpt.get("total_steps", 0))
+        return int(ckpt.get("epoch", 0))

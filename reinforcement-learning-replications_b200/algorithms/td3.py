@@ -23,6 +23,7 @@ logger = logging.getLogger(__name__)
 class _OffPolicyBase:
     n_q = 1
     algo = OffPolicyEngine.TD3  # the engine's step program (DDPG / TD3 by n_q, or SAC)
+    trainable_slots = (0, 1, 2)  # engine network (and optimizer) index of each trainable network, _trainable() order
     target_slots = (3, 4, 5)    # engine network index of each target network
     use_device_replay = True  # replay columns mirrored in HBM, minibatches gathered on the device (SURVEY 8f-4)
     use_device_rng = False    # opt-in: indices and target-smoothing noise drawn on the device (Philox) instead of with
@@ -84,7 +85,7 @@ class _OffPolicyBase:
         blob = e.state_buffer()
         assert blob.numel() == total * getattr(e, "K", 1)
         blob_np = blob.numpy()[lane * total:(lane + 1) * total]  # shares the page-locked memory
-        mods = {i: (m, l) for i, (m, l) in enumerate(zip(trainable, lins))}
+        mods = {i: (m, l) for i, m, l in zip(self.trainable_slots, trainable, lins)}
         mods.update({k: (m, l) for k, m, l in zip(self.target_slots, targets, lins[len(trainable):])})
         slots = []
         for kind, i, off, count in layout:
@@ -117,10 +118,10 @@ class _OffPolicyBase:
     def _fill_state(self, slots, trainable, lins):
         """Host modules and Adam states -> this learner's part of the blob; returns its [3] Adam step counts."""
         steps = [0, 0, 0]
-        for i, (m, l) in enumerate(zip(trainable, lins)):
+        for i, m, l in zip(self.trainable_slots, trainable, lins):
             adam_hparams(m.optimizer, l, "optimizer")  # refuses anything but a plain Adam over exactly this network
             steps[i] = self._adam_step_count(m.optimizer, l)
-        index = {id(m): i for i, m in enumerate(trainable)}
+        index = {id(m): i for i, m in zip(self.trainable_slots, trainable)}
         for kind, p_, m, view in slots:
             if kind == "params":
                 src = p_.detach()
@@ -140,7 +141,7 @@ class _OffPolicyBase:
 
     def _read_state(self, slots, trainable, steps) -> None:
         """This learner's part of the blob -> host modules and Adam states."""
-        index = {id(m): i for i, m in enumerate(trainable)}
+        index = {id(m): i for i, m in zip(self.trainable_slots, trainable)}
         for kind, p_, m, view in slots:
             if kind == "params":
                 np.copyto(p_.detach().numpy(), view, casting="same_kind")
@@ -382,7 +383,7 @@ def _make_eval_env(env):
 
 def _learn(self, num_epochs, batch_size, minibatch_size, num_start_steps, num_steps_before_update, num_train_steps,
            num_evaluation_episodes, evaluation_interval, model_saving_interval, output_dir) -> None:
-    """Shared host loop of TD3.learn / DDPG.learn / SAC.learn (ref: td3.py:94-212, ddpg.py:85-193).  One epoch is three
+    """Shared host loop of TD3.learn / DDPG.learn / SAC.learn / DQN.learn (ref: td3.py:94-212, ddpg.py:85-193).  One epoch is three
     phases (sample, train, evaluate and save), which LearnerGroup.learn runs in lockstep for its learners."""
     started = _learn_begin(self, output_dir)
     for epoch in range(1, num_epochs + 1):

@@ -26,3 +26,11 @@ class QFunction(_Critic):
     def forward(self, observation: Tensor, action: Tensor) -> Tensor:
         joint = torch.cat((observation, action), dim=-1)
         return self.network(joint).squeeze(-1)
+
+
+class DiscreteQFunction(_Critic):
+    """Q(s, .) for a discrete action space: the network maps an observation to one value per action, [..., n]
+    (DQN's critic)."""
+
+    def forward(self, observation: Tensor) -> Tensor:
+        return self.network(observation)

@@ -18,6 +18,8 @@
 // instantiation that serves all of them in one launch; a K = 1 engine runs the solo instantiations.
 // SAC (config algo = 1) is a second step program on the same engine: its head / soft-loss / temperature kernels and
 // enqueue_sac_steps, run as a captured graph or as plain launches like the TD3 / DDPG steps.
+// DQN (config algo = 2) is a third: a per-row Huber loss head on discrete actions (dqn_loss_kernel), a target copy
+// gated by a per-learner step table (dqn_target_copy_kernel) and enqueue_dqn_steps; networks 1 and 4 only.
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -527,6 +529,85 @@ __global__ void __launch_bounds__(GTHREADS) sac_alpha_step_kernel(const float* l
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// DQN (algo = 2; Mnih et al. 2015, Double DQN: van Hasselt et al. 2016).  The Q network maps obs -> [n] values; the
+// action column holds the action index as float32.
+// ---------------------------------------------------------------------------------------------------------------
+// index of the largest of q[0..n) as torch.argmax takes it: a NaN wins (the first NaN), ties go to the first index
+__device__ __forceinline__ int argmax_row(const float* q, int n) {
+  int best = 0;
+  float bv = q[0];
+  for (int j = 1; j < n && !isnan(bv); ++j) {
+    const float v = q[j];
+    if (isnan(v) || v > bv) bv = v, best = j;
+  }
+  return best;
+}
+
+// One CTA: per row i with action a = act[i]
+//   v = Q_targ(s')[i, argmax_j Q(s')[i, j]] (Double DQN: qn != NULL) or max_j Q_targ(s')[i, j],
+//   y = r + gamma (1 - d) v (td_target's order), delta = Q(s)[i, a] - y,
+//   loss = mean(0.5 delta^2 if |delta| < 1 else |delta| - 0.5)  (F.smooth_l1_loss, beta = 1),
+//   dOut[i, :] = 0 except dOut[i, a] = clamp(delta, -1, 1) / B, q_copy[i] = Q(s)[i, a] (the logged Q-value).
+// A row whose action is not an integer in [0, n) is never used as an index: it adds nothing to the loss or dOut, logs
+// NaN, and is counted in *bad_out (0 when every action is valid).
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) dqn_loss_kernel(const float* q, const float* qt_next, const float* qn,
+                                                           const float* act, const float* rew, const float* done,
+                                                           float gamma, int B, int n, float* dout, float* loss_out,
+                                                           float* q_copy, int* bad_out, size_t lane_stride) {
+  __shared__ double red[32];
+  __shared__ int bad_rows;
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q = lane_ptr(q, o), qt_next = lane_ptr(qt_next, o), qn = lane_ptr(qn, o), act = lane_ptr(act, o);
+    rew = lane_ptr(rew, o), done = lane_ptr(done, o), dout = lane_ptr(dout, o), loss_out = lane_ptr(loss_out, o);
+    q_copy = lane_ptr(q_copy, o), bad_out = lane_ptr(bad_out, o);
+  }
+  if (threadIdx.x == 0) bad_rows = 0;
+  __syncthreads();
+  const float inv = 1.0f / (float)B;
+  double acc = 0.0;
+  int bad = 0;
+  for (int i = threadIdx.x; i < B; i += blockDim.x) {
+    const float af = act[i];
+    const bool valid = af >= 0.f && af < (float)n && af == floorf(af);  // false for NaN
+    const int a = valid ? (int)af : -1;
+    float g = 0.f;
+    if (valid) {
+      const float* tn = qt_next + (size_t)i * n;
+      const float v = qn != nullptr ? tn[argmax_row(qn + (size_t)i * n, n)] : tn[argmax_row(tn, n)];
+      const float qi = q[(size_t)i * n + a];
+      const float d = qi - td_target(rew[i], done[i], v, nullptr, i, gamma);
+      const float ad = fabsf(d);
+      acc += ad < 1.f ? 0.5 * (double)d * (double)d : (double)ad - 0.5;
+      g = (d > 1.f ? 1.f : (d < -1.f ? -1.f : d)) * inv;  // NaN passes through, as torch's clamp lets it
+      q_copy[i] = qi;
+    } else {
+      q_copy[i] = __int_as_float(0x7fc00000);
+      ++bad;
+    }
+    for (int j = 0; j < n; ++j) dout[(size_t)i * n + j] = j == a ? g : 0.f;
+  }
+  if (bad) atomicAdd(&bad_rows, bad);
+  block_mean(acc, B, loss_out, red);  // its __syncthreads orders every thread's atomicAdd before thread 0 reads
+  if (threadIdx.x == 0) *bad_out = bad_rows;
+}
+
+// target <- param on the steps the copy table marks (flags[idx].x != 0): the graph launches the copy every step and
+// the host decides per learner, from its Q optimizer's step count, which steps it takes effect on
+template <bool LANES>
+__global__ void dqn_target_copy_kernel(float* target, const float* param, int n, const float2* flags, int idx,
+                                       size_t lane_stride) {
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    target = lane_ptr(target, o), param = lane_ptr(param, o), flags = lane_ptr(flags, o);
+  }
+  if (flags[idx].x == 0.f) return;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) target[i] = param[i];
+}
+
 }  // namespace b200rl
 
 using namespace b200rl;
@@ -592,6 +673,12 @@ struct b200rl_offpolicy {
   float* sac_state = nullptr;                               // {log_alpha, exp_avg, exp_avg_sq}
   float* out_logp = nullptr;                                // [max_steps] mean log pi of each policy step
   int64_t alpha_step[B200RL_MAX_LEARNERS] = {};
+  // DQN (cfg.algo == 2): networks 1 (Q) and 4 (target Q) only; the action column is 1 wide (the index as float32);
+  // adam_tab row 3 holds the target-copy flags of the call's steps
+  bool dqn = false, dqn_set = false;
+  b200rl_dqn_hparams dqn_hp{}, graph_dqn_hp{};
+  float* dqn_dout = nullptr;  // [B, n] gradient w.r.t. the Q output
+  int* dqn_bad = nullptr;     // [max_steps] rows of each step whose action was not a valid index
   std::vector<void*> allocs;
 };
 
@@ -742,19 +829,26 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
   B200RL_REQUIRE(n_learners >= 1 && n_learners <= B200RL_MAX_LEARNERS,
                  "offpolicy_create_group: n_learners must be 1..%d, got %d", B200RL_MAX_LEARNERS, n_learners);
   B200RL_REQUIRE(cfg->n_q == 1 || cfg->n_q == 2, "offpolicy_create: n_q must be 1 (DDPG) or 2 (TD3)");
-  B200RL_REQUIRE(cfg->algo == 0 || cfg->algo == 1, "offpolicy_create: algo must be 0 (DDPG / TD3) or 1 (SAC), got %d",
-                 cfg->algo);
-  const bool sac = cfg->algo == 1;
+  B200RL_REQUIRE(cfg->algo >= 0 && cfg->algo <= 2,
+                 "offpolicy_create: algo must be 0 (DDPG / TD3), 1 (SAC) or 2 (DQN), got %d", cfg->algo);
+  const bool sac = cfg->algo == 1, dqn = cfg->algo == 2;
   B200RL_REQUIRE(!sac || cfg->n_q == 2, "offpolicy_create: SAC needs n_q = 2 (twin soft critics), got %d", cfg->n_q);
+  B200RL_REQUIRE(!dqn || cfg->n_q == 1, "offpolicy_create: DQN needs n_q = 1 (one Q network), got %d", cfg->n_q);
   B200RL_REQUIRE(cfg->max_minibatch >= 1 && cfg->max_minibatch <= 65536 && cfg->max_steps >= 1,
                  "offpolicy_create: bad capacities");
-  const int64_t Pp = b200rl_mlp_param_count(&cfg->policy), Pq = b200rl_mlp_param_count(&cfg->q);
-  B200RL_REQUIRE(Pp > 0 && Pq > 0, "offpolicy_create: invalid MLP description");
-  const int O = cfg->policy.sizes[0], P_out = cfg->policy.sizes[cfg->policy.n_layers];
-  const int A = sac ? cfg->q.sizes[0] - O : P_out;  // SAC: the policy outputs [mean | log_std], 2A wide
+  if (dqn) {
+    const b200rl_mlp_desc zero{};
+    B200RL_REQUIRE(memcmp(&cfg->policy, &zero, sizeof(zero)) == 0,
+                   "offpolicy_create: DQN has no policy network: the policy description must be zeroed");
+  }
+  const int64_t Pp = dqn ? 0 : b200rl_mlp_param_count(&cfg->policy), Pq = b200rl_mlp_param_count(&cfg->q);
+  B200RL_REQUIRE((dqn || Pp > 0) && Pq > 0, "offpolicy_create: invalid MLP description");
+  const int O = dqn ? cfg->q.sizes[0] : cfg->policy.sizes[0], P_out = cfg->policy.sizes[cfg->policy.n_layers];
+  // SAC: the policy outputs [mean | log_std], 2A wide; DQN: the action column holds the index (1 wide)
+  const int A = dqn ? 1 : sac ? cfg->q.sizes[0] - O : P_out;
   B200RL_REQUIRE(!sac || (A >= 1 && P_out == 2 * A),
                  "offpolicy_create: the SAC policy must output [mean | log_std] = 2 x %d values, got %d", A, P_out);
-  B200RL_REQUIRE(cfg->q.sizes[0] == O + A && cfg->q.sizes[cfg->q.n_layers] == 1,
+  B200RL_REQUIRE(dqn || (cfg->q.sizes[0] == O + A && cfg->q.sizes[cfg->q.n_layers] == 1),
                  "offpolicy_create: Q network must map [obs %d + act %d] -> 1", O, A);
   B200RL_REQUIRE(device_sm_count() > 0, "offpolicy_create: no CUDA device");
   b200rl_offpolicy* h = new b200rl_offpolicy();
@@ -763,6 +857,7 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
   h->O = O;
   h->A = A;
   h->sac = sac;
+  h->dqn = dqn;
   int rc = 0;
   int maxw = O + A;
   for (int i = 0; i < 6; ++i) {
@@ -779,6 +874,7 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
     }
     if (cfg->n_q == 1 && (i == 2 || i == 5)) continue;
     if (sac && i == 3) continue;  // SAC has no target policy
+    if (dqn && (i == 0 || i == 3)) continue;  // DQN has no policy
     nb.present = true;
     if (i < 3) rc |= oalloc(h, &nb.grad, (size_t)nb.P);
   }
@@ -819,7 +915,7 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
   rc |= oalloc(h, &h->out_l1, S);
   rc |= oalloc(h, &h->out_l2, S);
   rc |= oalloc(h, &h->out_lp, S);
-  const size_t n_tab = sac ? 4 : 3;  // SAC: a fourth row for log_alpha's optimizer
+  const size_t n_tab = sac || dqn ? 4 : 3;  // SAC: a fourth row for log_alpha's optimizer; DQN: the copy flags
   rc |= oalloc(h, &h->adam_tab, n_tab * S);
   rc |= oalloc(h, &h->idx, S * B);
   if (sac) {
@@ -831,6 +927,10 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
     rc |= oalloc(h, &h->sac_alpha, S + 1);
     rc |= oalloc(h, &h->sac_state, 3);
     rc |= oalloc(h, &h->out_logp, S);
+  }
+  if (dqn) {
+    rc |= oalloc(h, &h->dqn_dout, B * (size_t)cfg->q.sizes[cfg->q.n_layers]);
+    rc |= oalloc(h, &h->dqn_bad, S);
   }
   rc |= arena_commit(h);
   if (rc == 0) {
@@ -976,6 +1076,17 @@ extern "C" int b200rl_offpolicy_set_sac(b200rl_offpolicy* h, const b200rl_sac_hp
   h->sac_hp = *sp;
   h->sac_hp.reserved = 0;  // part of the graph cache key
   h->sac_set = true;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hparams* dp) {
+  B200RL_REQUIRE(h && dp, "offpolicy_set_dqn: NULL argument");
+  B200RL_REQUIRE(h->dqn, "offpolicy_set_dqn: the engine was not created with algo = 2 (DQN)");
+  B200RL_REQUIRE(dp->target_update_interval >= 1, "offpolicy_set_dqn: target_update_interval must be >= 1, got %d",
+                 dp->target_update_interval);
+  B200RL_REQUIRE(dp->double_q == 0 || dp->double_q == 1, "offpolicy_set_dqn: double_q must be 0 or 1");
+  h->dqn_hp = *dp;
+  h->dqn_set = true;
   return 0;
 }
 
@@ -1284,6 +1395,69 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
   return 0;
 }
 
+// The S DQN steps.  Per step:
+//   s  : Q_targ(s') ---------------+-> loss -> dX chain -> Adam(Q) -> target copy (on the steps the flag table marks)
+//   s2 : Q(s') (Double DQN only) --+
+//   s3 : Q(s) ---------------------+   ........ Q's dW products
+// Q(s') reads the parameters at the start of the step: the step's Adam waits for the loss kernel, which joins it.
+static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s) {
+  const int O = h->O;
+  const int maxS = h->cfg.max_steps;
+  const bool dbl = h->dqn_hp.double_q != 0;
+  NetBuf &q = h->net[1], &qt = h->net[4];
+  const int L = q.d.n_layers, n = q.d.sizes[L];
+  const int ew = 256;
+  cudaStream_t s2 = h->s2, s3 = h->s3;
+  auto edge = [&](cudaStream_t from, cudaStream_t to) -> int {
+    B200RL_CUDA(cudaEventRecord(h->ev_fork, from));
+    B200RL_CUDA(cudaStreamWaitEvent(to, h->ev_fork, 0));
+    return 0;
+  };
+  for (int st = 0; st < S; ++st) {
+    const float* s_obs = h->obs + (size_t)st * B * O;
+    const float* s_act = h->act + (size_t)st * B;
+    const float* s_rew = h->rew + (size_t)st * B;
+    const float* s_nobs = h->nobs + (size_t)st * B * O;
+    const float* s_done = h->done + (size_t)st * B;
+    float* qa[B200RL_MAX_LAYERS + 1];  // Q(s): its stack is what the backward pass reads
+    qa[0] = const_cast<float*>(s_obs);
+    for (int l = 1; l <= L; ++l) qa[l] = h->acts[1][l];
+    if (edge(s, s3)) return 1;
+    if (net_forward(h, q, qa, B, s3)) return 1;
+    float* qn[B200RL_MAX_LAYERS + 1];
+    if (dbl) {
+      qn[0] = const_cast<float*>(s_nobs);
+      for (int l = 1; l <= L; ++l) qn[l] = h->acts[3][l];
+      if (edge(s, s2)) return 1;
+      if (net_forward(h, q, qn, B, s2)) return 1;
+    }
+    float* tq[B200RL_MAX_LAYERS + 1];
+    tq[0] = const_cast<float*>(s_nobs);
+    for (int l = 1; l <= L; ++l) tq[l] = h->acts_tq[l];
+    if (net_forward(h, qt, tq, B, s)) return 1;
+    if (dbl && edge(s2, s)) return 1;
+    if (edge(s3, s)) return 1;
+    LAUNCH_LANES(h, dqn_loss_kernel, 1, GTHREADS, s, qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done,
+                 (float)hp->gamma, B, n, h->dqn_dout, h->out_l1 + st, h->out_q1 + (size_t)st * B, h->dqn_bad + st);
+    B200RL_CUDA(cudaGetLastError());
+    count_launch(1);
+    if (net_backward(h, q, qa, h->dqn_dout, n, B, true, nullptr, s, false, nullptr, 0, 0, s3)) return 1;
+    if (adam_net(h, q, h->adam_tab + (size_t)maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, s)) return 1;
+    LAUNCH_LANES(h, dqn_target_copy_kernel, (unsigned)((q.P + ew - 1) / ew), ew, s, qt.params, q.params, (int)q.P,
+                 h->adam_tab + (size_t)3 * maxS, st);
+    B200RL_CUDA(cudaGetLastError());
+    count_launch(1);
+  }
+  return 0;
+}
+
+// DQN engines: b200rl_offpolicy_set_dqn must have been called
+static int dqn_ready(const b200rl_offpolicy* h, const char* what) {
+  if (!h->dqn) return 0;
+  B200RL_REQUIRE(h->dqn_set, "%s: a DQN engine needs b200rl_offpolicy_set_dqn before it trains", what);
+  return 0;
+}
+
 // SAC engines: b200rl_offpolicy_set_sac must have been called, and the host paths must hand over the [S, 2, B, A] draws
 static int sac_ready(const b200rl_offpolicy* h, bool noise_given, const char* what) {
   if (!h->sac) return 0;
@@ -1303,8 +1477,8 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   // Adam's step-dependent scalars for the steps of this call (torch's host-side double arithmetic), one small upload
   // (a group: one table per learner, from that learner's step counts, uploaded with one strided copy)
   const int maxS = h->cfg.max_steps;
-  const int n_pol_expected = h->sac ? S : (S + hp->policy_delay - 1) / hp->policy_delay;  // SAC: no delay
-  const size_t tab_n = (h->sac ? 4 : 3) * (size_t)maxS;
+  const int n_pol_expected = h->dqn ? 0 : h->sac ? S : (S + hp->policy_delay - 1) / hp->policy_delay;  // SAC: no delay
+  const size_t tab_n = (h->sac || h->dqn ? 4 : 3) * (size_t)maxS;
   const bool learn_alpha = h->sac && h->sac_hp.learn_alpha;
   for (int z = 0; z < h->K; ++z) {
     float2* tab = h->h_adam_tab + z * tab_n;
@@ -1318,6 +1492,9 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
       for (int k = 0; k < S; ++k)
         adam_scalars(h->alpha_step[z] + k + 1, h->sac_hp.alpha_lr, h->sac_hp.alpha_beta1, h->sac_hp.alpha_beta2,
                      &tab[(size_t)3 * maxS + k].x, &tab[(size_t)3 * maxS + k].y);
+    if (h->dqn)  // copy after the steps that bring the Q optimizer's count to a multiple of the interval
+      for (int k = 0; k < S; ++k)
+        tab[(size_t)3 * maxS + k] = make_float2((h->net[1].step[z] + k + 1) % h->dqn_hp.target_update_interval == 0, 0.f);
   }
   B200RL_CUDA(cudaMemcpy2DAsync(h->adam_tab, h->lane_stride, h->h_adam_tab, tab_n * sizeof(float2),
                                 tab_n * sizeof(float2), h->K, cudaMemcpyHostToDevice, s));
@@ -1329,12 +1506,15 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
     if (h->sac) {
       if (enqueue_sac_steps(h, hp, S, B, s)) return 1;
       n_pol = S;
+    } else if (h->dqn) {
+      if (enqueue_dqn_steps(h, hp, S, B, s)) return 1;
     } else if (enqueue_steps(h, hp, S, B, s, &n_pol)) {
       return 1;
     }
   } else {
     if (h->graph == nullptr || h->graph_S != S || h->graph_B != B || memcmp(&h->graph_hp, hp, sizeof(*hp)) != 0 ||
-        memcmp(&h->graph_sac_hp, &h->sac_hp, sizeof(h->sac_hp)) != 0) {
+        memcmp(&h->graph_sac_hp, &h->sac_hp, sizeof(h->sac_hp)) != 0 ||
+        memcmp(&h->graph_dqn_hp, &h->dqn_hp, sizeof(h->dqn_hp)) != 0) {
       if (h->graph) {
         cudaGraphExecDestroy(h->graph);
         h->graph = nullptr;
@@ -1345,6 +1525,8 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
       if (h->sac) {
         rc = enqueue_sac_steps(h, hp, S, B, s);
         n_pol = S;
+      } else if (h->dqn) {
+        rc = enqueue_dqn_steps(h, hp, S, B, s);
       } else {
         rc = enqueue_steps(h, hp, S, B, s, &n_pol);
       }
@@ -1368,6 +1550,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
       h->graph_B = B;
       h->graph_hp = *hp;
       h->graph_sac_hp = h->sac_hp;
+      h->graph_dqn_hp = h->dqn_hp;
       h->graph_npol = n_pol;
     }
     n_pol = h->graph_npol;
@@ -1391,8 +1574,15 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   if (n_pol > 0)
     B200RL_CUDA(cudaMemcpy2DAsync(policy_losses, (size_t)S * 4, h->out_lp, ls, (size_t)n_pol * 4, K,
                                   cudaMemcpyDeviceToHost, s));
+  std::vector<int> bad(h->dqn ? K * S : 0);
+  if (h->dqn)
+    B200RL_CUDA(cudaMemcpy2DAsync(bad.data(), (size_t)S * 4, h->dqn_bad, ls, (size_t)S * 4, K, cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaStreamSynchronize(s));
   *n_policy_updates = n_pol;
+  for (size_t i = 0; i < bad.size(); ++i)
+    B200RL_REQUIRE(bad[i] == 0, "offpolicy_train: DQN learner %d, step %d: %d minibatch rows hold an action that is not "
+                   "an integer in [0, %d); those rows were left out of the update", (int)(i / S), (int)(i % S), bad[i],
+                   h->net[1].d.sizes[h->net[1].d.n_layers]);
   return 0;
 }
 
@@ -1401,15 +1591,15 @@ extern "C" int b200rl_offpolicy_train(b200rl_offpolicy* h, const b200rl_offpolic
                                       const float* done, const float* noise, float* q1_values, float* q2_values,
                                       float* q1_losses, float* q2_losses, float* policy_losses,
                                       int32_t* n_policy_updates, void* stream) {
-  B200RL_REQUIRE(h && hp && obs && act && rew && next_obs && done && q1_values && q1_losses && policy_losses &&
-                     n_policy_updates, "offpolicy_train: NULL argument");
+  B200RL_REQUIRE(h && hp && obs && act && rew && next_obs && done && q1_values && q1_losses &&
+                     (policy_losses || h->dqn) && n_policy_updates, "offpolicy_train: NULL argument");
   B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
                  "offpolicy_train: S=%d B=%d exceed the capacities", S, B);
   const bool td3 = h->cfg.n_q == 2;
   B200RL_REQUIRE(!td3 || (q2_values && q2_losses), "offpolicy_train: TD3 needs the Q2 outputs");
-  B200RL_REQUIRE(!hp->use_target_noise || noise, "offpolicy_train: target noise requested but no noise given");
-  B200RL_REQUIRE(hp->policy_delay >= 1, "offpolicy_train: policy_delay must be >= 1");
-  if (sac_ready(h, noise != nullptr, "offpolicy_train")) return 2;
+  B200RL_REQUIRE(h->dqn || !hp->use_target_noise || noise, "offpolicy_train: target noise requested but no noise given");
+  B200RL_REQUIRE(h->dqn || hp->policy_delay >= 1, "offpolicy_train: policy_delay must be >= 1");
+  if (sac_ready(h, noise != nullptr, "offpolicy_train") || dqn_ready(h, "offpolicy_train")) return 2;
   cudaStream_t user = static_cast<cudaStream_t>(stream);
   cudaStream_t s = h->gs;  // everything runs on the engine's stream, ordered after the caller's
   const int O = h->O, A = h->A;
@@ -1427,7 +1617,7 @@ extern "C" int b200rl_offpolicy_train(b200rl_offpolicy* h, const b200rl_offpolic
       up(h->nobs, next_obs, SB * O * 4) || up(h->done, done, SB * 4))
     return 1;
   if (h->sac && up(h->eps, noise, 2 * SB * A * 4)) return 1;
-  if (!h->sac && hp->use_target_noise && up(h->eps, noise, SB * A * 4)) return 1;
+  if (!h->sac && !h->dqn && hp->use_target_noise && up(h->eps, noise, SB * A * 4)) return 1;
 
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
 }
@@ -1471,16 +1661,17 @@ extern "C" int b200rl_offpolicy_train_gather_group(b200rl_offpolicy* h, const b2
                                                    const float* noise, float* q1_values, float* q2_values,
                                                    float* q1_losses, float* q2_losses, float* policy_losses,
                                                    int32_t* n_policy_updates, void* stream) {
-  B200RL_REQUIRE(h && hp && idx && q1_values && q1_losses && policy_losses && n_policy_updates,
+  B200RL_REQUIRE(h && hp && idx && q1_values && q1_losses && (policy_losses || h->dqn) && n_policy_updates,
                  "offpolicy_train_gather: NULL argument");
   if (int rc = check_replay(h, rb, "offpolicy_train_gather")) return rc;
   B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
                  "offpolicy_train_gather: S=%d B=%d exceed the capacities", S, B);
   const bool td3 = h->cfg.n_q == 2;
   B200RL_REQUIRE(!td3 || (q2_values && q2_losses), "offpolicy_train_gather: TD3 needs the Q2 outputs");
-  B200RL_REQUIRE(!hp->use_target_noise || noise, "offpolicy_train_gather: target noise requested but no noise given");
-  B200RL_REQUIRE(hp->policy_delay >= 1, "offpolicy_train_gather: policy_delay must be >= 1");
-  if (sac_ready(h, noise != nullptr, "offpolicy_train_gather")) return 2;
+  B200RL_REQUIRE(h->dqn || !hp->use_target_noise || noise,
+                 "offpolicy_train_gather: target noise requested but no noise given");
+  B200RL_REQUIRE(h->dqn || hp->policy_delay >= 1, "offpolicy_train_gather: policy_delay must be >= 1");
+  if (sac_ready(h, noise != nullptr, "offpolicy_train_gather") || dqn_ready(h, "offpolicy_train_gather")) return 2;
   const size_t SB = (size_t)S * B;
   for (int z = 0; z < h->K; ++z)
     for (size_t i = 0; i < SB; ++i)
@@ -1497,7 +1688,7 @@ extern "C" int b200rl_offpolicy_train_gather_group(b200rl_offpolicy* h, const b2
   // the minibatches are gathered on the device from the replay columns: only the indices (and noise) cross PCIe
   const size_t ls = h->lane_stride;
   B200RL_CUDA(cudaMemcpy2DAsync(h->idx, ls, idx, SB * 8, SB * 8, h->K, cudaMemcpyHostToDevice, s));
-  const size_t n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise ? SB * A : 0);
+  const size_t n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise && !h->dqn ? SB * A : 0);
   if (n_eps) B200RL_CUDA(cudaMemcpy2DAsync(h->eps, ls, noise, n_eps * 4, n_eps * 4, h->K, cudaMemcpyHostToDevice, s));
   if (gather_columns(h, rb, (long long)SB, s)) return 1;
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
@@ -1526,8 +1717,8 @@ extern "C" int b200rl_offpolicy_train_gather_rng_group(b200rl_offpolicy* h, cons
                                                        const uint64_t* seed, const uint64_t* call, float* q1_values,
                                                        float* q2_values, float* q1_losses, float* q2_losses,
                                                        float* policy_losses, int32_t* n_policy_updates, void* stream) {
-  B200RL_REQUIRE(h && hp && ring_start && ring_size && seed && call && q1_values && q1_losses && policy_losses &&
-                     n_policy_updates, "offpolicy_train_gather_rng: NULL argument");
+  B200RL_REQUIRE(h && hp && ring_start && ring_size && seed && call && q1_values && q1_losses &&
+                     (policy_losses || h->dqn) && n_policy_updates, "offpolicy_train_gather_rng: NULL argument");
   if (int rc = check_replay(h, rb, "offpolicy_train_gather_rng")) return rc;
   B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
                  "offpolicy_train_gather_rng: S=%d B=%d exceed the capacities", S, B);
@@ -1539,8 +1730,8 @@ extern "C" int b200rl_offpolicy_train_gather_rng_group(b200rl_offpolicy* h, cons
   }
   const bool td3 = h->cfg.n_q == 2;
   B200RL_REQUIRE(!td3 || (q2_values && q2_losses), "offpolicy_train_gather_rng: TD3 needs the Q2 outputs");
-  B200RL_REQUIRE(hp->policy_delay >= 1, "offpolicy_train_gather_rng: policy_delay must be >= 1");
-  if (sac_ready(h, true, "offpolicy_train_gather_rng")) return 2;
+  B200RL_REQUIRE(h->dqn || hp->policy_delay >= 1, "offpolicy_train_gather_rng: policy_delay must be >= 1");
+  if (sac_ready(h, true, "offpolicy_train_gather_rng") || dqn_ready(h, "offpolicy_train_gather_rng")) return 2;
   cudaStream_t user = static_cast<cudaStream_t>(stream);
   cudaStream_t s = h->gs;
   const int A = h->A;
@@ -1549,7 +1740,7 @@ extern "C" int b200rl_offpolicy_train_gather_rng_group(b200rl_offpolicy* h, cons
   if (S == 0) return 0;
   B200RL_CUDA(cudaEventRecord(h->ev, user));
   B200RL_CUDA(cudaStreamWaitEvent(s, h->ev, 0));
-  const long long n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise ? SB * A : 0);
+  const long long n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise && !h->dqn ? SB * A : 0);  // DQN: indices only
   const long long n_thr = ((SB > n_eps ? SB : n_eps) + 3) / 4;
   const dim3 grid((unsigned)((n_thr + 255) / 256));
   if (h->K == 1) {

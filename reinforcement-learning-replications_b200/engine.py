@@ -319,16 +319,18 @@ class OnPolicyEngine:
 
 
 class OffPolicyEngine:
-    """Device-resident state of one DDPG / TD3 (``algo`` 0) or SAC (``algo`` 1) learner (C ABI: b200rl_offpolicy_*).
-    SAC: ``n_q`` = 2, the policy maps obs -> [mean | log_std] (2A outputs), there is no target policy (network 3), and
-    ``set_sac`` must be called before the first train call.
+    """Device-resident state of one DDPG / TD3 (``algo`` 0), SAC (``algo`` 1) or DQN (``algo`` 2) learner (C ABI:
+    b200rl_offpolicy_*).  SAC: ``n_q`` = 2, the policy maps obs -> [mean | log_std] (2A outputs), there is no target
+    policy (network 3), and ``set_sac`` must be called before the first train call.  DQN: ``policy_sizes`` = None,
+    ``n_q`` = 1, the Q network maps obs -> [n actions], only networks 1 (Q) and 4 (target Q) exist, actions are indices
+    (act [S,B]), and ``set_dqn`` must be called before the first train call.
 
     ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
     launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
     is [K][per-learner blob] with [K][3] step counts, and the per-network accessors are refused."""
 
     NETS = {"policy": 0, "q1": 1, "q2": 2, "target_policy": 3, "target_q1": 4, "target_q2": 5}
-    TD3, SAC = 0, 1
+    TD3, SAC, DQN = 0, 1, 2
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
                  q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1):
@@ -336,15 +338,16 @@ class OffPolicyEngine:
         self.lib = _lib.load()
         current_stream_handle()
         cfg = OffPolicyConfig()
-        cfg.policy = MlpDesc.make(policy_sizes, *policy_acts)
+        if policy_sizes is not None:  # DQN: no policy, the description stays zeroed
+            cfg.policy = MlpDesc.make(policy_sizes, *policy_acts)
         cfg.q = MlpDesc.make(q_sizes, *q_acts)
         cfg.n_q, cfg.max_minibatch, cfg.max_steps = int(n_q), int(max_minibatch), int(max_steps)
         cfg.algo = int(algo)
         self.algo = int(algo)
         self.n_q, self.max_minibatch, self.max_steps = int(n_q), int(max_minibatch), int(max_steps)
-        self.policy_sizes, self.q_sizes = list(policy_sizes), list(q_sizes)
+        self.policy_sizes, self.q_sizes = None if policy_sizes is None else list(policy_sizes), list(q_sizes)
         self.policy_acts, self.q_acts = tuple(policy_acts), tuple(q_acts)
-        self.n_policy = int(self.lib.b200rl_mlp_param_count(cfg.policy))
+        self.n_policy = 0 if policy_sizes is None else int(self.lib.b200rl_mlp_param_count(cfg.policy))
         self.n_qp = int(self.lib.b200rl_mlp_param_count(cfg.q))
         self.K = int(n_learners)
         h = C.c_void_p()
@@ -396,13 +399,17 @@ class OffPolicyEngine:
         """[(kind, net index, offset, count)] of one learner's state blob: ("params", 0..5) then ("m" / "v", 0..2);
         every segment starts on a multiple of 64 floats (b200rl.h).  A group's blob is K of these back to back."""
         pad = lambda n: (n + 63) & ~63
-        present = [0, 1] + ([2] if self.n_q == 2 else []) + ([] if self.algo == self.SAC else [3]) + [4] + \
-            ([5] if self.n_q == 2 else [])
+        if self.algo == self.DQN:
+            present, optimized = [1, 4], [1]
+        else:
+            present = [0, 1] + ([2] if self.n_q == 2 else []) + ([] if self.algo == self.SAC else [3]) + [4] + \
+                ([5] if self.n_q == 2 else [])
+            optimized = [0, 1] + ([2] if self.n_q == 2 else [])
         out, off = [], 0
         for i in present:
             out.append(("params", i, off, self._n(i)))
             off += pad(self._n(i))
-        for i in [0, 1] + ([2] if self.n_q == 2 else []):
+        for i in optimized:
             for kind in ("m", "v"):
                 out.append((kind, i, off, self._n(i)))
                 off += pad(self._n(i))
@@ -477,6 +484,13 @@ class OffPolicyEngine:
         check(self.lib.b200rl_offpolicy_get_alpha_group(self.h, _ptr(la), _ptr(m), _ptr(v), _ptr(st)), "get_alpha")
         return [(float(la[z]), float(m[z]), float(v[z]), int(st[z])) for z in range(self.K)]
 
+    # ---- DQN ----
+    def set_dqn(self, target_update_interval: int, double_q: bool) -> None:
+        from ._lib import DqnHparams
+        dp = DqnHparams()
+        dp.target_update_interval, dp.double_q = int(target_update_interval), int(bool(double_q))
+        check(self.lib.b200rl_offpolicy_set_dqn(self.h, C.byref(dp)), "set_dqn")
+
     def sac_outputs(self, S: int):
         """(mean log pi per step [S], alpha used by each step [S]) of the last train call (a group: [K, S] each)."""
         lp, al = np.zeros((self.K, S), np.float32), np.zeros((self.K, S), np.float32)
@@ -490,7 +504,10 @@ class OffPolicyEngine:
 
     def _outputs(self, S, q1v, q2v, l1, l2, lp, npol):
         """The logged quantities; a solo engine drops the leading [K] axis."""
-        out = dict(q1_values=q1v, q2_values=q2v, q1_losses=l1, q2_losses=l2, policy_losses=lp[:, :npol.value])
+        if self.algo == self.DQN:
+            out = dict(q1_values=q1v, q1_losses=l1)
+        else:
+            out = dict(q1_values=q1v, q2_values=q2v, q1_losses=l1, q2_losses=l2, policy_losses=lp[:, :npol.value])
         if self.K == 1:
             out = {k: v[0] for k, v in out.items()}
         if self.algo == self.SAC:
@@ -508,7 +525,10 @@ class OffPolicyEngine:
 
     def train(self, hp, obs, act, rew, next_obs, done, noise=None):
         """obs/next_obs [S,B,O], act [S,B,A], rew/done [S,B], noise [S,B,A] or None (SAC: [S,2,B,A], required) -> dict
-        of logged quantities (SAC adds log_prob_means and alphas).  A group: every array with a leading [K] axis."""
+        of logged quantities (SAC adds log_prob_means and alphas).  A group: every array with a leading [K] axis.
+        DQN: act [S,B] action indices, noise None; the dict holds q1_values and q1_losses."""
+        if self.algo == self.DQN:
+            act = np.asarray(act, np.float32)[..., None]
         obs, act, next_obs = (self._lead(x, np.float32, 4) for x in (obs, act, next_obs))
         rew, done = self._lead(rew, np.float32, 3), self._lead(done, np.float32, 3)
         noise = None if noise is None else self._lead(noise, np.float32, 5 if self.algo == self.SAC else 4)
@@ -542,11 +562,12 @@ class OffPolicyEngine:
         """(physical rows [S,B] int64, noise [S,B,A] (SAC: [S,2,B,A]) float32 or None) of the last train_gather /
         train_gather_rng call; a group: both with a leading [K] axis."""
         idx = np.empty((self.K, S, B), np.int64)
-        if self.algo == self.SAC:
-            shape = (self.K, S, 2, B, self.policy_sizes[-1] // 2)
-        else:
-            shape = (self.K, S, B, self.policy_sizes[-1])
-        noise = np.empty(shape, np.float32) if with_noise else None
+        with_noise = with_noise and self.algo != self.DQN  # DQN draws indices only
+        noise = None
+        if with_noise and self.algo == self.SAC:
+            noise = np.empty((self.K, S, 2, B, self.policy_sizes[-1] // 2), np.float32)
+        elif with_noise:
+            noise = np.empty((self.K, S, B, self.policy_sizes[-1]), np.float32)
         check(self.lib.b200rl_offpolicy_get_draws(self.h, S, B, _ptr(idx), _ptr(noise), current_stream_handle()), "get_draws")
         if self.K == 1:
             return idx[0], None if noise is None else noise[0]

@@ -1,5 +1,5 @@
-from .base import (CategoricalPolicy, DeterministicPolicy, GaussianPolicy, Policy, RandomPolicy,
-                   SquashedGaussianPolicy, StochasticPolicy)
+from .base import (CategoricalPolicy, DeterministicPolicy, EpsilonGreedyPolicy, GaussianPolicy, GreedyPolicy, Policy,
+                   RandomPolicy, SquashedGaussianPolicy, StochasticPolicy)
 
 __all__ = ["Policy", "StochasticPolicy", "CategoricalPolicy", "GaussianPolicy", "SquashedGaussianPolicy",
-           "DeterministicPolicy", "RandomPolicy"]
+           "DeterministicPolicy", "RandomPolicy", "GreedyPolicy", "EpsilonGreedyPolicy"]

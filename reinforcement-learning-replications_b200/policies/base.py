@@ -145,3 +145,44 @@ class RandomPolicy(Policy):
 
     def get_action_numpy(self, observation: np.ndarray) -> np.ndarray:
         return np.asarray(self.action_space.sample())
+
+
+class GreedyPolicy(Policy):
+    """argmax_a Q(s, a) of a DiscreteQFunction (torch.argmax: the first index among equal maxima); DQN's evaluation
+    policy."""
+
+    def __init__(self, q_function: nn.Module) -> None:
+        super().__init__()
+        self.q_function = q_function
+
+    def _greedy(self, observation: Tensor) -> Tensor:
+        with torch.no_grad():
+            return torch.argmax(self.q_function(observation), dim=-1)
+
+    def get_action_tensor(self, observation: Tensor) -> Tensor:
+        return self._greedy(observation)
+
+    def get_action_numpy(self, observation: np.ndarray) -> np.ndarray:
+        return np.asarray(self._greedy(torch.from_numpy(np.asarray(observation, np.float32))).numpy())
+
+
+class EpsilonGreedyPolicy(GreedyPolicy):
+    """With probability ``epsilon`` a uniform action from ``action_space.sample()``, otherwise the greedy action.  Every
+    action draws one ``np.random.random()`` (global NumPy stream), also when it then acts greedily; a batch of
+    observations [N, O] draws one per row, in row order."""
+
+    def __init__(self, q_function: nn.Module, action_space, epsilon: float) -> None:
+        super().__init__(q_function)
+        self.action_space = action_space
+        self.epsilon = float(epsilon)
+
+    def get_action_numpy(self, observation: np.ndarray) -> np.ndarray:
+        observation = np.asarray(observation, np.float32)
+        if observation.ndim == 1:
+            if np.random.random() < self.epsilon:
+                return np.asarray(self.action_space.sample())
+            return np.asarray(self._greedy(torch.from_numpy(observation)).numpy())
+        return np.stack([self.get_action_numpy(o) for o in observation])
+
+    def get_action_tensor(self, observation: Tensor) -> Tensor:
+        return torch.as_tensor(self.get_action_numpy(observation.detach().cpu().numpy()))

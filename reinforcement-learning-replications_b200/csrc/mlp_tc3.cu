@@ -4,18 +4,22 @@
 // Why (reference: /root/reference/src/rl_replicas/algorithms/ppo.py:173-181 policy loop, :186-192 value loop): the two
 // loops touch disjoint parameters and read the same fixed inputs (advantages and returns are computed before either
 // loop, :142-161), so step i of both can share one pass over the batch.  Compared with two mlp_tc2 launches:
-//   * the two tiles ("slots") a CTA keeps in flight are now the POLICY chain and the VALUE chain of the SAME tile:
-//     the observation operand is staged once for both;
+//   * the POLICY chain and the VALUE chain of the SAME tile run side by side, and the observation operand is staged
+//     once for both.  Rows are independent in the forward / backward chain, so each (network, 64-row half) is one
+//     warpgroup that issues its own m64 products and keeps the accumulator in registers: its epilogues work on the
+//     wgmma fragment and hand over to its next product through a warpgroup-local barrier.  A fifth warpgroup brings
+//     the observations in and issues the weight-gradient products (accumulators in L2, tc_common.cuh) off the chains'
+//     critical path; mbarriers tell it when both halves of a network have delivered a stage's operands, and tell the
+//     chains when it has finished reading a buffer they are about to overwrite;
 //   * the observations are split into their fp16 pairs ONCE PER UPDATE by pack_obs_kernel (every step of the update
 //     reads the same observations) into ready-made SWIZZLE_128B tile images [128 rows][h cols 0..31 | l cols 32..63];
 //     the step kernel brings a tile image in with ONE 16 KB bulk copy (cp.async.bulk + mbarrier complete_tx) issued by
-//     the MMA warp a tile ahead -- no epilogue job touches the observations any more (E0 of mlp_tc2 is gone);
+//     the producer warpgroup -- no epilogue touches the observations any more (E0 of mlp_tc2 is gone);
 //   * column 31 of the image is 1.0, so the bias gradients db1 / db2 still fall out of the weight-gradient products;
 //   * dLoss/dOut of both chains goes into the X buffer of the OTHER parity (it is idle between the previous tile's
 //     dW1 and the next tile's bulk copy), which is what makes two X buffers fit next to 4 x 32 KB of activations and
 //     2 x 28 KB of weights;
-//   * tanh'(H1) is taken from the fp16 pair in shared memory like tanh'(H2): no fp32 copy of H1 in accumulator memory,
-//     which is what makes both chains' accumulators fit (416 of 512 columns);
+//   * tanh'(H1) and tanh'(H2) are taken from the fp16 pairs in shared memory: no fp32 copy of H in registers;
 //   * one reduction + Adam launch for both networks (reduce_adam3_kernel), one all-reduce per iteration.
 // A range / precision trip (fp16 operands) raises a sticky flag; the engine then restores its snapshot and redoes the
 // update on the two-loop path whose wide-range kernels have no such limits.
@@ -32,9 +36,9 @@
 namespace b200rl {
 
 constexpr int T3_ROWS = 128;
-constexpr int T3_EPI_WARPS = 16;
-constexpr int T3_EPI_THREADS = T3_EPI_WARPS * 32;
-constexpr int T3_THREADS = T3_EPI_THREADS + 128;  // + the issuing warpgroup
+constexpr int T3_CHAIN_WARPS = 16;  // four chain warpgroups, one per (network, 64-row half of the tile)
+constexpr int T3_CHAIN_THREADS = T3_CHAIN_WARPS * 32;
+constexpr int T3_THREADS = T3_CHAIN_THREADS + 128;  // + the producer / weight-gradient warpgroup
 
 // ---- shared-memory map (bytes from the 1024-aligned base) ----
 constexpr uint32_t S3_XB = 0;                        // X(k) | dOut(k) buffers, parity k & 1 and (k + 1) & 1
@@ -49,7 +53,7 @@ constexpr uint32_t S3_DIST = S3_BIAS + 2 * 640;      // var[16], log_scale[16], 
 constexpr uint32_t S3_SCALE = S3_DIST + 256;         // per net 16 floats
 constexpr uint32_t S3_XS = S3_SCALE + 128;           // 2^ex_k [32], 2^-ex_k [32]
 constexpr uint32_t S3_RED = S3_XS + 256;             // setup reduction scratch [20 warps][8] floats
-constexpr uint32_t S3_BARS = S3_RED + 640;           // ready[2] chain[2] xfull[2] (8 B each), bad flag
+constexpr uint32_t S3_BARS = S3_RED + 640;           // 15 mbarriers (8 B each), bad flag at +120
 constexpr uint32_t S3_TOTAL = S3_BARS + 128;
 constexpr uint32_t T3_SMEM_BYTES = S3_TOTAL + 1024;  // + alignment slack
 static_assert(T3_SMEM_BYTES <= 227 * 1024, "mlp_tc3 shared memory");
@@ -57,19 +61,26 @@ static_assert(T3_SMEM_BYTES <= 227 * 1024, "mlp_tc3 shared memory");
 constexpr uint32_t S3_END_DB3 = 0;                   // [16 warps][16] floats
 constexpr uint32_t S3_END_SC = 1024;                 // [16 warps][8] doubles
 
-// ---- accumulator column map (fp32) ----
-constexpr uint32_t ACC_CHAIN = 80, ACC_Z = 0, ACC_OUT = 64;       // per chain: Z1 -> Z2 -> dH2 -> dH1 share Z
+// ---- accumulator column map of the weight gradients (fp32) ----
 // per net: DW2 (64) | DB2 (16, col 15 = db2) | DW1 (64: products with X's h columns, then with its l columns; col 31 =
 // db1) | DW3 (32: products with dOut's h columns, then l).  The B operands of dW1 / dW3 hold their two splits side
 // by side in one swizzle atom, so ONE product per k-step covers both; the halves are added when the accumulators
-// are read, once per launch.  2 x 80 + 2 x 176 = 512 columns: all of accumulator memory.
-constexpr uint32_t ACC_GRAD = 160, ACC_GRAD_NET = 176;
+// are read, once per launch.  2 x 176 of the 512 columns.
+constexpr uint32_t ACC_GRAD_NET = 176;
+// Running b3 sums: rows are tile rows, column 16 m + a holds sum class m (0..3) of output a (policy a < 15, value
+// a = 15).  A row's output of tile k of network c goes to class (k + 2 c) & 3, and every class is added in tile order.
+// The read-out then reduces class m with warp group m: the per-CTA sum is computed in the same order as when loss
+// warps rotated over the tiles, so the b3 gradients do not depend on which thread evaluated a row.
+constexpr uint32_t ACC_DB3 = 2 * ACC_GRAD_NET;
+static_assert(ACC_DB3 + 4 * 16 <= ACC_COLS, "mlp_tc3 accumulator columns");
 constexpr uint32_t ACC_DW2 = 0, ACC_DB2 = 64, ACC_DW1 = 80, ACC_DW3 = 144;
 
 #ifdef B200RL_TC3_TIMING
-// CTA 0: [0..9] job wait cycles (2 * (stage - 1) + chain), [10..19] job work cycles, [20..29] issuer: wait for the
-// stage inputs, [30..39] issuer: issuing, [40] issuer: waiting for the bulk copy, [41] tiles of the CTA
-__device__ unsigned long long g_tc3_t[48];
+// CTA 0, chain warpgroup wg = 2 c + h: [10 wg + s - 1] cycles stage s (E1..E5) waited on an mbarrier, [10 wg + 4 + s]
+// cycles of stage s in all; gradient warpgroup: [40 + 3 c + s - 3] cycles waited for the operands of stage s (3..5) of
+// network c, [46 + 3 c + s - 3] cycles issuing its products; [52] tiles of the CTA, [53] set-up, [54] tile loop,
+// [55] read-out
+__device__ unsigned long long g_tc3_t[64];
 #endif
 
 enum { C3_G = 0, C3_U1, C3_U2, C3_U3, C3_UH2, C3_UH1, C3_W1, C3_W2, C3_W3, C3_OW3, C3_OW2, C3_OW1, C3_OB, C3_N };
@@ -145,6 +156,59 @@ __global__ void __launch_bounds__(128) pack_obs_kernel(const float* __restrict__
 }
 
 // ------------------------------------------------------------------------------------------------------------------
+// products
+// ------------------------------------------------------------------------------------------------------------------
+// D[64 x N] (+)= sum over TERMS of A_t B_t, KSTEPS k-steps of 16 each, as ONE group of wgmma m64nNk16: every k-step of
+// every term back to back, one commit, one wait.  The fragment stays in the caller's registers.
+template <int N, int TA, int TB, int TERMS, int KSTEPS>
+__device__ __forceinline__ void wg_mma(float (&d)[N / 2], const uint32_t (&alo)[TERMS], const uint32_t (&blo)[TERMS],
+                                       uint32_t a_hi, uint32_t b_hi, uint32_t a_k, uint32_t b_k, uint32_t accumulate) {
+  wgmma_fence();
+#pragma unroll
+  for (int s = 0; s < TERMS; ++s)
+#pragma unroll
+    for (int k = 0; k < KSTEPS; ++k)
+      wgmma_run<N, false, TA, TB>(d, ((uint64_t)a_hi << 32) | (alo[s] + (uint32_t)k * a_k),
+                                  ((uint64_t)b_hi << 32) | (blo[s] + (uint32_t)k * b_k), s == 0 && k == 0 ? accumulate : 1u);
+  wgmma_commit();
+  wgmma_wait_all();
+}
+// chain product of one 64-row half (A K-major, `a` already at the half's rows): (h,l) + (l,h) + (h,h), smallest terms
+// first, overwriting the fragment
+template <int N, int TB, int KSTEPS>
+__device__ __forceinline__ void chain_mma(float (&d)[N / 2], const Op2 a, const Op2 b) {
+  const uint32_t alo[3] = {a.lo, a.lo + a.split_step, a.lo}, blo[3] = {b.lo + b.split_step, b.lo, b.lo};
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+  wg_mma<N, K_MAJOR, TB, 3, KSTEPS>(d, alo, blo, a.hi, b.hi, a.k_step, b.k_step, 0u);
+}
+// weight-gradient product over the whole tile (both operands MN-major): A stacks its two splits along M (rows 0..63 h,
+// 64..127 l: the two m64 halves), B split l (B_SPLITS == 2) then h.  Each half's fragment is loaded from the
+// accumulator memory and stored back; on the launch's first tile (`first`) the product overwrites it.
+template <int N, int KSTEPS, int B_SPLITS>
+__device__ __forceinline__ void grad_mma(float* acc_cta, uint32_t acc_col, bool first, const Op2 a, const Op2 b) {
+  const int t = (int)(threadIdx.x & 127u), w = t >> 5, l = t & 31;
+  const uint32_t a_half = (a.lo >> 16) & 0x3FFFu;  // the leading byte offset: A's l split
+  float* const frag0 = acc_cta + (acc_col + 2 * (l & 3)) * ACC_LANES + 16 * w + (l >> 2);
+#pragma unroll 1
+  for (int h = 0; h < 2; ++h) {
+    float* frag = frag0 + 64 * h;
+    float d[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) d[i] = first ? 0.f : frag[(8 * (i >> 2) + (i & 1)) * ACC_LANES + 8 * ((i >> 1) & 1)];
+    uint32_t alo[B_SPLITS], blo[B_SPLITS];
+#pragma unroll
+    for (int s = 0; s < B_SPLITS; ++s) {
+      alo[s] = a.lo + (uint32_t)h * a_half;
+      blo[s] = b.lo + (s + 1 < B_SPLITS ? b.split_step : 0u);
+    }
+    wg_mma<N, MN_MAJOR, MN_MAJOR, B_SPLITS, KSTEPS>(d, alo, blo, a.hi, b.hi, a.k_step, b.k_step, first ? 0u : 1u);
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) frag[(8 * (i >> 2) + (i & 1)) * ACC_LANES + 8 * ((i >> 1) & 1)] = d[i];
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
 // the step kernel
 // ------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p) {
@@ -165,20 +229,19 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   float* s_scale = reinterpret_cast<float*>(sm + S3_SCALE);
   float* s_xs = reinterpret_cast<float*>(sm + S3_XS);
   float* s_red = reinterpret_cast<float*>(sm + S3_RED);
-  int* s_bad = reinterpret_cast<int*>(sm + S3_BARS + 48);
-  // ready[c] at +8c, chain[c] at +16+8c, xfull[b] at +32+8b
+  int* s_bad = reinterpret_cast<int*>(sm + S3_BARS + 120);
   const uint32_t bars = base + S3_BARS;
   const int n_in = p.n_in;
   bool bad = false;
 #ifdef B200RL_TC3_TIMING
-  unsigned long long tacc[48];
-  for (int i = 0; i < 48; ++i) tacc[i] = 0;
+  unsigned long long tacc[64];
+  for (int i = 0; i < 64; ++i) tacc[i] = 0;
   const long long t_kernel0 = clock64();
 #endif
 
   // ---- one-time setup: scales; weights of both networks as fp16 pairs; biases ----
   // Only the weight operands need zero padding (X tiles arrive whole by bulk copy, H and dOut are fully written by
-  // their jobs before any MMA reads them).  Both parameter vectors (44 KB) are first brought into the still unused
+  // their epilogues before any MMA reads them).  Both parameter vectors (44 KB) are first brought into the still unused
   // activation buffers with independent, coalesced loads: the two passes below (maxima, then conversion) would
   // otherwise pay an L2 round trip per element, one after the other (17 of the 18 us this set-up took on B200).
   for (uint32_t i = S3_W / 16 + tid; i < S3_OPERANDS_END / 16; i += T3_THREADS) reinterpret_cast<uint4*>(sm)[i] = make_uint4(0, 0, 0, 0);
@@ -312,207 +375,241 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   if (bad) *s_bad = 1;  // non-finite bias
   bad = false;
   if (tid == 0) {
-    for (int c = 0; c < 2; ++c) {
-      mbar_init(bars + 8 * c, T3_EPI_THREADS);  // ready[c]: every epilogue thread arrives once per job of chain c
-      mbar_init(bars + 16 + 8 * c, 1);          // chain[c]: acc_commit
-      mbar_init(bars + 32 + 8 * c, 1);          // xfull[b]: arrive.expect_tx by the MMA warp + the copy's bytes
+    mbar_init(bars + 0, 1);  // xfull[b]: arrive.expect_tx by the producer + the copy's bytes
+    mbar_init(bars + 8, 1);
+    for (int i = 0; i < 6; ++i) {
+      mbar_init(bars + 16 + 8 * i, 2);  // ready[c][s]: one arrive per chain warpgroup of network c
+      mbar_init(bars + 64 + 8 * i, 1);  // done[c][s]: the gradient warpgroup
     }
+    mbar_init(bars + 112, 1);  // dofree
     fence_mbar_init();
   }
   fence_proxy_async_smem();
   __syncthreads();
 
   const long long num_tiles = (p.n_rows + T3_ROWS - 1) / T3_ROWS;
-  const long long cta_tiles = (num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;  // tiles blockIdx.x + k * gridDim.x
+  const int cta_tiles = (int)((num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x);  // tiles blockIdx.x + k * gridDim.x
   const int c_first = run_p ? 0 : 1, c_last = run_v ? 1 : 0;
 
-  if (warp >= T3_EPI_WARPS) {
-    // =============================== MMA issuer (and bulk-copy producer) warpgroup =============================
-    constexpr int K = K_MAJOR, MN = MN_MAJOR;
-    const uint32_t ub = base, ubar = bars;
-    // views at chain 0 / net 0 / X buffer 0; the others are reached by adding byte offsets to the descriptors
-    const Op2 X_K = op2_kmajor(ub + S3_XB, 64);                     // A: X, h at +0, l at +64 bytes
-    const Op2 X_M = op2_mnmajor(ub + S3_XB, T2_ACT, 64);            // B, N = 64: features h 0..31 (col 31 = ones) | l
-    const Op2 X_M16 = op2_mnmajor(ub + S3_XB + 32, T2_ACT, 64);     // B, N = 16: h cols 16..31 (col 31 = ones)
-    const Op2 DO_K = op2_kmajor(ub + S3_XB, 32);                    // A, K = 16: dOut h at +0, l at +32 bytes
-    const Op2 DO_M = op2_mnmajor(ub + S3_XB, T2_ACT, 32);           // B, N = 32: dOut h | l
-    const Op2 H1_K = op2_kmajor(ub + S3_H, T2_ACT), H2_K = op2_kmajor(ub + S3_H + 2 * T2_ACT, T2_ACT);
+  constexpr int K = K_MAJOR, MN = MN_MAJOR;
+  const uint32_t ub = base;
+  // mbarriers: xfull[b] at +8b; ready[c][s - 3] at +16 + 8 (3c + s - 3) (count 2: one arrive per chain warpgroup of
+  // network c); done[c][s - 3] at +64 + 8 (3c + s - 3) (the weight-gradient products of stage s have read the buffers);
+  // dofree at +112 (every reader of this tile's X buffer has retired: the next tile's dOut may go there)
+  auto bar_ready = [&](int c, int s) { return bars + 16u + 8u * (uint32_t)(3 * c + s - 3); };
+  auto bar_done = [&](int c, int s) { return bars + 64u + 8u * (uint32_t)(3 * c + s - 3); };
+  const uint32_t bar_dofree = bars + 112;
+
+  if (warp >= T3_CHAIN_WARPS) {
+    // ============================ producer / weight-gradient warpgroup ============================
+    // views at chain 0 / X buffer 0; the others are reached by adding byte offsets to the descriptors
+    const Op2 X_M = op2_mnmajor(ub + S3_XB, T2_ACT, 64);         // B, N = 64: features h 0..31 (col 31 = ones) | l
+    const Op2 X_M16 = op2_mnmajor(ub + S3_XB + 32, T2_ACT, 64);  // B, N = 16: h cols 16..31 (col 31 = ones)
+    const Op2 DO_M = op2_mnmajor(ub + S3_XB, T2_ACT, 32);        // B, N = 32: dOut h | l
     const Op2 H1_M = op2_mnmajor(ub + S3_H, T2_ACT, T2_ACT), H2_M = op2_mnmajor(ub + S3_H + 2 * T2_ACT, T2_ACT, T2_ACT);
+    auto load_x = [&](int k) {  // tile k of this CTA -> X buffer k & 1
+      const uint32_t b = (uint32_t)(k & 1);
+      const long long tile = blockIdx.x + (long long)k * gridDim.x;
+      uint32_t e;
+      asm volatile("{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\tselp.u32 %0, 1, 0, q;\n\t}" : "=r"(e));
+      if (e && warp == T3_CHAIN_WARPS) {  // one thread of the warpgroup
+        mbar_arrive_expect_tx(bars + 8 * b, T2_ACT);
+        bulk_copy_g2s(ub + S3_XB + b * T2_ACT, p.ximg + (size_t)tile * T2_ACT, T2_ACT, bars + 8 * b);
+      }
+      __syncwarp();
+    };
+    if (cta_tiles > 0) load_x(0);
+#pragma unroll 1
+    for (int k = 0; k < cta_tiles; ++k) {
+      const uint32_t xo = (uint32_t)(k & 1) * T2_ACT, dob = (uint32_t)((k + 1) & 1) * T2_ACT;
+      const bool first = k == 0;  // the first tile's products overwrite the accumulators
+#pragma unroll 1
+      for (int stage = 3; stage <= 5; ++stage) {
+#pragma unroll 1
+        for (int c = c_first; c <= c_last; ++c) {
+          const uint32_t co = c * S3_CHAIN, gcol = c * ACC_GRAD_NET;
+#ifdef B200RL_TC3_TIMING
+          const long long it0 = clock64();
+#endif
+          mbar_wait(bar_ready(c, stage), (uint32_t)(k & 1));  // both halves of network c have delivered the operands
+#ifdef B200RL_TC3_TIMING
+          const long long it1 = clock64();
+          tacc[40 + 3 * c + stage - 3] += (unsigned long long)(it1 - it0);
+#endif
+          if (stage == 3) {
+            // dW3^T[i][o] += sum_r H2[r][i] dOut[r][o]
+            grad_mma<32, 8, 1>(acc, gcol + ACC_DW3, first, op2_at(H2_M, co), op2_at(DO_M, dob + c * 64));
+          } else if (stage == 4) {
+            // every chain warpgroup's dH2 and both dW3 have read dOut: its buffer takes the next tile's observations
+            if (c == c_last && k + 1 < cta_tiles) load_x(k + 1);
+            // dW2[o][i] += sum_r dZ2[r][o] H1[r][i] ; db2[o] += sum_r dZ2[r][o] * 1 (ones column of X)
+            grad_mma<64, 8, 2>(acc, gcol + ACC_DW2, first, op2_at(H2_M, co), op2_at(H1_M, co));
+            grad_mma<16, 8, 1>(acc, gcol + ACC_DB2, first, op2_at(H2_M, co), op2_at(X_M16, xo));
+          } else {
+            // dW1[o][i] += sum_r dZ1[r][o] X[r][i]; column 31 (ones) collects db1
+            grad_mma<64, 8, 1>(acc, gcol + ACC_DW1, first, op2_at(H1_M, co), op2_at(X_M, xo));
+          }
+          asm volatile("bar.sync 5, 128;" ::: "memory");  // every warp's share of the products has retired
+          if ((tid & 127) == 0) {
+            mbar_arrive(bar_done(c, stage));
+            if (stage == 5 && c == c_last) mbar_arrive(bar_dofree);
+          }
+#ifdef B200RL_TC3_TIMING
+          tacc[46 + 3 * c + stage - 3] += (unsigned long long)(clock64() - it1);
+#endif
+        }
+      }
+    }
+#ifdef B200RL_TC3_TIMING
+    if (tid == T3_CHAIN_THREADS && blockIdx.x == 0) {
+      for (int i = 40; i < 52; ++i) g_tc3_t[i] = tacc[i];
+      g_tc3_t[52] = (unsigned long long)cta_tiles;
+    }
+#endif
+    asm volatile("bar.sync 7, %0;" ::"n"(T3_THREADS) : "memory");  // the read-out may begin
+  } else {
+    // ====================== chain warpgroup wg = 2 c + hf: network c, rows 64 hf .. 64 hf + 63 ======================
+    // Z1 -> E1 -> Z2 -> E2 -> OUT -> E3 -> dH2 -> E4 -> dH1 -> E5 with the accumulator in this warpgroup's registers.
+    // Fragment element i of a thread is row r0 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 q + (i & 1) (wgmma D layout).
+    const int wg = warp >> 2, c = wg >> 1, hf = wg & 1;
+    const int quad = lane >> 2, q = lane & 3;
+    const int r0 = 64 * hf + 16 * (warp & 3) + quad;  // == quad (mod 8): the swizzle phase of both fragment rows
+    const uint32_t rows = (uint32_t)hf * (64u * 128u);  // this half in a K-major buffer
+    const uint32_t co = c * S3_CHAIN, wo = c * S3_WNET, so = S3_H + co;
+    const Op2 X_K = op2_at(op2_kmajor(ub + S3_XB, 64), rows);  // A: X, h at +0, l at +64 bytes
+    const Op2 DO_K = op2_at(op2_kmajor(ub + S3_XB, 32), rows);  // A, K = 16: dOut h at +0, l at +32 bytes
+    const Op2 H1_K = op2_at(op2_kmajor(ub + S3_H, T2_ACT), rows), H2_K = op2_at(op2_kmajor(ub + S3_H + 2 * T2_ACT, T2_ACT), rows);
     const Op2 W1T_M = op2_mnmajor(ub + S3_W, 32 * 128, T3_W1T);
     const Op2 W2_K = op2_kmajor(ub + S3_W + 2 * T3_W1T, T3_W2), W2_M = op2_mnmajor(ub + S3_W + 2 * T3_W1T, 64 * 128, T3_W2);
     const Op2 W3_K = op2_kmajor(ub + S3_W + 2 * T3_W1T + 2 * T3_W2, T3_W3),
               W3_M = op2_mnmajor(ub + S3_W + 2 * T3_W1T + 2 * T3_W2, 16 * 128, T3_W3);
-    uint32_t accmask = 0u;  // bit (3 c + j): the accumulator j of chain c holds data (the first product overwrites it)
-    uint32_t par_ready = 0u;  // bit c: phase parity of ready[c]
-    auto load_x = [&](long long k) {  // tile k of this CTA -> X buffer k & 1
-      const uint32_t b = (uint32_t)(k & 1);
-      const long long tile = blockIdx.x + k * gridDim.x;
-      uint32_t e;
-      asm volatile("{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\tselp.u32 %0, 1, 0, q;\n\t}" : "=r"(e));
-      if (e && warp == T3_EPI_WARPS) {  // one thread of the warpgroup
-        mbar_arrive_expect_tx(ubar + 32 + 8 * b, T2_ACT);
-        bulk_copy_g2s(ub + S3_XB + b * T2_ACT, p.ximg + (size_t)tile * T2_ACT, T2_ACT, ubar + 32 + 8 * b);
-      }
-      __syncwarp();
-    };
-    auto issue_z1 = [&](const int c, long long k) {  // Z1 = X W1^T of tile k for chain c
-      const uint32_t b = (uint32_t)(k & 1);
-#ifdef B200RL_TC3_TIMING
-      const long long xt0 = clock64();
-#endif
-      mbar_wait(ubar + 32 + 8 * b, (uint32_t)((k >> 1) & 1));
-#ifdef B200RL_TC3_TIMING
-      tacc[40] += (unsigned long long)(clock64() - xt0);
-#endif
-      issue_chain3<64, MN, 2>(acc, c * ACC_CHAIN + ACC_Z, op2_at(X_K, b * T2_ACT), op2_at(W1T_M, c * S3_WNET));
-    };
-    if (cta_tiles > 0) {
-      load_x(0);
-#pragma unroll 1
-      for (int c = c_first; c <= c_last; ++c) {
-        issue_z1(c, 0);
-        acc_commit(ubar + 16 + 8 * c);
-      }
-    }
-#pragma unroll 1
-    for (long long k = 0; k < cta_tiles; ++k) {
-      const uint32_t xo = (uint32_t)(k & 1) * T2_ACT, dob = (uint32_t)((k + 1) & 1) * T2_ACT;
-#pragma unroll 1
-      for (int stage = 1; stage <= 5; ++stage) {
-#pragma unroll 1
-        for (int c = c_first; c <= c_last; ++c) {
-          const uint32_t co = c * S3_CHAIN, wo = c * S3_WNET;
-          const uint32_t acol = c * ACC_CHAIN, gcol = ACC_GRAD + c * ACC_GRAD_NET;
-#ifdef B200RL_TC3_TIMING
-          const long long it0 = clock64();
-#endif
-          mbar_wait(ubar + 8 * c, (par_ready >> c) & 1u);  // every epilogue thread has delivered the stage inputs
-          par_ready ^= 1u << c;
-#ifdef B200RL_TC3_TIMING
-          const long long it1 = clock64();
-          tacc[20 + 2 * (stage - 1) + c] += (unsigned long long)(it1 - it0);
-#endif
-          // issue_chain3 <N, B major, k-steps>, issue_stacked <N, k-steps, B splits>
-          if (stage == 1) {  // Z2 = H1 W2^T
-            issue_chain3<64, K, 4>(acc, acol + ACC_Z, op2_at(H1_K, co), op2_at(W2_K, wo));
-          } else if (stage == 2) {  // OUT = H2 W3^T
-            issue_chain3<16, K, 4>(acc, acol + ACC_OUT, op2_at(H2_K, co), op2_at(W3_K, wo));
-          } else if (stage == 3) {
-            // dH2 = dOut W3 ; dW3^T[i][o] += sum_r H2[r][i] dOut[r][o] (must retire before H2 becomes dZ2 in place)
-            issue_chain3<64, MN, 1>(acc, acol + ACC_Z, op2_at(DO_K, dob + c * 64), op2_at(W3_M, wo));
-            issue_stacked<32, 8, 1>(acc, gcol + ACC_DW3, (accmask >> (3 * c)) & 1u, op2_at(H2_M, co),
-                                    op2_at(DO_M, dob + c * 64));  // N = 32: dOut h | l
-            accmask |= 1u << (3 * c);
-          } else if (stage == 4) {
-            // both chains' stage-3 products have retired (their E4 jobs waited for them before arriving here): the
-            // dOut buffer is free -> bring the NEXT tile's observations into it
-            if (c == c_last && k + 1 < cta_tiles) load_x(k + 1);
-            // dH1 = dZ2 W2 ; dW2[o][i] += sum_r dZ2[r][o] H1[r][i] ; db2[o] += sum_r dZ2[r][o] * 1 (ones column of X)
-            issue_chain3<64, MN, 4>(acc, acol + ACC_Z, op2_at(H2_K, co), op2_at(W2_M, wo));
-            issue_stacked<64, 8, 2>(acc, gcol + ACC_DW2, (accmask >> (3 * c + 1)) & 1u, op2_at(H2_M, co), op2_at(H1_M, co));
-            issue_stacked<16, 8, 1>(acc, gcol + ACC_DB2, (accmask >> (3 * c + 1)) & 1u, op2_at(H2_M, co), op2_at(X_M16, xo));
-            accmask |= 1u << (3 * c + 1);
-          } else {
-            // dW1[o][i] += sum_r dZ1[r][o] X[r][i]; column 31 (ones) collects db1.  Then the next tile's Z1.
-            issue_stacked<64, 8, 1>(acc, gcol + ACC_DW1, (accmask >> (3 * c + 2)) & 1u, op2_at(H1_M, co), op2_at(X_M, xo));
-            accmask |= 1u << (3 * c + 2);
-            if (k + 1 < cta_tiles) issue_z1(c, k + 1);
-          }
-          acc_commit(ubar + 16 + 8 * c);
-          __syncwarp();
-#ifdef B200RL_TC3_TIMING
-          tacc[30 + 2 * (stage - 1) + c] += (unsigned long long)(clock64() - it1);
-#endif
-        }
-      }
-    }
-#ifdef B200RL_TC3_TIMING
-    if (lane == 0 && blockIdx.x == 0) {
-      for (int i = 20; i <= 40; ++i) g_tc3_t[i] = tacc[i];
-      g_tc3_t[41] = (unsigned long long)cta_tiles;
-    }
-#endif
-  } else {
-    // =============================== epilogue warps: one pool of 16 ===================================
-    // Jobs run in the fixed order (policy, E1) (value, E1) (policy, E2) ... (value, E5) | next tile, all 16 warps on
-    // one job at a time (16 columns each), so the MMAs a job hands over run under the other chain's next job.
-    const int q = warp & 3, part = warp >> 2;
-    const int r = 32 * q + lane;                          // row of the tile == accumulator row
-    const int cs = 16 * part;
-    uint32_t ph_chain = 0u;  // bit c: phase parity of chain[c]
+    const bool runs = c == 0 ? run_p : run_v;
+    const float* scl = s_scale + 16 * c;
+    const float* bias = s_bias + 160 * c;
     const float sH = pow2i(T2_H_EXP), hh = pow2i(-2 * T2_H_EXP);
     const int A_out = p.net[0].n_out;
-    double sc[5] = {0, 0, 0, 0, 0};  // policy: loss terms, old_logp - logp, entropy, logp, logp^2
-    double vs = 0.0;                 // value: squared errors
-    int rows_done = 0;
-    float db3[15], db3v = 0.f;
+    // per-thread sums of the rows this thread owns in E3.  Policy: loss terms, old_logp - logp, entropy, logp,
+    // logp^2; value: sc[0] = squared errors.  (The b3 sums live in accumulator memory, ACC_DB3.)
+    double sc[5] = {0, 0, 0, 0, 0};
+
+    // byte offset of columns 8 j + 2 q, +1 of fragment row r0 + 8 r in the SWIZZLE_128B buffer `buf`
+    auto frag_off = [&](uint32_t buf, int j, int r) -> uint32_t {
+      return buf + (uint32_t)(r0 + 8 * r) * 128u + ((uint32_t)(j ^ quad) << 4) + 4u * (uint32_t)q;
+    };
+    auto store_pairs = [&](uint32_t buf, const float (&x)[32]) {
 #pragma unroll
-    for (int a = 0; a < 15; ++a) db3[a] = 0.f;
-    float adv_mean, adv_std;
-    adv_mean_std(p.adv_stats, adv_mean, adv_std);
-    const float adv_inv_std = 1.f / adv_std;
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          uint32_t h, l;
+          split2h(x[4 * j + 2 * r], x[4 * j + 2 * r + 1], h, l);
+          const uint32_t off = frag_off(buf, j, r);
+          *reinterpret_cast<uint32_t*>(sm + off) = h;
+          *reinterpret_cast<uint32_t*>(sm + off + T2_ACT) = l;
+        }
+    };
+    // E1 / E2: Z * unscale + bias -> tanh(.) * 2^14
+    auto act = [&](float (&z)[32], float unscale, const float* bs) {
+#pragma unroll
+      for (int g = 0; g < 2; ++g) {
+        float t[16];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const int e = 16 * g + i;
+          t[i] = fmaf(z[e], unscale, bs[8 * (e >> 2) + 2 * q + (e & 1)]);
+        }
+        tanh16_scaled(t, sH);
+#pragma unroll
+        for (int i = 0; i < 16; ++i) z[16 * g + i] = t[i];
+      }
+    };
+    // E4 / E5: dZ (scaled) = dH * unscale * (1 - H^2), H read back from its fp16 pair in `buf`.
+    // (1 - H^2) * 2^28 = fma(-Hs, Hs, 2^28) with Hs = H * 2^14 as stored; 2^-28 is folded into the unscale factor
+    auto dtanh = [&](float (&g)[32], float unscale, uint32_t buf) {
+      const float one28 = 268435456.f;
+      float m = 0.f;
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const uint32_t off = frag_off(buf, j, r);
+          const uint32_t hw = *reinterpret_cast<const uint32_t*>(sm + off);
+          const uint32_t lw = *reinterpret_cast<const uint32_t*>(sm + off + T2_ACT);
+          const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&hw));
+          const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&lw));
+          const float x0 = a.x + b.x, x1 = a.y + b.y;
+          float& g0 = g[4 * j + 2 * r];
+          float& g1 = g[4 * j + 2 * r + 1];
+          g0 = (g0 * unscale) * fmaf(-x0, x0, one28);
+          g1 = (g1 * unscale) * fmaf(-x1, x1, one28);
+          m = fmaxf(m, fmaxf(fabsf(g0), fabsf(g1)));
+        }
+      if (!(m <= T2_RANGE)) bad = true;  // magnitude only: the inputs were checked
+    };
+    // this warpgroup's shared-memory writes -> visible to its own next product and to the gradient warpgroup
+    auto wg_sync = [&]() {
+      fence_proxy_async_smem();
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+    };
+    auto deliver = [&](int s) {
+      wg_sync();
+      if ((tid & 127) == 0) mbar_arrive(bar_ready(c, s));
+    };
+#ifdef B200RL_TC3_TIMING
+    long long t_mark = 0, t_loop0 = 0, t_loop_end = 0;
+#endif
+    auto wait = [&](int s, uint32_t bar, uint32_t parity) {
+#ifdef B200RL_TC3_TIMING
+      const long long w0 = clock64();
+#endif
+      mbar_wait(bar, parity);
+#ifdef B200RL_TC3_TIMING
+      tacc[10 * wg + s - 1] += (unsigned long long)(clock64() - w0);
+#endif
+    };
+    auto stage_end = [&](int s) {
+#ifdef B200RL_TC3_TIMING
+      const long long t = clock64();
+      tacc[10 * wg + 4 + s] += (unsigned long long)(t - t_mark);
+      t_mark = t;
+#endif
+    };
 
 #ifdef B200RL_TC3_TIMING
-    long long t_work0 = 0;
+    t_loop0 = clock64();
+    t_mark = t_loop0;
 #endif
-    auto job = [&](const int c, const int stage, const long long k) {
-      const uint32_t acol = (uint32_t)c * ACC_CHAIN;
-      const uint32_t so = S3_H + (uint32_t)c * S3_CHAIN;
-      const uint32_t bar_ready = bars + 8 * c, bar_chain = bars + 16 + 8 * c;
-      const float* scl = s_scale + 16 * c;
-      const float* bias = s_bias + 160 * c;
-      const long long tile = blockIdx.x + k * gridDim.x;
-      const long long row = tile * T3_ROWS + r;
-      const bool valid = row < p.n_rows;
-      const bool loss_warp = part == (int)((k + 2 * c) & 3);  // rotates; the two chains use different warps
-      auto arrive = [&]() {
-        fence_proxy_async_smem();
-        mbar_arrive(bar_ready);
-      };
-      auto wait_chain = [&]() {
-#ifdef B200RL_TC3_TIMING
-        const long long w0 = clock64();
-#endif
-        mbar_wait(bar_chain, (ph_chain >> c) & 1u);
-        ph_chain ^= 1u << c;
-#ifdef B200RL_TC3_TIMING
-        {
-          const long long w1 = clock64();
-          tacc[2 * (stage - 1) + c] += (unsigned long long)(w1 - w0);
-          t_work0 = w1;
-        }
-#endif
-      };
-      if (stage == 1 || stage == 2) {
-        // ---- E1 / E2: Z (accumulator memory) * unscale + bias -> tanh -> fp16 pairs ----
-        wait_chain();
-        const float unscale = scl[stage == 1 ? C3_U1 : C3_U2];
-        const float* bs = bias + (stage == 1 ? 0 : 64);
-        const uint32_t dst = so + (stage == 1 ? 0u : 2 * T2_ACT);
-        float z[16];
-        acc_ld<16>(acc, r, acol + ACC_Z + cs, z);
+    if (runs) {
+#pragma unroll 1
+      for (int k = 0; k < cta_tiles; ++k) {
+        const long long tile = blockIdx.x + (long long)k * gridDim.x;
+        const uint32_t xo = (uint32_t)(k & 1) * T2_ACT, dob = (uint32_t)((k + 1) & 1) * T2_ACT;
+        float d[32];
+        // ---- Z1 = X W1^T -> E1 -> H1 ----
+        wait(1, bars + 8 * (uint32_t)(k & 1), (uint32_t)((k >> 1) & 1));  // the tile's observations have arrived
+        chain_mma<64, MN, 2>(d, op2_at(X_K, xo), op2_at(W1T_M, wo));
+        act(d, scl[C3_U1], bias);
+        if (k > 0) wait(1, bar_done(c, 5), (uint32_t)((k - 1) & 1));  // dW2, db2, dW1 of the last tile have read H1, H2
+        store_pairs(so, d);
+        wg_sync();
+        stage_end(1);
+        // ---- Z2 = H1 W2^T -> E2 -> H2 ----
+        chain_mma<64, K, 4>(d, op2_at(H1_K, co), op2_at(W2_K, wo));
+        act(d, scl[C3_U2], bias + 64);
+        store_pairs(so + 2 * T2_ACT, d);
+        wg_sync();
+        stage_end(2);
+        // ---- OUT = H2 W3^T -> E3: loss head, one row per owner thread (lanes q = 0, 1 own rows r0, r0 + 8) ----
+        const int orow = r0 + 8 * q;
+        const long long row = tile * T3_ROWS + orow;
+        const bool owner = q < 2, valid = owner && row < p.n_rows;
+        float pf_act[15], pf_in = 0.f, pf_old = 0.f;  // pf_in: the advantage (policy) or the return (value)
 #pragma unroll
-        for (int j = 0; j < 16; ++j) z[j] = fmaf(z[j], unscale, bs[cs + j]);
-        tanh16_scaled(z, sH);  // tanh(z) * 2^14
-#pragma unroll
-        for (int ch = 0; ch < 2; ++ch) {
-          float x[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) x[j] = z[8 * ch + j];
-          store_chunk2(sm, dst, r, (cs >> 3) + ch, x);
-        }
-        arrive();
-      } else if (stage == 3) {
-        // ---- E3: loss epilogue, one row per thread, on this tile's loss warps of this chain ----
-        const uint32_t dob = S3_XB + (uint32_t)((k + 1) & 1) * T2_ACT;  // the X buffer of the other parity
-        float x0[8], x1[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) x0[j] = x1[j] = 0.f;
-        if (c == 0) {
-          float pf_act[15], pf_adv = 0.f, pf_old = 0.f;
-#pragma unroll
-          for (int a = 0; a < 15; ++a) pf_act[a] = 0.f;
-          if (loss_warp && valid) {  // issue the loads before waiting for OUT
+        for (int a = 0; a < 15; ++a) pf_act[a] = 0.f;
+        // this row's running b3 sums of its class (ACC_DB3); a class starts at zero on its first tile, k < 4
+        float* const s3p = acc + (ACC_DB3 + 16u * (uint32_t)((k + 2 * c) & 3)) * ACC_LANES + orow;
+        if (valid) {  // issue the loads before the product
+          if (c == 0) {
             if (p.dist == B200RL_DIST_GAUSSIAN) {
 #pragma unroll
               for (int a = 0; a < 15; ++a)
@@ -520,18 +617,35 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
             } else {
               pf_act[0] = __ldg(p.actions + row);
             }
-            pf_adv = __ldg(p.adv_raw + row);
+            pf_in = __ldg(p.adv_raw + row);
             pf_old = __ldg(p.old_logp + row);
+          } else {
+            pf_in = __ldg(p.target + row);
           }
-          wait_chain();
-          if (loss_warp) {
-            float o[16];
-            acc_ld<16>(acc, r, acol + ACC_OUT, o);
-            float out[16], dout[16];
-            const float u3 = scl[C3_U3];
+        }
+        float o[8];
+        chain_mma<16, K, 4>(o, op2_at(H2_K, co), op2_at(W3_K, wo));
+        float out[16];  // the owner's output row, gathered from its quad
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+          for (int qq = 0; qq < 4; ++qq)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float v0 = __shfl_sync(0xffffffffu, o[4 * j + e], (lane & ~3) | qq);
+              const float v1 = __shfl_sync(0xffffffffu, o[4 * j + 2 + e], (lane & ~3) | qq);
+              out[8 * j + 2 * qq + e] = q == 0 ? v0 : v1;
+            }
+        float x0[8], x1[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) x0[j] = x1[j] = 0.f;
+        if (owner) {
+          const float u3 = scl[C3_U3], sG = scl[C3_G];
+          if (c == 0) {
+            float dout[16];
 #pragma unroll
             for (int a = 0; a < 16; ++a) {
-              out[a] = fmaf(o[a], u3, bias[128 + a]);
+              out[a] = fmaf(out[a], u3, bias[128 + a]);
               dout[a] = 0.f;
             }
             if (valid) {
@@ -542,41 +656,39 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
                 gaussian_logp<15>(pf_act, out, s_dist + 16, VarRecip{s_dist + 48, s_dist + 32}, A_out, lp, ent, dlp);
               else
                 categorical_logp<15>(out, (int)pf_act[0], A_out, lp, ent, dlp);  // value.long()
-              float adv = pf_adv;
-              if (p.adv_stats != nullptr) adv = (adv - adv_mean) * adv_inv_std;  // utils.py:91
+              float adv = pf_in;
+              if (p.adv_stats != nullptr) {  // utils.py:91 (the statistics are re-read here: registers)
+                float adv_mean, adv_std;
+                adv_mean_std(p.adv_stats, adv_mean, adv_std);
+                adv = (adv - adv_mean) * (1.f / adv_std);
+              }
               float coef;
               const float term = policy_loss(B200RL_LOSS_PPO_CLIP, lp, pf_old, adv, p.inv_n, p.clip_lo, p.clip_hi, coef);
 #pragma unroll
               for (int a = 0; a < 15; ++a) dout[a] = coef * dlp[a];
               add_policy_row_sums(sc, term, lp, ent, pf_old, true);
-              rows_done += 1;
             }
-            const float sG = scl[C3_G];
 #pragma unroll
-            for (int a = 0; a < 15; ++a) db3[a] += dout[a];
+            for (int a = 0; a < 15; ++a) s3p[a * ACC_LANES] = (k >= 4 ? s3p[a * ACC_LANES] : 0.f) + dout[a];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
               x0[j] = dout[j] * sG;
               x1[j] = j < 7 ? dout[8 + j] * sG : 0.f;
             }
-          }
-        } else {
-          float pf_tgt = 0.f;
-          if (loss_warp && valid) pf_tgt = __ldg(p.target + row);
-          wait_chain();
-          if (loss_warp) {
-            float o[8];
-            acc_ld<8>(acc, r, acol + ACC_OUT, o);
+          } else {
+            float s3 = k >= 4 ? s3p[15 * ACC_LANES] : 0.f;
             if (valid) {
               float dout;
-              vs += (double)value_mse(fmaf(o[0], scl[C3_U3], bias[128]), pf_tgt, p.inv_n, dout);
-              db3v += dout;
-              x0[0] = dout * scl[C3_G];
+              sc[0] += (double)value_mse(fmaf(out[0], u3, bias[128]), pf_in, p.inv_n, dout);
+              s3 += dout;
+              x0[0] = dout * sG;
             }
+            s3p[15 * ACC_LANES] = s3;
           }
-        }
-        if (loss_warp) {
           if (out_of_range8(x0) || out_of_range8(x1)) bad = true;
+        }
+        if (k > 0) wait(3, bar_dofree, (uint32_t)((k - 1) & 1));  // the last tile's X buffer is free for dOut
+        if (owner) {
           // 16 columns h, then 16 columns l, at fp16 columns 32 c .. 32 c + 31 of the dOut buffer
           uint4 h0, l0, h1, l1;
           split2h(x0[0], x0[1], h0.x, l0.x);
@@ -587,84 +699,55 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
           split2h(x1[2], x1[3], h1.y, l1.y);
           split2h(x1[4], x1[5], h1.z, l1.z);
           split2h(x1[6], x1[7], h1.w, l1.w);
-          uint8_t* rowp = sm + dob + (uint32_t)r * 128u;
-          const uint32_t sw = (uint32_t)(r & 7), c4 = 4u * (uint32_t)c;
+          uint8_t* rowp = sm + S3_XB + dob + (uint32_t)orow * 128u;
+          const uint32_t sw = (uint32_t)(orow & 7), c4 = 4u * (uint32_t)c;
           *reinterpret_cast<uint4*>(rowp + (((c4 + 0u) ^ sw) << 4)) = h0;
           *reinterpret_cast<uint4*>(rowp + (((c4 + 1u) ^ sw) << 4)) = h1;
           *reinterpret_cast<uint4*>(rowp + (((c4 + 2u) ^ sw) << 4)) = l0;
           *reinterpret_cast<uint4*>(rowp + (((c4 + 3u) ^ sw) << 4)) = l1;
         }
-        arrive();
-      } else {
-        // ---- E4 / E5: dZ (scaled) = dH_acc * unscale * (1 - H^2), H re-read from its fp16 pair, written in place ----
-        // (Alternatives measured on B200, before the port to wgmma -- loading this thread's H chunks BEFORE the wait -- it wrote them itself two jobs ago -- to hide the
-        // shared-memory latency under the barrier: 0.551 vs 0.525 ms, the 16 extra live registers spill at the 96 cap;
-        // a second commit right behind the dH product, so that this job computes while the weight-gradient products
-        // still read H and only its stores wait for them, measured 2 % SLOWER: 0.5515 vs 0.540 ms.  With `setmaxnreg`
-        // -- a full fifth warpgroup of 128 threads whose idle warps hand their registers over: 104 per epilogue thread
-        // and 64 for the MMA warp, or 112 / 32; registers are conserved inside the CTA, 640 x 96 = 128 AUX + 512 EPI --
-        // the spills go away and the prefetch is STILL slower (0.540 vs 0.522 ms): early shared-memory reads compete
-        // with the tensor pipe's operand fetches, which are what the waiting job is waiting for.  All reverted.)
-        wait_chain();  // dH (and the weight-gradient products that still read H)
-        // (1 - H^2) * 2^28 = fma(-Hs, Hs, 2^28) with Hs = H * 2^14 as stored; 2^-28 is folded into the unscale factor
-        const float unscale = scl[stage == 4 ? C3_UH2 : C3_UH1] * hh;
-        const uint32_t buf = so + (stage == 4 ? 2 * T2_ACT : 0u);
-        const float one28 = 268435456.f;
-        float g[16];
-        acc_ld<16>(acc, r, acol + ACC_Z + cs, g);
-#pragma unroll
-        for (int ch = 0; ch < 2; ++ch) {
-          float x[8];
-          load_chunk2(sm, buf, r, (cs >> 3) + ch, x);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) x[j] = (g[8 * ch + j] * unscale) * fmaf(-x[j], x[j], one28);
-          if (too_large8(x)) bad = true;
-          store_chunk2(sm, buf, r, (cs >> 3) + ch, x);
-        }
-        arrive();
-      }
-    };
-
-#ifdef B200RL_TC3_TIMING
-    const long long t_loop0 = clock64();
-#endif
-#pragma unroll 1
-    for (long long k = 0; k < cta_tiles; ++k) {
-#pragma unroll 1
-      for (int stage = 1; stage <= 5; ++stage) {
-#pragma unroll 1
-        for (int c = c_first; c <= c_last; ++c) {
-          job(c, stage, k);  // one copy of the job code (instruction cache)
-#ifdef B200RL_TC3_TIMING
-          tacc[10 + 2 * (stage - 1) + c] += (unsigned long long)(clock64() - t_work0);
-#endif
-        }
+        deliver(3);
+        stage_end(3);
+        // ---- dH2 = dOut W3 -> E4 -> dZ2, in place of H2 ----
+        chain_mma<64, MN, 1>(d, op2_at(DO_K, dob + c * 64), op2_at(W3_M, wo));
+        dtanh(d, scl[C3_UH2] * hh, so + 2 * T2_ACT);
+        wait(4, bar_done(c, 3), (uint32_t)(k & 1));  // dW3 has read H2
+        store_pairs(so + 2 * T2_ACT, d);
+        deliver(4);
+        stage_end(4);
+        // ---- dH1 = dZ2 W2 -> E5 -> dZ1, in place of H1 ----
+        chain_mma<64, MN, 4>(d, op2_at(H2_K, co), op2_at(W2_M, wo));
+        dtanh(d, scl[C3_UH1] * hh, so);
+        wait(5, bar_done(c, 4), (uint32_t)(k & 1));  // dW2 has read H1
+        store_pairs(so, d);
+        deliver(5);
+        stage_end(5);
       }
     }
-
 #ifdef B200RL_TC3_TIMING
-    const long long t_loop_end = clock64();
+    t_loop_end = clock64();
+    if ((tid & 127) == 0 && blockIdx.x == 0)
+      for (int i = 0; i < 10; ++i) g_tc3_t[10 * wg + i] = tacc[10 * wg + i];
 #endif
+
+    asm volatile("bar.sync 7, %0;" ::"n"(T3_THREADS) : "memory");  // with the gradient warpgroup: every product has
+                                                                   // retired and its accumulators are stored
     // ---- per-CTA results ----
-    if (cta_tiles > 0) {
-#pragma unroll 1
-      for (int c = c_first; c <= c_last; ++c)  // the last dW1 of each chain
-        mbar_wait(bars + 16 + 8 * c, (ph_chain >> c) & 1u);
-    }
-    asm volatile("bar.sync 2, %0;" ::"n"(T3_EPI_THREADS) : "memory");  // every MMA of the CTA has retired
     {
       // stacked accumulators: rows 0..63 = h-split half (partial row 2b), rows 64..127 = l-split half (row 2b + 1);
       // 8 jobs per net (dW2 x 4 column blocks, dW1 x 2, dW3, db2); warp `part` takes jobs part, part + 4 of both nets
-      float* dst_row = p.partials + ((size_t)blockIdx.x * 2 + (q >> 1)) * (size_t)(p.P[0] + p.P[1]);
-      const int m = 32 * (q & 1) + lane;  // feature index
+      const int qw = warp & 3, part = warp >> 2;
+      const int r = 32 * qw + lane;
+      float* dst_row = p.partials + ((size_t)blockIdx.x * 2 + (qw >> 1)) * (size_t)(p.P[0] + p.P[1]);
+      const int m = 32 * (qw & 1) + lane;  // feature index
       float v[16], w[16];
 #pragma unroll 1
-      for (int c = c_first; c <= c_last; ++c) {
-        const Tc3Net& nn = p.net[c];
-        float* dst = dst_row + (c == 0 ? 0 : p.P[0]);
-        const float* scl = s_scale + 16 * c;
+      for (int cn = c_first; cn <= c_last; ++cn) {
+        const Tc3Net& nn = p.net[cn];
+        float* dst = dst_row + (cn == 0 ? 0 : p.P[0]);
+        const float* scn = s_scale + 16 * cn;
         const bool have = cta_tiles > 0;
-        const uint32_t gcol = ACC_GRAD + c * ACC_GRAD_NET;
+        const uint32_t gcol = cn * ACC_GRAD_NET;
 #pragma unroll 1
         for (int jb = part; jb < 8; jb += 4) {
           // columns of this job, and of its second half where the operand's l columns went to their own block
@@ -678,49 +761,49 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
             for (int j = 0; j < 16; ++j) v[j] = w[j] = 0.f;  // a CTA without tiles: accumulator memory was never written
           }
           if (jb < 4) {  // dW2 [h2 o][h1 i]: columns 16 jb .. +15
-            const float u = scl[C3_OW2];
+            const float u = scn[C3_OW2];
             if (m < nn.h2)
 #pragma unroll
               for (int j = 0; j < 16; ++j)
                 if (16 * jb + j < nn.h1) dst[nn.w_off[1] + m * nn.h1 + 16 * jb + j] = v[j] * u;
           } else if (jb < 6) {  // dW1 [h1 o][n_in i] in columns 0..30, db1 in column 31
             const int c0 = 16 * (jb - 4);
-            const float u = scl[C3_OW1];
+            const float u = scn[C3_OW1];
             if (m < nn.h1) {
 #pragma unroll
               for (int j = 0; j < 16; ++j)
                 if (c0 + j < n_in)
                   dst[nn.w_off[0] + m * n_in + c0 + j] = ((v[j] + w[j]) * u) * s_xs[32 + c0 + j];
-              if (jb == 5) dst[nn.b_off[0] + m] = (v[15] + w[15]) * scl[C3_OB];
+              if (jb == 5) dst[nn.b_off[0] + m] = (v[15] + w[15]) * scn[C3_OB];
             }
           } else if (jb == 6) {  // dW3^T [h2 i][16 o]
-            const float u = scl[C3_OW3];
+            const float u = scn[C3_OW3];
             if (m < nn.h2)
 #pragma unroll
               for (int a = 0; a < 15; ++a)
                 if (a < nn.n_out) dst[nn.w_off[2] + a * nn.h2 + m] = (v[a] + w[a]) * u;
           } else {  // db2 (column 15 = sum_r dZ2[r][o] * ones)
-            if (m < nn.h2) dst[nn.b_off[1] + m] = v[15] * scl[C3_OB];
+            if (m < nn.h2) dst[nn.b_off[1] + m] = v[15] * scn[C3_OB];
           }
         }
       }
     }
-    // per-thread sums -> per-warp sums (tree) -> the 16 warps in order: fixed order => reproducible.  The scratch
-    // aliases the X buffers (idle now).
+    // per-thread sums -> per-warp sums (tree) -> the warps in order: fixed order => reproducible.  The scratch aliases
+    // the X buffers (idle now).
     float* e_db3 = reinterpret_cast<float*>(sm + S3_XB + S3_END_DB3);
     double* e_sc = reinterpret_cast<double*>(sm + S3_XB + S3_END_SC);
-#pragma unroll
-    for (int a = 0; a < 15; ++a) {
-      float t = db3[a];
-#pragma unroll
-      for (int o2 = 16; o2 > 0; o2 >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o2);
-      if (lane == 0) e_db3[warp * 16 + a] = t;
-    }
     {
-      float t = db3v;
+      // b3: warp 4 m + j takes class m of rows 32 j .. 32 j + 31 (see ACC_DB3); a class without tiles was never written
+      const int m = warp >> 2, rr = 32 * (warp & 3) + lane;
 #pragma unroll
-      for (int o2 = 16; o2 > 0; o2 >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o2);
-      if (lane == 0) e_db3[warp * 16 + 15] = t;
+      for (int a = 0; a < 16; ++a) {
+        const int cn = a == 15 ? 1 : 0;
+        const bool have = (cn == 0 ? run_p : run_v) && ((m - 2 * cn) & 3) < cta_tiles;
+        float t = have ? acc[(ACC_DB3 + 16 * m + a) * ACC_LANES + rr] : 0.f;
+#pragma unroll
+        for (int o2 = 16; o2 > 0; o2 >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o2);
+        if (lane == 0) e_db3[warp * 16 + a] = t;
+      }
     }
 #pragma unroll
     for (int kk = 0; kk < 5; ++kk) {
@@ -728,20 +811,23 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
       if (lane == 0) e_sc[warp * 8 + kk] = t;
     }
     {
+      // policy rows evaluated: the valid rows this thread owned, counted here rather than in a register of the loop
+      int rows_done = 0;
+      if (c == 0 && runs && q < 2)
+        for (int k = 0; k < cta_tiles; ++k) rows_done += (blockIdx.x + (long long)k * gridDim.x) * T3_ROWS + r0 + 8 * q < p.n_rows;
       const double t = warp_sum((double)rows_done);
       if (lane == 0) e_sc[warp * 8 + 5] = t;
-      const double t2 = warp_sum(vs);
-      if (lane == 0) e_sc[warp * 8 + 6] = t2;
     }
-    asm volatile("bar.sync 2, %0;" ::"n"(T3_EPI_THREADS) : "memory");
+    asm volatile("bar.sync 6, %0;" ::"n"(T3_CHAIN_THREADS) : "memory");
     const size_t Ptot = (size_t)(p.P[0] + p.P[1]);
-    if (tid < 16) {  // b3 gradients: the 16 per-warp totals in warp order
-      const int c = tid == 15 ? 1 : 0, a = tid == 15 ? 0 : tid;
-      const bool runs = c == 0 ? run_p : run_v;
-      if (runs && a < p.net[c].n_out) {
+    constexpr int NW = T3_CHAIN_WARPS / 2;  // warps per network: policy 0..7, value 8..15
+    if (tid < 16) {  // b3 gradients: the 16 per-warp totals in warp order; policy a = 0..14, value in slot 15
+      const int cn = tid == 15 ? 1 : 0, a = tid == 15 ? 0 : tid;
+      const bool ran = cn == 0 ? run_p : run_v;
+      if (ran && a < p.net[cn].n_out) {
         float t = 0.f;
-        for (int w = 0; w < T3_EPI_WARPS; ++w) t += e_db3[w * 16 + tid];
-        const size_t off = (c == 0 ? 0 : (size_t)p.P[0]) + p.net[c].b_off[2] + a;
+        for (int w = 0; w < T3_CHAIN_WARPS; ++w) t += e_db3[w * 16 + tid];
+        const size_t off = (cn == 0 ? 0 : (size_t)p.P[0]) + p.net[cn].b_off[2] + a;
         p.partials[((size_t)blockIdx.x * 2) * Ptot + off] = t;
         p.partials[((size_t)blockIdx.x * 2 + 1) * Ptot + off] = 0.f;
       }
@@ -750,9 +836,9 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
       const int s = tid - 32;
       double t = 0.0;
       if (s < 6) {
-        for (int w = 0; w < T3_EPI_WARPS; ++w) t += e_sc[w * 8 + s];
+        for (int w = 0; w < NW; ++w) t += e_sc[w * 8 + s];
       } else if (s == 8) {
-        for (int w = 0; w < T3_EPI_WARPS; ++w) t += e_sc[w * 8 + 6];
+        for (int w = NW; w < 2 * NW; ++w) t += e_sc[w * 8 + 0];
       }
       p.scalar_partials[((size_t)blockIdx.x * 2) * (2 * B200RL_N_SCALARS) + s] = t;
       p.scalar_partials[((size_t)blockIdx.x * 2 + 1) * (2 * B200RL_N_SCALARS) + s] = 0.0;
@@ -760,10 +846,9 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     if (bad) *s_bad = 1;
 #ifdef B200RL_TC3_TIMING
     if (tid == 0 && blockIdx.x == 0) {
-      for (int i = 0; i < 20; ++i) g_tc3_t[i] = tacc[i];
-      g_tc3_t[42] = (unsigned long long)(t_loop0 - t_kernel0);   // setup
-      g_tc3_t[43] = (unsigned long long)(t_loop_end - t_loop0);  // tile loop
-      g_tc3_t[44] = (unsigned long long)(clock64() - t_loop_end);  // read-out
+      g_tc3_t[53] = (unsigned long long)(t_loop0 - t_kernel0);      // setup
+      g_tc3_t[54] = (unsigned long long)(t_loop_end - t_loop0);     // tile loop (chain warpgroup 0)
+      g_tc3_t[55] = (unsigned long long)(clock64() - t_loop_end);   // read-out
     }
 #endif
   }
@@ -1042,11 +1127,11 @@ int launch_reduce_adam3(const Ra3Args& a, cudaStream_t s) {
 }  // namespace b200rl
 
 #ifdef B200RL_TC3_TIMING
-extern "C" int b200rl_debug_tc3_timing(unsigned long long* out48, int reset) {
+extern "C" int b200rl_debug_tc3_timing(unsigned long long* out64, int reset) {
   if (reset) {
-    unsigned long long z[48] = {0};
+    unsigned long long z[64] = {0};
     return (int)cudaMemcpyToSymbol(b200rl::g_tc3_t, z, sizeof(z));
   }
-  return (int)cudaMemcpyFromSymbol(out48, b200rl::g_tc3_t, sizeof(unsigned long long) * 48);
+  return (int)cudaMemcpyFromSymbol(out64, b200rl::g_tc3_t, sizeof(unsigned long long) * 64);
 }
 #endif

@@ -42,15 +42,19 @@ if __name__ == "__main__":
         import ctypes as C
         from rl_replicas_b200 import _lib
         lib = _lib.load()
-        out = (C.c_ulonglong * 48)()
+        out = (C.c_ulonglong * 64)()
         lib.b200rl_debug_tc3_timing(out, 1)
         e.run_stage("fused_step_kernel", hp)
         torch.cuda.synchronize()
         lib.b200rl_debug_tc3_timing(out, 0)
-        tiles = max(int(out[41]), 1)
-        names = [f"E{s}{'pv'[c]}" for s in range(1, 6) for c in range(2)]
-        print("tiles of CTA 0:", tiles, "setup", int(out[42]), "tile loop", int(out[43]), "read-out", int(out[44]), "cycles")
-        print("job wait  / tile:", {n: int(out[i]) // tiles for i, n in enumerate(names)}, "sum", sum(int(out[i]) for i in range(10)) // tiles)
-        print("job work  / tile:", {n: int(out[10 + i]) // tiles for i, n in enumerate(names)}, "sum", sum(int(out[10 + i]) for i in range(10)) // tiles)
-        print("issuer wait/tile:", {n.replace('E', 'S'): int(out[20 + i]) // tiles for i, n in enumerate(names)}, "sum", sum(int(out[20 + i]) for i in range(10)) // tiles)
-        print("issuer issue/tile:", {n.replace('E', 'S'): int(out[30 + i]) // tiles for i, n in enumerate(names)}, "sum", sum(int(out[30 + i]) for i in range(10)) // tiles, "xfull wait", int(out[40]) // tiles)
+        tiles = max(int(out[52]), 1)
+        print("tiles of CTA 0:", tiles, "set-up", int(out[53]), "tile loop", int(out[54]), "read-out", int(out[55]), "cycles")
+        for wg in range(4):
+            wait = [int(out[10 * wg + s]) // tiles for s in range(5)]
+            work = [(int(out[10 * wg + 5 + s]) - int(out[10 * wg + s])) // tiles for s in range(5)]
+            name = f"{'pv'[wg >> 1]}{wg & 1}"
+            print(f"chain {name} wait / tile:", dict(zip(("E1", "E2", "E3", "E4", "E5"), wait)), "sum", sum(wait))
+            print(f"chain {name} work / tile:", dict(zip(("E1", "E2", "E3", "E4", "E5"), work)), "sum", sum(work))
+        keys = [f"{st}{'pv'[c]}" for c in range(2) for st in ("dW3", "dW2", "dW1")]
+        print("gradient wait  / tile:", {k: int(out[40 + i]) // tiles for i, k in enumerate(keys)}, "sum", sum(int(out[40 + i]) for i in range(6)) // tiles)
+        print("gradient issue / tile:", {k: int(out[46 + i]) // tiles for i, k in enumerate(keys)}, "sum", sum(int(out[46 + i]) for i in range(6)) // tiles)

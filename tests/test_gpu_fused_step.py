@@ -147,14 +147,27 @@ def test_fused_step_range_trip_is_redone_on_the_wide_range_path():
     assert f.last_update_stats.fused == 1
 
 
-def test_fused_step_is_bit_reproducible():
+def _assert_bit_reproducible(n_envs, horizon):
+    """Two PPO updates of 4 + 4 fused iterations on the same learner state and batch leave identical networks."""
     from rl_replicas_b200 import synthetic
     rng = np.random.default_rng(6)
     ps, vs = [17, 64, 64, 6], [17, 64, 64, 1]
     pl, vl = _layers(rng, ps), _layers(rng, vs)
     log_std = np.full(6, -0.5, np.float32)
-    b = synthetic.fixed_batch(300, 100, 17, 6, seed=1, mean_fn=lambda o: O.mlp_forward(pl, o)[0])
+    b = synthetic.fixed_batch(n_envs, horizon, 17, 6, seed=1, mean_fn=lambda o: O.mlp_forward(pl, o)[0])
     hp = dict(num_policy_gradients=4, num_value_gradients=4, max_kl_divergence=float("inf"))
     runs = [_run(ps, vs, "gaussian", pl, vl, log_std, b, **hp) for _ in range(2)]
+    assert all(r.last_update_stats.fused == 1 for r in runs)
     np.testing.assert_array_equal(flat(runs[0].policy.network), flat(runs[1].policy.network))
     np.testing.assert_array_equal(flat(runs[0].value_function.network), flat(runs[1].value_function.network))
+
+
+def test_fused_step_is_bit_reproducible():
+    _assert_bit_reproducible(300, 100)
+
+
+def test_fused_step_is_bit_reproducible_at_nine_tiles_per_cta():
+    """Nine full 128-row tiles on every CTA (the grid is one CTA per SM): both observation buffers, the b3 class sums
+    and the mbarrier phases go round several times per launch."""
+    import torch
+    _assert_bit_reproducible(9 * torch.cuda.get_device_properties(0).multi_processor_count, 128)

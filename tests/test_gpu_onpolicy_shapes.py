@@ -34,7 +34,10 @@ pytestmark = pytest.mark.gpu
 
 # Largest errors measured on an H100 over all cases of each path (gradients against their conditioning scale):
 # fp16x2 2.1e-6, bf16x3 2.0e-6, fp32 1.8e-6, fvp 1.4e-6; each bar is about 4x that.  The first three are the one-row
-# case, whose single row gets no averaging of its rounding errors; every multi-row case stays under 1.5e-6.
+# case, whose single row gets no averaging of its rounding errors; every multi-row case stays under 1.5e-6.  The fused
+# step (mlp_tc3, fp16x2) measured on an H100 80GB HBM3 at 700 W: gradients at most 4.1e-7 (one tile of 65 rows), with
+# no growth in tiles per CTA (largest policy / value tensor 6.6e-8 / 3.0e-8 at 1 tile per CTA, 3.8e-8 / 1.2e-7 at 4-5,
+# 3.4e-8 / 1.6e-7 at 9); its scalar sums at most 1.2e-6 (the PPO loss sum with 8-sigma actions).
 BAR = {"fp16x2": 8e-6, "bf16x3": 8e-6, "fp32": 7e-6, "fvp": 6e-6}
 ARITH = {"tc2": "fp16x2", "tc": "bf16x3", "fp32": "fp32"}
 CLIP, CLIP_MARGIN, KINK = 0.2, 1e-3, 1e-6
@@ -124,18 +127,29 @@ def draw_obs(rng, sizes_list, n, hidden):
     return pool[keep]
 
 
-def policy_problem(sizes, dist, n, seed, hidden="tanh", log_std=None, sigmas=None, out_scale=None, obs_outlier=None):
+def policy_problem(sizes, dist, n, seed, hidden="tanh", log_std=None, sigmas=None, out_scale=None, obs_outlier=None,
+                   vs=None, obs_scale=None, ret_scale=None):
     """Policy and value networks, observations, actions, advantages and old log-probs.  log_std: the value of every
-    entry (default a spread over [-0.8, -0.2]); sigmas: in every row one action coordinate (at random) exactly this
-    many standard deviations from the mean, the others a normal draw; out_scale: the policy's last layer scaled so that
-    max |output| (mean or logit) is this; obs_outlier: observation row 11 multiplied by this."""
+    entry, or one value per entry (default a spread over [-0.8, -0.2]); sigmas: in every row one action coordinate (at
+    random) exactly this many standard deviations from the mean, the others a normal draw; out_scale: the policy's last
+    layer scaled so that max |output| (mean or logit) is this; obs_outlier: observation row 11 multiplied by this; vs:
+    the value network's sizes (default the policy's with one output); obs_scale: observation column j multiplied by
+    obs_scale[j] (a scalar: every column) and column j of both first layers divided by it, so that the networks see
+    inputs of the usual size (a column scaled by 0 is all zeros and its weights stay); ret_scale: the returns
+    multiplied by this."""
     rng = np.random.default_rng(seed)
     A = sizes[-1]
-    vs = sizes[:-1] + [1]
+    vs = sizes[:-1] + [1] if vs is None else vs
     flat, vflat = net(rng, sizes), net(rng, vs)
     obs = draw_obs(rng, [(sizes, flat), (vs, vflat)], n, hidden)
     if obs_outlier is not None:
         obs[11] *= np.float32(obs_outlier)
+    if obs_scale is not None:
+        col = np.broadcast_to(np.asarray(obs_scale, np.float32), (sizes[0],))
+        obs *= col[None, :]
+        for f, s in ((flat, sizes), (vflat, vs)):
+            w1 = f[:s[0] * s[1]].reshape(s[1], s[0])
+            w1 /= np.where(col != 0, col, np.float32(1))[None, :]
     ls = None
     if dist == "gaussian":
         ls = np.full(A, log_std, np.float32) if log_std is not None else np.linspace(-0.8, -0.2, A).astype(np.float32)
@@ -160,7 +174,7 @@ def policy_problem(sizes, dist, n, seed, hidden="tanh", log_std=None, sigmas=Non
     near = R.clip_margin(np.exp(logp - old_logp), CLIP) < CLIP_MARGIN
     old_logp[near] += np.float32(5e-3)
     assert R.clip_margin(np.exp(logp - old_logp), CLIP).min() >= CLIP_MARGIN
-    ret = (5.0 * rng.standard_normal(n)).astype(np.float32)
+    ret = (5.0 * (1.0 if ret_scale is None else ret_scale) * rng.standard_normal(n)).astype(np.float32)
     return dict(sizes=sizes, vs=vs, dist=dist, flat=flat, vflat=vflat, obs=obs, act=act, log_std=ls, adv_raw=adv_raw,
                 stats=stats, old_logp=old_logp, ret=ret, hidden=hidden, n=n)
 
@@ -503,20 +517,16 @@ def engine_grad_errs(e, b, ps, vs, dist, log_std):
     return errs
 
 
-@pytest.mark.parametrize("ps,vs,dist,n_envs,horizon,fused", [
-    ([31, 64, 64, 15], [31, 64, 64, 1], "gaussian", 7, 139, 1),      # obs 31, 15 outputs; 973 rows: 7 tiles + 77 rows
-    ([31, 63, 32, 15], [31, 1, 64, 1], "categorical", 3, 43, 1),     # uneven widths; 129 rows: one 128-row tile + 1 row
-    # obs 32: the fused step refuses it, so PPO takes the two-loop path with the absmax hint slots 0..31 (batch) and
-    # 32..63 (last observations) exactly full
-    ([32, 64, 64, 15], [32, 64, 64, 1], "gaussian", 7, 139, 0),
-])
-def test_engine_step_gradients(ps, vs, dist, n_envs, horizon, fused, path):
+def test_engine_step_gradients(path):
     """One PPO update with one policy and one value step from zeroed Adam state: the policy_grad / value_grad views hold
-    the gradients at the initial parameters, from the engine's own advantages, returns and old log-probs."""
+    the gradients at the initial parameters, from the engine's own advantages, returns and old log-probs.  obs 32: the
+    fused step refuses it, so PPO takes the two-loop path with the absmax hint slots 0..31 (batch) and 32..63 (last
+    observations) exactly full.  (The fused step's gradients: test_fused_step_gradients.)"""
     from rl_replicas_b200.engine import OnPolicyEngine
+    ps, vs, dist, n_envs, horizon = [32, 64, 64, 15], [32, 64, 64, 1], "gaussian", 7, 139
     e, b, log_std, pol0, val0 = engine_for(ps, vs, dist, n_envs, horizon, seed=ps[-1] + n_envs)
     st = e.update(OnPolicyEngine.hparams(num_policy_gradients=1, num_value_gradients=1, max_kl_divergence=math.inf))
-    assert st.fused == fused and st.policy_steps_applied == 1 and st.value_steps_applied == 1
+    assert st.fused == 0 and st.policy_steps_applied == 1 and st.value_steps_applied == 1
     errs = {}
     v = lambda k: e.view(k).cpu().numpy()
     ref_p = R.policy_loss(pol0, ps, b["obs"], b["act"], dist, "ppo_clip", log_std, v("adv_raw"), v("adv_stats"),
@@ -526,7 +536,7 @@ def test_engine_step_gradients(ps, vs, dist, n_envs, horizon, fused, path):
     errs.update(grad_errs(v("value_grad")[:val0.size], ref_v, vs, "value.d"))
     errs["values"] = rel_err(v("values"), R.values(val0, vs, b["obs"]))
     e.close()
-    report(f"{'fused step' if fused else 'two-loop step'} {ps} {vs} n={b['obs'].shape[0]}", "fp16x2", errs)
+    report(f"two-loop step {ps} {vs} n={b['obs'].shape[0]}", "fp16x2", errs)
 
 
 def test_run_stage_views_show_the_buffer_the_stage_wrote(path):
@@ -545,6 +555,193 @@ def test_run_stage_views_show_the_buffer_the_stage_wrote(path):
         e.run_stage(st, hp)
     report("run_stage fused after a two-loop update", "fp16x2", engine_grad_errs(e, b, ps, vs, "gaussian", log_std))
     e.close()
+
+
+# One fused launch on chosen inputs.  Rows may depend on S, the SM count: the grid is min(tiles, S) and CTA b runs tiles
+# b, b + S, b + 2 S, ..., so 128 S rows are one tile per CTA.  Each row keeps its b3 gradient in four running sums, one
+# per tile class k mod 4, that add to an earlier tile's sum from tile k = 4 on: 5 tiles per CTA and more.
+OBS_COLUMNS = np.r_[10.0 ** np.linspace(-3, 3, 16), 0.0]  # 16 feature scales 1e-3 .. 1e3 and an all-zero column
+FUSED_CASES = {
+    # one tile: the second 64-row half empty, holding one row, one row short of full
+    "one_tile_64": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=64),
+    "one_tile_65": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=65),
+    "one_tile_127": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=127),
+    "one_tile_64_cat": dict(sizes=[8, 64, 64, 15], dist="categorical", n=64),
+    "one_tile_65_cat": dict(sizes=[8, 64, 64, 15], dist="categorical", n=65),
+    "one_tile_127_cat": dict(sizes=[8, 64, 64, 15], dist="categorical", n=127),
+    # obs 31, 15 outputs; 973 rows: 7 tiles + 77 rows
+    "obs31_out15_973": dict(sizes=[31, 64, 64, 15], dist="gaussian", n=973),
+    # uneven widths, a value network whose first hidden layer is one unit wide; 129 rows: one tile + 1 row
+    "uneven_129_cat": dict(sizes=[31, 63, 32, 15], vs=[31, 1, 64, 1], dist="categorical", n=129),
+    # one full round, 1 tile per CTA: the widest observation, the most outputs
+    "full_round": dict(sizes=[31, 64, 64, 15], dist="gaussian", n=lambda S: 128 * S),
+    # 2 tiles per CTA (both observation buffers and their phases), the last tile half full
+    "2_tiles": dict(sizes=[31, 64, 63, 15], dist="categorical", n=lambda S: 128 * 2 * S - 64),
+    # 5 tiles on half of the CTAs, 4 on the others, the last tile one row
+    "4_5_tiles": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=lambda S: 128 * (4 * S + S // 2) + 1),
+    "4_5_tiles_cat": dict(sizes=[8, 64, 64, 15], dist="categorical", n=lambda S: 128 * (4 * S + S // 2) + 1),
+    # 9 tiles per CTA, ragged last tile
+    "9_tiles": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=lambda S: 128 * 9 * S - 51),
+    # hidden layers one unit wide in both networks
+    "narrow": dict(sizes=[1, 1, 64, 2], vs=[1, 64, 1, 1], dist="categorical", n=3000),
+    # distributions at their edges (see GATE_CASES)
+    "log_std_-5": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=3000, log_std=-5.0, out_scale=0.02),
+    "log_std_+1": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=3000, log_std=1.0),
+    "actions_8_sigma": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=3000, log_std=-0.5, sigmas=8.0),
+    "logits_30": dict(sizes=[8, 64, 64, 15], dist="categorical", n=3000, out_scale=30.0),
+    # sigmas e^-5 .. e^1 under one gradient scale (set by the smallest)
+    "log_std_spread": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=3000, log_std=np.linspace(-5.0, 1.0, 6),
+                           out_scale=0.02),
+    # data-parallel: these rows are a quarter of the global batch
+    "n_global_4n": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=3000, dp=4),
+    # operand ranges the power-of-two scales absorb: the step stays on the fused path
+    "obs_x1e3": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=3000, obs_scale=1e3),
+    "obs_x1e-4": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=3000, obs_scale=1e-4),
+    "ret_x3e4": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=3000, ret_scale=3e4),
+    "ret_x1e-3": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=3000, ret_scale=1e-3),
+    "obs_columns": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=3000, obs_scale=OBS_COLUMNS),
+}
+
+
+def fused_problem(name):
+    c = dict(FUSED_CASES[name])
+    n, dp = c.pop("n"), c.pop("dp", 1)
+    n = n(sms()) if callable(n) else n
+    pb = policy_problem(c.pop("sizes"), c.pop("dist"), n, seed=500 + list(FUSED_CASES).index(name), **c)
+    pb["n_global"] = dp * n
+    return pb
+
+
+def perturbed(pb, seed):
+    """The policy with its output bias moved in a random direction, by 0.5 in sigma units (Gaussian: log-ratios of
+    rows about N(-1/8, 1/4)) or by 1 (logits): PPO ratios spread past both clip bounds, the KL from the unperturbed
+    policy is clearly positive, and no ratio is so large that a gradient row leaves fp16's range."""
+    A = pb["sizes"][-1]
+    w = np.random.default_rng(seed).standard_normal(A)
+    w /= np.linalg.norm(w)
+    flat = pb["flat"].copy()
+    flat[-A:] += (0.5 * np.exp(pb["log_std"].astype(np.float64)) * w if pb["dist"] == "gaussian" else w
+                  ).astype(np.float32)
+    return flat
+
+
+def fused_engine(pb, policy, old_policy):
+    """An engine whose batch holds the problem's observations and actions, with its returns as the rewards (episodes of
+    100 rows, every other one done): with gamma = 0 the scan's returns are the rewards, so the returns' absmax, which
+    sets the value gradient's scale, is the problem's."""
+    from rl_replicas_b200.engine import OLD_POLICY, POLICY, VALUE, OnPolicyEngine
+    n = pb["n"]
+    off = np.r_[np.arange(0, n, 100), n].astype(np.int64)
+    b = dict(obs=pb["obs"], act=pb["act"], rew=pb["ret"].astype(np.float64), last_obs=pb["obs"][off[1:] - 1],
+             ep_offsets=off, ep_done=np.arange(off.size - 1) % 2 == 0)
+    e = OnPolicyEngine(pb["sizes"], pb["vs"], pb["dist"], n, off.size - 1)
+    e.set_params(POLICY, policy)
+    e.set_params(OLD_POLICY, old_policy)
+    e.set_params(VALUE, pb["vflat"])
+    if pb["log_std"] is not None:
+        e.set_log_std(pb["log_std"])
+    e.set_adam(POLICY, None, None, 0)
+    e.set_adam(VALUE, None, None, 0)
+    e.load_batch(b)
+    return e
+
+
+def fused_hp(pb, K=1, Kv=1, max_kl=math.inf):
+    from rl_replicas_b200.engine import OnPolicyEngine
+    return OnPolicyEngine.hparams(gamma=0.0, gae_lambda=0.0, max_kl_divergence=max_kl, num_policy_gradients=K,
+                                  num_value_gradients=Kv, n_global_rows=pb["n_global"])
+
+
+def bits(x):
+    return np.ascontiguousarray(x).view(np.uint32 if x.dtype == np.float32 else np.uint64)
+
+
+def assert_clip_binds_both_ways(ref, n):
+    if n >= 100:
+        assert (ref["ratio"] > 1 + CLIP).any() and (ref["ratio"] < 1 - CLIP).any()
+
+
+@pytest.mark.parametrize("name", list(FUSED_CASES))
+def test_fused_step_gradients(name, path):
+    """policy_grad / value_grad of one fused launch (run_stage "fused_step") on the problem's advantages, statistics
+    and old log-probs, against the reference."""
+    pb = fused_problem(name)
+    s, vs, n, ng = pb["sizes"], pb["vs"], pb["n"], pb["n_global"]
+    e = fused_engine(pb, pb["flat"], pb["flat"])
+    hp = fused_hp(pb)
+    e.run_stage("preamble", hp)
+    np.testing.assert_array_equal(bits(e.view("ret").cpu().numpy()), bits(pb["ret"]))
+    for k in ("adv_raw", "stats", "old_logp"):
+        e.view("adv_stats" if k == "stats" else k).copy_(torch.from_numpy(pb[k]))
+    e.run_stage("pack_obs", hp)
+    e.run_stage("fused_step", hp)
+    got_p, got_v = e.view("policy_grad").cpu().numpy(), e.view("value_grad").cpu().numpy()
+    e.close()
+    ref_p = R.policy_loss(pb["flat"], s, pb["obs"], pb["act"], pb["dist"], "ppo_clip", pb["log_std"], pb["adv_raw"],
+                          pb["stats"], pb["old_logp"], CLIP, n_global=ng)
+    ref_v = R.value_loss(pb["vflat"], vs, pb["obs"], pb["ret"], n_global=ng)
+    assert_clip_binds_both_ways(ref_p, n)
+    errs = grad_errs(got_p, ref_p, s, "policy.d")
+    errs.update(grad_errs(got_v, ref_v, vs, "value.d"))
+    report(f"fused step {name} {s} {vs} n={n} n_global={ng}", "fp16x2", errs)
+
+
+@pytest.mark.parametrize("name", list(FUSED_CASES))
+def test_fused_step_scalar_sums(name, path):
+    """One PPO update with one step of each loop, the policy moved off the network the actions were drawn around: it
+    stays on the fused path, and the scalar sums of its launch (slot 0: policy, slot K + 1 = 2: value) match the
+    reference from the engine's own advantages, statistics and old log-probs."""
+    pb = fused_problem(name)
+    s, vs, n, ng = pb["sizes"], pb["vs"], pb["n"], pb["n_global"]
+    pol = perturbed(pb, 1 + list(FUSED_CASES).index(name))
+    e = fused_engine(pb, pol, pb["flat"])
+    st = e.update(fused_hp(pb))
+    v = lambda k: e.view(k).cpu().numpy()
+    adv_raw, stats, old_logp = v("adv_raw"), v("adv_stats"), v("old_logp")
+    slots = e.scalar_history()
+    e.close()
+    assert st.fused == 1 and st.policy_steps_applied == 1 and st.value_steps_applied == 1
+    ref = R.policy_loss(pol, s, pb["obs"], pb["act"], pb["dist"], "ppo_clip", pb["log_std"], adv_raw, stats, old_logp,
+                        CLIP, n_global=ng)
+    assert_clip_binds_both_ways(ref, n)
+    ref_v = R.value_loss(pb["vflat"], vs, pb["obs"], pb["ret"], n_global=ng)
+    s0 = slots[0]
+    errs = {"loss": scal_err(s0[0], ref["loss_sum"], ref["loss_abs_sum"]),
+            "kl": scal_err(s0[1], ref["kl_sum"], ref["logp_abs_sum"]),
+            "entropy_sum": scal_err(s0[2], ref["entropy_sum"]),
+            "logp_sum": scal_err(s0[3], ref["logp_sum"], ref["logp_abs_sum"]),
+            "logp2_sum": scal_err(s0[4], ref["logp2_sum"]),
+            "mse.loss": scal_err(slots[2][0], ref_v["loss_sum"])}
+    assert s0[5] == n
+    report(f"fused step sums {name} {s} {vs} n={n} n_global={ng}", "fp16x2", errs)
+
+
+@pytest.mark.parametrize("tiles", [1, 5])
+def test_fused_value_only_launches_match_full_launches(tiles, path):
+    """The device-side KL stop fires at step 0 of three: launches 1 and 2 run the value chain alone (no host poll in
+    between).  Everything of the value loop is bit-identical to the same update without a KL limit."""
+    from rl_replicas_b200.engine import POLICY, VALUE
+    K = 3
+    pb = policy_problem([17, 64, 64, 6], "gaussian", 128 * tiles * sms() - 37, seed=600 + tiles)
+    pb["n_global"] = pb["n"]
+    pol = perturbed(pb, 2)
+    args = (pb["sizes"], pb["obs"], pb["act"], "gaussian", "eval", pb["log_std"])
+    kl0 = float(np.mean(R.policy_loss(pb["flat"], *args)["logp"] - R.policy_loss(pol, *args)["logp"]))
+    assert kl0 > 1e-3  # the KL carried by step 0 (POLICY against the OLD_POLICY the actions came from)
+    runs = {}
+    for label, max_kl in (("stop", kl0 / 3), ("no limit", math.inf)):
+        e = fused_engine(pb, pol, pb["flat"])
+        st = e.update(fused_hp(pb, K=K, Kv=K, max_kl=max_kl))
+        m, vv, _ = e.get_adam(VALUE)
+        runs[label] = dict(st=st, pol=e.get_params(POLICY), val=e.get_params(VALUE), m=m, v=vv,
+                           grad=e.view("value_grad").cpu().numpy(), slots=e.scalar_history()[K + 1:2 * K + 1])
+        e.close()
+    a, b = runs["stop"], runs["no limit"]
+    assert (a["st"].policy_steps_applied, a["st"].value_steps_applied, a["st"].fused) == (0, K, 1)
+    assert (b["st"].policy_steps_applied, b["st"].value_steps_applied, b["st"].fused) == (K, K, 1)
+    np.testing.assert_array_equal(bits(a["pol"]), bits(pol))
+    for k in ("val", "m", "v", "grad", "slots"):
+        np.testing.assert_array_equal(bits(a[k]), bits(b[k]), err_msg=k)
 
 
 # ---- refusals: host-side checks before any launch ------------------------------------------------------------------

@@ -505,6 +505,69 @@ int b200rl_offpolicy_set_alpha_group(b200rl_offpolicy* h, const float* log_alpha
 int b200rl_offpolicy_get_alpha_group(b200rl_offpolicy* h, float* log_alpha, float* exp_avg, float* exp_avg_sq,
                                      int64_t* step);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Prioritized experience replay for DQN (Schaul et al. 2016, proportional).  Each learner's replay buffer has one
+ * priority per physical row, held on the device in a sum tree (layout below); rows that are not live have priority 0.
+ * Step st of a prioritized call, for each learner:
+ *   draw:    M = the sum of the priorities; for j in 0..B-1, u_j = (j + U_j) * (M / B) with U_j = the top 24 bits of
+ *            Philox4x32-10(counter (j, st, call, 0x9E5), key seed) times 2^-24 (a stream of its own, apart from the
+ *            index and noise draws of train_gather_rng); idx_j = the leaf whose cumulative interval holds u_j.  A leaf
+ *            of priority 0 is never drawn, even when rounding puts u_j at or past the last boundary.
+ *   weights: w_j = (min_k p[idx_k] / p[idx_j])^beta (Schaul's (N P(j))^-beta over its largest value in the minibatch),
+ *            beta = min(1, beta_start + (1 - beta_start) t / beta_anneal_steps), t = the Q optimizer's step count
+ *            before the step (so the schedule carries across calls and get_state / set_state).
+ *   update:  the DQN / Double DQN step with loss (1/B) sum_j w_j huber(delta_j) and output gradient
+ *            w_j clamp(delta_j, -1, 1) / B (q1_losses logs this weighted loss); with every w_j = 1 it is bit for bit the
+ *            unweighted step.
+ *   priorities: for each row j in order (a leaf drawn twice keeps its last row's value), leaf idx_j <- (|delta_j| +
+ *            eps)^alpha with delta_j from before the Adam step, and the running max m <- max(m, that value).  A row
+ *            with an invalid action keeps its leaf as it was; a non-finite |delta_j| or priority leaves its leaf
+ *            unchanged and is counted: the call then returns an error naming the learner and the step.  Interior
+ *            nodes never hold a NaN.
+ *   Step st + 1 draws from the tree step st left.
+ * The draw, the weights and the gather of the five columns are one kernel, the priority update a second one beside the
+ * backward pass: two launches per step more than train_gather_rng's steps, and no per-call draw or gather launches.
+ *
+ * Tree layout (float32, b200rl_per_tree_floats(leaves) floats): level 0 = the leaves (one per physical row), level
+ * k + 1 = the sums of 32 consecutive nodes of level k, added in index order; every level padded with zeros to a
+ * multiple of 32 floats, levels back to back; the last level is [root, running max m, 0 ...].  The buffer owns the
+ * tree (zeroed, m = 1 at creation) and keeps it: b200rl_per_tree_set_range gives rows an append wrote priority m,
+ * b200rl_per_tree_build recomputes every interior node from the leaves.  Interior nodes are always recomputed from
+ * their children, never adjusted by differences: no drift, and groups stay bit-identical to solo engines.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  double alpha;              /* >= 0: priority = (|delta| + eps)^alpha */
+  double eps;                /* > 0 */
+  double beta_start;         /* in [0, 1] */
+  int64_t beta_anneal_steps; /* >= 1 */
+} b200rl_per_hparams;
+
+/* Required before a prioritized call of a DQN engine (other engines are refused); part of the cached graph's key. */
+int b200rl_offpolicy_set_per(b200rl_offpolicy* h, const b200rl_per_hparams* pp);
+/* S prioritized DQN steps on device replay columns (as for train_gather) with `rows` physical rows and their tree
+ * (rows leaves, device memory).  (seed, call) key the draws.  Outputs as for DQN: q1_values [S,B], q1_losses [S]. */
+int b200rl_offpolicy_train_prioritized(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int32_t S, int32_t B,
+                                       const float* d_obs, const float* d_act, const float* d_rew,
+                                       const float* d_next_obs, const float* d_done, int64_t rows, float* tree,
+                                       uint64_t seed, uint64_t call, float* q1_values, float* q1_losses, void* stream);
+/* The same for a learner group: replay[K], trees[K] (K distinct trees: learners never share one), seed[K], call[K];
+ * outputs [K, S, B] and [K, S] */
+int b200rl_offpolicy_train_prioritized_group(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int32_t S,
+                                             int32_t B, const b200rl_offpolicy_replay* replay, float* const* trees,
+                                             const uint64_t* seed, const uint64_t* call, float* q1_values,
+                                             float* q1_losses, void* stream);
+/* Of the last prioritized call (host [K, S, B] each): the drawn rows, their weights and the new priorities they wrote
+ * (NaN for a row that wrote none) -- what a test replays through the oracle.  Refused when the engine's last train
+ * call that ran steps was not a prioritized one (it overwrote the drawn rows). */
+int b200rl_offpolicy_get_per_draws(b200rl_offpolicy* h, int32_t S, int32_t B, int64_t* idx, float* weights,
+                                   float* priorities, void* stream);
+/* Floats of a tree over `leaves` rows (1 <= leaves < 2^31; -1 otherwise). */
+int64_t b200rl_per_tree_floats(int64_t leaves);
+/* Every interior node recomputed from the leaves (stream-ordered). */
+int b200rl_per_tree_build(float* tree, int64_t leaves, void* stream);
+/* Leaves start .. start + count - 1 (modulo leaves: the range may wrap) <- the running max m, ancestors recomputed. */
+int b200rl_per_tree_set_range(float* tree, int64_t leaves, int64_t start, int64_t count, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

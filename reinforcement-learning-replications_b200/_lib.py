@@ -94,6 +94,11 @@ class DqnHparams(C.Structure):
     _fields_ = [("target_update_interval", C.c_int32), ("double_q", C.c_int32)]
 
 
+class PerHparams(C.Structure):
+    _fields_ = [("alpha", C.c_double), ("eps", C.c_double), ("beta_start", C.c_double),
+                ("beta_anneal_steps", C.c_int64)]
+
+
 class OffPolicyReplay(C.Structure):
     _fields_ = [("obs", C.c_void_p), ("act", C.c_void_p), ("rew", C.c_void_p), ("next_obs", C.c_void_p),
                 ("done", C.c_void_p), ("rows", C.c_int64)]
@@ -183,6 +188,16 @@ SIGNATURES = {
     "b200rl_offpolicy_train_gather_rng_group": (C.c_int, [C.c_void_p, C.POINTER(OffPolicyHparams), C.c_int32, C.c_int32,
                                                           C.POINTER(OffPolicyReplay)] + [C.c_void_p] * 9 +
                                                 [C.POINTER(C.c_int32), C.c_void_p]),
+    "b200rl_offpolicy_set_per": (C.c_int, [C.c_void_p, C.POINTER(PerHparams)]),
+    "b200rl_offpolicy_train_prioritized": (C.c_int, [C.c_void_p, C.POINTER(OffPolicyHparams), C.c_int32, C.c_int32] +
+                                           [C.c_void_p] * 5 + [C.c_int64, C.c_void_p, C.c_uint64, C.c_uint64] +
+                                           [C.c_void_p] * 3),
+    "b200rl_offpolicy_train_prioritized_group": (C.c_int, [C.c_void_p, C.POINTER(OffPolicyHparams), C.c_int32,
+                                                           C.c_int32, C.POINTER(OffPolicyReplay)] + [C.c_void_p] * 6),
+    "b200rl_offpolicy_get_per_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32] + [C.c_void_p] * 4),
+    "b200rl_per_tree_floats": (C.c_int64, [C.c_int64]),
+    "b200rl_per_tree_build": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p]),
+    "b200rl_per_tree_set_range": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p]),
     "b200rl_offpolicy_set_alpha_group": (C.c_int, [C.c_void_p] * 5),
     "b200rl_offpolicy_get_alpha_group": (C.c_int, [C.c_void_p] * 5),
     "b200rl_discounted_cumsum": (C.c_int, [C.c_void_p, C.c_int64, C.c_double, C.c_void_p, C.c_void_p]),

@@ -10,6 +10,7 @@ import torch
 from .._lib import OffPolicyHparams
 from ..engine import OffPolicyEngine
 from ..policies import EpsilonGreedyPolicy, GreedyPolicy
+from ..replay_buffer import PrioritizedReplayBuffer
 from ._onpolicy import adam_hparams, describe_mlp
 from .td3 import _learn, _make_eval_env, _OffPolicyBase
 
@@ -19,6 +20,10 @@ class DQN(_OffPolicyBase):
     y = r + gamma (1 - d) Q_targ(s', argmax_a' Q(s', a')) (``double_q``) or r + gamma (1 - d) max_a' Q_targ(s', a'),
     one Adam step on F.smooth_l1_loss(Q(s, a), y), and Q_targ <- Q whenever the Q optimizer's step count reaches a
     multiple of ``target_update_interval`` (the count carries across train() calls and checkpoints).
+
+    With a ``PrioritizedReplayBuffer`` every train() call takes the prioritized device path (draws keyed by
+    ``device_rng_seed``, whatever ``use_device_rng`` says): minibatches drawn in proportion to the priorities, the loss
+    weighted by the importance weights, and the rows' priorities updated from their TD errors (b200rl.h).
 
     Acting: ``exploration_policy`` before ``num_start_steps``, then epsilon-greedy with epsilon falling linearly from
     ``epsilon_start`` to ``epsilon_end`` over the first ``epsilon_decay_steps`` environment steps; evaluation is greedy."""
@@ -96,11 +101,32 @@ class DQN(_OffPolicyBase):
         e.set_dqn(self.target_update_interval, self.double_q)
 
     def _stage_inputs(self, replay_buffer, S: int, B: int, noisy: bool):
+        if isinstance(replay_buffer, PrioritizedReplayBuffer):
+            # always the prioritized device path, keyed like the uniform device draws (device_rng_seed, call count)
+            if not getattr(self, "use_device_replay", True):
+                raise ValueError("a PrioritizedReplayBuffer needs use_device_replay = True: its draws and priority "
+                                 "updates run on the device")
+            if S == 0:
+                return None, None
+            self._device_rng_calls = getattr(self, "_device_rng_calls", 0) + 1
+            t0 = self._adam_step_count(self.q_function.optimizer, describe_mlp(self.q_function.network)[3])
+            self._last_beta = replay_buffer.beta(t0 + S - 1)  # the last step's beta, logged as replay/beta
+            return "per", (getattr(self, "device_rng_seed", 0), self._device_rng_calls)
+        self._last_beta = None
         mode, inputs = super()._stage_inputs(replay_buffer, S, B, noisy)
         if mode == "host":  # the action column as [S, B] indices
             obs, act, rew, nobs, done, _ = inputs
             inputs = (obs, act.reshape(S, B), rew, nobs, done, None)
         return mode, inputs
+
+    @staticmethod
+    def _call_engine(e, hp, replay_buffer, S: int, B: int, mode, inputs):
+        if mode != "per":
+            return _OffPolicyBase._call_engine(e, hp, replay_buffer, S, B, mode, inputs)
+        e.set_per(*replay_buffer.per_settings())
+        tree = replay_buffer.device_tree()
+        columns, rows = replay_buffer.device_columns()
+        return e.train_prioritized(hp, columns, rows, tree, S, B, *inputs)
 
     def _train_schedule(self):
         return False, 1
@@ -122,6 +148,8 @@ class DQN(_OffPolicyBase):
         mm.record_scalar("q-function/max_q-value", float(np.max(q)))
         mm.record_scalar("q-function/min_q-value", float(np.min(q)))
         mm.record_scalar("exploration/epsilon", self.epsilon(), steps, tensorboard=True)
+        if getattr(self, "_last_beta", None) is not None:
+            mm.record_scalar("replay/beta", self._last_beta, steps, tensorboard=True)
 
     def save_model(self, current_epoch: int, model_path: str) -> None:
         torch.save({

@@ -25,6 +25,7 @@ import torch
 
 from .._lib import MAX_LEARNERS
 from ..engine import OffPolicyEngine
+from ..replay_buffer import PrioritizedReplayBuffer
 from ._onpolicy import adam_hparams, describe_mlp
 from .td3 import _learn_begin, _learn_evaluate_save, _learn_sample, _OffPolicyBase
 
@@ -45,6 +46,11 @@ def _signature(agent) -> list:
         for attr in ("gamma", "target_update_interval", "double_q", "epsilon_start", "epsilon_end", "epsilon_decay_steps",
                      "use_device_replay", "use_device_rng"):
             sig.append((attr, getattr(agent, attr, None)))
+        rb = getattr(agent, "replay_buffer", None)
+        sig.append(("prioritized replay", isinstance(rb, PrioritizedReplayBuffer)))
+        for attr in ("alpha", "eps", "beta_start", "beta_anneal_steps"):
+            sig.append((f"prioritized replay {attr}", getattr(rb, attr, None) if isinstance(rb, PrioritizedReplayBuffer)
+                        else None))
         return sig
     sig.append(("action limit", float(agent.env.action_space.high[0])))
     for attr in ("gamma", "polyak_rho", "target_noise_scale", "target_noise_clip", "policy_delay", "use_device_replay",
@@ -56,6 +62,19 @@ def _signature(agent) -> list:
                  adam_hparams(agent.alpha_optimizer, [], "alpha optimizer", extra=[agent.log_alpha])),
                 ("log_std bounds", (agent.policy.log_std_min, agent.policy.log_std_max))]
     return sig
+
+
+def _check_prioritized_buffers(members) -> None:
+    """Each member's PrioritizedReplayBuffer must be its own: the priority updates of all members run at once, and two
+    of them writing one sum tree would race."""
+    seen = {}
+    for k, m in enumerate(members):
+        rb = getattr(m, "replay_buffer", None)
+        if isinstance(rb, PrioritizedReplayBuffer):
+            if id(rb) in seen:
+                raise ValueError(f"LearnerGroup: members {seen[id(rb)]} and {k} share one PrioritizedReplayBuffer; "
+                                 "every prioritized member needs a buffer of its own")
+            seen[id(rb)] = k
 
 
 def _rng_state():
@@ -92,6 +111,7 @@ class LearnerGroup:
             for (name, want), (_, got) in zip(_signature(self.members[0]), _signature(agent)):
                 if got != want:
                     raise ValueError(f"LearnerGroup: {name} differs from the first member's ({got!r} != {want!r})")
+        _check_prioritized_buffers(self.members + [agent])
         self.members.append(agent)
         self._streams.append(_rng_state())
         self._close_engine()
@@ -138,6 +158,7 @@ class LearnerGroup:
         """``agent.train(agent.replay_buffer, num_train_steps, minibatch_size)`` for every member, each on its own replay
         buffer and random stream, as one engine call."""
         members = self._check()
+        _check_prioritized_buffers(members)  # a member's buffer may have been replaced since add()
         S, B = int(num_train_steps), int(minibatch_size)
         if len(members) == 1 or S == 0:  # nothing to batch: the members' own calls
             for k, m in enumerate(members):
@@ -167,7 +188,13 @@ class LearnerGroup:
         if members[0].algo == OffPolicyEngine.DQN:
             e.set_dqn(members[0].target_update_interval, members[0].double_q)
         hp = members[0]._hparams(noisy, delay)
-        if mode == "rng":
+        if mode == "per":
+            e.set_per(*members[0].replay_buffer.per_settings())
+            trees = [m.replay_buffer.device_tree() for m in members]
+            replays = [m.replay_buffer.device_columns() for m in members]
+            out = e.train_prioritized_group(hp, replays, trees, S, B, [st[1][0] for st in staged],
+                                            [st[1][1] for st in staged])
+        elif mode == "rng":
             replays = [m.replay_buffer.device_columns() for m in members]
             rings = [m.replay_buffer.ring() for m in members]
             out = e.train_gather_rng_group(hp, replays, [r[0] for r in rings], [r[1] for r in rings], S, B,

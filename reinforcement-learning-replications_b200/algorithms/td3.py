@@ -14,6 +14,7 @@ import torch
 from .._lib import OffPolicyHparams
 from ..engine import OffPolicyEngine
 from ..metrics_manager import MetricsManager
+from ..replay_buffer import PrioritizedReplayBuffer
 from ..utils import add_noise_to_get_action
 from ._onpolicy import adam_hparams, describe_mlp
 
@@ -198,6 +199,9 @@ class _OffPolicyBase:
         # host side, same random streams as the reference: numpy RNG for the indices (replay_buffer.py:58), torch CPU
         # RNG for the target-smoothing noise (td3.py:328); the two streams are independent, so drawing all minibatches
         # first and all noise second consumes each exactly as the interleaved reference loop does.
+        if isinstance(replay_buffer, PrioritizedReplayBuffer):
+            raise ValueError(f"{type(self).__name__} does not train on a PrioritizedReplayBuffer: prioritized replay is "
+                             "implemented for DQN only")
         device_replay = (S > 0 and getattr(self, "use_device_replay", True) and hasattr(replay_buffer, "device_columns")
                          and hasattr(replay_buffer, "sample_indices"))
         # opt-in (SURVEY 8f-4): indices and smoothing noise drawn on the device -- not the reference's random streams

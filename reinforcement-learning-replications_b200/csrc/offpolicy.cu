@@ -20,6 +20,9 @@
 // enqueue_sac_steps, run as a captured graph or as plain launches like the TD3 / DDPG steps.
 // DQN (config algo = 2) is a third: a per-row Huber loss head on discrete actions (dqn_loss_kernel), a target copy
 // gated by a per-learner step table (dqn_target_copy_kernel) and enqueue_dqn_steps; networks 1 and 4 only.
+// Prioritized replay for DQN (train_prioritized): a 32-way sum tree per replay buffer, drawn from, weighed and gathered
+// by per_draw_kernel and updated by per_update_kernel inside the same step program.
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -551,11 +554,14 @@ __device__ __forceinline__ int argmax_row(const float* q, int n) {
 //   dOut[i, :] = 0 except dOut[i, a] = clamp(delta, -1, 1) / B, q_copy[i] = Q(s)[i, a] (the logged Q-value).
 // A row whose action is not an integer in [0, n) is never used as an index: it adds nothing to the loss or dOut, logs
 // NaN, and is counted in *bad_out (0 when every action is valid).
-template <bool LANES>
-__global__ void __launch_bounds__(GTHREADS) dqn_loss_kernel(const float* q, const float* qt_next, const float* qn,
-                                                           const float* act, const float* rew, const float* done,
-                                                           float gamma, int B, int n, float* dout, float* loss_out,
-                                                           float* q_copy, int* bad_out, size_t lane_stride) {
+// WEIGHTED (prioritized replay): row i's loss and gradient are scaled by w[i] -- loss = (1/B) sum_i w_i huber(delta_i),
+// dOut[i, a] = w_i clamp(delta_i, -1, 1) / B -- and absd[i] = |delta_i| (-1 for a row with an invalid action).  With
+// every w_i = 1 both are bit for bit those of the unweighted head: the products by 1 are exact.
+template <bool LANES, bool WEIGHTED>
+__device__ __forceinline__ void dqn_loss_rows(const float* q, const float* qt_next, const float* qn, const float* act,
+                                              const float* rew, const float* done, float gamma, int B, int n,
+                                              float* dout, float* loss_out, float* q_copy, int* bad_out, const float* w,
+                                              float* absd, size_t lane_stride) {
   __shared__ double red[32];
   __shared__ int bad_rows;
   if (LANES) {
@@ -563,6 +569,7 @@ __global__ void __launch_bounds__(GTHREADS) dqn_loss_kernel(const float* q, cons
     q = lane_ptr(q, o), qt_next = lane_ptr(qt_next, o), qn = lane_ptr(qn, o), act = lane_ptr(act, o);
     rew = lane_ptr(rew, o), done = lane_ptr(done, o), dout = lane_ptr(dout, o), loss_out = lane_ptr(loss_out, o);
     q_copy = lane_ptr(q_copy, o), bad_out = lane_ptr(bad_out, o);
+    if (WEIGHTED) w = lane_ptr(w, o), absd = lane_ptr(absd, o);
   }
   if (threadIdx.x == 0) bad_rows = 0;
   __syncthreads();
@@ -580,11 +587,21 @@ __global__ void __launch_bounds__(GTHREADS) dqn_loss_kernel(const float* q, cons
       const float qi = q[(size_t)i * n + a];
       const float d = qi - td_target(rew[i], done[i], v, nullptr, i, gamma);
       const float ad = fabsf(d);
-      acc += ad < 1.f ? 0.5 * (double)d * (double)d : (double)ad - 0.5;
-      g = (d > 1.f ? 1.f : (d < -1.f ? -1.f : d)) * inv;  // NaN passes through, as torch's clamp lets it
+      const double hub = ad < 1.f ? 0.5 * (double)d * (double)d : (double)ad - 0.5;
+      const float c = d > 1.f ? 1.f : (d < -1.f ? -1.f : d);  // NaN passes through, as torch's clamp lets it
+      if (WEIGHTED) {
+        const float wi = w[i];
+        acc += (double)wi * hub;
+        g = (wi * c) * inv;
+        absd[i] = ad;
+      } else {
+        acc += hub;
+        g = c * inv;
+      }
       q_copy[i] = qi;
     } else {
       q_copy[i] = __int_as_float(0x7fc00000);
+      if (WEIGHTED) absd[i] = -1.f;
       ++bad;
     }
     for (int j = 0; j < n; ++j) dout[(size_t)i * n + j] = j == a ? g : 0.f;
@@ -592,6 +609,26 @@ __global__ void __launch_bounds__(GTHREADS) dqn_loss_kernel(const float* q, cons
   if (bad) atomicAdd(&bad_rows, bad);
   block_mean(acc, B, loss_out, red);  // its __syncthreads orders every thread's atomicAdd before thread 0 reads
   if (threadIdx.x == 0) *bad_out = bad_rows;
+}
+
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) dqn_loss_kernel(const float* q, const float* qt_next, const float* qn,
+                                                           const float* act, const float* rew, const float* done,
+                                                           float gamma, int B, int n, float* dout, float* loss_out,
+                                                           float* q_copy, int* bad_out, size_t lane_stride) {
+  dqn_loss_rows<LANES, false>(q, qt_next, qn, act, rew, done, gamma, B, n, dout, loss_out, q_copy, bad_out, nullptr,
+                              nullptr, lane_stride);
+}
+
+// the prioritized-replay head: importance weights w [B] in, |delta| [B] out (see dqn_loss_rows)
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) dqn_per_loss_kernel(const float* q, const float* qt_next, const float* qn,
+                                                               const float* act, const float* rew, const float* done,
+                                                               float gamma, int B, int n, float* dout, float* loss_out,
+                                                               float* q_copy, int* bad_out, const float* w, float* absd,
+                                                               size_t lane_stride) {
+  dqn_loss_rows<LANES, true>(q, qt_next, qn, act, rew, done, gamma, B, n, dout, loss_out, q_copy, bad_out, w, absd,
+                             lane_stride);
 }
 
 // target <- param on the steps the copy table marks (flags[idx].x != 0): the graph launches the copy every step and
@@ -606,6 +643,213 @@ __global__ void dqn_target_copy_kernel(float* target, const float* param, int n,
   if (flags[idx].x == 0.f) return;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) target[i] = param[i];
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Prioritized experience replay (Schaul et al. 2016, proportional variant).  A sum tree over the physical rows of a
+// replay buffer with 32 children per node, all levels in one float array (b200rl.h, b200rl_per_tree_floats): level 0
+// holds the leaves, level k + 1 the sums of 32 consecutive nodes of level k, every level padded with zeros to a multiple
+// of 32 floats so that a node's children are one aligned 128-byte line.  The last level is [root, running max, 0...].
+// An interior node is always recomputed from its children by per_node_sum (never updated by adding a difference), so
+// the tree carries no drift and any two ways of reaching the same leaves give the same bits.  Nothing here depends on
+// DQN: the draw and the tree update take a row count, the tree and the replay columns.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int PER_FAN = 32, PER_MAX_LEVELS = 8;
+
+// offsets of levels 0..top of a tree over n leaves; returns top (the root's level, >= 1)
+__host__ __device__ __forceinline__ int per_levels(long long n, long long* off) {
+  off[0] = 0;
+  long long c = n;
+  int k = 0;
+  do {
+    off[k + 1] = off[k] + ((c + PER_FAN - 1) / PER_FAN) * PER_FAN;
+    c = (c + PER_FAN - 1) / PER_FAN;
+    ++k;
+  } while (c > 1);
+  return k;
+}
+
+// the sum of the 32 children at ch[0..32), added in index order: the one rule every interior node is computed by
+__device__ __forceinline__ float per_node_sum(const float* ch) {
+  float s = 0.f;
+#pragma unroll
+  for (int v = 0; v < PER_FAN / 4; ++v) {
+    const float4 x = reinterpret_cast<const float4*>(ch)[v];
+    s += x.x;
+    s += x.y;
+    s += x.z;
+    s += x.w;
+  }
+  return s;
+}
+
+// level `parent` nodes [lo, hi) recomputed from level parent - 1 (tree building; one thread per node)
+__global__ void per_tree_level_kernel(float* tree, long long child_off, long long parent_off, long long lo,
+                                      long long hi) {
+  const long long i = lo + (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < hi) tree[parent_off + i] = per_node_sum(tree + child_off + i * PER_FAN);
+}
+
+// leaves [lo, lo + count) <- the running max (read on the device: it is whatever the last train call left)
+__global__ void per_tree_fill_kernel(float* tree, long long lo, long long count, long long max_at) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < count) tree[lo + i] = tree[max_at];
+}
+
+// the tree, the row count and the replay columns of every learner of a launch
+template <bool LANES>
+struct PerLanes {
+  static constexpr int N = LANES ? B200RL_MAX_LEARNERS : 1;
+  float* tree[N];
+  long long rows[N];
+  const float *obs[N], *act[N], *rew[N], *next_obs[N], *done[N];
+};
+
+// One CTA per learner, one thread per row (looping for B > blockDim): the stratified proportional draw of step st, the
+// importance weights and the gather of the five staged columns.
+//   u_j = (j + U_j) * (M / B), M = the root, U_j = the top 24 bits of Philox4x32-10(counter (j, st, call, 0x9E5),
+//   key seed) times 2^-24; descend from the root: at each node take the first child with a nonzero value whose
+//   inclusive prefix (summed in per_node_sum's order, so the last prefix is the parent itself) exceeds u, else the last
+//   nonzero child, and subtract the exclusive prefix;  w_j = (min_k p[idx_k] / p[idx_j])^beta.
+// seed and call are the two 64-bit words at keys[0..2), beta the .y of betas[st]: they change between calls and are read
+// from device memory, so a captured graph stays valid.
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) per_draw_kernel(const PerLanes<LANES> pl, const float2* betas,
+                                                           const unsigned long long* keys, int st, int B, int O, int A,
+                                                           long long* idx, float* w, float* obs, float* act, float* rew,
+                                                           float* nobs, float* done, size_t lane_stride) {
+  __shared__ float red[32];
+  const int z = LANES ? blockIdx.z : 0;
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    betas = lane_ptr(betas, o), keys = lane_ptr(keys, o), idx = lane_ptr(idx, o), w = lane_ptr(w, o);
+    obs = lane_ptr(obs, o), act = lane_ptr(act, o), rew = lane_ptr(rew, o), nobs = lane_ptr(nobs, o);
+    done = lane_ptr(done, o);
+  }
+  const float* tree = pl.tree[z];
+  long long off[PER_MAX_LEVELS + 1];
+  const int top = per_levels(pl.rows[z], off);
+  const float M = tree[off[top]];
+  const unsigned long long seed = keys[0], call = keys[1];
+  const uint2 key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
+  const float beta = betas[st].y, step = M / (float)B;
+  float pmin = INFINITY;
+  for (int j = threadIdx.x; j < B; j += blockDim.x) {
+    const uint4 r = philox4x32_10(make_uint4((unsigned)j, (unsigned)st, (unsigned)call, 0x9E5u), key);
+    float u = ((float)j + (float)(r.x >> 8) * 5.9604644775390625e-8f) * step;
+    long long node = 0;
+    for (int k = top; k >= 1; --k) {
+      const float* ch = tree + off[k - 1] + node * PER_FAN;
+      float c[PER_FAN];
+#pragma unroll
+      for (int v = 0; v < PER_FAN / 4; ++v) {
+        const float4 x = reinterpret_cast<const float4*>(ch)[v];
+        c[4 * v] = x.x, c[4 * v + 1] = x.y, c[4 * v + 2] = x.z, c[4 * v + 3] = x.w;
+      }
+      int pick = -1, last = 0;
+      float s = 0.f, before = 0.f, before_last = 0.f;
+#pragma unroll
+      for (int i = 0; i < PER_FAN; ++i) {
+        const float prev = s;
+        s += c[i];
+        if (c[i] > 0.f) {
+          last = i, before_last = prev;
+          if (pick < 0 && u < s) pick = i, before = prev;
+        }
+      }
+      if (pick < 0) pick = last, before = before_last;  // rounding put u at or past the last boundary
+      u = fmaxf(u - before, 0.f);
+      node = node * PER_FAN + pick;
+    }
+    const float p = tree[node];
+    idx[j] = node;
+    w[j] = p;
+    pmin = fminf(pmin, p);
+  }
+  // min over the minibatch (exact in any order)
+  for (int o = 16; o > 0; o >>= 1) pmin = fminf(pmin, __shfl_xor_sync(0xffffffffu, pmin, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = pmin;
+  __syncthreads();
+  pmin = red[0];
+  for (int i = 1; i < (int)(blockDim.x >> 5); ++i) pmin = fminf(pmin, red[i]);
+  for (int j = threadIdx.x; j < B; j += blockDim.x) w[j] = powf(pmin / w[j], beta);
+  // the gather (idx written above by this CTA: visible after the __syncthreads)
+  const float* src[5] = {pl.obs[z], pl.act[z], pl.rew[z], pl.next_obs[z], pl.done[z]};
+  float* dst[5] = {obs, act, rew, nobs, done};
+  const int width[5] = {O, A, 1, O, 1};
+#pragma unroll
+  for (int c = 0; c < 5; ++c) {
+    const int wd = width[c];
+    for (int i = threadIdx.x; i < B * wd; i += blockDim.x) {
+      const int r = i / wd;
+      dst[c][i] = src[c][idx[r] * wd + (i - r * wd)];
+    }
+  }
+}
+
+// One CTA per learner: the priority update of one step.  Row j (in row order; a later row on the same leaf wins) sets
+// leaf idx[j] to (absd[j] + eps)^alpha and raises the running max to it; a row with absd = -1 (invalid action) is
+// skipped, and a non-finite |delta| or priority leaves its leaf unchanged and is counted in *bad_out.  Then every
+// ancestor of a drawn leaf is recomputed, level by level.  newp [B] = the new priority of each row (NaN when skipped).
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) per_update_kernel(const PerLanes<LANES> pl, const long long* idx,
+                                                             const float* absd, int B, float alpha, float eps,
+                                                             float* newp, int* bad_out, size_t lane_stride) {
+  __shared__ long long leaf_s[GTHREADS];
+  __shared__ float red[32];
+  __shared__ int bad_rows;
+  const int z = LANES ? blockIdx.z : 0;
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    idx = lane_ptr(idx, o), absd = lane_ptr(absd, o), newp = lane_ptr(newp, o), bad_out = lane_ptr(bad_out, o);
+  }
+  float* tree = pl.tree[z];
+  long long off[PER_MAX_LEVELS + 1];
+  const int top = per_levels(pl.rows[z], off);
+  if (threadIdx.x == 0) bad_rows = 0;
+  float mx = 0.f;
+  int bad = 0;
+  for (int base = 0; base < B; base += blockDim.x) {  // rows in chunks of blockDim, in order
+    const int j = base + threadIdx.x;
+    long long leaf = -1;
+    float p = 0.f;
+    if (j < B) {
+      const float ad = absd[j];
+      p = __int_as_float(0x7fc00000);
+      if (ad != -1.f) {
+        p = powf(ad + eps, alpha);
+        if (isfinite(ad) && isfinite(p)) leaf = idx[j], mx = fmaxf(mx, p);
+        else ++bad;
+      }
+      newp[j] = p;
+    }
+    leaf_s[threadIdx.x] = leaf;
+    __syncthreads();
+    if (leaf >= 0) {
+      bool last = true;
+      const int n = min((int)blockDim.x, B - base);
+      for (int k = threadIdx.x + 1; k < n && last; ++k) last = leaf_s[k] != leaf;
+      if (last) tree[leaf] = p;
+    }
+    __syncthreads();
+  }
+  if (bad) atomicAdd(&bad_rows, bad);
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
+  for (int k = 1; k <= top; ++k) {  // the leaves' writes (and each level's) are visible to the CTA after the barrier
+    __syncthreads();
+    for (int j = threadIdx.x; j < B; j += blockDim.x) {
+      const long long node = idx[j] >> (5 * k);
+      tree[off[k] + node] = per_node_sum(tree + off[k - 1] + node * PER_FAN);
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) mx = fmaxf(mx, red[i]);
+    float& m = tree[off[top] + 1];
+    m = fmaxf(m, mx);
+    *bad_out = bad_rows;
+  }
 }
 
 }  // namespace b200rl
@@ -679,6 +923,16 @@ struct b200rl_offpolicy {
   b200rl_dqn_hparams dqn_hp{}, graph_dqn_hp{};
   float* dqn_dout = nullptr;  // [B, n] gradient w.r.t. the Q output
   int* dqn_bad = nullptr;     // [max_steps] rows of each step whose action was not a valid index
+  // prioritized replay (DQN engines): a prioritized call draws, weighs and gathers inside the step program; adam_tab
+  // row 3's .y then holds each step's beta and the table's last two float2 the call's (seed, call) words
+  bool per_set = false, per_run = false;
+  bool per_last = false;                       // the last call that ran steps was a prioritized one
+  b200rl_per_hparams per_hp{};
+  PerLanes<true> per_lanes{};                  // this call's trees and columns (entry 0 for a solo engine)
+  std::vector<char> graph_per_key;             // per_run, per_hp and per_lanes of the cached graph
+  float *per_w = nullptr, *per_newp = nullptr;  // [max_steps * B] importance weights / new priorities of each row
+  float* per_absd = nullptr;                    // [B] |delta| of the current step
+  int* per_bad = nullptr;                       // [max_steps] rows of each step whose new priority was not finite
   std::vector<void*> allocs;
 };
 
@@ -916,7 +1170,7 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
   rc |= oalloc(h, &h->out_l2, S);
   rc |= oalloc(h, &h->out_lp, S);
   const size_t n_tab = sac || dqn ? 4 : 3;  // SAC: a fourth row for log_alpha's optimizer; DQN: the copy flags
-  rc |= oalloc(h, &h->adam_tab, n_tab * S);
+  rc |= oalloc(h, &h->adam_tab, n_tab * S + (dqn ? 2 : 0));  // DQN: + the prioritized draw's (seed, call)
   rc |= oalloc(h, &h->idx, S * B);
   if (sac) {
     rc |= oalloc(h, &h->sac_act_next, B * (size_t)A);
@@ -931,6 +1185,10 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
   if (dqn) {
     rc |= oalloc(h, &h->dqn_dout, B * (size_t)cfg->q.sizes[cfg->q.n_layers]);
     rc |= oalloc(h, &h->dqn_bad, S);
+    rc |= oalloc(h, &h->per_w, S * B);
+    rc |= oalloc(h, &h->per_newp, S * B);
+    rc |= oalloc(h, &h->per_absd, B);
+    rc |= oalloc(h, &h->per_bad, S);
   }
   rc |= arena_commit(h);
   if (rc == 0) {
@@ -948,7 +1206,7 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
         q += state_pad(h->net[i].P);
       }
   }
-  if (!rc && cudaMallocHost(reinterpret_cast<void**>(&h->h_adam_tab), h->K * n_tab * S * sizeof(float2)) != cudaSuccess)
+  if (!rc && cudaMallocHost(reinterpret_cast<void**>(&h->h_adam_tab), h->K * (n_tab * S + (dqn ? 2 : 0)) * sizeof(float2)) != cudaSuccess)
     rc = 1;
   if (!rc && cudaStreamCreateWithFlags(&h->gs, cudaStreamNonBlocking) != cudaSuccess) rc = 1;
   if (!rc && cudaEventCreateWithFlags(&h->ev, cudaEventDisableTiming) != cudaSuccess) rc = 1;
@@ -1087,6 +1345,18 @@ extern "C" int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hp
   B200RL_REQUIRE(dp->double_q == 0 || dp->double_q == 1, "offpolicy_set_dqn: double_q must be 0 or 1");
   h->dqn_hp = *dp;
   h->dqn_set = true;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_set_per(b200rl_offpolicy* h, const b200rl_per_hparams* pp) {
+  B200RL_REQUIRE(h && pp, "offpolicy_set_per: NULL argument");
+  B200RL_REQUIRE(h->dqn, "offpolicy_set_per: prioritized replay is implemented for DQN engines (algo = 2) only");
+  B200RL_REQUIRE(pp->alpha >= 0.0 && std::isfinite(pp->alpha), "offpolicy_set_per: alpha must be >= 0");
+  B200RL_REQUIRE(pp->eps > 0.0 && std::isfinite(pp->eps), "offpolicy_set_per: eps must be > 0");
+  B200RL_REQUIRE(pp->beta_start >= 0.0 && pp->beta_start <= 1.0, "offpolicy_set_per: beta_start must be in [0, 1]");
+  B200RL_REQUIRE(pp->beta_anneal_steps >= 1, "offpolicy_set_per: beta_anneal_steps must be >= 1");
+  h->per_hp = *pp;
+  h->per_set = true;
   return 0;
 }
 
@@ -1395,11 +1665,20 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
   return 0;
 }
 
+static PerLanes<false> per_solo(const PerLanes<true>& l) {
+  PerLanes<false> s;
+  s.tree[0] = l.tree[0], s.rows[0] = l.rows[0];
+  s.obs[0] = l.obs[0], s.act[0] = l.act[0], s.rew[0] = l.rew[0], s.next_obs[0] = l.next_obs[0], s.done[0] = l.done[0];
+  return s;
+}
+
 // The S DQN steps.  Per step:
 //   s  : Q_targ(s') ---------------+-> loss -> dX chain -> Adam(Q) -> target copy (on the steps the flag table marks)
 //   s2 : Q(s') (Double DQN only) --+
 //   s3 : Q(s) ---------------------+   ........ Q's dW products
 // Q(s') reads the parameters at the start of the step: the step's Adam waits for the loss kernel, which joins it.
+// A prioritized call (h->per_run) opens each step with the draw on s (draw, weights, gather), takes the weighted loss
+// head, and runs the priority update on s4 beside the backward pass; the next step's draw joins it.
 static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s) {
   const int O = h->O;
   const int maxS = h->cfg.max_steps;
@@ -1407,13 +1686,33 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
   NetBuf &q = h->net[1], &qt = h->net[4];
   const int L = q.d.n_layers, n = q.d.sizes[L];
   const int ew = 256;
-  cudaStream_t s2 = h->s2, s3 = h->s3;
+  cudaStream_t s2 = h->s2, s3 = h->s3, s4 = h->s4;
   auto edge = [&](cudaStream_t from, cudaStream_t to) -> int {
     B200RL_CUDA(cudaEventRecord(h->ev_fork, from));
     B200RL_CUDA(cudaStreamWaitEvent(to, h->ev_fork, 0));
     return 0;
   };
+  const bool per = h->per_run;
+  const float2* betas = h->adam_tab + (size_t)3 * maxS;
+  const unsigned long long* keys = reinterpret_cast<const unsigned long long*>(h->adam_tab + (size_t)4 * maxS);
+  const float alpha = (float)h->per_hp.alpha, eps = (float)h->per_hp.eps;
+  const dim3 lanes = lane_grid(dim3(1), h->K);
   for (int st = 0; st < S; ++st) {
+    if (per) {
+      if (st > 0 && edge(s4, s)) return 1;  // the previous step's priorities are in the tree
+      long long* s_idx = h->idx + (size_t)st * B;
+      float* s_w = h->per_w + (size_t)st * B;
+      float* dst[5] = {h->obs + (size_t)st * B * O, h->act + (size_t)st * B, h->rew + (size_t)st * B,
+                       h->nobs + (size_t)st * B * O, h->done + (size_t)st * B};
+      if (h->K == 1)
+        per_draw_kernel<false><<<1, GTHREADS, 0, s>>>(per_solo(h->per_lanes), betas, keys, st, B, O, 1, s_idx, s_w,
+                                                       dst[0], dst[1], dst[2], dst[3], dst[4], 0);
+      else
+        per_draw_kernel<true><<<lanes, GTHREADS, 0, s>>>(h->per_lanes, betas, keys, st, B, O, 1, s_idx, s_w, dst[0],
+                                                        dst[1], dst[2], dst[3], dst[4], h->lane_stride);
+      B200RL_CUDA(cudaGetLastError());
+      count_launch(1);
+    }
     const float* s_obs = h->obs + (size_t)st * B * O;
     const float* s_act = h->act + (size_t)st * B;
     const float* s_rew = h->rew + (size_t)st * B;
@@ -1437,10 +1736,29 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
     if (net_forward(h, qt, tq, B, s)) return 1;
     if (dbl && edge(s2, s)) return 1;
     if (edge(s3, s)) return 1;
-    LAUNCH_LANES(h, dqn_loss_kernel, 1, GTHREADS, s, qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done,
-                 (float)hp->gamma, B, n, h->dqn_dout, h->out_l1 + st, h->out_q1 + (size_t)st * B, h->dqn_bad + st);
-    B200RL_CUDA(cudaGetLastError());
-    count_launch(1);
+    if (per) {
+      LAUNCH_LANES(h, dqn_per_loss_kernel, 1, GTHREADS, s, qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done,
+                   (float)hp->gamma, B, n, h->dqn_dout, h->out_l1 + st, h->out_q1 + (size_t)st * B, h->dqn_bad + st,
+                   h->per_w + (size_t)st * B, h->per_absd);
+      B200RL_CUDA(cudaGetLastError());
+      count_launch(1);
+      if (edge(s, s4)) return 1;
+      const long long* s_idx = h->idx + (size_t)st * B;
+      float* s_newp = h->per_newp + (size_t)st * B;
+      if (h->K == 1)
+        per_update_kernel<false><<<1, GTHREADS, 0, s4>>>(per_solo(h->per_lanes), s_idx, h->per_absd, B, alpha, eps,
+                                                         s_newp, h->per_bad + st, 0);
+      else
+        per_update_kernel<true><<<lanes, GTHREADS, 0, s4>>>(h->per_lanes, s_idx, h->per_absd, B, alpha, eps, s_newp,
+                                                           h->per_bad + st, h->lane_stride);
+      B200RL_CUDA(cudaGetLastError());
+      count_launch(1);
+    } else {
+      LAUNCH_LANES(h, dqn_loss_kernel, 1, GTHREADS, s, qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done,
+                   (float)hp->gamma, B, n, h->dqn_dout, h->out_l1 + st, h->out_q1 + (size_t)st * B, h->dqn_bad + st);
+      B200RL_CUDA(cudaGetLastError());
+      count_launch(1);
+    }
     if (net_backward(h, q, qa, h->dqn_dout, n, B, true, nullptr, s, false, nullptr, 0, 0, s3)) return 1;
     if (adam_net(h, q, h->adam_tab + (size_t)maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, s)) return 1;
     LAUNCH_LANES(h, dqn_target_copy_kernel, (unsigned)((q.P + ew - 1) / ew), ew, s, qt.params, q.params, (int)q.P,
@@ -1448,6 +1766,7 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
     B200RL_CUDA(cudaGetLastError());
     count_launch(1);
   }
+  if (per && edge(s4, s)) return 1;
   return 0;
 }
 
@@ -1473,12 +1792,13 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   const bool td3 = h->cfg.n_q == 2;
   cudaStream_t s = h->gs;
   const size_t SB = (size_t)S * B;
+  h->per_last = h->per_run;  // what get_per_draws may report
 
   // Adam's step-dependent scalars for the steps of this call (torch's host-side double arithmetic), one small upload
   // (a group: one table per learner, from that learner's step counts, uploaded with one strided copy)
   const int maxS = h->cfg.max_steps;
   const int n_pol_expected = h->dqn ? 0 : h->sac ? S : (S + hp->policy_delay - 1) / hp->policy_delay;  // SAC: no delay
-  const size_t tab_n = (h->sac || h->dqn ? 4 : 3) * (size_t)maxS;
+  const size_t tab_n = (h->sac || h->dqn ? 4 : 3) * (size_t)maxS + (h->dqn ? 2 : 0);
   const bool learn_alpha = h->sac && h->sac_hp.learn_alpha;
   for (int z = 0; z < h->K; ++z) {
     float2* tab = h->h_adam_tab + z * tab_n;
@@ -1495,6 +1815,12 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
     if (h->dqn)  // copy after the steps that bring the Q optimizer's count to a multiple of the interval
       for (int k = 0; k < S; ++k)
         tab[(size_t)3 * maxS + k] = make_float2((h->net[1].step[z] + k + 1) % h->dqn_hp.target_update_interval == 0, 0.f);
+    if (h->per_run)  // beta = min(1, beta0 + (1 - beta0) t / anneal), t = the Q optimizer's count before the step
+      for (int k = 0; k < S; ++k) {
+        const double b0 = h->per_hp.beta_start;
+        const double t = (double)(h->net[1].step[z] + k);
+        tab[(size_t)3 * maxS + k].y = (float)std::min(1.0, b0 + (1.0 - b0) * t / (double)h->per_hp.beta_anneal_steps);
+      }
   }
   B200RL_CUDA(cudaMemcpy2DAsync(h->adam_tab, h->lane_stride, h->h_adam_tab, tab_n * sizeof(float2),
                                 tab_n * sizeof(float2), h->K, cudaMemcpyHostToDevice, s));
@@ -1512,9 +1838,17 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
       return 1;
     }
   } else {
+    // a prioritized graph holds the trees' and the columns' addresses, the row counts and alpha / eps in its nodes
+    std::vector<char> per_key;
+    if (h->per_run) {
+      const char* a = reinterpret_cast<const char*>(&h->per_hp);
+      const char* b = reinterpret_cast<const char*>(&h->per_lanes);
+      per_key.assign(a, a + sizeof(h->per_hp));
+      per_key.insert(per_key.end(), b, b + sizeof(h->per_lanes));
+    }
     if (h->graph == nullptr || h->graph_S != S || h->graph_B != B || memcmp(&h->graph_hp, hp, sizeof(*hp)) != 0 ||
         memcmp(&h->graph_sac_hp, &h->sac_hp, sizeof(h->sac_hp)) != 0 ||
-        memcmp(&h->graph_dqn_hp, &h->dqn_hp, sizeof(h->dqn_hp)) != 0) {
+        memcmp(&h->graph_dqn_hp, &h->dqn_hp, sizeof(h->dqn_hp)) != 0 || h->graph_per_key != per_key) {
       if (h->graph) {
         cudaGraphExecDestroy(h->graph);
         h->graph = nullptr;
@@ -1551,6 +1885,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
       h->graph_hp = *hp;
       h->graph_sac_hp = h->sac_hp;
       h->graph_dqn_hp = h->dqn_hp;
+      h->graph_per_key = per_key;
       h->graph_npol = n_pol;
     }
     n_pol = h->graph_npol;
@@ -1574,15 +1909,21 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   if (n_pol > 0)
     B200RL_CUDA(cudaMemcpy2DAsync(policy_losses, (size_t)S * 4, h->out_lp, ls, (size_t)n_pol * 4, K,
                                   cudaMemcpyDeviceToHost, s));
-  std::vector<int> bad(h->dqn ? K * S : 0);
+  std::vector<int> bad(h->dqn ? K * S : 0), per_bad(h->per_run ? K * S : 0);
   if (h->dqn)
     B200RL_CUDA(cudaMemcpy2DAsync(bad.data(), (size_t)S * 4, h->dqn_bad, ls, (size_t)S * 4, K, cudaMemcpyDeviceToHost, s));
+  if (h->per_run)
+    B200RL_CUDA(cudaMemcpy2DAsync(per_bad.data(), (size_t)S * 4, h->per_bad, ls, (size_t)S * 4, K,
+                                  cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaStreamSynchronize(s));
   *n_policy_updates = n_pol;
   for (size_t i = 0; i < bad.size(); ++i)
     B200RL_REQUIRE(bad[i] == 0, "offpolicy_train: DQN learner %d, step %d: %d minibatch rows hold an action that is not "
                    "an integer in [0, %d); those rows were left out of the update", (int)(i / S), (int)(i % S), bad[i],
                    h->net[1].d.sizes[h->net[1].d.n_layers]);
+  for (size_t i = 0; i < per_bad.size(); ++i)
+    B200RL_REQUIRE(per_bad[i] == 0, "offpolicy_train_prioritized: DQN learner %d, step %d: %d minibatch rows gave a "
+                   "non-finite priority; their leaves were left unchanged", (int)(i / S), (int)(i % S), per_bad[i]);
   return 0;
 }
 
@@ -1790,5 +2131,122 @@ extern "C" int b200rl_offpolicy_get_draws(b200rl_offpolicy* h, int32_t S, int32_
   if (noise)
     B200RL_CUDA(cudaMemcpy2DAsync(noise, n_eps * 4, h->eps, h->lane_stride, n_eps * 4, h->K, cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaStreamSynchronize(s));
+  return 0;
+}
+
+/* Prioritized replay (DQN engines): each step draws its minibatch from the learner's sum tree, weighs the rows, and
+ * writes the new priorities back into the tree, all inside the step program (see b200rl.h). */
+extern "C" int b200rl_offpolicy_train_prioritized_group(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp,
+                                                        int32_t S, int32_t B, const b200rl_offpolicy_replay* rb,
+                                                        float* const* trees, const uint64_t* seed, const uint64_t* call,
+                                                        float* q1_values, float* q1_losses, void* stream) {
+  B200RL_REQUIRE(h && hp && trees && seed && call && q1_values && q1_losses,
+                 "offpolicy_train_prioritized: NULL argument");
+  B200RL_REQUIRE(h->dqn, "offpolicy_train_prioritized: prioritized replay is implemented for DQN engines (algo = 2) "
+                 "only");
+  B200RL_REQUIRE(h->per_set, "offpolicy_train_prioritized: call b200rl_offpolicy_set_per first");
+  if (int rc = check_replay(h, rb, "offpolicy_train_prioritized")) return rc;
+  if (dqn_ready(h, "offpolicy_train_prioritized")) return 2;
+  B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
+                 "offpolicy_train_prioritized: S=%d B=%d exceed the capacities", S, B);
+  for (int z = 0; z < h->K; ++z) {
+    B200RL_REQUIRE(trees[z] != nullptr, "offpolicy_train_prioritized: learner %d: NULL tree", z);
+    B200RL_REQUIRE(rb[z].rows < ((int64_t)1 << 31), "offpolicy_train_prioritized: learner %d: more than 2^31 - 1 rows",
+                   z);
+    // every learner's update kernel rewrites its tree's leaves and interior nodes concurrently with the others: two
+    // learners on one tree would race (stale interior sums, a lost running max)
+    for (int y = 0; y < z; ++y)
+      B200RL_REQUIRE(trees[y] != trees[z], "offpolicy_train_prioritized: learners %d and %d share one tree: every "
+                     "learner of a group needs its own prioritized replay buffer", y, z);
+  }
+  if (S == 0) return 0;
+  cudaStream_t s = h->gs;
+  B200RL_CUDA(cudaEventRecord(h->ev, static_cast<cudaStream_t>(stream)));
+  B200RL_CUDA(cudaStreamWaitEvent(s, h->ev, 0));
+  h->per_lanes = PerLanes<true>{};
+  const size_t tab_n = (size_t)4 * h->cfg.max_steps + 2;
+  for (int z = 0; z < h->K; ++z) {
+    PerLanes<true>& l = h->per_lanes;
+    l.tree[z] = trees[z], l.rows[z] = rb[z].rows;
+    l.obs[z] = rb[z].obs, l.act[z] = rb[z].act, l.rew[z] = rb[z].rew, l.next_obs[z] = rb[z].next_obs;
+    l.done[z] = rb[z].done;
+    unsigned long long* keys = reinterpret_cast<unsigned long long*>(h->h_adam_tab + z * tab_n + tab_n - 2);
+    keys[0] = seed[z], keys[1] = call[z];  // uploaded with the table by run_staged
+  }
+  h->per_run = true;
+  int32_t n_pol = 0;
+  const int rc = run_staged(h, hp, S, B, q1_values, nullptr, q1_losses, nullptr, nullptr, &n_pol);
+  h->per_run = false;
+  return rc;
+}
+
+extern "C" int b200rl_offpolicy_train_prioritized(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int32_t S,
+                                                  int32_t B, const float* d_obs, const float* d_act, const float* d_rew,
+                                                  const float* d_next_obs, const float* d_done, int64_t rows,
+                                                  float* tree, uint64_t seed, uint64_t call, float* q1_values,
+                                                  float* q1_losses, void* stream) {
+  B200RL_REQUIRE(h == nullptr || h->K == 1,
+                 "offpolicy_train_prioritized: a learner group takes train_prioritized_group");
+  const b200rl_offpolicy_replay rb = {d_obs, d_act, d_rew, d_next_obs, d_done, rows};
+  return b200rl_offpolicy_train_prioritized_group(h, hp, S, B, &rb, &tree, &seed, &call, q1_values, q1_losses, stream);
+}
+
+extern "C" int b200rl_offpolicy_get_per_draws(b200rl_offpolicy* h, int32_t S, int32_t B, int64_t* idx, float* weights,
+                                              float* priorities, void* stream) {
+  B200RL_REQUIRE(h && h->dqn && idx && weights && priorities && S >= 0 && S <= h->cfg.max_steps && B >= 1 &&
+                     B <= h->cfg.max_minibatch, "offpolicy_get_per_draws: bad arguments");
+  B200RL_REQUIRE(h->per_last, "offpolicy_get_per_draws: the engine's last train call was not a prioritized one");
+  (void)stream;
+  cudaStream_t s = h->gs;
+  const size_t SB = (size_t)S * B, ls = h->lane_stride;
+  B200RL_CUDA(cudaMemcpy2DAsync(idx, SB * 8, h->idx, ls, SB * 8, h->K, cudaMemcpyDeviceToHost, s));
+  B200RL_CUDA(cudaMemcpy2DAsync(weights, SB * 4, h->per_w, ls, SB * 4, h->K, cudaMemcpyDeviceToHost, s));
+  B200RL_CUDA(cudaMemcpy2DAsync(priorities, SB * 4, h->per_newp, ls, SB * 4, h->K, cudaMemcpyDeviceToHost, s));
+  B200RL_CUDA(cudaStreamSynchronize(s));
+  return 0;
+}
+
+extern "C" int64_t b200rl_per_tree_floats(int64_t leaves) {
+  if (leaves < 1 || leaves >= ((int64_t)1 << 31)) return -1;
+  long long off[PER_MAX_LEVELS + 1];
+  const int top = per_levels(leaves, off);
+  return off[top] + PER_FAN;
+}
+
+// parents of the leaves [lo, hi), level by level up to the root
+static int per_tree_ancestors(float* tree, long long leaves, long long lo, long long hi, cudaStream_t s) {
+  long long off[PER_MAX_LEVELS + 1];
+  const int top = per_levels(leaves, off);
+  for (int k = 1; k <= top; ++k) {
+    lo /= PER_FAN;
+    hi = (hi + PER_FAN - 1) / PER_FAN;
+    per_tree_level_kernel<<<(unsigned)((hi - lo + 255) / 256), 256, 0, s>>>(tree, off[k - 1], off[k], lo, hi);
+    B200RL_CUDA(cudaGetLastError());
+    count_launch(1);
+  }
+  return 0;
+}
+
+extern "C" int b200rl_per_tree_build(float* tree, int64_t leaves, void* stream) {
+  B200RL_REQUIRE(tree && b200rl_per_tree_floats(leaves) > 0, "per_tree_build: bad arguments (leaves %lld)",
+                 (long long)leaves);
+  return per_tree_ancestors(tree, leaves, 0, leaves, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b200rl_per_tree_set_range(float* tree, int64_t leaves, int64_t start, int64_t count, void* stream) {
+  B200RL_REQUIRE(tree && b200rl_per_tree_floats(leaves) > 0 && start >= 0 && start < leaves && count >= 0 &&
+                     count <= leaves, "per_tree_set_range: bad arguments (leaves %lld, start %lld, count %lld)",
+                 (long long)leaves, (long long)start, (long long)count);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const long long max_at = b200rl_per_tree_floats(leaves) - PER_FAN + 1;
+  const long long first = std::min<long long>(count, leaves - start);
+  const long long seg[2][2] = {{start, first}, {0, count - first}};  // wrap-aware
+  for (const auto& g : seg) {
+    if (g[1] == 0) continue;
+    per_tree_fill_kernel<<<(unsigned)((g[1] + 255) / 256), 256, 0, s>>>(tree, g[0], g[1], max_at);
+    B200RL_CUDA(cudaGetLastError());
+    count_launch(1);
+    if (per_tree_ancestors(tree, leaves, g[0], g[0] + g[1], s)) return 1;
+  }
   return 0;
 }

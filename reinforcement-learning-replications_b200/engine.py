@@ -491,6 +491,51 @@ class OffPolicyEngine:
         dp.target_update_interval, dp.double_q = int(target_update_interval), int(bool(double_q))
         check(self.lib.b200rl_offpolicy_set_dqn(self.h, C.byref(dp)), "set_dqn")
 
+    # ---- prioritized replay (DQN) ----
+    def set_per(self, alpha: float, eps: float, beta_start: float, beta_anneal_steps: int) -> None:
+        from ._lib import PerHparams
+        pp = PerHparams()
+        pp.alpha, pp.eps, pp.beta_start, pp.beta_anneal_steps = float(alpha), float(eps), float(beta_start), \
+            int(beta_anneal_steps)
+        check(self.lib.b200rl_offpolicy_set_per(self.h, C.byref(pp)), "set_per")
+
+    def train_prioritized(self, hp, columns, rows: int, tree, S: int, B: int, seed: int, call: int):
+        """S prioritized DQN steps on a device replay (``columns``, ``rows``) and its sum tree ``tree`` (a CUDA float32
+        tensor, b200rl_per_tree_floats(rows) long; the steps update it in place), draws keyed by (``seed``, ``call``)."""
+        return self.train_prioritized_group(hp, [(columns, rows)], [tree], S, B, [seed], [call])
+
+    def train_prioritized_group(self, hp, replays, trees, S: int, B: int, seeds, calls):
+        """``train_prioritized`` for every learner: K (columns, rows) pairs, K trees, K seeds and calls."""
+        rb = self._replays(replays)
+        if len(trees) != self.K:
+            raise ValueError(f"expected the trees of {self.K} learners, got {len(trees)}")
+        import torch
+        for z, (t, (_, rows)) in enumerate(zip(trees, replays)):
+            need = int(self.lib.b200rl_per_tree_floats(int(rows)))
+            if not (torch.is_tensor(t) and t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()
+                    and t.numel() == need):
+                raise ValueError(f"learner {z}: the tree must be a contiguous float32 CUDA tensor of "
+                                 f"b200rl_per_tree_floats({int(rows)}) = {need} floats, got "
+                                 f"{getattr(t, 'dtype', type(t))} {tuple(getattr(t, 'shape', ()))} "
+                                 f"on {getattr(t, 'device', '?')}")
+        tp = (C.c_void_p * self.K)(*[t.data_ptr() for t in trees])
+        keys = [np.asarray([int(x) & (2 ** 64 - 1) for x in v], np.uint64) for v in (seeds, calls)]
+        q1v, _, l1, _, _, _ = self._out_buffers(S, B)
+        check(self.lib.b200rl_offpolicy_train_prioritized_group(self.h, C.byref(hp), S, B, rb, tp, *[_ptr(x) for x in keys],
+                                                                _ptr(q1v), _ptr(l1), current_stream_handle()),
+              "offpolicy_train_prioritized")
+        out = dict(q1_values=q1v, q1_losses=l1)
+        return {k: v[0] for k, v in out.items()} if self.K == 1 else out
+
+    def get_per_draws(self, S: int, B: int):
+        """(rows [S,B] int64, importance weights [S,B], new priorities [S,B] (NaN where a row wrote none)) of the last
+        prioritized call; a group: each with a leading [K] axis."""
+        idx = np.empty((self.K, S, B), np.int64)
+        w, p = np.empty((self.K, S, B), np.float32), np.empty((self.K, S, B), np.float32)
+        check(self.lib.b200rl_offpolicy_get_per_draws(self.h, S, B, _ptr(idx), _ptr(w), _ptr(p), current_stream_handle()),
+              "get_per_draws")
+        return (idx[0], w[0], p[0]) if self.K == 1 else (idx, w, p)
+
     def sac_outputs(self, S: int):
         """(mean log pi per step [S], alpha used by each step [S]) of the last train call (a group: [K, S] each)."""
         lp, al = np.zeros((self.K, S), np.float32), np.zeros((self.K, S), np.float32)

@@ -1,3 +1,4 @@
+import ctypes as C
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -145,3 +146,99 @@ class ReplayBuffer:
     rewards = property(lambda self: [float(x) for x in self._view("rewards")])
     next_observations = property(lambda self: self._view("next_observations"))
     dones = property(lambda self: [bool(x) for x in self._view("dones")])
+
+
+class PrioritizedReplayBuffer(ReplayBuffer):
+    """A ``ReplayBuffer`` with one priority per physical row for prioritized experience replay (Schaul et al. 2016,
+    proportional variant), used by ``DQN.train``: each train step draws its minibatch in proportion to the priorities,
+    weighs the rows by (min_k p_k / p_j)^beta and writes (|TD error| + ``eps``)^``alpha`` back for the rows it drew, all on
+    the device (b200rl.h, "Prioritized experience replay").  beta rises linearly from ``beta_start`` to 1 over
+    ``beta_anneal_steps`` Q optimizer steps.
+
+    The priorities live in a sum tree on the device (a torch CUDA tensor owned here).  Rows that are not live have
+    priority 0; rows written by ``add_experience`` (ring overwrites included) get the running max of all priorities so
+    far (1 at the start) when the device mirror is next refreshed.  The columns are allocated at ``buffer_size`` rows on
+    the first append, so rows never move.  There is no host-side draw: ``sample_indices`` and ``sample_minibatch``
+    refuse rather than sample uniformly.  Priorities are not part of checkpoints."""
+
+    def __init__(self, buffer_size: int = int(1e6), alpha: float = 0.6, beta_start: float = 0.4,
+                 beta_anneal_steps: int = 100_000, eps: float = 1e-6) -> None:
+        super().__init__(buffer_size)
+        if not alpha >= 0.0:
+            raise ValueError(f"alpha must be >= 0, got {alpha}")
+        if not 0.0 <= beta_start <= 1.0:
+            raise ValueError(f"beta_start must be in [0, 1], got {beta_start}")
+        if int(beta_anneal_steps) < 1:
+            raise ValueError(f"beta_anneal_steps must be >= 1, got {beta_anneal_steps}")
+        if not eps > 0.0:
+            raise ValueError(f"eps must be > 0, got {eps}")
+        if self.buffer_size >= 2 ** 31:
+            raise ValueError(f"buffer_size must be below 2^31, got {self.buffer_size}")
+        self.alpha, self.beta_start, self.beta_anneal_steps, self.eps = float(alpha), float(beta_start), \
+            int(beta_anneal_steps), float(eps)
+        self._tree = None             # the sum tree (built with the device mirror)
+        self._prio_dirty: List = []   # physical row ranges appended since the tree was last refreshed
+
+    def per_settings(self):
+        """(alpha, eps, beta_start, beta_anneal_steps): what the engine's b200rl_per_hparams take."""
+        return self.alpha, self.eps, self.beta_start, self.beta_anneal_steps
+
+    def beta(self, t: int) -> float:
+        """beta of a train step taken at Q optimizer step count ``t`` (the count before the step)."""
+        return min(1.0, self.beta_start + (1.0 - self.beta_start) * t / self.beta_anneal_steps)
+
+    def _allocate(self, rows: int, samples) -> None:
+        super()._allocate(self.buffer_size, samples)  # full size at once: rows keep their place, and so their priority
+
+    def add_experience(self, experience: Experience) -> None:
+        if hasattr(experience, "transition_columns"):
+            n = len(experience.transition_columns()[0])
+        else:
+            n = len(experience.flattened_rewards)
+        super().add_experience(experience)
+        n = min(n, self.buffer_size)
+        if n == 0 or self._tree is None:  # no tree yet: its first build gives every live row the initial max
+            return
+        start = (self._head + self.current_size - n) % self._capacity
+        if self._prio_dirty:  # consecutive appends continue the previous range
+            s0, c0 = self._prio_dirty[-1]
+            if (s0 + c0) % self._capacity == start:
+                self._prio_dirty[-1] = (s0, min(c0 + n, self._capacity))
+                return
+        self._prio_dirty.append((start, n))
+
+    def device_columns(self):
+        from . import _lib
+        from .engine import current_stream_handle
+        import torch
+        cols, rows = super().device_columns()
+        lib = _lib.load()
+        if self._tree is None:
+            n = int(lib.b200rl_per_tree_floats(rows))
+            self._tree = torch.zeros(n, dtype=torch.float32, device="cuda")
+            self._tree[n - 31] = 1.0  # the running max m (b200rl.h: the last level is [root, m, 0 ...])
+            self._prio_dirty = self._live_ranges()
+        stream = current_stream_handle()
+        for start, count in self._prio_dirty:
+            _lib.check(lib.b200rl_per_tree_set_range(C.c_void_p(self._tree.data_ptr()), rows, start, count, stream),
+                       "per_tree_set_range")
+        self._prio_dirty = []
+        return cols, rows
+
+    def device_tree(self):
+        """The sum tree (CUDA float32 tensor, b200rl.h layout) with every append so far given its priority."""
+        self.device_columns()
+        return self._tree
+
+    def priorities(self) -> np.ndarray:
+        """The leaves: one priority per physical row (``capacity`` rows), as float32 on the host."""
+        return self.device_tree()[:self._capacity].cpu().numpy()
+
+    def max_priority(self) -> float:
+        """The running max m that new rows receive."""
+        t = self.device_tree()
+        return float(t[t.numel() - 31])
+
+    def sample_indices(self, minibatch_size: int) -> np.ndarray:
+        raise NotImplementedError("PrioritizedReplayBuffer draws its minibatches on the device, in proportion to the "
+                                  "priorities, inside DQN.train; it has no uniform host-side draw")

@@ -339,7 +339,7 @@ typedef struct {
   int32_t max_minibatch;   /* capacity: rows per minibatch */
   int32_t max_steps;       /* capacity: train steps per call */
   int32_t algo;            /* 0 = DDPG / TD3 (by n_q), 1 = SAC (see b200rl_offpolicy_set_sac), 2 = DQN (see
-                            * b200rl_offpolicy_set_dqn) */
+                            * b200rl_offpolicy_set_dqn), 3 = C51 (see b200rl_offpolicy_set_c51) */
 } b200rl_offpolicy_config;
 
 typedef struct {
@@ -463,6 +463,34 @@ typedef struct {
 
 /* Required once before the first train call of a DQN engine; part of the cached graph's key. */
 int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hparams* hp);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * C51 on the same engine (config algo = 3, n_q = 1; Bellemare, Dabney & Munos 2017): a DQN engine whose Q network maps
+ * obs -> [n_actions x n_atoms] logits, row-major (action a owns columns a N .. a N + N - 1).  Everything the DQN
+ * section says holds (networks, state blob, action column, hparams, target copies, outputs, invalid actions, graph,
+ * groups; b200rl_offpolicy_set_dqn is required too) except the loss.  With N = n_atoms:
+ *   support  dz = (v_max - v_min) / (N - 1), z_i = float32(v_min + i dz), both evaluated in double
+ *   p(s, a)  = exp(log_softmax) of action a's N logits, x - max - log(sum exp(x - max)) in float32; every sum over
+ *            atoms runs in index order; Q(s, a) = sum_i z_i p_i(s, a)
+ *   a*       = argmax_a Q(s', a) with the expected values of Q (double_q = 1; at the start of the step) or of Q_targ
+ *            (torch's argmax: a NaN wins, ties go to the first index)
+ *   target   Tz_j = clamp(r + gamma (1 - d) z_j, v_min, v_max), b_j = (Tz_j - v_min) / dz,
+ *            m_i = sum_j max(0, 1 - |b_j - i|) p_j(s', a*) from Q_targ (summed over j in index order)
+ *   loss     one Adam step (optimizer 1) on mean_B(-sum_i m_i log p_i(s, a)); the gradient w.r.t. the action's logits is
+ *            (p_i(s, a) sum_k m_k - m_i) / B, every other logit's 0
+ * Outputs: q1_values [S,B] = Q(s, a) before the update, q1_losses [S] = the mean cross-entropy (summed in double).
+ * The head is deterministic (no float atomics): a group's learners stay bit-identical to solo engines.  Prioritized
+ * replay is not implemented for C51: b200rl_offpolicy_set_per and the train_prioritized calls refuse a C51 engine.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t n_atoms;  /* N, 2..256; the Q network's output width must be a multiple of N */
+  int32_t reserved; /* ignored */
+  double v_min, v_max; /* finite, v_min < v_max */
+} b200rl_c51_hparams;
+
+/* Required once before the first train call of a C51 engine and refused on other engines; writes the support into
+ * every learner's arena; part of the cached graph's key. */
+int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hparams* hp);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Learner groups: K independent off-policy learners (same config, same hyper-parameters, their own parameters, Adam

@@ -94,6 +94,10 @@ class DqnHparams(C.Structure):
     _fields_ = [("target_update_interval", C.c_int32), ("double_q", C.c_int32)]
 
 
+class C51Hparams(C.Structure):
+    _fields_ = [("n_atoms", C.c_int32), ("reserved", C.c_int32), ("v_min", C.c_double), ("v_max", C.c_double)]
+
+
 class PerHparams(C.Structure):
     _fields_ = [("alpha", C.c_double), ("eps", C.c_double), ("beta_start", C.c_double),
                 ("beta_anneal_steps", C.c_int64)]
@@ -181,6 +185,7 @@ SIGNATURES = {
                                              C.POINTER(C.c_float), C.POINTER(C.c_int64)]),
     "b200rl_offpolicy_sac_outputs": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "b200rl_offpolicy_set_dqn": (C.c_int, [C.c_void_p, C.POINTER(DqnHparams)]),
+    "b200rl_offpolicy_set_c51": (C.c_int, [C.c_void_p, C.POINTER(C51Hparams)]),
     "b200rl_offpolicy_create_group": (C.c_int, [C.POINTER(OffPolicyConfig), C.c_int32, C.POINTER(C.c_void_p)]),
     "b200rl_offpolicy_train_gather_group": (C.c_int, [C.c_void_p, C.POINTER(OffPolicyHparams), C.c_int32, C.c_int32,
                                                       C.POINTER(OffPolicyReplay)] + [C.c_void_p] * 7 +

@@ -1,3 +1,4 @@
+from .c51 import C51
 from .dqn import DQN
 from .group import LearnerGroup
 from .ppo import PPO
@@ -6,4 +7,4 @@ from .td3 import DDPG, TD3
 from .trpo import TRPO
 from .vpg import VPG
 
-__all__ = ["VPG", "TRPO", "PPO", "DDPG", "TD3", "SAC", "DQN", "LearnerGroup"]
+__all__ = ["VPG", "TRPO", "PPO", "DDPG", "TD3", "SAC", "DQN", "C51", "LearnerGroup"]

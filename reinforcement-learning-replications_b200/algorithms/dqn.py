@@ -40,9 +40,10 @@ class DQN(_OffPolicyBase):
             raise ValueError("DQN needs a discrete action space (one with .n)")
         sizes, _, _, lins = describe_mlp(q_function.network)
         obs_shape = getattr(getattr(env, "observation_space", None), "shape", None)
-        if sizes[-1] != int(n) or (obs_shape and sizes[0] != int(np.prod(obs_shape))):
-            want = f"{int(np.prod(obs_shape))} -> {int(n)}" if obs_shape else f"obs -> {int(n)}"
-            raise ValueError(f"the Q network must map {want} (one value per action), got {sizes[0]} -> {sizes[-1]}")
+        width, what = self._output_width(q_function, int(n))
+        if sizes[-1] != width or (obs_shape and sizes[0] != int(np.prod(obs_shape))):
+            want = f"{int(np.prod(obs_shape))} -> {width}" if obs_shape else f"obs -> {width}"
+            raise ValueError(f"the Q network must map {want} ({what}), got {sizes[0]} -> {sizes[-1]}")
         adam_hparams(q_function.optimizer, lins, "q-function optimizer")
         if int(target_update_interval) < 1:
             raise ValueError(f"target_update_interval must be >= 1, got {target_update_interval}")
@@ -59,6 +60,11 @@ class DQN(_OffPolicyBase):
         self.target_q_function = copy.deepcopy(q_function)
         for p in self.target_q_function.network.parameters():
             p.requires_grad = False
+
+    @staticmethod
+    def _output_width(q_function, n: int):
+        """(width of the Q network's output for n actions, what it holds)."""
+        return n, "one value per action"
 
     def epsilon(self) -> float:
         """epsilon at the current total step count: linear from epsilon_start to epsilon_end, then constant."""

@@ -1,4 +1,4 @@
-"""LearnerGroup: several independent TD3 / DDPG / SAC / DQN learners (typically one per seed) trained side by side by ONE
+"""LearnerGroup: several independent TD3 / DDPG / SAC / DQN / C51 learners (typically one per seed) trained side by side by ONE
 off-policy engine, every operation of a train step one launch for all of them (b200rl_offpolicy_create_group).
 
 The contract: each member ends up bit for bit where it would be had it run alone.  Members keep everything of their
@@ -34,7 +34,7 @@ def _signature(agent) -> list:
     """[(attribute, value)] that every member of a group shares (one engine trains them all), in the order in which a
     refusal reports the first difference."""
     trainable, _ = agent._nets()
-    dqn = agent.algo == OffPolicyEngine.DQN
+    dqn = agent.algo in (OffPolicyEngine.DQN, OffPolicyEngine.C51)
     names = ["q_function"] if dqn else ["policy"] + (["q_function_1", "q_function_2"] if agent.n_q == 2 else ["q_function"])
     sig = [("class", type(agent).__name__)]
     for name, m in zip(names, trainable):
@@ -46,6 +46,9 @@ def _signature(agent) -> list:
         for attr in ("gamma", "target_update_interval", "double_q", "epsilon_start", "epsilon_end", "epsilon_decay_steps",
                      "use_device_replay", "use_device_rng"):
             sig.append((attr, getattr(agent, attr, None)))
+        if agent.algo == OffPolicyEngine.C51:
+            for attr in ("n_atoms", "v_min", "v_max"):
+                sig.append((attr, getattr(agent.q_function, attr)))
         rb = getattr(agent, "replay_buffer", None)
         sig.append(("prioritized replay", isinstance(rb, PrioritizedReplayBuffer)))
         for attr in ("alpha", "eps", "beta_start", "beta_anneal_steps"):
@@ -102,7 +105,7 @@ class LearnerGroup:
     def add(self, agent) -> None:
         """Add ``agent``; the current state of the global random generators becomes its private stream."""
         if not isinstance(agent, _OffPolicyBase):
-            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or DQN) learners, got {type(agent).__name__}")
+            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or DQN / C51) learners, got {type(agent).__name__}")
         if any(m is agent for m in self.members):
             raise ValueError("LearnerGroup: this agent is already a member")
         if len(self.members) >= MAX_LEARNERS:
@@ -140,11 +143,12 @@ class LearnerGroup:
 
     def _ensure_engine(self, S: int, B: int) -> OffPolicyEngine:
         m = self.members[0]
-        if m.algo == OffPolicyEngine.DQN:  # no policy network
+        discrete = m.algo in (OffPolicyEngine.DQN, OffPolicyEngine.C51)
+        if discrete:  # no policy network
             psz, pact, pout = None, "relu", "tanh"
         else:
             psz, pact, pout, _ = describe_mlp(m.policy.network)
-        qsz, qact, qout, _ = describe_mlp(m._nets()[0][0 if m.algo == OffPolicyEngine.DQN else 1].network)
+        qsz, qact, qout, _ = describe_mlp(m._nets()[0][0 if discrete else 1].network)
         e = self._engine
         if (e is None or e.K != len(self.members) or e.max_minibatch < B or e.max_steps < S or e.policy_sizes != psz
                 or e.q_sizes != qsz or e.policy_acts != (pact, pout) or e.q_acts != (qact, qout)):
@@ -185,8 +189,11 @@ class LearnerGroup:
         if sac:
             e.set_sac(members[0]._sac_hparams())
             e.set_alpha_group([m._alpha_state() for m in members])
-        if members[0].algo == OffPolicyEngine.DQN:
+        if members[0].algo in (OffPolicyEngine.DQN, OffPolicyEngine.C51):
             e.set_dqn(members[0].target_update_interval, members[0].double_q)
+        if members[0].algo == OffPolicyEngine.C51:
+            q = members[0].q_function
+            e.set_c51(q.n_atoms, q.v_min, q.v_max)
         hp = members[0]._hparams(noisy, delay)
         if mode == "per":
             e.set_per(*members[0].replay_buffer.per_settings())

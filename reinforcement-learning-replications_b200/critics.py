@@ -2,6 +2,8 @@
 
 The update engine reads ``.network`` (a 3-layer ``MLP``) and ``.optimizer`` (Adam hyper-parameters and state) from
 these objects; ``forward`` is only used on the host (rollouts, evaluation, the CPU oracle)."""
+import math
+
 import torch
 from torch import Tensor, nn
 from torch.optim import Optimizer
@@ -34,3 +36,37 @@ class DiscreteQFunction(_Critic):
 
     def forward(self, observation: Tensor) -> Tensor:
         return self.network(observation)
+
+
+class CategoricalQFunction(_Critic):
+    """A return distribution per action over a fixed support (C51's critic): the network maps an observation to
+    ``n_actions x n_atoms`` logits, action a owning columns a*n_atoms .. (a+1)*n_atoms - 1.  ``forward`` returns the
+    expected values [..., n_actions], so greedy and epsilon-greedy policies and the evaluator use it as they use a
+    ``DiscreteQFunction``."""
+
+    MAX_ATOMS = 256  # the engine's limit (b200rl.h)
+
+    def __init__(self, network: nn.Module, optimizer: Optimizer, n_atoms: int = 51, v_min: float = -10.0,
+                 v_max: float = 10.0) -> None:
+        super().__init__(network, optimizer)
+        if not 2 <= int(n_atoms) <= self.MAX_ATOMS:
+            raise ValueError(f"n_atoms must be 2..{self.MAX_ATOMS}, got {n_atoms}")
+        v_min, v_max = float(v_min), float(v_max)
+        if not (math.isfinite(v_min) and math.isfinite(v_max) and v_min < v_max):
+            raise ValueError(f"the support needs finite v_min < v_max, got [{v_min}, {v_max}]")
+        self.n_atoms, self.v_min, self.v_max = int(n_atoms), v_min, v_max
+        # z_i = float32(v_min + i dz), evaluated in double as the engine does (torch.linspace rounds differently)
+        dz = (v_max - v_min) / (self.n_atoms - 1)
+        self.support = torch.tensor([v_min + i * dz for i in range(self.n_atoms)], dtype=torch.float64).float()
+
+    def log_distribution(self, observation: Tensor) -> Tensor:
+        """log p(s, a) [..., n_actions, n_atoms]."""
+        logits = self.network(observation)
+        return torch.log_softmax(logits.unflatten(-1, (-1, self.n_atoms)), dim=-1)
+
+    def distribution(self, observation: Tensor) -> Tensor:
+        """p(s, a) [..., n_actions, n_atoms]."""
+        return self.log_distribution(observation).exp()
+
+    def forward(self, observation: Tensor) -> Tensor:
+        return (self.distribution(observation) * self.support).sum(-1)

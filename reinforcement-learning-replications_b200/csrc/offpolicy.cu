@@ -20,6 +20,7 @@
 // enqueue_sac_steps, run as a captured graph or as plain launches like the TD3 / DDPG steps.
 // DQN (config algo = 2) is a third: a per-row Huber loss head on discrete actions (dqn_loss_kernel), a target copy
 // gated by a per-learner step table (dqn_target_copy_kernel) and enqueue_dqn_steps; networks 1 and 4 only.
+// C51 (config algo = 3) is DQN's step program with a categorical head over return distributions (c51_loss_kernel).
 // Prioritized replay for DQN (train_prioritized): a 32-way sum tree per replay buffer, drawn from, weighed and gathered
 // by per_draw_kernel and updated by per_update_kernel inside the same step program.
 #include <algorithm>
@@ -646,6 +647,176 @@ __global__ void dqn_target_copy_kernel(float* target, const float* param, int n,
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// C51 (algo = 3; Bellemare, Dabney & Munos 2017): DQN's step program with a categorical head.  The Q network maps obs
+// -> [n * N] logits, action a owning columns a*N .. a*N + N - 1; p(s, a) = softmax over them, Q(s, a) = sum_i z_i p_i.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int C51_MAX_ATOMS = 256, C51_WARPS = 8;
+constexpr int C51_SMEM_FLOATS = 48 * 1024 / 4;  // the dynamic shared memory of one CTA without an opt-in
+
+// warps per CTA of the head at n actions x N atoms: each warp holds 3N + n floats, the CTA the support (N floats)
+__host__ __device__ __forceinline__ int c51_warps(int n, int N) {
+  const int w = (C51_SMEM_FLOATS - N) / (3 * N + n);
+  return w < C51_WARPS ? w : C51_WARPS;
+}
+
+// sum_j z_j p_j of one action's N logits x, p = exp(x - max - log(sum exp(x - max))); every sum in index order
+__device__ __forceinline__ float c51_expected(const float* x, const float* z, int N) {
+  float m = x[0];
+  for (int j = 1; j < N; ++j) m = fmaxf(m, x[j]);
+  float s = 0.f;
+  for (int j = 0; j < N; ++j) s += expf(x[j] - m);
+  const float ls = logf(s);
+  float e = 0.f;
+  for (int j = 0; j < N; ++j) e += z[j] * expf((x[j] - m) - ls);
+  return e;
+}
+
+// The warp's log_softmax of one action's N logits x (lane l: atoms l, l + 32, ...): logp[k] for atom lane + 32k, and
+// p = exp(logp) in sp[0..N).  The same arithmetic as c51_expected: the max is exact in any order, the sum runs in index
+// order (every lane adds up sp itself).
+__device__ __forceinline__ void c51_warp_log_softmax(const float* x, int N, float* sp, float (&logp)[C51_MAX_ATOMS / 32]) {
+  const int lane = threadIdx.x & 31;
+  float m = -INFINITY;
+#pragma unroll
+  for (int k = 0; k < C51_MAX_ATOMS / 32; ++k)
+    if (lane + 32 * k < N) m = fmaxf(m, x[lane + 32 * k]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+#pragma unroll
+  for (int k = 0; k < C51_MAX_ATOMS / 32; ++k)
+    if (lane + 32 * k < N) {
+      logp[k] = x[lane + 32 * k] - m;
+      sp[lane + 32 * k] = expf(logp[k]);
+    }
+  __syncwarp();
+  float s = 0.f;
+  for (int j = 0; j < N; ++j) s += sp[j];
+  const float ls = logf(s);
+  __syncwarp();
+#pragma unroll
+  for (int k = 0; k < C51_MAX_ATOMS / 32; ++k)
+    if (lane + 32 * k < N) {
+      logp[k] -= ls;
+      sp[lane + 32 * k] = expf(logp[k]);
+    }
+  __syncwarp();
+}
+
+// One warp per row i with action a = act[i] (a grid of ceil(B / warps) CTAs per learner):
+//   a* = argmax_j Q(s')_j over the expected values of qn (Double DQN: qn != NULL) or of qt_next (argmax_row's rule),
+//   Tz_j = clamp(r + gamma (1 - d) z_j, v_min, v_max), b_j = (Tz_j - v_min) / dz,
+//   m_i = sum_j max(0, 1 - |b_j - i|) p_j(s', a*) from Q_targ(s'), L_i = -sum_i m_i log p_i(s, a),
+//   dOut[i, a*N + k] = (p_k(s, a) sum m - m_k) * (1 / B) and 0 elsewhere, q_copy[i] = Q(s, a) (the logged Q-value).
+// A row whose action is not an integer in [0, n) is never used as an index: its dOut row is 0, its loss 0, q_copy NaN,
+// and it is counted.  The last CTA of a learner to finish (sync[0] counts them) writes *loss_out = mean L, summed in
+// double as block_mean sums, and *bad_out = the invalid rows (sync[1]), and leaves both counters at 0 for the next
+// launch.  No atomics touch a float: the head is deterministic.
+template <bool LANES>
+__global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
+    const float* q, const float* qt_next, const float* qn, const float* act, const float* rew, const float* done,
+    const float* support, float gamma, float v_min, float v_max, float dz, int B, int n, int N, float* dout,
+    float* row_loss, float* q_copy, int* sync, float* loss_out, int* bad_out, size_t lane_stride) {
+  extern __shared__ float c51_smem[];
+  __shared__ double red[32];
+  __shared__ bool last;
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q = lane_ptr(q, o), qt_next = lane_ptr(qt_next, o), qn = lane_ptr(qn, o), act = lane_ptr(act, o);
+    rew = lane_ptr(rew, o), done = lane_ptr(done, o), support = lane_ptr(support, o), dout = lane_ptr(dout, o);
+    row_loss = lane_ptr(row_loss, o), q_copy = lane_ptr(q_copy, o), sync = lane_ptr(sync, o);
+    loss_out = lane_ptr(loss_out, o), bad_out = lane_ptr(bad_out, o);
+  }
+  const int nN = n * N, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float* z = c51_smem;
+  for (int j = threadIdx.x; j < N; j += blockDim.x) z[j] = support[j];
+  __syncthreads();
+  float* sp = c51_smem + N + warp * (3 * N + n);  // p(s', a*), then p(s, a)
+  float* sb = sp + N;                             // b_j, then m_i
+  float* sx = sb + N;                             // log p(s, a)
+  float* sq = sx + N;                             // expected values of Q(s') (argmax net)
+  const int i = blockIdx.x * (blockDim.x >> 5) + warp;
+  if (i < B) {
+    const float af = act[i];
+    const bool valid = af >= 0.f && af < (float)n && af == floorf(af);  // false for NaN
+    const int a = valid ? (int)af : -1;
+    float* drow = dout + (size_t)i * nN;
+    for (int c = lane; c < nN; c += 32)
+      if (c / N != a) drow[c] = 0.f;
+    if (!valid) {
+      if (lane == 0) {
+        q_copy[i] = __int_as_float(0x7fc00000);
+        row_loss[i] = 0.f;
+        atomicAdd(sync + 1, 1);
+      }
+    } else {
+      // a*: the expected values of the argmax net, one lane per action, then argmax_row over them
+      const float* an = (qn != nullptr ? qn : qt_next) + (size_t)i * nN;
+      for (int j = lane; j < n; j += 32) sq[j] = c51_expected(an + (size_t)j * N, z, N);
+      __syncwarp();
+      const int a_star = argmax_row(sq, n);
+      float logp[C51_MAX_ATOMS / 32];
+      c51_warp_log_softmax(qt_next + (size_t)i * nN + (size_t)a_star * N, N, sp, logp);
+      const float g1d = gamma * (1.f - done[i]), r = rew[i];
+#pragma unroll
+      for (int k = 0; k < C51_MAX_ATOMS / 32; ++k)
+        if (lane + 32 * k < N) {
+          float tz = r + g1d * z[lane + 32 * k];
+          tz = tz < v_min ? v_min : (tz > v_max ? v_max : tz);  // NaN passes through, as torch's clamp lets it
+          sb[lane + 32 * k] = (tz - v_min) / dz;
+        }
+      __syncwarp();
+      float m[C51_MAX_ATOMS / 32];
+#pragma unroll
+      for (int k = 0; k < C51_MAX_ATOMS / 32; ++k)
+        if (lane + 32 * k < N) {
+          const float at = (float)(lane + 32 * k);
+          float acc = 0.f;
+          for (int j = 0; j < N; ++j) {
+            float w = 1.f - fabsf(sb[j] - at);
+            w = w < 0.f ? 0.f : w;
+            acc += w * sp[j];
+          }
+          m[k] = acc;
+        }
+      __syncwarp();  // every lane is done with sp and sb
+      c51_warp_log_softmax(q + (size_t)i * nN + (size_t)a * N, N, sp, logp);
+#pragma unroll
+      for (int k = 0; k < C51_MAX_ATOMS / 32; ++k)
+        if (lane + 32 * k < N) sb[lane + 32 * k] = m[k], sx[lane + 32 * k] = logp[k];
+      __syncwarp();
+      float qv = 0.f, ce = 0.f, msum = 0.f;
+      for (int j = 0; j < N; ++j) {
+        qv += z[j] * sp[j];
+        ce += sb[j] * sx[j];
+        msum += sb[j];
+      }
+      const float inv = 1.0f / (float)B;  // dqn_loss_rows' scaling
+#pragma unroll
+      for (int k = 0; k < C51_MAX_ATOMS / 32; ++k)
+        if (lane + 32 * k < N) drow[(size_t)a * N + lane + 32 * k] = (sp[lane + 32 * k] * msum - m[k]) * inv;
+      if (lane == 0) {
+        q_copy[i] = qv;
+        row_loss[i] = -ce;
+      }
+    }
+  }
+  // the last CTA of this learner reads every row's loss
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(sync, 1) == (int)gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double acc = 0.0;
+  for (int r = threadIdx.x; r < B; r += blockDim.x) acc += (double)__ldcg(row_loss + r);
+  block_mean(acc, B, loss_out, red);
+  if (threadIdx.x == 0) {
+    *bad_out = atomicExch(sync + 1, 0);
+    sync[0] = 0;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // Prioritized experience replay (Schaul et al. 2016, proportional variant).  A sum tree over the physical rows of a
 // replay buffer with 32 children per node, all levels in one float array (b200rl.h, b200rl_per_tree_floats): level 0
 // holds the leaves, level k + 1 the sums of 32 consecutive nodes of level k, every level padded with zeros to a multiple
@@ -923,6 +1094,12 @@ struct b200rl_offpolicy {
   b200rl_dqn_hparams dqn_hp{}, graph_dqn_hp{};
   float* dqn_dout = nullptr;  // [B, n] gradient w.r.t. the Q output
   int* dqn_bad = nullptr;     // [max_steps] rows of each step whose action was not a valid index
+  // C51 (cfg.algo == 3): a DQN engine (h->dqn is set) whose loss head is c51_loss_kernel
+  bool c51 = false, c51_set = false;
+  b200rl_c51_hparams c51_hp{}, graph_c51_hp{};
+  float* c51_support = nullptr;   // [C51_MAX_ATOMS] z_0 .. z_{N-1}
+  float* c51_row_loss = nullptr;  // [B] each row's cross-entropy of the current step
+  int* c51_sync = nullptr;        // {CTAs done, invalid rows} of the current step; 0 between launches
   // prioritized replay (DQN engines): a prioritized call draws, weighs and gathers inside the step program; adam_tab
   // row 3's .y then holds each step's beta and the table's last two float2 the call's (seed, call) words
   bool per_set = false, per_run = false;
@@ -1083,9 +1260,9 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
   B200RL_REQUIRE(n_learners >= 1 && n_learners <= B200RL_MAX_LEARNERS,
                  "offpolicy_create_group: n_learners must be 1..%d, got %d", B200RL_MAX_LEARNERS, n_learners);
   B200RL_REQUIRE(cfg->n_q == 1 || cfg->n_q == 2, "offpolicy_create: n_q must be 1 (DDPG) or 2 (TD3)");
-  B200RL_REQUIRE(cfg->algo >= 0 && cfg->algo <= 2,
-                 "offpolicy_create: algo must be 0 (DDPG / TD3), 1 (SAC) or 2 (DQN), got %d", cfg->algo);
-  const bool sac = cfg->algo == 1, dqn = cfg->algo == 2;
+  B200RL_REQUIRE(cfg->algo >= 0 && cfg->algo <= 3,
+                 "offpolicy_create: algo must be 0 (DDPG / TD3), 1 (SAC), 2 (DQN) or 3 (C51), got %d", cfg->algo);
+  const bool sac = cfg->algo == 1, c51 = cfg->algo == 3, dqn = cfg->algo == 2 || c51;  // C51 is a DQN engine
   B200RL_REQUIRE(!sac || cfg->n_q == 2, "offpolicy_create: SAC needs n_q = 2 (twin soft critics), got %d", cfg->n_q);
   B200RL_REQUIRE(!dqn || cfg->n_q == 1, "offpolicy_create: DQN needs n_q = 1 (one Q network), got %d", cfg->n_q);
   B200RL_REQUIRE(cfg->max_minibatch >= 1 && cfg->max_minibatch <= 65536 && cfg->max_steps >= 1,
@@ -1112,6 +1289,7 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
   h->A = A;
   h->sac = sac;
   h->dqn = dqn;
+  h->c51 = c51;
   int rc = 0;
   int maxw = O + A;
   for (int i = 0; i < 6; ++i) {
@@ -1189,6 +1367,11 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
     rc |= oalloc(h, &h->per_newp, S * B);
     rc |= oalloc(h, &h->per_absd, B);
     rc |= oalloc(h, &h->per_bad, S);
+  }
+  if (c51) {
+    rc |= oalloc(h, &h->c51_support, C51_MAX_ATOMS);
+    rc |= oalloc(h, &h->c51_row_loss, B);
+    rc |= oalloc(h, &h->c51_sync, 2);
   }
   rc |= arena_commit(h);
   if (rc == 0) {
@@ -1348,8 +1531,36 @@ extern "C" int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hp
   return 0;
 }
 
+extern "C" int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hparams* cp) {
+  B200RL_REQUIRE(h && cp, "offpolicy_set_c51: NULL argument");
+  B200RL_REQUIRE(h->c51, "offpolicy_set_c51: the engine was not created with algo = 3 (C51)");
+  const int N = cp->n_atoms, width = h->net[1].d.sizes[h->net[1].d.n_layers];
+  B200RL_REQUIRE(N >= 2 && N <= C51_MAX_ATOMS, "offpolicy_set_c51: n_atoms must be 2..%d, got %d", C51_MAX_ATOMS, N);
+  B200RL_REQUIRE(std::isfinite(cp->v_min) && std::isfinite(cp->v_max) && cp->v_min < cp->v_max,
+                 "offpolicy_set_c51: the support needs finite v_min < v_max, got [%g, %g]", cp->v_min, cp->v_max);
+  B200RL_REQUIRE(width % N == 0, "offpolicy_set_c51: the Q network's output width %d is not n_actions x n_atoms for "
+                 "n_atoms = %d", width, N);
+  B200RL_REQUIRE(c51_warps(width / N, N) >= 1, "offpolicy_set_c51: %d actions x %d atoms is too wide for the head's "
+                 "shared memory", width / N, N);
+  b200rl_c51_hparams hp = *cp;
+  hp.reserved = 0;  // part of the graph cache key
+  if (h->c51_set && memcmp(&hp, &h->c51_hp, sizeof(hp)) == 0) return 0;  // the support is already in place
+  // z_i = float32(v_min + i dz), dz = (v_max - v_min) / (N - 1), in double (not linspace's rounding)
+  const double dz = (cp->v_max - cp->v_min) / (N - 1);
+  std::vector<float> z((size_t)h->K * C51_MAX_ATOMS, 0.f);  // one row per learner
+  for (int k = 0; k < h->K; ++k)
+    for (int i = 0; i < N; ++i) z[(size_t)k * C51_MAX_ATOMS + i] = (float)(cp->v_min + i * dz);
+  B200RL_CUDA(cudaMemcpy2DAsync(h->c51_support, h->lane_stride, z.data(), C51_MAX_ATOMS * sizeof(float),
+                                C51_MAX_ATOMS * sizeof(float), h->K, cudaMemcpyHostToDevice, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  h->c51_hp = hp;
+  h->c51_set = true;
+  return 0;
+}
+
 extern "C" int b200rl_offpolicy_set_per(b200rl_offpolicy* h, const b200rl_per_hparams* pp) {
   B200RL_REQUIRE(h && pp, "offpolicy_set_per: NULL argument");
+  B200RL_REQUIRE(!h->c51, "offpolicy_set_per: prioritized replay is not implemented for C51 engines");
   B200RL_REQUIRE(h->dqn, "offpolicy_set_per: prioritized replay is implemented for DQN engines (algo = 2) only");
   B200RL_REQUIRE(pp->alpha >= 0.0 && std::isfinite(pp->alpha), "offpolicy_set_per: alpha must be >= 0");
   B200RL_REQUIRE(pp->eps > 0.0 && std::isfinite(pp->eps), "offpolicy_set_per: eps must be > 0");
@@ -1677,6 +1888,7 @@ static PerLanes<false> per_solo(const PerLanes<true>& l) {
 //   s2 : Q(s') (Double DQN only) --+
 //   s3 : Q(s) ---------------------+   ........ Q's dW products
 // Q(s') reads the parameters at the start of the step: the step's Adam waits for the loss kernel, which joins it.
+// A C51 engine (h->c51) takes c51_loss_kernel as its loss head; nothing else in the step differs.
 // A prioritized call (h->per_run) opens each step with the draw on s (draw, weights, gather), takes the weighted loss
 // head, and runs the priority update on s4 beside the backward pass; the next step's draw joins it.
 static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s) {
@@ -1753,6 +1965,24 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
                                                            h->per_bad + st, h->lane_stride);
       B200RL_CUDA(cudaGetLastError());
       count_launch(1);
+    } else if (h->c51) {
+      const int N = h->c51_hp.n_atoms, W = c51_warps(n / N, N);
+      const dim3 grid((unsigned)((B + W - 1) / W), 1, (unsigned)h->K);
+      const size_t smem = sizeof(float) * (size_t)(N + W * (3 * N + n / N));
+      const float vmin = (float)h->c51_hp.v_min, vmax = (float)h->c51_hp.v_max;
+      const float dz = (float)((h->c51_hp.v_max - h->c51_hp.v_min) / (N - 1));
+      if (h->K == 1)
+        c51_loss_kernel<false><<<grid, W * 32, smem, s>>>(
+            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, h->c51_support, (float)hp->gamma, vmin, vmax,
+            dz, B, n / N, N, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync, h->out_l1 + st,
+            h->dqn_bad + st, 0);
+      else
+        c51_loss_kernel<true><<<grid, W * 32, smem, s>>>(
+            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, h->c51_support, (float)hp->gamma, vmin, vmax,
+            dz, B, n / N, N, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync, h->out_l1 + st,
+            h->dqn_bad + st, h->lane_stride);
+      B200RL_CUDA(cudaGetLastError());
+      count_launch(1);
     } else {
       LAUNCH_LANES(h, dqn_loss_kernel, 1, GTHREADS, s, qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done,
                    (float)hp->gamma, B, n, h->dqn_dout, h->out_l1 + st, h->out_q1 + (size_t)st * B, h->dqn_bad + st);
@@ -1774,6 +2004,7 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
 static int dqn_ready(const b200rl_offpolicy* h, const char* what) {
   if (!h->dqn) return 0;
   B200RL_REQUIRE(h->dqn_set, "%s: a DQN engine needs b200rl_offpolicy_set_dqn before it trains", what);
+  B200RL_REQUIRE(!h->c51 || h->c51_set, "%s: a C51 engine needs b200rl_offpolicy_set_c51 before it trains", what);
   return 0;
 }
 
@@ -1848,7 +2079,8 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
     }
     if (h->graph == nullptr || h->graph_S != S || h->graph_B != B || memcmp(&h->graph_hp, hp, sizeof(*hp)) != 0 ||
         memcmp(&h->graph_sac_hp, &h->sac_hp, sizeof(h->sac_hp)) != 0 ||
-        memcmp(&h->graph_dqn_hp, &h->dqn_hp, sizeof(h->dqn_hp)) != 0 || h->graph_per_key != per_key) {
+        memcmp(&h->graph_dqn_hp, &h->dqn_hp, sizeof(h->dqn_hp)) != 0 ||
+        memcmp(&h->graph_c51_hp, &h->c51_hp, sizeof(h->c51_hp)) != 0 || h->graph_per_key != per_key) {
       if (h->graph) {
         cudaGraphExecDestroy(h->graph);
         h->graph = nullptr;
@@ -1885,6 +2117,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
       h->graph_hp = *hp;
       h->graph_sac_hp = h->sac_hp;
       h->graph_dqn_hp = h->dqn_hp;
+      h->graph_c51_hp = h->c51_hp;
       h->graph_per_key = per_key;
       h->graph_npol = n_pol;
     }
@@ -1917,10 +2150,11 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
                                   cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaStreamSynchronize(s));
   *n_policy_updates = n_pol;
+  const int n_actions = h->net[1].d.sizes[h->net[1].d.n_layers] / (h->c51 ? h->c51_hp.n_atoms : 1);
   for (size_t i = 0; i < bad.size(); ++i)
-    B200RL_REQUIRE(bad[i] == 0, "offpolicy_train: DQN learner %d, step %d: %d minibatch rows hold an action that is not "
-                   "an integer in [0, %d); those rows were left out of the update", (int)(i / S), (int)(i % S), bad[i],
-                   h->net[1].d.sizes[h->net[1].d.n_layers]);
+    B200RL_REQUIRE(bad[i] == 0, "offpolicy_train: %s learner %d, step %d: %d minibatch rows hold an action that is not "
+                   "an integer in [0, %d); those rows were left out of the update", h->c51 ? "C51" : "DQN",
+                   (int)(i / S), (int)(i % S), bad[i], n_actions);
   for (size_t i = 0; i < per_bad.size(); ++i)
     B200RL_REQUIRE(per_bad[i] == 0, "offpolicy_train_prioritized: DQN learner %d, step %d: %d minibatch rows gave a "
                    "non-finite priority; their leaves were left unchanged", (int)(i / S), (int)(i % S), per_bad[i]);
@@ -2142,6 +2376,7 @@ extern "C" int b200rl_offpolicy_train_prioritized_group(b200rl_offpolicy* h, con
                                                         float* q1_values, float* q1_losses, void* stream) {
   B200RL_REQUIRE(h && hp && trees && seed && call && q1_values && q1_losses,
                  "offpolicy_train_prioritized: NULL argument");
+  B200RL_REQUIRE(!h->c51, "offpolicy_train_prioritized: prioritized replay is not implemented for C51 engines");
   B200RL_REQUIRE(h->dqn, "offpolicy_train_prioritized: prioritized replay is implemented for DQN engines (algo = 2) "
                  "only");
   B200RL_REQUIRE(h->per_set, "offpolicy_train_prioritized: call b200rl_offpolicy_set_per first");

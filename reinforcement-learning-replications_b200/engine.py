@@ -319,18 +319,19 @@ class OnPolicyEngine:
 
 
 class OffPolicyEngine:
-    """Device-resident state of one DDPG / TD3 (``algo`` 0), SAC (``algo`` 1) or DQN (``algo`` 2) learner (C ABI:
-    b200rl_offpolicy_*).  SAC: ``n_q`` = 2, the policy maps obs -> [mean | log_std] (2A outputs), there is no target
-    policy (network 3), and ``set_sac`` must be called before the first train call.  DQN: ``policy_sizes`` = None,
-    ``n_q`` = 1, the Q network maps obs -> [n actions], only networks 1 (Q) and 4 (target Q) exist, actions are indices
-    (act [S,B]), and ``set_dqn`` must be called before the first train call.
+    """Device-resident state of one DDPG / TD3 (``algo`` 0), SAC (``algo`` 1), DQN (``algo`` 2) or C51 (``algo`` 3)
+    learner (C ABI: b200rl_offpolicy_*).  SAC: ``n_q`` = 2, the policy maps obs -> [mean | log_std] (2A outputs), there
+    is no target policy (network 3), and ``set_sac`` must be called before the first train call.  DQN: ``policy_sizes``
+    = None, ``n_q`` = 1, the Q network maps obs -> [n actions], only networks 1 (Q) and 4 (target Q) exist, actions are
+    indices (act [S,B]), and ``set_dqn`` must be called before the first train call.  C51 is a DQN engine whose Q
+    network maps obs -> [n actions x n atoms] logits; it needs ``set_c51`` as well as ``set_dqn``.
 
     ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
     launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
     is [K][per-learner blob] with [K][3] step counts, and the per-network accessors are refused."""
 
     NETS = {"policy": 0, "q1": 1, "q2": 2, "target_policy": 3, "target_q1": 4, "target_q2": 5}
-    TD3, SAC, DQN = 0, 1, 2
+    TD3, SAC, DQN, C51 = 0, 1, 2, 3
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
                  q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1):
@@ -344,6 +345,7 @@ class OffPolicyEngine:
         cfg.n_q, cfg.max_minibatch, cfg.max_steps = int(n_q), int(max_minibatch), int(max_steps)
         cfg.algo = int(algo)
         self.algo = int(algo)
+        self.discrete = self.algo in (self.DQN, self.C51)  # DQN's networks, inputs and outputs
         self.n_q, self.max_minibatch, self.max_steps = int(n_q), int(max_minibatch), int(max_steps)
         self.policy_sizes, self.q_sizes = None if policy_sizes is None else list(policy_sizes), list(q_sizes)
         self.policy_acts, self.q_acts = tuple(policy_acts), tuple(q_acts)
@@ -399,7 +401,7 @@ class OffPolicyEngine:
         """[(kind, net index, offset, count)] of one learner's state blob: ("params", 0..5) then ("m" / "v", 0..2);
         every segment starts on a multiple of 64 floats (b200rl.h).  A group's blob is K of these back to back."""
         pad = lambda n: (n + 63) & ~63
-        if self.algo == self.DQN:
+        if self.discrete:
             present, optimized = [1, 4], [1]
         else:
             present = [0, 1] + ([2] if self.n_q == 2 else []) + ([] if self.algo == self.SAC else [3]) + [4] + \
@@ -491,6 +493,14 @@ class OffPolicyEngine:
         dp.target_update_interval, dp.double_q = int(target_update_interval), int(bool(double_q))
         check(self.lib.b200rl_offpolicy_set_dqn(self.h, C.byref(dp)), "set_dqn")
 
+    # ---- C51 ----
+    def set_c51(self, n_atoms: int, v_min: float, v_max: float) -> None:
+        """The categorical head's support: ``n_atoms`` atoms from ``v_min`` to ``v_max`` (b200rl.h)."""
+        from ._lib import C51Hparams
+        cp = C51Hparams()
+        cp.n_atoms, cp.v_min, cp.v_max = int(n_atoms), float(v_min), float(v_max)
+        check(self.lib.b200rl_offpolicy_set_c51(self.h, C.byref(cp)), "set_c51")
+
     # ---- prioritized replay (DQN) ----
     def set_per(self, alpha: float, eps: float, beta_start: float, beta_anneal_steps: int) -> None:
         from ._lib import PerHparams
@@ -549,7 +559,7 @@ class OffPolicyEngine:
 
     def _outputs(self, S, q1v, q2v, l1, l2, lp, npol):
         """The logged quantities; a solo engine drops the leading [K] axis."""
-        if self.algo == self.DQN:
+        if self.discrete:
             out = dict(q1_values=q1v, q1_losses=l1)
         else:
             out = dict(q1_values=q1v, q2_values=q2v, q1_losses=l1, q2_losses=l2, policy_losses=lp[:, :npol.value])
@@ -572,7 +582,7 @@ class OffPolicyEngine:
         """obs/next_obs [S,B,O], act [S,B,A], rew/done [S,B], noise [S,B,A] or None (SAC: [S,2,B,A], required) -> dict
         of logged quantities (SAC adds log_prob_means and alphas).  A group: every array with a leading [K] axis.
         DQN: act [S,B] action indices, noise None; the dict holds q1_values and q1_losses."""
-        if self.algo == self.DQN:
+        if self.discrete:
             act = np.asarray(act, np.float32)[..., None]
         obs, act, next_obs = (self._lead(x, np.float32, 4) for x in (obs, act, next_obs))
         rew, done = self._lead(rew, np.float32, 3), self._lead(done, np.float32, 3)
@@ -607,7 +617,7 @@ class OffPolicyEngine:
         """(physical rows [S,B] int64, noise [S,B,A] (SAC: [S,2,B,A]) float32 or None) of the last train_gather /
         train_gather_rng call; a group: both with a leading [K] axis."""
         idx = np.empty((self.K, S, B), np.int64)
-        with_noise = with_noise and self.algo != self.DQN  # DQN draws indices only
+        with_noise = with_noise and not self.discrete  # DQN and C51 draw indices only
         noise = None
         if with_noise and self.algo == self.SAC:
             noise = np.empty((self.K, S, 2, B, self.policy_sizes[-1] // 2), np.float32)

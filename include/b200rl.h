@@ -589,6 +589,34 @@ int b200rl_offpolicy_train_prioritized_group(b200rl_offpolicy* h, const b200rl_o
  * call that ran steps was not a prioritized one (it overwrote the drawn rows). */
 int b200rl_offpolicy_get_per_draws(b200rl_offpolicy* h, int32_t S, int32_t B, int64_t* idx, float* weights,
                                    float* priorities, void* stream);
+/* ------------------------------------------------------------------------------------------------------------
+ * n-step returns for DQN and C51 (Rainbow's multi-step targets).  Each learner's replay buffer keeps, beside its five
+ * columns, a float32 0/1 episode-end column over the same physical rows: row i is 1 when it was the last row of an
+ * episode (a cut-off at the end of a sampling call counts) in the append that wrote it.  Every append ends on a marked
+ * row, so the newest live row is always marked and a window never reads past the ring's head or into a row a ring
+ * overwrite replaced.  For a drawn start row p0, with gamma = float32(hp.gamma), in float32 with every product and sum
+ * rounded on its own (no contraction):
+ *   p = p0;  R = rew[p];  g = gamma
+ *   for k = 1 .. n-1:  if done[p] != 0 or ends[p] != 0: break
+ *                      p = (p + 1) % rows  (the window may cross the wrap);  R = R + g rew[p];  g = g gamma
+ *   the staged row: obs[p0], act[p0], rew := R, next_obs := next_obs[p], done := done[p], discount := g
+ * The loss heads use discount where the one-step target uses gamma: DQN y = R + discount (1 - d) v (td_target's order),
+ * C51 Tz_j = clamp(R + discount (1 - d) z_j, v_min, v_max); a prioritized step's priority is that of the n-step delta.
+ * Double DQN takes its argmax at next_obs[p].  A window never reaches across an episode end: such a row bootstraps
+ * from its own next_obs with a shorter horizon.  n = 1 is exactly the one-step update, on the one-step kernels.
+ * On the gather paths one kernel walks the windows and stages all columns (in place of the five column gathers); on
+ * the prioritized path the draw kernel does.  The host-staged b200rl_offpolicy_train refuses n > 1.
+ * ------------------------------------------------------------------------------------------------------------ */
+/* n_step 1..32 for the engine's next train calls (1 clears it); episode_ends[K] = each learner's device episode-end
+ * column over the `rows` of the replay passed to the next call (required for n_step > 1; buffers that grow reallocate,
+ * so set it before every call).  Refused on TD3, DDPG and SAC engines.  n_step is part of the cached graph's key, and so
+ * are the columns on the prioritized path (its draw walks them inside the graph). */
+int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, const float* const* episode_ends);
+/* Of the last n-step call (host [K, S, B] each): each row's last window row, its return R and its discount g -- what a
+ * test replays through the oracle.  Refused when the engine's last train call that ran steps was not an n-step one. */
+int b200rl_offpolicy_get_nstep_draws(b200rl_offpolicy* h, int32_t S, int32_t B, int64_t* last_rows, float* returns,
+                                     float* discounts, void* stream);
+
 /* Floats of a tree over `leaves` rows (1 <= leaves < 2^31; -1 otherwise). */
 int64_t b200rl_per_tree_floats(int64_t leaves);
 /* Every interior node recomputed from the leaves (stream-ordered). */

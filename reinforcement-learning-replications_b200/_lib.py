@@ -200,6 +200,8 @@ SIGNATURES = {
     "b200rl_offpolicy_train_prioritized_group": (C.c_int, [C.c_void_p, C.POINTER(OffPolicyHparams), C.c_int32,
                                                            C.c_int32, C.POINTER(OffPolicyReplay)] + [C.c_void_p] * 6),
     "b200rl_offpolicy_get_per_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32] + [C.c_void_p] * 4),
+    "b200rl_offpolicy_set_nstep": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
+    "b200rl_offpolicy_get_nstep_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32] + [C.c_void_p] * 4),
     "b200rl_per_tree_floats": (C.c_int64, [C.c_int64]),
     "b200rl_per_tree_build": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p]),
     "b200rl_per_tree_set_range": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p]),

@@ -25,6 +25,16 @@ class DQN(_OffPolicyBase):
     ``device_rng_seed``, whatever ``use_device_rng`` says): minibatches drawn in proportion to the priorities, the loss
     weighted by the importance weights, and the rows' priorities updated from their TD errors (b200rl.h).
 
+    ``n_step`` (1..32) > 1 trains on n-step returns (b200rl.h, "n-step returns"): from a drawn row the window takes up to
+    n consecutive transitions of its episode, R = r_0 + gamma r_1 + ... + gamma^(k-1) r_(k-1) with the k rows it took,
+    and the target bootstraps from the last row's next observation with discount gamma^k: y = R + gamma^k (1 - d) v,
+    d and v (Double DQN's argmax too) taken at that row.  A window stops at a done row and at the last row of an episode
+    in the append that wrote it -- a segment ``BatchSampler`` cut off at the end of a ``sample()`` call included, also
+    with ``is_continuous=True``: such a row bootstraps from its own next observation with a shorter horizon.  Windows
+    are assembled on the device from the replay ring (with prioritized replay too, where the priority is the n-step
+    TD error's), so n_step > 1 needs ``use_device_replay = True`` and a replay buffer with ``device_episode_ends``.
+    ``n_step = 1`` is exactly the one-step update.  n_step is a constructor argument, not part of checkpoints.
+
     Acting: ``exploration_policy`` before ``num_start_steps``, then epsilon-greedy with epsilon falling linearly from
     ``epsilon_start`` to ``epsilon_end`` over the first ``epsilon_decay_steps`` environment steps; evaluation is greedy."""
     n_q = 1
@@ -34,7 +44,7 @@ class DQN(_OffPolicyBase):
 
     def __init__(self, q_function, exploration_policy, env, sampler, replay_buffer, evaluator, gamma: float = 0.99,
                  target_update_interval: int = 1000, double_q: bool = False, epsilon_start: float = 1.0,
-                 epsilon_end: float = 0.05, epsilon_decay_steps: int = 10000) -> None:
+                 epsilon_end: float = 0.05, epsilon_decay_steps: int = 10000, n_step: int = 1) -> None:
         n = getattr(env.action_space, "n", None)
         if n is None:
             raise ValueError("DQN needs a discrete action space (one with .n)")
@@ -47,6 +57,8 @@ class DQN(_OffPolicyBase):
         adam_hparams(q_function.optimizer, lins, "q-function optimizer")
         if int(target_update_interval) < 1:
             raise ValueError(f"target_update_interval must be >= 1, got {target_update_interval}")
+        if isinstance(n_step, bool) or not isinstance(n_step, (int, np.integer)) or not 1 <= n_step <= 32:
+            raise ValueError(f"n_step must be an integer from 1 to 32, got {n_step!r}")
         self.q_function, self.exploration_policy = q_function, exploration_policy
         self.env, self.sampler, self.replay_buffer, self.evaluator = env, sampler, replay_buffer, evaluator
         self.gamma = gamma
@@ -54,6 +66,7 @@ class DQN(_OffPolicyBase):
         self.epsilon_start, self.epsilon_end = float(epsilon_start), float(epsilon_end)
         self.epsilon_decay_steps = int(epsilon_decay_steps)
         self.n_actions = int(n)
+        self.n_step = int(n_step)
         self.epsilon_greedy_policy = EpsilonGreedyPolicy(q_function, env.action_space, epsilon_start)
         self.policy = self.evaluation_policy = GreedyPolicy(q_function)  # acting greedily (evaluation)
         self.evaluation_env = _make_eval_env(env)
@@ -107,6 +120,13 @@ class DQN(_OffPolicyBase):
         e.set_dqn(self.target_update_interval, self.double_q)
 
     def _stage_inputs(self, replay_buffer, S: int, B: int, noisy: bool):
+        if self.n_step > 1:  # the windows are assembled on the device from the replay ring
+            if not getattr(self, "use_device_replay", True):
+                raise ValueError(f"n_step = {self.n_step} needs use_device_replay = True: n-step windows are assembled on "
+                                 "the device from the replay columns")
+            if not hasattr(replay_buffer, "device_episode_ends"):
+                raise ValueError(f"n_step = {self.n_step} needs a replay buffer with device_episode_ends (a ReplayBuffer "
+                                 f"or PrioritizedReplayBuffer), got {type(replay_buffer).__name__}")
         if isinstance(replay_buffer, PrioritizedReplayBuffer):
             # always the prioritized device path, keyed like the uniform device draws (device_rng_seed, call count)
             if not getattr(self, "use_device_replay", True):
@@ -125,8 +145,9 @@ class DQN(_OffPolicyBase):
             inputs = (obs, act.reshape(S, B), rew, nobs, done, None)
         return mode, inputs
 
-    @staticmethod
-    def _call_engine(e, hp, replay_buffer, S: int, B: int, mode, inputs):
+    def _call_engine(self, e, hp, replay_buffer, S: int, B: int, mode, inputs):
+        if mode is not None:
+            e.set_nstep(self.n_step, [replay_buffer.device_episode_ends()] if self.n_step > 1 else None)
         if mode != "per":
             return _OffPolicyBase._call_engine(e, hp, replay_buffer, S, B, mode, inputs)
         e.set_per(*replay_buffer.per_settings())

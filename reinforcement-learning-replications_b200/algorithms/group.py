@@ -44,7 +44,7 @@ def _signature(agent) -> list:
     if dqn:
         sig.append(("action count", agent.n_actions))
         for attr in ("gamma", "target_update_interval", "double_q", "epsilon_start", "epsilon_end", "epsilon_decay_steps",
-                     "use_device_replay", "use_device_rng"):
+                     "use_device_replay", "use_device_rng", "n_step"):
             sig.append((attr, getattr(agent, attr, None)))
         if agent.algo == OffPolicyEngine.C51:
             for attr in ("n_atoms", "v_min", "v_max"):
@@ -195,6 +195,9 @@ class LearnerGroup:
             q = members[0].q_function
             e.set_c51(q.n_atoms, q.v_min, q.v_max)
         hp = members[0]._hparams(noisy, delay)
+        if members[0].algo in (OffPolicyEngine.DQN, OffPolicyEngine.C51):
+            n = members[0].n_step
+            e.set_nstep(n, [m.replay_buffer.device_episode_ends() for m in members] if n > 1 else None)
         if mode == "per":
             e.set_per(*members[0].replay_buffer.per_settings())
             trees = [m.replay_buffer.device_tree() for m in members]

@@ -23,6 +23,8 @@
 // C51 (config algo = 3) is DQN's step program with a categorical head over return distributions (c51_loss_kernel).
 // Prioritized replay for DQN (train_prioritized): a 32-way sum tree per replay buffer, drawn from, weighed and gathered
 // by per_draw_kernel and updated by per_update_kernel inside the same step program.
+// n-step returns for DQN / C51 (set_nstep): nstep_gather_kernel (or per_draw_nstep_kernel) walks each drawn row's window
+// and stages its return and discount; the *_nstep_loss_kernel heads read the per-row discount in place of gamma.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -284,6 +286,69 @@ __global__ void gather_rows_kernel(const LaneSrc<LANES> src, const long long* id
   if (i >= n_out * width) return;
   const long long r = i / width;
   out[i] = table[idx[r] * width + (i - r * width)];
+}
+
+// ---- n-step returns (DQN / C51; b200rl_offpolicy_set_nstep) ----
+constexpr int NSTEP_MAX = 32;
+
+// One window from start row p (b200rl.h, "n-step returns"): R = rew[p], g = gamma; for k = 1 .. n - 1 stop at a row that
+// is done or ends an episode, else step to the physical successor and take R += g rew, g *= gamma.  Every product and
+// sum is rounded on its own (no contraction), so a float32 host walk gives the same bits.  Returns the last row.
+__device__ __forceinline__ long long nstep_walk(const float* rew, const float* done, const float* ends, long long rows,
+                                                long long p, int n, float gamma, float& R, float& g) {
+  R = rew[p];
+  g = gamma;
+  for (int k = 1; k < n; ++k) {
+    if (done[p] != 0.f || ends[p] != 0.f) break;
+    p = p + 1 == rows ? 0 : p + 1;  // the window may cross the wrap
+    R = __fadd_rn(R, __fmul_rn(g, rew[p]));
+    g = __fmul_rn(g, gamma);
+  }
+  return p;
+}
+
+// out[r, :] = table[rows[r], :] for the CTA's nr rows, consecutive threads on consecutive floats
+__device__ __forceinline__ void copy_rows(const float* table, const long long* rows, int width, int nr, float* out) {
+  for (int i = threadIdx.x; i < nr * width; i += blockDim.x) {
+    const int r = i / width;
+    out[i] = table[rows[r] * width + (i - r * width)];
+  }
+}
+
+// the replay columns, episode-end column and row count of every learner of a launch
+template <bool LANES>
+struct NStepSrc {
+  static constexpr int N = LANES ? B200RL_MAX_LEARNERS : 1;
+  const float *obs[N], *act[N], *rew[N], *next_obs[N], *done[N], *ends[N];
+  long long rows[N];
+};
+
+// The n-step gather of train_gather[_rng] (replaces the five gather_rows_kernel launches): thread i walks the window of
+// start row idx[i] and stages rew := R, done := done[last], disc := g and last; then the CTA copies obs and act from the
+// start rows and next_obs from the last rows.
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) nstep_gather_kernel(const NStepSrc<LANES> src, const long long* idx,
+                                                               long long n_out, int O, int A, int n, float gamma,
+                                                               float* obs, float* act, float* rew, float* nobs,
+                                                               float* done, float* disc, long long* last,
+                                                               size_t lane_stride) {
+  const int z = LANES ? blockIdx.z : 0;
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    idx = lane_ptr(idx, o), obs = lane_ptr(obs, o), act = lane_ptr(act, o), rew = lane_ptr(rew, o);
+    nobs = lane_ptr(nobs, o), done = lane_ptr(done, o), disc = lane_ptr(disc, o), last = lane_ptr(last, o);
+  }
+  const long long r0 = (long long)blockIdx.x * blockDim.x, i = r0 + threadIdx.x;
+  if (i < n_out) {
+    float R, g;
+    const long long p = nstep_walk(src.rew[z], src.done[z], src.ends[z], src.rows[z], idx[i], n, gamma, R, g);
+    rew[i] = R, disc[i] = g, done[i] = src.done[z][p], last[i] = p;
+  }
+  __syncthreads();  // the CTA's last rows are visible to all its threads
+  const int nr = (int)min((long long)blockDim.x, n_out - r0);
+  copy_rows(src.obs[z], idx + r0, O, nr, obs + r0 * O);
+  copy_rows(src.act[z], idx + r0, A, nr, act + r0 * A);
+  copy_rows(src.next_obs[z], last + r0, O, nr, nobs + r0 * O);
 }
 
 // y = r + gamma * (1 - d) * min(q1t, q2t)   (td3.py:337-339; ddpg.py:280: single target Q)
@@ -558,11 +623,12 @@ __device__ __forceinline__ int argmax_row(const float* q, int n) {
 // WEIGHTED (prioritized replay): row i's loss and gradient are scaled by w[i] -- loss = (1/B) sum_i w_i huber(delta_i),
 // dOut[i, a] = w_i clamp(delta_i, -1, 1) / B -- and absd[i] = |delta_i| (-1 for a row with an invalid action).  With
 // every w_i = 1 both are bit for bit those of the unweighted head: the products by 1 are exact.
-template <bool LANES, bool WEIGHTED>
+// NSTEP (n-step returns): row i's discount is disc[i] (gamma^k of its window) in place of gamma.
+template <bool LANES, bool WEIGHTED, bool NSTEP = false>
 __device__ __forceinline__ void dqn_loss_rows(const float* q, const float* qt_next, const float* qn, const float* act,
                                               const float* rew, const float* done, float gamma, int B, int n,
                                               float* dout, float* loss_out, float* q_copy, int* bad_out, const float* w,
-                                              float* absd, size_t lane_stride) {
+                                              float* absd, size_t lane_stride, const float* disc = nullptr) {
   __shared__ double red[32];
   __shared__ int bad_rows;
   if (LANES) {
@@ -571,6 +637,7 @@ __device__ __forceinline__ void dqn_loss_rows(const float* q, const float* qt_ne
     rew = lane_ptr(rew, o), done = lane_ptr(done, o), dout = lane_ptr(dout, o), loss_out = lane_ptr(loss_out, o);
     q_copy = lane_ptr(q_copy, o), bad_out = lane_ptr(bad_out, o);
     if (WEIGHTED) w = lane_ptr(w, o), absd = lane_ptr(absd, o);
+    if (NSTEP) disc = lane_ptr(disc, o);
   }
   if (threadIdx.x == 0) bad_rows = 0;
   __syncthreads();
@@ -586,7 +653,7 @@ __device__ __forceinline__ void dqn_loss_rows(const float* q, const float* qt_ne
       const float* tn = qt_next + (size_t)i * n;
       const float v = qn != nullptr ? tn[argmax_row(qn + (size_t)i * n, n)] : tn[argmax_row(tn, n)];
       const float qi = q[(size_t)i * n + a];
-      const float d = qi - td_target(rew[i], done[i], v, nullptr, i, gamma);
+      const float d = qi - td_target(rew[i], done[i], v, nullptr, i, NSTEP ? disc[i] : gamma);
       const float ad = fabsf(d);
       const double hub = ad < 1.f ? 0.5 * (double)d * (double)d : (double)ad - 0.5;
       const float c = d > 1.f ? 1.f : (d < -1.f ? -1.f : d);  // NaN passes through, as torch's clamp lets it
@@ -630,6 +697,17 @@ __global__ void __launch_bounds__(GTHREADS) dqn_per_loss_kernel(const float* q, 
                                                                size_t lane_stride) {
   dqn_loss_rows<LANES, true>(q, qt_next, qn, act, rew, done, gamma, B, n, dout, loss_out, q_copy, bad_out, w, absd,
                              lane_stride);
+}
+
+// the n-step heads: row i's discount disc[i] in place of gamma; WEIGHTED as dqn_per_loss_kernel (w, absd NULL otherwise)
+template <bool LANES, bool WEIGHTED>
+__global__ void __launch_bounds__(GTHREADS) dqn_nstep_loss_kernel(const float* q, const float* qt_next, const float* qn,
+                                                                 const float* act, const float* rew, const float* done,
+                                                                 const float* disc, int B, int n, float* dout,
+                                                                 float* loss_out, float* q_copy, int* bad_out,
+                                                                 const float* w, float* absd, size_t lane_stride) {
+  dqn_loss_rows<LANES, WEIGHTED, true>(q, qt_next, qn, act, rew, done, 0.f, B, n, dout, loss_out, q_copy, bad_out, w,
+                                       absd, lane_stride, disc);
 }
 
 // target <- param on the steps the copy table marks (flags[idx].x != 0): the graph launches the copy every step and
@@ -711,11 +789,12 @@ __device__ __forceinline__ void c51_warp_log_softmax(const float* x, int N, floa
 // and it is counted.  The last CTA of a learner to finish (sync[0] counts them) writes *loss_out = mean L, summed in
 // double as block_mean sums, and *bad_out = the invalid rows (sync[1]), and leaves both counters at 0 for the next
 // launch.  No atomics touch a float: the head is deterministic.
-template <bool LANES>
-__global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
+// NSTEP (n-step returns): row i's discount is disc[i] (gamma^k of its window) in place of gamma.
+template <bool LANES, bool NSTEP>
+__device__ __forceinline__ void c51_loss_rows(
     const float* q, const float* qt_next, const float* qn, const float* act, const float* rew, const float* done,
     const float* support, float gamma, float v_min, float v_max, float dz, int B, int n, int N, float* dout,
-    float* row_loss, float* q_copy, int* sync, float* loss_out, int* bad_out, size_t lane_stride) {
+    float* row_loss, float* q_copy, int* sync, float* loss_out, int* bad_out, size_t lane_stride, const float* disc) {
   extern __shared__ float c51_smem[];
   __shared__ double red[32];
   __shared__ bool last;
@@ -725,6 +804,7 @@ __global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
     rew = lane_ptr(rew, o), done = lane_ptr(done, o), support = lane_ptr(support, o), dout = lane_ptr(dout, o);
     row_loss = lane_ptr(row_loss, o), q_copy = lane_ptr(q_copy, o), sync = lane_ptr(sync, o);
     loss_out = lane_ptr(loss_out, o), bad_out = lane_ptr(bad_out, o);
+    if (NSTEP) disc = lane_ptr(disc, o);
   }
   const int nN = n * N, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   float* z = c51_smem;
@@ -756,7 +836,7 @@ __global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
       const int a_star = argmax_row(sq, n);
       float logp[C51_MAX_ATOMS / 32];
       c51_warp_log_softmax(qt_next + (size_t)i * nN + (size_t)a_star * N, N, sp, logp);
-      const float g1d = gamma * (1.f - done[i]), r = rew[i];
+      const float g1d = (NSTEP ? disc[i] : gamma) * (1.f - done[i]), r = rew[i];
 #pragma unroll
       for (int k = 0; k < C51_MAX_ATOMS / 32; ++k)
         if (lane + 32 * k < N) {
@@ -814,6 +894,25 @@ __global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
     *bad_out = atomicExch(sync + 1, 0);
     sync[0] = 0;
   }
+}
+
+template <bool LANES>
+__global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
+    const float* q, const float* qt_next, const float* qn, const float* act, const float* rew, const float* done,
+    const float* support, float gamma, float v_min, float v_max, float dz, int B, int n, int N, float* dout,
+    float* row_loss, float* q_copy, int* sync, float* loss_out, int* bad_out, size_t lane_stride) {
+  c51_loss_rows<LANES, false>(q, qt_next, qn, act, rew, done, support, gamma, v_min, v_max, dz, B, n, N, dout, row_loss,
+                              q_copy, sync, loss_out, bad_out, lane_stride, nullptr);
+}
+
+// the n-step head: row i's discount disc[i] in place of gamma
+template <bool LANES>
+__global__ void __launch_bounds__(C51_WARPS * 32) c51_nstep_loss_kernel(
+    const float* q, const float* qt_next, const float* qn, const float* act, const float* rew, const float* done,
+    const float* disc, const float* support, float v_min, float v_max, float dz, int B, int n, int N, float* dout,
+    float* row_loss, float* q_copy, int* sync, float* loss_out, int* bad_out, size_t lane_stride) {
+  c51_loss_rows<LANES, true>(q, qt_next, qn, act, rew, done, support, 0.f, v_min, v_max, dz, B, n, N, dout, row_loss,
+                             q_copy, sync, loss_out, bad_out, lane_stride, disc);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -883,23 +982,12 @@ struct PerLanes {
 //   inclusive prefix (summed in per_node_sum's order, so the last prefix is the parent itself) exceeds u, else the last
 //   nonzero child, and subtract the exclusive prefix;  w_j = (min_k p[idx_k] / p[idx_j])^beta.
 // seed and call are the two 64-bit words at keys[0..2), beta the .y of betas[st]: they change between calls and are read
-// from device memory, so a captured graph stays valid.
-template <bool LANES>
-__global__ void __launch_bounds__(GTHREADS) per_draw_kernel(const PerLanes<LANES> pl, const float2* betas,
-                                                           const unsigned long long* keys, int st, int B, int O, int A,
-                                                           long long* idx, float* w, float* obs, float* act, float* rew,
-                                                           float* nobs, float* done, size_t lane_stride) {
+// from device memory, so a captured graph stays valid.  Ends with a __syncthreads after idx and w are written.
+__device__ __forceinline__ void per_draw_rows(const float* tree, long long rows, const float2* betas,
+                                              const unsigned long long* keys, int st, int B, long long* idx, float* w) {
   __shared__ float red[32];
-  const int z = LANES ? blockIdx.z : 0;
-  if (LANES) {
-    const size_t o = blockIdx.z * lane_stride;
-    betas = lane_ptr(betas, o), keys = lane_ptr(keys, o), idx = lane_ptr(idx, o), w = lane_ptr(w, o);
-    obs = lane_ptr(obs, o), act = lane_ptr(act, o), rew = lane_ptr(rew, o), nobs = lane_ptr(nobs, o);
-    done = lane_ptr(done, o);
-  }
-  const float* tree = pl.tree[z];
   long long off[PER_MAX_LEVELS + 1];
-  const int top = per_levels(pl.rows[z], off);
+  const int top = per_levels(rows, off);
   const float M = tree[off[top]];
   const unsigned long long seed = keys[0], call = keys[1];
   const uint2 key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
@@ -944,6 +1032,21 @@ __global__ void __launch_bounds__(GTHREADS) per_draw_kernel(const PerLanes<LANES
   pmin = red[0];
   for (int i = 1; i < (int)(blockDim.x >> 5); ++i) pmin = fminf(pmin, red[i]);
   for (int j = threadIdx.x; j < B; j += blockDim.x) w[j] = powf(pmin / w[j], beta);
+}
+
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) per_draw_kernel(const PerLanes<LANES> pl, const float2* betas,
+                                                           const unsigned long long* keys, int st, int B, int O, int A,
+                                                           long long* idx, float* w, float* obs, float* act, float* rew,
+                                                           float* nobs, float* done, size_t lane_stride) {
+  const int z = LANES ? blockIdx.z : 0;
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    betas = lane_ptr(betas, o), keys = lane_ptr(keys, o), idx = lane_ptr(idx, o), w = lane_ptr(w, o);
+    obs = lane_ptr(obs, o), act = lane_ptr(act, o), rew = lane_ptr(rew, o), nobs = lane_ptr(nobs, o);
+    done = lane_ptr(done, o);
+  }
+  per_draw_rows(pl.tree[z], pl.rows[z], betas, keys, st, B, idx, w);
   // the gather (idx written above by this CTA: visible after the __syncthreads)
   const float* src[5] = {pl.obs[z], pl.act[z], pl.rew[z], pl.next_obs[z], pl.done[z]};
   float* dst[5] = {obs, act, rew, nobs, done};
@@ -956,6 +1059,35 @@ __global__ void __launch_bounds__(GTHREADS) per_draw_kernel(const PerLanes<LANES
       dst[c][i] = src[c][idx[r] * wd + (i - r * wd)];
     }
   }
+}
+
+// per_draw_kernel with n-step returns: the same draw and weights, then row j's window from idx[j] (nstep_walk over the
+// learner's episode-end column ends.p[z]) stages rew := R, done := done[last], disc := g and last; obs and act come from
+// the drawn rows, next_obs from the last rows.
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) per_draw_nstep_kernel(const PerLanes<LANES> pl, const LaneSrc<LANES> ends,
+                                                                 const float2* betas, const unsigned long long* keys,
+                                                                 int st, int B, int O, int A, int n, float gamma,
+                                                                 long long* idx, float* w, float* obs, float* act,
+                                                                 float* rew, float* nobs, float* done, float* disc,
+                                                                 long long* last, size_t lane_stride) {
+  const int z = LANES ? blockIdx.z : 0;
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    betas = lane_ptr(betas, o), keys = lane_ptr(keys, o), idx = lane_ptr(idx, o), w = lane_ptr(w, o);
+    obs = lane_ptr(obs, o), act = lane_ptr(act, o), rew = lane_ptr(rew, o), nobs = lane_ptr(nobs, o);
+    done = lane_ptr(done, o), disc = lane_ptr(disc, o), last = lane_ptr(last, o);
+  }
+  per_draw_rows(pl.tree[z], pl.rows[z], betas, keys, st, B, idx, w);
+  for (int j = threadIdx.x; j < B; j += blockDim.x) {
+    float R, g;
+    const long long p = nstep_walk(pl.rew[z], pl.done[z], ends.p[z], pl.rows[z], idx[j], n, gamma, R, g);
+    rew[j] = R, disc[j] = g, done[j] = pl.done[z][p], last[j] = p;
+  }
+  __syncthreads();  // every row's last row is visible to the CTA
+  copy_rows(pl.obs[z], idx, O, B, obs);
+  copy_rows(pl.act[z], idx, A, B, act);
+  copy_rows(pl.next_obs[z], last, O, B, nobs);
 }
 
 // One CTA per learner: the priority update of one step.  Row j (in row order; a later row on the same leaf wins) sets
@@ -1110,6 +1242,13 @@ struct b200rl_offpolicy {
   float *per_w = nullptr, *per_newp = nullptr;  // [max_steps * B] importance weights / new priorities of each row
   float* per_absd = nullptr;                    // [B] |delta| of the current step
   int* per_bad = nullptr;                       // [max_steps] rows of each step whose new priority was not finite
+  // n-step returns (DQN engines; b200rl_offpolicy_set_nstep): an n-step call stages R in rew, done[last] in done, and
+  // each row's discount and last row beside them
+  int nstep = 1, graph_nstep = 1;
+  LaneSrc<true> nstep_ends{};         // each learner's episode-end column (n > 1)
+  bool nstep_last = false;            // the last call that ran steps was an n-step one
+  float* nstep_disc = nullptr;        // [max_steps * B] gamma^k of each row's window
+  long long* nstep_rows = nullptr;    // [max_steps * B] the last row of each row's window
   std::vector<void*> allocs;
 };
 
@@ -1367,6 +1506,8 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
     rc |= oalloc(h, &h->per_newp, S * B);
     rc |= oalloc(h, &h->per_absd, B);
     rc |= oalloc(h, &h->per_bad, S);
+    rc |= oalloc(h, &h->nstep_disc, S * B);
+    rc |= oalloc(h, &h->nstep_rows, S * B);
   }
   if (c51) {
     rc |= oalloc(h, &h->c51_support, C51_MAX_ATOMS);
@@ -1568,6 +1709,25 @@ extern "C" int b200rl_offpolicy_set_per(b200rl_offpolicy* h, const b200rl_per_hp
   B200RL_REQUIRE(pp->beta_anneal_steps >= 1, "offpolicy_set_per: beta_anneal_steps must be >= 1");
   h->per_hp = *pp;
   h->per_set = true;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, const float* const* episode_ends) {
+  B200RL_REQUIRE(h, "offpolicy_set_nstep: NULL engine");
+  B200RL_REQUIRE(h->dqn, "offpolicy_set_nstep: n-step returns are implemented for DQN and C51 engines (algo = 2 or 3) "
+                 "only");
+  B200RL_REQUIRE(n_step >= 1 && n_step <= NSTEP_MAX, "offpolicy_set_nstep: n_step must be 1..%d, got %d", NSTEP_MAX,
+                 n_step);
+  LaneSrc<true> ends{};
+  if (n_step > 1) {
+    B200RL_REQUIRE(episode_ends != nullptr, "offpolicy_set_nstep: n_step = %d needs the episode-end columns", n_step);
+    for (int z = 0; z < h->K; ++z) {
+      B200RL_REQUIRE(episode_ends[z] != nullptr, "offpolicy_set_nstep: learner %d: NULL episode-end column", z);
+      ends.p[z] = episode_ends[z];
+    }
+  }
+  h->nstep = n_step;
+  h->nstep_ends = ends;
   return 0;
 }
 
@@ -1905,6 +2065,7 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
     return 0;
   };
   const bool per = h->per_run;
+  const bool nstep = h->nstep > 1;  // the loss heads read each row's staged discount
   const float2* betas = h->adam_tab + (size_t)3 * maxS;
   const unsigned long long* keys = reinterpret_cast<const unsigned long long*>(h->adam_tab + (size_t)4 * maxS);
   const float alpha = (float)h->per_hp.alpha, eps = (float)h->per_hp.eps;
@@ -1916,7 +2077,18 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
       float* s_w = h->per_w + (size_t)st * B;
       float* dst[5] = {h->obs + (size_t)st * B * O, h->act + (size_t)st * B, h->rew + (size_t)st * B,
                        h->nobs + (size_t)st * B * O, h->done + (size_t)st * B};
-      if (h->K == 1)
+      float* s_disc = h->nstep_disc + (size_t)st * B;
+      long long* s_last = h->nstep_rows + (size_t)st * B;
+      const float g = (float)hp->gamma;
+      if (nstep && h->K == 1)
+        per_draw_nstep_kernel<false><<<1, GTHREADS, 0, s>>>(per_solo(h->per_lanes), LaneSrc<false>{{h->nstep_ends.p[0]}},
+                                                             betas, keys, st, B, O, 1, h->nstep, g, s_idx, s_w, dst[0],
+                                                             dst[1], dst[2], dst[3], dst[4], s_disc, s_last, 0);
+      else if (nstep)
+        per_draw_nstep_kernel<true><<<lanes, GTHREADS, 0, s>>>(h->per_lanes, h->nstep_ends, betas, keys, st, B, O, 1,
+                                                              h->nstep, g, s_idx, s_w, dst[0], dst[1], dst[2], dst[3],
+                                                              dst[4], s_disc, s_last, h->lane_stride);
+      else if (h->K == 1)
         per_draw_kernel<false><<<1, GTHREADS, 0, s>>>(per_solo(h->per_lanes), betas, keys, st, B, O, 1, s_idx, s_w,
                                                        dst[0], dst[1], dst[2], dst[3], dst[4], 0);
       else
@@ -1948,10 +2120,20 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
     if (net_forward(h, qt, tq, B, s)) return 1;
     if (dbl && edge(s2, s)) return 1;
     if (edge(s3, s)) return 1;
+    const float* s_disc = h->nstep_disc + (size_t)st * B;
     if (per) {
-      LAUNCH_LANES(h, dqn_per_loss_kernel, 1, GTHREADS, s, qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done,
-                   (float)hp->gamma, B, n, h->dqn_dout, h->out_l1 + st, h->out_q1 + (size_t)st * B, h->dqn_bad + st,
-                   h->per_w + (size_t)st * B, h->per_absd);
+      if (nstep && h->K == 1)
+        dqn_nstep_loss_kernel<false, true><<<1, GTHREADS, 0, s>>>(
+            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, B, n, h->dqn_dout, h->out_l1 + st,
+            h->out_q1 + (size_t)st * B, h->dqn_bad + st, h->per_w + (size_t)st * B, h->per_absd, 0);
+      else if (nstep)
+        dqn_nstep_loss_kernel<true, true><<<lanes, GTHREADS, 0, s>>>(
+            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, B, n, h->dqn_dout, h->out_l1 + st,
+            h->out_q1 + (size_t)st * B, h->dqn_bad + st, h->per_w + (size_t)st * B, h->per_absd, h->lane_stride);
+      else
+        LAUNCH_LANES(h, dqn_per_loss_kernel, 1, GTHREADS, s, qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done,
+                     (float)hp->gamma, B, n, h->dqn_dout, h->out_l1 + st, h->out_q1 + (size_t)st * B, h->dqn_bad + st,
+                     h->per_w + (size_t)st * B, h->per_absd);
       B200RL_CUDA(cudaGetLastError());
       count_launch(1);
       if (edge(s, s4)) return 1;
@@ -1971,7 +2153,17 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
       const size_t smem = sizeof(float) * (size_t)(N + W * (3 * N + n / N));
       const float vmin = (float)h->c51_hp.v_min, vmax = (float)h->c51_hp.v_max;
       const float dz = (float)((h->c51_hp.v_max - h->c51_hp.v_min) / (N - 1));
-      if (h->K == 1)
+      if (nstep && h->K == 1)
+        c51_nstep_loss_kernel<false><<<grid, W * 32, smem, s>>>(
+            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, h->c51_support, vmin, vmax, dz, B,
+            n / N, N, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync, h->out_l1 + st,
+            h->dqn_bad + st, 0);
+      else if (nstep)
+        c51_nstep_loss_kernel<true><<<grid, W * 32, smem, s>>>(
+            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, h->c51_support, vmin, vmax, dz, B,
+            n / N, N, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync, h->out_l1 + st,
+            h->dqn_bad + st, h->lane_stride);
+      else if (h->K == 1)
         c51_loss_kernel<false><<<grid, W * 32, smem, s>>>(
             qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, h->c51_support, (float)hp->gamma, vmin, vmax,
             dz, B, n / N, N, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync, h->out_l1 + st,
@@ -1984,8 +2176,17 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
       B200RL_CUDA(cudaGetLastError());
       count_launch(1);
     } else {
-      LAUNCH_LANES(h, dqn_loss_kernel, 1, GTHREADS, s, qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done,
-                   (float)hp->gamma, B, n, h->dqn_dout, h->out_l1 + st, h->out_q1 + (size_t)st * B, h->dqn_bad + st);
+      if (nstep && h->K == 1)
+        dqn_nstep_loss_kernel<false, false><<<1, GTHREADS, 0, s>>>(
+            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, B, n, h->dqn_dout, h->out_l1 + st,
+            h->out_q1 + (size_t)st * B, h->dqn_bad + st, nullptr, nullptr, 0);
+      else if (nstep)
+        dqn_nstep_loss_kernel<true, false><<<lanes, GTHREADS, 0, s>>>(
+            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, B, n, h->dqn_dout, h->out_l1 + st,
+            h->out_q1 + (size_t)st * B, h->dqn_bad + st, nullptr, nullptr, h->lane_stride);
+      else
+        LAUNCH_LANES(h, dqn_loss_kernel, 1, GTHREADS, s, qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done,
+                     (float)hp->gamma, B, n, h->dqn_dout, h->out_l1 + st, h->out_q1 + (size_t)st * B, h->dqn_bad + st);
       B200RL_CUDA(cudaGetLastError());
       count_launch(1);
     }
@@ -2024,6 +2225,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   cudaStream_t s = h->gs;
   const size_t SB = (size_t)S * B;
   h->per_last = h->per_run;  // what get_per_draws may report
+  h->nstep_last = h->nstep > 1;  // and get_nstep_draws
 
   // Adam's step-dependent scalars for the steps of this call (torch's host-side double arithmetic), one small upload
   // (a group: one table per learner, from that learner's step counts, uploaded with one strided copy)
@@ -2069,18 +2271,22 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
       return 1;
     }
   } else {
-    // a prioritized graph holds the trees' and the columns' addresses, the row counts and alpha / eps in its nodes
+    // a prioritized graph holds the trees' and the columns' addresses, the row counts and alpha / eps in its nodes,
+    // and an n-step one the episode-end columns too (its draw kernel walks them)
     std::vector<char> per_key;
     if (h->per_run) {
       const char* a = reinterpret_cast<const char*>(&h->per_hp);
       const char* b = reinterpret_cast<const char*>(&h->per_lanes);
+      const char* c = reinterpret_cast<const char*>(&h->nstep_ends);
       per_key.assign(a, a + sizeof(h->per_hp));
       per_key.insert(per_key.end(), b, b + sizeof(h->per_lanes));
+      per_key.insert(per_key.end(), c, c + sizeof(h->nstep_ends));
     }
     if (h->graph == nullptr || h->graph_S != S || h->graph_B != B || memcmp(&h->graph_hp, hp, sizeof(*hp)) != 0 ||
         memcmp(&h->graph_sac_hp, &h->sac_hp, sizeof(h->sac_hp)) != 0 ||
         memcmp(&h->graph_dqn_hp, &h->dqn_hp, sizeof(h->dqn_hp)) != 0 ||
-        memcmp(&h->graph_c51_hp, &h->c51_hp, sizeof(h->c51_hp)) != 0 || h->graph_per_key != per_key) {
+        memcmp(&h->graph_c51_hp, &h->c51_hp, sizeof(h->c51_hp)) != 0 || h->graph_per_key != per_key ||
+        h->graph_nstep != h->nstep) {
       if (h->graph) {
         cudaGraphExecDestroy(h->graph);
         h->graph = nullptr;
@@ -2119,6 +2325,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
       h->graph_dqn_hp = h->dqn_hp;
       h->graph_c51_hp = h->c51_hp;
       h->graph_per_key = per_key;
+      h->graph_nstep = h->nstep;
       h->graph_npol = n_pol;
     }
     n_pol = h->graph_npol;
@@ -2175,6 +2382,8 @@ extern "C" int b200rl_offpolicy_train(b200rl_offpolicy* h, const b200rl_offpolic
   B200RL_REQUIRE(h->dqn || !hp->use_target_noise || noise, "offpolicy_train: target noise requested but no noise given");
   B200RL_REQUIRE(h->dqn || hp->policy_delay >= 1, "offpolicy_train: policy_delay must be >= 1");
   if (sac_ready(h, noise != nullptr, "offpolicy_train") || dqn_ready(h, "offpolicy_train")) return 2;
+  B200RL_REQUIRE(h->nstep == 1, "offpolicy_train: n-step returns (n_step = %d) need the device replay columns: use "
+                 "train_gather, train_gather_rng or train_prioritized", h->nstep);
   cudaStream_t user = static_cast<cudaStream_t>(stream);
   cudaStream_t s = h->gs;  // everything runs on the engine's stream, ordered after the caller's
   const int O = h->O, A = h->A;
@@ -2198,9 +2407,32 @@ extern "C" int b200rl_offpolicy_train(b200rl_offpolicy* h, const b200rl_offpolic
 }
 
 // The five staged columns (obs, act, rew, next_obs, done) gathered from each learner's replay columns at the rows in
-// h->idx: one launch per column for all learners
-static int gather_columns(b200rl_offpolicy* h, const b200rl_offpolicy_replay* rb, long long SB, cudaStream_t s) {
+// h->idx: one launch per column for all learners; with n-step returns one nstep_gather_kernel launch, which also stages
+// the discounts and last rows
+static int gather_columns(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, const b200rl_offpolicy_replay* rb,
+                          long long SB, cudaStream_t s) {
   const int O = h->O, A = h->A;
+  if (h->nstep > 1) {
+    NStepSrc<true> src{};
+    for (int z = 0; z < h->K; ++z)
+      src.obs[z] = rb[z].obs, src.act[z] = rb[z].act, src.rew[z] = rb[z].rew, src.next_obs[z] = rb[z].next_obs,
+      src.done[z] = rb[z].done, src.ends[z] = h->nstep_ends.p[z], src.rows[z] = rb[z].rows;
+    const dim3 grid((unsigned)((SB + GTHREADS - 1) / GTHREADS));
+    const float g = (float)hp->gamma;
+    if (h->K == 1) {
+      const NStepSrc<false> one = {{src.obs[0]}, {src.act[0]}, {src.rew[0]}, {src.next_obs[0]}, {src.done[0]},
+                                   {src.ends[0]}, {src.rows[0]}};
+      nstep_gather_kernel<false><<<grid, GTHREADS, 0, s>>>(one, h->idx, SB, O, A, h->nstep, g, h->obs, h->act, h->rew,
+                                                           h->nobs, h->done, h->nstep_disc, h->nstep_rows, 0);
+    } else {
+      nstep_gather_kernel<true><<<lane_grid(grid, h->K), GTHREADS, 0, s>>>(src, h->idx, SB, O, A, h->nstep, g, h->obs,
+                                                                           h->act, h->rew, h->nobs, h->done,
+                                                                           h->nstep_disc, h->nstep_rows, h->lane_stride);
+    }
+    B200RL_CUDA(cudaGetLastError());
+    count_launch(1);
+    return 0;
+  }
   float* dst[5] = {h->obs, h->act, h->rew, h->nobs, h->done};
   const int w[5] = {O, A, 1, O, 1};
   for (int c = 0; c < 5; ++c) {
@@ -2265,7 +2497,7 @@ extern "C" int b200rl_offpolicy_train_gather_group(b200rl_offpolicy* h, const b2
   B200RL_CUDA(cudaMemcpy2DAsync(h->idx, ls, idx, SB * 8, SB * 8, h->K, cudaMemcpyHostToDevice, s));
   const size_t n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise && !h->dqn ? SB * A : 0);
   if (n_eps) B200RL_CUDA(cudaMemcpy2DAsync(h->eps, ls, noise, n_eps * 4, n_eps * 4, h->K, cudaMemcpyHostToDevice, s));
-  if (gather_columns(h, rb, (long long)SB, s)) return 1;
+  if (gather_columns(h, hp, rb, (long long)SB, s)) return 1;
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
 }
 
@@ -2331,7 +2563,7 @@ extern "C" int b200rl_offpolicy_train_gather_rng_group(b200rl_offpolicy* h, cons
   }
   B200RL_CUDA(cudaGetLastError());
   count_launch(1);
-  if (gather_columns(h, rb, SB, s)) return 1;
+  if (gather_columns(h, hp, rb, SB, s)) return 1;
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
 }
 
@@ -2437,6 +2669,21 @@ extern "C" int b200rl_offpolicy_get_per_draws(b200rl_offpolicy* h, int32_t S, in
   B200RL_CUDA(cudaMemcpy2DAsync(idx, SB * 8, h->idx, ls, SB * 8, h->K, cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaMemcpy2DAsync(weights, SB * 4, h->per_w, ls, SB * 4, h->K, cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaMemcpy2DAsync(priorities, SB * 4, h->per_newp, ls, SB * 4, h->K, cudaMemcpyDeviceToHost, s));
+  B200RL_CUDA(cudaStreamSynchronize(s));
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_get_nstep_draws(b200rl_offpolicy* h, int32_t S, int32_t B, int64_t* last_rows,
+                                                float* returns, float* discounts, void* stream) {
+  B200RL_REQUIRE(h && h->dqn && last_rows && returns && discounts && S >= 0 && S <= h->cfg.max_steps && B >= 1 &&
+                     B <= h->cfg.max_minibatch, "offpolicy_get_nstep_draws: bad arguments");
+  B200RL_REQUIRE(h->nstep_last, "offpolicy_get_nstep_draws: the engine's last train call was not an n-step one");
+  (void)stream;
+  cudaStream_t s = h->gs;
+  const size_t SB = (size_t)S * B, ls = h->lane_stride;
+  B200RL_CUDA(cudaMemcpy2DAsync(last_rows, SB * 8, h->nstep_rows, ls, SB * 8, h->K, cudaMemcpyDeviceToHost, s));
+  B200RL_CUDA(cudaMemcpy2DAsync(returns, SB * 4, h->rew, ls, SB * 4, h->K, cudaMemcpyDeviceToHost, s));
+  B200RL_CUDA(cudaMemcpy2DAsync(discounts, SB * 4, h->nstep_disc, ls, SB * 4, h->K, cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaStreamSynchronize(s));
   return 0;
 }

@@ -546,6 +546,31 @@ class OffPolicyEngine:
               "get_per_draws")
         return (idx[0], w[0], p[0]) if self.K == 1 else (idx, w, p)
 
+    # ---- n-step returns (DQN / C51) ----
+    def set_nstep(self, n_step: int, episode_ends=None) -> None:
+        """Window length ``n_step`` (1..32; 1 clears it) of the next train calls, with ``episode_ends`` = K float32 CUDA
+        tensors (each learner's ``device_episode_ends()``, over the rows of the replay it trains on) when n_step > 1."""
+        import torch
+        ptrs = None
+        if int(n_step) > 1:
+            if episode_ends is None or len(episode_ends) != self.K:
+                raise ValueError(f"set_nstep: n_step = {n_step} needs the episode-end columns of {self.K} learners")
+            for z, t in enumerate(episode_ends):
+                if not (torch.is_tensor(t) and t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+                    raise ValueError(f"set_nstep: learner {z}: the episode-end column must be a contiguous float32 CUDA "
+                                     f"tensor, got {getattr(t, 'dtype', type(t))} on {getattr(t, 'device', '?')}")
+            ptrs = (C.c_void_p * self.K)(*[t.data_ptr() for t in episode_ends])
+        check(self.lib.b200rl_offpolicy_set_nstep(self.h, int(n_step), ptrs), "set_nstep")
+
+    def get_nstep_draws(self, S: int, B: int):
+        """(last window row [S,B] int64, return R [S,B], discount [S,B] float32) of each row of the last n-step call;
+        a group: each with a leading [K] axis."""
+        last = np.empty((self.K, S, B), np.int64)
+        R, g = np.empty((self.K, S, B), np.float32), np.empty((self.K, S, B), np.float32)
+        check(self.lib.b200rl_offpolicy_get_nstep_draws(self.h, S, B, _ptr(last), _ptr(R), _ptr(g),
+                                                        current_stream_handle()), "get_nstep_draws")
+        return (last[0], R[0], g[0]) if self.K == 1 else (last, R, g)
+
     def sac_outputs(self, S: int):
         """(mean log pi per step [S], alpha used by each step [S]) of the last train call (a group: [K, S] each)."""
         lp, al = np.zeros((self.K, S), np.float32), np.zeros((self.K, S), np.float32)

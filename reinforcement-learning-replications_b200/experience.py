@@ -145,6 +145,11 @@ class PackedExperience(Experience):
         act = self._act[:n] if self._a >= 1 else self._act[:n, 0]
         return obs, act, self._rew[:n], nxt, self._done[:n]
 
+    @property
+    def ep_offsets(self) -> np.ndarray:
+        """[E+1] int64: episode k holds rows ep_offsets[k] .. ep_offsets[k+1] - 1."""
+        return np.asarray(self._offsets, dtype=np.int64)
+
     # ---- the reference's nested-list API, as views ----
     def _episodes(self, column):
         return [list(column[b:e]) for b, e in zip(self._offsets[:-1], self._offsets[1:])]

@@ -17,7 +17,14 @@ class ReplayBuffer:
     and a minibatch is ONE fancy-index gather per column instead of the reference's per-transition Python-list walk
     (1.2 ms per 256-sample minibatch there, SURVEY a20).  ``sample_indices`` + ``gather`` expose the two halves so the
     off-policy trainer can draw all S minibatches of a ``train`` call at once.  The reference's list attributes
-    (``observations`` ...) remain available as read-only views in logical order."""
+    (``observations`` ...) remain available as read-only views in logical order.
+
+    Beside the five columns the buffer keeps one flag per row for n-step returns: ``episode_ends[i]`` is true when row i
+    was the last row of an episode in the experience that appended it -- the episode boundaries of a ``PackedExperience``
+    (``ep_offsets``) or of a nested-list ``Experience`` (its episode lengths; a segment a sampler cut off at the end of a
+    ``sample()`` call is an episode there), and only the last row for any other object with ``transition_columns()``.
+    Every append ends on a marked row, so the newest live row is always marked: a window of consecutive rows that stops
+    at the first marked or done row never reads past the ring's head, nor a row a ring overwrite replaced."""
 
     COLUMNS = ("observations", "actions", "rewards", "next_observations", "dones")
 
@@ -27,7 +34,9 @@ class ReplayBuffer:
         self._head: int = 0           # physical row of logical index 0
         self._capacity: int = 0       # allocated rows (<= buffer_size)
         self._cols: Dict[str, Optional[np.ndarray]] = {k: None for k in self.COLUMNS}
+        self._ends: Optional[np.ndarray] = None  # [capacity] bool: the row ended an episode of its append
         self._dev = None              # device mirror (torch CUDA tensors, float32), built lazily by device_columns()
+        self._dev_ends = None         # device mirror of _ends (float32 0/1), built by the first device_episode_ends()
         self._dev_dirty: List = []    # physical row ranges written since the mirror was last refreshed
 
     # ---- storage ----
@@ -38,6 +47,7 @@ class ReplayBuffer:
             # rewards stay float64 and dones bool, like the values the reference's lists hold
             dt = np.float64 if k == "rewards" else (np.bool_ if k == "dones" else np.float32)
             self._cols[k] = np.empty((rows,) + first.shape, dtype=dt)
+        self._ends = np.zeros(rows, dtype=np.bool_)
         self._capacity = rows
 
     def _grow(self, need: int) -> None:
@@ -51,8 +61,11 @@ class ReplayBuffer:
             new = np.empty((new_cap,) + old.shape[1:], dtype=old.dtype)
             new[:self.current_size] = old[order]
             self._cols[k] = new
+        ends = np.zeros(new_cap, dtype=np.bool_)
+        ends[:self.current_size] = self._ends[order]
+        self._ends = ends
         self._head, self._capacity = 0, new_cap
-        self._dev = None  # reallocated: the mirror is rebuilt on the next device_columns()
+        self._dev = self._dev_ends = None  # reallocated: the mirrors are rebuilt on their next request
 
     def _physical(self, logical: np.ndarray) -> np.ndarray:
         return (self._head + logical) % self._capacity if self._capacity else logical
@@ -66,10 +79,12 @@ class ReplayBuffer:
         n = len(new[0])
         if n == 0:
             return
+        ends = self._episode_ends_of(experience, n)
         if self._capacity == 0:
             self._allocate(n, new)
         if n >= self.buffer_size:  # only the newest buffer_size transitions survive (front deletion in the reference)
             new = tuple(v[n - self.buffer_size:] for v in new)
+            ends = ends[n - self.buffer_size:]
             n = self.buffer_size
         total = self.current_size + n
         if min(total, self.buffer_size) > self._capacity:
@@ -85,6 +100,9 @@ class ReplayBuffer:
             col[start:start + first] = arr[:first]
             if first < n:
                 col[:n - first] = arr[first:]
+        self._ends[start:start + first] = ends[:first]
+        if first < n:
+            self._ends[:n - first] = ends[first:]
         self.current_size += n
         if self._dev is not None:  # no mirror yet: its first build uploads everything anyway
             self._dev_dirty.append((start, first))
@@ -92,6 +110,25 @@ class ReplayBuffer:
                 self._dev_dirty.append((0, n - first))
             if len(self._dev_dirty) > 256:  # many small appends between two train() calls: one full refresh is cheaper
                 self._dev_dirty = self._live_ranges()
+
+    @staticmethod
+    def _episode_ends_of(experience, n: int) -> np.ndarray:
+        """[n] bool: the rows of this append that end an episode (see the class docstring); the last is always set."""
+        ends = np.zeros(n, dtype=np.bool_)
+        offsets = getattr(experience, "ep_offsets", None)
+        if offsets is not None:  # PackedExperience
+            ends[np.asarray(offsets, np.int64)[1:] - 1] = True
+        elif not hasattr(experience, "transition_columns"):  # nested lists: one list per episode
+            ends[np.cumsum([len(ep) for ep in experience.rewards]) - 1] = True
+        ends[-1] = True
+        return ends
+
+    @property
+    def episode_ends(self) -> List:
+        """The episode-end flags in logical order (a read-only view, like ``dones``)."""
+        if self._ends is None:
+            return []
+        return [bool(x) for x in self._ends[self._physical(np.arange(self.current_size))]]
 
     def _live_ranges(self) -> List:
         first = min(self.current_size, self._capacity - self._head)  # the rows that hold data, wrap-around aware
@@ -119,8 +156,22 @@ class ReplayBuffer:
             for k, d in zip(self.COLUMNS, self._dev):
                 host = np.ascontiguousarray(self._cols[k][start:start + count], dtype=np.float32)
                 d[start:start + count].copy_(torch.from_numpy(host))
+            if self._dev_ends is not None:
+                self._dev_ends[start:start + count].copy_(torch.from_numpy(self._ends[start:start + count].astype(np.float32)))
         self._dev_dirty = []
         return self._dev, self._capacity
+
+    def device_episode_ends(self):
+        """The episode-end flags as a float32 0/1 CUDA tensor with ``capacity`` rows in physical row order, beside
+        ``device_columns()`` (what n-step returns walk).  Built on the first request, then refreshed from the same
+        written row ranges as the columns."""
+        import torch
+        if self._capacity == 0:
+            raise ValueError("device_episode_ends: the buffer is empty")
+        if self._dev_ends is None:
+            self._dev_ends = torch.from_numpy(self._ends.astype(np.float32)).to("cuda")
+        self.device_columns()
+        return self._dev_ends
 
     # ---- sampling ----
     def sample_indices(self, minibatch_size: int) -> np.ndarray:

@@ -23,8 +23,9 @@
 // C51 (config algo = 3) is DQN's step program with a categorical head over return distributions (c51_loss_kernel).
 // Prioritized replay for DQN (train_prioritized): a 32-way sum tree per replay buffer, drawn from, weighed and gathered
 // by per_draw_kernel and updated by per_update_kernel inside the same step program.
-// n-step returns for DQN / C51 (set_nstep): nstep_gather_kernel (or per_draw_nstep_kernel) walks each drawn row's window
-// and stages its return and discount; the *_nstep_loss_kernel heads read the per-row discount in place of gamma.
+// n-step returns for DQN / C51 (set_nstep): nstep_gather_kernel (or per_draw_kernel's NSTEP instantiation) walks each
+// drawn row's window and stages its return and discount; the loss heads' NSTEP instantiations read the per-row discount
+// in place of gamma.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -315,11 +316,13 @@ __device__ __forceinline__ void copy_rows(const float* table, const long long* r
   }
 }
 
-// the replay columns, episode-end column and row count of every learner of a launch
+// the replay columns, episode-end column (n-step calls), sum tree (prioritized calls) and row count of every learner
+// of a launch
 template <bool LANES>
-struct NStepSrc {
+struct ReplayLanes {
   static constexpr int N = LANES ? B200RL_MAX_LEARNERS : 1;
-  const float *obs[N], *act[N], *rew[N], *next_obs[N], *done[N], *ends[N];
+  LaneSrc<LANES> obs, act, rew, next_obs, done, ends;
+  float* tree[N];
   long long rows[N];
 };
 
@@ -327,7 +330,7 @@ struct NStepSrc {
 // start row idx[i] and stages rew := R, done := done[last], disc := g and last; then the CTA copies obs and act from the
 // start rows and next_obs from the last rows.
 template <bool LANES>
-__global__ void __launch_bounds__(GTHREADS) nstep_gather_kernel(const NStepSrc<LANES> src, const long long* idx,
+__global__ void __launch_bounds__(GTHREADS) nstep_gather_kernel(const ReplayLanes<LANES> src, const long long* idx,
                                                                long long n_out, int O, int A, int n, float gamma,
                                                                float* obs, float* act, float* rew, float* nobs,
                                                                float* done, float* disc, long long* last,
@@ -341,14 +344,14 @@ __global__ void __launch_bounds__(GTHREADS) nstep_gather_kernel(const NStepSrc<L
   const long long r0 = (long long)blockIdx.x * blockDim.x, i = r0 + threadIdx.x;
   if (i < n_out) {
     float R, g;
-    const long long p = nstep_walk(src.rew[z], src.done[z], src.ends[z], src.rows[z], idx[i], n, gamma, R, g);
-    rew[i] = R, disc[i] = g, done[i] = src.done[z][p], last[i] = p;
+    const long long p = nstep_walk(src.rew.p[z], src.done.p[z], src.ends.p[z], src.rows[z], idx[i], n, gamma, R, g);
+    rew[i] = R, disc[i] = g, done[i] = src.done.p[z][p], last[i] = p;
   }
   __syncthreads();  // the CTA's last rows are visible to all its threads
   const int nr = (int)min((long long)blockDim.x, n_out - r0);
-  copy_rows(src.obs[z], idx + r0, O, nr, obs + r0 * O);
-  copy_rows(src.act[z], idx + r0, A, nr, act + r0 * A);
-  copy_rows(src.next_obs[z], last + r0, O, nr, nobs + r0 * O);
+  copy_rows(src.obs.p[z], idx + r0, O, nr, obs + r0 * O);
+  copy_rows(src.act.p[z], idx + r0, A, nr, act + r0 * A);
+  copy_rows(src.next_obs.p[z], last + r0, O, nr, nobs + r0 * O);
 }
 
 // y = r + gamma * (1 - d) * min(q1t, q2t)   (td3.py:337-339; ddpg.py:280: single target Q)
@@ -624,11 +627,13 @@ __device__ __forceinline__ int argmax_row(const float* q, int n) {
 // dOut[i, a] = w_i clamp(delta_i, -1, 1) / B -- and absd[i] = |delta_i| (-1 for a row with an invalid action).  With
 // every w_i = 1 both are bit for bit those of the unweighted head: the products by 1 are exact.
 // NSTEP (n-step returns): row i's discount is disc[i] (gamma^k of its window) in place of gamma.
-template <bool LANES, bool WEIGHTED, bool NSTEP = false>
-__device__ __forceinline__ void dqn_loss_rows(const float* q, const float* qt_next, const float* qn, const float* act,
-                                              const float* rew, const float* done, float gamma, int B, int n,
-                                              float* dout, float* loss_out, float* q_copy, int* bad_out, const float* w,
-                                              float* absd, size_t lane_stride, const float* disc = nullptr) {
+// Each flag's operands are read only by the instantiations that set it.
+template <bool LANES, bool WEIGHTED, bool NSTEP>
+__global__ void __launch_bounds__(GTHREADS) dqn_loss_kernel(const float* q, const float* qt_next, const float* qn,
+                                                           const float* act, const float* rew, const float* done,
+                                                           const float* disc, float gamma, int B, int n, float* dout,
+                                                           float* loss_out, float* q_copy, int* bad_out, const float* w,
+                                                           float* absd, size_t lane_stride) {
   __shared__ double red[32];
   __shared__ int bad_rows;
   if (LANES) {
@@ -677,37 +682,6 @@ __device__ __forceinline__ void dqn_loss_rows(const float* q, const float* qt_ne
   if (bad) atomicAdd(&bad_rows, bad);
   block_mean(acc, B, loss_out, red);  // its __syncthreads orders every thread's atomicAdd before thread 0 reads
   if (threadIdx.x == 0) *bad_out = bad_rows;
-}
-
-template <bool LANES>
-__global__ void __launch_bounds__(GTHREADS) dqn_loss_kernel(const float* q, const float* qt_next, const float* qn,
-                                                           const float* act, const float* rew, const float* done,
-                                                           float gamma, int B, int n, float* dout, float* loss_out,
-                                                           float* q_copy, int* bad_out, size_t lane_stride) {
-  dqn_loss_rows<LANES, false>(q, qt_next, qn, act, rew, done, gamma, B, n, dout, loss_out, q_copy, bad_out, nullptr,
-                              nullptr, lane_stride);
-}
-
-// the prioritized-replay head: importance weights w [B] in, |delta| [B] out (see dqn_loss_rows)
-template <bool LANES>
-__global__ void __launch_bounds__(GTHREADS) dqn_per_loss_kernel(const float* q, const float* qt_next, const float* qn,
-                                                               const float* act, const float* rew, const float* done,
-                                                               float gamma, int B, int n, float* dout, float* loss_out,
-                                                               float* q_copy, int* bad_out, const float* w, float* absd,
-                                                               size_t lane_stride) {
-  dqn_loss_rows<LANES, true>(q, qt_next, qn, act, rew, done, gamma, B, n, dout, loss_out, q_copy, bad_out, w, absd,
-                             lane_stride);
-}
-
-// the n-step heads: row i's discount disc[i] in place of gamma; WEIGHTED as dqn_per_loss_kernel (w, absd NULL otherwise)
-template <bool LANES, bool WEIGHTED>
-__global__ void __launch_bounds__(GTHREADS) dqn_nstep_loss_kernel(const float* q, const float* qt_next, const float* qn,
-                                                                 const float* act, const float* rew, const float* done,
-                                                                 const float* disc, int B, int n, float* dout,
-                                                                 float* loss_out, float* q_copy, int* bad_out,
-                                                                 const float* w, float* absd, size_t lane_stride) {
-  dqn_loss_rows<LANES, WEIGHTED, true>(q, qt_next, qn, act, rew, done, 0.f, B, n, dout, loss_out, q_copy, bad_out, w,
-                                       absd, lane_stride, disc);
 }
 
 // target <- param on the steps the copy table marks (flags[idx].x != 0): the graph launches the copy every step and
@@ -789,12 +763,12 @@ __device__ __forceinline__ void c51_warp_log_softmax(const float* x, int N, floa
 // and it is counted.  The last CTA of a learner to finish (sync[0] counts them) writes *loss_out = mean L, summed in
 // double as block_mean sums, and *bad_out = the invalid rows (sync[1]), and leaves both counters at 0 for the next
 // launch.  No atomics touch a float: the head is deterministic.
-// NSTEP (n-step returns): row i's discount is disc[i] (gamma^k of its window) in place of gamma.
+// NSTEP (n-step returns): row i's discount is disc[i] (gamma^k of its window) in place of gamma (unread otherwise).
 template <bool LANES, bool NSTEP>
-__device__ __forceinline__ void c51_loss_rows(
+__global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
     const float* q, const float* qt_next, const float* qn, const float* act, const float* rew, const float* done,
-    const float* support, float gamma, float v_min, float v_max, float dz, int B, int n, int N, float* dout,
-    float* row_loss, float* q_copy, int* sync, float* loss_out, int* bad_out, size_t lane_stride, const float* disc) {
+    const float* disc, const float* support, float gamma, float v_min, float v_max, float dz, int B, int n, int N,
+    float* dout, float* row_loss, float* q_copy, int* sync, float* loss_out, int* bad_out, size_t lane_stride) {
   extern __shared__ float c51_smem[];
   __shared__ double red[32];
   __shared__ bool last;
@@ -870,7 +844,7 @@ __device__ __forceinline__ void c51_loss_rows(
         ce += sb[j] * sx[j];
         msum += sb[j];
       }
-      const float inv = 1.0f / (float)B;  // dqn_loss_rows' scaling
+      const float inv = 1.0f / (float)B;  // dqn_loss_kernel's scaling
 #pragma unroll
       for (int k = 0; k < C51_MAX_ATOMS / 32; ++k)
         if (lane + 32 * k < N) drow[(size_t)a * N + lane + 32 * k] = (sp[lane + 32 * k] * msum - m[k]) * inv;
@@ -894,25 +868,6 @@ __device__ __forceinline__ void c51_loss_rows(
     *bad_out = atomicExch(sync + 1, 0);
     sync[0] = 0;
   }
-}
-
-template <bool LANES>
-__global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
-    const float* q, const float* qt_next, const float* qn, const float* act, const float* rew, const float* done,
-    const float* support, float gamma, float v_min, float v_max, float dz, int B, int n, int N, float* dout,
-    float* row_loss, float* q_copy, int* sync, float* loss_out, int* bad_out, size_t lane_stride) {
-  c51_loss_rows<LANES, false>(q, qt_next, qn, act, rew, done, support, gamma, v_min, v_max, dz, B, n, N, dout, row_loss,
-                              q_copy, sync, loss_out, bad_out, lane_stride, nullptr);
-}
-
-// the n-step head: row i's discount disc[i] in place of gamma
-template <bool LANES>
-__global__ void __launch_bounds__(C51_WARPS * 32) c51_nstep_loss_kernel(
-    const float* q, const float* qt_next, const float* qn, const float* act, const float* rew, const float* done,
-    const float* disc, const float* support, float v_min, float v_max, float dz, int B, int n, int N, float* dout,
-    float* row_loss, float* q_copy, int* sync, float* loss_out, int* bad_out, size_t lane_stride) {
-  c51_loss_rows<LANES, true>(q, qt_next, qn, act, rew, done, support, 0.f, v_min, v_max, dz, B, n, N, dout, row_loss,
-                             q_copy, sync, loss_out, bad_out, lane_stride, disc);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -966,17 +921,8 @@ __global__ void per_tree_fill_kernel(float* tree, long long lo, long long count,
   if (i < count) tree[lo + i] = tree[max_at];
 }
 
-// the tree, the row count and the replay columns of every learner of a launch
-template <bool LANES>
-struct PerLanes {
-  static constexpr int N = LANES ? B200RL_MAX_LEARNERS : 1;
-  float* tree[N];
-  long long rows[N];
-  const float *obs[N], *act[N], *rew[N], *next_obs[N], *done[N];
-};
-
-// One CTA per learner, one thread per row (looping for B > blockDim): the stratified proportional draw of step st, the
-// importance weights and the gather of the five staged columns.
+// One CTA per learner, one thread per row (looping for B > blockDim): the stratified proportional draw of step st and
+// the importance weights.
 //   u_j = (j + U_j) * (M / B), M = the root, U_j = the top 24 bits of Philox4x32-10(counter (j, st, call, 0x9E5),
 //   key seed) times 2^-24; descend from the root: at each node take the first child with a nonzero value whose
 //   inclusive prefix (summed in per_node_sum's order, so the last prefix is the parent itself) exceeds u, else the last
@@ -1034,60 +980,49 @@ __device__ __forceinline__ void per_draw_rows(const float* tree, long long rows,
   for (int j = threadIdx.x; j < B; j += blockDim.x) w[j] = powf(pmin / w[j], beta);
 }
 
-template <bool LANES>
-__global__ void __launch_bounds__(GTHREADS) per_draw_kernel(const PerLanes<LANES> pl, const float2* betas,
+// The draw of a prioritized step, then the minibatch staged from the drawn rows (idx was written above by this CTA:
+// visible after the __syncthreads).  Without NSTEP the five columns are gathered.  With NSTEP (n-step returns) row j's
+// window from idx[j] (nstep_walk over the learner's episode-end column) stages rew := R, done := done[last], disc := g
+// and last; obs and act come from the drawn rows, next_obs from the last rows.  n, gamma, disc and last are read by the
+// NSTEP instantiations only.
+template <bool LANES, bool NSTEP>
+__global__ void __launch_bounds__(GTHREADS) per_draw_kernel(const ReplayLanes<LANES> pl, const float2* betas,
                                                            const unsigned long long* keys, int st, int B, int O, int A,
-                                                           long long* idx, float* w, float* obs, float* act, float* rew,
-                                                           float* nobs, float* done, size_t lane_stride) {
+                                                           int n, float gamma, long long* idx, float* w, float* obs,
+                                                           float* act, float* rew, float* nobs, float* done,
+                                                           float* disc, long long* last, size_t lane_stride) {
   const int z = LANES ? blockIdx.z : 0;
   if (LANES) {
     const size_t o = blockIdx.z * lane_stride;
     betas = lane_ptr(betas, o), keys = lane_ptr(keys, o), idx = lane_ptr(idx, o), w = lane_ptr(w, o);
     obs = lane_ptr(obs, o), act = lane_ptr(act, o), rew = lane_ptr(rew, o), nobs = lane_ptr(nobs, o);
     done = lane_ptr(done, o);
+    if (NSTEP) disc = lane_ptr(disc, o), last = lane_ptr(last, o);
   }
   per_draw_rows(pl.tree[z], pl.rows[z], betas, keys, st, B, idx, w);
-  // the gather (idx written above by this CTA: visible after the __syncthreads)
-  const float* src[5] = {pl.obs[z], pl.act[z], pl.rew[z], pl.next_obs[z], pl.done[z]};
-  float* dst[5] = {obs, act, rew, nobs, done};
-  const int width[5] = {O, A, 1, O, 1};
+  if (NSTEP) {
+    for (int j = threadIdx.x; j < B; j += blockDim.x) {
+      float R, g;
+      const long long p = nstep_walk(pl.rew.p[z], pl.done.p[z], pl.ends.p[z], pl.rows[z], idx[j], n, gamma, R, g);
+      rew[j] = R, disc[j] = g, done[j] = pl.done.p[z][p], last[j] = p;
+    }
+    __syncthreads();  // every row's last row is visible to the CTA
+    copy_rows(pl.obs.p[z], idx, O, B, obs);
+    copy_rows(pl.act.p[z], idx, A, B, act);
+    copy_rows(pl.next_obs.p[z], last, O, B, nobs);
+  } else {
+    const float* src[5] = {pl.obs.p[z], pl.act.p[z], pl.rew.p[z], pl.next_obs.p[z], pl.done.p[z]};
+    float* dst[5] = {obs, act, rew, nobs, done};
+    const int width[5] = {O, A, 1, O, 1};
 #pragma unroll
-  for (int c = 0; c < 5; ++c) {
-    const int wd = width[c];
-    for (int i = threadIdx.x; i < B * wd; i += blockDim.x) {
-      const int r = i / wd;
-      dst[c][i] = src[c][idx[r] * wd + (i - r * wd)];
+    for (int c = 0; c < 5; ++c) {
+      const int wd = width[c];
+      for (int i = threadIdx.x; i < B * wd; i += blockDim.x) {
+        const int r = i / wd;
+        dst[c][i] = src[c][idx[r] * wd + (i - r * wd)];
+      }
     }
   }
-}
-
-// per_draw_kernel with n-step returns: the same draw and weights, then row j's window from idx[j] (nstep_walk over the
-// learner's episode-end column ends.p[z]) stages rew := R, done := done[last], disc := g and last; obs and act come from
-// the drawn rows, next_obs from the last rows.
-template <bool LANES>
-__global__ void __launch_bounds__(GTHREADS) per_draw_nstep_kernel(const PerLanes<LANES> pl, const LaneSrc<LANES> ends,
-                                                                 const float2* betas, const unsigned long long* keys,
-                                                                 int st, int B, int O, int A, int n, float gamma,
-                                                                 long long* idx, float* w, float* obs, float* act,
-                                                                 float* rew, float* nobs, float* done, float* disc,
-                                                                 long long* last, size_t lane_stride) {
-  const int z = LANES ? blockIdx.z : 0;
-  if (LANES) {
-    const size_t o = blockIdx.z * lane_stride;
-    betas = lane_ptr(betas, o), keys = lane_ptr(keys, o), idx = lane_ptr(idx, o), w = lane_ptr(w, o);
-    obs = lane_ptr(obs, o), act = lane_ptr(act, o), rew = lane_ptr(rew, o), nobs = lane_ptr(nobs, o);
-    done = lane_ptr(done, o), disc = lane_ptr(disc, o), last = lane_ptr(last, o);
-  }
-  per_draw_rows(pl.tree[z], pl.rows[z], betas, keys, st, B, idx, w);
-  for (int j = threadIdx.x; j < B; j += blockDim.x) {
-    float R, g;
-    const long long p = nstep_walk(pl.rew[z], pl.done[z], ends.p[z], pl.rows[z], idx[j], n, gamma, R, g);
-    rew[j] = R, disc[j] = g, done[j] = pl.done[z][p], last[j] = p;
-  }
-  __syncthreads();  // every row's last row is visible to the CTA
-  copy_rows(pl.obs[z], idx, O, B, obs);
-  copy_rows(pl.act[z], idx, A, B, act);
-  copy_rows(pl.next_obs[z], last, O, B, nobs);
 }
 
 // One CTA per learner: the priority update of one step.  Row j (in row order; a later row on the same leaf wins) sets
@@ -1095,7 +1030,7 @@ __global__ void __launch_bounds__(GTHREADS) per_draw_nstep_kernel(const PerLanes
 // skipped, and a non-finite |delta| or priority leaves its leaf unchanged and is counted in *bad_out.  Then every
 // ancestor of a drawn leaf is recomputed, level by level.  newp [B] = the new priority of each row (NaN when skipped).
 template <bool LANES>
-__global__ void __launch_bounds__(GTHREADS) per_update_kernel(const PerLanes<LANES> pl, const long long* idx,
+__global__ void __launch_bounds__(GTHREADS) per_update_kernel(const ReplayLanes<LANES> pl, const long long* idx,
                                                              const float* absd, int B, float alpha, float eps,
                                                              float* newp, int* bad_out, size_t lane_stride) {
   __shared__ long long leaf_s[GTHREADS];
@@ -1171,6 +1106,20 @@ struct NetBuf {
   int w_off[B200RL_MAX_LAYERS], b_off[B200RL_MAX_LAYERS];
 };
 
+// What a captured step program holds in its nodes besides the engine's own buffers: a graph is replayed only for a call
+// with the same key.  Zero-initialised as a whole (compared with memcmp).  A prioritized call's nodes also hold alpha /
+// eps and the trees' and columns' addresses and row counts (and with n > 1 the episode-end columns its draw walks);
+// `per` and `replay` stay zero for every other call.
+struct GraphKey {
+  int S, B, nstep;
+  b200rl_offpolicy_hparams hp;
+  b200rl_sac_hparams sac;
+  b200rl_dqn_hparams dqn;
+  b200rl_c51_hparams c51;
+  b200rl_per_hparams per;
+  ReplayLanes<true> replay;
+};
+
 struct b200rl_offpolicy {
   b200rl_offpolicy_config cfg;
   // learners of the group (1 = a solo engine) and the byte distance between their arenas: every pointer below is
@@ -1206,13 +1155,13 @@ struct b200rl_offpolicy {
   cudaStream_t gs = nullptr;     // internal stream (the caller's may be the legacy default stream: not capturable)
   cudaEvent_t ev = nullptr;
   cudaGraphExec_t graph = nullptr;
-  b200rl_offpolicy_hparams graph_hp;
-  int graph_S = -1, graph_B = -1, graph_npol = 0, graph_launches = 0;
+  GraphKey graph_key;  // the call the graph was captured for
+  int graph_npol = 0, graph_launches = 0;
   float* state = nullptr;  // parameters + Adam state of every network, blob order (see b200rl_offpolicy_create)
   int64_t state_n = 0;
   // SAC (cfg.algo == 1): network 3 is absent; h->eps holds [S, 2, B, A] (the draw for s', then the one for s)
   bool sac = false, sac_set = false;
-  b200rl_sac_hparams sac_hp{}, graph_sac_hp{};
+  b200rl_sac_hparams sac_hp{};
   float *sac_act_next = nullptr, *sac_logp_next = nullptr;  // [B, A] / [B]: a' and log pi(a' | s')
   float *sac_act = nullptr, *sac_logp = nullptr;            // the same at s (the policy step)
   float* sac_dout = nullptr;                                // [B, 2A] gradient w.r.t. the policy output
@@ -1223,12 +1172,12 @@ struct b200rl_offpolicy {
   // DQN (cfg.algo == 2): networks 1 (Q) and 4 (target Q) only; the action column is 1 wide (the index as float32);
   // adam_tab row 3 holds the target-copy flags of the call's steps
   bool dqn = false, dqn_set = false;
-  b200rl_dqn_hparams dqn_hp{}, graph_dqn_hp{};
+  b200rl_dqn_hparams dqn_hp{};
   float* dqn_dout = nullptr;  // [B, n] gradient w.r.t. the Q output
   int* dqn_bad = nullptr;     // [max_steps] rows of each step whose action was not a valid index
   // C51 (cfg.algo == 3): a DQN engine (h->dqn is set) whose loss head is c51_loss_kernel
   bool c51 = false, c51_set = false;
-  b200rl_c51_hparams c51_hp{}, graph_c51_hp{};
+  b200rl_c51_hparams c51_hp{};
   float* c51_support = nullptr;   // [C51_MAX_ATOMS] z_0 .. z_{N-1}
   float* c51_row_loss = nullptr;  // [B] each row's cross-entropy of the current step
   int* c51_sync = nullptr;        // {CTAs done, invalid rows} of the current step; 0 between launches
@@ -1237,18 +1186,18 @@ struct b200rl_offpolicy {
   bool per_set = false, per_run = false;
   bool per_last = false;                       // the last call that ran steps was a prioritized one
   b200rl_per_hparams per_hp{};
-  PerLanes<true> per_lanes{};                  // this call's trees and columns (entry 0 for a solo engine)
-  std::vector<char> graph_per_key;             // per_run, per_hp and per_lanes of the cached graph
   float *per_w = nullptr, *per_newp = nullptr;  // [max_steps * B] importance weights / new priorities of each row
   float* per_absd = nullptr;                    // [B] |delta| of the current step
   int* per_bad = nullptr;                       // [max_steps] rows of each step whose new priority was not finite
   // n-step returns (DQN engines; b200rl_offpolicy_set_nstep): an n-step call stages R in rew, done[last] in done, and
   // each row's discount and last row beside them
-  int nstep = 1, graph_nstep = 1;
+  int nstep = 1;
   LaneSrc<true> nstep_ends{};         // each learner's episode-end column (n > 1)
   bool nstep_last = false;            // the last call that ran steps was an n-step one
   float* nstep_disc = nullptr;        // [max_steps * B] gamma^k of each row's window
   long long* nstep_rows = nullptr;    // [max_steps * B] the last row of each row's window
+  // the replay columns, episode-end columns, trees and row counts of this call (train_gather[_rng], train_prioritized)
+  ReplayLanes<true> replay{};
   std::vector<void*> allocs;
 };
 
@@ -1282,21 +1231,43 @@ inline dim3 lane_grid(dim3 g, int K) {
   return g;
 }
 
-// one launch for every learner: a solo engine runs kern<false> (the solo kernel), a group kern<true> over blockIdx.z
-#define LAUNCH_LANES(h, kern, grid, block, s, ...)                                                 \
-  do {                                                                                             \
-    if ((h)->K == 1) kern<false><<<(grid), (block), 0, (s)>>>(__VA_ARGS__, (size_t)0);             \
-    else kern<true><<<lane_grid((grid), (h)->K), (block), 0, (s)>>>(__VA_ARGS__, (h)->lane_stride); \
-  } while (0)
+// The LANES = false slice of a per-learner table: learner 0's entry, a solo engine's only one.  Every other kernel
+// argument is the same for both instantiations.
+template <typename T>
+const T& solo(const T& arg) { return arg; }
+LaneSrc<false> solo(const LaneSrc<true>& t) { return {{t.p[0]}}; }
+DrawKeys<false> solo(const DrawKeys<true>& k) {
+  return {{k.seed[0]}, {k.call[0]}, {k.start[0]}, {k.size[0]}, {k.capacity[0]}};
+}
+ReplayLanes<false> solo(const ReplayLanes<true>& r) {
+  return {solo(r.obs), solo(r.act), solo(r.rew), solo(r.next_obs), solo(r.done), solo(r.ends),
+          {r.tree[0]}, {r.rows[0]}};
+}
 
-template <int MODE>
-int gemm(const b200rl_offpolicy* h, const GemmArgs& g, cudaStream_t s) {
-  dim3 grid((g.N + GT - 1) / GT, (g.M + GT - 1) / GT);
-  if (h->K == 1) gemm_kernel<MODE, false><<<grid, GTHREADS, 0, s>>>(g, 0);
-  else gemm_kernel<MODE, true><<<lane_grid(grid, h->K), GTHREADS, 0, s>>>(g, h->lane_stride);
+// One launch for every learner: a solo engine runs the solo kernel kern<false> on `grid` with each table argument cut
+// to its solo slice, a group kern<true> over blockIdx.z = learner.  `args` are the kernel's arguments up to its lane
+// stride, tables in their LANES = true form.
+template <typename... Solo, typename... Lanes, typename... Args>
+int launch(const b200rl_offpolicy* h, void (*solo_kern)(Solo...), void (*lanes_kern)(Lanes...), dim3 grid, dim3 block,
+           size_t smem, cudaStream_t s, const Args&... args) {
+  if (h->K == 1) solo_kern<<<grid, block, smem, s>>>(solo(args)..., (size_t)0);
+  else lanes_kern<<<lane_grid(grid, h->K), block, smem, s>>>(args..., h->lane_stride);
   B200RL_CUDA(cudaGetLastError());
   count_launch(1);
   return 0;
+}
+
+// work queued on `to` from here on waits for everything queued on `from` so far (a graph edge under capture)
+int edge(const b200rl_offpolicy* h, cudaStream_t from, cudaStream_t to) {
+  B200RL_CUDA(cudaEventRecord(h->ev_fork, from));
+  B200RL_CUDA(cudaStreamWaitEvent(to, h->ev_fork, 0));
+  return 0;
+}
+
+template <int MODE>
+int gemm(const b200rl_offpolicy* h, const GemmArgs& g, cudaStream_t s) {
+  const dim3 grid((g.N + GT - 1) / GT, (g.M + GT - 1) / GT);
+  return launch(h, gemm_kernel<MODE, false>, gemm_kernel<MODE, true>, grid, GTHREADS, 0, s, g);
 }
 
 // forward through one network: acts[0] = input [rows, n0] (ld = n0); acts[l+1] = layer outputs.
@@ -1796,12 +1767,6 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
   const int Lq = q1.d.n_layers, Lp = pi.d.n_layers;
   const int ew = 256;
   cudaStream_t s2 = h->s2, s3 = h->s3, s4 = h->s4;
-  // work queued on `to` from here on waits for everything queued on `from` so far (a graph edge under capture)
-  auto edge = [&](cudaStream_t from, cudaStream_t to) -> int {
-    B200RL_CUDA(cudaEventRecord(h->ev_fork, from));
-    B200RL_CUDA(cudaStreamWaitEvent(to, h->ev_fork, 0));
-    return 0;
-  };
   int n_pol = 0;
   // A step is a dependency graph, not a sequence; the branches below are what the kernels actually need:
   //   s  : target policy -> Q1 target ---------+-> Q1 loss -> Q1 dX chain -----+-> Adam(Q1) -> [policy step] -> polyak
@@ -1821,7 +1786,7 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
       qa[qi][0] = const_cast<float*>(s_obs);
       for (int l = 1; l <= Lq; ++l) qa[qi][l] = h->acts[qi == 0 ? 1 : 4][l];
       cudaStream_t qs = qi == 0 ? s3 : s4;
-      if (edge(s, qs)) return 1;
+      if (edge(h, s, qs)) return 1;
       if (net_forward(h, qi == 0 ? q1 : q2, qa[qi], B, qs, s_act, A, O)) return 1;
     }
     // ---- targets (td3.py:325-341 / ddpg.py:275-282): the smoothing noise rides on the last layer's epilogue;
@@ -1836,7 +1801,7 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
     for (int l = 1; l < Lq; ++l) tq[l] = h->acts_tq[l];  // apart from the target policy's stack, whose output it reads
     tq[Lq] = h->qt1;
     if (td3) {
-      if (edge(s, s2)) return 1;
+      if (edge(h, s, s2)) return 1;
       float* tq2[B200RL_MAX_LAYERS + 1];
       tq2[0] = const_cast<float*>(s_nobs);
       for (int l = 1; l < Lq; ++l) tq2[l] = h->acts[3][l];
@@ -1844,26 +1809,25 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
       if (net_forward(h, q2t, tq2, B, s2, ta[Lp], A, O)) return 1;
     }
     if (net_forward(h, q1t, tq, B, s, ta[Lp], A, O)) return 1;
-    if (td3 && edge(s2, s)) return 1;  // both target values are complete on `s`
+    if (td3 && edge(h, s2, s)) return 1;  // both target values are complete on `s`
     // ---- Q steps (td3.py:343-358): TD target + MSE + dq in one kernel, backward, Adam ----
     if (td3) {
-      if (edge(s, s2)) return 1;   // the targets
-      if (edge(s4, s2)) return 1;  // Q2's forward pass
+      if (edge(h, s, s2)) return 1;   // the targets
+      if (edge(h, s4, s2)) return 1;  // Q2's forward pass
     }
-    if (edge(s3, s)) return 1;     // Q1's forward pass
+    if (edge(h, s3, s)) return 1;     // Q1's forward pass
     for (int qi = (td3 ? 1 : 0); qi >= 0; --qi) {
       NetBuf& qn = qi == 0 ? q1 : q2;
       cudaStream_t qs = qi == 0 ? s : s2;
       float* dq = qi == 0 ? h->dq : h->dq2;
-      LAUNCH_LANES(h, q_loss_kernel, 1, GTHREADS, qs, qa[qi][Lq], s_rew, s_done, h->qt1, td3 ? h->qt2 : nullptr,
-                   (float)hp->gamma, B, dq, (qi == 0 ? h->out_l1 : h->out_l2) + st,
-                   (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B);
-      B200RL_CUDA(cudaGetLastError());
-      count_launch(1);
+      if (launch(h, q_loss_kernel<false>, q_loss_kernel<true>, 1, GTHREADS, 0, qs, qa[qi][Lq], s_rew, s_done, h->qt1,
+                 td3 ? h->qt2 : nullptr, (float)hp->gamma, B, dq, (qi == 0 ? h->out_l1 : h->out_l2) + st,
+                 (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B))
+        return 1;
       if (net_backward(h, qn, qa[qi], dq, 1, B, true, nullptr, qs, qi != 0, s_act, A, O, qi == 0 ? s3 : s4)) return 1;
       if (adam_net(h, qn, h->adam_tab + (size_t)(1 + qi) * maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, qs)) return 1;
     }
-    if (td3 && edge(s2, s)) return 1;
+    if (td3 && edge(h, s2, s)) return 1;
     // ---- delayed policy step + polyak (td3.py:244-263, 301-323; ddpg: every step) ----
     if (st % hp->policy_delay == 0) {
       float* pa[B200RL_MAX_LAYERS + 1];
@@ -1874,10 +1838,9 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
       qp[0] = const_cast<float*>(s_obs);
       for (int l = 1; l <= Lq; ++l) qp[l] = h->acts[1][l];
       if (net_forward(h, q1, qp, B, s, pa[Lp], A, O)) return 1;  // Q1 with its freshly updated parameters (td3.py:309)
-      LAUNCH_LANES(h, q_loss_kernel, 1, GTHREADS, s, qp[Lq], nullptr, nullptr, nullptr, nullptr, 0.f, B, h->dq,
-                   h->out_lp + n_pol, nullptr);
-      B200RL_CUDA(cudaGetLastError());
-      count_launch(1);
+      if (launch(h, q_loss_kernel<false>, q_loss_kernel<true>, 1, GTHREADS, 0, s, qp[Lq], nullptr, nullptr, nullptr,
+                 nullptr, 0.f, B, h->dq, h->out_lp + n_pol, nullptr))
+        return 1;
       // gradient w.r.t. Q1's input; its action columns are the gradient w.r.t. pi(s) (Q parameters frozen)
       if (net_backward(h, q1, qp, h->dq, 1, B, false, h->x_cat, s)) return 1;
       if (net_backward(h, pi, pa, h->x_cat + O, O + A, B, true, nullptr, s, false, nullptr, 0, 0, s3)) return 1;
@@ -1891,10 +1854,9 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
         pk.n[k] = (int)h->net[k].P;
         nmax = pk.n[k] > nmax ? pk.n[k] : nmax;
       }
-      LAUNCH_LANES(h, polyak_kernel, (nmax + ew - 1) / ew, ew, s, pk, (float)hp->polyak_rho,
-                   (float)(1.0 - hp->polyak_rho));
-      B200RL_CUDA(cudaGetLastError());
-      count_launch(1);
+      if (launch(h, polyak_kernel<false>, polyak_kernel<true>, (nmax + ew - 1) / ew, ew, 0, s, pk,
+                 (float)hp->polyak_rho, (float)(1.0 - hp->polyak_rho)))
+        return 1;
       ++n_pol;
     }
   }
@@ -1919,19 +1881,9 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
   const float lmin = (float)sp.log_std_min, lmax = (float)sp.log_std_max, limit = (float)hp->action_limit;
   const int ew = 256, rows_grid = (B + 127) / 128;
   cudaStream_t s2 = h->s2, s3 = h->s3, s4 = h->s4;
-  auto edge = [&](cudaStream_t from, cudaStream_t to) -> int {
-    B200RL_CUDA(cudaEventRecord(h->ev_fork, from));
-    B200RL_CUDA(cudaStreamWaitEvent(to, h->ev_fork, 0));
-    return 0;
-  };
-  auto launched = [&]() -> int {
-    B200RL_CUDA(cudaGetLastError());
-    count_launch(1);
-    return 0;
-  };
-  LAUNCH_LANES(h, sac_alpha_init_kernel, (S + 1 + ew - 1) / ew, ew, s, h->sac_alpha, S + 1, h->sac_state,
-               sp.learn_alpha, (float)sp.alpha);
-  if (launched()) return 1;
+  if (launch(h, sac_alpha_init_kernel<false>, sac_alpha_init_kernel<true>, (S + 1 + ew - 1) / ew, ew, 0, s,
+             h->sac_alpha, S + 1, h->sac_state, sp.learn_alpha, (float)sp.alpha))
+    return 1;
   PolyakArgs pk{};  // 1 -> 4, 2 -> 5
   pk.n_nets = 2;
   for (int k = 0; k < 2; ++k) {
@@ -1954,93 +1906,94 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
       qa[qi][0] = const_cast<float*>(s_obs);
       for (int l = 1; l <= Lq; ++l) qa[qi][l] = h->acts[qi == 0 ? 1 : 4][l];
       cudaStream_t qs = qi == 0 ? s3 : s4;
-      if (edge(s, qs)) return 1;
+      if (edge(h, s, qs)) return 1;
       if (net_forward(h, qi == 0 ? q1 : q2, qa[qi], B, qs, s_act, A, O)) return 1;
     }
     float* pa[B200RL_MAX_LAYERS + 1];
     pa[0] = const_cast<float*>(s_obs);
     for (int l = 1; l <= Lp; ++l) pa[l] = h->acts[2][l];
     if (net_forward(h, pi, pa, B, s3)) return 1;
-    LAUNCH_LANES(h, sac_squash_kernel, rows_grid, 128, s3, pa[Lp], eps_cur, B, A, lmin, lmax, limit, h->sac_act,
-                 h->sac_logp);
-    if (launched()) return 1;
+    if (launch(h, sac_squash_kernel<false>, sac_squash_kernel<true>, rows_grid, 128, 0, s3, pa[Lp], eps_cur, B, A, lmin,
+               lmax, limit, h->sac_act, h->sac_logp))
+      return 1;
     // ---- soft targets: a', log pi' from the current policy at s'; the target critics read [s' | a'] in place ----
     float* ta[B200RL_MAX_LAYERS + 1];
     ta[0] = const_cast<float*>(s_nobs);
     for (int l = 1; l <= Lp; ++l) ta[l] = h->acts[0][l];
     if (net_forward(h, pi, ta, B, s)) return 1;
-    LAUNCH_LANES(h, sac_squash_kernel, rows_grid, 128, s, ta[Lp], eps_next, B, A, lmin, lmax, limit, h->sac_act_next,
-                 h->sac_logp_next);
-    if (launched()) return 1;
+    if (launch(h, sac_squash_kernel<false>, sac_squash_kernel<true>, rows_grid, 128, 0, s, ta[Lp], eps_next, B, A, lmin,
+               lmax, limit, h->sac_act_next, h->sac_logp_next))
+      return 1;
     float* tq[2][B200RL_MAX_LAYERS + 1];
     for (int qi = 0; qi < 2; ++qi) {
       tq[qi][0] = const_cast<float*>(s_nobs);
       for (int l = 1; l < Lq; ++l) tq[qi][l] = qi == 0 ? h->acts_tq[l] : h->acts[3][l];
       tq[qi][Lq] = qi == 0 ? h->qt1 : h->qt2;
     }
-    if (edge(s, s2)) return 1;
+    if (edge(h, s, s2)) return 1;
     if (net_forward(h, q2t, tq[1], B, s2, h->sac_act_next, A, O)) return 1;
     if (net_forward(h, q1t, tq[0], B, s, h->sac_act_next, A, O)) return 1;
-    if (edge(s2, s)) return 1;
+    if (edge(h, s2, s)) return 1;
     // ---- critic step: soft TD target + MSE + dq, backward, Adam (Q2 on s2, Q1 on s) ----
-    if (edge(s, s2)) return 1;
-    if (edge(s4, s2)) return 1;
-    if (edge(s3, s)) return 1;
+    if (edge(h, s, s2)) return 1;
+    if (edge(h, s4, s2)) return 1;
+    if (edge(h, s3, s)) return 1;
     for (int qi = 1; qi >= 0; --qi) {
       NetBuf& qn = qi == 0 ? q1 : q2;
       cudaStream_t qs = qi == 0 ? s : s2;
       float* dq = qi == 0 ? h->dq : h->dq2;
-      LAUNCH_LANES(h, sac_q_loss_kernel, 1, GTHREADS, qs, qa[qi][Lq], s_rew, s_done, h->qt1, h->qt2, h->sac_logp_next,
-                   alpha, (float)hp->gamma, B, dq, (qi == 0 ? h->out_l1 : h->out_l2) + st,
-                   (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B);
-      if (launched()) return 1;
+      if (launch(h, sac_q_loss_kernel<false>, sac_q_loss_kernel<true>, 1, GTHREADS, 0, qs, qa[qi][Lq], s_rew, s_done,
+                 h->qt1, h->qt2, h->sac_logp_next, alpha, (float)hp->gamma, B, dq,
+                 (qi == 0 ? h->out_l1 : h->out_l2) + st, (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B))
+        return 1;
       if (net_backward(h, qn, qa[qi], dq, 1, B, true, nullptr, qs, qi != 0, s_act, A, O, qi == 0 ? s3 : s4)) return 1;
       if (adam_net(h, qn, h->adam_tab + (size_t)(1 + qi) * maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, qs)) return 1;
     }
-    if (edge(s2, s)) return 1;
+    if (edge(h, s2, s)) return 1;
     // ---- polyak beside the policy step: the targets are next read by the next step ----
-    if (edge(s, s4)) return 1;
-    LAUNCH_LANES(h, polyak_kernel, (pk.n[0] + ew - 1) / ew, ew, s4, pk, (float)hp->polyak_rho,
-                 (float)(1.0 - hp->polyak_rho));
-    if (launched()) return 1;
+    if (edge(h, s, s4)) return 1;
+    if (launch(h, polyak_kernel<false>, polyak_kernel<true>, (pk.n[0] + ew - 1) / ew, ew, 0, s4, pk,
+               (float)hp->polyak_rho, (float)(1.0 - hp->polyak_rho)))
+      return 1;
     // ---- policy step: both updated critics on [s | a_pi], differentiated w.r.t. their input only ----
     float* qp[2][B200RL_MAX_LAYERS + 1];
     for (int qi = 0; qi < 2; ++qi) {
       qp[qi][0] = const_cast<float*>(s_obs);
       for (int l = 1; l <= Lq; ++l) qp[qi][l] = h->acts[qi == 0 ? 1 : 4][l];
     }
-    if (edge(s, s2)) return 1;
+    if (edge(h, s, s2)) return 1;
     if (net_forward(h, q2, qp[1], B, s2, h->sac_act, A, O)) return 1;
     if (net_forward(h, q1, qp[0], B, s, h->sac_act, A, O)) return 1;
-    if (edge(s2, s)) return 1;
-    LAUNCH_LANES(h, sac_policy_loss_kernel, 1, GTHREADS, s, qp[0][Lq], qp[1][Lq], h->sac_logp, alpha, B, h->dq, h->dq2,
-                 h->out_lp + st, h->out_logp + st);
-    if (launched()) return 1;
-    if (edge(s, s2)) return 1;
+    if (edge(h, s2, s)) return 1;
+    if (launch(h, sac_policy_loss_kernel<false>, sac_policy_loss_kernel<true>, 1, GTHREADS, 0, s, qp[0][Lq], qp[1][Lq],
+               h->sac_logp, alpha, B, h->dq, h->dq2, h->out_lp + st, h->out_logp + st))
+      return 1;
+    if (edge(h, s, s2)) return 1;
     if (net_backward(h, q2, qp[1], h->dq2, 1, B, false, h->x_cat2, s2, true)) return 1;
     if (sp.learn_alpha) {  // -mean(log_alpha (log pi + target_entropy)), one Adam step; alpha[st + 1] = exp(log_alpha)
-      LAUNCH_LANES(h, sac_alpha_step_kernel, 1, GTHREADS, s2, h->sac_logp, B, (float)sp.target_entropy, h->sac_state,
-                   h->adam_tab + (size_t)3 * maxS, st, (float)(1.0 - sp.alpha_beta1), (float)sp.alpha_beta2,
-                   (float)(1.0 - sp.alpha_beta2), (float)sp.alpha_eps, h->sac_alpha + st + 1);
-      if (launched()) return 1;
+      if (launch(h, sac_alpha_step_kernel<false>, sac_alpha_step_kernel<true>, 1, GTHREADS, 0, s2, h->sac_logp, B,
+                 (float)sp.target_entropy, h->sac_state, h->adam_tab + (size_t)3 * maxS, st,
+                 (float)(1.0 - sp.alpha_beta1), (float)sp.alpha_beta2, (float)(1.0 - sp.alpha_beta2),
+                 (float)sp.alpha_eps, h->sac_alpha + st + 1))
+        return 1;
     }
     if (net_backward(h, q1, qp[0], h->dq, 1, B, false, h->x_cat, s)) return 1;
-    if (edge(s2, s)) return 1;
-    LAUNCH_LANES(h, sac_squash_backward_kernel, (B * A + ew - 1) / ew, ew, s, pa[Lp], eps_cur, h->x_cat + O,
-                 h->x_cat2 + O, O + A, B, A, lmin, lmax, limit, alpha, h->sac_dout);
-    if (launched()) return 1;
+    if (edge(h, s2, s)) return 1;
+    if (launch(h, sac_squash_backward_kernel<false>, sac_squash_backward_kernel<true>, (B * A + ew - 1) / ew, ew, 0, s,
+               pa[Lp], eps_cur, h->x_cat + O, h->x_cat2 + O, O + A, B, A, lmin, lmax, limit, alpha, h->sac_dout))
+      return 1;
     if (net_backward(h, pi, pa, h->sac_dout, 2 * A, B, true, nullptr, s, false, nullptr, 0, 0, s3)) return 1;
     if (adam_net(h, pi, h->adam_tab, st, hp->policy_beta1, hp->policy_beta2, hp->policy_eps, s)) return 1;
-    if (edge(s4, s)) return 1;
+    if (edge(h, s4, s)) return 1;
   }
   return 0;
 }
 
-static PerLanes<false> per_solo(const PerLanes<true>& l) {
-  PerLanes<false> s;
-  s.tree[0] = l.tree[0], s.rows[0] = l.rows[0];
-  s.obs[0] = l.obs[0], s.act[0] = l.act[0], s.rew[0] = l.rew[0], s.next_obs[0] = l.next_obs[0], s.done[0] = l.done[0];
-  return s;
+// dqn_loss_kernel<LANES, WEIGHTED, NSTEP> of a call: WEIGHTED for prioritized replay, NSTEP for n-step returns
+template <bool LANES>
+static auto dqn_head(bool weighted, bool nstep) {
+  return weighted ? (nstep ? dqn_loss_kernel<LANES, true, true> : dqn_loss_kernel<LANES, true, false>)
+                  : (nstep ? dqn_loss_kernel<LANES, false, true> : dqn_loss_kernel<LANES, false, false>);
 }
 
 // The S DQN steps.  Per step:
@@ -2059,162 +2012,87 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
   const int L = q.d.n_layers, n = q.d.sizes[L];
   const int ew = 256;
   cudaStream_t s2 = h->s2, s3 = h->s3, s4 = h->s4;
-  auto edge = [&](cudaStream_t from, cudaStream_t to) -> int {
-    B200RL_CUDA(cudaEventRecord(h->ev_fork, from));
-    B200RL_CUDA(cudaStreamWaitEvent(to, h->ev_fork, 0));
-    return 0;
-  };
   const bool per = h->per_run;
   const bool nstep = h->nstep > 1;  // the loss heads read each row's staged discount
   const float2* betas = h->adam_tab + (size_t)3 * maxS;
   const unsigned long long* keys = reinterpret_cast<const unsigned long long*>(h->adam_tab + (size_t)4 * maxS);
   const float alpha = (float)h->per_hp.alpha, eps = (float)h->per_hp.eps;
-  const dim3 lanes = lane_grid(dim3(1), h->K);
   for (int st = 0; st < S; ++st) {
+    float* s_obs = h->obs + (size_t)st * B * O;
+    float* s_act = h->act + (size_t)st * B;
+    float* s_rew = h->rew + (size_t)st * B;
+    float* s_nobs = h->nobs + (size_t)st * B * O;
+    float* s_done = h->done + (size_t)st * B;
+    float* s_disc = h->nstep_disc + (size_t)st * B;
+    long long* s_idx = h->idx + (size_t)st * B;
+    float* s_w = h->per_w + (size_t)st * B;
     if (per) {
-      if (st > 0 && edge(s4, s)) return 1;  // the previous step's priorities are in the tree
-      long long* s_idx = h->idx + (size_t)st * B;
-      float* s_w = h->per_w + (size_t)st * B;
-      float* dst[5] = {h->obs + (size_t)st * B * O, h->act + (size_t)st * B, h->rew + (size_t)st * B,
-                       h->nobs + (size_t)st * B * O, h->done + (size_t)st * B};
-      float* s_disc = h->nstep_disc + (size_t)st * B;
-      long long* s_last = h->nstep_rows + (size_t)st * B;
-      const float g = (float)hp->gamma;
-      if (nstep && h->K == 1)
-        per_draw_nstep_kernel<false><<<1, GTHREADS, 0, s>>>(per_solo(h->per_lanes), LaneSrc<false>{{h->nstep_ends.p[0]}},
-                                                             betas, keys, st, B, O, 1, h->nstep, g, s_idx, s_w, dst[0],
-                                                             dst[1], dst[2], dst[3], dst[4], s_disc, s_last, 0);
-      else if (nstep)
-        per_draw_nstep_kernel<true><<<lanes, GTHREADS, 0, s>>>(h->per_lanes, h->nstep_ends, betas, keys, st, B, O, 1,
-                                                              h->nstep, g, s_idx, s_w, dst[0], dst[1], dst[2], dst[3],
-                                                              dst[4], s_disc, s_last, h->lane_stride);
-      else if (h->K == 1)
-        per_draw_kernel<false><<<1, GTHREADS, 0, s>>>(per_solo(h->per_lanes), betas, keys, st, B, O, 1, s_idx, s_w,
-                                                       dst[0], dst[1], dst[2], dst[3], dst[4], 0);
-      else
-        per_draw_kernel<true><<<lanes, GTHREADS, 0, s>>>(h->per_lanes, betas, keys, st, B, O, 1, s_idx, s_w, dst[0],
-                                                        dst[1], dst[2], dst[3], dst[4], h->lane_stride);
-      B200RL_CUDA(cudaGetLastError());
-      count_launch(1);
+      if (st > 0 && edge(h, s4, s)) return 1;  // the previous step's priorities are in the tree
+      if (launch(h, nstep ? per_draw_kernel<false, true> : per_draw_kernel<false, false>,
+                 nstep ? per_draw_kernel<true, true> : per_draw_kernel<true, false>, 1, GTHREADS, 0, s, h->replay,
+                 betas, keys, st, B, O, 1, h->nstep, (float)hp->gamma, s_idx, s_w, s_obs, s_act, s_rew, s_nobs, s_done,
+                 s_disc, h->nstep_rows + (size_t)st * B))
+        return 1;
     }
-    const float* s_obs = h->obs + (size_t)st * B * O;
-    const float* s_act = h->act + (size_t)st * B;
-    const float* s_rew = h->rew + (size_t)st * B;
-    const float* s_nobs = h->nobs + (size_t)st * B * O;
-    const float* s_done = h->done + (size_t)st * B;
     float* qa[B200RL_MAX_LAYERS + 1];  // Q(s): its stack is what the backward pass reads
-    qa[0] = const_cast<float*>(s_obs);
+    qa[0] = s_obs;
     for (int l = 1; l <= L; ++l) qa[l] = h->acts[1][l];
-    if (edge(s, s3)) return 1;
+    if (edge(h, s, s3)) return 1;
     if (net_forward(h, q, qa, B, s3)) return 1;
     float* qn[B200RL_MAX_LAYERS + 1];
     if (dbl) {
-      qn[0] = const_cast<float*>(s_nobs);
+      qn[0] = s_nobs;
       for (int l = 1; l <= L; ++l) qn[l] = h->acts[3][l];
-      if (edge(s, s2)) return 1;
+      if (edge(h, s, s2)) return 1;
       if (net_forward(h, q, qn, B, s2)) return 1;
     }
     float* tq[B200RL_MAX_LAYERS + 1];
-    tq[0] = const_cast<float*>(s_nobs);
+    tq[0] = s_nobs;
     for (int l = 1; l <= L; ++l) tq[l] = h->acts_tq[l];
     if (net_forward(h, qt, tq, B, s)) return 1;
-    if (dbl && edge(s2, s)) return 1;
-    if (edge(s3, s)) return 1;
-    const float* s_disc = h->nstep_disc + (size_t)st * B;
-    if (per) {
-      if (nstep && h->K == 1)
-        dqn_nstep_loss_kernel<false, true><<<1, GTHREADS, 0, s>>>(
-            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, B, n, h->dqn_dout, h->out_l1 + st,
-            h->out_q1 + (size_t)st * B, h->dqn_bad + st, h->per_w + (size_t)st * B, h->per_absd, 0);
-      else if (nstep)
-        dqn_nstep_loss_kernel<true, true><<<lanes, GTHREADS, 0, s>>>(
-            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, B, n, h->dqn_dout, h->out_l1 + st,
-            h->out_q1 + (size_t)st * B, h->dqn_bad + st, h->per_w + (size_t)st * B, h->per_absd, h->lane_stride);
-      else
-        LAUNCH_LANES(h, dqn_per_loss_kernel, 1, GTHREADS, s, qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done,
-                     (float)hp->gamma, B, n, h->dqn_dout, h->out_l1 + st, h->out_q1 + (size_t)st * B, h->dqn_bad + st,
-                     h->per_w + (size_t)st * B, h->per_absd);
-      B200RL_CUDA(cudaGetLastError());
-      count_launch(1);
-      if (edge(s, s4)) return 1;
-      const long long* s_idx = h->idx + (size_t)st * B;
-      float* s_newp = h->per_newp + (size_t)st * B;
-      if (h->K == 1)
-        per_update_kernel<false><<<1, GTHREADS, 0, s4>>>(per_solo(h->per_lanes), s_idx, h->per_absd, B, alpha, eps,
-                                                         s_newp, h->per_bad + st, 0);
-      else
-        per_update_kernel<true><<<lanes, GTHREADS, 0, s4>>>(h->per_lanes, s_idx, h->per_absd, B, alpha, eps, s_newp,
-                                                           h->per_bad + st, h->lane_stride);
-      B200RL_CUDA(cudaGetLastError());
-      count_launch(1);
-    } else if (h->c51) {
+    if (dbl && edge(h, s2, s)) return 1;
+    if (edge(h, s3, s)) return 1;
+    if (h->c51) {
       const int N = h->c51_hp.n_atoms, W = c51_warps(n / N, N);
-      const dim3 grid((unsigned)((B + W - 1) / W), 1, (unsigned)h->K);
       const size_t smem = sizeof(float) * (size_t)(N + W * (3 * N + n / N));
       const float vmin = (float)h->c51_hp.v_min, vmax = (float)h->c51_hp.v_max;
       const float dz = (float)((h->c51_hp.v_max - h->c51_hp.v_min) / (N - 1));
-      if (nstep && h->K == 1)
-        c51_nstep_loss_kernel<false><<<grid, W * 32, smem, s>>>(
-            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, h->c51_support, vmin, vmax, dz, B,
-            n / N, N, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync, h->out_l1 + st,
-            h->dqn_bad + st, 0);
-      else if (nstep)
-        c51_nstep_loss_kernel<true><<<grid, W * 32, smem, s>>>(
-            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, h->c51_support, vmin, vmax, dz, B,
-            n / N, N, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync, h->out_l1 + st,
-            h->dqn_bad + st, h->lane_stride);
-      else if (h->K == 1)
-        c51_loss_kernel<false><<<grid, W * 32, smem, s>>>(
-            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, h->c51_support, (float)hp->gamma, vmin, vmax,
-            dz, B, n / N, N, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync, h->out_l1 + st,
-            h->dqn_bad + st, 0);
-      else
-        c51_loss_kernel<true><<<grid, W * 32, smem, s>>>(
-            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, h->c51_support, (float)hp->gamma, vmin, vmax,
-            dz, B, n / N, N, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync, h->out_l1 + st,
-            h->dqn_bad + st, h->lane_stride);
-      B200RL_CUDA(cudaGetLastError());
-      count_launch(1);
-    } else {
-      if (nstep && h->K == 1)
-        dqn_nstep_loss_kernel<false, false><<<1, GTHREADS, 0, s>>>(
-            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, B, n, h->dqn_dout, h->out_l1 + st,
-            h->out_q1 + (size_t)st * B, h->dqn_bad + st, nullptr, nullptr, 0);
-      else if (nstep)
-        dqn_nstep_loss_kernel<true, false><<<lanes, GTHREADS, 0, s>>>(
-            qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, B, n, h->dqn_dout, h->out_l1 + st,
-            h->out_q1 + (size_t)st * B, h->dqn_bad + st, nullptr, nullptr, h->lane_stride);
-      else
-        LAUNCH_LANES(h, dqn_loss_kernel, 1, GTHREADS, s, qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done,
-                     (float)hp->gamma, B, n, h->dqn_dout, h->out_l1 + st, h->out_q1 + (size_t)st * B, h->dqn_bad + st);
-      B200RL_CUDA(cudaGetLastError());
-      count_launch(1);
+      if (launch(h, nstep ? c51_loss_kernel<false, true> : c51_loss_kernel<false, false>,
+                 nstep ? c51_loss_kernel<true, true> : c51_loss_kernel<true, false>, (B + W - 1) / W, W * 32, smem, s,
+                 qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, h->c51_support, (float)hp->gamma,
+                 vmin, vmax, dz, B, n / N, N, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync,
+                 h->out_l1 + st, h->dqn_bad + st))
+        return 1;
+    } else if (launch(h, dqn_head<false>(per, nstep), dqn_head<true>(per, nstep), 1, GTHREADS, 0, s, qa[L], tq[L],
+                      dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, (float)hp->gamma, B, n, h->dqn_dout,
+                      h->out_l1 + st, h->out_q1 + (size_t)st * B, h->dqn_bad + st, s_w, h->per_absd)) {
+      return 1;
+    }
+    if (per) {
+      if (edge(h, s, s4)) return 1;
+      if (launch(h, per_update_kernel<false>, per_update_kernel<true>, 1, GTHREADS, 0, s4, h->replay, s_idx,
+                 h->per_absd, B, alpha, eps, h->per_newp + (size_t)st * B, h->per_bad + st))
+        return 1;
     }
     if (net_backward(h, q, qa, h->dqn_dout, n, B, true, nullptr, s, false, nullptr, 0, 0, s3)) return 1;
     if (adam_net(h, q, h->adam_tab + (size_t)maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, s)) return 1;
-    LAUNCH_LANES(h, dqn_target_copy_kernel, (unsigned)((q.P + ew - 1) / ew), ew, s, qt.params, q.params, (int)q.P,
-                 h->adam_tab + (size_t)3 * maxS, st);
-    B200RL_CUDA(cudaGetLastError());
-    count_launch(1);
+    if (launch(h, dqn_target_copy_kernel<false>, dqn_target_copy_kernel<true>, (unsigned)((q.P + ew - 1) / ew), ew, 0,
+               s, qt.params, q.params, (int)q.P, h->adam_tab + (size_t)3 * maxS, st))
+      return 1;
   }
-  if (per && edge(s4, s)) return 1;
+  if (per && edge(h, s4, s)) return 1;
   return 0;
 }
 
-// DQN engines: b200rl_offpolicy_set_dqn must have been called
-static int dqn_ready(const b200rl_offpolicy* h, const char* what) {
-  if (!h->dqn) return 0;
-  B200RL_REQUIRE(h->dqn_set, "%s: a DQN engine needs b200rl_offpolicy_set_dqn before it trains", what);
-  B200RL_REQUIRE(!h->c51 || h->c51_set, "%s: a C51 engine needs b200rl_offpolicy_set_c51 before it trains", what);
-  return 0;
-}
-
-// SAC engines: b200rl_offpolicy_set_sac must have been called, and the host paths must hand over the [S, 2, B, A] draws
-static int sac_ready(const b200rl_offpolicy* h, bool noise_given, const char* what) {
-  if (!h->sac) return 0;
-  B200RL_REQUIRE(h->sac_set, "%s: a SAC engine needs b200rl_offpolicy_set_sac before it trains", what);
-  B200RL_REQUIRE(noise_given, "%s: SAC needs the noise draws [S, 2, B, A]", what);
-  return 0;
+// The step program of the engine's algorithm on `s` (plain launches or under stream capture); *n_pol = its policy steps
+static int enqueue_program(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s,
+                           int* n_pol) {
+  if (h->sac) {
+    *n_pol = S;
+    return enqueue_sac_steps(h, hp, S, B, s);
+  }
+  if (h->dqn) return enqueue_dqn_steps(h, hp, S, B, s);
+  return enqueue_steps(h, hp, S, B, s, n_pol);
 }
 
 // Runs the S steps on minibatches ALREADY staged in h->obs ... h->eps (stream h->gs) and reads the logs back.
@@ -2262,46 +2140,21 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   const char* genv = getenv("B200RL_OFFPOLICY_GRAPH");
   const bool use_graph = !(genv != nullptr && genv[0] == '0');
   if (!use_graph) {
-    if (h->sac) {
-      if (enqueue_sac_steps(h, hp, S, B, s)) return 1;
-      n_pol = S;
-    } else if (h->dqn) {
-      if (enqueue_dqn_steps(h, hp, S, B, s)) return 1;
-    } else if (enqueue_steps(h, hp, S, B, s, &n_pol)) {
-      return 1;
-    }
+    if (enqueue_program(h, hp, S, B, s, &n_pol)) return 1;
   } else {
-    // a prioritized graph holds the trees' and the columns' addresses, the row counts and alpha / eps in its nodes,
-    // and an n-step one the episode-end columns too (its draw kernel walks them)
-    std::vector<char> per_key;
-    if (h->per_run) {
-      const char* a = reinterpret_cast<const char*>(&h->per_hp);
-      const char* b = reinterpret_cast<const char*>(&h->per_lanes);
-      const char* c = reinterpret_cast<const char*>(&h->nstep_ends);
-      per_key.assign(a, a + sizeof(h->per_hp));
-      per_key.insert(per_key.end(), b, b + sizeof(h->per_lanes));
-      per_key.insert(per_key.end(), c, c + sizeof(h->nstep_ends));
-    }
-    if (h->graph == nullptr || h->graph_S != S || h->graph_B != B || memcmp(&h->graph_hp, hp, sizeof(*hp)) != 0 ||
-        memcmp(&h->graph_sac_hp, &h->sac_hp, sizeof(h->sac_hp)) != 0 ||
-        memcmp(&h->graph_dqn_hp, &h->dqn_hp, sizeof(h->dqn_hp)) != 0 ||
-        memcmp(&h->graph_c51_hp, &h->c51_hp, sizeof(h->c51_hp)) != 0 || h->graph_per_key != per_key ||
-        h->graph_nstep != h->nstep) {
+    GraphKey key;
+    memset(&key, 0, sizeof(key));
+    key.S = S, key.B = B, key.nstep = h->nstep;
+    key.hp = *hp, key.sac = h->sac_hp, key.dqn = h->dqn_hp, key.c51 = h->c51_hp;
+    if (h->per_run) key.per = h->per_hp, key.replay = h->replay;
+    if (h->graph == nullptr || memcmp(&key, &h->graph_key, sizeof(key)) != 0) {
       if (h->graph) {
         cudaGraphExecDestroy(h->graph);
         h->graph = nullptr;
       }
       const int64_t l0 = launches_total();
       B200RL_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-      int rc;
-      if (h->sac) {
-        rc = enqueue_sac_steps(h, hp, S, B, s);
-        n_pol = S;
-      } else if (h->dqn) {
-        rc = enqueue_dqn_steps(h, hp, S, B, s);
-      } else {
-        rc = enqueue_steps(h, hp, S, B, s, &n_pol);
-      }
+      const int rc = enqueue_program(h, hp, S, B, s, &n_pol);
       cudaGraph_t g = nullptr;
       const cudaError_t ce = cudaStreamEndCapture(s, &g);
       if (rc || ce != cudaSuccess || g == nullptr) {
@@ -2318,14 +2171,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
       }
       h->graph_launches = (int)(launches_total() - l0);
       count_launch(-h->graph_launches);  // counted per replay below
-      h->graph_S = S;
-      h->graph_B = B;
-      h->graph_hp = *hp;
-      h->graph_sac_hp = h->sac_hp;
-      h->graph_dqn_hp = h->dqn_hp;
-      h->graph_c51_hp = h->c51_hp;
-      h->graph_per_key = per_key;
-      h->graph_nstep = h->nstep;
+      h->graph_key = key;
       h->graph_npol = n_pol;
     }
     n_pol = h->graph_npol;
@@ -2368,6 +2214,33 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   return 0;
 }
 
+// The front matter of every train call after its NULL checks: the checks all calls share, then `own` (the call's own
+// checks), then -1 for S = 0 (nothing to run) or the engine's stream joined to the caller's `stream`.  noise_given: the
+// call hands over (or draws) the noise its engine needs.
+template <typename Own>
+static int train_begin(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int32_t S, int32_t B, bool noise_given,
+                       bool q2_given, int32_t* n_policy_updates, void* stream, const char* what, Own own) {
+  B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
+                 "%s: S=%d B=%d exceed the capacities", what, S, B);
+  B200RL_REQUIRE(h->cfg.n_q != 2 || q2_given, "%s: TD3 needs the Q2 outputs", what);
+  B200RL_REQUIRE(h->dqn || !hp->use_target_noise || noise_given, "%s: target noise requested but no noise given", what);
+  B200RL_REQUIRE(h->dqn || hp->policy_delay >= 1, "%s: policy_delay must be >= 1", what);
+  if (h->sac) {
+    B200RL_REQUIRE(h->sac_set, "%s: a SAC engine needs b200rl_offpolicy_set_sac before it trains", what);
+    B200RL_REQUIRE(noise_given, "%s: SAC needs the noise draws [S, 2, B, A]", what);
+  }
+  if (h->dqn) {
+    B200RL_REQUIRE(h->dqn_set, "%s: a DQN engine needs b200rl_offpolicy_set_dqn before it trains", what);
+    B200RL_REQUIRE(!h->c51 || h->c51_set, "%s: a C51 engine needs b200rl_offpolicy_set_c51 before it trains", what);
+  }
+  if (int rc = own()) return rc;
+  *n_policy_updates = 0;
+  if (S == 0) return -1;
+  B200RL_CUDA(cudaEventRecord(h->ev, static_cast<cudaStream_t>(stream)));
+  B200RL_CUDA(cudaStreamWaitEvent(h->gs, h->ev, 0));
+  return 0;
+}
+
 extern "C" int b200rl_offpolicy_train(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int32_t S, int32_t B,
                                       const float* obs, const float* act, const float* rew, const float* next_obs,
                                       const float* done, const float* noise, float* q1_values, float* q2_values,
@@ -2375,23 +2248,17 @@ extern "C" int b200rl_offpolicy_train(b200rl_offpolicy* h, const b200rl_offpolic
                                       int32_t* n_policy_updates, void* stream) {
   B200RL_REQUIRE(h && hp && obs && act && rew && next_obs && done && q1_values && q1_losses &&
                      (policy_losses || h->dqn) && n_policy_updates, "offpolicy_train: NULL argument");
-  B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
-                 "offpolicy_train: S=%d B=%d exceed the capacities", S, B);
-  const bool td3 = h->cfg.n_q == 2;
-  B200RL_REQUIRE(!td3 || (q2_values && q2_losses), "offpolicy_train: TD3 needs the Q2 outputs");
-  B200RL_REQUIRE(h->dqn || !hp->use_target_noise || noise, "offpolicy_train: target noise requested but no noise given");
-  B200RL_REQUIRE(h->dqn || hp->policy_delay >= 1, "offpolicy_train: policy_delay must be >= 1");
-  if (sac_ready(h, noise != nullptr, "offpolicy_train") || dqn_ready(h, "offpolicy_train")) return 2;
-  B200RL_REQUIRE(h->nstep == 1, "offpolicy_train: n-step returns (n_step = %d) need the device replay columns: use "
-                 "train_gather, train_gather_rng or train_prioritized", h->nstep);
-  cudaStream_t user = static_cast<cudaStream_t>(stream);
+  const auto own = [&] {
+    B200RL_REQUIRE(h->nstep == 1, "offpolicy_train: n-step returns (n_step = %d) need the device replay columns: use "
+                   "train_gather, train_gather_rng or train_prioritized", h->nstep);
+    return 0;
+  };
+  if (int rc = train_begin(h, hp, S, B, noise != nullptr, q2_values && q2_losses, n_policy_updates, stream,
+                           "offpolicy_train", own))
+    return rc < 0 ? 0 : rc;
   cudaStream_t s = h->gs;  // everything runs on the engine's stream, ordered after the caller's
   const int O = h->O, A = h->A;
   const size_t SB = (size_t)S * B;
-  *n_policy_updates = 0;
-  if (S == 0) return 0;
-  B200RL_CUDA(cudaEventRecord(h->ev, user));
-  B200RL_CUDA(cudaStreamWaitEvent(s, h->ev, 0));
   // one host -> device upload of every minibatch of this train() call ([K, S, B, ...] into the K arenas)
   auto up = [&](void* dst, const void* src, size_t bytes) -> int {
     B200RL_CUDA(cudaMemcpy2DAsync(dst, h->lane_stride, src, bytes, bytes, h->K, cudaMemcpyHostToDevice, s));
@@ -2406,53 +2273,37 @@ extern "C" int b200rl_offpolicy_train(b200rl_offpolicy* h, const b200rl_offpolic
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
 }
 
-// The five staged columns (obs, act, rew, next_obs, done) gathered from each learner's replay columns at the rows in
-// h->idx: one launch per column for all learners; with n-step returns one nstep_gather_kernel launch, which also stages
-// the discounts and last rows
-static int gather_columns(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, const b200rl_offpolicy_replay* rb,
-                          long long SB, cudaStream_t s) {
+// The five staged columns (obs, act, rew, next_obs, done) gathered from the call's replay table at the rows in h->idx:
+// one launch per column for all learners; with n-step returns one nstep_gather_kernel launch, which also stages the
+// discounts and last rows
+static int gather_columns(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, long long SB, cudaStream_t s) {
   const int O = h->O, A = h->A;
-  if (h->nstep > 1) {
-    NStepSrc<true> src{};
-    for (int z = 0; z < h->K; ++z)
-      src.obs[z] = rb[z].obs, src.act[z] = rb[z].act, src.rew[z] = rb[z].rew, src.next_obs[z] = rb[z].next_obs,
-      src.done[z] = rb[z].done, src.ends[z] = h->nstep_ends.p[z], src.rows[z] = rb[z].rows;
-    const dim3 grid((unsigned)((SB + GTHREADS - 1) / GTHREADS));
-    const float g = (float)hp->gamma;
-    if (h->K == 1) {
-      const NStepSrc<false> one = {{src.obs[0]}, {src.act[0]}, {src.rew[0]}, {src.next_obs[0]}, {src.done[0]},
-                                   {src.ends[0]}, {src.rows[0]}};
-      nstep_gather_kernel<false><<<grid, GTHREADS, 0, s>>>(one, h->idx, SB, O, A, h->nstep, g, h->obs, h->act, h->rew,
-                                                           h->nobs, h->done, h->nstep_disc, h->nstep_rows, 0);
-    } else {
-      nstep_gather_kernel<true><<<lane_grid(grid, h->K), GTHREADS, 0, s>>>(src, h->idx, SB, O, A, h->nstep, g, h->obs,
-                                                                           h->act, h->rew, h->nobs, h->done,
-                                                                           h->nstep_disc, h->nstep_rows, h->lane_stride);
-    }
-    B200RL_CUDA(cudaGetLastError());
-    count_launch(1);
-    return 0;
-  }
+  const ReplayLanes<true>& r = h->replay;
+  if (h->nstep > 1)
+    return launch(h, nstep_gather_kernel<false>, nstep_gather_kernel<true>, (unsigned)((SB + GTHREADS - 1) / GTHREADS),
+                  GTHREADS, 0, s, r, h->idx, SB, O, A, h->nstep, (float)hp->gamma, h->obs, h->act, h->rew, h->nobs,
+                  h->done, h->nstep_disc, h->nstep_rows);
+  const LaneSrc<true>* src[5] = {&r.obs, &r.act, &r.rew, &r.next_obs, &r.done};
   float* dst[5] = {h->obs, h->act, h->rew, h->nobs, h->done};
   const int w[5] = {O, A, 1, O, 1};
-  for (int c = 0; c < 5; ++c) {
-    const long long n = SB * w[c];
-    const dim3 grid((unsigned)((n + 255) / 256));
-    auto col = [&](int z) {
-      const float* p[5] = {rb[z].obs, rb[z].act, rb[z].rew, rb[z].next_obs, rb[z].done};
-      return p[c];
-    };
-    if (h->K == 1) {
-      gather_rows_kernel<false><<<grid, 256, 0, s>>>(LaneSrc<false>{{col(0)}}, h->idx, w[c], SB, dst[c], 0);
-    } else {
-      LaneSrc<true> src{};
-      for (int z = 0; z < h->K; ++z) src.p[z] = col(z);
-      gather_rows_kernel<true><<<lane_grid(grid, h->K), 256, 0, s>>>(src, h->idx, w[c], SB, dst[c], h->lane_stride);
-    }
-    B200RL_CUDA(cudaGetLastError());
-    count_launch(1);
-  }
+  for (int c = 0; c < 5; ++c)
+    if (launch(h, gather_rows_kernel<false>, gather_rows_kernel<true>, (unsigned)((SB * w[c] + 255) / 256), 256, 0, s,
+               *src[c], h->idx, w[c], SB, dst[c]))
+      return 1;
   return 0;
+}
+
+// The call's replay table: each learner's columns, row count, episode-end column (set_nstep) and tree (trees NULL:
+// none)
+static void set_replay(b200rl_offpolicy* h, const b200rl_offpolicy_replay* rb, float* const* trees) {
+  ReplayLanes<true>& r = h->replay;
+  r = ReplayLanes<true>{};
+  for (int z = 0; z < h->K; ++z) {
+    r.obs.p[z] = rb[z].obs, r.act.p[z] = rb[z].act, r.rew.p[z] = rb[z].rew, r.next_obs.p[z] = rb[z].next_obs;
+    r.done.p[z] = rb[z].done, r.ends.p[z] = h->nstep_ends.p[z];
+    r.tree[z] = trees != nullptr ? trees[z] : nullptr;
+    r.rows[z] = rb[z].rows;
+  }
 }
 
 static int check_replay(const b200rl_offpolicy* h, const b200rl_offpolicy_replay* rb, const char* what) {
@@ -2471,33 +2322,27 @@ extern "C" int b200rl_offpolicy_train_gather_group(b200rl_offpolicy* h, const b2
   B200RL_REQUIRE(h && hp && idx && q1_values && q1_losses && (policy_losses || h->dqn) && n_policy_updates,
                  "offpolicy_train_gather: NULL argument");
   if (int rc = check_replay(h, rb, "offpolicy_train_gather")) return rc;
-  B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
-                 "offpolicy_train_gather: S=%d B=%d exceed the capacities", S, B);
-  const bool td3 = h->cfg.n_q == 2;
-  B200RL_REQUIRE(!td3 || (q2_values && q2_losses), "offpolicy_train_gather: TD3 needs the Q2 outputs");
-  B200RL_REQUIRE(h->dqn || !hp->use_target_noise || noise,
-                 "offpolicy_train_gather: target noise requested but no noise given");
-  B200RL_REQUIRE(h->dqn || hp->policy_delay >= 1, "offpolicy_train_gather: policy_delay must be >= 1");
-  if (sac_ready(h, noise != nullptr, "offpolicy_train_gather") || dqn_ready(h, "offpolicy_train_gather")) return 2;
   const size_t SB = (size_t)S * B;
-  for (int z = 0; z < h->K; ++z)
-    for (size_t i = 0; i < SB; ++i)
-      B200RL_REQUIRE(idx[z * SB + i] >= 0 && idx[z * SB + i] < rb[z].rows,
-                     "offpolicy_train_gather: index %lld outside the %lld replay rows", (long long)idx[z * SB + i],
-                     (long long)rb[z].rows);
-  cudaStream_t user = static_cast<cudaStream_t>(stream);
+  const auto own = [&] {
+    for (int z = 0; z < h->K; ++z)
+      for (size_t i = 0; i < SB; ++i)
+        B200RL_REQUIRE(idx[z * SB + i] >= 0 && idx[z * SB + i] < rb[z].rows,
+                       "offpolicy_train_gather: index %lld outside the %lld replay rows", (long long)idx[z * SB + i],
+                       (long long)rb[z].rows);
+    return 0;
+  };
+  if (int rc = train_begin(h, hp, S, B, noise != nullptr, q2_values && q2_losses, n_policy_updates, stream,
+                           "offpolicy_train_gather", own))
+    return rc < 0 ? 0 : rc;
+  set_replay(h, rb, nullptr);
   cudaStream_t s = h->gs;
   const int A = h->A;
-  *n_policy_updates = 0;
-  if (S == 0) return 0;
-  B200RL_CUDA(cudaEventRecord(h->ev, user));
-  B200RL_CUDA(cudaStreamWaitEvent(s, h->ev, 0));
   // the minibatches are gathered on the device from the replay columns: only the indices (and noise) cross PCIe
   const size_t ls = h->lane_stride;
   B200RL_CUDA(cudaMemcpy2DAsync(h->idx, ls, idx, SB * 8, SB * 8, h->K, cudaMemcpyHostToDevice, s));
   const size_t n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise && !h->dqn ? SB * A : 0);
   if (n_eps) B200RL_CUDA(cudaMemcpy2DAsync(h->eps, ls, noise, n_eps * 4, n_eps * 4, h->K, cudaMemcpyHostToDevice, s));
-  if (gather_columns(h, hp, rb, (long long)SB, s)) return 1;
+  if (gather_columns(h, hp, (long long)SB, s)) return 1;
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
 }
 
@@ -2527,43 +2372,32 @@ extern "C" int b200rl_offpolicy_train_gather_rng_group(b200rl_offpolicy* h, cons
   B200RL_REQUIRE(h && hp && ring_start && ring_size && seed && call && q1_values && q1_losses &&
                      (policy_losses || h->dqn) && n_policy_updates, "offpolicy_train_gather_rng: NULL argument");
   if (int rc = check_replay(h, rb, "offpolicy_train_gather_rng")) return rc;
-  B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
-                 "offpolicy_train_gather_rng: S=%d B=%d exceed the capacities", S, B);
-  for (int z = 0; z < h->K; ++z) {
-    const long long rows = rb[z].rows;
-    B200RL_REQUIRE(ring_size[z] >= 1 && ring_size[z] <= rows && ring_start[z] >= 0 && ring_start[z] < rows,
-                   "offpolicy_train_gather_rng: bad ring (rows %lld, start %lld, size %lld)", rows,
-                   (long long)ring_start[z], (long long)ring_size[z]);
-  }
-  const bool td3 = h->cfg.n_q == 2;
-  B200RL_REQUIRE(!td3 || (q2_values && q2_losses), "offpolicy_train_gather_rng: TD3 needs the Q2 outputs");
-  B200RL_REQUIRE(h->dqn || hp->policy_delay >= 1, "offpolicy_train_gather_rng: policy_delay must be >= 1");
-  if (sac_ready(h, true, "offpolicy_train_gather_rng") || dqn_ready(h, "offpolicy_train_gather_rng")) return 2;
-  cudaStream_t user = static_cast<cudaStream_t>(stream);
+  const auto own = [&] {
+    for (int z = 0; z < h->K; ++z) {
+      const long long rows = rb[z].rows;
+      B200RL_REQUIRE(ring_size[z] >= 1 && ring_size[z] <= rows && ring_start[z] >= 0 && ring_start[z] < rows,
+                     "offpolicy_train_gather_rng: bad ring (rows %lld, start %lld, size %lld)", rows,
+                     (long long)ring_start[z], (long long)ring_size[z]);
+    }
+    return 0;
+  };
+  if (int rc = train_begin(h, hp, S, B, true, q2_values && q2_losses, n_policy_updates, stream,
+                           "offpolicy_train_gather_rng", own))
+    return rc < 0 ? 0 : rc;
+  set_replay(h, rb, nullptr);
   cudaStream_t s = h->gs;
   const int A = h->A;
   const long long SB = (long long)S * B;
-  *n_policy_updates = 0;
-  if (S == 0) return 0;
-  B200RL_CUDA(cudaEventRecord(h->ev, user));
-  B200RL_CUDA(cudaStreamWaitEvent(s, h->ev, 0));
   const long long n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise && !h->dqn ? SB * A : 0);  // DQN: indices only
   const long long n_thr = ((SB > n_eps ? SB : n_eps) + 3) / 4;
-  const dim3 grid((unsigned)((n_thr + 255) / 256));
-  if (h->K == 1) {
-    const DrawKeys<false> k = {{seed[0]}, {call[0]}, {ring_start[0]}, {ring_size[0]}, {rb[0].rows}};
-    draw_minibatches_kernel<false><<<grid, 256, 0, s>>>(h->idx, SB, n_eps ? h->eps : nullptr, n_eps, k, 0);
-  } else {
-    DrawKeys<true> k{};
-    for (int z = 0; z < h->K; ++z)
-      k.seed[z] = seed[z], k.call[z] = call[z], k.start[z] = ring_start[z], k.size[z] = ring_size[z],
-      k.capacity[z] = rb[z].rows;
-    draw_minibatches_kernel<true><<<lane_grid(grid, h->K), 256, 0, s>>>(h->idx, SB, n_eps ? h->eps : nullptr, n_eps, k,
-                                                                        h->lane_stride);
-  }
-  B200RL_CUDA(cudaGetLastError());
-  count_launch(1);
-  if (gather_columns(h, hp, rb, SB, s)) return 1;
+  DrawKeys<true> keys{};
+  for (int z = 0; z < h->K; ++z)
+    keys.seed[z] = seed[z], keys.call[z] = call[z], keys.start[z] = ring_start[z], keys.size[z] = ring_size[z],
+    keys.capacity[z] = rb[z].rows;
+  if (launch(h, draw_minibatches_kernel<false>, draw_minibatches_kernel<true>, (unsigned)((n_thr + 255) / 256), 256, 0,
+             s, h->idx, SB, n_eps ? h->eps : nullptr, n_eps, keys))
+    return 1;
+  if (gather_columns(h, hp, SB, s)) return 1;
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
 }
 
@@ -2613,35 +2447,29 @@ extern "C" int b200rl_offpolicy_train_prioritized_group(b200rl_offpolicy* h, con
                  "only");
   B200RL_REQUIRE(h->per_set, "offpolicy_train_prioritized: call b200rl_offpolicy_set_per first");
   if (int rc = check_replay(h, rb, "offpolicy_train_prioritized")) return rc;
-  if (dqn_ready(h, "offpolicy_train_prioritized")) return 2;
-  B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
-                 "offpolicy_train_prioritized: S=%d B=%d exceed the capacities", S, B);
-  for (int z = 0; z < h->K; ++z) {
-    B200RL_REQUIRE(trees[z] != nullptr, "offpolicy_train_prioritized: learner %d: NULL tree", z);
-    B200RL_REQUIRE(rb[z].rows < ((int64_t)1 << 31), "offpolicy_train_prioritized: learner %d: more than 2^31 - 1 rows",
-                   z);
-    // every learner's update kernel rewrites its tree's leaves and interior nodes concurrently with the others: two
-    // learners on one tree would race (stale interior sums, a lost running max)
-    for (int y = 0; y < z; ++y)
-      B200RL_REQUIRE(trees[y] != trees[z], "offpolicy_train_prioritized: learners %d and %d share one tree: every "
-                     "learner of a group needs its own prioritized replay buffer", y, z);
-  }
-  if (S == 0) return 0;
-  cudaStream_t s = h->gs;
-  B200RL_CUDA(cudaEventRecord(h->ev, static_cast<cudaStream_t>(stream)));
-  B200RL_CUDA(cudaStreamWaitEvent(s, h->ev, 0));
-  h->per_lanes = PerLanes<true>{};
+  const auto own = [&] {
+    for (int z = 0; z < h->K; ++z) {
+      B200RL_REQUIRE(trees[z] != nullptr, "offpolicy_train_prioritized: learner %d: NULL tree", z);
+      B200RL_REQUIRE(rb[z].rows < ((int64_t)1 << 31),
+                     "offpolicy_train_prioritized: learner %d: more than 2^31 - 1 rows", z);
+      // every learner's update kernel rewrites its tree's leaves and interior nodes concurrently with the others: two
+      // learners on one tree would race (stale interior sums, a lost running max)
+      for (int y = 0; y < z; ++y)
+        B200RL_REQUIRE(trees[y] != trees[z], "offpolicy_train_prioritized: learners %d and %d share one tree: every "
+                       "learner of a group needs its own prioritized replay buffer", y, z);
+    }
+    return 0;
+  };
+  int32_t n_pol = 0;
+  if (int rc = train_begin(h, hp, S, B, true, false, &n_pol, stream, "offpolicy_train_prioritized", own))
+    return rc < 0 ? 0 : rc;
+  set_replay(h, rb, trees);
   const size_t tab_n = (size_t)4 * h->cfg.max_steps + 2;
   for (int z = 0; z < h->K; ++z) {
-    PerLanes<true>& l = h->per_lanes;
-    l.tree[z] = trees[z], l.rows[z] = rb[z].rows;
-    l.obs[z] = rb[z].obs, l.act[z] = rb[z].act, l.rew[z] = rb[z].rew, l.next_obs[z] = rb[z].next_obs;
-    l.done[z] = rb[z].done;
     unsigned long long* keys = reinterpret_cast<unsigned long long*>(h->h_adam_tab + z * tab_n + tab_n - 2);
     keys[0] = seed[z], keys[1] = call[z];  // uploaded with the table by run_staged
   }
   h->per_run = true;
-  int32_t n_pol = 0;
   const int rc = run_staged(h, hp, S, B, q1_values, nullptr, q1_losses, nullptr, nullptr, &n_pol);
   h->per_run = false;
   return rc;

@@ -493,6 +493,36 @@ typedef struct {
 int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hparams* hp);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * QR-DQN on the same engine (Dabney, Rowland, Bellemare & Munos 2018): a DQN engine (config algo = 2) after
+ * b200rl_offpolicy_set_qr, whose Q network maps obs -> [n_actions x n_quantiles] quantile locations, row-major (action a
+ * owns columns a N .. a N + N - 1; theta_i(s, a) is the i-th).  Everything the DQN section says holds (networks, state
+ * blob, action column, hparams, target copies, outputs, invalid actions, graph, groups, prioritized replay, n-step
+ * returns; b200rl_offpolicy_set_dqn is required too) except the loss.  With N = n_quantiles, in float32:
+ *   tau_i    = (float)(2i + 1) / (float)(2N)
+ *   Q(s, a)  = (sum_i theta_i(s, a)) / N, summed over i in index order; q1_values logs it
+ *   a*       = argmax_a Q(s', a) with the means of Q (double_q = 1; at the start of the step) or of Q_targ
+ *            (torch's argmax: a NaN wins, ties go to the first index)
+ *   target   T_j = r + (g (1 - d)) theta_j(s', a*) from Q_targ, g = gamma (n-step: the row's discount)
+ *   loss     u_ij = T_j - theta_i(s, a), rho_i(u) = |tau_i - 1{u < 0}| h(u), h(u) = 0.5 u^2 if |u| < 1 else |u| - 0.5
+ *            (kappa = 1); the row's L = (1/N) sum_i sum_j rho_i(u_ij), over j in index order, then over i in index
+ *            order; one Adam step (optimizer 1) on (1/B) sum_b L_b, summed in double in a fixed order
+ *   gradient w.r.t. the action's quantile i: -(sum_j |tau_i - 1{u_ij < 0}| clamp(u_ij, -1, 1)) / N times (1/B); every
+ *            other output's 0
+ * Prioritized replay: the loss is (1/B) sum_b w_b L_b and the gradient row b is scaled by w_b (with every w_b = 1 bit
+ * for bit the unweighted step); the priority of row b is (L_b + eps)^alpha with its unweighted L_b from before the
+ * Adam step, which takes the place of |delta| in the prioritized replay section (non-finite: counted, and the call
+ * fails).  The head is deterministic (no float atomics): a group's learners stay bit-identical to solo engines.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t n_quantiles; /* N, 1..256; the Q network's output width must be a multiple of N */
+  int32_t reserved;    /* ignored */
+} b200rl_qr_hparams;
+
+/* Makes the engine's loss head QR-DQN's for every later train call; refused on engines not created with algo = 2
+ * (TD3 / DDPG, SAC, C51); part of the cached graph's key. */
+int b200rl_offpolicy_set_qr(b200rl_offpolicy* h, const b200rl_qr_hparams* hp);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Learner groups: K independent off-policy learners (same config, same hyper-parameters, their own parameters, Adam
  * states, step counts, minibatches, noise, replay buffers and temperature) trained by one engine, every operation of a
  * step ONE launch for all K.  Each learner's arithmetic -- tile shapes, summation order, Adam's operation order -- is

@@ -98,6 +98,10 @@ class C51Hparams(C.Structure):
     _fields_ = [("n_atoms", C.c_int32), ("reserved", C.c_int32), ("v_min", C.c_double), ("v_max", C.c_double)]
 
 
+class QrHparams(C.Structure):
+    _fields_ = [("n_quantiles", C.c_int32), ("reserved", C.c_int32)]
+
+
 class PerHparams(C.Structure):
     _fields_ = [("alpha", C.c_double), ("eps", C.c_double), ("beta_start", C.c_double),
                 ("beta_anneal_steps", C.c_int64)]
@@ -186,6 +190,7 @@ SIGNATURES = {
     "b200rl_offpolicy_sac_outputs": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "b200rl_offpolicy_set_dqn": (C.c_int, [C.c_void_p, C.POINTER(DqnHparams)]),
     "b200rl_offpolicy_set_c51": (C.c_int, [C.c_void_p, C.POINTER(C51Hparams)]),
+    "b200rl_offpolicy_set_qr": (C.c_int, [C.c_void_p, C.POINTER(QrHparams)]),
     "b200rl_offpolicy_create_group": (C.c_int, [C.POINTER(OffPolicyConfig), C.c_int32, C.POINTER(C.c_void_p)]),
     "b200rl_offpolicy_train_gather_group": (C.c_int, [C.c_void_p, C.POINTER(OffPolicyHparams), C.c_int32, C.c_int32,
                                                       C.POINTER(OffPolicyReplay)] + [C.c_void_p] * 7 +

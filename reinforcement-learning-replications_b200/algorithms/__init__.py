@@ -2,9 +2,10 @@ from .c51 import C51
 from .dqn import DQN
 from .group import LearnerGroup
 from .ppo import PPO
+from .qrdqn import QRDQN
 from .sac import SAC
 from .td3 import DDPG, TD3
 from .trpo import TRPO
 from .vpg import VPG
 
-__all__ = ["VPG", "TRPO", "PPO", "DDPG", "TD3", "SAC", "DQN", "C51", "LearnerGroup"]
+__all__ = ["VPG", "TRPO", "PPO", "DDPG", "TD3", "SAC", "DQN", "C51", "QRDQN", "LearnerGroup"]

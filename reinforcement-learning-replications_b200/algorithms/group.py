@@ -1,4 +1,4 @@
-"""LearnerGroup: several independent TD3 / DDPG / SAC / DQN / C51 learners (typically one per seed) trained side by side by ONE
+"""LearnerGroup: several independent TD3 / DDPG / SAC / DQN / C51 / QR-DQN learners (typically one per seed) trained side by side by ONE
 off-policy engine, every operation of a train step one launch for all of them (b200rl_offpolicy_create_group).
 
 The contract: each member ends up bit for bit where it would be had it run alone.  Members keep everything of their
@@ -27,6 +27,7 @@ from .._lib import MAX_LEARNERS
 from ..engine import OffPolicyEngine
 from ..replay_buffer import PrioritizedReplayBuffer
 from ._onpolicy import adam_hparams, describe_mlp
+from .qrdqn import QRDQN
 from .td3 import _learn_begin, _learn_evaluate_save, _learn_sample, _OffPolicyBase
 
 
@@ -49,6 +50,7 @@ def _signature(agent) -> list:
         if agent.algo == OffPolicyEngine.C51:
             for attr in ("n_atoms", "v_min", "v_max"):
                 sig.append((attr, getattr(agent.q_function, attr)))
+        sig.append(("n_quantiles", getattr(agent.q_function, "n_quantiles", None)))
         rb = getattr(agent, "replay_buffer", None)
         sig.append(("prioritized replay", isinstance(rb, PrioritizedReplayBuffer)))
         for attr in ("alpha", "eps", "beta_start", "beta_anneal_steps"):
@@ -105,7 +107,7 @@ class LearnerGroup:
     def add(self, agent) -> None:
         """Add ``agent``; the current state of the global random generators becomes its private stream."""
         if not isinstance(agent, _OffPolicyBase):
-            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or DQN / C51) learners, got {type(agent).__name__}")
+            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or DQN / C51 / QR-DQN) learners, got {type(agent).__name__}")
         if any(m is agent for m in self.members):
             raise ValueError("LearnerGroup: this agent is already a member")
         if len(self.members) >= MAX_LEARNERS:
@@ -194,6 +196,8 @@ class LearnerGroup:
         if members[0].algo == OffPolicyEngine.C51:
             q = members[0].q_function
             e.set_c51(q.n_atoms, q.v_min, q.v_max)
+        if isinstance(members[0], QRDQN):
+            e.set_qr(members[0].q_function.n_quantiles)
         hp = members[0]._hparams(noisy, delay)
         if members[0].algo in (OffPolicyEngine.DQN, OffPolicyEngine.C51):
             n = members[0].n_step

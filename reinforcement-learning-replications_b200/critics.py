@@ -70,3 +70,29 @@ class CategoricalQFunction(_Critic):
 
     def forward(self, observation: Tensor) -> Tensor:
         return (self.distribution(observation) * self.support).sum(-1)
+
+
+class QuantileQFunction(_Critic):
+    """A return distribution per action as ``n_quantiles`` quantile locations (QR-DQN's critic): the network maps an
+    observation to ``n_actions x n_quantiles`` values, action a owning columns a*n_quantiles .. (a+1)*n_quantiles - 1,
+    located at the quantile midpoints ``taus``.  ``forward`` returns their means [..., n_actions], so greedy and
+    epsilon-greedy policies and the evaluator use it as they use a ``DiscreteQFunction``."""
+
+    MAX_QUANTILES = 256  # the engine's limit (b200rl.h)
+
+    def __init__(self, network: nn.Module, optimizer: Optimizer, n_quantiles: int = 200) -> None:
+        super().__init__(network, optimizer)
+        if isinstance(n_quantiles, bool) or int(n_quantiles) != n_quantiles or \
+                not 1 <= int(n_quantiles) <= self.MAX_QUANTILES:
+            raise ValueError(f"n_quantiles must be an integer from 1 to {self.MAX_QUANTILES}, got {n_quantiles!r}")
+        self.n_quantiles = int(n_quantiles)
+        # tau_i = (2i + 1) / (2N), one float32 division as the engine computes it
+        N = self.n_quantiles
+        self.taus = torch.arange(1, 2 * N, 2, dtype=torch.float32) / torch.tensor(2 * N, dtype=torch.float32)
+
+    def quantiles(self, observation: Tensor) -> Tensor:
+        """theta(s, a) [..., n_actions, n_quantiles]."""
+        return self.network(observation).unflatten(-1, (-1, self.n_quantiles))
+
+    def forward(self, observation: Tensor) -> Tensor:
+        return self.quantiles(observation).sum(-1) / self.n_quantiles

@@ -21,6 +21,8 @@
 // DQN (config algo = 2) is a third: a per-row Huber loss head on discrete actions (dqn_loss_kernel), a target copy
 // gated by a per-learner step table (dqn_target_copy_kernel) and enqueue_dqn_steps; networks 1 and 4 only.
 // C51 (config algo = 3) is DQN's step program with a categorical head over return distributions (c51_loss_kernel).
+// QR-DQN (set_qr on a DQN engine) is DQN's step program with a quantile Huber head (qr_loss_kernel), prioritized replay
+// and n-step returns included.
 // Prioritized replay for DQN (train_prioritized): a 32-way sum tree per replay buffer, drawn from, weighed and gathered
 // by per_draw_kernel and updated by per_update_kernel inside the same step program.
 // n-step returns for DQN / C51 (set_nstep): nstep_gather_kernel (or per_draw_kernel's NSTEP instantiation) walks each
@@ -871,6 +873,135 @@ __global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// QR-DQN (b200rl_offpolicy_set_qr; Dabney, Rowland, Bellemare & Munos 2018): a head of the DQN engine.  The Q network
+// maps obs -> [n * N] quantile locations, action a owning columns a*N .. a*N + N - 1; Q(s, a) = their mean.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int QR_MAX_QUANTILES = 256;
+
+// shared-memory floats of one row at n actions x N quantiles: T and the quantile losses, theta(s, a), the argmax
+// net's means and its row
+__host__ __device__ __forceinline__ int qr_smem_floats(int n, int N) { return 2 * N + n + n * N; }
+
+// sum_k x[k] / N over one action's N quantiles (in shared memory), added in index order
+__device__ __forceinline__ float qr_mean(const float* x, int N) {
+  float s = 0.f;
+#pragma unroll 8
+  for (int k = 0; k < N; ++k) s += x[k];
+  return s / (float)N;
+}
+
+// One CTA per row i with action a = act[i] (grid = B rows per learner), thread t owning quantile t (blockDim = N
+// rounded up to whole warps): every row spreads its N^2 pairs over N threads, and each thread's sum over the target
+// quantiles j runs in index order.  The sums in index order (the means, the row loss) read rows the CTA first copies to
+// shared memory with coalesced loads.
+//   a* = argmax_j Q(s')_j over the means of qn (Double DQN: qn != NULL) or of qt_next (argmax_row's rule),
+//   T_j = r + gamma (1 - d) theta_j(s', a*) from Q_targ (C51's Tz order), u_tj = T_j - theta_t(s, a),
+//   tau_t = (2t + 1) / (2N), k_tj = |tau_t - 1{u_tj < 0}|, h(u) = 0.5 u^2 if |u| < 1 else |u| - 0.5,
+//   L = (1/N) sum_t sum_j k_tj h(u_tj)  (j, then t, in index order),
+//   dOut[i, a*N + t] = -(sum_j k_tj clamp(u_tj, -1, 1)) / N * (1 / B) and 0 elsewhere, q_copy[i] = Q(s, a).
+// A row whose action is not an integer in [0, n) is never used as an index: its dOut row is 0, its loss 0, q_copy NaN,
+// and it is counted.  The last CTA of a learner to finish sums the row losses and reads and resets the counters as
+// c51_loss_kernel does; no atomics touch a float.
+// WEIGHTED (prioritized replay): row i's loss and gradient are scaled by w[i], and absd[i] = its unweighted L (-1 for
+// a row with an invalid action), the base of its priority.  With every w_i = 1 both are bit for bit those of the
+// unweighted head.  NSTEP: row i's discount is disc[i] in place of gamma.  Each flag's operands are read only by the
+// instantiations that set it.
+template <bool LANES, bool WEIGHTED, bool NSTEP>
+__global__ void __launch_bounds__(QR_MAX_QUANTILES) qr_loss_kernel(
+    const float* q, const float* qt_next, const float* qn, const float* act, const float* rew, const float* done,
+    const float* disc, float gamma, int B, int n, int N, float* dout, float* row_loss, float* q_copy, int* sync,
+    float* loss_out, int* bad_out, const float* w, float* absd, size_t lane_stride) {
+  extern __shared__ float qr_smem[];
+  __shared__ double red[32];
+  __shared__ bool last;
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q = lane_ptr(q, o), qt_next = lane_ptr(qt_next, o), qn = lane_ptr(qn, o), act = lane_ptr(act, o);
+    rew = lane_ptr(rew, o), done = lane_ptr(done, o), dout = lane_ptr(dout, o), row_loss = lane_ptr(row_loss, o);
+    q_copy = lane_ptr(q_copy, o), sync = lane_ptr(sync, o), loss_out = lane_ptr(loss_out, o);
+    bad_out = lane_ptr(bad_out, o);
+    if (WEIGHTED) w = lane_ptr(w, o), absd = lane_ptr(absd, o);
+    if (NSTEP) disc = lane_ptr(disc, o);
+  }
+  const int nN = n * N, t = threadIdx.x, i = blockIdx.x;
+  float* st = qr_smem;        // T_j, then each quantile's loss sum
+  float* sth = st + N;        // theta(s, a)
+  float* sq = sth + N;        // the means of the argmax net
+  float* sa = sq + n;         // the argmax net's row
+  const float af = act[i];
+  const bool valid = af >= 0.f && af < (float)n && af == floorf(af);  // false for NaN
+  const int a = valid ? (int)af : -1;
+  float* drow = dout + (size_t)i * nN;
+  for (int c = t; c < nN; c += blockDim.x)
+    if (c / N != a) drow[c] = 0.f;
+  if (!valid) {
+    if (t == 0) {
+      q_copy[i] = __int_as_float(0x7fc00000);
+      row_loss[i] = 0.f;
+      if (WEIGHTED) absd[i] = -1.f;
+      atomicAdd(sync + 1, 1);
+    }
+  } else {
+    const float* an = (qn != nullptr ? qn : qt_next) + (size_t)i * nN;
+    for (int c = t; c < nN; c += blockDim.x) sa[c] = an[c];
+    const float th = t < N ? q[(size_t)i * nN + (size_t)a * N + t] : 0.f;
+    if (t < N) sth[t] = th;
+    __syncthreads();
+    for (int j = t; j < n; j += blockDim.x) sq[j] = qr_mean(sa + (size_t)j * N, N);
+    __syncthreads();
+    const int a_star = argmax_row(sq, n);
+    const float g1d = (NSTEP ? disc[i] : gamma) * (1.f - done[i]), r = rew[i];
+    const float* tq = qn != nullptr ? qt_next + (size_t)i * nN : sa;  // without Double DQN the argmax net is Q_targ
+    if (t < N) st[t] = r + g1d * tq[(size_t)a_star * N + t];
+    __syncthreads();
+    float lsum = 0.f, gsum = 0.f;
+    if (t < N) {
+      const float tau = (float)(2 * t + 1) / (float)(2 * N);
+      for (int j = 0; j < N; ++j) {
+        const float u = st[j] - th;
+        const float k = fabsf(tau - (u < 0.f ? 1.f : 0.f));
+        const float au = fabsf(u);
+        const float hu = au < 1.f ? 0.5f * u * u : au - 0.5f;
+        const float c = u > 1.f ? 1.f : (u < -1.f ? -1.f : u);  // NaN passes through, as torch's clamp lets it
+        lsum += k * hu;
+        gsum += k * c;
+      }
+    }
+    __syncthreads();  // every thread is done with T
+    const float inv = 1.0f / (float)B;  // dqn_loss_kernel's scaling
+    if (t < N) {
+      st[t] = lsum;
+      const float g = -gsum / (float)N;
+      drow[(size_t)a * N + t] = (WEIGHTED ? w[i] * g : g) * inv;
+    }
+    __syncthreads();
+    if (t == 0) {
+      float L = 0.f, qv = 0.f;
+#pragma unroll 8
+      for (int k = 0; k < N; ++k) L += st[k], qv += sth[k];
+      L /= (float)N;
+      q_copy[i] = qv / (float)N;
+      row_loss[i] = WEIGHTED ? w[i] * L : L;
+      if (WEIGHTED) absd[i] = L;
+    }
+  }
+  // the last CTA of this learner reads every row's loss
+  __threadfence();
+  __syncthreads();
+  if (t == 0) last = atomicAdd(sync, 1) == (int)gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double acc = 0.0;
+  for (int r = t; r < B; r += blockDim.x) acc += (double)__ldcg(row_loss + r);
+  block_mean(acc, B, loss_out, red);
+  if (t == 0) {
+    *bad_out = atomicExch(sync + 1, 0);
+    sync[0] = 0;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // Prioritized experience replay (Schaul et al. 2016, proportional variant).  A sum tree over the physical rows of a
 // replay buffer with 32 children per node, all levels in one float array (b200rl.h, b200rl_per_tree_floats): level 0
 // holds the leaves, level k + 1 the sums of 32 consecutive nodes of level k, every level padded with zeros to a multiple
@@ -1116,6 +1247,7 @@ struct GraphKey {
   b200rl_sac_hparams sac;
   b200rl_dqn_hparams dqn;
   b200rl_c51_hparams c51;
+  b200rl_qr_hparams qr;
   b200rl_per_hparams per;
   ReplayLanes<true> replay;
 };
@@ -1179,8 +1311,11 @@ struct b200rl_offpolicy {
   bool c51 = false, c51_set = false;
   b200rl_c51_hparams c51_hp{};
   float* c51_support = nullptr;   // [C51_MAX_ATOMS] z_0 .. z_{N-1}
-  float* c51_row_loss = nullptr;  // [B] each row's cross-entropy of the current step
+  float* c51_row_loss = nullptr;  // [B] each row's cross-entropy (QR-DQN: quantile loss) of the current step
   int* c51_sync = nullptr;        // {CTAs done, invalid rows} of the current step; 0 between launches
+  // QR-DQN (b200rl_offpolicy_set_qr on a DQN engine): the loss head is qr_loss_kernel, with C51's row losses and counters
+  bool qr = false;
+  b200rl_qr_hparams qr_hp{};
   // prioritized replay (DQN engines): a prioritized call draws, weighs and gathers inside the step program; adam_tab
   // row 3's .y then holds each step's beta and the table's last two float2 the call's (seed, call) words
   bool per_set = false, per_run = false;
@@ -1479,12 +1614,10 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
     rc |= oalloc(h, &h->per_bad, S);
     rc |= oalloc(h, &h->nstep_disc, S * B);
     rc |= oalloc(h, &h->nstep_rows, S * B);
-  }
-  if (c51) {
-    rc |= oalloc(h, &h->c51_support, C51_MAX_ATOMS);
-    rc |= oalloc(h, &h->c51_row_loss, B);
+    rc |= oalloc(h, &h->c51_row_loss, B);  // C51's and QR-DQN's heads
     rc |= oalloc(h, &h->c51_sync, 2);
   }
+  if (c51) rc |= oalloc(h, &h->c51_support, C51_MAX_ATOMS);
   rc |= arena_commit(h);
   if (rc == 0) {
     float* q = h->state;
@@ -1667,6 +1800,22 @@ extern "C" int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hp
   B200RL_CUDA(cudaStreamSynchronize(h->gs));
   h->c51_hp = hp;
   h->c51_set = true;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_set_qr(b200rl_offpolicy* h, const b200rl_qr_hparams* qp) {
+  B200RL_REQUIRE(h && qp, "offpolicy_set_qr: NULL argument");
+  B200RL_REQUIRE(h->dqn && !h->c51, "offpolicy_set_qr: the engine was not created with algo = 2 (DQN)");
+  const int N = qp->n_quantiles, width = h->net[1].d.sizes[h->net[1].d.n_layers];
+  B200RL_REQUIRE(N >= 1 && N <= QR_MAX_QUANTILES, "offpolicy_set_qr: n_quantiles must be 1..%d, got %d",
+                 QR_MAX_QUANTILES, N);
+  B200RL_REQUIRE(width % N == 0, "offpolicy_set_qr: the Q network's output width %d is not n_actions x n_quantiles "
+                 "for n_quantiles = %d", width, N);
+  B200RL_REQUIRE(qr_smem_floats(width / N, N) <= C51_SMEM_FLOATS, "offpolicy_set_qr: %d actions x %d quantiles is too wide for the "
+                 "head's shared memory", width / N, N);
+  h->qr_hp = *qp;
+  h->qr_hp.reserved = 0;  // part of the graph cache key
+  h->qr = true;
   return 0;
 }
 
@@ -1996,12 +2145,20 @@ static auto dqn_head(bool weighted, bool nstep) {
                   : (nstep ? dqn_loss_kernel<LANES, false, true> : dqn_loss_kernel<LANES, false, false>);
 }
 
+// the same choice of qr_loss_kernel
+template <bool LANES>
+static auto qr_head(bool weighted, bool nstep) {
+  return weighted ? (nstep ? qr_loss_kernel<LANES, true, true> : qr_loss_kernel<LANES, true, false>)
+                  : (nstep ? qr_loss_kernel<LANES, false, true> : qr_loss_kernel<LANES, false, false>);
+}
+
 // The S DQN steps.  Per step:
 //   s  : Q_targ(s') ---------------+-> loss -> dX chain -> Adam(Q) -> target copy (on the steps the flag table marks)
 //   s2 : Q(s') (Double DQN only) --+
 //   s3 : Q(s) ---------------------+   ........ Q's dW products
 // Q(s') reads the parameters at the start of the step: the step's Adam waits for the loss kernel, which joins it.
-// A C51 engine (h->c51) takes c51_loss_kernel as its loss head; nothing else in the step differs.
+// A C51 engine (h->c51) takes c51_loss_kernel as its loss head, a QR-DQN engine (h->qr) qr_loss_kernel; nothing else
+// in the step differs.
 // A prioritized call (h->per_run) opens each step with the draw on s (draw, weights, gather), takes the weighted loss
 // head, and runs the priority update on s4 beside the backward pass; the next step's draw joins it.
 static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s) {
@@ -2062,6 +2219,13 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
                  qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, h->c51_support, (float)hp->gamma,
                  vmin, vmax, dz, B, n / N, N, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync,
                  h->out_l1 + st, h->dqn_bad + st))
+        return 1;
+    } else if (h->qr) {
+      const int N = h->qr_hp.n_quantiles;
+      if (launch(h, qr_head<false>(per, nstep), qr_head<true>(per, nstep), B, (N + 31) / 32 * 32,
+                 sizeof(float) * (size_t)qr_smem_floats(n / N, N), s, qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done,
+                 s_disc, (float)hp->gamma, B, n / N, N, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B,
+                 h->c51_sync, h->out_l1 + st, h->dqn_bad + st, s_w, h->per_absd))
         return 1;
     } else if (launch(h, dqn_head<false>(per, nstep), dqn_head<true>(per, nstep), 1, GTHREADS, 0, s, qa[L], tq[L],
                       dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, (float)hp->gamma, B, n, h->dqn_dout,
@@ -2145,7 +2309,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
     GraphKey key;
     memset(&key, 0, sizeof(key));
     key.S = S, key.B = B, key.nstep = h->nstep;
-    key.hp = *hp, key.sac = h->sac_hp, key.dqn = h->dqn_hp, key.c51 = h->c51_hp;
+    key.hp = *hp, key.sac = h->sac_hp, key.dqn = h->dqn_hp, key.c51 = h->c51_hp, key.qr = h->qr_hp;
     if (h->per_run) key.per = h->per_hp, key.replay = h->replay;
     if (h->graph == nullptr || memcmp(&key, &h->graph_key, sizeof(key)) != 0) {
       if (h->graph) {
@@ -2203,14 +2367,17 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
                                   cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaStreamSynchronize(s));
   *n_policy_updates = n_pol;
-  const int n_actions = h->net[1].d.sizes[h->net[1].d.n_layers] / (h->c51 ? h->c51_hp.n_atoms : 1);
+  const int n_actions = h->net[1].d.sizes[h->net[1].d.n_layers] /
+                        (h->c51 ? h->c51_hp.n_atoms : h->qr ? h->qr_hp.n_quantiles : 1);
+  const char* algo = h->c51 ? "C51" : h->qr ? "QR-DQN" : "DQN";
   for (size_t i = 0; i < bad.size(); ++i)
     B200RL_REQUIRE(bad[i] == 0, "offpolicy_train: %s learner %d, step %d: %d minibatch rows hold an action that is not "
-                   "an integer in [0, %d); those rows were left out of the update", h->c51 ? "C51" : "DQN",
-                   (int)(i / S), (int)(i % S), bad[i], n_actions);
+                   "an integer in [0, %d); those rows were left out of the update", algo, (int)(i / S), (int)(i % S),
+                   bad[i], n_actions);
   for (size_t i = 0; i < per_bad.size(); ++i)
-    B200RL_REQUIRE(per_bad[i] == 0, "offpolicy_train_prioritized: DQN learner %d, step %d: %d minibatch rows gave a "
-                   "non-finite priority; their leaves were left unchanged", (int)(i / S), (int)(i % S), per_bad[i]);
+    B200RL_REQUIRE(per_bad[i] == 0, "offpolicy_train_prioritized: %s learner %d, step %d: %d minibatch rows gave a "
+                   "non-finite priority; their leaves were left unchanged", algo, (int)(i / S), (int)(i % S),
+                   per_bad[i]);
   return 0;
 }
 

@@ -324,7 +324,8 @@ class OffPolicyEngine:
     is no target policy (network 3), and ``set_sac`` must be called before the first train call.  DQN: ``policy_sizes``
     = None, ``n_q`` = 1, the Q network maps obs -> [n actions], only networks 1 (Q) and 4 (target Q) exist, actions are
     indices (act [S,B]), and ``set_dqn`` must be called before the first train call.  C51 is a DQN engine whose Q
-    network maps obs -> [n actions x n atoms] logits; it needs ``set_c51`` as well as ``set_dqn``.
+    network maps obs -> [n actions x n atoms] logits; it needs ``set_c51`` as well as ``set_dqn``.  QR-DQN is a DQN
+    engine after ``set_qr``: its Q network maps obs -> [n actions x n quantiles] quantile locations.
 
     ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
     launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
@@ -500,6 +501,15 @@ class OffPolicyEngine:
         cp = C51Hparams()
         cp.n_atoms, cp.v_min, cp.v_max = int(n_atoms), float(v_min), float(v_max)
         check(self.lib.b200rl_offpolicy_set_c51(self.h, C.byref(cp)), "set_c51")
+
+    # ---- QR-DQN ----
+    def set_qr(self, n_quantiles: int) -> None:
+        """Makes the loss head QR-DQN's quantile Huber loss over ``n_quantiles`` quantiles for every later train call
+        (a DQN engine only; b200rl.h)."""
+        from ._lib import QrHparams
+        qp = QrHparams()
+        qp.n_quantiles = int(n_quantiles)
+        check(self.lib.b200rl_offpolicy_set_qr(self.h, C.byref(qp)), "set_qr")
 
     # ---- prioritized replay (DQN) ----
     def set_per(self, alpha: float, eps: float, beta_start: float, beta_anneal_steps: int) -> None:

@@ -138,7 +138,7 @@ int b200rl_absmax(const float* x, int64_t n, float* out, void* stream);
 int b200rl_absmax_cols(const float* x, int64_t rows, int32_t cols, float* out, void* stream);
 
 /* Number of mlp_loss_grad launches (since process start) whose fp16 tensor-core pass left the fp16 range and were
- * recomputed by the wide-range bf16 kernel queued behind it.  Synchronises the device; diagnostics / tests only. */
+ * recomputed by the fp32 kernel queued behind it.  Synchronises the device; diagnostics / tests only. */
 int64_t b200rl_tc_fallback_count(void);
 
 /* ------------------------------------------------------------------------------------------------------------

@@ -14,7 +14,7 @@
 
 namespace b200rl {
 
-bool tc2_path_enabled(const b200rl_mlp_desc& d);
+bool use_tc(const b200rl_mlp_desc& d);  // mlp_fused.cu: the tensor-core kernels take this network
 
 static thread_local std::string g_error;
 static std::atomic<int64_t> g_launches{0};  // engines of different host threads count into it
@@ -747,7 +747,7 @@ static int run_update(b200rl_onpolicy* h, const b200rl_ppo_hparams* hp, b200rl_a
   B200RL_REQUIRE(hp->num_policy_gradients >= 0 && hp->num_value_gradients >= 0, "update: negative step count");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const bool fused = policy_loss == B200RL_LOSS_PPO_CLIP && h->fused_ok && !h->train_log_std && fused_step_enabled() &&
-                     tc2_path_enabled(h->cfg.policy) && tc2_path_enabled(h->cfg.value) &&
+                     use_tc(h->cfg.policy) && use_tc(h->cfg.value) &&
                      hp->num_policy_gradients > 0 && hp->num_value_gradients > 0;
   bool tripped = false;
   if (run_update_impl(h, hp, ar, user, stats, s, policy_loss, fused, &tripped)) return 1;

@@ -4,7 +4,11 @@
 // policies/categorical_policy.py:22-32, algorithms/ppo.py:237-257 + autograd backward (:234), :259-269, :282-287
 // (+ :277), algorithms/vpg.py:200-206, algorithms/trpo.py:154-165, utils.py:60-71 and utils.py:90-92 (on load).
 //
-// Data flow (fp32 CUDA-core path; the tensor-core path in mlp_tc.cu keeps the same flow):
+// It is also the wide-range re-run of the fp16 tensor-core kernels (mlp_tc2.cu, mlp_tc_fvp.cu): every launch of theirs
+// queues this kernel behind it, predicated on the launch's status slot, and it recomputes a launch whose values left
+// fp16's range.
+//
+// Data flow (fp32 CUDA-core path; the tensor-core kernels keep the same flow):
 //   * grid = min(#tiles, #SMs) persistent CTAs, tile = 64 rows, static round-robin tile -> CTA map (deterministic).
 //   * all weights live in shared memory for the whole launch, in both [out][in] and [in][out] order, so every
 //     tile product is the SAME k-major inner loop  C[m][n] += A[k][m] * B[k][n]  with float4 shared loads:
@@ -148,11 +152,10 @@ struct FusedArgs {
   const unsigned* run_if;  // when set: run only if *run_if == seq (re-run of a tensor-core launch that left fp16's range)
   unsigned seq;
   int total_rows;          // partial rows the consumer reduces (> gridDim.x when standing in for / sized like a tensor-core launch)
-  unsigned long long* rerun_counter;  // b200rl_tc_fallback_count's device counter
   int train_log_std;       // Gaussian: partial rows carry dLoss/dlog_std in columns P .. P + A - 1 (row stride P + A)
 };
 
-unsigned long long* tc_fallback_counter_ptr();  // mlp_tc.cu
+__device__ unsigned long long g_tc_fallbacks;  // re-runs of a tensor-core launch that fired (b200rl_tc_fallback_count)
 
 __device__ __forceinline__ float apply_act(float z, int kind) {
   if (kind == B200RL_ACT_TANH) return tanhf(z);
@@ -224,7 +227,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_fused_kernel(const FusedAr
   if (p.skip_flag != nullptr && *p.skip_flag != 0) return;  // early stop: the whole launch is a no-op
   if (p.run_if != nullptr) {
     if (*p.run_if != p.seq) return;  // the tensor-core result stands
-    if (blockIdx.x == 0 && tid == 0 && p.rerun_counter != nullptr) atomicAdd(p.rerun_counter, 1ull);
+    if (blockIdx.x == 0 && tid == 0) atomicAdd(&g_tc_fallbacks, 1ull);
   }
   // the consumer reduces total_rows partial rows: those beyond this grid are zero
   for (int row = (int)gridDim.x + (int)blockIdx.x; row < p.total_rows; row += (int)gridDim.x) {
@@ -574,29 +577,28 @@ static int fused_grid(const MlpLayout& lay, int64_t n_rows) {
   return (int)(tiles < sms ? (tiles < 1 ? 1 : tiles) : sms);
 }
 
-// tensor-core path (mlp_tc.cu)
+// fp16 x 2 tensor-core kernels (mlp_tc2.cu, mlp_tc_fvp.cu): two partial rows per CTA
 bool tc_shape_ok(const b200rl_mlp_desc& d);
-int launch_mlp_tc(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, cudaStream_t s);
-// second-generation tensor-core path (mlp_tc2.cu): fp16 x 2 splits, two partial rows per CTA
 int launch_mlp_tc2(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, int total_rows, cudaStream_t s);
-// B200RL_TC_MODE=bf16 pins the bf16 x 3 kernel (A/B runs); default is the fp16 x 2 kernel with bf16 x 3 as its
-// wide-range fallback
-int tc_fvp_total_rows(const b200rl_mlp_desc& mlp, int64_t n_rows);
-int tc_fwd_total_rows(const b200rl_mlp_desc& mlp, int64_t n_rows);
-static bool use_tc2() {
-  const char* e = getenv("B200RL_TC_MODE");
-  return !(e != nullptr && e[0] == 'b');
-}
+int launch_mlp_tc_fvp(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, int total_rows, cudaStream_t s);
 
-// B200RL_DISABLE_TC=1 forces the fp32 CUDA-core kernel (A/B parity runs); read on every call so tests can flip it.
-static bool use_tc(const b200rl_mlp_desc& d) {
+// The tensor-core kernels are in use for this network: its shape is in their gate, and B200RL_DISABLE_TC=1 (fp32
+// kernels only, for A/B parity runs) is not set.  Read on every call so tests can flip it.
+bool use_tc(const b200rl_mlp_desc& d) {
   const char* e = getenv("B200RL_DISABLE_TC");
   if (e != nullptr && e[0] == '1') return false;
   return tc_shape_ok(d);
 }
 
-// the fp16 x 2 tensor-core path is in use for this network (shape gate + the A/B environment switches)
-bool tc2_path_enabled(const b200rl_mlp_desc& d) { return use_tc(d) && use_tc2(); }
+// Partial rows of a tensor-core launch: its own two per CTA, or the grid of its fp32 re-run (with that layout) if that
+// is larger.  The consumer reduces this many rows whichever of the two kernels wrote them.
+static int tc_total_rows(const b200rl_mlp_desc& mlp, int64_t n_rows, bool backward, bool fvp) {
+  MlpLayout lay;
+  if (build_layout(mlp, backward, &lay, fvp)) return -1;
+  const int g = tc_grid(n_rows), f = fused_grid(lay, n_rows);
+  if (g <= 0 || f <= 0) return -1;
+  return 2 * g > f ? 2 * g : f;
+}
 
 }  // namespace b200rl
 
@@ -612,27 +614,18 @@ extern "C" int64_t b200rl_mlp_param_count(const b200rl_mlp_desc* mlp) {
   return p;
 }
 
-// with_backward: 0 forward only (EVAL), 1 forward + backward, 2 Fisher-vector product, 3 forward only with out_full / old_out /
-// NO_TC / a loss other than EVAL
-// (launches that use out_full / old_out / B200RL_FLAG_NO_TC)
+// with_backward: 0 forward only (EVAL), 1 forward + backward, 2 Fisher-vector product, 3 forward only with out_full /
+// old_out / NO_TC / a loss other than EVAL, 4 forward + backward on the fp32 kernel (NO_TC or train_log_std)
 extern "C" int b200rl_mlp_grid(const b200rl_mlp_desc* mlp, int64_t n_rows, int with_backward) {
   if (!mlp) return -1;
-  if (with_backward >= 0 && with_backward < 2 && use_tc(*mlp)) {
-    if (!use_tc2()) return tc_grid(n_rows);
-    const int g = tc_grid(n_rows);
-    return g > 0 ? 2 * g : -1;
-  }
-  if (with_backward == 2 && use_tc(*mlp) && use_tc2()) return tc_fvp_total_rows(*mlp, n_rows);
-  if (with_backward == 3 && use_tc(*mlp) && use_tc2()) return tc_fwd_total_rows(*mlp, n_rows);
+  const bool backward = with_backward == 1 || with_backward == 2 || with_backward == 4, fvp = with_backward == 2;
+  if (with_backward >= 0 && with_backward <= 3 && use_tc(*mlp)) return tc_total_rows(*mlp, n_rows, backward, fvp);
   MlpLayout lay;
-  if (build_layout(*mlp, with_backward == 1 || with_backward == 2 || with_backward == 4, &lay, with_backward == 2)) return -1;
+  if (build_layout(*mlp, backward, &lay, fvp)) return -1;
   return fused_grid(lay, n_rows);
 }
 
 namespace b200rl {
-int tc_fvp_total_rows(const b200rl_mlp_desc& mlp, int64_t n_rows);
-int launch_mlp_tc_fvp(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, int total_rows, cudaStream_t s);
-
 // the fp32 kernel, optionally as the predicated re-run of a tensor-core launch (run_if / seq / total_rows)
 static int launch_fused(const b200rl_mlp_loss_grad_args* a, const unsigned* run_if, unsigned seq, int total_rows,
                         cudaStream_t s) {
@@ -644,7 +637,6 @@ static int launch_fused(const b200rl_mlp_loss_grad_args* a, const unsigned* run_
   k.run_if = run_if;
   k.seq = seq;
   k.total_rows = total_rows;
-  k.rerun_counter = run_if != nullptr ? tc_fallback_counter_ptr() : nullptr;
   const int mode = fvp ? 2 : (backward ? 1 : 0);
   const size_t smem_bytes = (size_t)k.lay.total_floats * sizeof(float);
   const size_t static_bytes = fused_static_smem(k.lay.tm, mode);
@@ -704,25 +696,14 @@ int launch_fused_fallback(const b200rl_mlp_loss_grad_args* a, const unsigned* ru
   return launch_fused(a, run_if, seq, total_rows, s);
 }
 
-// partial rows of a forward-only launch that carries out_full / old_out / B200RL_FLAG_NO_TC (b200rl_mlp_grid mode 3): the
-// fp16 kernel's two per CTA, or the fp32 kernel's grid (its re-run, or the launch itself under NO_TC) if that is larger
-int tc_fwd_total_rows(const b200rl_mlp_desc& mlp, int64_t n_rows) {
-  MlpLayout lay;
-  if (build_layout(mlp, false, &lay, false)) return -1;
-  const int g = tc_grid(n_rows), f = fused_grid(lay, n_rows);
-  if (g <= 0 || f <= 0) return -1;
-  return 2 * g > f ? 2 * g : f;
-}
-
-// partial rows of a tensor-core FVP launch: its own two per CTA, or the fp32 re-run's grid if that is larger
-int tc_fvp_total_rows(const b200rl_mlp_desc& mlp, int64_t n_rows) {
-  MlpLayout lay;
-  if (build_layout(mlp, true, &lay, true)) return -1;
-  const int g = tc_grid(n_rows), f = fused_grid(lay, n_rows);
-  if (g <= 0 || f <= 0) return -1;
-  return 2 * g > f ? 2 * g : f;
-}
 }  // namespace b200rl
+
+extern "C" int64_t b200rl_tc_fallback_count(void) {
+  unsigned long long v = 0;
+  if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+  if (cudaMemcpyFromSymbol(&v, g_tc_fallbacks, sizeof(v)) != cudaSuccess) return -1;
+  return (int64_t)v;
+}
 
 extern "C" int b200rl_mlp_loss_grad(const b200rl_mlp_loss_grad_args* a, void* stream) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -736,7 +717,7 @@ extern "C" int b200rl_mlp_loss_grad(const b200rl_mlp_loss_grad_args* a, void* st
   const int L = k.lay.L;
   B200RL_REQUIRE(a->n_rows >= 0, "mlp_loss_grad: negative n_rows");
   if (a->n_rows == 0) {  // an empty shard (data-parallel ranks may hold none): every partial row is zero
-    const int rows = b200rl_mlp_grid(&a->mlp, 0, fvp ? 2 : (backward ? 1 : ((a->out_full || a->old_out || (a->flags & B200RL_FLAG_NO_TC) || a->loss != B200RL_LOSS_EVAL) ? 3 : 0)));
+    const int rows = b200rl_mlp_grid(&a->mlp, 0, fvp ? 2 : (backward ? 1 : 0));
     B200RL_REQUIRE(rows > 0, "mlp_loss_grad: no CUDA device");
     if (backward) B200RL_REQUIRE(a->partials, "mlp_loss_grad: partials is NULL");
     if (backward)
@@ -766,23 +747,17 @@ extern "C" int b200rl_mlp_loss_grad(const b200rl_mlp_loss_grad_args* a, void* st
     if (fvp) B200RL_REQUIRE(a->direction, "mlp_loss_grad: FVP needs the direction vector");
   }
   if (backward) B200RL_REQUIRE(a->partials, "mlp_loss_grad: partials is NULL");
-  const int64_t n_glob_all = a->n_global > 0 ? a->n_global : a->n_rows;
-  if (fvp && use_tc(a->mlp) && use_tc2() && !(a->flags & B200RL_FLAG_NO_TC) && !a->out_full && !a->old_out) {
-    const int total = tc_fvp_total_rows(a->mlp, a->n_rows);
-    B200RL_REQUIRE(total > 0, "mlp_loss_grad: no CUDA device");
-    return launch_mlp_tc_fvp(a, n_glob_all, total, s);
-  }
-  // raw outputs / the true KL exist on the fp16 kernel's forward-only variant (not on the bf16 x 3 kernel, not with backward)
+  const int64_t n_glob = a->n_global > 0 ? a->n_global : a->n_rows;
+  // The tensor-core kernels take a launch in their shape gate unless it sets NO_TC.  They produce raw outputs / the
+  // true KL on mlp_tc2's forward-only variant only, and dLoss/dlog_std not at all (FVP launches ignore train_log_std).
   const bool wants_out = a->out_full != nullptr || a->old_out != nullptr;
-  const bool out_on_tc = wants_out && forward_only && use_tc2();
-  const bool needs_fp32 = fvp || (wants_out && !out_on_tc) || (a->flags & B200RL_FLAG_NO_TC) || a->train_log_std;
-  // forward-only launches whose re-run is the fp32 kernel (raw outputs / true KL, a loss other than EVAL) or that run on
-  // it outright (NO_TC) write b200rl_mlp_grid(mode 3) partial rows
-  const bool mode3 = forward_only && (wants_out || (a->flags & B200RL_FLAG_NO_TC) || a->loss != B200RL_LOSS_EVAL);
-  const int rows3 = (mode3 && use_tc(a->mlp) && use_tc2()) ? tc_fwd_total_rows(a->mlp, a->n_rows) : 0;
-  if (!needs_fp32 && use_tc(a->mlp)) {
-    const int64_t n_glob_tc = a->n_global > 0 ? a->n_global : a->n_rows;
-    return use_tc2() ? launch_mlp_tc2(a, n_glob_tc, rows3, s) : launch_mlp_tc(a, n_glob_tc, s);
+  const bool tc = use_tc(a->mlp) && !(a->flags & B200RL_FLAG_NO_TC) && (forward_only || !wants_out);
+  if (tc && (fvp || !a->train_log_std)) {
+    const int rows = tc_total_rows(a->mlp, a->n_rows, backward, fvp);
+    B200RL_REQUIRE(rows > 0, "mlp_loss_grad: no CUDA device");
+    return fvp ? launch_mlp_tc_fvp(a, n_glob, rows, s) : launch_mlp_tc2(a, n_glob, rows, s);
   }
-  return launch_fused(a, nullptr, 0u, rows3, s);
+  // a forward-only launch in the gate writes the partial rows b200rl_mlp_grid reports for the tensor-core path
+  const int rows = forward_only && use_tc(a->mlp) ? tc_total_rows(a->mlp, a->n_rows, false, false) : 0;
+  return launch_fused(a, nullptr, 0u, rows, s);
 }

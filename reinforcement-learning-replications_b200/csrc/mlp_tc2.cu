@@ -1,11 +1,13 @@
-// mlp_tc2: second-generation tensor-core kernel for the fused MLP step (wgmma, sm_90a).
+// mlp_tc2: tensor-core kernel for the fused MLP step (wgmma, sm_90a).
 //
-// Same contract and data flow as mlp_tc.cu / mlp_fused.cu (see mlp_fused.cu for the reference file:line map) and the
-// same shape gate (3 Linear layers, tanh hidden layers of width <= 64 -- zero-padded to 64 --, obs <= 32, out <= 15).
-// What changed against the bf16 x 3 kernel, and why.  The kernels were first written for B200 (tcgen05); the figures in
-// this note were measured there with the per-stage clocks of tools/profile_step.py, not on H100:
+// Same contract and data flow as mlp_fused.cu (see there for the reference file:line map).  Shape gate (tc_shape_ok,
+// shared with mlp_tc_fvp.cu): 3 Linear layers, tanh hidden layers of width <= 64 -- zero-padded to 64 --, identity
+// output, obs <= 32, out <= 15.
+// Why two fp16 splits and not three bf16 ones (a first kernel split every operand into three bf16 values and ran six
+// products per logical product).  The kernels were first written for B200 (tcgen05); the figures in this note were
+// measured there with the per-stage clocks of tools/profile_step.py, not on H100:
 //   * a tcgen05.mma of these small shapes cost 30..50 cycles on B200 whatever its size (instruction floor / SS-mode
-//     operand feed), so the 282 MMAs per 128-row tile of the bf16 x 3 kernel -- not the math -- set its pace.  Here every
+//     operand feed), so the 282 MMAs per 128-row tile of that kernel -- not the math -- set its pace.  Here every
 //     fp32 operand is split into TWO fp16 values x*2^e = h + l (22 mantissa bits, 3.0e-7 worst-case relative error
 //     per product with the (l,l) term dropped) after an exact power-of-two pre-scale that parks it in fp16's normal
 //     range.  A logical product is then 3 MMAs (h.l, l.h, h.h) on the forward/back-propagation chain and 2 MMAs for
@@ -24,7 +26,7 @@
 // fp16 has a narrow exponent range: the scales come from the data (max |W| per layer computed per CTA, max |obs| and
 // max |target| from a pre-pass or the caller) and every converted value is range-checked.  A launch that sees a
 // value outside +-60000 after scaling raises its slot in a status ring and the host has already queued the
-// bf16 x 3 kernel (mlp_tc.cu, unlimited range) behind it, predicated on that slot: it recomputes the launch.
+// fp32 kernel (mlp_fused.cu, unlimited range) behind it, predicated on that slot: it recomputes the launch.
 // The two halves of the stacked accumulators are emitted as TWO partial rows per CTA (b200rl_mlp_grid reports
 // 2 x CTAs), so the fixed-order reduction of b200rl_reduce_partials adds them -- no in-kernel combine.
 #include <cuda_fp16.h>
@@ -104,7 +106,7 @@ struct Tc2Args {
   const float* target_absmax;  // device scalar (MSE) or NULL
   float* out_full;             // forward-only launches: raw network outputs [n_rows, n_out]
   const float* old_out;        // forward-only launches: outputs of the old policy -> true KL(old || new) in scalar 6
-  int total_rows;              // partial rows the consumer reduces when that is more than two per CTA (else 0)
+  int total_rows;              // partial rows the consumer reduces (at least two per CTA)
   unsigned* status;            // status-ring slot of this launch
   unsigned seq;                // value to store there when the launch must be redone by the wide-range kernel
   float* acc_mem;              // accumulator memory, ACC_CTA_FLOATS per CTA (tc_common.cuh)
@@ -713,7 +715,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) mlp_tc2_kernel(const Tc2Args p)
 
   // ---- teardown ----
   __syncthreads();
-  if (tid == 0 && *s_bad != 0) *p.status = p.seq;  // this launch is redone by the bf16 x 3 kernel queued behind it
+  if (tid == 0 && *s_bad != 0) *p.status = p.seq;  // this launch is redone by the fp32 kernel queued behind it
 }
 
 // max |x| over a device array (pre-pass for the observation / target scale when the caller gave no hint)
@@ -795,11 +797,16 @@ int launch_absmax_cols(const float* x, long long rows, int cols, float* out, cud
   return 0;
 }
 
-int launch_mlp_tc_fallback(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, const unsigned* run_if, unsigned seq,
-                           int partial_rows, cudaStream_t s);
 int launch_fused_fallback(const b200rl_mlp_loss_grad_args* a, const unsigned* run_if, unsigned seq, int total_rows,
                           cudaStream_t s);  // mlp_fused.cu: the fp32 kernel as the predicated re-run
 
+bool tc_shape_ok(const b200rl_mlp_desc& d) {
+  return d.n_layers == 3 && d.sizes[1] >= 1 && d.sizes[1] <= 64 && d.sizes[2] >= 1 && d.sizes[2] <= 64 &&
+         d.sizes[0] >= 1 && d.sizes[0] <= 32 &&
+         d.sizes[3] >= 1 && d.sizes[3] <= 15 && d.hidden_act == B200RL_ACT_TANH && d.out_act == B200RL_ACT_IDENTITY;
+}
+
+// total_rows: the partial rows the consumer reduces (b200rl_mlp_grid), at least two per CTA
 int launch_mlp_tc2(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, int total_rows, cudaStream_t s) {
   unsigned* status_slot = nullptr;
   unsigned seq = 0;
@@ -862,12 +869,8 @@ int launch_mlp_tc2(const b200rl_mlp_loss_grad_args* a, int64_t n_glob, int total
     mlp_tc2_kernel<false><<<grid, T2_THREADS, T2_SMEM_BYTES, s>>>(k);
   B200RL_CUDA(cudaGetLastError());
   count_launch(launches + 1);
-  // wide-range re-run, predicated on this launch's status slot (a few microseconds when it does not fire); the bf16 x 3
-  // kernel does not produce raw outputs / the true KL, the fp32 kernel does
-  const int rows = total_rows > 2 * grid ? total_rows : 2 * grid;
-  if (a->out_full != nullptr || a->old_out != nullptr || (!backward && a->loss != B200RL_LOSS_EVAL))
-    return launch_fused_fallback(a, status_slot, seq, rows, s);
-  return launch_mlp_tc_fallback(a, n_glob, status_slot, seq, rows, s);
+  // wide-range re-run, predicated on this launch's status slot (a few microseconds when it does not fire)
+  return launch_fused_fallback(a, status_slot, seq, total_rows, s);
 }
 
 }  // namespace b200rl

@@ -168,8 +168,8 @@ __device__ __forceinline__ void wg_mma(float (&d)[N / 2], const uint32_t (&alo)[
   for (int s = 0; s < TERMS; ++s)
 #pragma unroll
     for (int k = 0; k < KSTEPS; ++k)
-      wgmma_run<N, false, TA, TB>(d, ((uint64_t)a_hi << 32) | (alo[s] + (uint32_t)k * a_k),
-                                  ((uint64_t)b_hi << 32) | (blo[s] + (uint32_t)k * b_k), s == 0 && k == 0 ? accumulate : 1u);
+      wgmma_run<N, TA, TB>(d, ((uint64_t)a_hi << 32) | (alo[s] + (uint32_t)k * a_k),
+                           ((uint64_t)b_hi << 32) | (blo[s] + (uint32_t)k * b_k), s == 0 && k == 0 ? accumulate : 1u);
   wgmma_commit();
   wgmma_wait_all();
 }

@@ -1,6 +1,6 @@
-// Per-row distribution and loss math of the on-policy kernels (mlp_fused.cu, mlp_tc.cu, mlp_tc2.cu, mlp_tc3.cu,
-// mlp_tc_fvp.cu): log-prob, entropy, d logp / d out, the PPO / VPG / TRPO surrogates, the value MSE, TRPO's true KL
-// and its Fisher metric.  One thread evaluates one row.  The functions take pointers and sizes, so every kernel keeps
+// Per-row distribution and loss math of the on-policy kernels (mlp_fused.cu, mlp_tc2.cu, mlp_tc3.cu, mlp_tc_fvp.cu):
+// log-prob, entropy, d logp / d out, the PPO / VPG / TRPO surrogates, the value MSE, TRPO's true KL and its Fisher
+// metric.  One thread evaluates one row.  The functions take pointers and sizes, so every kernel keeps
 // its own layout: outputs, actions and tangents may sit in registers or shared memory; inputs read from global memory
 // are passed as Ldg.  Loops over the action dimension run to the compile-time bound NA (15 in the tensor-core kernels,
 // 16 in the fp32 kernel) and are guarded by a < A_out.
@@ -31,7 +31,7 @@ __device__ __forceinline__ NormalConsts normal_consts(const float* log_std, int 
 }
 
 // The two ways the kernels divide by the variance.  They round differently, so each kernel keeps its own.
-// VarDiv divides, as torch does: the fp32 and bf16 x 3 kernels.
+// VarDiv divides, as torch does: the fp32 kernel, which also recomputes the fp16 launches that leave fp16's range.
 struct VarDiv {
   const float* var;
   __device__ __forceinline__ float over_var(float x, int a) const { return x / var[a]; }

@@ -156,60 +156,17 @@ __device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t a, uint64
       : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
       : "memory");
 }
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_bf16_n16(float (&d)[8], uint64_t a, uint64_t b, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
-      : "memory");
-}
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_bf16_n32(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
-      : "memory");
-}
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_bf16_n48(float (&d)[24], uint64_t a, uint64_t b, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, %27, %28;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
-      : "memory");
-}
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_bf16_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
-      : "memory");
-}
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-template <int N, bool BF16, int TA, int TB>
+template <int N, int TA, int TB>
 __device__ __forceinline__ void wgmma_run(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
-  if constexpr (BF16) {
-    if constexpr (N == 16) wgmma_bf16_n16<TA, TB>(d, a, b, scale_d);
-    else if constexpr (N == 32) wgmma_bf16_n32<TA, TB>(d, a, b, scale_d);
-    else if constexpr (N == 48) wgmma_bf16_n48<TA, TB>(d, a, b, scale_d);
-    else wgmma_bf16_n64<TA, TB>(d, a, b, scale_d);
-  } else {
-    if constexpr (N == 16) wgmma_f16_n16<TA, TB>(d, a, b, scale_d);
-    else if constexpr (N == 32) wgmma_f16_n32<TA, TB>(d, a, b, scale_d);
-    else if constexpr (N == 48) wgmma_f16_n48<TA, TB>(d, a, b, scale_d);
-    else wgmma_f16_n64<TA, TB>(d, a, b, scale_d);
-  }
+  if constexpr (N == 16) wgmma_f16_n16<TA, TB>(d, a, b, scale_d);
+  else if constexpr (N == 32) wgmma_f16_n32<TA, TB>(d, a, b, scale_d);
+  else if constexpr (N == 48) wgmma_f16_n48<TA, TB>(d, a, b, scale_d);
+  else wgmma_f16_n64<TA, TB>(d, a, b, scale_d);
 }
 
 // Operand majors (template arguments TA / TB of the products): K-major, or MN-major (read transposed).
@@ -217,9 +174,9 @@ constexpr int K_MAJOR = 0, MN_MAJOR = 1;
 
 // Accumulator columns acc_col .. acc_col + N - 1 (+)= sum over `terms` of A_t B_t, each `ksteps` k-steps of 16
 // (descriptor low words advance by a_k / b_k per k-step; the high words are shared); the first product overwrites
-// unless `acc_first`.  M = 128 runs as two m64nNk16 halves (A's low word advanced to rows 64..127); M = 64 as one, its
-// row m stored at row (m % 16) + 32 (m / 16).  Executed by all 128 threads of the issuing warpgroup.
-template <int N, bool BF16, int TA, int TB, bool M64, int T>
+// unless `acc_first`.  M = 128 runs as two m64nNk16 halves (A's low word advanced to rows 64..127).  Executed by all
+// 128 threads of the issuing warpgroup.
+template <int N, int TA, int TB, int T>
 __device__ __forceinline__ void mma_product(float* acc_cta, uint32_t acc_col, const uint32_t (&alo)[T],
                                             const uint32_t (&blo)[T], int terms, uint32_t a_hi, uint32_t b_hi,
                                             uint32_t a_k, uint32_t b_k, int ksteps, bool acc_first) {
@@ -229,12 +186,11 @@ __device__ __forceinline__ void mma_product(float* acc_cta, uint32_t acc_col, co
   const uint32_t a_half = TA == MN_MAJOR ? ((alo[0] >> 16) & 0x3FFFu) : (64u * 128u) >> 4;
   float* acc = acc_cta + acc_col * ACC_LANES;
 #pragma unroll 1
-  for (int h = 0; h < (M64 ? 1 : 2); ++h) {
+  for (int h = 0; h < 2; ++h) {
     // this thread's fragment (wgmma D layout): rows m0 and m0 + 8, columns 2 (l % 4) + 8 j + {0, 1}.  One base
     // pointer, the rest immediate offsets: per-element offsets would be loop-invariant and kept live across the issuer.
     const int m0 = 16 * w + (l >> 2) + 64 * h;
-    const int row0 = M64 ? (m0 & 15) + 32 * (m0 >> 4) : m0;
-    float* frag = acc + 2 * (l & 3) * ACC_LANES + row0;
+    float* frag = acc + 2 * (l & 3) * ACC_LANES + m0;
     float d[N / 2];
 #pragma unroll
     for (int i = 0; i < N / 2; ++i)
@@ -247,7 +203,7 @@ __device__ __forceinline__ void mma_product(float* acc_cta, uint32_t acc_col, co
       uint32_t a = alo[s] + (uint32_t)h * a_half, b = blo[s];
 #pragma unroll 1
       for (int k = 0; k < ksteps; ++k) {
-        wgmma_run<N, BF16, TA, TB>(d, ((uint64_t)a_hi << 32) | a, ((uint64_t)b_hi << 32) | b, scale);
+        wgmma_run<N, TA, TB>(d, ((uint64_t)a_hi << 32) | a, ((uint64_t)b_hi << 32) | b, scale);
         scale = 1u;
         a += a_k;
         b += b_k;

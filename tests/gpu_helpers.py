@@ -39,8 +39,9 @@ def gae_scan(rew, values, last_values, ep_offsets, ep_done, gamma=0.99, lam=0.97
 
 
 def loss_grad(sizes, flat, obs, loss, dist="none", act=None, log_std=None, adv_raw=None, adv_stats=None, old_logp=None,
-              target=None, clip=0.2, hidden_act="tanh", n_global=0, want_rows=True):
-    """Returns dict(grad, scalars[8], rows)."""
+              target=None, clip=0.2, hidden_act="tanh", n_global=0, want_rows=True, obs_absmax=None):
+    """Returns dict(grad, scalars[8], rows).  obs_absmax: the per-feature range hint of the fp16 kernels (default: the
+    library's pre-pass computes it)."""
     lib = _lib.load()
     a = LossGradArgs()
     a.mlp = MlpDesc.make(sizes, hidden_act, "identity")
@@ -53,7 +54,8 @@ def loss_grad(sizes, flat, obs, loss, dist="none", act=None, log_std=None, adv_r
     assert grid > 0
     keep = dict(params=dev(flat, np.float32), obs=dev(obs, np.float32))
     for k, v, dt in (("actions", act, np.float32), ("log_std", log_std, np.float32), ("adv_raw", adv_raw, np.float32),
-                     ("adv_stats", adv_stats, np.float64), ("old_logp", old_logp, np.float32), ("target", target, np.float32)):
+                     ("adv_stats", adv_stats, np.float64), ("old_logp", old_logp, np.float32), ("target", target, np.float32),
+                     ("obs_absmax", obs_absmax, np.float32)):
         if v is not None:
             keep[k] = dev(v, dt)
     rows = torch.zeros(max(n, 1), dtype=torch.float32, device="cuda") if want_rows else None

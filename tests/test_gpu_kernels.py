@@ -228,8 +228,8 @@ def test_tc2_scaled_operands_stay_on_the_fp16_path(obs_scale, w_scale, ret_scale
 
 def test_tc2_out_of_range_launch_is_redone_by_the_wide_range_kernel():
     """One observation of 1e30 cannot be represented after scaling (the rest of the batch underflows next to it is
-    fine, but a gradient outlier 1e12 times the typical one is not): the status slot fires and the bf16 x 3 kernel
-    queued behind recomputes the launch -- results still match the oracle."""
+    fine, but a gradient outlier 1e12 times the typical one is not): the status slot fires and the fp32 kernel queued
+    behind recomputes the launch -- results still match the oracle."""
     from gpu_helpers import loss_grad
     rng = np.random.default_rng(6)
     n, sizes = 2000, [17, 64, 64, 6]
@@ -257,35 +257,24 @@ def test_tc2_nan_input_is_reported_not_hidden():
     assert np.isnan(r["rows"][3]) and np.isfinite(np.delete(r["rows"], 3)).all()
 
 
-def test_tc_mode_bf16_matches(monkeypatch):
-    """B200RL_TC_MODE=bf16 pins the bf16 x 3 kernel (one partial row per CTA): same results through the same ABI."""
-    from gpu_helpers import loss_grad
-    rng = np.random.default_rng(9)
-    n, sizes = 4000, [17, 64, 64, 1]
-    layers = _net(rng, sizes)
-    obs = rng.standard_normal((n, sizes[0])).astype(np.float32)
-    ret = (5 * rng.standard_normal(n)).astype(np.float32)
-    ref = O.value_loss_and_grad(layers, obs, ret)
-    fast = loss_grad(sizes, O.flatten_layers(layers), obs, "mse", "none", target=ret)
-    monkeypatch.setenv("B200RL_TC_MODE", "bf16")
-    wide = loss_grad(sizes, O.flatten_layers(layers), obs, "mse", "none", target=ret)
-    assert rel_err(fast["grad"], ref["grad"]) < TOL and rel_err(wide["grad"], ref["grad"]) < TOL
-    assert rel_err(fast["grad"], wide["grad"]) < TOL
-
-
+@pytest.mark.parametrize("outlier", [None, 1e6], ids=["in_range", "obs_row_1e6"])
 @pytest.mark.parametrize("sizes", [[17, 64, 32, 6], [9, 33, 20, 3]])
-def test_padded_hidden_widths_on_the_wide_range_kernel(sizes, monkeypatch):
-    """Hidden layers narrower than 64 are zero-padded inside both tensor-core kernels (B200RL_TC_MODE=bf16 pins the
-    bf16 x 3 one, which is also the re-run path of the fp16 kernel)."""
+def test_padded_hidden_widths_on_the_wide_range_kernel(sizes, outlier):
+    """Hidden layers narrower than 64 are zero-padded inside the fp16 kernel; with one observation row of 1e6 in every
+    feature (every other row then sits below the precision guard) the launch is redone by the fp32 kernel, which takes
+    the same shapes."""
     from gpu_helpers import loss_grad
-    monkeypatch.setenv("B200RL_TC_MODE", "bf16")
     rng = np.random.default_rng(21)
     n = 3001
     vs = sizes[:-1] + [1]
     layers = _net(rng, vs)
     obs = rng.standard_normal((n, vs[0])).astype(np.float32)
+    if outlier is not None:
+        obs[11] = np.float32(outlier)
     ret = (5 * rng.standard_normal(n)).astype(np.float32)
+    before = _fallbacks()
     r = loss_grad(vs, O.flatten_layers(layers), obs, "mse", "none", target=ret)
+    assert _fallbacks() == before + (outlier is not None)
     ref = O.value_loss_and_grad(layers, obs, ret)
     assert rel_err(r["grad"], ref["grad"]) < TOL
 

@@ -3,15 +3,18 @@ tensor, at the edges of each kernel's shape gate and at the edges of the distrib
 
 Paths, chosen with the switches the library reads on every call:
 * "tc2": fp16 x 2 tensor-core kernel (mlp_tc2.cu), the default for 3-layer Tanh networks with obs <= 32, hidden <= 64,
-  out <= 15.  Asserted by the fallback counter staying put (a launch that leaves fp16's range is redone by mlp_tc.cu).
-* "tc": bf16 x 3 tensor-core kernel (mlp_tc.cu), B200RL_TC_MODE=bf16.  Asserted by its grid (one partial row per CTA).
+  out <= 15.  Asserted by the fallback counter staying put (a launch that leaves fp16's range is redone by the fp32
+  kernel, mlp_fused.cu).
+* "rerun": the default path with an obs_absmax hint 1e6 times the largest |observation|, which puts every row below
+  the fp16 kernel's precision guard: each launch is redone by the fp32 kernel queued behind it, into the tensor-core
+  path's partial rows.  Asserted by the fallback counter (+1 per launch) and by the grid.
 * "fp32": the CUDA-core kernel (mlp_fused.cu), B200RL_DISABLE_TC=1 or any shape outside the gate.  Asserted by its grid
   at 640 rows: 10, 20 or 40 CTAs for tiles of 64, 32 or 16 rows.
 * FVP: mlp_tc_fvp.cu inside the gate, the fp32 kernel's FVP mode outside it (or under B200RL_DISABLE_TC=1).
 * the fused PPO step (mlp_tc3.cu) through the engine, asserted by last_update_stats.fused.
 
-Bars.  One per arithmetic: BAR["fp16x2"] (mlp_tc2 and mlp_tc3), BAR["bf16x3"], BAR["fp32"], BAR["fvp"] (both FVP
-kernels), each about 4x the largest error measured on an H100 over all cases of its path.  Every quantity is measured
+Bars.  One per arithmetic: BAR["fp16x2"] (mlp_tc2 and mlp_tc3), BAR["fp32"], BAR["fvp"] (both FVP kernels), each
+about 4x the largest error measured on an H100 over all cases of its path.  Every quantity is measured
 against the scale of its own float32 rounding: per-row vectors and F v against max |ref| of that tensor; each W / b
 gradient against the largest, over its entries, sum over rows of |that row's contribution| (oracle/onpolicy_f64),
 since a gradient whose rows cancel is only known to ~2^-24 of that however the kernel sums it; the loss sum against
@@ -33,13 +36,13 @@ from oracle import onpolicy_f64 as R
 pytestmark = pytest.mark.gpu
 
 # Largest errors measured on an H100 over all cases of each path (gradients against their conditioning scale):
-# fp16x2 2.1e-6, bf16x3 2.0e-6, fp32 1.8e-6, fvp 1.4e-6; each bar is about 4x that.  The first three are the one-row
+# fp16x2 2.1e-6, fp32 1.8e-6, fvp 1.4e-6; each bar is about 4x that.  The first two are the one-row
 # case, whose single row gets no averaging of its rounding errors; every multi-row case stays under 1.5e-6.  The fused
 # step (mlp_tc3, fp16x2) measured on an H100 80GB HBM3 at 700 W: gradients at most 4.1e-7 (one tile of 65 rows), with
 # no growth in tiles per CTA (largest policy / value tensor 6.6e-8 / 3.0e-8 at 1 tile per CTA, 3.8e-8 / 1.2e-7 at 4-5,
 # 3.4e-8 / 1.6e-7 at 9); its scalar sums at most 1.2e-6 (the PPO loss sum with 8-sigma actions).
-BAR = {"fp16x2": 8e-6, "bf16x3": 8e-6, "fp32": 7e-6, "fvp": 6e-6}
-ARITH = {"tc2": "fp16x2", "tc": "bf16x3", "fp32": "fp32"}
+BAR = {"fp16x2": 8e-6, "fp32": 7e-6, "fvp": 6e-6}
+ARITH = {"tc2": "fp16x2", "rerun": "fp32", "fp32": "fp32"}
 CLIP, CLIP_MARGIN, KINK = 0.2, 1e-3, 1e-6
 # the fp32 kernel's limits for a [17, h, h, 6] policy: the largest equal hidden width whose backward layout fits
 # 227 KiB of shared memory, and the largest whose Fisher-vector-product layout does (README)
@@ -80,12 +83,10 @@ def mixed_tiles():
 
 @pytest.fixture
 def path(request, monkeypatch):
-    for k in ("B200RL_TC_MODE", "B200RL_DISABLE_TC", "B200RL_FUSED_STEP"):
+    for k in ("B200RL_DISABLE_TC", "B200RL_FUSED_STEP"):
         monkeypatch.delenv(k, raising=False)
     name = getattr(request, "param", "default")
-    if name == "tc":
-        monkeypatch.setenv("B200RL_TC_MODE", "bf16")
-    elif name == "fp32":
+    if name == "fp32":
         monkeypatch.setenv("B200RL_DISABLE_TC", "1")
     return name
 
@@ -205,9 +206,10 @@ def report(label, arith, errs):
         assert v < BAR[arith], (label, k, v, BAR[arith])
 
 
-def run_policy_and_value(pb, launch_check):
+def run_policy_and_value(pb, launch_check, obs_absmax=None):
     """Every policy loss, the evaluation launch, the value MSE and the value evaluation of one problem; returns the
-    per-quantity errors.  launch_check(what) is a context manager around each launch (Fired)."""
+    per-quantity errors.  launch_check(what) is a context manager around each launch (Fired); obs_absmax: the range
+    hint every launch passes (default none: the library's pre-pass)."""
     from gpu_helpers import loss_grad
     s, dist, n, h = pb["sizes"], pb["dist"], pb["n"], pb["hidden"]
     errs = {}
@@ -215,7 +217,7 @@ def run_policy_and_value(pb, launch_check):
         with launch_check(loss):
             got = loss_grad(s, pb["flat"], pb["obs"], loss, dist, act=pb["act"], log_std=pb["log_std"],
                             adv_raw=pb["adv_raw"], adv_stats=pb["stats"], old_logp=pb["old_logp"], clip=CLIP,
-                            hidden_act=h)
+                            hidden_act=h, obs_absmax=obs_absmax)
         ref = R.policy_loss(pb["flat"], s, pb["obs"], pb["act"], dist, loss, pb["log_std"], pb["adv_raw"], pb["stats"],
                             pb["old_logp"], CLIP, h)
         errs.update(grad_errs(got["grad"], ref, s, f"{loss}.d"))
@@ -228,7 +230,8 @@ def run_policy_and_value(pb, launch_check):
         if loss == "ppo_clip" and n >= 100:
             assert (ref["ratio"] > 1 + CLIP).any() and (ref["ratio"] < 1 - CLIP).any()  # the clip binds both ways
     with launch_check("eval"):
-        got = loss_grad(s, pb["flat"], pb["obs"], "eval", dist, act=pb["act"], log_std=pb["log_std"], hidden_act=h)
+        got = loss_grad(s, pb["flat"], pb["obs"], "eval", dist, act=pb["act"], log_std=pb["log_std"], hidden_act=h,
+                        obs_absmax=obs_absmax)
     ref = R.policy_loss(pb["flat"], s, pb["obs"], pb["act"], dist, "eval", pb["log_std"], hidden=h)
     sc = got["scalars"]
     errs["eval.logp"] = rel_err(got["rows"], ref["logp"])
@@ -237,19 +240,20 @@ def run_policy_and_value(pb, launch_check):
     errs["eval.logp2_sum"] = scal_err(sc[4], ref["logp2_sum"])
     assert sc[5] == n
     with launch_check("mse"):
-        got = loss_grad(pb["vs"], pb["vflat"], pb["obs"], "mse", "none", target=pb["ret"], hidden_act=h)
+        got = loss_grad(pb["vs"], pb["vflat"], pb["obs"], "mse", "none", target=pb["ret"], hidden_act=h,
+                        obs_absmax=obs_absmax)
     ref = R.value_loss(pb["vflat"], pb["vs"], pb["obs"], pb["ret"], h)
     errs.update(grad_errs(got["grad"], ref, pb["vs"], "mse.d"))
     errs["mse.loss"] = scal_err(got["scalars"][0], ref["loss_sum"])
     with launch_check("values"):
-        got = loss_grad(pb["vs"], pb["vflat"], pb["obs"], "eval", "none", hidden_act=h)
+        got = loss_grad(pb["vs"], pb["vflat"], pb["obs"], "eval", "none", hidden_act=h, obs_absmax=obs_absmax)
     errs["values"] = rel_err(got["rows"], ref["values"])
     return errs
 
 
 class Fired(dict):
     """Counts, per launch, how often the fp16 range guard fired (launches that left fp16's range are redone by the
-    bf16 x 3 kernel): ``with fired("ppo_clip"): ...``.  Checked after the errors are printed."""
+    fp32 kernel): ``with fired("ppo_clip"): ...``.  Checked after the errors are printed."""
 
     def __call__(self, what):
         return _Count(self, what)
@@ -294,13 +298,14 @@ GATE_CASES = {
     "actions_8_sigma": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=3000, log_std=-0.5, sigmas=8.0),
     "logits_30": dict(sizes=[8, 64, 64, 15], dist="categorical", n=3000, out_scale=30.0),
     # one observation row 1e6 times the others: after scaling, the other rows would lose their low fp16 splits, so the
-    # default path's guard has the bf16 x 3 kernel redo its launches (the predicated re-run)
+    # default path's guard has the fp32 kernel redo its launches (the predicated re-run)
     "obs_row_1e6": dict(sizes=[17, 64, 64, 6], dist="gaussian", n=2000, obs_outlier=1e6),
 }
-# launches of the default path that legitimately leave fp16's range (and are redone by the bf16 x 3 kernel):
+# launches of the default path that legitimately leave fp16's range (and are redone by the fp32 kernel):
 # {case: {launch: count}}.  The power-of-two pre-scales absorb log_std -5 / +1, 8-sigma actions and logits of +-30;
 # only the outlier row trips the guard, in every launch.
-TC2_TRIPS = {"obs_row_1e6": {k: 1 for k in ("ppo_clip", "vpg", "trpo_surrogate", "eval", "mse", "values")}}
+LAUNCHES = ("ppo_clip", "vpg", "trpo_surrogate", "eval", "mse", "values")
+TC2_TRIPS = {"obs_row_1e6": {k: 1 for k in LAUNCHES}}
 
 
 def rows_of(n):
@@ -313,23 +318,23 @@ def make(case, seed, hidden="tanh"):
     return policy_problem(sizes, dist, n, seed, hidden, **c)
 
 
-@pytest.mark.parametrize("path", ["tc2", "tc", "fp32"], indirect=True)
+@pytest.mark.parametrize("path", ["tc2", "rerun", "fp32"], indirect=True)
 @pytest.mark.parametrize("name", list(GATE_CASES))
 def test_gate_case(name, path):
     pb = make(GATE_CASES[name], seed=list(GATE_CASES).index(name))
     n = pb["n"]
-    if path == "tc2":
-        assert grid(pb["sizes"], n, 1) == 2 * tc_grid(n)
-    elif path == "tc":
-        assert grid(pb["sizes"], n, 1) == tc_grid(n)
-    else:
+    if path == "fp32":
         assert grid(pb["sizes"], 640, 1) == 10
+    else:  # the fp32 re-run writes the tensor-core path's partial rows, zeroing those past its own grid
+        assert grid(pb["sizes"], n, 1) == 2 * tc_grid(n)
+    hint = np.full(pb["sizes"][0], 1e6 * np.abs(pb["obs"]).max(), np.float32) if path == "rerun" else None
     fired = Fired()
-    errs = run_policy_and_value(pb, fired)
-    # launches the guard sent to the bf16 x 3 kernel carry that kernel's arithmetic
+    errs = run_policy_and_value(pb, fired, hint)
+    # launches the guard sent to the fp32 kernel carry that kernel's arithmetic
     report(f"{name} n={n}" + (f" fp16 range trips {dict(fired)}" if fired else ""),
-           "bf16x3" if fired else ARITH[path], errs)
-    assert fired == (TC2_TRIPS.get(name, {}) if path == "tc2" else {})
+           "fp32" if fired else ARITH[path], errs)
+    expect = {"tc2": TC2_TRIPS.get(name, {}), "rerun": {k: 1 for k in LAUNCHES}, "fp32": {}}[path]
+    assert fired == expect
 
 
 # ---- cases outside the gate: the fp32 kernel, at every tile height ------------------------------------------------

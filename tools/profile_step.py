@@ -27,17 +27,13 @@ if __name__ == "__main__":
         import torch
         torch.cuda.synchronize()
         out = (C.c_ulonglong * 24)()
-        kind = os.environ["B200RL_TC_TIMING"]
-        (_lib.load().b200rl_debug_tc2_timing if kind == "2" else _lib.load().b200rl_debug_tc_timing)(out)
-        names = (["obs", "F1wait", "act1", "F2wait", "act2", "F3wait", "loss", "S3wait", "dz2", "S4wait", "dz1", "S5wait",
-                  "offwait"] if kind != "2" else
-                 ["E0wait", "E0work", "E1wait", "E1work", "E2wait", "E2work", "E3wait", "E3work", "E4wait", "E4work",
-                  "E5wait", "E5work", "-"])
+        _lib.load().b200rl_debug_tc2_timing(out)
+        names = ["E0wait", "E0work", "E1wait", "E1work", "E2wait", "E2work", "E3wait", "E3work", "E4wait", "E4work",
+                 "E5wait", "E5work", "-"]
         tiles = (envs * 1000 // 128 + 147) // 148
         print("cycles per tile (CTA 0, last backward launch):", {n: int(out[i]) // tiles for i, n in enumerate(names)},
               "total", sum(int(out[i]) for i in range(13)) // tiles)
-        if kind == "2":
-            print("issuer cycles per tile:", {n: int(out[16 + i]) // tiles for i, n in
-                                              enumerate(["F1", "F2", "F3", "S3", "S4", "S5", "idle"])})
+        print("issuer cycles per tile:", {n: int(out[16 + i]) // tiles for i, n in
+                                          enumerate(["F1", "F2", "F3", "S3", "S4", "S5", "idle"])})
     from rl_replicas_b200 import _lib as _L
     print("tc fallbacks:", _L.load().b200rl_tc_fallback_count())

@@ -8,9 +8,10 @@
 //     once for both.  Rows are independent in the forward / backward chain, so each (network, 64-row half) is one
 //     warpgroup that issues its own m64 products and keeps the accumulator in registers: its epilogues work on the
 //     wgmma fragment and hand over to its next product through a warpgroup-local barrier.  A fifth warpgroup brings
-//     the observations in and issues the weight-gradient products (accumulators in L2, tc_common.cuh) off the chains'
-//     critical path; mbarriers tell it when both halves of a network have delivered a stage's operands, and tell the
-//     chains when it has finished reading a buffer they are about to overwrite;
+//     the observations in and issues the weight-gradient products off the chains' critical path; mbarriers tell it
+//     when both halves of a network have delivered a stage's operands, and tell the chains when it has finished
+//     reading a buffer they are about to overwrite.  Its accumulators stay in L2 (tc_common.cuh), stored fragment by
+//     fragment (grad_acc_off), and each fragment is prefetched into L1 while the products before it run (grad_mma);
 //   * the observations are split into their fp16 pairs ONCE PER UPDATE by pack_obs_kernel (every step of the update
 //     reads the same observations) into ready-made SWIZZLE_128B tile images [128 rows][h cols 0..31 | l cols 32..63];
 //     the step kernel brings a tile image in with ONE 16 KB bulk copy (cp.async.bulk + mbarrier complete_tx) issued by
@@ -65,7 +66,8 @@ constexpr uint32_t S3_END_SC = 1024;                 // [16 warps][8] doubles
 // per net: DW2 (64) | DB2 (16, col 15 = db2) | DW1 (64: products with X's h columns, then with its l columns; col 31 =
 // db1) | DW3 (32: products with dOut's h columns, then l).  The B operands of dW1 / dW3 hold their two splits side
 // by side in one swizzle atom, so ONE product per k-step covers both; the halves are added when the accumulators
-// are read, once per launch.  2 x 176 of the 512 columns.
+// are read, once per launch.  2 x 176 of the 512 columns; inside a product's columns the floats are fragment-major
+// (grad_acc_off), not (row, column).
 constexpr uint32_t ACC_GRAD_NET = 176;
 // Running b3 sums: rows are tile rows, column 16 m + a holds sum class m (0..3) of output a (policy a < 15, value
 // a = 15).  A row's output of tile k of network c goes to class (k + 2 c) & 3, and every class is added in tile order.
@@ -75,12 +77,29 @@ constexpr uint32_t ACC_DB3 = 2 * ACC_GRAD_NET;
 static_assert(ACC_DB3 + 4 * 16 <= ACC_COLS, "mlp_tc3 accumulator columns");
 constexpr uint32_t ACC_DW2 = 0, ACC_DB2 = 64, ACC_DW1 = 80, ACC_DW3 = 144;
 
+// Offset (floats into the CTA's accumulator block) of element (row, col) of the weight-gradient product with n columns
+// that starts at accumulator column `pcol`.  Its n x 128 floats are fragment-major, not (row, column): the two m64
+// halves' wgmma fragments one after the other, and in a fragment the 16-byte chunk j of issuing thread t (fragment
+// elements 4 j .. 4 j + 3) is chunk 128 j + t.  A thread then loads and stores its fragment with n / 8 vector accesses,
+// each of them 512 contiguous bytes per warp, and within the tile loop only the thread that wrote a float reads it.
+__device__ __forceinline__ uint32_t grad_acc_off(uint32_t pcol, int n, int row, int col) {
+  const int rr = row & 63;
+  // wgmma D layout: thread t = 32 w + l holds rows 16 w + l / 4 (+ 8) and columns 8 j + 2 (l % 4) (+ 1)
+  const int t = 32 * (rr >> 4) + 4 * (rr & 7) + ((col >> 1) & 3);
+  const int e = 2 * ((rr >> 3) & 1) + (col & 1);
+  return pcol * ACC_LANES + (uint32_t)((row >> 6) * 64 * n + 4 * (128 * (col >> 3) + t) + e);
+}
+
 #ifdef B200RL_TC3_TIMING
 // CTA 0, chain warpgroup wg = 2 c + h: [10 wg + s - 1] cycles stage s (E1..E5) waited on an mbarrier, [10 wg + 4 + s]
 // cycles of stage s in all; gradient warpgroup: [40 + 3 c + s - 3] cycles waited for the operands of stage s (3..5) of
-// network c, [46 + 3 c + s - 3] cycles issuing its products; [52] tiles of the CTA, [53] set-up, [54] tile loop,
-// [55] read-out
+// network c, [46 + 3 c + s - 3] cycles issuing its products, split over all stages into [56] waiting for its fragment
+// loads (and asking for the next fragment), [57] wgmma_fence .. wgmma_wait_all, [58] fragment stores and the hand-over
+// (bar.sync 5, mbar_arrive); [52] tiles of the CTA, [53] set-up, [54] tile loop, [55] read-out
 __device__ unsigned long long g_tc3_t[64];
+#define TC3_TACC tacc
+#else
+#define TC3_TACC nullptr
 #endif
 
 enum { C3_G = 0, C3_U1, C3_U2, C3_U3, C3_UH2, C3_UH1, C3_W1, C3_W2, C3_W3, C3_OW3, C3_OW2, C3_OW1, C3_OB, C3_N };
@@ -182,20 +201,53 @@ __device__ __forceinline__ void chain_mma(float (&d)[N / 2], const Op2 a, const 
   for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
   wg_mma<N, K_MAJOR, TB, 3, KSTEPS>(d, alo, blo, a.hi, b.hi, a.k_step, b.k_step, 0u);
 }
+// This thread's fragment of the first m64 half of the weight-gradient product at column pcol, whatever its N:
+// grad_acc_off's layout puts chunk j of the fragment 512 j floats further and the second half 64 N floats further.
+__device__ __forceinline__ float* grad_frag(float* acc_cta, uint32_t pcol) {
+  const int t = (int)(threadIdx.x & 127u);
+  return acc_cta + grad_acc_off(pcol, 0, 16 * (t >> 5) + ((t & 31) >> 2), 2 * (t & 3));
+}
+// Asks for the `chunks` 16-byte fragment chunks (at most 8) from `src` to be brought into L1, without waiting.
+__device__ __forceinline__ void grad_prefetch(const float* src, int chunks) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+    if (j < chunks) asm volatile("prefetch.global.L1 [%0];" ::"l"(src + 512 * j));
+}
 // weight-gradient product over the whole tile (both operands MN-major): A stacks its two splits along M (rows 0..63 h,
-// 64..127 l: the two m64 halves), B split l (B_SPLITS == 2) then h.  Each half's fragment is loaded from the
-// accumulator memory and stored back; on the launch's first tile (`first`) the product overwrites it.
+// 64..127 l: the two m64 halves), B split l (B_SPLITS == 2) then h.  Each half loads its fragment from the accumulator
+// memory, asks for the fragment of the half after it (this product's second half, then `next_chunks` chunks of the
+// product at column `next_col`) to be brought into L1, runs its wgmma group and stores the fragment back.  The L2
+// round trip of a fragment thus runs under the products of the half before it, and the half's own loads hit L1.  A
+// second fragment held in registers would not fit next to the one the wgmma group holds (96 registers a thread).  On
+// the launch's first tile (`first`) the products overwrite and nothing is loaded.
 template <int N, int KSTEPS, int B_SPLITS>
-__device__ __forceinline__ void grad_mma(float* acc_cta, uint32_t acc_col, bool first, const Op2 a, const Op2 b) {
-  const int t = (int)(threadIdx.x & 127u), w = t >> 5, l = t & 31;
+__device__ __forceinline__ void grad_mma(float* acc_cta, uint32_t acc_col, bool first, const Op2 a, const Op2 b,
+                                         uint32_t next_col, int next_chunks, unsigned long long* tacc) {
   const uint32_t a_half = (a.lo >> 16) & 0x3FFFu;  // the leading byte offset: A's l split
-  float* const frag0 = acc_cta + (acc_col + 2 * (l & 3)) * ACC_LANES + 16 * w + (l >> 2);
+  float* const frag0 = grad_frag(acc_cta, acc_col);
 #pragma unroll 1
   for (int h = 0; h < 2; ++h) {
-    float* frag = frag0 + 64 * h;
+#ifdef B200RL_TC3_TIMING
+    const long long t0 = clock64();
+#endif
+    float* const frag = frag0 + 64 * N * h;
     float d[N / 2];
 #pragma unroll
-    for (int i = 0; i < N / 2; ++i) d[i] = first ? 0.f : frag[(8 * (i >> 2) + (i & 1)) * ACC_LANES + 8 * ((i >> 1) & 1)];
+    for (int j = 0; j < N / 8; ++j) {
+      const float4 v = first ? make_float4(0.f, 0.f, 0.f, 0.f) : *reinterpret_cast<const float4*>(frag + 512 * j);
+      d[4 * j] = v.x;
+      d[4 * j + 1] = v.y;
+      d[4 * j + 2] = v.z;
+      d[4 * j + 3] = v.w;
+    }
+    if (h == 0)
+      grad_prefetch(frag + 64 * N, first ? 0 : N / 8);
+    else
+      grad_prefetch(grad_frag(acc_cta, next_col), next_chunks);
+#ifdef B200RL_TC3_TIMING
+    wgmma_fence();  // waits on the fragment's loads, though not reliably on all of them: some latency counts in [57]
+    const long long t1 = clock64();
+#endif
     uint32_t alo[B_SPLITS], blo[B_SPLITS];
 #pragma unroll
     for (int s = 0; s < B_SPLITS; ++s) {
@@ -203,8 +255,17 @@ __device__ __forceinline__ void grad_mma(float* acc_cta, uint32_t acc_col, bool 
       blo[s] = b.lo + (s + 1 < B_SPLITS ? b.split_step : 0u);
     }
     wg_mma<N, MN_MAJOR, MN_MAJOR, B_SPLITS, KSTEPS>(d, alo, blo, a.hi, b.hi, a.k_step, b.k_step, first ? 0u : 1u);
+#ifdef B200RL_TC3_TIMING
+    const long long t2 = clock64();
+#endif
 #pragma unroll
-    for (int i = 0; i < N / 2; ++i) frag[(8 * (i >> 2) + (i & 1)) * ACC_LANES + 8 * ((i >> 1) & 1)] = d[i];
+    for (int j = 0; j < N / 8; ++j)
+      *reinterpret_cast<float4*>(frag + 512 * j) = make_float4(d[4 * j], d[4 * j + 1], d[4 * j + 2], d[4 * j + 3]);
+#ifdef B200RL_TC3_TIMING
+    tacc[56] += (unsigned long long)(t1 - t0);
+    tacc[57] += (unsigned long long)(t2 - t1);
+    tacc[58] += (unsigned long long)(clock64() - t2);
+#endif
   }
 }
 
@@ -418,6 +479,9 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
       }
       __syncwarp();
     };
+    // first product of each stage: its accumulator columns within a network, and its N
+    auto lead_col = [](int stage) { return stage == 3 ? ACC_DW3 : (stage == 4 ? ACC_DW2 : ACC_DW1); };
+    auto lead_n = [](int stage) { return stage == 3 ? 32 : 64; };
     if (cta_tiles > 0) load_x(0);
 #pragma unroll 1
     for (int k = 0; k < cta_tiles; ++k) {
@@ -428,6 +492,14 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
 #pragma unroll 1
         for (int c = c_first; c <= c_last; ++c) {
           const uint32_t co = c * S3_CHAIN, gcol = c * ACC_GRAD_NET;
+          // the last half-product of this (stage, network) prefetches the first half-product after it: the next
+          // network's, the next stage's, or the next tile's first stage; none after the last tile, and none on the
+          // first (where every product overwrites)
+          const bool wrap = c == c_last && stage == 5;
+          const int ns = c < c_last ? stage : (stage < 5 ? stage + 1 : 3), nc = c < c_last ? c + 1 : c_first;
+          const bool nload = wrap ? k + 1 < cta_tiles : !first;
+          const uint32_t next = nc * ACC_GRAD_NET + lead_col(ns);
+          const int next_chunks = nload ? lead_n(ns) / 8 : 0;
 #ifdef B200RL_TC3_TIMING
           const long long it0 = clock64();
 #endif
@@ -438,24 +510,33 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
 #endif
           if (stage == 3) {
             // dW3^T[i][o] += sum_r H2[r][i] dOut[r][o]
-            grad_mma<32, 8, 1>(acc, gcol + ACC_DW3, first, op2_at(H2_M, co), op2_at(DO_M, dob + c * 64));
+            grad_mma<32, 8, 1>(acc, gcol + ACC_DW3, first, op2_at(H2_M, co), op2_at(DO_M, dob + c * 64), next,
+                               next_chunks, TC3_TACC);
           } else if (stage == 4) {
             // every chain warpgroup's dH2 and both dW3 have read dOut: its buffer takes the next tile's observations
             if (c == c_last && k + 1 < cta_tiles) load_x(k + 1);
             // dW2[o][i] += sum_r dZ2[r][o] H1[r][i] ; db2[o] += sum_r dZ2[r][o] * 1 (ones column of X)
-            grad_mma<64, 8, 2>(acc, gcol + ACC_DW2, first, op2_at(H2_M, co), op2_at(H1_M, co));
-            grad_mma<16, 8, 1>(acc, gcol + ACC_DB2, first, op2_at(H2_M, co), op2_at(X_M16, xo));
+            grad_mma<64, 8, 2>(acc, gcol + ACC_DW2, first, op2_at(H2_M, co), op2_at(H1_M, co),
+                               gcol + ACC_DB2, first ? 0 : 2, TC3_TACC);
+            grad_mma<16, 8, 1>(acc, gcol + ACC_DB2, first, op2_at(H2_M, co), op2_at(X_M16, xo), next, next_chunks,
+                               TC3_TACC);
           } else {
             // dW1[o][i] += sum_r dZ1[r][o] X[r][i]; column 31 (ones) collects db1
-            grad_mma<64, 8, 1>(acc, gcol + ACC_DW1, first, op2_at(H1_M, co), op2_at(X_M, xo));
+            grad_mma<64, 8, 1>(acc, gcol + ACC_DW1, first, op2_at(H1_M, co), op2_at(X_M, xo), next, next_chunks,
+                               TC3_TACC);
           }
+#ifdef B200RL_TC3_TIMING
+          const long long ih = clock64();
+#endif
           asm volatile("bar.sync 5, 128;" ::: "memory");  // every warp's share of the products has retired
           if ((tid & 127) == 0) {
             mbar_arrive(bar_done(c, stage));
             if (stage == 5 && c == c_last) mbar_arrive(bar_dofree);
           }
 #ifdef B200RL_TC3_TIMING
-          tacc[46 + 3 * c + stage - 3] += (unsigned long long)(clock64() - it1);
+          const long long it2 = clock64();
+          tacc[46 + 3 * c + stage - 3] += (unsigned long long)(it2 - it1);
+          tacc[58] += (unsigned long long)(it2 - ih);
 #endif
         }
       }
@@ -463,6 +544,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
 #ifdef B200RL_TC3_TIMING
     if (tid == T3_CHAIN_THREADS && blockIdx.x == 0) {
       for (int i = 40; i < 52; ++i) g_tc3_t[i] = tacc[i];
+      for (int i = 56; i < 59; ++i) g_tc3_t[i] = tacc[i];
       g_tc3_t[52] = (unsigned long long)cta_tiles;
     }
 #endif
@@ -750,12 +832,19 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
         const uint32_t gcol = cn * ACC_GRAD_NET;
 #pragma unroll 1
         for (int jb = part; jb < 8; jb += 4) {
-          // columns of this job, and of its second half where the operand's l columns went to their own block
-          const uint32_t col = jb < 4 ? ACC_DW2 + 16 * jb : (jb < 6 ? ACC_DW1 + 16 * (jb - 4) : (jb == 6 ? ACC_DW3 : ACC_DB2));
-          const uint32_t col2 = jb < 4 ? col : (jb < 6 ? col + 32 : (jb == 6 ? col + 16 : col));
+          // the job's product (first column, N), the job's columns in it, and those of its second half where the
+          // operand's l columns went to their own block
+          const uint32_t pcol = gcol + (jb < 4 ? ACC_DW2 : (jb < 6 ? ACC_DW1 : (jb == 6 ? ACC_DW3 : ACC_DB2)));
+          const int pn = jb < 6 ? 64 : (jb == 6 ? 32 : 16);
+          const int col = jb < 4 ? 16 * jb : (jb < 6 ? 16 * (jb - 4) : 0);
+          const int col2 = jb < 4 ? col : (jb < 6 ? col + 32 : (jb == 6 ? 16 : col));
           if (have) {
-            acc_ld<16>(acc, r, gcol + col, v);
-            acc_ld<16>(acc, r, gcol + col2, w);
+            // col and col2 are multiples of 8: column col + j of row r sits grad_acc_off(0, pn, 0, j) after column col
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+              v[j] = acc[grad_acc_off(pcol, pn, r, col) + grad_acc_off(0, pn, 0, j)];
+              w[j] = acc[grad_acc_off(pcol, pn, r, col2) + grad_acc_off(0, pn, 0, j)];
+            }
           } else {
 #pragma unroll
             for (int j = 0; j < 16; ++j) v[j] = w[j] = 0.f;  // a CTA without tiles: accumulator memory was never written

@@ -58,3 +58,5 @@ if __name__ == "__main__":
         keys = [f"{st}{'pv'[c]}" for c in range(2) for st in ("dW3", "dW2", "dW1")]
         print("gradient wait  / tile:", {k: int(out[40 + i]) // tiles for i, k in enumerate(keys)}, "sum", sum(int(out[40 + i]) for i in range(6)) // tiles)
         print("gradient issue / tile:", {k: int(out[46 + i]) // tiles for i, k in enumerate(keys)}, "sum", sum(int(out[46 + i]) for i in range(6)) // tiles)
+        split = ("fragment loads", "fence .. wait_all", "stores + hand-over")
+        print("gradient issue split / tile:", {k: int(out[56 + i]) // tiles for i, k in enumerate(split)})

@@ -14,6 +14,7 @@ float32 rounding (oracle/onpolicy.py does), so a kernel error that a float32 ora
 * ``forward_kl``: raw outputs and the true KL(old || new) per row (trpo.py:167-175).
 * ``fvp``: the Fisher-vector product the way the reference forms it: double backprop of the mean KL(old || new) with the
   old distribution detached (conjugate_gradient_optimizer.py:133-167), at damping 0.
+* ``gae_scan``: returns and GAE advantages before their float32 cast, with their conditioning scales (numpy / scipy).
 
 Every gradient also comes with its scale: per entry, the sum over rows of the magnitudes of the rows' contributions.
 Where those contributions cancel, a float32 sum over rows is only accurate to ~2^-24 of that scale, not of the result,
@@ -237,3 +238,49 @@ def clip_margin(ratio, clip: float = 0.2) -> np.ndarray:
     rounding of a bound may be clipped differently by a float32 kernel, which is not an error of the kernel."""
     r = np.asarray(ratio, dtype=np.float64)
     return np.minimum(np.abs(r - (1.0 - clip)) / (1.0 - clip), np.abs(r - (1.0 + clip)) / (1.0 + clip))
+
+
+def _segmented_reverse_scan(x: np.ndarray, off: np.ndarray, lens: np.ndarray, a: float) -> np.ndarray:
+    """y_i = x_i + a * y_{i+1} inside every episode, y = 0 past its end, in float64 (lfilter, ref: utils.py:28).
+    Episodes of one length run as one [episodes, length] block, so a batch of millions of items takes seconds."""
+    from scipy.signal import lfilter
+    y = np.empty_like(x)
+    order = np.argsort(lens, kind="stable")
+    for grp in np.split(order, np.flatnonzero(np.diff(lens[order])) + 1):
+        L = int(lens[grp[0]])
+        idx = off[grp][:, None] + np.arange(L)[None, :]
+        y[idx] = lfilter([1.0], [1.0, -a], x[idx][:, ::-1], axis=1)[:, ::-1]
+    return y
+
+
+def gae_scan(rewards, values, last_values, ep_offsets, ep_done, gamma: float, lam: float):
+    """Returns and GAE advantages of a packed batch, UNROUNDED float64 (oracle/onpolicy.py's gae_and_returns before its
+    final cast), with a conditioning scale per output.  The two float32 details of the reference are kept:
+      delta_i = (r_i + f32(f32(gamma) * v_{i+1})) - v_i,  with v_L = V(last_obs) on the last step even when done;
+      the return of the last step adds gamma * V(last_obs), in float64, only when the episode is not done.
+    The scales S_adv / S_ret run the same recurrences over the magnitudes of every term (|r| + |f32 product| + |v| and
+    |r| + |gamma * V_L|, coefficients |gamma * lam| and |gamma|): float64 reassociation of a scan is accurate to a few
+    ulp of S, not of the result.  Returns (adv64, ret64, S_adv, S_ret), each [N] float64."""
+    off = np.asarray(ep_offsets, dtype=np.int64)
+    lens = np.diff(off)
+    n = int(off[-1])
+    r = np.asarray(rewards, dtype=np.float64)
+    v = np.asarray(values, dtype=np.float32)
+    lv = np.asarray(last_values, dtype=np.float32)
+    last = off[1:] - 1
+    vnext = np.empty(n, dtype=np.float32)
+    vnext[:-1] = v[1:]
+    vnext[last] = lv
+    prod = (np.float32(gamma) * vnext).astype(np.float64)  # float32 product, exactly rounded
+    delta = (r + prod) - v.astype(np.float64)
+    boot = np.where(np.asarray(ep_done, dtype=bool), 0.0, gamma * lv.astype(np.float64))
+    rb = r.copy()
+    rb[last] += boot
+    rb_abs = np.abs(r)
+    rb_abs[last] += np.abs(boot)
+    gl = gamma * lam
+    adv = _segmented_reverse_scan(delta, off, lens, gl)
+    ret = _segmented_reverse_scan(rb, off, lens, gamma)
+    s_adv = _segmented_reverse_scan(np.abs(r) + np.abs(prod) + np.abs(v.astype(np.float64)), off, lens, abs(gl))
+    s_ret = _segmented_reverse_scan(rb_abs, off, lens, abs(gamma))
+    return adv, ret, s_adv, s_ret

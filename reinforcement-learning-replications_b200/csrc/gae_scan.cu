@@ -41,7 +41,8 @@ constexpr int SCAN_RECS = 8;
 constexpr int SCAN_MAXE = 48;  // episodes per tile staged in shared memory (more: global-memory path)
 
 // Workspace header.  The workspace is zeroed ONCE (at allocation); after that every launch cleans up after itself:
-// look-back records carry the launch epoch as their tag (a stale record from an earlier launch reads as "not ready"), and the last
+// look-back records carry the negated launch epoch as their tag (a stale record from an earlier launch, or statistics an
+// earlier launch of another n left in the same bytes, read as "not ready"), and the last
 // CTA to finish resets the done counter and bumps the epoch.  => one kernel launch per scan, no memset.
 struct ScanHeader {
   int reserved0;
@@ -227,7 +228,10 @@ __global__ void __launch_bounds__(SCAN_THREADS, 3) gae_scan_kernel(const ScanArg
   }
 
   // ================================== scan warps ====================================
-  const double tag = (double)(s_epoch + 1);  // records of THIS launch carry this tag (0 = never written)
+  // Records of THIS launch carry this tag (0 = never written).  It is negative because record slots share workspace
+  // bytes with the per-tile / per-episode statistics of earlier launches of a different n, and those land sums of
+  // squares (>= 0) in the tag slot: a positive tag could equal one and a stale slot would read as published.
+  const double tag = -(double)(s_epoch + 1);
   for (int k = 0; k < n_mine; ++k) {
     const int tile = T - 1 - c - k * G, b = k & 1;
     if (!sbar_wait(sm_addr(&bars[b]), (k >> 1) & 1)) {

@@ -165,3 +165,23 @@ def test_gradient_scales_bound_the_gradients(loss):
                                        for i, (w, b) in enumerate(layers)]), sizes[:-1] + [1], obs[:1], np.ones(1))
     for k, g in v["grads"].items():
         np.testing.assert_allclose(v["scales"][k], np.abs(g), rtol=1e-12, atol=1e-300)
+
+
+@pytest.mark.parametrize("f64", [True, False])
+def test_gae_scan_reference_rounds_to_the_float32_oracle(f64):
+    """The unrounded float64 scan reference, cast to float32, is the float32 oracle bit for bit, on ragged episodes
+    (lengths 1 and 2 among them) with nonzero values, done and not-done episodes, and float64 or float32 rewards."""
+    rng = np.random.default_rng(11)
+    lens = np.concatenate([[1, 2, 1], rng.integers(1, 90, 300), [2]])
+    off = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+    n, e = int(off[-1]), lens.size
+    rew = rng.standard_normal(n) if f64 else rng.standard_normal(n).astype(np.float32)
+    values = rng.standard_normal(n).astype(np.float32)
+    last_values = rng.standard_normal(e).astype(np.float32)
+    done = rng.random(e) < 0.5
+    for gamma, lam in ((0.99, 0.97), (1.0, 1.0), (0.0, 0.5), (0.9, 0.0)):
+        adv64, ret64, s_adv, s_ret = R.gae_scan(rew, values, last_values, off, done, gamma, lam)
+        adv, ret = O.gae_and_returns(rew, values, last_values, off, done, gamma, lam)
+        np.testing.assert_array_equal(adv64.astype(np.float32), adv)
+        np.testing.assert_array_equal(ret64.astype(np.float32), ret)
+        assert np.all(s_adv >= np.abs(adv64)) and np.all(s_ret >= np.abs(ret64))

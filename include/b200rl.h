@@ -274,7 +274,8 @@ int b200rl_onpolicy_fvp(b200rl_onpolicy* h, const float* host_v, float* host_out
 
 /* Device views for tests / profiling (pointers stay owned by the engine):
  * name: "values","last_values","adv_raw","ret","old_logp","adv_stats","policy_grad","value_grad",
- *       "policy_params","old_policy_params","value_params" */
+ *       "policy_params","old_policy_params","value_params", and after a TRPO update its conjugate-gradient state
+ *       "cg_x","cg_r","cg_p","cg_descent" and "cg_z" (F x of the step-size product, without damping) */
 int b200rl_onpolicy_device_view(b200rl_onpolicy* h, const char* name, void** ptr, int64_t* count, int32_t* dtype);
 
 /* One-shot gradient exchange over peer-mapped device memory (data-parallel runs on ONE node: NVLink / NVSwitch).

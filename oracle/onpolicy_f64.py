@@ -15,6 +15,8 @@ float32 rounding (oracle/onpolicy.py does), so a kernel error that a float32 ora
 * ``fvp``: the Fisher-vector product the way the reference forms it: double backprop of the mean KL(old || new) with the
   old distribution detached (conjugate_gradient_optimizer.py:133-167), at damping 0.
 * ``gae_scan``: returns and GAE advantages before their float32 cast, with their conditioning scales (numpy / scipy).
+* the TRPO step one stage at a time, so that a test can replay each stage from a kernel's own state: ``cg_iteration``,
+  ``step_size``, ``line_search_eval`` and ``trpo_decisions`` (conjugate_gradient_optimizer.py).
 
 Every gradient also comes with its scale: per entry, the sum over rows of the magnitudes of the rows' contributions.
 Where those contributions cancel, a float32 sum over rows is only accurate to ~2^-24 of that scale, not of the result,
@@ -284,3 +286,69 @@ def gae_scan(rewards, values, last_values, ep_offsets, ep_done, gamma: float, la
     s_adv = _segmented_reverse_scan(np.abs(r) + np.abs(prod) + np.abs(v.astype(np.float64)), off, lens, abs(gl))
     s_ret = _segmented_reverse_scan(rb_abs, off, lens, abs(gamma))
     return adv, ret, s_adv, s_ret
+
+
+# ---- the TRPO step, stage by stage (conjugate_gradient_optimizer.py) -----------------------------------------------
+def cg_iteration(F, x, r, p, rdotr: float, damping: float):
+    """One conjugate-gradient iteration (conjugate_gradient_optimizer.py:190-201) in float64 from the state (x, r, p,
+    rdotr), with z = F(p) + damping p (:165) and F a float64 callable.  Returns dict(x, r, p, v, mu, rdotr (the new
+    r . r), z) and, per output vector, the scale of its float32 rounding: elementwise the larger magnitude of the two
+    terms that form it, sx = max(|x|, |v p|), sr = max(|r|, |v z|), and for p' = r' + mu p, which inherits the rounding
+    of r' (large against r' itself where r - v z cancels), sp = max(sr, |mu p|)."""
+    x, r, p = (np.asarray(a, dtype=np.float64) for a in (x, r, p))
+    z = np.asarray(F(p), dtype=np.float64) + damping * p
+    v = rdotr / float(p @ z)
+    x1 = x + v * p
+    r1 = r - v * z
+    new = float(r1 @ r1)
+    mu = new / rdotr
+    p1 = r1 + mu * p
+    return dict(x=x1, r=r1, p=p1, v=v, mu=mu, rdotr=new, z=z, sx=np.maximum(np.abs(x), np.abs(v * p)),
+                sr=np.maximum(np.abs(r), np.abs(v * z)),
+                sp=np.maximum(np.maximum(np.abs(r), np.abs(v * z)), np.abs(mu * p)))
+
+
+def step_size(x, Fx, damping: float, delta: float, f32_xhx=None):
+    """x^T (F + damping I) x and the step size sqrt(2 delta / (xHx + 1e-8)), NaN -> 1 (conjugate_gradient_optimizer.py:
+    83-95), in float64: returns (xhx, step).  f32_xhx: replay the float32 rule of the kernel from this xHx instead
+    (trpo.cu step_size_kernel: every operation rounded to float32), and the step is a np.float32."""
+    x = np.asarray(x, dtype=np.float64)
+    xhx = float(x @ (np.asarray(Fx, dtype=np.float64) + damping * x))
+    if f32_xhx is not None:
+        f = np.float32
+        with np.errstate(invalid="ignore", divide="ignore"):
+            step = np.sqrt(f(2.0) * f(delta) * (f(1.0) / (f(f32_xhx) + f(1e-8))))
+        return xhx, (f(1.0) if np.isnan(step) else f(step))
+    step = math.sqrt(2.0 * delta / (xhx + 1e-8)) if xhx + 1e-8 > 0 else math.nan
+    return xhx, (1.0 if math.isnan(step) else step)
+
+
+def line_search_eval(flat, sizes, obs, act, dist: str, old_flat, adv_raw, adv_stats, old_logp, log_std=None,
+                     hidden: str = "tanh"):
+    """One line-search evaluation (trpo.py:154-175) at the parameters ``flat``: the surrogate's loss sum
+    -sum(exp(logp - old_logp) adv) with its sum of |term| (the scale of a float32 sum's rounding), and the sum over rows
+    of the true KL(old || new), old = the network at ``old_flat``: dict(loss_sum, loss_abs_sum, kl_sum)."""
+    with torch.no_grad():
+        out = mlp(_t(flat), sizes, _t(obs), hidden, "identity")[0]
+        ls = _t(log_std) if dist == "gaussian" else None
+        logp = _log_prob(dist, _dist(dist, out, ls), act)
+        terms = -(torch.exp(logp - _t(old_logp)) * normalized_advantages(adv_raw, adv_stats))
+        old_out = mlp(_t(old_flat), sizes, _t(obs), hidden, "identity")[0]
+        kl = kl_divergence(_dist(dist, old_out, ls), _dist(dist, out, ls))
+        if dist == "gaussian":
+            kl = kl.sum(-1)
+    return dict(loss_sum=float(terms.sum()), loss_abs_sum=float(terms.abs().sum()), kl_sum=float(kl.sum()))
+
+
+def trpo_decisions(loss_before: float, new_losses: Sequence[float], kls: Sequence[float], delta: float):
+    """The backtracking line search's rule (conjugate_gradient_optimizer.py:115-124, 233-250) over the evaluations
+    k = 0, 1, ...: accept the first k with new_loss < loss_before and kl <= delta; after the loop, reject (restore the
+    parameters) iff the last evaluation is NaN, or new_loss >= loss_before, or kl >= delta.  Returns dict(accepted
+    (index or -1), rejected, evaluated (how many evaluations the search makes), loss_margin and kl_margin: per k the
+    signed margins loss_before - new_loss and delta - kl, both positive where that k passes)."""
+    loss_m = [loss_before - float(l) for l in new_losses]
+    kl_m = [delta - float(k) for k in kls]
+    accepted = next((k for k, (a, b) in enumerate(zip(loss_m, kl_m)) if a > 0 and b >= 0), -1)
+    last = accepted if accepted >= 0 else len(loss_m) - 1
+    rejected = bool(math.isnan(loss_m[last]) or math.isnan(kl_m[last]) or loss_m[last] <= 0 or kl_m[last] <= 0)
+    return dict(accepted=accepted, rejected=rejected, evaluated=last + 1, loss_margin=loss_m, kl_margin=kl_m)

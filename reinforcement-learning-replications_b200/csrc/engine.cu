@@ -1004,6 +1004,9 @@ extern "C" int b200rl_onpolicy_device_view(b200rl_onpolicy* h, const char* name,
       {"policy_params", h->pol, h->Pp, 0},        {"old_policy_params", h->old_pol, h->Pp, 0},
       {"value_params", h->val, h->Pv, 0},         {"obs", h->obs, h->n_rows * h->obs_dim, 0},
       {"cg_x", h->cg_x, h->cg_x ? h->Pp : 0, 0},  {"cg_descent", h->cg_descent, h->cg_descent ? h->Pp : 0, 0},
+      // the conjugate-gradient state after the last update: residual, direction, and F x of the step-size product
+      {"cg_r", h->cg_r, h->cg_r ? h->Pp : 0, 0},  {"cg_p", h->cg_p, h->cg_p ? h->Pp : 0, 0},
+      {"cg_z", h->cg_z, h->cg_z ? h->Pp : 0, 0},
   };
   for (const V& v : views)
     if (strcmp(v.n, name) == 0) {

@@ -76,8 +76,8 @@ def test_trpo_train_matches_reference(case):
 
 
 def test_trpo_vs_oracle_and_rejection():
-    """Against the numpy oracle on a seeded batch, plus the reject/restore branch (delta so small that no backtrack
-    ratio satisfies the constraint ... the step must be rejected and the parameters restored bit-exactly)."""
+    """Against the numpy oracle on a seeded batch, plus the reject/restore branch (a KL limit no step can satisfy: the
+    step must be rejected and the parameters restored bit-exactly)."""
     g = load_golden("trpo_gaussian_small")
     policy = O.unflatten_layers(g["policy_flat0"], [27, 64, 64, 8])
     out = O.trpo_policy_step(policy, "gaussian", g["log_std"], g["obs"], g["act"], g["adv"])
@@ -87,17 +87,16 @@ def test_trpo_vs_oracle_and_rejection():
     assert ts.accepted_index == out["accepted"]
     assert abs(ts.step_size - out["step_size"]) < 2e-3 * out["step_size"]
     assert rel_err(flat(trpo.policy.network), out["policy_flat"]) < 2e-3
-    # rejection: huge damping makes x tiny -> fine; instead use an impossible constraint via max_backtracks = 1 and
-    # a delta below the KL of the full step
+    # rejection by construction: a negative KL limit, which no KL (a non-negative sum) can meet; the step size
+    # sqrt(2 delta / xHx) is NaN and falls back to 1, the one evaluation fails and the parameters are restored
     t2 = build_trpo(g, num_value_gradients=0)
     t2.policy.optimizer.max_backtracks = 1
-    t2.policy.optimizer.max_constraint = 1e-9  # step size scales with sqrt(delta) but kl <= 1e-9 fails in float32
-    t2.policy.optimizer.backtrack_ratio = 0.8
+    t2.policy.optimizer.max_constraint = -1.0
     t2.train_packed(batch_of(g))
-    if t2.last_trpo_stats.rejected:
-        np.testing.assert_array_equal(flat(t2.policy.network), g["policy_flat0"])
-    else:
-        assert t2.last_trpo_stats.kl <= 1e-9
+    ts2 = t2.last_trpo_stats
+    assert ts2.rejected == 1 and ts2.accepted_index == -1 and ts2.step_size == 1.0
+    np.testing.assert_array_equal(flat(t2.policy.network).view(np.uint32),
+                                  g["policy_flat0"].astype(np.float32).view(np.uint32))
 
 
 @pytest.mark.parametrize("sizes,dist", [([27, 64, 64, 8], "gaussian"), ([4, 64, 64, 2], "categorical"),

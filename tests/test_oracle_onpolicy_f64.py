@@ -185,3 +185,94 @@ def test_gae_scan_reference_rounds_to_the_float32_oracle(f64):
         np.testing.assert_array_equal(adv64.astype(np.float32), adv)
         np.testing.assert_array_equal(ret64.astype(np.float32), ret)
         assert np.all(s_adv >= np.abs(adv64)) and np.all(s_ret >= np.abs(ret64))
+
+
+def _cg_problem(dist, damping):
+    sizes = [3, 5, 4, 3]
+    layers, obs, act, log_std, adv_raw, stats, _ = _problem(sizes, dist, 9, 21)
+    flat = O.flatten_layers(layers)
+    logp = R.policy_loss(flat, sizes, obs, act, dist, "eval", log_std)["logp"].astype(np.float32)
+    g = R.policy_loss(flat, sizes, obs, act, dist, "trpo_surrogate", log_std, adv_raw, stats, logp)["grad"]
+    F = lambda v: R.fvp(flat, sizes, obs, dist, v, log_std)["fvp"]
+    return sizes, layers, flat, obs, act, log_std, adv_raw, stats, logp, g, F
+
+
+@pytest.mark.parametrize("dist", ["gaussian", "categorical"])
+def test_cg_iteration_solves_the_damped_system(dist):
+    """More iterations of cg_iteration than parameters reach numpy.linalg.solve(F + damping I, g), F formed column by
+    column from fvp_explicit; the scales bound the magnitudes of the iterates they belong to."""
+    damping = 1e-2
+    sizes, _, flat, obs, _, log_std, _, _, _, g, F = _cg_problem(dist, damping)
+    P = flat.size
+    Fm = np.stack([R.fvp_explicit(flat, sizes, obs, dist, e, log_std) for e in np.eye(P)], axis=1)
+    want = np.linalg.solve(Fm + damping * np.eye(P), g)
+    x, r, p, rdotr = np.zeros(P), g.copy(), g.copy(), float(g @ g)
+    for _ in range(P + 20):
+        it = R.cg_iteration(F, x, r, p, rdotr, damping)
+        for k, m in (("x", 2), ("r", 2), ("p", 3)):  # x', r': two terms; p' = r' + mu p, with |r'| <= 2 sr
+            assert (m * it["s" + k] >= np.abs(it[k]) * (1 - 1e-12)).all(), k
+        x, r, p, rdotr = it["x"], it["r"], it["p"], it["rdotr"]
+        if rdotr < 1e-28:
+            break
+    assert rel_err(x, want) < 1e-8
+
+
+@pytest.mark.parametrize("dist", ["gaussian", "categorical"])
+def test_cg_iterations_round_to_the_float32_oracle(dist):
+    """Ten float64 iterations from g, rounded to float32, against oracle.onpolicy.conjugate_gradient on the same
+    system (float32 vectors and float32 Fisher-vector products).  The damping keeps the system well conditioned, so
+    the two roundings do not send the iterates apart."""
+    damping = 1.0
+    sizes, layers, flat, obs, _, log_std, _, _, _, g, F = _cg_problem(dist, damping)
+    x, r, p, rdotr = np.zeros_like(g), g.copy(), g.copy(), float(g @ g)
+    for _ in range(10):
+        it = R.cg_iteration(F, x, r, p, rdotr, damping)
+        x, r, p, rdotr = it["x"], it["r"], it["p"], it["rdotr"]
+        if rdotr < 1e-10:
+            break
+    hvp = lambda v: O.fisher_vector_product(layers, dist, log_std, obs, v, damping)
+    want = O.conjugate_gradient(hvp, g.astype(np.float32), 10)
+    assert rel_err(x.astype(np.float32), want) < 1e-4
+
+
+def test_step_size_float32_replay_and_nan_rule():
+    """The float64 rule, its float32 replay (every operation rounded like the kernel's), and NaN -> 1."""
+    rng = np.random.default_rng(5)
+    x, Fx = rng.standard_normal(50), rng.standard_normal(50)
+    Fx = Fx + 3.0 * x  # x . F x > 0
+    xhx, step = R.step_size(x, Fx, 0.1, 0.01)
+    assert xhx == pytest.approx(float(x @ Fx) + 0.1 * float(x @ x), rel=1e-14)
+    assert step == pytest.approx(np.sqrt(0.02 / (xhx + 1e-8)), rel=1e-14)
+    f = np.float32
+    _, s32 = R.step_size(x, Fx, 0.1, 0.01, f32_xhx=f(xhx))
+    assert s32.dtype == np.float32 and s32 == np.sqrt(f(2.0) * f(0.01) * (f(1.0) / (f(xhx) + f(1e-8))))
+    assert abs(float(s32) - step) < 1e-6 * step
+    assert R.step_size(x, -Fx - x, 0.0, 0.01)[1] == 1.0  # a negative form: sqrt of a negative number -> 1
+    assert R.step_size(x, Fx, 0.0, 0.01, f32_xhx=f(-1.0))[1] == f(1.0)
+
+
+@pytest.mark.parametrize("dist", ["gaussian", "categorical"])
+def test_line_search_eval_and_decisions(dist):
+    """line_search_eval at theta_old is the surrogate loss at ratio 1 with zero KL; at a moved policy it matches
+    policy_loss and forward_kl; trpo_decisions takes the first k passing both tests, and rejects on the last one."""
+    sizes, _, flat, obs, act, log_std, adv_raw, stats, logp, g, _ = _cg_problem(dist, 0.0)
+    same = R.line_search_eval(flat, sizes, obs, act, dist, flat, adv_raw, stats, logp, log_std)
+    ref = R.policy_loss(flat, sizes, obs, act, dist, "trpo_surrogate", log_std, adv_raw, stats, logp)
+    assert same["loss_sum"] == pytest.approx(ref["loss_sum"], rel=1e-12, abs=1e-12)
+    assert same["loss_abs_sum"] == pytest.approx(ref["loss_abs_sum"], rel=1e-12)
+    assert abs(same["kl_sum"]) < 1e-12
+    moved = (flat - 0.05 * g / np.abs(g).max()).astype(np.float32)
+    ev = R.line_search_eval(moved, sizes, obs, act, dist, flat, adv_raw, stats, logp, log_std)
+    ref = R.policy_loss(moved, sizes, obs, act, dist, "trpo_surrogate", log_std, adv_raw, stats, logp)
+    old_out = R.forward_kl(flat, sizes, obs, dist, np.zeros((obs.shape[0], sizes[-1])), log_std)["out"]
+    assert ev["loss_sum"] == pytest.approx(ref["loss_sum"], rel=1e-12)
+    assert ev["kl_sum"] == pytest.approx(R.forward_kl(moved, sizes, obs, dist, old_out, log_std)["kl"].sum(), rel=1e-12)
+    assert ev["loss_sum"] < same["loss_sum"] and ev["kl_sum"] > 0
+    d = R.trpo_decisions(1.0, [1.2, 0.9, 0.5], [0.001, 0.02, 0.001], 0.01)
+    assert (d["accepted"], d["rejected"], d["evaluated"]) == (2, False, 3)
+    np.testing.assert_allclose(d["loss_margin"], [-0.2, 0.1, 0.5])
+    np.testing.assert_allclose(d["kl_margin"], [0.009, -0.01, 0.009])
+    d = R.trpo_decisions(1.0, [1.2, 0.9], [0.001, 0.02], 0.01)
+    assert (d["accepted"], d["rejected"], d["evaluated"]) == (-1, True, 2)
+    d = R.trpo_decisions(1.0, [0.9], [0.01], 0.01)  # kl == delta: accepted by the search, rejected after it
+    assert (d["accepted"], d["rejected"]) == (0, True)

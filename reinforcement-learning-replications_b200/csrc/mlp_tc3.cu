@@ -213,54 +213,95 @@ __device__ __forceinline__ void grad_prefetch(const float* src, int chunks) {
   for (int j = 0; j < 8; ++j)
     if (j < chunks) asm volatile("prefetch.global.L1 [%0];" ::"l"(src + 512 * j));
 }
-// weight-gradient product over the whole tile (both operands MN-major): A stacks its two splits along M (rows 0..63 h,
-// 64..127 l: the two m64 halves), B split l (B_SPLITS == 2) then h.  Each half loads its fragment from the accumulator
-// memory, asks for the fragment of the half after it (this product's second half, then `next_chunks` chunks of the
-// product at column `next_col`) to be brought into L1, runs its wgmma group and stores the fragment back.  The L2
-// round trip of a fragment thus runs under the products of the half before it, and the half's own loads hit L1.  A
-// second fragment held in registers would not fit next to the one the wgmma group holds (96 registers a thread).  On
-// the launch's first tile (`first`) the products overwrite and nothing is loaded.
-template <int N, int KSTEPS, int B_SPLITS>
+// The products of one weight-gradient wgmma group into fragment `d` (both operands MN-major): TERMS terms (B split l,
+// then h), KSTEPS k-steps each, A at descriptor low word `a_lo`; the first product overwrites on the first tile.
+template <int N, int KSTEPS, int TERMS>
+__device__ __forceinline__ void grad_products(float (&d)[N / 2], uint32_t a_lo, const Op2 a, const Op2 b, bool first) {
+  // an opaque copy per product: products that share A would otherwise share its k-step descriptors, held live (and
+  // spilled) next to the group's fragments
+  uint32_t b_lo = b.lo;
+  asm volatile("" : "+r"(a_lo), "+r"(b_lo));
+#pragma unroll
+  for (int s = 0; s < TERMS; ++s)
+#pragma unroll
+    for (int k = 0; k < KSTEPS; ++k)
+      wgmma_run<N, MN_MAJOR, MN_MAJOR>(d, ((uint64_t)a.hi << 32) | (a_lo + (uint32_t)k * a.k_step),
+                                       ((uint64_t)b.hi << 32) | (b_lo + (s + 1 < TERMS ? b.split_step : 0u) +
+                                                                 (uint32_t)k * b.k_step),
+                                       s == 0 && k == 0 ? (first ? 0u : 1u) : 1u);
+}
+// weight-gradient product over the whole tile: A stacks its two splits along M (rows 0..63 h, 64..127 l: the two m64
+// halves), B split l (B_SPLITS == 2) then h.  Each wgmma group loads its fragments from the accumulator memory, asks for
+// the fragment of the group after it (this product's second half, then `next_chunks` chunks of the product at column
+// `next_col`) to be brought into L1, runs its products and stores the fragments back.  A group's cost is mostly its
+// fragments' L2 round trip, whatever its width, so the groups hold as many products as 96 registers a thread allow:
+//   * BOTH: both m64 halves of an n32 product in one group -- 32 floats, chunks 0..7 as an n64 half's (grad_acc_off);
+//   * N2 > 0: with each half, the same half of a second, single-term product of width N2 with the same A (B = `b2`, at
+//     accumulator column `col2`).
+// Every accumulator still sees the same terms in the same order.  On the launch's first tile (`first`) the products
+// overwrite and nothing is loaded.
+template <int N, int KSTEPS, int B_SPLITS, int N2 = 0, bool BOTH = false>
 __device__ __forceinline__ void grad_mma(float* acc_cta, uint32_t acc_col, bool first, const Op2 a, const Op2 b,
-                                         uint32_t next_col, int next_chunks, unsigned long long* tacc) {
-  const uint32_t a_half = (a.lo >> 16) & 0x3FFFu;  // the leading byte offset: A's l split
+                                         uint32_t next_col, int next_chunks, unsigned long long* tacc,
+                                         uint32_t col2 = 0, const Op2 b2 = Op2{}) {
+  static_assert(!BOTH || (N == 32 && N2 == 0), "one group for both halves: an n32 product");
+  constexpr int CH = BOTH ? 8 : N / 8, CH2 = N2 / 8;  // fragment chunks of the group
+  const uint32_t a_half = (a.lo >> 16) & 0x3FFFu;     // the leading byte offset: A's l split
   float* const frag0 = grad_frag(acc_cta, acc_col);
+  float* const frag20 = grad_frag(acc_cta, col2);
 #pragma unroll 1
-  for (int h = 0; h < 2; ++h) {
+  for (int h = 0; h < (BOTH ? 1 : 2); ++h) {
 #ifdef B200RL_TC3_TIMING
     const long long t0 = clock64();
 #endif
     float* const frag = frag0 + 64 * N * h;
-    float d[N / 2];
+    float* const frag2 = frag20 + 64 * N2 * h;
+    float d[4 * CH], e[CH2 > 0 ? 4 * CH2 : 1];
 #pragma unroll
-    for (int j = 0; j < N / 8; ++j) {
+    for (int j = 0; j < CH; ++j) {
       const float4 v = first ? make_float4(0.f, 0.f, 0.f, 0.f) : *reinterpret_cast<const float4*>(frag + 512 * j);
       d[4 * j] = v.x;
       d[4 * j + 1] = v.y;
       d[4 * j + 2] = v.z;
       d[4 * j + 3] = v.w;
     }
-    if (h == 0)
-      grad_prefetch(frag + 64 * N, first ? 0 : N / 8);
-    else
+#pragma unroll
+    for (int j = 0; j < CH2; ++j) {
+      const float4 v = first ? make_float4(0.f, 0.f, 0.f, 0.f) : *reinterpret_cast<const float4*>(frag2 + 512 * j);
+      e[4 * j] = v.x;
+      e[4 * j + 1] = v.y;
+      e[4 * j + 2] = v.z;
+      e[4 * j + 3] = v.w;
+    }
+    if (h == 0 && !BOTH) {
+      grad_prefetch(frag + 64 * N, first ? 0 : CH);
+      grad_prefetch(frag2 + 64 * N2, first ? 0 : CH2);
+    } else {
       grad_prefetch(grad_frag(acc_cta, next_col), next_chunks);
+    }
 #ifdef B200RL_TC3_TIMING
     wgmma_fence();  // waits on the fragment's loads, though not reliably on all of them: some latency counts in [57]
     const long long t1 = clock64();
 #endif
-    uint32_t alo[B_SPLITS], blo[B_SPLITS];
-#pragma unroll
-    for (int s = 0; s < B_SPLITS; ++s) {
-      alo[s] = a.lo + (uint32_t)h * a_half;
-      blo[s] = b.lo + (s + 1 < B_SPLITS ? b.split_step : 0u);
+    wgmma_fence();
+    if constexpr (BOTH) {
+      grad_products<N, KSTEPS, B_SPLITS>(*reinterpret_cast<float(*)[N / 2]>(&d[0]), a.lo, a, b, first);
+      grad_products<N, KSTEPS, B_SPLITS>(*reinterpret_cast<float(*)[N / 2]>(&d[N / 2]), a.lo + a_half, a, b, first);
+    } else {
+      grad_products<N, KSTEPS, B_SPLITS>(d, a.lo + (uint32_t)h * a_half, a, b, first);
     }
-    wg_mma<N, MN_MAJOR, MN_MAJOR, B_SPLITS, KSTEPS>(d, alo, blo, a.hi, b.hi, a.k_step, b.k_step, first ? 0u : 1u);
+    if constexpr (N2 > 0) grad_products<N2, KSTEPS, 1>(e, a.lo + (uint32_t)h * a_half, a, b2, first);
+    wgmma_commit();
+    wgmma_wait_all();
 #ifdef B200RL_TC3_TIMING
     const long long t2 = clock64();
 #endif
 #pragma unroll
-    for (int j = 0; j < N / 8; ++j)
+    for (int j = 0; j < CH; ++j)
       *reinterpret_cast<float4*>(frag + 512 * j) = make_float4(d[4 * j], d[4 * j + 1], d[4 * j + 2], d[4 * j + 3]);
+#pragma unroll
+    for (int j = 0; j < CH2; ++j)
+      *reinterpret_cast<float4*>(frag2 + 512 * j) = make_float4(e[4 * j], e[4 * j + 1], e[4 * j + 2], e[4 * j + 3]);
 #ifdef B200RL_TC3_TIMING
     tacc[56] += (unsigned long long)(t1 - t0);
     tacc[57] += (unsigned long long)(t2 - t1);
@@ -479,9 +520,9 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
       }
       __syncwarp();
     };
-    // first product of each stage: its accumulator columns within a network, and its N
+    // first product of each stage: its accumulator columns within a network (its first group is 8 chunks: an n64 half,
+    // or both halves of dW3)
     auto lead_col = [](int stage) { return stage == 3 ? ACC_DW3 : (stage == 4 ? ACC_DW2 : ACC_DW1); };
-    auto lead_n = [](int stage) { return stage == 3 ? 32 : 64; };
     if (cta_tiles > 0) load_x(0);
 #pragma unroll 1
     for (int k = 0; k < cta_tiles; ++k) {
@@ -499,7 +540,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
           const int ns = c < c_last ? stage : (stage < 5 ? stage + 1 : 3), nc = c < c_last ? c + 1 : c_first;
           const bool nload = wrap ? k + 1 < cta_tiles : !first;
           const uint32_t next = nc * ACC_GRAD_NET + lead_col(ns);
-          const int next_chunks = nload ? lead_n(ns) / 8 : 0;
+          const int next_chunks = nload ? 8 : 0;
 #ifdef B200RL_TC3_TIMING
           const long long it0 = clock64();
 #endif
@@ -510,16 +551,14 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
 #endif
           if (stage == 3) {
             // dW3^T[i][o] += sum_r H2[r][i] dOut[r][o]
-            grad_mma<32, 8, 1>(acc, gcol + ACC_DW3, first, op2_at(H2_M, co), op2_at(DO_M, dob + c * 64), next,
-                               next_chunks, TC3_TACC);
+            grad_mma<32, 8, 1, 0, true>(acc, gcol + ACC_DW3, first, op2_at(H2_M, co), op2_at(DO_M, dob + c * 64),
+                                        next, next_chunks, TC3_TACC);
           } else if (stage == 4) {
             // every chain warpgroup's dH2 and both dW3 have read dOut: its buffer takes the next tile's observations
             if (c == c_last && k + 1 < cta_tiles) load_x(k + 1);
-            // dW2[o][i] += sum_r dZ2[r][o] H1[r][i] ; db2[o] += sum_r dZ2[r][o] * 1 (ones column of X)
-            grad_mma<64, 8, 2>(acc, gcol + ACC_DW2, first, op2_at(H2_M, co), op2_at(H1_M, co),
-                               gcol + ACC_DB2, first ? 0 : 2, TC3_TACC);
-            grad_mma<16, 8, 1>(acc, gcol + ACC_DB2, first, op2_at(H2_M, co), op2_at(X_M16, xo), next, next_chunks,
-                               TC3_TACC);
+            // dW2[o][i] += sum_r dZ2[r][o] H1[r][i] ; db2[o] += sum_r dZ2[r][o] * 1 (ones column of X), in dW2's groups
+            grad_mma<64, 8, 2, 16>(acc, gcol + ACC_DW2, first, op2_at(H2_M, co), op2_at(H1_M, co), next, next_chunks,
+                                   TC3_TACC, gcol + ACC_DB2, op2_at(X_M16, xo));
           } else {
             // dW1[o][i] += sum_r dZ1[r][o] X[r][i]; column 31 (ones) collects db1
             grad_mma<64, 8, 1>(acc, gcol + ACC_DW1, first, op2_at(H1_M, co), op2_at(X_M, xo), next, next_chunks,

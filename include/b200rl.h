@@ -341,6 +341,8 @@ typedef struct {
   int32_t max_steps;       /* capacity: train steps per call */
   int32_t algo;            /* 0 = DDPG / TD3 (by n_q), 1 = SAC (see b200rl_offpolicy_set_sac), 2 = DQN (see
                             * b200rl_offpolicy_set_dqn), 3 = C51 (see b200rl_offpolicy_set_c51) */
+  int32_t dueling_k;       /* 0 = the Q network is a plain MLP; K >= 1 = a dueling Q network (algo 2 / 3 only; see
+                            * "Dueling Q networks" below) */
 } b200rl_offpolicy_config;
 
 typedef struct {
@@ -522,6 +524,32 @@ typedef struct {
 /* Makes the engine's loss head QR-DQN's for every later train call; refused on engines not created with algo = 2
  * (TD3 / DDPG, SAC, C51); part of the cached graph's key. */
 int b200rl_offpolicy_set_qr(b200rl_offpolicy* h, const b200rl_qr_hparams* hp);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Dueling Q networks (Wang et al. 2016) for DQN, QR-DQN and C51: config dueling_k = K >= 1 on an algo 2 or 3 engine.
+ * The q description [obs, h1, h2, n K] (3 layers, hidden_act between layers, out_act identity) then describes
+ *   trunk      h   = act(x W1^T + b1)                                    W1 [h1, obs]
+ *   value      V   = act(h Wv^T + bv) Vo^T + vo                          Wv [h2, h1], Vo [K, h2]
+ *   advantage  A   = act(h Wa^T + ba) Ao^T + ao                          Wa [h2, h1], Ao [n K, h2]
+ *   output     Q[a, i] = V[i] + (A[a, i] - mean_i),  mean_i = (sum_b A[b, i]) / n        (action a owns columns
+ *              a K .. a K + K - 1 of A and Q, the layout of a plain Q network's output)
+ * in float32, the sum over actions b in index order and then one division by n; V[i] + (A[a, i] - mean_i) in that
+ * order.  The flat parameter vector of networks 1 and 4 (set_params, get_params, the state blob, Adam) is W1, b1, Wv,
+ * bv, Vo, vo, Wa, ba, Ao, ao: torch's parameters_to_vector of a module registering trunk, value and advantage in this
+ * order; its length is P = h1 (obs + 1) + 2 h2 (h1 + 1) + K (h2 + 1) + n K (h2 + 1).  Q feeds the engine's loss head
+ * unchanged: K = 1 for DQN, K = n_quantiles for QR-DQN (the quantile locations), K = n_atoms for C51 (the logits,
+ * aggregated before the softmax).  Backward: dV[i] = sum_a dQ[a, i] and dA[a, i] = dQ[a, i] - (sum_b dQ[b, i]) / n,
+ * both sums in index order; the trunk's input gradient dZv Wv + dZa Wa is one product whose k-sum runs over the value
+ * stream's units, then the advantage stream's.  Every sum has a fixed order: results are deterministic and a group's
+ * learners stay bit-identical to solo engines.  Prioritized replay, n-step returns, Double DQN, groups, the graph and
+ * plain launches work as for a plain Q network.  Launches: a forward pass of a network takes 6 (5 GEMMs and the
+ * aggregation) and the backward pass 9 (the aggregation's backward and 8 GEMMs), against 3 and 5 for a plain 3-layer
+ * network; with the loss head, Adam and the target copy a step of DQN, QR-DQN or C51 takes 24 launches (30 with
+ * double_q) where a plain 3-layer network's takes 14 (17), and a prioritized step adds its draw and priority update
+ * (2) to either.
+ * Refused at create: dueling_k < 0; dueling_k != 0 with algo 0 or 1; a q description that is not 3 layers, whose
+ * output width is not a multiple of dueling_k, or whose out_act is not identity.
+ * ------------------------------------------------------------------------------------------------------------ */
 
 /* ------------------------------------------------------------------------------------------------------------
  * Learner groups: K independent off-policy learners (same config, same hyper-parameters, their own parameters, Adam

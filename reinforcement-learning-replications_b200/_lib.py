@@ -80,7 +80,7 @@ class TrpoStats(C.Structure):
 
 class OffPolicyConfig(C.Structure):
     _fields_ = [("policy", MlpDesc), ("q", MlpDesc), ("n_q", C.c_int32), ("max_minibatch", C.c_int32),
-                ("max_steps", C.c_int32), ("algo", C.c_int32)]
+                ("max_steps", C.c_int32), ("algo", C.c_int32), ("dueling_k", C.c_int32)]
 
 
 class SacHparams(C.Structure):

@@ -30,6 +30,10 @@ class C51(DQN):
         N = q_function.n_atoms
         return n * N, f"{n} actions x {N} atoms logits"
 
+    @staticmethod
+    def _outputs_per_action(q_function):
+        return q_function.n_atoms, "n_atoms logits per action"
+
     def _upload_state(self, e, trainable, targets, lins) -> None:
         super()._upload_state(e, trainable, targets, lins)
         q = self.q_function

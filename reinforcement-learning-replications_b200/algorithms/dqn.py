@@ -9,10 +9,26 @@ import torch
 
 from .._lib import OffPolicyHparams
 from ..engine import OffPolicyEngine
+from ..networks import DuelingMLP
 from ..policies import EpsilonGreedyPolicy, GreedyPolicy
 from ..replay_buffer import PrioritizedReplayBuffer
-from ._onpolicy import adam_hparams, describe_mlp
+from ._onpolicy import _ACT_NAMES, adam_hparams, describe_mlp
 from .td3 import _learn, _make_eval_env, _OffPolicyBase
+
+
+def describe_q_network(module):
+    """(sizes, hidden activation, output activation, Linear layers in parameters() order, dueling K) of a DQN-family Q
+    network: an ``MLP`` as ``describe_mlp`` reads it (K = 0), or a ``DuelingMLP`` with sizes [obs, h_trunk, h_stream,
+    n_actions * K] and its five Linear layers (trunk, value hidden, value out, advantage hidden, advantage out)."""
+    if not isinstance(module, DuelingMLP):
+        return describe_mlp(module) + (0,)
+    acts = {type(m) for m in (module.trunk[1], module.value[1], module.advantage[1])}
+    if len(acts) != 1 or next(iter(acts)) not in _ACT_NAMES:
+        raise NotImplementedError(f"DuelingMLP activations must be one of Tanh, ReLU, Identity throughout, got "
+                                  f"{sorted(a.__name__ for a in acts)}")
+    linears = [module.trunk[0], module.value[0], module.value[2], module.advantage[0], module.advantage[2]]
+    sizes = module.sizes + [module.n_actions * module.outputs_per_action]
+    return sizes, _ACT_NAMES[acts.pop()], "identity", linears, module.outputs_per_action
 
 
 class DQN(_OffPolicyBase):
@@ -35,6 +51,9 @@ class DQN(_OffPolicyBase):
     TD error's), so n_step > 1 needs ``use_device_replay = True`` and a replay buffer with ``device_episode_ends``.
     ``n_step = 1`` is exactly the one-step update.  n_step is a constructor argument, not part of checkpoints.
 
+    The Q network is an ``MLP`` or a ``networks.DuelingMLP`` with ``n_actions`` = the action count and
+    ``outputs_per_action`` = 1 (C51: ``n_atoms``, QR-DQN: ``n_quantiles``); the engine runs either (b200rl.h).
+
     Acting: ``exploration_policy`` before ``num_start_steps``, then epsilon-greedy with epsilon falling linearly from
     ``epsilon_start`` to ``epsilon_end`` over the first ``epsilon_decay_steps`` environment steps; evaluation is greedy."""
     n_q = 1
@@ -48,7 +67,15 @@ class DQN(_OffPolicyBase):
         n = getattr(env.action_space, "n", None)
         if n is None:
             raise ValueError("DQN needs a discrete action space (one with .n)")
-        sizes, _, _, lins = describe_mlp(q_function.network)
+        net = q_function.network
+        if isinstance(net, DuelingMLP):
+            k, what_k = self._outputs_per_action(q_function)
+            if net.n_actions != int(n):
+                raise ValueError(f"the DuelingMLP has n_actions = {net.n_actions}, the action space has {int(n)} actions")
+            if net.outputs_per_action != k:
+                raise ValueError(f"{type(self).__name__} needs a DuelingMLP with outputs_per_action = {k} ({what_k}), "
+                                 f"got {net.outputs_per_action}")
+        sizes, _, _, lins, _ = describe_q_network(net)
         obs_shape = getattr(getattr(env, "observation_space", None), "shape", None)
         width, what = self._output_width(q_function, int(n))
         if sizes[-1] != width or (obs_shape and sizes[0] != int(np.prod(obs_shape))):
@@ -79,6 +106,11 @@ class DQN(_OffPolicyBase):
         """(width of the Q network's output for n actions, what it holds)."""
         return n, "one value per action"
 
+    @staticmethod
+    def _outputs_per_action(q_function):
+        """(outputs per action a DuelingMLP Q network must have, what they are)."""
+        return 1, "one value per action"
+
     def epsilon(self) -> float:
         """epsilon at the current total step count: linear from epsilon_start to epsilon_end, then constant."""
         t = getattr(self, "current_total_steps", 0)
@@ -98,19 +130,20 @@ class DQN(_OffPolicyBase):
         return [self.q_function], [self.target_q_function]
 
     def _ensure_engine(self, S: int, B: int) -> OffPolicyEngine:
-        qsz, qact, qout, _ = describe_mlp(self.q_function.network)
+        qsz, qact, qout, _, dk = describe_q_network(self.q_function.network)
         e = getattr(self, "_engine", None)
-        if e is None or e.q_sizes != qsz or e.max_minibatch < B or e.max_steps < S or e.q_acts != (qact, qout):
+        if (e is None or e.q_sizes != qsz or e.max_minibatch < B or e.max_steps < S or e.q_acts != (qact, qout)
+                or e.dueling_k != dk):
             if e is not None:
                 e.close()
-            e = OffPolicyEngine(None, qsz, 1, B, S, q_acts=(qact, qout), algo=self.algo)
+            e = OffPolicyEngine(None, qsz, 1, B, S, q_acts=(qact, qout), algo=self.algo, dueling_k=dk)
             self._engine = e
         return e
 
     def _hparams(self, noisy: bool, delay: int) -> OffPolicyHparams:
         hp = OffPolicyHparams()
         hp.gamma, hp.policy_delay = self.gamma, 1
-        lr, b1, b2, eps = adam_hparams(self.q_function.optimizer, describe_mlp(self.q_function.network)[3],
+        lr, b1, b2, eps = adam_hparams(self.q_function.optimizer, describe_q_network(self.q_function.network)[3],
                                        "q-function optimizer")
         hp.q1_lr, hp.q2_lr, hp.q_beta1, hp.q_beta2, hp.q_eps = lr, lr, b1, b2, eps
         return hp
@@ -135,7 +168,7 @@ class DQN(_OffPolicyBase):
             if S == 0:
                 return None, None
             self._device_rng_calls = getattr(self, "_device_rng_calls", 0) + 1
-            t0 = self._adam_step_count(self.q_function.optimizer, describe_mlp(self.q_function.network)[3])
+            t0 = self._adam_step_count(self.q_function.optimizer, describe_q_network(self.q_function.network)[3])
             self._last_beta = replay_buffer.beta(t0 + S - 1)  # the last step's beta, logged as replay/beta
             return "per", (getattr(self, "device_rng_seed", 0), self._device_rng_calls)
         self._last_beta = None
@@ -157,6 +190,10 @@ class DQN(_OffPolicyBase):
 
     def _train_schedule(self):
         return False, 1
+
+    def _learner_nets(self):
+        trainable, targets = self._nets()
+        return trainable, targets, [describe_q_network(m.network)[3] for m in trainable + targets]
 
     def learn(self, num_epochs: int = 2000, batch_size: int = 50, minibatch_size: int = 100,
               num_start_steps: int = 10000, num_steps_before_update: int = 1000, num_train_steps: int = 50,

@@ -27,6 +27,7 @@ from .._lib import MAX_LEARNERS
 from ..engine import OffPolicyEngine
 from ..replay_buffer import PrioritizedReplayBuffer
 from ._onpolicy import adam_hparams, describe_mlp
+from .dqn import describe_q_network
 from .qrdqn import QRDQN
 from .td3 import _learn_begin, _learn_evaluate_save, _learn_sample, _OffPolicyBase
 
@@ -39,7 +40,12 @@ def _signature(agent) -> list:
     names = ["q_function"] if dqn else ["policy"] + (["q_function_1", "q_function_2"] if agent.n_q == 2 else ["q_function"])
     sig = [("class", type(agent).__name__)]
     for name, m in zip(names, trainable):
-        sizes, hidden_act, out_act, lins = describe_mlp(m.network)
+        if dqn:
+            sizes, hidden_act, out_act, lins, k = describe_q_network(m.network)
+            sig.append((f"{name} network kind", "DuelingMLP" if k else "MLP"))
+            sig.append((f"{name} dueling (h_trunk, h_stream, outputs_per_action)", (sizes[1], sizes[2], k) if k else None))
+        else:
+            sizes, hidden_act, out_act, lins = describe_mlp(m.network)
         sig.append((f"{name} network", (tuple(sizes), hidden_act, out_act)))
         sig.append((f"{name} optimizer (lr, beta1, beta2, eps)", adam_hparams(m.optimizer, lins, f"{name} optimizer")))
     if dqn:
@@ -148,15 +154,17 @@ class LearnerGroup:
         discrete = m.algo in (OffPolicyEngine.DQN, OffPolicyEngine.C51)
         if discrete:  # no policy network
             psz, pact, pout = None, "relu", "tanh"
+            qsz, qact, qout, _, dk = describe_q_network(m.q_function.network)
         else:
             psz, pact, pout, _ = describe_mlp(m.policy.network)
-        qsz, qact, qout, _ = describe_mlp(m._nets()[0][0 if discrete else 1].network)
+            qsz, qact, qout, _ = describe_mlp(m._nets()[0][1].network)
+            dk = 0
         e = self._engine
         if (e is None or e.K != len(self.members) or e.max_minibatch < B or e.max_steps < S or e.policy_sizes != psz
-                or e.q_sizes != qsz or e.policy_acts != (pact, pout) or e.q_acts != (qact, qout)):
+                or e.q_sizes != qsz or e.policy_acts != (pact, pout) or e.q_acts != (qact, qout) or e.dueling_k != dk):
             self._close_engine()
             e = OffPolicyEngine(psz, qsz, m.n_q, B, S, (pact, pout), (qact, qout), algo=m.algo,
-                                n_learners=len(self.members))
+                                n_learners=len(self.members), dueling_k=dk)
             self._engine = e
         return e
 

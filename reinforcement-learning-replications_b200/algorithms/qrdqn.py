@@ -28,6 +28,10 @@ class QRDQN(DQN):
         N = q_function.n_quantiles
         return n * N, f"{n} actions x {N} quantiles"
 
+    @staticmethod
+    def _outputs_per_action(q_function):
+        return q_function.n_quantiles, "n_quantiles locations per action"
+
     def _upload_state(self, e, trainable, targets, lins) -> None:
         super()._upload_state(e, trainable, targets, lins)
         e.set_qr(self.q_function.n_quantiles)

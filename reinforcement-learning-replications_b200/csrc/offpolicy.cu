@@ -23,6 +23,9 @@
 // C51 (config algo = 3) is DQN's step program with a categorical head over return distributions (c51_loss_kernel).
 // QR-DQN (set_qr on a DQN engine) is DQN's step program with a quantile Huber head (qr_loss_kernel), prioritized replay
 // and n-step returns included.
+// Dueling Q networks (config dueling_k, DQN / QR-DQN / C51): dueling_forward / dueling_backward take the place of
+// net_forward / net_backward for networks 1 and 4 -- the same GEMMs plus dueling_forward_kernel / dueling_backward_kernel
+// between the last layer and the loss head; nothing else in the step program differs.
 // Prioritized replay for DQN (train_prioritized): a 32-way sum tree per replay buffer, drawn from, weighed and gathered
 // by per_draw_kernel and updated by per_update_kernel inside the same step program.
 // n-step returns for DQN / C51 (set_nstep): nstep_gather_kernel (or per_draw_kernel's NSTEP instantiation) walks each
@@ -63,6 +66,8 @@ __device__ __forceinline__ float smooth_target_action(float a, float eps, float 
 // MODE 1 (NN): C[M,N] = (A (.) act'(Y))[M,K] * B[K,N]                  dX = dZ * W,   A = dY, Y = layer output
 // MODE 2 (TN): C[M,N] = (A (.) act'(Y))[K,M]^T * B[K,N]                dW = dZ^T * X, A = dY [rows, out];
 //              and, when dbias is set, dbias[M] = column sums of (A (.) act'(Y)) -- the bias gradient rides along
+// MODE 3 (NN, split B): MODE 1 with rows >= ksplit of B read from A2[row - ksplit] (ld lda2): dX through a layer whose
+//              weight is two [out, in] blocks kept apart, the dueling streams' hidden layers [W_value; W_advantage]
 // All matrices row-major with explicit leading dimensions.  Y (same shape / ld as A) may be NULL (no derivative).
 struct GemmArgs {
   const float* A; int lda;
@@ -83,7 +88,7 @@ struct GemmArgs {
 // multiplied out of shared memory tile by tile.
 typedef float GemmTile[GK][GT + 2];
 
-template <int MODE>
+template <int MODE, bool SPLIT_B = false>  // MODE 3 runs as <1, true>: MODE 1 but for where B's rows come from
 __device__ __forceinline__ void gemm_tile(const GemmArgs& g, int bx, int by, GemmTile& As, GemmTile& Bs) {
   constexpr int KT = 8;  // k-tiles fetched ahead (registers: 8 per k-tile): K = 256 is ONE round of loads
   const int tid = threadIdx.x;
@@ -114,8 +119,12 @@ __device__ __forceinline__ void gemm_tile(const GemmArgs& g, int bx, int by, Gem
         const int gn = n0 + n, gk = k0 + k;
         float b = 0.f;
         if (gn < g.N && gk < g.K) {
-          if (MODE == 2 && g.A2 != nullptr && gn >= g.ksplit) b = g.A2[(size_t)gk * g.lda2 + (gn - g.ksplit)];
-          else b = MODE == 0 ? g.B[(size_t)gn * g.ldb + gk] : g.B[(size_t)gk * g.ldb + gn];
+          if constexpr (SPLIT_B) {
+            b = gk >= g.ksplit ? g.A2[(size_t)(gk - g.ksplit) * g.lda2 + gn] : g.B[(size_t)gk * g.ldb + gn];
+          } else {
+            if (MODE == 2 && g.A2 != nullptr && gn >= g.ksplit) b = g.A2[(size_t)gk * g.lda2 + (gn - g.ksplit)];
+            else b = MODE == 0 ? g.B[(size_t)gn * g.ldb + gk] : g.B[(size_t)gk * g.ldb + gn];
+          }
         }
         rb[e] = b;
       }
@@ -203,9 +212,9 @@ __global__ void __launch_bounds__(GTHREADS) gemm_kernel(const GemmArgs g, size_t
     a.dbias = lane_ptr(a.dbias, off);
     a.A2 = lane_ptr(a.A2, off);
     a.eps = lane_ptr(a.eps, off);
-    gemm_tile<MODE>(a, blockIdx.x, blockIdx.y, As, Bs);
+    gemm_tile<MODE == 3 ? 1 : MODE, MODE == 3>(a, blockIdx.x, blockIdx.y, As, Bs);
   } else {
-    gemm_tile<MODE>(g, blockIdx.x, blockIdx.y, As, Bs);
+    gemm_tile<MODE == 3 ? 1 : MODE, MODE == 3>(g, blockIdx.x, blockIdx.y, As, Bs);
   }
 }
 
@@ -698,6 +707,51 @@ __global__ void dqn_target_copy_kernel(float* target, const float* param, int n,
   if (flags[idx].x == 0.f) return;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) target[i] = param[i];
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Dueling Q networks (config dueling_k = K; Wang et al. 2016, eq. 9, per output column): the value stream's V [B, K] and
+// the advantage stream's A [B, n K] sit side by side in va [B, K + n K] (row b = [V_b | A_b], action a owning A's
+// columns a K .. a K + K - 1).  One thread per (row, column i < K); both sums run over the actions in index order.
+//   forward   mean_i = (sum_a A[a, i]) / n,  Q[a, i] = V[i] + (A[a, i] - mean_i)          -> q [B, n K]
+//   backward  s_i = sum_a dQ[a, i],  dV[i] = s_i,  dA[a, i] = dQ[a, i] - s_i / n            -> dva [B, K + n K]
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) dueling_forward_kernel(const float* va, int B, int n, int k, float* q,
+                                                                  size_t lane_stride) {
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    va = lane_ptr(va, o), q = lane_ptr(q, o);
+  }
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= B * k) return;
+  const int b = t / k, i = t - b * k;
+  const float* v = va + (size_t)b * (k + n * k);
+  const float* a = v + k + i;
+  float s = 0.f;
+  for (int j = 0; j < n; ++j) s += a[(size_t)j * k];
+  const float mean = s / (float)n, vi = v[i];
+  float* out = q + (size_t)b * n * k + i;
+  for (int j = 0; j < n; ++j) out[(size_t)j * k] = vi + (a[(size_t)j * k] - mean);
+}
+
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) dueling_backward_kernel(const float* dq, int B, int n, int k, float* dva,
+                                                                   size_t lane_stride) {
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    dq = lane_ptr(dq, o), dva = lane_ptr(dva, o);
+  }
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= B * k) return;
+  const int b = t / k, i = t - b * k;
+  const float* g = dq + (size_t)b * n * k + i;
+  float s = 0.f;
+  for (int j = 0; j < n; ++j) s += g[(size_t)j * k];
+  const float mean = s / (float)n;
+  float* dv = dva + (size_t)b * (k + n * k);
+  dv[i] = s;
+  float* da = dv + k + i;
+  for (int j = 0; j < n; ++j) da[(size_t)j * k] = g[(size_t)j * k] - mean;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1235,6 +1289,10 @@ struct NetBuf {
   bool present = false;
   int64_t step[B200RL_MAX_LEARNERS] = {};  // Adam step count of each learner
   int w_off[B200RL_MAX_LAYERS], b_off[B200RL_MAX_LAYERS];
+  // dueling Q network (config dueling_k = K > 0; d = [obs, h1, h2, n K]): its five Linear layers' offsets, in the
+  // order trunk, value hidden, value out, advantage hidden, advantage out
+  int duel_k = 0;
+  int dw_off[5] = {}, db_off[5] = {};
 };
 
 // What a captured step program holds in its nodes besides the engine's own buffers: a graph is replayed only for a call
@@ -1488,6 +1546,89 @@ int net_backward(b200rl_offpolicy* h, const NetBuf& nb, float* const* acts, cons
   return 0;
 }
 
+// A dueling Q network (nb.duel_k = K; nb.d = [O, h1, h2, n K]) on acts[0] = input [rows, O]: acts[1] = trunk [rows, h1],
+// acts[2] = [value hidden | advantage hidden] [rows, 2 h2], acts[4] = [V | A] [rows, K + n K], and acts[3] = Q [rows, n K]
+// (dueling_forward_kernel), the slot a plain network's output takes, where the loss heads read it.
+int dueling_forward(const b200rl_offpolicy* h, const NetBuf& nb, float* const* acts, int rows, cudaStream_t s) {
+  const int O = nb.d.sizes[0], h1 = nb.d.sizes[1], h2 = nb.d.sizes[2], nK = nb.d.sizes[3], K = nb.duel_k;
+  auto layer = [&](int l, const float* x, int ldx, int nin, float* y, int ldy, int nout, int act) {
+    GemmArgs g{};
+    g.A = x; g.lda = ldx;
+    g.B = nb.params + nb.dw_off[l]; g.ldb = nin;
+    g.C = y; g.ldc = ldy;
+    g.bias = nb.params + nb.db_off[l];
+    g.act = act;
+    g.M = rows; g.N = nout; g.K = nin;
+    return gemm<0>(h, g, s);
+  };
+  const int hid = nb.d.hidden_act, out = nb.d.out_act;
+  if (layer(0, acts[0], O, O, acts[1], h1, h1, hid) || layer(1, acts[1], h1, h1, acts[2], 2 * h2, h2, hid) ||
+      layer(3, acts[1], h1, h1, acts[2] + h2, 2 * h2, h2, hid) ||
+      layer(2, acts[2], 2 * h2, h2, acts[4], K + nK, K, out) ||
+      layer(4, acts[2] + h2, 2 * h2, h2, acts[4] + K, K + nK, nK, out))
+    return 1;
+  return launch(h, dueling_forward_kernel<false>, dueling_forward_kernel<true>, (unsigned)((rows * K + GTHREADS - 1) / GTHREADS),
+                GTHREADS, 0, s, acts[4], rows, nK / K, K, acts[3]);
+}
+
+// Its backward pass from dOut = dL/dQ [rows, n K] into nb.grad: dueling_backward_kernel, then each stream's output and
+// hidden layer, then the trunk, whose input gradient dZv Wv + dZa Wa is one split-B GEMM (k over [value | advantage]
+// in that order).  The dX chain stays on `s`, the weight-gradient products go to s_dw behind the gradient they read;
+// dbuf0 / dbuf1 / dbuf2 hold dL/d[V | A], dL/d(stream hidden) and dL/d(trunk), each written once per step.
+int dueling_backward(b200rl_offpolicy* h, const NetBuf& nb, float* const* acts, const float* dOut, int rows,
+                     cudaStream_t s, cudaStream_t s_dw) {
+  const int O = nb.d.sizes[0], h1 = nb.d.sizes[1], h2 = nb.d.sizes[2], nK = nb.d.sizes[3], K = nb.duel_k;
+  const int hid = nb.d.hidden_act;
+  float *dva = h->dbuf0, *dh2 = h->dbuf1, *dh1 = h->dbuf2;
+  auto fork = [&]() {  // what `s` has queued so far is complete before the next products on s_dw
+    B200RL_CUDA(cudaEventRecord(h->ev_side, s));
+    B200RL_CUDA(cudaStreamWaitEvent(s_dw, h->ev_side, 0));
+    return 0;
+  };
+  // dW[nout, nin] = (dY . act'(Y))^T X and db on s_dw
+  auto dw = [&](int l, const float* dY, int ldd, const float* Y, int act, const float* X, int ldx, int nout, int nin) {
+    GemmArgs g{};
+    g.A = dY; g.lda = ldd; g.Y = Y; g.ldy = ldd; g.act = act;
+    g.B = X; g.ldb = ldx;
+    g.C = nb.grad + nb.dw_off[l]; g.ldc = nin;
+    g.M = nout; g.N = nin; g.K = rows;
+    g.dbias = nb.grad + nb.db_off[l];
+    return gemm<2>(h, g, s_dw);
+  };
+  // dX[rows, nin] = dY[rows, nout] W[nout, nin] on s (the output layers are linear: no derivative)
+  auto dx = [&](int l, const float* dY, int ldd, float* dst, int ldc, int nout, int nin) {
+    GemmArgs g{};
+    g.A = dY; g.lda = ldd;
+    g.B = nb.params + nb.dw_off[l]; g.ldb = nin;
+    g.C = dst; g.ldc = ldc;
+    g.M = rows; g.N = nin; g.K = nout;
+    return gemm<1>(h, g, s);
+  };
+  if (launch(h, dueling_backward_kernel<false>, dueling_backward_kernel<true>,
+             (unsigned)((rows * K + GTHREADS - 1) / GTHREADS), GTHREADS, 0, s, dOut, rows, nK / K, K, dva))
+    return 1;
+  if (fork() || dw(2, dva, K + nK, nullptr, B200RL_ACT_IDENTITY, acts[2], 2 * h2, K, h2) ||
+      dw(4, dva + K, K + nK, nullptr, B200RL_ACT_IDENTITY, acts[2] + h2, 2 * h2, nK, h2))
+    return 1;
+  if (dx(2, dva, K + nK, dh2, 2 * h2, K, h2) || dx(4, dva + K, K + nK, dh2 + h2, 2 * h2, nK, h2)) return 1;
+  if (fork() || dw(1, dh2, 2 * h2, acts[2], hid, acts[1], h1, h2, h1) ||
+      dw(3, dh2 + h2, 2 * h2, acts[2] + h2, hid, acts[1], h1, h2, h1))
+    return 1;
+  {
+    GemmArgs g{};  // dX[rows, h1] = (dH . act'(H))[rows, 2 h2] [Wv; Wa][2 h2, h1]
+    g.A = dh2; g.lda = 2 * h2; g.Y = acts[2]; g.ldy = 2 * h2; g.act = hid;
+    g.B = nb.params + nb.dw_off[1]; g.ldb = h1;
+    g.A2 = nb.params + nb.dw_off[3]; g.lda2 = h1; g.ksplit = h2;
+    g.C = dh1; g.ldc = h1;
+    g.M = rows; g.N = h1; g.K = 2 * h2;
+    if (gemm<3>(h, g, s)) return 1;
+  }
+  if (fork() || dw(0, dh1, h1, acts[1], hid, acts[0], O, h1, O)) return 1;
+  B200RL_CUDA(cudaEventRecord(h->ev_side, s_dw));
+  B200RL_CUDA(cudaStreamWaitEvent(s, h->ev_side, 0));
+  return 0;
+}
+
 int adam_net(const b200rl_offpolicy* h, NetBuf& nb, const float2* table, int idx, double b1, double b2, double eps,
              cudaStream_t s) {
   return adam_step_table(nb.params, nb.grad, nb.m, nb.v, nb.P, table, idx, b1, b2, eps, s, h->K, h->lane_stride);
@@ -1517,8 +1658,24 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
     B200RL_REQUIRE(memcmp(&cfg->policy, &zero, sizeof(zero)) == 0,
                    "offpolicy_create: DQN has no policy network: the policy description must be zeroed");
   }
-  const int64_t Pp = dqn ? 0 : b200rl_mlp_param_count(&cfg->policy), Pq = b200rl_mlp_param_count(&cfg->q);
+  int64_t Pp = dqn ? 0 : b200rl_mlp_param_count(&cfg->policy), Pq = b200rl_mlp_param_count(&cfg->q);
   B200RL_REQUIRE((dqn || Pp > 0) && Pq > 0, "offpolicy_create: invalid MLP description");
+  const int DK = cfg->dueling_k;
+  B200RL_REQUIRE(DK == 0 || dqn, "offpolicy_create: dueling_k must be 0 unless algo = 2 (DQN / QR-DQN) or 3 (C51), got "
+                 "%d", DK);
+  if (DK != 0) {
+    const b200rl_mlp_desc& d = cfg->q;
+    B200RL_REQUIRE(DK >= 1, "offpolicy_create: dueling_k must be >= 1 (or 0: a plain MLP), got %d", DK);
+    B200RL_REQUIRE(d.n_layers == 3, "offpolicy_create: a dueling Q network is described as [obs, h_trunk, h_stream, "
+                   "n_actions x dueling_k] (3 layers), got %d layers", d.n_layers);
+    B200RL_REQUIRE(d.sizes[3] % DK == 0, "offpolicy_create: the dueling Q network's output width %d is not n_actions x "
+                   "dueling_k for dueling_k = %d", d.sizes[3], DK);
+    B200RL_REQUIRE(d.out_act == B200RL_ACT_IDENTITY, "offpolicy_create: a dueling Q network's stream outputs must be "
+                   "linear (out_act identity)");
+    // trunk, value hidden, value out, advantage hidden, advantage out
+    Pq = (int64_t)d.sizes[1] * (d.sizes[0] + 1) + 2 * (int64_t)d.sizes[2] * (d.sizes[1] + 1) +
+         (int64_t)(DK + d.sizes[3]) * (d.sizes[2] + 1);
+  }
   const int O = dqn ? cfg->q.sizes[0] : cfg->policy.sizes[0], P_out = cfg->policy.sizes[cfg->policy.n_layers];
   // SAC: the policy outputs [mean | log_std], 2A wide; DQN: the action column holds the index (1 wide)
   const int A = dqn ? 1 : sac ? cfg->q.sizes[0] - O : P_out;
@@ -1548,6 +1705,19 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
       nb.b_off[l] = off;
       off += nb.d.sizes[l + 1];
       maxw = nb.d.sizes[l + 1] > maxw ? nb.d.sizes[l + 1] : maxw;
+    }
+    if (DK != 0 && (i == 1 || i == 4)) {  // the activation stacks also hold [rows, 2 h2] and [rows, K + n K]
+      const int O_ = nb.d.sizes[0], h1 = nb.d.sizes[1], h2 = nb.d.sizes[2], nK = nb.d.sizes[3];
+      const int ins[5] = {O_, h1, h2, h1, h2}, outs[5] = {h1, h2, DK, h2, nK};
+      nb.duel_k = DK;
+      off = 0;
+      for (int l = 0; l < 5; ++l) {
+        nb.dw_off[l] = off;
+        off += outs[l] * ins[l];
+        nb.db_off[l] = off;
+        off += outs[l];
+      }
+      maxw = std::max(maxw, std::max(2 * h2, DK + nK));
     }
     if (cfg->n_q == 1 && (i == 2 || i == 5)) continue;
     if (sac && i == 3) continue;  // SAC has no target policy
@@ -2158,7 +2328,8 @@ static auto qr_head(bool weighted, bool nstep) {
 //   s3 : Q(s) ---------------------+   ........ Q's dW products
 // Q(s') reads the parameters at the start of the step: the step's Adam waits for the loss kernel, which joins it.
 // A C51 engine (h->c51) takes c51_loss_kernel as its loss head, a QR-DQN engine (h->qr) qr_loss_kernel; nothing else
-// in the step differs.
+// in the step differs.  A dueling Q network (q.duel_k) runs dueling_forward / dueling_backward in place of
+// net_forward / net_backward.
 // A prioritized call (h->per_run) opens each step with the draw on s (draw, weights, gather), takes the weighted loss
 // head, and runs the priority update on s4 beside the backward pass; the next step's draw joins it.
 static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s) {
@@ -2167,6 +2338,10 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
   const bool dbl = h->dqn_hp.double_q != 0;
   NetBuf &q = h->net[1], &qt = h->net[4];
   const int L = q.d.n_layers, n = q.d.sizes[L];
+  const int top = q.duel_k ? L + 1 : L;  // a dueling network's stack also holds [V | A] (dueling_forward)
+  auto forward = [&](float* const* acts, cudaStream_t st) {
+    return q.duel_k ? dueling_forward(h, q, acts, B, st) : net_forward(h, q, acts, B, st);
+  };
   const int ew = 256;
   cudaStream_t s2 = h->s2, s3 = h->s3, s4 = h->s4;
   const bool per = h->per_run;
@@ -2193,20 +2368,20 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
     }
     float* qa[B200RL_MAX_LAYERS + 1];  // Q(s): its stack is what the backward pass reads
     qa[0] = s_obs;
-    for (int l = 1; l <= L; ++l) qa[l] = h->acts[1][l];
+    for (int l = 1; l <= top; ++l) qa[l] = h->acts[1][l];
     if (edge(h, s, s3)) return 1;
-    if (net_forward(h, q, qa, B, s3)) return 1;
+    if (forward(qa, s3)) return 1;
     float* qn[B200RL_MAX_LAYERS + 1];
     if (dbl) {
       qn[0] = s_nobs;
-      for (int l = 1; l <= L; ++l) qn[l] = h->acts[3][l];
+      for (int l = 1; l <= top; ++l) qn[l] = h->acts[3][l];
       if (edge(h, s, s2)) return 1;
-      if (net_forward(h, q, qn, B, s2)) return 1;
+      if (forward(qn, s2)) return 1;
     }
     float* tq[B200RL_MAX_LAYERS + 1];
     tq[0] = s_nobs;
-    for (int l = 1; l <= L; ++l) tq[l] = h->acts_tq[l];
-    if (net_forward(h, qt, tq, B, s)) return 1;
+    for (int l = 1; l <= top; ++l) tq[l] = h->acts_tq[l];
+    if (q.duel_k ? dueling_forward(h, qt, tq, B, s) : net_forward(h, qt, tq, B, s)) return 1;
     if (dbl && edge(h, s2, s)) return 1;
     if (edge(h, s3, s)) return 1;
     if (h->c51) {
@@ -2238,7 +2413,9 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
                  h->per_absd, B, alpha, eps, h->per_newp + (size_t)st * B, h->per_bad + st))
         return 1;
     }
-    if (net_backward(h, q, qa, h->dqn_dout, n, B, true, nullptr, s, false, nullptr, 0, 0, s3)) return 1;
+    if (q.duel_k ? dueling_backward(h, q, qa, h->dqn_dout, B, s, s3)
+                 : net_backward(h, q, qa, h->dqn_dout, n, B, true, nullptr, s, false, nullptr, 0, 0, s3))
+      return 1;
     if (adam_net(h, q, h->adam_tab + (size_t)maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, s)) return 1;
     if (launch(h, dqn_target_copy_kernel<false>, dqn_target_copy_kernel<true>, (unsigned)((q.P + ew - 1) / ew), ew, 0,
                s, qt.params, q.params, (int)q.P, h->adam_tab + (size_t)3 * maxS, st))

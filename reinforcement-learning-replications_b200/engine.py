@@ -325,7 +325,9 @@ class OffPolicyEngine:
     = None, ``n_q`` = 1, the Q network maps obs -> [n actions], only networks 1 (Q) and 4 (target Q) exist, actions are
     indices (act [S,B]), and ``set_dqn`` must be called before the first train call.  C51 is a DQN engine whose Q
     network maps obs -> [n actions x n atoms] logits; it needs ``set_c51`` as well as ``set_dqn``.  QR-DQN is a DQN
-    engine after ``set_qr``: its Q network maps obs -> [n actions x n quantiles] quantile locations.
+    engine after ``set_qr``: its Q network maps obs -> [n actions x n quantiles] quantile locations.  ``dueling_k`` = K
+    >= 1 (DQN / QR-DQN / C51): the Q network is a dueling one, ``q_sizes`` = [obs, h_trunk, h_stream, n actions x K]
+    (b200rl.h, "Dueling Q networks").
 
     ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
     launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
@@ -335,7 +337,7 @@ class OffPolicyEngine:
     TD3, SAC, DQN, C51 = 0, 1, 2, 3
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
-                 q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1):
+                 q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1, dueling_k: int = 0):
         from ._lib import OffPolicyConfig
         self.lib = _lib.load()
         current_stream_handle()
@@ -344,14 +346,17 @@ class OffPolicyEngine:
             cfg.policy = MlpDesc.make(policy_sizes, *policy_acts)
         cfg.q = MlpDesc.make(q_sizes, *q_acts)
         cfg.n_q, cfg.max_minibatch, cfg.max_steps = int(n_q), int(max_minibatch), int(max_steps)
-        cfg.algo = int(algo)
-        self.algo = int(algo)
+        cfg.algo, cfg.dueling_k = int(algo), int(dueling_k)
+        self.algo, self.dueling_k = int(algo), int(dueling_k)
         self.discrete = self.algo in (self.DQN, self.C51)  # DQN's networks, inputs and outputs
         self.n_q, self.max_minibatch, self.max_steps = int(n_q), int(max_minibatch), int(max_steps)
         self.policy_sizes, self.q_sizes = None if policy_sizes is None else list(policy_sizes), list(q_sizes)
         self.policy_acts, self.q_acts = tuple(policy_acts), tuple(q_acts)
         self.n_policy = 0 if policy_sizes is None else int(self.lib.b200rl_mlp_param_count(cfg.policy))
         self.n_qp = int(self.lib.b200rl_mlp_param_count(cfg.q))
+        if self.dueling_k and len(self.q_sizes) == 4:  # trunk, both streams' hidden layers, V and A (b200rl.h)
+            O, h1, h2, w = self.q_sizes
+            self.n_qp = h1 * (O + 1) + 2 * h2 * (h1 + 1) + (self.dueling_k + w) * (h2 + 1)
         self.K = int(n_learners)
         h = C.c_void_p()
         check(self.lib.b200rl_offpolicy_create_group(C.byref(cfg), self.K, C.byref(h)), "offpolicy_create")

@@ -1,3 +1,4 @@
+from .dueling import DuelingMLP
 from .mlp import MLP
 
-__all__ = ["MLP"]
+__all__ = ["DuelingMLP", "MLP"]

@@ -7,11 +7,13 @@
 //   * the POLICY chain and the VALUE chain of the SAME tile run side by side, and the observation operand is staged
 //     once for both.  Rows are independent in the forward / backward chain, so each (network, 64-row half) is one
 //     warpgroup that issues its own m64 products and keeps the accumulator in registers: its epilogues work on the
-//     wgmma fragment and hand over to its next product through a warpgroup-local barrier.  A fifth warpgroup brings
-//     the observations in and issues the weight-gradient products off the chains' critical path; mbarriers tell it
-//     when both halves of a network have delivered a stage's operands, and tell the chains when it has finished
-//     reading a buffer they are about to overwrite.  Its accumulators stay in L2 (tc_common.cuh), stored fragment by
-//     fragment (grad_acc_off), and each fragment is prefetched into L1 while the products before it run (grad_mma);
+//     wgmma fragment and hand over to its next product through a warpgroup-local barrier.  Two more warpgroups, one
+//     per network, issue the weight-gradient products off the chains' critical path, side by side: the two networks'
+//     products share no accumulator and no written buffer.  mbarriers tell a gradient warpgroup when both halves of
+//     its network have delivered a stage's operands, and tell the chains when it has finished reading a buffer they
+//     are about to overwrite; the warpgroup of the last running network also brings the observations in.  The
+//     accumulators stay in L2 (tc_common.cuh), stored fragment by fragment (grad_acc_off), and each fragment is
+//     prefetched into L1 while the products before it run (grad_mma);
 //   * the observations are split into their fp16 pairs ONCE PER UPDATE by pack_obs_kernel (every step of the update
 //     reads the same observations) into ready-made SWIZZLE_128B tile images [128 rows][h cols 0..31 | l cols 32..63];
 //     the step kernel brings a tile image in with ONE 16 KB bulk copy (cp.async.bulk + mbarrier complete_tx) issued by
@@ -39,7 +41,7 @@ namespace b200rl {
 constexpr int T3_ROWS = 128;
 constexpr int T3_CHAIN_WARPS = 16;  // four chain warpgroups, one per (network, 64-row half of the tile)
 constexpr int T3_CHAIN_THREADS = T3_CHAIN_WARPS * 32;
-constexpr int T3_THREADS = T3_CHAIN_THREADS + 128;  // + the producer / weight-gradient warpgroup
+constexpr int T3_THREADS = T3_CHAIN_THREADS + 256;  // + one weight-gradient warpgroup per network
 
 // ---- shared-memory map (bytes from the 1024-aligned base) ----
 constexpr uint32_t S3_XB = 0;                        // X(k) | dOut(k) buffers, parity k & 1 and (k + 1) & 1
@@ -53,8 +55,8 @@ constexpr uint32_t S3_BIAS = S3_OPERANDS_END;        // per net: b1[64] b2[64] b
 constexpr uint32_t S3_DIST = S3_BIAS + 2 * 640;      // var[16], log_scale[16], 1/(2 var)[16], 1/var[16]
 constexpr uint32_t S3_SCALE = S3_DIST + 256;         // per net 16 floats
 constexpr uint32_t S3_XS = S3_SCALE + 128;           // 2^ex_k [32], 2^-ex_k [32]
-constexpr uint32_t S3_RED = S3_XS + 256;             // setup reduction scratch [20 warps][8] floats
-constexpr uint32_t S3_BARS = S3_RED + 640;           // 15 mbarriers (8 B each), bad flag at +120
+constexpr uint32_t S3_RED = S3_XS + 256;             // setup reduction scratch [24 warps][8] floats
+constexpr uint32_t S3_BARS = S3_RED + 4 * 8 * (T3_THREADS / 32);  // 15 mbarriers (8 B each), bad flag at +120
 constexpr uint32_t S3_TOTAL = S3_BARS + 128;
 constexpr uint32_t T3_SMEM_BYTES = S3_TOTAL + 1024;  // + alignment slack
 static_assert(T3_SMEM_BYTES <= 227 * 1024, "mlp_tc3 shared memory");
@@ -92,14 +94,15 @@ __device__ __forceinline__ uint32_t grad_acc_off(uint32_t pcol, int n, int row, 
 
 #ifdef B200RL_TC3_TIMING
 // CTA 0, chain warpgroup wg = 2 c + h: [10 wg + s - 1] cycles stage s (E1..E5) waited on an mbarrier, [10 wg + 4 + s]
-// cycles of stage s in all; gradient warpgroup: [40 + 3 c + s - 3] cycles waited for the operands of stage s (3..5) of
-// network c, [46 + 3 c + s - 3] cycles issuing its products, split over all stages into [56] waiting for its fragment
-// loads (and asking for the next fragment), [57] wgmma_fence .. wgmma_wait_all, [58] fragment stores and the hand-over
-// (bar.sync 5, mbar_arrive); [52] tiles of the CTA, [53] set-up, [54] tile loop, [55] read-out
+// cycles of stage s in all; gradient warpgroup of network c: [40 + 3 c + s - 3] cycles waited for the operands of stage
+// s (3..5) (stage 4 of the observations' producer: also for the other network to release the dOut buffer),
+// [46 + 3 c + s - 3] cycles issuing its products, split over all stages into [56 + 3 c] waiting for its fragment loads
+// (and asking for the next fragment), [57 + 3 c] wgmma_fence .. wgmma_wait_all, [58 + 3 c] fragment stores and the
+// hand-over (bar.sync, mbar_arrive); [52] tiles of the CTA, [53] set-up, [54] tile loop, [55] read-out
 __device__ unsigned long long g_tc3_t[64];
-#define TC3_TACC tacc
+#define TC3_TSPLIT(c) (tacc + 56 + 3 * (c))
 #else
-#define TC3_TACC nullptr
+#define TC3_TSPLIT(c) nullptr
 #endif
 
 enum { C3_G = 0, C3_U1, C3_U2, C3_U3, C3_UH2, C3_UH1, C3_W1, C3_W2, C3_W3, C3_OW3, C3_OW2, C3_OW1, C3_OB, C3_N };
@@ -234,7 +237,7 @@ __device__ __forceinline__ void grad_products(float (&d)[N / 2], uint32_t a_lo, 
 // halves), B split l (B_SPLITS == 2) then h.  Each wgmma group loads its fragments from the accumulator memory, asks for
 // the fragment of the group after it (this product's second half, then `next_chunks` chunks of the product at column
 // `next_col`) to be brought into L1, runs its products and stores the fragments back.  A group's cost is mostly its
-// fragments' L2 round trip, whatever its width, so the groups hold as many products as 96 registers a thread allow:
+// fragments' L2 round trip, whatever its width, so the groups hold as many products as 80 registers a thread allow:
 //   * BOTH: both m64 halves of an n32 product in one group -- 32 floats, chunks 0..7 as an n64 half's (grad_acc_off);
 //   * N2 > 0: with each half, the same half of a second, single-term product of width N2 with the same A (B = `b2`, at
 //     accumulator column `col2`).
@@ -242,7 +245,7 @@ __device__ __forceinline__ void grad_products(float (&d)[N / 2], uint32_t a_lo, 
 // overwrite and nothing is loaded.
 template <int N, int KSTEPS, int B_SPLITS, int N2 = 0, bool BOTH = false>
 __device__ __forceinline__ void grad_mma(float* acc_cta, uint32_t acc_col, bool first, const Op2 a, const Op2 b,
-                                         uint32_t next_col, int next_chunks, unsigned long long* tacc,
+                                         uint32_t next_col, int next_chunks, unsigned long long* tsplit,
                                          uint32_t col2 = 0, const Op2 b2 = Op2{}) {
   static_assert(!BOTH || (N == 32 && N2 == 0), "one group for both halves: an n32 product");
   constexpr int CH = BOTH ? 8 : N / 8, CH2 = N2 / 8;  // fragment chunks of the group
@@ -303,9 +306,9 @@ __device__ __forceinline__ void grad_mma(float* acc_cta, uint32_t acc_col, bool 
     for (int j = 0; j < CH2; ++j)
       *reinterpret_cast<float4*>(frag2 + 512 * j) = make_float4(e[4 * j], e[4 * j + 1], e[4 * j + 2], e[4 * j + 3]);
 #ifdef B200RL_TC3_TIMING
-    tacc[56] += (unsigned long long)(t1 - t0);
-    tacc[57] += (unsigned long long)(t2 - t1);
-    tacc[58] += (unsigned long long)(clock64() - t2);
+    tsplit[0] += (unsigned long long)(t1 - t0);
+    tsplit[1] += (unsigned long long)(t2 - t1);
+    tsplit[2] += (unsigned long long)(clock64() - t2);
 #endif
   }
 }
@@ -481,9 +484,9 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     mbar_init(bars + 8, 1);
     for (int i = 0; i < 6; ++i) {
       mbar_init(bars + 16 + 8 * i, 2);  // ready[c][s]: one arrive per chain warpgroup of network c
-      mbar_init(bars + 64 + 8 * i, 1);  // done[c][s]: the gradient warpgroup
+      mbar_init(bars + 64 + 8 * i, 1);  // done[c][s]: the gradient warpgroup of network c
     }
-    mbar_init(bars + 112, 1);  // dofree
+    mbar_init(bars + 112, (uint32_t)run_p + (uint32_t)run_v);  // dofree: one arrive per running network
     fence_mbar_init();
   }
   fence_proxy_async_smem();
@@ -503,18 +506,24 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   const uint32_t bar_dofree = bars + 112;
 
   if (warp >= T3_CHAIN_WARPS) {
-    // ============================ producer / weight-gradient warpgroup ============================
+    // ============ weight-gradient warpgroup of network c: warps 16..19 policy, 20..23 value ============
+    // Each issues its own network's products, stages 3..5 of every tile, on its own accumulator columns and H buffers;
+    // the two share only read-only operands (the X tile, the dOut buffer).  The warpgroup of c_last also produces the
+    // observation tiles.  A warpgroup whose network does not run in this launch has no tile work.
     // views at chain 0 / X buffer 0; the others are reached by adding byte offsets to the descriptors
     const Op2 X_M = op2_mnmajor(ub + S3_XB, T2_ACT, 64);         // B, N = 64: features h 0..31 (col 31 = ones) | l
     const Op2 X_M16 = op2_mnmajor(ub + S3_XB + 32, T2_ACT, 64);  // B, N = 16: h cols 16..31 (col 31 = ones)
     const Op2 DO_M = op2_mnmajor(ub + S3_XB, T2_ACT, 32);        // B, N = 32: dOut h | l
     const Op2 H1_M = op2_mnmajor(ub + S3_H, T2_ACT, T2_ACT), H2_M = op2_mnmajor(ub + S3_H + 2 * T2_ACT, T2_ACT, T2_ACT);
+    const int c = (warp - T3_CHAIN_WARPS) >> 2;
+    const bool runs = c == 0 ? run_p : run_v, producer = c == c_last, both = run_p && run_v;
+    const uint32_t co = c * S3_CHAIN, gcol = c * ACC_GRAD_NET;
     auto load_x = [&](int k) {  // tile k of this CTA -> X buffer k & 1
       const uint32_t b = (uint32_t)(k & 1);
       const long long tile = blockIdx.x + (long long)k * gridDim.x;
       uint32_t e;
       asm volatile("{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\tselp.u32 %0, 1, 0, q;\n\t}" : "=r"(e));
-      if (e && warp == T3_CHAIN_WARPS) {  // one thread of the warpgroup
+      if (e && (warp & 3) == 0) {  // one thread of the warpgroup
         mbar_arrive_expect_tx(bars + 8 * b, T2_ACT);
         bulk_copy_g2s(ub + S3_XB + b * T2_ACT, p.ximg + (size_t)tile * T2_ACT, T2_ACT, bars + 8 * b);
       }
@@ -523,68 +532,75 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     // first product of each stage: its accumulator columns within a network (its first group is 8 chunks: an n64 half,
     // or both halves of dW3)
     auto lead_col = [](int stage) { return stage == 3 ? ACC_DW3 : (stage == 4 ? ACC_DW2 : ACC_DW1); };
-    if (cta_tiles > 0) load_x(0);
+    if (producer && cta_tiles > 0) load_x(0);  // c_last always runs
 #pragma unroll 1
-    for (int k = 0; k < cta_tiles; ++k) {
+    for (int k = 0; runs && k < cta_tiles; ++k) {
       const uint32_t xo = (uint32_t)(k & 1) * T2_ACT, dob = (uint32_t)((k + 1) & 1) * T2_ACT;
       const bool first = k == 0;  // the first tile's products overwrite the accumulators
 #pragma unroll 1
       for (int stage = 3; stage <= 5; ++stage) {
-#pragma unroll 1
-        for (int c = c_first; c <= c_last; ++c) {
-          const uint32_t co = c * S3_CHAIN, gcol = c * ACC_GRAD_NET;
-          // the last half-product of this (stage, network) prefetches the first half-product after it: the next
-          // network's, the next stage's, or the next tile's first stage; none after the last tile, and none on the
-          // first (where every product overwrites)
-          const bool wrap = c == c_last && stage == 5;
-          const int ns = c < c_last ? stage : (stage < 5 ? stage + 1 : 3), nc = c < c_last ? c + 1 : c_first;
-          const bool nload = wrap ? k + 1 < cta_tiles : !first;
-          const uint32_t next = nc * ACC_GRAD_NET + lead_col(ns);
-          const int next_chunks = nload ? 8 : 0;
+        // the last half-product of this stage prefetches the first half-product after it: the next stage's, or the
+        // next tile's first stage; none after the last tile, and none on the first (where every product overwrites)
+        const bool nload = stage == 5 ? k + 1 < cta_tiles : !first;
+        const uint32_t next = gcol + lead_col(stage < 5 ? stage + 1 : 3);
+        const int next_chunks = nload ? 8 : 0;
 #ifdef B200RL_TC3_TIMING
-          const long long it0 = clock64();
+        const long long it0 = clock64();
 #endif
-          mbar_wait(bar_ready(c, stage), (uint32_t)(k & 1));  // both halves of network c have delivered the operands
-#ifdef B200RL_TC3_TIMING
-          const long long it1 = clock64();
-          tacc[40 + 3 * c + stage - 3] += (unsigned long long)(it1 - it0);
-#endif
-          if (stage == 3) {
-            // dW3^T[i][o] += sum_r H2[r][i] dOut[r][o]
-            grad_mma<32, 8, 1, 0, true>(acc, gcol + ACC_DW3, first, op2_at(H2_M, co), op2_at(DO_M, dob + c * 64),
-                                        next, next_chunks, TC3_TACC);
-          } else if (stage == 4) {
-            // every chain warpgroup's dH2 and both dW3 have read dOut: its buffer takes the next tile's observations
-            if (c == c_last && k + 1 < cta_tiles) load_x(k + 1);
-            // dW2[o][i] += sum_r dZ2[r][o] H1[r][i] ; db2[o] += sum_r dZ2[r][o] * 1 (ones column of X), in dW2's groups
-            grad_mma<64, 8, 2, 16>(acc, gcol + ACC_DW2, first, op2_at(H2_M, co), op2_at(H1_M, co), next, next_chunks,
-                                   TC3_TACC, gcol + ACC_DB2, op2_at(X_M16, xo));
-          } else {
-            // dW1[o][i] += sum_r dZ1[r][o] X[r][i]; column 31 (ones) collects db1
-            grad_mma<64, 8, 1>(acc, gcol + ACC_DW1, first, op2_at(H1_M, co), op2_at(X_M, xo), next, next_chunks,
-                               TC3_TACC);
-          }
-#ifdef B200RL_TC3_TIMING
-          const long long ih = clock64();
-#endif
-          asm volatile("bar.sync 5, 128;" ::: "memory");  // every warp's share of the products has retired
-          if ((tid & 127) == 0) {
-            mbar_arrive(bar_done(c, stage));
-            if (stage == 5 && c == c_last) mbar_arrive(bar_dofree);
-          }
-#ifdef B200RL_TC3_TIMING
-          const long long it2 = clock64();
-          tacc[46 + 3 * c + stage - 3] += (unsigned long long)(it2 - it1);
-          tacc[58] += (unsigned long long)(it2 - ih);
-#endif
+        mbar_wait(bar_ready(c, stage), (uint32_t)(k & 1));  // both halves of network c have delivered the operands
+        const bool load_next = stage == 4 && producer && k + 1 < cta_tiles;
+        if (load_next && both) {
+          // The next tile's observations go to this tile's dOut buffer: the policy network's dW3 and its chains' dH2
+          // must have read it too.  A parity wait is only right while the barrier is in tile k's phase or has just
+          // completed it.  Neither barrier can be a whole phase ahead: its tile k + 1 phase needs the policy chains
+          // past Z1 of tile k + 1, whose observations arrive only after the copy below.  Nor behind: this warpgroup's
+          // chains waited on dofree for tile k - 1, which the policy warpgroup arrives on after its tile k - 1 stages.
+          mbar_wait(bar_done(0, 3), (uint32_t)(k & 1));
+          mbar_wait(bar_ready(0, 4), (uint32_t)(k & 1));
         }
+#ifdef B200RL_TC3_TIMING
+        const long long it1 = clock64();
+        tacc[40 + 3 * c + stage - 3] += (unsigned long long)(it1 - it0);
+#endif
+        if (stage == 3) {
+          // dW3^T[i][o] += sum_r H2[r][i] dOut[r][o]
+          grad_mma<32, 8, 1, 0, true>(acc, gcol + ACC_DW3, first, op2_at(H2_M, co), op2_at(DO_M, dob + c * 64),
+                                      next, next_chunks, TC3_TSPLIT(c));
+        } else if (stage == 4) {
+          // every chain warpgroup's dH2 and every dW3 have read dOut: its buffer takes the next tile's observations
+          if (load_next) load_x(k + 1);
+          // dW2[o][i] += sum_r dZ2[r][o] H1[r][i] ; db2[o] += sum_r dZ2[r][o] * 1 (ones column of X), in dW2's groups
+          grad_mma<64, 8, 2, 16>(acc, gcol + ACC_DW2, first, op2_at(H2_M, co), op2_at(H1_M, co), next, next_chunks,
+                                 TC3_TSPLIT(c), gcol + ACC_DB2, op2_at(X_M16, xo));
+        } else {
+          // dW1[o][i] += sum_r dZ1[r][o] X[r][i]; column 31 (ones) collects db1
+          grad_mma<64, 8, 1>(acc, gcol + ACC_DW1, first, op2_at(H1_M, co), op2_at(X_M, xo), next, next_chunks,
+                             TC3_TSPLIT(c));
+        }
+#ifdef B200RL_TC3_TIMING
+        const long long ih = clock64();
+#endif
+        asm volatile("bar.sync %0, 128;" ::"r"(8 + c) : "memory");  // every warp's share of the products has retired
+        if ((tid & 127) == 0) {
+          mbar_arrive(bar_done(c, stage));
+          // db2 (stage 4) and dW1 (stage 5) were this network's readers of the tile's X buffer
+          if (stage == 5) mbar_arrive(bar_dofree);
+        }
+#ifdef B200RL_TC3_TIMING
+        const long long it2 = clock64();
+        tacc[46 + 3 * c + stage - 3] += (unsigned long long)(it2 - it1);
+        tacc[58 + 3 * c] += (unsigned long long)(it2 - ih);
+#endif
       }
     }
 #ifdef B200RL_TC3_TIMING
-    if (tid == T3_CHAIN_THREADS && blockIdx.x == 0) {
-      for (int i = 40; i < 52; ++i) g_tc3_t[i] = tacc[i];
-      for (int i = 56; i < 59; ++i) g_tc3_t[i] = tacc[i];
-      g_tc3_t[52] = (unsigned long long)cta_tiles;
+    if ((tid & 127) == 0 && blockIdx.x == 0) {
+      for (int s = 0; s < 3; ++s) {
+        g_tc3_t[40 + 3 * c + s] = tacc[40 + 3 * c + s];
+        g_tc3_t[46 + 3 * c + s] = tacc[46 + 3 * c + s];
+        g_tc3_t[56 + 3 * c + s] = tacc[56 + 3 * c + s];
+      }
+      if (producer) g_tc3_t[52] = (unsigned long long)cta_tiles;
     }
 #endif
     asm volatile("bar.sync 7, %0;" ::"n"(T3_THREADS) : "memory");  // the read-out may begin
@@ -851,7 +867,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
       for (int i = 0; i < 10; ++i) g_tc3_t[10 * wg + i] = tacc[10 * wg + i];
 #endif
 
-    asm volatile("bar.sync 7, %0;" ::"n"(T3_THREADS) : "memory");  // with the gradient warpgroup: every product has
+    asm volatile("bar.sync 7, %0;" ::"n"(T3_THREADS) : "memory");  // with the gradient warpgroups: every product has
                                                                    // retired and its accumulators are stored
     // ---- per-CTA results ----
     {

@@ -55,8 +55,12 @@ if __name__ == "__main__":
             name = f"{'pv'[wg >> 1]}{wg & 1}"
             print(f"chain {name} wait / tile:", dict(zip(("E1", "E2", "E3", "E4", "E5"), wait)), "sum", sum(wait))
             print(f"chain {name} work / tile:", dict(zip(("E1", "E2", "E3", "E4", "E5"), work)), "sum", sum(work))
-        keys = [f"{st}{'pv'[c]}" for c in range(2) for st in ("dW3", "dW2", "dW1")]
-        print("gradient wait  / tile:", {k: int(out[40 + i]) // tiles for i, k in enumerate(keys)}, "sum", sum(int(out[40 + i]) for i in range(6)) // tiles)
-        print("gradient issue / tile:", {k: int(out[46 + i]) // tiles for i, k in enumerate(keys)}, "sum", sum(int(out[46 + i]) for i in range(6)) // tiles)
+        keys = ("dW3", "dW2", "dW1")
         split = ("fragment loads", "fence .. wait_all", "stores + hand-over")
-        print("gradient issue split / tile:", {k: int(out[56 + i]) // tiles for i, k in enumerate(split)})
+        for c in range(2):  # one gradient warpgroup per network
+            wait = [int(out[40 + 3 * c + i]) // tiles for i in range(3)]
+            issue = [int(out[46 + 3 * c + i]) // tiles for i in range(3)]
+            name = "pv"[c]
+            print(f"gradient {name} wait  / tile:", dict(zip(keys, wait)), "sum", sum(wait))
+            print(f"gradient {name} issue / tile:", dict(zip(keys, issue)), "sum", sum(issue))
+            print(f"gradient {name} issue split / tile:", {k: int(out[56 + 3 * c + i]) // tiles for i, k in enumerate(split)})

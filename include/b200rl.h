@@ -343,6 +343,8 @@ typedef struct {
                             * b200rl_offpolicy_set_dqn), 3 = C51 (see b200rl_offpolicy_set_c51) */
   int32_t dueling_k;       /* 0 = the Q network is a plain MLP; K >= 1 = a dueling Q network (algo 2 / 3 only; see
                             * "Dueling Q networks" below) */
+  int32_t noisy_layers;    /* bit mask over the Q network's Linear layers in flat order: 0 = none; bit l = layer l is a
+                            * noisy layer (algo 2 / 3 only; see "Noisy networks" below) */
 } b200rl_offpolicy_config;
 
 typedef struct {
@@ -550,6 +552,43 @@ int b200rl_offpolicy_set_qr(b200rl_offpolicy* h, const b200rl_qr_hparams* hp);
  * Refused at create: dueling_k < 0; dueling_k != 0 with algo 0 or 1; a q description that is not 3 layers, whose
  * output width is not a multiple of dueling_k, or whose out_act is not identity.
  * ------------------------------------------------------------------------------------------------------------ */
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Noisy networks (Fortunato et al. 2018, factorized Gaussian noise) for DQN, QR-DQN and C51, plain or dueling: config
+ * noisy_layers = a bit mask over the Q network's Linear layers in flat order (an MLP's layers 0 .. n_layers - 1; a
+ * dueling network's trunk, value hidden, value out, advantage hidden, advantage out).  A noisy layer with `in` inputs
+ * and `out` outputs has W_mu, W_sigma [out, in] and b_mu, b_sigma [out]; for one draw of eps_in [in] and eps_out [out],
+ * each N(0, 1), in float32 with every product and sum rounded on its own (no contraction) and IEEE sqrt:
+ *   f(x) = copysign(sqrt(|x|), x),  e_ij = f(eps_out_i) f(eps_in_j)
+ *   W_ij = W_mu_ij + W_sigma_ij e_ij,  b_i = b_mu_i + b_sigma_i f(eps_out_i)
+ * The flat parameter vector of networks 1 and 4 (set_params, get_params, the state blob, Adam, the target copy) holds
+ * W_mu, W_sigma, b_mu, b_sigma for a noisy layer and W, b for a plain one, layer by layer: torch's parameters_to_vector
+ * of a module whose noisy layers register weight_mu, weight_sigma, bias_mu, bias_sigma in this order.
+ * Per train step and learner the online network draws one sample, which Q(s) and Double DQN's Q(s') share, and the
+ * target network an independent one; the loss head runs unchanged on the composed layers, the backward pass gives
+ * their dW and db, and dW_mu = dW, dW_sigma = dW e, db_mu = db, db_sigma = db f(eps_out) (e as the forward pass
+ * rounded it); Adam updates mu and sigma, and the target copy copies both.  q1_values logs Q(s)[a] under the step's
+ * online sample.
+ * Draws: the network's E = sum(in + out) over its noisy layers values are eps_in, eps_out of each noisy layer in layer
+ * order; values 4t .. 4t + 3 are the Box-Muller transform (as for train_gather_rng's noise) of Philox4x32-10(counter
+ * (t, st, call, 0xA00 | r), key seed), st = the step of the call, r = 0 for the online network and 1 for the target
+ * one.  (seed, call) come from b200rl_offpolicy_set_noise_keys, which every train call of such an engine needs afresh
+ * (train, train_gather, train_gather_rng, train_prioritized and their group forms; a call without them is refused);
+ * the keys live in device memory, so a cached graph is replayed across calls.
+ * Launches: one kernel draws and composes both networks at the start of a step, one maps dW, db to the noisy gradient
+ * before Adam: 2 per step more than the same network without noise (16 for a plain 3-layer DQN, QR-DQN or C51 step, 26
+ * for a dueling one; 19 and 32 with double_q; a prioritized step adds its 2).  Every sum has a fixed order and no
+ * float atomics are used: a group's learners stay bit-identical to solo engines.  Prioritized replay, n-step returns,
+ * Double DQN, dueling networks, groups, the graph and plain launches work as without noise; C51 with prioritized
+ * replay stays refused.
+ * Refused at create: noisy_layers != 0 with algo 0 or 1 (n_q is 1 for every engine that takes it); bits at or beyond
+ * the layer count.
+ * ------------------------------------------------------------------------------------------------------------ */
+/* seed[K], call[K]: the noise keys of the next train call, learner z's taken by its draws. */
+int b200rl_offpolicy_set_noise_keys(b200rl_offpolicy* h, const uint64_t* seed, const uint64_t* call);
+/* The raw N(0, 1) draws of the last train call's S steps: host eps [K, S, 2, E] (per step the online network's, then
+ * the target's) -- what a test replays through the oracle. */
+int b200rl_offpolicy_get_noisy_draws(b200rl_offpolicy* h, int32_t S, float* eps);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Learner groups: K independent off-policy learners (same config, same hyper-parameters, their own parameters, Adam

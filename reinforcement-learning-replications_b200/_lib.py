@@ -80,7 +80,8 @@ class TrpoStats(C.Structure):
 
 class OffPolicyConfig(C.Structure):
     _fields_ = [("policy", MlpDesc), ("q", MlpDesc), ("n_q", C.c_int32), ("max_minibatch", C.c_int32),
-                ("max_steps", C.c_int32), ("algo", C.c_int32), ("dueling_k", C.c_int32)]
+                ("max_steps", C.c_int32), ("algo", C.c_int32), ("dueling_k", C.c_int32),
+                ("noisy_layers", C.c_int32)]
 
 
 class SacHparams(C.Structure):
@@ -207,6 +208,8 @@ SIGNATURES = {
     "b200rl_offpolicy_get_per_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32] + [C.c_void_p] * 4),
     "b200rl_offpolicy_set_nstep": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
     "b200rl_offpolicy_get_nstep_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32] + [C.c_void_p] * 4),
+    "b200rl_offpolicy_set_noise_keys": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200rl_offpolicy_get_noisy_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
     "b200rl_per_tree_floats": (C.c_int64, [C.c_int64]),
     "b200rl_per_tree_build": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p]),
     "b200rl_per_tree_set_range": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p]),

@@ -14,6 +14,7 @@ import torch
 from torch import nn
 
 from ..engine import OLD_POLICY, POLICY, VALUE, OnPolicyEngine
+from ..networks import NoisyLinear, has_noisy_layers
 from ..packing import pack_experience
 from ..policies import CategoricalPolicy, GaussianPolicy
 
@@ -22,9 +23,10 @@ logger = logging.getLogger(__name__)
 _ACT_NAMES = {nn.Tanh: "tanh", nn.ReLU: "relu", nn.Identity: "identity"}
 
 
-def describe_mlp(module: nn.Module) -> Tuple[List[int], str, str, List[nn.Linear]]:
-    """(sizes, hidden activation, output activation, Linear layers) of an MLP built like ref networks/mlp.py:24-31.
-    Anything else is refused loudly -- the engine has no generic-module fallback."""
+def describe_mlp(module: nn.Module, allow_noisy: bool = False) -> Tuple[List[int], str, str, List[nn.Linear]]:
+    """(sizes, hidden activation, output activation, Linear layers) of an MLP built like ref networks/mlp.py:24-31
+    (``allow_noisy``: also with NoisyLinear layers, a NoisyMLP).  Anything else is refused loudly -- the engine has no
+    generic-module fallback."""
     seq = getattr(module, "network", module)
     mods = list(seq.children()) if isinstance(seq, nn.Sequential) else None
     if not mods:
@@ -32,6 +34,12 @@ def describe_mlp(module: nn.Module) -> Tuple[List[int], str, str, List[nn.Linear
     linears, acts = [], []
     for i, m in enumerate(mods):
         if i % 2 == 0:
+            if isinstance(m, NoisyLinear) and allow_noisy:
+                linears.append(m)
+                continue
+            if isinstance(m, NoisyLinear):
+                raise NotImplementedError(f"layer {i} is a NoisyLinear: noisy layers are implemented for DQN, C51 and "
+                                          "QR-DQN Q networks only")
             if not isinstance(m, nn.Linear) or m.bias is None:
                 raise NotImplementedError(f"layer {i} must be nn.Linear with bias, got {type(m).__name__}")
             linears.append(m)
@@ -51,9 +59,25 @@ def describe_mlp(module: nn.Module) -> Tuple[List[int], str, str, List[nn.Linear
     return sizes, hidden.pop(), acts[-1], linears
 
 
+def layer_params(layer) -> tuple:
+    """A layer's parameters in the engine's flat order: (weight, bias) of an nn.Linear, (weight_mu, weight_sigma,
+    bias_mu, bias_sigma) of a NoisyLinear."""
+    if isinstance(layer, NoisyLinear):
+        return layer.weight_mu, layer.weight_sigma, layer.bias_mu, layer.bias_sigma
+    return layer.weight, layer.bias
+
+
+def refuse_noisy(what: str, *modules) -> None:
+    """Refuse networks with noisy layers in the algorithms that do not implement them."""
+    for m in modules:
+        if m is not None and has_noisy_layers(m):
+            raise NotImplementedError(f"{what} does not take networks with noisy layers (NoisyLinear): they are "
+                                      "implemented for DQN, C51 and QR-DQN Q networks only")
+
+
 def flat_params(linears: List[nn.Linear]) -> np.ndarray:
     with torch.no_grad():
-        return torch.cat([t.detach().reshape(-1).float().cpu() for l in linears for t in (l.weight, l.bias)]).numpy()
+        return torch.cat([t.detach().reshape(-1).float().cpu() for l in linears for t in layer_params(l)]).numpy()
 
 
 def write_flat(linears: List[nn.Linear], flat: np.ndarray) -> None:
@@ -61,7 +85,7 @@ def write_flat(linears: List[nn.Linear], flat: np.ndarray) -> None:
     o = 0
     with torch.no_grad():
         for l in linears:
-            for t in (l.weight, l.bias):
+            for t in layer_params(l):
                 n = t.numel()
                 t.copy_(src[o:o + n].view_as(t))
                 o += n
@@ -76,7 +100,7 @@ def adam_hparams(optimizer, linears: List[nn.Linear], what: str, extra=()):
     if len(optimizer.param_groups) != 1:
         raise NotImplementedError(f"{what}: exactly one param group is supported")
     g = optimizer.param_groups[0]
-    want = [t for l in linears for t in (l.weight, l.bias)] + list(extra)
+    want = [t for l in linears for t in layer_params(l)] + list(extra)
     if len(g["params"]) != len(want) or any(a is not b for a, b in zip(g["params"], want)):
         raise NotImplementedError(
             f"{what}: optimizer must hold exactly the network's parameters in order "
@@ -87,7 +111,7 @@ def adam_hparams(optimizer, linears: List[nn.Linear], what: str, extra=()):
 
 
 def read_adam_state(optimizer, linears: List[nn.Linear], extra=()):
-    ps = [t for l in linears for t in (l.weight, l.bias)] + list(extra)
+    ps = [t for l in linears for t in layer_params(l)] + list(extra)
     if not all(p in optimizer.state and "exp_avg" in optimizer.state[p] for p in ps):
         return None, None, 0
     m = torch.cat([optimizer.state[p]["exp_avg"].reshape(-1).float() for p in ps]).numpy()
@@ -103,7 +127,7 @@ def write_adam_state(optimizer, linears: List[nn.Linear], m: np.ndarray, v: np.n
         return
     mt, vt = torch.from_numpy(m), torch.from_numpy(v)
     o = 0
-    for p in [t for l in linears for t in (l.weight, l.bias)] + list(extra):
+    for p in [t for l in linears for t in layer_params(l)] + list(extra):
         n = p.numel()
         st = optimizer.state[p]
         st["step"] = torch.tensor(float(step))  # torch keeps the step as a float32 scalar tensor

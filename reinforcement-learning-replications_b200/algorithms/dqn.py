@@ -9,8 +9,8 @@ import torch
 
 from .._lib import OffPolicyHparams
 from ..engine import OffPolicyEngine
-from ..networks import DuelingMLP
-from ..policies import EpsilonGreedyPolicy, GreedyPolicy
+from ..networks import DuelingMLP, NoisyLinear
+from ..policies import EpsilonGreedyPolicy, GreedyPolicy, NoisyGreedyPolicy
 from ..replay_buffer import PrioritizedReplayBuffer
 from ._onpolicy import _ACT_NAMES, adam_hparams, describe_mlp
 from .td3 import _learn, _make_eval_env, _OffPolicyBase
@@ -21,7 +21,7 @@ def describe_q_network(module):
     network: an ``MLP`` as ``describe_mlp`` reads it (K = 0), or a ``DuelingMLP`` with sizes [obs, h_trunk, h_stream,
     n_actions * K] and its five Linear layers (trunk, value hidden, value out, advantage hidden, advantage out)."""
     if not isinstance(module, DuelingMLP):
-        return describe_mlp(module) + (0,)
+        return describe_mlp(module, allow_noisy=True) + (0,)
     acts = {type(m) for m in (module.trunk[1], module.value[1], module.advantage[1])}
     if len(acts) != 1 or next(iter(acts)) not in _ACT_NAMES:
         raise NotImplementedError(f"DuelingMLP activations must be one of Tanh, ReLU, Identity throughout, got "
@@ -29,6 +29,11 @@ def describe_q_network(module):
     linears = [module.trunk[0], module.value[0], module.value[2], module.advantage[0], module.advantage[2]]
     sizes = module.sizes + [module.n_actions * module.outputs_per_action]
     return sizes, _ACT_NAMES[acts.pop()], "identity", linears, module.outputs_per_action
+
+
+def noisy_mask(linears) -> int:
+    """The engine's noisy_layers: bit l set for each NoisyLinear among the Q network's layers in flat order."""
+    return sum(1 << l for l, lin in enumerate(linears) if isinstance(lin, NoisyLinear))
 
 
 class DQN(_OffPolicyBase):
@@ -55,7 +60,14 @@ class DQN(_OffPolicyBase):
     ``outputs_per_action`` = 1 (C51: ``n_atoms``, QR-DQN: ``n_quantiles``); the engine runs either (b200rl.h).
 
     Acting: ``exploration_policy`` before ``num_start_steps``, then epsilon-greedy with epsilon falling linearly from
-    ``epsilon_start`` to ``epsilon_end`` over the first ``epsilon_decay_steps`` environment steps; evaluation is greedy."""
+    ``epsilon_start`` to ``epsilon_end`` over the first ``epsilon_decay_steps`` environment steps; evaluation is greedy.
+
+    Noisy networks (Fortunato et al. 2018): a Q network with ``networks.NoisyLinear`` layers (a ``NoisyMLP``, or a
+    ``DuelingMLP(..., noisy=True)``) explores through its weight noise instead: past ``num_start_steps`` acting is a
+    ``NoisyGreedyPolicy`` (fresh noise per action, then greedy; epsilon is not used), evaluation is greedy on the mean
+    weights.  Each train step draws the online and the target network's noise on the device (b200rl.h, "Noisy
+    networks"), keyed by ``device_rng_seed`` and the learner's own count of train calls, whatever ``use_device_rng``
+    says."""
     n_q = 1
     algo = OffPolicyEngine.DQN
     trainable_slots = (1,)  # the Q network is engine network 1, its optimizer row 1
@@ -96,6 +108,10 @@ class DQN(_OffPolicyBase):
         self.n_step = int(n_step)
         self.epsilon_greedy_policy = EpsilonGreedyPolicy(q_function, env.action_space, epsilon_start)
         self.policy = self.evaluation_policy = GreedyPolicy(q_function)  # acting greedily (evaluation)
+        self.noisy = noisy_mask(lins) != 0
+        if self.noisy:  # explores with its weight noise; evaluation on the mean weights
+            self.noisy_policy = NoisyGreedyPolicy(q_function)
+            self.policy = self.evaluation_policy = self.noisy_policy.deterministic()
         self.evaluation_env = _make_eval_env(env)
         self.target_q_function = copy.deepcopy(q_function)
         for p in self.target_q_function.network.parameters():
@@ -119,7 +135,10 @@ class DQN(_OffPolicyBase):
 
     @property
     def noised_policy(self):
-        """The acting policy after warm-up (the shared learn loop's name for it), at the current epsilon."""
+        """The acting policy after warm-up (the shared learn loop's name for it), at the current epsilon; a noisy Q
+        network's NoisyGreedyPolicy."""
+        if self.noisy:
+            return self.noisy_policy
         self.epsilon_greedy_policy.epsilon = self.epsilon()
         return self.epsilon_greedy_policy
 
@@ -130,13 +149,14 @@ class DQN(_OffPolicyBase):
         return [self.q_function], [self.target_q_function]
 
     def _ensure_engine(self, S: int, B: int) -> OffPolicyEngine:
-        qsz, qact, qout, _, dk = describe_q_network(self.q_function.network)
+        qsz, qact, qout, lins, dk = describe_q_network(self.q_function.network)
+        nm = noisy_mask(lins)
         e = getattr(self, "_engine", None)
         if (e is None or e.q_sizes != qsz or e.max_minibatch < B or e.max_steps < S or e.q_acts != (qact, qout)
-                or e.dueling_k != dk):
+                or e.dueling_k != dk or e.noisy_layers != nm):
             if e is not None:
                 e.close()
-            e = OffPolicyEngine(None, qsz, 1, B, S, q_acts=(qact, qout), algo=self.algo, dueling_k=dk)
+            e = OffPolicyEngine(None, qsz, 1, B, S, q_acts=(qact, qout), algo=self.algo, dueling_k=dk, noisy_layers=nm)
             self._engine = e
         return e
 
@@ -153,6 +173,9 @@ class DQN(_OffPolicyBase):
         e.set_dqn(self.target_update_interval, self.double_q)
 
     def _stage_inputs(self, replay_buffer, S: int, B: int, noisy: bool):
+        if self.noisy and S > 0:  # the weight noise's keys: this learner's own count of train calls
+            self._noise_calls = getattr(self, "_noise_calls", 0) + 1
+            self.noise_key = (getattr(self, "device_rng_seed", 0), self._noise_calls)
         if self.n_step > 1:  # the windows are assembled on the device from the replay ring
             if not getattr(self, "use_device_replay", True):
                 raise ValueError(f"n_step = {self.n_step} needs use_device_replay = True: n-step windows are assembled on "
@@ -179,6 +202,8 @@ class DQN(_OffPolicyBase):
         return mode, inputs
 
     def _call_engine(self, e, hp, replay_buffer, S: int, B: int, mode, inputs):
+        if mode is not None and self.noisy:
+            e.set_noise_keys(*([k] for k in self.noise_key))
         if mode is not None:
             e.set_nstep(self.n_step, [replay_buffer.device_episode_ends()] if self.n_step > 1 else None)
         if mode != "per":
@@ -211,7 +236,8 @@ class DQN(_OffPolicyBase):
         mm.record_scalar("q-function/avarage_q-value", float(np.mean(q)), steps, tensorboard=True)
         mm.record_scalar("q-function/max_q-value", float(np.max(q)))
         mm.record_scalar("q-function/min_q-value", float(np.min(q)))
-        mm.record_scalar("exploration/epsilon", self.epsilon(), steps, tensorboard=True)
+        if not self.noisy:
+            mm.record_scalar("exploration/epsilon", self.epsilon(), steps, tensorboard=True)
         if getattr(self, "_last_beta", None) is not None:
             mm.record_scalar("replay/beta", self._last_beta, steps, tensorboard=True)
 

@@ -27,7 +27,7 @@ from .._lib import MAX_LEARNERS
 from ..engine import OffPolicyEngine
 from ..replay_buffer import PrioritizedReplayBuffer
 from ._onpolicy import adam_hparams, describe_mlp
-from .dqn import describe_q_network
+from .dqn import describe_q_network, noisy_mask
 from .qrdqn import QRDQN
 from .td3 import _learn_begin, _learn_evaluate_save, _learn_sample, _OffPolicyBase
 
@@ -44,6 +44,7 @@ def _signature(agent) -> list:
             sizes, hidden_act, out_act, lins, k = describe_q_network(m.network)
             sig.append((f"{name} network kind", "DuelingMLP" if k else "MLP"))
             sig.append((f"{name} dueling (h_trunk, h_stream, outputs_per_action)", (sizes[1], sizes[2], k) if k else None))
+            sig.append((f"{name} noisy layers", noisy_mask(lins)))
         else:
             sizes, hidden_act, out_act, lins = describe_mlp(m.network)
         sig.append((f"{name} network", (tuple(sizes), hidden_act, out_act)))
@@ -154,17 +155,19 @@ class LearnerGroup:
         discrete = m.algo in (OffPolicyEngine.DQN, OffPolicyEngine.C51)
         if discrete:  # no policy network
             psz, pact, pout = None, "relu", "tanh"
-            qsz, qact, qout, _, dk = describe_q_network(m.q_function.network)
+            qsz, qact, qout, lins, dk = describe_q_network(m.q_function.network)
+            nm = noisy_mask(lins)
         else:
             psz, pact, pout, _ = describe_mlp(m.policy.network)
             qsz, qact, qout, _ = describe_mlp(m._nets()[0][1].network)
-            dk = 0
+            dk = nm = 0
         e = self._engine
         if (e is None or e.K != len(self.members) or e.max_minibatch < B or e.max_steps < S or e.policy_sizes != psz
-                or e.q_sizes != qsz or e.policy_acts != (pact, pout) or e.q_acts != (qact, qout) or e.dueling_k != dk):
+                or e.q_sizes != qsz or e.policy_acts != (pact, pout) or e.q_acts != (qact, qout) or e.dueling_k != dk
+                or e.noisy_layers != nm):
             self._close_engine()
             e = OffPolicyEngine(psz, qsz, m.n_q, B, S, (pact, pout), (qact, qout), algo=m.algo,
-                                n_learners=len(self.members), dueling_k=dk)
+                                n_learners=len(self.members), dueling_k=dk, noisy_layers=nm)
             self._engine = e
         return e
 
@@ -207,6 +210,8 @@ class LearnerGroup:
         if isinstance(members[0], QRDQN):
             e.set_qr(members[0].q_function.n_quantiles)
         hp = members[0]._hparams(noisy, delay)
+        if getattr(members[0], "noisy", False):
+            e.set_noise_keys(*zip(*[m.noise_key for m in members]))
         if members[0].algo in (OffPolicyEngine.DQN, OffPolicyEngine.C51):
             n = members[0].n_step
             e.set_nstep(n, [m.replay_buffer.device_episode_ends() for m in members] if n > 1 else None)

@@ -14,7 +14,7 @@ import torch
 
 from ..experience import Experience
 from ..metrics_manager import MetricsManager
-from ._onpolicy import OnPolicyTrainerMixin, adam_hparams
+from ._onpolicy import OnPolicyTrainerMixin, adam_hparams, refuse_noisy
 
 logger = logging.getLogger(__name__)
 
@@ -27,6 +27,7 @@ class PPO(OnPolicyTrainerMixin):
     def __init__(self, policy, value_function, env, sampler, gamma: float = 0.99, gae_lambda: float = 0.97,
                  clip_range: float = 0.2, max_kl_divergence: float = 0.01, num_policy_gradients: int = 80,
                  num_value_gradients: int = 80, distributed: bool = False, process_group=None) -> None:
+        refuse_noisy(type(self).__name__, policy, value_function)
         self.policy = policy
         self.value_function = value_function
         self.env = env

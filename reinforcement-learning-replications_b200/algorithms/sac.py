@@ -12,7 +12,7 @@ from torch import nn
 from .._lib import SacHparams
 from ..engine import OffPolicyEngine
 from ..policies import SquashedGaussianPolicy
-from ._onpolicy import adam_hparams, describe_mlp
+from ._onpolicy import adam_hparams, describe_mlp, refuse_noisy
 from .td3 import _learn, _make_eval_env, _OffPolicyBase
 
 
@@ -31,6 +31,7 @@ class SAC(_OffPolicyBase):
                  target_entropy=None, alpha_lr: float = 3e-4) -> None:
         if not isinstance(policy, SquashedGaussianPolicy):
             raise TypeError(f"SAC needs a SquashedGaussianPolicy, got {type(policy).__name__}")
+        refuse_noisy("SAC", policy, q_function_1, q_function_2)
         A = int(np.prod(env.action_space.shape))
         psz, _, _, plin = describe_mlp(policy.network)
         O = psz[0]

@@ -16,7 +16,7 @@ from ..engine import OffPolicyEngine
 from ..metrics_manager import MetricsManager
 from ..replay_buffer import PrioritizedReplayBuffer
 from ..utils import add_noise_to_get_action
-from ._onpolicy import adam_hparams, describe_mlp
+from ._onpolicy import adam_hparams, describe_mlp, layer_params, refuse_noisy
 
 logger = logging.getLogger(__name__)
 
@@ -93,7 +93,7 @@ class _OffPolicyBase:
             m, l = mods[i]
             o = off
             for lin in l:
-                for p_ in (lin.weight, lin.bias):
+                for p_ in layer_params(lin):
                     slots.append((kind, p_, m, blob_np[o:o + p_.numel()].reshape(tuple(p_.shape))))
                     o += p_.numel()
             assert o == off + count
@@ -102,7 +102,7 @@ class _OffPolicyBase:
 
     @staticmethod
     def _adam_step_count(optimizer, linears) -> int:
-        ps = [t for l in linears for t in (l.weight, l.bias)]
+        ps = [t for l in linears for t in layer_params(l)]
         if not all(p_ in optimizer.state and "exp_avg" in optimizer.state[p_] for p_ in ps):
             return 0
         steps = {int(float(optimizer.state[p_]["step"])) for p_ in ps}
@@ -279,6 +279,7 @@ class TD3(_OffPolicyBase):
     def __init__(self, policy, exploration_policy, q_function_1, q_function_2, env, sampler, replay_buffer, evaluator,
                  gamma: float = 0.99, polyak_rho: float = 0.995, action_noise_scale: float = 0.1,
                  target_noise_scale: float = 0.2, target_noise_clip: float = 0.5, policy_delay: int = 2) -> None:
+        refuse_noisy("TD3", policy, q_function_1, q_function_2)
         self.policy, self.exploration_policy = policy, exploration_policy
         self.q_function_1, self.q_function_2 = q_function_1, q_function_2
         self.env, self.sampler, self.replay_buffer, self.evaluator = env, sampler, replay_buffer, evaluator
@@ -331,6 +332,7 @@ class DDPG(_OffPolicyBase):
 
     def __init__(self, policy, exploration_policy, q_function, env, sampler, replay_buffer, evaluator,
                  gamma: float = 0.99, polyak_rho: float = 0.995, action_noise_scale: float = 0.1) -> None:
+        refuse_noisy("DDPG", policy, q_function)
         self.policy, self.exploration_policy, self.q_function = policy, exploration_policy, q_function
         self.env, self.sampler, self.replay_buffer, self.evaluator = env, sampler, replay_buffer, evaluator
         self.gamma, self.polyak_rho, self.action_noise_scale = gamma, polyak_rho, action_noise_scale

@@ -26,6 +26,9 @@
 // Dueling Q networks (config dueling_k, DQN / QR-DQN / C51): dueling_forward / dueling_backward take the place of
 // net_forward / net_backward for networks 1 and 4 -- the same GEMMs plus dueling_forward_kernel / dueling_backward_kernel
 // between the last layer and the loss head; nothing else in the step program differs.
+// Noisy networks (config noisy_layers, DQN / QR-DQN / C51, plain or dueling): noisy_compose_kernel draws both networks'
+// weight noise and composes their layers into the plain layout the GEMMs read at the start of each step, and
+// noisy_expand_kernel maps the composed layers' gradient to the noisy vector's before Adam.
 // Prioritized replay for DQN (train_prioritized): a 32-way sum tree per replay buffer, drawn from, weighed and gathered
 // by per_draw_kernel and updated by per_update_kernel inside the same step program.
 // n-step returns for DQN / C51 (set_nstep): nstep_gather_kernel (or per_draw_kernel's NSTEP instantiation) walks each
@@ -231,6 +234,17 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
   return c;
 }
 
+// Box-Muller of one Philox block: four N(0, 1) values (draw_minibatches_kernel's noise, noisy_draw's weight noise)
+__device__ __forceinline__ void box_muller4(uint4 r, float (&z)[4]) {
+  const float u1 = ((float)r.x + 1.0f) * 2.3283064365386963e-10f, u2 = (float)r.y * 2.3283064365386963e-10f;
+  const float u3 = ((float)r.z + 1.0f) * 2.3283064365386963e-10f, u4 = (float)r.w * 2.3283064365386963e-10f;
+  const float m1 = sqrtf(-2.f * logf(u1)), m2 = sqrtf(-2.f * logf(u3));
+  float s1, c1, s2, c2;
+  sincospif(2.f * u2, &s1, &c1);
+  sincospif(2.f * u4, &s2, &c2);
+  z[0] = m1 * c1, z[1] = m1 * s1, z[2] = m2 * c2, z[3] = m2 * s2;
+}
+
 // (seed, call, ring) of every learner of a launch: one entry for the solo kernel, one per learner for LANES
 template <bool LANES>
 struct DrawKeys {
@@ -266,13 +280,8 @@ __global__ void draw_minibatches_kernel(long long* idx, long long n_idx, float* 
   }
   if (eps != nullptr && 4 * t < n_eps) {
     const uint4 r = philox4x32_10(make_uint4((unsigned)t, (unsigned)(t >> 32), (unsigned)call, 0xE95u), key);
-    const float u1 = ((float)r.x + 1.0f) * 2.3283064365386963e-10f, u2 = (float)r.y * 2.3283064365386963e-10f;
-    const float u3 = ((float)r.z + 1.0f) * 2.3283064365386963e-10f, u4 = (float)r.w * 2.3283064365386963e-10f;
-    const float m1 = sqrtf(-2.f * logf(u1)), m2 = sqrtf(-2.f * logf(u3));
-    float s1, c1, s2, c2;
-    sincospif(2.f * u2, &s1, &c1);
-    sincospif(2.f * u4, &s2, &c2);
-    const float z[4] = {m1 * c1, m1 * s1, m2 * c2, m2 * s2};
+    float z[4];
+    box_muller4(r, z);
 #pragma unroll
     for (int j = 0; j < 4; ++j)
       if (4 * t + j < n_eps) eps[4 * t + j] = z[j];
@@ -752,6 +761,161 @@ __global__ void __launch_bounds__(GTHREADS) dueling_backward_kernel(const float*
   dv[i] = s;
   float* da = dv + k + i;
   for (int j = 0; j < n; ++j) da[(size_t)j * k] = g[(size_t)j * k] - mean;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Noisy networks (config noisy_layers; Fortunato et al. 2018, factorized Gaussian noise).  A noisy layer's
+// parameters are W_mu, W_sigma [out, in], b_mu, b_sigma [out] in the noisy vector; per draw eps_in [in], eps_out [out]
+// ~ N(0, 1), f(x) = copysign(sqrt(|x|), x), e_ij = f(eps_out_i) f(eps_in_j), and the composed layer the GEMMs read is
+// W = W_mu + W_sigma e, b = b_mu + b_sigma f(eps_out), every product and sum rounded on its own.  A plain layer of the
+// network is copied.  The work is cut into tiles of up to NOISY_TR rows x NOISY_TC columns of one layer's W (the tiles
+// of the first column also take the rows' biases): one CTA each, in layer order.
+constexpr int NOISY_MAX_LAYERS = 5;  // a dueling network's five Linear layers
+constexpr int NOISY_TR = 32, NOISY_TC = 256;
+
+struct NoisyLayout {
+  int n;          // Linear layers in flat order
+  unsigned mask;  // bit l: layer l is noisy
+  int in[NOISY_MAX_LAYERS], out[NOISY_MAX_LAYERS];
+  int cw[NOISY_MAX_LAYERS], cb[NOISY_MAX_LAYERS];  // W and b in the composed (plain-layout) vector
+  int fw[NOISY_MAX_LAYERS], fb[NOISY_MAX_LAYERS];  // W (W_mu, then W_sigma) and b (b_mu, then b_sigma) in the noisy vector
+  int eo[NOISY_MAX_LAYERS];                        // eps_in of a noisy layer in the draw vector; eps_out follows it
+  int E;                                           // draws per network: the sum of in + out over the noisy layers
+  int tiles[NOISY_MAX_LAYERS + 1];                 // first tile of each layer; tiles[n] = all tiles
+};
+
+__device__ __forceinline__ float noisy_f(float x) { return copysignf(sqrtf(fabsf(x)), x); }
+
+// draw k of network r (0 online, 1 target) at step st: element k % 4 of the Box-Muller block k / 4, Philox counter
+// (k / 4, st, call, 0xA00 | r) under key seed
+__device__ __forceinline__ float noisy_draw(int k, int st, int r, unsigned long long seed, unsigned long long call) {
+  const uint4 c = philox4x32_10(make_uint4((unsigned)(k >> 2), (unsigned)st, (unsigned)call, 0xA00u | (unsigned)r),
+                                make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
+  float z[4];
+  box_muller4(c, z);
+  const int j = k & 3;  // selected, not indexed: z stays in registers
+  return j == 0 ? z[0] : j == 1 ? z[1] : j == 2 ? z[2] : z[3];
+}
+
+// The tile of CTA `bid`: its layer l, first row r0 and column c0, rows nr and columns nc
+__device__ __forceinline__ int noisy_tile(const NoisyLayout& lay, int bid, int& r0, int& c0, int& nr, int& nc) {
+  int l = 0;
+  while (bid >= lay.tiles[l + 1]) ++l;
+  const int ct = (lay.in[l] + NOISY_TC - 1) / NOISY_TC, t = bid - lay.tiles[l];
+  r0 = (t / ct) * NOISY_TR, c0 = (t % ct) * NOISY_TC;
+  nr = min(NOISY_TR, lay.out[l] - r0), nc = min(NOISY_TC, lay.in[l] - c0);
+  return l;
+}
+
+// One launch per step for both networks (blockIdx.y = r: 0 composes the online network from flat_q into comp_q, 1 the
+// target from flat_t into comp_t), each from its own draw.  The tile's f(eps_in) and f(eps_out) are drawn into shared
+// memory; the CTAs past the tiles write the network's E raw draws, one Box-Muller block per thread, to draws[r * E ..]
+// (the step's slice of the call's [S, 2, E] record, which noisy_expand_kernel and b200rl_offpolicy_get_noisy_draws
+// read).  keys = the learner's (seed, call).
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) noisy_compose_kernel(const NoisyLayout lay, const float* flat_q,
+                                                                const float* flat_t, float* comp_q, float* comp_t,
+                                                                const unsigned long long* keys, int st, float* draws,
+                                                                size_t lane_stride) {
+  __shared__ float fi[NOISY_TC], fo[NOISY_TR];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    flat_q = lane_ptr(flat_q, o), flat_t = lane_ptr(flat_t, o), comp_q = lane_ptr(comp_q, o);
+    comp_t = lane_ptr(comp_t, o), keys = lane_ptr(keys, o), draws = lane_ptr(draws, o);
+  }
+  const int r = blockIdx.y;
+  const float* flat = r ? flat_t : flat_q;
+  float* comp = r ? comp_t : comp_q;
+  const unsigned long long seed = keys[0], call = keys[1];
+  if ((int)blockIdx.x >= lay.tiles[lay.n]) {
+    const int t = ((int)blockIdx.x - lay.tiles[lay.n]) * blockDim.x + threadIdx.x;
+    if (4 * t >= lay.E) return;
+    const uint4 c = philox4x32_10(make_uint4((unsigned)t, (unsigned)st, (unsigned)call, 0xA00u | (unsigned)r),
+                                  make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
+    float z[4];
+    box_muller4(c, z);
+    float* d = draws + ((size_t)st * 2 + r) * lay.E + 4 * t;
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (4 * t + j < lay.E) d[j] = z[j];
+    return;
+  }
+  int r0, c0, nr, nc;
+  const int l = noisy_tile(lay, blockIdx.x, r0, c0, nr, nc);
+  const int in = lay.in[l], out = lay.out[l];
+  const float* W = flat + lay.fw[l];
+  const float* b = flat + lay.fb[l];
+  float* cW = comp + lay.cw[l];
+  float* cb = comp + lay.cb[l];
+  if (!((lay.mask >> l) & 1u)) {  // a plain layer: copied
+    for (int i = threadIdx.x; i < nr * nc; i += blockDim.x) {
+      const size_t at = (size_t)(r0 + i / nc) * in + c0 + i % nc;
+      cW[at] = W[at];
+    }
+    if (c0 == 0)
+      for (int i = threadIdx.x; i < nr; i += blockDim.x) cb[r0 + i] = b[r0 + i];
+    return;
+  }
+  for (int j = threadIdx.x; j < nc; j += blockDim.x) fi[j] = noisy_f(noisy_draw(lay.eo[l] + c0 + j, st, r, seed, call));
+  for (int i = threadIdx.x; i < nr; i += blockDim.x)
+    fo[i] = noisy_f(noisy_draw(lay.eo[l] + in + r0 + i, st, r, seed, call));
+  __syncthreads();
+  const float* Ws = W + (size_t)out * in;
+  for (int i = threadIdx.x; i < nr * nc; i += blockDim.x) {
+    const int ri = i / nc, cj = i - ri * nc;
+    const size_t at = (size_t)(r0 + ri) * in + c0 + cj;
+    cW[at] = __fadd_rn(W[at], __fmul_rn(Ws[at], __fmul_rn(fo[ri], fi[cj])));
+  }
+  if (c0 == 0)
+    for (int i = threadIdx.x; i < nr; i += blockDim.x) cb[r0 + i] = __fadd_rn(b[r0 + i], __fmul_rn(b[out + r0 + i], fo[i]));
+}
+
+// After the backward pass: the composed layer's gradient (dW, db in grad, plain layout) -> the noisy vector's
+// (ngrad): dW_mu = dW, dW_sigma = dW e, db_mu = db, db_sigma = db f(eps_out), with e recomputed from the online
+// network's raw draws of step st as noisy_compose_kernel rounded it; a plain layer's gradient is copied.
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) noisy_expand_kernel(const NoisyLayout lay, const float* grad,
+                                                               const float* draws, int st, float* ngrad,
+                                                               size_t lane_stride) {
+  __shared__ float fi[NOISY_TC], fo[NOISY_TR];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    grad = lane_ptr(grad, o), draws = lane_ptr(draws, o), ngrad = lane_ptr(ngrad, o);
+  }
+  int r0, c0, nr, nc;
+  const int l = noisy_tile(lay, blockIdx.x, r0, c0, nr, nc);
+  const int in = lay.in[l], out = lay.out[l];
+  const float* dW = grad + lay.cw[l];
+  const float* db = grad + lay.cb[l];
+  float* gW = ngrad + lay.fw[l];
+  float* gb = ngrad + lay.fb[l];
+  if (!((lay.mask >> l) & 1u)) {
+    for (int i = threadIdx.x; i < nr * nc; i += blockDim.x) {
+      const size_t at = (size_t)(r0 + i / nc) * in + c0 + i % nc;
+      gW[at] = dW[at];
+    }
+    if (c0 == 0)
+      for (int i = threadIdx.x; i < nr; i += blockDim.x) gb[r0 + i] = db[r0 + i];
+    return;
+  }
+  const float* d = draws + (size_t)st * 2 * lay.E + lay.eo[l];
+  for (int j = threadIdx.x; j < nc; j += blockDim.x) fi[j] = noisy_f(d[c0 + j]);
+  for (int i = threadIdx.x; i < nr; i += blockDim.x) fo[i] = noisy_f(d[in + r0 + i]);
+  __syncthreads();
+  float* gWs = gW + (size_t)out * in;
+  for (int i = threadIdx.x; i < nr * nc; i += blockDim.x) {
+    const int ri = i / nc, cj = i - ri * nc;
+    const size_t at = (size_t)(r0 + ri) * in + c0 + cj;
+    const float g = dW[at];
+    gW[at] = g;
+    gWs[at] = __fmul_rn(g, __fmul_rn(fo[ri], fi[cj]));
+  }
+  if (c0 == 0)
+    for (int i = threadIdx.x; i < nr; i += blockDim.x) {
+      const float g = db[r0 + i];
+      gb[r0 + i] = g;
+      gb[out + r0 + i] = __fmul_rn(g, fo[i]);
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1293,6 +1457,11 @@ struct NetBuf {
   // order trunk, value hidden, value out, advantage hidden, advantage out
   int duel_k = 0;
   int dw_off[5] = {}, db_off[5] = {};
+  // the vector set_params / get_params, the state blob, Adam and the target copy work on, P_flat floats: params /
+  // grad themselves, except for networks 1 and 4 of an engine with noisy layers, where params / grad hold the composed
+  // network the GEMMs read and flat / flat_grad the noisy vector (noisy_compose_kernel, noisy_expand_kernel)
+  float *flat = nullptr, *flat_grad = nullptr;
+  int64_t P_flat = 0;
 };
 
 // What a captured step program holds in its nodes besides the engine's own buffers: a graph is replayed only for a call
@@ -1389,6 +1558,11 @@ struct b200rl_offpolicy {
   bool nstep_last = false;            // the last call that ran steps was an n-step one
   float* nstep_disc = nullptr;        // [max_steps * B] gamma^k of each row's window
   long long* nstep_rows = nullptr;    // [max_steps * B] the last row of each row's window
+  // noisy layers (config noisy_layers != 0; DQN engines): adam_tab's last two float2 hold the (seed, call) words of
+  // set_noise_keys, which every train call needs afresh
+  bool noisy = false, noisy_keys = false;
+  NoisyLayout noisy_lay{};
+  float* noisy_draws = nullptr;  // [max_steps][2][E] raw draws of the call's steps (online, target)
   // the replay columns, episode-end columns, trees and row counts of this call (train_gather[_rng], train_prioritized)
   ReplayLanes<true> replay{};
   std::vector<void*> allocs;
@@ -1397,6 +1571,12 @@ struct b200rl_offpolicy {
 namespace {
 
 inline int64_t state_pad(int64_t n) { return (n + 63) & ~(int64_t)63; }
+
+// float2 entries of one learner's adam_tab: the Adam scalar rows (+ SAC's temperature row or DQN's copy flags), then
+// DQN's prioritized (seed, call) at 4 max_steps and a noisy engine's noise (seed, call) after it
+inline size_t adam_tab_len(const b200rl_offpolicy* h) {
+  return (h->sac || h->dqn ? 4 : 3) * (size_t)h->cfg.max_steps + (h->dqn ? 2 : 0) + (h->noisy ? 2 : 0);
+}
 
 // A piece of the learner arena: recorded here (256-byte aligned), placed by arena_commit
 template <typename T>
@@ -1631,7 +1811,8 @@ int dueling_backward(b200rl_offpolicy* h, const NetBuf& nb, float* const* acts, 
 
 int adam_net(const b200rl_offpolicy* h, NetBuf& nb, const float2* table, int idx, double b1, double b2, double eps,
              cudaStream_t s) {
-  return adam_step_table(nb.params, nb.grad, nb.m, nb.v, nb.P, table, idx, b1, b2, eps, s, h->K, h->lane_stride);
+  return adam_step_table(nb.flat, nb.flat_grad, nb.m, nb.v, nb.P_flat, table, idx, b1, b2, eps, s, h->K,
+                         h->lane_stride);
 }
 
 }  // namespace
@@ -1676,6 +1857,12 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
     Pq = (int64_t)d.sizes[1] * (d.sizes[0] + 1) + 2 * (int64_t)d.sizes[2] * (d.sizes[1] + 1) +
          (int64_t)(DK + d.sizes[3]) * (d.sizes[2] + 1);
   }
+  const unsigned NM = (unsigned)cfg->noisy_layers;
+  const int n_lin = DK != 0 ? 5 : cfg->q.n_layers;  // the Q network's Linear layers in flat order
+  B200RL_REQUIRE(NM == 0 || dqn, "offpolicy_create: noisy_layers must be 0 unless algo = 2 (DQN / QR-DQN) or 3 (C51), "
+                 "got 0x%x", NM);
+  B200RL_REQUIRE((NM >> n_lin) == 0, "offpolicy_create: noisy_layers 0x%x has bits beyond the Q network's %d Linear "
+                 "layers", NM, n_lin);
   const int O = dqn ? cfg->q.sizes[0] : cfg->policy.sizes[0], P_out = cfg->policy.sizes[cfg->policy.n_layers];
   // SAC: the policy outputs [mean | log_std], 2A wide; DQN: the action column holds the index (1 wide)
   const int A = dqn ? 1 : sac ? cfg->q.sizes[0] - O : P_out;
@@ -1692,6 +1879,7 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
   h->sac = sac;
   h->dqn = dqn;
   h->c51 = c51;
+  h->noisy = NM != 0;
   int rc = 0;
   int maxw = O + A;
   for (int i = 0; i < 6; ++i) {
@@ -1719,20 +1907,44 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
       }
       maxw = std::max(maxw, std::max(2 * h2, DK + nK));
     }
+    nb.P_flat = nb.P;
+    if (NM != 0 && (i == 1 || i == 4)) {  // the noisy vector: [W_mu, W_sigma, b_mu, b_sigma] per noisy layer, [W, b] else
+      NoisyLayout& lay = h->noisy_lay;
+      const b200rl_mlp_desc& d = nb.d;
+      const int ins[5] = {d.sizes[0], d.sizes[1], d.sizes[2], d.sizes[1], d.sizes[2]};
+      const int outs[5] = {d.sizes[1], d.sizes[2], DK, d.sizes[2], d.sizes[3]};
+      lay = NoisyLayout{};
+      lay.n = n_lin, lay.mask = NM;
+      int fo = 0;
+      for (int l = 0; l < n_lin; ++l) {
+        const int in = DK ? ins[l] : d.sizes[l], out = DK ? outs[l] : d.sizes[l + 1], w = (NM >> l) & 1u ? 2 : 1;
+        lay.in[l] = in, lay.out[l] = out;
+        lay.cw[l] = DK ? nb.dw_off[l] : nb.w_off[l], lay.cb[l] = DK ? nb.db_off[l] : nb.b_off[l];
+        lay.fw[l] = fo, fo += w * out * in;
+        lay.fb[l] = fo, fo += w * out;
+        if (w == 2) lay.eo[l] = lay.E, lay.E += in + out;
+        lay.tiles[l + 1] = lay.tiles[l] + ((out + NOISY_TR - 1) / NOISY_TR) * ((in + NOISY_TC - 1) / NOISY_TC);
+      }
+      nb.P_flat = fo;
+    }
     if (cfg->n_q == 1 && (i == 2 || i == 5)) continue;
     if (sac && i == 3) continue;  // SAC has no target policy
     if (dqn && (i == 0 || i == 3)) continue;  // DQN has no policy
     nb.present = true;
     if (i < 3) rc |= oalloc(h, &nb.grad, (size_t)nb.P);
+    if (nb.P_flat != nb.P) {  // the composed network beside the noisy vector in the slab (and its gradient)
+      rc |= oalloc(h, &nb.params, (size_t)nb.P);
+      if (i < 3) rc |= oalloc(h, &nb.flat_grad, (size_t)nb.P_flat);
+    }
   }
   // parameters and Adam state live in ONE slab in the order of the state blob (b200rl_offpolicy_get_state): the
   // parameters of networks 0..5, then exp_avg / exp_avg_sq of optimizers 0..2, every segment padded to 64 floats
   {
     int64_t n = 0;
     for (int i = 0; i < 6; ++i)
-      if (h->net[i].present) n += state_pad(h->net[i].P);
+      if (h->net[i].present) n += state_pad(h->net[i].P_flat);
     for (int i = 0; i < 3; ++i)
-      if (h->net[i].present) n += 2 * state_pad(h->net[i].P);
+      if (h->net[i].present) n += 2 * state_pad(h->net[i].P_flat);
     h->state_n = n;
     rc |= oalloc(h, &h->state, (size_t)n);
   }
@@ -1762,9 +1974,9 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
   rc |= oalloc(h, &h->out_l1, S);
   rc |= oalloc(h, &h->out_l2, S);
   rc |= oalloc(h, &h->out_lp, S);
-  const size_t n_tab = sac || dqn ? 4 : 3;  // SAC: a fourth row for log_alpha's optimizer; DQN: the copy flags
-  rc |= oalloc(h, &h->adam_tab, n_tab * S + (dqn ? 2 : 0));  // DQN: + the prioritized draw's (seed, call)
+  rc |= oalloc(h, &h->adam_tab, adam_tab_len(h));
   rc |= oalloc(h, &h->idx, S * B);
+  if (h->noisy) rc |= oalloc(h, &h->noisy_draws, S * 2 * (size_t)h->noisy_lay.E);
   if (sac) {
     rc |= oalloc(h, &h->sac_act_next, B * (size_t)A);
     rc |= oalloc(h, &h->sac_logp_next, B);
@@ -1791,20 +2003,22 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
   rc |= arena_commit(h);
   if (rc == 0) {
     float* q = h->state;
-    for (int i = 0; i < 6; ++i)
-      if (h->net[i].present) {
-        h->net[i].params = q;
-        q += state_pad(h->net[i].P);
-      }
+    for (int i = 0; i < 6; ++i) {
+      NetBuf& nb = h->net[i];
+      if (!nb.present) continue;
+      nb.flat = q;
+      if (nb.P_flat == nb.P) nb.params = q, nb.flat_grad = nb.grad;
+      q += state_pad(nb.P_flat);
+    }
     for (int i = 0; i < 3; ++i)
       if (h->net[i].present) {
         h->net[i].m = q;
-        q += state_pad(h->net[i].P);
+        q += state_pad(h->net[i].P_flat);
         h->net[i].v = q;
-        q += state_pad(h->net[i].P);
+        q += state_pad(h->net[i].P_flat);
       }
   }
-  if (!rc && cudaMallocHost(reinterpret_cast<void**>(&h->h_adam_tab), h->K * (n_tab * S + (dqn ? 2 : 0)) * sizeof(float2)) != cudaSuccess)
+  if (!rc && cudaMallocHost(reinterpret_cast<void**>(&h->h_adam_tab), h->K * adam_tab_len(h) * sizeof(float2)) != cudaSuccess)
     rc = 1;
   if (!rc && cudaStreamCreateWithFlags(&h->gs, cudaStreamNonBlocking) != cudaSuccess) rc = 1;
   if (!rc && cudaEventCreateWithFlags(&h->ev, cudaEventDisableTiming) != cudaSuccess) rc = 1;
@@ -1841,19 +2055,19 @@ extern "C" void b200rl_offpolicy_destroy(b200rl_offpolicy* h) {
 extern "C" int b200rl_offpolicy_set_params(b200rl_offpolicy* h, int which, const float* host_flat, int64_t n,
                                            void* stream) {
   B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_set_params: a learner group moves its state with get_state / set_state");
-  B200RL_REQUIRE(h && host_flat && which >= 0 && which < 6 && h->net[which].params, "offpolicy_set_params: bad net");
-  B200RL_REQUIRE(n == h->net[which].P, "offpolicy_set_params: expects %lld floats", (long long)h->net[which].P);
-  B200RL_CUDA(cudaMemcpyAsync(h->net[which].params, host_flat, (size_t)n * 4, cudaMemcpyHostToDevice,
+  B200RL_REQUIRE(h && host_flat && which >= 0 && which < 6 && h->net[which].flat, "offpolicy_set_params: bad net");
+  B200RL_REQUIRE(n == h->net[which].P_flat, "offpolicy_set_params: expects %lld floats", (long long)h->net[which].P_flat);
+  B200RL_CUDA(cudaMemcpyAsync(h->net[which].flat, host_flat, (size_t)n * 4, cudaMemcpyHostToDevice,
                               static_cast<cudaStream_t>(stream)));
   return 0;
 }
 
 extern "C" int b200rl_offpolicy_get_params(b200rl_offpolicy* h, int which, float* host_flat, int64_t n, void* stream) {
   B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_get_params: a learner group moves its state with get_state / set_state");
-  B200RL_REQUIRE(h && host_flat && which >= 0 && which < 6 && h->net[which].params, "offpolicy_get_params: bad net");
-  B200RL_REQUIRE(n == h->net[which].P, "offpolicy_get_params: expects %lld floats", (long long)h->net[which].P);
+  B200RL_REQUIRE(h && host_flat && which >= 0 && which < 6 && h->net[which].flat, "offpolicy_get_params: bad net");
+  B200RL_REQUIRE(n == h->net[which].P_flat, "offpolicy_get_params: expects %lld floats", (long long)h->net[which].P_flat);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  B200RL_CUDA(cudaMemcpyAsync(host_flat, h->net[which].params, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+  B200RL_CUDA(cudaMemcpyAsync(host_flat, h->net[which].flat, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaStreamSynchronize(s));
   return 0;
 }
@@ -1863,7 +2077,7 @@ extern "C" int b200rl_offpolicy_set_adam(b200rl_offpolicy* h, int which, const f
   B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_set_adam: a learner group moves its state with get_state / set_state");
   B200RL_REQUIRE(h && which >= 0 && which < 3 && h->net[which].m, "offpolicy_set_adam: bad net");
   NetBuf& nb = h->net[which];
-  B200RL_REQUIRE(n == nb.P && step >= 0, "offpolicy_set_adam: expects %lld floats", (long long)nb.P);
+  B200RL_REQUIRE(n == nb.P_flat && step >= 0, "offpolicy_set_adam: expects %lld floats", (long long)nb.P_flat);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (exp_avg) B200RL_CUDA(cudaMemcpyAsync(nb.m, exp_avg, (size_t)n * 4, cudaMemcpyHostToDevice, s));
   else B200RL_CUDA(cudaMemsetAsync(nb.m, 0, (size_t)n * 4, s));
@@ -1879,7 +2093,7 @@ extern "C" int b200rl_offpolicy_get_adam(b200rl_offpolicy* h, int which, float* 
   B200RL_REQUIRE(h && which >= 0 && which < 3 && h->net[which].m && exp_avg && exp_avg_sq && step,
                  "offpolicy_get_adam: bad arguments");
   NetBuf& nb = h->net[which];
-  B200RL_REQUIRE(n == nb.P, "offpolicy_get_adam: expects %lld floats", (long long)nb.P);
+  B200RL_REQUIRE(n == nb.P_flat, "offpolicy_get_adam: expects %lld floats", (long long)nb.P_flat);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200RL_CUDA(cudaMemcpyAsync(exp_avg, nb.m, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaMemcpyAsync(exp_avg_sq, nb.v, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
@@ -2018,6 +2232,27 @@ extern "C" int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, c
   }
   h->nstep = n_step;
   h->nstep_ends = ends;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_set_noise_keys(b200rl_offpolicy* h, const uint64_t* seed, const uint64_t* call) {
+  B200RL_REQUIRE(h && seed && call, "offpolicy_set_noise_keys: NULL argument");
+  B200RL_REQUIRE(h->noisy, "offpolicy_set_noise_keys: the engine has no noisy layers (config noisy_layers = 0)");
+  const size_t n = adam_tab_len(h);
+  for (int z = 0; z < h->K; ++z) {  // uploaded with the table by run_staged
+    unsigned long long* keys = reinterpret_cast<unsigned long long*>(h->h_adam_tab + z * n + n - 2);
+    keys[0] = seed[z], keys[1] = call[z];
+  }
+  h->noisy_keys = true;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_get_noisy_draws(b200rl_offpolicy* h, int32_t S, float* eps) {
+  B200RL_REQUIRE(h && eps && S >= 0 && S <= h->cfg.max_steps, "offpolicy_get_noisy_draws: bad arguments");
+  B200RL_REQUIRE(h->noisy, "offpolicy_get_noisy_draws: the engine has no noisy layers (config noisy_layers = 0)");
+  const size_t w = (size_t)S * 2 * h->noisy_lay.E * 4;
+  if (w) B200RL_CUDA(cudaMemcpy2DAsync(eps, w, h->noisy_draws, h->lane_stride, w, h->K, cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
   return 0;
 }
 
@@ -2349,7 +2584,15 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
   const float2* betas = h->adam_tab + (size_t)3 * maxS;
   const unsigned long long* keys = reinterpret_cast<const unsigned long long*>(h->adam_tab + (size_t)4 * maxS);
   const float alpha = (float)h->per_hp.alpha, eps = (float)h->per_hp.eps;
+  const NoisyLayout& lay = h->noisy_lay;
+  const unsigned long long* noise_keys = keys + 2;
+  const unsigned compose_ctas = (unsigned)(lay.tiles[lay.n] + ((lay.E + 3) / 4 + GTHREADS - 1) / GTHREADS);  // + draws
   for (int st = 0; st < S; ++st) {
+    // noisy layers: both networks' weights drawn and composed behind the previous step's Adam and target copy, ahead
+    // of every forward pass of this one
+    if (h->noisy && launch(h, noisy_compose_kernel<false>, noisy_compose_kernel<true>, dim3(compose_ctas, 2), GTHREADS,
+                           0, s, lay, q.flat, qt.flat, q.params, qt.params, noise_keys, st, h->noisy_draws))
+      return 1;
     float* s_obs = h->obs + (size_t)st * B * O;
     float* s_act = h->act + (size_t)st * B;
     float* s_rew = h->rew + (size_t)st * B;
@@ -2416,9 +2659,12 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
     if (q.duel_k ? dueling_backward(h, q, qa, h->dqn_dout, B, s, s3)
                  : net_backward(h, q, qa, h->dqn_dout, n, B, true, nullptr, s, false, nullptr, 0, 0, s3))
       return 1;
+    if (h->noisy && launch(h, noisy_expand_kernel<false>, noisy_expand_kernel<true>, (unsigned)lay.tiles[lay.n],
+                           GTHREADS, 0, s, lay, q.grad, h->noisy_draws, st, q.flat_grad))
+      return 1;
     if (adam_net(h, q, h->adam_tab + (size_t)maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, s)) return 1;
-    if (launch(h, dqn_target_copy_kernel<false>, dqn_target_copy_kernel<true>, (unsigned)((q.P + ew - 1) / ew), ew, 0,
-               s, qt.params, q.params, (int)q.P, h->adam_tab + (size_t)3 * maxS, st))
+    if (launch(h, dqn_target_copy_kernel<false>, dqn_target_copy_kernel<true>, (unsigned)((q.P_flat + ew - 1) / ew), ew,
+               0, s, qt.flat, q.flat, (int)q.P_flat, h->adam_tab + (size_t)3 * maxS, st))
       return 1;
   }
   if (per && edge(h, s4, s)) return 1;
@@ -2450,7 +2696,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   // (a group: one table per learner, from that learner's step counts, uploaded with one strided copy)
   const int maxS = h->cfg.max_steps;
   const int n_pol_expected = h->dqn ? 0 : h->sac ? S : (S + hp->policy_delay - 1) / hp->policy_delay;  // SAC: no delay
-  const size_t tab_n = (h->sac || h->dqn ? 4 : 3) * (size_t)maxS + (h->dqn ? 2 : 0);
+  const size_t tab_n = adam_tab_len(h);
   const bool learn_alpha = h->sac && h->sac_hp.learn_alpha;
   for (int z = 0; z < h->K; ++z) {
     float2* tab = h->h_adam_tab + z * tab_n;
@@ -2577,7 +2823,10 @@ static int train_begin(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, 
     B200RL_REQUIRE(h->dqn_set, "%s: a DQN engine needs b200rl_offpolicy_set_dqn before it trains", what);
     B200RL_REQUIRE(!h->c51 || h->c51_set, "%s: a C51 engine needs b200rl_offpolicy_set_c51 before it trains", what);
   }
+  B200RL_REQUIRE(!h->noisy || h->noisy_keys, "%s: an engine with noisy layers needs fresh keys from "
+                 "b200rl_offpolicy_set_noise_keys before every train call", what);
   if (int rc = own()) return rc;
+  h->noisy_keys = false;  // this call consumes them
   *n_policy_updates = 0;
   if (S == 0) return -1;
   B200RL_CUDA(cudaEventRecord(h->ev, static_cast<cudaStream_t>(stream)));
@@ -2808,9 +3057,10 @@ extern "C" int b200rl_offpolicy_train_prioritized_group(b200rl_offpolicy* h, con
   if (int rc = train_begin(h, hp, S, B, true, false, &n_pol, stream, "offpolicy_train_prioritized", own))
     return rc < 0 ? 0 : rc;
   set_replay(h, rb, trees);
-  const size_t tab_n = (size_t)4 * h->cfg.max_steps + 2;
+  const size_t tab_n = adam_tab_len(h);
   for (int z = 0; z < h->K; ++z) {
-    unsigned long long* keys = reinterpret_cast<unsigned long long*>(h->h_adam_tab + z * tab_n + tab_n - 2);
+    unsigned long long* keys =
+        reinterpret_cast<unsigned long long*>(h->h_adam_tab + z * tab_n + (size_t)4 * h->cfg.max_steps);
     keys[0] = seed[z], keys[1] = call[z];  // uploaded with the table by run_staged
   }
   h->per_run = true;

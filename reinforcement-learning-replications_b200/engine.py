@@ -327,7 +327,8 @@ class OffPolicyEngine:
     network maps obs -> [n actions x n atoms] logits; it needs ``set_c51`` as well as ``set_dqn``.  QR-DQN is a DQN
     engine after ``set_qr``: its Q network maps obs -> [n actions x n quantiles] quantile locations.  ``dueling_k`` = K
     >= 1 (DQN / QR-DQN / C51): the Q network is a dueling one, ``q_sizes`` = [obs, h_trunk, h_stream, n actions x K]
-    (b200rl.h, "Dueling Q networks").
+    (b200rl.h, "Dueling Q networks").  ``noisy_layers`` (DQN / QR-DQN / C51): bit mask of the Q network's noisy Linear
+    layers in flat order; every train call then needs ``set_noise_keys`` first (b200rl.h, "Noisy networks").
 
     ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
     launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
@@ -337,7 +338,8 @@ class OffPolicyEngine:
     TD3, SAC, DQN, C51 = 0, 1, 2, 3
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
-                 q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1, dueling_k: int = 0):
+                 q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1, dueling_k: int = 0,
+                 noisy_layers: int = 0):
         from ._lib import OffPolicyConfig
         self.lib = _lib.load()
         current_stream_handle()
@@ -346,8 +348,8 @@ class OffPolicyEngine:
             cfg.policy = MlpDesc.make(policy_sizes, *policy_acts)
         cfg.q = MlpDesc.make(q_sizes, *q_acts)
         cfg.n_q, cfg.max_minibatch, cfg.max_steps = int(n_q), int(max_minibatch), int(max_steps)
-        cfg.algo, cfg.dueling_k = int(algo), int(dueling_k)
-        self.algo, self.dueling_k = int(algo), int(dueling_k)
+        cfg.algo, cfg.dueling_k, cfg.noisy_layers = int(algo), int(dueling_k), int(noisy_layers)
+        self.algo, self.dueling_k, self.noisy_layers = int(algo), int(dueling_k), int(noisy_layers)
         self.discrete = self.algo in (self.DQN, self.C51)  # DQN's networks, inputs and outputs
         self.n_q, self.max_minibatch, self.max_steps = int(n_q), int(max_minibatch), int(max_steps)
         self.policy_sizes, self.q_sizes = None if policy_sizes is None else list(policy_sizes), list(q_sizes)
@@ -357,10 +359,21 @@ class OffPolicyEngine:
         if self.dueling_k and len(self.q_sizes) == 4:  # trunk, both streams' hidden layers, V and A (b200rl.h)
             O, h1, h2, w = self.q_sizes
             self.n_qp = h1 * (O + 1) + 2 * h2 * (h1 + 1) + (self.dueling_k + w) * (h2 + 1)
+        noisy = [(i, o) for l, (i, o) in enumerate(self.q_layers()) if self.noisy_layers >> l & 1]
+        self.n_qp += sum(o * (i + 1) for i, o in noisy)  # W_sigma and b_sigma of each noisy layer
+        self.noise_width = sum(i + o for i, o in noisy)  # E: draws per network and step
         self.K = int(n_learners)
         h = C.c_void_p()
         check(self.lib.b200rl_offpolicy_create_group(C.byref(cfg), self.K, C.byref(h)), "offpolicy_create")
         self.h = h
+
+    def q_layers(self):
+        """(in, out) of the Q network's Linear layers in flat order (a dueling network: trunk, value hidden, value out,
+        advantage hidden, advantage out)."""
+        if self.dueling_k and len(self.q_sizes) == 4:
+            O, h1, h2, w = self.q_sizes
+            return [(O, h1), (h1, h2), (h2, self.dueling_k), (h1, h2), (h2, w)]
+        return list(zip(self.q_sizes[:-1], self.q_sizes[1:]))
 
     def close(self):
         if getattr(self, "h", None):
@@ -498,6 +511,22 @@ class OffPolicyEngine:
         dp = DqnHparams()
         dp.target_update_interval, dp.double_q = int(target_update_interval), int(bool(double_q))
         check(self.lib.b200rl_offpolicy_set_dqn(self.h, C.byref(dp)), "set_dqn")
+
+    # ---- noisy networks (DQN / C51) ----
+    def set_noise_keys(self, seeds, calls) -> None:
+        """The (seed, call) keys of the next train call's weight noise, one of each per learner (b200rl.h, "Noisy
+        networks"); an engine with noisy layers refuses a train call without fresh keys."""
+        keys = [np.asarray([int(x) & (2 ** 64 - 1) for x in v], np.uint64) for v in (seeds, calls)]
+        if any(k.size != self.K for k in keys):
+            raise ValueError(f"set_noise_keys: expected the keys of {self.K} learners")
+        check(self.lib.b200rl_offpolicy_set_noise_keys(self.h, *[_ptr(k) for k in keys]), "set_noise_keys")
+
+    def get_noisy_draws(self, S: int):
+        """Raw N(0, 1) draws [S, 2, E] (per step the online network's, then the target's; E = sum(in + out) over the
+        noisy layers, eps_in then eps_out of each in layer order) of the last train call; a group: [K, S, 2, E]."""
+        eps = np.empty((self.K, S, 2, self.noise_width), np.float32)
+        check(self.lib.b200rl_offpolicy_get_noisy_draws(self.h, int(S), _ptr(eps)), "get_noisy_draws")
+        return eps[0] if self.K == 1 else eps
 
     # ---- C51 ----
     def set_c51(self, n_atoms: int, v_min: float, v_max: float) -> None:

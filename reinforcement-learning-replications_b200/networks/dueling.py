@@ -8,14 +8,18 @@ from typing import List, Sequence, Type
 
 from torch import Tensor, nn
 
+from .noisy import NoisyLinear
+
 
 class DuelingMLP(nn.Module):
     """``sizes`` = [obs, h_trunk, h_stream]; ``outputs_per_action`` = K values per action: 1 for DQN, n_atoms logits for
     C51, n_quantiles locations for QR-DQN.  forward: h = trunk(x), V = value(h) [..., K], A = advantage(h) [..., n, K],
-    Q = V + (A - mean over actions of A), flattened to [..., n K] (action a owns columns a K .. a K + K - 1)."""
+    Q = V + (A - mean over actions of A), flattened to [..., n K] (action a owns columns a K .. a K + K - 1).
+    ``noisy`` = True makes the four stream layers ``NoisyLinear`` (initial sigma_0 / sqrt(in)) and keeps the trunk plain,
+    as Rainbow does."""
 
     def __init__(self, sizes: Sequence[int], n_actions: int, outputs_per_action: int = 1,
-                 activation_function: Type[nn.Module] = nn.ReLU) -> None:
+                 activation_function: Type[nn.Module] = nn.ReLU, noisy: bool = False, sigma_0: float = 0.5) -> None:
         super().__init__()
         self.sizes: List[int] = [int(w) for w in sizes]
         if len(self.sizes) != 3 or min(self.sizes) < 1:
@@ -27,8 +31,9 @@ class DuelingMLP(nn.Module):
         O, h1, h2 = self.sizes
         K, n = self.outputs_per_action, self.n_actions
         self.trunk = nn.Sequential(nn.Linear(O, h1), activation_function())
-        self.value = nn.Sequential(nn.Linear(h1, h2), activation_function(), nn.Linear(h2, K))
-        self.advantage = nn.Sequential(nn.Linear(h1, h2), activation_function(), nn.Linear(h2, n * K))
+        lin = (lambda i, o: NoisyLinear(i, o, sigma_0)) if noisy else nn.Linear
+        self.value = nn.Sequential(lin(h1, h2), activation_function(), lin(h2, K))
+        self.advantage = nn.Sequential(lin(h1, h2), activation_function(), lin(h2, n * K))
 
     def forward(self, input: Tensor) -> Tensor:
         h = self.trunk(input)

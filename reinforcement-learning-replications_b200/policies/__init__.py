@@ -1,5 +1,6 @@
-from .base import (CategoricalPolicy, DeterministicPolicy, EpsilonGreedyPolicy, GaussianPolicy, GreedyPolicy, Policy,
-                   RandomPolicy, SquashedGaussianPolicy, StochasticPolicy)
+from .base import (CategoricalPolicy, DeterministicPolicy, EpsilonGreedyPolicy, GaussianPolicy, GreedyPolicy,
+                   NoisyGreedyPolicy, Policy, RandomPolicy, SquashedGaussianPolicy, StochasticPolicy)
 
 __all__ = ["Policy", "StochasticPolicy", "CategoricalPolicy", "GaussianPolicy", "SquashedGaussianPolicy",
-           "DeterministicPolicy", "RandomPolicy", "GreedyPolicy", "EpsilonGreedyPolicy"]
+           "DeterministicPolicy", "RandomPolicy", "GreedyPolicy", "EpsilonGreedyPolicy",
+           "NoisyGreedyPolicy"]

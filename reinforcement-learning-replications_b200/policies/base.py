@@ -13,6 +13,8 @@ from torch import Tensor, nn
 from torch.distributions import Categorical, Distribution, Independent, Normal
 from torch.optim import Optimizer
 
+from ..networks.noisy import reset_noise
+
 
 class Policy(nn.Module, ABC):
     """ref: policies/policy.py:8-30"""
@@ -186,3 +188,28 @@ class EpsilonGreedyPolicy(GreedyPolicy):
 
     def get_action_tensor(self, observation: Tensor) -> Tensor:
         return torch.as_tensor(self.get_action_numpy(observation.detach().cpu().numpy()))
+
+
+class NoisyGreedyPolicy(GreedyPolicy):
+    """Acting with a noisy Q network (``networks.NoisyLinear``; Fortunato et al. 2018): every call first redraws the
+    noise of every noisy layer (torch's default CPU generator; a batch of observations shares one sample), then acts
+    greedily in train mode, on the noisy weights.  NumPy's stream is left alone.  ``deterministic()`` is the
+    evaluation view: greedy on the mean weights."""
+
+    def _greedy(self, observation: Tensor) -> Tensor:
+        reset_noise(self.q_function)
+        return super()._greedy(observation)
+
+    def deterministic(self) -> "Policy":
+        """A view that acts greedily with the network in eval mode (the mean weights mu), restoring the mode after."""
+        return _MeanGreedyPolicy(self.q_function)
+
+
+class _MeanGreedyPolicy(GreedyPolicy):
+    def _greedy(self, observation: Tensor) -> Tensor:
+        was = self.q_function.training
+        self.q_function.eval()
+        try:
+            return super()._greedy(observation)
+        finally:
+            self.q_function.train(was)

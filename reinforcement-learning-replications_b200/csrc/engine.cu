@@ -1007,6 +1007,9 @@ extern "C" int b200rl_onpolicy_device_view(b200rl_onpolicy* h, const char* name,
       // the conjugate-gradient state after the last update: residual, direction, and F x of the step-size product
       {"cg_r", h->cg_r, h->cg_r ? h->Pp : 0, 0},  {"cg_p", h->cg_p, h->cg_p ? h->Pp : 0, 0},
       {"cg_z", h->cg_z, h->cg_z ? h->Pp : 0, 0},
+      // the fused step kernel's per-slot partial rows [2 slots][P0 + P1] and scalar rows [2 slots][16]
+      {"fused_partials", h->partials, h->fused_ok ? 2 * (int64_t)tc_grid(h->n_rows) * (h->Pp + h->Pv) : 0, 0},
+      {"fused_scalar_partials", h->scalar_partials, h->fused_ok ? 2 * (int64_t)tc_grid(h->n_rows) * 2 * B200RL_N_SCALARS : 0, 1},
   };
   for (const V& v : views)
     if (strcmp(v.n, name) == 0) {
@@ -1121,12 +1124,20 @@ extern "C" int b200rl_onpolicy_run_stage(b200rl_onpolicy* h, const char* stage, 
   if (strcmp(stage, "value_grad_kernel") == 0)
     return launch_fused(h, h->cfg.value, B200RL_LOSS_MSE, B200RL_DIST_NONE, h->val, h->obs, h->n_rows, n_glob, 0.0,
                         false, false, nullptr, true, nullptr, s);
-  if (strcmp(stage, "pack_obs") == 0 || strcmp(stage, "fused_step_kernel") == 0 || strcmp(stage, "fused_step") == 0) {
+  const bool fused_one = strcmp(stage, "fused_step_kernel_policy") == 0 || strcmp(stage, "fused_step_kernel_value") == 0;
+  if (strcmp(stage, "pack_obs") == 0 || strcmp(stage, "fused_step_kernel") == 0 || strcmp(stage, "fused_step") == 0 ||
+      fused_one) {
     B200RL_REQUIRE(h->fused_ok, "run_stage: the networks do not fit the fused step kernel");
     if (strcmp(stage, "pack_obs") == 0) {
       B200RL_CUDA(cudaMemsetAsync(h->trip, 0, 4 * sizeof(float), s));
       if (!h->hints_valid && b200rl_absmax_cols(h->obs, h->n_rows, h->obs_dim, h->absmax, s)) return 1;
       return launch_pack_obs(h->obs, h->n_rows, h->obs_dim, h->absmax, h->ximg, h->xscale, h->trip, s);
+    }
+    if (fused_one) {  // the step kernel with one network running: what each network's share of the launch costs
+      Tc3Args k = tc3_args(h, hp, n_glob);
+      k.run_policy = stage[18] == 'p';
+      k.run_value = stage[18] == 'v';
+      return launch_mlp_tc3(k, s);
     }
     // one iteration of both loops on the packed observations ("pack_obs" and "preamble" first): the step kernel
     // alone, or with the reduction of its partial rows (mode 1: parameters stay as they are)

@@ -4,24 +4,23 @@
 // Why (reference: /root/reference/src/rl_replicas/algorithms/ppo.py:173-181 policy loop, :186-192 value loop): the two
 // loops touch disjoint parameters and read the same fixed inputs (advantages and returns are computed before either
 // loop, :142-161), so step i of both can share one pass over the batch.  Compared with two mlp_tc2 launches:
-//   * the POLICY chain and the VALUE chain of the SAME tile run side by side, and the observation operand is staged
-//     once for both.  Rows are independent in the forward / backward chain, so each (network, 64-row half) is one
-//     warpgroup that issues its own m64 products and keeps the accumulator in registers: its epilogues work on the
-//     wgmma fragment and hand over to its next product through a warpgroup-local barrier.  Two more warpgroups, one
-//     per network, issue the weight-gradient products off the chains' critical path, side by side: the two networks'
-//     products share no accumulator and no written buffer.  mbarriers tell a gradient warpgroup when both halves of
-//     its network have delivered a stage's operands, and tell the chains when it has finished reading a buffer they
-//     are about to overwrite; the warpgroup of the last running network also brings the observations in.  The
-//     accumulators stay in L2 (tc_common.cuh), stored fragment by fragment (grad_acc_off), and each fragment is
-//     prefetched into L1 while the products before it run (grad_mma);
+//   * the two networks share only the read-only observation tile, so each runs in CTAs of its own: CTA c G + slot
+//     runs network c on the tiles of slot `slot`, the policy CTAs as the first wave and the value CTAs as the second.
+//     Rows are independent in the forward / backward chain, so each 64-row half of a tile is one warpgroup that
+//     issues its own m64 products and keeps the accumulator in registers: its epilogues work on the wgmma fragment
+//     and hand over to its next product through a warpgroup-local barrier.  Two more warpgroups, one per m64 half of
+//     the stacked A operands (the h and the l split), issue the weight-gradient products off the chains' critical
+//     path, and keep their accumulators (88 floats a thread) in registers for the whole launch; they are stored once,
+//     in grad_acc_off's layout, for the read-out.  mbarriers tell the gradient warpgroups when both chain halves have
+//     delivered a stage's operands, and tell the chains when both have finished reading a buffer they are about to
+//     overwrite.  dZ2, dZ1 and dOut have buffers of their own, so the gradient products run about one tile behind the
+//     chains; the h-split warpgroup also brings the observations in;
 //   * the observations are split into their fp16 pairs ONCE PER UPDATE by pack_obs_kernel (every step of the update
 //     reads the same observations) into ready-made SWIZZLE_128B tile images [128 rows][h cols 0..31 | l cols 32..63];
 //     the step kernel brings a tile image in with ONE 16 KB bulk copy (cp.async.bulk + mbarrier complete_tx) issued by
 //     the producer warpgroup -- no epilogue touches the observations any more (E0 of mlp_tc2 is gone);
 //   * column 31 of the image is 1.0, so the bias gradients db1 / db2 still fall out of the weight-gradient products;
-//   * dLoss/dOut of both chains goes into the X buffer of the OTHER parity (it is idle between the previous tile's
-//     dW1 and the next tile's bulk copy), which is what makes two X buffers fit next to 4 x 32 KB of activations and
-//     2 x 28 KB of weights;
+//   * two X buffers: the next tile's bulk copy goes into the buffer of the previous tile once its dW1 has retired;
 //   * tanh'(H1) and tanh'(H2) are taken from the fp16 pairs in shared memory: no fp32 copy of H in registers;
 //   * one reduction + Adam launch for both networks (reduce_adam3_kernel), one all-reduce per iteration.
 // A range / precision trip (fp16 operands) raises a sticky flag; the engine then restores its snapshot and redoes the
@@ -39,24 +38,27 @@
 namespace b200rl {
 
 constexpr int T3_ROWS = 128;
-constexpr int T3_CHAIN_WARPS = 16;  // four chain warpgroups, one per (network, 64-row half of the tile)
-constexpr int T3_CHAIN_THREADS = T3_CHAIN_WARPS * 32;
-constexpr int T3_THREADS = T3_CHAIN_THREADS + 256;  // + one weight-gradient warpgroup per network
+constexpr int T3_CHAIN_WARPS = 8;  // two chain warpgroups, one per 64-row half of the tile
+constexpr int T3_THREADS = T3_CHAIN_WARPS * 32 + 256;  // + one weight-gradient warpgroup per m64 half of the A operand
+constexpr int T3_WARPS = T3_THREADS / 32;
 
-// ---- shared-memory map (bytes from the 1024-aligned base) ----
-constexpr uint32_t S3_XB = 0;                        // X(k) | dOut(k) buffers, parity k & 1 and (k + 1) & 1
-constexpr uint32_t S3_H = 2 * T2_ACT;                // per chain: H1 h, H1 l, H2 h, H2 l
-constexpr uint32_t S3_CHAIN = 4 * T2_ACT;
+// ---- shared-memory map (bytes from the 1024-aligned base); one network per CTA ----
+constexpr uint32_t S3_XB = 0;                        // X(k) in buffer k & 1
+constexpr uint32_t S3_H1 = 2 * T2_ACT;               // fp16 pairs (h, then l): H1, H2, dZ2, dZ1
+constexpr uint32_t S3_H2 = S3_H1 + 2 * T2_ACT;
+constexpr uint32_t S3_DZ2 = S3_H2 + 2 * T2_ACT;
+constexpr uint32_t S3_DZ1 = S3_DZ2 + 2 * T2_ACT;
 constexpr uint32_t T3_W1T = 32 * 128, T3_W2 = 64 * 128, T3_W3 = 16 * 128;  // one split of each weight operand
-constexpr uint32_t S3_W = S3_H + 2 * S3_CHAIN;       // per net: W1T h,l | W2 h,l | W3 h,l
+constexpr uint32_t S3_DO = S3_DZ1 + 2 * T2_ACT;      // dOut: 16 columns h, then 16 columns l, at column 32 c
+constexpr uint32_t S3_W = S3_DO + T2_ACT;            // W1T h,l | W2 h,l | W3 h,l
 constexpr uint32_t S3_WNET = 2 * T3_W1T + 2 * T3_W2 + 2 * T3_W3;
-constexpr uint32_t S3_OPERANDS_END = S3_W + 2 * S3_WNET;
+constexpr uint32_t S3_OPERANDS_END = S3_W + S3_WNET;
 constexpr uint32_t S3_BIAS = S3_OPERANDS_END;        // per net: b1[64] b2[64] b3[16] + pad = 160 floats
 constexpr uint32_t S3_DIST = S3_BIAS + 2 * 640;      // var[16], log_scale[16], 1/(2 var)[16], 1/var[16]
 constexpr uint32_t S3_SCALE = S3_DIST + 256;         // per net 16 floats
 constexpr uint32_t S3_XS = S3_SCALE + 128;           // 2^ex_k [32], 2^-ex_k [32]
-constexpr uint32_t S3_RED = S3_XS + 256;             // setup reduction scratch [24 warps][8] floats
-constexpr uint32_t S3_BARS = S3_RED + 4 * 8 * (T3_THREADS / 32);  // 15 mbarriers (8 B each), bad flag at +120
+constexpr uint32_t S3_RED = S3_XS + 256;             // setup reduction scratch [16 warps][8] floats
+constexpr uint32_t S3_BARS = S3_RED + 4 * 8 * T3_WARPS;  // 8 mbarriers (8 B each), bad flag at +120
 constexpr uint32_t S3_TOTAL = S3_BARS + 128;
 constexpr uint32_t T3_SMEM_BYTES = S3_TOTAL + 1024;  // + alignment slack
 static_assert(T3_SMEM_BYTES <= 227 * 1024, "mlp_tc3 shared memory");
@@ -93,16 +95,12 @@ __device__ __forceinline__ uint32_t grad_acc_off(uint32_t pcol, int n, int row, 
 }
 
 #ifdef B200RL_TC3_TIMING
-// CTA 0, chain warpgroup wg = 2 c + h: [10 wg + s - 1] cycles stage s (E1..E5) waited on an mbarrier, [10 wg + 4 + s]
-// cycles of stage s in all; gradient warpgroup of network c: [40 + 3 c + s - 3] cycles waited for the operands of stage
-// s (3..5) (stage 4 of the observations' producer: also for the other network to release the dOut buffer),
-// [46 + 3 c + s - 3] cycles issuing its products, split over all stages into [56 + 3 c] waiting for its fragment loads
-// (and asking for the next fragment), [57 + 3 c] wgmma_fence .. wgmma_wait_all, [58 + 3 c] fragment stores and the
-// hand-over (bar.sync, mbar_arrive); [52] tiles of the CTA, [53] set-up, [54] tile loop, [55] read-out
+// CTA 0, chain warpgroup wg (64-row half): [10 wg + s - 1] cycles stage s (E1..E5) waited on an mbarrier,
+// [10 wg + 4 + s] cycles of stage s in all; gradient warpgroup g (m64 half of A): [40 + 3 g + s - 3] cycles waited for
+// the operands of stage s (3..5) (stage 4 of the observations' producer: also for the other half's dW3 to release the
+// dOut buffer), [46 + 3 g + s - 3] cycles issuing its products, waiting for them and handing the buffers back;
+// [52] tiles of the CTA, [53] set-up, [54] tile loop, [55] read-out
 __device__ unsigned long long g_tc3_t[64];
-#define TC3_TSPLIT(c) (tacc + 56 + 3 * (c))
-#else
-#define TC3_TSPLIT(c) nullptr
 #endif
 
 enum { C3_G = 0, C3_U1, C3_U2, C3_U3, C3_UH2, C3_UH1, C3_W1, C3_W2, C3_W3, C3_OW3, C3_OW2, C3_OW1, C3_OB, C3_N };
@@ -210,14 +208,8 @@ __device__ __forceinline__ float* grad_frag(float* acc_cta, uint32_t pcol) {
   const int t = (int)(threadIdx.x & 127u);
   return acc_cta + grad_acc_off(pcol, 0, 16 * (t >> 5) + ((t & 31) >> 2), 2 * (t & 3));
 }
-// Asks for the `chunks` 16-byte fragment chunks (at most 8) from `src` to be brought into L1, without waiting.
-__device__ __forceinline__ void grad_prefetch(const float* src, int chunks) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j)
-    if (j < chunks) asm volatile("prefetch.global.L1 [%0];" ::"l"(src + 512 * j));
-}
-// The products of one weight-gradient wgmma group into fragment `d` (both operands MN-major): TERMS terms (B split l,
-// then h), KSTEPS k-steps each, A at descriptor low word `a_lo`; the first product overwrites on the first tile.
+// The products of one weight-gradient fragment `d` (both operands MN-major): TERMS terms (B split l, then h), KSTEPS
+// k-steps each, A at descriptor low word `a_lo`; the first product overwrites on the first tile.
 template <int N, int KSTEPS, int TERMS>
 __device__ __forceinline__ void grad_products(float (&d)[N / 2], uint32_t a_lo, const Op2 a, const Op2 b, bool first) {
   // an opaque copy per product: products that share A would otherwise share its k-step descriptors, held live (and
@@ -233,84 +225,14 @@ __device__ __forceinline__ void grad_products(float (&d)[N / 2], uint32_t a_lo, 
                                                                  (uint32_t)k * b.k_step),
                                        s == 0 && k == 0 ? (first ? 0u : 1u) : 1u);
 }
-// weight-gradient product over the whole tile: A stacks its two splits along M (rows 0..63 h, 64..127 l: the two m64
-// halves), B split l (B_SPLITS == 2) then h.  Each wgmma group loads its fragments from the accumulator memory, asks for
-// the fragment of the group after it (this product's second half, then `next_chunks` chunks of the product at column
-// `next_col`) to be brought into L1, runs its products and stores the fragments back.  A group's cost is mostly its
-// fragments' L2 round trip, whatever its width, so the groups hold as many products as 80 registers a thread allow:
-//   * BOTH: both m64 halves of an n32 product in one group -- 32 floats, chunks 0..7 as an n64 half's (grad_acc_off);
-//   * N2 > 0: with each half, the same half of a second, single-term product of width N2 with the same A (B = `b2`, at
-//     accumulator column `col2`).
-// Every accumulator still sees the same terms in the same order.  On the launch's first tile (`first`) the products
-// overwrite and nothing is loaded.
-template <int N, int KSTEPS, int B_SPLITS, int N2 = 0, bool BOTH = false>
-__device__ __forceinline__ void grad_mma(float* acc_cta, uint32_t acc_col, bool first, const Op2 a, const Op2 b,
-                                         uint32_t next_col, int next_chunks, unsigned long long* tsplit,
-                                         uint32_t col2 = 0, const Op2 b2 = Op2{}) {
-  static_assert(!BOTH || (N == 32 && N2 == 0), "one group for both halves: an n32 product");
-  constexpr int CH = BOTH ? 8 : N / 8, CH2 = N2 / 8;  // fragment chunks of the group
-  const uint32_t a_half = (a.lo >> 16) & 0x3FFFu;     // the leading byte offset: A's l split
-  float* const frag0 = grad_frag(acc_cta, acc_col);
-  float* const frag20 = grad_frag(acc_cta, col2);
-#pragma unroll 1
-  for (int h = 0; h < (BOTH ? 1 : 2); ++h) {
-#ifdef B200RL_TC3_TIMING
-    const long long t0 = clock64();
-#endif
-    float* const frag = frag0 + 64 * N * h;
-    float* const frag2 = frag20 + 64 * N2 * h;
-    float d[4 * CH], e[CH2 > 0 ? 4 * CH2 : 1];
+// Stores this thread's fragment of m64 half `h` of the weight-gradient product with N columns at accumulator column
+// `pcol` in grad_acc_off's layout: chunk j (fragment elements 4 j .. 4 j + 3) 512 j floats further.
+template <int N>
+__device__ __forceinline__ void grad_store(float* acc_cta, uint32_t pcol, int h, const float (&d)[N / 2]) {
+  float* const frag = grad_frag(acc_cta, pcol) + 64 * N * h;
 #pragma unroll
-    for (int j = 0; j < CH; ++j) {
-      const float4 v = first ? make_float4(0.f, 0.f, 0.f, 0.f) : *reinterpret_cast<const float4*>(frag + 512 * j);
-      d[4 * j] = v.x;
-      d[4 * j + 1] = v.y;
-      d[4 * j + 2] = v.z;
-      d[4 * j + 3] = v.w;
-    }
-#pragma unroll
-    for (int j = 0; j < CH2; ++j) {
-      const float4 v = first ? make_float4(0.f, 0.f, 0.f, 0.f) : *reinterpret_cast<const float4*>(frag2 + 512 * j);
-      e[4 * j] = v.x;
-      e[4 * j + 1] = v.y;
-      e[4 * j + 2] = v.z;
-      e[4 * j + 3] = v.w;
-    }
-    if (h == 0 && !BOTH) {
-      grad_prefetch(frag + 64 * N, first ? 0 : CH);
-      grad_prefetch(frag2 + 64 * N2, first ? 0 : CH2);
-    } else {
-      grad_prefetch(grad_frag(acc_cta, next_col), next_chunks);
-    }
-#ifdef B200RL_TC3_TIMING
-    wgmma_fence();  // waits on the fragment's loads, though not reliably on all of them: some latency counts in [57]
-    const long long t1 = clock64();
-#endif
-    wgmma_fence();
-    if constexpr (BOTH) {
-      grad_products<N, KSTEPS, B_SPLITS>(*reinterpret_cast<float(*)[N / 2]>(&d[0]), a.lo, a, b, first);
-      grad_products<N, KSTEPS, B_SPLITS>(*reinterpret_cast<float(*)[N / 2]>(&d[N / 2]), a.lo + a_half, a, b, first);
-    } else {
-      grad_products<N, KSTEPS, B_SPLITS>(d, a.lo + (uint32_t)h * a_half, a, b, first);
-    }
-    if constexpr (N2 > 0) grad_products<N2, KSTEPS, 1>(e, a.lo + (uint32_t)h * a_half, a, b2, first);
-    wgmma_commit();
-    wgmma_wait_all();
-#ifdef B200RL_TC3_TIMING
-    const long long t2 = clock64();
-#endif
-#pragma unroll
-    for (int j = 0; j < CH; ++j)
-      *reinterpret_cast<float4*>(frag + 512 * j) = make_float4(d[4 * j], d[4 * j + 1], d[4 * j + 2], d[4 * j + 3]);
-#pragma unroll
-    for (int j = 0; j < CH2; ++j)
-      *reinterpret_cast<float4*>(frag2 + 512 * j) = make_float4(e[4 * j], e[4 * j + 1], e[4 * j + 2], e[4 * j + 3]);
-#ifdef B200RL_TC3_TIMING
-    tsplit[0] += (unsigned long long)(t1 - t0);
-    tsplit[1] += (unsigned long long)(t2 - t1);
-    tsplit[2] += (unsigned long long)(clock64() - t2);
-#endif
-  }
+  for (int j = 0; j < N / 8; ++j)
+    *reinterpret_cast<float4*>(frag + 512 * j) = make_float4(d[4 * j], d[4 * j + 1], d[4 * j + 2], d[4 * j + 3]);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -318,13 +240,22 @@ __device__ __forceinline__ void grad_mma(float* acc_cta, uint32_t acc_col, bool 
 // ------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p) {
   extern __shared__ uint8_t smem_raw[];
-  // chain 0 = policy, chain 1 = value; which of them run is the same for every thread of the grid
+  // Network c of this CTA (0 policy, 1 value) and its tile slot: with both networks launched, CTA c G + slot; with
+  // one, CTA slot.  Both CTAs of a slot take tiles slot + k G and share accumulator block `slot` (disjoint columns).
+  // Network-major order: the G policy CTAs (one per SM) make the first wave and the value CTAs the second, so every
+  // SM runs one CTA of each network.  Interleaved, the SMs that drew a policy CTA for the first wave would have been
+  // freed last and drawn half of the second wave's policy CTAs too.
+  const bool two = p.run_policy != 0 && p.run_value != 0;
+  const int G = two ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  const int c = two ? (int)blockIdx.x / G : (p.run_policy != 0 ? 0 : 1);
+  const int slot = (int)blockIdx.x - c * (two ? G : 0);
+  // which network runs is the same for every thread of the grid
   const bool run_p = p.run_policy != 0 && (p.stop_flag == nullptr || *p.stop_flag == 0);
   const bool run_v = p.run_value != 0;
-  if (!run_p && !run_v) return;
+  if (!(c == 0 ? run_p : run_v)) return;
   if (*p.x_bad != 0.f) return;  // the packed observations left the fp16 range: the engine redoes the update (wide-range path)
   const int tid = threadIdx.x, lane = tid & 31;
-  float* const acc = p.acc_mem + (size_t)blockIdx.x * ACC_CTA_FLOATS;
+  float* const acc = p.acc_mem + (size_t)slot * ACC_CTA_FLOATS;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // provably warp-uniform (see mlp_tc2.cu)
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
@@ -344,16 +275,17 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   const long long t_kernel0 = clock64();
 #endif
 
-  // ---- one-time setup: scales; weights of both networks as fp16 pairs; biases ----
-  // Only the weight operands need zero padding (X tiles arrive whole by bulk copy, H and dOut are fully written by
+  // ---- one-time setup: scales; weights of this CTA's network as fp16 pairs; biases ----
+  // Only the weight operands need zero padding (X tiles arrive whole by bulk copy, H, dZ and dOut are fully written by
   // their epilogues before any MMA reads them).  Both parameter vectors (44 KB) are first brought into the still unused
   // activation buffers with independent, coalesced loads: the two passes below (maxima, then conversion) would
-  // otherwise pay an L2 round trip per element, one after the other (17 of the 18 us this set-up took on B200).
+  // otherwise pay an L2 round trip per element, one after the other (17 of the 18 us this set-up took on B200).  Every
+  // CTA checks both networks' parameters, so a range trip is raised whichever networks run.
   for (uint32_t i = S3_W / 16 + tid; i < S3_OPERANDS_END / 16; i += T3_THREADS) reinterpret_cast<uint4*>(sm)[i] = make_uint4(0, 0, 0, 0);
   if (tid == 0) *s_bad = 0;
   if (tid < 64) s_xs[tid] = __ldg(p.xscale + tid);
-  float* s_par = reinterpret_cast<float*>(sm + S3_H);
-  static_assert(2 * S3_CHAIN >= 4 * (2 * 6000 + 64), "parameter staging area");
+  float* s_par = reinterpret_cast<float*>(sm + S3_H1);
+  static_assert(S3_W - S3_H1 >= 4 * (2 * 6000 + 64), "parameter staging area");
 #pragma unroll 1
   for (int net = 0; net < 2; ++net) {
     const float* par = p.params[net];
@@ -401,7 +333,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     const int net = tid;
     const Tc3Net& nn = p.net[net];
     float m1 = 0.f, m2 = 0.f, m3 = 0.f;
-    for (int w = 0; w < T3_THREADS / 32; ++w) {
+    for (int w = 0; w < T3_WARPS; ++w) {
       m1 = fmaxf(m1, s_red[w * 8 + 4 * net + 0]);
       m2 = fmaxf(m2, s_red[w * 8 + 4 * net + 1]);
       m3 = fmaxf(m3, s_red[w * 8 + 4 * net + 2]);
@@ -442,7 +374,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   for (int net = 0; net < 2; ++net) {
     const Tc3Net& nn = p.net[net];
     const float* par = s_par + (net == 0 ? 0 : p.P[0]);
-    const uint32_t wb = S3_W + net * S3_WNET;
+    const uint32_t wb = S3_W;
     auto put = [&](uint32_t buf, uint32_t stride, int r, int c, float x) {
       const __half hb = __float2half_rn(x);
       const __half lb = __float2half_rn(x - __half2float(hb));
@@ -452,12 +384,14 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     };
     const float* sc = s_scale + 16 * net;
     const float sw1 = sc[C3_W1], sw2 = sc[C3_W2], sw3 = sc[C3_W3];
-    for (int idx = tid; idx < nn.h1 * n_in; idx += T3_THREADS)  // W1 transposed: row = input, column = output
-      put(wb, T3_W1T, idx % n_in, idx / n_in, ((*(par + nn.w_off[0] + idx)) * s_xs[32 + idx % n_in]) * sw1);
-    for (int idx = tid; idx < nn.h2 * nn.h1; idx += T3_THREADS)
-      put(wb + 2 * T3_W1T, T3_W2, idx / nn.h1, idx % nn.h1, (*(par + nn.w_off[1] + idx)) * sw2);
-    for (int idx = tid; idx < nn.n_out * nn.h2; idx += T3_THREADS)
-      put(wb + 2 * T3_W1T + 2 * T3_W2, T3_W3, idx / nn.h2, idx % nn.h2, (*(par + nn.w_off[2] + idx)) * sw3);
+    if (net == c) {
+      for (int idx = tid; idx < nn.h1 * n_in; idx += T3_THREADS)  // W1 transposed: row = input, column = output
+        put(wb, T3_W1T, idx % n_in, idx / n_in, ((*(par + nn.w_off[0] + idx)) * s_xs[32 + idx % n_in]) * sw1);
+      for (int idx = tid; idx < nn.h2 * nn.h1; idx += T3_THREADS)
+        put(wb + 2 * T3_W1T, T3_W2, idx / nn.h1, idx % nn.h1, (*(par + nn.w_off[1] + idx)) * sw2);
+      for (int idx = tid; idx < nn.n_out * nn.h2; idx += T3_THREADS)
+        put(wb + 2 * T3_W1T + 2 * T3_W2, T3_W3, idx / nn.h2, idx % nn.h2, (*(par + nn.w_off[2] + idx)) * sw3);
+    }
     float* bb = s_bias + 160 * net;
     for (int i = tid; i < 64; i += T3_THREADS) {
       bb[i] = i < nn.h1 ? (*(par + nn.b_off[0] + i)) : 0.f;
@@ -471,56 +405,62 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   }
   if (p.dist == B200RL_DIST_GAUSSIAN)
     for (int a = tid; a < p.net[0].n_out; a += T3_THREADS) {
-      const NormalConsts c = normal_consts(p.log_std, a);
-      s_dist[a] = c.var;
-      s_dist[16 + a] = c.log_scale;
-      s_dist[32 + a] = c.inv_2var;
-      s_dist[48 + a] = c.inv_var;
+      const NormalConsts nc = normal_consts(p.log_std, a);
+      s_dist[a] = nc.var;
+      s_dist[16 + a] = nc.log_scale;
+      s_dist[32 + a] = nc.inv_2var;
+      s_dist[48 + a] = nc.inv_var;
     }
   if (bad) *s_bad = 1;  // non-finite bias
   bad = false;
   if (tid == 0) {
     mbar_init(bars + 0, 1);  // xfull[b]: arrive.expect_tx by the producer + the copy's bytes
     mbar_init(bars + 8, 1);
-    for (int i = 0; i < 6; ++i) {
-      mbar_init(bars + 16 + 8 * i, 2);  // ready[c][s]: one arrive per chain warpgroup of network c
-      mbar_init(bars + 64 + 8 * i, 1);  // done[c][s]: the gradient warpgroup of network c
+    for (int i = 0; i < 3; ++i) {
+      mbar_init(bars + 16 + 8 * i, 2);  // ready[s]: one arrive per chain warpgroup
+      mbar_init(bars + 40 + 8 * i, 2);  // done[s]: one arrive per gradient warpgroup
     }
-    mbar_init(bars + 112, (uint32_t)run_p + (uint32_t)run_v);  // dofree: one arrive per running network
     fence_mbar_init();
   }
   fence_proxy_async_smem();
   __syncthreads();
 
   const long long num_tiles = (p.n_rows + T3_ROWS - 1) / T3_ROWS;
-  const int cta_tiles = (int)((num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x);  // tiles blockIdx.x + k * gridDim.x
-  const int c_first = run_p ? 0 : 1, c_last = run_v ? 1 : 0;
+  const int cta_tiles = (int)((num_tiles - slot + G - 1) / G);  // tiles slot + k * G
 
   constexpr int K = K_MAJOR, MN = MN_MAJOR;
   const uint32_t ub = base;
-  // mbarriers: xfull[b] at +8b; ready[c][s - 3] at +16 + 8 (3c + s - 3) (count 2: one arrive per chain warpgroup of
-  // network c); done[c][s - 3] at +64 + 8 (3c + s - 3) (the weight-gradient products of stage s have read the buffers);
-  // dofree at +112 (every reader of this tile's X buffer has retired: the next tile's dOut may go there)
-  auto bar_ready = [&](int c, int s) { return bars + 16u + 8u * (uint32_t)(3 * c + s - 3); };
-  auto bar_done = [&](int c, int s) { return bars + 64u + 8u * (uint32_t)(3 * c + s - 3); };
-  const uint32_t bar_dofree = bars + 112;
+  // mbarriers: xfull[b] at +8b; ready[s - 3] at +16 + 8 (s - 3) (both chain warpgroups have delivered the operands of
+  // stage s); done[s - 3] at +40 + 8 (s - 3) (both gradient warpgroups' products of stage s have read their buffers)
+  auto bar_ready = [&](int s) { return bars + 16u + 8u * (uint32_t)(s - 3); };
+  auto bar_done = [&](int s) { return bars + 40u + 8u * (uint32_t)(s - 3); };
+  // the per-thread sums of the chain rows this thread owned (read out below).  Policy: loss terms, old_logp - logp,
+  // entropy, logp, logp^2; value: sc[0] = squared errors.  (The b3 sums live in accumulator memory, ACC_DB3.)
+  double sc[5] = {0, 0, 0, 0, 0};
+  int rows_done = 0;  // policy rows evaluated
+#ifdef B200RL_TC3_TIMING
+  long long t_loop0 = 0, t_loop_end = 0;
+#endif
 
   if (warp >= T3_CHAIN_WARPS) {
-    // ============ weight-gradient warpgroup of network c: warps 16..19 policy, 20..23 value ============
-    // Each issues its own network's products, stages 3..5 of every tile, on its own accumulator columns and H buffers;
-    // the two share only read-only operands (the X tile, the dOut buffer).  The warpgroup of c_last also produces the
-    // observation tiles.  A warpgroup whose network does not run in this launch has no tile work.
-    // views at chain 0 / X buffer 0; the others are reached by adding byte offsets to the descriptors
+    // ============ weight-gradient warpgroup g: rows 64 g .. 64 g + 63 of every stacked A operand (split h / l) ============
+    // Issues its half of the stage 3..5 products of every tile into accumulators that stay in its registers for the
+    // whole launch: dW3 n32, dW2 n64, db2 n16, dW1 n64 (88 floats).  Each product sees the same terms in the same order
+    // as when the fragments went through L2 tile by tile.  Warpgroup 0 also brings the observation tiles in.
+    // views at X buffer 0; the other is reached by adding a byte offset to the descriptors
     const Op2 X_M = op2_mnmajor(ub + S3_XB, T2_ACT, 64);         // B, N = 64: features h 0..31 (col 31 = ones) | l
     const Op2 X_M16 = op2_mnmajor(ub + S3_XB + 32, T2_ACT, 64);  // B, N = 16: h cols 16..31 (col 31 = ones)
-    const Op2 DO_M = op2_mnmajor(ub + S3_XB, T2_ACT, 32);        // B, N = 32: dOut h | l
-    const Op2 H1_M = op2_mnmajor(ub + S3_H, T2_ACT, T2_ACT), H2_M = op2_mnmajor(ub + S3_H + 2 * T2_ACT, T2_ACT, T2_ACT);
-    const int c = (warp - T3_CHAIN_WARPS) >> 2;
-    const bool runs = c == 0 ? run_p : run_v, producer = c == c_last, both = run_p && run_v;
-    const uint32_t co = c * S3_CHAIN, gcol = c * ACC_GRAD_NET;
+    const Op2 DO_M = op2_at(op2_mnmajor(ub + S3_DO, T2_ACT, 32), c * 64);  // B, N = 32: dOut h | l
+    const Op2 H1_M = op2_mnmajor(ub + S3_H1, T2_ACT, T2_ACT), H2_M = op2_mnmajor(ub + S3_H2, T2_ACT, T2_ACT);
+    const Op2 DZ2_M = op2_mnmajor(ub + S3_DZ2, T2_ACT, T2_ACT), DZ1_M = op2_mnmajor(ub + S3_DZ1, T2_ACT, T2_ACT);
+    const int g = (warp - T3_CHAIN_WARPS) >> 2;
+    const bool producer = g == 0;
+    const uint32_t ah = (uint32_t)g * (T2_ACT >> 4);  // this half's split of an A operand: descriptor low-word offset
+    const uint32_t gcol = c * ACC_GRAD_NET;
+    float w3[16], w2[32], b2[8], w1[32];
     auto load_x = [&](int k) {  // tile k of this CTA -> X buffer k & 1
       const uint32_t b = (uint32_t)(k & 1);
-      const long long tile = blockIdx.x + (long long)k * gridDim.x;
+      const long long tile = slot + (long long)k * G;
       uint32_t e;
       asm volatile("{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\tselp.u32 %0, 1, 0, q;\n\t}" : "=r"(e));
       if (e && (warp & 3) == 0) {  // one thread of the warpgroup
@@ -529,105 +469,99 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
       }
       __syncwarp();
     };
-    // first product of each stage: its accumulator columns within a network (its first group is 8 chunks: an n64 half,
-    // or both halves of dW3)
-    auto lead_col = [](int stage) { return stage == 3 ? ACC_DW3 : (stage == 4 ? ACC_DW2 : ACC_DW1); };
-    if (producer && cta_tiles > 0) load_x(0);  // c_last always runs
+    // every warp's share of the stage's products has retired: its buffers go back to the chains
+    auto release = [&](int stage) {
+      wgmma_commit();
+      wgmma_wait_all();
+      asm volatile("bar.sync %0, 128;" ::"r"(8 + g) : "memory");
+      if ((tid & 127) == 0) mbar_arrive(bar_done(stage));
+    };
+    if (producer && cta_tiles > 0) load_x(0);
 #pragma unroll 1
-    for (int k = 0; runs && k < cta_tiles; ++k) {
-      const uint32_t xo = (uint32_t)(k & 1) * T2_ACT, dob = (uint32_t)((k + 1) & 1) * T2_ACT;
+    for (int k = 0; k < cta_tiles; ++k) {
+      const uint32_t xo = (uint32_t)(k & 1) * T2_ACT;
       const bool first = k == 0;  // the first tile's products overwrite the accumulators
-#pragma unroll 1
-      for (int stage = 3; stage <= 5; ++stage) {
-        // the last half-product of this stage prefetches the first half-product after it: the next stage's, or the
-        // next tile's first stage; none after the last tile, and none on the first (where every product overwrites)
-        const bool nload = stage == 5 ? k + 1 < cta_tiles : !first;
-        const uint32_t next = gcol + lead_col(stage < 5 ? stage + 1 : 3);
-        const int next_chunks = nload ? 8 : 0;
-#ifdef B200RL_TC3_TIMING
-        const long long it0 = clock64();
-#endif
-        mbar_wait(bar_ready(c, stage), (uint32_t)(k & 1));  // both halves of network c have delivered the operands
-        const bool load_next = stage == 4 && producer && k + 1 < cta_tiles;
-        if (load_next && both) {
-          // The next tile's observations go to this tile's dOut buffer: the policy network's dW3 and its chains' dH2
-          // must have read it too.  A parity wait is only right while the barrier is in tile k's phase or has just
-          // completed it.  Neither barrier can be a whole phase ahead: its tile k + 1 phase needs the policy chains
-          // past Z1 of tile k + 1, whose observations arrive only after the copy below.  Nor behind: this warpgroup's
-          // chains waited on dofree for tile k - 1, which the policy warpgroup arrives on after its tile k - 1 stages.
-          mbar_wait(bar_done(0, 3), (uint32_t)(k & 1));
-          mbar_wait(bar_ready(0, 4), (uint32_t)(k & 1));
-        }
-#ifdef B200RL_TC3_TIMING
-        const long long it1 = clock64();
-        tacc[40 + 3 * c + stage - 3] += (unsigned long long)(it1 - it0);
-#endif
-        if (stage == 3) {
-          // dW3^T[i][o] += sum_r H2[r][i] dOut[r][o]
-          grad_mma<32, 8, 1, 0, true>(acc, gcol + ACC_DW3, first, op2_at(H2_M, co), op2_at(DO_M, dob + c * 64),
-                                      next, next_chunks, TC3_TSPLIT(c));
-        } else if (stage == 4) {
-          // every chain warpgroup's dH2 and every dW3 have read dOut: its buffer takes the next tile's observations
-          if (load_next) load_x(k + 1);
-          // dW2[o][i] += sum_r dZ2[r][o] H1[r][i] ; db2[o] += sum_r dZ2[r][o] * 1 (ones column of X), in dW2's groups
-          grad_mma<64, 8, 2, 16>(acc, gcol + ACC_DW2, first, op2_at(H2_M, co), op2_at(H1_M, co), next, next_chunks,
-                                 TC3_TSPLIT(c), gcol + ACC_DB2, op2_at(X_M16, xo));
-        } else {
-          // dW1[o][i] += sum_r dZ1[r][o] X[r][i]; column 31 (ones) collects db1
-          grad_mma<64, 8, 1>(acc, gcol + ACC_DW1, first, op2_at(H1_M, co), op2_at(X_M, xo), next, next_chunks,
-                             TC3_TSPLIT(c));
-        }
-#ifdef B200RL_TC3_TIMING
-        const long long ih = clock64();
-#endif
-        asm volatile("bar.sync %0, 128;" ::"r"(8 + c) : "memory");  // every warp's share of the products has retired
-        if ((tid & 127) == 0) {
-          mbar_arrive(bar_done(c, stage));
-          // db2 (stage 4) and dW1 (stage 5) were this network's readers of the tile's X buffer
-          if (stage == 5) mbar_arrive(bar_dofree);
-        }
-#ifdef B200RL_TC3_TIMING
-        const long long it2 = clock64();
-        tacc[46 + 3 * c + stage - 3] += (unsigned long long)(it2 - it1);
-        tacc[58 + 3 * c] += (unsigned long long)(it2 - ih);
-#endif
+      if (producer && k + 1 < cta_tiles) {
+        // tile k + 1 goes to the buffer of tile k - 1, whose last readers (db2 and dW1 of both halves) have retired
+        // once done[5] completes its tile k - 1 phase.  It cannot be a phase further: its tile k phase needs this
+        // warpgroup's own tile k arrival.
+        if (k > 0) mbar_wait(bar_done(5), (uint32_t)((k - 1) & 1));
+        load_x(k + 1);
       }
+#ifdef B200RL_TC3_TIMING
+      long long it0 = clock64(), it1;
+#define TC3_GSPLIT(s)                                                   \
+  it1 = clock64();                                                      \
+  tacc[40 + 3 * g + (s) - 3] += (unsigned long long)(it1 - it0);
+#define TC3_GEND(s)                                                     \
+  it0 = clock64();                                                      \
+  tacc[46 + 3 * g + (s) - 3] += (unsigned long long)(it0 - it1);
+#else
+#define TC3_GSPLIT(s)
+#define TC3_GEND(s)
+#endif
+      // dW3^T[i][o] += sum_r H2[r][i] dOut[r][o]
+      mbar_wait(bar_ready(3), (uint32_t)(k & 1));
+      TC3_GSPLIT(3)
+      wgmma_fence();
+      grad_products<32, 8, 1>(w3, H2_M.lo + ah, H2_M, DO_M, first);
+      release(3);
+      TC3_GEND(3)
+      // dW2[o][i] += sum_r dZ2[r][o] H1[r][i] ; db2[o] += sum_r dZ2[r][o] * 1 (ones column of X)
+      mbar_wait(bar_ready(4), (uint32_t)(k & 1));
+      TC3_GSPLIT(4)
+      wgmma_fence();
+      grad_products<64, 8, 2>(w2, DZ2_M.lo + ah, DZ2_M, H1_M, first);
+      grad_products<16, 8, 1>(b2, DZ2_M.lo + ah, DZ2_M, op2_at(X_M16, xo), first);
+      release(4);
+      TC3_GEND(4)
+      // dW1[o][i] += sum_r dZ1[r][o] X[r][i]; column 31 (ones) collects db1
+      mbar_wait(bar_ready(5), (uint32_t)(k & 1));
+      TC3_GSPLIT(5)
+      wgmma_fence();
+      grad_products<64, 8, 1>(w1, DZ1_M.lo + ah, DZ1_M, op2_at(X_M, xo), first);
+      release(5);
+      TC3_GEND(5)
+#undef TC3_GSPLIT
+#undef TC3_GEND
+    }
+    if (cta_tiles > 0) {  // once per launch: the fragments into the CTA's accumulator block, read out below
+      grad_store<32>(acc, gcol + ACC_DW3, g, w3);
+      grad_store<64>(acc, gcol + ACC_DW2, g, w2);
+      grad_store<16>(acc, gcol + ACC_DB2, g, b2);
+      grad_store<64>(acc, gcol + ACC_DW1, g, w1);
     }
 #ifdef B200RL_TC3_TIMING
     if ((tid & 127) == 0 && blockIdx.x == 0) {
       for (int s = 0; s < 3; ++s) {
-        g_tc3_t[40 + 3 * c + s] = tacc[40 + 3 * c + s];
-        g_tc3_t[46 + 3 * c + s] = tacc[46 + 3 * c + s];
-        g_tc3_t[56 + 3 * c + s] = tacc[56 + 3 * c + s];
+        g_tc3_t[40 + 3 * g + s] = tacc[40 + 3 * g + s];
+        g_tc3_t[46 + 3 * g + s] = tacc[46 + 3 * g + s];
       }
       if (producer) g_tc3_t[52] = (unsigned long long)cta_tiles;
     }
 #endif
-    asm volatile("bar.sync 7, %0;" ::"n"(T3_THREADS) : "memory");  // the read-out may begin
   } else {
-    // ====================== chain warpgroup wg = 2 c + hf: network c, rows 64 hf .. 64 hf + 63 ======================
+    // ========================= chain warpgroup wg: rows 64 wg .. 64 wg + 63 of the tile =========================
     // Z1 -> E1 -> Z2 -> E2 -> OUT -> E3 -> dH2 -> E4 -> dH1 -> E5 with the accumulator in this warpgroup's registers.
     // Fragment element i of a thread is row r0 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 q + (i & 1) (wgmma D layout).
-    const int wg = warp >> 2, c = wg >> 1, hf = wg & 1;
+    // dZ2 and dZ1 have buffers of their own, so the gradient products of a tile can run while the chains go on to the
+    // next one: a chain only waits for the previous tile's readers of a buffer it is about to overwrite.
+    const int wg = warp >> 2;
     const int quad = lane >> 2, q = lane & 3;
-    const int r0 = 64 * hf + 16 * (warp & 3) + quad;  // == quad (mod 8): the swizzle phase of both fragment rows
-    const uint32_t rows = (uint32_t)hf * (64u * 128u);  // this half in a K-major buffer
-    const uint32_t co = c * S3_CHAIN, wo = c * S3_WNET, so = S3_H + co;
+    const int r0 = 64 * wg + 16 * (warp & 3) + quad;  // == quad (mod 8): the swizzle phase of both fragment rows
+    const uint32_t rows = (uint32_t)wg * (64u * 128u);  // this half in a K-major buffer
     const Op2 X_K = op2_at(op2_kmajor(ub + S3_XB, 64), rows);  // A: X, h at +0, l at +64 bytes
-    const Op2 DO_K = op2_at(op2_kmajor(ub + S3_XB, 32), rows);  // A, K = 16: dOut h at +0, l at +32 bytes
-    const Op2 H1_K = op2_at(op2_kmajor(ub + S3_H, T2_ACT), rows), H2_K = op2_at(op2_kmajor(ub + S3_H + 2 * T2_ACT, T2_ACT), rows);
+    const Op2 DO_K = op2_at(op2_kmajor(ub + S3_DO, 32), rows + c * 64);  // A, K = 16: dOut h at +0, l at +32 bytes
+    const Op2 H1_K = op2_at(op2_kmajor(ub + S3_H1, T2_ACT), rows), H2_K = op2_at(op2_kmajor(ub + S3_H2, T2_ACT), rows);
+    const Op2 DZ2_K = op2_at(op2_kmajor(ub + S3_DZ2, T2_ACT), rows);
     const Op2 W1T_M = op2_mnmajor(ub + S3_W, 32 * 128, T3_W1T);
     const Op2 W2_K = op2_kmajor(ub + S3_W + 2 * T3_W1T, T3_W2), W2_M = op2_mnmajor(ub + S3_W + 2 * T3_W1T, 64 * 128, T3_W2);
     const Op2 W3_K = op2_kmajor(ub + S3_W + 2 * T3_W1T + 2 * T3_W2, T3_W3),
               W3_M = op2_mnmajor(ub + S3_W + 2 * T3_W1T + 2 * T3_W2, 16 * 128, T3_W3);
-    const bool runs = c == 0 ? run_p : run_v;
     const float* scl = s_scale + 16 * c;
     const float* bias = s_bias + 160 * c;
     const float sH = pow2i(T2_H_EXP), hh = pow2i(-2 * T2_H_EXP);
     const int A_out = p.net[0].n_out;
-    // per-thread sums of the rows this thread owns in E3.  Policy: loss terms, old_logp - logp, entropy, logp,
-    // logp^2; value: sc[0] = squared errors.  (The b3 sums live in accumulator memory, ACC_DB3.)
-    double sc[5] = {0, 0, 0, 0, 0};
 
     // byte offset of columns 8 j + 2 q, +1 of fragment row r0 + 8 r in the SWIZZLE_128B buffer `buf`
     auto frag_off = [&](uint32_t buf, int j, int r) -> uint32_t {
@@ -690,10 +624,10 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     };
     auto deliver = [&](int s) {
       wg_sync();
-      if ((tid & 127) == 0) mbar_arrive(bar_ready(c, s));
+      if ((tid & 127) == 0) mbar_arrive(bar_ready(s));
     };
 #ifdef B200RL_TC3_TIMING
-    long long t_mark = 0, t_loop0 = 0, t_loop_end = 0;
+    long long t_mark = 0;
 #endif
     auto wait = [&](int s, uint32_t bar, uint32_t parity) {
 #ifdef B200RL_TC3_TIMING
@@ -716,24 +650,25 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     t_loop0 = clock64();
     t_mark = t_loop0;
 #endif
-    if (runs) {
+    {
 #pragma unroll 1
       for (int k = 0; k < cta_tiles; ++k) {
-        const long long tile = blockIdx.x + (long long)k * gridDim.x;
-        const uint32_t xo = (uint32_t)(k & 1) * T2_ACT, dob = (uint32_t)((k + 1) & 1) * T2_ACT;
+        const long long tile = slot + (long long)k * G;
+        const uint32_t xo = (uint32_t)(k & 1) * T2_ACT;
         float d[32];
         // ---- Z1 = X W1^T -> E1 -> H1 ----
         wait(1, bars + 8 * (uint32_t)(k & 1), (uint32_t)((k >> 1) & 1));  // the tile's observations have arrived
-        chain_mma<64, MN, 2>(d, op2_at(X_K, xo), op2_at(W1T_M, wo));
+        chain_mma<64, MN, 2>(d, op2_at(X_K, xo), W1T_M);
         act(d, scl[C3_U1], bias);
-        if (k > 0) wait(1, bar_done(c, 5), (uint32_t)((k - 1) & 1));  // dW2, db2, dW1 of the last tile have read H1, H2
-        store_pairs(so, d);
+        // dW3, dW2 and db2 of the last tile have read H2, dOut, dZ2 and H1 (the chains' own products, in order)
+        if (k > 0) wait(1, bar_done(4), (uint32_t)((k - 1) & 1));
+        store_pairs(S3_H1, d);
         wg_sync();
         stage_end(1);
         // ---- Z2 = H1 W2^T -> E2 -> H2 ----
-        chain_mma<64, K, 4>(d, op2_at(H1_K, co), op2_at(W2_K, wo));
+        chain_mma<64, K, 4>(d, H1_K, W2_K);
         act(d, scl[C3_U2], bias + 64);
-        store_pairs(so + 2 * T2_ACT, d);
+        store_pairs(S3_H2, d);
         wg_sync();
         stage_end(2);
         // ---- OUT = H2 W3^T -> E3: loss head, one row per owner thread (lanes q = 0, 1 own rows r0, r0 + 8) ----
@@ -761,7 +696,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
           }
         }
         float o[8];
-        chain_mma<16, K, 4>(o, op2_at(H2_K, co), op2_at(W3_K, wo));
+        chain_mma<16, K, 4>(o, H2_K, W3_K);
         float out[16];  // the owner's output row, gathered from its quad
 #pragma unroll
         for (int j = 0; j < 2; ++j)
@@ -824,7 +759,6 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
           }
           if (out_of_range8(x0) || out_of_range8(x1)) bad = true;
         }
-        if (k > 0) wait(3, bar_dofree, (uint32_t)((k - 1) & 1));  // the last tile's X buffer is free for dOut
         if (owner) {
           // 16 columns h, then 16 columns l, at fp16 columns 32 c .. 32 c + 31 of the dOut buffer
           uint4 h0, l0, h1, l1;
@@ -836,7 +770,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
           split2h(x1[2], x1[3], h1.y, l1.y);
           split2h(x1[4], x1[5], h1.z, l1.z);
           split2h(x1[6], x1[7], h1.w, l1.w);
-          uint8_t* rowp = sm + S3_XB + dob + (uint32_t)orow * 128u;
+          uint8_t* rowp = sm + S3_DO + (uint32_t)orow * 128u;
           const uint32_t sw = (uint32_t)(orow & 7), c4 = 4u * (uint32_t)c;
           *reinterpret_cast<uint4*>(rowp + (((c4 + 0u) ^ sw) << 4)) = h0;
           *reinterpret_cast<uint4*>(rowp + (((c4 + 1u) ^ sw) << 4)) = h1;
@@ -845,18 +779,17 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
         }
         deliver(3);
         stage_end(3);
-        // ---- dH2 = dOut W3 -> E4 -> dZ2, in place of H2 ----
-        chain_mma<64, MN, 1>(d, op2_at(DO_K, dob + c * 64), op2_at(W3_M, wo));
-        dtanh(d, scl[C3_UH2] * hh, so + 2 * T2_ACT);
-        wait(4, bar_done(c, 3), (uint32_t)(k & 1));  // dW3 has read H2
-        store_pairs(so + 2 * T2_ACT, d);
+        // ---- dH2 = dOut W3 -> E4 -> dZ2 ----
+        chain_mma<64, MN, 1>(d, DO_K, W3_M);
+        dtanh(d, scl[C3_UH2] * hh, S3_H2);
+        store_pairs(S3_DZ2, d);
         deliver(4);
         stage_end(4);
-        // ---- dH1 = dZ2 W2 -> E5 -> dZ1, in place of H1 ----
-        chain_mma<64, MN, 4>(d, op2_at(H2_K, co), op2_at(W2_M, wo));
-        dtanh(d, scl[C3_UH1] * hh, so);
-        wait(5, bar_done(c, 4), (uint32_t)(k & 1));  // dW2 has read H1
-        store_pairs(so, d);
+        // ---- dH1 = dZ2 W2 -> E5 -> dZ1 ----
+        chain_mma<64, MN, 4>(d, DZ2_K, W2_M);
+        dtanh(d, scl[C3_UH1] * hh, S3_H1);
+        if (k > 0) wait(5, bar_done(5), (uint32_t)((k - 1) & 1));  // dW1 of the last tile has read dZ1
+        store_pairs(S3_DZ1, d);
         deliver(5);
         stage_end(5);
       }
@@ -866,136 +799,136 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     if ((tid & 127) == 0 && blockIdx.x == 0)
       for (int i = 0; i < 10; ++i) g_tc3_t[10 * wg + i] = tacc[10 * wg + i];
 #endif
-
-    asm volatile("bar.sync 7, %0;" ::"n"(T3_THREADS) : "memory");  // with the gradient warpgroups: every product has
-                                                                   // retired and its accumulators are stored
-    // ---- per-CTA results ----
-    {
-      // stacked accumulators: rows 0..63 = h-split half (partial row 2b), rows 64..127 = l-split half (row 2b + 1);
-      // 8 jobs per net (dW2 x 4 column blocks, dW1 x 2, dW3, db2); warp `part` takes jobs part, part + 4 of both nets
-      const int qw = warp & 3, part = warp >> 2;
-      const int r = 32 * qw + lane;
-      float* dst_row = p.partials + ((size_t)blockIdx.x * 2 + (qw >> 1)) * (size_t)(p.P[0] + p.P[1]);
-      const int m = 32 * (qw & 1) + lane;  // feature index
-      float v[16], w[16];
-#pragma unroll 1
-      for (int cn = c_first; cn <= c_last; ++cn) {
-        const Tc3Net& nn = p.net[cn];
-        float* dst = dst_row + (cn == 0 ? 0 : p.P[0]);
-        const float* scn = s_scale + 16 * cn;
-        const bool have = cta_tiles > 0;
-        const uint32_t gcol = cn * ACC_GRAD_NET;
-#pragma unroll 1
-        for (int jb = part; jb < 8; jb += 4) {
-          // the job's product (first column, N), the job's columns in it, and those of its second half where the
-          // operand's l columns went to their own block
-          const uint32_t pcol = gcol + (jb < 4 ? ACC_DW2 : (jb < 6 ? ACC_DW1 : (jb == 6 ? ACC_DW3 : ACC_DB2)));
-          const int pn = jb < 6 ? 64 : (jb == 6 ? 32 : 16);
-          const int col = jb < 4 ? 16 * jb : (jb < 6 ? 16 * (jb - 4) : 0);
-          const int col2 = jb < 4 ? col : (jb < 6 ? col + 32 : (jb == 6 ? 16 : col));
-          if (have) {
-            // col and col2 are multiples of 8: column col + j of row r sits grad_acc_off(0, pn, 0, j) after column col
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              v[j] = acc[grad_acc_off(pcol, pn, r, col) + grad_acc_off(0, pn, 0, j)];
-              w[j] = acc[grad_acc_off(pcol, pn, r, col2) + grad_acc_off(0, pn, 0, j)];
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = w[j] = 0.f;  // a CTA without tiles: accumulator memory was never written
-          }
-          if (jb < 4) {  // dW2 [h2 o][h1 i]: columns 16 jb .. +15
-            const float u = scn[C3_OW2];
-            if (m < nn.h2)
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (16 * jb + j < nn.h1) dst[nn.w_off[1] + m * nn.h1 + 16 * jb + j] = v[j] * u;
-          } else if (jb < 6) {  // dW1 [h1 o][n_in i] in columns 0..30, db1 in column 31
-            const int c0 = 16 * (jb - 4);
-            const float u = scn[C3_OW1];
-            if (m < nn.h1) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (c0 + j < n_in)
-                  dst[nn.w_off[0] + m * n_in + c0 + j] = ((v[j] + w[j]) * u) * s_xs[32 + c0 + j];
-              if (jb == 5) dst[nn.b_off[0] + m] = (v[15] + w[15]) * scn[C3_OB];
-            }
-          } else if (jb == 6) {  // dW3^T [h2 i][16 o]
-            const float u = scn[C3_OW3];
-            if (m < nn.h2)
-#pragma unroll
-              for (int a = 0; a < 15; ++a)
-                if (a < nn.n_out) dst[nn.w_off[2] + a * nn.h2 + m] = (v[a] + w[a]) * u;
-          } else {  // db2 (column 15 = sum_r dZ2[r][o] * ones)
-            if (m < nn.h2) dst[nn.b_off[1] + m] = v[15] * scn[C3_OB];
-          }
-        }
-      }
-    }
-    // per-thread sums -> per-warp sums (tree) -> the warps in order: fixed order => reproducible.  The scratch aliases
-    // the X buffers (idle now).
-    float* e_db3 = reinterpret_cast<float*>(sm + S3_XB + S3_END_DB3);
-    double* e_sc = reinterpret_cast<double*>(sm + S3_XB + S3_END_SC);
-    {
-      // b3: warp 4 m + j takes class m of rows 32 j .. 32 j + 31 (see ACC_DB3); a class without tiles was never written
-      const int m = warp >> 2, rr = 32 * (warp & 3) + lane;
-#pragma unroll
-      for (int a = 0; a < 16; ++a) {
-        const int cn = a == 15 ? 1 : 0;
-        const bool have = (cn == 0 ? run_p : run_v) && ((m - 2 * cn) & 3) < cta_tiles;
-        float t = have ? acc[(ACC_DB3 + 16 * m + a) * ACC_LANES + rr] : 0.f;
-#pragma unroll
-        for (int o2 = 16; o2 > 0; o2 >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o2);
-        if (lane == 0) e_db3[warp * 16 + a] = t;
-      }
-    }
-#pragma unroll
-    for (int kk = 0; kk < 5; ++kk) {
-      const double t = warp_sum(sc[kk]);
-      if (lane == 0) e_sc[warp * 8 + kk] = t;
-    }
-    {
-      // policy rows evaluated: the valid rows this thread owned, counted here rather than in a register of the loop
-      int rows_done = 0;
-      if (c == 0 && runs && q < 2)
-        for (int k = 0; k < cta_tiles; ++k) rows_done += (blockIdx.x + (long long)k * gridDim.x) * T3_ROWS + r0 + 8 * q < p.n_rows;
-      const double t = warp_sum((double)rows_done);
-      if (lane == 0) e_sc[warp * 8 + 5] = t;
-    }
-    asm volatile("bar.sync 6, %0;" ::"n"(T3_CHAIN_THREADS) : "memory");
-    const size_t Ptot = (size_t)(p.P[0] + p.P[1]);
-    constexpr int NW = T3_CHAIN_WARPS / 2;  // warps per network: policy 0..7, value 8..15
-    if (tid < 16) {  // b3 gradients: the 16 per-warp totals in warp order; policy a = 0..14, value in slot 15
-      const int cn = tid == 15 ? 1 : 0, a = tid == 15 ? 0 : tid;
-      const bool ran = cn == 0 ? run_p : run_v;
-      if (ran && a < p.net[cn].n_out) {
-        float t = 0.f;
-        for (int w = 0; w < T3_CHAIN_WARPS; ++w) t += e_db3[w * 16 + tid];
-        const size_t off = (cn == 0 ? 0 : (size_t)p.P[0]) + p.net[cn].b_off[2] + a;
-        p.partials[((size_t)blockIdx.x * 2) * Ptot + off] = t;
-        p.partials[((size_t)blockIdx.x * 2 + 1) * Ptot + off] = 0.f;
-      }
-    }
-    if (tid >= 32 && tid < 32 + 2 * B200RL_N_SCALARS) {  // scalar sums: policy 0..7, value 8..15
-      const int s = tid - 32;
-      double t = 0.0;
-      if (s < 6) {
-        for (int w = 0; w < NW; ++w) t += e_sc[w * 8 + s];
-      } else if (s == 8) {
-        for (int w = NW; w < 2 * NW; ++w) t += e_sc[w * 8 + 0];
-      }
-      p.scalar_partials[((size_t)blockIdx.x * 2) * (2 * B200RL_N_SCALARS) + s] = t;
-      p.scalar_partials[((size_t)blockIdx.x * 2 + 1) * (2 * B200RL_N_SCALARS) + s] = 0.0;
-    }
-    if (bad) *s_bad = 1;
-#ifdef B200RL_TC3_TIMING
-    if (tid == 0 && blockIdx.x == 0) {
-      g_tc3_t[53] = (unsigned long long)(t_loop0 - t_kernel0);      // setup
-      g_tc3_t[54] = (unsigned long long)(t_loop_end - t_loop0);     // tile loop (chain warpgroup 0)
-      g_tc3_t[55] = (unsigned long long)(clock64() - t_loop_end);   // read-out
-    }
-#endif
+    // the valid rows this thread owned, counted here rather than in a register of the loop
+    if (c == 0 && q < 2)
+      for (int k = 0; k < cta_tiles; ++k) rows_done += (slot + (long long)k * G) * T3_ROWS + r0 + 8 * q < p.n_rows;
   }
+
+  asm volatile("bar.sync 7, %0;" ::"n"(T3_THREADS) : "memory");  // every product has retired and its accumulators
+                                                                 // are stored
+  // ---- per-CTA results: this network's entries of partial rows 2 slot and 2 slot + 1 (the other CTA of the slot
+  // writes the other network's) ----
+  {
+    // stacked accumulators: rows 0..63 = h-split half (partial row 2b), rows 64..127 = l-split half (row 2b + 1);
+    // 8 jobs (dW2 x 4 column blocks, dW1 x 2, dW3, db2); warp `part` takes jobs part, part + 4
+    const int qw = warp & 3, part = warp >> 2;
+    const int r = 32 * qw + lane;
+    float* dst_row = p.partials + ((size_t)slot * 2 + (qw >> 1)) * (size_t)(p.P[0] + p.P[1]);
+    const int m = 32 * (qw & 1) + lane;  // feature index
+    float v[16], w[16];
+    const Tc3Net& nn = p.net[c];
+    float* dst = dst_row + (c == 0 ? 0 : p.P[0]);
+    const float* scn = s_scale + 16 * c;
+    const bool have = cta_tiles > 0;
+    const uint32_t gcol = c * ACC_GRAD_NET;
+#pragma unroll 1
+    for (int jb = part; jb < 8; jb += 4) {
+      // the job's product (first column, N), the job's columns in it, and those of its second half where the
+      // operand's l columns went to their own block
+      const uint32_t pcol = gcol + (jb < 4 ? ACC_DW2 : (jb < 6 ? ACC_DW1 : (jb == 6 ? ACC_DW3 : ACC_DB2)));
+      const int pn = jb < 6 ? 64 : (jb == 6 ? 32 : 16);
+      const int col = jb < 4 ? 16 * jb : (jb < 6 ? 16 * (jb - 4) : 0);
+      const int col2 = jb < 4 ? col : (jb < 6 ? col + 32 : (jb == 6 ? 16 : col));
+      if (have) {
+        // col and col2 are multiples of 8: column col + j of row r sits grad_acc_off(0, pn, 0, j) after column col
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          v[j] = acc[grad_acc_off(pcol, pn, r, col) + grad_acc_off(0, pn, 0, j)];
+          w[j] = acc[grad_acc_off(pcol, pn, r, col2) + grad_acc_off(0, pn, 0, j)];
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < 16; ++j) v[j] = w[j] = 0.f;  // a CTA without tiles: accumulator memory was never written
+      }
+      if (jb < 4) {  // dW2 [h2 o][h1 i]: columns 16 jb .. +15
+        const float u = scn[C3_OW2];
+        if (m < nn.h2)
+#pragma unroll
+          for (int j = 0; j < 16; ++j)
+            if (16 * jb + j < nn.h1) dst[nn.w_off[1] + m * nn.h1 + 16 * jb + j] = v[j] * u;
+      } else if (jb < 6) {  // dW1 [h1 o][n_in i] in columns 0..30, db1 in column 31
+        const int c0 = 16 * (jb - 4);
+        const float u = scn[C3_OW1];
+        if (m < nn.h1) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j)
+            if (c0 + j < n_in)
+              dst[nn.w_off[0] + m * n_in + c0 + j] = ((v[j] + w[j]) * u) * s_xs[32 + c0 + j];
+          if (jb == 5) dst[nn.b_off[0] + m] = (v[15] + w[15]) * scn[C3_OB];
+        }
+      } else if (jb == 6) {  // dW3^T [h2 i][16 o]
+        const float u = scn[C3_OW3];
+        if (m < nn.h2)
+#pragma unroll
+          for (int a = 0; a < 15; ++a)
+            if (a < nn.n_out) dst[nn.w_off[2] + a * nn.h2 + m] = (v[a] + w[a]) * u;
+      } else {  // db2 (column 15 = sum_r dZ2[r][o] * ones)
+        if (m < nn.h2) dst[nn.b_off[1] + m] = v[15] * scn[C3_OB];
+      }
+    }
+  }
+  // per-thread sums -> per-warp sums (tree) -> the warps in order: fixed order => reproducible.  The scratch aliases
+  // the X buffers (idle now).
+  float* e_db3 = reinterpret_cast<float*>(sm + S3_XB + S3_END_DB3);
+  double* e_sc = reinterpret_cast<double*>(sm + S3_XB + S3_END_SC);
+  {
+    // b3: warp 4 m + j takes class m of rows 32 j .. 32 j + 31 (see ACC_DB3); a class without tiles was never written
+    const int m = warp >> 2, rr = 32 * (warp & 3) + lane;
+#pragma unroll
+    for (int a = 0; a < 16; ++a) {
+      const int cn = a == 15 ? 1 : 0;
+      const bool have = cn == c && ((m - 2 * cn) & 3) < cta_tiles;
+      float t = have ? acc[(ACC_DB3 + 16 * m + a) * ACC_LANES + rr] : 0.f;
+#pragma unroll
+      for (int o2 = 16; o2 > 0; o2 >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o2);
+      if (lane == 0) e_db3[warp * 16 + a] = t;
+    }
+  }
+#pragma unroll
+  for (int kk = 0; kk < 5; ++kk) {
+    const double t = warp_sum(sc[kk]);
+    if (lane == 0) e_sc[warp * 8 + kk] = t;
+  }
+  {
+    const double t = warp_sum((double)rows_done);
+    if (lane == 0) e_sc[warp * 8 + 5] = t;
+  }
+  __syncthreads();
+  const size_t Ptot = (size_t)(p.P[0] + p.P[1]);
+  if (tid < 16) {  // b3 gradients: the 16 per-warp totals in warp order; policy a = 0..14, value in slot 15
+    const int cn = tid == 15 ? 1 : 0, a = tid == 15 ? 0 : tid;
+    if (cn == c && a < p.net[cn].n_out) {
+      float t = 0.f;
+      for (int w = 0; w < T3_WARPS; ++w) t += e_db3[w * 16 + tid];
+      const size_t off = (cn == 0 ? 0 : (size_t)p.P[0]) + p.net[cn].b_off[2] + a;
+      p.partials[((size_t)slot * 2) * Ptot + off] = t;
+      p.partials[((size_t)slot * 2 + 1) * Ptot + off] = 0.f;
+    }
+  }
+  // scalar sums: policy 0..7, value 8..15, written by the CTA of their network; a network that does not run gets
+  // zeros from the CTA of the one that does
+  const bool other_runs = c == 0 ? run_v : run_p;
+  if (tid >= 32 && tid < 32 + 2 * B200RL_N_SCALARS && ((tid - 32) / B200RL_N_SCALARS == c || !other_runs)) {
+    const int s = tid - 32;
+    double t = 0.0;
+    if (s / B200RL_N_SCALARS == c) {
+      if (s < 6) {
+        for (int w = 0; w < T3_CHAIN_WARPS; ++w) t += e_sc[w * 8 + s];
+      } else if (s == 8) {
+        for (int w = 0; w < T3_CHAIN_WARPS; ++w) t += e_sc[w * 8 + 0];
+      }
+    }
+    p.scalar_partials[((size_t)slot * 2) * (2 * B200RL_N_SCALARS) + s] = t;
+    p.scalar_partials[((size_t)slot * 2 + 1) * (2 * B200RL_N_SCALARS) + s] = 0.0;
+  }
+  if (bad) *s_bad = 1;
+#ifdef B200RL_TC3_TIMING
+  if (tid == 0 && blockIdx.x == 0) {
+    g_tc3_t[53] = (unsigned long long)(t_loop0 - t_kernel0);      // setup
+    g_tc3_t[54] = (unsigned long long)(t_loop_end - t_loop0);     // tile loop (chain warpgroup 0)
+    g_tc3_t[55] = (unsigned long long)(clock64() - t_loop_end);   // read-out
+  }
+#endif
 
   // ---- teardown ----
   __syncthreads();
@@ -1234,13 +1167,14 @@ int launch_pack_obs(const float* obs, int64_t n_rows, int n_in, const float* abs
 
 int launch_mlp_tc3(const Tc3Args& k, cudaStream_t s) {
   if (tc3_configure()) return 1;
-  const int grid = tc_grid(k.n_rows);
+  const int grid = tc_grid(k.n_rows);  // tile slots: one accumulator block and one pair of partial rows each
   B200RL_REQUIRE(grid > 0, "mlp_tc3: no CUDA device");
   Tc3Args kk = k;
   kk.acc_mem = acc_mem(grid, s);
   B200RL_REQUIRE(kk.acc_mem != nullptr, "mlp_tc3: no accumulator memory (allocation failed, or the stream is being captured): %s",
                  cudaGetErrorString(cudaGetLastError()));
-  mlp_tc3_kernel<<<grid, T3_THREADS, T3_SMEM_BYTES, s>>>(kk);
+  // one CTA per (slot, network): 2 slot + c when both networks run
+  mlp_tc3_kernel<<<(k.run_policy && k.run_value) ? 2 * grid : grid, T3_THREADS, T3_SMEM_BYTES, s>>>(kk);
   B200RL_CUDA(cudaGetLastError());
   count_launch(1);
   return 0;

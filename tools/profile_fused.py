@@ -49,18 +49,15 @@ if __name__ == "__main__":
         lib.b200rl_debug_tc3_timing(out, 0)
         tiles = max(int(out[52]), 1)
         print("tiles of CTA 0:", tiles, "set-up", int(out[53]), "tile loop", int(out[54]), "read-out", int(out[55]), "cycles")
-        for wg in range(4):
+        # CTA 0: the policy network's CTA of slot 0 (the value network's when only the value network runs)
+        for wg in range(2):  # chain warpgroups: rows 0..63, 64..127
             wait = [int(out[10 * wg + s]) // tiles for s in range(5)]
             work = [(int(out[10 * wg + 5 + s]) - int(out[10 * wg + s])) // tiles for s in range(5)]
-            name = f"{'pv'[wg >> 1]}{wg & 1}"
-            print(f"chain {name} wait / tile:", dict(zip(("E1", "E2", "E3", "E4", "E5"), wait)), "sum", sum(wait))
-            print(f"chain {name} work / tile:", dict(zip(("E1", "E2", "E3", "E4", "E5"), work)), "sum", sum(work))
+            print(f"chain {wg} wait / tile:", dict(zip(("E1", "E2", "E3", "E4", "E5"), wait)), "sum", sum(wait))
+            print(f"chain {wg} work / tile:", dict(zip(("E1", "E2", "E3", "E4", "E5"), work)), "sum", sum(work))
         keys = ("dW3", "dW2", "dW1")
-        split = ("fragment loads", "fence .. wait_all", "stores + hand-over")
-        for c in range(2):  # one gradient warpgroup per network
-            wait = [int(out[40 + 3 * c + i]) // tiles for i in range(3)]
-            issue = [int(out[46 + 3 * c + i]) // tiles for i in range(3)]
-            name = "pv"[c]
-            print(f"gradient {name} wait  / tile:", dict(zip(keys, wait)), "sum", sum(wait))
-            print(f"gradient {name} issue / tile:", dict(zip(keys, issue)), "sum", sum(issue))
-            print(f"gradient {name} issue split / tile:", {k: int(out[56 + 3 * c + i]) // tiles for i, k in enumerate(split)})
+        for g in range(2):  # gradient warpgroups: the h and the l half of the stacked A operands
+            wait = [int(out[40 + 3 * g + i]) // tiles for i in range(3)]
+            issue = [int(out[46 + 3 * g + i]) // tiles for i in range(3)]
+            print(f"gradient {'hl'[g]} wait  / tile:", dict(zip(keys, wait)), "sum", sum(wait))
+            print(f"gradient {'hl'[g]} issue / tile:", dict(zip(keys, issue)), "sum", sum(issue))

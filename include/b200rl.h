@@ -340,7 +340,8 @@ typedef struct {
   int32_t max_minibatch;   /* capacity: rows per minibatch */
   int32_t max_steps;       /* capacity: train steps per call */
   int32_t algo;            /* 0 = DDPG / TD3 (by n_q), 1 = SAC (see b200rl_offpolicy_set_sac), 2 = DQN (see
-                            * b200rl_offpolicy_set_dqn), 3 = C51 (see b200rl_offpolicy_set_c51) */
+                            * b200rl_offpolicy_set_dqn), 3 = C51 (see b200rl_offpolicy_set_c51), 4 = IQN (created by
+                            * b200rl_offpolicy_create_iqn only; see "IQN" below) */
   int32_t dueling_k;       /* 0 = the Q network is a plain MLP; K >= 1 = a dueling Q network (algo 2 / 3 only; see
                             * "Dueling Q networks" below) */
   int32_t noisy_layers;    /* bit mask over the Q network's Linear layers in flat order: 0 = none; bit l = layer l is a
@@ -589,6 +590,67 @@ int b200rl_offpolicy_set_noise_keys(b200rl_offpolicy* h, const uint64_t* seed, c
 /* The raw N(0, 1) draws of the last train call's S steps: host eps [K, S, 2, E] (per step the online network's, then
  * the target's) -- what a test replays through the oracle. */
 int b200rl_offpolicy_get_noisy_draws(b200rl_offpolicy* h, int32_t S, float* eps);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * IQN on the same engine (config algo = 4, n_q = 1; Dabney, Ostrovski, Silver & Munos 2018): a DQN engine over an
+ * implicit quantile network.  Everything the DQN section says holds (networks, state blob, action column, hparams,
+ * target copies, outputs, invalid actions, graph, groups, prioritized replay, n-step returns;
+ * b200rl_offpolicy_set_dqn is required too) except the network and the loss.  An IQN engine is created by
+ * b200rl_offpolicy_create_iqn from a config with algo = 4 and the counts of a b200rl_iqn_config, which size its per-row
+ * buffers; b200rl_offpolicy_create and create_group refuse algo 4.  With n_cos, N = n, N' = n_target and K = k (each
+ * 1..256) and the q description [obs, d, h, n_actions] (3 layers, hidden_act between layers, out_act identity), in
+ * float32:
+ *   draws    step st of a call draws, per row b, N + N' + K fractions in the order online, target, argmax: draw
+ *            t = b (N + N' + K) + j is word t % 4 of Philox4x32-10(counter (t / 4, st, call, 0xB00), key seed) = r, and
+ *            tau = (2 (r >> 9) + 1) 2^-24, an odd multiple of 2^-24 in (0, 1), exact in float32.  (seed, call) come
+ *            from b200rl_offpolicy_set_noise_keys, which every train call of an IQN engine needs afresh; the domain
+ *            tag 0xB00 keeps these draws apart from the noisy networks' 0xA00.
+ *   features x_i = cospi(float32(i tau)), i = 0 .. n_cos - 1: the product i tau rounded once, then CUDA's cospif (at
+ *            most 1 ulp from cos(pi x)).  The draw kernel materialises them for the step's forward passes.
+ *   network  on R = B M rows (M fractions per row, network row b M + i for fraction i of row b):
+ *            psi = act(x W_psi^T + b_psi) [B, d], phi = act(cos W_phi^T + b_phi) [R, d] (two GEMMs),
+ *            z[b M + i] = psi[b] * phi[b M + i] (one float32 product per element),
+ *            Z = act(z W_h^T + b_h) W_out^T + b_out [R, n_actions] (two GEMMs).  Every GEMM is the engine's fp32
+ *            product with its k-sum in index order.  The flat parameter vector of networks 1 and 4 is W_psi [d, obs],
+ *            b_psi, W_phi [d, n_cos], b_phi, W_h [h, d], b_h, W_out [n_actions, h], b_out: torch's
+ *            parameters_to_vector of a module registering the embedding, the tau embedding and the head in this order.
+ *   passes   Q(s) with the N online fractions; Q_targ(s') once with the N' target and K argmax fractions of each row
+ *            (psi(s') shared); with double_q, Q(s') with the K argmax fractions.
+ *   a*       = argmax_a (sum_k Z(s', tau~_k, a)) / K over the argmax samples of Q (double_q = 1; at the start of the
+ *            step) or of Q_targ, the sum over k in index order (torch's argmax: a NaN wins, ties go to the first index)
+ *   target   T_j = r + (g (1 - d)) Z_targ(s', tau'_j, a*), g = gamma (n-step: the row's discount)
+ *   loss     u_ij = T_j - theta_i, theta_i = Z(s, tau_i, a); rho_ij = |tau_i - 1{u_ij < 0}| h(u_ij), h(u) = 0.5 u^2 if
+ *            |u| < 1 else |u| - 0.5 (kappa = 1); the row's L = (1/N') sum_i sum_j rho_ij, over j in index order, then
+ *            over i in index order; one Adam step (optimizer 1) on (1/B) sum_b L_b, summed in double in a fixed order
+ *   gradient dZ[b N + i, a] = -(sum_j |tau_i - 1{u_ij < 0}| clamp(u_ij, -1, 1)) / N' * w_b / B (w_b = 1 without
+ *            prioritized replay), 0 in every other column; the GEMMs' dW and dX modes with the activation derivatives
+ *            read from the layer outputs, and for the product dphi = dz * psi[b] and dpsi[b] = sum_i dz[b N + i] *
+ *            phi[b N + i] (each product rounded, the sum over i in index order).  No input gradient.
+ * q1_values logs (sum_i theta_i) / N.  Prioritized replay: the priority of row b is (L_b + eps)^alpha of its unweighted
+ * L_b, as for QR-DQN (non-finite: counted, and the call fails).  The head and every sum have a fixed order and no float
+ * atomics are used: a group's learners stay bit-identical to solo engines, learner z's draws being those of a solo
+ * engine given z's keys.  Launches per step: the draw 1, each forward pass 5, the head 1, the backward pass 7 (4
+ * weight-gradient GEMMs, 2 input-gradient GEMMs, the product's backward), Adam 1, the target copy 1: 21, 26 with
+ * double_q; a prioritized step adds its draw and priority update (2).  Runs as a CUDA graph, or as plain launches with
+ * B200RL_OFFPOLICY_GRAPH=0.
+ * Refused at create: create_iqn with another algo, algo 4 through create / create_group, or with dueling_k or
+ * noisy_layers; a count outside 1..256; a q description that is not 3 layers or whose out_act is not identity; too many actions for
+ * the head's shared memory; max_minibatch x max(N, N' + K) above 65535 x 32 network rows.  b200rl_offpolicy_set_qr
+ * refuses an IQN engine.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t n_cos;    /* cosine features of a fraction */
+  int32_t n;        /* N: fractions per row for Q(s) */
+  int32_t n_target; /* N': fractions per row for the target samples of Q_targ(s') */
+  int32_t k;        /* K: fractions per row for the argmax over actions */
+} b200rl_iqn_config;
+
+/* An IQN engine of n_learners learners (1 = a solo engine; 1 <= n_learners <= B200RL_MAX_LEARNERS): cfg->algo = 4. */
+int b200rl_offpolicy_create_iqn(const b200rl_offpolicy_config* cfg, const b200rl_iqn_config* iqn, int32_t n_learners,
+                                b200rl_offpolicy** out);
+/* The fractions of the last train call that ran steps: host taus [K, S, B, N + N' + K] (per row the online, target
+ * and argmax ones; B that call's minibatch) -- what a test replays through the oracle. */
+int b200rl_offpolicy_get_iqn_draws(b200rl_offpolicy* h, int32_t S, float* taus);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Learner groups: K independent off-policy learners (same config, same hyper-parameters, their own parameters, Adam

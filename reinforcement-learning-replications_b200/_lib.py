@@ -84,6 +84,10 @@ class OffPolicyConfig(C.Structure):
                 ("noisy_layers", C.c_int32)]
 
 
+class IqnConfig(C.Structure):
+    _fields_ = [("n_cos", C.c_int32), ("n", C.c_int32), ("n_target", C.c_int32), ("k", C.c_int32)]
+
+
 class SacHparams(C.Structure):
     _fields_ = [("alpha", C.c_double), ("target_entropy", C.c_double), ("alpha_lr", C.c_double),
                 ("alpha_beta1", C.c_double), ("alpha_beta2", C.c_double), ("alpha_eps", C.c_double),
@@ -193,6 +197,8 @@ SIGNATURES = {
     "b200rl_offpolicy_set_c51": (C.c_int, [C.c_void_p, C.POINTER(C51Hparams)]),
     "b200rl_offpolicy_set_qr": (C.c_int, [C.c_void_p, C.POINTER(QrHparams)]),
     "b200rl_offpolicy_create_group": (C.c_int, [C.POINTER(OffPolicyConfig), C.c_int32, C.POINTER(C.c_void_p)]),
+    "b200rl_offpolicy_create_iqn": (C.c_int, [C.POINTER(OffPolicyConfig), C.POINTER(IqnConfig), C.c_int32,
+                                              C.POINTER(C.c_void_p)]),
     "b200rl_offpolicy_train_gather_group": (C.c_int, [C.c_void_p, C.POINTER(OffPolicyHparams), C.c_int32, C.c_int32,
                                                       C.POINTER(OffPolicyReplay)] + [C.c_void_p] * 7 +
                                             [C.POINTER(C.c_int32), C.c_void_p]),
@@ -210,6 +216,7 @@ SIGNATURES = {
     "b200rl_offpolicy_get_nstep_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32] + [C.c_void_p] * 4),
     "b200rl_offpolicy_set_noise_keys": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200rl_offpolicy_get_noisy_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
+    "b200rl_offpolicy_get_iqn_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
     "b200rl_per_tree_floats": (C.c_int64, [C.c_int64]),
     "b200rl_per_tree_build": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p]),
     "b200rl_per_tree_set_range": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p]),

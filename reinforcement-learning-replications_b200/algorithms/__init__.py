@@ -1,6 +1,7 @@
 from .c51 import C51
 from .dqn import DQN
 from .group import LearnerGroup
+from .iqn import IQN
 from .ppo import PPO
 from .qrdqn import QRDQN
 from .sac import SAC
@@ -8,4 +9,4 @@ from .td3 import DDPG, TD3
 from .trpo import TRPO
 from .vpg import VPG
 
-__all__ = ["VPG", "TRPO", "PPO", "DDPG", "TD3", "SAC", "DQN", "C51", "QRDQN", "LearnerGroup"]
+__all__ = ["VPG", "TRPO", "PPO", "DDPG", "TD3", "SAC", "DQN", "C51", "QRDQN", "IQN", "LearnerGroup"]

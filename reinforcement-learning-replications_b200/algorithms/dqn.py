@@ -9,7 +9,7 @@ import torch
 
 from .._lib import OffPolicyHparams
 from ..engine import OffPolicyEngine
-from ..networks import DuelingMLP, NoisyLinear
+from ..networks import DuelingMLP, ImplicitQuantileMLP, NoisyLinear
 from ..policies import EpsilonGreedyPolicy, GreedyPolicy, NoisyGreedyPolicy
 from ..replay_buffer import PrioritizedReplayBuffer
 from ._onpolicy import _ACT_NAMES, adam_hparams, describe_mlp
@@ -19,7 +19,15 @@ from .td3 import _learn, _make_eval_env, _OffPolicyBase
 def describe_q_network(module):
     """(sizes, hidden activation, output activation, Linear layers in parameters() order, dueling K) of a DQN-family Q
     network: an ``MLP`` as ``describe_mlp`` reads it (K = 0), or a ``DuelingMLP`` with sizes [obs, h_trunk, h_stream,
-    n_actions * K] and its five Linear layers (trunk, value hidden, value out, advantage hidden, advantage out)."""
+    n_actions * K] and its five Linear layers (trunk, value hidden, value out, advantage hidden, advantage out), or an
+    ``ImplicitQuantileMLP`` with sizes [obs, d, h, n_actions] and its four (psi, phi, head hidden, head out; K = 0)."""
+    if isinstance(module, ImplicitQuantileMLP):
+        acts = {type(m) for m in (module.embedding[1], module.tau_embedding[1], module.head[1])}
+        if len(acts) != 1 or next(iter(acts)) not in _ACT_NAMES:
+            raise NotImplementedError(f"ImplicitQuantileMLP activations must be one of Tanh, ReLU, Identity throughout, "
+                                      f"got {sorted(a.__name__ for a in acts)}")
+        linears = [module.embedding[0], module.tau_embedding[0], module.head[0], module.head[2]]
+        return module.sizes + [module.n_actions], _ACT_NAMES[acts.pop()], "identity", linears, 0
     if not isinstance(module, DuelingMLP):
         return describe_mlp(module, allow_noisy=True) + (0,)
     acts = {type(m) for m in (module.trunk[1], module.value[1], module.advantage[1])}
@@ -148,15 +156,24 @@ class DQN(_OffPolicyBase):
     def _nets(self):
         return [self.q_function], [self.target_q_function]
 
-    def _ensure_engine(self, S: int, B: int) -> OffPolicyEngine:
+    def _engine_config(self):
+        """(Q network sizes, its (hidden, output) activations, the other OffPolicyEngine arguments) of this learner's
+        engine."""
         qsz, qact, qout, lins, dk = describe_q_network(self.q_function.network)
-        nm = noisy_mask(lins)
+        return qsz, (qact, qout), dict(dueling_k=dk, noisy_layers=noisy_mask(lins))
+
+    def _needs_draw_keys(self) -> bool:
+        """Whether every train call hands the engine (seed, call) keys for its device draws (set_noise_keys)."""
+        return self.noisy
+
+    def _ensure_engine(self, S: int, B: int) -> OffPolicyEngine:
+        qsz, qacts, kw = self._engine_config()
         e = getattr(self, "_engine", None)
-        if (e is None or e.q_sizes != qsz or e.max_minibatch < B or e.max_steps < S or e.q_acts != (qact, qout)
-                or e.dueling_k != dk or e.noisy_layers != nm):
+        if (e is None or e.q_sizes != qsz or e.max_minibatch < B or e.max_steps < S or e.q_acts != qacts
+                or any(getattr(e, k) != v for k, v in kw.items())):
             if e is not None:
                 e.close()
-            e = OffPolicyEngine(None, qsz, 1, B, S, q_acts=(qact, qout), algo=self.algo, dueling_k=dk, noisy_layers=nm)
+            e = OffPolicyEngine(None, qsz, 1, B, S, q_acts=qacts, algo=self.algo, **kw)
             self._engine = e
         return e
 
@@ -173,7 +190,7 @@ class DQN(_OffPolicyBase):
         e.set_dqn(self.target_update_interval, self.double_q)
 
     def _stage_inputs(self, replay_buffer, S: int, B: int, noisy: bool):
-        if self.noisy and S > 0:  # the weight noise's keys: this learner's own count of train calls
+        if self._needs_draw_keys() and S > 0:  # the device draws' keys: this learner's own count of train calls
             self._noise_calls = getattr(self, "_noise_calls", 0) + 1
             self.noise_key = (getattr(self, "device_rng_seed", 0), self._noise_calls)
         if self.n_step > 1:  # the windows are assembled on the device from the replay ring
@@ -202,7 +219,7 @@ class DQN(_OffPolicyBase):
         return mode, inputs
 
     def _call_engine(self, e, hp, replay_buffer, S: int, B: int, mode, inputs):
-        if mode is not None and self.noisy:
+        if mode is not None and self._needs_draw_keys():
             e.set_noise_keys(*([k] for k in self.noise_key))
         if mode is not None:
             e.set_nstep(self.n_step, [replay_buffer.device_episode_ends()] if self.n_step > 1 else None)

@@ -1,4 +1,4 @@
-"""LearnerGroup: several independent TD3 / DDPG / SAC / DQN / C51 / QR-DQN learners (typically one per seed) trained side by side by ONE
+"""LearnerGroup: several independent TD3 / DDPG / SAC / DQN / C51 / QR-DQN / IQN learners (typically one per seed) trained side by side by ONE
 off-policy engine, every operation of a train step one launch for all of them (b200rl_offpolicy_create_group).
 
 The contract: each member ends up bit for bit where it would be had it run alone.  Members keep everything of their
@@ -25,6 +25,7 @@ import torch
 
 from .._lib import MAX_LEARNERS
 from ..engine import OffPolicyEngine
+from ..networks import ImplicitQuantileMLP
 from ..replay_buffer import PrioritizedReplayBuffer
 from ._onpolicy import adam_hparams, describe_mlp
 from .dqn import describe_q_network, noisy_mask
@@ -36,13 +37,14 @@ def _signature(agent) -> list:
     """[(attribute, value)] that every member of a group shares (one engine trains them all), in the order in which a
     refusal reports the first difference."""
     trainable, _ = agent._nets()
-    dqn = agent.algo in (OffPolicyEngine.DQN, OffPolicyEngine.C51)
+    dqn = agent.algo in OffPolicyEngine.DISCRETE
     names = ["q_function"] if dqn else ["policy"] + (["q_function_1", "q_function_2"] if agent.n_q == 2 else ["q_function"])
     sig = [("class", type(agent).__name__)]
     for name, m in zip(names, trainable):
         if dqn:
             sizes, hidden_act, out_act, lins, k = describe_q_network(m.network)
-            sig.append((f"{name} network kind", "DuelingMLP" if k else "MLP"))
+            kind = type(m.network).__name__ if isinstance(m.network, ImplicitQuantileMLP) else "DuelingMLP" if k else "MLP"
+            sig.append((f"{name} network kind", kind))
             sig.append((f"{name} dueling (h_trunk, h_stream, outputs_per_action)", (sizes[1], sizes[2], k) if k else None))
             sig.append((f"{name} noisy layers", noisy_mask(lins)))
         else:
@@ -58,6 +60,7 @@ def _signature(agent) -> list:
             for attr in ("n_atoms", "v_min", "v_max"):
                 sig.append((attr, getattr(agent.q_function, attr)))
         sig.append(("n_quantiles", getattr(agent.q_function, "n_quantiles", None)))
+        sig.append(("IQN (n_cos, n_quantiles, n_target_quantiles, n_policy_quantiles)", getattr(agent, "iqn_config", None)))
         rb = getattr(agent, "replay_buffer", None)
         sig.append(("prioritized replay", isinstance(rb, PrioritizedReplayBuffer)))
         for attr in ("alpha", "eps", "beta_start", "beta_anneal_steps"):
@@ -114,7 +117,7 @@ class LearnerGroup:
     def add(self, agent) -> None:
         """Add ``agent``; the current state of the global random generators becomes its private stream."""
         if not isinstance(agent, _OffPolicyBase):
-            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or DQN / C51 / QR-DQN) learners, got {type(agent).__name__}")
+            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or DQN / C51 / QR-DQN / IQN) learners, got {type(agent).__name__}")
         if any(m is agent for m in self.members):
             raise ValueError("LearnerGroup: this agent is already a member")
         if len(self.members) >= MAX_LEARNERS:
@@ -152,22 +155,21 @@ class LearnerGroup:
 
     def _ensure_engine(self, S: int, B: int) -> OffPolicyEngine:
         m = self.members[0]
-        discrete = m.algo in (OffPolicyEngine.DQN, OffPolicyEngine.C51)
+        discrete = m.algo in OffPolicyEngine.DISCRETE
         if discrete:  # no policy network
             psz, pact, pout = None, "relu", "tanh"
-            qsz, qact, qout, lins, dk = describe_q_network(m.q_function.network)
-            nm = noisy_mask(lins)
+            qsz, (qact, qout), kw = m._engine_config()
         else:
             psz, pact, pout, _ = describe_mlp(m.policy.network)
             qsz, qact, qout, _ = describe_mlp(m._nets()[0][1].network)
-            dk = nm = 0
+            kw = dict(dueling_k=0, noisy_layers=0)
         e = self._engine
         if (e is None or e.K != len(self.members) or e.max_minibatch < B or e.max_steps < S or e.policy_sizes != psz
-                or e.q_sizes != qsz or e.policy_acts != (pact, pout) or e.q_acts != (qact, qout) or e.dueling_k != dk
-                or e.noisy_layers != nm):
+                or e.q_sizes != qsz or e.policy_acts != (pact, pout) or e.q_acts != (qact, qout)
+                or any(getattr(e, k) != v for k, v in kw.items())):
             self._close_engine()
             e = OffPolicyEngine(psz, qsz, m.n_q, B, S, (pact, pout), (qact, qout), algo=m.algo,
-                                n_learners=len(self.members), dueling_k=dk, noisy_layers=nm)
+                                n_learners=len(self.members), **kw)
             self._engine = e
         return e
 
@@ -202,7 +204,7 @@ class LearnerGroup:
         if sac:
             e.set_sac(members[0]._sac_hparams())
             e.set_alpha_group([m._alpha_state() for m in members])
-        if members[0].algo in (OffPolicyEngine.DQN, OffPolicyEngine.C51):
+        if members[0].algo in OffPolicyEngine.DISCRETE:
             e.set_dqn(members[0].target_update_interval, members[0].double_q)
         if members[0].algo == OffPolicyEngine.C51:
             q = members[0].q_function
@@ -210,9 +212,9 @@ class LearnerGroup:
         if isinstance(members[0], QRDQN):
             e.set_qr(members[0].q_function.n_quantiles)
         hp = members[0]._hparams(noisy, delay)
-        if getattr(members[0], "noisy", False):
+        if members[0].algo in OffPolicyEngine.DISCRETE and members[0]._needs_draw_keys():
             e.set_noise_keys(*zip(*[m.noise_key for m in members]))
-        if members[0].algo in (OffPolicyEngine.DQN, OffPolicyEngine.C51):
+        if members[0].algo in OffPolicyEngine.DISCRETE:
             n = members[0].n_step
             e.set_nstep(n, [m.replay_buffer.device_episode_ends() for m in members] if n > 1 else None)
         if mode == "per":

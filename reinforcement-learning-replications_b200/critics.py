@@ -96,3 +96,37 @@ class QuantileQFunction(_Critic):
 
     def forward(self, observation: Tensor) -> Tensor:
         return self.quantiles(observation).sum(-1) / self.n_quantiles
+
+
+class ImplicitQuantileQFunction(_Critic):
+    """The return distribution per action as a quantile function (IQN's critic): the network (an
+    ``ImplicitQuantileMLP``) maps an observation and fractions tau to Z(s, tau, a).  ``n_quantiles``,
+    ``n_target_quantiles`` and ``n_policy_quantiles`` are N, N' and K of the paper: the fractions a train step samples
+    per minibatch row for the online network, for the target network and for the argmax over actions.
+
+    ``forward`` returns Q(s, a) = the mean of Z over the K fixed midpoints (2k + 1) / (2K), [..., n_actions], so greedy
+    and epsilon-greedy policies and the evaluator use it as they use a ``DiscreteQFunction`` and evaluation is
+    deterministic.  The paper samples the K fractions when acting; sampled-fraction and risk-sensitive acting are not
+    implemented."""
+
+    MAX_QUANTILES = 256  # the engine's limit on N, N' and K (b200rl.h)
+
+    def __init__(self, network: nn.Module, optimizer: Optimizer, n_quantiles: int = 64, n_target_quantiles: int = 64,
+                 n_policy_quantiles: int = 32) -> None:
+        super().__init__(network, optimizer)
+        for name, v in (("n_quantiles", n_quantiles), ("n_target_quantiles", n_target_quantiles),
+                        ("n_policy_quantiles", n_policy_quantiles)):
+            if isinstance(v, bool) or int(v) != v or not 1 <= int(v) <= self.MAX_QUANTILES:
+                raise ValueError(f"{name} must be an integer from 1 to {self.MAX_QUANTILES}, got {v!r}")
+        self.n_quantiles, self.n_target_quantiles = int(n_quantiles), int(n_target_quantiles)
+        self.n_policy_quantiles = int(n_policy_quantiles)
+        K = self.n_policy_quantiles
+        self.policy_taus = torch.arange(1, 2 * K, 2, dtype=torch.float32) / torch.tensor(2 * K, dtype=torch.float32)
+
+    def quantiles(self, observation: Tensor, taus: Tensor) -> Tensor:
+        """Z(s, tau, a) [..., n_actions, M] at the fractions ``taus`` [..., M]."""
+        return self.network(observation, taus).transpose(-1, -2)
+
+    def forward(self, observation: Tensor) -> Tensor:
+        taus = self.policy_taus.expand(*observation.shape[:-1], self.n_policy_quantiles)
+        return self.quantiles(observation, taus).sum(-1) / self.n_policy_quantiles

@@ -29,6 +29,9 @@
 // Noisy networks (config noisy_layers, DQN / QR-DQN / C51, plain or dueling): noisy_compose_kernel draws both networks'
 // weight noise and composes their layers into the plain layout the GEMMs read at the start of each step, and
 // noisy_expand_kernel maps the composed layers' gradient to the noisy vector's before Adam.
+// IQN (config algo = 4) is DQN's step program over an implicit quantile network: iqn_draw_kernel draws the step's
+// fractions and their cosine features, iqn_forward / iqn_backward run the network on one row per fraction, and
+// iqn_loss_kernel is the loss head.
 // Prioritized replay for DQN (train_prioritized): a 32-way sum tree per replay buffer, drawn from, weighed and gathered
 // by per_draw_kernel and updated by per_update_kernel inside the same step program.
 // n-step returns for DQN / C51 (set_nstep): nstep_gather_kernel (or per_draw_kernel's NSTEP instantiation) walks each
@@ -1220,6 +1223,213 @@ __global__ void __launch_bounds__(QR_MAX_QUANTILES) qr_loss_kernel(
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// IQN (algo = 4; Dabney, Ostrovski, Silver & Munos 2018): DQN's step program over an implicit quantile network.  Every
+// minibatch row fans out into one network row per sampled fraction tau: Z(s, tau) = head(psi(s) * phi(cos(pi i tau))),
+// psi and the head plain GEMM layers, phi a GEMM layer over the fraction's cosine features (b200rl.h, "IQN").
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int IQN_MAX = 256;  // the largest n_cos, N, N' and K
+
+// The activations of one IQN forward pass on B rows with M fractions each (R = B M network rows)
+struct IqnPass {
+  float* psi;  // [B, d]
+  float* phi;  // [R, d]
+  float* z;    // [R, d]  psi(s) * phi(tau)
+  float* hid;  // [R, h]
+  float* out;  // [R, n]  Z(s, tau)
+};
+
+// Draw t of step st (t = b (N + N' + K) + j for row b's j-th fraction): lane t % 4 of Philox4x32-10(counter
+// (t / 4, st, call, 0xB00), key seed) = r, and tau = (2 (r >> 9) + 1) 2^-24, an odd multiple of 2^-24 in (0, 1)
+__device__ __forceinline__ float iqn_tau(long long t, int st, unsigned long long seed, unsigned long long call) {
+  const uint4 c = philox4x32_10(make_uint4((unsigned)(t >> 2), (unsigned)st, (unsigned)call, 0xB00u),
+                                make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
+  const int j = (int)(t & 3);  // selected, not indexed: c stays in registers
+  const unsigned r = j == 0 ? c.x : j == 1 ? c.y : j == 2 ? c.z : c.w;
+  return (float)(2u * (r >> 9) + 1u) * 5.9604644775390625e-8f;
+}
+
+// One thread per (draw t, feature i) of step st over the B rows' Mt = N + N' + K draws: tau goes to the call's record
+// (taus = the step's [B, Mt] slice; written by the i = 0 threads), x_i = cospi(float32(i tau)) to the rows of the
+// forward passes that read it: an online draw (j < N) to cos_q row b N + j; a target or argmax draw to cos_t row
+// b (N' + K) + j - N; an argmax draw (j >= N + N') also to cos_n row b K + j - N - N' (Double DQN's Q(s')).
+template <bool LANES>
+__global__ void iqn_draw_kernel(int B, int N, int Nt, int K, int n_cos, const unsigned long long* keys, int st,
+                                float* taus, float* cos_q, float* cos_t, float* cos_n, size_t lane_stride) {
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    keys = lane_ptr(keys, o), taus = lane_ptr(taus, o), cos_q = lane_ptr(cos_q, o), cos_t = lane_ptr(cos_t, o);
+    cos_n = lane_ptr(cos_n, o);
+  }
+  const int Mt = N + Nt + K;
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= (long long)B * Mt * n_cos) return;
+  const long long t = e / n_cos;
+  const int i = (int)(e - t * n_cos);
+  const float tau = iqn_tau(t, st, keys[0], keys[1]);
+  if (i == 0) taus[t] = tau;
+  const float x = cospif(__fmul_rn((float)i, tau));
+  const long long b = t / Mt;
+  const int j = (int)(t - b * Mt);
+  if (j < N) {
+    cos_q[(b * N + j) * n_cos + i] = x;
+  } else {
+    cos_t[(b * (Nt + K) + j - N) * n_cos + i] = x;
+    if (j >= N + Nt) cos_n[(b * K + j - N - Nt) * n_cos + i] = x;
+  }
+}
+
+// z[r, c] = psi[r / M, c] * phi[r, c] over the R = B M rows of width d: one float32 product per element
+template <bool LANES>
+__global__ void iqn_mul_kernel(const float* psi, const float* phi, long long R, int M, int d, float* z,
+                               size_t lane_stride) {
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    psi = lane_ptr(psi, o), phi = lane_ptr(phi, o), z = lane_ptr(z, o);
+  }
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= R * d) return;
+  const long long r = e / d;
+  const int c = (int)(e - r * d);
+  z[e] = __fmul_rn(psi[(r / M) * d + c], phi[e]);
+}
+
+// The product's backward pass, one thread per (row b, column c) over its N online rows:
+//   dphi[b N + i, c] = dz[b N + i, c] psi[b, c],  dpsi[b, c] = sum_i dz[b N + i, c] phi[b N + i, c]
+// the sum over i in index order, every product rounded before it is added.
+template <bool LANES>
+__global__ void iqn_mul_backward_kernel(const float* dz, const float* psi, const float* phi, int B, int N, int d,
+                                        float* dphi, float* dpsi, size_t lane_stride) {
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    dz = lane_ptr(dz, o), psi = lane_ptr(psi, o), phi = lane_ptr(phi, o), dphi = lane_ptr(dphi, o);
+    dpsi = lane_ptr(dpsi, o);
+  }
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= B * d) return;
+  const int b = e / d, c = e - b * d;
+  const float p = psi[e];
+  float s = 0.f;
+  for (int i = 0; i < N; ++i) {
+    const size_t at = ((size_t)b * N + i) * d + c;
+    const float g = dz[at];
+    dphi[at] = __fmul_rn(g, p);
+    s = __fadd_rn(s, __fmul_rn(g, phi[at]));
+  }
+  dpsi[e] = s;
+}
+
+// shared-memory floats of one row's head: T_j and then the samples' loss sums, theta(s, tau_i, a), the argmax means
+__host__ __device__ __forceinline__ int iqn_smem_floats(int n, int N, int Nt) { return (N > Nt ? N : Nt) + N + n; }
+
+// One CTA per row i with action a = act[i] (grid = B rows per learner), thread t owning online sample t (blockDim = N
+// rounded up to whole warps; every sum below runs in index order, no float atomics).  q = Z(s) [B N, n], qt_next =
+// Q_targ(s') [B (N' + K), n] (per row its N' target samples, then its K argmax samples), qn = Double DQN's Q(s')
+// [B K, n] or NULL, taus = the step's fractions [B, N + N' + K] (the online ones first).
+//   a* = argmax_a (sum_k Z(s', tau~_k, a)) / K over the argmax samples of qn, or of qt_next without Double DQN,
+//   T_j = r + gamma (1 - d) Z_targ(s', tau'_j, a*), u_tj = T_j - theta_t with theta_t = Z(s, tau_t, a),
+//   k_tj = |tau_t - 1{u_tj < 0}|, h(u) = 0.5 u^2 if |u| < 1 else |u| - 0.5,
+//   L = (1/N') sum_t sum_j k_tj h(u_tj)  (j, then t),
+//   dOut[i N + t, a] = -(sum_j k_tj clamp(u_tj, -1, 1)) / N' * (1 / B) and 0 in every other column of the row's N
+//   online rows, q_copy[i] = (sum_t theta_t) / N.
+// Invalid actions, the row losses, the counters, WEIGHTED and NSTEP as in qr_loss_kernel.
+template <bool LANES, bool WEIGHTED, bool NSTEP>
+__global__ void __launch_bounds__(IQN_MAX) iqn_loss_kernel(
+    const float* q, const float* qt_next, const float* qn, const float* taus, const float* act, const float* rew,
+    const float* done, const float* disc, float gamma, int B, int n, int N, int Nt, int K, float* dout,
+    float* row_loss, float* q_copy, int* sync, float* loss_out, int* bad_out, const float* w, float* absd,
+    size_t lane_stride) {
+  extern __shared__ float iqn_smem[];
+  __shared__ double red[32];
+  __shared__ bool last;
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q = lane_ptr(q, o), qt_next = lane_ptr(qt_next, o), qn = lane_ptr(qn, o), taus = lane_ptr(taus, o);
+    act = lane_ptr(act, o), rew = lane_ptr(rew, o), done = lane_ptr(done, o), dout = lane_ptr(dout, o);
+    row_loss = lane_ptr(row_loss, o), q_copy = lane_ptr(q_copy, o), sync = lane_ptr(sync, o);
+    loss_out = lane_ptr(loss_out, o), bad_out = lane_ptr(bad_out, o);
+    if (WEIGHTED) w = lane_ptr(w, o), absd = lane_ptr(absd, o);
+    if (NSTEP) disc = lane_ptr(disc, o);
+  }
+  const int t = threadIdx.x, i = blockIdx.x;
+  float* st = iqn_smem;                // T_j, then each online sample's loss sum
+  float* sth = st + (N > Nt ? N : Nt);  // theta(s, tau_t, a)
+  float* sq = sth + N;                 // the argmax samples' means per action
+  const float af = act[i];
+  const bool valid = af >= 0.f && af < (float)n && af == floorf(af);  // false for NaN
+  const int a = valid ? (int)af : -1;
+  float* drow = dout + (size_t)i * N * n;
+  for (int c = t; c < N * n; c += blockDim.x)
+    if (c % n != a) drow[c] = 0.f;
+  if (!valid) {
+    if (t == 0) {
+      q_copy[i] = __int_as_float(0x7fc00000);
+      row_loss[i] = 0.f;
+      if (WEIGHTED) absd[i] = -1.f;
+      atomicAdd(sync + 1, 1);
+    }
+  } else {
+    const float th = t < N ? q[((size_t)i * N + t) * n + a] : 0.f;
+    if (t < N) sth[t] = th;
+    const float* an = qn != nullptr ? qn + (size_t)i * K * n : qt_next + ((size_t)i * (Nt + K) + Nt) * n;
+    for (int c = t; c < n; c += blockDim.x) {
+      float s = 0.f;
+      for (int k = 0; k < K; ++k) s += an[(size_t)k * n + c];
+      sq[c] = s / (float)K;
+    }
+    __syncthreads();
+    const int a_star = argmax_row(sq, n);
+    const float g1d = (NSTEP ? disc[i] : gamma) * (1.f - done[i]), r = rew[i];
+    const float* tq = qt_next + (size_t)i * (Nt + K) * n + a_star;
+    for (int j = t; j < Nt; j += blockDim.x) st[j] = r + g1d * tq[(size_t)j * n];
+    __syncthreads();
+    float lsum = 0.f, gsum = 0.f;
+    if (t < N) {
+      const float tau = taus[(size_t)i * (N + Nt + K) + t];
+      for (int j = 0; j < Nt; ++j) {
+        const float u = st[j] - th;
+        const float k = fabsf(tau - (u < 0.f ? 1.f : 0.f));
+        const float au = fabsf(u);
+        const float hu = au < 1.f ? 0.5f * u * u : au - 0.5f;
+        const float c = u > 1.f ? 1.f : (u < -1.f ? -1.f : u);  // NaN passes through, as torch's clamp lets it
+        lsum += k * hu;
+        gsum += k * c;
+      }
+    }
+    __syncthreads();  // every thread is done with T
+    const float inv = 1.0f / (float)B;  // dqn_loss_kernel's scaling
+    const float wi = WEIGHTED ? w[i] : 1.f;
+    if (t < N) {
+      st[t] = lsum;
+      const float g = -gsum / (float)Nt;
+      drow[(size_t)t * n + a] = (WEIGHTED ? wi * g : g) * inv;
+    }
+    __syncthreads();
+    if (t == 0) {
+      float L = 0.f, qv = 0.f;
+      for (int k = 0; k < N; ++k) L += st[k], qv += sth[k];
+      L /= (float)Nt;
+      q_copy[i] = qv / (float)N;
+      row_loss[i] = WEIGHTED ? wi * L : L;
+      if (WEIGHTED) absd[i] = L;
+    }
+  }
+  // the last CTA of this learner reads every row's loss
+  __threadfence();
+  __syncthreads();
+  if (t == 0) last = atomicAdd(sync, 1) == (int)gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double acc = 0.0;
+  for (int r = t; r < B; r += blockDim.x) acc += (double)__ldcg(row_loss + r);
+  block_mean(acc, B, loss_out, red);
+  if (t == 0) {
+    *bad_out = atomicExch(sync + 1, 0);
+    sync[0] = 0;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // Prioritized experience replay (Schaul et al. 2016, proportional variant).  A sum tree over the physical rows of a
 // replay buffer with 32 children per node, all levels in one float array (b200rl.h, b200rl_per_tree_floats): level 0
 // holds the leaves, level k + 1 the sums of 32 consecutive nodes of level k, every level padded with zeros to a multiple
@@ -1456,7 +1666,8 @@ struct NetBuf {
   // dueling Q network (config dueling_k = K > 0; d = [obs, h1, h2, n K]): its five Linear layers' offsets, in the
   // order trunk, value hidden, value out, advantage hidden, advantage out
   int duel_k = 0;
-  int dw_off[5] = {}, db_off[5] = {};
+  int dw_off[5] = {}, db_off[5] = {};  // an IQN network (config algo = 4) keeps its four layers' offsets here too: psi,
+                                       // phi, head hidden, head out
   // the vector set_params / get_params, the state blob, Adam and the target copy work on, P_flat floats: params /
   // grad themselves, except for networks 1 and 4 of an engine with noisy layers, where params / grad hold the composed
   // network the GEMMs read and flat / flat_grad the noisy vector (noisy_compose_kernel, noisy_expand_kernel)
@@ -1563,6 +1774,15 @@ struct b200rl_offpolicy {
   bool noisy = false, noisy_keys = false;
   NoisyLayout noisy_lay{};
   float* noisy_draws = nullptr;  // [max_steps][2][E] raw draws of the call's steps (online, target)
+  // IQN (cfg.algo == 4): a DQN engine (h->dqn is set) over an implicit quantile network; its draws take their keys from
+  // set_noise_keys, in the adam_tab slot a noisy engine's keys take
+  bool iqn = false;
+  b200rl_iqn_config iqn_cfg{};         // n_cos, N, N', K
+  int iqn_last_B = 0;                  // the minibatch of the last call that ran steps (0: none yet)
+  float* iqn_taus = nullptr;           // [max_steps][B][N + N' + K] fractions of the call's steps
+  float *iqn_cos_q = nullptr, *iqn_cos_t = nullptr, *iqn_cos_n = nullptr;  // the step's cosine features (iqn_draw_kernel)
+  IqnPass iqn_pass[3] = {};            // Q(s) with N, Q_targ(s') with N' + K, Q(s') with K fractions per row
+  float *iqn_dhid = nullptr, *iqn_dz = nullptr, *iqn_dphi = nullptr, *iqn_dpsi = nullptr;  // the backward pass's
   // the replay columns, episode-end columns, trees and row counts of this call (train_gather[_rng], train_prioritized)
   ReplayLanes<true> replay{};
   std::vector<void*> allocs;
@@ -1573,9 +1793,9 @@ namespace {
 inline int64_t state_pad(int64_t n) { return (n + 63) & ~(int64_t)63; }
 
 // float2 entries of one learner's adam_tab: the Adam scalar rows (+ SAC's temperature row or DQN's copy flags), then
-// DQN's prioritized (seed, call) at 4 max_steps and a noisy engine's noise (seed, call) after it
+// DQN's prioritized (seed, call) at 4 max_steps and a noisy or IQN engine's draw keys (seed, call) after it
 inline size_t adam_tab_len(const b200rl_offpolicy* h) {
-  return (h->sac || h->dqn ? 4 : 3) * (size_t)h->cfg.max_steps + (h->dqn ? 2 : 0) + (h->noisy ? 2 : 0);
+  return (h->sac || h->dqn ? 4 : 3) * (size_t)h->cfg.max_steps + (h->dqn ? 2 : 0) + (h->noisy || h->iqn ? 2 : 0);
 }
 
 // A piece of the learner arena: recorded here (256-byte aligned), placed by arena_commit
@@ -1809,6 +2029,72 @@ int dueling_backward(b200rl_offpolicy* h, const NetBuf& nb, float* const* acts, 
   return 0;
 }
 
+// An IQN network (nb.d = [obs, d, h, n]) on x [B, obs] and the cosine features cos [B M, n_cos] of M fractions per
+// row: psi, phi, their product and the head's two layers into p, 5 launches.
+int iqn_forward(const b200rl_offpolicy* h, const NetBuf& nb, const float* x, const float* cos, int B, int M,
+                const IqnPass& p, cudaStream_t s) {
+  const int O = nb.d.sizes[0], D = nb.d.sizes[1], H = nb.d.sizes[2], n = nb.d.sizes[3], C = h->iqn_cfg.n_cos;
+  const int R = B * M, hid = nb.d.hidden_act;
+  auto layer = [&](int l, const float* X, int rows, int nin, float* Y, int nout, int act) {
+    GemmArgs g{};
+    g.A = X; g.lda = nin;
+    g.B = nb.params + nb.dw_off[l]; g.ldb = nin;
+    g.C = Y; g.ldc = nout;
+    g.bias = nb.params + nb.db_off[l];
+    g.act = act;
+    g.M = rows; g.N = nout; g.K = nin;
+    return gemm<0>(h, g, s);
+  };
+  if (layer(0, x, B, O, p.psi, D, hid) || layer(1, cos, R, C, p.phi, D, hid)) return 1;
+  if (launch(h, iqn_mul_kernel<false>, iqn_mul_kernel<true>, (unsigned)(((long long)R * D + GTHREADS - 1) / GTHREADS),
+             GTHREADS, 0, s, p.psi, p.phi, (long long)R, M, D, p.z))
+    return 1;
+  return layer(2, p.z, R, D, p.hid, H, hid) || layer(3, p.hid, R, H, p.out, n, nb.d.out_act);
+}
+
+// Its backward pass from dOut = dL/dZ [B N, n] into nb.grad, 7 launches: the dX chain (dhid, dz, the product's
+// backward) on `s`, the four weight-gradient products on s_dw behind the gradient they read.  No input gradient.
+int iqn_backward(b200rl_offpolicy* h, const NetBuf& nb, const float* x, const float* cos, int B, const IqnPass& p,
+                 const float* dOut, cudaStream_t s, cudaStream_t s_dw) {
+  const int O = nb.d.sizes[0], D = nb.d.sizes[1], H = nb.d.sizes[2], n = nb.d.sizes[3], C = h->iqn_cfg.n_cos;
+  const int N = h->iqn_cfg.n, R = B * N, hid = nb.d.hidden_act;
+  auto fork = [&]() {  // what `s` has queued so far is complete before the next products on s_dw
+    B200RL_CUDA(cudaEventRecord(h->ev_side, s));
+    B200RL_CUDA(cudaStreamWaitEvent(s_dw, h->ev_side, 0));
+    return 0;
+  };
+  // dW[nout, nin] = (dY . act'(Y))^T X and db on s_dw
+  auto dw = [&](int l, const float* dY, const float* Y, int act, const float* X, int rows, int nout, int nin) {
+    GemmArgs g{};
+    g.A = dY; g.lda = nout; g.Y = Y; g.ldy = nout; g.act = act;
+    g.B = X; g.ldb = nin;
+    g.C = nb.grad + nb.dw_off[l]; g.ldc = nin;
+    g.M = nout; g.N = nin; g.K = rows;
+    g.dbias = nb.grad + nb.db_off[l];
+    return gemm<2>(h, g, s_dw);
+  };
+  // dX[R, nin] = (dY . act'(Y))[R, nout] W[nout, nin] on s
+  auto dx = [&](int l, const float* dY, const float* Y, int act, float* dst, int nout, int nin) {
+    GemmArgs g{};
+    g.A = dY; g.lda = nout; g.Y = Y; g.ldy = nout; g.act = act;
+    g.B = nb.params + nb.dw_off[l]; g.ldb = nin;
+    g.C = dst; g.ldc = nin;
+    g.M = R; g.N = nin; g.K = nout;
+    return gemm<1>(h, g, s);
+  };
+  const int idt = B200RL_ACT_IDENTITY;
+  if (fork() || dw(3, dOut, nullptr, idt, p.hid, R, n, H) || dx(3, dOut, nullptr, idt, h->iqn_dhid, n, H)) return 1;
+  if (fork() || dw(2, h->iqn_dhid, p.hid, hid, p.z, R, H, D) || dx(2, h->iqn_dhid, p.hid, hid, h->iqn_dz, H, D))
+    return 1;
+  if (launch(h, iqn_mul_backward_kernel<false>, iqn_mul_backward_kernel<true>, (unsigned)((B * D + GTHREADS - 1) / GTHREADS),
+             GTHREADS, 0, s, h->iqn_dz, p.psi, p.phi, B, N, D, h->iqn_dphi, h->iqn_dpsi))
+    return 1;
+  if (fork() || dw(1, h->iqn_dphi, p.phi, hid, cos, R, D, C) || dw(0, h->iqn_dpsi, p.psi, hid, x, B, D, O)) return 1;
+  B200RL_CUDA(cudaEventRecord(h->ev_side, s_dw));
+  B200RL_CUDA(cudaStreamWaitEvent(s, h->ev_side, 0));
+  return 0;
+}
+
 int adam_net(const b200rl_offpolicy* h, NetBuf& nb, const float2* table, int idx, double b1, double b2, double eps,
              cudaStream_t s) {
   return adam_step_table(nb.flat, nb.flat_grad, nb.m, nb.v, nb.P_flat, table, idx, b1, b2, eps, s, h->K,
@@ -1817,19 +2103,20 @@ int adam_net(const b200rl_offpolicy* h, NetBuf& nb, const float2* table, int idx
 
 }  // namespace
 
-extern "C" int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200rl_offpolicy** out) {
-  return b200rl_offpolicy_create_group(cfg, 1, out);
-}
-
-extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg, int32_t n_learners,
-                                             b200rl_offpolicy** out) {
+// The engine of create_group (ic = NULL) and of create_iqn (ic = the IQN counts, config algo 4)
+static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_config* ic, int32_t n_learners,
+                         b200rl_offpolicy** out) {
   B200RL_REQUIRE(cfg && out, "offpolicy_create: NULL argument");
   B200RL_REQUIRE(n_learners >= 1 && n_learners <= B200RL_MAX_LEARNERS,
                  "offpolicy_create_group: n_learners must be 1..%d, got %d", B200RL_MAX_LEARNERS, n_learners);
   B200RL_REQUIRE(cfg->n_q == 1 || cfg->n_q == 2, "offpolicy_create: n_q must be 1 (DDPG) or 2 (TD3)");
-  B200RL_REQUIRE(cfg->algo >= 0 && cfg->algo <= 3,
-                 "offpolicy_create: algo must be 0 (DDPG / TD3), 1 (SAC), 2 (DQN) or 3 (C51), got %d", cfg->algo);
-  const bool sac = cfg->algo == 1, c51 = cfg->algo == 3, dqn = cfg->algo == 2 || c51;  // C51 is a DQN engine
+  B200RL_REQUIRE((cfg->algo >= 0 && cfg->algo <= 3) || (cfg->algo == 4 && ic != nullptr),
+                 "offpolicy_create: algo must be 0 (DDPG / TD3), 1 (SAC), 2 (DQN) or 3 (C51), got %d (algo 4, IQN, is "
+                 "created by b200rl_offpolicy_create_iqn with its counts)", cfg->algo);
+  B200RL_REQUIRE(ic == nullptr || cfg->algo == 4, "offpolicy_create_iqn: the config's algo must be 4 (IQN), got %d",
+                 cfg->algo);
+  const bool sac = cfg->algo == 1, c51 = cfg->algo == 3, iqn = cfg->algo == 4;
+  const bool dqn = cfg->algo == 2 || c51 || iqn;  // C51 and IQN are DQN engines
   B200RL_REQUIRE(!sac || cfg->n_q == 2, "offpolicy_create: SAC needs n_q = 2 (twin soft critics), got %d", cfg->n_q);
   B200RL_REQUIRE(!dqn || cfg->n_q == 1, "offpolicy_create: DQN needs n_q = 1 (one Q network), got %d", cfg->n_q);
   B200RL_REQUIRE(cfg->max_minibatch >= 1 && cfg->max_minibatch <= 65536 && cfg->max_steps >= 1,
@@ -1857,6 +2144,27 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
     Pq = (int64_t)d.sizes[1] * (d.sizes[0] + 1) + 2 * (int64_t)d.sizes[2] * (d.sizes[1] + 1) +
          (int64_t)(DK + d.sizes[3]) * (d.sizes[2] + 1);
   }
+  const int IC = iqn ? ic->n_cos : 0, IN = iqn ? ic->n : 0, INt = iqn ? ic->n_target : 0, IK = iqn ? ic->k : 0;
+  if (iqn) {
+    const b200rl_mlp_desc& d = cfg->q;
+    B200RL_REQUIRE(DK == 0 && cfg->noisy_layers == 0, "offpolicy_create: IQN takes neither dueling_k nor noisy_layers: "
+                   "dueling and noisy IQN networks are not implemented");
+    B200RL_REQUIRE(IC >= 1 && IC <= IQN_MAX && IN >= 1 && IN <= IQN_MAX && INt >= 1 && INt <= IQN_MAX && IK >= 1 &&
+                   IK <= IQN_MAX, "offpolicy_create: the IQN counts n_cos, n, n_target and k must each be 1..%d, got "
+                   "%d, %d, %d, %d", IQN_MAX, IC, IN, INt, IK);
+    B200RL_REQUIRE(d.n_layers == 3, "offpolicy_create: an IQN network is described as [obs, d, h, n_actions] (3 "
+                   "layers), got %d layers", d.n_layers);
+    B200RL_REQUIRE(d.out_act == B200RL_ACT_IDENTITY, "offpolicy_create: an IQN network's output must be linear "
+                   "(out_act identity)");
+    B200RL_REQUIRE(iqn_smem_floats(d.sizes[3], IN, INt) <= C51_SMEM_FLOATS, "offpolicy_create: %d actions are too "
+                   "many for the IQN head's shared memory", d.sizes[3]);
+    B200RL_REQUIRE((long long)cfg->max_minibatch * std::max(IN, INt + IK) <= 65535LL * GT, "offpolicy_create: "
+                   "max_minibatch %d x %d fractions per row exceed the %lld network rows of one pass",
+                   cfg->max_minibatch, std::max(IN, INt + IK), 65535LL * GT);
+    // psi, phi, head hidden, head out
+    Pq = (int64_t)d.sizes[1] * (d.sizes[0] + 1) + (int64_t)d.sizes[1] * (IC + 1) +
+         (int64_t)d.sizes[2] * (d.sizes[1] + 1) + (int64_t)d.sizes[3] * (d.sizes[2] + 1);
+  }
   const unsigned NM = (unsigned)cfg->noisy_layers;
   const int n_lin = DK != 0 ? 5 : cfg->q.n_layers;  // the Q network's Linear layers in flat order
   B200RL_REQUIRE(NM == 0 || dqn, "offpolicy_create: noisy_layers must be 0 unless algo = 2 (DQN / QR-DQN) or 3 (C51), "
@@ -1879,6 +2187,8 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
   h->sac = sac;
   h->dqn = dqn;
   h->c51 = c51;
+  h->iqn = iqn;
+  if (iqn) h->iqn_cfg = *ic;
   h->noisy = NM != 0;
   int rc = 0;
   int maxw = O + A;
@@ -1906,6 +2216,17 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
         off += outs[l];
       }
       maxw = std::max(maxw, std::max(2 * h2, DK + nK));
+    }
+    if (iqn && (i == 1 || i == 4)) {
+      const int ins[4] = {nb.d.sizes[0], IC, nb.d.sizes[1], nb.d.sizes[2]};
+      const int outs[4] = {nb.d.sizes[1], nb.d.sizes[1], nb.d.sizes[2], nb.d.sizes[3]};
+      off = 0;
+      for (int l = 0; l < 4; ++l) {
+        nb.dw_off[l] = off;
+        off += outs[l] * ins[l];
+        nb.db_off[l] = off;
+        off += outs[l];
+      }
     }
     nb.P_flat = nb.P;
     if (NM != 0 && (i == 1 || i == 4)) {  // the noisy vector: [W_mu, W_sigma, b_mu, b_sigma] per noisy layer, [W, b] else
@@ -1988,7 +2309,7 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
     rc |= oalloc(h, &h->out_logp, S);
   }
   if (dqn) {
-    rc |= oalloc(h, &h->dqn_dout, B * (size_t)cfg->q.sizes[cfg->q.n_layers]);
+    rc |= oalloc(h, &h->dqn_dout, B * (size_t)cfg->q.sizes[cfg->q.n_layers] * (iqn ? IN : 1));
     rc |= oalloc(h, &h->dqn_bad, S);
     rc |= oalloc(h, &h->per_w, S * B);
     rc |= oalloc(h, &h->per_newp, S * B);
@@ -2000,6 +2321,27 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
     rc |= oalloc(h, &h->c51_sync, 2);
   }
   if (c51) rc |= oalloc(h, &h->c51_support, C51_MAX_ATOMS);
+  if (iqn) {
+    const size_t D = cfg->q.sizes[1], H = cfg->q.sizes[2], n = cfg->q.sizes[3];
+    rc |= oalloc(h, &h->iqn_taus, S * B * (IN + INt + IK));
+    rc |= oalloc(h, &h->iqn_cos_q, B * IN * (size_t)IC);
+    rc |= oalloc(h, &h->iqn_cos_t, B * (INt + IK) * (size_t)IC);
+    rc |= oalloc(h, &h->iqn_cos_n, B * IK * (size_t)IC);
+    const int M[3] = {IN, INt + IK, IK};
+    for (int k = 0; k < 3; ++k) {
+      const size_t R = B * M[k];
+      IqnPass& p = h->iqn_pass[k];
+      rc |= oalloc(h, &p.psi, B * D);
+      rc |= oalloc(h, &p.phi, R * D);
+      rc |= oalloc(h, &p.z, R * D);
+      rc |= oalloc(h, &p.hid, R * H);
+      rc |= oalloc(h, &p.out, R * n);
+    }
+    rc |= oalloc(h, &h->iqn_dhid, B * IN * H);
+    rc |= oalloc(h, &h->iqn_dz, B * IN * D);
+    rc |= oalloc(h, &h->iqn_dphi, B * IN * D);
+    rc |= oalloc(h, &h->iqn_dpsi, B * D);
+  }
   rc |= arena_commit(h);
   if (rc == 0) {
     float* q = h->state;
@@ -2034,6 +2376,21 @@ extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg,
   }
   *out = h;
   return 0;
+}
+
+extern "C" int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200rl_offpolicy** out) {
+  return create_engine(cfg, nullptr, 1, out);
+}
+
+extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg, int32_t n_learners,
+                                             b200rl_offpolicy** out) {
+  return create_engine(cfg, nullptr, n_learners, out);
+}
+
+extern "C" int b200rl_offpolicy_create_iqn(const b200rl_offpolicy_config* cfg, const b200rl_iqn_config* iqn,
+                                           int32_t n_learners, b200rl_offpolicy** out) {
+  B200RL_REQUIRE(iqn, "offpolicy_create_iqn: NULL IQN counts");
+  return create_engine(cfg, iqn, n_learners, out);
 }
 
 extern "C" void b200rl_offpolicy_destroy(b200rl_offpolicy* h) {
@@ -2189,7 +2546,7 @@ extern "C" int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hp
 
 extern "C" int b200rl_offpolicy_set_qr(b200rl_offpolicy* h, const b200rl_qr_hparams* qp) {
   B200RL_REQUIRE(h && qp, "offpolicy_set_qr: NULL argument");
-  B200RL_REQUIRE(h->dqn && !h->c51, "offpolicy_set_qr: the engine was not created with algo = 2 (DQN)");
+  B200RL_REQUIRE(h->dqn && !h->c51 && !h->iqn, "offpolicy_set_qr: the engine was not created with algo = 2 (DQN)");
   const int N = qp->n_quantiles, width = h->net[1].d.sizes[h->net[1].d.n_layers];
   B200RL_REQUIRE(N >= 1 && N <= QR_MAX_QUANTILES, "offpolicy_set_qr: n_quantiles must be 1..%d, got %d",
                  QR_MAX_QUANTILES, N);
@@ -2237,7 +2594,8 @@ extern "C" int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, c
 
 extern "C" int b200rl_offpolicy_set_noise_keys(b200rl_offpolicy* h, const uint64_t* seed, const uint64_t* call) {
   B200RL_REQUIRE(h && seed && call, "offpolicy_set_noise_keys: NULL argument");
-  B200RL_REQUIRE(h->noisy, "offpolicy_set_noise_keys: the engine has no noisy layers (config noisy_layers = 0)");
+  B200RL_REQUIRE(h->noisy || h->iqn, "offpolicy_set_noise_keys: the engine has no noisy layers (config noisy_layers = "
+                 "0)");
   const size_t n = adam_tab_len(h);
   for (int z = 0; z < h->K; ++z) {  // uploaded with the table by run_staged
     unsigned long long* keys = reinterpret_cast<unsigned long long*>(h->h_adam_tab + z * n + n - 2);
@@ -2252,6 +2610,16 @@ extern "C" int b200rl_offpolicy_get_noisy_draws(b200rl_offpolicy* h, int32_t S, 
   B200RL_REQUIRE(h->noisy, "offpolicy_get_noisy_draws: the engine has no noisy layers (config noisy_layers = 0)");
   const size_t w = (size_t)S * 2 * h->noisy_lay.E * 4;
   if (w) B200RL_CUDA(cudaMemcpy2DAsync(eps, w, h->noisy_draws, h->lane_stride, w, h->K, cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_get_iqn_draws(b200rl_offpolicy* h, int32_t S, float* taus) {
+  B200RL_REQUIRE(h && taus && S >= 0 && S <= h->cfg.max_steps, "offpolicy_get_iqn_draws: bad arguments");
+  B200RL_REQUIRE(h->iqn, "offpolicy_get_iqn_draws: the engine was not created with algo = 4 (IQN)");
+  B200RL_REQUIRE(h->iqn_last_B > 0, "offpolicy_get_iqn_draws: the engine has not run a train step yet");
+  const size_t w = (size_t)S * h->iqn_last_B * (h->iqn_cfg.n + h->iqn_cfg.n_target + h->iqn_cfg.k) * 4;
+  if (w) B200RL_CUDA(cudaMemcpy2DAsync(taus, w, h->iqn_taus, h->lane_stride, w, h->K, cudaMemcpyDeviceToHost, h->gs));
   B200RL_CUDA(cudaStreamSynchronize(h->gs));
   return 0;
 }
@@ -2557,6 +2925,13 @@ static auto qr_head(bool weighted, bool nstep) {
                   : (nstep ? qr_loss_kernel<LANES, false, true> : qr_loss_kernel<LANES, false, false>);
 }
 
+// and of iqn_loss_kernel
+template <bool LANES>
+static auto iqn_head(bool weighted, bool nstep) {
+  return weighted ? (nstep ? iqn_loss_kernel<LANES, true, true> : iqn_loss_kernel<LANES, true, false>)
+                  : (nstep ? iqn_loss_kernel<LANES, false, true> : iqn_loss_kernel<LANES, false, false>);
+}
+
 // The S DQN steps.  Per step:
 //   s  : Q_targ(s') ---------------+-> loss -> dX chain -> Adam(Q) -> target copy (on the steps the flag table marks)
 //   s2 : Q(s') (Double DQN only) --+
@@ -2564,7 +2939,9 @@ static auto qr_head(bool weighted, bool nstep) {
 // Q(s') reads the parameters at the start of the step: the step's Adam waits for the loss kernel, which joins it.
 // A C51 engine (h->c51) takes c51_loss_kernel as its loss head, a QR-DQN engine (h->qr) qr_loss_kernel; nothing else
 // in the step differs.  A dueling Q network (q.duel_k) runs dueling_forward / dueling_backward in place of
-// net_forward / net_backward.
+// net_forward / net_backward.  An IQN engine (h->iqn) opens each step with iqn_draw_kernel on s, runs iqn_forward for
+// Q(s) with the N online fractions, Q_targ(s') with the N' target and K argmax fractions and Double DQN's Q(s') with
+// the K argmax fractions, takes iqn_loss_kernel as its loss head and iqn_backward as its backward pass.
 // A prioritized call (h->per_run) opens each step with the draw on s (draw, weights, gather), takes the weighted loss
 // head, and runs the priority update on s4 beside the backward pass; the next step's draw joins it.
 static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s) {
@@ -2608,6 +2985,37 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
                  betas, keys, st, B, O, 1, h->nstep, (float)hp->gamma, s_idx, s_w, s_obs, s_act, s_rew, s_nobs, s_done,
                  s_disc, h->nstep_rows + (size_t)st * B))
         return 1;
+    }
+    if (h->iqn) {
+      const int N = h->iqn_cfg.n, Nt = h->iqn_cfg.n_target, K = h->iqn_cfg.k, C = h->iqn_cfg.n_cos;
+      float* taus = h->iqn_taus + (size_t)st * B * (N + Nt + K);
+      if (launch(h, iqn_draw_kernel<false>, iqn_draw_kernel<true>,
+                 (unsigned)(((long long)B * (N + Nt + K) * C + GTHREADS - 1) / GTHREADS), GTHREADS, 0, s, B, N, Nt, K, C,
+                 noise_keys, st, taus, h->iqn_cos_q, h->iqn_cos_t, h->iqn_cos_n))
+        return 1;
+      if (edge(h, s, s3) || iqn_forward(h, q, s_obs, h->iqn_cos_q, B, N, h->iqn_pass[0], s3)) return 1;
+      if (dbl && (edge(h, s, s2) || iqn_forward(h, q, s_nobs, h->iqn_cos_n, B, K, h->iqn_pass[2], s2))) return 1;
+      if (iqn_forward(h, qt, s_nobs, h->iqn_cos_t, B, Nt + K, h->iqn_pass[1], s)) return 1;
+      if (dbl && edge(h, s2, s)) return 1;
+      if (edge(h, s3, s)) return 1;
+      if (launch(h, iqn_head<false>(per, nstep), iqn_head<true>(per, nstep), B, (std::max(N, 32) + 31) / 32 * 32,
+                 sizeof(float) * (size_t)iqn_smem_floats(n, N, Nt), s, h->iqn_pass[0].out, h->iqn_pass[1].out,
+                 dbl ? h->iqn_pass[2].out : nullptr, taus, s_act, s_rew, s_done, s_disc, (float)hp->gamma, B, n, N, Nt,
+                 K, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync, h->out_l1 + st,
+                 h->dqn_bad + st, s_w, h->per_absd))
+        return 1;
+      if (per) {
+        if (edge(h, s, s4)) return 1;
+        if (launch(h, per_update_kernel<false>, per_update_kernel<true>, 1, GTHREADS, 0, s4, h->replay, s_idx,
+                   h->per_absd, B, alpha, eps, h->per_newp + (size_t)st * B, h->per_bad + st))
+          return 1;
+      }
+      if (iqn_backward(h, q, s_obs, h->iqn_cos_q, B, h->iqn_pass[0], h->dqn_dout, s, s3)) return 1;
+      if (adam_net(h, q, h->adam_tab + (size_t)maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, s)) return 1;
+      if (launch(h, dqn_target_copy_kernel<false>, dqn_target_copy_kernel<true>, (unsigned)((q.P_flat + ew - 1) / ew),
+                 ew, 0, s, qt.flat, q.flat, (int)q.P_flat, h->adam_tab + (size_t)3 * maxS, st))
+        return 1;
+      continue;
     }
     float* qa[B200RL_MAX_LAYERS + 1];  // Q(s): its stack is what the backward pass reads
     qa[0] = s_obs;
@@ -2691,6 +3099,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   const size_t SB = (size_t)S * B;
   h->per_last = h->per_run;  // what get_per_draws may report
   h->nstep_last = h->nstep > 1;  // and get_nstep_draws
+  if (h->iqn) h->iqn_last_B = B;  // and get_iqn_draws
 
   // Adam's step-dependent scalars for the steps of this call (torch's host-side double arithmetic), one small upload
   // (a group: one table per learner, from that learner's step counts, uploaded with one strided copy)
@@ -2792,7 +3201,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   *n_policy_updates = n_pol;
   const int n_actions = h->net[1].d.sizes[h->net[1].d.n_layers] /
                         (h->c51 ? h->c51_hp.n_atoms : h->qr ? h->qr_hp.n_quantiles : 1);
-  const char* algo = h->c51 ? "C51" : h->qr ? "QR-DQN" : "DQN";
+  const char* algo = h->c51 ? "C51" : h->qr ? "QR-DQN" : h->iqn ? "IQN" : "DQN";
   for (size_t i = 0; i < bad.size(); ++i)
     B200RL_REQUIRE(bad[i] == 0, "offpolicy_train: %s learner %d, step %d: %d minibatch rows hold an action that is not "
                    "an integer in [0, %d); those rows were left out of the update", algo, (int)(i / S), (int)(i % S),
@@ -2824,6 +3233,8 @@ static int train_begin(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, 
     B200RL_REQUIRE(!h->c51 || h->c51_set, "%s: a C51 engine needs b200rl_offpolicy_set_c51 before it trains", what);
   }
   B200RL_REQUIRE(!h->noisy || h->noisy_keys, "%s: an engine with noisy layers needs fresh keys from "
+                 "b200rl_offpolicy_set_noise_keys before every train call", what);
+  B200RL_REQUIRE(!h->iqn || h->noisy_keys, "%s: an IQN engine needs fresh keys for its fraction draws from "
                  "b200rl_offpolicy_set_noise_keys before every train call", what);
   if (int rc = own()) return rc;
   h->noisy_keys = false;  // this call consumes them

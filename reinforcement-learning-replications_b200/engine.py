@@ -328,18 +328,21 @@ class OffPolicyEngine:
     engine after ``set_qr``: its Q network maps obs -> [n actions x n quantiles] quantile locations.  ``dueling_k`` = K
     >= 1 (DQN / QR-DQN / C51): the Q network is a dueling one, ``q_sizes`` = [obs, h_trunk, h_stream, n actions x K]
     (b200rl.h, "Dueling Q networks").  ``noisy_layers`` (DQN / QR-DQN / C51): bit mask of the Q network's noisy Linear
-    layers in flat order; every train call then needs ``set_noise_keys`` first (b200rl.h, "Noisy networks").
+    layers in flat order; every train call then needs ``set_noise_keys`` first (b200rl.h, "Noisy networks").  IQN
+    (``algo`` 4) is a DQN engine over an implicit quantile network: ``q_sizes`` = [obs, d, h, n actions] and ``iqn`` =
+    (n_cos, N, N', K); every train call needs ``set_noise_keys`` first, the keys of its fraction draws (b200rl.h, "IQN").
 
     ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
     launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
     is [K][per-learner blob] with [K][3] step counts, and the per-network accessors are refused."""
 
     NETS = {"policy": 0, "q1": 1, "q2": 2, "target_policy": 3, "target_q1": 4, "target_q2": 5}
-    TD3, SAC, DQN, C51 = 0, 1, 2, 3
+    TD3, SAC, DQN, C51, IQN = 0, 1, 2, 3, 4
+    DISCRETE = (DQN, C51, IQN)  # the algos with DQN's networks, inputs and outputs
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
                  q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1, dueling_k: int = 0,
-                 noisy_layers: int = 0):
+                 noisy_layers: int = 0, iqn=None):
         from ._lib import OffPolicyConfig
         self.lib = _lib.load()
         current_stream_handle()
@@ -350,7 +353,8 @@ class OffPolicyEngine:
         cfg.n_q, cfg.max_minibatch, cfg.max_steps = int(n_q), int(max_minibatch), int(max_steps)
         cfg.algo, cfg.dueling_k, cfg.noisy_layers = int(algo), int(dueling_k), int(noisy_layers)
         self.algo, self.dueling_k, self.noisy_layers = int(algo), int(dueling_k), int(noisy_layers)
-        self.discrete = self.algo in (self.DQN, self.C51)  # DQN's networks, inputs and outputs
+        self.iqn = None if iqn is None else tuple(int(x) for x in iqn)
+        self.discrete = self.algo in self.DISCRETE
         self.n_q, self.max_minibatch, self.max_steps = int(n_q), int(max_minibatch), int(max_steps)
         self.policy_sizes, self.q_sizes = None if policy_sizes is None else list(policy_sizes), list(q_sizes)
         self.policy_acts, self.q_acts = tuple(policy_acts), tuple(q_acts)
@@ -359,12 +363,19 @@ class OffPolicyEngine:
         if self.dueling_k and len(self.q_sizes) == 4:  # trunk, both streams' hidden layers, V and A (b200rl.h)
             O, h1, h2, w = self.q_sizes
             self.n_qp = h1 * (O + 1) + 2 * h2 * (h1 + 1) + (self.dueling_k + w) * (h2 + 1)
+        if self.iqn is not None and len(self.q_sizes) == 4:  # psi, phi, head hidden, head out (b200rl.h, "IQN")
+            O, d, hh, n = self.q_sizes
+            self.n_qp = d * (O + 1) + d * (self.iqn[0] + 1) + hh * (d + 1) + n * (hh + 1)
         noisy = [(i, o) for l, (i, o) in enumerate(self.q_layers()) if self.noisy_layers >> l & 1]
         self.n_qp += sum(o * (i + 1) for i, o in noisy)  # W_sigma and b_sigma of each noisy layer
         self.noise_width = sum(i + o for i, o in noisy)  # E: draws per network and step
         self.K = int(n_learners)
         h = C.c_void_p()
-        check(self.lib.b200rl_offpolicy_create_group(C.byref(cfg), self.K, C.byref(h)), "offpolicy_create")
+        if self.iqn is None:
+            check(self.lib.b200rl_offpolicy_create_group(C.byref(cfg), self.K, C.byref(h)), "offpolicy_create")
+        else:  # IQN's counts size its per-row buffers (b200rl.h, "IQN")
+            check(self.lib.b200rl_offpolicy_create_iqn(C.byref(cfg), C.byref(_lib.IqnConfig(*self.iqn)), self.K,
+                                                       C.byref(h)), "offpolicy_create_iqn")
         self.h = h
 
     def q_layers(self):
@@ -528,6 +539,17 @@ class OffPolicyEngine:
         check(self.lib.b200rl_offpolicy_get_noisy_draws(self.h, int(S), _ptr(eps)), "get_noisy_draws")
         return eps[0] if self.K == 1 else eps
 
+    # ---- IQN ----
+    def get_iqn_draws(self, S: int):
+        """The fractions [S, B, N + N' + K] (per row the online, target and argmax ones) of the first S steps of the
+        last train call that ran steps, B its minibatch; a group: [K, S, B, N + N' + K]."""
+        _, N, Nt, K = self.iqn
+        buf = np.empty(self.K * S * self.max_minibatch * (N + Nt + K), np.float32)  # room for any call's minibatch
+        check(self.lib.b200rl_offpolicy_get_iqn_draws(self.h, int(S), _ptr(buf)), "get_iqn_draws")
+        B = getattr(self, "_last_B", 0)
+        taus = buf[:self.K * S * B * (N + Nt + K)].reshape(self.K, S, B, N + Nt + K)
+        return taus[0] if self.K == 1 else taus
+
     # ---- C51 ----
     def set_c51(self, n_atoms: int, v_min: float, v_max: float) -> None:
         """The categorical head's support: ``n_atoms`` atoms from ``v_min`` to ``v_max`` (b200rl.h)."""
@@ -623,6 +645,8 @@ class OffPolicyEngine:
 
     def _out_buffers(self, S, B):
         K = self.K
+        if S > 0:
+            self._last_B = B  # the minibatch of the call's steps, get_iqn_draws's
         return (np.zeros((K, S, B), np.float32), np.zeros((K, S, B), np.float32), np.zeros((K, S), np.float32),
                 np.zeros((K, S), np.float32), np.zeros((K, max(S, 1)), np.float32), C.c_int32())
 

@@ -15,6 +15,12 @@
 //     delivered a stage's operands, and tell the chains when both have finished reading a buffer they are about to
 //     overwrite.  dZ2, dZ1 and dOut have buffers of their own, so the gradient products run about one tile behind the
 //     chains; the h-split warpgroup also brings the observations in;
+//   * the chain epilogues move the fp16 pairs between the wgmma fragment and the swizzled activation buffers with
+//     stmatrix / ldmatrix: 8 stmatrix.x4 per buffer written and 8 ldmatrix.x4 per buffer read back, instead of 32
+//     st.shared / ld.shared.b32 each (same bytes at the same addresses).  Splitting each n64 chain product into two
+//     n32 groups, to run the epilogue of one half under the product of the other, made the launch slower (more
+//     shared-memory reads of A per product), and so did issuing the b3 running-sum loads before the OUT product
+//     (126 registers instead of 122); neither is kept (README);
 //   * the observations are split into their fp16 pairs ONCE PER UPDATE by pack_obs_kernel (every step of the update
 //     reads the same observations) into ready-made SWIZZLE_128B tile images [128 rows][h cols 0..31 | l cols 32..63];
 //     the step kernel brings a tile image in with ONE 16 KB bulk copy (cp.async.bulk + mbarrier complete_tx) issued by
@@ -201,6 +207,18 @@ __device__ __forceinline__ void chain_mma(float (&d)[N / 2], const Op2 a, const 
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
   wg_mma<N, K_MAJOR, TB, 3, KSTEPS>(d, alo, blo, a.hi, b.hi, a.k_step, b.k_step, 0u);
+}
+// Four 8 x 8 fp16 matrices between registers and shared memory; lane l gives the address of row l & 7 of matrix l >> 3
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]),
+               "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
 }
 // This thread's fragment of the first m64 half of the weight-gradient product at column pcol, whatever its N:
 // grad_acc_off's layout puts chunk j of the fragment 512 j floats further and the second half 64 N floats further.
@@ -563,21 +581,23 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     const float sH = pow2i(T2_H_EXP), hh = pow2i(-2 * T2_H_EXP);
     const int A_out = p.net[0].n_out;
 
-    // byte offset of columns 8 j + 2 q, +1 of fragment row r0 + 8 r in the SWIZZLE_128B buffer `buf`
-    auto frag_off = [&](uint32_t buf, int j, int r) -> uint32_t {
-      return buf + (uint32_t)(r0 + 8 * r) * 128u + ((uint32_t)(j ^ quad) << 4) + 4u * (uint32_t)q;
-    };
+    // A packed pair of fragment elements (4 j + 2 r, +1: row r0 + 8 r, columns 8 j + 2 q, +1) is this thread's share of
+    // the 8 x 8 fp16 matrix (rows 8 r .. 8 r + 7 of the warp's 16, 16-byte chunk j), as stmatrix / ldmatrix lay it out,
+    // and a row of that matrix is one 16-byte chunk of a SWIZZLE_128B buffer.  One .x4 access moves matrices
+    // (j, 0), (j, 1), (j + 1, 0), (j + 1, 1) for even j, i.e. fragment elements 4 j .. 4 j + 7; lane l gives the address
+    // of row l & 7 of matrix l >> 3: at `buf` + mat_off(j), chunk (j + (l >> 4)) ^ (l & 7) = j ^ ((l >> 4) ^ (l & 7)).
+    const uint32_t mat_row = base + (uint32_t)(64 * wg + 16 * (warp & 3) + 8 * ((lane >> 3) & 1) + (lane & 7)) * 128u;
+    const uint32_t mat_chunk = (uint32_t)((lane >> 4) ^ (lane & 7)) << 4;
+    auto mat_off = [&](uint32_t buf, int j) -> uint32_t { return mat_row + buf + (((uint32_t)j << 4) ^ mat_chunk); };
     auto store_pairs = [&](uint32_t buf, const float (&x)[32]) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
+      for (int j = 0; j < 8; j += 2) {
+        uint32_t h[4], l[4];
 #pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          uint32_t h, l;
-          split2h(x[4 * j + 2 * r], x[4 * j + 2 * r + 1], h, l);
-          const uint32_t off = frag_off(buf, j, r);
-          *reinterpret_cast<uint32_t*>(sm + off) = h;
-          *reinterpret_cast<uint32_t*>(sm + off + T2_ACT) = l;
-        }
+        for (int m = 0; m < 4; ++m) split2h(x[4 * j + 2 * m], x[4 * j + 2 * m + 1], h[m], l[m]);
+        stmatrix_x4(mat_off(buf, j), h);
+        stmatrix_x4(mat_off(buf + T2_ACT, j), l);
+      }
     };
     // E1 / E2: Z * unscale + bias -> tanh(.) * 2^14
     auto act = [&](float (&z)[32], float unscale, const float* bs) {
@@ -600,21 +620,22 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
       const float one28 = 268435456.f;
       float m = 0.f;
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
+      for (int j = 0; j < 8; j += 2) {
+        uint32_t hw[4], lw[4];
+        ldmatrix_x4(mat_off(buf, j), hw);
+        ldmatrix_x4(mat_off(buf + T2_ACT, j), lw);
 #pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          const uint32_t off = frag_off(buf, j, r);
-          const uint32_t hw = *reinterpret_cast<const uint32_t*>(sm + off);
-          const uint32_t lw = *reinterpret_cast<const uint32_t*>(sm + off + T2_ACT);
-          const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&hw));
-          const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&lw));
+        for (int i = 0; i < 4; ++i) {
+          const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&hw[i]));
+          const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&lw[i]));
           const float x0 = a.x + b.x, x1 = a.y + b.y;
-          float& g0 = g[4 * j + 2 * r];
-          float& g1 = g[4 * j + 2 * r + 1];
+          float& g0 = g[4 * j + 2 * i];
+          float& g1 = g[4 * j + 2 * i + 1];
           g0 = (g0 * unscale) * fmaf(-x0, x0, one28);
           g1 = (g1 * unscale) * fmaf(-x1, x1, one28);
           m = fmaxf(m, fmaxf(fabsf(g0), fabsf(g1)));
         }
+      }
       if (!(m <= T2_RANGE)) bad = true;  // magnitude only: the inputs were checked
     };
     // this warpgroup's shared-memory writes -> visible to its own next product and to the gradient warpgroup

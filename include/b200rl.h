@@ -336,12 +336,13 @@ typedef struct b200rl_offpolicy b200rl_offpolicy;
 typedef struct {
   b200rl_mlp_desc policy;  /* [obs, hidden..., act]      (ref: policies/deterministic_policy.py); SAC: [obs, ..., 2 act] */
   b200rl_mlp_desc q;       /* [obs + act, hidden..., 1]  (ref: q_function.py:20-32) */
-  int32_t n_q;             /* 1 = DDPG, 2 = TD3 (algo 0); SAC needs 2, DQN 1 */
+  int32_t n_q;             /* 1 = DDPG, 2 = TD3 (algo 0); SAC and discrete SAC need 2, DQN 1 */
   int32_t max_minibatch;   /* capacity: rows per minibatch */
   int32_t max_steps;       /* capacity: train steps per call */
   int32_t algo;            /* 0 = DDPG / TD3 (by n_q), 1 = SAC (see b200rl_offpolicy_set_sac), 2 = DQN (see
                             * b200rl_offpolicy_set_dqn), 3 = C51 (see b200rl_offpolicy_set_c51), 4 = IQN (created by
-                            * b200rl_offpolicy_create_iqn only; see "IQN" below) */
+                            * b200rl_offpolicy_create_iqn only; see "IQN" below), 5 = discrete SAC (see
+                            * "Discrete SAC" below) */
   int32_t dueling_k;       /* 0 = the Q network is a plain MLP; K >= 1 = a dueling Q network (algo 2 / 3 only; see
                             * "Dueling Q networks" below) */
   int32_t noisy_layers;    /* bit mask over the Q network's Linear layers in flat order: 0 = none; bit l = layer l is a
@@ -442,6 +443,45 @@ int b200rl_offpolicy_set_alpha(b200rl_offpolicy* h, float log_alpha, float exp_a
 int b200rl_offpolicy_get_alpha(b200rl_offpolicy* h, float* log_alpha, float* exp_avg, float* exp_avg_sq, int64_t* step);
 /* After a train call of S steps: mean log pi of each policy step and the alpha each step used (host [S] each). */
 int b200rl_offpolicy_sac_outputs(b200rl_offpolicy* h, int32_t S, float* log_prob_means, float* alphas);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Discrete SAC on the same engine (config algo = 5, n_q = 2; Christodoulou 2019, "Soft Actor-Critic for Discrete
+ * Action Settings").  policy = [obs, hidden..., n] maps obs -> n logits (Identity output layer); q = [obs, hidden...,
+ * n] maps obs -> one value per action for both critics and their targets (n >= 2, both widths equal).  Networks 0, 1,
+ * 2, 4, 5 are present (no target policy), so the state blob, steps[3], set_alpha / get_alpha and sac_outputs keep
+ * SAC's layout.  The action column is one float32 per row holding the action index (act [S,B] for train, d_act [rows]
+ * for the gather paths), as for DQN.  Per train step on (s, a, r, s', d), with alpha = alpha[st] (the temperature at
+ * the start of the step), in float32:
+ *   log pi     log pi_j = (x_j - max x) - log(sum_k exp(x_k - max x)) of the logits x, every sum over actions in index
+ *              order; pi_j = exp(log pi_j) (the log-softmax form: a vanishing probability gives pi log pi = 0)
+ *   critics    V(s') = sum_j pi'_j (min(Q1targ, Q2targ)(s')_j - alpha log pi'_j), pi' the policy at s' at the start of
+ *              the step; y = r + gamma (1 - d) V(s'); one Adam step each (optimizers 1, 2) on mean_B (Qk(s)[a] - y)^2,
+ *              whose gradient w.r.t. critic k's outputs is 2 (Qk(s)[a] - y) / B in column a and 0 elsewhere
+ *   policy     with the critics just updated (no gradient into them), m_j = min(Q1, Q2)(s)_j, c_j = alpha log pi_j - m_j:
+ *              one Adam step (optimizer 0) on mean_B L, L = sum_j pi_j c_j; the logit gradient is
+ *              pi_k (c_k - L) / B (the alpha term of d log pi cancels: sum_j pi_j = 1); pi is the policy at the start
+ *              of the step
+ *   alpha      learn_alpha = 1: one Adam step on -mean_B(log_alpha (E + target_entropy)), E = sum_j pi_j log pi_j from
+ *              the policy step's pi(s); alpha = exp(log_alpha) from the next step on (target_entropy: 0.98 log n is
+ *              the paper's choice); learn_alpha = 0: alpha is the fixed value
+ *   polyak     Q1targ, Q2targ every step
+ * b200rl_offpolicy_set_sac is required once before the first train call; its log_std_min / log_std_max are ignored.
+ * hparams: gamma, polyak_rho and the Adam fields apply; policy_delay, use_target_noise, target_noise_* and
+ * action_limit are ignored.  No noise is used: train / train_gather take noise = NULL, train_gather_rng draws indices
+ * only, get_draws returns no noise.  Outputs: q1_values / q2_values [S,B] = Qk(s)[a] before the update, q1_losses /
+ * q2_losses [S], policy_losses [S] (mean L, *n_policy_updates = S); sac_outputs gives mean E per step (in place of SAC's
+ * mean log pi) and the alpha each step used.  A row whose action is not an integer in [0, n) is never used as an index,
+ * adds nothing to either critic's loss or gradient and logs NaN; the call then returns an error naming the learner and
+ * the step (the update has still run).  The heads reduce in a fixed order with no float atomics: a group's learners stay
+ * bit-identical to solo engines.  Runs as a CUDA graph, or as plain launches with B200RL_OFFPOLICY_GRAPH=0.
+ * Launches, with Lq and Lp the critics' and the policy's Linear layers: 1 per call (the temperature table), then per
+ * step 10 Lq + 4 Lp + 4, one more with learn_alpha = 1 (forward passes: Q1, Q2 and pi at s, pi, Q1targ, Q2targ at s',
+ * the updated Q1, Q2 at s; 2 critic heads; backward passes of 2 L - 1 launches, weight gradients and the dX chain
+ * down to the first hidden layer, for both critics and the policy; 3 Adam steps; polyak; the policy head; the
+ * temperature step): 46 per step at two hidden layers, 47 with a learned temperature.
+ * Not implemented, and refused: dueling_k or noisy_layers != 0 at create; set_dqn, set_c51, set_qr, set_per, set_nstep,
+ * set_noise_keys and the train_prioritized calls (prioritized replay, n-step returns, noisy, dueling and IQN networks).
+ * ------------------------------------------------------------------------------------------------------------ */
 
 /* ------------------------------------------------------------------------------------------------------------
  * DQN on the same engine (config algo = 2, n_q = 1; Mnih et al. 2015, Double DQN: van Hasselt et al. 2016).  The

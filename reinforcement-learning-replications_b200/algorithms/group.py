@@ -1,4 +1,4 @@
-"""LearnerGroup: several independent TD3 / DDPG / SAC / DQN / C51 / QR-DQN / IQN learners (typically one per seed) trained side by side by ONE
+"""LearnerGroup: several independent TD3 / DDPG / SAC / discrete SAC / DQN / C51 / QR-DQN / IQN learners (typically one per seed) trained side by side by ONE
 off-policy engine, every operation of a train step one launch for all of them (b200rl_offpolicy_create_group).
 
 The contract: each member ends up bit for bit where it would be had it run alone.  Members keep everything of their
@@ -67,15 +67,19 @@ def _signature(agent) -> list:
             sig.append((f"prioritized replay {attr}", getattr(rb, attr, None) if isinstance(rb, PrioritizedReplayBuffer)
                         else None))
         return sig
-    sig.append(("action limit", float(agent.env.action_space.high[0])))
+    if agent.algo == OffPolicyEngine.DSAC:
+        sig.append(("action count", agent.n_actions))
+    else:
+        sig.append(("action limit", float(agent.env.action_space.high[0])))
     for attr in ("gamma", "polyak_rho", "target_noise_scale", "target_noise_clip", "policy_delay", "use_device_replay",
                  "use_device_rng"):
         sig.append((attr, getattr(agent, attr, None)))
-    if agent.algo == OffPolicyEngine.SAC:
+    if agent.algo in OffPolicyEngine.SOFT:
         sig += [("alpha", agent.alpha), ("learn_alpha", agent.learn_alpha), ("target_entropy", agent.target_entropy),
                 ("alpha optimizer (lr, beta1, beta2, eps)",
-                 adam_hparams(agent.alpha_optimizer, [], "alpha optimizer", extra=[agent.log_alpha])),
-                ("log_std bounds", (agent.policy.log_std_min, agent.policy.log_std_max))]
+                 adam_hparams(agent.alpha_optimizer, [], "alpha optimizer", extra=[agent.log_alpha]))]
+    if agent.algo == OffPolicyEngine.SAC:
+        sig.append(("log_std bounds", (agent.policy.log_std_min, agent.policy.log_std_max)))
     return sig
 
 
@@ -117,7 +121,7 @@ class LearnerGroup:
     def add(self, agent) -> None:
         """Add ``agent``; the current state of the global random generators becomes its private stream."""
         if not isinstance(agent, _OffPolicyBase):
-            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or DQN / C51 / QR-DQN / IQN) learners, got {type(agent).__name__}")
+            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or DiscreteSAC / DQN / C51 / QR-DQN / IQN) learners, got {type(agent).__name__}")
         if any(m is agent for m in self.members):
             raise ValueError("LearnerGroup: this agent is already a member")
         if len(self.members) >= MAX_LEARNERS:
@@ -200,7 +204,7 @@ class LearnerGroup:
             steps.append(m._fill_state(slots, trainable, lins))
             plans.append((slots, trainable))
         e.set_state(None, steps)
-        sac = members[0].algo == OffPolicyEngine.SAC
+        sac = members[0].algo in OffPolicyEngine.SOFT
         if sac:
             e.set_sac(members[0]._sac_hparams())
             e.set_alpha_group([m._alpha_state() for m in members])

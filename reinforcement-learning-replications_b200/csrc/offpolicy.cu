@@ -625,6 +625,123 @@ __global__ void __launch_bounds__(GTHREADS) sac_alpha_step_kernel(const float* l
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Discrete SAC (algo = 5; Christodoulou 2019).  The policy network maps obs -> [n] logits, both critics and their
+// targets obs -> [n] Q-values; the action column holds the action index as float32.  Every expectation over actions
+// is exact: no noise, no squash head, and no gradient through the critics into the policy.
+// ---------------------------------------------------------------------------------------------------------------
+// log_softmax of one row's n logits x: log pi_j = (x_j - m) - ls with m = max_j x_j and ls = log(sum_j exp(x_j - m)),
+// the sum in index order (c51_expected's arithmetic); returns ls and sets m.  pi_j = exp(log pi_j), so a vanishing
+// probability gives pi log pi = 0, never 0 * -inf.
+__device__ __forceinline__ float dsac_log_norm(const float* x, int n, float& m) {
+  m = x[0];
+  for (int j = 1; j < n; ++j) m = fmaxf(m, x[j]);
+  float s = 0.f;
+  for (int j = 0; j < n; ++j) s += expf(x[j] - m);
+  return logf(s);
+}
+
+// One CTA per critic (each critic's launch on its own stream): per row i with action a = act[i],
+//   V(s') = sum_j pi'_j (min(Q1targ, Q2targ)(s')_j - alpha log pi'_j) from the policy's logits at s' (index order),
+//   y = r + gamma (1 - d) V(s'), loss = mean((Q(s)[a] - y)^2),
+//   dOut[i, :] = 0 except dOut[i, a] = 2 (Q(s)[a] - y) / B, q_copy[i] = Q(s)[a] (the logged Q-value).
+// A row whose action is not an integer in [0, n) is never used as an index: it adds nothing to the loss or dOut, logs
+// NaN, and is counted in *bad_out (when bad_out != NULL; both critics see the same actions, so one of them counts).
+// The loss is summed as q_loss_kernel sums it, in a fixed order with no float atomics.
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) dsac_q_loss_kernel(const float* q, const float* logits_next,
+                                                              const float* q1t, const float* q2t, const float* act,
+                                                              const float* rew, const float* done, const float* alpha,
+                                                              float gamma, int B, int n, float* dout, float* loss_out,
+                                                              float* q_copy, int* bad_out, size_t lane_stride) {
+  __shared__ double red[32];
+  __shared__ int bad_rows;
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q = lane_ptr(q, o), logits_next = lane_ptr(logits_next, o), q1t = lane_ptr(q1t, o), q2t = lane_ptr(q2t, o);
+    act = lane_ptr(act, o), rew = lane_ptr(rew, o), done = lane_ptr(done, o), alpha = lane_ptr(alpha, o);
+    dout = lane_ptr(dout, o), loss_out = lane_ptr(loss_out, o), q_copy = lane_ptr(q_copy, o);
+    bad_out = lane_ptr(bad_out, o);
+  }
+  if (threadIdx.x == 0) bad_rows = 0;
+  __syncthreads();
+  const float al = *alpha;
+  const float inv = 1.0f / (float)B;
+  double acc = 0.0;
+  int bad = 0;
+  for (int i = threadIdx.x; i < B; i += blockDim.x) {
+    const float af = act[i];
+    const bool valid = af >= 0.f && af < (float)n && af == floorf(af);  // false for NaN
+    const int a = valid ? (int)af : -1;
+    float g = 0.f;
+    if (valid) {
+      const float *x = logits_next + (size_t)i * n, *t1 = q1t + (size_t)i * n, *t2 = q2t + (size_t)i * n;
+      float m;
+      const float ls = dsac_log_norm(x, n, m);
+      float v = 0.f;
+      for (int j = 0; j < n; ++j) {
+        const float lp = (x[j] - m) - ls;
+        v += expf(lp) * (fminf(t1[j], t2[j]) - al * lp);
+      }
+      const float qi = q[(size_t)i * n + a];
+      const float d = qi - (rew[i] + gamma * (1.f - done[i]) * v);
+      acc += (double)d * (double)d;
+      g = (2.f * d) * inv;
+      q_copy[i] = qi;
+    } else {
+      q_copy[i] = __int_as_float(0x7fc00000);
+      ++bad;
+    }
+    for (int j = 0; j < n; ++j) dout[(size_t)i * n + j] = j == a ? g : 0.f;
+  }
+  if (bad) atomicAdd(&bad_rows, bad);
+  block_mean(acc, B, loss_out, red);  // its __syncthreads orders every thread's atomicAdd before thread 0 reads
+  if (threadIdx.x == 0 && bad_out != nullptr) *bad_out = bad_rows;
+}
+
+// One CTA: the policy step's head.  Per row i, with pi from the logits x of the policy at s, m_j = min(Q1, Q2)(s)_j of
+// the critics just updated and c_j = alpha log pi_j - m_j:
+//   L_i = sum_j pi_j c_j, E_i = sum_j pi_j log pi_j (index order),
+//   dOut[i, k] = pi_k (c_k - L_i) / B (the alpha term of d log pi cancels: sum_j pi_j = 1), ent[i] = E_i;
+// *loss_out = mean L_i and *ent_mean_out = mean E_i, each summed as block_mean sums.  ent is what
+// sac_alpha_step_kernel reads in place of log pi.
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) dsac_policy_loss_kernel(const float* logits, const float* q1,
+                                                                   const float* q2, const float* alpha, int B, int n,
+                                                                   float* dout, float* ent, float* loss_out,
+                                                                   float* ent_mean_out, size_t lane_stride) {
+  __shared__ double red[32], red_e[32];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    logits = lane_ptr(logits, o), q1 = lane_ptr(q1, o), q2 = lane_ptr(q2, o), alpha = lane_ptr(alpha, o);
+    dout = lane_ptr(dout, o), ent = lane_ptr(ent, o), loss_out = lane_ptr(loss_out, o);
+    ent_mean_out = lane_ptr(ent_mean_out, o);
+  }
+  const float al = *alpha;
+  const float inv = 1.0f / (float)B;
+  double acc = 0.0, acc_e = 0.0;
+  for (int i = threadIdx.x; i < B; i += blockDim.x) {
+    const float *x = logits + (size_t)i * n, *a1 = q1 + (size_t)i * n, *a2 = q2 + (size_t)i * n;
+    float m;
+    const float ls = dsac_log_norm(x, n, m);
+    float L = 0.f, E = 0.f;
+    for (int j = 0; j < n; ++j) {
+      const float lp = (x[j] - m) - ls, p = expf(lp);
+      L += p * (al * lp - fminf(a1[j], a2[j]));
+      E += p * lp;
+    }
+    for (int j = 0; j < n; ++j) {
+      const float lp = (x[j] - m) - ls;
+      dout[(size_t)i * n + j] = (expf(lp) * ((al * lp - fminf(a1[j], a2[j])) - L)) * inv;
+    }
+    ent[i] = E;
+    acc += (double)L;
+    acc_e += (double)E;
+  }
+  block_mean(acc, B, loss_out, red);
+  block_mean(acc_e, B, ent_mean_out, red_e);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // DQN (algo = 2; Mnih et al. 2015, Double DQN: van Hasselt et al. 2016).  The Q network maps obs -> [n] values; the
 // action column holds the action index as float32.
 // ---------------------------------------------------------------------------------------------------------------
@@ -1739,6 +1856,10 @@ struct b200rl_offpolicy {
   float* sac_state = nullptr;                               // {log_alpha, exp_avg, exp_avg_sq}
   float* out_logp = nullptr;                                // [max_steps] mean log pi of each policy step
   int64_t alpha_step[B200RL_MAX_LEARNERS] = {};
+  // discrete SAC (cfg.algo == 5): SAC's networks, temperature and outputs (every SAC buffer above except the act /
+  // log pi ones), DQN's index action column (A = 1) and invalid-action count (dqn_bad); h->sac stays false.  dq / dq2
+  // are [B, n], sac_dout the policy's [B, n] logit gradient and sac_logp each row's E_i = sum_j pi_j log pi_j
+  bool dsac = false;
   // DQN (cfg.algo == 2): networks 1 (Q) and 4 (target Q) only; the action column is 1 wide (the index as float32);
   // adam_tab row 3 holds the target-copy flags of the call's steps
   bool dqn = false, dqn_set = false;
@@ -1795,7 +1916,7 @@ inline int64_t state_pad(int64_t n) { return (n + 63) & ~(int64_t)63; }
 // float2 entries of one learner's adam_tab: the Adam scalar rows (+ SAC's temperature row or DQN's copy flags), then
 // DQN's prioritized (seed, call) at 4 max_steps and a noisy or IQN engine's draw keys (seed, call) after it
 inline size_t adam_tab_len(const b200rl_offpolicy* h) {
-  return (h->sac || h->dqn ? 4 : 3) * (size_t)h->cfg.max_steps + (h->dqn ? 2 : 0) + (h->noisy || h->iqn ? 2 : 0);
+  return (h->sac || h->dsac || h->dqn ? 4 : 3) * (size_t)h->cfg.max_steps + (h->dqn ? 2 : 0) + (h->noisy || h->iqn ? 2 : 0);
 }
 
 // A piece of the learner arena: recorded here (256-byte aligned), placed by arena_commit
@@ -2110,14 +2231,18 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   B200RL_REQUIRE(n_learners >= 1 && n_learners <= B200RL_MAX_LEARNERS,
                  "offpolicy_create_group: n_learners must be 1..%d, got %d", B200RL_MAX_LEARNERS, n_learners);
   B200RL_REQUIRE(cfg->n_q == 1 || cfg->n_q == 2, "offpolicy_create: n_q must be 1 (DDPG) or 2 (TD3)");
-  B200RL_REQUIRE((cfg->algo >= 0 && cfg->algo <= 3) || (cfg->algo == 4 && ic != nullptr),
-                 "offpolicy_create: algo must be 0 (DDPG / TD3), 1 (SAC), 2 (DQN) or 3 (C51), got %d (algo 4, IQN, is "
-                 "created by b200rl_offpolicy_create_iqn with its counts)", cfg->algo);
+  B200RL_REQUIRE((cfg->algo >= 0 && cfg->algo <= 3) || cfg->algo == 5 || (cfg->algo == 4 && ic != nullptr),
+                 "offpolicy_create: algo must be 0 (DDPG / TD3), 1 (SAC), 2 (DQN), 3 (C51) or 5 (discrete SAC), got %d "
+                 "(algo 4, IQN, is created by b200rl_offpolicy_create_iqn with its counts)", cfg->algo);
   B200RL_REQUIRE(ic == nullptr || cfg->algo == 4, "offpolicy_create_iqn: the config's algo must be 4 (IQN), got %d",
                  cfg->algo);
-  const bool sac = cfg->algo == 1, c51 = cfg->algo == 3, iqn = cfg->algo == 4;
+  const bool sac = cfg->algo == 1, c51 = cfg->algo == 3, iqn = cfg->algo == 4, dsac = cfg->algo == 5;
   const bool dqn = cfg->algo == 2 || c51 || iqn;  // C51 and IQN are DQN engines
   B200RL_REQUIRE(!sac || cfg->n_q == 2, "offpolicy_create: SAC needs n_q = 2 (twin soft critics), got %d", cfg->n_q);
+  B200RL_REQUIRE(!dsac || cfg->n_q == 2, "offpolicy_create: discrete SAC (algo = 5) needs n_q = 2 (twin soft critics), "
+                 "got %d", cfg->n_q);
+  B200RL_REQUIRE(!dsac || (cfg->dueling_k == 0 && cfg->noisy_layers == 0), "offpolicy_create: discrete SAC (algo = 5) "
+                 "takes neither dueling_k nor noisy_layers: dueling and noisy networks are not implemented for it");
   B200RL_REQUIRE(!dqn || cfg->n_q == 1, "offpolicy_create: DQN needs n_q = 1 (one Q network), got %d", cfg->n_q);
   B200RL_REQUIRE(cfg->max_minibatch >= 1 && cfg->max_minibatch <= 65536 && cfg->max_steps >= 1,
                  "offpolicy_create: bad capacities");
@@ -2173,10 +2298,16 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
                  "layers", NM, n_lin);
   const int O = dqn ? cfg->q.sizes[0] : cfg->policy.sizes[0], P_out = cfg->policy.sizes[cfg->policy.n_layers];
   // SAC: the policy outputs [mean | log_std], 2A wide; DQN: the action column holds the index (1 wide)
-  const int A = dqn ? 1 : sac ? cfg->q.sizes[0] - O : P_out;
+  const int A = dqn || dsac ? 1 : sac ? cfg->q.sizes[0] - O : P_out;
   B200RL_REQUIRE(!sac || (A >= 1 && P_out == 2 * A),
                  "offpolicy_create: the SAC policy must output [mean | log_std] = 2 x %d values, got %d", A, P_out);
-  B200RL_REQUIRE(dqn || (cfg->q.sizes[0] == O + A && cfg->q.sizes[cfg->q.n_layers] == 1),
+  if (dsac) {  // policy and critics both map obs -> [n]
+    const int nq = cfg->q.sizes[cfg->q.n_layers];
+    B200RL_REQUIRE(cfg->q.sizes[0] == O && nq == P_out && nq >= 2, "offpolicy_create: discrete SAC (algo = 5) needs a "
+                   "policy [obs, ..., n] and critics [obs, ..., n] with n >= 2 actions, got policy %d -> %d and critics "
+                   "%d -> %d", O, P_out, cfg->q.sizes[0], nq);
+  }
+  B200RL_REQUIRE(dqn || dsac || (cfg->q.sizes[0] == O + A && cfg->q.sizes[cfg->q.n_layers] == 1),
                  "offpolicy_create: Q network must map [obs %d + act %d] -> 1", O, A);
   B200RL_REQUIRE(device_sm_count() > 0, "offpolicy_create: no CUDA device");
   b200rl_offpolicy* h = new b200rl_offpolicy();
@@ -2185,6 +2316,7 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   h->O = O;
   h->A = A;
   h->sac = sac;
+  h->dsac = dsac;
   h->dqn = dqn;
   h->c51 = c51;
   h->iqn = iqn;
@@ -2249,7 +2381,7 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
       nb.P_flat = fo;
     }
     if (cfg->n_q == 1 && (i == 2 || i == 5)) continue;
-    if (sac && i == 3) continue;  // SAC has no target policy
+    if ((sac || dsac) && i == 3) continue;  // SAC has no target policy
     if (dqn && (i == 0 || i == 3)) continue;  // DQN has no policy
     nb.present = true;
     if (i < 3) rc |= oalloc(h, &nb.grad, (size_t)nb.P);
@@ -2284,12 +2416,13 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   rc |= oalloc(h, &h->x_cat2, B * (size_t)(O + A));
   rc |= oalloc(h, &h->qt1, B);
   rc |= oalloc(h, &h->qt2, B);
-  rc |= oalloc(h, &h->dq, B);
+  const size_t n_dq = dsac ? (size_t)cfg->q.sizes[cfg->q.n_layers] : 1;  // discrete SAC: [B, n] per critic
+  rc |= oalloc(h, &h->dq, B * n_dq);
   rc |= oalloc(h, &h->dbuf0, B * (size_t)maxw);
   rc |= oalloc(h, &h->dbuf1, B * (size_t)maxw);
   rc |= oalloc(h, &h->dbuf2, B * (size_t)maxw);
   rc |= oalloc(h, &h->dbuf3, B * (size_t)maxw);
-  rc |= oalloc(h, &h->dq2, B);
+  rc |= oalloc(h, &h->dq2, B * n_dq);
   rc |= oalloc(h, &h->out_q1, S * B);
   rc |= oalloc(h, &h->out_q2, S * B);
   rc |= oalloc(h, &h->out_l1, S);
@@ -2307,6 +2440,14 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
     rc |= oalloc(h, &h->sac_alpha, S + 1);
     rc |= oalloc(h, &h->sac_state, 3);
     rc |= oalloc(h, &h->out_logp, S);
+  }
+  if (dsac) {
+    rc |= oalloc(h, &h->sac_logp, B);
+    rc |= oalloc(h, &h->sac_dout, B * n_dq);
+    rc |= oalloc(h, &h->sac_alpha, S + 1);
+    rc |= oalloc(h, &h->sac_state, 3);
+    rc |= oalloc(h, &h->out_logp, S);
+    rc |= oalloc(h, &h->dqn_bad, S);
   }
   if (dqn) {
     rc |= oalloc(h, &h->dqn_dout, B * (size_t)cfg->q.sizes[cfg->q.n_layers] * (iqn ? IN : 1));
@@ -2497,7 +2638,8 @@ extern "C" int b200rl_offpolicy_set_state(b200rl_offpolicy* h, const float* blob
 
 extern "C" int b200rl_offpolicy_set_sac(b200rl_offpolicy* h, const b200rl_sac_hparams* sp) {
   B200RL_REQUIRE(h && sp, "offpolicy_set_sac: NULL argument");
-  B200RL_REQUIRE(h->sac, "offpolicy_set_sac: the engine was not created with algo = 1 (SAC)");
+  B200RL_REQUIRE(h->sac || h->dsac, "offpolicy_set_sac: the engine was not created with algo = 1 (SAC) or 5 (discrete "
+                 "SAC)");
   B200RL_REQUIRE(sp->learn_alpha == 0 || sp->learn_alpha == 1, "offpolicy_set_sac: learn_alpha must be 0 or 1");
   B200RL_REQUIRE(sp->log_std_min <= sp->log_std_max, "offpolicy_set_sac: log_std_min > log_std_max");
   h->sac_hp = *sp;
@@ -2508,6 +2650,8 @@ extern "C" int b200rl_offpolicy_set_sac(b200rl_offpolicy* h, const b200rl_sac_hp
 
 extern "C" int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hparams* dp) {
   B200RL_REQUIRE(h && dp, "offpolicy_set_dqn: NULL argument");
+  B200RL_REQUIRE(!h->dsac, "offpolicy_set_dqn: a discrete SAC engine (algo = 5) takes b200rl_offpolicy_set_sac, not "
+                 "set_dqn");
   B200RL_REQUIRE(h->dqn, "offpolicy_set_dqn: the engine was not created with algo = 2 (DQN)");
   B200RL_REQUIRE(dp->target_update_interval >= 1, "offpolicy_set_dqn: target_update_interval must be >= 1, got %d",
                  dp->target_update_interval);
@@ -2519,6 +2663,7 @@ extern "C" int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hp
 
 extern "C" int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hparams* cp) {
   B200RL_REQUIRE(h && cp, "offpolicy_set_c51: NULL argument");
+  B200RL_REQUIRE(!h->dsac, "offpolicy_set_c51: a discrete SAC engine (algo = 5) has no categorical head");
   B200RL_REQUIRE(h->c51, "offpolicy_set_c51: the engine was not created with algo = 3 (C51)");
   const int N = cp->n_atoms, width = h->net[1].d.sizes[h->net[1].d.n_layers];
   B200RL_REQUIRE(N >= 2 && N <= C51_MAX_ATOMS, "offpolicy_set_c51: n_atoms must be 2..%d, got %d", C51_MAX_ATOMS, N);
@@ -2546,6 +2691,7 @@ extern "C" int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hp
 
 extern "C" int b200rl_offpolicy_set_qr(b200rl_offpolicy* h, const b200rl_qr_hparams* qp) {
   B200RL_REQUIRE(h && qp, "offpolicy_set_qr: NULL argument");
+  B200RL_REQUIRE(!h->dsac, "offpolicy_set_qr: a discrete SAC engine (algo = 5) has no quantile head");
   B200RL_REQUIRE(h->dqn && !h->c51 && !h->iqn, "offpolicy_set_qr: the engine was not created with algo = 2 (DQN)");
   const int N = qp->n_quantiles, width = h->net[1].d.sizes[h->net[1].d.n_layers];
   B200RL_REQUIRE(N >= 1 && N <= QR_MAX_QUANTILES, "offpolicy_set_qr: n_quantiles must be 1..%d, got %d",
@@ -2562,6 +2708,8 @@ extern "C" int b200rl_offpolicy_set_qr(b200rl_offpolicy* h, const b200rl_qr_hpar
 
 extern "C" int b200rl_offpolicy_set_per(b200rl_offpolicy* h, const b200rl_per_hparams* pp) {
   B200RL_REQUIRE(h && pp, "offpolicy_set_per: NULL argument");
+  B200RL_REQUIRE(!h->dsac, "offpolicy_set_per: prioritized replay is not implemented for discrete SAC engines (algo = "
+                 "5)");
   B200RL_REQUIRE(!h->c51, "offpolicy_set_per: prioritized replay is not implemented for C51 engines");
   B200RL_REQUIRE(h->dqn, "offpolicy_set_per: prioritized replay is implemented for DQN engines (algo = 2) only");
   B200RL_REQUIRE(pp->alpha >= 0.0 && std::isfinite(pp->alpha), "offpolicy_set_per: alpha must be >= 0");
@@ -2575,6 +2723,8 @@ extern "C" int b200rl_offpolicy_set_per(b200rl_offpolicy* h, const b200rl_per_hp
 
 extern "C" int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, const float* const* episode_ends) {
   B200RL_REQUIRE(h, "offpolicy_set_nstep: NULL engine");
+  B200RL_REQUIRE(!h->dsac, "offpolicy_set_nstep: n-step returns are not implemented for discrete SAC engines (algo = "
+                 "5)");
   B200RL_REQUIRE(h->dqn, "offpolicy_set_nstep: n-step returns are implemented for DQN and C51 engines (algo = 2 or 3) "
                  "only");
   B200RL_REQUIRE(n_step >= 1 && n_step <= NSTEP_MAX, "offpolicy_set_nstep: n_step must be 1..%d, got %d", NSTEP_MAX,
@@ -2594,6 +2744,7 @@ extern "C" int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, c
 
 extern "C" int b200rl_offpolicy_set_noise_keys(b200rl_offpolicy* h, const uint64_t* seed, const uint64_t* call) {
   B200RL_REQUIRE(h && seed && call, "offpolicy_set_noise_keys: NULL argument");
+  B200RL_REQUIRE(!h->dsac, "offpolicy_set_noise_keys: a discrete SAC engine (algo = 5) draws no noise");
   B200RL_REQUIRE(h->noisy || h->iqn, "offpolicy_set_noise_keys: the engine has no noisy layers (config noisy_layers = "
                  "0)");
   const size_t n = adam_tab_len(h);
@@ -2626,7 +2777,7 @@ extern "C" int b200rl_offpolicy_get_iqn_draws(b200rl_offpolicy* h, int32_t S, fl
 
 extern "C" int b200rl_offpolicy_set_alpha_group(b200rl_offpolicy* h, const float* log_alpha, const float* exp_avg,
                                                 const float* exp_avg_sq, const int64_t* step) {
-  B200RL_REQUIRE(h && h->sac, "offpolicy_set_alpha: not a SAC engine");
+  B200RL_REQUIRE(h && (h->sac || h->dsac), "offpolicy_set_alpha: not a SAC engine");
   B200RL_REQUIRE(log_alpha && exp_avg && exp_avg_sq && step, "offpolicy_set_alpha: NULL argument");
   float v[B200RL_MAX_LEARNERS][3];
   for (int z = 0; z < h->K; ++z) {
@@ -2642,7 +2793,8 @@ extern "C" int b200rl_offpolicy_set_alpha_group(b200rl_offpolicy* h, const float
 
 extern "C" int b200rl_offpolicy_get_alpha_group(b200rl_offpolicy* h, float* log_alpha, float* exp_avg,
                                                 float* exp_avg_sq, int64_t* step) {
-  B200RL_REQUIRE(h && h->sac && log_alpha && exp_avg && exp_avg_sq && step, "offpolicy_get_alpha: bad arguments");
+  B200RL_REQUIRE(h && (h->sac || h->dsac) && log_alpha && exp_avg && exp_avg_sq && step,
+                 "offpolicy_get_alpha: bad arguments");
   float v[B200RL_MAX_LEARNERS][3];
   B200RL_CUDA(cudaMemcpy2DAsync(v, sizeof(v[0]), h->sac_state, h->lane_stride, sizeof(v[0]), h->K,
                                 cudaMemcpyDeviceToHost, h->gs));
@@ -2667,7 +2819,7 @@ extern "C" int b200rl_offpolicy_get_alpha(b200rl_offpolicy* h, float* log_alpha,
 }
 
 extern "C" int b200rl_offpolicy_sac_outputs(b200rl_offpolicy* h, int32_t S, float* log_prob_means, float* alphas) {
-  B200RL_REQUIRE(h && h->sac && log_prob_means && alphas && S >= 0 && S <= h->cfg.max_steps,
+  B200RL_REQUIRE(h && (h->sac || h->dsac) && log_prob_means && alphas && S >= 0 && S <= h->cfg.max_steps,
                  "offpolicy_sac_outputs: bad arguments");
   const size_t w = (size_t)S * 4;
   if (S > 0) {
@@ -2911,6 +3063,119 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
   return 0;
 }
 
+// The S discrete SAC steps (Christodoulou 2019: one critic step, one policy step, the optional temperature step and
+// polyak; the order of enqueue_sac_steps).  Per step the branches are:
+//   s  : pi(s') -> Q1targ(s') ---+-> Q1 head -> Q1 bwd, Adam -+-> Q1(s) -+-> policy head -> pi bwd, Adam -+->
+//   s2 :           Q2targ(s') ---+-> Q2 head -> Q2 bwd, Adam -+-> Q2(s) -+   -> temperature step --------+
+//   s3 : Q1(s) -> pi(s) ........... Q1's dW products ....................... pi's dW products
+//   s4 : Q2(s) .................... Q2's dW products -> polyak (both critic pairs)
+// The heads need no input gradient of any network: every backward pass is the weight-gradient products and the dX
+// chain down to the first hidden layer.  pi(s) is the policy at the start of the step (it is updated last); the
+// policy head reads the critics just updated, with no gradient into them.  Step st reads alpha[st]; the temperature
+// step writes alpha[st + 1] from the policy head's E_i.
+static int enqueue_dsac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s) {
+  const int O = h->O;
+  const int maxS = h->cfg.max_steps;
+  const b200rl_sac_hparams& sp = h->sac_hp;
+  NetBuf &pi = h->net[0], &q1 = h->net[1], &q2 = h->net[2], &q1t = h->net[4], &q2t = h->net[5];
+  const int Lq = q1.d.n_layers, Lp = pi.d.n_layers, n = q1.d.sizes[Lq];
+  const int ew = 256;
+  cudaStream_t s2 = h->s2, s3 = h->s3, s4 = h->s4;
+  if (launch(h, sac_alpha_init_kernel<false>, sac_alpha_init_kernel<true>, (S + 1 + ew - 1) / ew, ew, 0, s,
+             h->sac_alpha, S + 1, h->sac_state, sp.learn_alpha, (float)sp.alpha))
+    return 1;
+  PolyakArgs pk{};  // 1 -> 4, 2 -> 5
+  pk.n_nets = 2;
+  for (int k = 0; k < 2; ++k) {
+    pk.target[k] = h->net[4 + k].params;
+    pk.param[k] = h->net[1 + k].params;
+    pk.n[k] = (int)h->net[1 + k].P;
+  }
+  for (int st = 0; st < S; ++st) {
+    float* s_obs = h->obs + (size_t)st * B * O;
+    const float* s_act = h->act + (size_t)st * B;
+    const float* s_rew = h->rew + (size_t)st * B;
+    float* s_nobs = h->nobs + (size_t)st * B * O;
+    const float* s_done = h->done + (size_t)st * B;
+    const float* alpha = h->sac_alpha + st;
+    // ---- the critics on s (the logged Q-values); pi(s) with the pre-update policy behind Q1's ----
+    float* qa[2][B200RL_MAX_LAYERS + 1];
+    for (int qi = 0; qi < 2; ++qi) {
+      qa[qi][0] = s_obs;
+      for (int l = 1; l <= Lq; ++l) qa[qi][l] = h->acts[qi == 0 ? 1 : 4][l];
+      cudaStream_t qs = qi == 0 ? s3 : s4;
+      if (edge(h, s, qs)) return 1;
+      if (net_forward(h, qi == 0 ? q1 : q2, qa[qi], B, qs)) return 1;
+    }
+    float* pa[B200RL_MAX_LAYERS + 1];
+    pa[0] = s_obs;
+    for (int l = 1; l <= Lp; ++l) pa[l] = h->acts[2][l];
+    if (net_forward(h, pi, pa, B, s3)) return 1;
+    // ---- soft targets: pi(s') and both target critics on s' ----
+    float* ta[B200RL_MAX_LAYERS + 1];
+    ta[0] = s_nobs;
+    for (int l = 1; l <= Lp; ++l) ta[l] = h->acts[0][l];
+    float* tq[2][B200RL_MAX_LAYERS + 1];
+    for (int qi = 0; qi < 2; ++qi) {
+      tq[qi][0] = s_nobs;
+      for (int l = 1; l <= Lq; ++l) tq[qi][l] = qi == 0 ? h->acts_tq[l] : h->acts[3][l];
+    }
+    if (edge(h, s, s2)) return 1;
+    if (net_forward(h, q2t, tq[1], B, s2)) return 1;
+    if (net_forward(h, pi, ta, B, s)) return 1;
+    if (net_forward(h, q1t, tq[0], B, s)) return 1;
+    if (edge(h, s2, s)) return 1;
+    // ---- critic step: V(s'), y, MSE and dOut in each head, weight-gradient backward, Adam (Q2 on s2, Q1 on s) ----
+    if (edge(h, s, s2)) return 1;
+    if (edge(h, s4, s2)) return 1;
+    if (edge(h, s3, s)) return 1;
+    for (int qi = 1; qi >= 0; --qi) {
+      NetBuf& qn = qi == 0 ? q1 : q2;
+      cudaStream_t qs = qi == 0 ? s : s2;
+      float* dq = qi == 0 ? h->dq : h->dq2;
+      if (launch(h, dsac_q_loss_kernel<false>, dsac_q_loss_kernel<true>, 1, GTHREADS, 0, qs, qa[qi][Lq], ta[Lp],
+                 tq[0][Lq], tq[1][Lq], s_act, s_rew, s_done, alpha, (float)hp->gamma, B, n, dq,
+                 (qi == 0 ? h->out_l1 : h->out_l2) + st, (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B,
+                 qi == 0 ? h->dqn_bad + st : nullptr))
+        return 1;
+      if (net_backward(h, qn, qa[qi], dq, n, B, true, nullptr, qs, qi != 0, nullptr, 0, 0, qi == 0 ? s3 : s4)) return 1;
+      if (adam_net(h, qn, h->adam_tab + (size_t)(1 + qi) * maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, qs)) return 1;
+    }
+    if (edge(h, s2, s)) return 1;
+    // ---- polyak beside the policy step: the targets are next read by the next step ----
+    if (edge(h, s, s4)) return 1;
+    if (launch(h, polyak_kernel<false>, polyak_kernel<true>, (pk.n[0] + ew - 1) / ew, ew, 0, s4, pk,
+               (float)hp->polyak_rho, (float)(1.0 - hp->polyak_rho)))
+      return 1;
+    // ---- policy step: both updated critics on s, the head, pi's backward pass and Adam ----
+    float* qp[2][B200RL_MAX_LAYERS + 1];
+    for (int qi = 0; qi < 2; ++qi) {
+      qp[qi][0] = s_obs;
+      for (int l = 1; l <= Lq; ++l) qp[qi][l] = h->acts[qi == 0 ? 1 : 4][l];
+    }
+    if (edge(h, s, s2)) return 1;
+    if (net_forward(h, q2, qp[1], B, s2)) return 1;
+    if (net_forward(h, q1, qp[0], B, s)) return 1;
+    if (edge(h, s2, s)) return 1;
+    if (launch(h, dsac_policy_loss_kernel<false>, dsac_policy_loss_kernel<true>, 1, GTHREADS, 0, s, pa[Lp], qp[0][Lq],
+               qp[1][Lq], alpha, B, n, h->sac_dout, h->sac_logp, h->out_lp + st, h->out_logp + st))
+      return 1;
+    if (sp.learn_alpha) {  // -mean(log_alpha (E_i + target_entropy)), one Adam step; alpha[st + 1] = exp(log_alpha)
+      if (edge(h, s, s2)) return 1;
+      if (launch(h, sac_alpha_step_kernel<false>, sac_alpha_step_kernel<true>, 1, GTHREADS, 0, s2, h->sac_logp, B,
+                 (float)sp.target_entropy, h->sac_state, h->adam_tab + (size_t)3 * maxS, st,
+                 (float)(1.0 - sp.alpha_beta1), (float)sp.alpha_beta2, (float)(1.0 - sp.alpha_beta2),
+                 (float)sp.alpha_eps, h->sac_alpha + st + 1))
+        return 1;
+    }
+    if (net_backward(h, pi, pa, h->sac_dout, n, B, true, nullptr, s, false, nullptr, 0, 0, s3)) return 1;
+    if (adam_net(h, pi, h->adam_tab, st, hp->policy_beta1, hp->policy_beta2, hp->policy_eps, s)) return 1;
+    if (sp.learn_alpha && edge(h, s2, s)) return 1;
+    if (edge(h, s4, s)) return 1;
+  }
+  return 0;
+}
+
 // dqn_loss_kernel<LANES, WEIGHTED, NSTEP> of a call: WEIGHTED for prioritized replay, NSTEP for n-step returns
 template <bool LANES>
 static auto dqn_head(bool weighted, bool nstep) {
@@ -3086,6 +3351,10 @@ static int enqueue_program(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* 
     *n_pol = S;
     return enqueue_sac_steps(h, hp, S, B, s);
   }
+  if (h->dsac) {
+    *n_pol = S;
+    return enqueue_dsac_steps(h, hp, S, B, s);
+  }
   if (h->dqn) return enqueue_dqn_steps(h, hp, S, B, s);
   return enqueue_steps(h, hp, S, B, s, n_pol);
 }
@@ -3104,9 +3373,9 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   // Adam's step-dependent scalars for the steps of this call (torch's host-side double arithmetic), one small upload
   // (a group: one table per learner, from that learner's step counts, uploaded with one strided copy)
   const int maxS = h->cfg.max_steps;
-  const int n_pol_expected = h->dqn ? 0 : h->sac ? S : (S + hp->policy_delay - 1) / hp->policy_delay;  // SAC: no delay
+  const int n_pol_expected = h->dqn ? 0 : h->sac || h->dsac ? S : (S + hp->policy_delay - 1) / hp->policy_delay;  // SAC: no delay
   const size_t tab_n = adam_tab_len(h);
-  const bool learn_alpha = h->sac && h->sac_hp.learn_alpha;
+  const bool learn_alpha = (h->sac || h->dsac) && h->sac_hp.learn_alpha;
   for (int z = 0; z < h->K; ++z) {
     float2* tab = h->h_adam_tab + z * tab_n;
     for (int k = 0; k < n_pol_expected; ++k)
@@ -3191,8 +3460,8 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   if (n_pol > 0)
     B200RL_CUDA(cudaMemcpy2DAsync(policy_losses, (size_t)S * 4, h->out_lp, ls, (size_t)n_pol * 4, K,
                                   cudaMemcpyDeviceToHost, s));
-  std::vector<int> bad(h->dqn ? K * S : 0), per_bad(h->per_run ? K * S : 0);
-  if (h->dqn)
+  std::vector<int> bad(h->dqn || h->dsac ? K * S : 0), per_bad(h->per_run ? K * S : 0);
+  if (h->dqn || h->dsac)
     B200RL_CUDA(cudaMemcpy2DAsync(bad.data(), (size_t)S * 4, h->dqn_bad, ls, (size_t)S * 4, K, cudaMemcpyDeviceToHost, s));
   if (h->per_run)
     B200RL_CUDA(cudaMemcpy2DAsync(per_bad.data(), (size_t)S * 4, h->per_bad, ls, (size_t)S * 4, K,
@@ -3201,7 +3470,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   *n_policy_updates = n_pol;
   const int n_actions = h->net[1].d.sizes[h->net[1].d.n_layers] /
                         (h->c51 ? h->c51_hp.n_atoms : h->qr ? h->qr_hp.n_quantiles : 1);
-  const char* algo = h->c51 ? "C51" : h->qr ? "QR-DQN" : h->iqn ? "IQN" : "DQN";
+  const char* algo = h->c51 ? "C51" : h->qr ? "QR-DQN" : h->iqn ? "IQN" : h->dsac ? "discrete SAC" : "DQN";
   for (size_t i = 0; i < bad.size(); ++i)
     B200RL_REQUIRE(bad[i] == 0, "offpolicy_train: %s learner %d, step %d: %d minibatch rows hold an action that is not "
                    "an integer in [0, %d); those rows were left out of the update", algo, (int)(i / S), (int)(i % S),
@@ -3222,12 +3491,15 @@ static int train_begin(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, 
   B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
                  "%s: S=%d B=%d exceed the capacities", what, S, B);
   B200RL_REQUIRE(h->cfg.n_q != 2 || q2_given, "%s: TD3 needs the Q2 outputs", what);
-  B200RL_REQUIRE(h->dqn || !hp->use_target_noise || noise_given, "%s: target noise requested but no noise given", what);
-  B200RL_REQUIRE(h->dqn || hp->policy_delay >= 1, "%s: policy_delay must be >= 1", what);
+  B200RL_REQUIRE(h->dqn || h->dsac || !hp->use_target_noise || noise_given, "%s: target noise requested but no noise "
+                 "given", what);
+  B200RL_REQUIRE(h->dqn || h->dsac || hp->policy_delay >= 1, "%s: policy_delay must be >= 1", what);
   if (h->sac) {
     B200RL_REQUIRE(h->sac_set, "%s: a SAC engine needs b200rl_offpolicy_set_sac before it trains", what);
     B200RL_REQUIRE(noise_given, "%s: SAC needs the noise draws [S, 2, B, A]", what);
   }
+  B200RL_REQUIRE(!h->dsac || h->sac_set, "%s: a discrete SAC engine needs b200rl_offpolicy_set_sac before it trains",
+                 what);
   if (h->dqn) {
     B200RL_REQUIRE(h->dqn_set, "%s: a DQN engine needs b200rl_offpolicy_set_dqn before it trains", what);
     B200RL_REQUIRE(!h->c51 || h->c51_set, "%s: a C51 engine needs b200rl_offpolicy_set_c51 before it trains", what);
@@ -3272,7 +3544,7 @@ extern "C" int b200rl_offpolicy_train(b200rl_offpolicy* h, const b200rl_offpolic
       up(h->nobs, next_obs, SB * O * 4) || up(h->done, done, SB * 4))
     return 1;
   if (h->sac && up(h->eps, noise, 2 * SB * A * 4)) return 1;
-  if (!h->sac && !h->dqn && hp->use_target_noise && up(h->eps, noise, SB * A * 4)) return 1;
+  if (!h->sac && !h->dqn && !h->dsac && hp->use_target_noise && up(h->eps, noise, SB * A * 4)) return 1;
 
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
 }
@@ -3344,7 +3616,7 @@ extern "C" int b200rl_offpolicy_train_gather_group(b200rl_offpolicy* h, const b2
   // the minibatches are gathered on the device from the replay columns: only the indices (and noise) cross PCIe
   const size_t ls = h->lane_stride;
   B200RL_CUDA(cudaMemcpy2DAsync(h->idx, ls, idx, SB * 8, SB * 8, h->K, cudaMemcpyHostToDevice, s));
-  const size_t n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise && !h->dqn ? SB * A : 0);
+  const size_t n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise && !h->dqn && !h->dsac ? SB * A : 0);
   if (n_eps) B200RL_CUDA(cudaMemcpy2DAsync(h->eps, ls, noise, n_eps * 4, n_eps * 4, h->K, cudaMemcpyHostToDevice, s));
   if (gather_columns(h, hp, (long long)SB, s)) return 1;
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
@@ -3392,7 +3664,8 @@ extern "C" int b200rl_offpolicy_train_gather_rng_group(b200rl_offpolicy* h, cons
   cudaStream_t s = h->gs;
   const int A = h->A;
   const long long SB = (long long)S * B;
-  const long long n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise && !h->dqn ? SB * A : 0);  // DQN: indices only
+  // DQN and discrete SAC: indices only
+  const long long n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise && !h->dqn && !h->dsac ? SB * A : 0);
   const long long n_thr = ((SB > n_eps ? SB : n_eps) + 3) / 4;
   DrawKeys<true> keys{};
   for (int z = 0; z < h->K; ++z)
@@ -3447,6 +3720,8 @@ extern "C" int b200rl_offpolicy_train_prioritized_group(b200rl_offpolicy* h, con
   B200RL_REQUIRE(h && hp && trees && seed && call && q1_values && q1_losses,
                  "offpolicy_train_prioritized: NULL argument");
   B200RL_REQUIRE(!h->c51, "offpolicy_train_prioritized: prioritized replay is not implemented for C51 engines");
+  B200RL_REQUIRE(!h->dsac, "offpolicy_train_prioritized: prioritized replay is not implemented for discrete SAC "
+                 "engines (algo = 5)");
   B200RL_REQUIRE(h->dqn, "offpolicy_train_prioritized: prioritized replay is implemented for DQN engines (algo = 2) "
                  "only");
   B200RL_REQUIRE(h->per_set, "offpolicy_train_prioritized: call b200rl_offpolicy_set_per first");

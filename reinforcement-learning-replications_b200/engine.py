@@ -331,14 +331,19 @@ class OffPolicyEngine:
     layers in flat order; every train call then needs ``set_noise_keys`` first (b200rl.h, "Noisy networks").  IQN
     (``algo`` 4) is a DQN engine over an implicit quantile network: ``q_sizes`` = [obs, d, h, n actions] and ``iqn`` =
     (n_cos, N, N', K); every train call needs ``set_noise_keys`` first, the keys of its fraction draws (b200rl.h, "IQN").
+    Discrete SAC (``algo`` 5) has SAC's networks, temperature and outputs over a discrete action space: the policy maps
+    obs -> [n] logits, both critics obs -> [n] values, actions are indices (act [S,B]) as for DQN, no noise is used,
+    and ``set_sac`` must be called before the first train call (b200rl.h, "Discrete SAC").
 
     ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
     launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
     is [K][per-learner blob] with [K][3] step counts, and the per-network accessors are refused."""
 
     NETS = {"policy": 0, "q1": 1, "q2": 2, "target_policy": 3, "target_q1": 4, "target_q2": 5}
-    TD3, SAC, DQN, C51, IQN = 0, 1, 2, 3, 4
+    TD3, SAC, DQN, C51, IQN, DSAC = 0, 1, 2, 3, 4, 5
     DISCRETE = (DQN, C51, IQN)  # the algos with DQN's networks, inputs and outputs
+    INDEX_ACTIONS = DISCRETE + (DSAC,)  # the algos whose action column holds an action index
+    SOFT = (SAC, DSAC)  # the algos with SAC's networks, temperature and outputs
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
                  q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1, dueling_k: int = 0,
@@ -354,7 +359,8 @@ class OffPolicyEngine:
         cfg.algo, cfg.dueling_k, cfg.noisy_layers = int(algo), int(dueling_k), int(noisy_layers)
         self.algo, self.dueling_k, self.noisy_layers = int(algo), int(dueling_k), int(noisy_layers)
         self.iqn = None if iqn is None else tuple(int(x) for x in iqn)
-        self.discrete = self.algo in self.DISCRETE
+        self.discrete = self.algo in self.DISCRETE  # DQN's networks and outputs
+        self.index_actions = self.algo in self.INDEX_ACTIONS  # act [S,B] indices, no noise
         self.n_q, self.max_minibatch, self.max_steps = int(n_q), int(max_minibatch), int(max_steps)
         self.policy_sizes, self.q_sizes = None if policy_sizes is None else list(policy_sizes), list(q_sizes)
         self.policy_acts, self.q_acts = tuple(policy_acts), tuple(q_acts)
@@ -434,7 +440,7 @@ class OffPolicyEngine:
         if self.discrete:
             present, optimized = [1, 4], [1]
         else:
-            present = [0, 1] + ([2] if self.n_q == 2 else []) + ([] if self.algo == self.SAC else [3]) + [4] + \
+            present = [0, 1] + ([2] if self.n_q == 2 else []) + ([] if self.algo in self.SOFT else [3]) + [4] + \
                 ([5] if self.n_q == 2 else [])
             optimized = [0, 1] + ([2] if self.n_q == 2 else [])
         out, off = [], 0
@@ -658,7 +664,7 @@ class OffPolicyEngine:
             out = dict(q1_values=q1v, q2_values=q2v, q1_losses=l1, q2_losses=l2, policy_losses=lp[:, :npol.value])
         if self.K == 1:
             out = {k: v[0] for k, v in out.items()}
-        if self.algo == self.SAC:
+        if self.algo in self.SOFT:
             out["log_prob_means"], out["alphas"] = self.sac_outputs(S)
         return out
 
@@ -674,8 +680,9 @@ class OffPolicyEngine:
     def train(self, hp, obs, act, rew, next_obs, done, noise=None):
         """obs/next_obs [S,B,O], act [S,B,A], rew/done [S,B], noise [S,B,A] or None (SAC: [S,2,B,A], required) -> dict
         of logged quantities (SAC adds log_prob_means and alphas).  A group: every array with a leading [K] axis.
-        DQN: act [S,B] action indices, noise None; the dict holds q1_values and q1_losses."""
-        if self.discrete:
+        DQN: act [S,B] action indices, noise None; the dict holds q1_values and q1_losses.  Discrete SAC: act [S,B]
+        action indices, noise None; the dict is SAC's."""
+        if self.index_actions:
             act = np.asarray(act, np.float32)[..., None]
         obs, act, next_obs = (self._lead(x, np.float32, 4) for x in (obs, act, next_obs))
         rew, done = self._lead(rew, np.float32, 3), self._lead(done, np.float32, 3)
@@ -710,7 +717,7 @@ class OffPolicyEngine:
         """(physical rows [S,B] int64, noise [S,B,A] (SAC: [S,2,B,A]) float32 or None) of the last train_gather /
         train_gather_rng call; a group: both with a leading [K] axis."""
         idx = np.empty((self.K, S, B), np.int64)
-        with_noise = with_noise and not self.discrete  # DQN and C51 draw indices only
+        with_noise = with_noise and not self.index_actions  # DQN, C51 and discrete SAC draw indices only
         noise = None
         if with_noise and self.algo == self.SAC:
             noise = np.empty((self.K, S, 2, B, self.policy_sizes[-1] // 2), np.float32)

@@ -342,7 +342,8 @@ typedef struct {
   int32_t algo;            /* 0 = DDPG / TD3 (by n_q), 1 = SAC (see b200rl_offpolicy_set_sac), 2 = DQN (see
                             * b200rl_offpolicy_set_dqn), 3 = C51 (see b200rl_offpolicy_set_c51), 4 = IQN (created by
                             * b200rl_offpolicy_create_iqn only; see "IQN" below), 5 = discrete SAC (see
-                            * "Discrete SAC" below) */
+                            * "Discrete SAC" below), 6 = D4PG (created by b200rl_offpolicy_create_d4pg only; see
+                            * "D4PG" below) */
   int32_t dueling_k;       /* 0 = the Q network is a plain MLP; K >= 1 = a dueling Q network (algo 2 / 3 only; see
                             * "Dueling Q networks" below) */
   int32_t noisy_layers;    /* bit mask over the Q network's Linear layers in flat order: 0 = none; bit l = layer l is a
@@ -693,6 +694,51 @@ int b200rl_offpolicy_create_iqn(const b200rl_offpolicy_config* cfg, const b200rl
 int b200rl_offpolicy_get_iqn_draws(b200rl_offpolicy* h, int32_t S, float* taus);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * D4PG on the same engine (config algo = 6, n_q = 1; Barth-Maron et al. 2018, "Distributed Distributional
+ * Deterministic Policy Gradients"): DDPG with a categorical critic, n-step returns and prioritized replay.  Created by
+ * b200rl_offpolicy_create_d4pg from a config with algo = 6 and a b200rl_d4pg_config; b200rl_offpolicy_create and
+ * create_group refuse algo 6.  Networks are DDPG's (0 policy, 1 critic, 3 target policy, 4 target critic), so the state
+ * blob, steps[3], hparams and outputs keep DDPG's layout.  policy = [obs, ..., A] is DDPG's deterministic policy,
+ * q = [obs + A, ..., N] maps [s | a] to N logits over the support.  With N = n_atoms, in float32:
+ *   support  dz = (v_max - v_min) / (N - 1), z_i = float32(v_min + i dz), both evaluated in double (C51's)
+ *   p(s, a)  = exp(log_softmax) of the N logits, x - max - log(sum exp(x - max)); Q(s, a) = sum_i z_i p_i(s, a), every
+ *            sum over atoms in index order
+ *   target   a' = mu_targ(s') (no smoothing: hparams.use_target_noise must be 0); Tz_j = clamp(r + g (1 - d) z_j,
+ *            v_min, v_max), g = gamma (n-step: the row's discount), b_j = (Tz_j - v_min) / dz,
+ *            m_i = sum_j max(0, 1 - |b_j - i|) p_j(s', a') from the target critic (C51's projection)
+ *   critic   CE_b = -sum_i m_i log p_i(s, a); one Adam step (optimizer 1) on (1/B) sum_b w_b CE_b (w_b = 1 without
+ *            prioritized replay); the logit gradient is w_b (p_i(s, a) sum_k m_k - m_i) / B
+ *   policy   with the critic just updated: one Adam step (optimizer 0) on -(1/B) sum_b Q(s_b, mu(s_b)); the gradient
+ *            w.r.t. the critic's logits is -(1/B) p_k (z_k - Q), backpropagated through the critic's action input
+ *            columns into the policy (critic parameters frozen), as DDPG's is
+ *   polyak   both targets, every policy step (hparams.policy_delay applies as for DDPG; D4PG uses 1)
+ * Outputs: q1_values [S,B] = Q(s, a) before the update, q1_losses [S] = the weighted mean CE (summed in double),
+ * policy_losses = -mean Q per policy step.  Prioritized replay (the section below): the draw gathers A action columns,
+ * beta follows the critic optimizer's count, and the priority of row b is (KL_b + eps)^alpha with
+ * KL_b = CE_b + sum_i m_i log m_i (0 log 0 = 0; a rounding-level negative KL counts as 0), from before the Adam step;
+ * with every w_b = 1 loss and gradient are bit for bit the unweighted step's.  n-step returns as the section below
+ * states them (set_nstep).  train_prioritized[_group] return no policy losses: b200rl_offpolicy_get_policy_losses reads
+ * them.  The heads reduce in a fixed order with no float atomics: a group's learners stay bit-identical to solo engines.
+ * Runs as a CUDA graph, or as plain launches with B200RL_OFFPOLICY_GRAPH=0.  Launches per step are DDPG's (the two
+ * heads take the places of its two loss kernels); a prioritized step adds its draw and priority update (2).
+ * Refused at create: create_d4pg with another algo, algo 6 through create / create_group; n_q != 1; dueling_k or
+ * noisy_layers != 0; n_atoms outside 2..256; a non-finite support or v_min >= v_max; a critic that does not map
+ * obs + A -> N.  set_c51, set_qr, set_dqn, set_sac and set_noise_keys refuse a D4PG engine.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t n_atoms;  /* N, 2..256: the critic's output width */
+  int32_t reserved; /* ignored */
+  double v_min, v_max; /* finite, v_min < v_max */
+} b200rl_d4pg_config;
+
+/* A D4PG engine of n_learners learners (1 = a solo engine; 1 <= n_learners <= B200RL_MAX_LEARNERS): cfg->algo = 6. */
+int b200rl_offpolicy_create_d4pg(const b200rl_offpolicy_config* cfg, const b200rl_d4pg_config* d4pg,
+                                 int32_t n_learners, b200rl_offpolicy** out);
+/* The policy losses of the last train call that ran steps (host [K, S]; the first *n_policy_updates of each row):
+ * what a prioritized call, which takes no policy-loss buffer, logged.  Refused on DQN engines. */
+int b200rl_offpolicy_get_policy_losses(b200rl_offpolicy* h, int32_t S, float* policy_losses, int32_t* n_policy_updates);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Learner groups: K independent off-policy learners (same config, same hyper-parameters, their own parameters, Adam
  * states, step counts, minibatches, noise, replay buffers and temperature) trained by one engine, every operation of a
  * step ONE launch for all K.  Each learner's arithmetic -- tile shapes, summation order, Adam's operation order -- is
@@ -770,7 +816,8 @@ typedef struct {
   int64_t beta_anneal_steps; /* >= 1 */
 } b200rl_per_hparams;
 
-/* Required before a prioritized call of a DQN engine (other engines are refused); part of the cached graph's key. */
+/* Required before a prioritized call of a DQN or D4PG engine (other engines are refused); part of the cached graph's
+ * key. */
 int b200rl_offpolicy_set_per(b200rl_offpolicy* h, const b200rl_per_hparams* pp);
 /* S prioritized DQN steps on device replay columns (as for train_gather) with `rows` physical rows and their tree
  * (rows leaves, device memory).  (seed, call) key the draws.  Outputs as for DQN: q1_values [S,B], q1_losses [S]. */
@@ -809,7 +856,7 @@ int b200rl_offpolicy_get_per_draws(b200rl_offpolicy* h, int32_t S, int32_t B, in
  * ------------------------------------------------------------------------------------------------------------ */
 /* n_step 1..32 for the engine's next train calls (1 clears it); episode_ends[K] = each learner's device episode-end
  * column over the `rows` of the replay passed to the next call (required for n_step > 1; buffers that grow reallocate,
- * so set it before every call).  Refused on TD3, DDPG and SAC engines.  n_step is part of the cached graph's key, and so
+ * so set it before every call).  Refused on TD3, DDPG and SAC engines (D4PG engines take it).  n_step is part of the cached graph's key, and so
  * are the columns on the prioritized path (its draw walks them inside the graph). */
 int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, const float* const* episode_ends);
 /* Of the last n-step call (host [K, S, B] each): each row's last window row, its return R and its discount g -- what a

@@ -1,4 +1,5 @@
 from .c51 import C51
+from .d4pg import D4PG
 from .discrete_sac import DiscreteSAC
 from .dqn import DQN
 from .group import LearnerGroup
@@ -10,4 +11,4 @@ from .td3 import DDPG, TD3
 from .trpo import TRPO
 from .vpg import VPG
 
-__all__ = ["VPG", "TRPO", "PPO", "DDPG", "TD3", "SAC", "DiscreteSAC", "DQN", "C51", "QRDQN", "IQN", "LearnerGroup"]
+__all__ = ["VPG", "TRPO", "PPO", "DDPG", "D4PG", "TD3", "SAC", "DiscreteSAC", "DQN", "C51", "QRDQN", "IQN", "LearnerGroup"]

@@ -11,7 +11,6 @@ from .._lib import OffPolicyHparams
 from ..engine import OffPolicyEngine
 from ..networks import DuelingMLP, ImplicitQuantileMLP, NoisyLinear
 from ..policies import EpsilonGreedyPolicy, GreedyPolicy, NoisyGreedyPolicy
-from ..replay_buffer import PrioritizedReplayBuffer
 from ._onpolicy import _ACT_NAMES, adam_hparams, describe_mlp
 from .td3 import _learn, _make_eval_env, _OffPolicyBase
 
@@ -193,25 +192,10 @@ class DQN(_OffPolicyBase):
         if self._needs_draw_keys() and S > 0:  # the device draws' keys: this learner's own count of train calls
             self._noise_calls = getattr(self, "_noise_calls", 0) + 1
             self.noise_key = (getattr(self, "device_rng_seed", 0), self._noise_calls)
-        if self.n_step > 1:  # the windows are assembled on the device from the replay ring
-            if not getattr(self, "use_device_replay", True):
-                raise ValueError(f"n_step = {self.n_step} needs use_device_replay = True: n-step windows are assembled on "
-                                 "the device from the replay columns")
-            if not hasattr(replay_buffer, "device_episode_ends"):
-                raise ValueError(f"n_step = {self.n_step} needs a replay buffer with device_episode_ends (a ReplayBuffer "
-                                 f"or PrioritizedReplayBuffer), got {type(replay_buffer).__name__}")
-        if isinstance(replay_buffer, PrioritizedReplayBuffer):
-            # always the prioritized device path, keyed like the uniform device draws (device_rng_seed, call count)
-            if not getattr(self, "use_device_replay", True):
-                raise ValueError("a PrioritizedReplayBuffer needs use_device_replay = True: its draws and priority "
-                                 "updates run on the device")
-            if S == 0:
-                return None, None
-            self._device_rng_calls = getattr(self, "_device_rng_calls", 0) + 1
-            t0 = self._adam_step_count(self.q_function.optimizer, describe_q_network(self.q_function.network)[3])
-            self._last_beta = replay_buffer.beta(t0 + S - 1)  # the last step's beta, logged as replay/beta
-            return "per", (getattr(self, "device_rng_seed", 0), self._device_rng_calls)
-        self._last_beta = None
+        staged = self._stage_nstep_and_prioritized(replay_buffer, S, self.q_function.optimizer,
+                                                   describe_q_network(self.q_function.network)[3])
+        if staged is not None:
+            return staged
         mode, inputs = super()._stage_inputs(replay_buffer, S, B, noisy)
         if mode == "host":  # the action column as [S, B] indices
             obs, act, rew, nobs, done, _ = inputs
@@ -221,14 +205,7 @@ class DQN(_OffPolicyBase):
     def _call_engine(self, e, hp, replay_buffer, S: int, B: int, mode, inputs):
         if mode is not None and self._needs_draw_keys():
             e.set_noise_keys(*([k] for k in self.noise_key))
-        if mode is not None:
-            e.set_nstep(self.n_step, [replay_buffer.device_episode_ends()] if self.n_step > 1 else None)
-        if mode != "per":
-            return _OffPolicyBase._call_engine(e, hp, replay_buffer, S, B, mode, inputs)
-        e.set_per(*replay_buffer.per_settings())
-        tree = replay_buffer.device_tree()
-        columns, rows = replay_buffer.device_columns()
-        return e.train_prioritized(hp, columns, rows, tree, S, B, *inputs)
+        return self._call_nstep_and_prioritized(e, hp, replay_buffer, S, B, mode, inputs)
 
     def _train_schedule(self):
         return False, 1

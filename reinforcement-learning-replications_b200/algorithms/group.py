@@ -1,4 +1,4 @@
-"""LearnerGroup: several independent TD3 / DDPG / SAC / discrete SAC / DQN / C51 / QR-DQN / IQN learners (typically one per seed) trained side by side by ONE
+"""LearnerGroup: several independent TD3 / DDPG / D4PG / SAC / discrete SAC / DQN / C51 / QR-DQN / IQN learners (typically one per seed) trained side by side by ONE
 off-policy engine, every operation of a train step one launch for all of them (b200rl_offpolicy_create_group).
 
 The contract: each member ends up bit for bit where it would be had it run alone.  Members keep everything of their
@@ -61,12 +61,7 @@ def _signature(agent) -> list:
                 sig.append((attr, getattr(agent.q_function, attr)))
         sig.append(("n_quantiles", getattr(agent.q_function, "n_quantiles", None)))
         sig.append(("IQN (n_cos, n_quantiles, n_target_quantiles, n_policy_quantiles)", getattr(agent, "iqn_config", None)))
-        rb = getattr(agent, "replay_buffer", None)
-        sig.append(("prioritized replay", isinstance(rb, PrioritizedReplayBuffer)))
-        for attr in ("alpha", "eps", "beta_start", "beta_anneal_steps"):
-            sig.append((f"prioritized replay {attr}", getattr(rb, attr, None) if isinstance(rb, PrioritizedReplayBuffer)
-                        else None))
-        return sig
+        return sig + _prioritized_signature(agent)
     if agent.algo == OffPolicyEngine.DSAC:
         sig.append(("action count", agent.n_actions))
     else:
@@ -80,7 +75,19 @@ def _signature(agent) -> list:
                  adam_hparams(agent.alpha_optimizer, [], "alpha optimizer", extra=[agent.log_alpha]))]
     if agent.algo == OffPolicyEngine.SAC:
         sig.append(("log_std bounds", (agent.policy.log_std_min, agent.policy.log_std_max)))
+    if agent.algo == OffPolicyEngine.D4PG:
+        sig.append(("(n_atoms, v_min, v_max)", agent.d4pg_config))
+        sig.append(("n_step", agent.n_step))
+        sig += _prioritized_signature(agent)
     return sig
+
+
+def _prioritized_signature(agent) -> list:
+    """Whether the member trains on a PrioritizedReplayBuffer, and its settings (the engine takes one set)."""
+    rb = getattr(agent, "replay_buffer", None)
+    per = isinstance(rb, PrioritizedReplayBuffer)
+    return [("prioritized replay", per)] + [(f"prioritized replay {attr}", getattr(rb, attr, None) if per else None)
+                                            for attr in ("alpha", "eps", "beta_start", "beta_anneal_steps")]
 
 
 def _check_prioritized_buffers(members) -> None:
@@ -121,7 +128,7 @@ class LearnerGroup:
     def add(self, agent) -> None:
         """Add ``agent``; the current state of the global random generators becomes its private stream."""
         if not isinstance(agent, _OffPolicyBase):
-            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or DiscreteSAC / DQN / C51 / QR-DQN / IQN) learners, got {type(agent).__name__}")
+            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or D4PG / DiscreteSAC / DQN / C51 / QR-DQN / IQN) learners, got {type(agent).__name__}")
         if any(m is agent for m in self.members):
             raise ValueError("LearnerGroup: this agent is already a member")
         if len(self.members) >= MAX_LEARNERS:
@@ -166,7 +173,7 @@ class LearnerGroup:
         else:
             psz, pact, pout, _ = describe_mlp(m.policy.network)
             qsz, qact, qout, _ = describe_mlp(m._nets()[0][1].network)
-            kw = dict(dueling_k=0, noisy_layers=0)
+            kw = dict(dueling_k=0, noisy_layers=0, **m._engine_extra())
         e = self._engine
         if (e is None or e.K != len(self.members) or e.max_minibatch < B or e.max_steps < S or e.policy_sizes != psz
                 or e.q_sizes != qsz or e.policy_acts != (pact, pout) or e.q_acts != (qact, qout)
@@ -218,7 +225,7 @@ class LearnerGroup:
         hp = members[0]._hparams(noisy, delay)
         if members[0].algo in OffPolicyEngine.DISCRETE and members[0]._needs_draw_keys():
             e.set_noise_keys(*zip(*[m.noise_key for m in members]))
-        if members[0].algo in OffPolicyEngine.DISCRETE:
+        if members[0].algo in OffPolicyEngine.DISCRETE + (OffPolicyEngine.D4PG,):
             n = members[0].n_step
             e.set_nstep(n, [m.replay_buffer.device_episode_ends() for m in members] if n > 1 else None)
         if mode == "per":

@@ -57,16 +57,22 @@ class _OffPolicyBase:
                 p.requires_grad = False
         return targets
 
+    def _engine_extra(self) -> dict:
+        """OffPolicyEngine arguments beyond the shapes and the algo (D4PG: its critic's support)."""
+        return {}
+
     def _ensure_engine(self, S: int, B: int) -> OffPolicyEngine:
         psz, pact, pout, _ = describe_mlp(self.policy.network)
         trainable, _ = self._nets()
         qsz, qact, qout, _ = describe_mlp(trainable[1].network)
+        kw = self._engine_extra()
         e = getattr(self, "_engine", None)
         if (e is None or e.policy_sizes != psz or e.q_sizes != qsz or e.max_minibatch < B or e.max_steps < S
-                or e.policy_acts != (pact, pout) or e.q_acts != (qact, qout)):
+                or e.policy_acts != (pact, pout) or e.q_acts != (qact, qout)
+                or any(getattr(e, k) != v for k, v in kw.items())):
             if e is not None:
                 e.close()
-            e = OffPolicyEngine(psz, qsz, self.n_q, B, S, (pact, pout), (qact, qout), algo=self.algo)
+            e = OffPolicyEngine(psz, qsz, self.n_q, B, S, (pact, pout), (qact, qout), algo=self.algo, **kw)
             self._engine = e
         return e
 
@@ -232,6 +238,48 @@ class _OffPolicyBase:
             nobs = stack("next_observations", np.float32)
             done = stack("dones", np.float32)                       # bool -> .int() (td3.py:228), used as (1 - d)
             return "host", (obs, act, rew, nobs, done, noise)
+
+    # n-step returns and prioritized replay (DQN's family and D4PG): what _stage_inputs / _call_engine add to the
+    # uniform paths above
+    def _stage_nstep_and_prioritized(self, replay_buffer, S: int, critic_optimizer, critic_linears):
+        """The n-step checks, then for a PrioritizedReplayBuffer the staging of the prioritized device call: its keys
+        (``device_rng_seed``, this learner's count of device-drawn calls) and the last step's beta, logged as
+        replay/beta (beta follows ``critic_optimizer``'s step count).  Returns ("per", keys) or (None, None) for S = 0
+        with a prioritized buffer, and None for any other buffer (the uniform paths stage the call)."""
+        n_step = getattr(self, "n_step", 1)
+        if n_step > 1:  # the windows are assembled on the device from the replay ring
+            if not getattr(self, "use_device_replay", True):
+                raise ValueError(f"n_step = {n_step} needs use_device_replay = True: n-step windows are assembled on "
+                                 "the device from the replay columns")
+            if not hasattr(replay_buffer, "device_episode_ends"):
+                raise ValueError(f"n_step = {n_step} needs a replay buffer with device_episode_ends (a ReplayBuffer "
+                                 f"or PrioritizedReplayBuffer), got {type(replay_buffer).__name__}")
+        if not isinstance(replay_buffer, PrioritizedReplayBuffer):
+            self._last_beta = None
+            return None
+        # always the prioritized device path, keyed like the uniform device draws (device_rng_seed, call count)
+        if not getattr(self, "use_device_replay", True):
+            raise ValueError("a PrioritizedReplayBuffer needs use_device_replay = True: its draws and priority "
+                             "updates run on the device")
+        if S == 0:
+            return None, None
+        self._device_rng_calls = getattr(self, "_device_rng_calls", 0) + 1
+        t0 = self._adam_step_count(critic_optimizer, critic_linears)
+        self._last_beta = replay_buffer.beta(t0 + S - 1)  # the last step's beta, logged as replay/beta
+        return "per", (getattr(self, "device_rng_seed", 0), self._device_rng_calls)
+
+    def _call_nstep_and_prioritized(self, e, hp, replay_buffer, S: int, B: int, mode, inputs):
+        """The engine call of a learner with n-step returns and prioritized replay: the window length (and episode
+        ends) first, then the prioritized call for mode "per" or the uniform paths' call."""
+        if mode is not None:
+            n_step = getattr(self, "n_step", 1)
+            e.set_nstep(n_step, [replay_buffer.device_episode_ends()] if n_step > 1 else None)
+        if mode != "per":
+            return _OffPolicyBase._call_engine(e, hp, replay_buffer, S, B, mode, inputs)
+        e.set_per(*replay_buffer.per_settings())
+        tree = replay_buffer.device_tree()
+        columns, rows = replay_buffer.device_columns()
+        return e.train_prioritized(hp, columns, rows, tree, S, B, *inputs)
 
     @staticmethod
     def _call_engine(e, hp, replay_buffer, S: int, B: int, mode, inputs):

@@ -38,11 +38,9 @@ class DiscreteQFunction(_Critic):
         return self.network(observation)
 
 
-class CategoricalQFunction(_Critic):
-    """A return distribution per action over a fixed support (C51's critic): the network maps an observation to
-    ``n_actions x n_atoms`` logits, action a owning columns a*n_atoms .. (a+1)*n_atoms - 1.  ``forward`` returns the
-    expected values [..., n_actions], so greedy and epsilon-greedy policies and the evaluator use it as they use a
-    ``DiscreteQFunction``."""
+class _CategoricalSupport(_Critic):
+    """A critic whose network outputs logits over ``n_atoms`` fixed atoms from ``v_min`` to ``v_max`` (the support of
+    C51's and D4PG's critics)."""
 
     MAX_ATOMS = 256  # the engine's limit (b200rl.h)
 
@@ -59,6 +57,13 @@ class CategoricalQFunction(_Critic):
         dz = (v_max - v_min) / (self.n_atoms - 1)
         self.support = torch.tensor([v_min + i * dz for i in range(self.n_atoms)], dtype=torch.float64).float()
 
+
+class CategoricalQFunction(_CategoricalSupport):
+    """A return distribution per action over a fixed support (C51's critic): the network maps an observation to
+    ``n_actions x n_atoms`` logits, action a owning columns a*n_atoms .. (a+1)*n_atoms - 1.  ``forward`` returns the
+    expected values [..., n_actions], so greedy and epsilon-greedy policies and the evaluator use it as they use a
+    ``DiscreteQFunction``."""
+
     def log_distribution(self, observation: Tensor) -> Tensor:
         """log p(s, a) [..., n_actions, n_atoms]."""
         logits = self.network(observation)
@@ -70,6 +75,23 @@ class CategoricalQFunction(_Critic):
 
     def forward(self, observation: Tensor) -> Tensor:
         return (self.distribution(observation) * self.support).sum(-1)
+
+
+class DistributionalQFunction(_CategoricalSupport):
+    """A return distribution over a fixed support for a continuous action (D4PG's critic): the network maps the
+    concatenated pair [s | a] to ``n_atoms`` logits.  ``forward`` returns the expected value Q(s, a) = sum_i z_i p_i
+    with the trailing axis dropped, so host code written for a ``QFunction`` uses it unchanged."""
+
+    def log_distribution(self, observation: Tensor, action: Tensor) -> Tensor:
+        """log p(s, a) [..., n_atoms]."""
+        return torch.log_softmax(self.network(torch.cat((observation, action), dim=-1)), dim=-1)
+
+    def distribution(self, observation: Tensor, action: Tensor) -> Tensor:
+        """p(s, a) [..., n_atoms]."""
+        return self.log_distribution(observation, action).exp()
+
+    def forward(self, observation: Tensor, action: Tensor) -> Tensor:
+        return (self.distribution(observation, action) * self.support).sum(-1)
 
 
 class QuantileQFunction(_Critic):

@@ -37,6 +37,9 @@
 // n-step returns for DQN / C51 (set_nstep): nstep_gather_kernel (or per_draw_kernel's NSTEP instantiation) walks each
 // drawn row's window and stages its return and discount; the loss heads' NSTEP instantiations read the per-row discount
 // in place of gamma.
+// D4PG (config algo = 6, create_d4pg) is DDPG's step program (enqueue_steps) with a categorical critic over [s | a]:
+// c51_loss_kernel (act = NULL, n = 1) as the critic's head, d4pg_policy_loss_kernel as the policy's, and DQN's
+// prioritized draw / priority update and n-step staging.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -1103,12 +1106,19 @@ __device__ __forceinline__ void c51_warp_log_softmax(const float* x, int N, floa
 // and it is counted.  The last CTA of a learner to finish (sync[0] counts them) writes *loss_out = mean L, summed in
 // double as block_mean sums, and *bad_out = the invalid rows (sync[1]), and leaves both counters at 0 for the next
 // launch.  No atomics touch a float: the head is deterministic.
+// act == NULL (D4PG's critic over [s | a], n = 1): every row's action is index 0 and a* = 0; no row is invalid.
+// WEIGHTED (prioritized replay, D4PG engines): row i's loss and gradient are scaled by w[i], and absd[i] = KL_i =
+// L_i + sum_j m_j log m_j (0 log 0 = 0, summed in index order; a rounding-level negative KL is raised to 0, a NaN
+// passes), the base of its priority (-1 for a row with an invalid action).  With every w_i = 1 loss and gradient are
+// bit for bit those of the unweighted head: the products by 1 are exact.
 // NSTEP (n-step returns): row i's discount is disc[i] (gamma^k of its window) in place of gamma (unread otherwise).
-template <bool LANES, bool NSTEP>
+// Each flag's operands are read only by the instantiations that set it.
+template <bool LANES, bool WEIGHTED, bool NSTEP>
 __global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
     const float* q, const float* qt_next, const float* qn, const float* act, const float* rew, const float* done,
     const float* disc, const float* support, float gamma, float v_min, float v_max, float dz, int B, int n, int N,
-    float* dout, float* row_loss, float* q_copy, int* sync, float* loss_out, int* bad_out, size_t lane_stride) {
+    float* dout, float* row_loss, float* q_copy, int* sync, float* loss_out, int* bad_out, const float* w, float* absd,
+    size_t lane_stride) {
   extern __shared__ float c51_smem[];
   __shared__ double red[32];
   __shared__ bool last;
@@ -1118,6 +1128,7 @@ __global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
     rew = lane_ptr(rew, o), done = lane_ptr(done, o), support = lane_ptr(support, o), dout = lane_ptr(dout, o);
     row_loss = lane_ptr(row_loss, o), q_copy = lane_ptr(q_copy, o), sync = lane_ptr(sync, o);
     loss_out = lane_ptr(loss_out, o), bad_out = lane_ptr(bad_out, o);
+    if (WEIGHTED) w = lane_ptr(w, o), absd = lane_ptr(absd, o);
     if (NSTEP) disc = lane_ptr(disc, o);
   }
   const int nN = n * N, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1130,7 +1141,7 @@ __global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
   float* sq = sx + N;                             // expected values of Q(s') (argmax net)
   const int i = blockIdx.x * (blockDim.x >> 5) + warp;
   if (i < B) {
-    const float af = act[i];
+    const float af = act != nullptr ? act[i] : 0.f;
     const bool valid = af >= 0.f && af < (float)n && af == floorf(af);  // false for NaN
     const int a = valid ? (int)af : -1;
     float* drow = dout + (size_t)i * nN;
@@ -1140,14 +1151,18 @@ __global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
       if (lane == 0) {
         q_copy[i] = __int_as_float(0x7fc00000);
         row_loss[i] = 0.f;
+        if (WEIGHTED) absd[i] = -1.f;
         atomicAdd(sync + 1, 1);
       }
     } else {
-      // a*: the expected values of the argmax net, one lane per action, then argmax_row over them
-      const float* an = (qn != nullptr ? qn : qt_next) + (size_t)i * nN;
-      for (int j = lane; j < n; j += 32) sq[j] = c51_expected(an + (size_t)j * N, z, N);
-      __syncwarp();
-      const int a_star = argmax_row(sq, n);
+      int a_star = 0;  // D4PG (act == NULL): the one action
+      if (act != nullptr) {
+        // a*: the expected values of the argmax net, one lane per action, then argmax_row over them
+        const float* an = (qn != nullptr ? qn : qt_next) + (size_t)i * nN;
+        for (int j = lane; j < n; j += 32) sq[j] = c51_expected(an + (size_t)j * N, z, N);
+        __syncwarp();
+        a_star = argmax_row(sq, n);
+      }
       float logp[C51_MAX_ATOMS / 32];
       c51_warp_log_softmax(qt_next + (size_t)i * nN + (size_t)a_star * N, N, sp, logp);
       const float g1d = (NSTEP ? disc[i] : gamma) * (1.f - done[i]), r = rew[i];
@@ -1178,19 +1193,28 @@ __global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
       for (int k = 0; k < C51_MAX_ATOMS / 32; ++k)
         if (lane + 32 * k < N) sb[lane + 32 * k] = m[k], sx[lane + 32 * k] = logp[k];
       __syncwarp();
-      float qv = 0.f, ce = 0.f, msum = 0.f;
+      float qv = 0.f, ce = 0.f, msum = 0.f, ment = 0.f;
       for (int j = 0; j < N; ++j) {
         qv += z[j] * sp[j];
         ce += sb[j] * sx[j];
         msum += sb[j];
+        if (WEIGHTED) ment += sb[j] > 0.f ? sb[j] * logf(sb[j]) : 0.f;
       }
       const float inv = 1.0f / (float)B;  // dqn_loss_kernel's scaling
+      const float wi = WEIGHTED ? w[i] : 1.f;
 #pragma unroll
       for (int k = 0; k < C51_MAX_ATOMS / 32; ++k)
-        if (lane + 32 * k < N) drow[(size_t)a * N + lane + 32 * k] = (sp[lane + 32 * k] * msum - m[k]) * inv;
+        if (lane + 32 * k < N) {
+          const float g = sp[lane + 32 * k] * msum - m[k];
+          drow[(size_t)a * N + lane + 32 * k] = (WEIGHTED ? wi * g : g) * inv;
+        }
       if (lane == 0) {
         q_copy[i] = qv;
-        row_loss[i] = -ce;
+        row_loss[i] = WEIGHTED ? wi * -ce : -ce;
+        if (WEIGHTED) {
+          const float kl = -ce + ment;
+          absd[i] = kl < 0.f ? 0.f : kl;  // NaN passes
+        }
       }
     }
   }
@@ -1208,6 +1232,54 @@ __global__ void __launch_bounds__(C51_WARPS * 32) c51_loss_kernel(
     *bad_out = atomicExch(sync + 1, 0);
     sync[0] = 0;
   }
+}
+
+// D4PG's policy head (algo = 6): one warp per row i of the critic's N logits x at [s | mu(s)] (the grid and shared
+// memory of c51_loss_kernel at n = 1): p = c51_warp_log_softmax's, Q = sum_j z_j p_j in index order,
+//   dOut[i, k] = -(p_k (z_k - Q)) * (1 / B)   (the gradient of -(1/B) sum_i Q_i w.r.t. the logits), row_loss[i] = -Q.
+// The last CTA of a learner to finish (sync[0] counts them) writes *loss_out = -mean Q, summed in double as
+// c51_loss_kernel sums, and leaves the counter at 0.  No atomics touch a float.
+template <bool LANES>
+__global__ void __launch_bounds__(C51_WARPS * 32) d4pg_policy_loss_kernel(const float* q, const float* support, int B,
+                                                                          int N, float* dout, float* row_loss, int* sync,
+                                                                          float* loss_out, size_t lane_stride) {
+  extern __shared__ float d4pg_smem[];
+  __shared__ double red[32];
+  __shared__ bool last;
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q = lane_ptr(q, o), support = lane_ptr(support, o), dout = lane_ptr(dout, o), row_loss = lane_ptr(row_loss, o);
+    sync = lane_ptr(sync, o), loss_out = lane_ptr(loss_out, o);
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float* z = d4pg_smem;
+  for (int j = threadIdx.x; j < N; j += blockDim.x) z[j] = support[j];
+  __syncthreads();
+  float* sp = d4pg_smem + N + warp * N;  // p(s, mu(s))
+  const int i = blockIdx.x * (blockDim.x >> 5) + warp;
+  if (i < B) {
+    float logp[C51_MAX_ATOMS / 32];
+    c51_warp_log_softmax(q + (size_t)i * N, N, sp, logp);
+    float qv = 0.f;
+    for (int j = 0; j < N; ++j) qv += z[j] * sp[j];
+    const float inv = 1.0f / (float)B;
+    float* drow = dout + (size_t)i * N;
+#pragma unroll
+    for (int k = 0; k < C51_MAX_ATOMS / 32; ++k)
+      if (lane + 32 * k < N) drow[lane + 32 * k] = -(sp[lane + 32 * k] * (z[lane + 32 * k] - qv)) * inv;
+    if (lane == 0) row_loss[i] = -qv;
+  }
+  // the last CTA of this learner reads every row's loss
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(sync, 1) == (int)gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double acc = 0.0;
+  for (int r = threadIdx.x; r < B; r += blockDim.x) acc += (double)__ldcg(row_loss + r);
+  block_mean(acc, B, loss_out, red);
+  if (threadIdx.x == 0) sync[0] = 0;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1844,6 +1916,7 @@ struct b200rl_offpolicy {
   cudaGraphExec_t graph = nullptr;
   GraphKey graph_key;  // the call the graph was captured for
   int graph_npol = 0, graph_launches = 0;
+  int last_npol = 0;   // the policy steps of the last train call that ran steps (get_policy_losses)
   float* state = nullptr;  // parameters + Adam state of every network, blob order (see b200rl_offpolicy_create)
   int64_t state_n = 0;
   // SAC (cfg.algo == 1): network 3 is absent; h->eps holds [S, 2, B, A] (the draw for s', then the one for s)
@@ -1904,6 +1977,10 @@ struct b200rl_offpolicy {
   float *iqn_cos_q = nullptr, *iqn_cos_t = nullptr, *iqn_cos_n = nullptr;  // the step's cosine features (iqn_draw_kernel)
   IqnPass iqn_pass[3] = {};            // Q(s) with N, Q_targ(s') with N' + K, Q(s') with K fractions per row
   float *iqn_dhid = nullptr, *iqn_dz = nullptr, *iqn_dphi = nullptr, *iqn_dpsi = nullptr;  // the backward pass's
+  // D4PG (cfg.algo == 6): DDPG's networks with an N-wide critic; C51's support, row losses and counters, DQN's
+  // prioritized and n-step buffers; dq and qt1 are [B, N]
+  bool d4pg = false;
+  b200rl_d4pg_config d4pg_cfg{};
   // the replay columns, episode-end columns, trees and row counts of this call (train_gather[_rng], train_prioritized)
   ReplayLanes<true> replay{};
   std::vector<void*> allocs;
@@ -1913,10 +1990,12 @@ namespace {
 
 inline int64_t state_pad(int64_t n) { return (n + 63) & ~(int64_t)63; }
 
-// float2 entries of one learner's adam_tab: the Adam scalar rows (+ SAC's temperature row or DQN's copy flags), then
-// DQN's prioritized (seed, call) at 4 max_steps and a noisy or IQN engine's draw keys (seed, call) after it
+// float2 entries of one learner's adam_tab: the Adam scalar rows (+ SAC's temperature row, DQN's copy flags or D4PG's
+// betas), then DQN's or D4PG's prioritized (seed, call) at 4 max_steps and a noisy or IQN engine's draw keys (seed,
+// call) after it
 inline size_t adam_tab_len(const b200rl_offpolicy* h) {
-  return (h->sac || h->dsac || h->dqn ? 4 : 3) * (size_t)h->cfg.max_steps + (h->dqn ? 2 : 0) + (h->noisy || h->iqn ? 2 : 0);
+  const bool per = h->dqn || h->d4pg;  // engines that take prioritized replay: row 3's .y holds the betas
+  return (h->sac || h->dsac || per ? 4 : 3) * (size_t)h->cfg.max_steps + (per ? 2 : 0) + (h->noisy || h->iqn ? 2 : 0);
 }
 
 // A piece of the learner arena: recorded here (256-byte aligned), placed by arena_commit
@@ -2224,19 +2303,38 @@ int adam_net(const b200rl_offpolicy* h, NetBuf& nb, const float2* table, int idx
 
 }  // namespace
 
-// The engine of create_group (ic = NULL) and of create_iqn (ic = the IQN counts, config algo 4)
-static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_config* ic, int32_t n_learners,
-                         b200rl_offpolicy** out) {
+// The engine of create_group (ic = dc = NULL), of create_iqn (ic = the IQN counts, config algo 4) and of create_d4pg
+// (dc = the support, config algo 6)
+static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_config* ic,
+                         const b200rl_d4pg_config* dc, int32_t n_learners, b200rl_offpolicy** out) {
   B200RL_REQUIRE(cfg && out, "offpolicy_create: NULL argument");
   B200RL_REQUIRE(n_learners >= 1 && n_learners <= B200RL_MAX_LEARNERS,
                  "offpolicy_create_group: n_learners must be 1..%d, got %d", B200RL_MAX_LEARNERS, n_learners);
   B200RL_REQUIRE(cfg->n_q == 1 || cfg->n_q == 2, "offpolicy_create: n_q must be 1 (DDPG) or 2 (TD3)");
-  B200RL_REQUIRE((cfg->algo >= 0 && cfg->algo <= 3) || cfg->algo == 5 || (cfg->algo == 4 && ic != nullptr),
+  B200RL_REQUIRE((cfg->algo >= 0 && cfg->algo <= 3) || cfg->algo == 5 || (cfg->algo == 4 && ic != nullptr) ||
+                     (cfg->algo == 6 && dc != nullptr),
                  "offpolicy_create: algo must be 0 (DDPG / TD3), 1 (SAC), 2 (DQN), 3 (C51) or 5 (discrete SAC), got %d "
-                 "(algo 4, IQN, is created by b200rl_offpolicy_create_iqn with its counts)", cfg->algo);
+                 "(algo 4, IQN, is created by b200rl_offpolicy_create_iqn with its counts, algo 6, D4PG, by "
+                 "b200rl_offpolicy_create_d4pg with its support)", cfg->algo);
   B200RL_REQUIRE(ic == nullptr || cfg->algo == 4, "offpolicy_create_iqn: the config's algo must be 4 (IQN), got %d",
                  cfg->algo);
+  B200RL_REQUIRE(dc == nullptr || cfg->algo == 6, "offpolicy_create_d4pg: the config's algo must be 6 (D4PG), got %d",
+                 cfg->algo);
   const bool sac = cfg->algo == 1, c51 = cfg->algo == 3, iqn = cfg->algo == 4, dsac = cfg->algo == 5;
+  const bool d4pg = cfg->algo == 6 && dc != nullptr;
+  const int NA = d4pg ? dc->n_atoms : 0;
+  if (d4pg) {
+    B200RL_REQUIRE(cfg->n_q == 1, "offpolicy_create_d4pg: D4PG needs n_q = 1 (one distributional critic), got %d",
+                   cfg->n_q);
+    B200RL_REQUIRE(cfg->dueling_k == 0 && cfg->noisy_layers == 0, "offpolicy_create_d4pg: D4PG takes neither "
+                   "dueling_k nor noisy_layers: dueling and noisy networks are not implemented for it");
+    B200RL_REQUIRE(NA >= 2 && NA <= C51_MAX_ATOMS, "offpolicy_create_d4pg: n_atoms must be 2..%d, got %d",
+                   C51_MAX_ATOMS, NA);
+    B200RL_REQUIRE(std::isfinite(dc->v_min) && std::isfinite(dc->v_max) && dc->v_min < dc->v_max,
+                   "offpolicy_create_d4pg: the support needs finite v_min < v_max, got [%g, %g]", dc->v_min, dc->v_max);
+    B200RL_REQUIRE(c51_warps(1, NA) >= 1, "offpolicy_create_d4pg: %d atoms are too many for the head's shared memory",
+                   NA);
+  }
   const bool dqn = cfg->algo == 2 || c51 || iqn;  // C51 and IQN are DQN engines
   B200RL_REQUIRE(!sac || cfg->n_q == 2, "offpolicy_create: SAC needs n_q = 2 (twin soft critics), got %d", cfg->n_q);
   B200RL_REQUIRE(!dsac || cfg->n_q == 2, "offpolicy_create: discrete SAC (algo = 5) needs n_q = 2 (twin soft critics), "
@@ -2307,8 +2405,11 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
                    "policy [obs, ..., n] and critics [obs, ..., n] with n >= 2 actions, got policy %d -> %d and critics "
                    "%d -> %d", O, P_out, cfg->q.sizes[0], nq);
   }
-  B200RL_REQUIRE(dqn || dsac || (cfg->q.sizes[0] == O + A && cfg->q.sizes[cfg->q.n_layers] == 1),
+  B200RL_REQUIRE(dqn || dsac || d4pg || (cfg->q.sizes[0] == O + A && cfg->q.sizes[cfg->q.n_layers] == 1),
                  "offpolicy_create: Q network must map [obs %d + act %d] -> 1", O, A);
+  B200RL_REQUIRE(!d4pg || (cfg->q.sizes[0] == O + A && cfg->q.sizes[cfg->q.n_layers] == NA),
+                 "offpolicy_create_d4pg: the critic must map [obs %d + act %d] -> %d atoms' logits, got %d -> %d", O, A,
+                 NA, cfg->q.sizes[0], cfg->q.sizes[cfg->q.n_layers]);
   B200RL_REQUIRE(device_sm_count() > 0, "offpolicy_create: no CUDA device");
   b200rl_offpolicy* h = new b200rl_offpolicy();
   h->cfg = *cfg;
@@ -2321,6 +2422,8 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   h->c51 = c51;
   h->iqn = iqn;
   if (iqn) h->iqn_cfg = *ic;
+  h->d4pg = d4pg;
+  if (d4pg) h->d4pg_cfg = *dc, h->d4pg_cfg.reserved = 0;
   h->noisy = NM != 0;
   int rc = 0;
   int maxw = O + A;
@@ -2414,9 +2517,10 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   for (int l = 0; l <= B200RL_MAX_LAYERS; ++l) rc |= oalloc(h, &h->acts_tq[l], B * (size_t)maxw);
   rc |= oalloc(h, &h->x_cat, B * (size_t)(O + A));
   rc |= oalloc(h, &h->x_cat2, B * (size_t)(O + A));
-  rc |= oalloc(h, &h->qt1, B);
+  // discrete SAC: [B, n] per critic; D4PG: [B, N] (the target critic's logits, the output gradient)
+  const size_t n_dq = dsac || d4pg ? (size_t)cfg->q.sizes[cfg->q.n_layers] : 1;
+  rc |= oalloc(h, &h->qt1, B * n_dq);
   rc |= oalloc(h, &h->qt2, B);
-  const size_t n_dq = dsac ? (size_t)cfg->q.sizes[cfg->q.n_layers] : 1;  // discrete SAC: [B, n] per critic
   rc |= oalloc(h, &h->dq, B * n_dq);
   rc |= oalloc(h, &h->dbuf0, B * (size_t)maxw);
   rc |= oalloc(h, &h->dbuf1, B * (size_t)maxw);
@@ -2461,7 +2565,18 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
     rc |= oalloc(h, &h->c51_row_loss, B);  // C51's and QR-DQN's heads
     rc |= oalloc(h, &h->c51_sync, 2);
   }
-  if (c51) rc |= oalloc(h, &h->c51_support, C51_MAX_ATOMS);
+  if (d4pg) {
+    rc |= oalloc(h, &h->dqn_bad, S);  // the head's invalid-row count, always 0 (no action column)
+    rc |= oalloc(h, &h->per_w, S * B);
+    rc |= oalloc(h, &h->per_newp, S * B);
+    rc |= oalloc(h, &h->per_absd, B);
+    rc |= oalloc(h, &h->per_bad, S);
+    rc |= oalloc(h, &h->nstep_disc, S * B);
+    rc |= oalloc(h, &h->nstep_rows, S * B);
+    rc |= oalloc(h, &h->c51_row_loss, B);
+    rc |= oalloc(h, &h->c51_sync, 2);
+  }
+  if (c51 || d4pg) rc |= oalloc(h, &h->c51_support, C51_MAX_ATOMS);
   if (iqn) {
     const size_t D = cfg->q.sizes[1], H = cfg->q.sizes[2], n = cfg->q.sizes[3];
     rc |= oalloc(h, &h->iqn_taus, S * B * (IN + INt + IK));
@@ -2511,6 +2626,15 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   if (!rc && cudaEventCreateWithFlags(&h->ev_side, cudaEventDisableTiming) != cudaSuccess) rc = 1;
   if (!rc && cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming) != cudaSuccess) rc = 1;
   if (!rc && cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming) != cudaSuccess) rc = 1;
+  if (!rc && d4pg) {  // the support, z_i = float32(v_min + i dz) in double as set_c51 writes it, in every arena
+    const double dz = (dc->v_max - dc->v_min) / (NA - 1);
+    std::vector<float> z((size_t)h->K * C51_MAX_ATOMS, 0.f);
+    for (int k = 0; k < h->K; ++k)
+      for (int i = 0; i < NA; ++i) z[(size_t)k * C51_MAX_ATOMS + i] = (float)(dc->v_min + i * dz);
+    if (cudaMemcpy2D(h->c51_support, h->lane_stride, z.data(), C51_MAX_ATOMS * sizeof(float),
+                     C51_MAX_ATOMS * sizeof(float), h->K, cudaMemcpyHostToDevice) != cudaSuccess)
+      rc = 1;
+  }
   if (rc) {
     b200rl_offpolicy_destroy(h);
     return 1;
@@ -2520,18 +2644,24 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
 }
 
 extern "C" int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200rl_offpolicy** out) {
-  return create_engine(cfg, nullptr, 1, out);
+  return create_engine(cfg, nullptr, nullptr, 1, out);
 }
 
 extern "C" int b200rl_offpolicy_create_group(const b200rl_offpolicy_config* cfg, int32_t n_learners,
                                              b200rl_offpolicy** out) {
-  return create_engine(cfg, nullptr, n_learners, out);
+  return create_engine(cfg, nullptr, nullptr, n_learners, out);
 }
 
 extern "C" int b200rl_offpolicy_create_iqn(const b200rl_offpolicy_config* cfg, const b200rl_iqn_config* iqn,
                                            int32_t n_learners, b200rl_offpolicy** out) {
   B200RL_REQUIRE(iqn, "offpolicy_create_iqn: NULL IQN counts");
-  return create_engine(cfg, iqn, n_learners, out);
+  return create_engine(cfg, iqn, nullptr, n_learners, out);
+}
+
+extern "C" int b200rl_offpolicy_create_d4pg(const b200rl_offpolicy_config* cfg, const b200rl_d4pg_config* d4pg,
+                                            int32_t n_learners, b200rl_offpolicy** out) {
+  B200RL_REQUIRE(d4pg, "offpolicy_create_d4pg: NULL D4PG support");
+  return create_engine(cfg, nullptr, d4pg, n_learners, out);
 }
 
 extern "C" void b200rl_offpolicy_destroy(b200rl_offpolicy* h) {
@@ -2664,6 +2794,8 @@ extern "C" int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hp
 extern "C" int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hparams* cp) {
   B200RL_REQUIRE(h && cp, "offpolicy_set_c51: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_c51: a discrete SAC engine (algo = 5) has no categorical head");
+  B200RL_REQUIRE(!h->d4pg, "offpolicy_set_c51: a D4PG engine (algo = 6) takes its support at create "
+                 "(b200rl_offpolicy_create_d4pg)");
   B200RL_REQUIRE(h->c51, "offpolicy_set_c51: the engine was not created with algo = 3 (C51)");
   const int N = cp->n_atoms, width = h->net[1].d.sizes[h->net[1].d.n_layers];
   B200RL_REQUIRE(N >= 2 && N <= C51_MAX_ATOMS, "offpolicy_set_c51: n_atoms must be 2..%d, got %d", C51_MAX_ATOMS, N);
@@ -2711,7 +2843,8 @@ extern "C" int b200rl_offpolicy_set_per(b200rl_offpolicy* h, const b200rl_per_hp
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_per: prioritized replay is not implemented for discrete SAC engines (algo = "
                  "5)");
   B200RL_REQUIRE(!h->c51, "offpolicy_set_per: prioritized replay is not implemented for C51 engines");
-  B200RL_REQUIRE(h->dqn, "offpolicy_set_per: prioritized replay is implemented for DQN engines (algo = 2) only");
+  B200RL_REQUIRE(h->dqn || h->d4pg, "offpolicy_set_per: prioritized replay is implemented for DQN engines (algo = 2) "
+                 "and D4PG engines (algo = 6) only");
   B200RL_REQUIRE(pp->alpha >= 0.0 && std::isfinite(pp->alpha), "offpolicy_set_per: alpha must be >= 0");
   B200RL_REQUIRE(pp->eps > 0.0 && std::isfinite(pp->eps), "offpolicy_set_per: eps must be > 0");
   B200RL_REQUIRE(pp->beta_start >= 0.0 && pp->beta_start <= 1.0, "offpolicy_set_per: beta_start must be in [0, 1]");
@@ -2725,8 +2858,8 @@ extern "C" int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, c
   B200RL_REQUIRE(h, "offpolicy_set_nstep: NULL engine");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_nstep: n-step returns are not implemented for discrete SAC engines (algo = "
                  "5)");
-  B200RL_REQUIRE(h->dqn, "offpolicy_set_nstep: n-step returns are implemented for DQN and C51 engines (algo = 2 or 3) "
-                 "only");
+  B200RL_REQUIRE(h->dqn || h->d4pg, "offpolicy_set_nstep: n-step returns are implemented for DQN and C51 engines "
+                 "(algo = 2 or 3) and D4PG engines (algo = 6) only");
   B200RL_REQUIRE(n_step >= 1 && n_step <= NSTEP_MAX, "offpolicy_set_nstep: n_step must be 1..%d, got %d", NSTEP_MAX,
                  n_step);
   LaneSrc<true> ends{};
@@ -2830,8 +2963,21 @@ extern "C" int b200rl_offpolicy_sac_outputs(b200rl_offpolicy* h, int32_t S, floa
   return 0;
 }
 
+// c51_loss_kernel<LANES, WEIGHTED, NSTEP> of a call: WEIGHTED for prioritized replay (D4PG engines), NSTEP for n-step
+// returns
+template <bool LANES>
+static auto c51_head(bool weighted, bool nstep) {
+  return weighted ? (nstep ? c51_loss_kernel<LANES, true, true> : c51_loss_kernel<LANES, true, false>)
+                  : (nstep ? c51_loss_kernel<LANES, false, true> : c51_loss_kernel<LANES, false, false>);
+}
+
 // Enqueue the S train steps on `s` (plain launches or under stream capture).  Everything that varies between calls
 // with the same (S, B, hyper-parameters) is read from device buffers: staged minibatches, Adam scalar tables.
+// A D4PG engine (h->d4pg) differs in its heads and staging only: the critic's head is c51_loss_kernel on its N logits
+// (act = NULL, n = 1; the target logits from Q1targ at [s' | mu_targ(s')]), the policy's d4pg_policy_loss_kernel, the
+// dOut of both backward passes N wide.  A prioritized call (h->per_run) opens each step with the draw on s (draw,
+// weights, gather or n-step walk) and runs the priority update on s4 beside the critic's backward pass; the next
+// step's draw joins it.
 static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s,
                          int* n_pol_out) {
   const bool td3 = h->cfg.n_q == 2;
@@ -2842,6 +2988,14 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
   const int ew = 256;
   cudaStream_t s2 = h->s2, s3 = h->s3, s4 = h->s4;
   int n_pol = 0;
+  const bool d4pg = h->d4pg, per = h->per_run, nstep = h->nstep > 1;
+  const int NQ = d4pg ? h->d4pg_cfg.n_atoms : 1;  // the critics' output width
+  const int W = d4pg ? c51_warps(1, NQ) : 1;      // the D4PG heads' warps per CTA
+  const size_t head_smem = sizeof(float) * (size_t)(NQ + W * (3 * NQ + 1));
+  const float vmin = (float)h->d4pg_cfg.v_min, vmax = (float)h->d4pg_cfg.v_max;
+  const float dz = d4pg ? (float)((h->d4pg_cfg.v_max - h->d4pg_cfg.v_min) / (NQ - 1)) : 0.f;
+  const float2* betas = h->adam_tab + (size_t)3 * maxS;
+  const unsigned long long* keys = reinterpret_cast<const unsigned long long*>(h->adam_tab + (size_t)4 * maxS);
   // A step is a dependency graph, not a sequence; the branches below are what the kernels actually need:
   //   s  : target policy -> Q1 target ---------+-> Q1 loss -> Q1 dX chain -----+-> Adam(Q1) -> [policy step] -> polyak
   //   s2 :               -> Q2 target ---------+-> Q2 loss -> Q2 dX chain -----+-> Adam(Q2)
@@ -2849,11 +3003,22 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
   //   s4 : Q2 forward on [s | a] .................................. Q2's dW products
   // Critical path per step: 6 + 1 + 3 + 1 kernels (was 7 + 10 in a single chain), policy steps 14 more (was 19).
   for (int st = 0; st < S; ++st) {
-    const float* s_obs = h->obs + (size_t)st * B * O;
-    const float* s_act = h->act + (size_t)st * B * A;
-    const float* s_rew = h->rew + (size_t)st * B;
-    const float* s_nobs = h->nobs + (size_t)st * B * O;
-    const float* s_done = h->done + (size_t)st * B;
+    float* s_obs = h->obs + (size_t)st * B * O;
+    float* s_act = h->act + (size_t)st * B * A;
+    float* s_rew = h->rew + (size_t)st * B;
+    float* s_nobs = h->nobs + (size_t)st * B * O;
+    float* s_done = h->done + (size_t)st * B;
+    float* s_disc = d4pg ? h->nstep_disc + (size_t)st * B : nullptr;
+    long long* s_idx = h->idx + (size_t)st * B;
+    float* s_w = per ? h->per_w + (size_t)st * B : nullptr;
+    if (per) {  // D4PG: the step's prioritized draw ahead of everything that reads its minibatch
+      if (st > 0 && edge(h, s4, s)) return 1;  // the previous step's priorities are in the tree
+      if (launch(h, nstep ? per_draw_kernel<false, true> : per_draw_kernel<false, false>,
+                 nstep ? per_draw_kernel<true, true> : per_draw_kernel<true, false>, 1, GTHREADS, 0, s, h->replay,
+                 betas, keys, st, B, O, A, h->nstep, (float)hp->gamma, s_idx, s_w, s_obs, s_act, s_rew, s_nobs, s_done,
+                 s_disc, h->nstep_rows + (size_t)st * B))
+        return 1;
+    }
     // ---- the critics' forward passes on [s | a]: their values are also the logged Q-values (td3.py:231-235) ----
     float* qa[2][B200RL_MAX_LAYERS + 1];
     for (int qi = 0; qi < (td3 ? 2 : 1); ++qi) {
@@ -2894,11 +3059,25 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
       NetBuf& qn = qi == 0 ? q1 : q2;
       cudaStream_t qs = qi == 0 ? s : s2;
       float* dq = qi == 0 ? h->dq : h->dq2;
-      if (launch(h, q_loss_kernel<false>, q_loss_kernel<true>, 1, GTHREADS, 0, qs, qa[qi][Lq], s_rew, s_done, h->qt1,
-                 td3 ? h->qt2 : nullptr, (float)hp->gamma, B, dq, (qi == 0 ? h->out_l1 : h->out_l2) + st,
-                 (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B))
+      if (d4pg) {  // the projected cross-entropy on the critic's logits; Q1targ's logits are in qt1
+        if (launch(h, c51_head<false>(per, nstep), c51_head<true>(per, nstep), (B + W - 1) / W, W * 32, head_smem, s,
+                   qa[0][Lq], h->qt1, nullptr, nullptr, s_rew, s_done, s_disc, h->c51_support, (float)hp->gamma, vmin,
+                   vmax, dz, B, 1, NQ, h->dq, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync,
+                   h->out_l1 + st, h->dqn_bad + st, s_w, h->per_absd))
+          return 1;
+        if (per) {
+          if (edge(h, s, s4)) return 1;
+          if (launch(h, per_update_kernel<false>, per_update_kernel<true>, 1, GTHREADS, 0, s4, h->replay, s_idx,
+                     h->per_absd, B, (float)h->per_hp.alpha, (float)h->per_hp.eps, h->per_newp + (size_t)st * B,
+                     h->per_bad + st))
+            return 1;
+        }
+      } else if (launch(h, q_loss_kernel<false>, q_loss_kernel<true>, 1, GTHREADS, 0, qs, qa[qi][Lq], s_rew, s_done,
+                        h->qt1, td3 ? h->qt2 : nullptr, (float)hp->gamma, B, dq,
+                        (qi == 0 ? h->out_l1 : h->out_l2) + st, (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B)) {
         return 1;
-      if (net_backward(h, qn, qa[qi], dq, 1, B, true, nullptr, qs, qi != 0, s_act, A, O, qi == 0 ? s3 : s4)) return 1;
+      }
+      if (net_backward(h, qn, qa[qi], dq, NQ, B, true, nullptr, qs, qi != 0, s_act, A, O, qi == 0 ? s3 : s4)) return 1;
       if (adam_net(h, qn, h->adam_tab + (size_t)(1 + qi) * maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, qs)) return 1;
     }
     if (td3 && edge(h, s2, s)) return 1;
@@ -2912,11 +3091,17 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
       qp[0] = const_cast<float*>(s_obs);
       for (int l = 1; l <= Lq; ++l) qp[l] = h->acts[1][l];
       if (net_forward(h, q1, qp, B, s, pa[Lp], A, O)) return 1;  // Q1 with its freshly updated parameters (td3.py:309)
-      if (launch(h, q_loss_kernel<false>, q_loss_kernel<true>, 1, GTHREADS, 0, s, qp[Lq], nullptr, nullptr, nullptr,
-                 nullptr, 0.f, B, h->dq, h->out_lp + n_pol, nullptr))
+      if (d4pg) {  // -mean of the expected values; the logit gradient -(1/B) p_k (z_k - Q)
+        if (launch(h, d4pg_policy_loss_kernel<false>, d4pg_policy_loss_kernel<true>, (B + W - 1) / W, W * 32,
+                   sizeof(float) * (size_t)(NQ + W * NQ), s, qp[Lq], h->c51_support, B, NQ, h->dq, h->c51_row_loss,
+                   h->c51_sync, h->out_lp + n_pol))
+          return 1;
+      } else if (launch(h, q_loss_kernel<false>, q_loss_kernel<true>, 1, GTHREADS, 0, s, qp[Lq], nullptr, nullptr,
+                        nullptr, nullptr, 0.f, B, h->dq, h->out_lp + n_pol, nullptr)) {
         return 1;
+      }
       // gradient w.r.t. Q1's input; its action columns are the gradient w.r.t. pi(s) (Q parameters frozen)
-      if (net_backward(h, q1, qp, h->dq, 1, B, false, h->x_cat, s)) return 1;
+      if (net_backward(h, q1, qp, h->dq, NQ, B, false, h->x_cat, s)) return 1;
       if (net_backward(h, pi, pa, h->x_cat + O, O + A, B, true, nullptr, s, false, nullptr, 0, 0, s3)) return 1;
       if (adam_net(h, pi, h->adam_tab, n_pol, hp->policy_beta1, hp->policy_beta2, hp->policy_eps, s)) return 1;
       PolyakArgs pk{};
@@ -2934,6 +3119,7 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
       ++n_pol;
     }
   }
+  if (per && edge(h, s4, s)) return 1;
   *n_pol_out = n_pol;
   return 0;
 }
@@ -3305,11 +3491,10 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
       const size_t smem = sizeof(float) * (size_t)(N + W * (3 * N + n / N));
       const float vmin = (float)h->c51_hp.v_min, vmax = (float)h->c51_hp.v_max;
       const float dz = (float)((h->c51_hp.v_max - h->c51_hp.v_min) / (N - 1));
-      if (launch(h, nstep ? c51_loss_kernel<false, true> : c51_loss_kernel<false, false>,
-                 nstep ? c51_loss_kernel<true, true> : c51_loss_kernel<true, false>, (B + W - 1) / W, W * 32, smem, s,
+      if (launch(h, c51_head<false>(false, nstep), c51_head<true>(false, nstep), (B + W - 1) / W, W * 32, smem, s,
                  qa[L], tq[L], dbl ? qn[L] : nullptr, s_act, s_rew, s_done, s_disc, h->c51_support, (float)hp->gamma,
                  vmin, vmax, dz, B, n / N, N, h->dqn_dout, h->c51_row_loss, h->out_q1 + (size_t)st * B, h->c51_sync,
-                 h->out_l1 + st, h->dqn_bad + st))
+                 h->out_l1 + st, h->dqn_bad + st, nullptr, nullptr))
         return 1;
     } else if (h->qr) {
       const int N = h->qr_hp.n_quantiles;
@@ -3457,9 +3642,10 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
     B200RL_CUDA(cudaMemcpy2DAsync(q2_values, SB * 4, h->out_q2, ls, SB * 4, K, cudaMemcpyDeviceToHost, s));
     B200RL_CUDA(cudaMemcpy2DAsync(q2_losses, (size_t)S * 4, h->out_l2, ls, (size_t)S * 4, K, cudaMemcpyDeviceToHost, s));
   }
-  if (n_pol > 0)
+  if (n_pol > 0 && policy_losses != nullptr)  // NULL: a prioritized call (get_policy_losses reads them)
     B200RL_CUDA(cudaMemcpy2DAsync(policy_losses, (size_t)S * 4, h->out_lp, ls, (size_t)n_pol * 4, K,
                                   cudaMemcpyDeviceToHost, s));
+  h->last_npol = n_pol;
   std::vector<int> bad(h->dqn || h->dsac ? K * S : 0), per_bad(h->per_run ? K * S : 0);
   if (h->dqn || h->dsac)
     B200RL_CUDA(cudaMemcpy2DAsync(bad.data(), (size_t)S * 4, h->dqn_bad, ls, (size_t)S * 4, K, cudaMemcpyDeviceToHost, s));
@@ -3470,7 +3656,8 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   *n_policy_updates = n_pol;
   const int n_actions = h->net[1].d.sizes[h->net[1].d.n_layers] /
                         (h->c51 ? h->c51_hp.n_atoms : h->qr ? h->qr_hp.n_quantiles : 1);
-  const char* algo = h->c51 ? "C51" : h->qr ? "QR-DQN" : h->iqn ? "IQN" : h->dsac ? "discrete SAC" : "DQN";
+  const char* algo = h->c51 ? "C51" : h->qr ? "QR-DQN" : h->iqn ? "IQN" : h->dsac ? "discrete SAC" : h->d4pg ? "D4PG"
+                                                                                                       : "DQN";
   for (size_t i = 0; i < bad.size(); ++i)
     B200RL_REQUIRE(bad[i] == 0, "offpolicy_train: %s learner %d, step %d: %d minibatch rows hold an action that is not "
                    "an integer in [0, %d); those rows were left out of the update", algo, (int)(i / S), (int)(i % S),
@@ -3494,6 +3681,8 @@ static int train_begin(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, 
   B200RL_REQUIRE(h->dqn || h->dsac || !hp->use_target_noise || noise_given, "%s: target noise requested but no noise "
                  "given", what);
   B200RL_REQUIRE(h->dqn || h->dsac || hp->policy_delay >= 1, "%s: policy_delay must be >= 1", what);
+  B200RL_REQUIRE(!h->d4pg || !hp->use_target_noise, "%s: D4PG has no target-policy smoothing: use_target_noise must be "
+                 "0", what);
   if (h->sac) {
     B200RL_REQUIRE(h->sac_set, "%s: a SAC engine needs b200rl_offpolicy_set_sac before it trains", what);
     B200RL_REQUIRE(noise_given, "%s: SAC needs the noise draws [S, 2, B, A]", what);
@@ -3722,8 +3911,8 @@ extern "C" int b200rl_offpolicy_train_prioritized_group(b200rl_offpolicy* h, con
   B200RL_REQUIRE(!h->c51, "offpolicy_train_prioritized: prioritized replay is not implemented for C51 engines");
   B200RL_REQUIRE(!h->dsac, "offpolicy_train_prioritized: prioritized replay is not implemented for discrete SAC "
                  "engines (algo = 5)");
-  B200RL_REQUIRE(h->dqn, "offpolicy_train_prioritized: prioritized replay is implemented for DQN engines (algo = 2) "
-                 "only");
+  B200RL_REQUIRE(h->dqn || h->d4pg, "offpolicy_train_prioritized: prioritized replay is implemented for DQN engines "
+                 "(algo = 2) and D4PG engines (algo = 6) only");
   B200RL_REQUIRE(h->per_set, "offpolicy_train_prioritized: call b200rl_offpolicy_set_per first");
   if (int rc = check_replay(h, rb, "offpolicy_train_prioritized")) return rc;
   const auto own = [&] {
@@ -3768,7 +3957,7 @@ extern "C" int b200rl_offpolicy_train_prioritized(b200rl_offpolicy* h, const b20
 
 extern "C" int b200rl_offpolicy_get_per_draws(b200rl_offpolicy* h, int32_t S, int32_t B, int64_t* idx, float* weights,
                                               float* priorities, void* stream) {
-  B200RL_REQUIRE(h && h->dqn && idx && weights && priorities && S >= 0 && S <= h->cfg.max_steps && B >= 1 &&
+  B200RL_REQUIRE(h && (h->dqn || h->d4pg) && idx && weights && priorities && S >= 0 && S <= h->cfg.max_steps && B >= 1 &&
                      B <= h->cfg.max_minibatch, "offpolicy_get_per_draws: bad arguments");
   B200RL_REQUIRE(h->per_last, "offpolicy_get_per_draws: the engine's last train call was not a prioritized one");
   (void)stream;
@@ -3781,9 +3970,24 @@ extern "C" int b200rl_offpolicy_get_per_draws(b200rl_offpolicy* h, int32_t S, in
   return 0;
 }
 
+extern "C" int b200rl_offpolicy_get_policy_losses(b200rl_offpolicy* h, int32_t S, float* policy_losses,
+                                                  int32_t* n_policy_updates) {
+  B200RL_REQUIRE(h && policy_losses && n_policy_updates && S >= 0 && S <= h->cfg.max_steps,
+                 "offpolicy_get_policy_losses: bad arguments");
+  B200RL_REQUIRE(!h->dqn, "offpolicy_get_policy_losses: a DQN engine has no policy");
+  const int n = std::min(S, h->last_npol);
+  if (n > 0)
+    B200RL_CUDA(cudaMemcpy2DAsync(policy_losses, (size_t)S * 4, h->out_lp, h->lane_stride, (size_t)n * 4, h->K,
+                                  cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  *n_policy_updates = n;
+  return 0;
+}
+
 extern "C" int b200rl_offpolicy_get_nstep_draws(b200rl_offpolicy* h, int32_t S, int32_t B, int64_t* last_rows,
                                                 float* returns, float* discounts, void* stream) {
-  B200RL_REQUIRE(h && h->dqn && last_rows && returns && discounts && S >= 0 && S <= h->cfg.max_steps && B >= 1 &&
+  B200RL_REQUIRE(h && (h->dqn || h->d4pg) && last_rows && returns && discounts && S >= 0 && S <= h->cfg.max_steps &&
+                     B >= 1 &&
                      B <= h->cfg.max_minibatch, "offpolicy_get_nstep_draws: bad arguments");
   B200RL_REQUIRE(h->nstep_last, "offpolicy_get_nstep_draws: the engine's last train call was not an n-step one");
   (void)stream;

@@ -333,21 +333,23 @@ class OffPolicyEngine:
     (n_cos, N, N', K); every train call needs ``set_noise_keys`` first, the keys of its fraction draws (b200rl.h, "IQN").
     Discrete SAC (``algo`` 5) has SAC's networks, temperature and outputs over a discrete action space: the policy maps
     obs -> [n] logits, both critics obs -> [n] values, actions are indices (act [S,B]) as for DQN, no noise is used,
-    and ``set_sac`` must be called before the first train call (b200rl.h, "Discrete SAC").
+    and ``set_sac`` must be called before the first train call (b200rl.h, "Discrete SAC").  D4PG (``algo`` 6) has
+    DDPG's networks with a categorical critic: ``q_sizes`` = [obs + act, ..., N] and ``d4pg`` = (N, v_min, v_max), the
+    critic's support; it takes ``set_per`` / ``train_prioritized`` and ``set_nstep`` as DQN does (b200rl.h, "D4PG").
 
     ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
     launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
     is [K][per-learner blob] with [K][3] step counts, and the per-network accessors are refused."""
 
     NETS = {"policy": 0, "q1": 1, "q2": 2, "target_policy": 3, "target_q1": 4, "target_q2": 5}
-    TD3, SAC, DQN, C51, IQN, DSAC = 0, 1, 2, 3, 4, 5
+    TD3, SAC, DQN, C51, IQN, DSAC, D4PG = 0, 1, 2, 3, 4, 5, 6
     DISCRETE = (DQN, C51, IQN)  # the algos with DQN's networks, inputs and outputs
     INDEX_ACTIONS = DISCRETE + (DSAC,)  # the algos whose action column holds an action index
     SOFT = (SAC, DSAC)  # the algos with SAC's networks, temperature and outputs
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
                  q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1, dueling_k: int = 0,
-                 noisy_layers: int = 0, iqn=None):
+                 noisy_layers: int = 0, iqn=None, d4pg=None):
         from ._lib import OffPolicyConfig
         self.lib = _lib.load()
         current_stream_handle()
@@ -359,6 +361,7 @@ class OffPolicyEngine:
         cfg.algo, cfg.dueling_k, cfg.noisy_layers = int(algo), int(dueling_k), int(noisy_layers)
         self.algo, self.dueling_k, self.noisy_layers = int(algo), int(dueling_k), int(noisy_layers)
         self.iqn = None if iqn is None else tuple(int(x) for x in iqn)
+        self.d4pg = None if d4pg is None else (int(d4pg[0]), float(d4pg[1]), float(d4pg[2]))
         self.discrete = self.algo in self.DISCRETE  # DQN's networks and outputs
         self.index_actions = self.algo in self.INDEX_ACTIONS  # act [S,B] indices, no noise
         self.n_q, self.max_minibatch, self.max_steps = int(n_q), int(max_minibatch), int(max_steps)
@@ -377,11 +380,15 @@ class OffPolicyEngine:
         self.noise_width = sum(i + o for i, o in noisy)  # E: draws per network and step
         self.K = int(n_learners)
         h = C.c_void_p()
-        if self.iqn is None:
-            check(self.lib.b200rl_offpolicy_create_group(C.byref(cfg), self.K, C.byref(h)), "offpolicy_create")
-        else:  # IQN's counts size its per-row buffers (b200rl.h, "IQN")
+        if self.iqn is not None:  # IQN's counts size its per-row buffers (b200rl.h, "IQN")
             check(self.lib.b200rl_offpolicy_create_iqn(C.byref(cfg), C.byref(_lib.IqnConfig(*self.iqn)), self.K,
                                                        C.byref(h)), "offpolicy_create_iqn")
+        elif self.d4pg is not None:  # the critic's support is fixed at creation (b200rl.h, "D4PG")
+            n_atoms, v_min, v_max = self.d4pg
+            check(self.lib.b200rl_offpolicy_create_d4pg(C.byref(cfg), C.byref(_lib.D4pgConfig(n_atoms, 0, v_min, v_max)),
+                                                        self.K, C.byref(h)), "offpolicy_create_d4pg")
+        else:
+            check(self.lib.b200rl_offpolicy_create_group(C.byref(cfg), self.K, C.byref(h)), "offpolicy_create")
         self.h = h
 
     def q_layers(self):
@@ -573,7 +580,7 @@ class OffPolicyEngine:
         qp.n_quantiles = int(n_quantiles)
         check(self.lib.b200rl_offpolicy_set_qr(self.h, C.byref(qp)), "set_qr")
 
-    # ---- prioritized replay (DQN) ----
+    # ---- prioritized replay (DQN, D4PG) ----
     def set_per(self, alpha: float, eps: float, beta_start: float, beta_anneal_steps: int) -> None:
         from ._lib import PerHparams
         pp = PerHparams()
@@ -602,11 +609,15 @@ class OffPolicyEngine:
                                  f"on {getattr(t, 'device', '?')}")
         tp = (C.c_void_p * self.K)(*[t.data_ptr() for t in trees])
         keys = [np.asarray([int(x) & (2 ** 64 - 1) for x in v], np.uint64) for v in (seeds, calls)]
-        q1v, _, l1, _, _, _ = self._out_buffers(S, B)
+        q1v, _, l1, _, lp, npol = self._out_buffers(S, B)
         check(self.lib.b200rl_offpolicy_train_prioritized_group(self.h, C.byref(hp), S, B, rb, tp, *[_ptr(x) for x in keys],
                                                                 _ptr(q1v), _ptr(l1), current_stream_handle()),
               "offpolicy_train_prioritized")
         out = dict(q1_values=q1v, q1_losses=l1)
+        if not self.discrete:  # D4PG: the policy losses the call logged
+            check(self.lib.b200rl_offpolicy_get_policy_losses(self.h, int(S), _ptr(lp), C.byref(npol)),
+                  "get_policy_losses")
+            out["policy_losses"] = lp[:, :npol.value]
         return {k: v[0] for k, v in out.items()} if self.K == 1 else out
 
     def get_per_draws(self, S: int, B: int):
@@ -618,7 +629,7 @@ class OffPolicyEngine:
               "get_per_draws")
         return (idx[0], w[0], p[0]) if self.K == 1 else (idx, w, p)
 
-    # ---- n-step returns (DQN / C51) ----
+    # ---- n-step returns (DQN / C51 / D4PG) ----
     def set_nstep(self, n_step: int, episode_ends=None) -> None:
         """Window length ``n_step`` (1..32; 1 clears it) of the next train calls, with ``episode_ends`` = K float32 CUDA
         tensors (each learner's ``device_episode_ends()``, over the rows of the replay it trains on) when n_step > 1."""

@@ -249,19 +249,20 @@ extern "C" int b200rl_onpolicy_create(const b200rl_onpolicy_config* cfg, b200rl_
   const int A = cfg->policy.sizes[cfg->policy.n_layers];
   h->act_cols = cfg->dist == B200RL_DIST_GAUSSIAN ? A : 1;
   const size_t N = (size_t)cfg->max_rows, E = (size_t)cfg->max_episodes;
+  const size_t N_tiles = (N + 127) / 128 * 128;  // the fused step copies its per-row loss inputs in whole 128-row tiles
   const size_t Pmax = (size_t)(Pp > Pv ? Pp : Pv);
   int rc = 0;
   rc |= dev_alloc(h, &h->obs, N * h->obs_dim + 64);  // + slack: the tc kernel stages whole 16-byte chunks
-  rc |= dev_alloc(h, &h->act, N * h->act_cols);
+  rc |= dev_alloc(h, &h->act, N_tiles * h->act_cols);
   rc |= dev_alloc(h, &h->last_obs, E * h->obs_dim + 64);
   rc |= dev_alloc(h, reinterpret_cast<char**>(&h->rew), N * (cfg->rewards_f64 ? 8 : 4));
   rc |= dev_alloc(h, &h->off, E + 1);
   rc |= dev_alloc(h, &h->done, E);
   rc |= dev_alloc(h, &h->values, N);
   rc |= dev_alloc(h, &h->last_values, E);
-  rc |= dev_alloc(h, &h->adv_raw, N);
-  rc |= dev_alloc(h, &h->ret, N);
-  rc |= dev_alloc(h, &h->old_logp, N);
+  rc |= dev_alloc(h, &h->adv_raw, N_tiles);
+  rc |= dev_alloc(h, &h->ret, N_tiles);
+  rc |= dev_alloc(h, &h->old_logp, N_tiles);
   rc |= dev_alloc(h, &h->adv_stats, 4);
   h->scan_ws_bytes = b200rl_gae_scan_workspace_bytes(cfg->max_rows);
   rc |= dev_alloc(h, reinterpret_cast<char**>(&h->scan_ws), h->scan_ws_bytes);

@@ -25,6 +25,9 @@
 //     reads the same observations) into ready-made SWIZZLE_128B tile images [128 rows][h cols 0..31 | l cols 32..63];
 //     the step kernel brings a tile image in with ONE 16 KB bulk copy (cp.async.bulk + mbarrier complete_tx) issued by
 //     the producer warpgroup -- no epilogue touches the observations any more (E0 of mlp_tc2 is gone);
+//   * the same producer copies each tile's per-row loss inputs (actions, adv_raw and old_logp, or the returns) into a
+//     double-buffered shared area on the tile's mbarrier, and the advantage statistics are read once at set-up: the
+//     loss head (E3) no longer waits on global memory in the middle of the chain;
 //   * column 31 of the image is 1.0, so the bias gradients db1 / db2 still fall out of the weight-gradient products;
 //   * two X buffers: the next tile's bulk copy goes into the buffer of the previous tile once its dW1 has retired;
 //   * tanh'(H1) and tanh'(H2) are taken from the fp16 pairs in shared memory: no fp32 copy of H in registers;
@@ -63,9 +66,15 @@ constexpr uint32_t S3_BIAS = S3_OPERANDS_END;        // per net: b1[64] b2[64] b
 constexpr uint32_t S3_DIST = S3_BIAS + 2 * 640;      // var[16], log_scale[16], 1/(2 var)[16], 1/var[16]
 constexpr uint32_t S3_SCALE = S3_DIST + 256;         // per net 16 floats
 constexpr uint32_t S3_XS = S3_SCALE + 128;           // 2^ex_k [32], 2^-ex_k [32]
-constexpr uint32_t S3_RED = S3_XS + 256;             // setup reduction scratch [16 warps][8] floats
+constexpr uint32_t S3_ADV = S3_XS + 256;             // advantage mean, 1 / std
+constexpr uint32_t S3_RED = S3_ADV + 16;             // setup reduction scratch [16 warps][8] floats
 constexpr uint32_t S3_BARS = S3_RED + 4 * 8 * T3_WARPS;  // 8 mbarriers (8 B each), bad flag at +120
-constexpr uint32_t S3_TOTAL = S3_BARS + 128;
+// Per-row loss inputs of tile k in buffer k & 1, copied in with its observations (floats): policy: actions [128][A_out]
+// (one column for a categorical policy) at 0, adv_raw at T3_LI_IN, old_logp at T3_LI_OLD; value: returns at T3_LI_IN.
+constexpr uint32_t T3_LI_IN = 15 * T3_ROWS, T3_LI_OLD = 16 * T3_ROWS;
+constexpr uint32_t T3_LI_BYTES = 17 * T3_ROWS * 4;
+constexpr uint32_t S3_LOSS = S3_BARS + 128;
+constexpr uint32_t S3_TOTAL = S3_LOSS + 2 * T3_LI_BYTES;
 constexpr uint32_t T3_SMEM_BYTES = S3_TOTAL + 1024;  // + alignment slack
 static_assert(T3_SMEM_BYTES <= 227 * 1024, "mlp_tc3 shared memory");
 // end-of-kernel scratch, aliased onto the X buffers (every MMA has retired by then)
@@ -282,6 +291,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   float* s_dist = reinterpret_cast<float*>(sm + S3_DIST);
   float* s_scale = reinterpret_cast<float*>(sm + S3_SCALE);
   float* s_xs = reinterpret_cast<float*>(sm + S3_XS);
+  float* s_adv = reinterpret_cast<float*>(sm + S3_ADV);
   float* s_red = reinterpret_cast<float*>(sm + S3_RED);
   int* s_bad = reinterpret_cast<int*>(sm + S3_BARS + 120);
   const uint32_t bars = base + S3_BARS;
@@ -300,7 +310,13 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
   // otherwise pay an L2 round trip per element, one after the other (17 of the 18 us this set-up took on B200).  Every
   // CTA checks both networks' parameters, so a range trip is raised whichever networks run.
   for (uint32_t i = S3_W / 16 + tid; i < S3_OPERANDS_END / 16; i += T3_THREADS) reinterpret_cast<uint4*>(sm)[i] = make_uint4(0, 0, 0, 0);
-  if (tid == 0) *s_bad = 0;
+  if (tid == 0) {
+    *s_bad = 0;
+    float adv_mean, adv_std;  // utils.py:91 (mean 0, std 1 without statistics)
+    adv_mean_std(p.adv_stats, adv_mean, adv_std);
+    s_adv[0] = adv_mean;
+    s_adv[1] = 1.f / adv_std;
+  }
   if (tid < 64) s_xs[tid] = __ldg(p.xscale + tid);
   float* s_par = reinterpret_cast<float*>(sm + S3_H1);
   static_assert(S3_W - S3_H1 >= 4 * (2 * 6000 + 64), "parameter staging area");
@@ -476,14 +492,27 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     const uint32_t ah = (uint32_t)g * (T2_ACT >> 4);  // this half's split of an A operand: descriptor low-word offset
     const uint32_t gcol = c * ACC_GRAD_NET;
     float w3[16], w2[32], b2[8], w1[32];
-    auto load_x = [&](int k) {  // tile k of this CTA -> X buffer k & 1
-      const uint32_t b = (uint32_t)(k & 1);
+    // tile k of this CTA -> X buffer k & 1, and its per-row loss inputs -> loss-input buffer k & 1.  The engine pads
+    // those columns to whole tiles, so the last tile's copies stay inside their allocations.
+    const uint32_t act_bytes = T3_ROWS * 4u * (uint32_t)(p.dist == B200RL_DIST_GAUSSIAN ? p.net[0].n_out : 1);
+    auto load_x = [&](int k) {
+      const uint32_t b = (uint32_t)(k & 1), bar = bars + 8 * b;
       const long long tile = slot + (long long)k * G;
+      const size_t row0 = (size_t)tile * T3_ROWS;
+      const uint32_t li = ub + S3_LOSS + b * T3_LI_BYTES;
       uint32_t e;
       asm volatile("{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\tselp.u32 %0, 1, 0, q;\n\t}" : "=r"(e));
       if (e && (warp & 3) == 0) {  // one thread of the warpgroup
-        mbar_arrive_expect_tx(bars + 8 * b, T2_ACT);
-        bulk_copy_g2s(ub + S3_XB + b * T2_ACT, p.ximg + (size_t)tile * T2_ACT, T2_ACT, bars + 8 * b);
+        if (c == 0) {
+          mbar_arrive_expect_tx(bar, T2_ACT + act_bytes + 2 * T3_ROWS * 4);
+          bulk_copy_g2s(li, reinterpret_cast<const uint8_t*>(p.actions) + (size_t)tile * act_bytes, act_bytes, bar);
+          bulk_copy_g2s(li + 4 * T3_LI_IN, p.adv_raw + row0, T3_ROWS * 4, bar);
+          bulk_copy_g2s(li + 4 * T3_LI_OLD, p.old_logp + row0, T3_ROWS * 4, bar);
+        } else {
+          mbar_arrive_expect_tx(bar, T2_ACT + T3_ROWS * 4);
+          bulk_copy_g2s(li + 4 * T3_LI_IN, p.target + row0, T3_ROWS * 4, bar);
+        }
+        bulk_copy_g2s(ub + S3_XB + b * T2_ACT, p.ximg + (size_t)tile * T2_ACT, T2_ACT, bar);
       }
       __syncwarp();
     };
@@ -500,9 +529,9 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
       const uint32_t xo = (uint32_t)(k & 1) * T2_ACT;
       const bool first = k == 0;  // the first tile's products overwrite the accumulators
       if (producer && k + 1 < cta_tiles) {
-        // tile k + 1 goes to the buffer of tile k - 1, whose last readers (db2 and dW1 of both halves) have retired
-        // once done[5] completes its tile k - 1 phase.  It cannot be a phase further: its tile k phase needs this
-        // warpgroup's own tile k arrival.
+        // tile k + 1 goes to the buffers of tile k - 1, whose last readers (db2 and dW1 of both halves; the chains'
+        // E3 for the loss inputs) are done once done[5] completes its tile k - 1 phase.  It cannot be a phase
+        // further: its tile k phase needs this warpgroup's own tile k arrival.
         if (k > 0) mbar_wait(bar_done(5), (uint32_t)((k - 1) & 1));
         load_x(k + 1);
       }
@@ -696,28 +725,28 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
         const int orow = r0 + 8 * q;
         const long long row = tile * T3_ROWS + orow;
         const bool owner = q < 2, valid = owner && row < p.n_rows;
+        // this row's running b3 sums of its class (ACC_DB3); a class starts at zero on its first tile, k < 4
+        float* const s3p = acc + (ACC_DB3 + 16u * (uint32_t)((k + 2 * c) & 3)) * ACC_LANES + orow;
+        float o[8];
+        chain_mma<16, K, 4>(o, H2_K, W3_K);
+        // the row's loss inputs, copied in with the tile's observations (xfull[k & 1], waited for above)
+        const float* li = reinterpret_cast<const float*>(sm + S3_LOSS + (uint32_t)(k & 1) * T3_LI_BYTES);
         float pf_act[15], pf_in = 0.f, pf_old = 0.f;  // pf_in: the advantage (policy) or the return (value)
 #pragma unroll
         for (int a = 0; a < 15; ++a) pf_act[a] = 0.f;
-        // this row's running b3 sums of its class (ACC_DB3); a class starts at zero on its first tile, k < 4
-        float* const s3p = acc + (ACC_DB3 + 16u * (uint32_t)((k + 2 * c) & 3)) * ACC_LANES + orow;
-        if (valid) {  // issue the loads before the product
+        if (valid) {
           if (c == 0) {
             if (p.dist == B200RL_DIST_GAUSSIAN) {
 #pragma unroll
               for (int a = 0; a < 15; ++a)
-                if (a < A_out) pf_act[a] = __ldg(p.actions + row * A_out + a);
+                if (a < A_out) pf_act[a] = li[orow * A_out + a];
             } else {
-              pf_act[0] = __ldg(p.actions + row);
+              pf_act[0] = li[orow];
             }
-            pf_in = __ldg(p.adv_raw + row);
-            pf_old = __ldg(p.old_logp + row);
-          } else {
-            pf_in = __ldg(p.target + row);
+            pf_old = li[T3_LI_OLD + orow];
           }
+          pf_in = li[T3_LI_IN + orow];
         }
-        float o[8];
-        chain_mma<16, K, 4>(o, H2_K, W3_K);
         float out[16];  // the owner's output row, gathered from its quad
 #pragma unroll
         for (int j = 0; j < 2; ++j)
@@ -749,12 +778,7 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
                 gaussian_logp<15>(pf_act, out, s_dist + 16, VarRecip{s_dist + 48, s_dist + 32}, A_out, lp, ent, dlp);
               else
                 categorical_logp<15>(out, (int)pf_act[0], A_out, lp, ent, dlp);  // value.long()
-              float adv = pf_in;
-              if (p.adv_stats != nullptr) {  // utils.py:91 (the statistics are re-read here: registers)
-                float adv_mean, adv_std;
-                adv_mean_std(p.adv_stats, adv_mean, adv_std);
-                adv = (adv - adv_mean) * (1.f / adv_std);
-              }
+              const float adv = (pf_in - s_adv[0]) * s_adv[1];
               float coef;
               const float term = policy_loss(B200RL_LOSS_PPO_CLIP, lp, pf_old, adv, p.inv_n, p.clip_lo, p.clip_hi, coef);
 #pragma unroll

@@ -8,7 +8,7 @@
 //     runs network c on the tiles of slot `slot`, the policy CTAs as the first wave and the value CTAs as the second.
 //     Rows are independent in the forward / backward chain, so each 64-row half of a tile is one warpgroup that
 //     issues its own m64 products and keeps the accumulator in registers: its epilogues work on the wgmma fragment
-//     and hand over to its next product through a warpgroup-local barrier.  Two more warpgroups, one per m64 half of
+//     and hand their result to its next product in registers.  Two more warpgroups, one per m64 half of
 //     the stacked A operands (the h and the l split), issue the weight-gradient products off the chains' critical
 //     path, and keep their accumulators (88 floats a thread) in registers for the whole launch; they are stored once,
 //     in grad_acc_off's layout, for the read-out.  mbarriers tell the gradient warpgroups when both chain halves have
@@ -21,6 +21,10 @@
 //     n32 groups, to run the epilogue of one half under the product of the other, made the launch slower (more
 //     shared-memory reads of A per product), and so did issuing the b3 running-sum loads before the OUT product
 //     (126 registers instead of 122); neither is kept (README);
+//   * Z2, OUT, dH2 and dH1 take their A operand from registers (wgmma RS form): the fp16 pairs an epilogue splits
+//     for stmatrix are already the next product's A fragment, so the chain neither reads its own activations back
+//     from shared memory nor synchronises its warpgroup before a product.  The buffers are still written, for the
+//     gradient warpgroups and for dtanh, and deliver(3) / deliver(4) run under dH2 / dH1 (README);
 //   * the observations are split into their fp16 pairs ONCE PER UPDATE by pack_obs_kernel (every step of the update
 //     reads the same observations) into ready-made SWIZZLE_128B tile images [128 rows][h cols 0..31 | l cols 32..63];
 //     the step kernel brings a tile image in with ONE 16 KB bulk copy (cp.async.bulk + mbarrier complete_tx) issued by
@@ -111,8 +115,9 @@ __device__ __forceinline__ uint32_t grad_acc_off(uint32_t pcol, int n, int row, 
 
 #ifdef B200RL_TC3_TIMING
 // CTA 0, chain warpgroup wg (64-row half): [10 wg + s - 1] cycles stage s (E1..E5) waited on an mbarrier,
-// [10 wg + 4 + s] cycles of stage s in all; gradient warpgroup g (m64 half of A): [40 + 3 g + s - 3] cycles waited for
-// the operands of stage s (3..5) (stage 4 of the observations' producer: also for the other half's dW3 to release the
+// [10 wg + 4 + s] cycles of stage s in all (a stage ends when its result is stored, or delivered where it is handed to
+// the gradient warpgroups; deliver(3) / deliver(4) come after the issue of dH2 / dH1); gradient warpgroup g (m64 half
+// of A): [40 + 3 g + s - 3] cycles waited for the operands of stage s (3..5) (stage 4 of the observations' producer: also for the other half's dW3 to release the
 // dOut buffer), [46 + 3 g + s - 3] cycles issuing its products, waiting for them and handing the buffers back;
 // [52] tiles of the CTA, [53] set-up, [54] tile loop, [55] read-out
 __device__ unsigned long long g_tc3_t[64];
@@ -216,6 +221,25 @@ __device__ __forceinline__ void chain_mma(float (&d)[N / 2], const Op2 a, const 
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
   wg_mma<N, K_MAJOR, TB, 3, KSTEPS>(d, alo, blo, a.hi, b.hi, a.k_step, b.k_step, 0u);
+}
+// chain_mma with A from registers: ah[s] / al[s] = this thread's A fragment of k-step s in the h / l split (the previous
+// epilogue's pairs, wgmma_f16_n64_rs).  The same terms in the same order, issued and committed but not waited for:
+// until the caller's wgmma_wait_all, nothing may read or write d, ah or al.
+template <int N, int TB, int KSTEPS>
+__device__ __forceinline__ void chain_mma_rs(float (&d)[N / 2], const uint32_t (&ah)[KSTEPS][4],
+                                             const uint32_t (&al)[KSTEPS][4], const Op2 b) {
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+  wgmma_fence();
+  auto desc = [&](uint32_t lo) { return ((uint64_t)b.hi << 32) | lo; };
+#pragma unroll
+  for (int k = 0; k < KSTEPS; ++k)
+    wgmma_run_rs<N, TB>(d, ah[k], desc(b.lo + b.split_step + (uint32_t)k * b.k_step), k == 0 ? 0u : 1u);
+#pragma unroll
+  for (int k = 0; k < KSTEPS; ++k) wgmma_run_rs<N, TB>(d, al[k], desc(b.lo + (uint32_t)k * b.k_step), 1u);
+#pragma unroll
+  for (int k = 0; k < KSTEPS; ++k) wgmma_run_rs<N, TB>(d, ah[k], desc(b.lo + (uint32_t)k * b.k_step), 1u);
+  wgmma_commit();
 }
 // Four 8 x 8 fp16 matrices between registers and shared memory; lane l gives the address of row l & 7 of matrix l >> 3
 __device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
@@ -597,10 +621,8 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     const int quad = lane >> 2, q = lane & 3;
     const int r0 = 64 * wg + 16 * (warp & 3) + quad;  // == quad (mod 8): the swizzle phase of both fragment rows
     const uint32_t rows = (uint32_t)wg * (64u * 128u);  // this half in a K-major buffer
+    // Z1's A, X, comes from shared memory (the bulk copy puts it there); the later products take A from registers
     const Op2 X_K = op2_at(op2_kmajor(ub + S3_XB, 64), rows);  // A: X, h at +0, l at +64 bytes
-    const Op2 DO_K = op2_at(op2_kmajor(ub + S3_DO, 32), rows + c * 64);  // A, K = 16: dOut h at +0, l at +32 bytes
-    const Op2 H1_K = op2_at(op2_kmajor(ub + S3_H1, T2_ACT), rows), H2_K = op2_at(op2_kmajor(ub + S3_H2, T2_ACT), rows);
-    const Op2 DZ2_K = op2_at(op2_kmajor(ub + S3_DZ2, T2_ACT), rows);
     const Op2 W1T_M = op2_mnmajor(ub + S3_W, 32 * 128, T3_W1T);
     const Op2 W2_K = op2_kmajor(ub + S3_W + 2 * T3_W1T, T3_W2), W2_M = op2_mnmajor(ub + S3_W + 2 * T3_W1T, 64 * 128, T3_W2);
     const Op2 W3_K = op2_kmajor(ub + S3_W + 2 * T3_W1T + 2 * T3_W2, T3_W3),
@@ -615,17 +637,23 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
     // and a row of that matrix is one 16-byte chunk of a SWIZZLE_128B buffer.  One .x4 access moves matrices
     // (j, 0), (j, 1), (j + 1, 0), (j + 1, 1) for even j, i.e. fragment elements 4 j .. 4 j + 7; lane l gives the address
     // of row l & 7 of matrix l >> 3: at `buf` + mat_off(j), chunk (j + (l >> 4)) ^ (l & 7) = j ^ ((l >> 4) ^ (l & 7)).
+    // The four registers of one .x4 access (j = 2 s) are also the wgmma A fragment of k-step s, in the order a0..a3:
+    // the chain's next product takes them from registers (chain_mma_rs) instead of reading the buffer back.
     const uint32_t mat_row = base + (uint32_t)(64 * wg + 16 * (warp & 3) + 8 * ((lane >> 3) & 1) + (lane & 7)) * 128u;
     const uint32_t mat_chunk = (uint32_t)((lane >> 4) ^ (lane & 7)) << 4;
     auto mat_off = [&](uint32_t buf, int j) -> uint32_t { return mat_row + buf + (((uint32_t)j << 4) ^ mat_chunk); };
-    auto store_pairs = [&](uint32_t buf, const float (&x)[32]) {
+    uint32_t ph[4][4], pl[4][4];  // the fragment's fp16 pairs, h and l split: [k-step of the next product][a0..a3]
+    auto split_pairs = [&](const float (&x)[32]) {
 #pragma unroll
-      for (int j = 0; j < 8; j += 2) {
-        uint32_t h[4], l[4];
+      for (int s = 0; s < 4; ++s)
 #pragma unroll
-        for (int m = 0; m < 4; ++m) split2h(x[4 * j + 2 * m], x[4 * j + 2 * m + 1], h[m], l[m]);
-        stmatrix_x4(mat_off(buf, j), h);
-        stmatrix_x4(mat_off(buf + T2_ACT, j), l);
+        for (int m = 0; m < 4; ++m) split2h(x[8 * s + 2 * m], x[8 * s + 2 * m + 1], ph[s][m], pl[s][m]);
+    };
+    auto store_pairs = [&](uint32_t buf) {
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        stmatrix_x4(mat_off(buf, 2 * s), ph[s]);
+        stmatrix_x4(mat_off(buf + T2_ACT, 2 * s), pl[s]);
       }
     };
     // E1 / E2: Z * unscale + bias -> tanh(.) * 2^14
@@ -667,13 +695,12 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
       }
       if (!(m <= T2_RANGE)) bad = true;  // magnitude only: the inputs were checked
     };
-    // this warpgroup's shared-memory writes -> visible to its own next product and to the gradient warpgroup
-    auto wg_sync = [&]() {
+    // this warpgroup's shared-memory writes -> visible to the gradient warpgroups' products of stage s (the barrier also
+    // orders H1 / H2 before dtanh reads them back).  deliver(3) and deliver(4) run under the chain's next product, whose
+    // registers and operands they do not touch.
+    auto deliver = [&](int s) {
       fence_proxy_async_smem();
       asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-    };
-    auto deliver = [&](int s) {
-      wg_sync();
       if ((tid & 127) == 0) mbar_arrive(bar_ready(s));
     };
 #ifdef B200RL_TC3_TIMING
@@ -710,16 +737,19 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
         wait(1, bars + 8 * (uint32_t)(k & 1), (uint32_t)((k >> 1) & 1));  // the tile's observations have arrived
         chain_mma<64, MN, 2>(d, op2_at(X_K, xo), W1T_M);
         act(d, scl[C3_U1], bias);
+        split_pairs(d);
         // dW3, dW2 and db2 of the last tile have read H2, dOut, dZ2 and H1 (the chains' own products, in order)
         if (k > 0) wait(1, bar_done(4), (uint32_t)((k - 1) & 1));
-        store_pairs(S3_H1, d);
-        wg_sync();
+        // H1 and H2 are written for the gradient warpgroups (deliver(4), deliver(3)) and for this warp's own dtanh; no
+        // chain product reads them back, so no warpgroup barrier follows
+        store_pairs(S3_H1);
         stage_end(1);
         // ---- Z2 = H1 W2^T -> E2 -> H2 ----
-        chain_mma<64, K, 4>(d, H1_K, W2_K);
+        chain_mma_rs<64, K, 4>(d, ph, pl, W2_K);
+        wgmma_wait_all();
         act(d, scl[C3_U2], bias + 64);
-        store_pairs(S3_H2, d);
-        wg_sync();
+        split_pairs(d);
+        store_pairs(S3_H2);
         stage_end(2);
         // ---- OUT = H2 W3^T -> E3: loss head, one row per owner thread (lanes q = 0, 1 own rows r0, r0 + 8) ----
         const int orow = r0 + 8 * q;
@@ -728,7 +758,8 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
         // this row's running b3 sums of its class (ACC_DB3); a class starts at zero on its first tile, k < 4
         float* const s3p = acc + (ACC_DB3 + 16u * (uint32_t)((k + 2 * c) & 3)) * ACC_LANES + orow;
         float o[8];
-        chain_mma<16, K, 4>(o, H2_K, W3_K);
+        chain_mma_rs<16, K, 4>(o, ph, pl, W3_K);
+        wgmma_wait_all();
         // the row's loss inputs, copied in with the tile's observations (xfull[k & 1], waited for above)
         const float* li = reinterpret_cast<const float*>(sm + S3_LOSS + (uint32_t)(k & 1) * T3_LI_BYTES);
         float pf_act[15], pf_in = 0.f, pf_old = 0.f;  // pf_in: the advantage (policy) or the return (value)
@@ -822,19 +853,31 @@ __global__ void __launch_bounds__(T3_THREADS, 1) mlp_tc3_kernel(const Tc3Args p)
           *reinterpret_cast<uint4*>(rowp + (((c4 + 2u) ^ sw) << 4)) = l0;
           *reinterpret_cast<uint4*>(rowp + (((c4 + 3u) ^ sw) << 4)) = l1;
         }
-        deliver(3);
-        stage_end(3);
         // ---- dH2 = dOut W3 -> E4 -> dZ2 ----
-        chain_mma<64, MN, 1>(d, DO_K, W3_M);
+        // The warp's 16 dOut rows were written by its own owner lanes: read back as the A fragment of the one k-step
+        // (chunks 4 c, 4 c + 1 of the h split, 4 c + 2, 4 c + 3 of the l split) after a warp-level barrier only
+        __syncwarp();
+        {
+          uint32_t doh[1][4], dol[1][4];
+          ldmatrix_x4(mat_off(S3_DO, 4 * c), doh[0]);
+          ldmatrix_x4(mat_off(S3_DO, 4 * c + 2), dol[0]);
+          chain_mma_rs<64, MN, 1>(d, doh, dol, W3_M);
+          deliver(3);
+          stage_end(3);
+          wgmma_wait_all();
+        }
         dtanh(d, scl[C3_UH2] * hh, S3_H2);
-        store_pairs(S3_DZ2, d);
+        split_pairs(d);
+        store_pairs(S3_DZ2);
+        // ---- dH1 = dZ2 W2 -> E5 -> dZ1 ----
+        chain_mma_rs<64, MN, 4>(d, ph, pl, W2_M);
         deliver(4);
         stage_end(4);
-        // ---- dH1 = dZ2 W2 -> E5 -> dZ1 ----
-        chain_mma<64, MN, 4>(d, DZ2_K, W2_M);
+        wgmma_wait_all();
         dtanh(d, scl[C3_UH1] * hh, S3_H1);
         if (k > 0) wait(5, bar_done(5), (uint32_t)((k - 1) & 1));  // dW1 of the last tile has read dZ1
-        store_pairs(S3_DZ1, d);
+        split_pairs(d);
+        store_pairs(S3_DZ1);
         deliver(5);
         stage_end(5);
       }

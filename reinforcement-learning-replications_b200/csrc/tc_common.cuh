@@ -1,5 +1,5 @@
-// Hand-written sm_90a primitives of the tensor-core kernels: warpgroup MMA (wgmma) on shared-memory descriptors,
-// the per-CTA accumulator memory the kernels address by (row, column), mbarrier and proxy fences.
+// Hand-written sm_90a primitives of the tensor-core kernels: warpgroup MMA (wgmma) on shared-memory descriptors, or
+// with A from registers, the per-CTA accumulator memory the kernels address by (row, column), mbarrier and proxy fences.
 // PTX spellings follow the CUDA 12.9 ISA.
 //
 // Work split.  The epilogue warps of a kernel hold one row of a 128-row tile per thread and read or write
@@ -157,6 +157,29 @@ __device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t a, uint64
       : "memory");
 }
 
+// D[64 x N] (+)= A[64 x 16] B[16 x N] with A from registers (K-major, fp16): a[0..3] = this thread's packed pairs of
+// rows m0 and m0 + 8 (m0 = 16 warp + lane / 4) at columns 2 (lane % 4) + {0, 1}, then of the same rows at 8 columns
+// further.  That is the layout of fragment elements 8 s .. 8 s + 7 of an f32 accumulator, so columns 16 s .. 16 s + 15
+// of one product can be k-step s of the next.  The RS form has no transpose for A; TB: B read MN-major.
+template <int TB>
+__device__ __forceinline__ void wgmma_f16_n16_rs(float (&d)[8], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, %14;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d), "n"(TB)
+      : "memory");
+}
+template <int TB>
+__device__ __forceinline__ void wgmma_f16_n64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, %38;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d), "n"(TB)
+      : "memory");
+}
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
@@ -167,6 +190,12 @@ __device__ __forceinline__ void wgmma_run(float (&d)[N / 2], uint64_t a, uint64_
   else if constexpr (N == 32) wgmma_f16_n32<TA, TB>(d, a, b, scale_d);
   else if constexpr (N == 48) wgmma_f16_n48<TA, TB>(d, a, b, scale_d);
   else wgmma_f16_n64<TA, TB>(d, a, b, scale_d);
+}
+template <int N, int TB>
+__device__ __forceinline__ void wgmma_run_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+  static_assert(N == 16 || N == 64, "register-A wgmma shape without a wrapper");
+  if constexpr (N == 16) wgmma_f16_n16_rs<TB>(d, a, b, scale_d);
+  else wgmma_f16_n64_rs<TB>(d, a, b, scale_d);
 }
 
 // Operand majors (template arguments TA / TB of the products): K-major, or MN-major (read transposed).

@@ -343,7 +343,7 @@ typedef struct {
                             * b200rl_offpolicy_set_dqn), 3 = C51 (see b200rl_offpolicy_set_c51), 4 = IQN (created by
                             * b200rl_offpolicy_create_iqn only; see "IQN" below), 5 = discrete SAC (see
                             * "Discrete SAC" below), 6 = D4PG (created by b200rl_offpolicy_create_d4pg only; see
-                            * "D4PG" below) */
+                            * "D4PG" below), 7 = TQC (created by b200rl_offpolicy_create_tqc only; see "TQC" below) */
   int32_t dueling_k;       /* 0 = the Q network is a plain MLP; K >= 1 = a dueling Q network (algo 2 / 3 only; see
                             * "Dueling Q networks" below) */
   int32_t noisy_layers;    /* bit mask over the Q network's Linear layers in flat order: 0 = none; bit l = layer l is a
@@ -737,6 +737,48 @@ int b200rl_offpolicy_create_d4pg(const b200rl_offpolicy_config* cfg, const b200r
 /* The policy losses of the last train call that ran steps (host [K, S]; the first *n_policy_updates of each row):
  * what a prioritized call, which takes no policy-loss buffer, logged.  Refused on DQN engines. */
 int b200rl_offpolicy_get_policy_losses(b200rl_offpolicy* h, int32_t S, float* policy_losses, int32_t* n_policy_updates);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * TQC on the same engine (config algo = 7, n_q = 2; Kuznetsov, Shvechikov, Grishin & Vetrov 2020, "Controlling
+ * Overestimation Bias with Truncated Mixture of Continuous Distributional Quantile Critics"): SAC with two quantile
+ * critics and a truncated, pooled target.  Created by b200rl_offpolicy_create_tqc from a config with algo = 7 and a
+ * b200rl_tqc_config; b200rl_offpolicy_create and create_group refuse algo 7.  Networks, the state blob, steps[3],
+ * hparams, the noise layout [S, 2, B, A], set_sac (required), set_alpha / get_alpha and sac_outputs are SAC's; the
+ * critics q = [obs + A, ..., M] map [s | a] to M quantile locations theta_n^m at tau_m = (2m + 1) / (2M) (float32,
+ * QR-DQN's).  With N = 2 critics, d = n_drop_per_net, kN = N (M - d) and alpha = alpha[st], per step in float32:
+ *   target   a', log pi' = head(pi(s'), eps') as for SAC; the 2M atoms theta_targ_n^m(s', a') of both target critics
+ *            are sorted ascending (NaN last, as torch.sort) and the first kN kept, z_(1) <= ... <= z_(kN);
+ *            y_i = r + gamma (1 - d_done) (z_(i) - alpha log pi') in SAC's order of operations.  The kept sequence of
+ *            values is unique whatever the ties, so the target is deterministic.
+ *   critics  per critic n (optimizers 1, 2): u_mi = y_i - theta_n^m(s, a), rho(u) = |tau_m - 1{u < 0}| h(u), h the
+ *            Huber function at kappa = 1; the row loss L = (1 / (kN M)) sum_m sum_i rho(u_mi) (i ascending, then m in
+ *            index order); one Adam step on (1/B) sum_b L_b (summed in double in a fixed order), whose gradient w.r.t.
+ *            theta_n^m is -(sum_i |tau_m - 1{u_mi < 0}| clamp(u_mi, -1, 1)) / (kN M) / B
+ *   policy   with the critics just updated: one Adam step (optimizer 0) on
+ *            mean_B(alpha log pi - (1 / (2M)) sum_n sum_m theta_n^m(s, a_pi)); every output column of both critics
+ *            carries -1 / (2 M B), backpropagated through their action columns into SAC's squash backward pass (critic
+ *            parameters frozen)
+ *   alpha, polyak  SAC's
+ * Outputs: q{n}_values [S,B] = (sum_m theta_n^m(s, a)) / M before the update (index order), q{n}_losses [S] the critic
+ * losses above, policy_losses [S], and sac_outputs' log-prob means and alphas as for SAC.  train, train_gather,
+ * train_gather_rng and their group forms all work, as a CUDA graph or as plain launches with B200RL_OFFPOLICY_GRAPH=0.
+ * The heads reduce in a fixed order with no float atomics: a group's learners stay bit-identical to solo engines.
+ * Launches, with Lq and Lp the critics' and the policy's Linear layers: 1 per call (the temperature table), then per
+ * step SAC's 12 Lq + 4 Lp + 7 (+1 with learn_alpha = 1) plus the target kernel: 56 per step at two hidden layers, 57
+ * with a learned temperature.
+ * Refused at create: create_tqc with another algo, algo 7 through create / create_group; n_q != 2; dueling_k or
+ * noisy_layers != 0; n_quantiles outside 1..256; n_drop_per_net outside 0..n_quantiles - 1; critics that do not map
+ * obs + A -> M.  set_dqn, set_c51, set_qr, set_per, set_nstep, set_noise_keys and the train_prioritized calls refuse a
+ * TQC engine (prioritized replay and n-step returns are not implemented for it).
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t n_quantiles;    /* M, 1..256: each critic's output width */
+  int32_t n_drop_per_net; /* d, 0..M - 1: the largest d atoms per critic dropped from the pooled target */
+} b200rl_tqc_config;
+
+/* A TQC engine of n_learners learners (1 = a solo engine; 1 <= n_learners <= B200RL_MAX_LEARNERS): cfg->algo = 7. */
+int b200rl_offpolicy_create_tqc(const b200rl_offpolicy_config* cfg, const b200rl_tqc_config* tqc, int32_t n_learners,
+                                b200rl_offpolicy** out);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Learner groups: K independent off-policy learners (same config, same hyper-parameters, their own parameters, Adam

@@ -92,6 +92,10 @@ class D4pgConfig(C.Structure):
     _fields_ = [("n_atoms", C.c_int32), ("reserved", C.c_int32), ("v_min", C.c_double), ("v_max", C.c_double)]
 
 
+class TqcConfig(C.Structure):
+    _fields_ = [("n_quantiles", C.c_int32), ("n_drop_per_net", C.c_int32)]
+
+
 class SacHparams(C.Structure):
     _fields_ = [("alpha", C.c_double), ("target_entropy", C.c_double), ("alpha_lr", C.c_double),
                 ("alpha_beta1", C.c_double), ("alpha_beta2", C.c_double), ("alpha_eps", C.c_double),
@@ -205,6 +209,8 @@ SIGNATURES = {
                                               C.POINTER(C.c_void_p)]),
     "b200rl_offpolicy_create_d4pg": (C.c_int, [C.POINTER(OffPolicyConfig), C.POINTER(D4pgConfig), C.c_int32,
                                                C.POINTER(C.c_void_p)]),
+    "b200rl_offpolicy_create_tqc": (C.c_int, [C.POINTER(OffPolicyConfig), C.POINTER(TqcConfig), C.c_int32,
+                                              C.POINTER(C.c_void_p)]),
     "b200rl_offpolicy_get_policy_losses": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int32)]),
     "b200rl_offpolicy_train_gather_group": (C.c_int, [C.c_void_p, C.POINTER(OffPolicyHparams), C.c_int32, C.c_int32,
                                                       C.POINTER(OffPolicyReplay)] + [C.c_void_p] * 7 +

@@ -8,7 +8,8 @@ from .ppo import PPO
 from .qrdqn import QRDQN
 from .sac import SAC
 from .td3 import DDPG, TD3
+from .tqc import TQC
 from .trpo import TRPO
 from .vpg import VPG
 
-__all__ = ["VPG", "TRPO", "PPO", "DDPG", "D4PG", "TD3", "SAC", "DiscreteSAC", "DQN", "C51", "QRDQN", "IQN", "LearnerGroup"]
+__all__ = ["VPG", "TRPO", "PPO", "DDPG", "D4PG", "TD3", "SAC", "TQC", "DiscreteSAC", "DQN", "C51", "QRDQN", "IQN", "LearnerGroup"]

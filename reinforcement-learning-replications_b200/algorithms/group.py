@@ -1,4 +1,4 @@
-"""LearnerGroup: several independent TD3 / DDPG / D4PG / SAC / discrete SAC / DQN / C51 / QR-DQN / IQN learners (typically one per seed) trained side by side by ONE
+"""LearnerGroup: several independent TD3 / DDPG / D4PG / SAC / TQC / discrete SAC / DQN / C51 / QR-DQN / IQN learners (typically one per seed) trained side by side by ONE
 off-policy engine, every operation of a train step one launch for all of them (b200rl_offpolicy_create_group).
 
 The contract: each member ends up bit for bit where it would be had it run alone.  Members keep everything of their
@@ -73,8 +73,10 @@ def _signature(agent) -> list:
         sig += [("alpha", agent.alpha), ("learn_alpha", agent.learn_alpha), ("target_entropy", agent.target_entropy),
                 ("alpha optimizer (lr, beta1, beta2, eps)",
                  adam_hparams(agent.alpha_optimizer, [], "alpha optimizer", extra=[agent.log_alpha]))]
-    if agent.algo == OffPolicyEngine.SAC:
+    if agent.algo in OffPolicyEngine.SQUASHED:
         sig.append(("log_std bounds", (agent.policy.log_std_min, agent.policy.log_std_max)))
+    if agent.algo == OffPolicyEngine.TQC:
+        sig.append(("(n_quantiles, top_quantiles_to_drop_per_net)", agent.tqc_config))
     if agent.algo == OffPolicyEngine.D4PG:
         sig.append(("(n_atoms, v_min, v_max)", agent.d4pg_config))
         sig.append(("n_step", agent.n_step))
@@ -128,7 +130,7 @@ class LearnerGroup:
     def add(self, agent) -> None:
         """Add ``agent``; the current state of the global random generators becomes its private stream."""
         if not isinstance(agent, _OffPolicyBase):
-            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or D4PG / DiscreteSAC / DQN / C51 / QR-DQN / IQN) learners, got {type(agent).__name__}")
+            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or D4PG / TQC / DiscreteSAC / DQN / C51 / QR-DQN / IQN) learners, got {type(agent).__name__}")
         if any(m is agent for m in self.members):
             raise ValueError("LearnerGroup: this agent is already a member")
         if len(self.members) >= MAX_LEARNERS:

@@ -43,8 +43,9 @@ class SAC(_OffPolicyBase):
         adam_hparams(policy.optimizer, plin, "policy optimizer")
         for q in (q_function_1, q_function_2):
             qsz, _, _, qlin = describe_mlp(q.network)
-            if qsz[0] != O + A or qsz[-1] != 1:
-                raise ValueError(f"a Q network must map [obs {O} + act {A}] -> 1, got {qsz[0]} -> {qsz[-1]}")
+            width = self._critic_width(q)
+            if qsz[0] != O + A or qsz[-1] != width:
+                raise ValueError(f"a Q network must map [obs {O} + act {A}] -> {width}, got {qsz[0]} -> {qsz[-1]}")
             adam_hparams(q.optimizer, qlin, "q-function optimizer")
         if alpha <= 0:
             raise ValueError("alpha must be > 0")
@@ -65,6 +66,10 @@ class SAC(_OffPolicyBase):
         for t in (self.target_q_function_1, self.target_q_function_2):
             for p in t.network.parameters():
                 p.requires_grad = False
+
+    def _critic_width(self, q_function) -> int:
+        """The output width each critic network must have."""
+        return 1
 
     def _nets(self):
         return self._trainable(), [self.target_q_function_1, self.target_q_function_2]

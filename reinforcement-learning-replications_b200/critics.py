@@ -94,11 +94,9 @@ class DistributionalQFunction(_CategoricalSupport):
         return (self.distribution(observation, action) * self.support).sum(-1)
 
 
-class QuantileQFunction(_Critic):
-    """A return distribution per action as ``n_quantiles`` quantile locations (QR-DQN's critic): the network maps an
-    observation to ``n_actions x n_quantiles`` values, action a owning columns a*n_quantiles .. (a+1)*n_quantiles - 1,
-    located at the quantile midpoints ``taus``.  ``forward`` returns their means [..., n_actions], so greedy and
-    epsilon-greedy policies and the evaluator use it as they use a ``DiscreteQFunction``."""
+class _QuantileMidpoints(_Critic):
+    """A critic whose network outputs ``n_quantiles`` quantile locations per action, located at the quantile midpoints
+    ``taus`` (the quantiles of QR-DQN's and TQC's critics)."""
 
     MAX_QUANTILES = 256  # the engine's limit (b200rl.h)
 
@@ -112,12 +110,36 @@ class QuantileQFunction(_Critic):
         N = self.n_quantiles
         self.taus = torch.arange(1, 2 * N, 2, dtype=torch.float32) / torch.tensor(2 * N, dtype=torch.float32)
 
+
+class QuantileQFunction(_QuantileMidpoints):
+    """A return distribution per action as ``n_quantiles`` quantile locations (QR-DQN's critic): the network maps an
+    observation to ``n_actions x n_quantiles`` values, action a owning columns a*n_quantiles .. (a+1)*n_quantiles - 1,
+    located at the quantile midpoints ``taus``.  ``forward`` returns their means [..., n_actions], so greedy and
+    epsilon-greedy policies and the evaluator use it as they use a ``DiscreteQFunction``."""
+
     def quantiles(self, observation: Tensor) -> Tensor:
         """theta(s, a) [..., n_actions, n_quantiles]."""
         return self.network(observation).unflatten(-1, (-1, self.n_quantiles))
 
     def forward(self, observation: Tensor) -> Tensor:
         return self.quantiles(observation).sum(-1) / self.n_quantiles
+
+
+class ContinuousQuantileQFunction(_QuantileMidpoints):
+    """A return distribution for a continuous action as ``n_quantiles`` quantile locations (TQC's critic): the network
+    maps the concatenated pair [s | a] to ``n_quantiles`` values located at the quantile midpoints ``taus``.
+    ``forward`` returns their mean Q(s, a) with the trailing axis dropped, so host code written for a ``QFunction`` uses
+    it unchanged."""
+
+    def __init__(self, network: nn.Module, optimizer: Optimizer, n_quantiles: int = 25) -> None:
+        super().__init__(network, optimizer, n_quantiles)
+
+    def quantiles(self, observation: Tensor, action: Tensor) -> Tensor:
+        """theta(s, a) [..., n_quantiles]."""
+        return self.network(torch.cat((observation, action), dim=-1))
+
+    def forward(self, observation: Tensor, action: Tensor) -> Tensor:
+        return self.quantiles(observation, action).sum(-1) / self.n_quantiles
 
 
 class ImplicitQuantileQFunction(_Critic):

@@ -40,6 +40,8 @@
 // D4PG (config algo = 6, create_d4pg) is DDPG's step program (enqueue_steps) with a categorical critic over [s | a]:
 // c51_loss_kernel (act = NULL, n = 1) as the critic's head, d4pg_policy_loss_kernel as the policy's, and DQN's
 // prioritized draw / priority update and n-step staging.
+// TQC (config algo = 7, create_tqc) is SAC's step program (enqueue_sac_steps) with two quantile critics over [s | a]:
+// tqc_target_kernel truncates the pooled target atoms, tqc_critic_loss_kernel and tqc_policy_loss_kernel are the heads.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -625,6 +627,138 @@ __global__ void __launch_bounds__(GTHREADS) sac_alpha_step_kernel(const float* l
     state[2] = v;
     *alpha_next = expf(p);
   }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// TQC (algo = 7; Kuznetsov, Shvechikov, Grishin & Vetrov 2020): SAC's step program with two quantile critics over
+// [s | a], each mapping it to M quantile locations at tau_m = (2m + 1) / (2M).  The kernels below are its three heads;
+// everything else (squash head and its backward pass, temperature, polyak) is SAC's.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int TQC_MAX_QUANTILES = 256;  // M per critic; the pooled target holds up to 2M atoms
+
+// x precedes y in torch.sort's ascending order: NaN sorts last
+__device__ __forceinline__ bool tqc_before(float x, float y) { return !isnan(x) && (isnan(y) || x < y); }
+
+// One CTA per row i, one thread per pooled atom (blockDim = 2M rounded up to whole warps).  The 2M atoms
+// z = [Q1targ(s', a')_0..M-1 | Q2targ(s', a')_0..M-1] are ranked in shared memory: atom k's rank is the number of atoms
+// that precede it, ties (and NaNs) broken by pooled index, so the ranks are a permutation and the kept sequence is
+// torch.sort's whatever the ties.  The atoms of rank < kN are kept:
+//   y[i, rank] = r + gamma (1 - d) (z_k - alpha log pi(a' | s'))   (sac_q_loss_kernel's order of operations)
+template <bool LANES>
+__global__ void __launch_bounds__(2 * TQC_MAX_QUANTILES) tqc_target_kernel(
+    const float* q1t, const float* q2t, const float* rew, const float* done, const float* logp_next,
+    const float* alpha, float gamma, int M, int kN, float* y, size_t lane_stride) {
+  __shared__ float sz[2 * TQC_MAX_QUANTILES];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q1t = lane_ptr(q1t, o), q2t = lane_ptr(q2t, o), rew = lane_ptr(rew, o), done = lane_ptr(done, o);
+    logp_next = lane_ptr(logp_next, o), alpha = lane_ptr(alpha, o), y = lane_ptr(y, o);
+  }
+  const int i = blockIdx.x, k = threadIdx.x, n = 2 * M;
+  if (k < n) sz[k] = k < M ? q1t[(size_t)i * M + k] : q2t[(size_t)i * M + k - M];
+  __syncthreads();
+  if (k >= n) return;
+  const float x = sz[k];
+  int rank = 0;
+  for (int j = 0; j < n; ++j) {
+    const float v = sz[j];
+    rank += tqc_before(v, x) || (j < k && !tqc_before(x, v));  // v precedes x, or ties with it at a lower index
+  }
+  if (rank < kN) {
+    const float a = *alpha;
+    y[(size_t)i * kN + rank] = rew[i] + gamma * (1.f - done[i]) * (x - a * logp_next[i]);
+  }
+}
+
+// One CTA per row i, thread m owning critic quantile m (blockDim = M rounded up to whole warps): with
+// u_mj = y_ij - theta_m(s, a) over the kN kept target atoms j (ascending) and qr_loss_kernel's weights and Huber terms,
+//   L = (1 / (kN M)) sum_m sum_j k_mj h(u_mj)  (j, then m, in index order),
+//   dOut[i, m] = -(sum_j k_mj clamp(u_mj, -1, 1)) / (kN M) * (1 / B),  q_copy[i] = (sum_m theta_m) / M.
+// The last CTA of a learner to finish (sync counts them) writes *loss_out = mean L, summed in double as
+// qr_loss_kernel sums, and leaves the counter at 0.  No atomics touch a float.
+template <bool LANES>
+__global__ void __launch_bounds__(TQC_MAX_QUANTILES) tqc_critic_loss_kernel(
+    const float* q, const float* y, int B, int M, int kN, float* dout, float* row_loss, float* q_copy, int* sync,
+    float* loss_out, size_t lane_stride) {
+  __shared__ float sy[2 * TQC_MAX_QUANTILES], sl[TQC_MAX_QUANTILES], sth[TQC_MAX_QUANTILES];
+  __shared__ double red[32];
+  __shared__ bool last;
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q = lane_ptr(q, o), y = lane_ptr(y, o), dout = lane_ptr(dout, o), row_loss = lane_ptr(row_loss, o);
+    q_copy = lane_ptr(q_copy, o), sync = lane_ptr(sync, o), loss_out = lane_ptr(loss_out, o);
+  }
+  const int t = threadIdx.x, i = blockIdx.x;
+  for (int j = t; j < kN; j += blockDim.x) sy[j] = y[(size_t)i * kN + j];
+  const float th = t < M ? q[(size_t)i * M + t] : 0.f;
+  if (t < M) sth[t] = th;
+  __syncthreads();
+  const float norm = (float)(kN * M);
+  if (t < M) {
+    const float tau = (float)(2 * t + 1) / (float)(2 * M);
+    float lsum = 0.f, gsum = 0.f;
+    for (int j = 0; j < kN; ++j) {
+      const float u = sy[j] - th;
+      const float k = fabsf(tau - (u < 0.f ? 1.f : 0.f));
+      const float au = fabsf(u);
+      const float hu = au < 1.f ? 0.5f * u * u : au - 0.5f;
+      const float c = u > 1.f ? 1.f : (u < -1.f ? -1.f : u);  // NaN passes through, as torch's clamp lets it
+      lsum += k * hu;
+      gsum += k * c;
+    }
+    sl[t] = lsum;
+    dout[(size_t)i * M + t] = (-gsum / norm) * (1.0f / (float)B);
+  }
+  __syncthreads();
+  if (t == 0) {
+    float L = 0.f, qv = 0.f;
+    for (int m = 0; m < M; ++m) L += sl[m], qv += sth[m];
+    row_loss[i] = L / norm;
+    q_copy[i] = qv / (float)M;
+  }
+  // the last CTA of this learner reads every row's loss
+  __threadfence();
+  __syncthreads();
+  if (t == 0) last = atomicAdd(sync, 1) == (int)gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double acc = 0.0;
+  for (int r = t; r < B; r += blockDim.x) acc += (double)__ldcg(row_loss + r);
+  block_mean(acc, B, loss_out, red);
+  if (t == 0) sync[0] = 0;
+}
+
+// One CTA: the policy step's head at a = pi(s) on the critics just updated (q1, q2 [B, M]).  Per row the loss is
+// alpha log pi - (sum_m q1_m + sum_m q2_m) / (2M) (index order, Q1's quantiles first); *loss_out = its mean,
+// *logp_mean_out = mean log pi (each summed as block_mean sums), and every entry of dq1 and dq2 is -1 / (2 M B).
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) tqc_policy_loss_kernel(const float* q1, const float* q2, const float* logp,
+                                                                  const float* alpha, int B, int M, float* dq1,
+                                                                  float* dq2, float* loss_out, float* logp_mean_out,
+                                                                  size_t lane_stride) {
+  __shared__ double red[32], red_lp[32];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q1 = lane_ptr(q1, o), q2 = lane_ptr(q2, o), logp = lane_ptr(logp, o), alpha = lane_ptr(alpha, o);
+    dq1 = lane_ptr(dq1, o), dq2 = lane_ptr(dq2, o), loss_out = lane_ptr(loss_out, o);
+    logp_mean_out = lane_ptr(logp_mean_out, o);
+  }
+  const float a = *alpha;
+  const float g = -1.0f / (float)(2 * M * B);
+  for (int e = threadIdx.x; e < B * M; e += blockDim.x) dq1[e] = g, dq2[e] = g;
+  double acc = 0.0, acc_lp = 0.0;
+  for (int i = threadIdx.x; i < B; i += blockDim.x) {
+    const float *x1 = q1 + (size_t)i * M, *x2 = q2 + (size_t)i * M;
+    float s = 0.f;
+    for (int m = 0; m < M; ++m) s += x1[m];
+    for (int m = 0; m < M; ++m) s += x2[m];
+    const float lp = logp[i];
+    acc += (double)(a * lp - s / (float)(2 * M));
+    acc_lp += (double)lp;
+  }
+  block_mean(acc, B, loss_out, red);
+  block_mean(acc_lp, B, logp_mean_out, red_lp);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1981,6 +2115,13 @@ struct b200rl_offpolicy {
   // prioritized and n-step buffers; dq and qt1 are [B, N]
   bool d4pg = false;
   b200rl_d4pg_config d4pg_cfg{};
+  // TQC (cfg.algo == 7): a SAC engine (h->sac is set: every SAC buffer, the temperature and the outputs) whose critics
+  // map [s | a] -> M quantiles; qt1, qt2, dq and dq2 are [B, M]
+  bool tqc = false;
+  b200rl_tqc_config tqc_cfg{};
+  float* tqc_y = nullptr;         // [B, kN] the step's truncated target atoms, ascending
+  float* tqc_row_loss = nullptr;  // [2][B] each critic's row losses
+  int* tqc_sync = nullptr;        // [2] each critic head's CTAs done; 0 between launches
   // the replay columns, episode-end columns, trees and row counts of this call (train_gather[_rng], train_prioritized)
   ReplayLanes<true> replay{};
   std::vector<void*> allocs;
@@ -2303,16 +2444,17 @@ int adam_net(const b200rl_offpolicy* h, NetBuf& nb, const float2* table, int idx
 
 }  // namespace
 
-// The engine of create_group (ic = dc = NULL), of create_iqn (ic = the IQN counts, config algo 4) and of create_d4pg
-// (dc = the support, config algo 6)
+// The engine of create_group (ic = dc = tc = NULL), of create_iqn (ic = the IQN counts, config algo 4), of create_d4pg
+// (dc = the support, config algo 6) and of create_tqc (tc = the quantile counts, config algo 7)
 static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_config* ic,
-                         const b200rl_d4pg_config* dc, int32_t n_learners, b200rl_offpolicy** out) {
+                         const b200rl_d4pg_config* dc, int32_t n_learners, b200rl_offpolicy** out,
+                         const b200rl_tqc_config* tc = nullptr) {
   B200RL_REQUIRE(cfg && out, "offpolicy_create: NULL argument");
   B200RL_REQUIRE(n_learners >= 1 && n_learners <= B200RL_MAX_LEARNERS,
                  "offpolicy_create_group: n_learners must be 1..%d, got %d", B200RL_MAX_LEARNERS, n_learners);
   B200RL_REQUIRE(cfg->n_q == 1 || cfg->n_q == 2, "offpolicy_create: n_q must be 1 (DDPG) or 2 (TD3)");
   B200RL_REQUIRE((cfg->algo >= 0 && cfg->algo <= 3) || cfg->algo == 5 || (cfg->algo == 4 && ic != nullptr) ||
-                     (cfg->algo == 6 && dc != nullptr),
+                     (cfg->algo == 6 && dc != nullptr) || (cfg->algo == 7 && tc != nullptr),
                  "offpolicy_create: algo must be 0 (DDPG / TD3), 1 (SAC), 2 (DQN), 3 (C51) or 5 (discrete SAC), got %d "
                  "(algo 4, IQN, is created by b200rl_offpolicy_create_iqn with its counts, algo 6, D4PG, by "
                  "b200rl_offpolicy_create_d4pg with its support)", cfg->algo);
@@ -2320,7 +2462,20 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
                  cfg->algo);
   B200RL_REQUIRE(dc == nullptr || cfg->algo == 6, "offpolicy_create_d4pg: the config's algo must be 6 (D4PG), got %d",
                  cfg->algo);
-  const bool sac = cfg->algo == 1, c51 = cfg->algo == 3, iqn = cfg->algo == 4, dsac = cfg->algo == 5;
+  B200RL_REQUIRE(tc == nullptr || cfg->algo == 7, "offpolicy_create_tqc: the config's algo must be 7 (TQC), got %d",
+                 cfg->algo);
+  const bool tqc = cfg->algo == 7 && tc != nullptr;  // a SAC engine with quantile critics
+  const int TM = tqc ? tc->n_quantiles : 0, TD = tqc ? tc->n_drop_per_net : 0;
+  if (tqc) {
+    B200RL_REQUIRE(cfg->n_q == 2, "offpolicy_create_tqc: TQC needs n_q = 2 (two quantile critics), got %d", cfg->n_q);
+    B200RL_REQUIRE(cfg->dueling_k == 0 && cfg->noisy_layers == 0, "offpolicy_create_tqc: TQC takes neither dueling_k "
+                   "nor noisy_layers: dueling and noisy networks are not implemented for it");
+    B200RL_REQUIRE(TM >= 1 && TM <= TQC_MAX_QUANTILES, "offpolicy_create_tqc: n_quantiles must be 1..%d, got %d",
+                   TQC_MAX_QUANTILES, TM);
+    B200RL_REQUIRE(TD >= 0 && TD <= TM - 1, "offpolicy_create_tqc: n_drop_per_net must be 0..n_quantiles - 1 = %d, "
+                   "got %d", TM - 1, TD);
+  }
+  const bool sac = cfg->algo == 1 || tqc, c51 = cfg->algo == 3, iqn = cfg->algo == 4, dsac = cfg->algo == 5;
   const bool d4pg = cfg->algo == 6 && dc != nullptr;
   const int NA = d4pg ? dc->n_atoms : 0;
   if (d4pg) {
@@ -2405,8 +2560,11 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
                    "policy [obs, ..., n] and critics [obs, ..., n] with n >= 2 actions, got policy %d -> %d and critics "
                    "%d -> %d", O, P_out, cfg->q.sizes[0], nq);
   }
-  B200RL_REQUIRE(dqn || dsac || d4pg || (cfg->q.sizes[0] == O + A && cfg->q.sizes[cfg->q.n_layers] == 1),
+  B200RL_REQUIRE(dqn || dsac || d4pg || tqc || (cfg->q.sizes[0] == O + A && cfg->q.sizes[cfg->q.n_layers] == 1),
                  "offpolicy_create: Q network must map [obs %d + act %d] -> 1", O, A);
+  B200RL_REQUIRE(!tqc || (cfg->q.sizes[0] == O + A && cfg->q.sizes[cfg->q.n_layers] == TM),
+                 "offpolicy_create_tqc: the critics must map [obs %d + act %d] -> %d quantiles, got %d -> %d", O, A, TM,
+                 cfg->q.sizes[0], cfg->q.sizes[cfg->q.n_layers]);
   B200RL_REQUIRE(!d4pg || (cfg->q.sizes[0] == O + A && cfg->q.sizes[cfg->q.n_layers] == NA),
                  "offpolicy_create_d4pg: the critic must map [obs %d + act %d] -> %d atoms' logits, got %d -> %d", O, A,
                  NA, cfg->q.sizes[0], cfg->q.sizes[cfg->q.n_layers]);
@@ -2424,6 +2582,8 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   if (iqn) h->iqn_cfg = *ic;
   h->d4pg = d4pg;
   if (d4pg) h->d4pg_cfg = *dc, h->d4pg_cfg.reserved = 0;
+  h->tqc = tqc;
+  if (tqc) h->tqc_cfg = *tc;
   h->noisy = NM != 0;
   int rc = 0;
   int maxw = O + A;
@@ -2517,10 +2677,10 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   for (int l = 0; l <= B200RL_MAX_LAYERS; ++l) rc |= oalloc(h, &h->acts_tq[l], B * (size_t)maxw);
   rc |= oalloc(h, &h->x_cat, B * (size_t)(O + A));
   rc |= oalloc(h, &h->x_cat2, B * (size_t)(O + A));
-  // discrete SAC: [B, n] per critic; D4PG: [B, N] (the target critic's logits, the output gradient)
-  const size_t n_dq = dsac || d4pg ? (size_t)cfg->q.sizes[cfg->q.n_layers] : 1;
+  // discrete SAC: [B, n] per critic; D4PG: [B, N] (the target critic's logits, the output gradient); TQC: [B, M]
+  const size_t n_dq = dsac || d4pg || tqc ? (size_t)cfg->q.sizes[cfg->q.n_layers] : 1;
   rc |= oalloc(h, &h->qt1, B * n_dq);
-  rc |= oalloc(h, &h->qt2, B);
+  rc |= oalloc(h, &h->qt2, B * (tqc ? n_dq : 1));
   rc |= oalloc(h, &h->dq, B * n_dq);
   rc |= oalloc(h, &h->dbuf0, B * (size_t)maxw);
   rc |= oalloc(h, &h->dbuf1, B * (size_t)maxw);
@@ -2544,6 +2704,11 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
     rc |= oalloc(h, &h->sac_alpha, S + 1);
     rc |= oalloc(h, &h->sac_state, 3);
     rc |= oalloc(h, &h->out_logp, S);
+  }
+  if (tqc) {
+    rc |= oalloc(h, &h->tqc_y, B * (size_t)(2 * (TM - TD)));
+    rc |= oalloc(h, &h->tqc_row_loss, 2 * B);
+    rc |= oalloc(h, &h->tqc_sync, 2);
   }
   if (dsac) {
     rc |= oalloc(h, &h->sac_logp, B);
@@ -2664,6 +2829,12 @@ extern "C" int b200rl_offpolicy_create_d4pg(const b200rl_offpolicy_config* cfg, 
   return create_engine(cfg, nullptr, d4pg, n_learners, out);
 }
 
+extern "C" int b200rl_offpolicy_create_tqc(const b200rl_offpolicy_config* cfg, const b200rl_tqc_config* tqc,
+                                           int32_t n_learners, b200rl_offpolicy** out) {
+  B200RL_REQUIRE(tqc, "offpolicy_create_tqc: NULL TQC counts");
+  return create_engine(cfg, nullptr, nullptr, n_learners, out, tqc);
+}
+
 extern "C" void b200rl_offpolicy_destroy(b200rl_offpolicy* h) {
   if (!h) return;
   if (h->graph) cudaGraphExecDestroy(h->graph);
@@ -2782,6 +2953,7 @@ extern "C" int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hp
   B200RL_REQUIRE(h && dp, "offpolicy_set_dqn: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_dqn: a discrete SAC engine (algo = 5) takes b200rl_offpolicy_set_sac, not "
                  "set_dqn");
+  B200RL_REQUIRE(!h->tqc, "offpolicy_set_dqn: a TQC engine (algo = 7) takes b200rl_offpolicy_set_sac, not set_dqn");
   B200RL_REQUIRE(h->dqn, "offpolicy_set_dqn: the engine was not created with algo = 2 (DQN)");
   B200RL_REQUIRE(dp->target_update_interval >= 1, "offpolicy_set_dqn: target_update_interval must be >= 1, got %d",
                  dp->target_update_interval);
@@ -2794,6 +2966,7 @@ extern "C" int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hp
 extern "C" int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hparams* cp) {
   B200RL_REQUIRE(h && cp, "offpolicy_set_c51: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_c51: a discrete SAC engine (algo = 5) has no categorical head");
+  B200RL_REQUIRE(!h->tqc, "offpolicy_set_c51: a TQC engine (algo = 7) has no categorical head");
   B200RL_REQUIRE(!h->d4pg, "offpolicy_set_c51: a D4PG engine (algo = 6) takes its support at create "
                  "(b200rl_offpolicy_create_d4pg)");
   B200RL_REQUIRE(h->c51, "offpolicy_set_c51: the engine was not created with algo = 3 (C51)");
@@ -2824,6 +2997,8 @@ extern "C" int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hp
 extern "C" int b200rl_offpolicy_set_qr(b200rl_offpolicy* h, const b200rl_qr_hparams* qp) {
   B200RL_REQUIRE(h && qp, "offpolicy_set_qr: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_qr: a discrete SAC engine (algo = 5) has no quantile head");
+  B200RL_REQUIRE(!h->tqc, "offpolicy_set_qr: a TQC engine (algo = 7) takes its quantile counts at create "
+                 "(b200rl_offpolicy_create_tqc)");
   B200RL_REQUIRE(h->dqn && !h->c51 && !h->iqn, "offpolicy_set_qr: the engine was not created with algo = 2 (DQN)");
   const int N = qp->n_quantiles, width = h->net[1].d.sizes[h->net[1].d.n_layers];
   B200RL_REQUIRE(N >= 1 && N <= QR_MAX_QUANTILES, "offpolicy_set_qr: n_quantiles must be 1..%d, got %d",
@@ -2843,6 +3018,7 @@ extern "C" int b200rl_offpolicy_set_per(b200rl_offpolicy* h, const b200rl_per_hp
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_per: prioritized replay is not implemented for discrete SAC engines (algo = "
                  "5)");
   B200RL_REQUIRE(!h->c51, "offpolicy_set_per: prioritized replay is not implemented for C51 engines");
+  B200RL_REQUIRE(!h->tqc, "offpolicy_set_per: prioritized replay is not implemented for TQC engines (algo = 7)");
   B200RL_REQUIRE(h->dqn || h->d4pg, "offpolicy_set_per: prioritized replay is implemented for DQN engines (algo = 2) "
                  "and D4PG engines (algo = 6) only");
   B200RL_REQUIRE(pp->alpha >= 0.0 && std::isfinite(pp->alpha), "offpolicy_set_per: alpha must be >= 0");
@@ -2858,6 +3034,7 @@ extern "C" int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, c
   B200RL_REQUIRE(h, "offpolicy_set_nstep: NULL engine");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_nstep: n-step returns are not implemented for discrete SAC engines (algo = "
                  "5)");
+  B200RL_REQUIRE(!h->tqc, "offpolicy_set_nstep: n-step returns are not implemented for TQC engines (algo = 7)");
   B200RL_REQUIRE(h->dqn || h->d4pg, "offpolicy_set_nstep: n-step returns are implemented for DQN and C51 engines "
                  "(algo = 2 or 3) and D4PG engines (algo = 6) only");
   B200RL_REQUIRE(n_step >= 1 && n_step <= NSTEP_MAX, "offpolicy_set_nstep: n_step must be 1..%d, got %d", NSTEP_MAX,
@@ -2878,6 +3055,8 @@ extern "C" int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, c
 extern "C" int b200rl_offpolicy_set_noise_keys(b200rl_offpolicy* h, const uint64_t* seed, const uint64_t* call) {
   B200RL_REQUIRE(h && seed && call, "offpolicy_set_noise_keys: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_noise_keys: a discrete SAC engine (algo = 5) draws no noise");
+  B200RL_REQUIRE(!h->tqc, "offpolicy_set_noise_keys: a TQC engine (algo = 7) has no noisy layers; its policy's draws "
+                 "come with the train call");
   B200RL_REQUIRE(h->noisy || h->iqn, "offpolicy_set_noise_keys: the engine has no noisy layers (config noisy_layers = "
                  "0)");
   const size_t n = adam_tab_len(h);
@@ -3132,6 +3311,9 @@ static int enqueue_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp
 //   s4 : Q2 on [s | a] ............................... Q2's dW products -> polyak (both critic pairs)
 //        ... -> squash backward -> pi bwd, Adam on s; the temperature step rides on s2 behind Q2's dX chain.
 // Step st reads alpha[st]; the temperature step writes alpha[st + 1], so nothing it writes is read in the same step.
+// A TQC engine (h->tqc) differs in its heads only: tqc_target_kernel on s behind both target critics (the truncated
+// pooled atoms y), tqc_critic_loss_kernel in place of each soft Q loss, tqc_policy_loss_kernel in place of the policy
+// loss, and the critics' dOut M wide in every backward pass.
 static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s) {
   const int O = h->O, A = h->A;
   const int maxS = h->cfg.max_steps;
@@ -3141,6 +3323,9 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
   const float lmin = (float)sp.log_std_min, lmax = (float)sp.log_std_max, limit = (float)hp->action_limit;
   const int ew = 256, rows_grid = (B + 127) / 128;
   cudaStream_t s2 = h->s2, s3 = h->s3, s4 = h->s4;
+  const bool tqc = h->tqc;
+  const int NQ = tqc ? h->tqc_cfg.n_quantiles : 1;             // the critics' output width, M
+  const int kN = tqc ? 2 * (NQ - h->tqc_cfg.n_drop_per_net) : 0;  // target atoms kept
   if (launch(h, sac_alpha_init_kernel<false>, sac_alpha_init_kernel<true>, (S + 1 + ew - 1) / ew, ew, 0, s,
              h->sac_alpha, S + 1, h->sac_state, sp.learn_alpha, (float)sp.alpha))
     return 1;
@@ -3194,6 +3379,10 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
     if (net_forward(h, q2t, tq[1], B, s2, h->sac_act_next, A, O)) return 1;
     if (net_forward(h, q1t, tq[0], B, s, h->sac_act_next, A, O)) return 1;
     if (edge(h, s2, s)) return 1;
+    if (tqc && launch(h, tqc_target_kernel<false>, tqc_target_kernel<true>, B,
+                      (2 * NQ + 31) / 32 * 32, 0, s, h->qt1, h->qt2, s_rew, s_done,
+                      h->sac_logp_next, alpha, (float)hp->gamma, NQ, kN, h->tqc_y))
+      return 1;
     // ---- critic step: soft TD target + MSE + dq, backward, Adam (Q2 on s2, Q1 on s) ----
     if (edge(h, s, s2)) return 1;
     if (edge(h, s4, s2)) return 1;
@@ -3202,11 +3391,18 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
       NetBuf& qn = qi == 0 ? q1 : q2;
       cudaStream_t qs = qi == 0 ? s : s2;
       float* dq = qi == 0 ? h->dq : h->dq2;
-      if (launch(h, sac_q_loss_kernel<false>, sac_q_loss_kernel<true>, 1, GTHREADS, 0, qs, qa[qi][Lq], s_rew, s_done,
-                 h->qt1, h->qt2, h->sac_logp_next, alpha, (float)hp->gamma, B, dq,
-                 (qi == 0 ? h->out_l1 : h->out_l2) + st, (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B))
+      if (tqc) {  // the quantile Huber loss of the critic's M quantiles against the kN kept target atoms
+        if (launch(h, tqc_critic_loss_kernel<false>, tqc_critic_loss_kernel<true>, B,
+                   (NQ + 31) / 32 * 32, 0, qs, qa[qi][Lq], h->tqc_y, B, NQ, kN, dq,
+                   h->tqc_row_loss + (size_t)qi * B, (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B,
+                   h->tqc_sync + qi, (qi == 0 ? h->out_l1 : h->out_l2) + st))
+          return 1;
+      } else if (launch(h, sac_q_loss_kernel<false>, sac_q_loss_kernel<true>, 1, GTHREADS, 0, qs, qa[qi][Lq], s_rew,
+                        s_done, h->qt1, h->qt2, h->sac_logp_next, alpha, (float)hp->gamma, B, dq,
+                        (qi == 0 ? h->out_l1 : h->out_l2) + st, (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B)) {
         return 1;
-      if (net_backward(h, qn, qa[qi], dq, 1, B, true, nullptr, qs, qi != 0, s_act, A, O, qi == 0 ? s3 : s4)) return 1;
+      }
+      if (net_backward(h, qn, qa[qi], dq, NQ, B, true, nullptr, qs, qi != 0, s_act, A, O, qi == 0 ? s3 : s4)) return 1;
       if (adam_net(h, qn, h->adam_tab + (size_t)(1 + qi) * maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, qs)) return 1;
     }
     if (edge(h, s2, s)) return 1;
@@ -3225,11 +3421,16 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
     if (net_forward(h, q2, qp[1], B, s2, h->sac_act, A, O)) return 1;
     if (net_forward(h, q1, qp[0], B, s, h->sac_act, A, O)) return 1;
     if (edge(h, s2, s)) return 1;
-    if (launch(h, sac_policy_loss_kernel<false>, sac_policy_loss_kernel<true>, 1, GTHREADS, 0, s, qp[0][Lq], qp[1][Lq],
-               h->sac_logp, alpha, B, h->dq, h->dq2, h->out_lp + st, h->out_logp + st))
+    if (tqc) {  // every quantile of both critics carries -1 / (2 M B)
+      if (launch(h, tqc_policy_loss_kernel<false>, tqc_policy_loss_kernel<true>, 1, GTHREADS, 0, s, qp[0][Lq],
+                 qp[1][Lq], h->sac_logp, alpha, B, NQ, h->dq, h->dq2, h->out_lp + st, h->out_logp + st))
+        return 1;
+    } else if (launch(h, sac_policy_loss_kernel<false>, sac_policy_loss_kernel<true>, 1, GTHREADS, 0, s, qp[0][Lq],
+                      qp[1][Lq], h->sac_logp, alpha, B, h->dq, h->dq2, h->out_lp + st, h->out_logp + st)) {
       return 1;
+    }
     if (edge(h, s, s2)) return 1;
-    if (net_backward(h, q2, qp[1], h->dq2, 1, B, false, h->x_cat2, s2, true)) return 1;
+    if (net_backward(h, q2, qp[1], h->dq2, NQ, B, false, h->x_cat2, s2, true)) return 1;
     if (sp.learn_alpha) {  // -mean(log_alpha (log pi + target_entropy)), one Adam step; alpha[st + 1] = exp(log_alpha)
       if (launch(h, sac_alpha_step_kernel<false>, sac_alpha_step_kernel<true>, 1, GTHREADS, 0, s2, h->sac_logp, B,
                  (float)sp.target_entropy, h->sac_state, h->adam_tab + (size_t)3 * maxS, st,
@@ -3237,7 +3438,7 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
                  (float)sp.alpha_eps, h->sac_alpha + st + 1))
         return 1;
     }
-    if (net_backward(h, q1, qp[0], h->dq, 1, B, false, h->x_cat, s)) return 1;
+    if (net_backward(h, q1, qp[0], h->dq, NQ, B, false, h->x_cat, s)) return 1;
     if (edge(h, s2, s)) return 1;
     if (launch(h, sac_squash_backward_kernel<false>, sac_squash_backward_kernel<true>, (B * A + ew - 1) / ew, ew, 0, s,
                pa[Lp], eps_cur, h->x_cat + O, h->x_cat2 + O, O + A, B, A, lmin, lmax, limit, alpha, h->sac_dout))
@@ -3911,6 +4112,8 @@ extern "C" int b200rl_offpolicy_train_prioritized_group(b200rl_offpolicy* h, con
   B200RL_REQUIRE(!h->c51, "offpolicy_train_prioritized: prioritized replay is not implemented for C51 engines");
   B200RL_REQUIRE(!h->dsac, "offpolicy_train_prioritized: prioritized replay is not implemented for discrete SAC "
                  "engines (algo = 5)");
+  B200RL_REQUIRE(!h->tqc, "offpolicy_train_prioritized: prioritized replay is not implemented for TQC engines (algo = "
+                 "7)");
   B200RL_REQUIRE(h->dqn || h->d4pg, "offpolicy_train_prioritized: prioritized replay is implemented for DQN engines "
                  "(algo = 2) and D4PG engines (algo = 6) only");
   B200RL_REQUIRE(h->per_set, "offpolicy_train_prioritized: call b200rl_offpolicy_set_per first");

@@ -336,20 +336,23 @@ class OffPolicyEngine:
     and ``set_sac`` must be called before the first train call (b200rl.h, "Discrete SAC").  D4PG (``algo`` 6) has
     DDPG's networks with a categorical critic: ``q_sizes`` = [obs + act, ..., N] and ``d4pg`` = (N, v_min, v_max), the
     critic's support; it takes ``set_per`` / ``train_prioritized`` and ``set_nstep`` as DQN does (b200rl.h, "D4PG").
+    TQC (``algo`` 7) is a SAC engine whose critics map [s | a] to M quantiles: ``q_sizes`` = [obs + act, ..., M] and
+    ``tqc`` = (M, d), d the atoms per critic dropped from the pooled target (b200rl.h, "TQC").
 
     ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
     launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
     is [K][per-learner blob] with [K][3] step counts, and the per-network accessors are refused."""
 
     NETS = {"policy": 0, "q1": 1, "q2": 2, "target_policy": 3, "target_q1": 4, "target_q2": 5}
-    TD3, SAC, DQN, C51, IQN, DSAC, D4PG = 0, 1, 2, 3, 4, 5, 6
+    TD3, SAC, DQN, C51, IQN, DSAC, D4PG, TQC = 0, 1, 2, 3, 4, 5, 6, 7
     DISCRETE = (DQN, C51, IQN)  # the algos with DQN's networks, inputs and outputs
     INDEX_ACTIONS = DISCRETE + (DSAC,)  # the algos whose action column holds an action index
-    SOFT = (SAC, DSAC)  # the algos with SAC's networks, temperature and outputs
+    SOFT = (SAC, DSAC, TQC)  # the algos with SAC's networks, temperature and outputs
+    SQUASHED = (SAC, TQC)  # the algos with SAC's squashed-Gaussian policy and its [S, 2, B, A] noise
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
                  q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1, dueling_k: int = 0,
-                 noisy_layers: int = 0, iqn=None, d4pg=None):
+                 noisy_layers: int = 0, iqn=None, d4pg=None, tqc=None):
         from ._lib import OffPolicyConfig
         self.lib = _lib.load()
         current_stream_handle()
@@ -362,6 +365,7 @@ class OffPolicyEngine:
         self.algo, self.dueling_k, self.noisy_layers = int(algo), int(dueling_k), int(noisy_layers)
         self.iqn = None if iqn is None else tuple(int(x) for x in iqn)
         self.d4pg = None if d4pg is None else (int(d4pg[0]), float(d4pg[1]), float(d4pg[2]))
+        self.tqc = None if tqc is None else (int(tqc[0]), int(tqc[1]))
         self.discrete = self.algo in self.DISCRETE  # DQN's networks and outputs
         self.index_actions = self.algo in self.INDEX_ACTIONS  # act [S,B] indices, no noise
         self.n_q, self.max_minibatch, self.max_steps = int(n_q), int(max_minibatch), int(max_steps)
@@ -387,6 +391,9 @@ class OffPolicyEngine:
             n_atoms, v_min, v_max = self.d4pg
             check(self.lib.b200rl_offpolicy_create_d4pg(C.byref(cfg), C.byref(_lib.D4pgConfig(n_atoms, 0, v_min, v_max)),
                                                         self.K, C.byref(h)), "offpolicy_create_d4pg")
+        elif self.tqc is not None:  # the quantile counts size the critics' heads (b200rl.h, "TQC")
+            check(self.lib.b200rl_offpolicy_create_tqc(C.byref(cfg), C.byref(_lib.TqcConfig(*self.tqc)), self.K,
+                                                       C.byref(h)), "offpolicy_create_tqc")
         else:
             check(self.lib.b200rl_offpolicy_create_group(C.byref(cfg), self.K, C.byref(h)), "offpolicy_create")
         self.h = h
@@ -697,7 +704,7 @@ class OffPolicyEngine:
             act = np.asarray(act, np.float32)[..., None]
         obs, act, next_obs = (self._lead(x, np.float32, 4) for x in (obs, act, next_obs))
         rew, done = self._lead(rew, np.float32, 3), self._lead(done, np.float32, 3)
-        noise = None if noise is None else self._lead(noise, np.float32, 5 if self.algo == self.SAC else 4)
+        noise = None if noise is None else self._lead(noise, np.float32, 5 if self.algo in self.SQUASHED else 4)
         S, B = obs.shape[1], obs.shape[2]
         q1v, q2v, l1, l2, lp, npol = self._out_buffers(S, B)
         check(self.lib.b200rl_offpolicy_train(self.h, C.byref(hp), S, B, _ptr(obs), _ptr(act), _ptr(rew), _ptr(next_obs),
@@ -730,7 +737,7 @@ class OffPolicyEngine:
         idx = np.empty((self.K, S, B), np.int64)
         with_noise = with_noise and not self.index_actions  # DQN, C51 and discrete SAC draw indices only
         noise = None
-        if with_noise and self.algo == self.SAC:
+        if with_noise and self.algo in self.SQUASHED:
             noise = np.empty((self.K, S, 2, B, self.policy_sizes[-1] // 2), np.float32)
         elif with_noise:
             noise = np.empty((self.K, S, B, self.policy_sizes[-1]), np.float32)
@@ -757,7 +764,7 @@ class OffPolicyEngine:
         ``idx`` [K,S,B], ``noise`` [K,S,B,A] (SAC [K,S,2,B,A]); a solo engine also takes them without the [K] axis."""
         rb = self._replays(replays)
         idx = self._lead(idx, np.int64, 3)
-        noise = None if noise is None else self._lead(noise, np.float32, 5 if self.algo == self.SAC else 4)
+        noise = None if noise is None else self._lead(noise, np.float32, 5 if self.algo in self.SQUASHED else 4)
         S, B = idx.shape[1], idx.shape[2]
         q1v, q2v, l1, l2, lp, npol = self._out_buffers(S, B)
         check(self.lib.b200rl_offpolicy_train_gather_group(self.h, C.byref(hp), S, B, rb, _ptr(idx), _ptr(noise),

@@ -343,7 +343,8 @@ typedef struct {
                             * b200rl_offpolicy_set_dqn), 3 = C51 (see b200rl_offpolicy_set_c51), 4 = IQN (created by
                             * b200rl_offpolicy_create_iqn only; see "IQN" below), 5 = discrete SAC (see
                             * "Discrete SAC" below), 6 = D4PG (created by b200rl_offpolicy_create_d4pg only; see
-                            * "D4PG" below), 7 = TQC (created by b200rl_offpolicy_create_tqc only; see "TQC" below) */
+                            * "D4PG" below), 7 = TQC (created by b200rl_offpolicy_create_tqc only; see "TQC" below),
+                            * 8 = CQL (created by b200rl_offpolicy_create_cql only; see "CQL" below) */
   int32_t dueling_k;       /* 0 = the Q network is a plain MLP; K >= 1 = a dueling Q network (algo 2 / 3 only; see
                             * "Dueling Q networks" below) */
   int32_t noisy_layers;    /* bit mask over the Q network's Linear layers in flat order: 0 = none; bit l = layer l is a
@@ -779,6 +780,75 @@ typedef struct {
 /* A TQC engine of n_learners learners (1 = a solo engine; 1 <= n_learners <= B200RL_MAX_LEARNERS): cfg->algo = 7. */
 int b200rl_offpolicy_create_tqc(const b200rl_offpolicy_config* cfg, const b200rl_tqc_config* tqc, int32_t n_learners,
                                 b200rl_offpolicy** out);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * CQL on the same engine (config algo = 8, n_q = 2; Kumar, Zhou, Tucker & Levine 2020, "Conservative Q-Learning for
+ * Offline Reinforcement Learning", CQL(H)): SAC whose critics also push down a log-sum-exp over sampled actions.
+ * Created by b200rl_offpolicy_create_cql from a config with algo = 8 and a b200rl_cql_config; create and create_group
+ * refuse algo 8.  Networks, the state blob, steps[3], set_sac (required), set_alpha / get_alpha, the noise layout
+ * [S, 2, B, A] and sac_outputs are SAC's; set_cql is required too.  With N = n_actions, T = temperature, w = weight,
+ * L = action_limit, A the action width, alpha = alpha[st] and per step in float32 (the policy and critics at the start
+ * of the step):
+ *   draws    per row i and j < N: u_ij = L (2 x_ij - 1) with x_ij uniform in [0, 1), log density lu = -A log(2L);
+ *            a^n_ij, log pi^n_ij = head(pi(s'_i), eps^n_ij) and a^s_ij, log pi^s_ij = head(pi(s_i), eps^s_ij) with
+ *            SAC's squash head, from the policy outputs the step computes anyway (the policy is not fanned out)
+ *   target   y_i = r + gamma (1 - d) (min(Q1targ, Q2targ)(s', a') - [backup_entropy] alpha log pi')
+ *   critic k c_ij = [Q_k(s_i, u_ij) - lu]_j ++ [Q_k(s_i, a^n_ij) - log pi^n_ij]_j ++ [Q_k(s_i, a^s_ij) - log pi^s_ij]_j
+ *            (3N values, every one at s_i); P_i = T logsumexp_j(c_ij / T) (max first, then the sum in index order);
+ *            gap_k = mean_i P_i - mean_i Q_k(s_i, a_i); w_eff = w, or alpha' w with the Lagrange step;
+ *            loss_k = mean_i (Q_k(s_i, a_i) - y_i)^2 + w_eff gap_k [- alpha' tau]; samples and log densities are
+ *            constants; d loss_k / d Q_k(s_i, sample j) = w_eff softmax_j(c_ij / T) / B and
+ *            d loss_k / d Q_k(s_i, a_i) = 2 (Q_k - y_i) / B - w_eff / B; one Adam step per critic
+ *   Lagrange (config lagrange = 1) alpha' = clamp(exp(log alpha'), 0, 1e6) at the start of the step; one Adam step on
+ *            log alpha' for -1/2 sum_k alpha' (w gap_k - tau) (gaps of this step's pre-update critics) with alpha_lr /
+ *            alpha_beta1 / alpha_beta2 / alpha_eps; step st reads alpha'[st] and writes alpha'[st + 1]
+ *   policy, temperature, polyak   SAC's, in SAC's order (the policy step reads the critics just updated)
+ * Each critic's forward and backward passes in the critic step run on R = (1 + 3N) B stacked rows: rows 0..B-1 are
+ * [s_i | a_i], row B + i 3N + j is sample j of row i in the block order above; the data rows' forward results and the
+ * order of the weight-gradient sums over them are SAC's, so weight = 0 reproduces a SAC engine bit for bit on the same
+ * draws.  Draws: a call with host draws (train, train_gather) needs b200rl_offpolicy_set_cql_draws first with
+ * [K][S][3][B][N][A] floats: x, then eps^s, then eps^n, each [B][N][A]; train_gather_rng draws them on the device
+ * (Philox tag 0xC91, x with 24 bits) and get_cql_draws reads them back in that layout.
+ * Outputs: SAC's (q{k}_losses the loss_k above) and cql_outputs' gaps [K][2][S] and alpha' [K][S] (1 without the
+ * Lagrange step).  The heads reduce in a fixed order with no float atomics: a group's learners stay bit-identical to
+ * solo engines.
+ * Launches, with Lq and Lp the critics' and the policy's Linear layers: 1 per call (the temperature table), 1 more with
+ * the Lagrange step (the alpha' table), then per step SAC's 12 Lq + 4 Lp + 7 (+1 with learn_alpha = 1) plus the staging
+ * kernel and the two penalty heads (+1 with the Lagrange step): 58 per step at two hidden layers, 59 with a learned
+ * temperature, 60 with both.  train_gather_rng adds one draw launch per call.
+ * Refused at create: create_cql with another algo, algo 8 through create / create_group; n_q != 2; dueling_k or
+ * noisy_layers != 0; n_actions outside 1..64; (1 + 3N) max_minibatch above 65535 x 32 rows.  Prioritized replay, n-step
+ * returns and noisy layers are refused as for SAC.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t n_actions; /* N, 1..64: samples per row from each of the three proposals */
+  int32_t lagrange;  /* 1 = learn alpha' against target_action_gap, 0 = a fixed weight */
+} b200rl_cql_config;
+
+typedef struct {
+  double weight;            /* w >= 0 */
+  double temperature;       /* T > 0 */
+  double target_action_gap; /* tau (Lagrange only) */
+  double alpha_lr, alpha_beta1, alpha_beta2, alpha_eps; /* the Adam settings of log alpha' (Lagrange only) */
+  int32_t backup_entropy;   /* 1 = SAC's soft target, 0 = no entropy term in the backup */
+  int32_t reserved;         /* zeroed by set_cql */
+} b200rl_cql_hparams;
+
+/* A CQL engine of n_learners learners (1 = a solo engine; 1 <= n_learners <= B200RL_MAX_LEARNERS): cfg->algo = 8. */
+int b200rl_offpolicy_create_cql(const b200rl_offpolicy_config* cfg, const b200rl_cql_config* cql, int32_t n_learners,
+                                b200rl_offpolicy** out);
+/* Required once before the first train call; part of the cached graph's key. */
+int b200rl_offpolicy_set_cql(b200rl_offpolicy* h, const b200rl_cql_hparams* hp);
+/* {log alpha', exp_avg, exp_avg_sq} and the Adam step count of each of the K learners. */
+int b200rl_offpolicy_set_alpha_prime_group(b200rl_offpolicy* h, const float* log_alpha_prime, const float* exp_avg,
+                                           const float* exp_avg_sq, const int64_t* step);
+int b200rl_offpolicy_get_alpha_prime_group(b200rl_offpolicy* h, float* log_alpha_prime, float* exp_avg,
+                                           float* exp_avg_sq, int64_t* step);
+/* gaps [K][2][S] and alpha' [K][S] of the last train call's steps. */
+int b200rl_offpolicy_cql_outputs(b200rl_offpolicy* h, int32_t S, float* gaps, float* alpha_primes);
+/* The host draws [K][S][3][B][N][A] of the next train / train_gather call, and the draws of the last call. */
+int b200rl_offpolicy_set_cql_draws(b200rl_offpolicy* h, int32_t S, int32_t B, const float* draws);
+int b200rl_offpolicy_get_cql_draws(b200rl_offpolicy* h, int32_t S, int32_t B, float* draws);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Learner groups: K independent off-policy learners (same config, same hyper-parameters, their own parameters, Adam

@@ -96,6 +96,16 @@ class TqcConfig(C.Structure):
     _fields_ = [("n_quantiles", C.c_int32), ("n_drop_per_net", C.c_int32)]
 
 
+class CqlConfig(C.Structure):
+    _fields_ = [("n_actions", C.c_int32), ("lagrange", C.c_int32)]
+
+
+class CqlHparams(C.Structure):
+    _fields_ = [("weight", C.c_double), ("temperature", C.c_double), ("target_action_gap", C.c_double),
+                ("alpha_lr", C.c_double), ("alpha_beta1", C.c_double), ("alpha_beta2", C.c_double),
+                ("alpha_eps", C.c_double), ("backup_entropy", C.c_int32), ("reserved", C.c_int32)]
+
+
 class SacHparams(C.Structure):
     _fields_ = [("alpha", C.c_double), ("target_entropy", C.c_double), ("alpha_lr", C.c_double),
                 ("alpha_beta1", C.c_double), ("alpha_beta2", C.c_double), ("alpha_eps", C.c_double),
@@ -234,6 +244,14 @@ SIGNATURES = {
     "b200rl_per_tree_build": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p]),
     "b200rl_per_tree_set_range": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p]),
     "b200rl_offpolicy_set_alpha_group": (C.c_int, [C.c_void_p] * 5),
+    "b200rl_offpolicy_create_cql": (C.c_int, [C.POINTER(OffPolicyConfig), C.POINTER(CqlConfig), C.c_int32,
+                                              C.POINTER(C.c_void_p)]),
+    "b200rl_offpolicy_set_cql": (C.c_int, [C.c_void_p, C.POINTER(CqlHparams)]),
+    "b200rl_offpolicy_set_alpha_prime_group": (C.c_int, [C.c_void_p] * 5),
+    "b200rl_offpolicy_get_alpha_prime_group": (C.c_int, [C.c_void_p] * 5),
+    "b200rl_offpolicy_cql_outputs": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "b200rl_offpolicy_set_cql_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
+    "b200rl_offpolicy_get_cql_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "b200rl_offpolicy_get_alpha_group": (C.c_int, [C.c_void_p] * 5),
     "b200rl_discounted_cumsum": (C.c_int, [C.c_void_p, C.c_int64, C.c_double, C.c_void_p, C.c_void_p]),
     "b200rl_gae_f64": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_double, C.c_double, C.c_void_p,

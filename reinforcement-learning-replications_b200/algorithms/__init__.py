@@ -1,4 +1,5 @@
 from .c51 import C51
+from .cql import CQL
 from .d4pg import D4PG
 from .discrete_sac import DiscreteSAC
 from .dqn import DQN
@@ -12,4 +13,4 @@ from .tqc import TQC
 from .trpo import TRPO
 from .vpg import VPG
 
-__all__ = ["VPG", "TRPO", "PPO", "DDPG", "D4PG", "TD3", "SAC", "TQC", "DiscreteSAC", "DQN", "C51", "QRDQN", "IQN", "LearnerGroup"]
+__all__ = ["VPG", "TRPO", "PPO", "DDPG", "D4PG", "TD3", "SAC", "TQC", "CQL", "DiscreteSAC", "DQN", "C51", "QRDQN", "IQN", "LearnerGroup"]

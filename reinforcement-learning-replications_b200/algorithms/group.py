@@ -1,4 +1,4 @@
-"""LearnerGroup: several independent TD3 / DDPG / D4PG / SAC / TQC / discrete SAC / DQN / C51 / QR-DQN / IQN learners (typically one per seed) trained side by side by ONE
+"""LearnerGroup: several independent TD3 / DDPG / D4PG / SAC / TQC / CQL / discrete SAC / DQN / C51 / QR-DQN / IQN learners (typically one per seed) trained side by side by ONE
 off-policy engine, every operation of a train step one launch for all of them (b200rl_offpolicy_create_group).
 
 The contract: each member ends up bit for bit where it would be had it run alone.  Members keep everything of their
@@ -77,6 +77,9 @@ def _signature(agent) -> list:
         sig.append(("log_std bounds", (agent.policy.log_std_min, agent.policy.log_std_max)))
     if agent.algo == OffPolicyEngine.TQC:
         sig.append(("(n_quantiles, top_quantiles_to_drop_per_net)", agent.tqc_config))
+    if agent.algo == OffPolicyEngine.CQL:
+        sig.append(("(cql_n_actions, lagrange)", agent.cql_config))
+        sig.append(("CQL hyper-parameters", agent.cql_hparams()))
     if agent.algo == OffPolicyEngine.D4PG:
         sig.append(("(n_atoms, v_min, v_max)", agent.d4pg_config))
         sig.append(("n_step", agent.n_step))
@@ -105,6 +108,15 @@ def _check_prioritized_buffers(members) -> None:
             seen[id(rb)] = k
 
 
+def _stack_noise(parts):
+    """The members' inputs stacked on a leading [K] axis; a tuple (CQL's noise) part by part; None stays None."""
+    if parts[0] is None:
+        return None
+    if isinstance(parts[0], tuple):
+        return tuple(np.stack(x) for x in zip(*parts))
+    return np.stack(parts)
+
+
 def _rng_state():
     return random.getstate(), np.random.get_state(), torch.get_rng_state()
 
@@ -130,7 +142,7 @@ class LearnerGroup:
     def add(self, agent) -> None:
         """Add ``agent``; the current state of the global random generators becomes its private stream."""
         if not isinstance(agent, _OffPolicyBase):
-            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or D4PG / TQC / DiscreteSAC / DQN / C51 / QR-DQN / IQN) learners, got {type(agent).__name__}")
+            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or D4PG / TQC / CQL / DiscreteSAC / DQN / C51 / QR-DQN / IQN) learners, got {type(agent).__name__}")
         if any(m is agent for m in self.members):
             raise ValueError("LearnerGroup: this agent is already a member")
         if len(self.members) >= MAX_LEARNERS:
@@ -217,6 +229,10 @@ class LearnerGroup:
         if sac:
             e.set_sac(members[0]._sac_hparams())
             e.set_alpha_group([m._alpha_state() for m in members])
+        cql = members[0].algo == OffPolicyEngine.CQL
+        if cql:
+            e.set_cql(**members[0].cql_hparams())
+            e.set_alpha_prime_group([m._alpha_prime_state() for m in members])
         if members[0].algo in OffPolicyEngine.DISCRETE:
             e.set_dqn(members[0].target_update_interval, members[0].double_q)
         if members[0].algo == OffPolicyEngine.C51:
@@ -243,10 +259,10 @@ class LearnerGroup:
                                            [st[1][0] for st in staged], [st[1][1] for st in staged])
         elif mode == "gather":
             replays = [m.replay_buffer.device_columns() for m in members]
-            noise = None if staged[0][1][1] is None else np.stack([st[1][1] for st in staged])
+            noise = _stack_noise([st[1][1] for st in staged])
             out = e.train_gather_group(hp, replays, np.stack([st[1][0] for st in staged]), noise)
         else:
-            cols = [None if staged[0][1][i] is None else np.stack([st[1][i] for st in staged]) for i in range(6)]
+            cols = [_stack_noise([st[1][i] for st in staged]) for i in range(6)]
             out = e.train(hp, *cols)
         _, steps = e.get_state()
         for (slots, trainable), m, st in zip(plans, members, steps):
@@ -254,6 +270,9 @@ class LearnerGroup:
         if sac:
             for m, a in zip(members, e.get_alpha_group()):
                 m._store_alpha_state(*a)
+        if cql:
+            for m, a in zip(members, e.get_alpha_prime_group()):
+                m._store_alpha_prime_state(*a)
         for k, m in enumerate(members):
             m.last_train_output = {key: v[k] for key, v in out.items()}
             m._record_train(m.last_train_output)

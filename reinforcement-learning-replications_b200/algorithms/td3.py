@@ -319,6 +319,23 @@ class _OffPolicyBase:
         noisy, delay = self._train_schedule()
         self._record_train(self._run(replay_buffer, num_train_steps, minibatch_size, noisy=noisy, delay=delay))
 
+    def learn_offline(self, num_epochs: int, num_train_steps: int = 1000, minibatch_size: int = 256,
+                      num_evaluation_episodes: int = 10, evaluation_interval: int = 1, model_saving_interval: int = 1,
+                      output_dir: str = ".") -> None:
+        """Train on the fixed contents of ``self.replay_buffer`` (e.g. ``ReplayBuffer.from_dataset``) with no sampler:
+        each epoch runs ``num_train_steps`` train steps, logs ``epoch`` and ``total_train_steps``, then evaluates every
+        ``evaluation_interval`` and saves ``model.pt`` every ``model_saving_interval`` epochs as ``learn`` does."""
+        started = _learn_begin(self, output_dir)
+        mm = self.metrics_manager
+        for epoch in range(1, num_epochs + 1):
+            self.current_total_steps += int(num_train_steps)  # the train steps so far: the x-axis of the logs
+            self.train(self.replay_buffer, num_train_steps, minibatch_size)
+            mm.record_scalar("epoch", epoch)
+            mm.record_scalar("total_train_steps", self.current_total_steps)
+            _learn_evaluate_save(self, epoch, started, num_evaluation_episodes, evaluation_interval,
+                                 model_saving_interval, output_dir, progress=epoch)
+        mm.close()
+
 
 class TD3(_OffPolicyBase):
     """Same constructor arguments / defaults as ref algorithms/td3.py:46-62."""
@@ -439,6 +456,9 @@ def _learn(self, num_epochs, batch_size, minibatch_size, num_start_steps, num_st
            num_evaluation_episodes, evaluation_interval, model_saving_interval, output_dir) -> None:
     """Shared host loop of TD3.learn / DDPG.learn / SAC.learn / DQN.learn (ref: td3.py:94-212, ddpg.py:85-193).  One epoch is three
     phases (sample, train, evaluate and save), which LearnerGroup.learn runs in lockstep for its learners."""
+    if self.sampler is None or self.exploration_policy is None:
+        raise ValueError(f"{type(self).__name__}.learn needs a sampler and an exploration policy; without them "
+                         "(offline data) use learn_offline")
     started = _learn_begin(self, output_dir)
     for epoch in range(1, num_epochs + 1):
         if _learn_sample(self, epoch, batch_size, num_start_steps, num_steps_before_update):
@@ -481,9 +501,11 @@ def _learn_sample(self, epoch, batch_size, num_start_steps, num_steps_before_upd
 
 
 def _learn_evaluate_save(self, epoch, started, num_evaluation_episodes, evaluation_interval, model_saving_interval,
-                         output_dir) -> None:
+                         output_dir, progress=None) -> None:
+    """Evaluate and save when ``progress`` (the environment steps so far unless given) is a multiple of the interval."""
     mm = self.metrics_manager
-    if num_evaluation_episodes > 0 and self.current_total_steps % evaluation_interval == 0:
+    progress = self.current_total_steps if progress is None else progress
+    if num_evaluation_episodes > 0 and progress % evaluation_interval == 0:
         ev_policy = getattr(self, "evaluation_policy", self.policy)  # SAC: the deterministic view of its policy
         ev_returns, ev_lengths = self.evaluator.evaluate(ev_policy, self.evaluation_env, num_evaluation_episodes)
         mm.record_scalar("evaluation/average_episode_return", float(np.mean(ev_returns)), self.current_total_steps,
@@ -493,7 +515,7 @@ def _learn_evaluate_save(self, epoch, started, num_evaluation_episodes, evaluati
         mm.record_scalar("evaluation/min_episode_return", float(np.min(ev_returns)))
         mm.record_scalar("evaluation/average_episode_length", float(np.mean(ev_lengths)), self.current_total_steps,
                          tensorboard=True)
-    if self.current_total_steps % model_saving_interval == 0:
+    if progress % model_saving_interval == 0:
         self.save_model(epoch, os.path.join(output_dir, "model.pt"))
     mm.record_scalar("time", time.time() - started)
     mm.dump()

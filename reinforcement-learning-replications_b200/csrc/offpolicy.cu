@@ -468,8 +468,25 @@ __device__ __forceinline__ void block_mean(double acc, int n, float* loss_out, d
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float softplus_f(float x) { return x > 20.f ? x : log1pf(expf(x)); }  // F.softplus
 
-// One thread per row: u = mu + exp(clamp(log_std)) * eps, act = limit * tanh(u),
-// logp = sum_j Normal(mu, sigma).log_prob(u)_j - sum_j 2 (log 2 - u_j - softplus(-2 u_j))
+// One row of the squashed-Gaussian head (out = [mu | log_std] [2A], eps [A]): u = mu + exp(clamp(log_std)) * eps,
+// act = limit * tanh(u); returns logp = sum_j Normal(mu, sigma).log_prob(u)_j - sum_j 2 (log 2 - u_j - softplus(-2 u_j))
+__device__ __forceinline__ float sac_squash(const float* out, const float* eps, int A, float lmin, float lmax,
+                                            float limit, float* act) {
+  float lp = 0.f, corr = 0.f;
+  for (int j = 0; j < A; ++j) {
+    const float mu = out[j];
+    const float ls = fminf(fmaxf(out[A + j], lmin), lmax);
+    const float sigma = expf(ls);
+    const float u = __fadd_rn(mu, __fmul_rn(sigma, eps[j]));  // rsample: loc + eps * scale
+    const float d = u - mu;
+    lp += -(d * d) / (2.f * (sigma * sigma)) - ls - 0.918938533204672742f;  // - log sqrt(2 pi)
+    corr += 2.f * (0.693147180559945309f - u - softplus_f(-2.f * u));
+    act[j] = limit * tanhf(u);
+  }
+  return lp - corr;
+}
+
+// One thread per row: sac_squash of row r
 template <bool LANES>
 __global__ void sac_squash_kernel(const float* out, const float* eps, int B, int A, float lmin, float lmax, float limit,
                                   float* act, float* logp, size_t lane_stride) {
@@ -479,18 +496,7 @@ __global__ void sac_squash_kernel(const float* out, const float* eps, int B, int
   }
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= B) return;
-  float lp = 0.f, corr = 0.f;
-  for (int j = 0; j < A; ++j) {
-    const float mu = out[(size_t)r * 2 * A + j];
-    const float ls = fminf(fmaxf(out[(size_t)r * 2 * A + A + j], lmin), lmax);
-    const float sigma = expf(ls);
-    const float u = __fadd_rn(mu, __fmul_rn(sigma, eps[(size_t)r * A + j]));  // rsample: loc + eps * scale
-    const float d = u - mu;
-    lp += -(d * d) / (2.f * (sigma * sigma)) - ls - 0.918938533204672742f;  // - log sqrt(2 pi)
-    corr += 2.f * (0.693147180559945309f - u - softplus_f(-2.f * u));
-    act[(size_t)r * A + j] = limit * tanhf(u);
-  }
-  logp[r] = lp - corr;
+  logp[r] = sac_squash(out + (size_t)r * 2 * A, eps + (size_t)r * A, A, lmin, lmax, limit, act + (size_t)r * A);
 }
 
 // One CTA per critic: y = r + gamma (1 - d) (min(Q1targ, Q2targ)(s', a') - alpha log pi(a' | s')), loss = mean((q - y)^2),
@@ -759,6 +765,169 @@ __global__ void __launch_bounds__(GTHREADS) tqc_policy_loss_kernel(const float* 
   }
   block_mean(acc, B, loss_out, red);
   block_mean(acc_lp, B, logp_mean_out, red_lp);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// CQL (algo = 8; Kumar, Zhou, Tucker & Levine 2020, CQL(H)): SAC's step program whose critics also run on 3N sampled
+// actions per minibatch row.  The critics' forward and backward passes run on (1 + 3N) B stacked rows: rows 0..B-1 are
+// the data rows [s_i | a_i], row B + i 3N + j sample j of row i.  cql_stage_kernel builds that operand, SAC's soft MSE
+// head serves the data rows, cql_penalty_kernel adds the log-sum-exp penalty, cql_alpha_prime_kernel is the optional
+// Lagrange step.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int CQL_MAX_ACTIONS = 64;  // N; a row's penalty runs over 3N values
+constexpr int CQL_WARPS = 8;         // rows per penalty CTA
+constexpr float CQL_MAX_ALPHA_PRIME = 1e6f;
+
+// Philox tag of CQL's device draws: distinct from the index (0x1D5), noise (0xE95), IQN (0x9E5) and noisy (0xA00 | r)
+// blocks, so SAC's draws for the same (seed, call) are unchanged
+constexpr unsigned CQL_DRAW_TAG = 0xC91u;
+
+// draws [S][3][B][N][A] per learner: block 0 uniform x in [0, 1) (24-bit), blocks 1 and 2 N(0, 1) by Box-Muller.  One
+// thread = one Philox block = 4 consecutive values; each value takes the form of the block it falls in.
+template <bool LANES>
+__global__ void cql_draw_kernel(float* draws, long long n, long long block, const DrawKeys<LANES> keys,
+                                size_t lane_stride) {
+  const int zl = LANES ? blockIdx.z : 0;
+  if (LANES) draws = lane_ptr(draws, blockIdx.z * lane_stride);
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (4 * t >= n) return;
+  const unsigned long long seed = keys.seed[zl], call = keys.call[zl];
+  const uint4 r = philox4x32_10(make_uint4((unsigned)t, (unsigned)(t >> 32), (unsigned)call, CQL_DRAW_TAG),
+                                make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
+  float z[4];
+  box_muller4(r, z);
+  const unsigned v[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const long long e = 4 * t + j;
+    if (e < n) draws[e] = (e / block) % 3 == 0 ? (float)(v[j] >> 8) * 5.9604644775390625e-8f : z[j];
+  }
+}
+
+// One thread per stacked row r of the critics' operand x [(1 + 3N) B, O + A]: r < B copies [s_r | a_r]; r = B + i 3N + j
+// writes [s_i | action] and logp[i 3N + j], with the action u = limit (2 x - 1) and logp = lu for j < N, a squashed
+// sample of pi(.|s'_i) for N <= j < 2N and of pi(.|s_i) for 2N <= j < 3N (out_next / out_cur: the policy outputs at
+// s' / s; draws [3][B][N][A] the step's x, eps at s and eps at s', in that order).  The squash is sac_squash's.
+template <bool LANES>
+__global__ void cql_stage_kernel(const float* obs, const float* act, const float* out_next, const float* out_cur,
+                                 const float* draws, int B, int N, int O, int A, float lmin, float lmax, float limit,
+                                 float lu, float* x, float* logp, size_t lane_stride) {
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    obs = lane_ptr(obs, o), act = lane_ptr(act, o), out_next = lane_ptr(out_next, o), out_cur = lane_ptr(out_cur, o);
+    draws = lane_ptr(draws, o), x = lane_ptr(x, o), logp = lane_ptr(logp, o);
+  }
+  const int n3 = 3 * N;
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= (long long)B * (1 + n3)) return;
+  float* xr = x + r * (O + A);
+  if (r < B) {
+    for (int c = 0; c < O; ++c) xr[c] = obs[r * O + c];
+    for (int c = 0; c < A; ++c) xr[O + c] = act[r * A + c];
+    return;
+  }
+  const int k = (int)(r - B), i = k / n3, j = k - i * n3, blk = j / N, jj = j - blk * N;
+  for (int c = 0; c < O; ++c) xr[c] = obs[(size_t)i * O + c];
+  const float* d = draws + (((size_t)(blk == 0 ? 0 : 3 - blk) * B + i) * N + jj) * A;  // draws: x, eps at s, eps at s'
+  if (blk == 0) {
+    for (int c = 0; c < A; ++c) xr[O + c] = limit * (2.f * d[c] - 1.f);
+    logp[k] = lu;
+  } else {
+    logp[k] = sac_squash(blk == 1 ? out_next + (size_t)i * 2 * A : out_cur + (size_t)i * 2 * A, d, A, lmin, lmax,
+                         limit, xr + O);
+  }
+}
+
+// One warp per row i over its 3N sampled values q[B + i 3N + j] (CQL_WARPS rows per CTA): z_j = (q_j - logp_j) / T,
+// P_i = T (m + log sum_j exp(z_j - m)) with m = max_j z_j and the sum in index order; with w = weight (times
+// alpha'[0], clamped, when alpha_prime != NULL)
+//   dq[B + i 3N + j] = w softmax_j(z) / B,  dq[i] -= w / B  (behind SAC's soft MSE head, which wrote 2 (q - y) / B).
+// The last CTA of a learner (sync counts them) writes gap = mean_i P_i - mean_i q_i (each sum in double, fixed order),
+// adds w gap (- alpha' tau) to *loss_out and leaves the counter at 0.  No atomics touch a float.
+template <bool LANES>
+__global__ void __launch_bounds__(CQL_WARPS * 32) cql_penalty_kernel(
+    const float* q, const float* logp, int B, int N, float temperature, float weight, const float* alpha_prime,
+    float tau, float* dq, float* row_p, int* sync, float* loss_out, float* gap_out, size_t lane_stride) {
+  __shared__ float sz[CQL_WARPS][3 * CQL_MAX_ACTIONS];
+  __shared__ double red[32], red_q[32];
+  __shared__ bool last;
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q = lane_ptr(q, o), logp = lane_ptr(logp, o), alpha_prime = lane_ptr(alpha_prime, o), dq = lane_ptr(dq, o);
+    row_p = lane_ptr(row_p, o), sync = lane_ptr(sync, o), loss_out = lane_ptr(loss_out, o);
+    gap_out = lane_ptr(gap_out, o);
+  }
+  const int n3 = 3 * N, w_ = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int i = blockIdx.x * CQL_WARPS + w_;
+  const float ap = alpha_prime != nullptr ? fminf(*alpha_prime, CQL_MAX_ALPHA_PRIME) : 1.f;
+  const float w = alpha_prime != nullptr ? ap * weight : weight;
+  const float invB = 1.0f / (float)B;
+  if (i < B) {
+    const float* qi = q + B + (size_t)i * n3;
+    const float* li = logp + (size_t)i * n3;
+    for (int j = lane; j < n3; j += 32) sz[w_][j] = (qi[j] - li[j]) / temperature;
+    __syncwarp();
+    float m = sz[w_][0], s = 0.f;
+    for (int j = 1; j < n3; ++j) m = fmaxf(m, sz[w_][j]);
+    for (int j = 0; j < n3; ++j) s += expf(sz[w_][j] - m);
+    float* di = dq + B + (size_t)i * n3;
+    for (int j = lane; j < n3; j += 32) di[j] = w * (expf(sz[w_][j] - m) / s) * invB;
+    if (lane == 0) {
+      row_p[i] = temperature * (m + logf(s));
+      dq[i] = dq[i] - w * invB;
+    }
+  }
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(sync, 1) == (int)gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double acc = 0.0, acc_q = 0.0;
+  for (int r = threadIdx.x; r < B; r += blockDim.x) acc += (double)__ldcg(row_p + r), acc_q += (double)q[r];
+  acc = warp_sum(acc), acc_q = warp_sum(acc_q);
+  if (lane == 0) red[w_] = acc, red_q[w_] = acc_q;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double tp = 0.0, tq = 0.0;
+    for (int k = 0; k < CQL_WARPS; ++k) tp += red[k], tq += red_q[k];
+    const float gap = (float)(tp / (double)B) - (float)(tq / (double)B);
+    *gap_out = gap;
+    float l = *loss_out + w * gap;
+    if (alpha_prime != nullptr) l -= ap * tau;
+    *loss_out = l;
+    sync[0] = 0;
+  }
+}
+
+// One thread: the Lagrange step on log alpha' (state = {log alpha', exp_avg, exp_avg_sq}).  Its loss
+// -1/2 sum_k alpha' (weight gap_k - tau), alpha' = clamp(exp(log alpha'), 0, 1e6), has the gradient
+// g = -1/2 ((weight gap_1 - tau) + (weight gap_2 - tau)) exp(log alpha') (0 where the clamp is active); one
+// torch.optim.Adam step with the scalars of table[idx] (sac_alpha_step_kernel's arithmetic); alpha_next = the clamped
+// alpha' of the next step.
+template <bool LANES>
+__global__ void cql_alpha_prime_kernel(const float* gap1, const float* gap2, float weight, float tau, float* state,
+                                       const float2* table, int idx, float one_minus_b1, float b2, float one_minus_b2,
+                                       float eps, float* alpha_next, size_t lane_stride) {
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    gap1 = lane_ptr(gap1, o), gap2 = lane_ptr(gap2, o), state = lane_ptr(state, o), table = lane_ptr(table, o);
+    alpha_next = lane_ptr(alpha_next, o);
+  }
+  // every operation rounded explicitly, so that both instantiations compute the same bits
+  float p = state[0], m = state[1], v = state[2];
+  const float e = expf(p);
+  const float s = __fadd_rn(__fsub_rn(__fmul_rn(weight, *gap1), tau), __fsub_rn(__fmul_rn(weight, *gap2), tau));
+  const float g = e <= CQL_MAX_ALPHA_PRIME ? __fmul_rn(__fmul_rn(-0.5f, s), e) : 0.f;
+  const float2 t = table[idx];
+  m = __fadd_rn(m, __fmul_rn(one_minus_b1, __fsub_rn(g, m)));
+  v = __fmaf_rn(__fmul_rn(g, g), one_minus_b2, __fmul_rn(v, b2));
+  const float denom = __fadd_rn(__fdiv_rn(sqrtf(v), t.y), eps);
+  p = __fsub_rn(p, __fmul_rn(t.x, __fdiv_rn(m, denom)));
+  state[0] = p;
+  state[1] = m;
+  state[2] = v;
+  *alpha_next = fminf(expf(p), CQL_MAX_ALPHA_PRIME);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -2011,6 +2180,7 @@ struct GraphKey {
   b200rl_qr_hparams qr;
   b200rl_per_hparams per;
   ReplayLanes<true> replay;
+  b200rl_cql_hparams cql;
 };
 
 struct b200rl_offpolicy {
@@ -2122,6 +2292,23 @@ struct b200rl_offpolicy {
   float* tqc_y = nullptr;         // [B, kN] the step's truncated target atoms, ascending
   float* tqc_row_loss = nullptr;  // [2][B] each critic's row losses
   int* tqc_sync = nullptr;        // [2] each critic head's CTAs done; 0 between launches
+  // CQL (cfg.algo == 8): a SAC engine (h->sac is set) whose critics run on R = (1 + 3N) B stacked rows in the critic
+  // step; dq, dq2 and dbuf0..3 are R rows deep.  adam_tab row 4 holds the Lagrange step's Adam scalars.
+  bool cql = false, cql_set = false;
+  b200rl_cql_config cql_cfg{};
+  b200rl_cql_hparams cql_hp{};
+  int cql_staged_S = -1, cql_staged_B = -1;      // the (S, B) of host draws staged for the next train call
+  float* cql_draws = nullptr;                    // [max_steps][3][B][N][A] the call's draws (uniform x, eps at s', at s)
+  float* cql_x = nullptr;                        // [R, O + A] the stacked critic operand
+  float* cql_logp = nullptr;                     // [B, 3N] each sample's log density
+  float* cql_acts[2][B200RL_MAX_LAYERS + 1];     // the critics' activation stacks [R, width]
+  float* cql_row_p = nullptr;                    // [2][B] each critic's P_i
+  int* cql_sync = nullptr;                       // [2] each penalty head's CTAs done; 0 between launches
+  float* cql_gap = nullptr;                      // [2][max_steps] gap_k of each step
+  float* cql_ap = nullptr;                       // [max_steps + 1] alpha' of step st at [st]
+  float* cql_ap_state = nullptr;                 // {log alpha', exp_avg, exp_avg_sq}
+  float* cql_zero = nullptr;                     // one 0.f: the temperature of a backup without the entropy term
+  int64_t ap_step[B200RL_MAX_LEARNERS] = {};
   // the replay columns, episode-end columns, trees and row counts of this call (train_gather[_rng], train_prioritized)
   ReplayLanes<true> replay{};
   std::vector<void*> allocs;
@@ -2136,7 +2323,8 @@ inline int64_t state_pad(int64_t n) { return (n + 63) & ~(int64_t)63; }
 // call) after it
 inline size_t adam_tab_len(const b200rl_offpolicy* h) {
   const bool per = h->dqn || h->d4pg;  // engines that take prioritized replay: row 3's .y holds the betas
-  return (h->sac || h->dsac || per ? 4 : 3) * (size_t)h->cfg.max_steps + (per ? 2 : 0) + (h->noisy || h->iqn ? 2 : 0);
+  return (h->cql ? 5 : h->sac || h->dsac || per ? 4 : 3) * (size_t)h->cfg.max_steps + (per ? 2 : 0) +
+         (h->noisy || h->iqn ? 2 : 0);
 }
 
 // A piece of the learner arena: recorded here (256-byte aligned), placed by arena_commit
@@ -2448,22 +2636,40 @@ int adam_net(const b200rl_offpolicy* h, NetBuf& nb, const float2* table, int idx
 // (dc = the support, config algo 6) and of create_tqc (tc = the quantile counts, config algo 7)
 static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_config* ic,
                          const b200rl_d4pg_config* dc, int32_t n_learners, b200rl_offpolicy** out,
-                         const b200rl_tqc_config* tc = nullptr) {
+                         const b200rl_tqc_config* tc = nullptr, const b200rl_cql_config* cc = nullptr) {
   B200RL_REQUIRE(cfg && out, "offpolicy_create: NULL argument");
   B200RL_REQUIRE(n_learners >= 1 && n_learners <= B200RL_MAX_LEARNERS,
                  "offpolicy_create_group: n_learners must be 1..%d, got %d", B200RL_MAX_LEARNERS, n_learners);
   B200RL_REQUIRE(cfg->n_q == 1 || cfg->n_q == 2, "offpolicy_create: n_q must be 1 (DDPG) or 2 (TD3)");
   B200RL_REQUIRE((cfg->algo >= 0 && cfg->algo <= 3) || cfg->algo == 5 || (cfg->algo == 4 && ic != nullptr) ||
-                     (cfg->algo == 6 && dc != nullptr) || (cfg->algo == 7 && tc != nullptr),
+                     (cfg->algo == 6 && dc != nullptr) || (cfg->algo == 7 && tc != nullptr) ||
+                     (cfg->algo == 8 && cc != nullptr),
                  "offpolicy_create: algo must be 0 (DDPG / TD3), 1 (SAC), 2 (DQN), 3 (C51) or 5 (discrete SAC), got %d "
                  "(algo 4, IQN, is created by b200rl_offpolicy_create_iqn with its counts, algo 6, D4PG, by "
-                 "b200rl_offpolicy_create_d4pg with its support)", cfg->algo);
+                 "b200rl_offpolicy_create_d4pg with its support, algo 7, TQC, by b200rl_offpolicy_create_tqc, algo 8, "
+                 "CQL, by b200rl_offpolicy_create_cql)", cfg->algo);
   B200RL_REQUIRE(ic == nullptr || cfg->algo == 4, "offpolicy_create_iqn: the config's algo must be 4 (IQN), got %d",
                  cfg->algo);
   B200RL_REQUIRE(dc == nullptr || cfg->algo == 6, "offpolicy_create_d4pg: the config's algo must be 6 (D4PG), got %d",
                  cfg->algo);
   B200RL_REQUIRE(tc == nullptr || cfg->algo == 7, "offpolicy_create_tqc: the config's algo must be 7 (TQC), got %d",
                  cfg->algo);
+  B200RL_REQUIRE(cc == nullptr || cfg->algo == 8, "offpolicy_create_cql: the config's algo must be 8 (CQL), got %d",
+                 cfg->algo);
+  const bool cql = cfg->algo == 8 && cc != nullptr;  // a SAC engine whose critic step runs on stacked sampled rows
+  const int CN = cql ? cc->n_actions : 0;
+  if (cql) {
+    B200RL_REQUIRE(cfg->n_q == 2, "offpolicy_create_cql: CQL needs n_q = 2 (twin soft critics), got %d", cfg->n_q);
+    B200RL_REQUIRE(cfg->dueling_k == 0 && cfg->noisy_layers == 0, "offpolicy_create_cql: CQL takes neither dueling_k "
+                   "nor noisy_layers: dueling and noisy networks are not implemented for it");
+    B200RL_REQUIRE(CN >= 1 && CN <= CQL_MAX_ACTIONS, "offpolicy_create_cql: n_actions must be 1..%d, got %d",
+                   CQL_MAX_ACTIONS, CN);
+    B200RL_REQUIRE(cc->lagrange == 0 || cc->lagrange == 1, "offpolicy_create_cql: lagrange must be 0 or 1, got %d",
+                   cc->lagrange);
+    B200RL_REQUIRE((long long)cfg->max_minibatch * (1 + 3 * CN) <= 65535LL * GT, "offpolicy_create_cql: max_minibatch "
+                   "%d x %d stacked rows per row exceed the %lld network rows of one pass", cfg->max_minibatch,
+                   1 + 3 * CN, 65535LL * GT);
+  }
   const bool tqc = cfg->algo == 7 && tc != nullptr;  // a SAC engine with quantile critics
   const int TM = tqc ? tc->n_quantiles : 0, TD = tqc ? tc->n_drop_per_net : 0;
   if (tqc) {
@@ -2475,7 +2681,7 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
     B200RL_REQUIRE(TD >= 0 && TD <= TM - 1, "offpolicy_create_tqc: n_drop_per_net must be 0..n_quantiles - 1 = %d, "
                    "got %d", TM - 1, TD);
   }
-  const bool sac = cfg->algo == 1 || tqc, c51 = cfg->algo == 3, iqn = cfg->algo == 4, dsac = cfg->algo == 5;
+  const bool sac = cfg->algo == 1 || tqc || cql, c51 = cfg->algo == 3, iqn = cfg->algo == 4, dsac = cfg->algo == 5;
   const bool d4pg = cfg->algo == 6 && dc != nullptr;
   const int NA = d4pg ? dc->n_atoms : 0;
   if (d4pg) {
@@ -2584,6 +2790,8 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   if (d4pg) h->d4pg_cfg = *dc, h->d4pg_cfg.reserved = 0;
   h->tqc = tqc;
   if (tqc) h->tqc_cfg = *tc;
+  h->cql = cql;
+  if (cql) h->cql_cfg = *cc;
   h->noisy = NM != 0;
   int rc = 0;
   int maxw = O + A;
@@ -2666,6 +2874,8 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   }
   h->maxw = maxw;
   const size_t B = (size_t)cfg->max_minibatch, S = (size_t)cfg->max_steps;
+  const size_t R = B * (size_t)(1 + 3 * CN);  // CQL's stacked critic rows; the gradient buffers are that deep
+  const size_t RD = cql ? R : B;
   rc |= oalloc(h, &h->obs, S * B * O);
   rc |= oalloc(h, &h->act, S * B * A);
   rc |= oalloc(h, &h->rew, S * B);
@@ -2681,12 +2891,12 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   const size_t n_dq = dsac || d4pg || tqc ? (size_t)cfg->q.sizes[cfg->q.n_layers] : 1;
   rc |= oalloc(h, &h->qt1, B * n_dq);
   rc |= oalloc(h, &h->qt2, B * (tqc ? n_dq : 1));
-  rc |= oalloc(h, &h->dq, B * n_dq);
-  rc |= oalloc(h, &h->dbuf0, B * (size_t)maxw);
-  rc |= oalloc(h, &h->dbuf1, B * (size_t)maxw);
-  rc |= oalloc(h, &h->dbuf2, B * (size_t)maxw);
-  rc |= oalloc(h, &h->dbuf3, B * (size_t)maxw);
-  rc |= oalloc(h, &h->dq2, B * n_dq);
+  rc |= oalloc(h, &h->dq, RD * n_dq);
+  rc |= oalloc(h, &h->dbuf0, RD * (size_t)maxw);
+  rc |= oalloc(h, &h->dbuf1, RD * (size_t)maxw);
+  rc |= oalloc(h, &h->dbuf2, RD * (size_t)maxw);
+  rc |= oalloc(h, &h->dbuf3, RD * (size_t)maxw);
+  rc |= oalloc(h, &h->dq2, RD * n_dq);
   rc |= oalloc(h, &h->out_q1, S * B);
   rc |= oalloc(h, &h->out_q2, S * B);
   rc |= oalloc(h, &h->out_l1, S);
@@ -2709,6 +2919,19 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
     rc |= oalloc(h, &h->tqc_y, B * (size_t)(2 * (TM - TD)));
     rc |= oalloc(h, &h->tqc_row_loss, 2 * B);
     rc |= oalloc(h, &h->tqc_sync, 2);
+  }
+  if (cql) {
+    rc |= oalloc(h, &h->cql_draws, S * 3 * B * CN * A);
+    rc |= oalloc(h, &h->cql_x, R * (O + A));
+    rc |= oalloc(h, &h->cql_logp, B * 3 * CN);
+    for (int k = 0; k < 2; ++k)
+      for (int l = 1; l <= cfg->q.n_layers; ++l) rc |= oalloc(h, &h->cql_acts[k][l], R * (size_t)maxw);
+    rc |= oalloc(h, &h->cql_row_p, 2 * B);
+    rc |= oalloc(h, &h->cql_sync, 2);
+    rc |= oalloc(h, &h->cql_gap, 2 * S);
+    rc |= oalloc(h, &h->cql_ap, S + 1);
+    rc |= oalloc(h, &h->cql_ap_state, 3);
+    rc |= oalloc(h, &h->cql_zero, 1);
   }
   if (dsac) {
     rc |= oalloc(h, &h->sac_logp, B);
@@ -2833,6 +3056,12 @@ extern "C" int b200rl_offpolicy_create_tqc(const b200rl_offpolicy_config* cfg, c
                                            int32_t n_learners, b200rl_offpolicy** out) {
   B200RL_REQUIRE(tqc, "offpolicy_create_tqc: NULL TQC counts");
   return create_engine(cfg, nullptr, nullptr, n_learners, out, tqc);
+}
+
+extern "C" int b200rl_offpolicy_create_cql(const b200rl_offpolicy_config* cfg, const b200rl_cql_config* cql,
+                                           int32_t n_learners, b200rl_offpolicy** out) {
+  B200RL_REQUIRE(cql, "offpolicy_create_cql: NULL CQL config");
+  return create_engine(cfg, nullptr, nullptr, n_learners, out, nullptr, cql);
 }
 
 extern "C" void b200rl_offpolicy_destroy(b200rl_offpolicy* h) {
@@ -3142,6 +3371,104 @@ extern "C" int b200rl_offpolicy_sac_outputs(b200rl_offpolicy* h, int32_t S, floa
   return 0;
 }
 
+extern "C" int b200rl_offpolicy_set_cql(b200rl_offpolicy* h, const b200rl_cql_hparams* cp) {
+  B200RL_REQUIRE(h && cp, "offpolicy_set_cql: NULL argument");
+  B200RL_REQUIRE(h->cql, "offpolicy_set_cql: the engine was not created with algo = 8 (CQL)");
+  B200RL_REQUIRE(std::isfinite(cp->weight) && cp->weight >= 0.0, "offpolicy_set_cql: weight must be finite and >= 0, "
+                 "got %g", cp->weight);
+  B200RL_REQUIRE(std::isfinite(cp->temperature) && cp->temperature > 0.0, "offpolicy_set_cql: temperature must be "
+                 "finite and > 0, got %g", cp->temperature);
+  B200RL_REQUIRE(std::isfinite(cp->target_action_gap) && std::isfinite(cp->alpha_lr) && std::isfinite(cp->alpha_beta1) &&
+                 std::isfinite(cp->alpha_beta2) && std::isfinite(cp->alpha_eps), "offpolicy_set_cql: non-finite "
+                 "Lagrange settings");
+  B200RL_REQUIRE(cp->backup_entropy == 0 || cp->backup_entropy == 1, "offpolicy_set_cql: backup_entropy must be 0 or 1");
+  h->cql_hp = *cp;
+  h->cql_hp.reserved = 0;  // part of the graph cache key
+  h->cql_set = true;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_set_alpha_prime_group(b200rl_offpolicy* h, const float* log_alpha_prime,
+                                                      const float* exp_avg, const float* exp_avg_sq,
+                                                      const int64_t* step) {
+  B200RL_REQUIRE(h && h->cql, "offpolicy_set_alpha_prime: not a CQL engine (algo = 8)");
+  B200RL_REQUIRE(log_alpha_prime && exp_avg && exp_avg_sq && step, "offpolicy_set_alpha_prime: NULL argument");
+  float v[B200RL_MAX_LEARNERS][3];
+  for (int z = 0; z < h->K; ++z) {
+    B200RL_REQUIRE(step[z] >= 0, "offpolicy_set_alpha_prime: negative step count");
+    v[z][0] = log_alpha_prime[z], v[z][1] = exp_avg[z], v[z][2] = exp_avg_sq[z];
+  }
+  B200RL_CUDA(cudaMemcpy2DAsync(h->cql_ap_state, h->lane_stride, v, sizeof(v[0]), sizeof(v[0]), h->K,
+                                cudaMemcpyHostToDevice, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  for (int z = 0; z < h->K; ++z) h->ap_step[z] = step[z];
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_get_alpha_prime_group(b200rl_offpolicy* h, float* log_alpha_prime, float* exp_avg,
+                                                      float* exp_avg_sq, int64_t* step) {
+  B200RL_REQUIRE(h && h->cql && log_alpha_prime && exp_avg && exp_avg_sq && step,
+                 "offpolicy_get_alpha_prime: bad arguments");
+  float v[B200RL_MAX_LEARNERS][3];
+  B200RL_CUDA(cudaMemcpy2DAsync(v, sizeof(v[0]), h->cql_ap_state, h->lane_stride, sizeof(v[0]), h->K,
+                                cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  for (int z = 0; z < h->K; ++z) {
+    log_alpha_prime[z] = v[z][0], exp_avg[z] = v[z][1], exp_avg_sq[z] = v[z][2];
+    step[z] = h->ap_step[z];
+  }
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_cql_outputs(b200rl_offpolicy* h, int32_t S, float* gaps, float* alpha_primes) {
+  B200RL_REQUIRE(h && h->cql && gaps && alpha_primes && S >= 0 && S <= h->cfg.max_steps,
+                 "offpolicy_cql_outputs: bad arguments");
+  const size_t w = (size_t)S * 4, maxS = (size_t)h->cfg.max_steps;
+  for (int k = 0; k < 2 && S > 0; ++k)
+    B200RL_CUDA(cudaMemcpy2DAsync(gaps + (size_t)k * S, 2 * w, h->cql_gap + k * maxS, h->lane_stride, w, h->K,
+                                  cudaMemcpyDeviceToHost, h->gs));
+  if (S > 0)
+    B200RL_CUDA(cudaMemcpy2DAsync(alpha_primes, w, h->cql_ap, h->lane_stride, w, h->K, cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  if (!h->cql_cfg.lagrange)
+    for (size_t i = 0; i < (size_t)h->K * S; ++i) alpha_primes[i] = 1.f;
+  return 0;
+}
+
+static size_t cql_draw_floats(const b200rl_offpolicy* h, int S, int B) {
+  return (size_t)S * 3 * B * h->cql_cfg.n_actions * h->A;
+}
+
+// A CQL call with host draws consumes the ones b200rl_offpolicy_set_cql_draws staged for its (S, B)
+static int cql_take_draws(b200rl_offpolicy* h, int S, int B, const char* what) {
+  if (!h->cql) return 0;
+  B200RL_REQUIRE(h->cql_staged_S == S && h->cql_staged_B == B, "%s: a CQL engine needs its draws [S=%d, 3, B=%d, N, A] "
+                 "from b200rl_offpolicy_set_cql_draws before a call with host draws", what, S, B);
+  h->cql_staged_S = h->cql_staged_B = -1;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_set_cql_draws(b200rl_offpolicy* h, int32_t S, int32_t B, const float* draws) {
+  B200RL_REQUIRE(h && draws && h->cql, "offpolicy_set_cql_draws: bad arguments (a CQL engine, algo = 8, takes them)");
+  B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
+                 "offpolicy_set_cql_draws: S=%d B=%d exceed the capacities", S, B);
+  const size_t w = cql_draw_floats(h, S, B) * 4;
+  if (w) B200RL_CUDA(cudaMemcpy2DAsync(h->cql_draws, h->lane_stride, draws, w, w, h->K, cudaMemcpyHostToDevice, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  h->cql_staged_S = S, h->cql_staged_B = B;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_get_cql_draws(b200rl_offpolicy* h, int32_t S, int32_t B, float* draws) {
+  B200RL_REQUIRE(h && draws && h->cql, "offpolicy_get_cql_draws: bad arguments (a CQL engine, algo = 8, has them)");
+  B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps && B >= 1 && B <= h->cfg.max_minibatch,
+                 "offpolicy_get_cql_draws: S=%d B=%d exceed the capacities", S, B);
+  const size_t w = cql_draw_floats(h, S, B) * 4;
+  if (w) B200RL_CUDA(cudaMemcpy2DAsync(draws, w, h->cql_draws, h->lane_stride, w, h->K, cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  return 0;
+}
+
 // c51_loss_kernel<LANES, WEIGHTED, NSTEP> of a call: WEIGHTED for prioritized replay (D4PG engines), NSTEP for n-step
 // returns
 template <bool LANES>
@@ -3326,8 +3653,15 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
   const bool tqc = h->tqc;
   const int NQ = tqc ? h->tqc_cfg.n_quantiles : 1;             // the critics' output width, M
   const int kN = tqc ? 2 * (NQ - h->tqc_cfg.n_drop_per_net) : 0;  // target atoms kept
+  const bool cql = h->cql, lag = cql && h->cql_cfg.lagrange;
+  const b200rl_cql_hparams& cq = h->cql_hp;
+  const int CN = cql ? h->cql_cfg.n_actions : 0, R = B * (1 + 3 * CN);  // the critic step's stacked rows
+  const int rows = cql ? R : B;
   if (launch(h, sac_alpha_init_kernel<false>, sac_alpha_init_kernel<true>, (S + 1 + ew - 1) / ew, ew, 0, s,
              h->sac_alpha, S + 1, h->sac_state, sp.learn_alpha, (float)sp.alpha))
+    return 1;
+  if (lag && launch(h, sac_alpha_init_kernel<false>, sac_alpha_init_kernel<true>, 1, ew, 0, s, h->cql_ap, S + 1,
+                    h->cql_ap_state, 1, 0.f))
     return 1;
   PolyakArgs pk{};  // 1 -> 4, 2 -> 5
   pk.n_nets = 2;
@@ -3345,15 +3679,18 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
     const float* eps_next = h->eps + (size_t)(2 * st) * B * A;  // [S, 2, B, A]: the draw for s', then the one for s
     const float* eps_cur = eps_next + (size_t)B * A;
     const float* alpha = h->sac_alpha + st;
-    // ---- the critics on [s | a] (the logged Q-values); pi(s) with the pre-update policy behind Q1's ----
+    // ---- the critics on [s | a] (the logged Q-values); pi(s) with the pre-update policy behind Q1's.  CQL: pi(s)
+    // first, the critics on the stacked rows once both policy outputs are in ----
     float* qa[2][B200RL_MAX_LAYERS + 1];
     for (int qi = 0; qi < 2; ++qi) {
-      qa[qi][0] = const_cast<float*>(s_obs);
-      for (int l = 1; l <= Lq; ++l) qa[qi][l] = h->acts[qi == 0 ? 1 : 4][l];
+      qa[qi][0] = cql ? h->cql_x : const_cast<float*>(s_obs);
+      for (int l = 1; l <= Lq; ++l) qa[qi][l] = cql ? h->cql_acts[qi][l] : h->acts[qi == 0 ? 1 : 4][l];
       cudaStream_t qs = qi == 0 ? s3 : s4;
+      if (cql) continue;
       if (edge(h, s, qs)) return 1;
       if (net_forward(h, qi == 0 ? q1 : q2, qa[qi], B, qs, s_act, A, O)) return 1;
     }
+    if (cql && edge(h, s, s3)) return 1;
     float* pa[B200RL_MAX_LAYERS + 1];
     pa[0] = const_cast<float*>(s_obs);
     for (int l = 1; l <= Lp; ++l) pa[l] = h->acts[2][l];
@@ -3369,6 +3706,19 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
     if (launch(h, sac_squash_kernel<false>, sac_squash_kernel<true>, rows_grid, 128, 0, s, ta[Lp], eps_next, B, A, lmin,
                lmax, limit, h->sac_act_next, h->sac_logp_next))
       return 1;
+    if (cql) {  // the stacked operand [s | a] ++ [s_i | sampled actions], then both critics on it
+      if (edge(h, s3, s)) return 1;
+      const float lu = (float)(-(double)A * std::log(2.0 * hp->action_limit));
+      if (launch(h, cql_stage_kernel<false>, cql_stage_kernel<true>, (R + 127) / 128, 128, 0, s, s_obs, s_act, ta[Lp],
+                 pa[Lp], h->cql_draws + (size_t)st * 3 * B * CN * A, B, CN, O, A, lmin, lmax, limit, lu, h->cql_x,
+                 h->cql_logp))
+        return 1;
+      for (int qi = 0; qi < 2; ++qi) {
+        cudaStream_t qs = qi == 0 ? s3 : s4;
+        if (edge(h, s, qs)) return 1;
+        if (net_forward(h, qi == 0 ? q1 : q2, qa[qi], R, qs)) return 1;
+      }
+    }
     float* tq[2][B200RL_MAX_LAYERS + 1];
     for (int qi = 0; qi < 2; ++qi) {
       tq[qi][0] = const_cast<float*>(s_nobs);
@@ -3398,14 +3748,28 @@ static int enqueue_sac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
                    h->tqc_sync + qi, (qi == 0 ? h->out_l1 : h->out_l2) + st))
           return 1;
       } else if (launch(h, sac_q_loss_kernel<false>, sac_q_loss_kernel<true>, 1, GTHREADS, 0, qs, qa[qi][Lq], s_rew,
-                        s_done, h->qt1, h->qt2, h->sac_logp_next, alpha, (float)hp->gamma, B, dq,
+                        s_done, h->qt1, h->qt2, h->sac_logp_next,
+                        cql && !cq.backup_entropy ? (const float*)h->cql_zero : alpha, (float)hp->gamma, B, dq,
                         (qi == 0 ? h->out_l1 : h->out_l2) + st, (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B)) {
         return 1;
       }
-      if (net_backward(h, qn, qa[qi], dq, NQ, B, true, nullptr, qs, qi != 0, s_act, A, O, qi == 0 ? s3 : s4)) return 1;
+      if (cql && launch(h, cql_penalty_kernel<false>, cql_penalty_kernel<true>, (B + CQL_WARPS - 1) / CQL_WARPS,
+                        CQL_WARPS * 32, 0, qs, qa[qi][Lq], h->cql_logp, B, CN, (float)cq.temperature,
+                        (float)cq.weight, lag ? (const float*)(h->cql_ap + st) : nullptr,
+                        (float)cq.target_action_gap, dq, h->cql_row_p + (size_t)qi * B, h->cql_sync + qi,
+                        (qi == 0 ? h->out_l1 : h->out_l2) + st, h->cql_gap + (size_t)qi * maxS + st))
+        return 1;
+      if (net_backward(h, qn, qa[qi], dq, NQ, rows, true, nullptr, qs, qi != 0, cql ? nullptr : s_act, cql ? 0 : A,
+                       cql ? 0 : O, qi == 0 ? s3 : s4))
+        return 1;
       if (adam_net(h, qn, h->adam_tab + (size_t)(1 + qi) * maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, qs)) return 1;
     }
     if (edge(h, s2, s)) return 1;
+    if (lag && launch(h, cql_alpha_prime_kernel<false>, cql_alpha_prime_kernel<true>, 1, 1, 0, s, h->cql_gap + st,
+                      h->cql_gap + maxS + st, (float)cq.weight, (float)cq.target_action_gap, h->cql_ap_state,
+                      h->adam_tab + (size_t)4 * maxS, st, (float)(1.0 - cq.alpha_beta1), (float)cq.alpha_beta2,
+                      (float)(1.0 - cq.alpha_beta2), (float)cq.alpha_eps, h->cql_ap + st + 1))
+      return 1;
     // ---- polyak beside the policy step: the targets are next read by the next step ----
     if (edge(h, s, s4)) return 1;
     if (launch(h, polyak_kernel<false>, polyak_kernel<true>, (pk.n[0] + ew - 1) / ew, ew, 0, s4, pk,
@@ -3762,6 +4126,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   const int n_pol_expected = h->dqn ? 0 : h->sac || h->dsac ? S : (S + hp->policy_delay - 1) / hp->policy_delay;  // SAC: no delay
   const size_t tab_n = adam_tab_len(h);
   const bool learn_alpha = (h->sac || h->dsac) && h->sac_hp.learn_alpha;
+  const bool lagrange = h->cql && h->cql_cfg.lagrange;
   for (int z = 0; z < h->K; ++z) {
     float2* tab = h->h_adam_tab + z * tab_n;
     for (int k = 0; k < n_pol_expected; ++k)
@@ -3774,6 +4139,10 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
       for (int k = 0; k < S; ++k)
         adam_scalars(h->alpha_step[z] + k + 1, h->sac_hp.alpha_lr, h->sac_hp.alpha_beta1, h->sac_hp.alpha_beta2,
                      &tab[(size_t)3 * maxS + k].x, &tab[(size_t)3 * maxS + k].y);
+    if (lagrange)
+      for (int k = 0; k < S; ++k)
+        adam_scalars(h->ap_step[z] + k + 1, h->cql_hp.alpha_lr, h->cql_hp.alpha_beta1, h->cql_hp.alpha_beta2,
+                     &tab[(size_t)4 * maxS + k].x, &tab[(size_t)4 * maxS + k].y);
     if (h->dqn)  // copy after the steps that bring the Q optimizer's count to a multiple of the interval
       for (int k = 0; k < S; ++k)
         tab[(size_t)3 * maxS + k] = make_float2((h->net[1].step[z] + k + 1) % h->dqn_hp.target_update_interval == 0, 0.f);
@@ -3797,6 +4166,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
     memset(&key, 0, sizeof(key));
     key.S = S, key.B = B, key.nstep = h->nstep;
     key.hp = *hp, key.sac = h->sac_hp, key.dqn = h->dqn_hp, key.c51 = h->c51_hp, key.qr = h->qr_hp;
+    key.cql = h->cql_hp;
     if (h->per_run) key.per = h->per_hp, key.replay = h->replay;
     if (h->graph == nullptr || memcmp(&key, &h->graph_key, sizeof(key)) != 0) {
       if (h->graph) {
@@ -3834,6 +4204,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
     h->net[1].step[z] += S;
     if (td3) h->net[2].step[z] += S;
     if (learn_alpha) h->alpha_step[z] += S;
+    if (lagrange) h->ap_step[z] += S;
   }
   // one device -> host read of everything train() logs: [K, S, B] values, [K, S] losses
   const size_t ls = h->lane_stride, K = (size_t)h->K;
@@ -3888,6 +4259,7 @@ static int train_begin(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, 
     B200RL_REQUIRE(h->sac_set, "%s: a SAC engine needs b200rl_offpolicy_set_sac before it trains", what);
     B200RL_REQUIRE(noise_given, "%s: SAC needs the noise draws [S, 2, B, A]", what);
   }
+  B200RL_REQUIRE(!h->cql || h->cql_set, "%s: a CQL engine needs b200rl_offpolicy_set_cql before it trains", what);
   B200RL_REQUIRE(!h->dsac || h->sac_set, "%s: a discrete SAC engine needs b200rl_offpolicy_set_sac before it trains",
                  what);
   if (h->dqn) {
@@ -3934,6 +4306,7 @@ extern "C" int b200rl_offpolicy_train(b200rl_offpolicy* h, const b200rl_offpolic
       up(h->nobs, next_obs, SB * O * 4) || up(h->done, done, SB * 4))
     return 1;
   if (h->sac && up(h->eps, noise, 2 * SB * A * 4)) return 1;
+  if (cql_take_draws(h, S, B, "offpolicy_train")) return 1;
   if (!h->sac && !h->dqn && !h->dsac && hp->use_target_noise && up(h->eps, noise, SB * A * 4)) return 1;
 
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
@@ -4008,6 +4381,7 @@ extern "C" int b200rl_offpolicy_train_gather_group(b200rl_offpolicy* h, const b2
   B200RL_CUDA(cudaMemcpy2DAsync(h->idx, ls, idx, SB * 8, SB * 8, h->K, cudaMemcpyHostToDevice, s));
   const size_t n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise && !h->dqn && !h->dsac ? SB * A : 0);
   if (n_eps) B200RL_CUDA(cudaMemcpy2DAsync(h->eps, ls, noise, n_eps * 4, n_eps * 4, h->K, cudaMemcpyHostToDevice, s));
+  if (cql_take_draws(h, S, B, "offpolicy_train_gather")) return 1;
   if (gather_columns(h, hp, (long long)SB, s)) return 1;
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
 }
@@ -4064,6 +4438,12 @@ extern "C" int b200rl_offpolicy_train_gather_rng_group(b200rl_offpolicy* h, cons
   if (launch(h, draw_minibatches_kernel<false>, draw_minibatches_kernel<true>, (unsigned)((n_thr + 255) / 256), 256, 0,
              s, h->idx, SB, n_eps ? h->eps : nullptr, n_eps, keys))
     return 1;
+  if (h->cql) {  // CQL's draws under their own Philox tag
+    const long long n_cql = (long long)cql_draw_floats(h, S, B);
+    if (launch(h, cql_draw_kernel<false>, cql_draw_kernel<true>, (unsigned)((n_cql / 4 + 1 + 255) / 256), 256, 0, s,
+               h->cql_draws, n_cql, (long long)B * h->cql_cfg.n_actions * A, keys))
+      return 1;
+  }
   if (gather_columns(h, hp, SB, s)) return 1;
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
 }

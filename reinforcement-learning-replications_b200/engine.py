@@ -337,22 +337,24 @@ class OffPolicyEngine:
     DDPG's networks with a categorical critic: ``q_sizes`` = [obs + act, ..., N] and ``d4pg`` = (N, v_min, v_max), the
     critic's support; it takes ``set_per`` / ``train_prioritized`` and ``set_nstep`` as DQN does (b200rl.h, "D4PG").
     TQC (``algo`` 7) is a SAC engine whose critics map [s | a] to M quantiles: ``q_sizes`` = [obs + act, ..., M] and
-    ``tqc`` = (M, d), d the atoms per critic dropped from the pooled target (b200rl.h, "TQC").
+    ``tqc`` = (M, d), d the atoms per critic dropped from the pooled target (b200rl.h, "TQC").  CQL (``algo`` 8) is a SAC
+    engine whose critic step also runs on 3N sampled actions per row: ``cql`` = (N, lagrange); ``set_cql`` is required,
+    and a call with host draws takes ``noise`` = (SAC's [S, 2, B, A], CQL's [S, 3, B, N, A]) (b200rl.h, "CQL").
 
     ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
     launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
     is [K][per-learner blob] with [K][3] step counts, and the per-network accessors are refused."""
 
     NETS = {"policy": 0, "q1": 1, "q2": 2, "target_policy": 3, "target_q1": 4, "target_q2": 5}
-    TD3, SAC, DQN, C51, IQN, DSAC, D4PG, TQC = 0, 1, 2, 3, 4, 5, 6, 7
+    TD3, SAC, DQN, C51, IQN, DSAC, D4PG, TQC, CQL = 0, 1, 2, 3, 4, 5, 6, 7, 8
     DISCRETE = (DQN, C51, IQN)  # the algos with DQN's networks, inputs and outputs
     INDEX_ACTIONS = DISCRETE + (DSAC,)  # the algos whose action column holds an action index
-    SOFT = (SAC, DSAC, TQC)  # the algos with SAC's networks, temperature and outputs
-    SQUASHED = (SAC, TQC)  # the algos with SAC's squashed-Gaussian policy and its [S, 2, B, A] noise
+    SOFT = (SAC, DSAC, TQC, CQL)  # the algos with SAC's networks, temperature and outputs
+    SQUASHED = (SAC, TQC, CQL)  # the algos with SAC's squashed-Gaussian policy and its [S, 2, B, A] noise
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
                  q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1, dueling_k: int = 0,
-                 noisy_layers: int = 0, iqn=None, d4pg=None, tqc=None):
+                 noisy_layers: int = 0, iqn=None, d4pg=None, tqc=None, cql=None):
         from ._lib import OffPolicyConfig
         self.lib = _lib.load()
         current_stream_handle()
@@ -366,6 +368,7 @@ class OffPolicyEngine:
         self.iqn = None if iqn is None else tuple(int(x) for x in iqn)
         self.d4pg = None if d4pg is None else (int(d4pg[0]), float(d4pg[1]), float(d4pg[2]))
         self.tqc = None if tqc is None else (int(tqc[0]), int(tqc[1]))
+        self.cql = None if cql is None else (int(cql[0]), int(bool(cql[1])))
         self.discrete = self.algo in self.DISCRETE  # DQN's networks and outputs
         self.index_actions = self.algo in self.INDEX_ACTIONS  # act [S,B] indices, no noise
         self.n_q, self.max_minibatch, self.max_steps = int(n_q), int(max_minibatch), int(max_steps)
@@ -394,6 +397,9 @@ class OffPolicyEngine:
         elif self.tqc is not None:  # the quantile counts size the critics' heads (b200rl.h, "TQC")
             check(self.lib.b200rl_offpolicy_create_tqc(C.byref(cfg), C.byref(_lib.TqcConfig(*self.tqc)), self.K,
                                                        C.byref(h)), "offpolicy_create_tqc")
+        elif self.cql is not None:  # N and the Lagrange switch size the buffers (b200rl.h, "CQL")
+            check(self.lib.b200rl_offpolicy_create_cql(C.byref(cfg), C.byref(_lib.CqlConfig(*self.cql)), self.K,
+                                                       C.byref(h)), "offpolicy_create_cql")
         else:
             check(self.lib.b200rl_offpolicy_create_group(C.byref(cfg), self.K, C.byref(h)), "offpolicy_create")
         self.h = h
@@ -535,6 +541,67 @@ class OffPolicyEngine:
         st = np.zeros(self.K, np.int64)
         check(self.lib.b200rl_offpolicy_get_alpha_group(self.h, _ptr(la), _ptr(m), _ptr(v), _ptr(st)), "get_alpha")
         return [(float(la[z]), float(m[z]), float(v[z]), int(st[z])) for z in range(self.K)]
+
+    # ---- CQL ----
+    def set_cql(self, weight: float, temperature: float, target_action_gap: float = 0.0, alpha_lr: float = 3e-4,
+                alpha_betas=(0.9, 0.999), alpha_eps: float = 1e-8, backup_entropy: bool = False) -> None:
+        """The penalty's weight and temperature, the Lagrange step's gap and Adam settings, and whether the backup keeps
+        SAC's entropy term (b200rl.h, "CQL")."""
+        cp = _lib.CqlHparams(float(weight), float(temperature), float(target_action_gap), float(alpha_lr),
+                             float(alpha_betas[0]), float(alpha_betas[1]), float(alpha_eps), int(bool(backup_entropy)), 0)
+        check(self.lib.b200rl_offpolicy_set_cql(self.h, C.byref(cp)), "set_cql")
+
+    def set_alpha_prime(self, log_alpha_prime: float, exp_avg: float = 0.0, exp_avg_sq: float = 0.0,
+                        step: int = 0) -> None:
+        self.set_alpha_prime_group([(log_alpha_prime, exp_avg, exp_avg_sq, step)])
+
+    def get_alpha_prime(self):
+        """(log_alpha', exp_avg, exp_avg_sq, step) of the Lagrange multiplier, float32 values as Python floats."""
+        return self.get_alpha_prime_group()[0]
+
+    def set_alpha_prime_group(self, states) -> None:
+        """``states``: K tuples (log_alpha', exp_avg, exp_avg_sq, step), one per learner."""
+        la, m, v = (np.array([float(x[i]) for x in states], np.float32) for i in range(3))
+        st = np.array([int(x[3]) for x in states], np.int64)
+        if st.size != self.K:
+            raise ValueError(f"set_alpha_prime_group: expected {self.K} learners, got {st.size}")
+        check(self.lib.b200rl_offpolicy_set_alpha_prime_group(self.h, _ptr(la), _ptr(m), _ptr(v), _ptr(st)),
+              "set_alpha_prime")
+
+    def get_alpha_prime_group(self):
+        la, m, v = (np.zeros(self.K, np.float32) for _ in range(3))
+        st = np.zeros(self.K, np.int64)
+        check(self.lib.b200rl_offpolicy_get_alpha_prime_group(self.h, _ptr(la), _ptr(m), _ptr(v), _ptr(st)),
+              "get_alpha_prime")
+        return [(float(la[z]), float(m[z]), float(v[z]), int(st[z])) for z in range(self.K)]
+
+    def cql_outputs(self, S: int):
+        """(gap_1 [S], gap_2 [S], alpha' [S]) of the last train call's steps (alpha' 1 without the Lagrange step); a
+        group: each with a leading [K] axis."""
+        gaps, ap = np.zeros((self.K, 2, S), np.float32), np.zeros((self.K, S), np.float32)
+        check(self.lib.b200rl_offpolicy_cql_outputs(self.h, int(S), _ptr(gaps), _ptr(ap)), "cql_outputs")
+        out = gaps[:, 0], gaps[:, 1], ap
+        return tuple(x[0] for x in out) if self.K == 1 else out
+
+    def _cql_draws_shape(self, S, B):
+        return (self.K, S, 3, B, self.cql[0], self.policy_sizes[-1] // 2)
+
+    def get_cql_draws(self, S: int, B: int):
+        """CQL's draws [S, 3, B, N, A] of the last train call (x in [0, 1), eps at s, eps at s'); a group: [K, ...]."""
+        d = np.empty(self._cql_draws_shape(S, B), np.float32)
+        check(self.lib.b200rl_offpolicy_get_cql_draws(self.h, int(S), int(B), _ptr(d)), "get_cql_draws")
+        return d[0] if self.K == 1 else d
+
+    def _split_noise(self, noise, S, B):
+        """A CQL engine's (SAC noise, CQL draws): stages the draws for the call, returns SAC's part."""
+        if self.algo != self.CQL or not isinstance(noise, tuple):  # SAC's part alone: the engine asks for the draws
+            return noise
+        sac, draws = noise
+        draws = self._lead(draws, np.float32, 6)
+        if draws.shape != self._cql_draws_shape(S, B):
+            raise ValueError(f"CQL draws: expected shape {self._cql_draws_shape(S, B)}, got {draws.shape}")
+        check(self.lib.b200rl_offpolicy_set_cql_draws(self.h, int(S), int(B), _ptr(draws)), "set_cql_draws")
+        return sac
 
     # ---- DQN ----
     def set_dqn(self, target_update_interval: int, double_q: bool) -> None:
@@ -684,6 +751,8 @@ class OffPolicyEngine:
             out = {k: v[0] for k, v in out.items()}
         if self.algo in self.SOFT:
             out["log_prob_means"], out["alphas"] = self.sac_outputs(S)
+        if self.algo == self.CQL:
+            out["cql_gap_1"], out["cql_gap_2"], out["alpha_primes"] = self.cql_outputs(S)
         return out
 
     def _lead(self, a, dtype, ndim):
@@ -704,8 +773,9 @@ class OffPolicyEngine:
             act = np.asarray(act, np.float32)[..., None]
         obs, act, next_obs = (self._lead(x, np.float32, 4) for x in (obs, act, next_obs))
         rew, done = self._lead(rew, np.float32, 3), self._lead(done, np.float32, 3)
-        noise = None if noise is None else self._lead(noise, np.float32, 5 if self.algo in self.SQUASHED else 4)
         S, B = obs.shape[1], obs.shape[2]
+        noise = self._split_noise(noise, S, B)
+        noise = None if noise is None else self._lead(noise, np.float32, 5 if self.algo in self.SQUASHED else 4)
         q1v, q2v, l1, l2, lp, npol = self._out_buffers(S, B)
         check(self.lib.b200rl_offpolicy_train(self.h, C.byref(hp), S, B, _ptr(obs), _ptr(act), _ptr(rew), _ptr(next_obs),
                                               _ptr(done), _ptr(noise), _ptr(q1v), _ptr(q2v), _ptr(l1), _ptr(l2), _ptr(lp),
@@ -764,8 +834,9 @@ class OffPolicyEngine:
         ``idx`` [K,S,B], ``noise`` [K,S,B,A] (SAC [K,S,2,B,A]); a solo engine also takes them without the [K] axis."""
         rb = self._replays(replays)
         idx = self._lead(idx, np.int64, 3)
-        noise = None if noise is None else self._lead(noise, np.float32, 5 if self.algo in self.SQUASHED else 4)
         S, B = idx.shape[1], idx.shape[2]
+        noise = self._split_noise(noise, S, B)
+        noise = None if noise is None else self._lead(noise, np.float32, 5 if self.algo in self.SQUASHED else 4)
         q1v, q2v, l1, l2, lp, npol = self._out_buffers(S, B)
         check(self.lib.b200rl_offpolicy_train_gather_group(self.h, C.byref(hp), S, B, rb, _ptr(idx), _ptr(noise),
                                                            _ptr(q1v), _ptr(q2v), _ptr(l1), _ptr(l2), _ptr(lp),

@@ -39,6 +39,48 @@ class ReplayBuffer:
         self._dev_ends = None         # device mirror of _ends (float32 0/1), built by the first device_episode_ends()
         self._dev_dirty: List = []    # physical row ranges written since the mirror was last refreshed
 
+    @classmethod
+    def from_dataset(cls, dataset, buffer_size: Optional[int] = None) -> "ReplayBuffer":
+        """A buffer holding a fixed dataset with D4RL's keys: ``observations`` [n, O], ``actions`` [n, A], ``rewards``
+        [n], ``next_observations`` [n, O], ``terminals`` [n] and optionally ``timeouts`` [n].  dones = terminals; a row
+        ends an episode (for n-step windows) when it is terminal, timed out or the last row.  ``buffer_size`` defaults to
+        the dataset's length and may not be smaller: an offline learner cannot afford to drop rows silently."""
+        keys = ("observations", "actions", "rewards", "next_observations", "terminals")
+        missing = [k for k in keys if k not in dataset]
+        if missing:
+            raise ValueError(f"from_dataset: the dataset lacks {missing}")
+        cols = {k: np.asarray(dataset[k]) for k in keys}
+        if "timeouts" in dataset and dataset["timeouts"] is not None:
+            cols["timeouts"] = np.asarray(dataset["timeouts"])
+        n = len(cols["observations"])
+        if n == 0:
+            raise ValueError("from_dataset: the dataset has no rows")
+        lengths = {k: len(v) for k, v in cols.items()}
+        if any(m != n for m in lengths.values()):
+            raise ValueError(f"from_dataset: the columns differ in length: {lengths}")
+        for k in ("observations", "actions", "rewards", "next_observations"):
+            if not np.all(np.isfinite(cols[k].astype(np.float64))):
+                raise ValueError(f"from_dataset: {k} holds non-finite values")
+        size = n if buffer_size is None else int(buffer_size)
+        if size < n:
+            raise ValueError(f"from_dataset: buffer_size {size} is smaller than the dataset's {n} rows")
+        rb = cls(size)
+        terminals = cols["terminals"].astype(np.bool_).reshape(n)
+        new = (cols["observations"], cols["actions"], cols["rewards"].reshape(n), cols["next_observations"], terminals)
+        rb._allocate(n, new)
+        if rb._capacity < n:  # _allocate starts at 1024 rows at least, buffer_size rows at most
+            rb._grow(n)
+        for k, v in zip(cls.COLUMNS, new):
+            col = rb._cols[k]
+            col[:n] = np.asarray(v, dtype=col.dtype).reshape((n,) + col.shape[1:])
+        ends = terminals.copy()
+        if "timeouts" in cols:
+            ends |= cols["timeouts"].astype(np.bool_).reshape(n)
+        ends[-1] = True
+        rb._ends[:n] = ends
+        rb.current_size = n
+        return rb
+
     # ---- storage ----
     def _allocate(self, rows: int, samples) -> None:
         rows = min(max(rows, 1024), self.buffer_size)

@@ -344,7 +344,8 @@ typedef struct {
                             * b200rl_offpolicy_create_iqn only; see "IQN" below), 5 = discrete SAC (see
                             * "Discrete SAC" below), 6 = D4PG (created by b200rl_offpolicy_create_d4pg only; see
                             * "D4PG" below), 7 = TQC (created by b200rl_offpolicy_create_tqc only; see "TQC" below),
-                            * 8 = CQL (created by b200rl_offpolicy_create_cql only; see "CQL" below) */
+                            * 8 = CQL (created by b200rl_offpolicy_create_cql only; see "CQL" below), 9 = IQL
+                            * (created by b200rl_offpolicy_create_iql only; see "IQL" below) */
   int32_t dueling_k;       /* 0 = the Q network is a plain MLP; K >= 1 = a dueling Q network (algo 2 / 3 only; see
                             * "Dueling Q networks" below) */
   int32_t noisy_layers;    /* bit mask over the Q network's Linear layers in flat order: 0 = none; bit l = layer l is a
@@ -364,7 +365,7 @@ int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200rl_offpolicy
 void b200rl_offpolicy_destroy(b200rl_offpolicy* h);
 int b200rl_offpolicy_set_params(b200rl_offpolicy* h, int which, const float* host_flat, int64_t n, void* stream);
 int b200rl_offpolicy_get_params(b200rl_offpolicy* h, int which, float* host_flat, int64_t n, void* stream);
-/* which: 0 policy, 1 Q1, 2 Q2 optimizers */
+/* which: 0 policy, 1 Q1, 2 Q2 optimizers (and 3 V on an IQL engine) */
 int b200rl_offpolicy_set_adam(b200rl_offpolicy* h, int which, const float* exp_avg, const float* exp_avg_sq, int64_t n,
                               int64_t step, void* stream);
 int b200rl_offpolicy_get_adam(b200rl_offpolicy* h, int which, float* exp_avg, float* exp_avg_sq, int64_t n,
@@ -849,6 +850,67 @@ int b200rl_offpolicy_cql_outputs(b200rl_offpolicy* h, int32_t S, float* gaps, fl
 /* The host draws [K][S][3][B][N][A] of the next train / train_gather call, and the draws of the last call. */
 int b200rl_offpolicy_set_cql_draws(b200rl_offpolicy* h, int32_t S, int32_t B, const float* draws);
 int b200rl_offpolicy_get_cql_draws(b200rl_offpolicy* h, int32_t S, int32_t B, float* draws);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * IQL on the same engine (config algo = 9, n_q = 2; Kostrikov, Nair & Levine 2021, "Offline Reinforcement Learning
+ * with Implicit Q-Learning"): an expectile value network, an advantage-weighted policy and twin critics, none of which
+ * is ever evaluated at an action outside the minibatch.  Created by b200rl_offpolicy_create_iql from a config with
+ * algo = 9 and a b200rl_iql_config; create and create_group refuse algo 9.  Networks: 0 the policy [obs, ..., 2A]
+ * (outputs [m | l]), 1 / 2 the critics [obs + A, ..., 1], 3 the value network V = iql->value [obs, ..., 1], 4 / 5 the
+ * target critics; network 3 is trained (optimizer 3).  For an IQL engine the state blob is networks 0..5, then
+ * exp_avg / exp_avg_sq of optimizers 0..3, each segment padded as above; steps is [K][4]; set_adam / get_adam take
+ * which = 3.  Every other engine keeps its blob and steps[K][3].  With L = hparams.action_limit, tau = expectile,
+ * beta, W = max_weight, per train step in float32 on a minibatch (s, a, r, s', d) of B rows (the reference
+ * implementation's order: value, actor with the new V, critics with the new V, targets):
+ *   target   q^_i = min(Q1targ, Q2targ)(s_i, a_i) (torch.min: a NaN propagates)
+ *   value    (optimizer 3) u_i = q^_i - V(s_i), w_i = tau if u_i > 0 else 1 - tau; one Adam step on
+ *            L_V = mean_i w_i u_i^2, whose gradient w.r.t. V(s_i) is -2 w_i u_i / B; V' = the updated network
+ *   policy   (optimizer 0) mu = L tanh(m), log sigma = clamp(l, log_std_min, log_std_max);
+ *            log pi(a | s) = sum_j Normal(mu_j, sigma_j).log_prob(a_j) (a Gaussian whose mean is bounded, not a squashed
+ *            sample: a dataset action at +-L needs no atanh); e_i = min(exp(beta (q^_i - V'(s_i))), W), a constant (NaN
+ *            stays NaN); one Adam step on L_pi = -mean_i e_i log pi(a_i | s_i), whose output gradients are
+ *            -e_i (a_j - mu_j) / sigma_j^2 L (1 - tanh^2 m_j) / B (mean columns) and -e_i ((a_j - mu_j)^2 / sigma_j^2 - 1)
+ *            / B inside the clamp, 0 outside it (log-std columns); beta = 0 is behaviour cloning
+ *   critics  (optimizers 1, 2, the critics at the start of the step) y_i = r_i + gamma (1 - d_i) V'(s'_i); one Adam
+ *            step each on mean_i (Q_k(s_i, a_i) - y_i)^2
+ *   polyak   Q1targ, Q2targ with hparams.polyak_rho
+ * Nothing is drawn: train / train_gather take noise = NULL, train_gather_rng draws the indices only, get_draws returns
+ * no noise (its noise must be NULL).  hparams.use_target_noise must be 0 and policy_delay >= 1 (it does not apply).
+ * V's learning rate comes with each call (b200rl_iql_hparams.v_lr, read by run, not part of the cached graph's key),
+ * the rest of set_iql is part of the key.  Outputs: q{k}_values [S,B] (pre-update), q{k}_losses [S], policy_losses
+ * [S] = L_pi, and iql_outputs' value losses L_V, value means mean_i V(s_i) (before the value step) and weight means
+ * mean_i e_i, each [K][S].  The heads reduce in a fixed order with no float atomics (one CTA per head): a group's
+ * learners stay bit-identical to solo engines.  train, train_gather, train_gather_rng and their group forms all work,
+ * as a CUDA graph or as plain launches with B200RL_OFFPOLICY_GRAPH=0.
+ * Launches, with Lq, Lp and Lv the critics', the policy's and the value network's Linear layers: per step
+ * 8 Lq + 3 Lp + 5 Lv + 5 (8 forward passes, four weight-gradient backward passes without input gradients, the value,
+ * policy and two critic heads, four Adam steps, polyak): 53 per step at two hidden layers.
+ * Refused at create: create_iql with another algo, algo 9 through create / create_group; n_q != 2; dueling_k or
+ * noisy_layers != 0; a policy that is not [obs, ..., 2A], critics that are not [obs + A, ..., 1], a value network that
+ * is not [obs, ..., 1].  set_iql refuses tau outside (0, 1), beta < 0 or not finite, W <= 0 or not finite, log_std_min
+ * >= log_std_max, and non-finite Adam settings; it refuses every other engine.  set_sac, set_cql, set_dqn, set_c51,
+ * set_qr, set_per, set_nstep, set_noise_keys and the train_prioritized calls refuse an IQL engine.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  b200rl_mlp_desc value; /* V: [obs, hidden..., 1] */
+} b200rl_iql_config;
+
+typedef struct {
+  double expectile;                  /* tau in (0, 1) */
+  double beta;                       /* inverse temperature >= 0 (0 = behaviour cloning) */
+  double max_weight;                 /* W > 0: the AWR weights are clamped to it */
+  double log_std_min, log_std_max;   /* the policy's log-std clamp */
+  double v_lr, v_beta1, v_beta2, v_eps; /* torch.optim.Adam over V (v_lr is read per call) */
+} b200rl_iql_hparams;
+
+/* An IQL engine of n_learners learners (1 = a solo engine; 1 <= n_learners <= B200RL_MAX_LEARNERS): cfg->algo = 9. */
+int b200rl_offpolicy_create_iql(const b200rl_offpolicy_config* cfg, const b200rl_iql_config* iql, int32_t n_learners,
+                                b200rl_offpolicy** out);
+/* Required once before the first train call; part of the cached graph's key except v_lr. */
+int b200rl_offpolicy_set_iql(b200rl_offpolicy* h, const b200rl_iql_hparams* hp);
+/* value_losses, value_means and weight_means [K][S] of the last train call's steps. */
+int b200rl_offpolicy_iql_outputs(b200rl_offpolicy* h, int32_t S, float* value_losses, float* value_means,
+                                 float* weight_means);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Learner groups: K independent off-policy learners (same config, same hyper-parameters, their own parameters, Adam

@@ -106,6 +106,16 @@ class CqlHparams(C.Structure):
                 ("alpha_eps", C.c_double), ("backup_entropy", C.c_int32), ("reserved", C.c_int32)]
 
 
+class IqlConfig(C.Structure):
+    _fields_ = [("value", MlpDesc)]
+
+
+class IqlHparams(C.Structure):
+    _fields_ = [("expectile", C.c_double), ("beta", C.c_double), ("max_weight", C.c_double),
+                ("log_std_min", C.c_double), ("log_std_max", C.c_double), ("v_lr", C.c_double),
+                ("v_beta1", C.c_double), ("v_beta2", C.c_double), ("v_eps", C.c_double)]
+
+
 class SacHparams(C.Structure):
     _fields_ = [("alpha", C.c_double), ("target_entropy", C.c_double), ("alpha_lr", C.c_double),
                 ("alpha_beta1", C.c_double), ("alpha_beta2", C.c_double), ("alpha_eps", C.c_double),
@@ -253,6 +263,10 @@ SIGNATURES = {
     "b200rl_offpolicy_set_cql_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "b200rl_offpolicy_get_cql_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "b200rl_offpolicy_get_alpha_group": (C.c_int, [C.c_void_p] * 5),
+    "b200rl_offpolicy_create_iql": (C.c_int, [C.POINTER(OffPolicyConfig), C.POINTER(IqlConfig), C.c_int32,
+                                              C.POINTER(C.c_void_p)]),
+    "b200rl_offpolicy_set_iql": (C.c_int, [C.c_void_p, C.POINTER(IqlHparams)]),
+    "b200rl_offpolicy_iql_outputs": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200rl_discounted_cumsum": (C.c_int, [C.c_void_p, C.c_int64, C.c_double, C.c_void_p, C.c_void_p]),
     "b200rl_gae_f64": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_double, C.c_double, C.c_void_p,
                                  C.c_void_p]),

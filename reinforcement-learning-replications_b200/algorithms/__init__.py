@@ -4,6 +4,7 @@ from .d4pg import D4PG
 from .discrete_sac import DiscreteSAC
 from .dqn import DQN
 from .group import LearnerGroup
+from .iql import IQL
 from .iqn import IQN
 from .ppo import PPO
 from .qrdqn import QRDQN
@@ -13,4 +14,4 @@ from .tqc import TQC
 from .trpo import TRPO
 from .vpg import VPG
 
-__all__ = ["VPG", "TRPO", "PPO", "DDPG", "D4PG", "TD3", "SAC", "TQC", "CQL", "DiscreteSAC", "DQN", "C51", "QRDQN", "IQN", "LearnerGroup"]
+__all__ = ["VPG", "TRPO", "PPO", "DDPG", "D4PG", "TD3", "SAC", "TQC", "CQL", "IQL", "DiscreteSAC", "DQN", "C51", "QRDQN", "IQN", "LearnerGroup"]

@@ -1,4 +1,4 @@
-"""LearnerGroup: several independent TD3 / DDPG / D4PG / SAC / TQC / CQL / discrete SAC / DQN / C51 / QR-DQN / IQN learners (typically one per seed) trained side by side by ONE
+"""LearnerGroup: several independent TD3 / DDPG / D4PG / SAC / TQC / CQL / IQL / discrete SAC / DQN / C51 / QR-DQN / IQN learners (typically one per seed) trained side by side by ONE
 off-policy engine, every operation of a train step one launch for all of them (b200rl_offpolicy_create_group).
 
 The contract: each member ends up bit for bit where it would be had it run alone.  Members keep everything of their
@@ -39,6 +39,8 @@ def _signature(agent) -> list:
     trainable, _ = agent._nets()
     dqn = agent.algo in OffPolicyEngine.DISCRETE
     names = ["q_function"] if dqn else ["policy"] + (["q_function_1", "q_function_2"] if agent.n_q == 2 else ["q_function"])
+    if agent.algo == OffPolicyEngine.IQL:
+        names.append("value_function")
     sig = [("class", type(agent).__name__)]
     for name, m in zip(names, trainable):
         if dqn:
@@ -80,6 +82,9 @@ def _signature(agent) -> list:
     if agent.algo == OffPolicyEngine.CQL:
         sig.append(("(cql_n_actions, lagrange)", agent.cql_config))
         sig.append(("CQL hyper-parameters", agent.cql_hparams()))
+    if agent.algo == OffPolicyEngine.IQL:
+        sig.append(("log_std bounds", (agent.policy.log_std_min, agent.policy.log_std_max)))
+        sig.append(("IQL hyper-parameters (expectile, beta, max_weight)", (agent.expectile, agent.beta, agent.max_weight)))
     if agent.algo == OffPolicyEngine.D4PG:
         sig.append(("(n_atoms, v_min, v_max)", agent.d4pg_config))
         sig.append(("n_step", agent.n_step))
@@ -142,7 +147,7 @@ class LearnerGroup:
     def add(self, agent) -> None:
         """Add ``agent``; the current state of the global random generators becomes its private stream."""
         if not isinstance(agent, _OffPolicyBase):
-            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or D4PG / TQC / CQL / DiscreteSAC / DQN / C51 / QR-DQN / IQN) learners, got {type(agent).__name__}")
+            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or D4PG / TQC / CQL / IQL / DiscreteSAC / DQN / C51 / QR-DQN / IQN) learners, got {type(agent).__name__}")
         if any(m is agent for m in self.members):
             raise ValueError("LearnerGroup: this agent is already a member")
         if len(self.members) >= MAX_LEARNERS:
@@ -230,6 +235,8 @@ class LearnerGroup:
             e.set_sac(members[0]._sac_hparams())
             e.set_alpha_group([m._alpha_state() for m in members])
         cql = members[0].algo == OffPolicyEngine.CQL
+        if members[0].algo == OffPolicyEngine.IQL:
+            e.set_iql(**members[0].iql_hparams())
         if cql:
             e.set_cql(**members[0].cql_hparams())
             e.set_alpha_prime_group([m._alpha_prime_state() for m in members])

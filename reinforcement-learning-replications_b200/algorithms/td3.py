@@ -123,8 +123,9 @@ class _OffPolicyBase:
         e.set_state(None, self._fill_state(self._state_plan(e, trainable, targets, lins), trainable, lins))
 
     def _fill_state(self, slots, trainable, lins):
-        """Host modules and Adam states -> this learner's part of the blob; returns its [3] Adam step counts."""
-        steps = [0, 0, 0]
+        """Host modules and Adam states -> this learner's part of the blob; returns its Adam step counts, one per engine
+        optimizer row (3, or 4 with IQL's value network in slot 3)."""
+        steps = [0] * max(3, 1 + max(self.trainable_slots))
         for i, m, l in zip(self.trainable_slots, trainable, lins):
             adam_hparams(m.optimizer, l, "optimizer")  # refuses anything but a plain Adam over exactly this network
             steps[i] = self._adam_step_count(m.optimizer, l)
@@ -180,8 +181,9 @@ class _OffPolicyBase:
         hp.policy_delay, hp.use_target_noise = int(delay), int(noisy)
         hp.policy_lr, hp.policy_beta1, hp.policy_beta2, hp.policy_eps = adam_hparams(
             self.policy.optimizer, lin(self.policy), "policy optimizer")
+        q_last = trainable[2] if self.n_q == 2 else trainable[1]  # IQL's value function follows the critics
         q1 = adam_hparams(trainable[1].optimizer, lin(trainable[1]), "q-function optimizer")
-        q2 = adam_hparams(trainable[-1].optimizer, lin(trainable[-1]), "q-function optimizer")
+        q2 = adam_hparams(q_last.optimizer, lin(q_last), "q-function optimizer")
         if q1[1:] != q2[1:]:
             raise NotImplementedError("both Q optimizers must share betas / eps")
         hp.q1_lr, hp.q2_lr = q1[0], q2[0]

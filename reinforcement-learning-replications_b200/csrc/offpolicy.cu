@@ -42,6 +42,8 @@
 // prioritized draw / priority update and n-step staging.
 // TQC (config algo = 7, create_tqc) is SAC's step program (enqueue_sac_steps) with two quantile critics over [s | a]:
 // tqc_target_kernel truncates the pooled target atoms, tqc_critic_loss_kernel and tqc_policy_loss_kernel are the heads.
+// IQL (config algo = 9, create_iql) is a step program of its own (enqueue_iql_steps): network 3 is a trained value
+// network, iql_value_loss_kernel and iql_policy_loss_kernel are its heads, sac_q_loss_kernel the critics'.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -633,6 +635,82 @@ __global__ void __launch_bounds__(GTHREADS) sac_alpha_step_kernel(const float* l
     state[2] = v;
     *alpha_next = expf(p);
   }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// IQL (algo = 9; Kostrikov, Nair & Levine 2021): the expectile value head and the advantage-weighted policy head.  The
+// critics' head is sac_q_loss_kernel with V'(s') as both target inputs and a zero temperature and log density.
+// ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float torch_min(float a, float b) { return isnan(a) || a < b ? a : b; }  // NaN propagates
+
+// One CTA: q^ = min(q1t, q2t), u = q^ - v, w = tau (u > 0) or 1 - tau; loss = mean(w u^2), dv = -2 w u / B,
+// mean_out = mean(v) (the value network at the start of the step)
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) iql_value_loss_kernel(const float* q1t, const float* q2t, const float* v,
+                                                                 float tau, float one_minus_tau, int n, float* dv,
+                                                                 float* loss_out, float* mean_out, size_t lane_stride) {
+  __shared__ double red[32], red_v[32];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q1t = lane_ptr(q1t, o), q2t = lane_ptr(q2t, o), v = lane_ptr(v, o), dv = lane_ptr(dv, o);
+    loss_out = lane_ptr(loss_out, o), mean_out = lane_ptr(mean_out, o);
+  }
+  const float inv = 1.0f / (float)n;
+  double acc = 0.0, acc_v = 0.0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float vi = v[i];
+    const float u = torch_min(q1t[i], q2t[i]) - vi;
+    const float w = u > 0.f ? tau : one_minus_tau;
+    acc += (double)(w * (u * u));
+    acc_v += (double)vi;
+    dv[i] = -((2.f * w * u) * inv);
+  }
+  block_mean(acc, n, loss_out, red);
+  block_mean(acc_v, n, mean_out, red_v);
+}
+
+// One CTA, one thread per row i: the AWR head on the policy output out = [m | l] [B, 2A] at the dataset action act:
+// e_i = min(exp(beta (min(q1t, q2t) - v)), W) (NaN stays NaN), log pi_i = sum_j Normal(L tanh m_j, exp(clamp l_j))
+// .log_prob(a_j); loss = -mean(e log pi), weight_mean = mean(e), dout = d loss / d [m | l] (b200rl.h, "IQL")
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) iql_policy_loss_kernel(const float* out, const float* act, const float* q1t,
+                                                                  const float* q2t, const float* v, int n, int A,
+                                                                  float beta, float max_w, float lmin, float lmax,
+                                                                  float limit, float* dout, float* loss_out,
+                                                                  float* weight_mean_out, size_t lane_stride) {
+  __shared__ double red[32], red_w[32];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    out = lane_ptr(out, o), act = lane_ptr(act, o), q1t = lane_ptr(q1t, o), q2t = lane_ptr(q2t, o);
+    v = lane_ptr(v, o), dout = lane_ptr(dout, o);
+  }
+  const float inv = 1.0f / (float)n;
+  double acc = 0.0, acc_w = 0.0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float x = expf(beta * (torch_min(q1t[i], q2t[i]) - v[i]));
+    const float e = x > max_w ? max_w : x;
+    const float c = e * inv;
+    const float* row = out + (size_t)i * 2 * A;
+    float* drow = dout + (size_t)i * 2 * A;
+    float lp = 0.f;
+    for (int j = 0; j < A; ++j) {
+      const float t = tanhf(row[j]), raw = row[A + j];
+      const float ls = fminf(fmaxf(raw, lmin), lmax);
+      const float sigma = expf(ls), var = sigma * sigma;
+      const float d = act[(size_t)i * A + j] - limit * t;
+      lp += -(d * d) / (2.f * var) - ls - 0.918938533204672742f;  // - log sqrt(2 pi)
+      drow[j] = -(c * (d / var)) * (limit * (1.f - t * t));
+      drow[A + j] = (raw >= lmin && raw <= lmax) ? -(c * ((d * d) / var - 1.f)) : 0.f;
+    }
+    acc -= (double)(e * lp);
+    acc_w += (double)e;
+  }
+  if (LANES) {  // offset after the row loop: with both outputs live across it ptxas spills
+    const size_t o = blockIdx.z * lane_stride;
+    loss_out = lane_ptr(loss_out, o), weight_mean_out = lane_ptr(weight_mean_out, o);
+  }
+  block_mean(acc, n, loss_out, red);
+  block_mean(acc_w, n, weight_mean_out, red_w);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -2181,6 +2259,7 @@ struct GraphKey {
   b200rl_per_hparams per;
   ReplayLanes<true> replay;
   b200rl_cql_hparams cql;
+  b200rl_iql_hparams iql;  // v_lr zeroed: V's learning rate is read per call, like q1_lr / q2_lr
 };
 
 struct b200rl_offpolicy {
@@ -2309,6 +2388,15 @@ struct b200rl_offpolicy {
   float* cql_ap_state = nullptr;                 // {log alpha', exp_avg, exp_avg_sq}
   float* cql_zero = nullptr;                     // one 0.f: the temperature of a backup without the entropy term
   int64_t ap_step[B200RL_MAX_LEARNERS] = {};
+  // IQL (cfg.algo == 9): network 3 is the value network V, trained by optimizer 3 (adam_tab row 3); networks 0, 1, 2,
+  // 4, 5 are SAC's.  The critics' backward passes run beside the policy's, so Q1's takes a third gradient ping-pong.
+  bool iql = false, iql_set = false;
+  b200rl_iql_hparams iql_hp{};
+  float *dbuf4 = nullptr, *dbuf5 = nullptr;   // [B, maxw] Q1's gradient ping-pong
+  float* iql_dv = nullptr;                     // [B] d L_V / d V(s)
+  float* iql_dout = nullptr;                   // [B, 2A] d L_pi / d [m | l]
+  float* iql_zero = nullptr;                   // [B] zeros: the critics' head's temperature and log density
+  float *out_vl = nullptr, *out_vm = nullptr, *out_wm = nullptr;  // [max_steps] value loss, value mean, weight mean
   // the replay columns, episode-end columns, trees and row counts of this call (train_gather[_rng], train_prioritized)
   ReplayLanes<true> replay{};
   std::vector<void*> allocs;
@@ -2318,12 +2406,15 @@ namespace {
 
 inline int64_t state_pad(int64_t n) { return (n + 63) & ~(int64_t)63; }
 
+// the optimizers of the state blob and of steps[]: policy, Q1, Q2 (and V on an IQL engine)
+inline int n_opt(const b200rl_offpolicy* h) { return h->iql ? 4 : 3; }
+
 // float2 entries of one learner's adam_tab: the Adam scalar rows (+ SAC's temperature row, DQN's copy flags or D4PG's
 // betas), then DQN's or D4PG's prioritized (seed, call) at 4 max_steps and a noisy or IQN engine's draw keys (seed,
 // call) after it
 inline size_t adam_tab_len(const b200rl_offpolicy* h) {
   const bool per = h->dqn || h->d4pg;  // engines that take prioritized replay: row 3's .y holds the betas
-  return (h->cql ? 5 : h->sac || h->dsac || per ? 4 : 3) * (size_t)h->cfg.max_steps + (per ? 2 : 0) +
+  return (h->cql ? 5 : h->sac || h->dsac || h->iql || per ? 4 : 3) * (size_t)h->cfg.max_steps + (per ? 2 : 0) +
          (h->noisy || h->iqn ? 2 : 0);
 }
 
@@ -2428,13 +2519,15 @@ int net_forward(const b200rl_offpolicy* h, const NetBuf& nb, float* const* acts,
 // weight-gradient products go to that stream, behind the gradient they read, and the dX chain -- the critical path --
 // stays on `s`; both are joined before returning.
 int net_backward(b200rl_offpolicy* h, const NetBuf& nb, float* const* acts, const float* dOut, int ld_dout, int rows,
-                 bool want_param_grads, float* dx_out, cudaStream_t s, bool twin_branch = false,
+                 bool want_param_grads, float* dx_out, cudaStream_t s, int branch = 0,
                  const float* in_b = nullptr, int ld_b = 0, int ksplit = 0, cudaStream_t s_dw = nullptr) {
   const int L = nb.d.n_layers;
   const bool side = s_dw != nullptr && want_param_grads && L <= 3;
   const float* dY = dOut;
   int ldd = ld_dout;
-  float* pp[2] = {twin_branch ? h->dbuf2 : h->dbuf0, twin_branch ? h->dbuf3 : h->dbuf1};
+  // the gradient ping-pong of the branch: 0 dbuf0/1, 1 (the twin critic) dbuf2/3, 2 (IQL's Q1) dbuf4/5
+  float* pp[2] = {branch == 0 ? h->dbuf0 : branch == 1 ? h->dbuf2 : h->dbuf4,
+                  branch == 0 ? h->dbuf1 : branch == 1 ? h->dbuf3 : h->dbuf5};
   for (int l = L - 1; l >= 0; --l) {
     const int nout = nb.d.sizes[l + 1], nin = nb.d.sizes[l];
     const int act = (l == L - 1) ? nb.d.out_act : nb.d.hidden_act;
@@ -2633,21 +2726,23 @@ int adam_net(const b200rl_offpolicy* h, NetBuf& nb, const float2* table, int idx
 }  // namespace
 
 // The engine of create_group (ic = dc = tc = NULL), of create_iqn (ic = the IQN counts, config algo 4), of create_d4pg
-// (dc = the support, config algo 6) and of create_tqc (tc = the quantile counts, config algo 7)
+// (dc = the support, config algo 6), of create_tqc (tc = the quantile counts, config algo 7), of create_cql (cc, algo
+// 8) and of create_iql (vc = the value network, config algo 9)
 static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_config* ic,
                          const b200rl_d4pg_config* dc, int32_t n_learners, b200rl_offpolicy** out,
-                         const b200rl_tqc_config* tc = nullptr, const b200rl_cql_config* cc = nullptr) {
+                         const b200rl_tqc_config* tc = nullptr, const b200rl_cql_config* cc = nullptr,
+                         const b200rl_iql_config* vc = nullptr) {
   B200RL_REQUIRE(cfg && out, "offpolicy_create: NULL argument");
   B200RL_REQUIRE(n_learners >= 1 && n_learners <= B200RL_MAX_LEARNERS,
                  "offpolicy_create_group: n_learners must be 1..%d, got %d", B200RL_MAX_LEARNERS, n_learners);
   B200RL_REQUIRE(cfg->n_q == 1 || cfg->n_q == 2, "offpolicy_create: n_q must be 1 (DDPG) or 2 (TD3)");
   B200RL_REQUIRE((cfg->algo >= 0 && cfg->algo <= 3) || cfg->algo == 5 || (cfg->algo == 4 && ic != nullptr) ||
                      (cfg->algo == 6 && dc != nullptr) || (cfg->algo == 7 && tc != nullptr) ||
-                     (cfg->algo == 8 && cc != nullptr),
+                     (cfg->algo == 8 && cc != nullptr) || (cfg->algo == 9 && vc != nullptr),
                  "offpolicy_create: algo must be 0 (DDPG / TD3), 1 (SAC), 2 (DQN), 3 (C51) or 5 (discrete SAC), got %d "
                  "(algo 4, IQN, is created by b200rl_offpolicy_create_iqn with its counts, algo 6, D4PG, by "
                  "b200rl_offpolicy_create_d4pg with its support, algo 7, TQC, by b200rl_offpolicy_create_tqc, algo 8, "
-                 "CQL, by b200rl_offpolicy_create_cql)", cfg->algo);
+                 "CQL, by b200rl_offpolicy_create_cql, algo 9, IQL, by b200rl_offpolicy_create_iql)", cfg->algo);
   B200RL_REQUIRE(ic == nullptr || cfg->algo == 4, "offpolicy_create_iqn: the config's algo must be 4 (IQN), got %d",
                  cfg->algo);
   B200RL_REQUIRE(dc == nullptr || cfg->algo == 6, "offpolicy_create_d4pg: the config's algo must be 6 (D4PG), got %d",
@@ -2656,6 +2751,25 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
                  cfg->algo);
   B200RL_REQUIRE(cc == nullptr || cfg->algo == 8, "offpolicy_create_cql: the config's algo must be 8 (CQL), got %d",
                  cfg->algo);
+  B200RL_REQUIRE(vc == nullptr || cfg->algo == 9, "offpolicy_create_iql: the config's algo must be 9 (IQL), got %d",
+                 cfg->algo);
+  const bool iql = cfg->algo == 9 && vc != nullptr;  // policy, twin critics and a trained value network in slot 3
+  int64_t Pv = 0;
+  if (iql) {
+    B200RL_REQUIRE(cfg->n_q == 2, "offpolicy_create_iql: IQL needs n_q = 2 (twin critics), got %d", cfg->n_q);
+    B200RL_REQUIRE(cfg->dueling_k == 0 && cfg->noisy_layers == 0, "offpolicy_create_iql: IQL takes neither dueling_k "
+                   "nor noisy_layers: dueling and noisy networks are not implemented for it");
+    const b200rl_mlp_desc &p = cfg->policy, &q = cfg->q, &v = vc->value;
+    Pv = b200rl_mlp_param_count(&v);
+    const int O_ = p.sizes[0], A_ = q.sizes[0] - O_;
+    B200RL_REQUIRE(b200rl_mlp_param_count(&p) > 0 && A_ >= 1 && p.sizes[p.n_layers] == 2 * A_,
+                   "offpolicy_create_iql: the policy must map [obs %d] -> [mean | log_std] = 2 x %d values, got %d -> %d",
+                   O_, A_, O_, p.sizes[p.n_layers]);
+    B200RL_REQUIRE(b200rl_mlp_param_count(&q) > 0 && q.sizes[q.n_layers] == 1, "offpolicy_create_iql: the critics must "
+                   "map [obs %d + act %d] -> 1, got %d -> %d", O_, A_, q.sizes[0], q.sizes[q.n_layers]);
+    B200RL_REQUIRE(Pv > 0 && v.sizes[0] == O_ && v.sizes[v.n_layers] == 1, "offpolicy_create_iql: the value network "
+                   "must map [obs %d] -> 1, got %d -> %d", O_, v.sizes[0], v.sizes[v.n_layers]);
+  }
   const bool cql = cfg->algo == 8 && cc != nullptr;  // a SAC engine whose critic step runs on stacked sampled rows
   const int CN = cql ? cc->n_actions : 0;
   if (cql) {
@@ -2757,7 +2871,7 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
                  "layers", NM, n_lin);
   const int O = dqn ? cfg->q.sizes[0] : cfg->policy.sizes[0], P_out = cfg->policy.sizes[cfg->policy.n_layers];
   // SAC: the policy outputs [mean | log_std], 2A wide; DQN: the action column holds the index (1 wide)
-  const int A = dqn || dsac ? 1 : sac ? cfg->q.sizes[0] - O : P_out;
+  const int A = dqn || dsac ? 1 : sac || iql ? cfg->q.sizes[0] - O : P_out;
   B200RL_REQUIRE(!sac || (A >= 1 && P_out == 2 * A),
                  "offpolicy_create: the SAC policy must output [mean | log_std] = 2 x %d values, got %d", A, P_out);
   if (dsac) {  // policy and critics both map obs -> [n]
@@ -2792,13 +2906,14 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   if (tqc) h->tqc_cfg = *tc;
   h->cql = cql;
   if (cql) h->cql_cfg = *cc;
+  h->iql = iql;
   h->noisy = NM != 0;
   int rc = 0;
   int maxw = O + A;
   for (int i = 0; i < 6; ++i) {
     NetBuf& nb = h->net[i];
-    nb.d = (i == 0 || i == 3) ? cfg->policy : cfg->q;
-    nb.P = (i == 0 || i == 3) ? Pp : Pq;
+    nb.d = iql && i == 3 ? vc->value : (i == 0 || i == 3) ? cfg->policy : cfg->q;
+    nb.P = iql && i == 3 ? Pv : (i == 0 || i == 3) ? Pp : Pq;
     int off = 0;
     for (int l = 0; l < nb.d.n_layers; ++l) {
       nb.w_off[l] = off;
@@ -2855,19 +2970,20 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
     if ((sac || dsac) && i == 3) continue;  // SAC has no target policy
     if (dqn && (i == 0 || i == 3)) continue;  // DQN has no policy
     nb.present = true;
-    if (i < 3) rc |= oalloc(h, &nb.grad, (size_t)nb.P);
+    if (i < n_opt(h)) rc |= oalloc(h, &nb.grad, (size_t)nb.P);
     if (nb.P_flat != nb.P) {  // the composed network beside the noisy vector in the slab (and its gradient)
       rc |= oalloc(h, &nb.params, (size_t)nb.P);
       if (i < 3) rc |= oalloc(h, &nb.flat_grad, (size_t)nb.P_flat);
     }
   }
   // parameters and Adam state live in ONE slab in the order of the state blob (b200rl_offpolicy_get_state): the
-  // parameters of networks 0..5, then exp_avg / exp_avg_sq of optimizers 0..2, every segment padded to 64 floats
+  // parameters of networks 0..5, then exp_avg / exp_avg_sq of optimizers 0..2 (0..3 for IQL), every segment padded to
+  // 64 floats
   {
     int64_t n = 0;
     for (int i = 0; i < 6; ++i)
       if (h->net[i].present) n += state_pad(h->net[i].P_flat);
-    for (int i = 0; i < 3; ++i)
+    for (int i = 0; i < n_opt(h); ++i)
       if (h->net[i].present) n += 2 * state_pad(h->net[i].P_flat);
     h->state_n = n;
     rc |= oalloc(h, &h->state, (size_t)n);
@@ -2881,7 +2997,7 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   rc |= oalloc(h, &h->rew, S * B);
   rc |= oalloc(h, &h->nobs, S * B * O);
   rc |= oalloc(h, &h->done, S * B);
-  rc |= oalloc(h, &h->eps, (sac ? 2 : 1) * S * B * A);
+  rc |= oalloc(h, &h->eps, iql ? 0 : (sac ? 2 : 1) * S * B * A);  // IQL draws no noise
   for (int k = 0; k < 5; ++k)
     for (int l = 0; l <= B200RL_MAX_LAYERS; ++l) rc |= oalloc(h, &h->acts[k][l], B * (size_t)maxw);
   for (int l = 0; l <= B200RL_MAX_LAYERS; ++l) rc |= oalloc(h, &h->acts_tq[l], B * (size_t)maxw);
@@ -2932,6 +3048,16 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
     rc |= oalloc(h, &h->cql_ap, S + 1);
     rc |= oalloc(h, &h->cql_ap_state, 3);
     rc |= oalloc(h, &h->cql_zero, 1);
+  }
+  if (iql) {
+    rc |= oalloc(h, &h->dbuf4, B * (size_t)maxw);
+    rc |= oalloc(h, &h->dbuf5, B * (size_t)maxw);
+    rc |= oalloc(h, &h->iql_dv, B);
+    rc |= oalloc(h, &h->iql_dout, B * (size_t)(2 * A));
+    rc |= oalloc(h, &h->iql_zero, B);
+    rc |= oalloc(h, &h->out_vl, S);
+    rc |= oalloc(h, &h->out_vm, S);
+    rc |= oalloc(h, &h->out_wm, S);
   }
   if (dsac) {
     rc |= oalloc(h, &h->sac_logp, B);
@@ -2996,7 +3122,7 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
       if (nb.P_flat == nb.P) nb.params = q, nb.flat_grad = nb.grad;
       q += state_pad(nb.P_flat);
     }
-    for (int i = 0; i < 3; ++i)
+    for (int i = 0; i < n_opt(h); ++i)
       if (h->net[i].present) {
         h->net[i].m = q;
         q += state_pad(h->net[i].P_flat);
@@ -3064,6 +3190,12 @@ extern "C" int b200rl_offpolicy_create_cql(const b200rl_offpolicy_config* cfg, c
   return create_engine(cfg, nullptr, nullptr, n_learners, out, nullptr, cql);
 }
 
+extern "C" int b200rl_offpolicy_create_iql(const b200rl_offpolicy_config* cfg, const b200rl_iql_config* iql,
+                                           int32_t n_learners, b200rl_offpolicy** out) {
+  B200RL_REQUIRE(iql, "offpolicy_create_iql: NULL IQL config");
+  return create_engine(cfg, nullptr, nullptr, n_learners, out, nullptr, nullptr, iql);
+}
+
 extern "C" void b200rl_offpolicy_destroy(b200rl_offpolicy* h) {
   if (!h) return;
   if (h->graph) cudaGraphExecDestroy(h->graph);
@@ -3103,7 +3235,7 @@ extern "C" int b200rl_offpolicy_get_params(b200rl_offpolicy* h, int which, float
 extern "C" int b200rl_offpolicy_set_adam(b200rl_offpolicy* h, int which, const float* exp_avg, const float* exp_avg_sq,
                                          int64_t n, int64_t step, void* stream) {
   B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_set_adam: a learner group moves its state with get_state / set_state");
-  B200RL_REQUIRE(h && which >= 0 && which < 3 && h->net[which].m, "offpolicy_set_adam: bad net");
+  B200RL_REQUIRE(h && which >= 0 && which < n_opt(h) && h->net[which].m, "offpolicy_set_adam: bad net");
   NetBuf& nb = h->net[which];
   B200RL_REQUIRE(n == nb.P_flat && step >= 0, "offpolicy_set_adam: expects %lld floats", (long long)nb.P_flat);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -3118,7 +3250,7 @@ extern "C" int b200rl_offpolicy_set_adam(b200rl_offpolicy* h, int which, const f
 extern "C" int b200rl_offpolicy_get_adam(b200rl_offpolicy* h, int which, float* exp_avg, float* exp_avg_sq, int64_t n,
                                          int64_t* step, void* stream) {
   B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_get_adam: a learner group moves its state with get_state / set_state");
-  B200RL_REQUIRE(h && which >= 0 && which < 3 && h->net[which].m && exp_avg && exp_avg_sq && step,
+  B200RL_REQUIRE(h && which >= 0 && which < n_opt(h) && h->net[which].m && exp_avg && exp_avg_sq && step,
                  "offpolicy_get_adam: bad arguments");
   NetBuf& nb = h->net[which];
   B200RL_REQUIRE(n == nb.P_flat, "offpolicy_get_adam: expects %lld floats", (long long)nb.P_flat);
@@ -3131,8 +3263,8 @@ extern "C" int b200rl_offpolicy_get_adam(b200rl_offpolicy* h, int which, float* 
 }
 
 // Whole learner state in ONE call and ONE synchronisation: blob = for every present network 0..5 its parameters, then
-// for every optimizer 0..2 (policy, Q1, Q2) exp_avg and exp_avg_sq; steps[3] = Adam step counts.  A group moves
-// [K][blob] and steps[K][3] with one strided copy (the slab heads every learner's arena).
+// for every optimizer 0..2 (policy, Q1, Q2; IQL: 0..3, V last) exp_avg and exp_avg_sq; steps[n_opt] = Adam step counts.
+// A group moves [K][blob] and steps[K][n_opt] with one strided copy (the slab heads every learner's arena).
 static int64_t state_floats(const b200rl_offpolicy* h) { return h->K * h->state_n; }
 
 extern "C" int64_t b200rl_offpolicy_state_floats(b200rl_offpolicy* h) { return h ? state_floats(h) : -1; }
@@ -3144,8 +3276,9 @@ extern "C" int b200rl_offpolicy_get_state(b200rl_offpolicy* h, float* blob, int6
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200RL_CUDA(cudaMemcpy2DAsync(blob, (size_t)h->state_n * 4, h->state, h->lane_stride, (size_t)h->state_n * 4, h->K,
                                 cudaMemcpyDeviceToHost, s));
+  const int no = n_opt(h);
   for (int z = 0; z < h->K; ++z)
-    for (int i = 0; i < 3; ++i) steps[3 * z + i] = h->net[i].m ? h->net[i].step[z] : 0;
+    for (int i = 0; i < no; ++i) steps[no * z + i] = h->net[i].m ? h->net[i].step[z] : 0;
   B200RL_CUDA(cudaStreamSynchronize(s));
   return 0;
 }
@@ -3154,20 +3287,22 @@ extern "C" int b200rl_offpolicy_set_state(b200rl_offpolicy* h, const float* blob
                                           void* stream) {
   B200RL_REQUIRE(h && blob && steps && n_floats == state_floats(h), "offpolicy_set_state: bad arguments");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int no = n_opt(h);
   for (int z = 0; z < h->K; ++z)
-    for (int i = 0; i < 3; ++i)
-      if (h->net[i].m) B200RL_REQUIRE(steps[3 * z + i] >= 0, "offpolicy_set_state: negative step count");
+    for (int i = 0; i < no; ++i)
+      if (h->net[i].m) B200RL_REQUIRE(steps[no * z + i] >= 0, "offpolicy_set_state: negative step count");
   B200RL_CUDA(cudaMemcpy2DAsync(h->state, h->lane_stride, blob, (size_t)h->state_n * 4, (size_t)h->state_n * 4, h->K,
                                 cudaMemcpyHostToDevice, s));
   for (int z = 0; z < h->K; ++z)
-    for (int i = 0; i < 3; ++i)
-      if (h->net[i].m) h->net[i].step[z] = steps[3 * z + i];
+    for (int i = 0; i < no; ++i)
+      if (h->net[i].m) h->net[i].step[z] = steps[no * z + i];
   B200RL_CUDA(cudaStreamSynchronize(s));  // `blob` may be reused by the caller right away
   return 0;
 }
 
 extern "C" int b200rl_offpolicy_set_sac(b200rl_offpolicy* h, const b200rl_sac_hparams* sp) {
   B200RL_REQUIRE(h && sp, "offpolicy_set_sac: NULL argument");
+  B200RL_REQUIRE(!h->iql, "offpolicy_set_sac: an IQL engine (algo = 9) takes b200rl_offpolicy_set_iql, not set_sac");
   B200RL_REQUIRE(h->sac || h->dsac, "offpolicy_set_sac: the engine was not created with algo = 1 (SAC) or 5 (discrete "
                  "SAC)");
   B200RL_REQUIRE(sp->learn_alpha == 0 || sp->learn_alpha == 1, "offpolicy_set_sac: learn_alpha must be 0 or 1");
@@ -3183,6 +3318,7 @@ extern "C" int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hp
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_dqn: a discrete SAC engine (algo = 5) takes b200rl_offpolicy_set_sac, not "
                  "set_dqn");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_dqn: a TQC engine (algo = 7) takes b200rl_offpolicy_set_sac, not set_dqn");
+  B200RL_REQUIRE(!h->iql, "offpolicy_set_dqn: an IQL engine (algo = 9) takes b200rl_offpolicy_set_iql, not set_dqn");
   B200RL_REQUIRE(h->dqn, "offpolicy_set_dqn: the engine was not created with algo = 2 (DQN)");
   B200RL_REQUIRE(dp->target_update_interval >= 1, "offpolicy_set_dqn: target_update_interval must be >= 1, got %d",
                  dp->target_update_interval);
@@ -3196,6 +3332,7 @@ extern "C" int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hp
   B200RL_REQUIRE(h && cp, "offpolicy_set_c51: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_c51: a discrete SAC engine (algo = 5) has no categorical head");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_c51: a TQC engine (algo = 7) has no categorical head");
+  B200RL_REQUIRE(!h->iql, "offpolicy_set_c51: an IQL engine (algo = 9) has no categorical head");
   B200RL_REQUIRE(!h->d4pg, "offpolicy_set_c51: a D4PG engine (algo = 6) takes its support at create "
                  "(b200rl_offpolicy_create_d4pg)");
   B200RL_REQUIRE(h->c51, "offpolicy_set_c51: the engine was not created with algo = 3 (C51)");
@@ -3226,6 +3363,7 @@ extern "C" int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hp
 extern "C" int b200rl_offpolicy_set_qr(b200rl_offpolicy* h, const b200rl_qr_hparams* qp) {
   B200RL_REQUIRE(h && qp, "offpolicy_set_qr: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_qr: a discrete SAC engine (algo = 5) has no quantile head");
+  B200RL_REQUIRE(!h->iql, "offpolicy_set_qr: an IQL engine (algo = 9) has no quantile head");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_qr: a TQC engine (algo = 7) takes its quantile counts at create "
                  "(b200rl_offpolicy_create_tqc)");
   B200RL_REQUIRE(h->dqn && !h->c51 && !h->iqn, "offpolicy_set_qr: the engine was not created with algo = 2 (DQN)");
@@ -3248,6 +3386,7 @@ extern "C" int b200rl_offpolicy_set_per(b200rl_offpolicy* h, const b200rl_per_hp
                  "5)");
   B200RL_REQUIRE(!h->c51, "offpolicy_set_per: prioritized replay is not implemented for C51 engines");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_per: prioritized replay is not implemented for TQC engines (algo = 7)");
+  B200RL_REQUIRE(!h->iql, "offpolicy_set_per: prioritized replay is not implemented for IQL engines (algo = 9)");
   B200RL_REQUIRE(h->dqn || h->d4pg, "offpolicy_set_per: prioritized replay is implemented for DQN engines (algo = 2) "
                  "and D4PG engines (algo = 6) only");
   B200RL_REQUIRE(pp->alpha >= 0.0 && std::isfinite(pp->alpha), "offpolicy_set_per: alpha must be >= 0");
@@ -3264,6 +3403,7 @@ extern "C" int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, c
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_nstep: n-step returns are not implemented for discrete SAC engines (algo = "
                  "5)");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_nstep: n-step returns are not implemented for TQC engines (algo = 7)");
+  B200RL_REQUIRE(!h->iql, "offpolicy_set_nstep: n-step returns are not implemented for IQL engines (algo = 9)");
   B200RL_REQUIRE(h->dqn || h->d4pg, "offpolicy_set_nstep: n-step returns are implemented for DQN and C51 engines "
                  "(algo = 2 or 3) and D4PG engines (algo = 6) only");
   B200RL_REQUIRE(n_step >= 1 && n_step <= NSTEP_MAX, "offpolicy_set_nstep: n_step must be 1..%d, got %d", NSTEP_MAX,
@@ -3286,6 +3426,7 @@ extern "C" int b200rl_offpolicy_set_noise_keys(b200rl_offpolicy* h, const uint64
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_noise_keys: a discrete SAC engine (algo = 5) draws no noise");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_noise_keys: a TQC engine (algo = 7) has no noisy layers; its policy's draws "
                  "come with the train call");
+  B200RL_REQUIRE(!h->iql, "offpolicy_set_noise_keys: an IQL engine (algo = 9) draws no noise");
   B200RL_REQUIRE(h->noisy || h->iqn, "offpolicy_set_noise_keys: the engine has no noisy layers (config noisy_layers = "
                  "0)");
   const size_t n = adam_tab_len(h);
@@ -3373,6 +3514,7 @@ extern "C" int b200rl_offpolicy_sac_outputs(b200rl_offpolicy* h, int32_t S, floa
 
 extern "C" int b200rl_offpolicy_set_cql(b200rl_offpolicy* h, const b200rl_cql_hparams* cp) {
   B200RL_REQUIRE(h && cp, "offpolicy_set_cql: NULL argument");
+  B200RL_REQUIRE(!h->iql, "offpolicy_set_cql: an IQL engine (algo = 9) takes b200rl_offpolicy_set_iql, not set_cql");
   B200RL_REQUIRE(h->cql, "offpolicy_set_cql: the engine was not created with algo = 8 (CQL)");
   B200RL_REQUIRE(std::isfinite(cp->weight) && cp->weight >= 0.0, "offpolicy_set_cql: weight must be finite and >= 0, "
                  "got %g", cp->weight);
@@ -3432,6 +3574,38 @@ extern "C" int b200rl_offpolicy_cql_outputs(b200rl_offpolicy* h, int32_t S, floa
   B200RL_CUDA(cudaStreamSynchronize(h->gs));
   if (!h->cql_cfg.lagrange)
     for (size_t i = 0; i < (size_t)h->K * S; ++i) alpha_primes[i] = 1.f;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_set_iql(b200rl_offpolicy* h, const b200rl_iql_hparams* ip) {
+  B200RL_REQUIRE(h && ip, "offpolicy_set_iql: NULL argument");
+  B200RL_REQUIRE(h->iql, "offpolicy_set_iql: the engine was not created with algo = 9 (IQL)");
+  B200RL_REQUIRE(ip->expectile > 0.0 && ip->expectile < 1.0, "offpolicy_set_iql: expectile must be in (0, 1), got %g",
+                 ip->expectile);
+  B200RL_REQUIRE(std::isfinite(ip->beta) && ip->beta >= 0.0, "offpolicy_set_iql: beta must be finite and >= 0, got %g",
+                 ip->beta);
+  B200RL_REQUIRE(std::isfinite(ip->max_weight) && ip->max_weight > 0.0, "offpolicy_set_iql: max_weight must be finite "
+                 "and > 0, got %g", ip->max_weight);
+  B200RL_REQUIRE(std::isfinite(ip->log_std_min) && std::isfinite(ip->log_std_max) && ip->log_std_min < ip->log_std_max,
+                 "offpolicy_set_iql: the log-std bounds need finite log_std_min < log_std_max, got [%g, %g]",
+                 ip->log_std_min, ip->log_std_max);
+  B200RL_REQUIRE(std::isfinite(ip->v_lr) && std::isfinite(ip->v_beta1) && std::isfinite(ip->v_beta2) &&
+                 std::isfinite(ip->v_eps), "offpolicy_set_iql: non-finite Adam settings of the value network");
+  h->iql_hp = *ip;
+  h->iql_set = true;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_iql_outputs(b200rl_offpolicy* h, int32_t S, float* value_losses, float* value_means,
+                                            float* weight_means) {
+  B200RL_REQUIRE(h && h->iql && value_losses && value_means && weight_means && S >= 0 && S <= h->cfg.max_steps,
+                 "offpolicy_iql_outputs: bad arguments");
+  const size_t w = (size_t)S * 4;
+  float* dst[3] = {value_losses, value_means, weight_means};
+  const float* src[3] = {h->out_vl, h->out_vm, h->out_wm};
+  for (int k = 0; k < 3 && S > 0; ++k)
+    B200RL_CUDA(cudaMemcpy2DAsync(dst[k], w, src[k], h->lane_stride, w, h->K, cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
   return 0;
 }
 
@@ -3927,6 +4101,97 @@ static int enqueue_dsac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparam
   return 0;
 }
 
+// The S IQL steps (b200rl.h, "IQL": value step, policy step with the new V, critic step with the new V, polyak).  Per
+// step the branches are:
+//   s  : Q1targ(s, a) -> V(s) -+-> value head -> V bwd, Adam -> V'(s) -+----------------+-> Q1 head -> Q1 bwd, Adam -+->
+//   s2 : Q2targ(s, a) ---------+   (V's dW products)  -> V'(s') ------|----------------+-> Q2 head -> Q2 bwd, Adam -+
+//   s3 : pi(s) ........................................................+-> AWR head -> pi bwd, Adam ..................+
+//   s4 : Q1(s, a) -> Q2(s, a) (pre-update, the logged Q-values) ........................ Q2's dW products
+// then polyak on s.  No network needs an input gradient: every backward pass is the weight-gradient products and the
+// dX chain down to the first hidden layer.  The policy and critic branches share nothing but what they read, so each
+// backward pass has a gradient ping-pong of its own (pi dbuf0/1, Q2 dbuf2/3, Q1 dbuf4/5).
+static int enqueue_iql_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s) {
+  const int O = h->O, A = h->A;
+  const int maxS = h->cfg.max_steps;
+  const b200rl_iql_hparams& ip = h->iql_hp;
+  NetBuf &pi = h->net[0], &q1 = h->net[1], &q2 = h->net[2], &vn = h->net[3], &q1t = h->net[4], &q2t = h->net[5];
+  const int Lq = q1.d.n_layers, Lp = pi.d.n_layers, Lv = vn.d.n_layers;
+  const int ew = 256;
+  cudaStream_t s2 = h->s2, s3 = h->s3, s4 = h->s4;
+  PolyakArgs pk{};  // 1 -> 4, 2 -> 5
+  pk.n_nets = 2;
+  for (int k = 0; k < 2; ++k) {
+    pk.target[k] = h->net[4 + k].params;
+    pk.param[k] = h->net[1 + k].params;
+    pk.n[k] = (int)h->net[1 + k].P;
+  }
+  for (int st = 0; st < S; ++st) {
+    float* s_obs = h->obs + (size_t)st * B * O;
+    const float* s_act = h->act + (size_t)st * B * A;
+    const float* s_rew = h->rew + (size_t)st * B;
+    float* s_nobs = h->nobs + (size_t)st * B * O;
+    const float* s_done = h->done + (size_t)st * B;
+    float *qa[2][B200RL_MAX_LAYERS + 1], *tq[2][B200RL_MAX_LAYERS + 1];
+    float *pa[B200RL_MAX_LAYERS + 1], *va[B200RL_MAX_LAYERS + 1], *vn2[B200RL_MAX_LAYERS + 1];
+    for (int qi = 0; qi < 2; ++qi) {
+      qa[qi][0] = tq[qi][0] = s_obs;
+      for (int l = 1; l <= Lq; ++l) qa[qi][l] = h->acts[qi == 0 ? 1 : 4][l];
+      for (int l = 1; l < Lq; ++l) tq[qi][l] = qi == 0 ? h->acts_tq[l] : h->acts[3][l];
+      tq[qi][Lq] = qi == 0 ? h->qt1 : h->qt2;
+    }
+    pa[0] = va[0] = s_obs;
+    vn2[0] = s_nobs;
+    for (int l = 1; l <= Lp; ++l) pa[l] = h->acts[2][l];
+    for (int l = 1; l <= Lv; ++l) va[l] = h->acts[0][l], vn2[l] = h->acts[3][l];  // stack 3 is free once Q2targ is read
+    // ---- the step's start: the critics (logged), pi(s), both target critics and V(s), all at (s, a) ----
+    if (edge(h, s, s2) || edge(h, s, s3) || edge(h, s, s4)) return 1;
+    if (net_forward(h, q1, qa[0], B, s4, s_act, A, O) || net_forward(h, q2, qa[1], B, s4, s_act, A, O)) return 1;
+    if (net_forward(h, pi, pa, B, s3)) return 1;
+    if (net_forward(h, q2t, tq[1], B, s2, s_act, A, O)) return 1;
+    if (net_forward(h, q1t, tq[0], B, s, s_act, A, O) || net_forward(h, vn, va, B, s)) return 1;
+    if (edge(h, s2, s)) return 1;
+    // ---- value step: expectile head, V's backward pass and Adam, then V'(s) and V'(s') ----
+    if (launch(h, iql_value_loss_kernel<false>, iql_value_loss_kernel<true>, 1, GTHREADS, 0, s, h->qt1, h->qt2, va[Lv],
+               (float)ip.expectile, (float)(1.0 - ip.expectile), B, h->iql_dv, h->out_vl + st, h->out_vm + st))
+      return 1;
+    if (net_backward(h, vn, va, h->iql_dv, 1, B, true, nullptr, s, 0, nullptr, 0, 0, s2)) return 1;
+    if (adam_net(h, vn, h->adam_tab + (size_t)3 * maxS, st, ip.v_beta1, ip.v_beta2, ip.v_eps, s)) return 1;
+    if (edge(h, s, s2)) return 1;
+    if (net_forward(h, vn, vn2, B, s2)) return 1;
+    if (net_forward(h, vn, va, B, s)) return 1;
+    // ---- policy step on s3: the AWR head with V'(s), pi's backward pass and Adam ----
+    if (edge(h, s, s3)) return 1;
+    if (launch(h, iql_policy_loss_kernel<false>, iql_policy_loss_kernel<true>, 1, GTHREADS, 0, s3, pa[Lp], s_act,
+               h->qt1, h->qt2, va[Lv], B, A, (float)ip.beta, (float)ip.max_weight, (float)ip.log_std_min,
+               (float)ip.log_std_max, (float)hp->action_limit, h->iql_dout, h->out_lp + st, h->out_wm + st))
+      return 1;
+    if (net_backward(h, pi, pa, h->iql_dout, 2 * A, B, true, nullptr, s3, 0)) return 1;
+    if (adam_net(h, pi, h->adam_tab, st, hp->policy_beta1, hp->policy_beta2, hp->policy_eps, s3)) return 1;
+    // ---- critic step: y = r + gamma (1 - d) V'(s') in each head (both target inputs V'(s'), temperature 0),
+    // weight-gradient backward, Adam (Q2 on s2, Q1 on s) ----
+    if (edge(h, s4, s) || edge(h, s2, s) || edge(h, s, s2)) return 1;
+    for (int qi = 1; qi >= 0; --qi) {
+      NetBuf& qn = qi == 0 ? q1 : q2;
+      cudaStream_t qs = qi == 0 ? s : s2;
+      float* dq = qi == 0 ? h->dq : h->dq2;
+      if (launch(h, sac_q_loss_kernel<false>, sac_q_loss_kernel<true>, 1, GTHREADS, 0, qs, qa[qi][Lq], s_rew, s_done,
+                 vn2[Lv], vn2[Lv], h->iql_zero, h->iql_zero, (float)hp->gamma, B, dq,
+                 (qi == 0 ? h->out_l1 : h->out_l2) + st, (qi == 0 ? h->out_q1 : h->out_q2) + (size_t)st * B))
+        return 1;
+      if (net_backward(h, qn, qa[qi], dq, 1, B, true, nullptr, qs, qi == 0 ? 2 : 1, s_act, A, O,
+                       qi == 0 ? nullptr : s4))
+        return 1;
+      if (adam_net(h, qn, h->adam_tab + (size_t)(1 + qi) * maxS, st, hp->q_beta1, hp->q_beta2, hp->q_eps, qs)) return 1;
+    }
+    if (edge(h, s2, s)) return 1;
+    if (launch(h, polyak_kernel<false>, polyak_kernel<true>, (pk.n[0] + ew - 1) / ew, ew, 0, s, pk,
+               (float)hp->polyak_rho, (float)(1.0 - hp->polyak_rho)))
+      return 1;
+    if (edge(h, s3, s)) return 1;
+  }
+  return 0;
+}
+
 // dqn_loss_kernel<LANES, WEIGHTED, NSTEP> of a call: WEIGHTED for prioritized replay, NSTEP for n-step returns
 template <bool LANES>
 static auto dqn_head(bool weighted, bool nstep) {
@@ -4097,6 +4362,10 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
 // The step program of the engine's algorithm on `s` (plain launches or under stream capture); *n_pol = its policy steps
 static int enqueue_program(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s,
                            int* n_pol) {
+  if (h->iql) {
+    *n_pol = S;
+    return enqueue_iql_steps(h, hp, S, B, s);
+  }
   if (h->sac) {
     *n_pol = S;
     return enqueue_sac_steps(h, hp, S, B, s);
@@ -4123,7 +4392,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   // Adam's step-dependent scalars for the steps of this call (torch's host-side double arithmetic), one small upload
   // (a group: one table per learner, from that learner's step counts, uploaded with one strided copy)
   const int maxS = h->cfg.max_steps;
-  const int n_pol_expected = h->dqn ? 0 : h->sac || h->dsac ? S : (S + hp->policy_delay - 1) / hp->policy_delay;  // SAC: no delay
+  const int n_pol_expected = h->dqn ? 0 : h->sac || h->dsac || h->iql ? S : (S + hp->policy_delay - 1) / hp->policy_delay;  // SAC: no delay
   const size_t tab_n = adam_tab_len(h);
   const bool learn_alpha = (h->sac || h->dsac) && h->sac_hp.learn_alpha;
   const bool lagrange = h->cql && h->cql_cfg.lagrange;
@@ -4138,6 +4407,10 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
     if (learn_alpha)
       for (int k = 0; k < S; ++k)
         adam_scalars(h->alpha_step[z] + k + 1, h->sac_hp.alpha_lr, h->sac_hp.alpha_beta1, h->sac_hp.alpha_beta2,
+                     &tab[(size_t)3 * maxS + k].x, &tab[(size_t)3 * maxS + k].y);
+    if (h->iql)
+      for (int k = 0; k < S; ++k)
+        adam_scalars(h->net[3].step[z] + k + 1, h->iql_hp.v_lr, h->iql_hp.v_beta1, h->iql_hp.v_beta2,
                      &tab[(size_t)3 * maxS + k].x, &tab[(size_t)3 * maxS + k].y);
     if (lagrange)
       for (int k = 0; k < S; ++k)
@@ -4167,6 +4440,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
     key.S = S, key.B = B, key.nstep = h->nstep;
     key.hp = *hp, key.sac = h->sac_hp, key.dqn = h->dqn_hp, key.c51 = h->c51_hp, key.qr = h->qr_hp;
     key.cql = h->cql_hp;
+    key.iql = h->iql_hp, key.iql.v_lr = 0.0;
     if (h->per_run) key.per = h->per_hp, key.replay = h->replay;
     if (h->graph == nullptr || memcmp(&key, &h->graph_key, sizeof(key)) != 0) {
       if (h->graph) {
@@ -4205,6 +4479,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
     if (td3) h->net[2].step[z] += S;
     if (learn_alpha) h->alpha_step[z] += S;
     if (lagrange) h->ap_step[z] += S;
+    if (h->iql) h->net[3].step[z] += S;
   }
   // one device -> host read of everything train() logs: [K, S, B] values, [K, S] losses
   const size_t ls = h->lane_stride, K = (size_t)h->K;
@@ -4260,6 +4535,11 @@ static int train_begin(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, 
     B200RL_REQUIRE(noise_given, "%s: SAC needs the noise draws [S, 2, B, A]", what);
   }
   B200RL_REQUIRE(!h->cql || h->cql_set, "%s: a CQL engine needs b200rl_offpolicy_set_cql before it trains", what);
+  if (h->iql) {
+    B200RL_REQUIRE(h->iql_set, "%s: an IQL engine needs b200rl_offpolicy_set_iql before it trains", what);
+    B200RL_REQUIRE(!hp->use_target_noise && !noise_given, "%s: an IQL engine draws no noise: use_target_noise must be "
+                   "0 and the noise NULL", what);
+  }
   B200RL_REQUIRE(!h->dsac || h->sac_set, "%s: a discrete SAC engine needs b200rl_offpolicy_set_sac before it trains",
                  what);
   if (h->dqn) {
@@ -4421,7 +4701,7 @@ extern "C" int b200rl_offpolicy_train_gather_rng_group(b200rl_offpolicy* h, cons
     }
     return 0;
   };
-  if (int rc = train_begin(h, hp, S, B, true, q2_values && q2_losses, n_policy_updates, stream,
+  if (int rc = train_begin(h, hp, S, B, !h->iql, q2_values && q2_losses, n_policy_updates, stream,  // IQL: indices only
                            "offpolicy_train_gather_rng", own))
     return rc < 0 ? 0 : rc;
   set_replay(h, rb, nullptr);
@@ -4474,6 +4754,7 @@ extern "C" int b200rl_offpolicy_get_draws(b200rl_offpolicy* h, int32_t S, int32_
   const size_t SB = (size_t)S * B;
   static_assert(sizeof(long long) == sizeof(int64_t), "index width");
   const size_t n_eps = (h->sac ? 2 : 1) * SB * h->A;
+  B200RL_REQUIRE(!h->iql || noise == nullptr, "offpolicy_get_draws: an IQL engine draws no noise: noise must be NULL");
   B200RL_CUDA(cudaMemcpy2DAsync(idx, SB * 8, h->idx, h->lane_stride, SB * 8, h->K, cudaMemcpyDeviceToHost, s));
   if (noise)
     B200RL_CUDA(cudaMemcpy2DAsync(noise, n_eps * 4, h->eps, h->lane_stride, n_eps * 4, h->K, cudaMemcpyDeviceToHost, s));
@@ -4494,6 +4775,8 @@ extern "C" int b200rl_offpolicy_train_prioritized_group(b200rl_offpolicy* h, con
                  "engines (algo = 5)");
   B200RL_REQUIRE(!h->tqc, "offpolicy_train_prioritized: prioritized replay is not implemented for TQC engines (algo = "
                  "7)");
+  B200RL_REQUIRE(!h->iql, "offpolicy_train_prioritized: prioritized replay is not implemented for IQL engines (algo = "
+                 "9)");
   B200RL_REQUIRE(h->dqn || h->d4pg, "offpolicy_train_prioritized: prioritized replay is implemented for DQN engines "
                  "(algo = 2) and D4PG engines (algo = 6) only");
   B200RL_REQUIRE(h->per_set, "offpolicy_train_prioritized: call b200rl_offpolicy_set_per first");

@@ -339,14 +339,17 @@ class OffPolicyEngine:
     TQC (``algo`` 7) is a SAC engine whose critics map [s | a] to M quantiles: ``q_sizes`` = [obs + act, ..., M] and
     ``tqc`` = (M, d), d the atoms per critic dropped from the pooled target (b200rl.h, "TQC").  CQL (``algo`` 8) is a SAC
     engine whose critic step also runs on 3N sampled actions per row: ``cql`` = (N, lagrange); ``set_cql`` is required,
-    and a call with host draws takes ``noise`` = (SAC's [S, 2, B, A], CQL's [S, 3, B, N, A]) (b200rl.h, "CQL").
+    and a call with host draws takes ``noise`` = (SAC's [S, 2, B, A], CQL's [S, 3, B, N, A]) (b200rl.h, "CQL").  IQL
+    (``algo`` 9) has SAC's policy and critics and a trained value network in slot 3: ``iql`` = (sizes, (hidden, out
+    activation)) of V; ``set_iql`` is required, no noise is used, and the state has four optimizers (b200rl.h, "IQL").
 
     ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
     launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
-    is [K][per-learner blob] with [K][3] step counts, and the per-network accessors are refused."""
+    is [K][per-learner blob] with [K][n_opt] step counts (n_opt = 3, 4 for IQL), and the per-network accessors are
+    refused."""
 
     NETS = {"policy": 0, "q1": 1, "q2": 2, "target_policy": 3, "target_q1": 4, "target_q2": 5}
-    TD3, SAC, DQN, C51, IQN, DSAC, D4PG, TQC, CQL = 0, 1, 2, 3, 4, 5, 6, 7, 8
+    TD3, SAC, DQN, C51, IQN, DSAC, D4PG, TQC, CQL, IQL = 0, 1, 2, 3, 4, 5, 6, 7, 8, 9
     DISCRETE = (DQN, C51, IQN)  # the algos with DQN's networks, inputs and outputs
     INDEX_ACTIONS = DISCRETE + (DSAC,)  # the algos whose action column holds an action index
     SOFT = (SAC, DSAC, TQC, CQL)  # the algos with SAC's networks, temperature and outputs
@@ -354,7 +357,7 @@ class OffPolicyEngine:
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
                  q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1, dueling_k: int = 0,
-                 noisy_layers: int = 0, iqn=None, d4pg=None, tqc=None, cql=None):
+                 noisy_layers: int = 0, iqn=None, d4pg=None, tqc=None, cql=None, iql=None):
         from ._lib import OffPolicyConfig
         self.lib = _lib.load()
         current_stream_handle()
@@ -369,6 +372,9 @@ class OffPolicyEngine:
         self.d4pg = None if d4pg is None else (int(d4pg[0]), float(d4pg[1]), float(d4pg[2]))
         self.tqc = None if tqc is None else (int(tqc[0]), int(tqc[1]))
         self.cql = None if cql is None else (int(cql[0]), int(bool(cql[1])))
+        self.iql = None if iql is None else (tuple(int(x) for x in iql[0]), tuple(iql[1]))
+        self.n_opt = 4 if self.iql is not None else 3  # optimizers in the state blob and the step counts
+        self.n_value = 0
         self.discrete = self.algo in self.DISCRETE  # DQN's networks and outputs
         self.index_actions = self.algo in self.INDEX_ACTIONS  # act [S,B] indices, no noise
         self.n_q, self.max_minibatch, self.max_steps = int(n_q), int(max_minibatch), int(max_steps)
@@ -397,6 +403,11 @@ class OffPolicyEngine:
         elif self.tqc is not None:  # the quantile counts size the critics' heads (b200rl.h, "TQC")
             check(self.lib.b200rl_offpolicy_create_tqc(C.byref(cfg), C.byref(_lib.TqcConfig(*self.tqc)), self.K,
                                                        C.byref(h)), "offpolicy_create_tqc")
+        elif self.iql is not None:  # the value network's description (b200rl.h, "IQL")
+            vdesc = MlpDesc.make(list(self.iql[0]), *self.iql[1])
+            self.n_value = int(self.lib.b200rl_mlp_param_count(vdesc))
+            check(self.lib.b200rl_offpolicy_create_iql(C.byref(cfg), C.byref(_lib.IqlConfig(vdesc)), self.K,
+                                                       C.byref(h)), "offpolicy_create_iql")
         elif self.cql is not None:  # N and the Lagrange switch size the buffers (b200rl.h, "CQL")
             check(self.lib.b200rl_offpolicy_create_cql(C.byref(cfg), C.byref(_lib.CqlConfig(*self.cql)), self.K,
                                                        C.byref(h)), "offpolicy_create_cql")
@@ -424,6 +435,8 @@ class OffPolicyEngine:
             pass
 
     def _n(self, which):
+        if which == 3 and self.iql is not None:
+            return self.n_value
         return self.n_policy if which in (0, 3) else self.n_qp
 
     def set_params(self, which: int, flat: np.ndarray):
@@ -454,15 +467,15 @@ class OffPolicyEngine:
 
     # ---- whole state in one transfer ----
     def state_layout(self):
-        """[(kind, net index, offset, count)] of one learner's state blob: ("params", 0..5) then ("m" / "v", 0..2);
-        every segment starts on a multiple of 64 floats (b200rl.h).  A group's blob is K of these back to back."""
+        """[(kind, net index, offset, count)] of one learner's state blob: ("params", 0..5) then ("m" / "v", 0..2; IQL
+        0..3); every segment starts on a multiple of 64 floats (b200rl.h).  A group's blob is K of these back to back."""
         pad = lambda n: (n + 63) & ~63
         if self.discrete:
             present, optimized = [1, 4], [1]
         else:
             present = [0, 1] + ([2] if self.n_q == 2 else []) + ([] if self.algo in self.SOFT else [3]) + [4] + \
                 ([5] if self.n_q == 2 else [])
-            optimized = [0, 1] + ([2] if self.n_q == 2 else [])
+            optimized = [0, 1] + ([2] if self.n_q == 2 else []) + ([3] if self.iql is not None else [])
         out, off = [], 0
         for i in present:
             out.append(("params", i, off, self._n(i)))
@@ -490,24 +503,26 @@ class OffPolicyEngine:
         return buf
 
     def get_state(self):
-        """Device -> the persistent blob; returns (blob as numpy view, [3 Adam step counts]; a group: [K][3])."""
+        """Device -> the persistent blob; returns (blob as numpy view, [n_opt Adam step counts]; a group: [K][n_opt])."""
         buf = self.state_buffer()
-        steps = (C.c_int64 * (3 * self.K))()
+        n = self.n_opt
+        steps = (C.c_int64 * (n * self.K))()
         check(self.lib.b200rl_offpolicy_get_state(self.h, C.c_void_p(buf.data_ptr()), buf.numel(), steps,
                                                   current_stream_handle()), "get_state")
         st = [int(x) for x in steps]
-        return buf.numpy(), st if self.K == 1 else [st[3 * z:3 * z + 3] for z in range(self.K)]
+        return buf.numpy(), st if self.K == 1 else [st[n * z:n * z + n] for z in range(self.K)]
 
     def set_state(self, blob, steps):
         """``blob`` = None sends the persistent blob (fill ``state_buffer()`` first), else any float32 array of that size.
-        ``steps``: [3] Adam step counts (a group: [K][3])."""
+        ``steps``: [n_opt] Adam step counts (a group: [K][n_opt])."""
         buf = self.state_buffer()
         if blob is not None and not (isinstance(blob, np.ndarray) and blob.ctypes.data == buf.data_ptr()):
             buf.numpy()[:] = np.asarray(blob, dtype=np.float32).reshape(-1)
         flat = np.asarray(steps, dtype=np.int64).reshape(-1)
-        if flat.size != 3 * self.K:
-            raise ValueError(f"set_state: expected {3 * self.K} step counts, got {flat.size}")
-        st = (C.c_int64 * (3 * self.K))(*[int(x) for x in flat])
+        n = self.n_opt * self.K
+        if flat.size != n:
+            raise ValueError(f"set_state: expected {n} step counts, got {flat.size}")
+        st = (C.c_int64 * n)(*[int(x) for x in flat])
         check(self.lib.b200rl_offpolicy_set_state(self.h, C.c_void_p(buf.data_ptr()), buf.numel(), st,
                                                   current_stream_handle()), "set_state")
 
@@ -541,6 +556,22 @@ class OffPolicyEngine:
         st = np.zeros(self.K, np.int64)
         check(self.lib.b200rl_offpolicy_get_alpha_group(self.h, _ptr(la), _ptr(m), _ptr(v), _ptr(st)), "get_alpha")
         return [(float(la[z]), float(m[z]), float(v[z]), int(st[z])) for z in range(self.K)]
+
+    # ---- IQL ----
+    def set_iql(self, expectile: float, beta: float, max_weight: float, log_std_min: float, log_std_max: float,
+                v_lr: float, v_betas=(0.9, 0.999), v_eps: float = 1e-8) -> None:
+        """The expectile, the AWR inverse temperature and weight cap, the policy's log-std clamp and the value
+        network's Adam settings (b200rl.h, "IQL")."""
+        ip = _lib.IqlHparams(float(expectile), float(beta), float(max_weight), float(log_std_min), float(log_std_max),
+                             float(v_lr), float(v_betas[0]), float(v_betas[1]), float(v_eps))
+        check(self.lib.b200rl_offpolicy_set_iql(self.h, C.byref(ip)), "set_iql")
+
+    def iql_outputs(self, S: int):
+        """(value losses [S], mean V(s) before each value step [S], mean AWR weight [S]) of the last train call; a
+        group: each [K, S]."""
+        out = tuple(np.zeros((self.K, S), np.float32) for _ in range(3))
+        check(self.lib.b200rl_offpolicy_iql_outputs(self.h, int(S), *[_ptr(x) for x in out]), "iql_outputs")
+        return tuple(x[0] for x in out) if self.K == 1 else out
 
     # ---- CQL ----
     def set_cql(self, weight: float, temperature: float, target_action_gap: float = 0.0, alpha_lr: float = 3e-4,
@@ -753,6 +784,8 @@ class OffPolicyEngine:
             out["log_prob_means"], out["alphas"] = self.sac_outputs(S)
         if self.algo == self.CQL:
             out["cql_gap_1"], out["cql_gap_2"], out["alpha_primes"] = self.cql_outputs(S)
+        if self.algo == self.IQL:
+            out["value_losses"], out["value_means"], out["weight_means"] = self.iql_outputs(S)
         return out
 
     def _lead(self, a, dtype, ndim):
@@ -805,7 +838,7 @@ class OffPolicyEngine:
         """(physical rows [S,B] int64, noise [S,B,A] (SAC: [S,2,B,A]) float32 or None) of the last train_gather /
         train_gather_rng call; a group: both with a leading [K] axis."""
         idx = np.empty((self.K, S, B), np.int64)
-        with_noise = with_noise and not self.index_actions  # DQN, C51 and discrete SAC draw indices only
+        with_noise = with_noise and not self.index_actions and self.algo != self.IQL  # these draw indices only
         noise = None
         if with_noise and self.algo in self.SQUASHED:
             noise = np.empty((self.K, S, 2, B, self.policy_sizes[-1] // 2), np.float32)

@@ -1,6 +1,7 @@
 from .base import (CategoricalPolicy, DeterministicPolicy, EpsilonGreedyPolicy, GaussianPolicy, GreedyPolicy,
-                   NoisyGreedyPolicy, Policy, RandomPolicy, SquashedGaussianPolicy, StochasticPolicy)
+                   NoisyGreedyPolicy, Policy, RandomPolicy, SquashedGaussianPolicy, StochasticPolicy,
+                   TanhMeanGaussianPolicy)
 
-__all__ = ["Policy", "StochasticPolicy", "CategoricalPolicy", "GaussianPolicy", "SquashedGaussianPolicy",
+__all__ = ["Policy", "StochasticPolicy", "CategoricalPolicy", "GaussianPolicy", "SquashedGaussianPolicy", "TanhMeanGaussianPolicy",
            "DeterministicPolicy", "RandomPolicy", "GreedyPolicy", "EpsilonGreedyPolicy",
            "NoisyGreedyPolicy"]

@@ -116,6 +116,53 @@ class _SquashedMeanPolicy(Policy):
         return np.asarray(self.get_action_tensor(torch.from_numpy(observation).float()).numpy())
 
 
+class TanhMeanGaussianPolicy(StochasticPolicy):
+    """IQL's actor: network(obs) = [m | l] (2A outputs, Identity output), a diagonal Gaussian with mean
+    action_limit * tanh(m) and log std clamp(l, log_std_min, log_std_max).  Its mean is bounded by tanh, but a sample is
+    not squashed: ``log_prob`` of a dataset action at +-action_limit needs no atanh.  Acting samples and clips to
+    [-action_limit, action_limit]; ``deterministic()`` acts with action_limit * tanh(m), the action SAC's evaluation
+    policy takes from the same network.  The default bounds are IQL's reference implementation's."""
+
+    def __init__(self, network: nn.Module, optimizer: Optimizer, action_limit: float = 1.0, log_std_min: float = -5.0,
+                 log_std_max: float = 2.0):
+        super().__init__()
+        self.network = network
+        self.optimizer = optimizer
+        self.action_limit, self.log_std_min, self.log_std_max = float(action_limit), float(log_std_min), float(log_std_max)
+
+    def forward(self, observation: Tensor) -> Independent:
+        out = self.network(observation)
+        A = out.shape[-1] // 2
+        mu = self.action_limit * torch.tanh(out[..., :A])
+        log_std = torch.clamp(out[..., A:], self.log_std_min, self.log_std_max)
+        return Independent(Normal(mu, torch.exp(log_std)), 1)
+
+    def log_prob(self, observation: Tensor, action: Tensor) -> Tensor:
+        """sum_j Normal(mu_j, sigma_j).log_prob(action_j)."""
+        return self.forward(observation).log_prob(action)
+
+    def get_action_tensor(self, observation: Tensor) -> Tensor:
+        with torch.no_grad():
+            return torch.clamp(self.forward(observation).sample(), -self.action_limit, self.action_limit)
+
+    def deterministic(self) -> "Policy":
+        """A view that acts with action_limit * tanh(m) (evaluation); it shares this policy's network."""
+        return _TanhMeanPolicy(self)
+
+
+class _TanhMeanPolicy(Policy):
+    def __init__(self, policy: TanhMeanGaussianPolicy):
+        super().__init__()
+        self.policy = policy
+
+    def get_action_tensor(self, observation: Tensor) -> Tensor:
+        with torch.no_grad():
+            return self.policy.forward(observation).mean
+
+    def get_action_numpy(self, observation: np.ndarray) -> np.ndarray:
+        return np.asarray(self.get_action_tensor(torch.from_numpy(observation).float()).numpy())
+
+
 class DeterministicPolicy(Policy):
     """ref: policies/deterministic_policy.py:9-45"""
 

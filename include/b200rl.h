@@ -345,7 +345,8 @@ typedef struct {
                             * "Discrete SAC" below), 6 = D4PG (created by b200rl_offpolicy_create_d4pg only; see
                             * "D4PG" below), 7 = TQC (created by b200rl_offpolicy_create_tqc only; see "TQC" below),
                             * 8 = CQL (created by b200rl_offpolicy_create_cql only; see "CQL" below), 9 = IQL
-                            * (created by b200rl_offpolicy_create_iql only; see "IQL" below) */
+                            * (created by b200rl_offpolicy_create_iql only; see "IQL" below), 10 = REDQ (created
+                            * by b200rl_offpolicy_create_redq only; see "REDQ" below) */
   int32_t dueling_k;       /* 0 = the Q network is a plain MLP; K >= 1 = a dueling Q network (algo 2 / 3 only; see
                             * "Dueling Q networks" below) */
   int32_t noisy_layers;    /* bit mask over the Q network's Linear layers in flat order: 0 = none; bit l = layer l is a
@@ -365,7 +366,7 @@ int b200rl_offpolicy_create(const b200rl_offpolicy_config* cfg, b200rl_offpolicy
 void b200rl_offpolicy_destroy(b200rl_offpolicy* h);
 int b200rl_offpolicy_set_params(b200rl_offpolicy* h, int which, const float* host_flat, int64_t n, void* stream);
 int b200rl_offpolicy_get_params(b200rl_offpolicy* h, int which, float* host_flat, int64_t n, void* stream);
-/* which: 0 policy, 1 Q1, 2 Q2 optimizers (and 3 V on an IQL engine) */
+/* which: 0 policy, 1 Q1, 2 Q2 optimizers (and 3 V on an IQL engine; 1..N the critics on a REDQ engine) */
 int b200rl_offpolicy_set_adam(b200rl_offpolicy* h, int which, const float* exp_avg, const float* exp_avg_sq, int64_t n,
                               int64_t step, void* stream);
 int b200rl_offpolicy_get_adam(b200rl_offpolicy* h, int which, float* exp_avg, float* exp_avg_sq, int64_t n,
@@ -911,6 +912,64 @@ int b200rl_offpolicy_set_iql(b200rl_offpolicy* h, const b200rl_iql_hparams* hp);
 /* value_losses, value_means and weight_means [K][S] of the last train call's steps. */
 int b200rl_offpolicy_iql_outputs(b200rl_offpolicy* h, int32_t S, float* value_losses, float* value_means,
                                  float* weight_means);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * REDQ on the same engine (config algo = 10, n_q = 2; Chen, Wang, Zhou & Ross 2021, "Randomized Ensembled Double
+ * Q-Learning"): SAC's squashed-Gaussian policy over an ensemble of N critics whose target takes the min over a random
+ * subset of M target critics.  Created by b200rl_offpolicy_create_redq from a config with algo = 10 and a
+ * b200rl_redq_config {N, M}, 2 <= N <= 32, 1 <= M <= N; create and create_group refuse algo 10.
+ * Networks: 0 the policy [obs, ..., 2A], 1..N the critics [obs + A, ..., 1], N+1..2N their targets.  Optimizers: 0
+ * the policy, 1..N the critics.  The state blob is networks 0..2N in that order, then exp_avg / exp_avg_sq of
+ * optimizers 0..N, each segment padded as above; steps is [K][1 + N]; set_params / get_params / set_adam / get_adam
+ * take these indices.  Every other engine keeps its blob and steps[K][3] (IQL [K][4]).
+ * Per train step st of a call of S steps, on a minibatch (s, a, r, s', d) of B rows, with G = hparams.policy_delay
+ * >= 1 and alpha = alpha[st], in float32:
+ *   subset   M distinct indices Mst of 0..N-1
+ *   target   a', log pi' = head(pi(s'), eps') with SAC's head; only the M drawn target critics are evaluated;
+ *            y = r + gamma (1 - d) (min_{i in Mst} Q'_i(s', a') - alpha log pi') (fminf: a NaN target critic loses
+ *            to a number, as in SAC)
+ *   critics  every Q_i takes one Adam step on mean_b (Q_i(s, a) - y)^2 (the reference's mse_loss * N: each critic's
+ *            gradient is its own MSE's); the logged values are the values before the update
+ *   policy   on steps with (st + 1) % G == 0 or st == S - 1 (ceil(S / G) per call): one Adam step on
+ *            mean_b(alpha log pi - (1/N) sum_i Q_i(s, a_pi)), a_pi, log pi = head(pi(s), eps), with the critics
+ *            just updated (SAC's order and the paper's Algorithm 1; the reference code evaluates this loss with the
+ *            critics from before their Adam step); every critic output carries -1 / (N B), backpropagated through
+ *            the critics' action columns (summed over the critics in index order) into SAC's squash backward pass
+ *   alpha    learn_alpha = 1: SAC's temperature step on policy steps; alpha[st + 1] is its result there and alpha[st]
+ *            on the other steps
+ *   polyak   every step, all N target critics
+ * All N critics share one Adam table row (hparams.q1_lr, which must equal q2_lr): a call is refused when the critics'
+ * step counts differ.  Subsets: a train / train_gather call needs b200rl_offpolicy_set_redq_subsets first with
+ * int32 [K][S][M]; train_gather_rng draws them on the device (a partial Fisher-Yates shuffle over Philox4x32-10 keyed
+ * by (seed, call), tag 0x7ED; SAC's index and noise draws for the same key are unchanged); get_redq_subsets returns
+ * the last call's.  Noise: SAC's [S, 2, B, A]; slot 1 (the draw for s) is read on policy steps only.
+ * Outputs: the train call's q1 / q2 values and losses are critics 1 and 2; policy_losses has ceil(S / G) entries, as
+ * do sac_outputs' log-prob means (its alphas have S); redq_outputs returns every critic's values [K][N][S][B] and
+ * losses [K][N][S].  The heads reduce in a fixed order with no float atomics: a group's learners stay bit-identical to
+ * solo engines.  train, train_gather, train_gather_rng and their group forms all work, as a CUDA graph or as plain
+ * launches with B200RL_OFFPOLICY_GRAPH=0.
+ * Launches, with Lq and Lp the critics' and the policy's Linear layers, independent of N and M: 1 per call (the
+ * temperature table), then per step 4 Lq + Lp + 4, plus 2 Lq + 3 Lp + 3 (+1 with learn_alpha = 1) on a policy step:
+ * 19 and 37 (38) at two hidden layers.  train_gather_rng adds one subset draw per call.
+ * Refused at create: create_redq with another algo, algo 10 through create / create_group; n_q != 2; dueling_k or
+ * noisy_layers != 0; N outside 2..32, M outside 1..N; a policy that is not [obs, ..., 2A] or critics that are not
+ * [obs + A, ..., 1].  set_sac is required; set_dqn, set_c51, set_qr, set_per, set_nstep, set_noise_keys, set_cql,
+ * set_iql and the train_prioritized calls refuse a REDQ engine; set_redq_subsets refuses every other engine.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t n_critics; /* N, 2..32 */
+  int32_t n_min;     /* M, 1..N: target critics per step */
+} b200rl_redq_config;
+
+/* A REDQ engine of n_learners learners (1 = a solo engine; 1 <= n_learners <= B200RL_MAX_LEARNERS): cfg->algo = 10. */
+int b200rl_offpolicy_create_redq(const b200rl_offpolicy_config* cfg, const b200rl_redq_config* redq,
+                                 int32_t n_learners, b200rl_offpolicy** out);
+/* The subsets int32 [K][S][M] of the next train / train_gather call (each M distinct members of 0..N-1), and the
+ * subsets of the last call. */
+int b200rl_offpolicy_set_redq_subsets(b200rl_offpolicy* h, int32_t S, const int32_t* subsets);
+int b200rl_offpolicy_get_redq_subsets(b200rl_offpolicy* h, int32_t S, int32_t* subsets);
+/* q_values [K][N][S][B] (before each step's update) and q_losses [K][N][S] of every critic in the last train call. */
+int b200rl_offpolicy_redq_outputs(b200rl_offpolicy* h, int32_t S, float* q_values, float* q_losses);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Learner groups: K independent off-policy learners (same config, same hyper-parameters, their own parameters, Adam

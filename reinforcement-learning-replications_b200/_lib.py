@@ -106,6 +106,10 @@ class CqlHparams(C.Structure):
                 ("alpha_eps", C.c_double), ("backup_entropy", C.c_int32), ("reserved", C.c_int32)]
 
 
+class RedqConfig(C.Structure):
+    _fields_ = [("n_critics", C.c_int32), ("n_min", C.c_int32)]
+
+
 class IqlConfig(C.Structure):
     _fields_ = [("value", MlpDesc)]
 
@@ -267,6 +271,11 @@ SIGNATURES = {
                                               C.POINTER(C.c_void_p)]),
     "b200rl_offpolicy_set_iql": (C.c_int, [C.c_void_p, C.POINTER(IqlHparams)]),
     "b200rl_offpolicy_iql_outputs": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200rl_offpolicy_create_redq": (C.c_int, [C.POINTER(OffPolicyConfig), C.POINTER(RedqConfig), C.c_int32,
+                                               C.POINTER(C.c_void_p)]),
+    "b200rl_offpolicy_set_redq_subsets": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
+    "b200rl_offpolicy_get_redq_subsets": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
+    "b200rl_offpolicy_redq_outputs": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "b200rl_discounted_cumsum": (C.c_int, [C.c_void_p, C.c_int64, C.c_double, C.c_void_p, C.c_void_p]),
     "b200rl_gae_f64": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_double, C.c_double, C.c_void_p,
                                  C.c_void_p]),

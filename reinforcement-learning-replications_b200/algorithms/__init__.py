@@ -5,6 +5,7 @@ from .discrete_sac import DiscreteSAC
 from .dqn import DQN
 from .group import LearnerGroup
 from .iql import IQL
+from .redq import REDQ
 from .iqn import IQN
 from .ppo import PPO
 from .qrdqn import QRDQN
@@ -14,4 +15,4 @@ from .tqc import TQC
 from .trpo import TRPO
 from .vpg import VPG
 
-__all__ = ["VPG", "TRPO", "PPO", "DDPG", "D4PG", "TD3", "SAC", "TQC", "CQL", "IQL", "DiscreteSAC", "DQN", "C51", "QRDQN", "IQN", "LearnerGroup"]
+__all__ = ["VPG", "TRPO", "PPO", "DDPG", "D4PG", "TD3", "SAC", "TQC", "CQL", "IQL", "REDQ", "DiscreteSAC", "DQN", "C51", "QRDQN", "IQN", "LearnerGroup"]

@@ -44,6 +44,8 @@
 // tqc_target_kernel truncates the pooled target atoms, tqc_critic_loss_kernel and tqc_policy_loss_kernel are the heads.
 // IQL (config algo = 9, create_iql) is a step program of its own (enqueue_iql_steps): network 3 is a trained value
 // network, iql_value_loss_kernel and iql_policy_loss_kernel are its heads, sac_q_loss_kernel the critics'.
+// REDQ (config algo = 10, create_redq) is a step program of its own (enqueue_redq_steps): SAC's policy over N critics
+// run as one ensemble (gemm_ens_kernel, one launch per layer for all of them), the target over a drawn subset of M.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -1006,6 +1008,199 @@ __global__ void cql_alpha_prime_kernel(const float* gap1, const float* gap2, flo
   state[1] = m;
   state[2] = v;
   *alpha_next = fminf(expf(p), CQL_MAX_ALPHA_PRIME);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// REDQ (algo = 10; Chen, Wang, Zhou & Ross 2021): SAC's squashed-Gaussian policy over an ensemble of N critics.  The N
+// critics of a learner lie in one block of the arena (parameters, gradients, Adam moments, activations), each member at
+// a fixed byte stride from the first, so one launch per layer serves the whole ensemble: gemm_ens_kernel runs member
+// blockIdx.z % nm through gemm_tile, the tile function of every other network, so each critic's arithmetic is a solo
+// critic's.  The target pass reads its M members from the step's subset table.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int REDQ_MAX_CRITICS = 32;  // N; the ensemble axis of a launch is K N <= 512 CTAs deep in z
+constexpr unsigned REDQ_DRAW_TAG = 0x7EDu;  // Philox tag of the subset draws: SAC's index / noise draws stay unchanged
+
+// byte strides between consecutive members of the GemmArgs operands (0: an operand every member shares): the bias moves
+// with B (both in the parameter block), dbias with C (both in the gradient block), and A2 -- the action columns of the
+// first layer's input -- is shared by every member.  32 bits keep the kernel within its registers.
+struct EnsStrides {
+  unsigned a, b, c, y;
+};
+
+// z = learner nm + slot; the slot's member is sub[slot] (a subset table, per learner) or the slot itself.  The weights
+// and bias (B and bias in MODE 0 / 1) move with the member, every other operand with the slot; MODE 2 runs without a
+// table, where member and slot agree.
+template <int MODE, bool LANES>
+__global__ void __launch_bounds__(GTHREADS, 1) gemm_ens_kernel(const GemmArgs g, const EnsStrides es, const int* sub,
+                                                            int nm, size_t lane_stride) {
+  __shared__ GemmTile As, Bs;
+  const int lane = LANES ? (int)blockIdx.z / nm : 0, slot = (int)blockIdx.z - lane * nm;
+  const size_t off = LANES ? (size_t)lane * lane_stride : 0;
+  const int mem = sub != nullptr ? lane_ptr(sub, off)[slot] : slot;
+  GemmArgs a = g;
+  const size_t sl = (size_t)slot, ob = off + (size_t)(MODE == 2 ? slot : mem) * es.b, oc = off + sl * es.c;
+  a.A = lane_ptr(a.A, off + sl * es.a);
+  a.B = lane_ptr(a.B, ob);
+  a.C = lane_ptr(a.C, oc);
+  a.bias = lane_ptr(a.bias, ob);
+  a.Y = lane_ptr(a.Y, off + sl * es.y);
+  a.dbias = lane_ptr(a.dbias, oc);
+  a.A2 = lane_ptr(a.A2, off);
+  gemm_tile<MODE>(a, blockIdx.x, blockIdx.y, As, Bs);
+}
+
+// One Adam step for every critic of the ensemble (blockIdx.y = critic k) with the scalars of table[idx]: the arithmetic
+// of adam_step_kernel (adam.cu) on critic k's parameters and gradient (k pg bytes after critic 0's) and its moments
+// (k mv bytes after), the exp_avg_sq product rounded as that kernel's solo instantiation rounds it
+template <bool LANES>
+__global__ void __launch_bounds__(256) redq_adam_kernel(float* params, const float* grad, float* m, float* v,
+                                                        long long n, size_t pg, size_t mv, const float2* table, int idx,
+                                                        float one_minus_b1, float b2, float one_minus_b2, float eps,
+                                                        size_t lane_stride) {
+  const size_t o = LANES ? blockIdx.z * lane_stride : 0, k = blockIdx.y;
+  params = lane_ptr(params, o + k * pg), grad = lane_ptr(grad, o + k * pg);
+  m = lane_ptr(m, o + k * mv), v = lane_ptr(v, o + k * mv), table = lane_ptr(table, o);
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float2 t = table[idx];
+  const float g = grad[i];
+  float mi = m[i], vi = v[i];
+  mi = mi + one_minus_b1 * (g - mi);
+  vi = __fmaf_rn(vi, b2, __fmul_rn(__fmul_rn(g, g), one_minus_b2));
+  const float denom = sqrtf(vi) / t.y + eps;
+  m[i] = mi;
+  v[i] = vi;
+  params[i] = params[i] - t.x * (mi / denom);
+}
+
+// One thread per step: sub[st][0..M) = the first M entries of a partial Fisher-Yates shuffle of 0..N-1, entry j
+// swapping position j with j + floor(u (N - j) / 2^32), u the (j % 4)-th word of Philox block (j / 4, st, call, tag)
+template <bool LANES>
+__global__ void redq_draw_kernel(int* sub, int S, int N, int M, const DrawKeys<LANES> keys, size_t lane_stride) {
+  const int zl = LANES ? blockIdx.z : 0;
+  if (LANES) sub = lane_ptr(sub, blockIdx.z * lane_stride);
+  const int st = blockIdx.x * blockDim.x + threadIdx.x;
+  if (st >= S) return;
+  const unsigned long long seed = keys.seed[zl], call = keys.call[zl];
+  const uint2 key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
+  int perm[REDQ_MAX_CRITICS];
+  for (int j = 0; j < N; ++j) perm[j] = j;
+  uint4 r = make_uint4(0u, 0u, 0u, 0u);
+  for (int j = 0; j < M; ++j) {
+    if ((j & 3) == 0) r = philox4x32_10(make_uint4((unsigned)(j >> 2), (unsigned)st, (unsigned)call, REDQ_DRAW_TAG), key);
+    const unsigned u = (j & 3) == 0 ? r.x : (j & 3) == 1 ? r.y : (j & 3) == 2 ? r.z : r.w;
+    const int k = j + (int)(((unsigned long long)u * (unsigned long long)(N - j)) >> 32);
+    const int t = perm[j];
+    perm[j] = perm[k], perm[k] = t;
+    sub[st * M + j] = perm[j];
+  }
+}
+
+// One thread per row i: qmin[i] = fminf over the M gathered target critics qt[j qt_stride + i] in slot order (fminf: a
+// NaN loses to a number, as in SAC's target); thread 0 also carries the step's temperature to the next step,
+// alpha[1] = alpha[0] (a policy step's temperature step overwrites it later in the step)
+template <bool LANES>
+__global__ void redq_target_kernel(const float* qt, int qt_stride, int M, int B, float* qmin, float* alpha,
+                                   size_t lane_stride) {
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    qt = lane_ptr(qt, o), qmin = lane_ptr(qmin, o), alpha = lane_ptr(alpha, o);
+  }
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) alpha[1] = alpha[0];
+  if (i >= B) return;
+  float m = qt[i];
+  for (int j = 1; j < M; ++j) m = fminf(m, qt[(size_t)j * qt_stride + i]);
+  qmin[i] = m;
+}
+
+// One CTA per critic k = blockIdx.x: sac_q_loss_kernel's head with min(Q1targ, Q2targ) replaced by qmin:
+// y = r + gamma (1 - d) (qmin - alpha log pi'), loss_k = mean((q_k - y)^2), dq_k = 2 (q_k - y) / B, the logged values
+// q_copy_k = q_k.  Member k's q, dq, loss and q_copy are q_stride, B, loss_stride and copy_stride floats apart.
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) redq_q_loss_kernel(const float* q, int q_stride, const float* rew,
+                                                              const float* done, const float* qmin,
+                                                              const float* logp_next, const float* alpha, float gamma,
+                                                              int n, float* dq, float* loss_out, int loss_stride,
+                                                              float* q_copy, int copy_stride, size_t lane_stride) {
+  __shared__ double red[32];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q = lane_ptr(q, o), rew = lane_ptr(rew, o), done = lane_ptr(done, o), qmin = lane_ptr(qmin, o);
+    logp_next = lane_ptr(logp_next, o), alpha = lane_ptr(alpha, o), dq = lane_ptr(dq, o);
+    loss_out = lane_ptr(loss_out, o), q_copy = lane_ptr(q_copy, o);
+  }
+  const int k = blockIdx.x;
+  q += (size_t)k * q_stride, dq += (size_t)k * n, loss_out += (size_t)k * loss_stride;
+  q_copy += (size_t)k * copy_stride;
+  const float a = *alpha;
+  const float inv = 1.0f / (float)n;
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float qi = q[i];
+    q_copy[i] = qi;
+    const float y = rew[i] + gamma * (1.f - done[i]) * (qmin[i] - a * logp_next[i]);
+    const float d = qi - y;
+    acc += (double)d * (double)d;
+    dq[i] = (2.f * d) * inv;
+  }
+  block_mean(acc, n, loss_out, red);
+}
+
+// One CTA: the policy step's head at a = pi(s) on the N critics just updated (member k's output at q + k q_stride).
+// Per row the loss is alpha log pi - (sum_k q_k) / N (k in index order); *loss_out = its mean, *logp_mean_out = mean
+// log pi (each summed as block_mean sums), and every dq_k[i] (member k's at dq + k B) is -1 / (N B).
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) redq_policy_loss_kernel(const float* q, int q_stride, int N,
+                                                                   const float* logp, const float* alpha, int B,
+                                                                   float* dq, float* loss_out, float* logp_mean_out,
+                                                                   size_t lane_stride) {
+  __shared__ double red[32], red_lp[32];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q = lane_ptr(q, o), logp = lane_ptr(logp, o), alpha = lane_ptr(alpha, o), dq = lane_ptr(dq, o);
+    loss_out = lane_ptr(loss_out, o), logp_mean_out = lane_ptr(logp_mean_out, o);
+  }
+  const float a = *alpha;
+  const float g = -1.0f / (float)(N * B);
+  for (int e = threadIdx.x; e < N * B; e += blockDim.x) dq[e] = g;
+  double acc = 0.0, acc_lp = 0.0;
+  for (int i = threadIdx.x; i < B; i += blockDim.x) {
+    float s = 0.f;
+    for (int k = 0; k < N; ++k) s += q[(size_t)k * q_stride + i];
+    const float lp = logp[i];
+    acc += (double)(a * lp - s / (float)N);
+    acc_lp += (double)lp;
+  }
+  block_mean(acc, B, loss_out, red);
+  block_mean(acc_lp, B, logp_mean_out, red_lp);
+}
+
+// sac_squash_backward_kernel with dA = the sum of the N critics' action-column input gradients in index order (member
+// k's input gradient at dx + k dx_stride, row stride ldx); the rest of the arithmetic is that kernel's
+template <bool LANES>
+__global__ void redq_squash_backward_kernel(const float* out, const float* eps, const float* dx, int dx_stride, int N,
+                                            int ldx, int B, int A, float lmin, float lmax, float limit,
+                                            const float* alpha, float* dout, size_t lane_stride) {
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    out = lane_ptr(out, o), eps = lane_ptr(eps, o), dx = lane_ptr(dx, o), alpha = lane_ptr(alpha, o);
+    dout = lane_ptr(dout, o);
+  }
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * A) return;
+  const int r = i / A, j = i - r * A;
+  const float c = *alpha / (float)B;
+  const float mu = out[(size_t)r * 2 * A + j], raw = out[(size_t)r * 2 * A + A + j];
+  const float sigma = expf(fminf(fmaxf(raw, lmin), lmax));
+  const float e = eps[(size_t)r * A + j];
+  const float u = __fadd_rn(mu, __fmul_rn(sigma, e));
+  const float t = tanhf(u);
+  float dA = dx[(size_t)r * ldx + j];
+  for (int k = 1; k < N; ++k) dA = dA + dx[(size_t)k * dx_stride + (size_t)r * ldx + j];
+  const float gu = dA * limit * (1.f - t * t) + 2.f * c * t;
+  dout[(size_t)r * 2 * A + j] = gu;
+  dout[(size_t)r * 2 * A + A + j] = (raw >= lmin && raw <= lmax) ? gu * sigma * e - c : 0.f;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -2270,7 +2465,8 @@ struct b200rl_offpolicy {
   size_t lane_stride = 0;
   std::vector<std::pair<void**, size_t>> pieces;  // (pointer to set, offset in the arena) of every engine buffer
   size_t arena_bytes = 0;
-  NetBuf net[6];  // 0 pi, 1 Q1, 2 Q2, 3 pi_targ, 4 Q1_targ, 5 Q2_targ
+  NetBuf net[2 * REDQ_MAX_CRITICS + 1];  // 0 pi, 1 Q1, 2 Q2, 3 pi_targ, 4 Q1_targ, 5 Q2_targ (REDQ: 0 pi, 1..N the
+                                         // critics, N+1..2N their targets)
   int O = 0, A = 0, maxw = 0;
   // staged minibatches [S,B,*]
   float *obs = nullptr, *act = nullptr, *rew = nullptr, *nobs = nullptr, *done = nullptr, *eps = nullptr;
@@ -2397,6 +2593,20 @@ struct b200rl_offpolicy {
   float* iql_dout = nullptr;                   // [B, 2A] d L_pi / d [m | l]
   float* iql_zero = nullptr;                   // [B] zeros: the critics' head's temperature and log density
   float *out_vl = nullptr, *out_vm = nullptr, *out_wm = nullptr;  // [max_steps] value loss, value mean, weight mean
+  // REDQ (cfg.algo == 10): a SAC engine (h->sac is set: the policy, its buffers, the temperature and the outputs) whose
+  // N critics are networks 1..N, run as one ensemble.  Member k of every ensemble buffer below sits k member strides
+  // after member 0; out_q1 / out_l1 hold every critic's values [N][S][B] and losses [N][S] of the call.
+  bool redq = false;
+  b200rl_redq_config redq_cfg{};
+  int redq_staged_S = -1;                        // the S of host subsets staged for the next train call
+  int* redq_sub = nullptr;                       // [max_steps][M] the call's subsets
+  float* redq_acts[B200RL_MAX_LAYERS + 1];       // the critics' activation stacks, [N][B][maxw] per layer
+  float* redq_tacts[B200RL_MAX_LAYERS + 1];      // the drawn target critics' stacks, [M][B][maxw] per layer
+  float *redq_d0 = nullptr, *redq_d1 = nullptr;  // [N][B][maxw] gradient ping-pong
+  float* redq_dq = nullptr;                      // [N][B] d loss / d Q_k
+  float* redq_dx = nullptr;                      // [N][B][O + A] the critics' input gradients (policy step)
+  float* redq_qmin = nullptr;                    // [B] min over the drawn target critics
+  int redq_last_S = 0, redq_last_B = 0;          // the (S, B) of the last call that ran steps (redq_outputs)
   // the replay columns, episode-end columns, trees and row counts of this call (train_gather[_rng], train_prioritized)
   ReplayLanes<true> replay{};
   std::vector<void*> allocs;
@@ -2406,8 +2616,11 @@ namespace {
 
 inline int64_t state_pad(int64_t n) { return (n + 63) & ~(int64_t)63; }
 
-// the optimizers of the state blob and of steps[]: policy, Q1, Q2 (and V on an IQL engine)
-inline int n_opt(const b200rl_offpolicy* h) { return h->iql ? 4 : 3; }
+// the optimizers of the state blob and of steps[]: policy, Q1, Q2 (and V on an IQL engine; policy and N critics on a
+// REDQ engine)
+inline int n_opt(const b200rl_offpolicy* h) { return h->iql ? 4 : h->redq ? 1 + h->redq_cfg.n_critics : 3; }
+// the network slots of the engine: 6, or 1 + 2N on a REDQ engine
+inline int n_nets(const b200rl_offpolicy* h) { return h->redq ? 1 + 2 * h->redq_cfg.n_critics : 6; }
 
 // float2 entries of one learner's adam_tab: the Adam scalar rows (+ SAC's temperature row, DQN's copy flags or D4PG's
 // betas), then DQN's or D4PG's prioritized (seed, call) at 4 max_steps and a noisy or IQN engine's draw keys (seed,
@@ -2731,18 +2944,20 @@ int adam_net(const b200rl_offpolicy* h, NetBuf& nb, const float2* table, int idx
 static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_config* ic,
                          const b200rl_d4pg_config* dc, int32_t n_learners, b200rl_offpolicy** out,
                          const b200rl_tqc_config* tc = nullptr, const b200rl_cql_config* cc = nullptr,
-                         const b200rl_iql_config* vc = nullptr) {
+                         const b200rl_iql_config* vc = nullptr, const b200rl_redq_config* rq = nullptr) {
   B200RL_REQUIRE(cfg && out, "offpolicy_create: NULL argument");
   B200RL_REQUIRE(n_learners >= 1 && n_learners <= B200RL_MAX_LEARNERS,
                  "offpolicy_create_group: n_learners must be 1..%d, got %d", B200RL_MAX_LEARNERS, n_learners);
   B200RL_REQUIRE(cfg->n_q == 1 || cfg->n_q == 2, "offpolicy_create: n_q must be 1 (DDPG) or 2 (TD3)");
   B200RL_REQUIRE((cfg->algo >= 0 && cfg->algo <= 3) || cfg->algo == 5 || (cfg->algo == 4 && ic != nullptr) ||
                      (cfg->algo == 6 && dc != nullptr) || (cfg->algo == 7 && tc != nullptr) ||
-                     (cfg->algo == 8 && cc != nullptr) || (cfg->algo == 9 && vc != nullptr),
+                     (cfg->algo == 8 && cc != nullptr) || (cfg->algo == 9 && vc != nullptr) ||
+                     (cfg->algo == 10 && rq != nullptr),
                  "offpolicy_create: algo must be 0 (DDPG / TD3), 1 (SAC), 2 (DQN), 3 (C51) or 5 (discrete SAC), got %d "
                  "(algo 4, IQN, is created by b200rl_offpolicy_create_iqn with its counts, algo 6, D4PG, by "
                  "b200rl_offpolicy_create_d4pg with its support, algo 7, TQC, by b200rl_offpolicy_create_tqc, algo 8, "
-                 "CQL, by b200rl_offpolicy_create_cql, algo 9, IQL, by b200rl_offpolicy_create_iql)", cfg->algo);
+                 "CQL, by b200rl_offpolicy_create_cql, algo 9, IQL, by b200rl_offpolicy_create_iql, algo 10, REDQ, by "
+                 "b200rl_offpolicy_create_redq)", cfg->algo);
   B200RL_REQUIRE(ic == nullptr || cfg->algo == 4, "offpolicy_create_iqn: the config's algo must be 4 (IQN), got %d",
                  cfg->algo);
   B200RL_REQUIRE(dc == nullptr || cfg->algo == 6, "offpolicy_create_d4pg: the config's algo must be 6 (D4PG), got %d",
@@ -2753,6 +2968,27 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
                  cfg->algo);
   B200RL_REQUIRE(vc == nullptr || cfg->algo == 9, "offpolicy_create_iql: the config's algo must be 9 (IQL), got %d",
                  cfg->algo);
+  B200RL_REQUIRE(rq == nullptr || cfg->algo == 10, "offpolicy_create_redq: the config's algo must be 10 (REDQ), got "
+                 "%d", cfg->algo);
+  const bool redq = cfg->algo == 10 && rq != nullptr;  // SAC's policy over an ensemble of N critics
+  const int RN = redq ? rq->n_critics : 0;
+  if (redq) {
+    B200RL_REQUIRE(cfg->n_q == 2, "offpolicy_create_redq: REDQ needs n_q = 2 (its first two critics are the train "
+                   "call's q1 / q2), got %d", cfg->n_q);
+    B200RL_REQUIRE(cfg->dueling_k == 0 && cfg->noisy_layers == 0, "offpolicy_create_redq: REDQ takes neither "
+                   "dueling_k nor noisy_layers: dueling and noisy networks are not implemented for it");
+    B200RL_REQUIRE(RN >= 2 && RN <= REDQ_MAX_CRITICS, "offpolicy_create_redq: n_critics must be 2..%d, got %d",
+                   REDQ_MAX_CRITICS, RN);
+    B200RL_REQUIRE(rq->n_min >= 1 && rq->n_min <= RN, "offpolicy_create_redq: n_min must be 1..n_critics = %d, got %d",
+                   RN, rq->n_min);
+    const b200rl_mlp_desc &p = cfg->policy, &q = cfg->q;
+    const int O_ = p.sizes[0], A_ = q.sizes[0] - O_;
+    B200RL_REQUIRE(b200rl_mlp_param_count(&p) > 0 && A_ >= 1 && p.sizes[p.n_layers] == 2 * A_,
+                   "offpolicy_create_redq: the policy must map [obs %d] -> [mean | log_std] = 2 x %d values, got %d -> "
+                   "%d", O_, A_, O_, p.sizes[p.n_layers]);
+    B200RL_REQUIRE(b200rl_mlp_param_count(&q) > 0 && q.sizes[q.n_layers] == 1, "offpolicy_create_redq: the critics "
+                   "must map [obs %d + act %d] -> 1, got %d -> %d", O_, A_, q.sizes[0], q.sizes[q.n_layers]);
+  }
   const bool iql = cfg->algo == 9 && vc != nullptr;  // policy, twin critics and a trained value network in slot 3
   int64_t Pv = 0;
   if (iql) {
@@ -2795,7 +3031,7 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
     B200RL_REQUIRE(TD >= 0 && TD <= TM - 1, "offpolicy_create_tqc: n_drop_per_net must be 0..n_quantiles - 1 = %d, "
                    "got %d", TM - 1, TD);
   }
-  const bool sac = cfg->algo == 1 || tqc || cql, c51 = cfg->algo == 3, iqn = cfg->algo == 4, dsac = cfg->algo == 5;
+  const bool sac = cfg->algo == 1 || tqc || cql || redq, c51 = cfg->algo == 3, iqn = cfg->algo == 4, dsac = cfg->algo == 5;
   const bool d4pg = cfg->algo == 6 && dc != nullptr;
   const int NA = d4pg ? dc->n_atoms : 0;
   if (d4pg) {
@@ -2907,13 +3143,16 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   h->cql = cql;
   if (cql) h->cql_cfg = *cc;
   h->iql = iql;
+  h->redq = redq;
+  if (redq) h->redq_cfg = *rq;
   h->noisy = NM != 0;
   int rc = 0;
   int maxw = O + A;
-  for (int i = 0; i < 6; ++i) {
+  for (int i = 0; i < n_nets(h); ++i) {
     NetBuf& nb = h->net[i];
-    nb.d = iql && i == 3 ? vc->value : (i == 0 || i == 3) ? cfg->policy : cfg->q;
-    nb.P = iql && i == 3 ? Pv : (i == 0 || i == 3) ? Pp : Pq;
+    const bool pol = redq ? i == 0 : i == 0 || i == 3;
+    nb.d = iql && i == 3 ? vc->value : pol ? cfg->policy : cfg->q;
+    nb.P = iql && i == 3 ? Pv : pol ? Pp : Pq;
     int off = 0;
     for (int l = 0; l < nb.d.n_layers; ++l) {
       nb.w_off[l] = off;
@@ -2967,10 +3206,10 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
       nb.P_flat = fo;
     }
     if (cfg->n_q == 1 && (i == 2 || i == 5)) continue;
-    if ((sac || dsac) && i == 3) continue;  // SAC has no target policy
+    if ((sac || dsac) && !redq && i == 3) continue;  // SAC has no target policy
     if (dqn && (i == 0 || i == 3)) continue;  // DQN has no policy
     nb.present = true;
-    if (i < n_opt(h)) rc |= oalloc(h, &nb.grad, (size_t)nb.P);
+    if (i < n_opt(h)) rc |= oalloc(h, &nb.grad, (size_t)nb.P);  // REDQ: critic k's at k state_pad(P) after critic 1's
     if (nb.P_flat != nb.P) {  // the composed network beside the noisy vector in the slab (and its gradient)
       rc |= oalloc(h, &nb.params, (size_t)nb.P);
       if (i < 3) rc |= oalloc(h, &nb.flat_grad, (size_t)nb.P_flat);
@@ -2978,10 +3217,10 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   }
   // parameters and Adam state live in ONE slab in the order of the state blob (b200rl_offpolicy_get_state): the
   // parameters of networks 0..5, then exp_avg / exp_avg_sq of optimizers 0..2 (0..3 for IQL), every segment padded to
-  // 64 floats
+  // 64 floats (REDQ: networks 0..2N, optimizers 0..N)
   {
     int64_t n = 0;
-    for (int i = 0; i < 6; ++i)
+    for (int i = 0; i < n_nets(h); ++i)
       if (h->net[i].present) n += state_pad(h->net[i].P_flat);
     for (int i = 0; i < n_opt(h); ++i)
       if (h->net[i].present) n += 2 * state_pad(h->net[i].P_flat);
@@ -3013,9 +3252,9 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   rc |= oalloc(h, &h->dbuf2, RD * (size_t)maxw);
   rc |= oalloc(h, &h->dbuf3, RD * (size_t)maxw);
   rc |= oalloc(h, &h->dq2, RD * n_dq);
-  rc |= oalloc(h, &h->out_q1, S * B);
+  rc |= oalloc(h, &h->out_q1, S * B * (redq ? RN : 1));
   rc |= oalloc(h, &h->out_q2, S * B);
-  rc |= oalloc(h, &h->out_l1, S);
+  rc |= oalloc(h, &h->out_l1, S * (redq ? RN : 1));
   rc |= oalloc(h, &h->out_l2, S);
   rc |= oalloc(h, &h->out_lp, S);
   rc |= oalloc(h, &h->adam_tab, adam_tab_len(h));
@@ -3048,6 +3287,19 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
     rc |= oalloc(h, &h->cql_ap, S + 1);
     rc |= oalloc(h, &h->cql_ap_state, 3);
     rc |= oalloc(h, &h->cql_zero, 1);
+  }
+  if (redq) {
+    const size_t M = (size_t)rq->n_min;
+    rc |= oalloc(h, &h->redq_sub, S * M);
+    for (int l = 1; l <= cfg->q.n_layers; ++l) {
+      rc |= oalloc(h, &h->redq_acts[l], RN * B * (size_t)maxw);
+      rc |= oalloc(h, &h->redq_tacts[l], M * B * (size_t)maxw);
+    }
+    rc |= oalloc(h, &h->redq_d0, RN * B * (size_t)maxw);
+    rc |= oalloc(h, &h->redq_d1, RN * B * (size_t)maxw);
+    rc |= oalloc(h, &h->redq_dq, RN * B);
+    rc |= oalloc(h, &h->redq_dx, RN * B * (size_t)(O + A));
+    rc |= oalloc(h, &h->redq_qmin, B);
   }
   if (iql) {
     rc |= oalloc(h, &h->dbuf4, B * (size_t)maxw);
@@ -3115,7 +3367,7 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   rc |= arena_commit(h);
   if (rc == 0) {
     float* q = h->state;
-    for (int i = 0; i < 6; ++i) {
+    for (int i = 0; i < n_nets(h); ++i) {
       NetBuf& nb = h->net[i];
       if (!nb.present) continue;
       nb.flat = q;
@@ -3190,6 +3442,12 @@ extern "C" int b200rl_offpolicy_create_cql(const b200rl_offpolicy_config* cfg, c
   return create_engine(cfg, nullptr, nullptr, n_learners, out, nullptr, cql);
 }
 
+extern "C" int b200rl_offpolicy_create_redq(const b200rl_offpolicy_config* cfg, const b200rl_redq_config* redq,
+                                            int32_t n_learners, b200rl_offpolicy** out) {
+  B200RL_REQUIRE(redq, "offpolicy_create_redq: NULL argument");
+  return create_engine(cfg, nullptr, nullptr, n_learners, out, nullptr, nullptr, nullptr, redq);
+}
+
 extern "C" int b200rl_offpolicy_create_iql(const b200rl_offpolicy_config* cfg, const b200rl_iql_config* iql,
                                            int32_t n_learners, b200rl_offpolicy** out) {
   B200RL_REQUIRE(iql, "offpolicy_create_iql: NULL IQL config");
@@ -3215,7 +3473,7 @@ extern "C" void b200rl_offpolicy_destroy(b200rl_offpolicy* h) {
 extern "C" int b200rl_offpolicy_set_params(b200rl_offpolicy* h, int which, const float* host_flat, int64_t n,
                                            void* stream) {
   B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_set_params: a learner group moves its state with get_state / set_state");
-  B200RL_REQUIRE(h && host_flat && which >= 0 && which < 6 && h->net[which].flat, "offpolicy_set_params: bad net");
+  B200RL_REQUIRE(h && host_flat && which >= 0 && which < n_nets(h) && h->net[which].flat, "offpolicy_set_params: bad net");
   B200RL_REQUIRE(n == h->net[which].P_flat, "offpolicy_set_params: expects %lld floats", (long long)h->net[which].P_flat);
   B200RL_CUDA(cudaMemcpyAsync(h->net[which].flat, host_flat, (size_t)n * 4, cudaMemcpyHostToDevice,
                               static_cast<cudaStream_t>(stream)));
@@ -3224,7 +3482,7 @@ extern "C" int b200rl_offpolicy_set_params(b200rl_offpolicy* h, int which, const
 
 extern "C" int b200rl_offpolicy_get_params(b200rl_offpolicy* h, int which, float* host_flat, int64_t n, void* stream) {
   B200RL_REQUIRE(h == nullptr || h->K == 1, "offpolicy_get_params: a learner group moves its state with get_state / set_state");
-  B200RL_REQUIRE(h && host_flat && which >= 0 && which < 6 && h->net[which].flat, "offpolicy_get_params: bad net");
+  B200RL_REQUIRE(h && host_flat && which >= 0 && which < n_nets(h) && h->net[which].flat, "offpolicy_get_params: bad net");
   B200RL_REQUIRE(n == h->net[which].P_flat, "offpolicy_get_params: expects %lld floats", (long long)h->net[which].P_flat);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200RL_CUDA(cudaMemcpyAsync(host_flat, h->net[which].flat, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
@@ -3262,8 +3520,9 @@ extern "C" int b200rl_offpolicy_get_adam(b200rl_offpolicy* h, int which, float* 
   return 0;
 }
 
-// Whole learner state in ONE call and ONE synchronisation: blob = for every present network 0..5 its parameters, then
-// for every optimizer 0..2 (policy, Q1, Q2; IQL: 0..3, V last) exp_avg and exp_avg_sq; steps[n_opt] = Adam step counts.
+// Whole learner state in ONE call and ONE synchronisation: blob = for every present network 0..5 (REDQ: 0..2N) its
+// parameters, then for every optimizer 0..2 (policy, Q1, Q2; IQL: 0..3, V last; REDQ: 0..N) exp_avg and exp_avg_sq;
+// steps[n_opt] = Adam step counts.
 // A group moves [K][blob] and steps[K][n_opt] with one strided copy (the slab heads every learner's arena).
 static int64_t state_floats(const b200rl_offpolicy* h) { return h->K * h->state_n; }
 
@@ -3317,6 +3576,7 @@ extern "C" int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hp
   B200RL_REQUIRE(h && dp, "offpolicy_set_dqn: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_dqn: a discrete SAC engine (algo = 5) takes b200rl_offpolicy_set_sac, not "
                  "set_dqn");
+  B200RL_REQUIRE(!h->redq, "offpolicy_set_dqn: a REDQ engine (algo = 10) takes b200rl_offpolicy_set_sac, not set_dqn");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_dqn: a TQC engine (algo = 7) takes b200rl_offpolicy_set_sac, not set_dqn");
   B200RL_REQUIRE(!h->iql, "offpolicy_set_dqn: an IQL engine (algo = 9) takes b200rl_offpolicy_set_iql, not set_dqn");
   B200RL_REQUIRE(h->dqn, "offpolicy_set_dqn: the engine was not created with algo = 2 (DQN)");
@@ -3331,6 +3591,7 @@ extern "C" int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hp
 extern "C" int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hparams* cp) {
   B200RL_REQUIRE(h && cp, "offpolicy_set_c51: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_c51: a discrete SAC engine (algo = 5) has no categorical head");
+  B200RL_REQUIRE(!h->redq, "offpolicy_set_c51: a REDQ engine (algo = 10) has no categorical head");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_c51: a TQC engine (algo = 7) has no categorical head");
   B200RL_REQUIRE(!h->iql, "offpolicy_set_c51: an IQL engine (algo = 9) has no categorical head");
   B200RL_REQUIRE(!h->d4pg, "offpolicy_set_c51: a D4PG engine (algo = 6) takes its support at create "
@@ -3364,6 +3625,7 @@ extern "C" int b200rl_offpolicy_set_qr(b200rl_offpolicy* h, const b200rl_qr_hpar
   B200RL_REQUIRE(h && qp, "offpolicy_set_qr: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_qr: a discrete SAC engine (algo = 5) has no quantile head");
   B200RL_REQUIRE(!h->iql, "offpolicy_set_qr: an IQL engine (algo = 9) has no quantile head");
+  B200RL_REQUIRE(!h->redq, "offpolicy_set_qr: a REDQ engine (algo = 10) has no quantile critics");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_qr: a TQC engine (algo = 7) takes its quantile counts at create "
                  "(b200rl_offpolicy_create_tqc)");
   B200RL_REQUIRE(h->dqn && !h->c51 && !h->iqn, "offpolicy_set_qr: the engine was not created with algo = 2 (DQN)");
@@ -3385,6 +3647,7 @@ extern "C" int b200rl_offpolicy_set_per(b200rl_offpolicy* h, const b200rl_per_hp
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_per: prioritized replay is not implemented for discrete SAC engines (algo = "
                  "5)");
   B200RL_REQUIRE(!h->c51, "offpolicy_set_per: prioritized replay is not implemented for C51 engines");
+  B200RL_REQUIRE(!h->redq, "offpolicy_set_per: prioritized replay is not implemented for REDQ engines (algo = 10)");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_per: prioritized replay is not implemented for TQC engines (algo = 7)");
   B200RL_REQUIRE(!h->iql, "offpolicy_set_per: prioritized replay is not implemented for IQL engines (algo = 9)");
   B200RL_REQUIRE(h->dqn || h->d4pg, "offpolicy_set_per: prioritized replay is implemented for DQN engines (algo = 2) "
@@ -3402,6 +3665,7 @@ extern "C" int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, c
   B200RL_REQUIRE(h, "offpolicy_set_nstep: NULL engine");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_nstep: n-step returns are not implemented for discrete SAC engines (algo = "
                  "5)");
+  B200RL_REQUIRE(!h->redq, "offpolicy_set_nstep: n-step returns are not implemented for REDQ engines (algo = 10)");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_nstep: n-step returns are not implemented for TQC engines (algo = 7)");
   B200RL_REQUIRE(!h->iql, "offpolicy_set_nstep: n-step returns are not implemented for IQL engines (algo = 9)");
   B200RL_REQUIRE(h->dqn || h->d4pg, "offpolicy_set_nstep: n-step returns are implemented for DQN and C51 engines "
@@ -3424,6 +3688,8 @@ extern "C" int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, c
 extern "C" int b200rl_offpolicy_set_noise_keys(b200rl_offpolicy* h, const uint64_t* seed, const uint64_t* call) {
   B200RL_REQUIRE(h && seed && call, "offpolicy_set_noise_keys: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_noise_keys: a discrete SAC engine (algo = 5) draws no noise");
+  B200RL_REQUIRE(!h->redq, "offpolicy_set_noise_keys: a REDQ engine (algo = 10) has no noisy layers; its subsets come "
+                 "with set_redq_subsets or are drawn by train_gather_rng");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_noise_keys: a TQC engine (algo = 7) has no noisy layers; its policy's draws "
                  "come with the train call");
   B200RL_REQUIRE(!h->iql, "offpolicy_set_noise_keys: an IQL engine (algo = 9) draws no noise");
@@ -3515,6 +3781,7 @@ extern "C" int b200rl_offpolicy_sac_outputs(b200rl_offpolicy* h, int32_t S, floa
 extern "C" int b200rl_offpolicy_set_cql(b200rl_offpolicy* h, const b200rl_cql_hparams* cp) {
   B200RL_REQUIRE(h && cp, "offpolicy_set_cql: NULL argument");
   B200RL_REQUIRE(!h->iql, "offpolicy_set_cql: an IQL engine (algo = 9) takes b200rl_offpolicy_set_iql, not set_cql");
+  B200RL_REQUIRE(!h->redq, "offpolicy_set_cql: a REDQ engine (algo = 10) takes b200rl_offpolicy_set_sac, not set_cql");
   B200RL_REQUIRE(h->cql, "offpolicy_set_cql: the engine was not created with algo = 8 (CQL)");
   B200RL_REQUIRE(std::isfinite(cp->weight) && cp->weight >= 0.0, "offpolicy_set_cql: weight must be finite and >= 0, "
                  "got %g", cp->weight);
@@ -3579,6 +3846,7 @@ extern "C" int b200rl_offpolicy_cql_outputs(b200rl_offpolicy* h, int32_t S, floa
 
 extern "C" int b200rl_offpolicy_set_iql(b200rl_offpolicy* h, const b200rl_iql_hparams* ip) {
   B200RL_REQUIRE(h && ip, "offpolicy_set_iql: NULL argument");
+  B200RL_REQUIRE(!h->redq, "offpolicy_set_iql: a REDQ engine (algo = 10) takes b200rl_offpolicy_set_sac, not set_iql");
   B200RL_REQUIRE(h->iql, "offpolicy_set_iql: the engine was not created with algo = 9 (IQL)");
   B200RL_REQUIRE(ip->expectile > 0.0 && ip->expectile < 1.0, "offpolicy_set_iql: expectile must be in (0, 1), got %g",
                  ip->expectile);
@@ -3639,6 +3907,62 @@ extern "C" int b200rl_offpolicy_get_cql_draws(b200rl_offpolicy* h, int32_t S, in
                  "offpolicy_get_cql_draws: S=%d B=%d exceed the capacities", S, B);
   const size_t w = cql_draw_floats(h, S, B) * 4;
   if (w) B200RL_CUDA(cudaMemcpy2DAsync(draws, w, h->cql_draws, h->lane_stride, w, h->K, cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  return 0;
+}
+
+// A REDQ call with host subsets consumes the ones b200rl_offpolicy_set_redq_subsets staged for its S
+static int redq_take_subsets(b200rl_offpolicy* h, int S, const char* what) {
+  if (!h->redq) return 0;
+  B200RL_REQUIRE(h->redq_staged_S == S, "%s: a REDQ engine needs its subsets [S=%d, M] from "
+                 "b200rl_offpolicy_set_redq_subsets before a call with host draws", what, S);
+  h->redq_staged_S = -1;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_set_redq_subsets(b200rl_offpolicy* h, int32_t S, const int32_t* subsets) {
+  B200RL_REQUIRE(h && subsets, "offpolicy_set_redq_subsets: NULL argument");
+  B200RL_REQUIRE(h->redq, "offpolicy_set_redq_subsets: the engine was not created with algo = 10 (REDQ)");
+  B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps, "offpolicy_set_redq_subsets: S=%d exceeds the capacity %d", S,
+                 h->cfg.max_steps);
+  const int N = h->redq_cfg.n_critics, M = h->redq_cfg.n_min;
+  for (long long r = 0; r < (long long)h->K * S; ++r) {
+    const int32_t* e = subsets + r * M;
+    unsigned long long seen = 0;
+    for (int j = 0; j < M; ++j) {
+      B200RL_REQUIRE(e[j] >= 0 && e[j] < N && !((seen >> e[j]) & 1ull), "offpolicy_set_redq_subsets: learner %d, step "
+                     "%d: a subset needs %d distinct critics in 0..%d, got %d at position %d", (int)(r / (S ? S : 1)),
+                     (int)(r % (S ? S : 1)), M, N - 1, e[j], j);
+      seen |= 1ull << e[j];
+    }
+  }
+  const size_t w = (size_t)S * M * 4;
+  if (w) B200RL_CUDA(cudaMemcpy2DAsync(h->redq_sub, h->lane_stride, subsets, w, w, h->K, cudaMemcpyHostToDevice, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  h->redq_staged_S = S;
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_get_redq_subsets(b200rl_offpolicy* h, int32_t S, int32_t* subsets) {
+  B200RL_REQUIRE(h && subsets && h->redq, "offpolicy_get_redq_subsets: bad arguments (a REDQ engine, algo = 10, has "
+                 "them)");
+  B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps, "offpolicy_get_redq_subsets: S=%d exceeds the capacity", S);
+  const size_t w = (size_t)S * h->redq_cfg.n_min * 4;
+  if (w) B200RL_CUDA(cudaMemcpy2DAsync(subsets, w, h->redq_sub, h->lane_stride, w, h->K, cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_redq_outputs(b200rl_offpolicy* h, int32_t S, float* q_values, float* q_losses) {
+  B200RL_REQUIRE(h && h->redq && q_values && q_losses, "offpolicy_redq_outputs: bad arguments (a REDQ engine, algo = "
+                 "10, has them)");
+  B200RL_REQUIRE(S == h->redq_last_S, "offpolicy_redq_outputs: the last call ran S=%d steps, asked for %d",
+                 h->redq_last_S, S);
+  const size_t N = (size_t)h->redq_cfg.n_critics, wv = N * S * h->redq_last_B * 4, wl = N * S * 4;
+  if (wv) {
+    B200RL_CUDA(cudaMemcpy2DAsync(q_values, wv, h->out_q1, h->lane_stride, wv, h->K, cudaMemcpyDeviceToHost, h->gs));
+    B200RL_CUDA(cudaMemcpy2DAsync(q_losses, wl, h->out_l1, h->lane_stride, wl, h->K, cudaMemcpyDeviceToHost, h->gs));
+  }
   B200RL_CUDA(cudaStreamSynchronize(h->gs));
   return 0;
 }
@@ -4360,8 +4684,214 @@ static int enqueue_dqn_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams
 }
 
 // The step program of the engine's algorithm on `s` (plain launches or under stream capture); *n_pol = its policy steps
+// One launch of gemm_ens_kernel<MODE>: nm slots per learner (sub != NULL: their members from that table)
+template <int MODE>
+static int gemm_ens(const b200rl_offpolicy* h, const GemmArgs& g, const EnsStrides& es, const int* sub, int nm,
+                    cudaStream_t s) {
+  const dim3 grid((g.N + GT - 1) / GT, (g.M + GT - 1) / GT, (unsigned)(nm * h->K));
+  if (h->K == 1) gemm_ens_kernel<MODE, false><<<grid, GTHREADS, 0, s>>>(g, es, sub, nm, (size_t)0);
+  else gemm_ens_kernel<MODE, true><<<grid, GTHREADS, 0, s>>>(g, es, sub, nm, h->lane_stride);
+  B200RL_CUDA(cudaGetLastError());
+  count_launch(1);
+  return 0;
+}
+
+// net_forward of nm critics of the ensemble that starts at network `first` (1: the critics, N + 1: the targets) on
+// the shared input [x | a]: slot k's activations at acts[l] + k act_stride floats, its member k (sub == NULL) or sub[k].
+// Every member's GemmArgs are those net_forward gives a solo critic.
+static int ens_forward(const b200rl_offpolicy* h, int first, float* const* acts, size_t act_stride, const float* x,
+                       const float* a, int B, const int* sub, int nm, cudaStream_t s) {
+  const NetBuf& nb = h->net[first];
+  const int L = nb.d.n_layers;
+  const unsigned ps = (unsigned)(state_pad(nb.P) * 4), as = (unsigned)(act_stride * 4);
+  for (int l = 0; l < L; ++l) {
+    GemmArgs g{};
+    EnsStrides es{};
+    if (l == 0) {
+      g.A = x; g.lda = h->O;
+      g.A2 = a; g.lda2 = h->A; g.ksplit = h->O;
+    } else {
+      g.A = acts[l]; g.lda = nb.d.sizes[l]; es.a = as;
+    }
+    g.B = nb.params + nb.w_off[l]; g.ldb = nb.d.sizes[l]; es.b = ps;
+    g.C = acts[l + 1]; g.ldc = nb.d.sizes[l + 1]; es.c = as;
+    g.bias = nb.params + nb.b_off[l];
+    g.act = (l == L - 1) ? nb.d.out_act : nb.d.hidden_act;
+    g.M = B; g.N = nb.d.sizes[l + 1]; g.K = nb.d.sizes[l];
+    if (gemm_ens<0>(h, g, es, sub, nm, s)) return 1;
+  }
+  return 0;
+}
+
+// net_backward of all N critics on [x | a] from dOut (critic k's [B, 1] at dOut + k B): the weight gradients into the
+// critics' gradient block (want_grads; on s_dw beside the dX chain, at most 3 layers, as net_backward), the input
+// gradient into dx_out (critic k's [B, O + A] at dx_out + k B (O + A)) when dx_out != NULL
+static int ens_backward(b200rl_offpolicy* h, float* const* acts, const float* x, const float* a, const float* dOut,
+                        int B, bool want_grads, float* dx_out, cudaStream_t s, cudaStream_t s_dw) {
+  const NetBuf& nb = h->net[1];
+  const int L = nb.d.n_layers, N = h->redq_cfg.n_critics;
+  const bool side = s_dw != nullptr && want_grads && L <= 3;
+  const unsigned ps = (unsigned)(state_pad(nb.P) * 4), as = (unsigned)((size_t)h->cfg.max_minibatch * h->maxw * 4);
+  const float* dY = dOut;
+  int ldd = 1;
+  unsigned ds = (unsigned)B * 4;
+  float* pp[2] = {h->redq_d0, h->redq_d1};
+  for (int l = L - 1; l >= 0; --l) {
+    const int nout = nb.d.sizes[l + 1], nin = nb.d.sizes[l];
+    const int act = (l == L - 1) ? nb.d.out_act : nb.d.hidden_act;
+    if (want_grads) {
+      GemmArgs g{};
+      EnsStrides es{};
+      g.A = dY; g.lda = ldd; es.a = ds; g.Y = acts[l + 1]; g.ldy = nout; es.y = as; g.act = act;
+      if (l == 0) {
+        g.B = x; g.ldb = h->O;
+        g.A2 = a; g.lda2 = h->A; g.ksplit = h->O;
+      } else {
+        g.B = acts[l]; g.ldb = nin; es.b = as;
+      }
+      g.C = nb.grad + nb.w_off[l]; g.ldc = nin; es.c = ps;
+      g.M = nout; g.N = nin; g.K = B;
+      g.dbias = nb.grad + nb.b_off[l];
+      if (side) {
+        B200RL_CUDA(cudaEventRecord(h->ev_side, s));
+        B200RL_CUDA(cudaStreamWaitEvent(s_dw, h->ev_side, 0));
+      }
+      if (gemm_ens<2>(h, g, es, nullptr, N, side ? s_dw : s)) return 1;
+    }
+    if (l > 0 || dx_out) {
+      float* dst = (l == 0) ? dx_out : pp[l & 1];
+      const unsigned dst_s = (l == 0) ? (unsigned)(B * (h->O + h->A) * 4) : as;
+      GemmArgs g{};
+      EnsStrides es{};
+      g.A = dY; g.lda = ldd; es.a = ds; g.Y = acts[l + 1]; g.ldy = nout; es.y = as; g.act = act;
+      g.B = nb.params + nb.w_off[l]; g.ldb = nin; es.b = ps;
+      g.C = dst; g.ldc = nin; es.c = dst_s;
+      g.M = B; g.N = nin; g.K = nout;
+      if (gemm_ens<1>(h, g, es, nullptr, N, s)) return 1;
+      dY = dst, ldd = nin, ds = dst_s;
+    }
+  }
+  if (side) {
+    B200RL_CUDA(cudaEventRecord(h->ev_side, s_dw));
+    B200RL_CUDA(cudaStreamWaitEvent(s, h->ev_side, 0));
+  }
+  return 0;
+}
+
+// The S REDQ steps (b200rl.h, "REDQ"), SAC's order: critic step, then on policy steps the policy step and the
+// temperature step; polyak every step.  Per step the branches are:
+//   s  : pi(s') -> M target critics(s') -> target head -+-> critic head -> critics' bwd, Adam -+-> [policy step] -+->
+//   s3 : N critics(s, a) -> [pi(s)] --------------------+   ... pi's dW products              |                   |
+//   s4 :                     the critics' dW products ... -> polyak (all N targets) ----------+-------------------+
+//   s2 :                                                          [temperature step beside the policy's backward]
+// The critic ensemble is one launch per layer whatever N; the target ensemble reads its M members from the step's
+// subset table.  On a policy step the critics just updated run on [s | a_pi] and are differentiated w.r.t. their input
+// only; pi(s) is the policy at the start of the step.
+static int enqueue_redq_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s) {
+  const int O = h->O, A = h->A, N = h->redq_cfg.n_critics, M = h->redq_cfg.n_min, G = hp->policy_delay;
+  const int maxS = h->cfg.max_steps;
+  const b200rl_sac_hparams& sp = h->sac_hp;
+  NetBuf &pi = h->net[0], &q1 = h->net[1];
+  const int Lq = q1.d.n_layers, Lp = pi.d.n_layers;
+  const float lmin = (float)sp.log_std_min, lmax = (float)sp.log_std_max, limit = (float)hp->action_limit;
+  const int ew = 256, rows_grid = (B + 127) / 128;
+  const size_t astr = (size_t)h->cfg.max_minibatch * h->maxw;  // floats between two members' activations
+  const int pst = (int)state_pad(q1.P);                         // floats between two members' parameters
+  cudaStream_t s2 = h->s2, s3 = h->s3, s4 = h->s4;
+  if (launch(h, sac_alpha_init_kernel<false>, sac_alpha_init_kernel<true>, (S + 1 + ew - 1) / ew, ew, 0, s,
+             h->sac_alpha, S + 1, h->sac_state, sp.learn_alpha, (float)sp.alpha))
+    return 1;
+  PolyakArgs pk{};  // the critics' block onto the targets' block, padding included (zeros stay zeros)
+  pk.n_nets = 1;
+  pk.target[0] = h->net[N + 1].params;
+  pk.param[0] = q1.params;
+  pk.n[0] = N * pst;
+  float *qa[B200RL_MAX_LAYERS + 1], *pa[B200RL_MAX_LAYERS + 1], *ta[B200RL_MAX_LAYERS + 1];
+  for (int l = 1; l <= Lq; ++l) qa[l] = h->redq_acts[l];
+  for (int l = 1; l <= Lp; ++l) pa[l] = h->acts[2][l], ta[l] = h->acts[0][l];
+  int pol = 0;
+  for (int st = 0; st < S; ++st) {
+    float* s_obs = h->obs + (size_t)st * B * O;
+    const float* s_act = h->act + (size_t)st * B * A;
+    const float* s_rew = h->rew + (size_t)st * B;
+    float* s_nobs = h->nobs + (size_t)st * B * O;
+    const float* s_done = h->done + (size_t)st * B;
+    const float* eps_next = h->eps + (size_t)(2 * st) * B * A;  // [S, 2, B, A]: the draw for s', then the one for s
+    const float* eps_cur = eps_next + (size_t)B * A;
+    const float* alpha = h->sac_alpha + st;
+    const bool pstep = (st + 1) % G == 0 || st == S - 1;
+    pa[0] = s_obs, ta[0] = s_nobs;
+    // ---- the critics on [s | a] (the logged values) and, on a policy step, pi(s) with the pre-update policy ----
+    if (edge(h, s, s3)) return 1;
+    if (ens_forward(h, 1, qa, astr, s_obs, s_act, B, nullptr, N, s3)) return 1;
+    if (pstep) {
+      if (net_forward(h, pi, pa, B, s3)) return 1;
+      if (launch(h, sac_squash_kernel<false>, sac_squash_kernel<true>, rows_grid, 128, 0, s3, pa[Lp], eps_cur, B, A,
+                 lmin, lmax, limit, h->sac_act, h->sac_logp))
+        return 1;
+    }
+    // ---- soft target: a', log pi' from the current policy at s', the M drawn target critics on [s' | a'] ----
+    if (net_forward(h, pi, ta, B, s)) return 1;
+    if (launch(h, sac_squash_kernel<false>, sac_squash_kernel<true>, rows_grid, 128, 0, s, ta[Lp], eps_next, B, A, lmin,
+               lmax, limit, h->sac_act_next, h->sac_logp_next))
+      return 1;
+    if (ens_forward(h, N + 1, h->redq_tacts, astr, s_nobs, h->sac_act_next, B, h->redq_sub + (size_t)st * M, M, s))
+      return 1;
+    if (launch(h, redq_target_kernel<false>, redq_target_kernel<true>, rows_grid, 128, 0, s,
+               (const float*)h->redq_tacts[Lq], (int)astr, M, B, h->redq_qmin, h->sac_alpha + st))
+      return 1;
+    // ---- critic step: every critic's head, backward pass and Adam, one launch each for the ensemble ----
+    if (edge(h, s3, s)) return 1;
+    if (launch(h, redq_q_loss_kernel<false>, redq_q_loss_kernel<true>, N, GTHREADS, 0, s, (const float*)qa[Lq],
+               (int)astr, s_rew, s_done, (const float*)h->redq_qmin, (const float*)h->sac_logp_next, alpha,
+               (float)hp->gamma, B, h->redq_dq, h->out_l1 + st, S, h->out_q1 + (size_t)st * B, S * B))
+      return 1;
+    if (ens_backward(h, qa, s_obs, s_act, h->redq_dq, B, true, nullptr, s, s4)) return 1;
+    if (launch(h, redq_adam_kernel<false>, redq_adam_kernel<true>, dim3((unsigned)((q1.P + 255) / 256), N), 256, 0, s,
+               q1.flat, (const float*)q1.flat_grad, q1.m, q1.v, (long long)q1.P, (size_t)pst * 4, (size_t)2 * pst * 4,
+               (const float2*)(h->adam_tab + maxS), st, (float)(1.0 - hp->q_beta1), (float)hp->q_beta2,
+               (float)(1.0 - hp->q_beta2), (float)hp->q_eps))
+      return 1;
+    // ---- polyak beside the policy step: the targets are next read by the next step ----
+    if (edge(h, s, s4)) return 1;
+    if (launch(h, polyak_kernel<false>, polyak_kernel<true>, (pk.n[0] + ew - 1) / ew, ew, 0, s4, pk,
+               (float)hp->polyak_rho, (float)(1.0 - hp->polyak_rho)))
+      return 1;
+    if (pstep) {  // ---- policy step: the N updated critics on [s | a_pi], differentiated w.r.t. their input only ----
+      if (ens_forward(h, 1, qa, astr, s_obs, h->sac_act, B, nullptr, N, s)) return 1;
+      if (launch(h, redq_policy_loss_kernel<false>, redq_policy_loss_kernel<true>, 1, GTHREADS, 0, s,
+                 (const float*)qa[Lq], (int)astr, N, (const float*)h->sac_logp, alpha, B, h->redq_dq,
+                 h->out_lp + pol, h->out_logp + pol))
+        return 1;
+      if (sp.learn_alpha) {  // SAC's temperature step; alpha[st + 1] = exp(log_alpha)
+        if (edge(h, s, s2)) return 1;
+        if (launch(h, sac_alpha_step_kernel<false>, sac_alpha_step_kernel<true>, 1, GTHREADS, 0, s2, h->sac_logp, B,
+                   (float)sp.target_entropy, h->sac_state, h->adam_tab + (size_t)3 * maxS, pol,
+                   (float)(1.0 - sp.alpha_beta1), (float)sp.alpha_beta2, (float)(1.0 - sp.alpha_beta2),
+                   (float)sp.alpha_eps, h->sac_alpha + st + 1))
+          return 1;
+      }
+      if (ens_backward(h, qa, s_obs, h->sac_act, h->redq_dq, B, false, h->redq_dx, s, nullptr)) return 1;
+      if (launch(h, redq_squash_backward_kernel<false>, redq_squash_backward_kernel<true>, (B * A + ew - 1) / ew, ew, 0,
+                 s, (const float*)pa[Lp], eps_cur, (const float*)(h->redq_dx + O), B * (O + A), N, O + A, B, A, lmin,
+                 lmax, limit, alpha, h->sac_dout))
+        return 1;
+      if (net_backward(h, pi, pa, h->sac_dout, 2 * A, B, true, nullptr, s, 0, nullptr, 0, 0, s3)) return 1;
+      if (adam_net(h, pi, h->adam_tab, pol, hp->policy_beta1, hp->policy_beta2, hp->policy_eps, s)) return 1;
+      if (sp.learn_alpha && edge(h, s2, s)) return 1;
+      ++pol;
+    }
+    if (edge(h, s4, s)) return 1;
+  }
+  return 0;
+}
+
 static int enqueue_program(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s,
                            int* n_pol) {
+  if (h->redq) {
+    *n_pol = (S + hp->policy_delay - 1) / hp->policy_delay;
+    return enqueue_redq_steps(h, hp, S, B, s);
+  }
   if (h->iql) {
     *n_pol = S;
     return enqueue_iql_steps(h, hp, S, B, s);
@@ -4388,11 +4918,14 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   h->per_last = h->per_run;  // what get_per_draws may report
   h->nstep_last = h->nstep > 1;  // and get_nstep_draws
   if (h->iqn) h->iqn_last_B = B;  // and get_iqn_draws
+  if (h->redq) h->redq_last_S = S, h->redq_last_B = B;  // and redq_outputs
 
   // Adam's step-dependent scalars for the steps of this call (torch's host-side double arithmetic), one small upload
   // (a group: one table per learner, from that learner's step counts, uploaded with one strided copy)
   const int maxS = h->cfg.max_steps;
-  const int n_pol_expected = h->dqn ? 0 : h->sac || h->dsac || h->iql ? S : (S + hp->policy_delay - 1) / hp->policy_delay;  // SAC: no delay
+  const int n_pol_expected = h->dqn ? 0 : h->redq || !(h->sac || h->dsac || h->iql)
+                                                 ? (S + hp->policy_delay - 1) / hp->policy_delay
+                                                 : S;  // SAC: no delay
   const size_t tab_n = adam_tab_len(h);
   const bool learn_alpha = (h->sac || h->dsac) && h->sac_hp.learn_alpha;
   const bool lagrange = h->cql && h->cql_cfg.lagrange;
@@ -4477,7 +5010,8 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
     h->net[0].step[z] += n_pol;
     h->net[1].step[z] += S;
     if (td3) h->net[2].step[z] += S;
-    if (learn_alpha) h->alpha_step[z] += S;
+    for (int k = 3; h->redq && k <= h->redq_cfg.n_critics; ++k) h->net[k].step[z] += S;
+    if (learn_alpha) h->alpha_step[z] += h->redq ? n_pol : S;  // REDQ: one temperature step per policy step
     if (lagrange) h->ap_step[z] += S;
     if (h->iql) h->net[3].step[z] += S;
   }
@@ -4485,9 +5019,11 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   const size_t ls = h->lane_stride, K = (size_t)h->K;
   B200RL_CUDA(cudaMemcpy2DAsync(q1_values, SB * 4, h->out_q1, ls, SB * 4, K, cudaMemcpyDeviceToHost, s));
   B200RL_CUDA(cudaMemcpy2DAsync(q1_losses, (size_t)S * 4, h->out_l1, ls, (size_t)S * 4, K, cudaMemcpyDeviceToHost, s));
-  if (td3) {
-    B200RL_CUDA(cudaMemcpy2DAsync(q2_values, SB * 4, h->out_q2, ls, SB * 4, K, cudaMemcpyDeviceToHost, s));
-    B200RL_CUDA(cudaMemcpy2DAsync(q2_losses, (size_t)S * 4, h->out_l2, ls, (size_t)S * 4, K, cudaMemcpyDeviceToHost, s));
+  if (td3) {  // REDQ: critic 2's, right behind critic 1's
+    B200RL_CUDA(cudaMemcpy2DAsync(q2_values, SB * 4, h->redq ? h->out_q1 + SB : h->out_q2, ls, SB * 4, K,
+                                  cudaMemcpyDeviceToHost, s));
+    B200RL_CUDA(cudaMemcpy2DAsync(q2_losses, (size_t)S * 4, h->redq ? h->out_l1 + S : h->out_l2, ls, (size_t)S * 4, K,
+                                  cudaMemcpyDeviceToHost, s));
   }
   if (n_pol > 0 && policy_losses != nullptr)  // NULL: a prioritized call (get_policy_losses reads them)
     B200RL_CUDA(cudaMemcpy2DAsync(policy_losses, (size_t)S * 4, h->out_lp, ls, (size_t)n_pol * 4, K,
@@ -4535,6 +5071,15 @@ static int train_begin(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, 
     B200RL_REQUIRE(noise_given, "%s: SAC needs the noise draws [S, 2, B, A]", what);
   }
   B200RL_REQUIRE(!h->cql || h->cql_set, "%s: a CQL engine needs b200rl_offpolicy_set_cql before it trains", what);
+  if (h->redq) {  // one Adam table row serves every critic
+    B200RL_REQUIRE(hp->q1_lr == hp->q2_lr, "%s: REDQ's critics share one learning rate: q1_lr %g != q2_lr %g", what,
+                   hp->q1_lr, hp->q2_lr);
+    for (int z = 0; z < h->K; ++z)
+      for (int k = 2; k <= h->redq_cfg.n_critics; ++k)
+        B200RL_REQUIRE(h->net[k].step[z] == h->net[1].step[z], "%s: REDQ's critics share one Adam step count: learner "
+                       "%d, critic %d has %lld steps, critic 1 %lld", what, z, k, (long long)h->net[k].step[z],
+                       (long long)h->net[1].step[z]);
+  }
   if (h->iql) {
     B200RL_REQUIRE(h->iql_set, "%s: an IQL engine needs b200rl_offpolicy_set_iql before it trains", what);
     B200RL_REQUIRE(!hp->use_target_noise && !noise_given, "%s: an IQL engine draws no noise: use_target_noise must be "
@@ -4586,7 +5131,7 @@ extern "C" int b200rl_offpolicy_train(b200rl_offpolicy* h, const b200rl_offpolic
       up(h->nobs, next_obs, SB * O * 4) || up(h->done, done, SB * 4))
     return 1;
   if (h->sac && up(h->eps, noise, 2 * SB * A * 4)) return 1;
-  if (cql_take_draws(h, S, B, "offpolicy_train")) return 1;
+  if (cql_take_draws(h, S, B, "offpolicy_train") || redq_take_subsets(h, S, "offpolicy_train")) return 1;
   if (!h->sac && !h->dqn && !h->dsac && hp->use_target_noise && up(h->eps, noise, SB * A * 4)) return 1;
 
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
@@ -4661,7 +5206,8 @@ extern "C" int b200rl_offpolicy_train_gather_group(b200rl_offpolicy* h, const b2
   B200RL_CUDA(cudaMemcpy2DAsync(h->idx, ls, idx, SB * 8, SB * 8, h->K, cudaMemcpyHostToDevice, s));
   const size_t n_eps = h->sac ? 2 * SB * A : (hp->use_target_noise && !h->dqn && !h->dsac ? SB * A : 0);
   if (n_eps) B200RL_CUDA(cudaMemcpy2DAsync(h->eps, ls, noise, n_eps * 4, n_eps * 4, h->K, cudaMemcpyHostToDevice, s));
-  if (cql_take_draws(h, S, B, "offpolicy_train_gather")) return 1;
+  if (cql_take_draws(h, S, B, "offpolicy_train_gather") || redq_take_subsets(h, S, "offpolicy_train_gather"))
+    return 1;
   if (gather_columns(h, hp, (long long)SB, s)) return 1;
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
 }
@@ -4724,6 +5270,9 @@ extern "C" int b200rl_offpolicy_train_gather_rng_group(b200rl_offpolicy* h, cons
                h->cql_draws, n_cql, (long long)B * h->cql_cfg.n_actions * A, keys))
       return 1;
   }
+  if (h->redq && launch(h, redq_draw_kernel<false>, redq_draw_kernel<true>, (unsigned)((S + 127) / 128), 128, 0, s,
+                        h->redq_sub, (int)S, h->redq_cfg.n_critics, h->redq_cfg.n_min, keys))
+    return 1;
   if (gather_columns(h, hp, SB, s)) return 1;
   return run_staged(h, hp, S, B, q1_values, q2_values, q1_losses, q2_losses, policy_losses, n_policy_updates);
 }
@@ -4773,6 +5322,8 @@ extern "C" int b200rl_offpolicy_train_prioritized_group(b200rl_offpolicy* h, con
   B200RL_REQUIRE(!h->c51, "offpolicy_train_prioritized: prioritized replay is not implemented for C51 engines");
   B200RL_REQUIRE(!h->dsac, "offpolicy_train_prioritized: prioritized replay is not implemented for discrete SAC "
                  "engines (algo = 5)");
+  B200RL_REQUIRE(!h->redq, "offpolicy_train_prioritized: prioritized replay is not implemented for REDQ engines "
+                 "(algo = 10)");
   B200RL_REQUIRE(!h->tqc, "offpolicy_train_prioritized: prioritized replay is not implemented for TQC engines (algo = "
                  "7)");
   B200RL_REQUIRE(!h->iql, "offpolicy_train_prioritized: prioritized replay is not implemented for IQL engines (algo = "

@@ -342,6 +342,9 @@ class OffPolicyEngine:
     and a call with host draws takes ``noise`` = (SAC's [S, 2, B, A], CQL's [S, 3, B, N, A]) (b200rl.h, "CQL").  IQL
     (``algo`` 9) has SAC's policy and critics and a trained value network in slot 3: ``iql`` = (sizes, (hidden, out
     activation)) of V; ``set_iql`` is required, no noise is used, and the state has four optimizers (b200rl.h, "IQL").
+    REDQ (``algo`` 10) has SAC's policy, temperature and noise over N critics: ``redq`` = (N, M), M the target critics
+    drawn per step; networks 1..N are the critics and N+1..2N their targets, the state has 1 + N optimizers, and a call
+    with host draws takes ``noise`` = (SAC's [S, 2, B, A], subsets [S, M]) (b200rl.h, "REDQ").
 
     ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
     launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
@@ -349,15 +352,15 @@ class OffPolicyEngine:
     refused."""
 
     NETS = {"policy": 0, "q1": 1, "q2": 2, "target_policy": 3, "target_q1": 4, "target_q2": 5}
-    TD3, SAC, DQN, C51, IQN, DSAC, D4PG, TQC, CQL, IQL = 0, 1, 2, 3, 4, 5, 6, 7, 8, 9
+    TD3, SAC, DQN, C51, IQN, DSAC, D4PG, TQC, CQL, IQL, REDQ = 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10
     DISCRETE = (DQN, C51, IQN)  # the algos with DQN's networks, inputs and outputs
     INDEX_ACTIONS = DISCRETE + (DSAC,)  # the algos whose action column holds an action index
-    SOFT = (SAC, DSAC, TQC, CQL)  # the algos with SAC's networks, temperature and outputs
-    SQUASHED = (SAC, TQC, CQL)  # the algos with SAC's squashed-Gaussian policy and its [S, 2, B, A] noise
+    SOFT = (SAC, DSAC, TQC, CQL, REDQ)  # the algos with SAC's temperature and outputs
+    SQUASHED = (SAC, TQC, CQL, REDQ)  # the algos with SAC's squashed-Gaussian policy and its [S, 2, B, A] noise
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
                  q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1, dueling_k: int = 0,
-                 noisy_layers: int = 0, iqn=None, d4pg=None, tqc=None, cql=None, iql=None):
+                 noisy_layers: int = 0, iqn=None, d4pg=None, tqc=None, cql=None, iql=None, redq=None):
         from ._lib import OffPolicyConfig
         self.lib = _lib.load()
         current_stream_handle()
@@ -373,7 +376,9 @@ class OffPolicyEngine:
         self.tqc = None if tqc is None else (int(tqc[0]), int(tqc[1]))
         self.cql = None if cql is None else (int(cql[0]), int(bool(cql[1])))
         self.iql = None if iql is None else (tuple(int(x) for x in iql[0]), tuple(iql[1]))
-        self.n_opt = 4 if self.iql is not None else 3  # optimizers in the state blob and the step counts
+        self.redq = None if redq is None else (int(redq[0]), int(redq[1]))
+        # optimizers in the state blob and the step counts
+        self.n_opt = 4 if self.iql is not None else 1 + self.redq[0] if self.redq is not None else 3
         self.n_value = 0
         self.discrete = self.algo in self.DISCRETE  # DQN's networks and outputs
         self.index_actions = self.algo in self.INDEX_ACTIONS  # act [S,B] indices, no noise
@@ -408,6 +413,9 @@ class OffPolicyEngine:
             self.n_value = int(self.lib.b200rl_mlp_param_count(vdesc))
             check(self.lib.b200rl_offpolicy_create_iql(C.byref(cfg), C.byref(_lib.IqlConfig(vdesc)), self.K,
                                                        C.byref(h)), "offpolicy_create_iql")
+        elif self.redq is not None:  # the ensemble's size (b200rl.h, "REDQ")
+            check(self.lib.b200rl_offpolicy_create_redq(C.byref(cfg), C.byref(_lib.RedqConfig(*self.redq)), self.K,
+                                                        C.byref(h)), "offpolicy_create_redq")
         elif self.cql is not None:  # N and the Lagrange switch size the buffers (b200rl.h, "CQL")
             check(self.lib.b200rl_offpolicy_create_cql(C.byref(cfg), C.byref(_lib.CqlConfig(*self.cql)), self.K,
                                                        C.byref(h)), "offpolicy_create_cql")
@@ -435,6 +443,8 @@ class OffPolicyEngine:
             pass
 
     def _n(self, which):
+        if self.redq is not None:  # 0 the policy, 1..2N the critics and their targets
+            return self.n_policy if which == 0 else self.n_qp
         if which == 3 and self.iql is not None:
             return self.n_value
         return self.n_policy if which in (0, 3) else self.n_qp
@@ -472,6 +482,8 @@ class OffPolicyEngine:
         pad = lambda n: (n + 63) & ~63
         if self.discrete:
             present, optimized = [1, 4], [1]
+        elif self.redq is not None:
+            present, optimized = list(range(1 + 2 * self.redq[0])), list(range(1 + self.redq[0]))
         else:
             present = [0, 1] + ([2] if self.n_q == 2 else []) + ([] if self.algo in self.SOFT else [3]) + [4] + \
                 ([5] if self.n_q == 2 else [])
@@ -573,6 +585,28 @@ class OffPolicyEngine:
         check(self.lib.b200rl_offpolicy_iql_outputs(self.h, int(S), *[_ptr(x) for x in out]), "iql_outputs")
         return tuple(x[0] for x in out) if self.K == 1 else out
 
+    # ---- REDQ ----
+    def set_redq_subsets(self, subsets) -> None:
+        """The target subsets int32 [S, M] (a group: [K, S, M]) of the next train / train_gather call."""
+        sub = self._lead(subsets, np.int32, 3)
+        if sub.shape[2] != self.redq[1]:
+            raise ValueError(f"REDQ subsets: expected {self.redq[1]} critics per step, got shape {sub.shape}")
+        check(self.lib.b200rl_offpolicy_set_redq_subsets(self.h, int(sub.shape[1]), _ptr(sub)), "set_redq_subsets")
+
+    def get_redq_subsets(self, S: int):
+        """The subsets [S, M] of the last train call (a group: [K, S, M])."""
+        sub = np.empty((self.K, S, self.redq[1]), np.int32)
+        check(self.lib.b200rl_offpolicy_get_redq_subsets(self.h, int(S), _ptr(sub)), "get_redq_subsets")
+        return sub[0] if self.K == 1 else sub
+
+    def redq_outputs(self, S: int, B: int):
+        """(every critic's values [N, S, B] before each step's update, its losses [N, S]) of the last train call; a
+        group: each with a leading [K] axis."""
+        N = self.redq[0]
+        qv, ql = np.zeros((self.K, N, S, B), np.float32), np.zeros((self.K, N, S), np.float32)
+        check(self.lib.b200rl_offpolicy_redq_outputs(self.h, int(S), _ptr(qv), _ptr(ql)), "redq_outputs")
+        return (qv[0], ql[0]) if self.K == 1 else (qv, ql)
+
     # ---- CQL ----
     def set_cql(self, weight: float, temperature: float, target_action_gap: float = 0.0, alpha_lr: float = 3e-4,
                 alpha_betas=(0.9, 0.999), alpha_eps: float = 1e-8, backup_entropy: bool = False) -> None:
@@ -624,10 +658,14 @@ class OffPolicyEngine:
         return d[0] if self.K == 1 else d
 
     def _split_noise(self, noise, S, B):
-        """A CQL engine's (SAC noise, CQL draws): stages the draws for the call, returns SAC's part."""
-        if self.algo != self.CQL or not isinstance(noise, tuple):  # SAC's part alone: the engine asks for the draws
+        """A CQL engine's (SAC noise, CQL draws) or a REDQ engine's (SAC noise, subsets): stages the draws for the
+        call, returns SAC's part."""
+        if self.algo not in (self.CQL, self.REDQ) or not isinstance(noise, tuple):  # the engine asks for the draws
             return noise
         sac, draws = noise
+        if self.algo == self.REDQ:
+            self.set_redq_subsets(draws)
+            return sac
         draws = self._lead(draws, np.float32, 6)
         if draws.shape != self._cql_draws_shape(S, B):
             raise ValueError(f"CQL draws: expected shape {self._cql_draws_shape(S, B)}, got {draws.shape}")
@@ -786,6 +824,9 @@ class OffPolicyEngine:
             out["cql_gap_1"], out["cql_gap_2"], out["alpha_primes"] = self.cql_outputs(S)
         if self.algo == self.IQL:
             out["value_losses"], out["value_means"], out["weight_means"] = self.iql_outputs(S)
+        if self.algo == self.REDQ and S > 0:  # one mean log pi per policy step; every critic's values and losses
+            out["log_prob_means"] = out["log_prob_means"][..., :npol.value]
+            out["redq_q_values"], out["redq_q_losses"] = self.redq_outputs(S, self._last_B)
         return out
 
     def _lead(self, a, dtype, ndim):

@@ -346,7 +346,8 @@ typedef struct {
                             * "D4PG" below), 7 = TQC (created by b200rl_offpolicy_create_tqc only; see "TQC" below),
                             * 8 = CQL (created by b200rl_offpolicy_create_cql only; see "CQL" below), 9 = IQL
                             * (created by b200rl_offpolicy_create_iql only; see "IQL" below), 10 = REDQ (created
-                            * by b200rl_offpolicy_create_redq only; see "REDQ" below) */
+                            * by b200rl_offpolicy_create_redq only; see "REDQ" below), 11 = EDAC (created by
+                            * b200rl_offpolicy_create_edac only; see "EDAC" below) */
   int32_t dueling_k;       /* 0 = the Q network is a plain MLP; K >= 1 = a dueling Q network (algo 2 / 3 only; see
                             * "Dueling Q networks" below) */
   int32_t noisy_layers;    /* bit mask over the Q network's Linear layers in flat order: 0 = none; bit l = layer l is a
@@ -970,6 +971,61 @@ int b200rl_offpolicy_set_redq_subsets(b200rl_offpolicy* h, int32_t S, const int3
 int b200rl_offpolicy_get_redq_subsets(b200rl_offpolicy* h, int32_t S, int32_t* subsets);
 /* q_values [K][N][S][B] (before each step's update) and q_losses [K][N][S] of every critic in the last train call. */
 int b200rl_offpolicy_redq_outputs(b200rl_offpolicy* h, int32_t S, float* q_values, float* q_losses);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * EDAC and SAC-N on the same engine (config algo = 11, n_q = 2; An, Moon, Kim & Song 2021, "Uncertainty-Based Offline
+ * Reinforcement Learning with Diversified Q-Ensemble"): SAC's squashed-Gaussian policy over an ensemble of N critics,
+ * the target the min over all N target critics, and (eta > 0) a penalty that pushes the critics' action gradients
+ * apart.  eta = 0 is SAC-N.  Created by b200rl_offpolicy_create_edac from a config with algo = 11 and a
+ * b200rl_edac_config {N, eta}, 2 <= N <= 32, eta finite and >= 0 (fixed at create); create, create_group and
+ * create_redq refuse algo 11.  The engine has REDQ's layout: networks 0 the policy, 1..N the critics, N+1..2N their
+ * targets; optimizers 0..N; REDQ's state blob, steps[K][1 + N], set_params / get_params / set_adam / get_adam.
+ * Per train step st of a call of S steps, on a minibatch (s, a, r, s', d) of B rows, with alpha = alpha[st], in float32:
+ *   target   a', log pi' = head(pi(s'), eps') with SAC's head; y = r + gamma (1 - d) (min over all N target critics
+ *            of Q'_i(s', a') - alpha log pi') (fminf, as SAC and REDQ)
+ *   critics  every Q_i takes one Adam step on mean_b (Q_i(s, a) - y)^2 + eta D, both terms at the parameters from
+ *            before the step, with
+ *              D = (1 / (B (N - 1))) sum_b sum_{i != j} gh_i(b) . gh_j(b),  gh = g / (|g|_2 + 1e-10),
+ *              g_i(b) = d Q_i(s_b, a_b) / d a at the dataset action
+ *            (the authors' grad_loss); Adam steps on g_td + g_div, added in that order; the logged values are the
+ *            values before the update and the logged losses the TD losses
+ *   policy   every step: one Adam step on mean_b(alpha log pi - min_i Q_i(s, a_pi)), a_pi, log pi = head(pi(s), eps),
+ *            with the critics just updated (SAC's and REDQ's order here; the authors' code evaluates this loss with the
+ *            critics from before their update); per row the gradient goes to the first critic that attains the min
+ *            (lowest index on ties; a NaN loses to a number), through its action columns into SAC's squash backward
+ *   alpha    learn_alpha = 1: SAC's temperature step every step
+ *   polyak   every step, all N target critics
+ * The diversity gradient is computed without autograd (ReLU masks are piecewise constant): a ones-backward through the
+ * critics gives g, edac_diversity_kernel gives u = d(eta D) / d g and D, a tangent forward of u through the masks and
+ * the weight-gradient products give the parameter gradient of sum_b g . u; its bias and obs-column entries are exactly
+ * 0.  That pass runs beside the target path and joins before the critics' Adam step.  With eta > 0 the critics' hidden
+ * activation must be ReLU and their output identity.  All N critics share one Adam table row (hparams.q1_lr, which
+ * must equal q2_lr); hparams.policy_delay must be >= 1 and is otherwise not read.  Noise: SAC's [S, 2, B, A].  Nothing else is drawn:
+ * train_gather_rng draws SAC's indices and noise.  Outputs: the train call's q1 / q2 are critics 1 and 2, policy_losses
+ * and sac_outputs have S entries, redq_outputs returns every critic's values and TD losses, and edac_outputs D per step.
+ * The heads reduce in a fixed order with no float atomics: a group's learners stay bit-identical to solo engines.
+ * train, train_gather, train_gather_rng and their group forms all work, as a CUDA graph or as plain launches with
+ * B200RL_OFFPOLICY_GRAPH=0.
+ * Launches, with Lq and Lp the critics' and the policy's Linear layers, independent of N: 1 per call (the temperature
+ * table), then per step 6 Lq + 4 Lp + 7 (+1 with learn_alpha = 1), plus 3 Lq with eta > 0: 37 (38) and 46 (47) at two
+ * hidden layers.
+ * Refused at create: algo != 11; n_q != 2; dueling_k or noisy_layers != 0; N outside 2..32; a negative or non-finite
+ * eta; a policy that is not [obs, ..., 2A] or critics that are not [obs + A, ..., 1]; with eta > 0, critics whose
+ * hidden activation is not ReLU or whose output is not identity.  set_sac is required; set_redq_subsets,
+ * get_redq_subsets, set_dqn, set_c51, set_qr, set_per, set_nstep, set_noise_keys, set_cql, set_iql and the
+ * train_prioritized calls refuse an EDAC engine.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t n_critics; /* N, 2..32 */
+  int32_t reserved;  /* 0 */
+  double eta;        /* the diversity weight, finite and >= 0; 0 = SAC-N */
+} b200rl_edac_config;
+
+/* An EDAC engine of n_learners learners (1 = a solo engine; 1 <= n_learners <= B200RL_MAX_LEARNERS): cfg->algo = 11. */
+int b200rl_offpolicy_create_edac(const b200rl_offpolicy_config* cfg, const b200rl_edac_config* edac,
+                                 int32_t n_learners, b200rl_offpolicy** out);
+/* diversity [K][S]: D of every step of the last train call (0 with eta = 0). */
+int b200rl_offpolicy_edac_outputs(b200rl_offpolicy* h, int32_t S, float* diversity);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Learner groups: K independent off-policy learners (same config, same hyper-parameters, their own parameters, Adam

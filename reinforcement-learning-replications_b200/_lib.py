@@ -110,6 +110,10 @@ class RedqConfig(C.Structure):
     _fields_ = [("n_critics", C.c_int32), ("n_min", C.c_int32)]
 
 
+class EdacConfig(C.Structure):
+    _fields_ = [("n_critics", C.c_int32), ("reserved", C.c_int32), ("eta", C.c_double)]
+
+
 class IqlConfig(C.Structure):
     _fields_ = [("value", MlpDesc)]
 
@@ -276,6 +280,9 @@ SIGNATURES = {
     "b200rl_offpolicy_set_redq_subsets": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
     "b200rl_offpolicy_get_redq_subsets": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
     "b200rl_offpolicy_redq_outputs": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "b200rl_offpolicy_create_edac": (C.c_int, [C.POINTER(OffPolicyConfig), C.POINTER(EdacConfig), C.c_int32,
+                                               C.POINTER(C.c_void_p)]),
+    "b200rl_offpolicy_edac_outputs": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
     "b200rl_discounted_cumsum": (C.c_int, [C.c_void_p, C.c_int64, C.c_double, C.c_void_p, C.c_void_p]),
     "b200rl_gae_f64": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_double, C.c_double, C.c_void_p,
                                  C.c_void_p]),

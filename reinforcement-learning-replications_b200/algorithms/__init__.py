@@ -3,6 +3,7 @@ from .cql import CQL
 from .d4pg import D4PG
 from .discrete_sac import DiscreteSAC
 from .dqn import DQN
+from .edac import EDAC
 from .group import LearnerGroup
 from .iql import IQL
 from .redq import REDQ
@@ -15,4 +16,4 @@ from .tqc import TQC
 from .trpo import TRPO
 from .vpg import VPG
 
-__all__ = ["VPG", "TRPO", "PPO", "DDPG", "D4PG", "TD3", "SAC", "TQC", "CQL", "IQL", "REDQ", "DiscreteSAC", "DQN", "C51", "QRDQN", "IQN", "LearnerGroup"]
+__all__ = ["VPG", "TRPO", "PPO", "DDPG", "D4PG", "TD3", "SAC", "TQC", "CQL", "IQL", "REDQ", "EDAC", "DiscreteSAC", "DQN", "C51", "QRDQN", "IQN", "LearnerGroup"]

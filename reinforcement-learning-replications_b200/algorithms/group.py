@@ -1,4 +1,4 @@
-"""LearnerGroup: several independent TD3 / DDPG / D4PG / SAC / TQC / CQL / IQL / REDQ / discrete SAC / DQN / C51 / QR-DQN / IQN learners (typically one per seed) trained side by side by ONE
+"""LearnerGroup: several independent TD3 / DDPG / D4PG / SAC / TQC / CQL / IQL / REDQ / EDAC / discrete SAC / DQN / C51 / QR-DQN / IQN learners (typically one per seed) trained side by side by ONE
 off-policy engine, every operation of a train step one launch for all of them (b200rl_offpolicy_create_group).
 
 The contract: each member ends up bit for bit where it would be had it run alone.  Members keep everything of their
@@ -41,7 +41,7 @@ def _signature(agent) -> list:
     names = ["q_function"] if dqn else ["policy"] + (["q_function_1", "q_function_2"] if agent.n_q == 2 else ["q_function"])
     if agent.algo == OffPolicyEngine.IQL:
         names.append("value_function")
-    if agent.algo == OffPolicyEngine.REDQ:
+    if agent.algo in (OffPolicyEngine.REDQ, OffPolicyEngine.EDAC):
         names = ["policy"] + [f"q_function_{i}" for i in range(1, agent.n_critics + 1)]
     sig = [("class", type(agent).__name__)]
     for name, m in zip(names, trainable):
@@ -83,6 +83,8 @@ def _signature(agent) -> list:
         sig.append(("(n_quantiles, top_quantiles_to_drop_per_net)", agent.tqc_config))
     if agent.algo == OffPolicyEngine.REDQ:
         sig.append(("(n_critics, n_min)", agent.redq_config))
+    if agent.algo == OffPolicyEngine.EDAC:
+        sig.append(("(n_critics, eta)", agent.edac_config))
     if agent.algo == OffPolicyEngine.CQL:
         sig.append(("(cql_n_actions, lagrange)", agent.cql_config))
         sig.append(("CQL hyper-parameters", agent.cql_hparams()))
@@ -151,7 +153,7 @@ class LearnerGroup:
     def add(self, agent) -> None:
         """Add ``agent``; the current state of the global random generators becomes its private stream."""
         if not isinstance(agent, _OffPolicyBase):
-            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or D4PG / TQC / CQL / IQL / REDQ / DiscreteSAC / DQN / C51 / QR-DQN / IQN) learners, got {type(agent).__name__}")
+            raise ValueError(f"LearnerGroup: members must be TD3, DDPG or SAC (or D4PG / TQC / CQL / IQL / REDQ / EDAC / DiscreteSAC / DQN / C51 / QR-DQN / IQN) learners, got {type(agent).__name__}")
         if any(m is agent for m in self.members):
             raise ValueError("LearnerGroup: this agent is already a member")
         if len(self.members) >= MAX_LEARNERS:

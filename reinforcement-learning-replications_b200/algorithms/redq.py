@@ -35,31 +35,32 @@ class REDQ(SAC):
                  gamma: float = 0.99, polyak_rho: float = 0.995, alpha: float = 0.2, learn_alpha: bool = False,
                  target_entropy=None, alpha_lr: float = 3e-4, n_min: int = 2, policy_delay: int = 20) -> None:
         q_functions = list(q_functions)
-        N = len(q_functions)
+        N, name = len(q_functions), type(self).__name__
         if N < 2:
-            raise ValueError(f"REDQ needs at least 2 critics, got {N}")
+            raise ValueError(f"{name} needs at least 2 critics, got {N}")
         if N > 32:
-            raise ValueError(f"REDQ supports at most 32 critics, got {N}")
+            raise ValueError(f"{name} supports at most 32 critics, got {N}")
         if not 1 <= int(n_min) <= N:
             raise ValueError(f"n_min must be in 1..{N} (the number of critics), got {n_min}")
         if int(policy_delay) < 1:
             raise ValueError(f"policy_delay must be >= 1, got {policy_delay}")
         if isinstance(replay_buffer, PrioritizedReplayBuffer):
-            raise ValueError("REDQ does not train on a PrioritizedReplayBuffer: prioritized replay is not implemented "
-                             "for it")
+            raise ValueError(f"{name} does not train on a PrioritizedReplayBuffer: prioritized replay is not "
+                             "implemented for it")
         for q in q_functions:
             if isinstance(q, ContinuousQuantileQFunction) or isinstance(q.network, ImplicitQuantileMLP):
-                raise TypeError(f"REDQ's critics map [obs | act] to one value, got {type(q).__name__} over "
+                raise TypeError(f"{name}'s critics map [obs | act] to one value, got {type(q).__name__} over "
                                 f"{type(q.network).__name__}")
             if type(q.network).__name__ == "DuelingMLP":
-                raise TypeError("REDQ does not take dueling networks")
-        refuse_noisy("REDQ", policy, *q_functions)
+                raise TypeError(f"{name} does not take dueling networks")
+        refuse_noisy(name, policy, *q_functions)
         shapes = {(tuple(sz), hid, out) for sz, hid, out, _ in (describe_mlp(q.network) for q in q_functions)}
         if len(shapes) != 1:
-            raise ValueError(f"REDQ's critics must all have the same shape, got {sorted(shapes)}")
+            raise ValueError(f"{name}'s critics must all have the same shape, got {sorted(shapes)}")
         settings = {adam_hparams(q.optimizer, describe_mlp(q.network)[3], "q-function optimizer") for q in q_functions}
         if len(settings) != 1:
-            raise NotImplementedError(f"REDQ's critics share one Adam setting (lr, betas, eps), got {sorted(settings)}")
+            raise NotImplementedError(f"{name}'s critics share one Adam setting (lr, betas, eps), got "
+                                      f"{sorted(settings)}")
         super().__init__(policy, exploration_policy, q_functions[0], q_functions[1], env, sampler, replay_buffer,
                          evaluator, gamma=gamma, polyak_rho=polyak_rho, alpha=alpha, learn_alpha=learn_alpha,
                          target_entropy=target_entropy, alpha_lr=alpha_lr)

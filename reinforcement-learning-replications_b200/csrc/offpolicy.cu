@@ -83,6 +83,8 @@ __device__ __forceinline__ float smooth_target_action(float a, float eps, float 
 //              and, when dbias is set, dbias[M] = column sums of (A (.) act'(Y)) -- the bias gradient rides along
 // MODE 3 (NN, split B): MODE 1 with rows >= ksplit of B read from A2[row - ksplit] (ld lda2): dX through a layer whose
 //              weight is two [out, in] blocks kept apart, the dueling streams' hidden layers [W_value; W_advantage]
+// MODE 4 (NT, gated): C[M,N] = (A[M,K] * B[N,K]^T) (.) act'(Y)[M,N]      EDAC's tangent forward: MODE 0's product with
+//              no bias and no activation, its output gated by the derivative at the same position of Y (ld ldy)
 // All matrices row-major with explicit leading dimensions.  Y (same shape / ld as A) may be NULL (no derivative).
 struct GemmArgs {
   const float* A; int lda;
@@ -105,6 +107,7 @@ typedef float GemmTile[GK][GT + 2];
 
 template <int MODE, bool SPLIT_B = false>  // MODE 3 runs as <1, true>: MODE 1 but for where B's rows come from
 __device__ __forceinline__ void gemm_tile(const GemmArgs& g, int bx, int by, GemmTile& As, GemmTile& Bs) {
+  constexpr bool NT = MODE == 0 || MODE == 4;  // MODE 4 loads its operands as MODE 0 does
   constexpr int KT = 8;  // k-tiles fetched ahead (registers: 8 per k-tile): K = 256 is ONE round of loads
   const int tid = threadIdx.x;
   const int m0 = by * GT, n0 = bx * GT;
@@ -123,14 +126,14 @@ __device__ __forceinline__ void gemm_tile(const GemmArgs& g, int bx, int by, Gem
         float a = 0.f;
         if (gm < g.M && gk < g.K) {
           const size_t ia = MODE == 2 ? (size_t)gk * g.lda + gm : (size_t)gm * g.lda + gk;
-          if (MODE == 0 && g.A2 != nullptr && gk >= g.ksplit) a = g.A2[(size_t)gm * g.lda2 + (gk - g.ksplit)];
+          if (NT && g.A2 != nullptr && gk >= g.ksplit) a = g.A2[(size_t)gm * g.lda2 + (gk - g.ksplit)];
           else a = g.A[ia];
-          if (MODE != 0 && g.Y) a *= op_act_prime(g.Y[MODE == 2 ? (size_t)gk * g.ldy + gm : (size_t)gm * g.ldy + gk], g.act);
+          if (!NT && g.Y) a *= op_act_prime(g.Y[MODE == 2 ? (size_t)gk * g.ldy + gm : (size_t)gm * g.ldy + gk], g.act);
         }
         ra[e] = a;
       }
       {  // B
-        const int k = MODE == 0 ? lo : hi, n = MODE == 0 ? hi : lo;
+        const int k = NT ? lo : hi, n = NT ? hi : lo;
         const int gn = n0 + n, gk = k0 + k;
         float b = 0.f;
         if (gn < g.N && gk < g.K) {
@@ -138,7 +141,7 @@ __device__ __forceinline__ void gemm_tile(const GemmArgs& g, int bx, int by, Gem
             b = gk >= g.ksplit ? g.A2[(size_t)(gk - g.ksplit) * g.lda2 + gn] : g.B[(size_t)gk * g.ldb + gn];
           } else {
             if (MODE == 2 && g.A2 != nullptr && gn >= g.ksplit) b = g.A2[(size_t)gk * g.lda2 + (gn - g.ksplit)];
-            else b = MODE == 0 ? g.B[(size_t)gn * g.ldb + gk] : g.B[(size_t)gk * g.ldb + gn];
+            else b = NT ? g.B[(size_t)gn * g.ldb + gk] : g.B[(size_t)gk * g.ldb + gn];
           }
         }
         rb[e] = b;
@@ -150,7 +153,7 @@ __device__ __forceinline__ void gemm_tile(const GemmArgs& g, int bx, int by, Gem
     for (int e = 0; e < PER; ++e) {
       const int idx = tid + e * GTHREADS, hi = idx >> 5, lo = idx & 31;
       if (MODE == 2) As[hi][lo] = ra[e]; else As[lo][hi] = ra[e];
-      if (MODE == 0) Bs[lo][hi] = rb[e]; else Bs[hi][lo] = rb[e];
+      if (NT) Bs[lo][hi] = rb[e]; else Bs[hi][lo] = rb[e];
     }
   };
   float acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
@@ -193,6 +196,8 @@ __device__ __forceinline__ void gemm_tile(const GemmArgs& g, int bx, int by, Gem
         if (MODE == 0) {
           v = op_act(v + (g.bias ? g.bias[gn] : 0.f), g.act);
           if (g.eps != nullptr) v = smooth_target_action(v, g.eps[(size_t)gm * g.N + gn], g.sigma, g.clipv, g.limit);
+        } else if (MODE == 4) {
+          v *= op_act_prime(g.Y[(size_t)gm * g.ldy + gn], g.act);
         }
         g.C[(size_t)gm * g.ldc + gn] = v;
       }
@@ -1051,19 +1056,20 @@ __global__ void __launch_bounds__(GTHREADS, 1) gemm_ens_kernel(const GemmArgs g,
 
 // One Adam step for every critic of the ensemble (blockIdx.y = critic k) with the scalars of table[idx]: the arithmetic
 // of adam_step_kernel (adam.cu) on critic k's parameters and gradient (k pg bytes after critic 0's) and its moments
-// (k mv bytes after), the exp_avg_sq product rounded as that kernel's solo instantiation rounds it
+// (k mv bytes after), the exp_avg_sq product rounded as that kernel's solo instantiation rounds it.  grad2 != NULL (EDAC's
+// diversity gradient, laid out as grad): the step is on grad[i] + grad2[i], added in that order.
 template <bool LANES>
-__global__ void __launch_bounds__(256) redq_adam_kernel(float* params, const float* grad, float* m, float* v,
-                                                        long long n, size_t pg, size_t mv, const float2* table, int idx,
-                                                        float one_minus_b1, float b2, float one_minus_b2, float eps,
-                                                        size_t lane_stride) {
+__global__ void __launch_bounds__(256) redq_adam_kernel(float* params, const float* grad, const float* grad2, float* m,
+                                                        float* v, long long n, size_t pg, size_t mv,
+                                                        const float2* table, int idx, float one_minus_b1, float b2,
+                                                        float one_minus_b2, float eps, size_t lane_stride) {
   const size_t o = LANES ? blockIdx.z * lane_stride : 0, k = blockIdx.y;
-  params = lane_ptr(params, o + k * pg), grad = lane_ptr(grad, o + k * pg);
+  params = lane_ptr(params, o + k * pg), grad = lane_ptr(grad, o + k * pg), grad2 = lane_ptr(grad2, o + k * pg);
   m = lane_ptr(m, o + k * mv), v = lane_ptr(v, o + k * mv), table = lane_ptr(table, o);
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float2 t = table[idx];
-  const float g = grad[i];
+  const float g = grad2 != nullptr ? grad[i] + grad2[i] : grad[i];
   float mi = m[i], vi = v[i];
   mi = mi + one_minus_b1 * (g - mi);
   vi = __fmaf_rn(vi, b2, __fmul_rn(__fmul_rn(g, g), one_minus_b2));
@@ -1201,6 +1207,93 @@ __global__ void redq_squash_backward_kernel(const float* out, const float* eps, 
   const float gu = dA * limit * (1.f - t * t) + 2.f * c * t;
   dout[(size_t)r * 2 * A + j] = gu;
   dout[(size_t)r * 2 * A + A + j] = (raw >= lmin && raw <= lmax) ? gu * sigma * e - c : 0.f;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// EDAC / SAC-N (algo = 11; An, Moon, Kim & Song 2021): REDQ's ensemble with M = N, a policy step every step on the min
+// over all N critics, and (eta > 0) a penalty eta D that pushes the critics' action gradients g_k = dQ_k / da apart.  D's
+// parameter gradient is taken without autograd: with ReLU hidden layers the masks are fixed, and for u_k = d(eta D) /
+// d g_k held fixed it is the gradient of the directional derivative g_k . u_k, which the existing GEMM modes give:
+//   ones-backward (MODE 1 from dOut = 1; the first layer on its action columns only) -> g_k
+//   edac_diversity_kernel                                                             -> u_k, D
+//   tangent forward (MODE 4: h'_1 = act'(h_1) (.) u W_1a^T, h'_l = act'(h_l) (.) h'_{l-1} W_l^T)
+//   weight gradients (MODE 2 without dbias: dW_1[:, act] = sum_b d_1 u^T, dW_l = sum_b d_l h'_{l-1}^T)
+// with d_l the ones-backward's gated input gradients.  The bias and obs-column gradients of D are exactly 0.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int EDAC_THREADS = 1024;  // one CTA per learner, one warp per row at a time, lane k = critic k
+constexpr double EDAC_NORM_EPS = 1e-10;
+
+// The diversity head of one learner.  g: member k's action gradients [B][A] at g + k B A (u likewise).  Per row b, with
+// n_k = |g_k|, gh_k = g_k / (n_k + 1e-10) and S = sum_k gh_k: v_k = c (S - gh_k), c = 2 eta / (B (N - 1)), and
+// u_k = v_k / (n_k + 1e-10) - g_k (g_k . v_k) / (n_k (n_k + 1e-10)^2) (the second term 0 at n_k = 0, as torch's norm
+// backward).  *div_out = D = sum_b sum_{i != j} gh_i . gh_j / (B (N - 1)).  Arithmetic in double; the sums over the
+// critics are warp shuffle trees (every lane gets the same bits), the rows' sums block_mean's fixed order.
+template <bool LANES>
+__global__ void __launch_bounds__(EDAC_THREADS) edac_diversity_kernel(const float* g, int N, int B, int A, double c,
+                                                                      float* u, float* div_out, size_t lane_stride) {
+  __shared__ double red[32];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    g = lane_ptr(g, o), u = lane_ptr(u, o), div_out = lane_ptr(div_out, o);
+  }
+  const int lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  const bool on = lane < N;
+  const size_t mo = (size_t)(on ? lane : 0) * B * A;
+  double acc = 0.0;
+  for (int b = threadIdx.x >> 5; b < B; b += nw) {  // warp-uniform
+    const float* gr = g + mo + (size_t)b * A;
+    double nn = 0.0;
+    for (int j = 0; on && j < A; ++j) nn += (double)gr[j] * (double)gr[j];
+    const double n = sqrt(nn), inv = 1.0 / (n + EDAC_NORM_EPS);
+    double dot = 0.0, drow = 0.0;
+    for (int j = 0; j < A; ++j) {
+      const double gj = on ? (double)gr[j] : 0.0, gh = gj * inv, s = warp_sum(gh);
+      dot += gj * (c * (s - gh));
+      drow += gh * (s - gh);
+    }
+    const double corr = n > 0.0 ? dot / (n * (n + EDAC_NORM_EPS) * (n + EDAC_NORM_EPS)) : 0.0;
+    for (int j = 0; j < A; ++j) {
+      const double gj = on ? (double)gr[j] : 0.0, gh = gj * inv, s = warp_sum(gh);
+      if (on) u[mo + (size_t)b * A + j] = (float)(c * (s - gh) * inv - gj * corr);
+    }
+    drow = warp_sum(drow);
+    if (lane == 0) acc += drow;
+  }
+  block_mean(acc, B * (N - 1), div_out, red);
+}
+
+// One CTA: the policy step's head at a = pi(s) on the N critics just updated (member k's output at q + k q_stride).  Per
+// row the loss is alpha log pi - min_k q_k (the first critic that attains the min, in index order; a NaN loses to a
+// number, as fminf); *loss_out = its mean, *logp_mean_out = mean log pi (summed as redq_policy_loss_kernel sums them);
+// dq_k[i] (member k's at dq + k B) is -1 / B on row i's argmin critic and 0 on the others.
+template <bool LANES>
+__global__ void __launch_bounds__(GTHREADS) edac_policy_loss_kernel(const float* q, int q_stride, int N,
+                                                                   const float* logp, const float* alpha, int B,
+                                                                   float* dq, float* loss_out, float* logp_mean_out,
+                                                                   size_t lane_stride) {
+  __shared__ double red[32], red_lp[32];
+  if (LANES) {
+    const size_t o = blockIdx.z * lane_stride;
+    q = lane_ptr(q, o), logp = lane_ptr(logp, o), alpha = lane_ptr(alpha, o), dq = lane_ptr(dq, o);
+    loss_out = lane_ptr(loss_out, o), logp_mean_out = lane_ptr(logp_mean_out, o);
+  }
+  const float a = *alpha;
+  const float g = -1.0f / (float)B;
+  double acc = 0.0, acc_lp = 0.0;
+  for (int i = threadIdx.x; i < B; i += blockDim.x) {
+    float m = q[i];
+    int km = 0;
+    for (int k = 1; k < N; ++k) {
+      const float v = q[(size_t)k * q_stride + i];
+      if (v < m || (m != m && v == v)) m = v, km = k;
+    }
+    for (int k = 0; k < N; ++k) dq[(size_t)k * B + i] = k == km ? g : 0.f;
+    const float lp = logp[i];
+    acc += (double)(a * lp - m);
+    acc_lp += (double)lp;
+  }
+  block_mean(acc, B, loss_out, red);
+  block_mean(acc_lp, B, logp_mean_out, red_lp);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -2607,6 +2700,18 @@ struct b200rl_offpolicy {
   float* redq_dx = nullptr;                      // [N][B][O + A] the critics' input gradients (policy step)
   float* redq_qmin = nullptr;                    // [B] min over the drawn target critics
   int redq_last_S = 0, redq_last_B = 0;          // the (S, B) of the last call that ran steps (redq_outputs)
+  // EDAC / SAC-N (cfg.algo == 11): a REDQ engine (h->redq is set, M = N) with its own step program.  With eta > 0 the
+  // diversity pass keeps every hidden layer's ones-backward gradient and tangent in buffers of their own (the TD
+  // backward's redq_d0 / redq_d1 run at the same time), and its weight gradient in a second gradient block laid out as
+  // the critics' (zeroed at create; its obs columns and biases are never written)
+  bool edac = false;
+  double edac_eta = 0.0;
+  float* edac_ones = nullptr;                   // [max_minibatch] ones: the ones-backward's dOut
+  float* edac_e[B200RL_MAX_LAYERS + 1];         // [N][B][maxw] layer l's ungated input gradient of sum Q_k, l >= 1
+  float* edac_t[B200RL_MAX_LAYERS + 1];         // [N][B][maxw] layer l's tangent h'_l, l >= 1
+  float *edac_g = nullptr, *edac_u = nullptr;   // [N][B][A] the action gradients and d(eta D) / d g
+  float* edac_grad = nullptr;                   // [N][state_pad(P)] the diversity term's parameter gradient
+  float* edac_div = nullptr;                    // [max_steps] D per step
   // the replay columns, episode-end columns, trees and row counts of this call (train_gather[_rng], train_prioritized)
   ReplayLanes<true> replay{};
   std::vector<void*> allocs;
@@ -2944,7 +3049,8 @@ int adam_net(const b200rl_offpolicy* h, NetBuf& nb, const float2* table, int idx
 static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_config* ic,
                          const b200rl_d4pg_config* dc, int32_t n_learners, b200rl_offpolicy** out,
                          const b200rl_tqc_config* tc = nullptr, const b200rl_cql_config* cc = nullptr,
-                         const b200rl_iql_config* vc = nullptr, const b200rl_redq_config* rq = nullptr) {
+                         const b200rl_iql_config* vc = nullptr, const b200rl_redq_config* rq = nullptr,
+                         const b200rl_edac_config* ec = nullptr) {
   B200RL_REQUIRE(cfg && out, "offpolicy_create: NULL argument");
   B200RL_REQUIRE(n_learners >= 1 && n_learners <= B200RL_MAX_LEARNERS,
                  "offpolicy_create_group: n_learners must be 1..%d, got %d", B200RL_MAX_LEARNERS, n_learners);
@@ -2952,12 +3058,12 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   B200RL_REQUIRE((cfg->algo >= 0 && cfg->algo <= 3) || cfg->algo == 5 || (cfg->algo == 4 && ic != nullptr) ||
                      (cfg->algo == 6 && dc != nullptr) || (cfg->algo == 7 && tc != nullptr) ||
                      (cfg->algo == 8 && cc != nullptr) || (cfg->algo == 9 && vc != nullptr) ||
-                     (cfg->algo == 10 && rq != nullptr),
+                     (cfg->algo == 10 && rq != nullptr) || (cfg->algo == 11 && rq != nullptr && ec != nullptr),
                  "offpolicy_create: algo must be 0 (DDPG / TD3), 1 (SAC), 2 (DQN), 3 (C51) or 5 (discrete SAC), got %d "
                  "(algo 4, IQN, is created by b200rl_offpolicy_create_iqn with its counts, algo 6, D4PG, by "
                  "b200rl_offpolicy_create_d4pg with its support, algo 7, TQC, by b200rl_offpolicy_create_tqc, algo 8, "
                  "CQL, by b200rl_offpolicy_create_cql, algo 9, IQL, by b200rl_offpolicy_create_iql, algo 10, REDQ, by "
-                 "b200rl_offpolicy_create_redq)", cfg->algo);
+                 "b200rl_offpolicy_create_redq, algo 11, EDAC, by b200rl_offpolicy_create_edac)", cfg->algo);
   B200RL_REQUIRE(ic == nullptr || cfg->algo == 4, "offpolicy_create_iqn: the config's algo must be 4 (IQN), got %d",
                  cfg->algo);
   B200RL_REQUIRE(dc == nullptr || cfg->algo == 6, "offpolicy_create_d4pg: the config's algo must be 6 (D4PG), got %d",
@@ -2968,9 +3074,10 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
                  cfg->algo);
   B200RL_REQUIRE(vc == nullptr || cfg->algo == 9, "offpolicy_create_iql: the config's algo must be 9 (IQL), got %d",
                  cfg->algo);
-  B200RL_REQUIRE(rq == nullptr || cfg->algo == 10, "offpolicy_create_redq: the config's algo must be 10 (REDQ), got "
-                 "%d", cfg->algo);
-  const bool redq = cfg->algo == 10 && rq != nullptr;  // SAC's policy over an ensemble of N critics
+  B200RL_REQUIRE(rq == nullptr || cfg->algo == 10 || ec != nullptr, "offpolicy_create_redq: the config's algo must "
+                 "be 10 (REDQ), got %d", cfg->algo);
+  // SAC's policy over an ensemble of N critics (EDAC: create_edac passes M = N)
+  const bool redq = (cfg->algo == 10 || cfg->algo == 11) && rq != nullptr;
   const int RN = redq ? rq->n_critics : 0;
   if (redq) {
     B200RL_REQUIRE(cfg->n_q == 2, "offpolicy_create_redq: REDQ needs n_q = 2 (its first two critics are the train "
@@ -3145,6 +3252,8 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
   h->iql = iql;
   h->redq = redq;
   if (redq) h->redq_cfg = *rq;
+  h->edac = ec != nullptr;
+  if (ec) h->edac_eta = ec->eta;
   h->noisy = NM != 0;
   int rc = 0;
   int maxw = O + A;
@@ -3301,6 +3410,17 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
     rc |= oalloc(h, &h->redq_dx, RN * B * (size_t)(O + A));
     rc |= oalloc(h, &h->redq_qmin, B);
   }
+  if (ec != nullptr && ec->eta > 0.0) {
+    for (int l = 1; l < cfg->q.n_layers; ++l) {
+      rc |= oalloc(h, &h->edac_e[l], RN * B * (size_t)maxw);
+      rc |= oalloc(h, &h->edac_t[l], RN * B * (size_t)maxw);
+    }
+    rc |= oalloc(h, &h->edac_ones, B);
+    rc |= oalloc(h, &h->edac_g, RN * B * (size_t)A);
+    rc |= oalloc(h, &h->edac_u, RN * B * (size_t)A);
+    rc |= oalloc(h, &h->edac_grad, RN * (size_t)state_pad(h->net[1].P));
+  }
+  if (ec != nullptr) rc |= oalloc(h, &h->edac_div, S);
   if (iql) {
     rc |= oalloc(h, &h->dbuf4, B * (size_t)maxw);
     rc |= oalloc(h, &h->dbuf5, B * (size_t)maxw);
@@ -3401,6 +3521,13 @@ static int create_engine(const b200rl_offpolicy_config* cfg, const b200rl_iqn_co
                      C51_MAX_ATOMS * sizeof(float), h->K, cudaMemcpyHostToDevice) != cudaSuccess)
       rc = 1;
   }
+  if (!rc && h->edac_ones) {  // EDAC's ones-backward reads dOut = 1 from every arena
+    const size_t nb = (size_t)h->cfg.max_minibatch;
+    const std::vector<float> ones((size_t)h->K * nb, 1.f);
+    if (cudaMemcpy2D(h->edac_ones, h->lane_stride, ones.data(), nb * sizeof(float), nb * sizeof(float), h->K,
+                     cudaMemcpyHostToDevice) != cudaSuccess)
+      rc = 1;
+  }
   if (rc) {
     b200rl_offpolicy_destroy(h);
     return 1;
@@ -3446,6 +3573,35 @@ extern "C" int b200rl_offpolicy_create_redq(const b200rl_offpolicy_config* cfg, 
                                             int32_t n_learners, b200rl_offpolicy** out) {
   B200RL_REQUIRE(redq, "offpolicy_create_redq: NULL argument");
   return create_engine(cfg, nullptr, nullptr, n_learners, out, nullptr, nullptr, nullptr, redq);
+}
+
+extern "C" int b200rl_offpolicy_create_edac(const b200rl_offpolicy_config* cfg, const b200rl_edac_config* edac,
+                                            int32_t n_learners, b200rl_offpolicy** out) {
+  B200RL_REQUIRE(cfg && edac && out, "offpolicy_create_edac: NULL argument");
+  B200RL_REQUIRE(cfg->algo == 11, "offpolicy_create_edac: the config's algo must be 11 (EDAC), got %d", cfg->algo);
+  const int N = edac->n_critics;
+  B200RL_REQUIRE(N >= 2 && N <= REDQ_MAX_CRITICS, "offpolicy_create_edac: n_critics must be 2..%d, got %d",
+                 REDQ_MAX_CRITICS, N);
+  B200RL_REQUIRE(std::isfinite(edac->eta) && edac->eta >= 0.0, "offpolicy_create_edac: eta must be finite and >= 0, "
+                 "got %g", edac->eta);
+  B200RL_REQUIRE(cfg->n_q == 2, "offpolicy_create_edac: EDAC needs n_q = 2 (its first two critics are the train call's "
+                 "q1 / q2), got %d", cfg->n_q);
+  B200RL_REQUIRE(cfg->dueling_k == 0 && cfg->noisy_layers == 0, "offpolicy_create_edac: EDAC takes neither dueling_k "
+                 "nor noisy_layers: dueling and noisy networks are not implemented for it");
+  const b200rl_mlp_desc &p = cfg->policy, &q = cfg->q;
+  const int O = p.sizes[0], A = q.sizes[0] - O;
+  B200RL_REQUIRE(b200rl_mlp_param_count(&p) > 0 && A >= 1 && p.sizes[p.n_layers] == 2 * A, "offpolicy_create_edac: "
+                 "the policy must map [obs %d] -> [mean | log_std] = 2 x %d values, got %d -> %d", O, A, O,
+                 p.sizes[p.n_layers]);
+  B200RL_REQUIRE(b200rl_mlp_param_count(&q) > 0 && q.sizes[q.n_layers] == 1, "offpolicy_create_edac: the critics must "
+                 "map [obs %d + act %d] -> 1, got %d -> %d", O, A, q.sizes[0], q.sizes[q.n_layers]);
+  // the diversity pass differentiates the critics twice; with ReLU masks the second derivative has no term of its own
+  B200RL_REQUIRE(edac->eta == 0.0 || ((q.n_layers == 1 || q.hidden_act == B200RL_ACT_RELU) &&
+                                      q.out_act == B200RL_ACT_IDENTITY),
+                 "offpolicy_create_edac: eta > 0 needs ReLU hidden layers and an identity output in the critics (the "
+                 "diversity term of other activations is not implemented); eta = 0 (SAC-N) takes any");
+  const b200rl_redq_config rq{N, N};
+  return create_engine(cfg, nullptr, nullptr, n_learners, out, nullptr, nullptr, nullptr, &rq, edac);
 }
 
 extern "C" int b200rl_offpolicy_create_iql(const b200rl_offpolicy_config* cfg, const b200rl_iql_config* iql,
@@ -3576,6 +3732,7 @@ extern "C" int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hp
   B200RL_REQUIRE(h && dp, "offpolicy_set_dqn: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_dqn: a discrete SAC engine (algo = 5) takes b200rl_offpolicy_set_sac, not "
                  "set_dqn");
+  B200RL_REQUIRE(!h->edac, "offpolicy_set_dqn: an EDAC engine (algo = 11) takes b200rl_offpolicy_set_sac, not set_dqn");
   B200RL_REQUIRE(!h->redq, "offpolicy_set_dqn: a REDQ engine (algo = 10) takes b200rl_offpolicy_set_sac, not set_dqn");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_dqn: a TQC engine (algo = 7) takes b200rl_offpolicy_set_sac, not set_dqn");
   B200RL_REQUIRE(!h->iql, "offpolicy_set_dqn: an IQL engine (algo = 9) takes b200rl_offpolicy_set_iql, not set_dqn");
@@ -3591,6 +3748,7 @@ extern "C" int b200rl_offpolicy_set_dqn(b200rl_offpolicy* h, const b200rl_dqn_hp
 extern "C" int b200rl_offpolicy_set_c51(b200rl_offpolicy* h, const b200rl_c51_hparams* cp) {
   B200RL_REQUIRE(h && cp, "offpolicy_set_c51: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_c51: a discrete SAC engine (algo = 5) has no categorical head");
+  B200RL_REQUIRE(!h->edac, "offpolicy_set_c51: an EDAC engine (algo = 11) has no categorical head");
   B200RL_REQUIRE(!h->redq, "offpolicy_set_c51: a REDQ engine (algo = 10) has no categorical head");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_c51: a TQC engine (algo = 7) has no categorical head");
   B200RL_REQUIRE(!h->iql, "offpolicy_set_c51: an IQL engine (algo = 9) has no categorical head");
@@ -3625,6 +3783,7 @@ extern "C" int b200rl_offpolicy_set_qr(b200rl_offpolicy* h, const b200rl_qr_hpar
   B200RL_REQUIRE(h && qp, "offpolicy_set_qr: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_qr: a discrete SAC engine (algo = 5) has no quantile head");
   B200RL_REQUIRE(!h->iql, "offpolicy_set_qr: an IQL engine (algo = 9) has no quantile head");
+  B200RL_REQUIRE(!h->edac, "offpolicy_set_qr: an EDAC engine (algo = 11) has no quantile critics");
   B200RL_REQUIRE(!h->redq, "offpolicy_set_qr: a REDQ engine (algo = 10) has no quantile critics");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_qr: a TQC engine (algo = 7) takes its quantile counts at create "
                  "(b200rl_offpolicy_create_tqc)");
@@ -3647,6 +3806,7 @@ extern "C" int b200rl_offpolicy_set_per(b200rl_offpolicy* h, const b200rl_per_hp
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_per: prioritized replay is not implemented for discrete SAC engines (algo = "
                  "5)");
   B200RL_REQUIRE(!h->c51, "offpolicy_set_per: prioritized replay is not implemented for C51 engines");
+  B200RL_REQUIRE(!h->edac, "offpolicy_set_per: prioritized replay is not implemented for EDAC engines (algo = 11)");
   B200RL_REQUIRE(!h->redq, "offpolicy_set_per: prioritized replay is not implemented for REDQ engines (algo = 10)");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_per: prioritized replay is not implemented for TQC engines (algo = 7)");
   B200RL_REQUIRE(!h->iql, "offpolicy_set_per: prioritized replay is not implemented for IQL engines (algo = 9)");
@@ -3665,6 +3825,7 @@ extern "C" int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, c
   B200RL_REQUIRE(h, "offpolicy_set_nstep: NULL engine");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_nstep: n-step returns are not implemented for discrete SAC engines (algo = "
                  "5)");
+  B200RL_REQUIRE(!h->edac, "offpolicy_set_nstep: n-step returns are not implemented for EDAC engines (algo = 11)");
   B200RL_REQUIRE(!h->redq, "offpolicy_set_nstep: n-step returns are not implemented for REDQ engines (algo = 10)");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_nstep: n-step returns are not implemented for TQC engines (algo = 7)");
   B200RL_REQUIRE(!h->iql, "offpolicy_set_nstep: n-step returns are not implemented for IQL engines (algo = 9)");
@@ -3688,6 +3849,8 @@ extern "C" int b200rl_offpolicy_set_nstep(b200rl_offpolicy* h, int32_t n_step, c
 extern "C" int b200rl_offpolicy_set_noise_keys(b200rl_offpolicy* h, const uint64_t* seed, const uint64_t* call) {
   B200RL_REQUIRE(h && seed && call, "offpolicy_set_noise_keys: NULL argument");
   B200RL_REQUIRE(!h->dsac, "offpolicy_set_noise_keys: a discrete SAC engine (algo = 5) draws no noise");
+  B200RL_REQUIRE(!h->edac, "offpolicy_set_noise_keys: an EDAC engine (algo = 11) has no noisy layers; its policy's "
+                 "draws come with the train call");
   B200RL_REQUIRE(!h->redq, "offpolicy_set_noise_keys: a REDQ engine (algo = 10) has no noisy layers; its subsets come "
                  "with set_redq_subsets or are drawn by train_gather_rng");
   B200RL_REQUIRE(!h->tqc, "offpolicy_set_noise_keys: a TQC engine (algo = 7) has no noisy layers; its policy's draws "
@@ -3781,6 +3944,7 @@ extern "C" int b200rl_offpolicy_sac_outputs(b200rl_offpolicy* h, int32_t S, floa
 extern "C" int b200rl_offpolicy_set_cql(b200rl_offpolicy* h, const b200rl_cql_hparams* cp) {
   B200RL_REQUIRE(h && cp, "offpolicy_set_cql: NULL argument");
   B200RL_REQUIRE(!h->iql, "offpolicy_set_cql: an IQL engine (algo = 9) takes b200rl_offpolicy_set_iql, not set_cql");
+  B200RL_REQUIRE(!h->edac, "offpolicy_set_cql: an EDAC engine (algo = 11) takes b200rl_offpolicy_set_sac, not set_cql");
   B200RL_REQUIRE(!h->redq, "offpolicy_set_cql: a REDQ engine (algo = 10) takes b200rl_offpolicy_set_sac, not set_cql");
   B200RL_REQUIRE(h->cql, "offpolicy_set_cql: the engine was not created with algo = 8 (CQL)");
   B200RL_REQUIRE(std::isfinite(cp->weight) && cp->weight >= 0.0, "offpolicy_set_cql: weight must be finite and >= 0, "
@@ -3846,6 +4010,7 @@ extern "C" int b200rl_offpolicy_cql_outputs(b200rl_offpolicy* h, int32_t S, floa
 
 extern "C" int b200rl_offpolicy_set_iql(b200rl_offpolicy* h, const b200rl_iql_hparams* ip) {
   B200RL_REQUIRE(h && ip, "offpolicy_set_iql: NULL argument");
+  B200RL_REQUIRE(!h->edac, "offpolicy_set_iql: an EDAC engine (algo = 11) takes b200rl_offpolicy_set_sac, not set_iql");
   B200RL_REQUIRE(!h->redq, "offpolicy_set_iql: a REDQ engine (algo = 10) takes b200rl_offpolicy_set_sac, not set_iql");
   B200RL_REQUIRE(h->iql, "offpolicy_set_iql: the engine was not created with algo = 9 (IQL)");
   B200RL_REQUIRE(ip->expectile > 0.0 && ip->expectile < 1.0, "offpolicy_set_iql: expectile must be in (0, 1), got %g",
@@ -3913,7 +4078,7 @@ extern "C" int b200rl_offpolicy_get_cql_draws(b200rl_offpolicy* h, int32_t S, in
 
 // A REDQ call with host subsets consumes the ones b200rl_offpolicy_set_redq_subsets staged for its S
 static int redq_take_subsets(b200rl_offpolicy* h, int S, const char* what) {
-  if (!h->redq) return 0;
+  if (!h->redq || h->edac) return 0;  // EDAC's target takes every critic
   B200RL_REQUIRE(h->redq_staged_S == S, "%s: a REDQ engine needs its subsets [S=%d, M] from "
                  "b200rl_offpolicy_set_redq_subsets before a call with host draws", what, S);
   h->redq_staged_S = -1;
@@ -3922,6 +4087,8 @@ static int redq_take_subsets(b200rl_offpolicy* h, int S, const char* what) {
 
 extern "C" int b200rl_offpolicy_set_redq_subsets(b200rl_offpolicy* h, int32_t S, const int32_t* subsets) {
   B200RL_REQUIRE(h && subsets, "offpolicy_set_redq_subsets: NULL argument");
+  B200RL_REQUIRE(!h->edac, "offpolicy_set_redq_subsets: an EDAC engine (algo = 11) takes the min over all its target "
+                 "critics and draws no subsets");
   B200RL_REQUIRE(h->redq, "offpolicy_set_redq_subsets: the engine was not created with algo = 10 (REDQ)");
   B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps, "offpolicy_set_redq_subsets: S=%d exceeds the capacity %d", S,
                  h->cfg.max_steps);
@@ -3944,11 +4111,22 @@ extern "C" int b200rl_offpolicy_set_redq_subsets(b200rl_offpolicy* h, int32_t S,
 }
 
 extern "C" int b200rl_offpolicy_get_redq_subsets(b200rl_offpolicy* h, int32_t S, int32_t* subsets) {
-  B200RL_REQUIRE(h && subsets && h->redq, "offpolicy_get_redq_subsets: bad arguments (a REDQ engine, algo = 10, has "
-                 "them)");
+  B200RL_REQUIRE(h && subsets && h->redq && !h->edac, "offpolicy_get_redq_subsets: bad arguments (a REDQ engine, algo "
+                 "= 10, has them)");
   B200RL_REQUIRE(S >= 0 && S <= h->cfg.max_steps, "offpolicy_get_redq_subsets: S=%d exceeds the capacity", S);
   const size_t w = (size_t)S * h->redq_cfg.n_min * 4;
   if (w) B200RL_CUDA(cudaMemcpy2DAsync(subsets, w, h->redq_sub, h->lane_stride, w, h->K, cudaMemcpyDeviceToHost, h->gs));
+  B200RL_CUDA(cudaStreamSynchronize(h->gs));
+  return 0;
+}
+
+extern "C" int b200rl_offpolicy_edac_outputs(b200rl_offpolicy* h, int32_t S, float* diversity) {
+  B200RL_REQUIRE(h && h->edac && diversity, "offpolicy_edac_outputs: bad arguments (an EDAC engine, algo = 11, has "
+                 "them)");
+  B200RL_REQUIRE(S == h->redq_last_S, "offpolicy_edac_outputs: the last call ran S=%d steps, asked for %d",
+                 h->redq_last_S, S);
+  const size_t w = (size_t)S * 4;
+  if (w) B200RL_CUDA(cudaMemcpy2DAsync(diversity, w, h->edac_div, h->lane_stride, w, h->K, cudaMemcpyDeviceToHost, h->gs));
   B200RL_CUDA(cudaStreamSynchronize(h->gs));
   return 0;
 }
@@ -4848,7 +5026,7 @@ static int enqueue_redq_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparam
       return 1;
     if (ens_backward(h, qa, s_obs, s_act, h->redq_dq, B, true, nullptr, s, s4)) return 1;
     if (launch(h, redq_adam_kernel<false>, redq_adam_kernel<true>, dim3((unsigned)((q1.P + 255) / 256), N), 256, 0, s,
-               q1.flat, (const float*)q1.flat_grad, q1.m, q1.v, (long long)q1.P, (size_t)pst * 4, (size_t)2 * pst * 4,
+               q1.flat, (const float*)q1.flat_grad, (const float*)nullptr, q1.m, q1.v, (long long)q1.P, (size_t)pst * 4, (size_t)2 * pst * 4,
                (const float2*)(h->adam_tab + maxS), st, (float)(1.0 - hp->q_beta1), (float)hp->q_beta2,
                (float)(1.0 - hp->q_beta2), (float)hp->q_eps))
       return 1;
@@ -4886,8 +5064,170 @@ static int enqueue_redq_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparam
   return 0;
 }
 
+// EDAC's diversity pass (b200rl.h, "EDAC") on the critics' forward activations at [s | a]: 3 Lq launches for the whole
+// ensemble, the weight gradient of eta D into h->edac_grad and D into *div_out.  Layers are 0-based here: W_l maps
+// acts[l] to acts[l + 1], e[l] is the ungated input gradient of sum_b Q_k at acts[l] (l >= 1; the first layer's is g, on
+// the action columns only) and t[l] the tangent at acts[l].
+static int edac_diversity(b200rl_offpolicy* h, float* const* acts, int B, float* div_out, cudaStream_t s) {
+  const NetBuf& nb = h->net[1];
+  const int L = nb.d.n_layers, N = h->redq_cfg.n_critics, O = h->O, A = h->A;
+  const int* sz = nb.d.sizes;
+  const unsigned ps = (unsigned)(state_pad(nb.P) * 4), as = (unsigned)((size_t)h->cfg.max_minibatch * h->maxw * 4);
+  const unsigned gs = (unsigned)((size_t)B * A * 4);
+  // ones-backward: e[l] = (e[l + 1] (.) act'(acts[l + 1])) W_l from dOut = 1; the first layer's weight is read from its
+  // action columns (B = W_0 + O, ld O + A), so its product is g [B, A] directly
+  for (int l = L - 1; l >= 0; --l) {
+    GemmArgs g{};
+    EnsStrides es{};
+    const bool top = l == L - 1;
+    g.A = top ? h->edac_ones : h->edac_e[l + 1]; g.lda = top ? 1 : sz[l + 1]; es.a = top ? 0u : as;
+    g.Y = acts[l + 1]; g.ldy = sz[l + 1]; es.y = as; g.act = top ? nb.d.out_act : nb.d.hidden_act;
+    g.B = nb.params + nb.w_off[l] + (l == 0 ? O : 0); g.ldb = sz[l]; es.b = ps;
+    g.C = l == 0 ? h->edac_g : h->edac_e[l]; g.ldc = l == 0 ? A : sz[l]; es.c = l == 0 ? gs : as;
+    g.M = B; g.N = l == 0 ? A : sz[l]; g.K = sz[l + 1];
+    if (gemm_ens<1>(h, g, es, nullptr, N, s)) return 1;
+  }
+  const double c = 2.0 * h->edac_eta / ((double)B * (double)(N - 1));
+  if (launch(h, edac_diversity_kernel<false>, edac_diversity_kernel<true>, 1, EDAC_THREADS, 0, s,
+             (const float*)h->edac_g, N, B, A, c, h->edac_u, div_out))
+    return 1;
+  // tangent forward: t[1] = act'(acts[1]) (.) u W_0a^T, t[l + 1] = act'(acts[l + 1]) (.) t[l] W_l^T
+  for (int l = 0; l < L - 1; ++l) {
+    GemmArgs g{};
+    EnsStrides es{};
+    g.A = l == 0 ? h->edac_u : h->edac_t[l]; g.lda = l == 0 ? A : sz[l]; es.a = l == 0 ? gs : as;
+    g.B = nb.params + nb.w_off[l] + (l == 0 ? O : 0); g.ldb = sz[l]; es.b = ps;
+    g.C = h->edac_t[l + 1]; g.ldc = sz[l + 1]; es.c = as;
+    g.Y = acts[l + 1]; g.ldy = sz[l + 1]; es.y = as; g.act = nb.d.hidden_act;
+    g.M = B; g.N = sz[l + 1]; g.K = l == 0 ? A : sz[l];
+    if (gemm_ens<4>(h, g, es, nullptr, N, s)) return 1;
+  }
+  // weight gradients: dW_l = sum_b (e[l + 1] (.) act'(acts[l + 1]))^T t[l] (the first layer's action columns from u),
+  // no bias gradient
+  for (int l = 0; l < L; ++l) {
+    GemmArgs g{};
+    EnsStrides es{};
+    const bool top = l == L - 1;
+    g.A = top ? h->edac_ones : h->edac_e[l + 1]; g.lda = top ? 1 : sz[l + 1]; es.a = top ? 0u : as;
+    g.Y = acts[l + 1]; g.ldy = sz[l + 1]; es.y = as; g.act = top ? nb.d.out_act : nb.d.hidden_act;
+    g.B = l == 0 ? h->edac_u : h->edac_t[l]; g.ldb = l == 0 ? A : sz[l]; es.b = l == 0 ? gs : as;
+    g.C = h->edac_grad + nb.w_off[l] + (l == 0 ? O : 0); g.ldc = sz[l]; es.c = ps;
+    g.M = sz[l + 1]; g.N = l == 0 ? A : sz[l]; g.K = B;
+    if (gemm_ens<2>(h, g, es, nullptr, N, s)) return 1;
+  }
+  return 0;
+}
+
+// The S EDAC / SAC-N steps (b200rl.h, "EDAC"): REDQ's step program with every target critic, a policy step every step
+// on the min head, and (eta > 0) the diversity pass.  Per step the branches are:
+//   s  : pi(s') -> N target critics(s') -> target head -+-> critic head -> critics' bwd -+-> Adam -> policy step -+->
+//   s3 : N critics(s, a) -+-> pi(s) --------------------+   ... pi's dW products        |                       |
+//   s2 :                  +-> diversity pass (eta > 0) ----------------------------------+  [temperature step]   |
+//   s4 :                                       the critics' dW products ... -> polyak (all N targets) ----------+
+static int enqueue_edac_steps(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s) {
+  const int O = h->O, A = h->A, N = h->redq_cfg.n_critics;
+  const int maxS = h->cfg.max_steps;
+  const bool div = h->edac_eta > 0.0;
+  const b200rl_sac_hparams& sp = h->sac_hp;
+  NetBuf &pi = h->net[0], &q1 = h->net[1];
+  const int Lq = q1.d.n_layers, Lp = pi.d.n_layers;
+  const float lmin = (float)sp.log_std_min, lmax = (float)sp.log_std_max, limit = (float)hp->action_limit;
+  const int ew = 256, rows_grid = (B + 127) / 128;
+  const size_t astr = (size_t)h->cfg.max_minibatch * h->maxw;  // floats between two members' activations
+  const int pst = (int)state_pad(q1.P);                         // floats between two members' parameters
+  cudaStream_t s2 = h->s2, s3 = h->s3, s4 = h->s4;
+  if (launch(h, sac_alpha_init_kernel<false>, sac_alpha_init_kernel<true>, (S + 1 + ew - 1) / ew, ew, 0, s,
+             h->sac_alpha, S + 1, h->sac_state, sp.learn_alpha, (float)sp.alpha))
+    return 1;
+  PolyakArgs pk{};  // the critics' block onto the targets' block, padding included (zeros stay zeros)
+  pk.n_nets = 1;
+  pk.target[0] = h->net[N + 1].params;
+  pk.param[0] = q1.params;
+  pk.n[0] = N * pst;
+  float *qa[B200RL_MAX_LAYERS + 1], *pa[B200RL_MAX_LAYERS + 1], *ta[B200RL_MAX_LAYERS + 1];
+  for (int l = 1; l <= Lq; ++l) qa[l] = h->redq_acts[l];
+  for (int l = 1; l <= Lp; ++l) pa[l] = h->acts[2][l], ta[l] = h->acts[0][l];
+  for (int st = 0; st < S; ++st) {
+    float* s_obs = h->obs + (size_t)st * B * O;
+    const float* s_act = h->act + (size_t)st * B * A;
+    const float* s_rew = h->rew + (size_t)st * B;
+    float* s_nobs = h->nobs + (size_t)st * B * O;
+    const float* s_done = h->done + (size_t)st * B;
+    const float* eps_next = h->eps + (size_t)(2 * st) * B * A;  // [S, 2, B, A]: the draw for s', then the one for s
+    const float* eps_cur = eps_next + (size_t)B * A;
+    const float* alpha = h->sac_alpha + st;
+    pa[0] = s_obs, ta[0] = s_nobs;
+    // ---- the critics on [s | a] (the logged values, the diversity pass's masks) and pi(s) with the pre-update policy
+    if (edge(h, s, s3)) return 1;
+    if (ens_forward(h, 1, qa, astr, s_obs, s_act, B, nullptr, N, s3)) return 1;
+    if (div) {
+      if (edge(h, s3, s2)) return 1;
+      if (edac_diversity(h, qa, B, h->edac_div + st, s2)) return 1;
+    }
+    if (net_forward(h, pi, pa, B, s3)) return 1;
+    if (launch(h, sac_squash_kernel<false>, sac_squash_kernel<true>, rows_grid, 128, 0, s3, pa[Lp], eps_cur, B, A, lmin,
+               lmax, limit, h->sac_act, h->sac_logp))
+      return 1;
+    // ---- soft target: a', log pi' from the current policy at s', all N target critics on [s' | a'] ----
+    if (net_forward(h, pi, ta, B, s)) return 1;
+    if (launch(h, sac_squash_kernel<false>, sac_squash_kernel<true>, rows_grid, 128, 0, s, ta[Lp], eps_next, B, A, lmin,
+               lmax, limit, h->sac_act_next, h->sac_logp_next))
+      return 1;
+    if (ens_forward(h, N + 1, h->redq_tacts, astr, s_nobs, h->sac_act_next, B, nullptr, N, s)) return 1;
+    if (launch(h, redq_target_kernel<false>, redq_target_kernel<true>, rows_grid, 128, 0, s,
+               (const float*)h->redq_tacts[Lq], (int)astr, N, B, h->redq_qmin, h->sac_alpha + st))
+      return 1;
+    // ---- critic step: every critic's TD head and backward pass, then one Adam launch on g_td + g_div ----
+    if (edge(h, s3, s)) return 1;
+    if (launch(h, redq_q_loss_kernel<false>, redq_q_loss_kernel<true>, N, GTHREADS, 0, s, (const float*)qa[Lq],
+               (int)astr, s_rew, s_done, (const float*)h->redq_qmin, (const float*)h->sac_logp_next, alpha,
+               (float)hp->gamma, B, h->redq_dq, h->out_l1 + st, S, h->out_q1 + (size_t)st * B, S * B))
+      return 1;
+    if (ens_backward(h, qa, s_obs, s_act, h->redq_dq, B, true, nullptr, s, s4)) return 1;
+    if (div && edge(h, s2, s)) return 1;
+    if (launch(h, redq_adam_kernel<false>, redq_adam_kernel<true>, dim3((unsigned)((q1.P + 255) / 256), N), 256, 0, s,
+               q1.flat, (const float*)q1.flat_grad, (const float*)(div ? h->edac_grad : nullptr), q1.m, q1.v,
+               (long long)q1.P, (size_t)pst * 4, (size_t)2 * pst * 4, (const float2*)(h->adam_tab + maxS), st,
+               (float)(1.0 - hp->q_beta1), (float)hp->q_beta2, (float)(1.0 - hp->q_beta2), (float)hp->q_eps))
+      return 1;
+    // ---- polyak beside the policy step: the targets are next read by the next step ----
+    if (edge(h, s, s4)) return 1;
+    if (launch(h, polyak_kernel<false>, polyak_kernel<true>, (pk.n[0] + ew - 1) / ew, ew, 0, s4, pk,
+               (float)hp->polyak_rho, (float)(1.0 - hp->polyak_rho)))
+      return 1;
+    // ---- policy step: the N updated critics on [s | a_pi], differentiated w.r.t. their input only ----
+    if (ens_forward(h, 1, qa, astr, s_obs, h->sac_act, B, nullptr, N, s)) return 1;
+    if (launch(h, edac_policy_loss_kernel<false>, edac_policy_loss_kernel<true>, 1, GTHREADS, 0, s,
+               (const float*)qa[Lq], (int)astr, N, (const float*)h->sac_logp, alpha, B, h->redq_dq, h->out_lp + st,
+               h->out_logp + st))
+      return 1;
+    if (sp.learn_alpha) {  // SAC's temperature step; alpha[st + 1] = exp(log_alpha)
+      if (edge(h, s, s2)) return 1;
+      if (launch(h, sac_alpha_step_kernel<false>, sac_alpha_step_kernel<true>, 1, GTHREADS, 0, s2, h->sac_logp, B,
+                 (float)sp.target_entropy, h->sac_state, h->adam_tab + (size_t)3 * maxS, st,
+                 (float)(1.0 - sp.alpha_beta1), (float)sp.alpha_beta2, (float)(1.0 - sp.alpha_beta2),
+                 (float)sp.alpha_eps, h->sac_alpha + st + 1))
+        return 1;
+    }
+    if (ens_backward(h, qa, s_obs, h->sac_act, h->redq_dq, B, false, h->redq_dx, s, nullptr)) return 1;
+    if (launch(h, redq_squash_backward_kernel<false>, redq_squash_backward_kernel<true>, (B * A + ew - 1) / ew, ew, 0,
+               s, (const float*)pa[Lp], eps_cur, (const float*)(h->redq_dx + O), B * (O + A), N, O + A, B, A, lmin, lmax,
+               limit, alpha, h->sac_dout))
+      return 1;
+    if (net_backward(h, pi, pa, h->sac_dout, 2 * A, B, true, nullptr, s, 0, nullptr, 0, 0, s3)) return 1;
+    if (adam_net(h, pi, h->adam_tab, st, hp->policy_beta1, hp->policy_beta2, hp->policy_eps, s)) return 1;
+    if (sp.learn_alpha && edge(h, s2, s)) return 1;
+    if (edge(h, s4, s)) return 1;
+  }
+  return 0;
+}
+
 static int enqueue_program(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, int S, int B, cudaStream_t s,
                            int* n_pol) {
+  if (h->edac) {
+    *n_pol = S;
+    return enqueue_edac_steps(h, hp, S, B, s);
+  }
   if (h->redq) {
     *n_pol = (S + hp->policy_delay - 1) / hp->policy_delay;
     return enqueue_redq_steps(h, hp, S, B, s);
@@ -4923,7 +5263,7 @@ static int run_staged(b200rl_offpolicy* h, const b200rl_offpolicy_hparams* hp, i
   // Adam's step-dependent scalars for the steps of this call (torch's host-side double arithmetic), one small upload
   // (a group: one table per learner, from that learner's step counts, uploaded with one strided copy)
   const int maxS = h->cfg.max_steps;
-  const int n_pol_expected = h->dqn ? 0 : h->redq || !(h->sac || h->dsac || h->iql)
+  const int n_pol_expected = h->dqn ? 0 : (h->redq && !h->edac) || !(h->sac || h->dsac || h->iql)
                                                  ? (S + hp->policy_delay - 1) / hp->policy_delay
                                                  : S;  // SAC: no delay
   const size_t tab_n = adam_tab_len(h);
@@ -5270,7 +5610,7 @@ extern "C" int b200rl_offpolicy_train_gather_rng_group(b200rl_offpolicy* h, cons
                h->cql_draws, n_cql, (long long)B * h->cql_cfg.n_actions * A, keys))
       return 1;
   }
-  if (h->redq && launch(h, redq_draw_kernel<false>, redq_draw_kernel<true>, (unsigned)((S + 127) / 128), 128, 0, s,
+  if (h->redq && !h->edac && launch(h, redq_draw_kernel<false>, redq_draw_kernel<true>, (unsigned)((S + 127) / 128), 128, 0, s,
                         h->redq_sub, (int)S, h->redq_cfg.n_critics, h->redq_cfg.n_min, keys))
     return 1;
   if (gather_columns(h, hp, SB, s)) return 1;
@@ -5322,6 +5662,8 @@ extern "C" int b200rl_offpolicy_train_prioritized_group(b200rl_offpolicy* h, con
   B200RL_REQUIRE(!h->c51, "offpolicy_train_prioritized: prioritized replay is not implemented for C51 engines");
   B200RL_REQUIRE(!h->dsac, "offpolicy_train_prioritized: prioritized replay is not implemented for discrete SAC "
                  "engines (algo = 5)");
+  B200RL_REQUIRE(!h->edac, "offpolicy_train_prioritized: prioritized replay is not implemented for EDAC engines "
+                 "(algo = 11)");
   B200RL_REQUIRE(!h->redq, "offpolicy_train_prioritized: prioritized replay is not implemented for REDQ engines "
                  "(algo = 10)");
   B200RL_REQUIRE(!h->tqc, "offpolicy_train_prioritized: prioritized replay is not implemented for TQC engines (algo = "

@@ -344,7 +344,10 @@ class OffPolicyEngine:
     activation)) of V; ``set_iql`` is required, no noise is used, and the state has four optimizers (b200rl.h, "IQL").
     REDQ (``algo`` 10) has SAC's policy, temperature and noise over N critics: ``redq`` = (N, M), M the target critics
     drawn per step; networks 1..N are the critics and N+1..2N their targets, the state has 1 + N optimizers, and a call
-    with host draws takes ``noise`` = (SAC's [S, 2, B, A], subsets [S, M]) (b200rl.h, "REDQ").
+    with host draws takes ``noise`` = (SAC's [S, 2, B, A], subsets [S, M]) (b200rl.h, "REDQ").  EDAC (``algo`` 11)
+    has REDQ's layout with every target critic in the target, a policy step every step on the min over the critics, and
+    a diversity penalty of weight eta on the critics' action gradients: ``edac`` = (N, eta), eta = 0 being SAC-N; a call
+    takes SAC's noise alone, and ``edac_outputs`` returns the penalty D per step (b200rl.h, "EDAC").
 
     ``n_learners`` = K > 1: a group of K independent learners with the same shapes and hyper-parameters, every step one
     launch for all K (b200rl_offpolicy_create_group).  Inputs and outputs then carry a leading [K] axis, the state blob
@@ -352,15 +355,15 @@ class OffPolicyEngine:
     refused."""
 
     NETS = {"policy": 0, "q1": 1, "q2": 2, "target_policy": 3, "target_q1": 4, "target_q2": 5}
-    TD3, SAC, DQN, C51, IQN, DSAC, D4PG, TQC, CQL, IQL, REDQ = 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10
+    TD3, SAC, DQN, C51, IQN, DSAC, D4PG, TQC, CQL, IQL, REDQ, EDAC = 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11
     DISCRETE = (DQN, C51, IQN)  # the algos with DQN's networks, inputs and outputs
     INDEX_ACTIONS = DISCRETE + (DSAC,)  # the algos whose action column holds an action index
-    SOFT = (SAC, DSAC, TQC, CQL, REDQ)  # the algos with SAC's temperature and outputs
-    SQUASHED = (SAC, TQC, CQL, REDQ)  # the algos with SAC's squashed-Gaussian policy and its [S, 2, B, A] noise
+    SOFT = (SAC, DSAC, TQC, CQL, REDQ, EDAC)  # the algos with SAC's temperature and outputs
+    SQUASHED = (SAC, TQC, CQL, REDQ, EDAC)  # the algos with SAC's squashed-Gaussian policy and its [S, 2, B, A] noise
 
     def __init__(self, policy_sizes, q_sizes, n_q: int, max_minibatch: int, max_steps: int, policy_acts=("relu", "tanh"),
                  q_acts=("relu", "identity"), algo: int = 0, n_learners: int = 1, dueling_k: int = 0,
-                 noisy_layers: int = 0, iqn=None, d4pg=None, tqc=None, cql=None, iql=None, redq=None):
+                 noisy_layers: int = 0, iqn=None, d4pg=None, tqc=None, cql=None, iql=None, redq=None, edac=None):
         from ._lib import OffPolicyConfig
         self.lib = _lib.load()
         current_stream_handle()
@@ -376,7 +379,10 @@ class OffPolicyEngine:
         self.tqc = None if tqc is None else (int(tqc[0]), int(tqc[1]))
         self.cql = None if cql is None else (int(cql[0]), int(bool(cql[1])))
         self.iql = None if iql is None else (tuple(int(x) for x in iql[0]), tuple(iql[1]))
-        self.redq = None if redq is None else (int(redq[0]), int(redq[1]))
+        self.edac = None if edac is None else (int(edac[0]), float(edac[1]))
+        # an EDAC engine has REDQ's layout and outputs with M = N
+        self.redq = (self.edac[0], self.edac[0]) if self.edac is not None else None if redq is None else \
+            (int(redq[0]), int(redq[1]))
         # optimizers in the state blob and the step counts
         self.n_opt = 4 if self.iql is not None else 1 + self.redq[0] if self.redq is not None else 3
         self.n_value = 0
@@ -413,6 +419,10 @@ class OffPolicyEngine:
             self.n_value = int(self.lib.b200rl_mlp_param_count(vdesc))
             check(self.lib.b200rl_offpolicy_create_iql(C.byref(cfg), C.byref(_lib.IqlConfig(vdesc)), self.K,
                                                        C.byref(h)), "offpolicy_create_iql")
+        elif self.edac is not None:  # the ensemble's size and the diversity weight (b200rl.h, "EDAC")
+            check(self.lib.b200rl_offpolicy_create_edac(C.byref(cfg), C.byref(_lib.EdacConfig(self.edac[0], 0,
+                                                                                                self.edac[1])),
+                                                        self.K, C.byref(h)), "offpolicy_create_edac")
         elif self.redq is not None:  # the ensemble's size (b200rl.h, "REDQ")
             check(self.lib.b200rl_offpolicy_create_redq(C.byref(cfg), C.byref(_lib.RedqConfig(*self.redq)), self.K,
                                                         C.byref(h)), "offpolicy_create_redq")
@@ -606,6 +616,13 @@ class OffPolicyEngine:
         qv, ql = np.zeros((self.K, N, S, B), np.float32), np.zeros((self.K, N, S), np.float32)
         check(self.lib.b200rl_offpolicy_redq_outputs(self.h, int(S), _ptr(qv), _ptr(ql)), "redq_outputs")
         return (qv[0], ql[0]) if self.K == 1 else (qv, ql)
+
+    # ---- EDAC ----
+    def edac_outputs(self, S: int):
+        """The diversity penalty D [S] of every step of the last train call (0 with eta = 0; a group: [K, S])."""
+        d = np.zeros((self.K, S), np.float32)
+        check(self.lib.b200rl_offpolicy_edac_outputs(self.h, int(S), _ptr(d)), "edac_outputs")
+        return d[0] if self.K == 1 else d
 
     # ---- CQL ----
     def set_cql(self, weight: float, temperature: float, target_action_gap: float = 0.0, alpha_lr: float = 3e-4,
@@ -824,9 +841,11 @@ class OffPolicyEngine:
             out["cql_gap_1"], out["cql_gap_2"], out["alpha_primes"] = self.cql_outputs(S)
         if self.algo == self.IQL:
             out["value_losses"], out["value_means"], out["weight_means"] = self.iql_outputs(S)
-        if self.algo == self.REDQ and S > 0:  # one mean log pi per policy step; every critic's values and losses
-            out["log_prob_means"] = out["log_prob_means"][..., :npol.value]
+        if self.algo in (self.REDQ, self.EDAC) and S > 0:  # one mean log pi per policy step; every critic's values
+            out["log_prob_means"] = out["log_prob_means"][..., :npol.value]  # and losses
             out["redq_q_values"], out["redq_q_losses"] = self.redq_outputs(S, self._last_B)
+        if self.algo == self.EDAC and S > 0:
+            out["edac_diversity"] = self.edac_outputs(S)
         return out
 
     def _lead(self, a, dtype, ndim):
